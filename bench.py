@@ -12,7 +12,9 @@ transitions/s = x batch) on a synthetic 84x84x4 uint8 replay of 1M transitions, 
            asynchronous D2H of the step's loss every step.
 `roofline`: the dominant kernel of the step, timed with CUDA events on its stream (dz_profile_*).
 `cpu_baseline` / `--impl reference`: the oracle PORT of the reference algorithm on the host cores
-(JAX is not installable here or on the GPU box; see oracle/cpu_reference.py).
+(JAX is not a dependency of this project; see oracle/cpu_reference.py).
+`--dump-outputs DIR`: after the timed steps, what the last timed step computed (loss, per-example losses, priorities,
+grad norm, updated online parameters) as DIR/<name>.npy; inputs are seeded, so two builds compare output for output.
 """
 
 import argparse
@@ -53,7 +55,11 @@ def parse():
   ap.add_argument('--no-graph', action='store_true')
   ap.add_argument('--no-cpu-baseline', action='store_true')
   ap.add_argument('--cpu-steps', type=int, default=40)
-  return ap.parse_args()
+  ap.add_argument('--dump-outputs', metavar='DIR', default=None)
+  args = ap.parse_args()
+  if args.steps < 1:
+    ap.error('--steps must be >= 1')
+  return args
 
 
 def workload_name(args):
@@ -74,7 +80,7 @@ def config_of(args, target_period):
 
 
 class ClockSampler:
-  """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+  """nvidia-smi clocks / power limit / throttle reasons DURING the timed region."""
 
   def __init__(self, index):
     self.rows, self.proc, self.index = [], None, index
@@ -82,7 +88,7 @@ class ClockSampler:
   def start(self):
     q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
-         'clocks_event_reasons.sw_power_cap')
+         'clocks_event_reasons.sw_power_cap,power.limit')
     try:
       self.proc = subprocess.Popen(['nvidia-smi', '--query-gpu=' + q, '--format=csv,noheader,nounits', '-lms', '100',
                                     '-i', str(self.index)], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
@@ -100,17 +106,17 @@ class ClockSampler:
       return {'sm_mhz': None, 'sm_max_mhz': None, 'reasons': ['nvidia-smi unavailable']}
     time.sleep(0.15)
     self.proc.terminate()
-    sm, mx, reasons = [], [], set()
+    sm, mx, plim, reasons = [], [], [], set()
     for r in self.rows:
       try:
-        sm.append(float(r[1])); mx.append(float(r[2]))
+        sm.append(float(r[1])); mx.append(float(r[2])); plim.append(float(r[8]))
         for name, v in zip(('hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown', 'sw_power_cap'), r[4:8]):
           if v.strip().lower().startswith('active'):
             reasons.add(name)
       except Exception:
         pass
     return {'sm_mhz': float(np.median(sm)) if sm else None, 'sm_max_mhz': max(mx) if mx else None,
-            'reasons': sorted(reasons), 'samples': len(sm)}
+            'power_limit_w': max(plim) if plim else None, 'reasons': sorted(reasons), 'samples': len(sm)}
 
 
 def measured_peaks():
@@ -118,8 +124,23 @@ def measured_peaks():
   if os.path.exists(path):
     with open(path) as f:
       p = json.load(f)
-    return p.get('hbm_gbs', 6650.0), p.get('bf16_tflops', 1590.0), 'measured (MEASURED_PEAKS.json)'
-  return 6650.0, 1590.0, 'fallback (B200_PROFILING.md)'
+    return p.get('hbm_gbs', 3350.0), p.get('bf16_tflops', 989.0), 'measured (MEASURED_PEAKS.json)'
+  return 3350.0, 989.0, 'H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s'
+
+
+def dump_outputs(out_dir, L):
+  """What the learner step handed back in its last timed step, as float32 .npy files (the parameters are a fixed,
+  seeded sample of at most 4M of them, so the dump stays under 64 MB)."""
+  os.makedirs(out_dir, exist_ok=True)
+  torch.cuda.synchronize()
+  online = L.online.detach().cpu().numpy()
+  if online.size > (1 << 22):
+    idx = np.sort(np.random.RandomState(0).choice(online.size, 1 << 22, replace=False))
+    online = online[idx]
+  arrays = {'loss': L.loss, 'per_example_loss': L.per_example, 'priorities': L.priorities, 'grad_norm': L.grad_norm}
+  for k, v in arrays.items():
+    np.save(os.path.join(out_dir, k + '.npy'), v.detach().cpu().numpy().astype(np.float32))
+  np.save(os.path.join(out_dir, 'online_params.npy'), online.astype(np.float32))
 
 
 def host_cores():
@@ -151,7 +172,7 @@ def reference_arm(args, rank, world):
       'vs_baseline': None, 'dtype': 'f32 (f64 sum tree)', 'data': 'synthetic',
       'config': config_of(args, AGENT_SETUP[args.agent][3]),
       'impl_note': 'oracle port (numpy replay, one thread as the reference; torch-CPU float32 learner on all host cores); the '
-                   'JAX CPU path is not installable here or on the GPU box',
+                   'JAX CPU path is not a dependency of this project',
       'cpu_baseline': {'value': value, 'unit': 'grad-steps/s', 'cores': res['cores'], 'kind': 'port', 'sample': sample},
       'e2e': {'value': value, 'unit': 'grad-steps/s', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0},
       'gpu_launches': 0,
@@ -282,6 +303,8 @@ def main():
   barrier()
   clk = clocks.stop()
   ms = e0.elapsed_time(e1)
+  if args.dump_outputs and rank == 0:
+    dump_outputs(args.dump_outputs, L)
   collective_us = 1e3 * float(np.mean([a.elapsed_time(b) for a, b in coll_events])) if coll_events else None
   t = torch.tensor([ms], dtype=torch.float64, device=device)
   if dist is not None:
@@ -398,13 +421,6 @@ def main():
     dur_s = 1e-6 * single[name] / launches_in_step
     event_us = 1e3 * prof[name][1] / prof[name][0]
     timing_source = 'device %globaltimer stamps inside the CUDA-graph step (dz_debug_timeline)'
-  traffic, ncu_facts = None, {}
-  try:
-    with open(os.path.join(ROOT, 'profiles', 'r02_traffic.json')) as f:
-      ncu_facts = json.load(f).get(args.agent, {})
-    traffic = ncu_facts.get('dram_bytes', {}).get(name)
-  except Exception:
-    traffic = None
   # dense-contraction kernels: algorithmic FLOPs per launch (2*M*N*K per problem, SURVEY §2.1 shapes)
   npass = 3 if args.agent in ('rainbow', 'double_q', 'prioritized') else 2
   nq = 64
@@ -418,24 +434,24 @@ def main():
   if name in alg_bytes and name not in alg_flops:
     achieved = alg_bytes[name] / dur_s / 1e9
     roofline = {'kernel': name, 'bound': 'hbm', 'achieved': achieved, 'peak': hbm_peak, 'unit': 'GB/s',
-                'frac': achieved / hbm_peak, 'traffic': traffic, 'alg_bytes_per_launch': alg_bytes[name],
+                'frac': achieved / hbm_peak, 'alg_bytes_per_launch': alg_bytes[name],
                 'avg_launch_us': 1e6 * dur_s, 'peak_source': peak_src}
   elif name in alg_flops:
     achieved = alg_flops[name] / dur_s / 1e12
     roofline = {'kernel': name, 'bound': 'tensor', 'achieved': achieved, 'peak': tf_peak, 'unit': 'TFLOP/s',
-                'frac': achieved / tf_peak, 'traffic': traffic, 'alg_flops_per_launch': alg_flops[name],
+                'frac': achieved / tf_peak, 'alg_flops_per_launch': alg_flops[name],
                 'avg_launch_us': 1e6 * dur_s, 'peak_source': peak_src,
-                'note': ('tcgen05 kernel (csrc/dz_tcp.cuh): error-compensated 3xTF32, i.e. three kind::tf32 MMAs per fp32 product '
-                         'to hold the 1e-5 parity bar; `achieved` counts the algorithmic 2*M*N*K only, the peak is the measured '
+                'note': ('tensor-core kernel (csrc/dz_tcp.cuh): error-compensated 3xTF32, i.e. three tf32 MMAs per fp32 product '
+                         'to hold the 1e-5 parity bar; `achieved` counts the algorithmic 2*M*N*K only, the peak is the '
                          'dense bf16 tensor throughput')
                         if name.startswith('iqn_') and os.environ.get('DZ_PK_IQN', '1') != '0' else
-                        ('fp32 FMA kernel today (exact-fp32 products for the 1e-5 parity bar); the peak is the measured dense bf16 '
+                        ('fp32 FMA kernel today (exact-fp32 products for the 1e-5 parity bar); the peak is the dense bf16 '
                          'tensor throughput, i.e. the fraction states how far this contraction is from the tensor-core roofline')}
   else:
     flops = GFLOP_PER_STEP[args.agent] * 1e9
     achieved = flops / (1e-3 * total_ms / prof_steps) / 1e12
     roofline = {'kernel': name, 'bound': 'tensor', 'achieved': achieved, 'peak': tf_peak, 'unit': 'TFLOP/s',
-                'frac': achieved / tf_peak, 'traffic': traffic, 'avg_launch_us': 1e6 * dur_s, 'peak_source': peak_src,
+                'frac': achieved / tf_peak, 'avg_launch_us': 1e6 * dur_s, 'peak_source': peak_src,
                 'note': 'whole-step algorithmic FLOPs over summed kernel time'}
   roofline['kernel_time_share'] = graph_share or share
   roofline['timing_source'] = timing_source
@@ -454,7 +470,6 @@ def main():
   step_s = (graph_step_us * 1e-6) if graph_step_us else (ms_max / K / 1e3)
   roofline['step_hbm_frac'] = step_bytes / step_s / 1e9 / hbm_peak
   roofline['step_alg_bytes'] = step_bytes
-  roofline['conv_tensor_pipe_pct'] = ncu_facts.get('tensor_pipe_pct')   # ncu sm__pipe_tensor_cycles_active of this build (profiles/)
 
   # ---- (4) CPU baseline (rank 0, N = 1 only) ---------------------------------------------------------
   cpu = None
@@ -480,6 +495,7 @@ def main():
                 'collective': ('ncclBroadcast of the %.1f MB online blob into every rank\'s target' % (4 * P / 1e6)) if world > 1
                               else 'device-to-device copy online -> target (one rank)'},
         'collective_us': collective_us,
+        'gpu': torch.cuda.get_device_name(device),
         'clocks': clk,
         'e2e': {'value': e2e_value, 'unit': 'grad-steps/s', 'h2d_bytes_per_step': stage_bytes, 'd2h_bytes_per_step': 4,
                 'note': 'agent.learn(): host RandomState draws -> pinned -> H2D; async D2H of the loss each step'},

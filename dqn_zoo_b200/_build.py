@@ -1,4 +1,4 @@
-"""Builds libdqnzoo_b200.so in-tree with nvcc for sm_100a (no GPU needed: cross-compile)."""
+"""Builds libdqnzoo_b200.so in-tree with nvcc for sm_90a (no GPU needed: cross-compile)."""
 
 import os
 import subprocess
@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB_DIR = os.path.join(HERE, 'lib')
 LIB_PATH = os.path.join(LIB_DIR, 'libdqnzoo_b200.so')
 SOURCES = ['dz_replay.cu', 'dz_learner.cu', 'dz_tcp.cu', 'dz_umma.cu', 'dz_umma_net.cu', 'dz_preprocess.cu', 'dz_jaxprng.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 
 
@@ -46,7 +46,7 @@ def build(force=False, verbose=False):
       sys.stderr.write(out)
     if p.returncode:
       raise RuntimeError('nvcc failed on %s' % src)
-  cmd = [_nvcc(), '-gencode', 'arch=compute_100a,code=sm_100a', '-shared', '-o', LIB_PATH] + objs
+  cmd = [_nvcc(), '-gencode', 'arch=compute_90a,code=sm_90a', '-shared', '-o', LIB_PATH] + objs
   subprocess.check_call(cmd)
   return LIB_PATH
 

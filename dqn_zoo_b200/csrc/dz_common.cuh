@@ -1,4 +1,4 @@
-// Shared host/device helpers for the dqn_zoo_b200 CUDA library (sm_100a only).
+// Shared host/device helpers for the dqn_zoo_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -10,6 +10,10 @@
 #include <string>
 
 #include "../../include/dqn_zoo_b200.h"
+
+namespace dz {
+constexpr int kNumSMs = 132;   // H100 SXM: grid sizes of the grid-stride and one-CTA-per-SM kernels
+}  // namespace dz
 
 namespace dz {
 

@@ -23,7 +23,7 @@ int launch_update_priorities(const dz_replay_view* view, const int64_t* d_indice
                              double alpha, int64_t size, void* stream);
 
 
-// ---- packed-operand tcgen05 GEMM (dz_tcp.cuh / dz_tcp.cu) ------------------------------------------------------
+// ---- packed-operand tensor-core GEMM (dz_tcp.cuh / dz_tcp.cu) ------------------------------------------------------
 constexpr int kPkKB = 16;         // reduction elements per k-block / pipeline stage
 constexpr int kPkMaxJobs = 8;
 constexpr int kPkMaxProblems = 4;
@@ -58,7 +58,7 @@ struct PkProblem {
   float *img_hi, *img_lo; int img_rg;
   float *imgT_hi, *imgT_lo; int imgT_rg;
 };
-struct PkBatch { PkProblem p[kPkMaxProblems]; int n; int run_kb; };   // run_kb: k-blocks per accumulation run (0: default 4)
+struct PkBatch { PkProblem p[kPkMaxProblems]; int n; };
 
 
 inline int64_t pk_image_floats(int rows_pad, int red_pad) { return (int64_t)rows_pad * red_pad; }

@@ -83,7 +83,7 @@ extern "C" int dz_jax_uniform(const uint32_t* d_keys, const int64_t* counts, int
     mx = counts[b] > mx ? counts[b] : mx;
   }
   if (mx == 0) return DZ_OK;
-  dim3 grid((unsigned)std::min<long long>(ceil_div((mx + 1) / 2, 256), 148 * 8), (unsigned)nblocks);
+  dim3 grid((unsigned)std::min<long long>(ceil_div((mx + 1) / 2, 256), kNumSMs * 8), (unsigned)nblocks);
   DZ_LAUNCH(jax_uniform_kernel, grid, 256, 0, stream, job);
   return DZ_OK;
 }

@@ -233,7 +233,7 @@ __global__ void __launch_bounds__(256) finish_tn_kernel(const __grid_constant__ 
 struct FinishNT {  // split partials [M][K] (+ dual second half) of up to two NT problems -> summed, masked output
   const float* partial[2]; const float* a_scale[2]; int nsrc; int splits; long long stride; int M, K; int dual;
   const float* mask; float* out;
-  float* out_hi; float* out_lo;   // optional: the tf32 hi/lo pair the tcgen05 kernels read (saves a separate split launch)
+  float* out_hi; float* out_lo;   // optional: the tf32 hi/lo pair the tensor-core kernels read (saves a separate split launch)
 };
 struct FinishNTBatch { FinishNT f[2]; };   // blockIdx.y selects the job
 
@@ -409,7 +409,7 @@ __global__ void __launch_bounds__(256) iqn_hadamard_bwd_kernel(float* __restrict
   dfeat[i] = f > 0.f ? acc : 0.f;  // F is the post-ReLU conv3 output: mask for the conv3 pre-activation
 }
 
-// Packed variant for the tcgen05 path: same math, but dE is written ONLY as the hi/lo TF32 tile images of the
+// Packed variant for the tensor-core path: same math, but dE is written ONLY as the hi/lo TF32 tile images of the
 // transposed operand (rows k, reduction m = b*N + n; layout in dz_tcp.cuh) that the embedding weight-gradient GEMM
 // consumes.  One block = one sample b x 64 features; requires N == 64 and D % 64 == 0.
 __global__ void __launch_bounds__(256) iqn_hadamard_bwd_packed_kernel(const float* __restrict__ dHI, const float* __restrict__ E,
@@ -1042,7 +1042,7 @@ __global__ void __launch_bounds__(256) grad_norm_kernel(const float* __restrict_
 struct OptArgs {
   int kind; float lr, eps, decay, b1, b2, max_norm;
   float* p; const float* g; float* m; float* v; long long n; const float* norm; const int64_t* counters;
-  // split global norm (tcgen05 path): norm = sqrt(fc_sumsq[0] + sum of parts[0..nparts)), recomputed identically by every block
+  // split global norm (tensor-core path): norm = sqrt(fc_sumsq[0] + sum of parts[0..nparts)), recomputed identically by every block
   const float* parts; int nparts; const float* fc_sumsq; float* norm_out; float* user_norm;
   int stages;   // optimizer_bulk_kernel: depth of the shared-memory ring
 };
@@ -1331,7 +1331,7 @@ struct dz_learner {
   float* q_scratch;
   int norm_blocks;
   int fc_splits, head_splits, conv_splits, nt_splits;
-  // packed-operand tcgen05 path of the IQN 3136->512 layer (dz_tcp.cuh): hi/lo tile images + split partials
+  // packed-operand tensor-core path of the IQN 3136->512 layer (dz_tcp.cuh): hi/lo tile images + split partials
   bool pk_on;
   struct PkImg { float* hi; float* lo; int rows_pad, red_pad; };
   PkImg pk_act[3], pk_wT[2], pk_w, pk_actT, pk_dh1T, pk_dh1, pk_cos[3], pk_weT[2], pk_dET, pk_cosT;
@@ -1349,7 +1349,7 @@ struct dz_learner {
   cudaEvent_t ev_fork2, ev_join2;
   bool side2_dirty;
   float* norm_parts;                        // split-norm slots written by the conv weight-gradient finish kernels
-  // TMA-fed tcgen05 path of the batch-sized step (dz_umma_net.cu): torso + 3136 -> 512 layer(s), forward and input gradients
+  // TMA-fed tensor-core path of the batch-sized step (dz_umma_net.cu): torso + 3136 -> 512 layer(s), forward and input gradients
   UmNet* um;
   char* um_ws;
   int um_npass, um_set[3];
@@ -1357,9 +1357,9 @@ struct dz_learner {
 
 namespace {
 
-constexpr int kNormBlocks = 592;
+constexpr int kNormBlocks = kNumSMs * 4;
 
-// The packed-operand tcgen05 kernels carry IQN's 3136->512 layer whenever every network apply has >= 1024 rows
+// The packed-operand tensor-core kernels carry IQN's 3136->512 layer whenever every network apply has >= 1024 rows
 // (DZ_PK_IQN=0 falls back to the fp32-FMA kernels, for A/B timing).
 bool g_pk_iqn = true;
 int g_fc_splits = 0;      // DZ_FC_SPLITS override
@@ -1368,18 +1368,18 @@ int g_conv1_splits = 1;   // DZ_CONV1_SPLITS: split-K of the conv1 forward GEMM 
                           // the extra finish launch eats the gain, so the default stays 1.
 void read_env();
 
-// Split count for a one-CTA-per-SM kernel: minimise (waves of 148 CTAs) x (k-blocks per split).
+// Split count for a one-CTA-per-SM kernel: minimise (waves of kNumSMs CTAs) x (k-blocks per split).
 int pick_splits(int64_t tiles, int nkb, int max_splits) {
   int best = 1;
   int64_t best_cost = -1;
   for (int s = 1; s <= max_splits; ++s) {
-    int64_t cost = ceil_div(tiles * s, 148) * (ceil_div(nkb, s) + 6);   // +6: pipeline fill/drain per CTA
+    int64_t cost = ceil_div(tiles * s, kNumSMs) * (ceil_div(nkb, s) + 6);   // +6: pipeline fill/drain per CTA
     if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = s; }
   }
   return best;
 }
 
-// DZ_UMMA=0 keeps every contraction on the fp32-FMA kernels (A/B timing, geometries the tcgen05 path does not cover).
+// DZ_UMMA=0 keeps every contraction on the fp32-FMA kernels (A/B timing, geometries the tensor-core path does not cover).
 bool g_umma = true;
 int64_t noise_stride(const dz_learner_config& c, const Dims& d);
 struct NoiseVecs;
@@ -1644,7 +1644,7 @@ int finish_nn(const GemmBatch& gb, float* const* outs, bool dual, void* stream) 
     long long t = (long long)p.M * p.N;
     mx = t > mx ? t : mx;
   }
-  dim3 grid((unsigned)std::min<long long>(ceil_div(mx, 256), 148 * 8), gb.n);   // grid-stride kernels
+  dim3 grid((unsigned)std::min<long long>(ceil_div(mx, 256), kNumSMs * 8), gb.n);   // grid-stride kernels
   DZ_LAUNCH(finish_nn_kernel, grid, 256, 0, stream, fb);
   return DZ_OK;
 }
@@ -1681,7 +1681,7 @@ int forward_torso(dz_learner* l, const TorsoJob* jobs, int njobs, int nimg, void
   }
   DZ_TRY(run_nn("conv1_fwd", gb, false, stream));
   if (gb.p[0].splits > 1) DZ_TRY(finish_nn(gb, outs1, false, stream));
-  // conv2 / conv3: few output tiles (41 / 25 per pass) -> split K four ways so the grid covers the 148 SMs;
+  // conv2 / conv3: few output tiles (41 / 25 per pass) -> split K four ways so the grid covers the 132 SMs;
   // finish_nn adds the bias and ReLU.
   for (int layer = 2; layer <= 3; ++layer) {
     float* outs[kMaxProblems];
@@ -1818,7 +1818,7 @@ int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, c
 }
 
 // IQN embedding (latent -> 3136, ReLU, * state embedding) and 3136 -> 512 layer of the three network applies of
-// one update on the packed-operand tcgen05 kernels: one pack launch (cosine features + every weight operand of
+// one update on the packed-operand tensor-core kernels: one pack launch (cosine features + every weight operand of
 // this step), the embedding GEMM whose epilogue writes the hi/lo tile images of the next GEMMs directly (the fp32
 // `hi` tensors are never materialised), the split fc1 GEMM, one finish (bias + ReLU).
 int iqn_embed_fc1_forward_packed(dz_learner* l, const Pass* passes, const GemmBatch& fc1, bool keep_E0, void* stream) {
@@ -1869,7 +1869,6 @@ int iqn_embed_fc1_forward_packed(dz_learner* l, const Pass* passes, const GemmBa
   PkBatch kb;
   memset(&kb, 0, sizeof(kb));
   kb.n = 3;
-  kb.run_kb = 2;     // forward: feeds the ReLU mask and the quantile targets -> fp32-FMA-chain accuracy
   GemmBatch fin = fc1;
   float* outs[kMaxProblems] = {nullptr};
   long long off = 0;
@@ -1945,7 +1944,7 @@ int forward_heads_iqn(dz_learner* l, const Pass* passes, int np, int nimg, const
       h.out[i] = l->out[hp]; h.M[i] = nimg * l->n_head[hp];
       maxM = std::max(maxM, h.M[i]);
     }
-    dim3 grid((unsigned)std::min<int64_t>(ceil_div(maxM, 8), 148 * 2), (unsigned)np);
+    dim3 grid((unsigned)std::min<int64_t>(ceil_div(maxM, 8), kNumSMs * 2), (unsigned)np);
     DZ_LAUNCH_NAMED("iqn_head_fwd", iqn_head_fwd_kernel, grid, 256, 0, stream, h, d.out);
     return DZ_OK;
   }
@@ -1977,7 +1976,7 @@ int finish_nt_batch(const FinishNT* jobs, int njobs, void* stream) {
   memset(&fb, 0, sizeof(fb));
   long long total = 0;
   for (int j = 0; j < njobs; ++j) { fb.f[j] = jobs[j]; total = std::max(total, (long long)jobs[j].M * jobs[j].K); }
-  dim3 grid((unsigned)std::min<long long>(ceil_div(total, 256), 148 * 8), (unsigned)njobs);
+  dim3 grid((unsigned)std::min<long long>(ceil_div(total, 256), kNumSMs * 8), (unsigned)njobs);
   DZ_LAUNCH(finish_nt_kernel, grid, 256, 0, stream, fb);
   return DZ_OK;
 }
@@ -2137,7 +2136,7 @@ int backward_plain(dz_learner* l, void* stream) {
     p.A = l->dout; p.lda = d.out; p.M = B; p.N = d.out; p.K = 512;
     p.B = P + L.off("head/w"); p.ldb = d.out; p.C = l->dh1[0]; p.ldc = 512; p.mask = l->h1[0][0];
     // Wide heads (c51: 306 outputs, qr-dqn: 1206): with one CTA column per 64 outputs of dh1 the reduction over the head
-    // width is a serial chain (measured 24 / 65 us); split it and let the finish kernel apply the mask (and, on the tcgen05
+    // width is a serial chain (measured 24 / 65 us); split it and let the finish kernel apply the mask (and, on the tensor-core
     // path, write the tf32 hi/lo pair fc1_dgrad reads, which saves the separate split launch).
     const int splits = d.out > 64 ? (int)std::min<int64_t>(16, ceil_div(d.out, 96)) : 1;
     if (splits > 1) {
@@ -2161,7 +2160,7 @@ int backward_plain(dz_learner* l, void* stream) {
     gb.p[0] = p;
     DZ_TRY(run_tn("fc1_wgrad", gb, fork_side(l, stream)));
   }
-  if (l->um) {   // dact3 on the tcgen05 path: dh1 -> tf32 hi/lo, W streamed once through TMA, split partials + masked finish
+  if (l->um) {   // dact3 on the tensor-core path: dh1 -> tf32 hi/lo, W streamed once through TMA, split partials + masked finish
     if (!dh1_split_done) DZ_TRY(um_split_dh1(l->um, stream));
     DZ_TRY(um_backward_fc(l->um, nullptr, stream));
   } else {  // dact3 = dh1 * Wf^T, masked by act3 > 0
@@ -2212,7 +2211,7 @@ int backward_rainbow(dz_learner* l, const float* noise, void* stream) {
     gb.p[s] = p;
   }
   DZ_TRY(run_nt("noisy2_dgrad", gb, true, stream));
-  {   // both streams' dh1 in one launch; on the tcgen05 path it also writes the tf32 hi/lo pair noisy1_dgrad reads
+  {   // both streams' dh1 in one launch; on the tensor-core path it also writes the tf32 hi/lo pair noisy1_dgrad reads
     FinishNT jobs[2];
     for (int s = 0; s < 2; ++s)
       jobs[s] = make_finish_nt(&gb.p[s], 1, l->h1[0][s], l->dh1[s], true, l->um ? um_dh1_hi(l->um, s) : nullptr,
@@ -2280,14 +2279,14 @@ int backward_iqn(dz_learner* l, void* stream) {
     p.B = P + L.off("head/w"); p.ldb = d.out; p.C = l->dh1[0]; p.ldc = 512; p.mask = l->h1[0][0];
     gb.p[0] = p;
     if (M >= 512 && d.out <= kSkinnyMaxN) {
-      DZ_LAUNCH_NAMED("iqn_head_dgrad", iqn_head_dgrad_kernel, (unsigned)std::min<int64_t>(ceil_div((long long)M * 128, 256), 148 * 8),
+      DZ_LAUNCH_NAMED("iqn_head_dgrad", iqn_head_dgrad_kernel, (unsigned)std::min<int64_t>(ceil_div((long long)M * 128, 256), kNumSMs * 8),
                       256, 0, stream, l->dout, P + L.off("head/w"), l->h1[0][0], l->dh1[0], M, d.out);
     } else {
       DZ_TRY(run_nt("iqn_head_dgrad", gb, false, stream));
     }
   }
   if (l->pk_on) {
-    // dh1 in both operand orientations, then the two big contractions on the tcgen05 kernel
+    // dh1 in both operand orientations, then the two big contractions on the tensor-core kernel
     PackBatch pb;
     memset(&pb, 0, sizeof(pb));
     DZ_TRY(pk_add_job(pb, l->dh1[0], 512, 0, 512, M, l->pk_dh1T.rows_pad, l->pk_dh1T.red_pad, -1, l->pk_dh1T.hi, l->pk_dh1T.lo));
@@ -2299,7 +2298,6 @@ int backward_iqn(dz_learner* l, void* stream) {
     PkBatch kb;
     memset(&kb, 0, sizeof(kb));
     kb.n = 1;
-    kb.run_kb = 4;
     {  // fc1 wgrad: [feat + 1 (bias row), 512] = hi0^T(+ones) * dh1, reduction over the M rows, split partials
       PkProblem& p = kb.p[0];
       p.A = PkOperand{l->pk_actT.hi, l->pk_actT.lo, l->pk_actT.rows_pad / 8};
@@ -2312,7 +2310,7 @@ int backward_iqn(dz_learner* l, void* stream) {
     }
     {  // dHI[m,k] = sum_n dh1[m,n] W[k,n]
       PkProblem& p = kb.p[0];
-      memset(&p, 0, sizeof(p));   // (run_kb stays 4)
+      memset(&p, 0, sizeof(p));
       p.A = PkOperand{l->pk_dh1.hi, l->pk_dh1.lo, l->pk_dh1.rows_pad / 8};
       p.B = PkOperand{l->pk_w.hi, l->pk_w.lo, l->pk_w.rows_pad / 8};
       p.MI = M; p.NJ = d.feat; p.nkb = l->pk_dh1.red_pad / kPkKB;
@@ -2344,7 +2342,6 @@ int backward_iqn(dz_learner* l, void* stream) {
     PkBatch kb;
     memset(&kb, 0, sizeof(kb));
     kb.n = 1;
-    kb.run_kb = 4;
     PkProblem& p = kb.p[0];
     p.A = PkOperand{l->pk_dET.hi, l->pk_dET.lo, l->pk_dET.rows_pad / 8};
     p.B = PkOperand{l->pk_cosT.hi, l->pk_cosT.lo, l->pk_cosT.rows_pad / 8};
@@ -2370,12 +2367,12 @@ int backward_iqn(dz_learner* l, void* stream) {
   }
   long long mx = 0;
   for (int q = 0; q < fb.n; ++q) mx = std::max<long long>(mx, (long long)(fb.f[q].K + 1) * fb.f[q].N);
-  dim3 grid((unsigned)std::min<long long>(ceil_div(mx, 256), 148 * 8), fb.n);
+  dim3 grid((unsigned)std::min<long long>(ceil_div(mx, 256), kNumSMs * 8), fb.n);
   DZ_LAUNCH(finish_tn_kernel, grid, 256, 0, (l->side && l->side_dirty ? (void*)l->side : stream), fb);
   return DZ_OK;
 }
 
-// Split global norm (tcgen05 path, every agent but IQN): the sum of squares of everything behind the conv tensors is taken
+// Split global norm (tensor-core path, every agent but IQN): the sum of squares of everything behind the conv tensors is taken
 // on the second side stream as soon as the last FC / head weight gradient is written (norm_fc_range), the conv tensors'
 // partials come from the per-layer weight-gradient finish kernels, and the optimizer (or norm_finalize_kernel) combines them.
 bool split_norm_active(const dz_learner* l) { return l->um != nullptr && l->cfg.kind != DZ_IQN && l->side2 != nullptr; }
@@ -2423,7 +2420,7 @@ int run_optimizer(dz_learner* l, float* user_norm, bool apply, void* stream) {
       attr_done = true;
     }
     const long long nchunks = ((o.n >> 2) + kOptChunk - 1) / kOptChunk;
-    const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>(148LL * bulk_per_sm, nchunks));
+    const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>((long long)kNumSMs * bulk_per_sm, nchunks));
     const unsigned threads = kOptChunk * 4 / vec;
     if (c.optimizer == DZ_ADAM) {
       if (vec == 4) DZ_LAUNCH_NAMED("optimizer_kernel", (optimizer_bulk_kernel<DZ_ADAM, 4>), grid, threads, kOptSmem, stream, o);
@@ -2434,8 +2431,8 @@ int run_optimizer(dz_learner* l, float* user_norm, bool apply, void* stream) {
     }
     return DZ_OK;
   }
-  if (c.optimizer == DZ_ADAM) DZ_LAUNCH_NAMED("optimizer_kernel", optimizer_kernel<DZ_ADAM>, 148 * per_sm, 256, 0, stream, o);
-  else DZ_LAUNCH_NAMED("optimizer_kernel", optimizer_kernel<DZ_RMSPROP_CENTERED>, 148 * per_sm, 256, 0, stream, o);
+  if (c.optimizer == DZ_ADAM) DZ_LAUNCH_NAMED("optimizer_kernel", optimizer_kernel<DZ_ADAM>, kNumSMs * per_sm, 256, 0, stream, o);
+  else DZ_LAUNCH_NAMED("optimizer_kernel", optimizer_kernel<DZ_RMSPROP_CENTERED>, kNumSMs * per_sm, 256, 0, stream, o);
   return DZ_OK;
 }
 
@@ -2462,7 +2459,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   jobs[nj++] = TorsoJob{tg, batch->d_s_t_rows, 2};
   const bool um = l->um != nullptr;
   if (um) {
-    if (nj != l->um_npass) return fail(DZ_EINVAL, "tcgen05 path: pass count mismatch");
+    if (nj != l->um_npass) return fail(DZ_EINVAL, "tensor-core path: pass count mismatch");
     const uint8_t* const* rows[3] = {nullptr, nullptr, nullptr};
     for (int i = 0; i < nj; ++i) rows[i] = jobs[i].rows;
     if (weights_packed) DZ_TRY(join_side(l, stream));   // packed on the side stream, concurrently with the sampler
@@ -2797,10 +2794,10 @@ int dz_learner_sync_target(dz_learner* l, void* stream) {
   return DZ_OK;
 }
 
-// Debug hook: the tcgen05 launch named `tag` ("conv2_fwd", "conv3_fwd", "fc1_fwd", "fc1_dgrad", "conv3_dgrad", "conv2_dgrad",
+// Debug hook: the tensor-core launch named `tag` ("conv2_fwd", "conv3_fwd", "fc1_fwd", "fc1_dgrad", "conv3_dgrad", "conv2_dgrad",
 // "conv3_wgrad", "conv2_wgrad") writes the clock stamps of its CTA 0 into d_trace (512 int64); nullptr switches it off.
 int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace) {
-  if (!l->um) return fail(DZ_EINVAL, "the tcgen05 path is not active for this learner");
+  if (!l->um) return fail(DZ_EINVAL, "the tensor-core path is not active for this learner");
   um_net_trace(l->um, tag, d_trace);
   return DZ_OK;
 }
@@ -2823,7 +2820,7 @@ int dz_test_learner_buffer(dz_learner* l, const char* name, float** d_ptr, int64
   else if (n == "h1") { *d_ptr = l->h1[0][0]; *count = rows0 * 512; }
   else if (n == "dh1") { *d_ptr = l->dh1[0]; *count = rows0 * 512; }
   else if (n == "iqn_hi") {
-    if (l->pk_on) return fail(DZ_EINVAL, "iqn_hi is not materialised on the packed tcgen05 path (DZ_PK_IQN=0 keeps it)");
+    if (l->pk_on) return fail(DZ_EINVAL, "iqn_hi is not materialised on the packed tensor-core path (DZ_PK_IQN=0 keeps it)");
     *d_ptr = l->hi[0]; *count = l->hi[0] ? rows0 * l->d.feat : 0;
   }
   else if (n == "iqn_dhi") { *d_ptr = l->dhi; *count = l->dhi ? rows0 * l->d.feat : 0; }

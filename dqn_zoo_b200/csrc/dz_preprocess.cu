@@ -124,7 +124,7 @@ __global__ void __launch_bounds__(256) atari_preprocess_kernel(const PreprocessA
       // 255 * 1.5 * 2^-23 = 4.6e-5 of the exact value, and floor() can only be in doubt when the fractional part is
       // within 2^-13 of an integer.  With the reference's weights the exact luma is a multiple of 0.001 (up to
       // 1e-13), so that is the ~1 colour in 1000 whose luma IS an integer; only those pixels take the reference's
-      // float64 sequence (B200's scalar FP64 pipe is narrow; the instruction count is what bounds this kernel).
+      // float64 sequence (the instruction count is what bounds this kernel).
       const uint32_t v = px[e][0] * a.fr + px[e][1] * a.fg + px[e][2] * a.fb;
       const uint32_t frac = v & ((1u << 23) - 1);
       uint32_t y = v >> 23;

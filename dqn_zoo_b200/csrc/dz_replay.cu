@@ -538,7 +538,7 @@ using namespace dz;
 extern "C" {
 
 const char* dz_last_error(void) { return g_last_error.c_str(); }
-const char* dz_build_info(void) { return "dqn_zoo_b200 0.1 sm_100a " __DATE__ " " __TIME__; }
+const char* dz_build_info(void) { return "dqn_zoo_b200 0.1 sm_90a " __DATE__ " " __TIME__; }
 int64_t dz_launch_count(void) { return g_launches.load(); }
 
 // Debug: installs (or, with nullptr, removes) the device buffer every kernel of the library stamps at its start
@@ -646,7 +646,7 @@ int dz_replay_fill_synthetic(const dz_replay_view* view, int64_t row0, int64_t n
   if (row0 < 0 || row0 + n > view->capacity) return fail(DZ_ERANGE, "rows out of range");
   if (n == 0) return DZ_OK;
   int64_t total = n * 2 * (view->obs_bytes >> 3);
-  int grid = (int)(ceil_div(total, 256) < 148 * 32 ? ceil_div(total, 256) : 148 * 32);
+  int grid = (int)(ceil_div(total, 256) < kNumSMs * 32 ? ceil_div(total, 256) : kNumSMs * 32);
   DZ_LAUNCH(fill_obs_kernel, grid, 256, 0, stream, *view, row0, n, seed);
   DZ_LAUNCH(fill_scalars_kernel, (int)ceil_div(n, 256), 256, 0, stream, *view, row0, n, seed, num_actions, discount);
   return DZ_OK;

@@ -1,21 +1,17 @@
-// tcgen05 / TMEM helpers shared by the tensor-core kernels of the learner (sm_100a): mbarrier and elect.sync wrappers,
-// the kind::tf32 MMA / commit instructions, instruction- and (no-swizzle) shared-memory descriptors, and the tf32 split
+// Tensor-core helpers shared by the learner's GEMM kernels (sm_90a): mbarrier and elect.sync wrappers, the warp-level
+// m16n8k8 tf32 MMA with the shared-memory fragment loads of one k-step, and the tf32 split
 //
 //     x = hi + lo,  hi = rn_tf32(x),  lo = rn_tf32(x - hi)      (error-compensated 3xTF32: D += Ah*Bh + Al*Bh + Ah*Bl)
 //
 // that keeps every contraction within ~2^-21 relative of an fp32 FMA evaluation (the parity bar is 1e-5 on losses and
 // gradients).  The kernels themselves: dz_umma.cuh (TMA-fed family: torso + 3136->512 layers at batch 32), dz_umma_net.cu
 // (conv1 with the uint8 gather), dz_tcp.cuh (packed-operand GEMM of IQN's 2048-row layers).
-// (Round 1's register-loader kernel that lived here was retired in round 2: slower than the fp32-FMA kernels it was meant
-// to replace — profiles/r01_tc_vs_simt.md — and superseded by the TMA-fed family.)
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 namespace dz {
 namespace tc {
-
-constexpr int kChunkPad = 144;     // 128-byte core matrix + 16 bytes so 8 consecutive chunks hit distinct banks
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -26,8 +22,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 // One lane of a converged warp.  With elect.sync ptxas knows that exactly one thread runs the guarded region and
-// emits the tcgen05.mma / TMA instructions back to back; under `if (lane == 0)` it wraps EVERY such instruction in an
-// ELECT / BRA.U.ANY loop over the possibly-active lanes (measured: ~75 cycles per MMA instead of the pipe's 16-32).
+// emits the bulk-copy / TMA instructions back to back instead of wrapping each in a loop over the possibly-active lanes.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n .reg .pred P;\n elect.sync _|P, 0xffffffff;\n selp.u32 %0, 1, 0, P;\n}\n" : "=r"(pred));
@@ -48,40 +43,69 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
 }
 
-// 64-bit shared-memory matrix descriptor, SWIZZLE_NONE ("interleave") canonical layouts.
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version for sm_100
-  return d;                // base_offset 0, lbo_mode 0, layout_type 0 (no swizzle)
+// D += A * B for one 16 x 8 x 8 tile (mma.sync, fragments as in the PTX ISA's m16n8k8 .tf32 layout):
+//   a = {A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4]},  b = {B[t][g], B[t+4][g]},  d = {D[g][2t], D[g][2t+1], D[g+8][2t], D[g+8][2t+1]}
+// with g = lane / 4, t = lane % 4.
+__device__ __forceinline__ void mma_16x8x8(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
-__device__ __forceinline__ uint32_t make_idesc(int M, int N, int a_mn_major, int b_mn_major) {
-  uint32_t d = 0;
-  d |= 1u << 4;    // D format f32
-  d |= 2u << 7;    // A format tf32
-  d |= 2u << 10;   // B format tf32
-  d |= (uint32_t)a_mn_major << 15;
-  d |= (uint32_t)b_mn_major << 16;
-  d |= (uint32_t)(N >> 3) << 17;
-  d |= (uint32_t)(M >> 4) << 24;
-  return d;
+// One warp's share of one k-step of 8 reduction elements: rows [m0, m0 + 16 MT) x columns [n0, n0 + 8 NT) of
+//     D += Al*Bh + Ah*Bl + Ah*Bh      (Al*Bh skipped when A is exact, i.e. has no lo part: a_lo == nullptr)
+// a_off(m, k) / b_off(n, k): byte offset of an element inside one part (hi or lo) of the staged operand, so any
+// shared-memory arrangement (K-major or MN-major, swizzled or not) is read as it landed.  The tensor core adds into
+// its fp32 accumulator with round-towards-zero, so the three products of a k-step are formed from zero and added
+// into `sum` with an ordinary round-to-nearest add.
+template <int MT, int NT, class AOff, class BOff>
+__device__ __forceinline__ void warp_kstep_3xtf32(float (&sum)[MT][NT][4], const uint8_t* a_hi, const uint8_t* a_lo,
+                                                  const uint8_t* b_hi, const uint8_t* b_lo, int m0, int n0, int k0,
+                                                  AOff a_off, BOff b_off) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  uint32_t ah[MT][4], al[MT][4];
+#pragma unroll
+  for (int mt = 0; mt < MT; ++mt) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const uint32_t o = a_off(m0 + mt * 16 + g + (q & 1) * 8, k0 + t + (q >> 1) * 4);
+      ah[mt][q] = *reinterpret_cast<const uint32_t*>(a_hi + o);
+      al[mt][q] = a_lo ? *reinterpret_cast<const uint32_t*>(a_lo + o) : 0u;
+    }
+  }
+#pragma unroll
+  for (int nt = 0; nt < NT; ++nt) {
+    uint32_t bh[2], bl[2];
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const uint32_t o = b_off(n0 + nt * 8 + g, k0 + t + q * 4);
+      bh[q] = *reinterpret_cast<const uint32_t*>(b_hi + o);
+      bl[q] = *reinterpret_cast<const uint32_t*>(b_lo + o);
+    }
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) {
+      float p[4] = {0.f, 0.f, 0.f, 0.f};
+      if (a_lo) mma_16x8x8(p, al[mt], bh);             // small cross terms first
+      mma_16x8x8(p, ah[mt], bl);
+      mma_16x8x8(p, ah[mt], bh);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) sum[mt][nt][e] += p[e];
+    }
+  }
 }
 
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// Row / column of D that element e of fragment (mt, nt) of warp_kstep_3xtf32 holds, relative to (m0, n0).
+__device__ __forceinline__ int frag_row(int mt, int e) { return mt * 16 + ((threadIdx.x & 31) >> 2) + (e >> 1) * 8; }
+__device__ __forceinline__ int frag_col(int nt, int e) { return nt * 8 + 2 * (threadIdx.x & 3) + (e & 1); }
+
+// Byte offsets inside SWIZZLE_128B tiles (1024-byte aligned, 128-byte rows, 16-byte chunk c of row r stored at c ^ (r & 7)):
+//   K-major : row = MN index, 32 reduction elements per row
+//   MN-major: row = reduction index, 32 MN indices per row, 32-wide MN slabs `lbo` bytes apart
+__device__ __forceinline__ uint32_t sw128_kmajor(int mn, int k) {
+  return (uint32_t)(mn * 128 + ((((k >> 2) ^ mn) & 7) << 4) + ((k & 3) << 2));
 }
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ uint32_t sw128_mnmajor(int mn, int k, uint32_t lbo) {
+  return (uint32_t)(mn >> 5) * lbo + (uint32_t)(k * 128 + (((((mn & 31) >> 2) ^ k) & 7) << 4) + ((mn & 3) << 2));
 }
 
 // hi = rn_tf32(x), lo = rn_tf32(x - hi): round-to-nearest on both keeps the split error zero-mean

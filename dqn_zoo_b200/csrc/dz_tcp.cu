@@ -1,4 +1,4 @@
-// Host-side launchers of the packed-operand tcgen05 GEMM (dz_tcp.cuh) + a C-ABI self-test entry point.
+// Host-side launchers of the packed-operand tensor-core GEMM (dz_tcp.cuh) + a C-ABI self-test entry point.
 #include "dz_tcp.cuh"
 #include "dz_internal.cuh"
 
@@ -63,15 +63,8 @@ static int launch_pgemm_t(const char* tag, const PkBatch& kb, void* stream) {
   return DZ_OK;
 }
 
-int launch_pgemm(const char* tag, const PkBatch& kb_in, void* stream, int epi) {
-  if (kb_in.n <= 0 || kb_in.n > kPkMaxProblems) return fail(DZ_EINVAL, "pgemm batch size");
-  PkBatch kb = kb_in;
-  // Accumulation-run length in k-blocks of 16: every MMA accumulation truncates the fp32 accumulator (round
-  // towards zero, ~2e-8 relative), 6 accumulations per k-block.  Forward GEMMs feed ReLU masks and argmaxes, so
-  // they ask for 2 (12 truncations, the level of a sequential fp32 FMA chain); measured cost of draining that
-  // often: +6 % kernel time versus 8.
-  if (getenv("DZ_PK_RUN")) kb.run_kb = atoi(getenv("DZ_PK_RUN"));
-  if (kb.run_kb < 1) kb.run_kb = 4;
+int launch_pgemm(const char* tag, const PkBatch& kb, void* stream, int epi) {
+  if (kb.n <= 0 || kb.n > kPkMaxProblems) return fail(DZ_EINVAL, "pgemm batch size");
   return epi ? launch_pgemm_t<1>(tag, kb, stream) : launch_pgemm_t<0>(tag, kb, stream);
 }
 
@@ -105,7 +98,6 @@ extern "C" int dz_test_tc_pgemm(const float* d_A, int32_t a_rows, int32_t a_ld, 
   PkBatch kb;
   memset(&kb, 0, sizeof(kb));
   kb.n = 1;
-  kb.run_kb = 4;
   PkProblem& p = kb.p[0];
   p.A = PkOperand{a_hi, a_lo, ar / 8};
   p.B = PkOperand{b_hi, b_lo, br / 8};

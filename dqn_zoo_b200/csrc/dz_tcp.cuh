@@ -1,24 +1,21 @@
-// Packed-operand tcgen05 GEMM for the LARGE contractions of the learner (IQN's 3136->512 layer runs at
+// Packed-operand tensor-core GEMM for the LARGE contractions of the learner (IQN's 3136->512 layer runs at
 // M = batch * tau_samples = 2048 rows per network apply; networks.py:264-292, iqn/agent.py:178-214).
 //
 //     D[i,j] = sum_r A(i,r) * B(j,r)        fp32 in, fp32-grade out (error-compensated 3xTF32, see dz_tc.cuh)
 //
-// Unlike dz_tc.cuh (register-path loaders, built for the small implicit-GEMM layers) the hi/lo TF32 split is
-// taken OUT of the GEMM: a bandwidth-bound pack kernel writes each operand once as two "tile images"
-// (hi and lo parts) that are already in the canonical no-swizzle K-major shared-memory layout of the UMMA
-// descriptors, so that the GEMM's producer is ONE thread issuing cp.async.bulk copies (UBLKCP) that complete
-// on an mbarrier, the MMA issuer is one thread, and the remaining warps only drain TMEM.
+// The hi/lo TF32 split is taken OUT of the GEMM: a bandwidth-bound pack kernel writes each operand once as two
+// "tile images" (hi and lo parts) in a shared-memory layout whose m16n8k8 fragment loads are bank-conflict free,
+// so that the GEMM's producer is ONE thread issuing cp.async.bulk copies that complete on an mbarrier and the
+// MMA warps read the stages as they landed.
 //
 // Image layout of an operand with `rows_pad` rows (multiple of the tile height) and `red_pad` reduction
 // elements (multiple of 16), RG = rows_pad / 8:
 //     float index of element (row, r) = (((r / 16) * RG + row / 8) * 4 + (r % 16) / 4) * 32 + (row % 8) * 4 + r % 4
-// i.e. per 16-deep k-block all rows are contiguous, 8-row x 16-byte core matrices, LBO = 128 B (next core
-// matrix along the reduction), SBO = 512 B (next 8 rows).  A (TR rows x 16) tile is TR * 64 contiguous bytes.
+// i.e. per 16-deep k-block all rows are contiguous, 8-row x 16-byte blocks.  A (TR rows x 16) tile is TR * 64
+// contiguous bytes.
 //
-// Accuracy: the tensor core adds into its fp32 accumulator with round-towards-zero (measured: about 2e-8
-// relative per accumulation), so an accumulation run is limited to kRunKB k-blocks (128 reduction elements,
-// 48 MMA accumulations); the epilogue warps drain each finished run from TMEM and add it into registers with
-// ordinary round-to-nearest fp32 adds while the MMA warp already fills the other TMEM buffer.
+// Accuracy: the tensor core adds into its fp32 accumulator with round-towards-zero, so the products of each
+// k-step are added into the fp32 sums with ordinary round-to-nearest adds (dz_tc.cuh, warp_kstep_3xtf32).
 #pragma once
 #include "dz_tc.cuh"
 #include "dz_internal.cuh"
@@ -108,31 +105,24 @@ template <int BNJ, int EPI>
 struct PkSmem {
   static constexpr int kA = 128 * kPkKB * 4, kB = BNJ * kPkKB * 4;     // bytes of one part (hi or lo) of one stage
   static constexpr int kStage = 2 * kA + 2 * kB;
-  static constexpr int kStages = EPI ? 2 : 4;      // EPI 1 (short reduction, epilogue-bound): 2 CTAs per SM
+  static constexpr int kStages = EPI ? 2 : 4;      // EPI 1: short reduction (<= 8 k-blocks)
   static constexpr int kBars = 1024;
   static constexpr int kTotal = kBars + kStages * kStage;
 };
 
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, "
-      "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
+// Byte offset of element (row, r) inside one part of a stage (kPkKB = 16: one k-block, RG = rows / 8 row groups).
+__device__ __forceinline__ uint32_t pk_off(int row, int r) { return (uint32_t)((((row >> 3) * 4 + (r >> 2)) << 7) + ((row & 7) << 4) + ((r & 3) << 2)); }
 
 // grid = (tiles_j, tiles_i * splits, problems); dynamic smem = PkSmem<BNJ, EPI>::kTotal; 320 threads:
-//   warp 0: producer (lane 0 issues the bulk copies)      warp 1: TMEM allocator + MMA issuer
-//   warps 2..9: epilogue (TMEM lane quarter = warp % 4, column half = (warp - 2) / 4)
-// EPI 0: plain output (split partials, or + bias / ReLU), accumulation runs drained into registers.
-// EPI 1: IQN embedding epilogue (networks.py:279-284) for a SHORT reduction (one accumulation run, splits == 1):
+//   warp 0: producer (one lane issues the bulk copies)      warp 1: barrier set-up
+//   warps 2..9: MMA + epilogue, D rows [32 q, 32 q + 32) (q = warp % 4) x columns [BNJ/2 h, BNJ/2 (h + 1)) (h = (warp - 2) / 4)
+// EPI 0: plain output (split partials, or + bias / ReLU).
+// EPI 1: IQN embedding epilogue (networks.py:279-284) for a SHORT reduction (splits == 1):
 //        v = relu(acc + bias[j]) -> e0 (fp32, optional);  h = v * mul[i / mul_div][j] -> written straight as the
 //        hi/lo tile images of the NEXT GEMMs' operands (rows i, and optionally the transposed rows j).
+// The epilogues work on one D row per lane: the fragments are transposed 32 columns at a time through shared memory.
 template <int BNJ, int EPI>
-__global__ void __launch_bounds__(kThreadsP, EPI ? 2 : 1) tc_pgemm_kernel(const __grid_constant__ PkBatch batch) {
+__global__ void __launch_bounds__(kThreadsP, 1) tc_pgemm_kernel(const __grid_constant__ PkBatch batch) {
   dz::pdl_enter();
   extern __shared__ __align__(128) uint8_t smem[];
   using L = PkSmem<BNJ, EPI>;
@@ -145,33 +135,20 @@ __global__ void __launch_bounds__(kThreadsP, EPI ? 2 : 1) tc_pgemm_kernel(const 
   const int per = (p.nkb + p.splits - 1) / p.splits;
   const int kb0 = split * per;
   const int nkb = max(min(p.nkb, kb0 + per) - kb0, 0);
-  const int kRunKB = EPI ? (nkb > 0 ? nkb : 1) : batch.run_kb;   // k-blocks per accumulation run
-  const int nruns = (nkb + kRunKB - 1) / kRunKB;
 
   uint64_t* full = reinterpret_cast<uint64_t*>(smem);      // [ST]  bulk copies landed       (tx-count barrier)
-  uint64_t* empty = full + ST;                              // [ST]  MMAs consumed the stage
-  uint64_t* acc_full = empty + ST;                          // [2]   accumulation run complete in TMEM buffer b
-  uint64_t* acc_empty = acc_full + 2;                       // [2]   epilogue drained TMEM buffer b
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
+  uint64_t* empty = full + ST;                              // [ST]  MMA warps consumed the stage
   uint8_t* stage_base = smem + L::kBars;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int kTmemCols = EPI ? BNJ : 2 * BNJ;            // EPI 0: two accumulator buffers (512 columns)
+  constexpr int kCols = BNJ / 2;                // columns per MMA warp
+  constexpr int NT = kCols / 8;
 
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-      for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], kEpiWarps); }
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  if (warp == 1 && lane == 0) {
+    for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kEpiWarps); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     // ---------------------------------------------------------------- producer
@@ -194,43 +171,45 @@ __global__ void __launch_bounds__(kThreadsP, EPI ? 2 : 1) tc_pgemm_kernel(const 
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer
-    const uint32_t idesc = make_idesc(128, BNJ, 0, 0);
+  } else if (warp >= 2) {
+    // ---------------------------------------------------------------- MMA warps
+    const int ew = warp - 2;
+    const int quarter = warp & 3;
+    const int half = ew >> 2;
+    float acc[2][NT][4];
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[mt][nt][e] = 0.f;
     for (int it = 0; it < nkb; ++it) {
       const int s = it % ST;
-      const uint32_t ph = (uint32_t)(it / ST) & 1u;
-      const int run = it / kRunKB, in_run = it - run * kRunKB;
-      const int buf = run & 1;
-      if (in_run == 0) {
-        mbar_wait(&acc_empty[buf], (((uint32_t)run >> 1) & 1u) ^ 1u);   // buffer drained by the epilogue (free on first use)
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      }
-      mbar_wait(&full[s], ph);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (elect_one()) {   // elect.sync: ptxas emits the MMAs back to back (no ELECT / BRA.U.ANY loop around each)
-        const uint32_t st = smem_u32(stage_base + (size_t)s * L::kStage);
-        const uint32_t a_hi = st, a_lo = st + L::kA, b_hi = st + 2 * L::kA, b_lo = st + 2 * L::kA + L::kB;
-        const uint32_t d = tmem_base + (uint32_t)(buf * BNJ);
+      mbar_wait(&full[s], (uint32_t)(it / ST) & 1u);
+      const uint8_t* st = stage_base + (size_t)s * L::kStage;
 #pragma unroll
-        for (int k = 0; k < kPkKB / 8; ++k) {
-          const uint64_t dah = make_desc(a_hi + k * 256, 128, 512), dal = make_desc(a_lo + k * 256, 128, 512);
-          const uint64_t dbh = make_desc(b_hi + k * 256, 128, 512), dbl = make_desc(b_lo + k * 256, 128, 512);
-          mma_tf32(d, dal, dbh, idesc, (in_run > 0 || k > 0) ? 1u : 0u);   // small cross terms first
-          mma_tf32(d, dah, dbl, idesc, 1u);
-          mma_tf32(d, dah, dbh, idesc, 1u);
-        }
-        mma_commit(&empty[s]);
-        if (in_run == kRunKB - 1 || it == nkb - 1) mma_commit(&acc_full[buf]);
-      }
+      for (int k = 0; k < kPkKB / 8; ++k)
+        warp_kstep_3xtf32<2, NT>(acc, st, st + L::kA, st + 2 * L::kA, st + 2 * L::kA + L::kB, quarter * 32, half * kCols, 8 * k,
+                                 [](int m, int r) { return pk_off(m, r); }, [](int n, int r) { return pk_off(n, r); });
       __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);
     }
-  } else {
-    // ---------------------------------------------------------------- epilogue: drain runs, then write
-    const int ew = warp - 2;
-    const int quarter = warp & 3;                 // TMEM lanes [32*quarter, +32) are the ones this warp may read
-    const int half = ew >> 2;
-    constexpr int kCols = BNJ / 2;                // columns per warp
+    // every MMA warp is done with the stage buffers: they hold the per-warp transposition patches [32 rows][33]
+    asm volatile("bar.sync 1, %0;" ::"n"(kEpiWarps * 32) : "memory");
+    float* patch = reinterpret_cast<float*>(stage_base) + ew * 32 * 33;
+    // r[t] = D[row i0 + 32 quarter + lane][column j0 + half * kCols + c0 + t]
+    auto rows_of = [&](int c0, float (&r)[32]) {
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) patch[frag_row(mt, e) * 33 + frag_col(nt, e)] = acc[mt][c0 / 8 + nt][e];
+      __syncwarp();
+#pragma unroll
+      for (int t = 0; t < 32; ++t) r[t] = patch[lane * 33 + t];
+      __syncwarp();
+    };
     if constexpr (EPI == 1) {
       const int i = i0 + quarter * 32 + lane;
       const bool row_ok = i < p.MI;
@@ -240,21 +219,10 @@ __global__ void __launch_bounds__(kThreadsP, EPI ? 2 : 1) tc_pgemm_kernel(const 
       float* e0 = p.e0 ? p.e0 + (long long)i * p.e0_ld : nullptr;
       float* img_hi = p.img_hi; float* img_lo = p.img_lo; float* imgT_hi = p.imgT_hi; float* imgT_lo = p.imgT_lo;
       const long long rg1 = p.img_rg, rgT = p.imgT_rg;
-      if (nkb > 0) {
-        mbar_wait(&acc_full[0], 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      }
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(half * kCols);
-#pragma unroll 1
-      for (int c0 = 0; c0 < kCols; c0 += 32) {
-        uint32_t r[32];
-        if (nkb > 0) {
-          tmem_ld32(taddr + (uint32_t)c0, r);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        } else {
 #pragma unroll
-          for (int t = 0; t < 32; ++t) r[t] = 0u;
-        }
+      for (int c0 = 0; c0 < kCols; c0 += 32) {
+        float r[32];
+        rows_of(c0, r);
 #pragma unroll
         for (int t = 0; t < 32; t += 4) {
           const int j = j0 + half * kCols + c0 + t;          // NJ % 4 == 0: a group of four is all valid or all invalid
@@ -263,10 +231,10 @@ __global__ void __launch_bounds__(kThreadsP, EPI ? 2 : 1) tc_pgemm_kernel(const 
           if (ok) {
             const float4 b4 = *reinterpret_cast<const float4*>(bias + j);
             float4 v;
-            v.x = fmaxf(__uint_as_float(r[t]) + b4.x, 0.f);
-            v.y = fmaxf(__uint_as_float(r[t + 1]) + b4.y, 0.f);
-            v.z = fmaxf(__uint_as_float(r[t + 2]) + b4.z, 0.f);
-            v.w = fmaxf(__uint_as_float(r[t + 3]) + b4.w, 0.f);
+            v.x = fmaxf(r[t] + b4.x, 0.f);
+            v.y = fmaxf(r[t + 1] + b4.y, 0.f);
+            v.z = fmaxf(r[t + 2] + b4.z, 0.f);
+            v.w = fmaxf(r[t + 3] + b4.w, 0.f);
             if (e0) *reinterpret_cast<float4*>(e0 + j) = v;
             const float4 m4 = *reinterpret_cast<const float4*>(mulrow + j);
             h = make_float4(v.x * m4.x, v.y * m4.y, v.z * m4.z, v.w * m4.w);
@@ -298,28 +266,7 @@ __global__ void __launch_bounds__(kThreadsP, EPI ? 2 : 1) tc_pgemm_kernel(const 
         }
       }
     } else {
-    float sum[kCols];
-#pragma unroll
-    for (int t = 0; t < kCols; ++t) sum[t] = 0.f;
-    for (int run = 0; run < nruns; ++run) {
-      const int buf = run & 1;
-      mbar_wait(&acc_full[buf], ((uint32_t)run >> 1) & 1u);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * BNJ + half * kCols);
-#pragma unroll
-      for (int c0 = 0; c0 < kCols; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(taddr + (uint32_t)c0, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int t = 0; t < 32; ++t) sum[c0 + t] += __uint_as_float(r[t]);
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
-    }
-    const int i = i0 + quarter * 32 + lane;
-    if (i < p.MI) {
+      const int i = i0 + quarter * 32 + lane;
       float* dst = p.C + (long long)split * p.split_stride + (long long)i * p.sc_i;
       const int jb = j0 + half * kCols;
       const bool epi = p.splits == 1;
@@ -328,31 +275,31 @@ __global__ void __launch_bounds__(kThreadsP, EPI ? 2 : 1) tc_pgemm_kernel(const 
       const long long sc_j = p.sc_j;
       const bool v4 = sc_j == 1 && ((reinterpret_cast<uintptr_t>(dst + jb) & 15) == 0) && jb + kCols <= p.NJ;
 #pragma unroll
-      for (int t = 0; t < kCols; t += 4) {
-        float v[4] = {sum[t], sum[t + 1], sum[t + 2], sum[t + 3]};
+      for (int c0 = 0; c0 < kCols; c0 += 32) {
+        float r[32];
+        rows_of(c0, r);
+        if (i >= p.MI) continue;
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int j = jb + t + e;
-          if (bias && j < p.NJ) v[e] += bias[j];
-          if (relu) v[e] = fmaxf(v[e], 0.f);
-        }
-        if (v4) {
-          *reinterpret_cast<float4*>(dst + jb + t) = make_float4(v[0], v[1], v[2], v[3]);
-        } else {
+        for (int t = 0; t < 32; t += 4) {
+          float v[4] = {r[t], r[t + 1], r[t + 2], r[t + 3]};
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
-            const int j = jb + t + e;
-            if (j < p.NJ) dst[(long long)j * sc_j] = v[e];
+            const int j = jb + c0 + t + e;
+            if (bias && j < p.NJ) v[e] += bias[j];
+            if (relu) v[e] = fmaxf(v[e], 0.f);
+          }
+          if (v4) {
+            *reinterpret_cast<float4*>(dst + jb + c0 + t) = make_float4(v[0], v[1], v[2], v[3]);
+          } else {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const int j = jb + c0 + t + e;
+              if (j < p.NJ) dst[(long long)j * sc_j] = v[e];
+            }
           }
         }
       }
     }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
   }
 }
 

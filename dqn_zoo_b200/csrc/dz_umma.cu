@@ -1,4 +1,4 @@
-// Host side of the TMA-fed tcgen05 GEMM family + a C-ABI self test (plain GEMMs through every operand path).
+// Host side of the TMA-fed tensor-core GEMM family + a C-ABI self test (plain GEMMs through every operand path).
 #include <cudaTypedefs.h>
 
 #include "dz_umma_host.cuh"
@@ -20,7 +20,7 @@ PFN_cuTensorMapEncodeTiled_v12000 encode_fn() {
 
 }  // namespace
 
-int UmPlan::add_map(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box, bool mn_major) {
+int UmPlan::add_map(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box) {
   auto fn = encode_fn();
   if (!fn) { fail(DZ_ECUDA, "cuTensorMapEncodeTiled entry point not available"); return -1; }
   cuuint64_t gd[5] = {1, 1, 1, 1, 1};
@@ -43,7 +43,7 @@ int UmPlan::add_map(const void* base, int rank, const uint64_t* dims, const uint
   if (bx[0] * 4 > 128) { fail(DZ_EINVAL, "tensor map: inner box wider than the 128-byte swizzle span"); return -1; }
   CUtensorMap m;
   CUresult rc = fn(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<void*>(base), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   mn_major ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (rc != CUDA_SUCCESS) {
     char buf[256];
     snprintf(buf, sizeof(buf), "cuTensorMapEncodeTiled failed (%d): dims %llu %llu %llu %llu %llu strides %llu %llu %llu %llu box %u %u %u %u %u", (int)rc,
@@ -117,18 +117,11 @@ int UmPlan::launch(const char* tag, const UmLaunch& l, void* stream, long long* 
     const UmProblem& pr = probs[ctas[ci].prob];
     const uint32_t want = pr.B.mn_major ? (uint32_t)(l.njt / 32) * pr.B.lbo : (uint32_t)l.njt * 128u;
     if (pr.A.nparts != 2 || pr.B.nparts != 2 || pr.B.part_bytes != want)
-      return fail(DZ_EINVAL, "umma launch: operands must be hi/lo pairs with the B parts adjacent (one descriptor spans both)");
+      return fail(DZ_EINVAL, "umma launch: operands must be hi/lo pairs and the B tile must span NJT rows");
   }
   for (int ci = l.cta0; ci < l.cta0 + l.nctas; ++ci)
     if (ctas[ci].ops_per_stage > 32) return fail(DZ_EINVAL, "umma launch: more than 32 TMA ops per stage");
-  // two MMA-issuer warps need static slot ownership: stage count a multiple of 2 * run_stages (dz_umma.cuh)
-  int stages = l.stages;
-  {
-    uint32_t rs = 1;
-    for (int ci = l.cta0; ci < l.cta0 + l.nctas; ++ci) rs = std::max(rs, probs[ctas[ci].prob].run_stages);
-    const int rounded = (int)(l.stages / (2 * rs) * (2 * rs));
-    if (rounded >= (int)(2 * rs)) stages = rounded;
-  }
+  const int stages = l.stages;
   const size_t smem = 1024 + um::kCtlBytes + (size_t)stages * l.stage_bytes;
   if (smem > 227 * 1024) return fail(DZ_EINVAL, "umma launch needs too much shared memory");
   if ((size_t)stages * l.stage_bytes < (size_t)128 * l.njt * 4) return fail(DZ_EINVAL, "umma launch: stage buffers smaller than the store-phase staging tile");
@@ -139,10 +132,10 @@ int UmPlan::launch(const char* tag, const UmLaunch& l, void* stream, long long* 
   for (int q = 0; q < l.nmaps; ++q) lm.m[q] = maps[l.map_ids[q]];
   for (int q = l.nmaps; q < um::kMaxMapsPerLaunch; ++q) lm.m[q] = maps[l.map_ids[0]];
   if (v == 0)
-    DZ_LAUNCH_NAMED(tag, um::umma_gemm_kernel<32>, (unsigned)l.nctas, um::kThreadsG, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps, stages,
+    DZ_LAUNCH_NAMED(tag, um::umma_gemm_kernel<32>, (unsigned)l.nctas, um::kThreadsU, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps, stages,
                     l.stage_bytes, d_trace);
   else
-    DZ_LAUNCH_NAMED(tag, um::umma_gemm_kernel<64>, (unsigned)l.nctas, um::kThreadsG, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps, stages,
+    DZ_LAUNCH_NAMED(tag, um::umma_gemm_kernel<64>, (unsigned)l.nctas, um::kThreadsU, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps, stages,
                     l.stage_bytes, d_trace);
   return DZ_OK;
 }
@@ -175,7 +168,7 @@ using namespace dz;
 //                optionally scaled by d_scale_r[r] (applied to A).
 //   epi_rows = 1: UM_EPI_ROWS epilogue (+ d_bias[j], relu, tf32 hi/lo outputs in d_hi / d_lo besides d_C).
 extern "C" int dz_test_umma_gemm(const float* d_A, int32_t a_mn_major, const float* d_B, int32_t b_mn_major, int32_t MI, int32_t NJ,
-                                 int32_t R, int32_t convert, const float* d_scale_r, int32_t run_stages, int32_t epi_rows,
+                                 int32_t R, int32_t convert, const float* d_scale_r, int32_t stages, int32_t epi_rows,
                                  const float* d_bias, int32_t relu, float* d_C, float* d_hi, float* d_lo, void* stream) {
   if (NJ < 4 || NJ > 64 || NJ % 4 || MI % 4 || R % 4) return fail(DZ_EINVAL, "umma self test extents");
   const int njt = NJ <= 32 ? 32 : 64;
@@ -196,7 +189,7 @@ extern "C" int dz_test_umma_gemm(const float* d_A, int32_t a_mn_major, const flo
       uint32_t box[2];
       if (!mn_major) { dims[0] = (uint64_t)R; dims[1] = (uint64_t)rows; strides[0] = (uint64_t)R * 4; box[0] = 32; box[1] = (uint32_t)tile_rows; }
       else { dims[0] = (uint64_t)rows; dims[1] = (uint64_t)R; strides[0] = (uint64_t)rows * 4; box[0] = 32; box[1] = 32; }
-      out[part] = plan.add_map(src[part], 2, dims, strides, box, mn_major != 0);
+      out[part] = plan.add_map(src[part], 2, dims, strides, box);
       if (out[part] < 0) return DZ_EINVAL;
     }
     return DZ_OK;
@@ -210,7 +203,7 @@ extern "C" int dz_test_umma_gemm(const float* d_A, int32_t a_mn_major, const flo
   memset(&p, 0, sizeof(p));
   p.A = a_mn_major ? um_mnmajor(128, 32, convert != 0, convert ? d_scale_r : nullptr) : um_kmajor(128, true, convert != 0, convert ? d_scale_r : nullptr);
   p.B = b_mn_major ? um_mnmajor(njt, 32, convert != 0) : um_kmajor(njt, true, convert != 0);
-  p.ksteps = 4; p.run_stages = run_stages > 0 ? run_stages : 1; p.red_per_stage = 32;
+  p.ksteps = 4; p.red_per_stage = 32;
   p.MI = MI; p.NJ = NJ;
   if (epi_rows) {
     p.epi = UM_EPI_ROWS; p.out_f32 = d_C; p.out_hi = d_hi; p.out_lo = d_lo; p.bias = d_bias; p.relu = relu;
@@ -257,7 +250,7 @@ extern "C" int dz_test_umma_gemm(const float* d_A, int32_t a_mn_major, const flo
   rc = plan.localize_maps(l);
   if (rc == DZ_OK) rc = plan.upload();
   if (rc != DZ_OK) return rc;
-  l.njt = njt; l.stage_bytes = a_bytes + b_bytes; l.stages = 4; l.convert = convert != 0;   // 4 x <= 48 KB + control block fits
+  l.njt = njt; l.stage_bytes = a_bytes + b_bytes; l.stages = stages > 0 ? stages : 4; l.convert = convert != 0;   // 4 x <= 48 KB + control block fits
   rc = plan.launch("umma_selftest", l, stream);
   cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream);
   plan.release();

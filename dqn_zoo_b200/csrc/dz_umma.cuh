@@ -1,9 +1,9 @@
-// TMA-fed tcgen05 GEMM family for the batch-32 learner step (sm_100a): every conv / 512-wide FC contraction of
+// TMA-fed tensor-core GEMM family for the batch-32 learner step (sm_90a): every conv / 512-wide FC contraction of
 // networks.py:181-221 (dqn_torso, dqn_value_head) and :137-178 (noisy_linear), forward and input-gradient, as
 //
 //     D[i, j] = sum_r A(i, r) * B(j, r)          fp32 in, fp32-grade out (error-compensated 3xTF32)
 //
-// Operand tiles live in shared memory in the canonical 128-byte-swizzle UMMA layouts and are delivered by TMA
+// Operand tiles live in shared memory in 128-byte-swizzled layouts and are delivered by TMA
 // (cp.async.bulk.tensor, SWIZZLE_128B tensor maps) straight from the tensors' natural layouts:
 //
 //   K-major  (reduction index contiguous in the source): a stage is [rows][32 r] = rows x 128 B; convolutions get
@@ -11,13 +11,14 @@
 //            activation lands as dense 128-byte rows, negative / out-of-range coordinates are zero-filled by the TMA
 //            unit (that is the zero padding of the input-gradient convolutions).
 //   MN-major (row index contiguous in the source, e.g. W[k][n] for y = xW): a stage is [32 r][32 mn] slabs, LBO
-//            apart; the instruction descriptor's major bit does the transposition — no shuffles, no transposed copies.
+//            apart; the MMA warps' fragment loads do the transposition — no shuffles, no transposed copies.  (This is
+//            why the MMA is the warp-level m16n8k8 one: tf32 wgmma only reads K-major operands from shared memory.)
 //
 // Precision: activations are stored ONCE as tf32 hi/lo pairs by the producing epilogue (x = hi + lo, both exactly
 // representable), fp32 weights are split in place in shared memory by converter warps (raw tile -> hi in place, lo
 // in the sibling buffer; the split is position-wise, so it is swizzle-agnostic), D += Al*Bh + Ah*Bl + Ah*Bh.  The
-// tensor core truncates its fp32 accumulator (measured, dz_tcp.cuh), so accumulation runs are short (run_stages)
-// and are drained into registers with round-to-nearest adds while the next run fills the other TMEM buffer.
+// tensor core truncates its fp32 accumulator, so each k-step's products are added into the fp32 sums with
+// round-to-nearest adds (dz_tc.cuh, warp_kstep_3xtf32).
 //
 // The TMA "program" of every CTA (which boxes of which tensor map go where in each stage) is a table built once on
 // the host (dz_umma.cu): the device side is geometry-free.
@@ -54,7 +55,6 @@ enum : uint32_t { UM_EPI_PARTIAL = 0, UM_EPI_ROWS = 1 };
 struct UmProblem {
   UmOperand A, B;
   uint32_t ksteps;          // MMA k-steps per stage
-  uint32_t run_stages;      // stages per accumulation run
   uint32_t red_per_stage;   // reduction elements per stage
   uint32_t epi;
   int32_t MI, NJ;           // valid extents of D
@@ -93,8 +93,7 @@ using namespace tc;
 
 constexpr int kStagesMax = 8;
 constexpr int kConvWarps = 8;
-constexpr int kThreadsU = (2 + 4 + kConvWarps) * 32;   // producer, mma, 4 epilogue, 8 converter warps (conv1 kernels)
-constexpr int kThreadsG = kThreadsU + 32;              // umma_gemm_kernel: + a second MMA issuer (warp 14)
+constexpr int kThreadsU = (2 + 4 + kConvWarps) * 32;   // producer, barrier set-up, 4 MMA / epilogue, 8 converter warps
 
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
@@ -111,33 +110,6 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
                "l"(__cvta_generic_to_global(src)), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
-}
-
-// 64-bit shared-memory matrix descriptor, SWIZZLE_128B canonical layouts (cute/arch/mma_sm100_desc.hpp):
-//   K-major : rows of 128 B, 8-row groups SBO = 1024 B apart, LBO unused
-//   MN-major: 32-bit operands can only be transposed from the "128B swizzle, 32B atom" layout (SWIZZLE_128B_BASE32B;
-//             measured: plain SWIZZLE_128B / no-swizzle MN-major tf32 descriptors make the MMA return zeros, and CUTLASS
-//             sm100_common.inl says the same): [4 r rows][128 B of mn] atoms, 32-byte chunks XOR-ed with (row & 3) —
-//             the TMA mode CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.  LBO = bytes between atoms along MN, SBO = 512.
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type = 2) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;   // descriptor version (sm_100)
-  d |= (uint64_t)layout_type << 61;   // 2: SWIZZLE_128B, 1: SWIZZLE_128B_BASE32B
-  return d;
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, "
-      "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
 }
 
 __device__ __forceinline__ void split4(const float4 x, float4& h, float4& l) {
@@ -164,8 +136,8 @@ __device__ __forceinline__ void convert_part(const UmOperand& o, uint8_t* part0,
       if (o.mn_major) {          // rows are reduction indices, the 128 bytes of a row are 32 consecutive MN indices
         const int slab = row / rows_per_slab, rr = row - slab * rows_per_slab;
         if (sc) { const float s = sc[r0 + rr]; f.x = s; f.y = s; f.z = s; f.w = s; }
-        if (dual && si) {        // 32-byte atoms XOR-ed with (row & 3): logical 16-byte chunk of this physical one
-          const int cp = idx & 7, cl = ((((cp >> 1) ^ (row & 3)) << 1) | (cp & 1));
+        if (dual && si) {        // 16-byte chunks XOR-ed with (row & 7): logical chunk of this physical one
+          const int cl = (idx & 7) ^ (row & 7);
           const float4 t = *reinterpret_cast<const float4*>(si + i0 + slab * 32 + cl * 4);
           f.x *= t.x; f.y *= t.y; f.z *= t.z; f.w *= t.w;
         }
@@ -200,8 +172,8 @@ __device__ __forceinline__ void convert_hoist(const UmOperand& o, int i0, int i_
     h.si4[j] = make_float4(1.f, 1.f, 1.f, 1.f);
     h.si1[j] = 1.f;
     if (si) {
-      if (o.mn_major) {   // slab j, logical 16-byte chunk cl of the 32-byte-atom swizzle
-        const int cp = ct & 7, row = ct >> 3, cl = ((((cp >> 1) ^ (row & 3)) << 1) | (cp & 1));
+      if (o.mn_major) {   // slab j, logical 16-byte chunk cl of the 128-byte swizzle
+        const int cl = (ct & 7) ^ ((ct >> 3) & 7);
         const int i = min(i0 + j * 32 + cl * 4, i_limit - 4);
         h.si4[j] = *reinterpret_cast<const float4*>(si + i);
       } else {
@@ -257,15 +229,11 @@ __device__ __forceinline__ float4* stage_chunk(uint8_t* base, int r, int c) {
 }
 
 // grid = number of CTA descriptors; dynamic smem = kCtlBytes + stages * stage_bytes + 1024 (alignment slack).
-// Warp roles: 0 TMA producer | 1 and 14 MMA issuers | 2-5 accumulator drain (TMEM lane quarters) | 6-13 operand converters.
-// All twelve warps 2-13 take part in the final store phase (tile staged in shared memory, written out in full rows).
-// The two MMA warps alternate accumulation runs (warp 1: even runs into TMEM buffer 0, warp 14: odd runs into buffer 1):
-// the per-stage barrier waits / fences / commits of one overlap the MMAs of the other.
-// One k-step = TWO instructions: Ah x [Bh | Bl] (N = 2*NJT: hi and lo tiles of B are adjacent in shared memory, so one
-// descriptor spans both; columns [0,NJT) get Ah*Bh, [NJT,2*NJT) get Ah*Bl) and Al x Bh (N = NJT, added into [0,NJT)); the
-// drain adds the two column halves.  Against three N = NJT instructions this reads the A tile twice instead of 3 times.
+// Warp roles: 0 TMA producer | 1 barrier set-up | 2-5 MMA (warp 2 + q owns D rows [32q, 32q + 32), all NJT columns, as
+// m16n8k8 fragments read straight from the staged tiles) | 6-13 operand converters.  All twelve warps 2-13 take part in the
+// final store phase (tile staged in shared memory, written out in full rows).
 template <int NJT>
-__global__ void __launch_bounds__(kThreadsG, 1)
+__global__ void __launch_bounds__(kThreadsU, 1)
     umma_gemm_kernel(const __grid_constant__ UmMaps maps, const UmCta* __restrict__ ctas, const UmProblem* __restrict__ probs,
                      const UmTmaOp* __restrict__ ops, int nmaps, int stages, uint32_t stage_bytes, long long* __restrict__ trace) {
   if (threadIdx.x < nmaps) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&maps.m[threadIdx.x])) : "memory");
@@ -282,10 +250,7 @@ __global__ void __launch_bounds__(kThreadsG, 1)
 
   uint64_t* full = reinterpret_cast<uint64_t*>(smem);      // [ST] TMA landed
   uint64_t* ready = full + kStagesMax;                      // [ST] converters done (only with convert)
-  uint64_t* empty = ready + kStagesMax;                     // [ST] MMAs consumed the stage
-  uint64_t* acc_full = empty + kStagesMax;                  // [2]
-  uint64_t* acc_empty = acc_full + 2;                       // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
+  uint64_t* empty = ready + kStagesMax;                     // [ST] MMA warps consumed the stage
   UmProblem* p_smem = reinterpret_cast<UmProblem*>(smem + 1024);
   UmTmaOp* ops_smem = reinterpret_cast<UmTmaOp*>(smem + 2048);
   uint8_t* stage_base = smem + kCtlBytes;
@@ -293,43 +258,33 @@ __global__ void __launch_bounds__(kThreadsG, 1)
   static_assert(kCtlBytes % 1024 == 0, "stage base must stay 1024-byte aligned");
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int kTmemCols = 4 * NJT;                       // two buffers x (Ah*Bh + Al*Bh | Ah*Bl)
 
   // The CTA's problem and its whole TMA program go to shared memory once (coalesced): the producer's per-stage
   // work is then a shared-memory read, not a dependent global load per stage.
   {
     const uint4* src = reinterpret_cast<const uint4*>(probs + cta.prob);
     uint4* dst = reinterpret_cast<uint4*>(p_smem);
-    for (int i = threadIdx.x; i < (int)(sizeof(UmProblem) / 16); i += kThreadsG) dst[i] = src[i];
+    for (int i = threadIdx.x; i < (int)(sizeof(UmProblem) / 16); i += kThreadsU) dst[i] = src[i];
     const int nvec = min(nst * (int)cta.ops_per_stage, kMaxOpsPerCta) * 2;
     const uint4* osrc = reinterpret_cast<const uint4*>(ops + cta.op0);
     uint4* odst = reinterpret_cast<uint4*>(ops_smem);
-    for (int i = threadIdx.x; i < nvec; i += kThreadsG) odst[i] = osrc[i];
+    for (int i = threadIdx.x; i < nvec; i += kThreadsU) odst[i] = osrc[i];
   }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&ready[s], kConvWarps); mbar_init(&empty[s], 1); }
-      for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], 4); }
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  if (warp == 1 && lane == 0) {
+    for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&ready[s], kConvWarps); mbar_init(&empty[s], 4); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
   // griddepcontrol.wait is executed per role, right before the role's first access to data an earlier kernel may have
-  // produced (the MMA warp touches only shared memory and TMEM and does not need it).
+  // produced.
   const UmProblem& p = *p_smem;
-  const int run_stages = (int)p.run_stages;
-  const int nruns = (nst + run_stages - 1) / run_stages;
   const bool conv_a = p.A.convert != 0, conv_b = p.B.convert != 0;
   const bool any_conv = conv_a || conv_b;
   const uint32_t a_bytes = p.A.part_bytes * p.A.nparts;
-  // stores that stay row-per-lane coalesced (lane = D row, unit stride along i) are written straight from registers
+  // stores that stay coalesced along i (unit stride) are written straight from the MMA fragments
   const bool direct = p.epi == UM_EPI_PARTIAL && p.sc_i == 1;
+  constexpr int NT = NJT / 8;
+  float sum[2][NT][4];
 
   // TMA producers.  Issuing a tensor load costs the issuing warp ~130-300 cycles of operand set-up (shared-memory read of the
   // op, address arithmetic, moves to uniform registers), far more than the TMA unit needs — so the ops of a stage are spread
@@ -363,124 +318,57 @@ __global__ void __launch_bounds__(kThreadsG, 1)
       if (s == ST) { s = 0; ph ^= 1u; st_addr = smem_u32(stage_base); }
     }
   }
-  if (warp == 0) {
-  } else if (warp == 1 || warp == 14) {
-    // ---------------------------------------------------------------- MMA issuers (runs of parity `mw`, TMEM buffer `mw`)
-    // Descriptors: the upper word (SBO, version, layout type) and the LBO field are loop invariants; the start-address
-    // field (bits 0-13, address >> 4 — shared memory is < 256 KB, so sums never carry out of the field) is advanced
-    // with plain adds.
-    const int mw = warp == 1 ? 0 : 1;
-    const uint32_t idesc2 = make_idesc(128, 2 * NJT, (int)p.A.mn_major, (int)p.B.mn_major);
-    const uint32_t idesc1 = make_idesc(128, NJT, (int)p.A.mn_major, (int)p.B.mn_major);
-    const uint32_t a_up = (p.A.mn_major ? (512u >> 4) : (1024u >> 4)) | (1u << 14) | ((p.A.mn_major ? 1u : 2u) << 29);
-    const uint32_t b_up = (p.B.mn_major ? (512u >> 4) : (1024u >> 4)) | (1u << 14) | ((p.B.mn_major ? 1u : 2u) << 29);
-    const uint32_t a_lbo = (((p.A.mn_major ? p.A.lbo : 16u) >> 4) & 0x3FFFu) << 16;
-    const uint32_t b_lbo = (((p.B.mn_major ? p.B.lbo : 16u) >> 4) & 0x3FFFu) << 16;
-    const uint32_t a_stepq = p.A.kstep >> 4, b_stepq = p.B.kstep >> 4;
-    const uint32_t a_pbq = p.A.part_bytes >> 4;
+  if (warp >= 2 && warp < 6) {
+    // ---------------------------------------------------------------- MMA warps
+    const int m0 = (warp - 2) * 32;
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) sum[mt][nt][e] = 0.f;
+    const uint32_t a_lbo = p.A.lbo, b_lbo = p.B.lbo;
+    const bool a_mn = p.A.mn_major != 0, b_mn = p.B.mn_major != 0;
+    auto a_off = [&](int m, int k) { return a_mn ? sw128_mnmajor(m, k, a_lbo) : sw128_kmajor(m, k); };
+    auto b_off = [&](int n, int k) { return b_mn ? sw128_mnmajor(n, k, b_lbo) : sw128_kmajor(n, k); };
     const int ksteps = (int)p.ksteps;
-    const uint32_t stq0 = smem_u32(stage_base) >> 4, stageq = stage_bytes >> 4, a_bytesq = a_bytes >> 4;
-    // Slot ownership must be static for the two-warp scheme (a warp may only revisit slots it consumed itself, otherwise
-    // the 1-bit phase of full[s] could alias when it runs ahead of the other warp): ST a multiple of 2 * run_stages
-    // (UmPlan::launch rounds the stage count down accordingly).  Otherwise warp 1 issues every run and warp 14 idles.
-    const int nw = (ST % (2 * run_stages) == 0) ? 2 : 1;
-    for (int run = mw; run < nruns && mw < nw; run += nw) {
-      const int buf = run & 1;
-      const uint32_t d = tmem_base + (uint32_t)(buf * 2 * NJT);
-      mbar_wait(&acc_empty[buf], (((uint32_t)run >> 1) & 1u) ^ 1u);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      int it = run * run_stages;
-      const int run_end = min(it + run_stages, nst);
-      int s = it % ST;
-      uint32_t ph = (uint32_t)(it / ST) & 1u;
-      for (int in_run = 0; it < run_end; ++it, ++in_run) {
-        mbar_wait(any_conv ? &ready[s] : &full[s], ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (elect_one()) {
-          if (tr && it < 64) trace[64 + it] = clock64();                                           // [64,128): stage data ready
-          const uint32_t stq = stq0 + (uint32_t)s * stageq;
-          uint32_t ah = a_lbo + stq, al = ah + a_pbq;
-          uint32_t bh = b_lbo + stq + a_bytesq;
-          uint32_t acc = in_run > 0 ? 1u : 0u;
-          auto kstep = [&]() {
-            const uint64_t dah = ((uint64_t)a_up << 32) | ah, dal = ((uint64_t)a_up << 32) | al;
-            const uint64_t dbh = ((uint64_t)b_up << 32) | bh;
-            mma_tf32(d, dah, dbh, idesc2, acc);             // [Ah*Bh | Ah*Bl]
-            mma_tf32(d, dal, dbh, idesc1, 1u);              // += Al*Bh
-            acc = 1u;
-            ah += a_stepq; al += a_stepq; bh += b_stepq;
-          };
-          if (ksteps == 4) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) kstep();
-          } else {
-            for (int k = 0; k < ksteps; ++k) kstep();
-          }
-          mma_commit(&empty[s]);
-          if (it == run_end - 1) mma_commit(&acc_full[buf]);
-          if (it == nst - 1) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // the next kernel's set-up overlaps our epilogue
-          if (tr && it < 64) trace[128 + it] = clock64();                                          // [128,192): MMAs issued
-        }
-        __syncwarp();
-        if (++s == ST) { s = 0; ph ^= 1u; }
-      }
-    }
-    if (nst == 0 && mw == 0 && elect_one()) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  } else if (warp < 6) {
-    // ---------------------------------------------------------------- accumulator drain
-    const int quarter = warp & 3;
-    float sum[NJT];
-    dz::pdl_enter();
-    if (p.epi == UM_EPI_ROWS && p.bias != nullptr) {        // the bias is the initial value of the row sums (loaded while the
-      const float* __restrict__ bias = p.bias;              // first accumulation run is still in flight)
-#pragma unroll
-      for (int t = 0; t < NJT; t += 4) {
-        float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (t < p.NJ) b4 = *reinterpret_cast<const float4*>(bias + t);
-        sum[t] = b4.x; sum[t + 1] = b4.y; sum[t + 2] = b4.z; sum[t + 3] = b4.w;
-      }
-    } else {
-#pragma unroll
-      for (int t = 0; t < NJT; ++t) sum[t] = 0.f;
-    }
-    for (int run = 0; run < nruns; ++run) {
-      const int buf = run & 1;
-      mbar_wait(&acc_full[buf], ((uint32_t)run >> 1) & 1u);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (tr && warp == 2 && lane == 0 && run < 64) trace[192 + run] = clock64();                  // [192,256): accumulator ready
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * 2 * NJT);
-#pragma unroll
-      for (int c0 = 0; c0 < 2 * NJT; c0 += 32) {            // columns [0,NJT): Ah*Bh + Al*Bh, [NJT,2*NJT): Ah*Bl
-        uint32_t r[32];
-        tmem_ld32(taddr + (uint32_t)c0, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int t = 0; t < 32; ++t) sum[(c0 % NJT) + t] += __uint_as_float(r[t]);
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    int s = 0;
+    uint32_t ph = 0;
+    for (int it = 0; it < nst; ++it) {
+      mbar_wait(any_conv ? &ready[s] : &full[s], ph);
+      if (tr && warp == 2 && lane == 0 && it < 64) trace[64 + it] = clock64();                     // [64,128): stage data ready
+      const uint8_t* st = stage_base + (size_t)s * stage_bytes;
+      const uint8_t* bh = st + a_bytes;
+      for (int k = 0; k < ksteps; ++k)
+        warp_kstep_3xtf32<2, NT>(sum, st, st + p.A.part_bytes, bh, bh + p.B.part_bytes, m0, 0, 8 * k, a_off, b_off);
       __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
-      if (tr && warp == 2 && lane == 0 && run < 64) trace[256 + run] = clock64();                  // [256,320): run drained
+      if (lane == 0) mbar_arrive(&empty[s]);
+      if (tr && warp == 2 && lane == 0 && it < 64) trace[128 + it] = clock64();                    // [128,192): stage consumed
+      if (++s == ST) { s = 0; ph ^= 1u; }
     }
-    const int r = quarter * 32 + lane;
+    if (warp == 2 && lane == 0) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // the next kernel's set-up overlaps our epilogue
+    dz::pdl_enter();
     if (tr && warp == 2 && lane == 0) trace[320] = clock64();                                       // store phase starts
     if (direct) {
-      const int i = cta.i0 + r;
-      if (i < p.MI) {
-        float* dst = p.C + (long long)cta.split * p.split_stride + i;
-        const float s = p.scale_i ? p.scale_i[i] : 1.0f;
-        const long long sc_j = p.sc_j;
-        const int NJ = p.NJ;
+      float* dst = p.C + (long long)cta.split * p.split_stride;
+      const long long sc_j = p.sc_j;
 #pragma unroll
-        for (int t = 0; t < NJT; ++t)
-          if (t < NJ) dst[(long long)t * sc_j] = sum[t] * s;
-      }
-    } else {
-      // every MMA has completed (last acc_full) and with it every TMA write: the stage buffers are free -> staging tile
+      for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-      for (int c = 0; c < NJT / 4; ++c) *stage_chunk<NJT>(stage_base, r, c) = make_float4(sum[4 * c], sum[4 * c + 1], sum[4 * c + 2], sum[4 * c + 3]);
+        for (int e = 0; e < 4; e += 2) {
+          const int i = cta.i0 + m0 + frag_row(mt, e);
+          if (i >= p.MI) continue;
+          const float sc = p.scale_i ? p.scale_i[i] : 1.0f;
+#pragma unroll
+          for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int j = frag_col(nt, e + h);
+              if (j < p.NJ) dst[i + (long long)j * sc_j] = sum[mt][nt][e + h] * sc;
+            }
+        }
     }
-  } else if (any_conv) {
+  } else if (warp >= 6 && any_conv) {
     // ---------------------------------------------------------------- converter warps: raw fp32 -> hi / lo in place
     const int ct = threadIdx.x - 6 * 32;
     const UmOperand oa = p.A, ob = p.B;
@@ -497,7 +385,7 @@ __global__ void __launch_bounds__(kThreadsG, 1)
       if (fast_a) convert_part16k(oa, st, r0, ct, hoist);
       else if (conv_a) convert_part(oa, st, r0, cta.i0, ct);
       if (conv_b) convert_part(ob, st + a_bytes, r0, 0, ct);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // before the TMA unit refills the slot
       __syncwarp();
       if (lane == 0) mbar_arrive(&ready[s]);
       r0 += red;
@@ -508,6 +396,21 @@ __global__ void __launch_bounds__(kThreadsG, 1)
   if (!direct && warp >= 2 && warp < 14) {
     // ---------------------------------------------------------------- cooperative store phase (warps 2-13, 384 threads)
     if (warp >= 6 && !any_conv) dz::pdl_enter();          // idle converter warps: first access to global data is here
+    // every MMA warp is done reading the stage buffers (and with it every TMA write has landed): they become the staging tile
+    bar_sync_coop();
+    if (warp < 6) {
+      const int m0 = (warp - 2) * 32;
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+          for (int e = 0; e < 4; e += 2) {
+            const int r = m0 + frag_row(mt, e), c = frag_col(nt, e);
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(stage_chunk<NJT>(stage_base, r, c >> 2)) + (c & 3)) =
+                make_float2(sum[mt][nt][e], sum[mt][nt][e + 1]);
+          }
+    }
     bar_sync_coop();
     const int tid = threadIdx.x - 64;
     const int NJ = p.NJ, cpr = NJ >> 2;
@@ -520,6 +423,7 @@ __global__ void __launch_bounds__(kThreadsG, 1)
       const long long ld = p.out_ld;
       const bool relu = p.relu != 0;
       const float* __restrict__ maskp = p.mask;
+      const float* __restrict__ bias = p.bias;
       float* __restrict__ of = p.out_f32; float* __restrict__ oh = p.out_hi; float* __restrict__ ol = p.out_lo;
       const uint32_t inv_pw = pw >= 128 ? 0u : (65536u + (uint32_t)pw - 1u) / (uint32_t)pw;
 #pragma unroll
@@ -531,6 +435,7 @@ __global__ void __launch_bounds__(kThreadsG, 1)
         if (ro >= cta.ph_valid || ri >= cta.pw_valid) continue;
         const long long o = ((long long)cta.row_base + (long long)ro * p.rs_outer + (long long)ri * p.rs_inner) * ld + 4 * c;
         float4 v = *stage_chunk<NJT>(stage_base, r, c);
+        if (bias) { const float4 b4 = *reinterpret_cast<const float4*>(bias + 4 * c); v.x += b4.x; v.y += b4.y; v.z += b4.z; v.w += b4.w; }
         if (relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
         if (maskp) {
           const float4 m4 = *reinterpret_cast<const float4*>(maskp + o);
@@ -565,11 +470,6 @@ __global__ void __launch_bounds__(kThreadsG, 1)
     }
   }
   if (tr && warp == 2 && lane == 0) trace[321] = clock64();                                         // stores issued
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
-  }
   if (tr && threadIdx.x == 0) trace[322] = clock64();
 }
 

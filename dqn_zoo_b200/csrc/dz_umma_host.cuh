@@ -1,4 +1,4 @@
-// Host side of the TMA-fed tcgen05 GEMM family (dz_umma.cuh): tensor-map encoding and the per-launch tables
+// Host side of the TMA-fed tensor-core GEMM family (dz_umma.cuh): tensor-map encoding and the per-launch tables
 // (CTA descriptors, TMA programs).  A UmPlan is built once per learner and replayed every step.
 #pragma once
 #include <vector>
@@ -30,9 +30,8 @@ struct UmPlan {
   UmTmaOp* d_ops = nullptr;
 
   // 5-D fp32 tensor map with SWIZZLE_128B; dims/strides innermost first (strides in BYTES for dims 1..4; dims beyond
-  // `rank` are 1).  mn_major: the tile feeds an MN-major (transposing) descriptor -> 32-byte-atom flavour of the swizzle.
-  // Returns the map index or -1 (error string set).
-  int add_map(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box, bool mn_major = false);
+  // `rank` are 1).  Returns the map index or -1 (error string set).
+  int add_map(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box);
   // Rewrites the `map` field of the ops of launch `l` (ctas [cta0, cta0 + nctas)) from plan indices to launch-local slots.
   int localize_maps(UmLaunch& l);
   int upload();          // (re)allocates and copies all four tables

@@ -1,4 +1,4 @@
-// Torso (conv1-3) and 3136 -> 512 layer(s) of the batch-32 learner step on the TMA-fed tcgen05 kernels.
+// Torso (conv1-3) and 3136 -> 512 layer(s) of the batch-32 learner step on the TMA-fed tensor-core kernels.
 //   networks.py:181-204 dqn_torso, :82-103 conv, :207-221 dqn_value_head, :137-178 noisy_linear, :224-261 rainbow
 // Data flow (all activations are stored once as tf32 hi/lo pairs by the producing epilogue, plus an fp32 copy
 // for the layers that are still on the FMA kernels):
@@ -31,7 +31,7 @@ struct UmNet {
   UmLaunch l_conv2, l_conv3, l_dconv3, l_dconv2, l_fc, l_fcd, l_wconv3, l_wconv2;
   float *wg3_part, *wg2_part, *wg1_part;   // conv3 / conv2 weight-gradient split partials [S][K][64]; conv1: one [256][32] per CTA
   int wg3_splits, wg2_splits, wg1_ctas;
-  int map_g1[2];                           // dact1 hi / lo as a flat [B*h1*w1][32] tensor, 32-byte-atom swizzle
+  int map_g1[2];                           // dact1 hi / lo as a flat [B*h1*w1][32] tensor
   float* wg_scratch;                       // bias-gradient chunk sums [3][kWgMaxChunks][64]
   unsigned int* wg_ticket;                 // [4]
   int conv1_stag_bytes, conv1_tiles_per_pass;
@@ -105,8 +105,8 @@ __global__ void __launch_bounds__(256) um_pack_conv_kernel(const __grid_constant
 // replay.py:718-722 is this kernel's operand load).  Per 128-pixel output tile: one thread bulk-copies the
 // contiguous input rows the tile needs (cp.async.bulk, <= 4 segments) into a double-buffered staging area;
 // eight converter warps expand the bytes to exact tf32 values in the swizzled K-major A tile (K = 256 = 8 kernel
-// rows x 32); one thread issues the MMAs against the resident weight image (hi/lo); four warps drain TMEM,
-// add the bias, ReLU and write act1 as tf32 hi/lo (+ fp32).
+// rows x 32); four MMA warps (32 output pixels each) multiply it with the resident weight image (hi/lo), add the
+// bias, ReLU and write act1 as tf32 hi/lo.
 // ------------------------------------------------------------------------------------------------
 struct Conv1Args {
   CUtensorMap wmap[2][2];          // weight image [blob][hi / lo] (grid-constant: descriptor fetch from the constant bank)
@@ -118,7 +118,7 @@ struct Conv1Args {
   long long* trace;                // debug: clock stamps of CTA 0
 };
 
-constexpr int kC1W = 65536, kC1A = 131072, kC1Epi = 4096;
+constexpr int kC1W = 65536, kC1A = 131072;
 
 __global__ void __launch_bounds__(kThreadsU, 1) conv1_umma_kernel(const __grid_constant__ Conv1Args a) {
   if (threadIdx.x < 4) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&a.wmap[threadIdx.x >> 1][threadIdx.x & 1])) : "memory");
@@ -129,31 +129,19 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_umma_kernel(const __grid_c
   uint64_t* raw_empty = raw_full + 2;                        // [2] converters are done reading them
   uint64_t* w_full = raw_empty + 2;                          // [1] weight image landed (only reloaded when the pass changes)
   uint64_t* a_ready = w_full + 1;                            // [4] kernel-row pair (2j, 2j+1) of the A tile converted
-  uint64_t* a_empty = a_ready + 4;                           // [4] ... consumed by the MMAs
-  uint64_t* acc_full = a_empty + 4;                          // [2]
-  uint64_t* acc_empty = acc_full + 2;                        // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
+  uint64_t* a_empty = a_ready + 4;                           // [4] ... consumed by the four MMA warps
   uint8_t* w_smem = smem + 1024;
   uint8_t* a_smem = w_smem + kC1W;
   uint8_t* stag = a_smem + kC1A;
-  uint8_t* epi_smem = stag + 2 * (size_t)a.stag_bytes;       // 4 x 1 KB transposition patches of the epilogue warps
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int b = 0; b < 2; ++b) { mbar_init(&raw_full[b], 1); mbar_init(&raw_empty[b], kConvWarps); mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], 4); }
-      for (int j = 0; j < 4; ++j) { mbar_init(&a_ready[j], kConvWarps); mbar_init(&a_empty[j], 1); }
-      mbar_init(w_full, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(64) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  if (warp == 1 && lane == 0) {
+    for (int b = 0; b < 2; ++b) { mbar_init(&raw_full[b], 1); mbar_init(&raw_empty[b], kConvWarps); }
+    for (int j = 0; j < 4; ++j) { mbar_init(&a_ready[j], kConvWarps); mbar_init(&a_empty[j], 4); }
+    mbar_init(w_full, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
   dz::pdl_enter();                        // set-up above overlaps the previous kernel's tail; data accesses start here
   const bool tr = a.trace != nullptr && blockIdx.x == 0;
   if (tr && threadIdx.x == 0) { a.trace[323] = clock64(); a.trace[324] = clock64(); }
@@ -206,99 +194,62 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_umma_kernel(const __grid_c
       }
       __syncwarp();
     }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer
-    const uint32_t idesc = make_idesc(128, 32, 0, 0);
+  } else if (warp >= 2 && warp < 6) {
+    // ---------------------------------------------------------------- MMA + epilogue: D rows [32 q, 32 q + 32) of the tile
+    // A (exact tf32 bytes) slab kh = [128 pixels][32 (kw, c)], W slab kh = [32 n][32 (kw, c)] hi | lo, both K-major.
+    const int q = warp - 2, mw0 = q * 32;
+    auto kmaj = [](int mn, int k) { return sw128_kmajor(mn, k); };
     int cur_pass = -1, wn = 0;
     for (int tile = t_begin, n = 0; tile < t_end; ++tile, ++n) {
       const int pass = tile / a.tiles_per_pass;
-      if (pass != cur_pass) { mbar_wait(w_full, (uint32_t)wn & 1u); ++wn; cur_pass = pass; }
-      for (int slab = 0; slab < 8; ++slab) {
-        if ((slab & 1) == 0) mbar_wait(&a_ready[slab >> 1], (uint32_t)n & 1u);
-        const int g = n * 8 + slab, buf = g & 1;
-        mbar_wait(&acc_empty[buf], (((uint32_t)g >> 1) & 1u) ^ 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (elect_one()) {
-          // descriptor words: upper = SBO 1024 | version | SWIZZLE_128B, lower = LBO 16 | address >> 4 (advanced with adds)
-          constexpr uint32_t up = (1024u >> 4) | (1u << 14) | (2u << 29);
-          uint32_t al = (1u << 16) + ((smem_u32(a_smem) + slab * 16384) >> 4);
-          uint32_t wh = (1u << 16) + ((smem_u32(w_smem) + slab * 4096) >> 4), wl = wh + (32768u >> 4);
-          const uint32_t d = tmem_base + (uint32_t)(buf * 32);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t da = ((uint64_t)up << 32) | al;
-            mma_tf32(d, da, ((uint64_t)up << 32) | wl, idesc, k > 0 ? 1u : 0u);
-            mma_tf32(d, da, ((uint64_t)up << 32) | wh, idesc, 1u);
-            al += 2; wh += 2; wl += 2;
-          }
-          mma_commit(&acc_full[buf]);
-          if (slab & 1) mma_commit(&a_empty[slab >> 1]);
-          if (slab == 7 && tile == t_end - 1) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        }
-        __syncwarp();
-      }
-      if (tr && lane == 0 && n < 64) a.trace[128 + n] = clock64();                                  // [128,192): tile's MMAs issued
-    }
-    if (t_begin >= t_end && elect_one()) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  } else if (warp < 6) {
-    // ---------------------------------------------------------------- epilogue
-    const int quarter = warp & 3;
-    for (int tile = t_begin, n = 0; tile < t_end; ++tile, ++n) {
-      const int pass = tile / a.tiles_per_pass;
       const int m0 = (tile - pass * a.tiles_per_pass) * 128, m1 = min(m0 + 128, a.m_pass);
-      float sum[32];
-      {   // the bias is the initial value of the row sums (loaded while the tile's first MMAs are in flight)
+      if (pass != cur_pass) { mbar_wait(w_full, (uint32_t)wn & 1u); ++wn; cur_pass = pass; }
+      float sum[2][4][4];
+      {   // the bias is the initial value of the sums
         const float* __restrict__ bias = a.bias[pass];
 #pragma unroll
-        for (int t = 0; t < 32; t += 4) {
-          const float4 b4 = *reinterpret_cast<const float4*>(bias + t);
-          sum[t] = b4.x; sum[t + 1] = b4.y; sum[t + 2] = b4.z; sum[t + 3] = b4.w;
+        for (int nt = 0; nt < 4; ++nt) {
+          const float2 b2 = *reinterpret_cast<const float2*>(bias + frag_col(nt, 0));
+#pragma unroll
+          for (int mt = 0; mt < 2; ++mt) { sum[mt][nt][0] = b2.x; sum[mt][nt][1] = b2.y; sum[mt][nt][2] = b2.x; sum[mt][nt][3] = b2.y; }
         }
       }
       for (int slab = 0; slab < 8; ++slab) {
-        const int g = n * 8 + slab, buf = g & 1;
-        mbar_wait(&acc_full[buf], ((uint32_t)g >> 1) & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * 32), r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        if ((slab & 1) == 0) mbar_wait(&a_ready[slab >> 1], (uint32_t)n & 1u);
+        const uint8_t* as = a_smem + slab * 16384;
+        const uint8_t* ws = w_smem + slab * 4096;
 #pragma unroll
-        for (int t = 0; t < 32; ++t) sum[t] += __uint_as_float(r[t]);
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[buf]);
-      }
-      if (tr && warp == 2 && lane == 0 && n < 64) a.trace[192 + n] = clock64();                     // [192,256): tile drained
-      // The warp's 32 rows x 32 channels are ONE contiguous 4 KB block of act1: transpose it, 8 channels at a time, through
-      // a private XOR-swizzled 1 KB patch of shared memory (all that is left next to the 128 KB A tile), so that a store
-      // instruction writes 16 rows x 32 contiguous bytes (full sectors) instead of 32 rows x 16 bytes.
-      float4* patch = reinterpret_cast<float4*>(epi_smem + (warp - 2) * 1024);
-      const int mw0 = m0 + quarter * 32;                       // first row of this warp's block
-      const long long dst0 = ((long long)pass * a.m_pass + mw0) * 32;
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-#pragma unroll
-        for (int cc = 0; cc < 2; ++cc) {
-          const int t = q * 8 + cc * 4;
-          patch[lane * 2 + (cc ^ ((lane >> 2) & 1))] = make_float4(fmaxf(sum[t], 0.f), fmaxf(sum[t + 1], 0.f), fmaxf(sum[t + 2], 0.f), fmaxf(sum[t + 3], 0.f));
+        for (int k = 0; k < 4; ++k)
+          warp_kstep_3xtf32<2, 4>(sum, as, nullptr, ws, ws + 32768, mw0, 0, 8 * k, kmaj, kmaj);
+        if (slab & 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&a_empty[slab >> 1]);
         }
-        __syncwarp();
+      }
+      if (q == 0 && lane == 0 && tile == t_end - 1) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+      if (tr && warp == 2 && lane == 0 && n < 64) a.trace[192 + n] = clock64();                     // [192,256): tile's MMAs done
+      // The warp's 32 rows x 32 channels are ONE contiguous 4 KB block of act1; every store instruction writes eight rows
+      // x 32 contiguous bytes (full sectors).
+      const long long dst0 = ((long long)pass * a.m_pass + m0 + mw0) * 32;
 #pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const int row = j * 16 + (lane >> 1), cc = lane & 1;
-          if (mw0 + row < m1) {
-            const float4 v = patch[row * 2 + (cc ^ ((row >> 2) & 1))];
-            float4 h, l;
-            split4(v, h, l);
-            *reinterpret_cast<float4*>(a.out_hi + dst0 + row * 32 + q * 8 + 4 * cc) = h;
-            *reinterpret_cast<float4*>(a.out_lo + dst0 + row * 32 + q * 8 + 4 * cc) = l;
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int e = 0; e < 4; e += 2) {
+          const int row = frag_row(mt, e);
+          if (m0 + mw0 + row >= m1) continue;
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt) {
+            const float v0 = fmaxf(sum[mt][nt][e], 0.f), v1 = fmaxf(sum[mt][nt][e + 1], 0.f);
+            const float h0 = rn_tf32(v0), h1 = rn_tf32(v1);
+            const long long o = dst0 + row * 32 + frag_col(nt, e);
+            *reinterpret_cast<float2*>(a.out_hi + o) = make_float2(h0, h1);
+            *reinterpret_cast<float2*>(a.out_lo + o) = make_float2(rn_tf32(v0 - h0), rn_tf32(v1 - h1));
           }
         }
-        __syncwarp();
-      }
       if (tr && warp == 2 && lane == 0 && n < 64) a.trace[256 + n] = clock64();                     // [256,320): tile stored
     }
-  } else {
+    if (t_begin >= t_end && q == 0 && lane == 0) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  } else if (warp >= 6) {
     // ---------------------------------------------------------------- converters: uint8 rows -> exact tf32 A tile
     const int ct = threadIdx.x - 6 * 32;
     const int r = ct & 127, khp = ct >> 7;
@@ -346,7 +297,6 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_umma_kernel(const __grid_c
           f.w = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7443)) - 8388608.0f;
           *reinterpret_cast<float4*>(dstrow + ((kw ^ (r & 7)) << 4)) = f;
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncwarp();
         if (lane == 0) mbar_arrive(&a_ready[it]);
       }
@@ -354,19 +304,13 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_umma_kernel(const __grid_c
       if (lane == 0) mbar_arrive(&raw_empty[buf]);
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(64) : "memory");
-  }
   if (tr && threadIdx.x == 0) a.trace[322] = clock64();
 }
 
 // ------------------------------------------------------------------------------------------------
 // conv1 weight gradient: dW1[k][n] = (1/255) * sum_m X[m][k] * dact1[m][n], reduction over the B * h1 * w1 output pixels of
-// pass 0.  Same staging as the forward kernel (bulk-copied uint8 rows -> exact tf32 A tile), but the tile is written in
-// the 32-byte-atom swizzle and consumed through MN-major descriptors (rows = reduction index): A^T is never formed.
-// G = dact1 hi/lo arrives by TMA.  Two accumulators (k 0..127 | 128..255) x two TMEM buffers; one partial per CTA.
+// pass 0.  Same staging as the forward kernel (bulk-copied uint8 rows -> exact tf32 A tile); the MMA warps read the tile
+// MN-major (rows = reduction index): A^T is never formed.  G = dact1 hi/lo arrives by TMA.  One partial per CTA.
 // ------------------------------------------------------------------------------------------------
 struct Conv1WgArgs {
   CUtensorMap gmap[2];             // dact1 hi / lo
@@ -387,29 +331,18 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_wgrad_umma_kernel(const __
   uint64_t* g_full = raw_empty + 2;                          // [1] dact1 tile landed
   uint64_t* a_ready = g_full + 1;                            // [4] kernel-row pairs converted
   uint64_t* t_done = a_ready + 4;                            // [1] all MMAs of the tile done (A and G tiles free)
-  uint64_t* acc_full = t_done + 1;                           // [2]
-  uint64_t* acc_empty = acc_full + 2;                        // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
   uint8_t* g_smem = smem + 1024;
   uint8_t* a_smem = g_smem + kC1G;
   uint8_t* stag = a_smem + kC1A;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int b = 0; b < 2; ++b) { mbar_init(&raw_full[b], 1); mbar_init(&raw_empty[b], kConvWarps); mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], 4); }
-      for (int j = 0; j < 4; ++j) mbar_init(&a_ready[j], kConvWarps);
-      mbar_init(g_full, 1); mbar_init(t_done, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(128) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  if (warp == 1 && lane == 0) {
+    for (int b = 0; b < 2; ++b) { mbar_init(&raw_full[b], 1); mbar_init(&raw_empty[b], kConvWarps); }
+    for (int j = 0; j < 4; ++j) mbar_init(&a_ready[j], kConvWarps);
+    mbar_init(g_full, 1); mbar_init(t_done, 4);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
   dz::pdl_enter();                        // set-up above overlaps the previous kernel's tail; data accesses start here
 
   const int px = a.oh * a.ow;
@@ -450,69 +383,50 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_wgrad_umma_kernel(const __
       }
       __syncwarp();
     }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer
-    const uint32_t idesc = make_idesc(128, 32, 1, 1);     // both operands MN-major (rows of the tiles are the reduction)
+  } else if (warp >= 2 && warp < 6) {
+    // ---------------------------------------------------------------- MMA warps: rows k = 128 mt + 32 q + [0, 32) of dW1
+    // Both tiles are read MN-major (their rows are the reduction index m): A^T from the [8 kh][128 m][32 (kw, c)] tile,
+    // G from [128 m][32 n] hi | lo.
+    const int q = warp - 2;
+    float sum[2][2][4][4];
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) sum[mt][i][nt][e] = 0.f;
+    auto a_off = [](int kk, int m) { return sw128_mnmajor(kk, m, 16384u); };
+    auto g_off = [](int nn, int m) { return sw128_mnmajor(nn, m, 0u); };
     for (int tile = t_begin, n = 0; tile < t_end; ++tile, ++n) {
       mbar_wait(g_full, (uint32_t)n & 1u);
+#pragma unroll
       for (int mt = 0; mt < 2; ++mt) {                      // k 0..127 (kernel rows 0-3) | k 128..255 (kernel rows 4-7)
         mbar_wait(&a_ready[2 * mt], (uint32_t)n & 1u);
         mbar_wait(&a_ready[2 * mt + 1], (uint32_t)n & 1u);
-        const int g = n * 2 + mt, buf = g & 1;
-        mbar_wait(&acc_empty[buf], (((uint32_t)g >> 1) & 1u) ^ 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (elect_one()) {
-          // descriptor words: upper = SBO 512 | version | 32-byte-atom swizzle, lower = LBO 16384 | address >> 4
-          constexpr uint32_t up = (512u >> 4) | (1u << 14) | (1u << 29);
-          constexpr uint32_t lbo = (16384u >> 4) << 16;
-          uint32_t al = lbo + ((smem_u32(a_smem) + mt * 4 * 16384) >> 4);
-          uint32_t gh = lbo + (smem_u32(g_smem) >> 4), gl = gh + (16384u >> 4);
-          const uint32_t d = tmem_base + (uint32_t)(buf * 64 + mt * 32);
 #pragma unroll 4
-          for (int k = 0; k < 16; ++k) {
-            const uint64_t da = ((uint64_t)up << 32) | al;
-            mma_tf32(d, da, ((uint64_t)up << 32) | gl, idesc, k > 0 ? 1u : 0u);
-            mma_tf32(d, da, ((uint64_t)up << 32) | gh, idesc, 1u);
-            al += 64; gh += 64; gl += 64;
-          }
-          mma_commit(&acc_full[buf]);
-          if (mt == 1) mma_commit(t_done);
-          if (mt == 1 && tile == t_end - 1) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-        }
-        __syncwarp();
+        for (int k = 0; k < 16; ++k)
+          warp_kstep_3xtf32<2, 4>(sum[mt], a_smem, nullptr, g_smem, g_smem + 16384, mt * 128 + q * 32, 0, 8 * k, a_off, g_off);
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(t_done);
+      if (q == 0 && lane == 0 && tile == t_end - 1) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     }
-  } else if (warp < 6) {
-    // ---------------------------------------------------------------- epilogue: rows k of both accumulators
-    const int quarter = warp & 3;
-    float sum[2][32];
-#pragma unroll
-    for (int t = 0; t < 32; ++t) { sum[0][t] = 0.f; sum[1][t] = 0.f; }
-    for (int tile = t_begin, n = 0; tile < t_end; ++tile, ++n) {
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt) {
-        const int g = n * 2 + mt, buf = g & 1;
-        mbar_wait(&acc_full[buf], ((uint32_t)g >> 1) & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        uint32_t r[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * 64 + mt * 32), r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int t = 0; t < 32; ++t) sum[mt][t] += __uint_as_float(r[t]);
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[buf]);
-      }
-    }
+    if (t_begin >= t_end && q == 0 && lane == 0) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const float inv255 = 0.0039215688593685627f;
 #pragma unroll
-    for (int mt = 0; mt < 2; ++mt) {
-      float* dst = a.partial + ((long long)blockIdx.x * 256 + mt * 128 + quarter * 32 + lane) * 32;
+    for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-      for (int t = 0; t < 32; t += 4)
-        *reinterpret_cast<float4*>(dst + t) = make_float4(sum[mt][t] * inv255, sum[mt][t + 1] * inv255, sum[mt][t + 2] * inv255, sum[mt][t + 3] * inv255);
-    }
-  } else {
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; e += 2) {
+          float* dst = a.partial + ((long long)blockIdx.x * 256 + mt * 128 + q * 32 + frag_row(i, e)) * 32;
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt)
+            *reinterpret_cast<float2*>(dst + frag_col(nt, e)) = make_float2(sum[mt][i][nt][e] * inv255, sum[mt][i][nt][e + 1] * inv255);
+        }
+  } else if (warp >= 6) {
     // ---------------------------------------------------------------- converters
     const int ct = threadIdx.x - 6 * 32;
     const int r = ct & 127, khp = ct >> 7;
@@ -554,21 +468,14 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_wgrad_umma_kernel(const __
           f.y = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7441)) - 8388608.0f;
           f.z = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7442)) - 8388608.0f;
           f.w = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7443)) - 8388608.0f;
-          // 128B swizzle with 32-byte atoms: the 32-byte chunk index is XOR-ed with (row & 3)
-          *reinterpret_cast<float4*>(dstrow + ((((kw >> 1) ^ (r & 3)) << 5) | ((kw & 1) << 4))) = f;
+          *reinterpret_cast<float4*>(dstrow + ((kw ^ (r & 7)) << 4)) = f;
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncwarp();
         if (lane == 0) mbar_arrive(&a_ready[it]);
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&raw_empty[buf]);
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(128) : "memory");
   }
 }
 
@@ -636,7 +543,7 @@ __global__ void __launch_bounds__(256) um_fcd_finish_kernel(const float* __restr
 // finish adds the chunk sums in chunk order.  One launch covers several layers: blockIdx.y = layer; blocks
 // [0, kWgSumBlocks) add the partials, blocks beyond do the bias chunks.
 // Partial sums: a block owns 32 consecutive float4 columns; its 8 thread groups stride over the S partials (so the
-// up-to-148 loads of one column are 8 independent chains instead of one dependent chain), then group sums are added in
+// up-to-132 loads of one column are 8 independent chains instead of one dependent chain), then group sums are added in
 // group order through shared memory — a fixed association, hence bit-deterministic.
 constexpr int kWgChunkRows = 128, kWgMaxChunks = 256, kWgGroups = 8;
 // norm_part: this layer's slots of the split global gradient norm: [0, sum_blocks) = sum of squares of the dW values each
@@ -765,7 +672,7 @@ bool um_net_supported(const UmNetDesc& d) {
     }
     worst = std::max(worst, tot);
   }
-  if (2 * ((worst + 127) / 128 * 128) + 2048 + 65536 + 131072 + 4096 > 227 * 1024) return false;
+  if (2 * ((worst + 127) / 128 * 128) + 2048 + 65536 + 131072 > 227 * 1024) return false;
   return true;
 }
 
@@ -791,7 +698,7 @@ struct Carver {
   }
 };
 
-int fc_splits_for(int nprob, int nk) { return std::max(1, std::min(std::min(148 / (nprob * 4), 24), nk)); }
+int fc_splits_for(int nprob, int nk) { return std::max(1, std::min(std::min(kNumSMs / (nprob * 4), 24), nk)); }
 
 int64_t carve_net(UmNet* n, char* base) {
   const UmNetDesc& d = n->d;
@@ -810,12 +717,12 @@ int64_t carve_net(UmNet* n, char* base) {
   n->wd2_hi = c.f(128 * 256); n->wd2_lo = c.f(128 * 256);
   {
     const int groups = (d.B + 7) / 8;
-    n->wg3_splits = std::max(1, std::min(g.h3, 148 / 5));             // stages = h3 * groups, split over the output rows
-    n->wg2_splits = std::max(1, std::min(g.h2, 148 / 8));
+    n->wg3_splits = std::max(1, std::min(g.h3, kNumSMs / 5));             // stages = h3 * groups, split over the output rows
+    n->wg2_splits = std::max(1, std::min(g.h2, kNumSMs / 8));
     (void)groups;
     n->wg3_part = c.f((int64_t)n->wg3_splits * 576 * 64);
     n->wg2_part = c.f((int64_t)n->wg2_splits * 512 * 64);
-    n->wg1_ctas = std::min(148, (d.B * g.h1 * g.w1 + 127) / 128);
+    n->wg1_ctas = std::min(kNumSMs, (d.B * g.h1 * g.w1 + 127) / 128);
     n->wg1_part = c.f((int64_t)n->wg1_ctas * 256 * 32);
     n->wg_scratch = c.f(3 * 256 * 64);
     n->wg_ticket = reinterpret_cast<unsigned int*>(c.f(64));
@@ -827,7 +734,7 @@ int64_t carve_net(UmNet* n, char* base) {
     n->fcd_nsrc = d.nstream;
     n->fc_splits = fc_splits_for(n->fc_nprob, g.feat / 32);
     const int ktiles = (g.feat + 127) / 128;
-    n->fcd_splits = std::max(1, std::min(148 / (n->fcd_nsrc * ktiles), 8));
+    n->fcd_splits = std::max(1, std::min(kNumSMs / (n->fcd_nsrc * ktiles), 8));
     n->h1_buf = c.f((int64_t)d.npass * d.nstream * d.B * 512);
     n->dh1_f32 = c.f((int64_t)d.nstream * d.B * 512);
     n->dh1_hi = c.f((int64_t)d.nstream * d.B * 512);
@@ -886,7 +793,7 @@ int build_plan(UmNet* n) {
       const int blob = d.pass_target[p] ? 1 : 0;
       UmProblem pr;
       memset(&pr, 0, sizeof(pr));
-      pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.run_stages = 1; pr.red_per_stage = 32; pr.epi = UM_EPI_ROWS;
+      pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32; pr.epi = UM_EPI_ROWS;
       pr.MI = rows; pr.NJ = 64;
       pr.out_hi = n->act_hi[1]; pr.out_lo = n->act_lo[1]; pr.out_f32 = nullptr; pr.out_ld = 64;
       pr.bias = (blob ? d.target : d.online) + d.off_conv_b[1]; pr.relu = 1;
@@ -934,7 +841,7 @@ int build_plan(UmNet* n) {
       for (int half = 0; half < 2; ++half) {
         UmProblem pr;
         memset(&pr, 0, sizeof(pr));
-        pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.run_stages = 1; pr.red_per_stage = 32; pr.epi = UM_EPI_ROWS;
+        pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32; pr.epi = UM_EPI_ROWS;
         pr.MI = rows; pr.NJ = 32;
         pr.out_hi = n->act_hi[2] + 32 * half; pr.out_lo = n->act_lo[2] + 32 * half; pr.out_f32 = n->act_f32[2] + 32 * half;
         pr.out_ld = 64;
@@ -988,7 +895,7 @@ int build_plan(UmNet* n) {
     for (int half = 0; half < 2; ++half) {
       UmProblem pr;
       memset(&pr, 0, sizeof(pr));
-      pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.run_stages = 2; pr.red_per_stage = 32; pr.epi = UM_EPI_ROWS;
+      pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32; pr.epi = UM_EPI_ROWS;
       pr.MI = rows; pr.NJ = 32;
       pr.out_hi = n->dact_hi[1] + 32 * half; pr.out_lo = n->dact_lo[1] + 32 * half; pr.out_f32 = n->dact_f32[1] + 32 * half;
       pr.out_ld = 64;
@@ -1040,7 +947,7 @@ int build_plan(UmNet* n) {
     n->l_dconv2.stages = std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_dconv2.stage_bytes));
     UmProblem pr;
     memset(&pr, 0, sizeof(pr));
-    pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.run_stages = 2; pr.red_per_stage = 32; pr.epi = UM_EPI_ROWS;
+    pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32; pr.epi = UM_EPI_ROWS;
     pr.MI = rows; pr.NJ = 32;
     pr.out_hi = n->dact_hi[0]; pr.out_lo = n->dact_lo[0]; pr.out_f32 = n->dact_f32[0]; pr.out_ld = 32;
     pr.mask = n->act_hi[0];
@@ -1070,7 +977,7 @@ int build_plan(UmNet* n) {
   for (int part = 0; part < 2; ++part) {   // conv1 weight gradient: G operand
     uint64_t dims[2] = {32, (uint64_t)B * h1 * w1}, strides[1] = {128};
     uint32_t box[2] = {32, 128};
-    n->map_g1[part] = pl.add_map(part ? n->dact_lo[0] : n->dact_hi[0], 2, dims, strides, box, true);
+    n->map_g1[part] = pl.add_map(part ? n->dact_lo[0] : n->dact_hi[0], 2, dims, strides, box);
     if (n->map_g1[part] < 0) return DZ_EINVAL;
   }
   // =========================================================================== conv3 / conv2 weight gradients
@@ -1085,10 +992,10 @@ int build_plan(UmNet* n) {
         uint64_t dims[4] = {64, (uint64_t)w2, (uint64_t)h2, (uint64_t)PB};
         uint64_t strides[3] = {256, (uint64_t)w2 * 256, (uint64_t)h2 * w2 * 256};
         uint32_t box[4] = {32, (uint32_t)w3, 1, 8};
-        m_a[part] = pl.add_map(part ? n->act_lo[1] : n->act_hi[1], 4, dims, strides, box, true);
+        m_a[part] = pl.add_map(part ? n->act_lo[1] : n->act_hi[1], 4, dims, strides, box);
         uint64_t gd[4] = {64, (uint64_t)w3, (uint64_t)h3, (uint64_t)B};
         uint64_t gs[3] = {256, (uint64_t)w3 * 256, (uint64_t)h3 * w3 * 256};
-        m_g[part] = pl.add_map(part ? n->dact_lo[2] : n->dact_hi[2], 4, gd, gs, box, true);
+        m_g[part] = pl.add_map(part ? n->dact_lo[2] : n->dact_hi[2], 4, gd, gs, box);
         if (m_a[part] < 0 || m_g[part] < 0) return DZ_EINVAL;
       }
       const int rows = w3 * 8;                                  // reduction rows per stage (multiple of 8)
@@ -1099,7 +1006,7 @@ int build_plan(UmNet* n) {
       n->l_wconv3.stages = std::max(1, std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_wconv3.stage_bytes)));
       UmProblem pr;
       memset(&pr, 0, sizeof(pr));
-      pr.A = A; pr.B = Bo; pr.ksteps = (uint32_t)(rows / 8); pr.run_stages = 1; pr.red_per_stage = (uint32_t)rows;
+      pr.A = A; pr.B = Bo; pr.ksteps = (uint32_t)(rows / 8); pr.red_per_stage = (uint32_t)rows;
       pr.epi = UM_EPI_PARTIAL; pr.MI = 576; pr.NJ = 64;
       pr.C = n->wg3_part; pr.sc_i = 64; pr.sc_j = 1; pr.split_stride = 576 * 64;
       const int prob = (int)pl.probs.size();
@@ -1137,11 +1044,11 @@ int build_plan(UmNet* n) {
         uint64_t dims[5] = {64, (uint64_t)w1 / 2, 2, (uint64_t)h1 / 2, (uint64_t)PB};
         uint64_t strides[4] = {256, (uint64_t)w1 * 128, (uint64_t)2 * w1 * 128, (uint64_t)h1 * w1 * 128};
         uint32_t box[5] = {32, (uint32_t)w2, 1, 1, 8};
-        m_a[part] = pl.add_map(part ? n->act_lo[0] : n->act_hi[0], 5, dims, strides, box, true);
+        m_a[part] = pl.add_map(part ? n->act_lo[0] : n->act_hi[0], 5, dims, strides, box);
         uint64_t gd[4] = {64, (uint64_t)w2, (uint64_t)h2, (uint64_t)B};
         uint64_t gs[3] = {256, (uint64_t)w2 * 256, (uint64_t)h2 * w2 * 256};
         uint32_t gbox[4] = {32, (uint32_t)w2, 1, 8};
-        m_g[part] = pl.add_map(part ? n->dact_lo[1] : n->dact_hi[1], 4, gd, gs, gbox, true);
+        m_g[part] = pl.add_map(part ? n->dact_lo[1] : n->dact_hi[1], 4, gd, gs, gbox);
         if (m_a[part] < 0 || m_g[part] < 0) return DZ_EINVAL;
       }
       const int rows = w2 * 8;
@@ -1154,7 +1061,7 @@ int build_plan(UmNet* n) {
       for (int half = 0; half < 2; ++half) {
         UmProblem pr;
         memset(&pr, 0, sizeof(pr));
-        pr.A = A; pr.B = Bo; pr.ksteps = (uint32_t)(rows / 8); pr.run_stages = 1; pr.red_per_stage = (uint32_t)rows;
+        pr.A = A; pr.B = Bo; pr.ksteps = (uint32_t)(rows / 8); pr.red_per_stage = (uint32_t)rows;
         pr.epi = UM_EPI_PARTIAL; pr.MI = 512; pr.NJ = 32;
         pr.C = n->wg2_part + 32 * half; pr.sc_i = 64; pr.sc_j = 1; pr.split_stride = 512 * 64;
         const int prob = (int)pl.probs.size();
@@ -1213,13 +1120,13 @@ int build_plan(UmNet* n) {
           uint64_t dims3[3] = {32, (uint64_t)feat, 16}, strides3[2] = {2048, 128};
           uint32_t box3[3] = {32, 32, 4};
           if (wf3d) {
-            m_wf_fc[blob][s][sg] = pl.add_map(w, 3, dims3, strides3, box3, true);
+            m_wf_fc[blob][s][sg] = pl.add_map(w, 3, dims3, strides3, box3);
             if (m_wf_fc[blob][s][sg] < 0) wf3d = false;      // driver refused the permuted view: one op per slab instead
           }
           if (!wf3d) {
             if (blob || s || sg) return fail(DZ_EINVAL, "fc weight tensor maps: inconsistent encodings");
             uint32_t box2[2] = {32, 32};
-            m_wf_fc[blob][s][sg] = pl.add_map(w, 2, dims, strides, box2, true);
+            m_wf_fc[blob][s][sg] = pl.add_map(w, 2, dims, strides, box2);
           }
           if (m_wf_fc[blob][s][sg] < 0) return DZ_EINVAL;
           if (blob == 0) {
@@ -1241,7 +1148,7 @@ int build_plan(UmNet* n) {
           const int qi = p * d.nstream + s;
           UmProblem pr;
           memset(&pr, 0, sizeof(pr));
-          pr.A = um_mnmajor(128, 32, true, nullptr); pr.B = Bo; pr.ksteps = 4; pr.run_stages = 1; pr.red_per_stage = 32;
+          pr.A = um_mnmajor(128, 32, true, nullptr); pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32;
           if (d.noisy) pr.A.convert = 2;
           pr.epi = UM_EPI_PARTIAL; pr.MI = 512; pr.NJ = B;
           pr.C = n->fc_part + (int64_t)qi * S * B * 512; pr.sc_i = 1; pr.sc_j = 512; pr.split_stride = (long long)B * 512;
@@ -1285,7 +1192,7 @@ int build_plan(UmNet* n) {
       for (int s = 0; s < d.nstream; ++s) {
         UmProblem pr;
         memset(&pr, 0, sizeof(pr));
-        pr.A = um_kmajor(128, true, true, nullptr); pr.B = Bo; pr.ksteps = 4; pr.run_stages = 2; pr.red_per_stage = 32;
+        pr.A = um_kmajor(128, true, true, nullptr); pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32;
         if (d.noisy) pr.A.convert = 2;
         pr.epi = UM_EPI_PARTIAL; pr.MI = feat; pr.NJ = B;
         pr.C = n->fcd_part + (int64_t)s * S * B * feat; pr.sc_i = 1; pr.sc_j = feat; pr.split_stride = (long long)B * feat;
@@ -1343,7 +1250,7 @@ int64_t um_net_workspace_bytes(const UmNetDesc& d) {
 }
 
 int um_net_create(const UmNetDesc& d, char* base, UmNet** out) {
-  if (!um_net_supported(d)) return fail(DZ_EINVAL, "geometry not supported by the tcgen05 path");
+  if (!um_net_supported(d)) return fail(DZ_EINVAL, "geometry not supported by the tensor-core path");
   UmNet* n = new UmNet();
   n->d = d;
   carve_net(n, base);
@@ -1432,7 +1339,7 @@ int um_prefetch_fc(UmNet* n, void* stream) {
         a.ptr[a.n] = (blob ? d.target : d.online) + (sg ? d.off_fc_sw[s] : d.off_fc_w[s]);
         a.lines[a.n++] = lines;
       }
-  DZ_LAUNCH_NAMED("fc_prefetch", um_prefetch_kernel, 148 * 4, 256, 0, stream, a);
+  DZ_LAUNCH_NAMED("fc_prefetch", um_prefetch_kernel, kNumSMs * 4, 256, 0, stream, a);
   return DZ_OK;
 }
 
@@ -1452,9 +1359,9 @@ int um_forward_torso(UmNet* n, const uint8_t* const* const* rows, void* stream) 
   a.npass = d.npass; a.B = d.B; a.W = d.W; a.oh = n->h1; a.ow = n->w1; a.m_pass = d.B * n->h1 * n->w1;
   a.tiles_per_pass = n->conv1_tiles_per_pass; a.ntiles = a.tiles_per_pass * d.npass; a.stag_bytes = n->conv1_stag_bytes;
   a.trace = n->tr("conv1_fwd");
-  const size_t smem = 2048 + kC1W + kC1A + 2 * (size_t)a.stag_bytes + kC1Epi;
+  const size_t smem = 2048 + kC1W + kC1A + 2 * (size_t)a.stag_bytes;
   if (smem > 227 * 1024) return fail(DZ_EINVAL, "conv1 staging does not fit");
-  const unsigned grid = (unsigned)std::min(148, a.ntiles);
+  const unsigned grid = (unsigned)std::min(kNumSMs, a.ntiles);
   DZ_LAUNCH_NAMED("conv1_fwd", conv1_umma_kernel, grid, kThreadsU, smem, stream, a);
   DZ_TRY_RC(n->plan.launch("conv2_fwd", n->l_conv2, stream, n->tr("conv2_fwd")));
   DZ_TRY_RC(n->plan.launch("conv3_fwd", n->l_conv3, stream, n->tr("conv3_fwd")));
@@ -1463,7 +1370,7 @@ int um_forward_torso(UmNet* n, const uint8_t* const* const* rows, void* stream) 
 
 int um_forward_fc(UmNet* n, const float* noise, void* stream) {
   const UmNetDesc& d = n->d;
-  if (!d.use_fc) return fail(DZ_EINVAL, "fc layers are not on the tcgen05 path for this agent");
+  if (!d.use_fc) return fail(DZ_EINVAL, "fc layers are not on the tensor-core path for this agent");
   if (d.noisy) DZ_TRY_RC(apply_noise(n, noise, stream));
   DZ_TRY_RC(n->plan.launch(d.noisy ? "noisy1_fwd" : "fc1_fwd", n->l_fc, stream, n->tr("fc1_fwd")));
   FcFinishArgs a;
@@ -1489,11 +1396,11 @@ int um_split_dh1(UmNet* n, void* stream) {
 
 int um_backward_fc(UmNet* n, const float* noise, void* stream) {
   const UmNetDesc& d = n->d;
-  if (!d.use_fc) return fail(DZ_EINVAL, "fc layers are not on the tcgen05 path for this agent");
+  if (!d.use_fc) return fail(DZ_EINVAL, "fc layers are not on the tensor-core path for this agent");
   if (d.noisy) DZ_TRY_RC(apply_noise(n, noise, stream));
   DZ_TRY_RC(n->plan.launch(d.noisy ? "noisy1_dgrad" : "fc1_dgrad", n->l_fcd, stream, n->tr("fc1_dgrad")));
   const long long total = (long long)d.B * n->feat;
-  DZ_LAUNCH_NAMED("fcd_finish", um_fcd_finish_kernel, (unsigned)std::min<long long>(ceil_div(total / 4, 256), 148 * 4), 256, 0, stream,
+  DZ_LAUNCH_NAMED("fcd_finish", um_fcd_finish_kernel, (unsigned)std::min<long long>(ceil_div(total / 4, 256), kNumSMs * 4), 256, 0, stream,
                   n->fcd_part, n->fcd_nsrc * n->fcd_splits, total, n->act_hi[2], n->dact_f32[2], n->dact_hi[2], n->dact_lo[2], total / 4);
   return DZ_OK;
 }

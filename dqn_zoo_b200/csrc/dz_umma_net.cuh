@@ -1,4 +1,4 @@
-// The batch-32 learner step's torso and 512-wide FC layer on the TMA-fed tcgen05 kernels (dz_umma.cuh):
+// The batch-32 learner step's torso and 512-wide FC layer on the TMA-fed tensor-core kernels (dz_umma.cuh):
 // interface between dz_learner.cu and dz_umma_net.cu.  networks.py:181-204 (dqn_torso), :207-221 (dqn_value_head),
 // :137-178 (noisy_linear), :224-261 (rainbow streams).
 #pragma once

@@ -1,5 +1,5 @@
 /*
- * dqn_zoo_b200 — C ABI of the B200-native replay-sampler + learner-update hot path.
+ * dqn_zoo_b200 — C ABI of the H100-native replay-sampler + learner-update hot path.
  *
  * The reference (google-deepmind/dqn_zoo) has no FFI layer: its extension point is the
  * duck-typed Python surface `parts.Agent` / `replay.*` (SURVEY.md §8(b)).  This header is
@@ -34,7 +34,7 @@ extern "C" {
 #define DZ_ESTATE (-4)   /* device-side sticky error flag was raised by a previous kernel */
 
 const char* dz_last_error(void);
-/* "dqn_zoo_b200 <version> sm_100a <build date>"; also proves the library loaded. */
+/* "dqn_zoo_b200 <version> sm_90a <build date>"; also proves the library loaded. */
 const char* dz_build_info(void);
 /* Number of kernels this library has launched in this process (bench.py `gpu_launches`). */
 int64_t dz_launch_count(void);
@@ -305,7 +305,7 @@ int dz_learner_sync_target(dz_learner* l, void* stream);
 int dz_test_u8_to_unit(float* d_out256, void* stream);
 
 
-/* Self-test of the packed-operand tcgen05 GEMM (csrc/dz_tcp.cuh; the IQN 3136->512 layer's kernels): packs
+/* Self-test of the packed-operand tensor-core GEMM (csrc/dz_tcp.cuh; the IQN 3136->512 layer's kernels): packs
  * A (a_rows x red) and B (b_rows x red) from plain fp32 matrices (x_red_contig = 1: element (row, r) at
  * x[row*ld + r]; 0: at x[r*ld + row]) into hi/lo TF32 tile images inside d_work (dz_test_tc_pgemm_work floats),
  * then D[i,j] = sum_r A(i,r) B(j,r).  a_ones_row = a_rows appends a row of ones to A (bias-gradient row), -1: none.
@@ -346,7 +346,7 @@ int dz_test_threefry2x32(uint32_t k0, uint32_t k1, uint32_t c0, uint32_t c1, uin
  * tests/tools only. */
 int dz_test_learner_buffer(dz_learner* l, const char* name, float** d_ptr, int64_t* count);
 int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream);   /* device-to-device, tests only */
-/* Debug: the tcgen05 launch named `tag` writes the clock stamps of its CTA 0 into d_trace (512 int64). */
+/* Debug: the tensor-core launch named `tag` writes the clock stamps of its CTA 0 into d_trace (512 int64). */
 int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace);
 /* Debug: every kernel appends (globaltimer ns, gridDim.x << 32 | gridDim.y << 16 | blockDim.x) to d_buf right after its
  * dependencies completed; d_buf[0] (low 32 bits) counts the entries, entries start at d_buf[2].  d_buf: 2 + 2 * 4000
@@ -357,13 +357,14 @@ int dz_test_tc_pgemm(const float* d_A, int32_t a_rows, int32_t a_ld, int32_t a_r
                      int32_t b_rows, int32_t b_ld, int32_t b_red_contig, int32_t red, int32_t a_ones_row,
                      float* d_work, float* d_C, int64_t sc_i, int64_t sc_j, int32_t splits, int64_t split_stride,
                      const float* d_bias, int32_t relu, void* stream);
-/* Self-test of the TMA-fed tcgen05 GEMM family (csrc/dz_umma.cuh; conv / FC layers of the batch-32 step):
+/* Self-test of the TMA-fed tensor-core GEMM family (csrc/dz_umma.cuh; conv / FC layers of the batch-32 step):
  * C[MI][NJ] = sum_r A(i,r) B(j,r), NJ <= 64.  x_mn_major = 0: the operand is stored [rows][R]; 1: [R][rows] (the
- * instruction descriptor transposes).  convert = 0: operands pre-split into tf32 hi/lo arrays (activation path);
+ * MMA warps' fragment loads transpose).  convert = 0: operands pre-split into tf32 hi/lo arrays (activation path);
  * 1: raw fp32 tiles split in shared memory by the converter warps (weight path), A optionally scaled by
- * d_scale_r[r].  epi_rows = 1: row epilogue (+ d_bias[j], relu; tf32 hi/lo copies in d_hi / d_lo).  Synchronizes. */
+ * d_scale_r[r].  epi_rows = 1: row epilogue (+ d_bias[j], relu; tf32 hi/lo copies in d_hi / d_lo).  stages: depth of
+ * the shared-memory stage ring (0: 4; the launch fails when the ring does not fit).  Synchronizes. */
 int dz_test_umma_gemm(const float* d_A, int32_t a_mn_major, const float* d_B, int32_t b_mn_major, int32_t MI, int32_t NJ,
-                      int32_t R, int32_t convert, const float* d_scale_r, int32_t run_stages, int32_t epi_rows,
+                      int32_t R, int32_t convert, const float* d_scale_r, int32_t stages, int32_t epi_rows,
                       const float* d_bias, int32_t relu, float* d_C, float* d_hi, float* d_lo, void* stream);
 
 #ifdef __cplusplus

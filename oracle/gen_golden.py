@@ -25,6 +25,9 @@ sys.path.insert(0, os.path.dirname(HERE))
 
 from oracle import ref_import, replay_oracle, scenarios  # noqa: E402
 
+# a long random prioritized-replay run (ring wrap-around, many priority updates), recorded from the original
+LONG_RANDOM_PER = dict(capacity=257, alpha=0.5, usp=1e-3, normalize=True, batch=32, rounds=400, seed=31)
+
 
 def main():
   ref = ref_import.load_reference_replay()
@@ -37,6 +40,9 @@ def main():
     np.savez_compressed(os.path.join(out_dir, name + '.npz'), **res)
     print(name, {k: tuple(v.shape) for k, v in res.items()})
   ref._power = stock_power
+  res = scenarios.prioritized_replay_script(ref, **LONG_RANDOM_PER)
+  np.savez_compressed(os.path.join(out_dir, 'replay_long_random_per.npz'), **res)
+  print('replay_long_random_per', {k: tuple(v.shape) for k, v in res.items()})
 
 
 if __name__ == '__main__':

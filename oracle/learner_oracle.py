@@ -454,8 +454,8 @@ class Learner:
     g = {k: (v.grad if v.grad is not None else torch.zeros_like(v)) for k, v in p.items()}
     return loss.detach(), aux, g
 
-  def update(self, batch, weights=None, taus=None, noise=None):
-    loss, aux, g = self.grads(batch, weights, taus, noise)
+  def update(self, batch, weights=None, taus=None, noise=None, tap=None):
+    loss, aux, g = self.grads(batch, weights, taus, noise, tap=tap)
     self.online, self.state, gn = optimizer_step(self.opt, self.online, g, self.state)
     aux = dict(aux, loss=loss, grads=g, global_norm=gn)
     # priority rule: rainbow clip(|losses|,0,100) (`rainbow/agent.py:194`), prioritized |td| (`prioritized/agent.py:201`)

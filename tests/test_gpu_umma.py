@@ -1,4 +1,4 @@
-"""GPU: the TMA-fed tcgen05 GEMM family (csrc/dz_umma.cuh) against float64 numpy, through the C-ABI self-test hook.
+"""GPU: the TMA-fed tensor-core GEMM family (csrc/dz_umma.cuh) against float64 numpy, through the C-ABI self-test hook.
 
 Covers every operand path the learner uses: K-major and MN-major sources (the descriptor transposes), pre-split
 tf32 hi/lo operands (activations) and raw fp32 tiles split in shared memory by the converter warps (weights),
@@ -12,7 +12,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-def run_umma(Am, Bm, a_mn, b_mn, convert, scale=None, run_stages=1, epi_rows=False, bias=None, relu=False):
+def run_umma(Am, Bm, a_mn, b_mn, convert, scale=None, stages=0, epi_rows=False, bias=None, relu=False):
   """Am: logical A(i, r) [MI][R]; Bm: logical B(j, r) [NJ][R].  Returns (C, hi, lo) as float64 numpy."""
   from dqn_zoo_b200 import _lib
   dev = 'cuda'
@@ -26,7 +26,7 @@ def run_umma(Am, Bm, a_mn, b_mn, convert, scale=None, run_stages=1, epi_rows=Fal
   sc = None if scale is None else torch.as_tensor(scale, device=dev).contiguous()
   bs = None if bias is None else torch.as_tensor(bias, device=dev).contiguous()
   _lib.call('dz_test_umma_gemm', dA.data_ptr(), int(a_mn), dB.data_ptr(), int(b_mn), MI, NJ, R, int(convert),
-            0 if sc is None else sc.data_ptr(), run_stages, int(epi_rows), 0 if bs is None else bs.data_ptr(), int(relu),
+            0 if sc is None else sc.data_ptr(), stages, int(epi_rows), 0 if bs is None else bs.data_ptr(), int(relu),
             out.data_ptr(), hi.data_ptr() if epi_rows else 0, lo.data_ptr() if epi_rows else 0,
             torch.cuda.current_stream().cuda_stream)
   torch.cuda.synchronize()
@@ -61,12 +61,13 @@ def test_reduction_scale_in_the_converter(a_mn):
   assert rel(got, want) < 3e-6, rel(got, want)
 
 
-@pytest.mark.parametrize('run_stages', [1, 2, 4])
-def test_row_epilogue_bias_relu_and_split_outputs(run_stages):
+@pytest.mark.parametrize('stages', [1, 2, 4])
+def test_row_epilogue_bias_relu_and_split_outputs(stages):
+  """16 reduction stages through a ring of 1, 2 or 4 slots: every slot is refilled after its barrier phase flips."""
   Am, Bm = operands(300, 64, 512, 11)
   bias = np.random.RandomState(12).standard_normal(64).astype(np.float32)
   want = np.maximum(Am.astype(np.float64) @ Bm.astype(np.float64).T + bias.astype(np.float64)[None, :], 0.0)
-  got, hi, lo = run_umma(Am, Bm, 0, 0, 0, run_stages=run_stages, epi_rows=True, bias=bias, relu=True)
+  got, hi, lo = run_umma(Am, Bm, 0, 0, 0, stages=stages, epi_rows=True, bias=bias, relu=True)
   assert rel(got, want) < 3e-6, rel(got, want)
   # hi is a tf32 number (13 low mantissa bits clear), hi + lo reproduces the fp32 output to 2^-22
   assert np.all((hi.astype(np.float32).view(np.uint32) & 0x1FFF) == 0)
@@ -76,7 +77,7 @@ def test_row_epilogue_bias_relu_and_split_outputs(run_stages):
 
 @pytest.mark.parametrize('kind', ['dqn', 'double_q', 'c51', 'qrdqn', 'rainbow', 'iqn'])
 def test_tcgen05_path_is_active_at_the_baseline_geometry(kind):
-  """The 84x84x4, batch-32 learner of BASELINE.json must run its torso (and 3136->512 layer) on the tcgen05 kernels:
+  """The 84x84x4, batch-32 learner of BASELINE.json must run its torso (and 3136->512 layer) on the tensor-core kernels:
   a silent fall-back to the fp32-FMA kernels (geometry check, shared-memory budget) would keep every parity test green."""
   from dqn_zoo_b200 import _lib
   from dqn_zoo_b200 import learner as dl

@@ -92,7 +92,7 @@ def test_c_abi_library_exports_every_declared_symbol():
     assert hasattr(lib, name), 'library does not export %s' % name
   from dqn_zoo_b200 import _lib
   assert set(_lib.EXPORTS) == declared, set(_lib.EXPORTS) ^ declared
-  assert b'sm_100a' in _lib.lib.dz_build_info()
+  assert b'sm_90a' in _lib.lib.dz_build_info()
   # argument validation happens before any CUDA call
   cfg = _lib.LearnerConfig()
   cfg.kind = 99

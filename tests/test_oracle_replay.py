@@ -1,11 +1,15 @@
 """CPU: the oracle restatement vs (1) golden vectors made from the reference's replay.py,
-(2) the reference's known-answer tables, (3) the reference itself when it is mounted."""
+(2) the reference's known-answer tables."""
+
+import os
 
 import numpy as np
 import pytest
 
-from oracle import ref_import, replay_oracle, scenarios
+from oracle import gen_golden, replay_oracle, scenarios
 import replay_contract as rc
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 
 
 @pytest.mark.parametrize('name', list(scenarios.ALL))
@@ -18,22 +22,14 @@ def test_oracle_contract(fn):
   fn(replay_oracle)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason='reference not mounted (GPU box)')
-@pytest.mark.parametrize('fn', rc.CONTRACT, ids=lambda f: f.__name__)
-def test_contract_holds_for_the_reference_itself(fn):
-  """The contract file must describe the reference: run it on the reference's own classes."""
-  fn(ref_import.load_reference_replay())
-
-
-@pytest.mark.skipif(not ref_import.available(), reason='reference not mounted (GPU box)')
 def test_oracle_matches_reference_on_long_random_per_run():
-  ref = ref_import.load_reference_replay()
-  res = {}
-  for name, lib in (('ref', ref), ('oracle', replay_oracle)):
-    res[name] = scenarios.prioritized_replay_script(lib, capacity=257, alpha=0.5, usp=1e-3, normalize=True,
-                                                    batch=32, rounds=400, seed=31)
-  for k in res['ref']:
-    np.testing.assert_array_equal(res['ref'][k], res['oracle'][k], err_msg=k)
+  """Against the same script run on the original replay.py (tests/golden/replay_long_random_per.npz)."""
+  with np.load(os.path.join(GOLDEN, 'replay_long_random_per.npz')) as f:
+    want = {k: f[k] for k in f.files}
+  got = scenarios.prioritized_replay_script(replay_oracle, **gen_golden.LONG_RANDOM_PER)
+  assert sorted(got) == sorted(want)
+  for k in want:
+    np.testing.assert_array_equal(got[k], want[k], err_msg=k)
 
 
 def test_synthetic_rows_are_deterministic_and_in_range():

@@ -1,13 +1,14 @@
 """K independent learners (each with its own replay shard, parameters, optimizer state, CUDA stream and CUDA graph) on
 ONE GPU: aggregate learner grad-steps/s versus K.
 
-A single batch-32 learner step is a dependent chain of ~35 short kernels, most of which cover a fraction of the 148 SMs
-(the sampler is one block, the loss kernels 32, the tcgen05 conv kernels 35-128 CTAs): K shards interleave on the idle
+A single batch-32 learner step is a dependent chain of ~35 short kernels, most of which cover a fraction of the 132 SMs
+(the sampler is one block, the loss kernels 32, the tensor-core conv kernels 35-128 CTAs): K shards interleave on the idle
 SMs.  Each shard is exactly the object bench.py times (same agent class, same fused step); nothing is shared between
 shards, so per-learner results are the single-learner results (tests/test_gpu_agent.py covers those).
 
-  python tools/bench_multi_learner.py --agent rainbow --learners 1,2,3 [--capacity 1000000] [--steps 1500]
-Prints one JSON line per K."""
+  python tools/bench_multi_learner.py --agent rainbow --learners 1,2,3 [--capacity 250000] [--steps 1500]
+Prints one JSON line per K.  The default capacity (14.1 GB of replay per shard) lets three shards share an 80 GB H100;
+K shards of 1M transitions need 56.4 GB each."""
 
 import argparse
 import json
@@ -72,11 +73,16 @@ def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--agent', default='rainbow')
   ap.add_argument('--learners', default='1,2,3')
-  ap.add_argument('--capacity', type=int, default=1000000)
+  ap.add_argument('--capacity', type=int, default=250000)
   ap.add_argument('--steps', type=int, default=1500)
   ap.add_argument('--warmup', type=int, default=100)
   a = ap.parse_args()
-  for k in [int(x) for x in a.learners.split(',')]:
+  ks = [int(x) for x in a.learners.split(',')]
+  need = max(ks) * a.capacity * 2 * 84 * 84 * 4
+  free, _ = torch.cuda.mem_get_info()
+  if need > free:
+    ap.error('%d shards of %d transitions need %.1f GB of replay, %.1f GB of HBM is free' % (max(ks), a.capacity, need / 1e9, free / 1e9))
+  for k in ks:
     run(a.agent, k, a.capacity, a.steps, a.warmup)
 
 

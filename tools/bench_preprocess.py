@@ -68,7 +68,7 @@ def main():
     hbm = float(peaks.get('hbm_gbs', peaks.get('hbm_gbs_burst', 6650.0)))
     src = 'measured (MEASURED_PEAKS.json)'
   except Exception:
-    hbm, src = 6650.0, 'fallback (B200_PROFILING.md)'
+    hbm, src = 3350.0, 'H100 SXM data sheet (3.35 TB/s HBM3, 700 W)'
   # e2e: every stream emits every 4th tick; frames come from host memory
   rs = np.random.RandomState(2)
   frames = [rs.randint(0, 256, size=(H, W, 3), dtype=np.uint8) for _ in range(8)]

@@ -1,5 +1,5 @@
-"""Bring-up probe of the TMA-fed tcgen05 GEMM family: runs every operand path and prints the relative error of
-each (no assertions), plus a few hints when a path is wrong.  `python tools/umma_probe.py` on a B200."""
+"""Bring-up probe of the TMA-fed tensor-core GEMM family: runs every operand path and prints the relative error of
+each (no assertions), plus a few hints when a path is wrong.  `python tools/umma_probe.py` on an H100."""
 
 import os
 import sys

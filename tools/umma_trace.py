@@ -1,4 +1,4 @@
-"""Debug: clock-stamp timeline of CTA 0 of one tcgen05 launch inside a rainbow / dqn learner step.
+"""Debug: clock-stamp timeline of CTA 0 of one tensor-core launch inside a rainbow / dqn learner step.
   python tools/umma_trace.py --agent rainbow --tag conv2_fwd"""
 
 import argparse
@@ -43,17 +43,14 @@ def main():
     if tag.startswith('conv1'):
       nt = int((t[192:256] != 0).sum())
       print('== %s: tiles %d | exit %d' % (tag, nt, rel(t[322])))
-      for name, o in (('rows issued', 0), ('rows landed', 64), ('mma issued', 128), ('tile drained', 192), ('tile stored', 256)):
+      for name, o in (('rows issued', 0), ('rows landed', 64), ('tile mma done', 192), ('tile stored', 256)):
         print('  %-12s:' % name, [rel(x) for x in t[o:o + nt]])
       continue
     n = int((t[:64] != 0).sum())
-    runs = int((t[192:256] != 0).sum())
-    print('== %s: stages %d runs %d | setup done %d | epilogue math %d stores %d exit %d' % (tag, n, runs, rel(t[324]), rel(t[320]), rel(t[321]), rel(t[322])))
+    print('== %s: stages %d | setup done %d | epilogue %d stores %d exit %d' % (tag, n, rel(t[324]), rel(t[320]), rel(t[321]), rel(t[322])))
     print('  tma issued :', [rel(x) for x in t[:n]])
     print('  data ready :', [rel(x) for x in t[64:64 + n]])
-    print('  mma issued :', [rel(x) for x in t[128:128 + n]])
-    print('  acc ready  :', [rel(x) for x in t[192:192 + runs]])
-    print('  run drained:', [rel(x) for x in t[256:256 + runs]])
+    print('  consumed   :', [rel(x) for x in t[128:128 + n]])
 
 
 if __name__ == '__main__':
