@@ -43,10 +43,10 @@ void profile_geometry(unsigned gx, unsigned gy, unsigned bx);   // launch geomet
 // and is launched with the programmatic-stream-serialization attribute: the next kernel's launch and block
 // scheduling overlap the tail of the previous one, and all of its global-memory traffic still comes after
 // everything it depends on has completed and is visible.  Kernel-to-kernel edges captured into the CUDA graph become
-// programmatic edges.  Measured on the ~30-kernel learner steps: dqn 228 -> 217 us, rainbow 353 -> 338 us.  Triggering
-// the dependents EARLY (griddepcontrol.launch_dependents at kernel entry, -DDZ_PDL_EARLY) was slower (dqn 265 us):
-// the early CTAs spin at their wait and take issue slots and SM space from the kernel that is still running.
-// DZ_NO_PDL=1 launches with full serialization.
+// programmatic edges.  Measured before the H100 port on the ~30-kernel learner steps: dqn 228 -> 217 us, rainbow
+// 353 -> 338 us.  Dependents are not triggered early (griddepcontrol.launch_dependents at kernel entry): that was slower
+// there (dqn 265 us), because the early CTAs spin at their wait and take issue slots and SM space from the kernel that
+// is still running.
 // Debug timeline (dz_debug_timeline): when a buffer is installed, thread 0 of block 0 of EVERY kernel appends
 // (globaltimer, gridDim.x << 32 | gridDim.y << 16 | blockDim.x) right after its griddepcontrol.wait, i.e. at the moment
 // everything it depends on has completed.  Read back after a CUDA-graph replay this is the true timeline of the step
@@ -68,9 +68,6 @@ __device__ __forceinline__ void timeline_stamp() {
   }
 }
 __device__ __forceinline__ void pdl_enter() {
-#ifdef DZ_PDL_EARLY
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-#endif
   asm volatile("griddepcontrol.wait;" ::: "memory");
   timeline_stamp();
 }
@@ -79,29 +76,15 @@ void timeline_register(timeline_setter_t fn);      // dz_replay.cu
 static int timeline_set_this_tu(unsigned long long* p) { return (int)cudaMemcpyToSymbol(g_timeline, &p, sizeof(p)); }
 struct TimelineRegistrar { TimelineRegistrar() { timeline_register(timeline_set_this_tu); } };
 static TimelineRegistrar g_timeline_registrar;
-extern int g_pdl;   // -1 = read DZ_NO_PDL on first use
-extern int g_carveout;   // -1 = read DZ_CARVEOUT on first use; > 0: preferred shared-memory carveout (percent) for EVERY kernel
 
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
-  if (g_pdl < 0) { const char* e = getenv("DZ_NO_PDL"); g_pdl = (e && e[0] && e[0] != '0') ? 0 : 1; }
-  if (g_carveout < 0) { const char* e = getenv("DZ_CARVEOUT"); g_carveout = e ? atoi(e) : 0; }
-  if (g_carveout > 0) {   // experiment: one L1/shared split for the whole step, so consecutive kernels never reconfigure the SMs
-    static const void* done[64];
-    static int ndone = 0;
-    bool seen = false;
-    for (int i = 0; i < ndone; ++i) seen = seen || done[i] == (const void*)kernel;
-    if (!seen && ndone < 64) {
-      cudaFuncSetAttribute((const void*)kernel, cudaFuncAttributePreferredSharedMemoryCarveout, g_carveout);
-      done[ndone++] = (const void*)kernel;
-    }
-  }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = g_pdl ? 1 : 0;
+  cfg.attrs = attr; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 

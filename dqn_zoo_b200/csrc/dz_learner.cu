@@ -1100,74 +1100,15 @@ __device__ __forceinline__ float opt_one(const OptArgs& o, float p, float g, flo
   return p - o.lr * upd;
 }
 
-// 7 floats of traffic per parameter (read p,g,m,v; write p,m,v), 16-byte accesses, 4 independent
-// float4 quadruples per thread in flight.  Measured alternatives (rainbow, 52.7 us per launch incl. ~5 us of
-// event overhead): ld.global.cs on the gradient and/or st.global.cs on the moments: no change (52.7 / 53.0 us);
-// 4 quadruples per thread: 71 us (register pressure halves the resident threads); 4, 8, 12, 16 blocks per SM:
-// 43.9 / 45.0 / 45.8 / 46.7 us.
-template <int KIND>
-__global__ void __launch_bounds__(256) optimizer_kernel(OptArgs o) {
-  dz::pdl_enter();
-  const long long n4 = o.n >> 2;
-  float4* p4 = reinterpret_cast<float4*>(o.p);
-  const float4* g4 = reinterpret_cast<const float4*>(o.g);
-  float4* m4 = reinterpret_cast<float4*>(o.m);
-  float4* v4 = reinterpret_cast<float4*>(o.v);
-  constexpr int U = 2;
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  const long long first = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  // the first batch of loads is issued BEFORE the norm is formed: the split-norm reduction (shared memory, a block
-  // barrier, ~700 L2 reads per block) then hides behind the memory latency of the stream instead of preceding it
-  float4 p[U], g[U], m[U], v[U];
-#pragma unroll
-  for (int u = 0; u < U; ++u) {
-    long long i = first + u * stride;
-    if (i < n4) { p[u] = p4[i]; g[u] = g4[i]; m[u] = m4[i]; v[u] = v4[i]; }
-  }
-  float norm;
-  if (o.parts != nullptr) {
-    norm = split_norm(o.parts, o.nparts, o.fc_sumsq);
-    if (blockIdx.x == 0 && threadIdx.x == 0) { o.norm_out[0] = norm; if (o.user_norm) o.user_norm[0] = norm; }
-  } else {
-    norm = o.norm[0];
-  }
-  const bool clip = o.max_norm > 0.f && !(norm < o.max_norm);  // optax.clip_by_global_norm trigger
-  float c1 = 1.f, c2 = 1.f;
-  if (KIND == DZ_ADAM) {
-    float t = (float)o.counters[0];
-    c1 = 1.0f / (1.0f - powf(o.b1, t));
-    c2 = 1.0f / (1.0f - powf(o.b2, t));
-  }
-  for (long long i0 = first; i0 < n4; i0 += stride * U) {
-    if (i0 != first) {
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        long long i = i0 + u * stride;
-        if (i < n4) { p[u] = p4[i]; g[u] = g4[i]; m[u] = m4[i]; v[u] = v4[i]; }
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      long long i = i0 + u * stride;
-      if (i < n4) {
-        p[u].x = opt_one<KIND>(o, p[u].x, g[u].x, m[u].x, v[u].x, clip, norm, c1, c2);
-        p[u].y = opt_one<KIND>(o, p[u].y, g[u].y, m[u].y, v[u].y, clip, norm, c1, c2);
-        p[u].z = opt_one<KIND>(o, p[u].z, g[u].z, m[u].z, v[u].z, clip, norm, c1, c2);
-        p[u].w = opt_one<KIND>(o, p[u].w, g[u].w, m[u].w, v[u].w, clip, norm, c1, c2);
-        p4[i] = p[u]; m4[i] = m[u]; v4[i] = v[u];
-      }
-    }
-  }
-}
-
-// The same update as a bulk-copy (TMA 1-D) pipeline: the four streams of a 256-quadruple chunk land in shared memory by
-// cp.async.bulk (one elected thread, mbarrier complete_tx), 256 threads update them in place, and p / m / v leave by
-// cp.async.bulk stores.  Memory-level parallelism no longer depends on registers x resident warps: every CTA keeps
-// `stages` - 1 chunks (16 KB each) of loads in flight while it computes, and the LSU sees shared-memory traffic only.
-// Identical arithmetic (opt_one), identical results.
-constexpr int kOptStagesMax = 8;
-constexpr int kOptChunk = 256;                            // float4 per stream per stage = one per thread
+// The optimizer update (7 floats of traffic per parameter: read p, g, m, v; write p, m, v) as a bulk-copy (TMA 1-D)
+// pipeline: the four streams of a 256-quadruple chunk land in shared memory by cp.async.bulk (one elected thread,
+// mbarrier complete_tx), the threads update them in place, and p / m / v leave by cp.async.bulk stores.  Memory-level
+// parallelism does not depend on registers x resident warps: every CTA keeps `stages` - 1 chunks (16 KB each) of loads
+// in flight while it computes, and the LSU sees shared-memory traffic only.
+constexpr int kOptChunk = 256;                            // float4 per stream per stage
 constexpr int kOptStageBytes = 4 * kOptChunk * 16;        // p, g, m, v
+constexpr int kOptRingStages = 3;                         // OptArgs::stages of every launch
+constexpr int kOptBlocksPerSM = 4;
 
 __device__ __forceinline__ void opt_bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(tc::smem_u32(dst)),
@@ -1180,8 +1121,8 @@ __device__ __forceinline__ void opt_bulk_store(void* dst, const void* src, uint3
                : "memory");
 }
 
-template <int KIND, int V>   // V floats per thread and stage: 4 (256 threads) or 2 (512 threads, twice the warps per byte of shared memory)
-__global__ void __launch_bounds__(kOptChunk * 4 / V, V == 2 ? 4 : 1) optimizer_bulk_kernel(OptArgs o) {
+template <int KIND, int V>   // V = 2 floats per thread and stage: 512 threads
+__global__ void __launch_bounds__(kOptChunk * 4 / V, 4) optimizer_bulk_kernel(OptArgs o) {
   extern __shared__ __align__(128) unsigned char opt_sm[];
   const int kOptStages = o.stages;
   uint64_t* full = reinterpret_cast<uint64_t*>(opt_sm + kOptStages * kOptStageBytes);
@@ -1210,7 +1151,8 @@ __global__ void __launch_bounds__(kOptChunk * 4 / V, V == 2 ? 4 : 1) optimizer_b
     opt_bulk_load(st + 2 * kOptChunk * 16, m4 + q0, bytes, &full[s]);
     opt_bulk_load(st + 3 * kOptChunk * 16, v4 + q0, bytes, &full[s]);
   };
-  // the first loads are issued BEFORE the norm is formed (see optimizer_kernel)
+  // the first loads are issued BEFORE the norm is formed: the split-norm reduction (shared memory, a block barrier,
+  // ~700 L2 reads per block) then hides behind the memory latency of the stream instead of preceding it
   if (tid == 0)
     for (long long it = 0; it < mine && it < kOptStages; ++it) issue(it, (int)it);
   float norm;
@@ -1244,23 +1186,12 @@ __global__ void __launch_bounds__(kOptChunk * 4 / V, V == 2 ? 4 : 1) optimizer_b
       }
     }
     tc::mbar_wait(&full[s], phase);
-    if (V == 4) {
-      if (tid < valid) {
-        float4 p = sp[tid], g = sg[tid], m = smm[tid], v = sv[tid];
-        p.x = opt_one<KIND>(o, p.x, g.x, m.x, v.x, clip, norm, c1, c2);
-        p.y = opt_one<KIND>(o, p.y, g.y, m.y, v.y, clip, norm, c1, c2);
-        p.z = opt_one<KIND>(o, p.z, g.z, m.z, v.z, clip, norm, c1, c2);
-        p.w = opt_one<KIND>(o, p.w, g.w, m.w, v.w, clip, norm, c1, c2);
-        sp[tid] = p; smm[tid] = m; sv[tid] = v;
-      }
-    } else {
-      if (tid < 2 * valid) {
-        float2 p = reinterpret_cast<float2*>(sp)[tid], g = reinterpret_cast<float2*>(sg)[tid];
-        float2 m = reinterpret_cast<float2*>(smm)[tid], v = reinterpret_cast<float2*>(sv)[tid];
-        p.x = opt_one<KIND>(o, p.x, g.x, m.x, v.x, clip, norm, c1, c2);
-        p.y = opt_one<KIND>(o, p.y, g.y, m.y, v.y, clip, norm, c1, c2);
-        reinterpret_cast<float2*>(sp)[tid] = p; reinterpret_cast<float2*>(smm)[tid] = m; reinterpret_cast<float2*>(sv)[tid] = v;
-      }
+    if (tid < 2 * valid) {
+      float2 p = reinterpret_cast<float2*>(sp)[tid], g = reinterpret_cast<float2*>(sg)[tid];
+      float2 m = reinterpret_cast<float2*>(smm)[tid], v = reinterpret_cast<float2*>(sv)[tid];
+      p.x = opt_one<KIND>(o, p.x, g.x, m.x, v.x, clip, norm, c1, c2);
+      p.y = opt_one<KIND>(o, p.y, g.y, m.y, v.y, clip, norm, c1, c2);
+      reinterpret_cast<float2*>(sp)[tid] = p; reinterpret_cast<float2*>(smm)[tid] = m; reinterpret_cast<float2*>(sv)[tid] = v;
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the bulk stores
     __syncthreads();
@@ -1317,8 +1248,6 @@ struct dz_learner {
   float *cosf[3], *hi[3], *E0;             // iqn
   float* nn_partial;                        // split-K partials for the M=batch FC layers and heads
   float* conv_partial;                      // split-K partials for conv2/conv3 forward
-  float* conv1_partial;                     // split-K partials for conv1 forward (conv1_splits > 1)
-  int conv1_splits;
   float* nt_partial;                        // split partials of the input-gradient (NT) GEMMs
   float *dout, *doutv, *dh1[2], *dact3, *dtmp[2], *dcol, *dact2, *dact1, *dhi;
   float* tn_partial[4];                     // conv1/2/3 wgrad partials, [3] = iqn head/embed partial
@@ -1327,9 +1256,7 @@ struct dz_learner {
   const uint8_t** rows_sample[2];           // row tables filled by the fused sampler
   const uint8_t** rows_act;                 // 1-entry table for q_values
   int32_t* s_a; float *s_r, *s_d, *s_w;     // sampler-produced batch scalars
-  float *act_noise_zero;                    // zeros (acting without noise is never used; placeholder)
   float* q_scratch;
-  int norm_blocks;
   int fc_splits, head_splits, conv_splits, nt_splits;
   // packed-operand tensor-core path of the IQN 3136->512 layer (dz_tcp.cuh): hi/lo tile images + split partials
   bool pk_on;
@@ -1359,15 +1286,6 @@ namespace {
 
 constexpr int kNormBlocks = kNumSMs * 4;
 
-// The packed-operand tensor-core kernels carry IQN's 3136->512 layer whenever every network apply has >= 1024 rows
-// (DZ_PK_IQN=0 falls back to the fp32-FMA kernels, for A/B timing).
-bool g_pk_iqn = true;
-int g_fc_splits = 0;      // DZ_FC_SPLITS override
-int g_conv1_splits = 1;   // DZ_CONV1_SPLITS: split-K of the conv1 forward GEMM (K = 256).  Measured: rainbow (3 applies,
-                          // 600 tiles) 336 / 344 / 341 us per step for 1 / 2 / 3 splits, dqn (2 applies) 217 / 213 / 217 us:
-                          // the extra finish launch eats the gain, so the default stays 1.
-void read_env();
-
 // Split count for a one-CTA-per-SM kernel: minimise (waves of kNumSMs CTAs) x (k-blocks per split).
 int pick_splits(int64_t tiles, int nkb, int max_splits) {
   int best = 1;
@@ -1379,8 +1297,6 @@ int pick_splits(int64_t tiles, int nkb, int max_splits) {
   return best;
 }
 
-// DZ_UMMA=0 keeps every contraction on the fp32-FMA kernels (A/B timing, geometries the tensor-core path does not cover).
-bool g_umma = true;
 int64_t noise_stride(const dz_learner_config& c, const Dims& d);
 struct NoiseVecs;
 
@@ -1408,15 +1324,13 @@ int64_t carve(dz_learner* l, char* base) {
     l->hi[p] = iqn ? w.take<float>(rows * d.feat) : nullptr;
   }
   l->E0 = iqn ? w.take<float>((int64_t)B * nh[0] * d.feat) : nullptr;
-  l->fc_splits = g_fc_splits > 0 ? std::min(g_fc_splits, 64) : 14; l->head_splits = 8; l->conv_splits = 4; l->nt_splits = 8;
+  l->fc_splits = 14; l->head_splits = 8; l->conv_splits = 4; l->nt_splits = 8;
   {
     int64_t head_n = std::max<int64_t>(d.out, c.num_atoms);
     int64_t fc = (int64_t)kMaxProblems * l->fc_splits * 2 * B * 512;
     int64_t hd = (int64_t)kMaxProblems * l->head_splits * 2 * B * head_n;
     l->nn_partial = w.take<float>(std::max(fc, hd));
     l->conv_partial = w.take<float>((int64_t)3 * l->conv_splits * B * d.h2 * d.w2 * 64);
-    l->conv1_splits = std::max(1, std::min(g_conv1_splits, 4));
-    l->conv1_partial = l->conv1_splits > 1 ? w.take<float>((int64_t)3 * l->conv1_splits * B * d.h1 * d.w1 * 32) : nullptr;
     l->nt_partial = w.take<float>((int64_t)2 * l->nt_splits * 2 * B * std::max<int64_t>(d.feat, 512));
   }
   int64_t rows0 = (int64_t)B * nh[0];
@@ -1437,7 +1351,8 @@ int64_t carve(dz_learner* l, char* base) {
   l->tn_partial[2] = w.take<float>((int64_t)32 * 577 * 64);
   l->tn_partial[3] = iqn ? w.take<float>((int64_t)16 * (c.latent_dim + 1) * d.feat + 16 * 513 * 64) : nullptr;
   l->pk_on = false; l->pk_embed_bwd = false;
-  if (iqn && g_pk_iqn && rows0 >= 1024 && (int64_t)B * nh[1] >= 1024 && (int64_t)B * nh[2] >= 1024 && d.feat % 16 == 0 &&
+  // The packed-operand tensor-core kernels carry IQN's 3136->512 layer whenever every network apply has >= 1024 rows.
+  if (iqn && rows0 >= 1024 && (int64_t)B * nh[1] >= 1024 && (int64_t)B * nh[2] >= 1024 && d.feat % 16 == 0 &&
       c.latent_dim <= 128 && rows0 % 4 == 0 && ((int64_t)B * nh[1]) % 4 == 0 && ((int64_t)B * nh[2]) % 4 == 0) {
     l->pk_on = true;
     auto img = [&](dz_learner::PkImg& im, int64_t rows, int64_t red, int row_tile) {
@@ -1482,13 +1397,11 @@ int64_t carve(dz_learner* l, char* base) {
   l->q_scratch = w.take<float>(64);
   l->norm_parts = w.take<float>(1024);
   l->um_ws = nullptr;
-  if (g_umma) {
-    UmNetDesc ud = make_um_desc(l);
-    if (um_net_supported(ud)) {
-      int64_t bytes = um_net_workspace_bytes(ud);
-      l->um_ws = w.take<char>(bytes);
-      if (!base) l->um_ws = reinterpret_cast<char*>(1);   // size query: "enabled" marker only
-    }
+  UmNetDesc ud = make_um_desc(l);
+  if (um_net_supported(ud)) {
+    int64_t bytes = um_net_workspace_bytes(ud);
+    l->um_ws = w.take<char>(bytes);
+    if (!base) l->um_ws = reinterpret_cast<char*>(1);   // size query: "enabled" marker only
   }
   return w.used;
 }
@@ -1569,14 +1482,6 @@ int launch_batch(const char* tag, KernelT kernel, const GemmBatch& gb, dim3 grid
 }
 
 #define DZ_TRY(expr) do { int _s = (expr); if (_s != DZ_OK) return _s; } while (0)
-
-
-void read_env() {
-  g_pk_iqn = !(getenv("DZ_PK_IQN") != nullptr && std::string(getenv("DZ_PK_IQN")) == "0");
-  g_fc_splits = getenv("DZ_FC_SPLITS") ? atoi(getenv("DZ_FC_SPLITS")) : 0;
-  g_conv1_splits = getenv("DZ_CONV1_SPLITS") ? atoi(getenv("DZ_CONV1_SPLITS")) : 1;
-  g_umma = !(getenv("DZ_UMMA") != nullptr && std::string(getenv("DZ_UMMA")) == "0");
-}
 
 // ---- NN launch helpers (tile shapes chosen by M / N) -------------------------------------------
 
@@ -1666,21 +1571,16 @@ int forward_torso(dz_learner* l, const TorsoJob* jobs, int njobs, int nimg, void
   const Layout& L = l->lay;
   GemmBatch gb;
   gb.n = njobs;
-  float* outs1[kMaxProblems];
-  for (int i = 0; i < njobs; ++i) {   // conv1: uint8 rows gathered in place (K1 + K2 of SURVEY §2.1)
+  // conv1: uint8 rows gathered in place (K1 + K2 of SURVEY §2.1).  Not split over K (= 256): measured before the H100
+  // port, the extra finish launch ate the gain of 2 or 3 splits.
+  for (int i = 0; i < njobs; ++i) {
     GemmProblem p = zero_problem();
     set_conv(p, A_CONV_U8, jobs[i].rows, nimg, d.H, d.W, d.C, 8, 8, 4);
     p.B = jobs[i].params + L.off("conv1/w"); p.bias = jobs[i].params + L.off("conv1/b");
     p.N = 32; p.ldb = 32; p.ldc = 32; p.relu = 1; p.C = l->act1[jobs[i].set];
-    outs1[i] = p.C;
-    if (l->conv1_splits > 1 && nimg == l->B) {
-      p.splits = l->conv1_splits; p.split_stride = (long long)p.M * 32;
-      p.C = l->conv1_partial + (long long)i * p.splits * p.split_stride;
-    }
     gb.p[i] = p;
   }
   DZ_TRY(run_nn("conv1_fwd", gb, false, stream));
-  if (gb.p[0].splits > 1) DZ_TRY(finish_nn(gb, outs1, false, stream));
   // conv2 / conv3: few output tiles (41 / 25 per pass) -> split K four ways so the grid covers the 132 SMs;
   // finish_nn adds the bias and ReLU.
   for (int layer = 2; layer <= 3; ++layer) {
@@ -1985,17 +1885,16 @@ int finish_nt(const GemmProblem* probs, int nsrc, const float* mask, float* out,
   return finish_nt_batch(&f, 1, stream);
 }
 
-// Returns the side stream after making it wait for everything enqueued on `stream` so far (or `stream`
-// itself when there is no side stream).  join_side() makes `stream` wait for the side work again.
+// Returns the side stream after making it wait for everything enqueued on `stream` so far (or `stream` itself when
+// that ordering cannot be recorded).  join_side() makes `stream` wait for the side work again.
 void* fork_side(dz_learner* l, void* stream) {
-  if (!l->side) return stream;
   if (cudaEventRecord(l->ev_fork, (cudaStream_t)stream) != cudaSuccess) return stream;
   if (cudaStreamWaitEvent(l->side, l->ev_fork, 0) != cudaSuccess) return stream;
   l->side_dirty = true;
   return l->side;
 }
 int join_side(dz_learner* l, void* stream) {
-  if (!l->side || !l->side_dirty) return DZ_OK;
+  if (!l->side_dirty) return DZ_OK;
   DZ_CUDA_OK(cudaEventRecord(l->ev_join, l->side));
   DZ_CUDA_OK(cudaStreamWaitEvent((cudaStream_t)stream, l->ev_join, 0));
   l->side_dirty = false;
@@ -2003,14 +1902,13 @@ int join_side(dz_learner* l, void* stream) {
 }
 // Second side stream: `from` is the stream whose enqueued work it must wait for (the main stream or the first side stream).
 void* fork_side2(dz_learner* l, void* from, void* fallback) {
-  if (!l->side2) return fallback;
   if (cudaEventRecord(l->ev_fork2, (cudaStream_t)from) != cudaSuccess) return fallback;
   if (cudaStreamWaitEvent(l->side2, l->ev_fork2, 0) != cudaSuccess) return fallback;
   l->side2_dirty = true;
   return l->side2;
 }
 int join_side2(dz_learner* l, void* stream) {
-  if (!l->side2 || !l->side2_dirty) return DZ_OK;
+  if (!l->side2_dirty) return DZ_OK;
   DZ_CUDA_OK(cudaEventRecord(l->ev_join2, l->side2));
   DZ_CUDA_OK(cudaStreamWaitEvent((cudaStream_t)stream, l->ev_join2, 0));
   l->side2_dirty = false;
@@ -2061,7 +1959,7 @@ int backward_torso(dz_learner* l, const uint8_t* const* rows0, void* stream) {
   }
   // conv2 wgrad
   if (l->um) {   // conv2: on the second side stream, beside conv3's (both fit next to the input-gradient kernels)
-    void* ws = l->side2 ? fork_side2(l, stream, stream) : fork_side(l, stream);
+    void* ws = fork_side2(l, stream, stream);
     DZ_TRY(um_wgrad_conv2(l->um, ws));
     DZ_TRY(um_wgrad_finish_layer(l->um, 2, G + L.off("conv2/w"), G + L.off("conv2/b"), norm_parts, ws));
   } else {
@@ -2106,7 +2004,7 @@ int backward_torso(dz_learner* l, const uint8_t* const* rows0, void* stream) {
     DZ_TRY(run_tn("conv1_wgrad", gb, fork_side(l, stream)));
     fb.f[fb.n++] = FinishTN{p.C, splits, p.split_stride, p.K, 32, G + L.off("conv1/w"), nullptr, p.Cb, nullptr, nullptr, nullptr};
   }
-  void* ws = l->side && l->side_dirty ? (void*)l->side : stream;   // after conv1_wgrad on the same (side) stream
+  void* ws = l->side_dirty ? (void*)l->side : stream;   // after conv1_wgrad on the same (side) stream
   dim3 grid((unsigned)ceil_div(577 * 64, 256), fb.n);
   DZ_LAUNCH(finish_tn_kernel, grid, 256, 0, ws, fb);
   return join_side(l, stream);
@@ -2128,7 +2026,7 @@ int backward_plain(dz_learner* l, void* stream) {
     p.C = G + L.off("head/w"); p.Cb = shared ? l->scalars + 8 + kNormBlocks : G + L.off("head/b");
     gb.p[0] = p;
     DZ_TRY(run_tn("head_wgrad", gb, fork_side(l, stream)));
-    if (shared) DZ_LAUNCH(sum_to_scalar_kernel, 1, 128, 0, (l->side && l->side_dirty ? (void*)l->side : stream), l->scalars + 8 + kNormBlocks, d.out, G + L.off("head/b"));
+    if (shared) DZ_LAUNCH(sum_to_scalar_kernel, 1, 128, 0, (l->side_dirty ? (void*)l->side : stream), l->scalars + 8 + kNormBlocks, d.out, G + L.off("head/b"));
   }
   bool dh1_split_done = false;
   {  // dh1 = dout * Wh^T, masked by h1 > 0
@@ -2368,14 +2266,14 @@ int backward_iqn(dz_learner* l, void* stream) {
   long long mx = 0;
   for (int q = 0; q < fb.n; ++q) mx = std::max<long long>(mx, (long long)(fb.f[q].K + 1) * fb.f[q].N);
   dim3 grid((unsigned)std::min<long long>(ceil_div(mx, 256), kNumSMs * 8), fb.n);
-  DZ_LAUNCH(finish_tn_kernel, grid, 256, 0, (l->side && l->side_dirty ? (void*)l->side : stream), fb);
+  DZ_LAUNCH(finish_tn_kernel, grid, 256, 0, (l->side_dirty ? (void*)l->side : stream), fb);
   return DZ_OK;
 }
 
 // Split global norm (tensor-core path, every agent but IQN): the sum of squares of everything behind the conv tensors is taken
 // on the second side stream as soon as the last FC / head weight gradient is written (norm_fc_range), the conv tensors'
 // partials come from the per-layer weight-gradient finish kernels, and the optimizer (or norm_finalize_kernel) combines them.
-bool split_norm_active(const dz_learner* l) { return l->um != nullptr && l->cfg.kind != DZ_IQN && l->side2 != nullptr; }
+bool split_norm_active(const dz_learner* l) { return l->um != nullptr && l->cfg.kind != DZ_IQN; }
 
 int norm_fc_range(dz_learner* l, bool apply, void* stream) {
   const long long begin = l->lay.off(l->cfg.kind == DZ_RAINBOW ? "adv1/mu/w" : "fc1/w");
@@ -2402,37 +2300,19 @@ int run_optimizer(dz_learner* l, float* user_norm, bool apply, void* stream) {
   OptArgs o{c.optimizer, c.learning_rate, c.opt_eps, c.rms_decay, c.adam_b1, c.adam_b2, c.max_global_grad_norm,
             l->buf.d_online, l->buf.d_grads, l->buf.d_opt_state, l->buf.d_opt_state + n, n, norm, l->buf.d_counters,
             parts, nparts, l->scalars + 1, norm, user_norm};
-  static const int per_sm = getenv("DZ_OPT_BLOCKS") ? atoi(getenv("DZ_OPT_BLOCKS")) : 8;
-  // DZ_OPT_BULK=0: the register-staged kernel (A/B measurements)
-  static const bool bulk = !(getenv("DZ_OPT_BULK") && getenv("DZ_OPT_BULK")[0] == '0');
-  if (bulk) {
-    static const int bulk_per_sm = getenv("DZ_OPT_BLOCKS") ? atoi(getenv("DZ_OPT_BLOCKS")) : 4;
-    static const int stages = std::min(kOptStagesMax, std::max(2, getenv("DZ_OPT_STAGES") ? atoi(getenv("DZ_OPT_STAGES")) : 3));
-    const int kOptSmem = stages * kOptStageBytes + 64;
-    o.stages = stages;
-    static const int vec = (getenv("DZ_OPT_VEC") && atoi(getenv("DZ_OPT_VEC")) == 4) ? 4 : 2;
-    static bool attr_done = false;
-    if (!attr_done) {
-      DZ_CUDA_OK(cudaFuncSetAttribute(optimizer_bulk_kernel<DZ_ADAM, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptSmem));
-      DZ_CUDA_OK(cudaFuncSetAttribute(optimizer_bulk_kernel<DZ_RMSPROP_CENTERED, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptSmem));
-      DZ_CUDA_OK(cudaFuncSetAttribute(optimizer_bulk_kernel<DZ_ADAM, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptSmem));
-      DZ_CUDA_OK(cudaFuncSetAttribute(optimizer_bulk_kernel<DZ_RMSPROP_CENTERED, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptSmem));
-      attr_done = true;
-    }
-    const long long nchunks = ((o.n >> 2) + kOptChunk - 1) / kOptChunk;
-    const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>((long long)kNumSMs * bulk_per_sm, nchunks));
-    const unsigned threads = kOptChunk * 4 / vec;
-    if (c.optimizer == DZ_ADAM) {
-      if (vec == 4) DZ_LAUNCH_NAMED("optimizer_kernel", (optimizer_bulk_kernel<DZ_ADAM, 4>), grid, threads, kOptSmem, stream, o);
-      else DZ_LAUNCH_NAMED("optimizer_kernel", (optimizer_bulk_kernel<DZ_ADAM, 2>), grid, threads, kOptSmem, stream, o);
-    } else {
-      if (vec == 4) DZ_LAUNCH_NAMED("optimizer_kernel", (optimizer_bulk_kernel<DZ_RMSPROP_CENTERED, 4>), grid, threads, kOptSmem, stream, o);
-      else DZ_LAUNCH_NAMED("optimizer_kernel", (optimizer_bulk_kernel<DZ_RMSPROP_CENTERED, 2>), grid, threads, kOptSmem, stream, o);
-    }
-    return DZ_OK;
+  const int kOptSmem = kOptRingStages * kOptStageBytes + 64;
+  o.stages = kOptRingStages;
+  static bool attr_done = false;
+  if (!attr_done) {
+    DZ_CUDA_OK(cudaFuncSetAttribute(optimizer_bulk_kernel<DZ_ADAM, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptSmem));
+    DZ_CUDA_OK(cudaFuncSetAttribute(optimizer_bulk_kernel<DZ_RMSPROP_CENTERED, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptSmem));
+    attr_done = true;
   }
-  if (c.optimizer == DZ_ADAM) DZ_LAUNCH_NAMED("optimizer_kernel", optimizer_kernel<DZ_ADAM>, kNumSMs * per_sm, 256, 0, stream, o);
-  else DZ_LAUNCH_NAMED("optimizer_kernel", optimizer_kernel<DZ_RMSPROP_CENTERED>, kNumSMs * per_sm, 256, 0, stream, o);
+  const long long nchunks = ((o.n >> 2) + kOptChunk - 1) / kOptChunk;
+  const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>((long long)kNumSMs * kOptBlocksPerSM, nchunks));
+  const unsigned threads = kOptChunk * 4 / 2;
+  if (c.optimizer == DZ_ADAM) DZ_LAUNCH_NAMED("optimizer_kernel", (optimizer_bulk_kernel<DZ_ADAM, 2>), grid, threads, kOptSmem, stream, o);
+  else DZ_LAUNCH_NAMED("optimizer_kernel", (optimizer_bulk_kernel<DZ_RMSPROP_CENTERED, 2>), grid, threads, kOptSmem, stream, o);
   return DZ_OK;
 }
 
@@ -2464,11 +2344,6 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     for (int i = 0; i < nj; ++i) rows[i] = jobs[i].rows;
     if (weights_packed) DZ_TRY(join_side(l, stream));   // packed on the side stream, concurrently with the sampler
     else DZ_TRY(um_pack_weights(l->um, stream));
-    // Optional (DZ_PREFETCH=1): pull the 3136 -> 512 weight matrices into L2 beside the conv stack.  Measured on the
-    // rainbow step: no gain (noisy1_fwd 23.0 vs 22.2 us, step 253 vs 244 us) — the layer is bound by its per-CTA pipeline,
-    // not by DRAM — so it is off by default.
-    static const bool prefetch = getenv("DZ_PREFETCH") != nullptr && getenv("DZ_PREFETCH")[0] == '1';
-    if (prefetch && c.kind != DZ_IQN && l->side) DZ_TRY(um_prefetch_fc(l->um, fork_side(l, stream)));
     DZ_TRY(um_forward_torso(l->um, rows, stream));
     DZ_TRY(join_side(l, stream));
     if (c.kind != DZ_IQN) DZ_TRY(um_forward_fc(l->um, batch->d_noise, stream));
@@ -2564,7 +2439,6 @@ int dz_learner_plan_query(const dz_learner_config* cfg, dz_learner_plan* out) {
   out->param_count = tmp.lay.total;
   out->num_tensors = (int32_t)tmp.lay.t.size();
   out->opt_state_floats = 2 * tmp.lay.total;
-  read_env();
   out->workspace_bytes = carve(&tmp, nullptr);
   out->noise_floats = cfg->kind == DZ_RAINBOW ? 3 * noise_stride(*cfg, tmp.d) : 0;
   out->tau_floats = cfg->kind == DZ_IQN
@@ -2589,7 +2463,6 @@ int dz_learner_create(const dz_learner_config* cfg, const dz_learner_buffers* bu
   DZ_TRY(validate(*cfg));
   if (!buf->d_online || !buf->d_target || !buf->d_grads || !buf->d_opt_state || !buf->d_workspace || !buf->d_counters)
     return fail(DZ_EINVAL, "all learner buffers are required");
-  read_env();
   dz_learner* l = new dz_learner();
   l->cfg = *cfg;
   l->buf = *buf;
@@ -2617,20 +2490,11 @@ int dz_learner_create(const dz_learner_config* cfg, const dz_learner_buffers* bu
   }
   l->side = nullptr; l->ev_fork = nullptr; l->ev_join = nullptr; l->side_dirty = false;
   l->side2 = nullptr; l->ev_fork2 = nullptr; l->ev_join2 = nullptr; l->side2_dirty = false;
-  if (getenv("DZ_NO_SIDE_STREAM") == nullptr) {
-    if (cudaStreamCreateWithFlags(&l->side, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&l->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&l->ev_join, cudaEventDisableTiming) != cudaSuccess) {
-      l->side = nullptr;
-      cudaGetLastError();
-    }
-    if (l->side && (cudaStreamCreateWithFlags(&l->side2, cudaStreamNonBlocking) != cudaSuccess ||
-                    cudaEventCreateWithFlags(&l->ev_fork2, cudaEventDisableTiming) != cudaSuccess ||
-                    cudaEventCreateWithFlags(&l->ev_join2, cudaEventDisableTiming) != cudaSuccess)) {
-      l->side2 = nullptr;
-      cudaGetLastError();
-    }
-  }
+  cudaError_t se = cudaStreamCreateWithFlags(&l->side, cudaStreamNonBlocking);
+  if (se == cudaSuccess) se = cudaStreamCreateWithFlags(&l->side2, cudaStreamNonBlocking);
+  for (cudaEvent_t* ev : {&l->ev_fork, &l->ev_join, &l->ev_fork2, &l->ev_join2})
+    if (se == cudaSuccess) se = cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
+  if (se != cudaSuccess) { dz_learner_destroy(l); return fail(DZ_ECUDA, "side streams: %s", cudaGetErrorString(se)); }
   if (l->pk_on) {
     // fused epilogues only write the valid region of these images: zero the padding once, and set the constant
     // row of ones (bias-gradient row) of the transposed activation image
@@ -2660,6 +2524,8 @@ void dz_learner_destroy(dz_learner* l) {
   if (l->side2) { cudaStreamSynchronize(l->side2); cudaStreamDestroy(l->side2); }
   if (l->ev_fork) cudaEventDestroy(l->ev_fork);
   if (l->ev_join) cudaEventDestroy(l->ev_join);
+  if (l->ev_fork2) cudaEventDestroy(l->ev_fork2);
+  if (l->ev_join2) cudaEventDestroy(l->ev_join2);
   delete l;
 }
 
@@ -2672,7 +2538,7 @@ int dz_learner_learn(dz_learner* l, const dz_replay_view* replay, int32_t priori
   BatchExtras ex{l->rows_sample[0], l->rows_sample[1], l->s_a, l->s_r, l->s_d, prioritized ? l->s_w : nullptr, 1};
   if (replay->obs_bytes != (int64_t)l->d.H * l->d.W * l->d.C) return fail(DZ_EINVAL, "replay observation size does not match the network");
   // conv weight images do not depend on the sampled batch: pack them on the side stream while the sampler runs
-  const bool pack_aside = l->um != nullptr && l->side != nullptr;
+  const bool pack_aside = l->um != nullptr;
   if (pack_aside) {
     void* ws = fork_side(l, stream);
     DZ_TRY(um_pack_weights(l->um, ws));
@@ -2820,7 +2686,7 @@ int dz_test_learner_buffer(dz_learner* l, const char* name, float** d_ptr, int64
   else if (n == "h1") { *d_ptr = l->h1[0][0]; *count = rows0 * 512; }
   else if (n == "dh1") { *d_ptr = l->dh1[0]; *count = rows0 * 512; }
   else if (n == "iqn_hi") {
-    if (l->pk_on) return fail(DZ_EINVAL, "iqn_hi is not materialised on the packed tensor-core path (DZ_PK_IQN=0 keeps it)");
+    if (l->pk_on) return fail(DZ_EINVAL, "iqn_hi is not materialised on the packed tensor-core path");
     *d_ptr = l->hi[0]; *count = l->hi[0] ? rows0 * l->d.feat : 0;
   }
   else if (n == "iqn_dhi") { *d_ptr = l->dhi; *count = l->dhi ? rows0 * l->d.feat : 0; }

@@ -15,11 +15,7 @@ namespace dz {
 namespace {
 
 constexpr int kPrecisionBits = 32 - 8 - 2;   // Pillow Resample.c PRECISION_BITS for 8-bit images
-int g_band_rows = 0;                          // output rows per CTA (DZ_PRE_BAND overrides the default 12: 84 rows = 7 bands)
-int band_rows() {
-  if (g_band_rows == 0) { const char* e = getenv("DZ_PRE_BAND"); g_band_rows = e ? atoi(e) : 12; if (g_band_rows < 1) g_band_rows = 12; }
-  return g_band_rows;
-}
+constexpr int kBandRowsPerCTA = 12;           // output rows per CTA: 84 rows = 7 bands
 
 struct PreprocessArgs {
   const uint8_t* const* frame_a;
@@ -227,17 +223,17 @@ extern "C" int dz_atari_preprocess(const uint8_t* const* d_frame_a, const uint8_
   size_t smem = (size_t)max_band_rows * (2 * horizontal->in_size * 3 + horizontal->in_size + horizontal->out_size);
   smem = (smem + 15) / 16 * 16;
   a.tab_offset = (int)smem;
-  smem += sizeof(int32_t) * ((size_t)horizontal->out_size * (2 + horizontal->ksize) + (size_t)band_rows() * (2 + vertical->ksize) + 1) + 16;
-  a.band = band_rows();
+  smem += sizeof(int32_t) * ((size_t)horizontal->out_size * (2 + horizontal->ksize) + (size_t)kBandRowsPerCTA * (2 + vertical->ksize) + 1) + 16;
+  a.band = kBandRowsPerCTA;
   if (smem > 200 * 1024) return fail(DZ_EINVAL, "dz_atari_preprocess: band does not fit in shared memory");
   static size_t configured = 0;
   if (smem > 48 * 1024 && smem > configured) {
     DZ_CUDA_OK(cudaFuncSetAttribute(atari_preprocess_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = smem;
   }
-  dim3 grid((unsigned)ceil_div(vertical->out_size, band_rows()), (unsigned)n_env);
+  dim3 grid((unsigned)ceil_div(vertical->out_size, kBandRowsPerCTA), (unsigned)n_env);
   DZ_LAUNCH(atari_preprocess_kernel, grid, 256, smem, stream, a);
   return DZ_OK;
 }
 
-extern "C" int32_t dz_atari_preprocess_band_rows(void) { return band_rows(); }
+extern "C" int32_t dz_atari_preprocess_band_rows(void) { return kBandRowsPerCTA; }

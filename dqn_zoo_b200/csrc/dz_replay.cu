@@ -14,8 +14,6 @@ thread_local std::string g_last_error;
 std::atomic<int64_t> g_launches{0};
 std::vector<timeline_setter_t>& timeline_setters() { static std::vector<timeline_setter_t> v; return v; }
 void timeline_register(timeline_setter_t fn) { timeline_setters().push_back(fn); }
-int g_pdl = -1;
-int g_carveout = -1;
 bool g_profile = false;
 
 namespace {

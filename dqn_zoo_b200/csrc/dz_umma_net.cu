@@ -630,18 +630,6 @@ __global__ void __launch_bounds__(256) um_wgrad_finish_kernel(const __grid_const
   }
 }
 
-// L2 prefetch of the 3136 -> 512 weight matrices (both parameter sets): issued on the side stream at the start of the
-// step, while the sampler and the conv stack keep HBM idle, so that the weight-streaming GEMM later reads L2, not DRAM.
-struct PrefetchArgs { const float* ptr[8]; long long lines[8]; int n; };
-__global__ void __launch_bounds__(256) um_prefetch_kernel(const __grid_constant__ PrefetchArgs a) {
-  dz::pdl_enter();
-  for (int t = 0; t < a.n; ++t) {
-    const char* base = reinterpret_cast<const char*>(a.ptr[t]);
-    for (long long i = blockIdx.x * 256LL + threadIdx.x; i < a.lines[t]; i += (long long)gridDim.x * 256)
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(base + i * 128));
-  }
-}
-
 }  // namespace
 
 int um_split(const float* x, float* hi, float* lo, long long n, void* stream);   // dz_umma.cu
@@ -1324,22 +1312,6 @@ int um_pack_weights(UmNet* n, void* stream) {
   a.wd3_hi = n->wd3_hi; a.wd3_lo = n->wd3_lo; a.wd2_hi = n->wd2_hi; a.wd2_lo = n->wd2_lo;
   const int total = 2 * 77824 + 64 * 576 + 128 * 256;
   DZ_LAUNCH_NAMED("conv_pack", um_pack_conv_kernel, (unsigned)ceil_div(total, 256), 256, 0, stream, a);
-  return DZ_OK;
-}
-
-int um_prefetch_fc(UmNet* n, void* stream) {
-  const UmNetDesc& d = n->d;
-  if (!d.use_fc) return DZ_OK;
-  PrefetchArgs a;
-  memset(&a, 0, sizeof(a));
-  const long long lines = ((long long)n->feat * 512 * 4 + 127) / 128;
-  for (int blob = 0; blob < 2; ++blob)
-    for (int s = 0; s < d.nstream; ++s)
-      for (int sg = 0; sg < (d.noisy ? 2 : 1); ++sg) {
-        a.ptr[a.n] = (blob ? d.target : d.online) + (sg ? d.off_fc_sw[s] : d.off_fc_w[s]);
-        a.lines[a.n++] = lines;
-      }
-  DZ_LAUNCH_NAMED("fc_prefetch", um_prefetch_kernel, kNumSMs * 4, 256, 0, stream, a);
   return DZ_OK;
 }
 

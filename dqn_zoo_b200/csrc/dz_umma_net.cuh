@@ -42,7 +42,6 @@ float* um_dh1_lo(UmNet* n, int stream);
 
 // One launch each unless noted.  rows[p]: row-pointer table of pass p (uint8 observations, gathered in place).
 int um_pack_weights(UmNet* n, void* stream);                                   // conv weight images (both nets)
-int um_prefetch_fc(UmNet* n, void* stream);                                    // L2 prefetch of the 3136 -> 512 weights (both nets)
 int um_forward_torso(UmNet* n, const uint8_t* const* const* rows, void* stream);   // conv1, conv2, conv3
 int um_forward_fc(UmNet* n, const float* noise, void* stream);                 // fc1 / noisy1 + finish -> h1
 int um_split_dh1(UmNet* n, void* stream);                                      // dh1 fp32 -> hi/lo (if the producer wrote fp32 only)

@@ -106,7 +106,15 @@ def rel_err(got, want):
 @pytest.mark.parametrize('hw,B', [(84, 32), (44, 5)])
 @pytest.mark.parametrize('kind', KINDS)
 def test_loss_and_gradients_match_oracle(kind, hw, B):
+  check_loss_and_gradients(kind, hw, B)
+
+
+def check_loss_and_gradients(kind, hw, B, fma_torso=False):
   spec, net, L, O, rs = make_case(kind, B, hw, seed=3)
+  if fma_torso:   # the tensor-core path must not be active, or the caller would not test the fp32-FMA torso
+    from dqn_zoo_b200 import _lib
+    with pytest.raises(ValueError):
+      _lib.call('dz_test_learner_trace', L._h, b'', 0)
   arrs, batch, w, taus_o, taus_flat, noise_o, noise_flat = make_batch(spec, net, B, rs)
   tap = lo.ReluTap()
   loss, aux, grads = O.grads(batch, None if w is None else torch.tensor(w), taus_o, noise_o, tap=tap)
@@ -215,13 +223,12 @@ def test_update_is_run_to_run_deterministic():
   assert torch.equal(g1, L.grads)
 
 
+@pytest.mark.parametrize('hw,B', [(84, 65), (40, 32)])
 @pytest.mark.parametrize('kind', ['dqn', 'rainbow'])
-def test_fp32_fma_fallback_matches_oracle(kind, monkeypatch):
-  """DZ_UMMA=0 keeps every contraction on the fp32-FMA kernels (the path of geometries the tensor-core kernels do not cover,
-  e.g. tiny observations): same loss/gradient parity."""
-  monkeypatch.setenv('DZ_UMMA', '0')
-  test_loss_and_gradients_match_oracle(kind, 84, 32)
-  monkeypatch.delenv('DZ_UMMA')
+def test_fp32_fma_fallback_matches_oracle(kind, hw, B):
+  """Geometries the tensor-core torso does not cover run every contraction on the fp32-FMA kernels: batch > 64, and an
+  odd conv1 output (9x9 at 40x40; at batch <= 32 this also takes the split-K FMA layers).  Same loss/gradient parity."""
+  check_loss_and_gradients(kind, hw, B, fma_torso=True)
 
 
 def test_uint8_to_unit_conversion_is_correctly_rounded():
