@@ -33,6 +33,9 @@ inline int fail(int code, const char* fmt, const char* a = "", const char* b = "
     if (_e != cudaSuccess) return dz::fail(DZ_ECUDA, "%s: %s", #expr, cudaGetErrorString(_e)); \
   } while (0)
 
+// Returns a failing status code (anything but DZ_OK) from the enclosing function.
+#define DZ_TRY(expr) do { int _s = (expr); if (_s != DZ_OK) return _s; } while (0)
+
 // Optional per-launch CUDA-event timing (dz_profile_begin/end): used by bench.py to time the
 // dominant kernel on its own stream.  Off in every timed run.
 extern bool g_profile;
@@ -102,6 +105,8 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
   DZ_LAUNCH_NAMED(#kernel, kernel, grid, block, smem, stream, __VA_ARGS__)
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+// Output extent of a valid (unpadded) convolution: n inputs, kernel k, stride s.
+inline int conv_out(int n, int k, int s) { return (n - k) / s + 1; }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -61,6 +61,17 @@ struct PkProblem {
 struct PkBatch { PkProblem p[kPkMaxProblems]; int n; };
 
 
+// Packed "tile image" of a GEMM operand (dz_tcp.cuh) with `rows_pad` rows (multiple of the tile height) and `red_pad`
+// reduction elements (multiple of 16), rg = rows_pad / 8 row groups: the float index of element (row, r) is
+//     (((r / 16) * rg + row / 8) * 4 + (r % 16) / 4) * 32 + (row % 8) * 4 + r % 4
+// i.e. per 16-deep k-block all rows are contiguous, in 8-row x 16-byte blocks, so a (TR rows x 16) tile is TR * 64
+// contiguous bytes and the m16n8k8 fragment loads from it are bank-conflict free.
+__host__ __device__ __forceinline__ long long pk_index(int row, int r, int rg) {
+  return ((((long long)(r >> 4) * rg + (row >> 3)) * 4 + ((r & 15) >> 2)) << 5) + (row & 7) * 4 + (r & 3);
+}
+// Byte offset of element (row, r < kPkKB) inside one k-block of an image, i.e. 4 * pk_index(row, r, 0) in 32-bit
+// arithmetic.  Written out rather than through pk_index: the 64-bit form changes the GEMM's MMA loop code.
+__device__ __forceinline__ uint32_t pk_off(int row, int r) { return (uint32_t)((((row >> 3) * 4 + (r >> 2)) << 7) + ((row & 7) << 4) + ((r & 3) << 2)); }
 inline int64_t pk_image_floats(int rows_pad, int red_pad) { return (int64_t)rows_pad * red_pad; }
 int pk_add_job(PackBatch& pb, const float* src, int ld, int red_contig, int rows, int red, int rows_pad, int red_pad,
                int ones_row, float* hi, float* lo);

@@ -15,6 +15,7 @@
 #include <map>
 #include <vector>
 
+#include "dz_async.cuh"
 #include "dz_gemm.cuh"
 #include "dz_tc.cuh"
 #include "dz_internal.cuh"
@@ -39,8 +40,6 @@ struct Dims {
   int feat;          // h3*w3*64
   int out;           // head outputs (family dependent)
 };
-
-static inline int conv_out(int n, int k, int s) { return (n - k) / s + 1; }
 
 static Dims make_dims(const dz_learner_config& c) {
   Dims d;
@@ -251,9 +250,10 @@ __global__ void __launch_bounds__(256) finish_nt_kernel(const __grid_constant__ 
     if (f.mask && !(f.mask[i] > 0.f)) v = 0.f;
     f.out[i] = v;
     if (f.out_hi) {
-      const float h = tc::rn_tf32(v);
+      float h, l;
+      tc::split_tf32(v, h, l);
       f.out_hi[i] = h;
-      f.out_lo[i] = tc::rn_tf32(v - h);
+      f.out_lo[i] = l;
     }
   }
 }
@@ -289,13 +289,6 @@ __global__ void __launch_bounds__(256) col2im_kernel(const float* __restrict__ d
     }
     dx[i] = v;
   }
-}
-
-__global__ void add_mask_kernel(const float* __restrict__ a, const float* __restrict__ b, const float* __restrict__ act,
-                                float* __restrict__ out, long long n) {
-  dz::pdl_enter();
-  long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i < n) out[i] = act[i] > 0.f ? a[i] + b[i] : 0.f;
 }
 
 __global__ void sum_to_scalar_kernel(const float* __restrict__ v, int n, float* out) {
@@ -410,7 +403,7 @@ __global__ void __launch_bounds__(256) iqn_hadamard_bwd_kernel(float* __restrict
 }
 
 // Packed variant for the tensor-core path: same math, but dE is written ONLY as the hi/lo TF32 tile images of the
-// transposed operand (rows k, reduction m = b*N + n; layout in dz_tcp.cuh) that the embedding weight-gradient GEMM
+// transposed operand (rows k, reduction m = b*N + n; layout: pk_index) that the embedding weight-gradient GEMM
 // consumes.  One block = one sample b x 64 features; requires N == 64 and D % 64 == 0.
 __global__ void __launch_bounds__(256) iqn_hadamard_bwd_packed_kernel(const float* __restrict__ dHI, const float* __restrict__ E,
                                                                       const float* __restrict__ F, float* __restrict__ dfeat,
@@ -452,11 +445,8 @@ __global__ void __launch_bounds__(256) iqn_hadamard_bwd_packed_kernel(const floa
     const int k = k0 + rg * 8 + r, ml = kb * 16 + c * 4;
     float4 x = make_float4(tile[ml][rg * 8 + r], tile[ml + 1][rg * 8 + r], tile[ml + 2][rg * 8 + r], tile[ml + 3][rg * 8 + r]);
     float4 h, l;
-    h.x = tc::rn_tf32(x.x); l.x = tc::rn_tf32(x.x - h.x);
-    h.y = tc::rn_tf32(x.y); l.y = tc::rn_tf32(x.y - h.y);
-    h.z = tc::rn_tf32(x.z); l.z = tc::rn_tf32(x.z - h.z);
-    h.w = tc::rn_tf32(x.w); l.w = tc::rn_tf32(x.w - h.w);
-    const long long off = (((((long long)(b * 4 + kb) * rg_total + (k >> 3)) << 2) + c) << 5) + (k & 7) * 4;
+    tc::split_tf32(x, h, l);
+    const long long off = pk_index(k, b * N + ml, rg_total);
     *reinterpret_cast<float4*>(img_hi + off) = h;
     *reinterpret_cast<float4*>(img_lo + off) = l;
   }
@@ -1110,17 +1100,6 @@ constexpr int kOptStageBytes = 4 * kOptChunk * 16;        // p, g, m, v
 constexpr int kOptRingStages = 3;                         // OptArgs::stages of every launch
 constexpr int kOptBlocksPerSM = 4;
 
-__device__ __forceinline__ void opt_bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(tc::smem_u32(dst)),
-               "l"(__cvta_generic_to_global(src)), "r"(bytes), "r"(tc::smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void opt_bulk_store(void* dst, const void* src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(__cvta_generic_to_global(dst)),
-               "r"(tc::smem_u32(src)), "r"(bytes)
-               : "memory");
-}
-
 template <int KIND, int V>   // V = 2 floats per thread and stage: 512 threads
 __global__ void __launch_bounds__(kOptChunk * 4 / V, 4) optimizer_bulk_kernel(OptArgs o) {
   extern __shared__ __align__(128) unsigned char opt_sm[];
@@ -1135,8 +1114,8 @@ __global__ void __launch_bounds__(kOptChunk * 4 / V, 4) optimizer_bulk_kernel(Op
   float4* m4 = reinterpret_cast<float4*>(o.m);
   float4* v4 = reinterpret_cast<float4*>(o.v);
   if (tid == 0) {
-    for (int s = 0; s < kOptStages; ++s) tc::mbar_init(&full[s], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for (int s = 0; s < kOptStages; ++s) mbar_init(&full[s], 1);
+    fence_mbarrier_init();
   }
   __syncthreads();
   dz::pdl_enter();
@@ -1144,12 +1123,12 @@ __global__ void __launch_bounds__(kOptChunk * 4 / V, 4) optimizer_bulk_kernel(Op
     const long long c = blockIdx.x + it * gridDim.x;
     const long long q0 = c * kOptChunk;
     const uint32_t bytes = (uint32_t)(min((long long)kOptChunk, n4 - q0) * 16);
-    unsigned char* st = opt_sm + s * kOptStageBytes;
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(tc::smem_u32(&full[s])), "r"(4 * bytes) : "memory");
-    opt_bulk_load(st, p4 + q0, bytes, &full[s]);
-    opt_bulk_load(st + kOptChunk * 16, g4 + q0, bytes, &full[s]);
-    opt_bulk_load(st + 2 * kOptChunk * 16, m4 + q0, bytes, &full[s]);
-    opt_bulk_load(st + 3 * kOptChunk * 16, v4 + q0, bytes, &full[s]);
+    const uint32_t st = smem_u32(opt_sm + s * kOptStageBytes);
+    mbar_expect_tx(&full[s], 4 * bytes);
+    bulk_g2s(st, p4 + q0, bytes, &full[s]);
+    bulk_g2s(st + kOptChunk * 16, g4 + q0, bytes, &full[s]);
+    bulk_g2s(st + 2 * kOptChunk * 16, m4 + q0, bytes, &full[s]);
+    bulk_g2s(st + 3 * kOptChunk * 16, v4 + q0, bytes, &full[s]);
   };
   // the first loads are issued BEFORE the norm is formed: the split-norm reduction (shared memory, a block barrier,
   // ~700 L2 reads per block) then hides behind the memory latency of the stream instead of preceding it
@@ -1181,11 +1160,11 @@ __global__ void __launch_bounds__(kOptChunk * 4 / V, 4) optimizer_bulk_kernel(Op
     if (tid == 0 && it > 0) {   // refill the stage of iteration it - 1 as soon as its stores have finished READING it
       const long long next = it - 1 + kOptStages;
       if (next < mine) {
-        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+        bulk_wait_group_read();
         issue(next, s == 0 ? kOptStages - 1 : s - 1);
       }
     }
-    tc::mbar_wait(&full[s], phase);
+    mbar_wait(&full[s], phase);
     if (tid < 2 * valid) {
       float2 p = reinterpret_cast<float2*>(sp)[tid], g = reinterpret_cast<float2*>(sg)[tid];
       float2 m = reinterpret_cast<float2*>(smm)[tid], v = reinterpret_cast<float2*>(sv)[tid];
@@ -1193,18 +1172,18 @@ __global__ void __launch_bounds__(kOptChunk * 4 / V, 4) optimizer_bulk_kernel(Op
       p.y = opt_one<KIND>(o, p.y, g.y, m.y, v.y, clip, norm, c1, c2);
       reinterpret_cast<float2*>(sp)[tid] = p; reinterpret_cast<float2*>(smm)[tid] = m; reinterpret_cast<float2*>(sv)[tid] = v;
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the bulk stores
+    fence_proxy_async_shared();   // generic-proxy writes -> visible to the bulk stores
     __syncthreads();
     if (tid == 0) {
       const uint32_t bytes = (uint32_t)valid * 16;
-      opt_bulk_store(p4 + q0, sp, bytes);
-      opt_bulk_store(m4 + q0, smm, bytes);
-      opt_bulk_store(v4 + q0, sv, bytes);
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+      bulk_s2g(p4 + q0, sp, bytes);
+      bulk_s2g(m4 + q0, smm, bytes);
+      bulk_s2g(v4 + q0, sv, bytes);
+      bulk_commit_group();
     }
     if (++s == kOptStages) { s = 0; phase ^= 1u; }
   }
-  if (tid == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // stores complete before the grid does
+  if (tid == 0) bulk_wait_group();   // stores complete before the grid does
 }
 
 // epsilon-greedy over q[E][A] (dqn/agent.py:121-127): first maximum wins, as np.argmax / jnp.argmax.
@@ -1480,8 +1459,6 @@ int launch_batch(const char* tag, KernelT kernel, const GemmBatch& gb, dim3 grid
   DZ_LAUNCH_NAMED(tag, kernel, grid, threads, 0, stream, gb);
   return DZ_OK;
 }
-
-#define DZ_TRY(expr) do { int _s = (expr); if (_s != DZ_OK) return _s; } while (0)
 
 // ---- NN launch helpers (tile shapes chosen by M / N) -------------------------------------------
 

@@ -9,6 +9,7 @@
 // copies, takes their byte-wise max (__vmaxu4), converts to luma in float64 with the reference's rounding order (see oracle/processors_oracle.py:rgb2y —
 // products rounded separately, summed left to right, truncated), then runs Pillow's two fixed-point passes
 // (22-bit coefficients, int32 accumulators, uint8 intermediate image) out of shared memory.
+#include "dz_async.cuh"
 #include "dz_common.cuh"
 
 namespace dz {
@@ -30,32 +31,6 @@ struct PreprocessArgs {
   int tab_offset;                            // byte offset of the coefficient tables in shared memory
   int band;                                  // output rows per CTA
 };
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE_%=;\n"
-      "bra WAIT_%=;\n"
-      "DONE_%=:\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst_smem)),
-               "l"(__cvta_generic_to_global(src)), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
 
 __device__ __forceinline__ uint8_t clip8(int v) { return (uint8_t)(v < 0 ? 0 : (v > 255 ? 255 : v)); }
 
@@ -90,10 +65,10 @@ __global__ void __launch_bounds__(256) atari_preprocess_kernel(const PreprocessA
   const uint32_t bytes = (uint32_t)rows * (uint32_t)row_bytes;               // multiple of 16 (host-checked)
   if (threadIdx.x == 0) {
     mbar_init(bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbarrier_init();
     mbar_expect_tx(bar, (fa ? bytes : 0u) + (fb ? bytes : 0u));
-    if (fa) bulk_g2s(raw_a, fa + (size_t)r0 * row_bytes, bytes, bar);
-    if (fb) bulk_g2s(raw_b, fb + (size_t)r0 * row_bytes, bytes, bar);
+    if (fa) bulk_g2s(smem_u32(raw_a), fa + (size_t)r0 * row_bytes, bytes, bar);
+    if (fb) bulk_g2s(smem_u32(raw_b), fb + (size_t)r0 * row_bytes, bytes, bar);
   }
   for (int i = threadIdx.x; i < 2 * out_w; i += blockDim.x) hb[i] = a.h.d_bounds[i];
   for (int i = threadIdx.x; i < out_w * a.h.ksize; i += blockDim.x) hk[i] = a.h.d_kk[i];

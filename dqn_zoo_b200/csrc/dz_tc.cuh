@@ -1,5 +1,5 @@
-// Tensor-core helpers shared by the learner's GEMM kernels (sm_90a): mbarrier and elect.sync wrappers, the warp-level
-// m16n8k8 tf32 MMA with the shared-memory fragment loads of one k-step, and the tf32 split
+// Tensor-core helpers shared by the learner's GEMM kernels (sm_90a): the warp-level m16n8k8 tf32 MMA with the
+// shared-memory fragment loads of one k-step, the swizzled tile offsets, and the tf32 split
 //
 //     x = hi + lo,  hi = rn_tf32(x),  lo = rn_tf32(x - hi)      (error-compensated 3xTF32: D += Ah*Bh + Al*Bh + Ah*Bl)
 //
@@ -12,36 +12,6 @@
 
 namespace dz {
 namespace tc {
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// One lane of a converged warp.  With elect.sync ptxas knows that exactly one thread runs the guarded region and
-// emits the bulk-copy / TMA instructions back to back instead of wrapping each in a loop over the possibly-active lanes.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n .reg .pred P;\n elect.sync _|P, 0xffffffff;\n selp.u32 %0, 1, 0, P;\n}\n" : "=r"(pred));
-  return pred != 0;
-}
-
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE_%=;\n"
-      "bra WAIT_%=;\n"
-      "DONE_%=:\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
 
 // D += A * B for one 16 x 8 x 8 tile (mma.sync, fragments as in the PTX ISA's m16n8k8 .tf32 layout):
 //   a = {A[g][t], A[g+8][t], A[g][t+4], A[g+8][t+4]},  b = {B[t][g], B[t+4][g]},  d = {D[g][2t], D[g][2t+1], D[g+8][2t], D[g+8][2t+1]}
@@ -114,6 +84,16 @@ __device__ __forceinline__ float rn_tf32(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
   return __uint_as_float(r);
+}
+__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
+  hi = rn_tf32(x);
+  lo = rn_tf32(x - hi);
+}
+__device__ __forceinline__ void split_tf32(const float4& x, float4& hi, float4& lo) {
+  split_tf32(x.x, hi.x, lo.x);
+  split_tf32(x.y, hi.y, lo.y);
+  split_tf32(x.z, hi.z, lo.z);
+  split_tf32(x.w, hi.w, lo.w);
 }
 
 // 4x4 transpose across the 4 lanes of an aligned lane quad: on entry lane e holds S[r0+e][b..b+3],

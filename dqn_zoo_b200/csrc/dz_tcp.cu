@@ -22,7 +22,7 @@ namespace {
 __global__ void pk_ones_row_kernel(float* hi, int rg_total, int row, int red) {
   dz::pdl_enter();
   int m = blockIdx.x * blockDim.x + threadIdx.x;
-  if (m < red) hi[(((((long long)(m >> 4) * rg_total + (row >> 3)) << 2) + ((m & 15) >> 2)) << 5) + (row & 7) * 4 + (m & 3)] = 1.f;
+  if (m < red) hi[pk_index(row, m, rg_total)] = 1.f;
 }
 }  // namespace
 

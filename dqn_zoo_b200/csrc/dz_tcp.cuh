@@ -8,17 +8,14 @@
 // so that the GEMM's producer is ONE thread issuing cp.async.bulk copies that complete on an mbarrier and the
 // MMA warps read the stages as they landed.
 //
-// Image layout of an operand with `rows_pad` rows (multiple of the tile height) and `red_pad` reduction
-// elements (multiple of 16), RG = rows_pad / 8:
-//     float index of element (row, r) = (((r / 16) * RG + row / 8) * 4 + (r % 16) / 4) * 32 + (row % 8) * 4 + r % 4
-// i.e. per 16-deep k-block all rows are contiguous, 8-row x 16-byte blocks.  A (TR rows x 16) tile is TR * 64
-// contiguous bytes.
+// Image layout: pk_index (dz_internal.cuh).
 //
 // Accuracy: the tensor core adds into its fp32 accumulator with round-towards-zero, so the products of each
 // k-step are added into the fp32 sums with ordinary round-to-nearest adds (dz_tc.cuh, warp_kstep_3xtf32).
 #pragma once
-#include "dz_tc.cuh"
+#include "dz_async.cuh"
 #include "dz_internal.cuh"
+#include "dz_tc.cuh"
 
 namespace dz {
 
@@ -28,15 +25,6 @@ using namespace tc;
 
 constexpr int kEpiWarps = 8;
 constexpr int kThreadsP = (2 + kEpiWarps) * 32;
-
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
-               "l"(__cvta_generic_to_global(src)), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
 
 // ---- pack: fp32 matrix -> hi/lo tile images -----------------------------------------------------------------
 // One block = one 64-row x 64-deep tile, staged through shared memory so that both the source reads (either
@@ -89,11 +77,8 @@ __global__ void __launch_bounds__(256) tc_pack_kernel(const __grid_constant__ Pa
       const float* s = &tile[rg * 8 + r][kbl * 16 + c * 4];
       float4 x = make_float4(s[0], s[1], s[2], s[3]);
       float4 h, l;
-      h.x = rn_tf32(x.x); l.x = rn_tf32(x.x - h.x);
-      h.y = rn_tf32(x.y); l.y = rn_tf32(x.y - h.y);
-      h.z = rn_tf32(x.z); l.z = rn_tf32(x.z - h.z);
-      h.w = rn_tf32(x.w); l.w = rn_tf32(x.w - h.w);
-      const long long off = ((((long long)(red >> 4) * RG + (row >> 3)) * 4 + c) << 5) + r * 4;
+      split_tf32(x, h, l);
+      const long long off = pk_index(row, red, RG);
       *reinterpret_cast<float4*>(J.hi + off) = h;
       *reinterpret_cast<float4*>(J.lo + off) = l;
     }
@@ -109,9 +94,6 @@ struct PkSmem {
   static constexpr int kBars = 1024;
   static constexpr int kTotal = kBars + kStages * kStage;
 };
-
-// Byte offset of element (row, r) inside one part of a stage (kPkKB = 16: one k-block, RG = rows / 8 row groups).
-__device__ __forceinline__ uint32_t pk_off(int row, int r) { return (uint32_t)((((row >> 3) * 4 + (r >> 2)) << 7) + ((row & 7) << 4) + ((r & 3) << 2)); }
 
 // grid = (tiles_j, tiles_i * splits, problems); dynamic smem = PkSmem<BNJ, EPI>::kTotal; 320 threads:
 //   warp 0: producer (one lane issues the bulk copies)      warp 1: barrier set-up
@@ -146,7 +128,7 @@ __global__ void __launch_bounds__(kThreadsP, 1) tc_pgemm_kernel(const __grid_con
 
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kEpiWarps); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbarrier_init();
   }
   __syncthreads();
 
@@ -154,15 +136,13 @@ __global__ void __launch_bounds__(kThreadsP, 1) tc_pgemm_kernel(const __grid_con
     // ---------------------------------------------------------------- producer
     if (elect_one()) {
       const float* a_hi = p.A.hi; const float* a_lo = p.A.lo; const float* b_hi = p.B.hi; const float* b_lo = p.B.lo;
-      const long long a_rg = p.A.rg_total, b_rg = p.B.rg_total;
       for (int it = 0; it < nkb; ++it) {
         const int s = it % ST;
         const uint32_t ph = (uint32_t)(it / ST) & 1u;
         mbar_wait(&empty[s], ph ^ 1u);
         mbar_expect_tx(&full[s], (uint32_t)L::kStage);
-        const long long kb = kb0 + it;
-        const long long a_off = (kb * a_rg + (i0 >> 3)) * 128;       // floats: 4 chunks x 32 floats per row group
-        const long long b_off = (kb * b_rg + (j0 >> 3)) * 128;
+        const int r = (kb0 + it) * kPkKB;
+        const long long a_off = pk_index(i0, r, p.A.rg_total), b_off = pk_index(j0, r, p.B.rg_total);
         const uint32_t st = smem_u32(stage_base + (size_t)s * L::kStage);
         bulk_g2s(st, a_hi + a_off, L::kA, &full[s]);
         bulk_g2s(st + L::kA, a_lo + a_off, L::kA, &full[s]);
@@ -240,12 +220,9 @@ __global__ void __launch_bounds__(kThreadsP, 1) tc_pgemm_kernel(const __grid_con
             h = make_float4(v.x * m4.x, v.y * m4.y, v.z * m4.z, v.w * m4.w);
           }
           if (ok) {
-            const long long off = (((((long long)(j >> 4) * rg1 + (i >> 3)) << 2) + ((j & 15) >> 2)) << 5) + (i & 7) * 4;
+            const long long off = pk_index(i, j, rg1);
             float4 hh, ll;
-            hh.x = rn_tf32(h.x); ll.x = rn_tf32(h.x - hh.x);
-            hh.y = rn_tf32(h.y); ll.y = rn_tf32(h.y - hh.y);
-            hh.z = rn_tf32(h.z); ll.z = rn_tf32(h.z - hh.z);
-            hh.w = rn_tf32(h.w); ll.w = rn_tf32(h.w - hh.w);
+            split_tf32(h, hh, ll);
             *reinterpret_cast<float4*>(img_hi + off) = hh;
             *reinterpret_cast<float4*>(img_lo + off) = ll;
           }
@@ -253,12 +230,9 @@ __global__ void __launch_bounds__(kThreadsP, 1) tc_pgemm_kernel(const __grid_con
             const float4 ht = quad_transpose(h, lane);         // lane e: h[m0..m0+3] at column j + e
             const int jj = j + (lane & 3), m0 = i & ~3;
             if (m0 < p.MI && jj < NJ) {
-              const long long off = (((((long long)(m0 >> 4) * rgT + (jj >> 3)) << 2) + ((m0 & 15) >> 2)) << 5) + (jj & 7) * 4;
+              const long long off = pk_index(jj, m0, rgT);
               float4 hh, ll;
-              hh.x = rn_tf32(ht.x); ll.x = rn_tf32(ht.x - hh.x);
-              hh.y = rn_tf32(ht.y); ll.y = rn_tf32(ht.y - hh.y);
-              hh.z = rn_tf32(ht.z); ll.z = rn_tf32(ht.z - hh.z);
-              hh.w = rn_tf32(ht.w); ll.w = rn_tf32(ht.w - hh.w);
+              split_tf32(ht, hh, ll);
               *reinterpret_cast<float4*>(imgT_hi + off) = hh;
               *reinterpret_cast<float4*>(imgT_lo + off) = ll;
             }

@@ -98,8 +98,6 @@ int UmPlan::upload() {
   return DZ_OK;
 }
 
-#define DZ_TRY_CFG(expr) do { int _s = (expr); if (_s != DZ_OK) return _s; } while (0)
-
 int UmPlan::configure() {
   static bool done = false;
   if (done) return DZ_OK;
@@ -127,7 +125,7 @@ int UmPlan::launch(const char* tag, const UmLaunch& l, void* stream, long long* 
   if ((size_t)stages * l.stage_bytes < (size_t)128 * l.njt * 4) return fail(DZ_EINVAL, "umma launch: stage buffers smaller than the store-phase staging tile");
   const int v = l.njt == 32 ? 0 : 1;
   if (l.njt != 32 && l.njt != 64) return fail(DZ_EINVAL, "umma launch: NJT must be 32 or 64");
-  DZ_TRY_CFG(configure());
+  DZ_TRY(configure());
   um::UmMaps lm;
   for (int q = 0; q < l.nmaps; ++q) lm.m[q] = maps[l.map_ids[q]];
   for (int q = l.nmaps; q < um::kMaxMapsPerLaunch; ++q) lm.m[q] = maps[l.map_ids[0]];
@@ -145,9 +143,10 @@ __global__ void um_split_kernel(const float* __restrict__ x, float* __restrict__
   dz::pdl_enter();
   long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i < n) {
-    float h = tc::rn_tf32(x[i]);
+    float h, l;
+    tc::split_tf32(x[i], h, l);
     hi[i] = h;
-    lo[i] = tc::rn_tf32(x[i] - h);
+    lo[i] = l;
   }
 }
 }  // namespace
@@ -250,7 +249,7 @@ extern "C" int dz_test_umma_gemm(const float* d_A, int32_t a_mn_major, const flo
   rc = plan.localize_maps(l);
   if (rc == DZ_OK) rc = plan.upload();
   if (rc != DZ_OK) return rc;
-  l.njt = njt; l.stage_bytes = a_bytes + b_bytes; l.stages = stages > 0 ? stages : 4; l.convert = convert != 0;   // 4 x <= 48 KB + control block fits
+  l.njt = njt; l.stage_bytes = a_bytes + b_bytes; l.stages = stages > 0 ? stages : 4;   // 4 x <= 48 KB + control block fits
   rc = plan.launch("umma_selftest", l, stream);
   cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream);
   plan.release();

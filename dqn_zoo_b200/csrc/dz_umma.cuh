@@ -25,6 +25,7 @@
 #pragma once
 #include <cuda.h>
 
+#include "dz_async.cuh"
 #include "dz_internal.cuh"
 #include "dz_tc.cuh"
 
@@ -45,7 +46,6 @@ struct UmOperand {
                           //    137-178); the converters form w = mu + sigma * scale_r[r] * scale_i[i] and split THAT in place
   uint32_t mn_major;      // 0: K-major [rows][32 r];  1: MN-major slabs of [r rows][32 mn]
   uint32_t lbo;           // MN-major: bytes between 32-wide slabs (= r rows per stage * 128)
-  uint32_t kstep;         // bytes added to the descriptor start per MMA k-step of 8 (K-major 32, MN-major 1024)
   const float* scale_r;   // convert only: element *= scale_r[reduction index] before the split (noisy sigma weights)
   const float* scale_i;   // convert == 2 only: ... *= scale_i[row index of D / of the operand] (factorised noise, other factor)
 };
@@ -95,30 +95,6 @@ constexpr int kStagesMax = 8;
 constexpr int kConvWarps = 8;
 constexpr int kThreadsU = (2 + 4 + kConvWarps) * 32;   // producer, barrier set-up, 4 MMA / epilogue, 8 converter warps
 
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-
-__device__ __forceinline__ void tma_load_5d(uint32_t dst_smem, const void* map, uint64_t* bar, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(dst_smem),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-
-__device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
-               "l"(__cvta_generic_to_global(src)), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-
-__device__ __forceinline__ void split4(const float4 x, float4& h, float4& l) {
-  h.x = rn_tf32(x.x); l.x = rn_tf32(x.x - h.x);
-  h.y = rn_tf32(x.y); l.y = rn_tf32(x.y - h.y);
-  h.z = rn_tf32(x.z); l.z = rn_tf32(x.z - h.z);
-  h.w = rn_tf32(x.w); l.w = rn_tf32(x.w - h.w);
-}
-
 // In-place hi/lo split of one raw operand part (a sequence of 128-byte swizzled rows).  i0: MN index of the part's row 0.
 __device__ __forceinline__ void convert_part(const UmOperand& o, uint8_t* part0, int r0, int i0, int ct) {
   const int nchunks = (int)(o.part_bytes >> 4);
@@ -154,7 +130,7 @@ __device__ __forceinline__ void convert_part(const UmOperand& o, uint8_t* part0,
       }
     }
     float4 h, l;
-    split4(x, h, l);
+    split_tf32(x, h, l);
     *p = h;
     *p1 = l;
   }
@@ -205,7 +181,7 @@ __device__ __forceinline__ void convert_part16k(const UmOperand& o, uint8_t* par
     if (dual) { v.x = fmaf(g[j].x, f.x, v.x); v.y = fmaf(g[j].y, f.y, v.y); v.z = fmaf(g[j].z, f.z, v.z); v.w = fmaf(g[j].w, f.w, v.w); }
     else if (sc) { v.x *= f.x; v.y *= f.y; v.z *= f.z; v.w *= f.w; }
     float4 hh, ll;
-    split4(v, hh, ll);
+    split_tf32(v, hh, ll);
     *reinterpret_cast<float4*>(part0 + ((size_t)(ct + j * 256) << 4)) = hh;
     *reinterpret_cast<float4*>(part0 + 16384 + ((size_t)(ct + j * 256) << 4)) = ll;
   }
@@ -236,10 +212,9 @@ template <int NJT>
 __global__ void __launch_bounds__(kThreadsU, 1)
     umma_gemm_kernel(const __grid_constant__ UmMaps maps, const UmCta* __restrict__ ctas, const UmProblem* __restrict__ probs,
                      const UmTmaOp* __restrict__ ops, int nmaps, int stages, uint32_t stage_bytes, long long* __restrict__ trace) {
-  if (threadIdx.x < nmaps) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&maps.m[threadIdx.x])) : "memory");
+  if (threadIdx.x < nmaps) prefetch_tensormap(&maps.m[threadIdx.x]);
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
+  uint8_t* smem = smem_raw + smem_pad_1024(smem_raw);
   const bool tr = trace != nullptr && blockIdx.x == 0;
   // The plan tables (CTA descriptors, problems, TMA programs) are written once at plan upload, never by a kernel of the
   // step: the whole set-up below runs BEFORE griddepcontrol.wait, i.e. it overlaps the tail of the previous kernel
@@ -272,7 +247,7 @@ __global__ void __launch_bounds__(kThreadsU, 1)
   }
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&ready[s], kConvWarps); mbar_init(&empty[s], 4); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbarrier_init();
   }
   __syncthreads();
   // griddepcontrol.wait is executed per role, right before the role's first access to data an earlier kernel may have
@@ -385,7 +360,7 @@ __global__ void __launch_bounds__(kThreadsU, 1)
       if (fast_a) convert_part16k(oa, st, r0, ct, hoist);
       else if (conv_a) convert_part(oa, st, r0, cta.i0, ct);
       if (conv_b) convert_part(ob, st + a_bytes, r0, 0, ct);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // before the TMA unit refills the slot
+      fence_proxy_async_shared();   // before the TMA unit refills the slot
       __syncwarp();
       if (lane == 0) mbar_arrive(&ready[s]);
       r0 += red;
@@ -444,7 +419,7 @@ __global__ void __launch_bounds__(kThreadsU, 1)
         if (of) *reinterpret_cast<float4*>(of + o) = v;
         if (oh) {
           float4 h, l;
-          split4(v, h, l);
+          split_tf32(v, h, l);
           *reinterpret_cast<float4*>(oh + o) = h;
           *reinterpret_cast<float4*>(ol + o) = l;
         }

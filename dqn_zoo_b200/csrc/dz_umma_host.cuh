@@ -13,7 +13,6 @@ struct UmLaunch {
   int njt = 64;
   int stages = 4;
   uint32_t stage_bytes = 0;
-  bool convert = false;
   int nmaps = 0;
   int map_ids[um::kMaxMapsPerLaunch] = {0};   // plan map index of the launch-local map slot (the ops of this launch use slots)
 };
@@ -45,7 +44,7 @@ inline UmOperand um_kmajor(int rows, bool hi_lo, bool convert, const float* scal
   UmOperand o;
   memset(&o, 0, sizeof(o));
   o.part_bytes = (uint32_t)(((rows * 128) + 1023) / 1024 * 1024);
-  o.nparts = hi_lo ? 2 : 1; o.convert = convert ? 1 : 0; o.mn_major = 0; o.lbo = 0; o.kstep = 32; o.scale_r = scale_r;
+  o.nparts = hi_lo ? 2 : 1; o.convert = convert ? 1 : 0; o.mn_major = 0; o.lbo = 0; o.scale_r = scale_r;
   return o;
 }
 inline UmOperand um_mnmajor(int mn, int r_rows, bool convert, const float* scale_r = nullptr) {
@@ -53,7 +52,7 @@ inline UmOperand um_mnmajor(int mn, int r_rows, bool convert, const float* scale
   memset(&o, 0, sizeof(o));
   o.lbo = (uint32_t)(r_rows * 128);
   o.part_bytes = (uint32_t)((mn / 32) * o.lbo);
-  o.nparts = 2; o.convert = convert ? 1 : 0; o.mn_major = 1; o.kstep = 1024; o.scale_r = scale_r;
+  o.nparts = 2; o.convert = convert ? 1 : 0; o.mn_major = 1; o.scale_r = scale_r;
   return o;
 }
 

@@ -48,10 +48,6 @@ namespace {
 
 using namespace um;
 
-#define DZ_TRY_RC(expr) do { int _s = (expr); if (_s != DZ_OK) return _s; } while (0)
-
-inline int conv_out_dim(int n, int k, int s) { return (n - k) / s + 1; }
-
 // ------------------------------------------------------------------------------------------------
 // Conv weight images: K-major [N][K] tf32 hi/lo for the forward GEMMs (conv1 carries the 1/255 of networks.py:193),
 // and the input-gradient arrangements  Wd3[c][(kh,kw,n)] = W3[kh,kw,c,n],  Wd2[py,px][c][(ay,ax,n)] = W2[py+2ay,px+2ax,c,n].
@@ -95,9 +91,10 @@ __global__ void __launch_bounds__(256) um_pack_conv_kernel(const __grid_constant
       hi = a.wd2_hi + e; lo = a.wd2_lo + e;
     }
   }
-  const float h = rn_tf32(v);
+  float h, l;
+  split_tf32(v, h, l);
   *hi = h;
-  *lo = rn_tf32(v - h);
+  *lo = l;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -120,11 +117,67 @@ struct Conv1Args {
 
 constexpr int kC1W = 65536, kC1A = 131072;
 
+// Staging of the uint8 input rows.  For output-pixel tile [m0, m1), every image b the tile touches gets one segment of
+// the staging buffer, in image order: the contiguous input rows its output rows of the tile read (8x8 kernel, stride 4),
+// starting at input row `row0`.  px: output pixels per image, ow: output width, row_bytes: one input row.
+struct Conv1Segment { int row0, bytes; };
+__host__ __device__ __forceinline__ Conv1Segment conv1_segment(int b, int m0, int m1, int px, int ow, int row_bytes) {
+  const int plo = max(m0, b * px) - b * px, phi = min(m1, (b + 1) * px) - b * px;
+  const int oy0 = plo / ow;
+  return {4 * oy0, (4 * ((phi - 1) / ow - oy0) + 8) * row_bytes};
+}
+
+// Producer: bulk-copies the segments of tile [m0, m1) from the images' row pointers to `dst`, completing on `bar`.
+__device__ __forceinline__ void conv1_stage_tile(const uint8_t* const* rows, int m0, int m1, int px, int ow, int row_bytes,
+                                                 uint32_t dst, uint64_t* bar) {
+  const int b0 = m0 / px, b1 = (m1 - 1) / px;
+  uint32_t total = 0;
+  for (int b = b0; b <= b1; ++b) total += (uint32_t)conv1_segment(b, m0, m1, px, ow, row_bytes).bytes;
+  mbar_expect_tx(bar, total);
+  for (int b = b0; b <= b1; ++b) {
+    const Conv1Segment seg = conv1_segment(b, m0, m1, px, ow, row_bytes);
+    bulk_g2s(dst, rows[b] + (size_t)seg.row0 * row_bytes, (uint32_t)seg.bytes, bar);
+    dst += (uint32_t)seg.bytes;
+  }
+}
+
+// Converter: byte offset inside the staged tile [m0, m1) of the top-left input pixel of output pixel m's window.
+__device__ __forceinline__ int conv1_stage_offset(int m, int m0, int m1, int px, int ow, int row_bytes) {
+  const int b = m / px, p = m - b * px, oy = p / ow, ox = p - oy * ow;
+  int off = 0;
+  for (int bb = m0 / px; bb < b; ++bb) off += conv1_segment(bb, m0, m1, px, ow, row_bytes).bytes;
+  return off + (4 * oy - conv1_segment(b, m0, m1, px, ow, row_bytes).row0) * row_bytes + 16 * ox;
+}
+
+// Converter: one staged 32-byte kernel row (8 pixels x 4 channels) of tile row r, zeros when the row is beyond the batch ...
+__device__ __forceinline__ void conv1_load_row(const uint8_t* src, bool valid, uint4 (&u)[2]) {
+  if (valid) {
+    u[0] = *reinterpret_cast<const uint4*>(src);
+    u[1] = *reinterpret_cast<const uint4*>(src + 16);
+  } else {
+    u[0] = make_uint4(0, 0, 0, 0); u[1] = u[0];
+  }
+}
+// ... expanded to exact floats into row r of kernel row kh's slab of the swizzled K-major A tile [8 kh][128 r][32 (kw, c)].
+__device__ __forceinline__ void conv1_expand_row(const uint4 (&u)[2], uint8_t* a_tile, int kh, int r) {
+  uint8_t* dstrow = a_tile + kh * 16384 + r * 128;
+  const uint32_t w[8] = {u[0].x, u[0].y, u[0].z, u[0].w, u[1].x, u[1].y, u[1].z, u[1].w};
+#pragma unroll
+  for (int kw = 0; kw < 8; ++kw) {
+    // 0x4B000000 | byte = 8388608 + byte exactly; subtracting 2^23 leaves the byte as a float (an exact tf32 number)
+    float4 f;
+    f.x = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7440)) - 8388608.0f;
+    f.y = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7441)) - 8388608.0f;
+    f.z = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7442)) - 8388608.0f;
+    f.w = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7443)) - 8388608.0f;
+    *reinterpret_cast<float4*>(dstrow + ((kw ^ (r & 7)) << 4)) = f;
+  }
+}
+
 __global__ void __launch_bounds__(kThreadsU, 1) conv1_umma_kernel(const __grid_constant__ Conv1Args a) {
-  if (threadIdx.x < 4) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&a.wmap[threadIdx.x >> 1][threadIdx.x & 1])) : "memory");
+  if (threadIdx.x < 4) prefetch_tensormap(&a.wmap[threadIdx.x >> 1][threadIdx.x & 1]);
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
+  uint8_t* smem = smem_raw + smem_pad_1024(smem_raw);
   uint64_t* raw_full = reinterpret_cast<uint64_t*>(smem);   // [2] staged input rows landed
   uint64_t* raw_empty = raw_full + 2;                        // [2] converters are done reading them
   uint64_t* w_full = raw_empty + 2;                          // [1] weight image landed (only reloaded when the pass changes)
@@ -139,7 +192,7 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_umma_kernel(const __grid_c
     for (int b = 0; b < 2; ++b) { mbar_init(&raw_full[b], 1); mbar_init(&raw_empty[b], kConvWarps); }
     for (int j = 0; j < 4; ++j) { mbar_init(&a_ready[j], kConvWarps); mbar_init(&a_empty[j], 4); }
     mbar_init(w_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbarrier_init();
   }
   __syncthreads();
   dz::pdl_enter();                        // set-up above overlaps the previous kernel's tail; data accesses start here
@@ -161,22 +214,7 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_umma_kernel(const __grid_c
       const int m0 = (tile - pass * a.tiles_per_pass) * 128, m1 = min(m0 + 128, a.m_pass);
       mbar_wait(&raw_empty[buf], (((uint32_t)n >> 1) & 1u) ^ 1u);
       if (elect_one()) {
-        const int b0 = m0 / px, b1 = (m1 - 1) / px;
-        uint32_t total = 0;
-        for (int b = b0; b <= b1; ++b) {
-          const int plo = max(m0, b * px) - b * px, phi = min(m1, (b + 1) * px) - b * px;
-          total += (uint32_t)((4 * ((phi - 1) / a.ow - plo / a.ow) + 8) * row_bytes);
-        }
-        mbar_expect_tx(&raw_full[buf], total);
-        uint32_t off = 0;
-        const uint32_t dst0 = smem_u32(stag + (size_t)buf * a.stag_bytes);
-        for (int b = b0; b <= b1; ++b) {
-          const int plo = max(m0, b * px) - b * px, phi = min(m1, (b + 1) * px) - b * px;
-          const int oy0 = plo / a.ow;
-          const uint32_t bytes = (uint32_t)((4 * ((phi - 1) / a.ow - oy0) + 8) * row_bytes);
-          bulk_g2s(dst0 + off, a.rows[pass][b] + (size_t)(4 * oy0) * row_bytes, bytes, &raw_full[buf]);
-          off += bytes;
-        }
+        conv1_stage_tile(a.rows[pass], m0, m1, px, a.ow, row_bytes, smem_u32(stag + (size_t)buf * a.stag_bytes), &raw_full[buf]);
         if (tr && n < 64) a.trace[n] = clock64();                                                   // [0,64): row copies issued
       }
       __syncwarp();
@@ -240,10 +278,12 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_umma_kernel(const __grid_c
 #pragma unroll
           for (int nt = 0; nt < 4; ++nt) {
             const float v0 = fmaxf(sum[mt][nt][e], 0.f), v1 = fmaxf(sum[mt][nt][e + 1], 0.f);
-            const float h0 = rn_tf32(v0), h1 = rn_tf32(v1);
+            float h0, l0, h1, l1;
+            split_tf32(v0, h0, l0);
+            split_tf32(v1, h1, l1);
             const long long o = dst0 + row * 32 + frag_col(nt, e);
             *reinterpret_cast<float2*>(a.out_hi + o) = make_float2(h0, h1);
-            *reinterpret_cast<float2*>(a.out_lo + o) = make_float2(rn_tf32(v0 - h0), rn_tf32(v1 - h1));
+            *reinterpret_cast<float2*>(a.out_lo + o) = make_float2(l0, l1);
           }
         }
       if (tr && warp == 2 && lane == 0 && n < 64) a.trace[256 + n] = clock64();                     // [256,320): tile stored
@@ -259,18 +299,7 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_umma_kernel(const __grid_c
       const int m0 = (tile - pass * a.tiles_per_pass) * 128, m1 = min(m0 + 128, a.m_pass);
       const int m = m0 + r;
       const bool valid = m < m1;
-      // staging offset of this row's patch origin
-      int src_off = 0;
-      if (valid) {
-        const int b0 = m0 / px, b = m / px, p = m - b * px, oy = p / a.ow, ox = p - oy * a.ow;
-        int off = 0;
-        for (int bb = b0; bb < b; ++bb) {
-          const int plo = max(m0, bb * px) - bb * px, phi = min(m1, (bb + 1) * px) - bb * px;
-          off += (4 * ((phi - 1) / a.ow - plo / a.ow) + 8) * row_bytes;
-        }
-        const int plo = max(m0, b * px) - b * px;
-        src_off = off + (4 * (oy - plo / a.ow)) * row_bytes + 16 * ox;
-      }
+      const int src_off = valid ? conv1_stage_offset(m, m0, m1, px, a.ow, row_bytes) : 0;
       mbar_wait(&raw_full[buf], ((uint32_t)n >> 1) & 1u);
       if (tr && ct == 0 && n < 64) a.trace[64 + n] = clock64();                                     // [64,128): input rows landed
       const uint8_t* src = stag + (size_t)buf * a.stag_bytes + src_off;
@@ -278,25 +307,9 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_umma_kernel(const __grid_c
       for (int it = 0; it < 4; ++it) {
         const int kh = 2 * it + khp;
         uint4 u[2];
-        if (valid) {
-          u[0] = *reinterpret_cast<const uint4*>(src + kh * row_bytes);
-          u[1] = *reinterpret_cast<const uint4*>(src + kh * row_bytes + 16);
-        } else {
-          u[0] = make_uint4(0, 0, 0, 0); u[1] = u[0];
-        }
+        conv1_load_row(src + kh * row_bytes, valid, u);
         mbar_wait(&a_empty[it], ((uint32_t)n & 1u) ^ 1u);     // the previous tile's MMAs have consumed this kernel-row pair
-        uint8_t* dstrow = a_smem + kh * 16384 + r * 128;
-        const uint32_t w[8] = {u[0].x, u[0].y, u[0].z, u[0].w, u[1].x, u[1].y, u[1].z, u[1].w};
-#pragma unroll
-        for (int kw = 0; kw < 8; ++kw) {
-          // 0x4B000000 | byte = 8388608 + byte exactly; subtracting 2^23 leaves the byte as a float (an exact tf32 number)
-          float4 f;
-          f.x = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7440)) - 8388608.0f;
-          f.y = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7441)) - 8388608.0f;
-          f.z = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7442)) - 8388608.0f;
-          f.w = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7443)) - 8388608.0f;
-          *reinterpret_cast<float4*>(dstrow + ((kw ^ (r & 7)) << 4)) = f;
-        }
+        conv1_expand_row(u, a_smem, kh, r);
         __syncwarp();
         if (lane == 0) mbar_arrive(&a_ready[it]);
       }
@@ -322,10 +335,9 @@ struct Conv1WgArgs {
 constexpr int kC1G = 32768;      // dact1 tile: hi | lo, [128 rows][32 n] each
 
 __global__ void __launch_bounds__(kThreadsU, 1) conv1_wgrad_umma_kernel(const __grid_constant__ Conv1WgArgs a) {
-  if (threadIdx.x < 2) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&a.gmap[threadIdx.x])) : "memory");
+  if (threadIdx.x < 2) prefetch_tensormap(&a.gmap[threadIdx.x]);
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
+  uint8_t* smem = smem_raw + smem_pad_1024(smem_raw);
   uint64_t* raw_full = reinterpret_cast<uint64_t*>(smem);   // [2]
   uint64_t* raw_empty = raw_full + 2;                        // [2]
   uint64_t* g_full = raw_empty + 2;                          // [1] dact1 tile landed
@@ -340,7 +352,7 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_wgrad_umma_kernel(const __
     for (int b = 0; b < 2; ++b) { mbar_init(&raw_full[b], 1); mbar_init(&raw_empty[b], kConvWarps); }
     for (int j = 0; j < 4; ++j) mbar_init(&a_ready[j], kConvWarps);
     mbar_init(g_full, 1); mbar_init(t_done, 4);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    fence_mbarrier_init();
   }
   __syncthreads();
   dz::pdl_enter();                        // set-up above overlaps the previous kernel's tail; data accesses start here
@@ -356,24 +368,8 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_wgrad_umma_kernel(const __
       const int buf = n & 1;
       const int m0 = tile * 128, m1 = min(m0 + 128, a.m_pass);
       mbar_wait(&raw_empty[buf], (((uint32_t)n >> 1) & 1u) ^ 1u);
-      if (elect_one()) {
-        const int b0 = m0 / px, b1 = (m1 - 1) / px;
-        uint32_t total = 0;
-        for (int b = b0; b <= b1; ++b) {
-          const int plo = max(m0, b * px) - b * px, phi = min(m1, (b + 1) * px) - b * px;
-          total += (uint32_t)((4 * ((phi - 1) / a.ow - plo / a.ow) + 8) * row_bytes);
-        }
-        mbar_expect_tx(&raw_full[buf], total);
-        uint32_t off = 0;
-        const uint32_t dst0 = smem_u32(stag + (size_t)buf * a.stag_bytes);
-        for (int b = b0; b <= b1; ++b) {
-          const int plo = max(m0, b * px) - b * px, phi = min(m1, (b + 1) * px) - b * px;
-          const int oy0 = plo / a.ow;
-          const uint32_t bytes = (uint32_t)((4 * ((phi - 1) / a.ow - oy0) + 8) * row_bytes);
-          bulk_g2s(dst0 + off, a.rows[b] + (size_t)(4 * oy0) * row_bytes, bytes, &raw_full[buf]);
-          off += bytes;
-        }
-      }
+      if (elect_one())
+        conv1_stage_tile(a.rows, m0, m1, px, a.ow, row_bytes, smem_u32(stag + (size_t)buf * a.stag_bytes), &raw_full[buf]);
       __syncwarp();
       if (n > 0) mbar_wait(t_done, ((uint32_t)(n - 1)) & 1u);
       if (elect_one()) {
@@ -435,17 +431,7 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_wgrad_umma_kernel(const __
       const int m0 = tile * 128, m1 = min(m0 + 128, a.m_pass);
       const int m = m0 + r;
       const bool valid = m < m1;
-      int src_off = 0;
-      if (valid) {
-        const int b0 = m0 / px, b = m / px, p = m - b * px, oy = p / a.ow, ox = p - oy * a.ow;
-        int off = 0;
-        for (int bb = b0; bb < b; ++bb) {
-          const int plo = max(m0, bb * px) - bb * px, phi = min(m1, (bb + 1) * px) - bb * px;
-          off += (4 * ((phi - 1) / a.ow - plo / a.ow) + 8) * row_bytes;
-        }
-        const int plo = max(m0, b * px) - b * px;
-        src_off = off + (4 * (oy - plo / a.ow)) * row_bytes + 16 * ox;
-      }
+      const int src_off = valid ? conv1_stage_offset(m, m0, m1, px, a.ow, row_bytes) : 0;   // rows beyond the batch add zeros
       mbar_wait(&raw_full[buf], ((uint32_t)n >> 1) & 1u);
       if (n > 0) mbar_wait(t_done, ((uint32_t)(n - 1)) & 1u);     // previous tile's MMAs have consumed the A tile
       const uint8_t* src = stag + (size_t)buf * a.stag_bytes + src_off;
@@ -453,23 +439,8 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_wgrad_umma_kernel(const __
       for (int it = 0; it < 4; ++it) {
         const int kh = 2 * it + khp;
         uint4 u[2];
-        if (valid) {
-          u[0] = *reinterpret_cast<const uint4*>(src + kh * row_bytes);
-          u[1] = *reinterpret_cast<const uint4*>(src + kh * row_bytes + 16);
-        } else {
-          u[0] = make_uint4(0, 0, 0, 0); u[1] = u[0];     // rows beyond the batch contribute zeros to the reduction
-        }
-        uint8_t* dstrow = a_smem + kh * 16384 + r * 128;
-        const uint32_t w[8] = {u[0].x, u[0].y, u[0].z, u[0].w, u[1].x, u[1].y, u[1].z, u[1].w};
-#pragma unroll
-        for (int kw = 0; kw < 8; ++kw) {
-          float4 f;
-          f.x = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7440)) - 8388608.0f;
-          f.y = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7441)) - 8388608.0f;
-          f.z = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7442)) - 8388608.0f;
-          f.w = __uint_as_float(__byte_perm(w[kw], 0x4B000000u, 0x7443)) - 8388608.0f;
-          *reinterpret_cast<float4*>(dstrow + ((kw ^ (r & 7)) << 4)) = f;
-        }
+        conv1_load_row(src + kh * row_bytes, valid, u);
+        conv1_expand_row(u, a_smem, kh, r);
         __syncwarp();
         if (lane == 0) mbar_arrive(&a_ready[it]);
       }
@@ -530,7 +501,7 @@ __global__ void __launch_bounds__(256) um_fcd_finish_kernel(const float* __restr
     const float4 m = *reinterpret_cast<const float4*>(act_hi + i);
     v.x = m.x > 0.f ? v.x : 0.f; v.y = m.y > 0.f ? v.y : 0.f; v.z = m.z > 0.f ? v.z : 0.f; v.w = m.w > 0.f ? v.w : 0.f;
     float4 h, l;
-    split4(v, h, l);
+    split_tf32(v, h, l);
     *reinterpret_cast<float4*>(out + i) = v;
     *reinterpret_cast<float4*>(out_hi + i) = h;
     *reinterpret_cast<float4*>(out_lo + i) = l;
@@ -641,10 +612,10 @@ int um_split(const float* x, float* hi, float* lo, long long n, void* stream);  
 bool um_net_supported(const UmNetDesc& d) {
   if (d.B < 1 || d.B > 64 || d.npass < 1 || d.npass > 3) return false;
   if (d.W % 4 || d.H < 36 || d.W < 36) return false;
-  const int h1 = conv_out_dim(d.H, 8, 4), w1 = conv_out_dim(d.W, 8, 4);
+  const int h1 = conv_out(d.H, 8, 4), w1 = conv_out(d.W, 8, 4);
   if ((h1 & 1) || (w1 & 1)) return false;              // stride-2 parity view of act1
-  const int h2 = conv_out_dim(h1, 4, 2), w2 = conv_out_dim(w1, 4, 2);
-  const int h3 = conv_out_dim(h2, 3, 1), w3 = conv_out_dim(w2, 3, 1);
+  const int h2 = conv_out(h1, 4, 2), w2 = conv_out(w1, 4, 2);
+  const int h3 = conv_out(h2, 3, 1), w3 = conv_out(w2, 3, 1);
   if (h3 < 1 || w3 < 1) return false;
   if (h2 * w2 > 128 || (h1 / 2) * (w1 / 2) > 128 || h3 * w3 > 128) return false;
   if (h1 * w1 < 64) return false;                      // a 128-pixel conv1 tile spans at most 3 images
@@ -669,9 +640,9 @@ namespace {
 struct Geo { int h1, w1, h2, w2, h3, w3, feat, PB; };
 Geo geo_of(const UmNetDesc& d) {
   Geo g;
-  g.h1 = conv_out_dim(d.H, 8, 4); g.w1 = conv_out_dim(d.W, 8, 4);
-  g.h2 = conv_out_dim(g.h1, 4, 2); g.w2 = conv_out_dim(g.w1, 4, 2);
-  g.h3 = conv_out_dim(g.h2, 3, 1); g.w3 = conv_out_dim(g.w2, 3, 1);
+  g.h1 = conv_out(d.H, 8, 4); g.w1 = conv_out(d.W, 8, 4);
+  g.h2 = conv_out(g.h1, 4, 2); g.w2 = conv_out(g.w1, 4, 2);
+  g.h3 = conv_out(g.h2, 3, 1); g.w3 = conv_out(g.w2, 3, 1);
   g.feat = g.h3 * g.w3 * 64; g.PB = d.npass * d.B;
   return g;
 }
@@ -1127,7 +1098,7 @@ int build_plan(UmNet* n) {
     {
       UmOperand Bo = um_kmajor(njt, true, false);
       const int nk = feat / 32, S = n->fc_splits, per = (nk + S - 1) / S;
-      n->l_fc.cta0 = (int)pl.ctas.size(); n->l_fc.njt = njt; n->l_fc.convert = true;
+      n->l_fc.cta0 = (int)pl.ctas.size(); n->l_fc.njt = njt;
       n->l_fc.stage_bytes = 2 * 16384 + 2 * Bo.part_bytes;
       n->l_fc.stages = std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_fc.stage_bytes));
       for (int p = 0; p < d.npass; ++p) {
@@ -1174,7 +1145,7 @@ int build_plan(UmNet* n) {
     {
       UmOperand Bo = um_kmajor(njt, true, false);
       const int S = n->fcd_splits, per = (16 + S - 1) / S, ktiles = (feat + 127) / 128;
-      n->l_fcd.cta0 = (int)pl.ctas.size(); n->l_fcd.njt = njt; n->l_fcd.convert = true;
+      n->l_fcd.cta0 = (int)pl.ctas.size(); n->l_fcd.njt = njt;
       n->l_fcd.stage_bytes = 2 * 16384 + 2 * Bo.part_bytes;
       n->l_fcd.stages = std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_fcd.stage_bytes));
       for (int s = 0; s < d.nstream; ++s) {
@@ -1249,10 +1220,7 @@ int um_net_create(const UmNetDesc& d, char* base, UmNet** out) {
   for (int m0 = 0; m0 < m_pass; m0 += 128) {
     const int m1 = std::min(m0 + 128, m_pass);
     int tot = 0;
-    for (int b = m0 / px; b <= (m1 - 1) / px; ++b) {
-      const int plo = std::max(m0, b * px) - b * px, phi = std::min(m1, (b + 1) * px) - b * px;
-      tot += (4 * ((phi - 1) / n->w1 - plo / n->w1) + 8) * d.W * 4;
-    }
+    for (int b = m0 / px; b <= (m1 - 1) / px; ++b) tot += conv1_segment(b, m0, m1, px, n->w1, d.W * 4).bytes;
     worst = std::max(worst, tot);
   }
   n->conv1_stag_bytes = (worst + 127) / 128 * 128;
@@ -1335,16 +1303,16 @@ int um_forward_torso(UmNet* n, const uint8_t* const* const* rows, void* stream) 
   if (smem > 227 * 1024) return fail(DZ_EINVAL, "conv1 staging does not fit");
   const unsigned grid = (unsigned)std::min(kNumSMs, a.ntiles);
   DZ_LAUNCH_NAMED("conv1_fwd", conv1_umma_kernel, grid, kThreadsU, smem, stream, a);
-  DZ_TRY_RC(n->plan.launch("conv2_fwd", n->l_conv2, stream, n->tr("conv2_fwd")));
-  DZ_TRY_RC(n->plan.launch("conv3_fwd", n->l_conv3, stream, n->tr("conv3_fwd")));
+  DZ_TRY(n->plan.launch("conv2_fwd", n->l_conv2, stream, n->tr("conv2_fwd")));
+  DZ_TRY(n->plan.launch("conv3_fwd", n->l_conv3, stream, n->tr("conv3_fwd")));
   return DZ_OK;
 }
 
 int um_forward_fc(UmNet* n, const float* noise, void* stream) {
   const UmNetDesc& d = n->d;
   if (!d.use_fc) return fail(DZ_EINVAL, "fc layers are not on the tensor-core path for this agent");
-  if (d.noisy) DZ_TRY_RC(apply_noise(n, noise, stream));
-  DZ_TRY_RC(n->plan.launch(d.noisy ? "noisy1_fwd" : "fc1_fwd", n->l_fc, stream, n->tr("fc1_fwd")));
+  if (d.noisy) DZ_TRY(apply_noise(n, noise, stream));
+  DZ_TRY(n->plan.launch(d.noisy ? "noisy1_fwd" : "fc1_fwd", n->l_fc, stream, n->tr("fc1_fwd")));
   FcFinishArgs a;
   memset(&a, 0, sizeof(a));
   a.part = n->fc_part; a.S = n->fc_splits; a.B = d.B; a.nstream = d.nstream; a.noisy = d.noisy; a.npass = d.npass; a.h1 = n->h1_buf;
@@ -1369,8 +1337,8 @@ int um_split_dh1(UmNet* n, void* stream) {
 int um_backward_fc(UmNet* n, const float* noise, void* stream) {
   const UmNetDesc& d = n->d;
   if (!d.use_fc) return fail(DZ_EINVAL, "fc layers are not on the tensor-core path for this agent");
-  if (d.noisy) DZ_TRY_RC(apply_noise(n, noise, stream));
-  DZ_TRY_RC(n->plan.launch(d.noisy ? "noisy1_dgrad" : "fc1_dgrad", n->l_fcd, stream, n->tr("fc1_dgrad")));
+  if (d.noisy) DZ_TRY(apply_noise(n, noise, stream));
+  DZ_TRY(n->plan.launch(d.noisy ? "noisy1_dgrad" : "fc1_dgrad", n->l_fcd, stream, n->tr("fc1_dgrad")));
   const long long total = (long long)d.B * n->feat;
   DZ_LAUNCH_NAMED("fcd_finish", um_fcd_finish_kernel, (unsigned)std::min<long long>(ceil_div(total / 4, 256), kNumSMs * 4), 256, 0, stream,
                   n->fcd_part, n->fcd_nsrc * n->fcd_splits, total, n->act_hi[2], n->dact_f32[2], n->dact_hi[2], n->dact_lo[2], total / 4);
