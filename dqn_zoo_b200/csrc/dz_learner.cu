@@ -74,8 +74,10 @@ struct Layout {
     index[name] = (int)t.size();
     t.push_back(ti);
   }
-  int64_t off(const std::string& name) const { return t[index.at(name)].offset; }
-  bool has(const std::string& name) const { return index.count(name) != 0; }
+  int64_t off(const std::string& name) const {   // -1: no such tensor
+    auto it = index.find(name);
+    return it == index.end() ? -1 : t[it->second].offset;
+  }
 };
 
 static Layout make_layout(const dz_learner_config& c) {
@@ -101,6 +103,52 @@ static Layout make_layout(const dz_learner_config& c) {
   bool shared = c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED;
   L.add("head/b", {shared ? 1 : d.out});
   return L;
+}
+
+// Offsets into a parameter blob of every tensor the step's launches address; -1 where the agent kind has no such tensor.
+// Stream s = 0 is fc1 (rainbow: the advantage stream), s = 1 rainbow's value stream.  Layer 1 is the 512-wide layer,
+// layer 2 the head (plain heads: head/w, head/b; rainbow's mu has no bias).  sw / sb: noisy sigma weight / bias.
+struct ParamOffsets {
+  int64_t conv_w[3], conv_b[3];
+  int64_t w1[2], b1[2], sw1[2], sb1[2];
+  int64_t w2[2], b2[2], sw2[2], sb2[2];
+  int64_t embed_w, embed_b;
+  int64_t fc_begin;   // first offset after the conv tensors
+};
+
+static int param_offsets(const dz_learner_config& c, const Layout& L, ParamOffsets* out) {
+  ParamOffsets o;
+  bool missing = false;
+  auto need = [&](const std::string& name) {
+    const int64_t off = L.off(name);
+    missing |= off < 0;
+    return off;
+  };
+  for (int i = 0; i < 3; ++i) {
+    const std::string conv = "conv" + std::to_string(i + 1);
+    o.conv_w[i] = need(conv + "/w"); o.conv_b[i] = need(conv + "/b");
+  }
+  for (int s = 0; s < 2; ++s) {
+    o.w1[s] = o.b1[s] = o.sw1[s] = o.sb1[s] = -1;
+    o.w2[s] = o.b2[s] = o.sw2[s] = o.sb2[s] = -1;
+  }
+  o.embed_w = o.embed_b = -1;
+  if (c.kind == DZ_RAINBOW) {
+    const char* streams[2] = {"adv", "val"};
+    for (int s = 0; s < 2; ++s) {
+      const std::string p = streams[s];
+      o.w1[s] = need(p + "1/mu/w"); o.b1[s] = need(p + "1/mu/b"); o.sw1[s] = need(p + "1/sigma/w"); o.sb1[s] = need(p + "1/sigma/b");
+      o.w2[s] = need(p + "2/mu/w"); o.sw2[s] = need(p + "2/sigma/w"); o.sb2[s] = need(p + "2/sigma/b");
+    }
+  } else {
+    o.w1[0] = need("fc1/w"); o.b1[0] = need("fc1/b");
+    o.w2[0] = need("head/w"); o.b2[0] = need("head/b");
+    if (c.kind == DZ_IQN) { o.embed_w = need("embed/w"); o.embed_b = need("embed/b"); }
+  }
+  o.fc_begin = c.kind == DZ_IQN ? o.embed_w : o.w1[0];
+  if (missing) return fail(DZ_EINVAL, "parameter layout lacks a tensor of this agent kind");
+  *out = o;
+  return DZ_OK;
 }
 
 struct Bump {
@@ -559,140 +607,9 @@ __global__ void __launch_bounds__(64) loss_q_kernel(LossArgs L) {
 }
 
 // c51 / rainbow: categorical_[double_]q_learning with categorical_l2_project + cross entropy.
-// One CTA (4 warps) per example.  Softmaxes run one warp per (pass, action) with shuffle reductions, so the
-// whole kernel has five block barriers.
-__device__ __forceinline__ float warp_sum_all(float v) { return warp_sum(v); }
-
-__global__ void __launch_bounds__(128) loss_categorical_kernel(LossArgs L) {
-  dz::pdl_enter();
-  extern __shared__ float sm[];
-  const int b = blockIdx.x, K = L.atoms, A = L.A, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  float* cm_sel = sm;            // [K] mean over actions of the selector-pass advantages (rainbow)
-  float* cm_tgt = cm_sel + K;    // [K] same for the target pass
-  float* cm_tm1 = cm_tgt + K;    // [K] same for the online(s_tm1) pass
-  float* p_tgt = cm_tm1 + K;     // [K]
-  float* proj = p_tgt + K;       // [K]
-  float* p_tm1 = proj + K;       // [K] softmax(logits_tm1[a_tm1])
-  float* qsel = p_tm1 + K;       // [A]
-  float* scal = qsel + A;        // [4]: loss, sum(proj)
-  const bool rb = L.kind == DZ_RAINBOW;
-  auto support = [&](int i) { return (float)((double)(-L.vmax) + (double)i * (2.0 * (double)L.vmax / (double)(K - 1))); };
-
-  // 0. dueling column means (networks.py:251: mean over the action axis)
-  if (rb) {
-    for (int k = tid; k < K; k += blockDim.x) {
-      float m1 = 0.f, m2 = 0.f, m0 = 0.f;
-      for (int a = 0; a < A; ++a) {
-        m1 += L.adv1[((long long)b * A + a) * K + k];
-        m2 += L.adv2[((long long)b * A + a) * K + k];
-        m0 += L.adv0[((long long)b * A + a) * K + k];
-      }
-      cm_sel[k] = m1 / (float)A; cm_tgt[k] = m2 / (float)A; cm_tm1[k] = m0 / (float)A;
-    }
-  }
-  __syncthreads();
-  // logit k of (pass, action): pass 0 = online(s_tm1), 1 = selector, 2 = target
-  auto logit_of = [&](int pass, int a, int k) -> float {
-    if (rb) {
-      const float* adv = pass == 0 ? L.adv0 : (pass == 1 ? L.adv1 : L.adv2);
-      const float* val = pass == 0 ? L.val0 : (pass == 1 ? L.val1 : L.val2);
-      const float* cm = pass == 0 ? cm_tm1 : (pass == 1 ? cm_sel : cm_tgt);
-      return val[(long long)b * K + k] + adv[((long long)b * A + a) * K + k] - cm[k];
-    }
-    const float* out = pass == 0 ? L.out0 : L.out2;   // c51 selects with the target network
-    return out[((long long)b * A + a) * K + k];
-  };
-  // warp-level softmax of (pass, a): returns this lane's max/denominator; optionally writes probabilities
-  auto warp_softmax = [&](int pass, int a, float* probs, float& mx, float& den) {
-    float m = -INFINITY;
-    for (int k = lane; k < K; k += 32) m = fmaxf(m, logit_of(pass, a, k));
-    mx = warp_max(m);
-    float s = 0.f;
-    for (int k = lane; k < K; k += 32) s += expf(logit_of(pass, a, k) - mx);
-    den = warp_sum(s);
-    if (probs)
-      for (int k = lane; k < K; k += 32) probs[k] = expf(logit_of(pass, a, k) - mx) / den;
-  };
-
-  // 1. selector q-values, one warp per action
-  for (int a = warp; a < A; a += 4) {
-    float mx, den;
-    warp_softmax(rb ? 1 : 2, a, nullptr, mx, den);
-    float s = 0.f;
-    for (int k = lane; k < K; k += 32) s += (expf(logit_of(rb ? 1 : 2, a, k) - mx) / den) * support(k);
-    s = warp_sum(s);
-    if (lane == 0) qsel[a] = s;
-  }
-  __syncthreads();
-  int best = 0;
-  for (int a = 1; a < A; ++a)
-    if (qsel[a] > qsel[best]) best = a;
-  const int at = L.a[b];
-  // 2. target distribution (warp 0) and softmax of the taken action's online logits (warp 1)
-  float mx_tm1 = 0.f, den_tm1 = 1.f;
-  if (warp == 0) { float mx, den; warp_softmax(2, best, p_tgt, mx, den); }
-  if (warp == 1) {
-    warp_softmax(0, at, p_tm1, mx_tm1, den_tm1);
-    if (lane == 0) { scal[2] = mx_tm1; scal[3] = den_tm1; }
-  }
-  __syncthreads();
-  // 3. rlax.categorical_l2_project(r + discount*z, p, z)
-  const float r = L.r[b], dsc = L.disc[b];
-  const float zmin = support(0), zmax = support(K - 1);
-  for (int i = tid; i < K; i += blockDim.x) {
-    float zi = support(i);
-    float dpos = (i + 1 < K ? support(i + 1) : support(0)) - zi;      // roll(z,-1) - z
-    float dneg = zi - (i > 0 ? support(i - 1) : support(K - 1));      // z - roll(z,1)
-    dpos = dpos > 0.f ? 1.0f / dpos : 0.f;
-    dneg = dneg > 0.f ? 1.0f / dneg : 0.f;
-    float acc = 0.f;
-    for (int j = 0; j < K; ++j) {
-      float zp = fminf(fmaxf(r + dsc * support(j), zmin), zmax);
-      float delta = zp - zi;
-      float dhat = delta >= 0.f ? delta * dpos : -(delta * dneg);
-      acc += fminf(fmaxf(1.0f - dhat, 0.f), 1.0f) * p_tgt[j];
-    }
-    proj[i] = acc;
-  }
-  __syncthreads();
-  // 4. cross entropy with log_softmax(logits_tm1[a_tm1]) (warp 0)
-  if (warp == 0) {
-    const float mx = scal[2], logden = logf(scal[3]);
-    float ls = 0.f, ps = 0.f;
-    for (int k = lane; k < K; k += 32) {
-      ls += proj[k] * (logit_of(0, at, k) - mx - logden);
-      ps += proj[k];
-    }
-    ls = warp_sum(ls); ps = warp_sum(ps);
-    if (lane == 0) { scal[0] = -ls; scal[1] = ps; }
-  }
-  __syncthreads();
-  const float loss = scal[0], psum = scal[1];
-  const float w = L.w ? L.w[b] : 1.0f;
-  const float cot = w / (float)L.B;
-  // 5. gradient wrt the pass-0 head outputs
-  if (rb) {
-    for (int k = tid; k < K; k += blockDim.x) {
-      float dl = cot * (p_tm1[k] * psum - proj[k]);
-      L.dval[(long long)b * K + k] = dl;
-      for (int a = 0; a < A; ++a)
-        L.dadv[((long long)b * A + a) * K + k] = dl * ((a == at ? 1.0f : 0.0f) - 1.0f / (float)A);
-    }
-  } else {
-    for (int i = tid; i < A * K; i += blockDim.x) {
-      int a = i / K, k = i - a * K;
-      L.dout[(long long)b * A * K + i] = (a == at) ? cot * (p_tm1[k] * psum - proj[k]) : 0.f;
-    }
-  }
-  if (tid == 0) {
-    L.per_example[b] = loss;
-    if (L.priorities) L.priorities[b] = fminf(fmaxf(fabsf(loss), 0.f), 100.f);  // rainbow/agent.py:194
-    L.loss_terms[b] = w * loss;
-  }
-}
-
-// Same kernel with the example's head outputs staged in shared memory first (identical arithmetic, identical results):
-// the default whenever 3 * A * atoms floats fit (they do for every standard configuration).
+// One CTA (4 warps) per example.  Everything the example's loss reads from the three head passes is first staged in
+// shared memory; softmaxes then run one warp per (pass, action) with shuffle reductions, so the whole kernel has six
+// block barriers.  Dynamic shared memory: categorical_loss_smem().
 __global__ void __launch_bounds__(128) loss_categorical_staged_kernel(LossArgs L) {
   dz::pdl_enter();
   extern __shared__ float sm[];
@@ -841,6 +758,13 @@ __global__ void __launch_bounds__(128) loss_categorical_staged_kernel(LossArgs L
     if (L.priorities) L.priorities[b] = fminf(fmaxf(fabsf(loss), 0.f), 100.f);  // rainbow/agent.py:194
     L.loss_terms[b] = w * loss;
   }
+}
+
+// 6K + A + 4 floats of working arrays, K support atoms, and the staged [3][A*K] head outputs and [3][K] value outputs.
+// The largest configuration validate() accepts (A = 64, K = 128) needs 103,696 bytes, more than the default 48 KB.
+size_t categorical_loss_smem(const dz_learner_config& c) {
+  const size_t A = c.num_actions, K = c.num_atoms;
+  return (6 * K + A + 4 + K + 3 * A * K + 3 * K) * sizeof(float);
 }
 
 // qrdqn / iqn: rlax.quantile_q_learning with quantile_regression_loss (Huber kappa).
@@ -1098,10 +1022,12 @@ __device__ __forceinline__ float opt_one(const OptArgs& o, float p, float g, flo
 constexpr int kOptChunk = 256;                            // float4 per stream per stage
 constexpr int kOptStageBytes = 4 * kOptChunk * 16;        // p, g, m, v
 constexpr int kOptRingStages = 3;                         // OptArgs::stages of every launch
+constexpr int kOptSmem = kOptRingStages * kOptStageBytes + 64;   // the ring + its mbarriers
+constexpr int kOptThreads = kOptChunk * 2;                // 2 floats per thread and stream
 constexpr int kOptBlocksPerSM = 4;
 
-template <int KIND, int V>   // V = 2 floats per thread and stage: 512 threads
-__global__ void __launch_bounds__(kOptChunk * 4 / V, 4) optimizer_bulk_kernel(OptArgs o) {
+template <int KIND>
+__global__ void __launch_bounds__(kOptThreads, kOptBlocksPerSM) optimizer_bulk_kernel(OptArgs o) {
   extern __shared__ __align__(128) unsigned char opt_sm[];
   const int kOptStages = o.stages;
   uint64_t* full = reinterpret_cast<uint64_t*>(opt_sm + kOptStages * kOptStageBytes);
@@ -1186,6 +1112,11 @@ __global__ void __launch_bounds__(kOptChunk * 4 / V, 4) optimizer_bulk_kernel(Op
   if (tid == 0) bulk_wait_group();   // stores complete before the grid does
 }
 
+using OptKernel = void (*)(OptArgs);
+OptKernel optimizer_kernel_for(int kind) {
+  return kind == DZ_ADAM ? optimizer_bulk_kernel<DZ_ADAM> : optimizer_bulk_kernel<DZ_RMSPROP_CENTERED>;
+}
+
 // epsilon-greedy over q[E][A] (dqn/agent.py:121-127): first maximum wins, as np.argmax / jnp.argmax.
 __global__ void act_select_kernel(const float* __restrict__ q, int A, int E, const float* __restrict__ explore, float eps,
                                   int32_t* __restrict__ actions) {
@@ -1214,10 +1145,48 @@ __global__ void make_row_table_kernel(const uint8_t* base, long long stride, int
 // The learner object
 // ------------------------------------------------------------------------------------------------
 
+// A stream beside the caller's, joined back by events; under stream capture it becomes a parallel branch of the CUDA graph.
+struct SideStream {
+  cudaStream_t stream = nullptr;
+  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  bool dirty = false;   // work was enqueued since the last join
+
+  cudaError_t create() {
+    cudaError_t e = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming);
+    return e;
+  }
+  void destroy() {
+    if (stream) { cudaStreamSynchronize(stream); cudaStreamDestroy(stream); }
+    if (ev_fork) cudaEventDestroy(ev_fork);
+    if (ev_join) cudaEventDestroy(ev_join);
+  }
+  // Returns the side stream after making it wait for everything enqueued on `from` so far, or `fallback` when that
+  // ordering cannot be recorded.
+  void* fork(void* from, void* fallback) {
+    if (cudaEventRecord(ev_fork, (cudaStream_t)from) != cudaSuccess) return fallback;
+    if (cudaStreamWaitEvent(stream, ev_fork, 0) != cudaSuccess) return fallback;
+    dirty = true;
+    return stream;
+  }
+  // Makes `into` wait for the side work enqueued since the last join.
+  int join(void* into) {
+    if (!dirty) return DZ_OK;
+    DZ_CUDA_OK(cudaEventRecord(ev_join, stream));
+    DZ_CUDA_OK(cudaStreamWaitEvent((cudaStream_t)into, ev_join, 0));
+    dirty = false;
+    return DZ_OK;
+  }
+  // Where work that must follow the latest side work goes: the side stream while it has unjoined work, else `main`.
+  void* tail(void* main) const { return dirty ? (void*)stream : main; }
+};
+
 struct dz_learner {
   dz_learner_config cfg;
   dz_learner_buffers buf;
   Layout lay;
+  ParamOffsets po;
   Dims d;
   int B;           // train batch
   int n_head[3];   // rows per image in the head stage for pass 0/1/2 (IQN: tau samples; others 1)
@@ -1246,19 +1215,20 @@ struct dz_learner {
   float *pk_fwd_partial, *pk_wgrad_partial;
   int pk_fwd_splits, pk_wgrad_splits;
   // second stream for work that is off the critical path of the backward pass (weight gradients, priority
-  // write-back, noise generation); under stream capture it becomes a parallel branch of the CUDA graph
-  cudaStream_t side;
-  cudaEvent_t ev_fork, ev_join;
-  bool side_dirty;
+  // write-back, noise generation)
+  SideStream side;
   // third branch: the FC part of the split gradient norm and the conv2 weight gradient run beside the first side stream
-  cudaStream_t side2;
-  cudaEvent_t ev_fork2, ev_join2;
-  bool side2_dirty;
+  SideStream side2;
   float* norm_parts;                        // split-norm slots written by the conv weight-gradient finish kernels
   // TMA-fed tensor-core path of the batch-sized step (dz_umma_net.cu): torso + 3136 -> 512 layer(s), forward and input gradients
   UmNet* um;
   char* um_ws;
-  int um_npass, um_set[3];
+  int um_npass;
+  // The optimizer kernel's dynamic shared-memory limit is raised per learner (the attribute is per device) at the
+  // learner's first optimizer launch, not at creation: raising it loads the kernel (CUDA lazy loading), and loading it
+  // at creation left the dqn CUDA-graph step about 1% slower in most processes (measured on an H100 80GB HBM3 at 700 W,
+  // with every kernel's code unchanged).
+  bool opt_smem_set = false;
 };
 
 namespace {
@@ -1275,9 +1245,6 @@ int pick_splits(int64_t tiles, int nkb, int max_splits) {
   }
   return best;
 }
-
-int64_t noise_stride(const dz_learner_config& c, const Dims& d);
-struct NoiseVecs;
 
 UmNetDesc make_um_desc(const dz_learner* l);
 
@@ -1385,25 +1352,32 @@ int64_t carve(dz_learner* l, char* base) {
   return w.used;
 }
 
-// Noise layout of ONE apply: adv1_in[feat] adv1_out[512] adv2_in[512] adv2_out[A*atoms] val1_in[feat]
-// val1_out[512] val2_in[512] val2_out[atoms]; every vector starts on a 4-float boundary.
-inline int64_t pad4(int64_t n) { return (n + 3) / 4 * 4; }
-int64_t noise_stride(const dz_learner_config& c, const Dims& d) {
-  return 2 * (pad4(d.feat) + 512 + 512) + pad4((int64_t)c.num_actions * c.num_atoms) + pad4(c.num_atoms);
+// Rainbow noise of ONE apply, in this order: adv1_in[feat] adv1_out[512] adv2_in[512] adv2_out[A*atoms] val1_in[feat]
+// val1_out[512] val2_in[512] val2_out[atoms]; every vector starts on a 4-float boundary.  Offsets in floats.
+struct NoiseLayout {
+  int64_t stride;   // floats per apply
+  int64_t a1i, a1o, a2i, a2o, v1i, v1o, v2i, v2o;
+};
+NoiseLayout noise_layout(const dz_learner_config& c, const Dims& d) {
+  NoiseLayout n;
+  int64_t end = 0;
+  auto next = [&](int64_t len) { const int64_t at = end; end += (len + 3) / 4 * 4; return at; };
+  n.a1i = next(d.feat); n.a1o = next(512); n.a2i = next(512); n.a2o = next((int64_t)c.num_actions * c.num_atoms);
+  n.v1i = next(d.feat); n.v1o = next(512); n.v2i = next(512); n.v2o = next(c.num_atoms);
+  n.stride = end;
+  return n;
 }
 struct NoiseVecs { const float *a1i, *a1o, *a2i, *a2o, *v1i, *v1o, *v2i, *v2o; };
 NoiseVecs noise_of(const dz_learner_config& c, const Dims& d, const float* base, int apply) {
-  const float* p = base + (int64_t)apply * noise_stride(c, d);
-  NoiseVecs n;
-  n.a1i = p; p += pad4(d.feat); n.a1o = p; p += 512; n.a2i = p; p += 512; n.a2o = p; p += pad4((int64_t)c.num_actions * c.num_atoms);
-  n.v1i = p; p += pad4(d.feat); n.v1o = p; p += 512; n.v2i = p; p += 512; n.v2o = p;
-  return n;
+  const NoiseLayout n = noise_layout(c, d);
+  const float* p = base + (int64_t)apply * n.stride;
+  return NoiseVecs{p + n.a1i, p + n.a1o, p + n.a2i, p + n.a2o, p + n.v1i, p + n.v1o, p + n.v2i, p + n.v2o};
 }
 
 UmNetDesc make_um_desc(const dz_learner* l) {
   const dz_learner_config& c = l->cfg;
   const Dims& d = l->d;
-  const Layout& L = l->lay;
+  const ParamOffsets& o = l->po;
   UmNetDesc u;
   memset(&u, 0, sizeof(u));
   const bool needs_online_st = c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED || c.kind == DZ_RAINBOW;
@@ -1411,27 +1385,22 @@ UmNetDesc make_um_desc(const dz_learner* l) {
   u.npass = needs_online_st ? 3 : 2;
   u.pass_target[0] = 0; u.pass_target[1] = needs_online_st ? 0 : 1; u.pass_target[2] = 1;
   u.online = l->buf.d_online; u.target = l->buf.d_target;
-  const char* cw[3] = {"conv1/w", "conv2/w", "conv3/w"};
-  const char* cb[3] = {"conv1/b", "conv2/b", "conv3/b"};
-  for (int i = 0; i < 3; ++i) { u.off_conv_w[i] = L.off(cw[i]); u.off_conv_b[i] = L.off(cb[i]); }
+  for (int i = 0; i < 3; ++i) { u.off_conv_w[i] = o.conv_w[i]; u.off_conv_b[i] = o.conv_b[i]; }
   u.use_fc = c.kind != DZ_IQN;
   u.nstream = c.kind == DZ_RAINBOW ? 2 : 1;
   u.noisy = c.kind == DZ_RAINBOW ? 1 : 0;
   if (c.kind == DZ_RAINBOW) {
-    const char* st[2] = {"adv", "val"};
     for (int s = 0; s < 2; ++s) {
-      std::string pre = std::string(st[s]) + "1/";
-      u.off_fc_w[s] = L.off(pre + "mu/w"); u.off_fc_b[s] = L.off(pre + "mu/b");
-      u.off_fc_sw[s] = L.off(pre + "sigma/w"); u.off_fc_sb[s] = L.off(pre + "sigma/b");
+      u.off_fc_w[s] = o.w1[s]; u.off_fc_b[s] = o.b1[s];
+      u.off_fc_sw[s] = o.sw1[s]; u.off_fc_sb[s] = o.sb1[s];
     }
-    static float origin[1];
-    NoiseVecs nz = noise_of(c, d, origin, 0);
-    u.noise_stride = noise_stride(c, d);
-    u.noise_off_in[0] = nz.a1i - origin; u.noise_off_out[0] = nz.a1o - origin;
-    u.noise_off_in[1] = nz.v1i - origin; u.noise_off_out[1] = nz.v1o - origin;
+    const NoiseLayout nl = noise_layout(c, d);
+    u.noise_stride = nl.stride;
+    u.noise_off_in[0] = nl.a1i; u.noise_off_out[0] = nl.a1o;
+    u.noise_off_in[1] = nl.v1i; u.noise_off_out[1] = nl.v1o;
     for (int p = 0; p < 3; ++p) u.noise_apply[p] = p;
   } else if (u.use_fc) {
-    u.off_fc_w[0] = L.off("fc1/w"); u.off_fc_b[0] = L.off("fc1/b");
+    u.off_fc_w[0] = o.w1[0]; u.off_fc_b[0] = o.b1[0];
   }
   return u;
 }
@@ -1533,7 +1502,6 @@ int finish_nn(const GemmBatch& gb, float* const* outs, bool dual, void* stream) 
 
 struct Pass {        // one network.apply
   const float* params;     // online or target blob
-  const uint8_t* const* rows;  // image row table
   int set;                 // torso activation set index (0..2)
   int head;                // head pass index (0..2)
   int apply;               // noise apply index (rainbow)
@@ -1545,7 +1513,7 @@ struct TorsoJob { const float* params; const uint8_t* const* rows; int set; };
 
 int forward_torso(dz_learner* l, const TorsoJob* jobs, int njobs, int nimg, void* stream) {
   const Dims& d = l->d;
-  const Layout& L = l->lay;
+  const ParamOffsets& o = l->po;
   GemmBatch gb;
   gb.n = njobs;
   // conv1: uint8 rows gathered in place (K1 + K2 of SURVEY §2.1).  Not split over K (= 256): measured before the H100
@@ -1553,7 +1521,7 @@ int forward_torso(dz_learner* l, const TorsoJob* jobs, int njobs, int nimg, void
   for (int i = 0; i < njobs; ++i) {
     GemmProblem p = zero_problem();
     set_conv(p, A_CONV_U8, jobs[i].rows, nimg, d.H, d.W, d.C, 8, 8, 4);
-    p.B = jobs[i].params + L.off("conv1/w"); p.bias = jobs[i].params + L.off("conv1/b");
+    p.B = jobs[i].params + o.conv_w[0]; p.bias = jobs[i].params + o.conv_b[0];
     p.N = 32; p.ldb = 32; p.ldc = 32; p.relu = 1; p.C = l->act1[jobs[i].set];
     gb.p[i] = p;
   }
@@ -1566,11 +1534,11 @@ int forward_torso(dz_learner* l, const TorsoJob* jobs, int njobs, int nimg, void
       GemmProblem p = zero_problem();
       if (layer == 2) {
         set_conv(p, A_CONV_F32, l->act1[jobs[i].set], nimg, d.h1, d.w1, 32, 4, 4, 2);
-        p.B = jobs[i].params + L.off("conv2/w"); p.bias = jobs[i].params + L.off("conv2/b");
+        p.B = jobs[i].params + o.conv_w[1]; p.bias = jobs[i].params + o.conv_b[1];
         outs[i] = l->act2[jobs[i].set];
       } else {
         set_conv(p, A_CONV_F32, l->act2[jobs[i].set], nimg, d.h2, d.w2, 64, 3, 3, 1);
-        p.B = jobs[i].params + L.off("conv3/w"); p.bias = jobs[i].params + L.off("conv3/b");
+        p.B = jobs[i].params + o.conv_w[2]; p.bias = jobs[i].params + o.conv_b[2];
         outs[i] = l->act3[jobs[i].set];
       }
       p.N = 64; p.ldb = 64; p.ldc = 64; p.relu = 1;
@@ -1587,7 +1555,7 @@ int forward_torso(dz_learner* l, const TorsoJob* jobs, int njobs, int nimg, void
 // Heads for the dqn / double_q / prioritized / c51 / qrdqn family.
 int forward_heads_plain(dz_learner* l, const Pass* passes, int np, int nimg, void* stream, bool fc1_done = false) {
   const Dims& d = l->d;
-  const Layout& L = l->lay;
+  const ParamOffsets& o = l->po;
   GemmBatch gb;
   gb.n = np;
   float* outs[kMaxProblems];
@@ -1596,8 +1564,8 @@ int forward_heads_plain(dz_learner* l, const Pass* passes, int np, int nimg, voi
   for (int i = 0; i < np && !fc1_done; ++i) {
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->act3[passes[i].set]; p.lda = d.feat; p.M = nimg; p.K = d.feat;
-    p.B = passes[i].params + L.off("fc1/w"); p.N = 512; p.ldb = 512; p.ldc = 512;
-    p.bias = passes[i].params + L.off("fc1/b"); p.relu = 1;
+    p.B = passes[i].params + o.w1[0]; p.N = 512; p.ldb = 512; p.ldc = 512;
+    p.bias = passes[i].params + o.b1[0]; p.relu = 1;
     outs[i] = l->h1[passes[i].head][0];
     if (splits > 1) {
       p.splits = splits; p.split_stride = (long long)nimg * 512;
@@ -1614,8 +1582,8 @@ int forward_heads_plain(dz_learner* l, const Pass* passes, int np, int nimg, voi
   for (int i = 0; i < np; ++i) {
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->h1[passes[i].head][0]; p.lda = 512; p.M = nimg; p.K = 512;
-    p.B = passes[i].params + L.off("head/w"); p.N = d.out; p.ldb = d.out; p.ldc = d.out;
-    p.bias = passes[i].params + L.off("head/b"); p.bias_shared = shared ? 1 : 0;
+    p.B = passes[i].params + o.w2[0]; p.N = d.out; p.ldb = d.out; p.ldc = d.out;
+    p.bias = passes[i].params + o.b2[0]; p.bias_shared = shared ? 1 : 0;
     outs[i] = l->out[passes[i].head];
     if (nimg <= 32) {
       p.splits = l->head_splits; p.split_stride = (long long)nimg * d.out;
@@ -1633,23 +1601,21 @@ int forward_heads_plain(dz_learner* l, const Pass* passes, int np, int nimg, voi
 // Rainbow: two noisy streams (networks.py:224-261, :137-178).
 int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, const float* noise, void* stream, bool fc1_done = false) {
   const Dims& d = l->d;
-  const Layout& L = l->lay;
+  const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
   if (2 * np > kMaxProblems) return fail(DZ_EINVAL, "too many rainbow passes");
   GemmBatch gb;
   gb.n = 2 * np;
   float* outs[kMaxProblems];
   const int splits = nimg <= 32 ? l->fc_splits : 1;
-  const char* st[2] = {"adv", "val"};
   for (int i = 0; i < np && !fc1_done; ++i) {
     NoiseVecs nz = noise_of(c, d, noise, passes[i].apply);
     for (int s = 0; s < 2; ++s) {
-      std::string pre = std::string(st[s]) + "1/";
       GemmProblem p = zero_problem();
       p.a_mode = A_PLAIN; p.A = l->act3[passes[i].set]; p.lda = d.feat; p.M = nimg; p.K = d.feat;
-      p.B = passes[i].params + L.off(pre + "mu/w"); p.B2 = passes[i].params + L.off(pre + "sigma/w");
+      p.B = passes[i].params + o.w1[s]; p.B2 = passes[i].params + o.sw1[s];
       p.N = 512; p.ldb = 512; p.ldc = 512;
-      p.bias = passes[i].params + L.off(pre + "mu/b"); p.bias2 = passes[i].params + L.off(pre + "sigma/b");
+      p.bias = passes[i].params + o.b1[s]; p.bias2 = passes[i].params + o.sb1[s];
       p.a_scale = s == 0 ? nz.a1i : nz.v1i; p.c_scale = s == 0 ? nz.a1o : nz.v1o; p.relu = 1;
       int q = 2 * i + s;
       outs[q] = l->h1[passes[i].head][s];
@@ -1669,13 +1635,12 @@ int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, c
   for (int i = 0; i < np; ++i) {
     NoiseVecs nz = noise_of(c, d, noise, passes[i].apply);
     for (int s = 0; s < 2; ++s) {
-      std::string pre = std::string(st[s]) + "2/";
       int n_out = s == 0 ? c.num_actions * c.num_atoms : c.num_atoms;
       GemmProblem p = zero_problem();
       p.a_mode = A_PLAIN; p.A = l->h1[passes[i].head][s]; p.lda = 512; p.M = nimg; p.K = 512;
-      p.B = passes[i].params + L.off(pre + "mu/w"); p.B2 = passes[i].params + L.off(pre + "sigma/w");
+      p.B = passes[i].params + o.w2[s]; p.B2 = passes[i].params + o.sw2[s];
       p.N = n_out; p.ldb = n_out; p.ldc = n_out;
-      p.bias = nullptr; p.bias2 = passes[i].params + L.off(pre + "sigma/b");   // with_bias=False: mu has no bias
+      p.bias = nullptr; p.bias2 = passes[i].params + o.sb2[s];   // with_bias=False: mu has no bias
       p.a_scale = s == 0 ? nz.a2i : nz.v2i; p.c_scale = s == 0 ? nz.a2o : nz.v2o;
       int q = 2 * i + s;
       outs[q] = s == 0 ? l->out[passes[i].head] : l->outv[passes[i].head];
@@ -1700,7 +1665,7 @@ int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, c
 // `hi` tensors are never materialised), the split fc1 GEMM, one finish (bias + ReLU).
 int iqn_embed_fc1_forward_packed(dz_learner* l, const Pass* passes, const GemmBatch& fc1, bool keep_E0, void* stream) {
   const Dims& d = l->d;
-  const Layout& L = l->lay;
+  const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
   PackBatch pb;
   memset(&pb, 0, sizeof(pb));
@@ -1717,13 +1682,13 @@ int iqn_embed_fc1_forward_packed(dz_learner* l, const Pass* passes, const GemmBa
   }
   for (int k = 0; k < 2; ++k) {
     if (!blob[k]) continue;
-    DZ_TRY(pk_add_job(pb, blob[k] + L.off("embed/w"), d.feat, 0, d.feat, c.latent_dim, l->pk_weT[k].rows_pad, l->pk_weT[k].red_pad,
+    DZ_TRY(pk_add_job(pb, blob[k] + o.embed_w, d.feat, 0, d.feat, c.latent_dim, l->pk_weT[k].rows_pad, l->pk_weT[k].red_pad,
                       -1, l->pk_weT[k].hi, l->pk_weT[k].lo));
-    DZ_TRY(pk_add_job(pb, blob[k] + L.off("fc1/w"), 512, 0, 512, d.feat, l->pk_wT[k].rows_pad, l->pk_wT[k].red_pad, -1,
+    DZ_TRY(pk_add_job(pb, blob[k] + o.w1[0], 512, 0, 512, d.feat, l->pk_wT[k].rows_pad, l->pk_wT[k].red_pad, -1,
                       l->pk_wT[k].hi, l->pk_wT[k].lo));
   }
   // backward-time operand that only depends on forward-time tensors: W (rows k, reduction n) for the input gradient
-  DZ_TRY(pk_add_job(pb, l->buf.d_online + L.off("fc1/w"), 512, 1, d.feat, 512, l->pk_w.rows_pad, l->pk_w.red_pad, -1, l->pk_w.hi, l->pk_w.lo));
+  DZ_TRY(pk_add_job(pb, l->buf.d_online + o.w1[0], 512, 1, d.feat, 512, l->pk_w.rows_pad, l->pk_w.red_pad, -1, l->pk_w.hi, l->pk_w.lo));
   DZ_TRY(launch_pack("iqn_pack_fwd", pb, stream));
 
   PkBatch eb;
@@ -1735,7 +1700,7 @@ int iqn_embed_fc1_forward_packed(dz_learner* l, const Pass* passes, const GemmBa
     p.A = PkOperand{l->pk_cos[hp].hi, l->pk_cos[hp].lo, l->pk_cos[hp].rows_pad / 8};
     p.B = PkOperand{l->pk_weT[widx[i]].hi, l->pk_weT[widx[i]].lo, l->pk_weT[widx[i]].rows_pad / 8};
     p.MI = fc1.p[i].M; p.NJ = d.feat; p.nkb = l->pk_cos[hp].red_pad / kPkKB; p.splits = 1;
-    p.bias_j = passes[i].params + L.off("embed/b");
+    p.bias_j = passes[i].params + o.embed_b;
     p.mul = l->act3[passes[i].set]; p.mul_div = l->n_head[hp]; p.mul_ld = d.feat;
     p.e0 = (keep_E0 && hp == 0) ? l->E0 : nullptr; p.e0_ld = d.feat;
     p.img_hi = l->pk_act[hp].hi; p.img_lo = l->pk_act[hp].lo; p.img_rg = l->pk_act[hp].rows_pad / 8;
@@ -1773,7 +1738,7 @@ int iqn_embed_fc1_forward_packed(dz_learner* l, const Pass* passes, const GemmBa
 // IQN (networks.py:264-292): cosine embedding -> linear -> relu -> * state embedding -> value head.
 int forward_heads_iqn(dz_learner* l, const Pass* passes, int np, int nimg, const float* const* taus, bool keep_E0, void* stream) {
   const Dims& d = l->d;
-  const Layout& L = l->lay;
+  const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
   GemmBatch gb;
   gb.n = np;
@@ -1788,8 +1753,8 @@ int forward_heads_iqn(dz_learner* l, const Pass* passes, int np, int nimg, const
       int hp = passes[i].head;
       GemmProblem p = zero_problem();
       p.a_mode = A_PLAIN; p.A = l->cosf[hp]; p.lda = c.latent_dim; p.M = nimg * l->n_head[hp]; p.K = c.latent_dim;
-      p.B = passes[i].params + L.off("embed/w"); p.N = d.feat; p.ldb = d.feat; p.ldc = d.feat;
-      p.bias = passes[i].params + L.off("embed/b"); p.relu = 1;
+      p.B = passes[i].params + o.embed_w; p.N = d.feat; p.ldb = d.feat; p.ldc = d.feat;
+      p.bias = passes[i].params + o.embed_b; p.relu = 1;
       p.mul = l->act3[passes[i].set]; p.mul_div = l->n_head[hp];
       p.C = l->hi[hp]; p.C2 = (keep_E0 && hp == 0) ? l->E0 : nullptr;
       gb.p[i] = p;
@@ -1800,8 +1765,8 @@ int forward_heads_iqn(dz_learner* l, const Pass* passes, int np, int nimg, const
     int hp = passes[i].head;
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->hi[hp]; p.lda = d.feat; p.M = nimg * l->n_head[hp]; p.K = d.feat;
-    p.B = passes[i].params + L.off("fc1/w"); p.N = 512; p.ldb = 512; p.ldc = 512;
-    p.bias = passes[i].params + L.off("fc1/b"); p.relu = 1; p.C = l->h1[hp][0];
+    p.B = passes[i].params + o.w1[0]; p.N = 512; p.ldb = 512; p.ldc = 512;
+    p.bias = passes[i].params + o.b1[0]; p.relu = 1; p.C = l->h1[hp][0];
     gb.p[i] = p;
   }
   // M can be small when acting (1 x tau_samples_policy rows): same kernel family handles it
@@ -1817,7 +1782,7 @@ int forward_heads_iqn(dz_learner* l, const Pass* passes, int np, int nimg, const
     int maxM = 0;
     for (int i = 0; i < np; ++i) {
       int hp = passes[i].head;
-      h.A[i] = l->h1[hp][0]; h.W[i] = passes[i].params + L.off("head/w"); h.bias[i] = passes[i].params + L.off("head/b");
+      h.A[i] = l->h1[hp][0]; h.W[i] = passes[i].params + o.w2[0]; h.bias[i] = passes[i].params + o.b2[0];
       h.out[i] = l->out[hp]; h.M[i] = nimg * l->n_head[hp];
       maxM = std::max(maxM, h.M[i]);
     }
@@ -1829,8 +1794,8 @@ int forward_heads_iqn(dz_learner* l, const Pass* passes, int np, int nimg, const
     int hp = passes[i].head;
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->h1[hp][0]; p.lda = 512; p.M = nimg * l->n_head[hp]; p.K = 512;
-    p.B = passes[i].params + L.off("head/w"); p.N = d.out; p.ldb = d.out; p.ldc = d.out;
-    p.bias = passes[i].params + L.off("head/b"); p.C = l->out[hp];
+    p.B = passes[i].params + o.w2[0]; p.N = d.out; p.ldb = d.out; p.ldc = d.out;
+    p.bias = passes[i].params + o.b2[0]; p.C = l->out[hp];
     gb.p[i] = p;
   }
   DZ_TRY(run_nn("iqn_head_fwd", gb, false, stream));
@@ -1862,41 +1827,12 @@ int finish_nt(const GemmProblem* probs, int nsrc, const float* mask, float* out,
   return finish_nt_batch(&f, 1, stream);
 }
 
-// Returns the side stream after making it wait for everything enqueued on `stream` so far (or `stream` itself when
-// that ordering cannot be recorded).  join_side() makes `stream` wait for the side work again.
-void* fork_side(dz_learner* l, void* stream) {
-  if (cudaEventRecord(l->ev_fork, (cudaStream_t)stream) != cudaSuccess) return stream;
-  if (cudaStreamWaitEvent(l->side, l->ev_fork, 0) != cudaSuccess) return stream;
-  l->side_dirty = true;
-  return l->side;
-}
-int join_side(dz_learner* l, void* stream) {
-  if (!l->side_dirty) return DZ_OK;
-  DZ_CUDA_OK(cudaEventRecord(l->ev_join, l->side));
-  DZ_CUDA_OK(cudaStreamWaitEvent((cudaStream_t)stream, l->ev_join, 0));
-  l->side_dirty = false;
-  return DZ_OK;
-}
-// Second side stream: `from` is the stream whose enqueued work it must wait for (the main stream or the first side stream).
-void* fork_side2(dz_learner* l, void* from, void* fallback) {
-  if (cudaEventRecord(l->ev_fork2, (cudaStream_t)from) != cudaSuccess) return fallback;
-  if (cudaStreamWaitEvent(l->side2, l->ev_fork2, 0) != cudaSuccess) return fallback;
-  l->side2_dirty = true;
-  return l->side2;
-}
-int join_side2(dz_learner* l, void* stream) {
-  if (!l->side2_dirty) return DZ_OK;
-  DZ_CUDA_OK(cudaEventRecord(l->ev_join2, l->side2));
-  DZ_CUDA_OK(cudaStreamWaitEvent((cudaStream_t)stream, l->ev_join2, 0));
-  l->side2_dirty = false;
-  return DZ_OK;
-}
 bool split_norm_active(const dz_learner* l);
 
 // Torso backward from dact3 (already masked by act3 > 0): conv3/conv2/conv1 weight+bias grads.
 int backward_torso(dz_learner* l, const uint8_t* const* rows0, void* stream) {
   const Dims& d = l->d;
-  const Layout& L = l->lay;
+  const ParamOffsets& o = l->po;
   const int B = l->B;
   float* G = l->buf.d_grads;
   const float* P = l->buf.d_online;
@@ -1907,19 +1843,19 @@ int backward_torso(dz_learner* l, const uint8_t* const* rows0, void* stream) {
   // conv3 wgrad
   float* norm_parts = split_norm_active(l) ? l->norm_parts : nullptr;
   if (l->um) {   // conv3 weight gradient + its finish (partial sums, bias gradient, split-norm partials) on the side stream
-    void* ws = fork_side(l, stream);
+    void* ws = l->side.fork(stream, stream);
     DZ_TRY(um_wgrad_conv3(l->um, ws));
-    DZ_TRY(um_wgrad_finish_layer(l->um, 3, G + L.off("conv3/w"), G + L.off("conv3/b"), norm_parts, ws));
+    DZ_TRY(um_wgrad_finish_layer(l->um, 3, G + o.conv_w[2], G + o.conv_b[2], norm_parts, ws));
   } else {
     GemmProblem p = zero_problem();
     set_conv(p, A_CONV_F32, l->act2[0], B, d.h2, d.w2, 64, 3, 3, 1);
     p.B = l->dact3; p.N = 64; p.ldb = 64; p.ldc = 64;
-    p.Cb = G + L.off("conv3/b");
+    p.Cb = G + o.conv_b[2];
     int splits = (int)std::min<int64_t>(32, ceil_div(p.M, 64));
     p.splits = splits; p.split_stride = (long long)(p.K + 1) * 64; p.C = l->tn_partial[2];
     gb.n = 1; gb.p[0] = p;
-    DZ_TRY(run_tn("conv3_wgrad", gb, fork_side(l, stream)));
-    fb.f[fb.n++] = FinishTN{p.C, splits, p.split_stride, p.K, 64, G + L.off("conv3/w"), nullptr, p.Cb, nullptr, nullptr, nullptr};
+    DZ_TRY(run_tn("conv3_wgrad", gb, l->side.fork(stream, stream)));
+    fb.f[fb.n++] = FinishTN{p.C, splits, p.split_stride, p.K, 64, G + o.conv_w[2], nullptr, p.Cb, nullptr, nullptr, nullptr};
   }
   // conv3 dgrad: dcol = dpre3 * W3^T ; col2im with ReLU mask of act2
   if (l->um) {
@@ -1927,7 +1863,7 @@ int backward_torso(dz_learner* l, const uint8_t* const* rows0, void* stream) {
   } else {
     GemmProblem p = zero_problem();
     p.A = l->dact3; p.lda = 64; p.M = B * d.h3 * d.w3; p.N = 64; p.K = 576;
-    p.B = P + L.off("conv3/w"); p.ldb = 64; p.C = l->dcol; p.ldc = 576;
+    p.B = P + o.conv_w[2]; p.ldb = 64; p.C = l->dcol; p.ldc = 576;
     gb.n = 1; gb.p[0] = p;
     DZ_TRY(run_nt("conv3_dgrad", gb, false, stream));
     long long total = (long long)B * d.h2 * d.w2 * 64;
@@ -1936,19 +1872,19 @@ int backward_torso(dz_learner* l, const uint8_t* const* rows0, void* stream) {
   }
   // conv2 wgrad
   if (l->um) {   // conv2: on the second side stream, beside conv3's (both fit next to the input-gradient kernels)
-    void* ws = fork_side2(l, stream, stream);
+    void* ws = l->side2.fork(stream, stream);
     DZ_TRY(um_wgrad_conv2(l->um, ws));
-    DZ_TRY(um_wgrad_finish_layer(l->um, 2, G + L.off("conv2/w"), G + L.off("conv2/b"), norm_parts, ws));
+    DZ_TRY(um_wgrad_finish_layer(l->um, 2, G + o.conv_w[1], G + o.conv_b[1], norm_parts, ws));
   } else {
     GemmProblem p = zero_problem();
     set_conv(p, A_CONV_F32, l->act1[0], B, d.h1, d.w1, 32, 4, 4, 2);
     p.B = l->dact2; p.N = 64; p.ldb = 64; p.ldc = 64;
-    p.Cb = G + L.off("conv2/b");
+    p.Cb = G + o.conv_b[1];
     int splits = (int)std::min<int64_t>(32, ceil_div(p.M, 64));
     p.splits = splits; p.split_stride = (long long)(p.K + 1) * 64; p.C = l->tn_partial[1];
     gb.n = 1; gb.p[0] = p;
-    DZ_TRY(run_tn("conv2_wgrad", gb, fork_side(l, stream)));
-    fb.f[fb.n++] = FinishTN{p.C, splits, p.split_stride, p.K, 64, G + L.off("conv2/w"), nullptr, p.Cb, nullptr, nullptr, nullptr};
+    DZ_TRY(run_tn("conv2_wgrad", gb, l->side.fork(stream, stream)));
+    fb.f[fb.n++] = FinishTN{p.C, splits, p.split_stride, p.K, 64, G + o.conv_w[1], nullptr, p.Cb, nullptr, nullptr, nullptr};
   }
   // conv2 dgrad
   if (l->um) {
@@ -1956,7 +1892,7 @@ int backward_torso(dz_learner* l, const uint8_t* const* rows0, void* stream) {
   } else {
     GemmProblem p = zero_problem();
     p.A = l->dact2; p.lda = 64; p.M = B * d.h2 * d.w2; p.N = 64; p.K = 512;
-    p.B = P + L.off("conv2/w"); p.ldb = 64; p.C = l->dcol; p.ldc = 512;
+    p.B = P + o.conv_w[1]; p.ldb = 64; p.C = l->dcol; p.ldc = 512;
     gb.n = 1; gb.p[0] = p;
     DZ_TRY(run_nt("conv2_dgrad", gb, false, stream));
     long long total = (long long)B * d.h1 * d.w1 * 32;
@@ -1965,31 +1901,31 @@ int backward_torso(dz_learner* l, const uint8_t* const* rows0, void* stream) {
   }
   // conv1 wgrad (A = uint8 rows in place)
   if (l->um) {
-    void* ws = fork_side(l, stream);
+    void* ws = l->side.fork(stream, stream);
     DZ_TRY(um_wgrad_conv1(l->um, rows0, ws));
-    DZ_TRY(um_wgrad_finish_layer(l->um, 1, G + L.off("conv1/w"), G + L.off("conv1/b"), norm_parts, ws));
-    DZ_TRY(join_side2(l, stream));
-    return join_side(l, stream);
+    DZ_TRY(um_wgrad_finish_layer(l->um, 1, G + o.conv_w[0], G + o.conv_b[0], norm_parts, ws));
+    DZ_TRY(l->side2.join(stream));
+    return l->side.join(stream);
   } else {
     GemmProblem p = zero_problem();
     set_conv(p, A_CONV_U8, rows0, B, d.H, d.W, d.C, 8, 8, 4);
     p.B = l->dact1; p.N = 32; p.ldb = 32; p.ldc = 32;
-    p.Cb = G + L.off("conv1/b");
+    p.Cb = G + o.conv_b[0];
     int splits = (int)std::min<int64_t>(64, ceil_div(p.M, 64));
     p.splits = splits; p.split_stride = (long long)(p.K + 1) * 32; p.C = l->tn_partial[0];
     gb.n = 1; gb.p[0] = p;
-    DZ_TRY(run_tn("conv1_wgrad", gb, fork_side(l, stream)));
-    fb.f[fb.n++] = FinishTN{p.C, splits, p.split_stride, p.K, 32, G + L.off("conv1/w"), nullptr, p.Cb, nullptr, nullptr, nullptr};
+    DZ_TRY(run_tn("conv1_wgrad", gb, l->side.fork(stream, stream)));
+    fb.f[fb.n++] = FinishTN{p.C, splits, p.split_stride, p.K, 32, G + o.conv_w[0], nullptr, p.Cb, nullptr, nullptr, nullptr};
   }
-  void* ws = l->side_dirty ? (void*)l->side : stream;   // after conv1_wgrad on the same (side) stream
+  void* ws = l->side.tail(stream);   // after conv1_wgrad on the same (side) stream
   dim3 grid((unsigned)ceil_div(577 * 64, 256), fb.n);
   DZ_LAUNCH(finish_tn_kernel, grid, 256, 0, ws, fb);
-  return join_side(l, stream);
+  return l->side.join(stream);
 }
 
 int backward_plain(dz_learner* l, void* stream) {
   const Dims& d = l->d;
-  const Layout& L = l->lay;
+  const ParamOffsets& o = l->po;
   const int B = l->B;
   float* G = l->buf.d_grads;
   const float* P = l->buf.d_online;
@@ -2000,16 +1936,16 @@ int backward_plain(dz_learner* l, void* stream) {
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->h1[0][0]; p.lda = 512; p.M = B; p.K = 512;
     p.B = l->dout; p.N = d.out; p.ldb = d.out; p.ldc = d.out;
-    p.C = G + L.off("head/w"); p.Cb = shared ? l->scalars + 8 + kNormBlocks : G + L.off("head/b");
+    p.C = G + o.w2[0]; p.Cb = shared ? l->scalars + 8 + kNormBlocks : G + o.b2[0];
     gb.p[0] = p;
-    DZ_TRY(run_tn("head_wgrad", gb, fork_side(l, stream)));
-    if (shared) DZ_LAUNCH(sum_to_scalar_kernel, 1, 128, 0, (l->side_dirty ? (void*)l->side : stream), l->scalars + 8 + kNormBlocks, d.out, G + L.off("head/b"));
+    DZ_TRY(run_tn("head_wgrad", gb, l->side.fork(stream, stream)));
+    if (shared) DZ_LAUNCH(sum_to_scalar_kernel, 1, 128, 0, l->side.tail(stream), l->scalars + 8 + kNormBlocks, d.out, G + o.b2[0]);
   }
   bool dh1_split_done = false;
   {  // dh1 = dout * Wh^T, masked by h1 > 0
     GemmProblem p = zero_problem();
     p.A = l->dout; p.lda = d.out; p.M = B; p.N = d.out; p.K = 512;
-    p.B = P + L.off("head/w"); p.ldb = d.out; p.C = l->dh1[0]; p.ldc = 512; p.mask = l->h1[0][0];
+    p.B = P + o.w2[0]; p.ldb = d.out; p.C = l->dh1[0]; p.ldc = 512; p.mask = l->h1[0][0];
     // Wide heads (c51: 306 outputs, qr-dqn: 1206): with one CTA column per 64 outputs of dh1 the reduction over the head
     // width is a serial chain (measured 24 / 65 us); split it and let the finish kernel apply the mask (and, on the tensor-core
     // path, write the tf32 hi/lo pair fc1_dgrad reads, which saves the separate split launch).
@@ -2031,9 +1967,9 @@ int backward_plain(dz_learner* l, void* stream) {
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->act3[0]; p.lda = d.feat; p.M = B; p.K = d.feat;
     p.B = l->dh1[0]; p.N = 512; p.ldb = 512; p.ldc = 512;
-    p.C = G + L.off("fc1/w"); p.Cb = G + L.off("fc1/b");
+    p.C = G + o.w1[0]; p.Cb = G + o.b1[0];
     gb.p[0] = p;
-    DZ_TRY(run_tn("fc1_wgrad", gb, fork_side(l, stream)));
+    DZ_TRY(run_tn("fc1_wgrad", gb, l->side.fork(stream, stream)));
   }
   if (l->um) {   // dact3 on the tensor-core path: dh1 -> tf32 hi/lo, W streamed once through TMA, split partials + masked finish
     if (!dh1_split_done) DZ_TRY(um_split_dh1(l->um, stream));
@@ -2041,7 +1977,7 @@ int backward_plain(dz_learner* l, void* stream) {
   } else {  // dact3 = dh1 * Wf^T, masked by act3 > 0
     GemmProblem p = zero_problem();
     p.A = l->dh1[0]; p.lda = 512; p.M = B; p.N = 512; p.K = d.feat;
-    p.B = P + L.off("fc1/w"); p.ldb = 512; p.ldc = d.feat;
+    p.B = P + o.w1[0]; p.ldb = 512; p.ldc = d.feat;
     // weight-streaming GEMM with a 32-row output: split the reduction so ~400 CTAs keep HBM busy
     p.splits = l->nt_splits; p.split_stride = (long long)B * d.feat; p.C = l->nt_partial;
     gb.p[0] = p;
@@ -2053,32 +1989,29 @@ int backward_plain(dz_learner* l, void* stream) {
 
 int backward_rainbow(dz_learner* l, const float* noise, void* stream) {
   const Dims& d = l->d;
-  const Layout& L = l->lay;
+  const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
   const int B = l->B;
   float* G = l->buf.d_grads;
   const float* P = l->buf.d_online;
   NoiseVecs nz = noise_of(c, d, noise, 0);
-  const char* st[2] = {"adv", "val"};
   GemmBatch gb;
   gb.n = 2;
   for (int s = 0; s < 2; ++s) {  // second noisy layer weight grads
-    std::string pre = std::string(st[s]) + "2/";
     int n_out = s == 0 ? c.num_actions * c.num_atoms : c.num_atoms;
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->h1[0][s]; p.lda = 512; p.M = B; p.K = 512;
     p.B = s == 0 ? l->dout : l->doutv; p.N = n_out; p.ldb = n_out; p.ldc = n_out;
-    p.C = G + L.off(pre + "mu/w"); p.C2 = G + L.off(pre + "sigma/w"); p.Cb = nullptr; p.Cb2 = G + L.off(pre + "sigma/b");
+    p.C = G + o.w2[s]; p.C2 = G + o.sw2[s]; p.Cb = nullptr; p.Cb2 = G + o.sb2[s];
     p.a_scale = s == 0 ? nz.a2i : nz.v2i; p.c_scale = s == 0 ? nz.a2o : nz.v2o;
     gb.p[s] = p;
   }
-  DZ_TRY(run_tn("noisy2_wgrad", gb, fork_side(l, stream)));
+  DZ_TRY(run_tn("noisy2_wgrad", gb, l->side.fork(stream, stream)));
   for (int s = 0; s < 2; ++s) {  // dh1_s
-    std::string pre = std::string(st[s]) + "2/";
     int n_out = s == 0 ? c.num_actions * c.num_atoms : c.num_atoms;
     GemmProblem p = zero_problem();
     p.A = s == 0 ? l->dout : l->doutv; p.lda = n_out; p.M = B; p.N = n_out; p.K = 512;
-    p.B = P + L.off(pre + "mu/w"); p.B2 = P + L.off(pre + "sigma/w"); p.ldb = n_out;
+    p.B = P + o.w2[s]; p.B2 = P + o.sw2[s]; p.ldb = n_out;
     p.a_scale = s == 0 ? nz.a2i : nz.v2i; p.c_scale = s == 0 ? nz.a2o : nz.v2o;
     p.ldc = 512;
     p.splits = 4; p.split_stride = (long long)2 * B * 512;
@@ -2094,24 +2027,22 @@ int backward_rainbow(dz_learner* l, const float* noise, void* stream) {
     DZ_TRY(finish_nt_batch(jobs, 2, stream));
   }
   for (int s = 0; s < 2; ++s) {  // first noisy layer weight grads
-    std::string pre = std::string(st[s]) + "1/";
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->act3[0]; p.lda = d.feat; p.M = B; p.K = d.feat;
     p.B = l->dh1[s]; p.N = 512; p.ldb = 512; p.ldc = 512;
-    p.C = G + L.off(pre + "mu/w"); p.C2 = G + L.off(pre + "sigma/w"); p.Cb = G + L.off(pre + "mu/b"); p.Cb2 = G + L.off(pre + "sigma/b");
+    p.C = G + o.w1[s]; p.C2 = G + o.sw1[s]; p.Cb = G + o.b1[s]; p.Cb2 = G + o.sb1[s];
     p.a_scale = s == 0 ? nz.a1i : nz.v1i; p.c_scale = s == 0 ? nz.a1o : nz.v1o;
     gb.p[s] = p;
   }
-  DZ_TRY(run_tn("noisy1_wgrad", gb, fork_side(l, stream)));
+  DZ_TRY(run_tn("noisy1_wgrad", gb, l->side.fork(stream, stream)));
   if (l->um) {
     DZ_TRY(um_backward_fc(l->um, noise, stream));   // dh1 hi/lo came from the finish kernel above
     return DZ_OK;
   }
   for (int s = 0; s < 2; ++s) {  // dact3 contributions
-    std::string pre = std::string(st[s]) + "1/";
     GemmProblem p = zero_problem();
     p.A = l->dh1[s]; p.lda = 512; p.M = B; p.N = 512; p.K = d.feat;
-    p.B = P + L.off(pre + "mu/w"); p.B2 = P + L.off(pre + "sigma/w"); p.ldb = 512;
+    p.B = P + o.w1[s]; p.B2 = P + o.sw1[s]; p.ldb = 512;
     p.a_scale = s == 0 ? nz.a1i : nz.v1i; p.c_scale = s == 0 ? nz.a1o : nz.v1o;
     p.ldc = d.feat;
     p.splits = l->nt_splits; p.split_stride = (long long)2 * B * d.feat;
@@ -2126,7 +2057,7 @@ int backward_rainbow(dz_learner* l, const float* noise, void* stream) {
 
 int backward_iqn(dz_learner* l, void* stream) {
   const Dims& d = l->d;
-  const Layout& L = l->lay;
+  const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
   const int B = l->B, N = l->n_head[0], M = B * N;
   float* G = l->buf.d_grads;
@@ -2141,21 +2072,21 @@ int backward_iqn(dz_learner* l, void* stream) {
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->h1[0][0]; p.lda = 512; p.M = M; p.K = 512;
     p.B = l->dout; p.N = d.out; p.ldb = d.out; p.ldc = d.out;
-    p.Cb = G + L.off("head/b");
+    p.Cb = G + o.b2[0];
     int splits = (int)std::min<int64_t>(16, ceil_div(M, 64));
     p.splits = splits; p.split_stride = (long long)513 * d.out; p.C = part_head;
     gb.p[0] = p;
-    DZ_TRY(run_tn("iqn_head_wgrad", gb, fork_side(l, stream)));
-    fb.f[fb.n++] = FinishTN{p.C, splits, p.split_stride, 512, d.out, G + L.off("head/w"), nullptr, p.Cb, nullptr, nullptr, nullptr};
+    DZ_TRY(run_tn("iqn_head_wgrad", gb, l->side.fork(stream, stream)));
+    fb.f[fb.n++] = FinishTN{p.C, splits, p.split_stride, 512, d.out, G + o.w2[0], nullptr, p.Cb, nullptr, nullptr, nullptr};
   }
   {  // dh1
     GemmProblem p = zero_problem();
     p.A = l->dout; p.lda = d.out; p.M = M; p.N = d.out; p.K = 512;
-    p.B = P + L.off("head/w"); p.ldb = d.out; p.C = l->dh1[0]; p.ldc = 512; p.mask = l->h1[0][0];
+    p.B = P + o.w2[0]; p.ldb = d.out; p.C = l->dh1[0]; p.ldc = 512; p.mask = l->h1[0][0];
     gb.p[0] = p;
     if (M >= 512 && d.out <= kSkinnyMaxN) {
       DZ_LAUNCH_NAMED("iqn_head_dgrad", iqn_head_dgrad_kernel, (unsigned)std::min<int64_t>(ceil_div((long long)M * 128, 256), kNumSMs * 8),
-                      256, 0, stream, l->dout, P + L.off("head/w"), l->h1[0][0], l->dh1[0], M, d.out);
+                      256, 0, stream, l->dout, P + o.w2[0], l->h1[0][0], l->dh1[0], M, d.out);
     } else {
       DZ_TRY(run_nt("iqn_head_dgrad", gb, false, stream));
     }
@@ -2180,8 +2111,8 @@ int backward_iqn(dz_learner* l, void* stream) {
       p.MI = d.feat + 1; p.NJ = 512; p.nkb = l->pk_actT.red_pad / kPkKB;
       p.sc_i = 512; p.sc_j = 1; p.splits = l->pk_wgrad_splits; p.split_stride = (long long)(d.feat + 1) * 512;
       p.C = l->pk_wgrad_partial;
-      DZ_TRY(launch_pgemm("iqn_fc1_wgrad", kb, fork_side(l, stream)));
-      fb.f[fb.n++] = FinishTN{p.C, p.splits, p.split_stride, d.feat, 512, G + L.off("fc1/w"), nullptr, G + L.off("fc1/b"), nullptr, nullptr, nullptr};
+      DZ_TRY(launch_pgemm("iqn_fc1_wgrad", kb, l->side.fork(stream, stream)));
+      fb.f[fb.n++] = FinishTN{p.C, p.splits, p.split_stride, d.feat, 512, G + o.w1[0], nullptr, G + o.b1[0], nullptr, nullptr, nullptr};
     }
     {  // dHI[m,k] = sum_n dh1[m,n] W[k,n]
       PkProblem& p = kb.p[0];
@@ -2197,14 +2128,14 @@ int backward_iqn(dz_learner* l, void* stream) {
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->hi[0]; p.lda = d.feat; p.M = M; p.K = d.feat;
     p.B = l->dh1[0]; p.N = 512; p.ldb = 512; p.ldc = 512;
-    p.C = G + L.off("fc1/w"); p.Cb = G + L.off("fc1/b");
+    p.C = G + o.w1[0]; p.Cb = G + o.b1[0];
     gb.p[0] = p;
-    DZ_TRY(run_tn("iqn_fc1_wgrad", gb, fork_side(l, stream)));
+    DZ_TRY(run_tn("iqn_fc1_wgrad", gb, l->side.fork(stream, stream)));
   }
   {  // dHI = dh1 * Wf^T
     GemmProblem p = zero_problem();
     p.A = l->dh1[0]; p.lda = 512; p.M = M; p.N = 512; p.K = d.feat;
-    p.B = P + L.off("fc1/w"); p.ldb = 512; p.C = l->dhi; p.ldc = d.feat;
+    p.B = P + o.w1[0]; p.ldb = 512; p.C = l->dhi; p.ldc = d.feat;
     gb.p[0] = p;
     DZ_TRY(run_nt("iqn_fc1_dgrad", gb, false, stream));
   }
@@ -2223,8 +2154,8 @@ int backward_iqn(dz_learner* l, void* stream) {
     p.MI = d.feat; p.NJ = c.latent_dim + 1; p.nkb = l->pk_dET.red_pad / kPkKB;
     p.sc_i = 1; p.sc_j = d.feat; p.splits = l->pk_embed_wgrad_splits; p.split_stride = (long long)(c.latent_dim + 1) * d.feat;
     p.C = part_embed;
-    DZ_TRY(launch_pgemm("iqn_embed_wgrad", kb, fork_side(l, stream)));
-    fb.f[fb.n++] = FinishTN{p.C, p.splits, p.split_stride, c.latent_dim, d.feat, G + L.off("embed/w"), nullptr, G + L.off("embed/b"), nullptr, nullptr, nullptr};
+    DZ_TRY(launch_pgemm("iqn_embed_wgrad", kb, l->side.fork(stream, stream)));
+    fb.f[fb.n++] = FinishTN{p.C, p.splits, p.split_stride, c.latent_dim, d.feat, G + o.embed_w, nullptr, G + o.embed_b, nullptr, nullptr, nullptr};
   } else {
   DZ_LAUNCH(iqn_hadamard_bwd_kernel, (unsigned)ceil_div((long long)B * d.feat, 256), 256, 0, stream, l->dhi, l->E0, l->act3[0],
               l->dact3, B, N, d.feat);
@@ -2232,18 +2163,18 @@ int backward_iqn(dz_learner* l, void* stream) {
       GemmProblem p = zero_problem();
       p.a_mode = A_PLAIN; p.A = l->cosf[0]; p.lda = c.latent_dim; p.M = M; p.K = c.latent_dim;
       p.B = l->dhi; p.N = d.feat; p.ldb = d.feat; p.ldc = d.feat;
-      p.Cb = G + L.off("embed/b");
+      p.Cb = G + o.embed_b;
       int splits = (int)std::min<int64_t>(16, ceil_div(M, 64));
       p.splits = splits; p.split_stride = (long long)(c.latent_dim + 1) * d.feat; p.C = part_embed;
       gb.p[0] = p;
-      DZ_TRY(run_tn("iqn_embed_wgrad", gb, fork_side(l, stream)));
-      fb.f[fb.n++] = FinishTN{p.C, splits, p.split_stride, c.latent_dim, d.feat, G + L.off("embed/w"), nullptr, p.Cb, nullptr, nullptr, nullptr};
+      DZ_TRY(run_tn("iqn_embed_wgrad", gb, l->side.fork(stream, stream)));
+      fb.f[fb.n++] = FinishTN{p.C, splits, p.split_stride, c.latent_dim, d.feat, G + o.embed_w, nullptr, p.Cb, nullptr, nullptr, nullptr};
     }
   }
   long long mx = 0;
   for (int q = 0; q < fb.n; ++q) mx = std::max<long long>(mx, (long long)(fb.f[q].K + 1) * fb.f[q].N);
   dim3 grid((unsigned)std::min<long long>(ceil_div(mx, 256), kNumSMs * 8), fb.n);
-  DZ_LAUNCH(finish_tn_kernel, grid, 256, 0, (l->side_dirty ? (void*)l->side : stream), fb);
+  DZ_LAUNCH(finish_tn_kernel, grid, 256, 0, l->side.tail(stream), fb);
   return DZ_OK;
 }
 
@@ -2253,7 +2184,7 @@ int backward_iqn(dz_learner* l, void* stream) {
 bool split_norm_active(const dz_learner* l) { return l->um != nullptr && l->cfg.kind != DZ_IQN; }
 
 int norm_fc_range(dz_learner* l, bool apply, void* stream) {
-  const long long begin = l->lay.off(l->cfg.kind == DZ_RAINBOW ? "adv1/mu/w" : "fc1/w");
+  const long long begin = l->po.fc_begin;
   const long long n = l->lay.total - begin;
   DZ_LAUNCH(grad_norm_kernel, kNormBlocks, 256, 0, stream, l->buf.d_grads + begin, n, l->scalars + 8, l->ticket, l->scalars + 1,
             apply ? l->buf.d_counters : l->buf.d_counters + 3, (float*)nullptr, 1);
@@ -2277,19 +2208,15 @@ int run_optimizer(dz_learner* l, float* user_norm, bool apply, void* stream) {
   OptArgs o{c.optimizer, c.learning_rate, c.opt_eps, c.rms_decay, c.adam_b1, c.adam_b2, c.max_global_grad_norm,
             l->buf.d_online, l->buf.d_grads, l->buf.d_opt_state, l->buf.d_opt_state + n, n, norm, l->buf.d_counters,
             parts, nparts, l->scalars + 1, norm, user_norm};
-  const int kOptSmem = kOptRingStages * kOptStageBytes + 64;
   o.stages = kOptRingStages;
-  static bool attr_done = false;
-  if (!attr_done) {
-    DZ_CUDA_OK(cudaFuncSetAttribute(optimizer_bulk_kernel<DZ_ADAM, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptSmem));
-    DZ_CUDA_OK(cudaFuncSetAttribute(optimizer_bulk_kernel<DZ_RMSPROP_CENTERED, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptSmem));
-    attr_done = true;
+  const OptKernel kernel = optimizer_kernel_for(c.optimizer);
+  if (!l->opt_smem_set) {
+    DZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptSmem));
+    l->opt_smem_set = true;
   }
   const long long nchunks = ((o.n >> 2) + kOptChunk - 1) / kOptChunk;
   const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>((long long)kNumSMs * kOptBlocksPerSM, nchunks));
-  const unsigned threads = kOptChunk * 4 / 2;
-  if (c.optimizer == DZ_ADAM) DZ_LAUNCH_NAMED("optimizer_kernel", (optimizer_bulk_kernel<DZ_ADAM, 2>), grid, threads, kOptSmem, stream, o);
-  else DZ_LAUNCH_NAMED("optimizer_kernel", (optimizer_bulk_kernel<DZ_RMSPROP_CENTERED, 2>), grid, threads, kOptSmem, stream, o);
+  DZ_LAUNCH_NAMED("optimizer_kernel", kernel, grid, kOptThreads, kOptSmem, stream, o);
   return DZ_OK;
 }
 
@@ -2298,7 +2225,6 @@ struct WriteBack { const dz_replay_view* view; const int64_t* indices; const flo
 int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* out, int apply_update, float* max_seen,
                 const WriteBack* wb, void* stream, bool weights_packed = false) {
   const dz_learner_config& c = l->cfg;
-  const Dims& d = l->d;
   const int B = l->B;
   const float* on = l->buf.d_online;
   const float* tg = l->buf.d_target;
@@ -2306,7 +2232,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   if (c.kind == DZ_RAINBOW && !batch->d_noise) return fail(DZ_EINVAL, "rainbow update needs d_noise");
   if (c.kind == DZ_IQN && !batch->d_taus) return fail(DZ_EINVAL, "iqn update needs d_taus");
   if (!out || !out->d_loss || !out->d_per_example) return fail(DZ_EINVAL, "update outputs d_loss and d_per_example are required");
-  if (!(weights_packed && l->um != nullptr)) DZ_TRY(join_side(l, stream));   // pending side-stream work (asynchronous randomness)
+  if (!(weights_packed && l->um != nullptr)) DZ_TRY(l->side.join(stream));   // pending side-stream work (asynchronous randomness)
 
   // ---- forward: every network.apply of loss_fn in grouped launches
   TorsoJob jobs[3];
@@ -2319,10 +2245,10 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     if (nj != l->um_npass) return fail(DZ_EINVAL, "tensor-core path: pass count mismatch");
     const uint8_t* const* rows[3] = {nullptr, nullptr, nullptr};
     for (int i = 0; i < nj; ++i) rows[i] = jobs[i].rows;
-    if (weights_packed) DZ_TRY(join_side(l, stream));   // packed on the side stream, concurrently with the sampler
+    if (weights_packed) DZ_TRY(l->side.join(stream));   // packed on the side stream, concurrently with the sampler
     else DZ_TRY(um_pack_weights(l->um, stream));
     DZ_TRY(um_forward_torso(l->um, rows, stream));
-    DZ_TRY(join_side(l, stream));
+    DZ_TRY(l->side.join(stream));
     if (c.kind != DZ_IQN) DZ_TRY(um_forward_fc(l->um, batch->d_noise, stream));
   } else {
     DZ_TRY(forward_torso(l, jobs, nj, B, stream));
@@ -2330,21 +2256,21 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
 
   if (c.kind == DZ_IQN) {
     // online(s_tm1, tau_tm1) | target(s_t, tau_selector) | target(s_t, tau_t)   (iqn/agent.py:192-203)
-    Pass passes[3] = {{on, nullptr, 0, 0, 0}, {tg, nullptr, 2, 1, 0}, {tg, nullptr, 2, 2, 0}};
+    Pass passes[3] = {{on, 0, 0, 0}, {tg, 2, 1, 0}, {tg, 2, 2, 0}};
     const float* t0 = batch->d_taus;
     const float* t1 = t0 + (long long)B * c.tau_samples_s_tm1;
     const float* t2 = t1 + (long long)B * c.tau_samples_policy;
     const float* taus[3] = {t0, t1, t2};
     DZ_TRY(forward_heads_iqn(l, passes, 3, B, taus, true, stream));
   } else if (c.kind == DZ_RAINBOW) {
-    Pass passes[3] = {{on, nullptr, 0, 0, 0}, {on, nullptr, 1, 1, 1}, {tg, nullptr, 2, 2, 2}};
+    Pass passes[3] = {{on, 0, 0, 0}, {on, 1, 1, 1}, {tg, 2, 2, 2}};
     DZ_TRY(forward_heads_rainbow(l, passes, 3, B, batch->d_noise, stream, um));
   } else {
     Pass passes[3];
     int np = 0;
-    passes[np++] = Pass{on, nullptr, 0, 0, 0};
-    if (needs_online_st) passes[np++] = Pass{on, nullptr, 1, 1, 0};
-    passes[np++] = Pass{tg, nullptr, 2, 2, 0};
+    passes[np++] = Pass{on, 0, 0, 0};
+    if (needs_online_st) passes[np++] = Pass{on, 1, 1, 0};
+    passes[np++] = Pass{tg, 2, 2, 0};
     DZ_TRY(forward_heads_plain(l, passes, np, B, stream, um));
   }
 
@@ -2362,10 +2288,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   if (c.kind == DZ_DQN || c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED) {
     DZ_LAUNCH(loss_q_kernel, B, 64, 0, stream, L);
   } else if (c.kind == DZ_C51 || c.kind == DZ_RAINBOW) {
-    size_t smem = (6 * c.num_atoms + c.num_actions + 4) * sizeof(float);
-    const size_t staged = (size_t)(c.num_atoms + 3 * c.num_actions * c.num_atoms + 3 * c.num_atoms) * sizeof(float);
-    if (smem + staged <= 40 * 1024) DZ_LAUNCH_NAMED("loss_categorical_kernel", loss_categorical_staged_kernel, B, 128, smem + staged, stream, L);
-    else DZ_LAUNCH(loss_categorical_kernel, B, 128, smem, stream, L);
+    DZ_LAUNCH_NAMED("loss_categorical_kernel", loss_categorical_staged_kernel, B, 128, categorical_loss_smem(c), stream, L);
   } else {
     if (c.kind == DZ_QRDQN) { L.N = c.num_quantiles; L.Ksel = c.num_quantiles; L.Nt = c.num_quantiles; }
     else { L.N = c.tau_samples_s_tm1; L.Ksel = c.tau_samples_policy; L.Nt = c.tau_samples_s_t; }
@@ -2374,7 +2297,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   }
   {   // the scalar loss / running max priority and replay.update_priorities(ids, priorities) (rainbow/agent.py:198) are
       // independent of the backward pass: both leave the critical path for the side stream
-    void* ls = fork_side(l, stream);
+    void* ls = l->side.fork(stream, stream);
     DZ_LAUNCH(loss_mean_kernel, 1, 32, 0, ls, l->loss_terms, B, out->d_loss, max_seen, L.priorities);
     if (wb) DZ_TRY(launch_update_priorities(wb->view, wb->indices, wb->priorities, B, wb->alpha, wb->view->capacity, ls));
   }
@@ -2384,14 +2307,13 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   else if (c.kind == DZ_IQN) DZ_TRY(backward_iqn(l, stream));
   else DZ_TRY(backward_plain(l, stream));
   if (split_norm_active(l)) {   // every gradient behind the conv tensors is final once the side stream's FC / head wgrads are done
-    void* from = l->side_dirty ? (void*)l->side : stream;
-    DZ_TRY(norm_fc_range(l, apply_update != 0, fork_side2(l, from, stream)));
+    DZ_TRY(norm_fc_range(l, apply_update != 0, l->side2.fork(l->side.tail(stream), stream)));
   }
   DZ_TRY(backward_torso(l, batch->d_s_tm1_rows, stream));
 
   // ---- clip_by_global_norm + adam / rmsprop + apply_updates
-  DZ_TRY(join_side2(l, stream));
-  DZ_TRY(join_side(l, stream));
+  DZ_TRY(l->side2.join(stream));
+  DZ_TRY(l->side.join(stream));
   DZ_TRY(run_optimizer(l, out->d_grad_norm, apply_update != 0, stream));
   return DZ_OK;
 }
@@ -2411,13 +2333,14 @@ int dz_learner_plan_query(const dz_learner_config* cfg, dz_learner_plan* out) {
   memset(&tmp.buf, 0, sizeof(tmp.buf));
   tmp.cfg = *cfg;
   tmp.lay = make_layout(*cfg);
+  DZ_TRY(param_offsets(*cfg, tmp.lay, &tmp.po));
   tmp.d = make_dims(*cfg);
   tmp.B = cfg->batch;
   out->param_count = tmp.lay.total;
   out->num_tensors = (int32_t)tmp.lay.t.size();
   out->opt_state_floats = 2 * tmp.lay.total;
   out->workspace_bytes = carve(&tmp, nullptr);
-  out->noise_floats = cfg->kind == DZ_RAINBOW ? 3 * noise_stride(*cfg, tmp.d) : 0;
+  out->noise_floats = cfg->kind == DZ_RAINBOW ? 3 * noise_layout(*cfg, tmp.d).stride : 0;
   out->tau_floats = cfg->kind == DZ_IQN
                         ? (int64_t)cfg->batch * (cfg->tau_samples_s_tm1 + cfg->tau_samples_policy + cfg->tau_samples_s_t)
                         : 0;
@@ -2447,16 +2370,17 @@ int dz_learner_create(const dz_learner_config* cfg, const dz_learner_buffers* bu
   l->d = make_dims(*cfg);
   l->B = cfg->batch;
   l->um = nullptr;
+  int rc = param_offsets(*cfg, l->lay, &l->po);
+  if (rc != DZ_OK) { delete l; return rc; }
   carve(l, static_cast<char*>(buf->d_workspace));
   if (l->um_ws) {
     UmNetDesc ud = make_um_desc(l);
-    int rc = um_net_create(ud, l->um_ws, &l->um);
+    rc = um_net_create(ud, l->um_ws, &l->um);
     if (rc != DZ_OK) { delete l; return rc; }
-    const bool three = ud.npass == 3;
     l->um_npass = ud.npass;
-    l->um_set[0] = 0; l->um_set[1] = three ? 1 : 2; l->um_set[2] = 2;
+    const int um_set[3] = {0, ud.npass == 3 ? 1 : 2, 2};   // torso activation set of each tensor-core pass
     for (int i = 0; i < ud.npass; ++i) {   // the fp32 views the remaining FMA kernels, the losses and the tests read
-      const int set = l->um_set[i];
+      const int set = um_set[i];
       l->act1[set] = um_act_f32(l->um, 1, i); l->act2[set] = um_act_f32(l->um, 2, i); l->act3[set] = um_act_f32(l->um, 3, i);
       if (ud.use_fc)
         for (int s = 0; s < ud.nstream; ++s) l->h1[set][s] = um_h1_f32(l->um, i, s);
@@ -2465,13 +2389,16 @@ int dz_learner_create(const dz_learner_config* cfg, const dz_learner_buffers* bu
       for (int s = 0; s < ud.nstream; ++s) l->dh1[s] = um_dh1_f32(l->um, s);
     l->dact3 = um_dact_f32(l->um, 3); l->dact2 = um_dact_f32(l->um, 2); l->dact1 = um_dact_f32(l->um, 1);
   }
-  l->side = nullptr; l->ev_fork = nullptr; l->ev_join = nullptr; l->side_dirty = false;
-  l->side2 = nullptr; l->ev_fork2 = nullptr; l->ev_join2 = nullptr; l->side2_dirty = false;
-  cudaError_t se = cudaStreamCreateWithFlags(&l->side, cudaStreamNonBlocking);
-  if (se == cudaSuccess) se = cudaStreamCreateWithFlags(&l->side2, cudaStreamNonBlocking);
-  for (cudaEvent_t* ev : {&l->ev_fork, &l->ev_join, &l->ev_fork2, &l->ev_join2})
-    if (se == cudaSuccess) se = cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
+  cudaError_t se = l->side.create();
+  if (se == cudaSuccess) se = l->side2.create();
   if (se != cudaSuccess) { dz_learner_destroy(l); return fail(DZ_ECUDA, "side streams: %s", cudaGetErrorString(se)); }
+  // The categorical loss needs more than the default 48 KB of dynamic shared memory at large num_actions x num_atoms.
+  // The attribute is per device: set it for the device this learner is created on.
+  const size_t loss_smem = categorical_loss_smem(*cfg);
+  if ((cfg->kind == DZ_C51 || cfg->kind == DZ_RAINBOW) && loss_smem > 48 * 1024) {
+    se = cudaFuncSetAttribute(loss_categorical_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)loss_smem);
+    if (se != cudaSuccess) { dz_learner_destroy(l); return fail(DZ_ECUDA, "kernel attributes: %s", cudaGetErrorString(se)); }
+  }
   if (l->pk_on) {
     // fused epilogues only write the valid region of these images: zero the padding once, and set the constant
     // row of ones (bias-gradient row) of the transposed activation image
@@ -2497,12 +2424,8 @@ int dz_learner_create(const dz_learner_config* cfg, const dz_learner_buffers* bu
 void dz_learner_destroy(dz_learner* l) {
   if (!l) return;
   um_net_destroy(l->um);
-  if (l->side) { cudaStreamSynchronize(l->side); cudaStreamDestroy(l->side); }
-  if (l->side2) { cudaStreamSynchronize(l->side2); cudaStreamDestroy(l->side2); }
-  if (l->ev_fork) cudaEventDestroy(l->ev_fork);
-  if (l->ev_join) cudaEventDestroy(l->ev_join);
-  if (l->ev_fork2) cudaEventDestroy(l->ev_fork2);
-  if (l->ev_join2) cudaEventDestroy(l->ev_join2);
+  l->side.destroy();
+  l->side2.destroy();
   delete l;
 }
 
@@ -2517,7 +2440,7 @@ int dz_learner_learn(dz_learner* l, const dz_replay_view* replay, int32_t priori
   // conv weight images do not depend on the sampled batch: pack them on the side stream while the sampler runs
   const bool pack_aside = l->um != nullptr;
   if (pack_aside) {
-    void* ws = fork_side(l, stream);
+    void* ws = l->side.fork(stream, stream);
     DZ_TRY(um_pack_weights(l->um, ws));
   }
   DZ_TRY(launch_sample(replay, prioritized, &io->sample_in, &io->sample_out, B, ex, stream));
@@ -2538,7 +2461,7 @@ int dz_learner_learn(dz_learner* l, const dz_replay_view* replay, int32_t priori
 // enqueued on `stream` and before the next dz_learner_learn / dz_learner_update / dz_learner_q_values on `stream`; any
 // other consumer of the buffers must synchronise the device first.
 int dz_learner_generate_randomness_async(dz_learner* l, uint64_t seed, float* d_taus, float* d_noise, void* stream) {
-  return dz_learner_generate_randomness(l, seed, d_taus, d_noise, fork_side(l, stream));
+  return dz_learner_generate_randomness(l, seed, d_taus, d_noise, l->side.fork(stream, stream));
 }
 
 int dz_learner_generate_randomness(dz_learner* l, uint64_t seed, float* d_taus, float* d_noise, void* stream) {
@@ -2548,7 +2471,7 @@ int dz_learner_generate_randomness(dz_learner* l, uint64_t seed, float* d_taus, 
     DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_taus, n, seed, l->buf.d_counters, 0, 1u);
   }
   if (c.kind == DZ_RAINBOW && d_noise) {
-    long long n = 3 * noise_stride(c, l->d);
+    long long n = 3 * noise_layout(c, l->d).stride;
     DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_noise, n, seed, l->buf.d_counters, 1, 2u);
   }
   DZ_LAUNCH(bump_counter_kernel, 1, 1, 0, stream, l->buf.d_counters, 1);
@@ -2558,11 +2481,11 @@ int dz_learner_generate_randomness(dz_learner* l, uint64_t seed, float* d_taus, 
 int dz_learner_q_values(dz_learner* l, const uint8_t* d_obs, const float* d_taus, const float* d_noise, float* d_q_out, void* stream) {
   const dz_learner_config& c = l->cfg;
   const float* on = l->buf.d_online;
-  DZ_TRY(join_side(l, stream));   // pending side-stream work (asynchronous randomness)
+  DZ_TRY(l->side.join(stream));   // pending side-stream work (asynchronous randomness)
   DZ_LAUNCH(make_row_table_kernel, 1, 32, 0, stream, d_obs, (long long)0, 1, l->rows_act);
   TorsoJob job{on, l->rows_act, 1};   // use activation set 1 so a pending backward's set-0 buffers stay intact
   DZ_TRY(forward_torso(l, &job, 1, 1, stream));
-  Pass pass{on, nullptr, 1, 1, 0};
+  Pass pass{on, 1, 1, 0};
   int nq = 1;
   if (c.kind == DZ_IQN) {
     if (!d_taus) return fail(DZ_EINVAL, "iqn q_values needs taus[tau_samples_policy]");
@@ -2593,12 +2516,12 @@ int dz_learner_act_batch(dz_learner* l, const uint8_t* d_obs, int32_t E, const f
   const float* on = l->buf.d_online;
   if (E < 1 || E > l->B) return fail(DZ_EINVAL, "act_batch: 1 <= E <= learner batch");
   if (!d_obs || !d_q_out || !d_actions) return fail(DZ_EINVAL, "act_batch: null buffer");
-  DZ_TRY(join_side(l, stream));
+  DZ_TRY(l->side.join(stream));
   const long long obs_bytes = (long long)l->d.H * l->d.W * l->d.C;
   DZ_LAUNCH(make_row_table_kernel, (unsigned)ceil_div(E, 64), 64, 0, stream, d_obs, obs_bytes, (int)E, l->rows_act);
   TorsoJob job{on, l->rows_act, 1};
   DZ_TRY(forward_torso(l, &job, 1, E, stream));
-  Pass pass{on, nullptr, 1, 1, 0};
+  Pass pass{on, 1, 1, 0};
   int nq = 1;
   if (c.kind == DZ_IQN) {
     if (!d_taus) return fail(DZ_EINVAL, "iqn act_batch needs taus[E][tau_samples_policy]");

@@ -17,10 +17,12 @@ REL = 1e-5
 KINDS = list(lo.AGENT_KINDS)
 
 
-def make_case(kind, B, hw, seed, num_actions=6):
+def make_case(kind, B, hw, seed, num_actions=6, num_atoms=None):
   from dqn_zoo_b200 import learner as dl
   rs = np.random.RandomState(seed)
   small = dict(num_atoms=51, num_quantiles=201) if hw == 84 else dict(num_atoms=21, num_quantiles=33)
+  if num_atoms is not None:
+    small['num_atoms'] = num_atoms
   spec = lo.NetSpec(kind, num_actions, obs_hw=hw, **small)
   net = dl.NetworkSpec(kind, num_actions, obs_shape=(hw, hw, 4), tau_samples_s_tm1=64 if hw == 84 else 8,
                        tau_samples_policy=64 if hw == 84 else 5, tau_samples_s_t=64 if hw == 84 else 7, **small)
@@ -109,8 +111,8 @@ def test_loss_and_gradients_match_oracle(kind, hw, B):
   check_loss_and_gradients(kind, hw, B)
 
 
-def check_loss_and_gradients(kind, hw, B, fma_torso=False):
-  spec, net, L, O, rs = make_case(kind, B, hw, seed=3)
+def check_loss_and_gradients(kind, hw, B, fma_torso=False, **case):
+  spec, net, L, O, rs = make_case(kind, B, hw, seed=3, **case)
   if fma_torso:   # the tensor-core path must not be active, or the caller would not test the fp32-FMA torso
     from dqn_zoo_b200 import _lib
     with pytest.raises(ValueError):
@@ -148,6 +150,13 @@ def check_loss_and_gradients(kind, hw, B, fma_torso=False):
     worst[name] = rel_err(got, want)
   bad = {k: v for k, v in worst.items() if v > REL}
   assert not bad, bad
+
+
+@pytest.mark.parametrize('kind', ['c51', 'rainbow'])
+def test_largest_categorical_head_matches_oracle(kind):
+  """64 actions x 128 atoms, the largest categorical head the learner accepts: the loss kernel then stages 103,696
+  bytes of head outputs in shared memory, beyond the default 48 KB.  Same loss/gradient parity."""
+  check_loss_and_gradients(kind, 84, 32, num_actions=64, num_atoms=128)
 
 
 @pytest.mark.parametrize('kind', KINDS)
