@@ -115,10 +115,12 @@ _SIGNATURES = {
     'dz_test_learner_buffer': (i32, [vp, C.c_char_p, vp, vp]),
     'dz_test_copy': (i32, [vp, vp, i64, vp]),
     'dz_test_learner_trace': (i32, [vp, C.c_char_p, vp]),
+    'dz_test_learner_mma_path': (i32, [vp, C.c_char_p, C.POINTER(i32)]),
     'dz_debug_timeline': (i32, [vp]),
     'dz_test_tc_pgemm_work': (i64, [i32, i32, i32]),
     'dz_test_tc_pgemm': (i32, [vp, i32, i32, i32, vp, i32, i32, i32, i32, i32, vp, vp, i64, i64, i32, i64, vp, i32, vp]),
     'dz_test_umma_gemm': (i32, [vp, i32, vp, i32, i32, i32, i32, i32, vp, i32, i32, vp, i32, vp, vp, vp, vp]),
+    'dz_test_umma_gemm_path': (i32, [vp, i32, vp, i32, i32, i32, i32, i32, vp, i32, i32, vp, i32, vp, vp, vp, i32, vp]),
 }
 
 EXPORTS = tuple(_SIGNATURES)

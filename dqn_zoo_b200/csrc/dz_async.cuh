@@ -25,6 +25,13 @@ __device__ __forceinline__ void fence_mbarrier_init() { asm volatile("fence.mbar
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// Arrive only where `pred` holds, without a branch: code between asynchronous warpgroup MMAs must stay free of
+// divergent paths, or ptxas serialises the MMAs.
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %1, 0;\n@p mbarrier.arrive.shared::cta.b64 _, [%0];\n}\n" ::"r"(smem_u32(bar)),
+               "r"((int)pred)
+               : "memory");
+}
 // Arrive and add `bytes` to the phase's expected transaction count (the copies that complete on `bar`).
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");

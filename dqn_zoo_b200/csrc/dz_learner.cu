@@ -2568,6 +2568,16 @@ int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace) {
   return DZ_OK;
 }
 
+// Test hook: the MMA path of the tensor-core launch named `tag` (the tags of dz_test_learner_trace): 1 warp-level
+// mma.sync kernel, 2 wgmma kernel.
+int dz_test_learner_mma_path(dz_learner* l, const char* tag, int32_t* path) {
+  if (!l->um) return fail(DZ_EINVAL, "the tensor-core path is not active for this learner");
+  const int p = um_net_mma_path(l->um, tag);
+  if (p < 0) return fail(DZ_EINVAL, "no tensor-core launch '%s' in this learner", tag ? tag : "");
+  *path = p;
+  return DZ_OK;
+}
+
 // Test hook: device-to-device copy out of an internal buffer (tests hold only the raw pointer).
 int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream) {
   DZ_CUDA_OK(cudaMemcpyAsync(d_dst, d_src, (size_t)bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));

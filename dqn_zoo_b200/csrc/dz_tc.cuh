@@ -1,5 +1,6 @@
 // Tensor-core helpers shared by the learner's GEMM kernels (sm_90a): the warp-level m16n8k8 tf32 MMA with the
-// shared-memory fragment loads of one k-step, the swizzled tile offsets, and the tf32 split
+// shared-memory fragment loads of one k-step, the warpgroup MMA (wgmma) k-step on K-major swizzled tiles, the swizzled
+// tile offsets, and the tf32 split
 //
 //     x = hi + lo,  hi = rn_tf32(x),  lo = rn_tf32(x - hi)      (error-compensated 3xTF32: D += Ah*Bh + Al*Bh + Ah*Bl)
 //
@@ -62,6 +63,68 @@ __device__ __forceinline__ void warp_kstep_3xtf32(float (&sum)[MT][NT][4], const
       for (int e = 0; e < 4; ++e) sum[mt][nt][e] += p[e];
     }
   }
+}
+
+// ---- warpgroup MMA (wgmma, sm_90a) on K-major SWIZZLE_128B operands -----------------------------------------------
+// Shared-memory matrix descriptor of a K-major SWIZZLE_128B tile (the layout the TMA loads leave): 128-byte rows, groups
+// of 8 rows 1024 bytes apart (stride byte offset), 1024-byte aligned tile.  The leading byte offset is unused by this
+// layout.  A k-step of 8 tf32 elements further along the rows is the same descriptor with the start address 32 bytes on
+// (the swizzle is a function of the absolute address bits, as for the TMA unit that wrote the tile).
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Pins the accumulator registers between the asynchronous MMAs and ordinary register accesses (the compiler must not
+// move reads of d across a wgmma_wait, nor writes of d across an MMA issue).
+template <int NA>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[NA]) {
+#pragma unroll
+  for (int e = 0; e < NA; ++e) asm volatile("" : "+f"(d[e])::"memory");
+}
+
+// D (m64 x N, fp32) = A * B^T (+ D when scale_d != 0), A: 64 x 8, B: N x 8, both tf32 from shared-memory descriptors.
+// Per thread: d[4 i + 2 h + e] = D[16 w + g + 8 h][8 i + 2 t + e], w = warp of the warpgroup, g = lane / 4, t = lane % 4.
+__device__ __forceinline__ void wgmma_m64k8(float (&d)[16], uint64_t da, uint64_t db, int scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_m64k8(float (&d)[32], uint64_t da, uint64_t db, int scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+
+// Issues one k-step of 8 of the error-compensated product of a warpgroup's m64 x N tile as one wgmma group,
+//     d = Al*Bh, d += Ah*Bl, d += Ah*Bh        (the order and the zero start of warp_kstep_3xtf32)
+// from K-major SWIZZLE_128B hi/lo tiles at shared addresses a_hi / a_lo / b_hi / b_lo; k0: first reduction element.
+// The caller retires the group with wgmma_wait and adds d into its fp32 sums with round-to-nearest adds.
+template <int NA>
+__device__ __forceinline__ void wgmma_kstep_3xtf32(float (&d)[NA], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo, int k0) {
+  const uint32_t ko = (uint32_t)k0 * 4u;
+  const uint64_t ah = wgmma_desc_sw128(a_hi + ko), al = wgmma_desc_sw128(a_lo + ko);
+  const uint64_t bh = wgmma_desc_sw128(b_hi + ko), bl = wgmma_desc_sw128(b_lo + ko);
+  wgmma_fence_acc(d);
+  wgmma_fence();
+  wgmma_m64k8(d, al, bh, 0);                        // small cross terms first, from zero
+  wgmma_m64k8(d, ah, bl, 1);
+  wgmma_m64k8(d, ah, bh, 1);
+  wgmma_commit();
+  wgmma_fence_acc(d);
 }
 
 // Row / column of D that element e of fragment (mt, nt) of warp_kstep_3xtf32 holds, relative to (m0, n0).

@@ -103,11 +103,23 @@ int UmPlan::configure() {
   if (done) return DZ_OK;
   DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  DZ_CUDA_OK(cudaFuncSetAttribute(um::wgmma_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  DZ_CUDA_OK(cudaFuncSetAttribute(um::wgmma_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   done = true;
   return DZ_OK;
 }
 
-int UmPlan::launch(const char* tag, const UmLaunch& l, void* stream, long long* d_trace) const {
+bool UmPlan::wgmma_eligible(const UmLaunch& l) const {
+  for (int ci = l.cta0; ci < l.cta0 + l.nctas; ++ci) {
+    const UmProblem& pr = probs[ctas[ci].prob];
+    for (const UmOperand* o : {&pr.A, &pr.B})
+      if (o->mn_major || o->nparts != 2 || o->convert) return false;
+    if (pr.ksteps != 4) return false;
+  }
+  return true;
+}
+
+int UmPlan::launch(const char* tag, const UmLaunch& l, void* stream, long long* d_trace, int path) const {
   if (l.nctas <= 0) return DZ_OK;
   if (!d_ctas) return fail(DZ_EINVAL, "umma plan not uploaded");
   if (l.stages < 1 || l.stages > um::kStagesMax || l.stage_bytes % 1024) return fail(DZ_EINVAL, "umma launch geometry");
@@ -125,10 +137,25 @@ int UmPlan::launch(const char* tag, const UmLaunch& l, void* stream, long long* 
   if ((size_t)stages * l.stage_bytes < (size_t)128 * l.njt * 4) return fail(DZ_EINVAL, "umma launch: stage buffers smaller than the store-phase staging tile");
   const int v = l.njt == 32 ? 0 : 1;
   if (l.njt != 32 && l.njt != 64) return fail(DZ_EINVAL, "umma launch: NJT must be 32 or 64");
+  if (path != UM_PATH_AUTO && path != UM_PATH_MMA_SYNC && path != UM_PATH_WGMMA) return fail(DZ_EINVAL, "umma launch: unknown MMA path");
+  const bool wg = path == UM_PATH_AUTO ? wgmma_eligible(l) : path == UM_PATH_WGMMA;
+  if (wg && !wgmma_eligible(l)) return fail(DZ_EINVAL, "umma launch: the wgmma path needs K-major, pre-split operands and four k-steps per stage");
+  if (wg)
+    for (int ci = l.cta0; ci < l.cta0 + l.nctas; ++ci)   // both m64 halves of A (hi and lo) are read from inside the stage
+      if (probs[ctas[ci].prob].A.part_bytes + 16384u > l.stage_bytes) return fail(DZ_EINVAL, "umma launch: stage too small for the wgmma A reads");
   DZ_TRY(configure());
   um::UmMaps lm;
   for (int q = 0; q < l.nmaps; ++q) lm.m[q] = maps[l.map_ids[q]];
   for (int q = l.nmaps; q < um::kMaxMapsPerLaunch; ++q) lm.m[q] = maps[l.map_ids[0]];
+  if (wg) {
+    if (v == 0)
+      DZ_LAUNCH_NAMED(tag, um::wgmma_gemm_kernel<32>, (unsigned)l.nctas, um::kThreadsW, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps,
+                      stages, l.stage_bytes, d_trace);
+    else
+      DZ_LAUNCH_NAMED(tag, um::wgmma_gemm_kernel<64>, (unsigned)l.nctas, um::kThreadsW, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps,
+                      stages, l.stage_bytes, d_trace);
+    return DZ_OK;
+  }
   if (v == 0)
     DZ_LAUNCH_NAMED(tag, um::umma_gemm_kernel<32>, (unsigned)l.nctas, um::kThreadsU, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps, stages,
                     l.stage_bytes, d_trace);
@@ -160,16 +187,18 @@ int um_split(const float* x, float* hi, float* lo, long long n, void* stream) {
 
 using namespace dz;
 
-// Self test: C[MI][NJ] = sum_r A(i,r) B(j,r).
+// Self test: C[MI][NJ] = sum_r A(i,r) B(j,r); NJ and R multiples of 4, and MI too when A is MN-major (TMA row strides).
 //   a_mn_major = 0: d_A is [MI][R] (K-major source);  1: d_A is [R][MI] (MN-major source).  Same for B with NJ <= 64.
 //   convert = 0: operands are split into hi/lo by a helper kernel first (the layout the activations use);
 //   convert = 1: raw fp32 tiles are split in shared memory by the converter warps (the layout the weights use),
 //                optionally scaled by d_scale_r[r] (applied to A).
 //   epi_rows = 1: UM_EPI_ROWS epilogue (+ d_bias[j], relu, tf32 hi/lo outputs in d_hi / d_lo besides d_C).
-extern "C" int dz_test_umma_gemm(const float* d_A, int32_t a_mn_major, const float* d_B, int32_t b_mn_major, int32_t MI, int32_t NJ,
-                                 int32_t R, int32_t convert, const float* d_scale_r, int32_t stages, int32_t epi_rows,
-                                 const float* d_bias, int32_t relu, float* d_C, float* d_hi, float* d_lo, void* stream) {
-  if (NJ < 4 || NJ > 64 || NJ % 4 || MI % 4 || R % 4) return fail(DZ_EINVAL, "umma self test extents");
+//   path: 0 automatic (as the learner's launches), 1 mma.sync kernel, 2 wgmma kernel (K-major pre-split operands only).
+extern "C" int dz_test_umma_gemm_path(const float* d_A, int32_t a_mn_major, const float* d_B, int32_t b_mn_major, int32_t MI,
+                                      int32_t NJ, int32_t R, int32_t convert, const float* d_scale_r, int32_t stages,
+                                      int32_t epi_rows, const float* d_bias, int32_t relu, float* d_C, float* d_hi, float* d_lo,
+                                      int32_t path, void* stream) {
+  if (NJ < 4 || NJ > 64 || NJ % 4 || (a_mn_major && MI % 4) || R % 4) return fail(DZ_EINVAL, "umma self test extents");
   const int njt = NJ <= 32 ? 32 : 64;
   UmPlan plan;
   float *a_hi = nullptr, *a_lo = nullptr, *b_hi = nullptr, *b_lo = nullptr;
@@ -250,11 +279,18 @@ extern "C" int dz_test_umma_gemm(const float* d_A, int32_t a_mn_major, const flo
   if (rc == DZ_OK) rc = plan.upload();
   if (rc != DZ_OK) return rc;
   l.njt = njt; l.stage_bytes = a_bytes + b_bytes; l.stages = stages > 0 ? stages : 4;   // 4 x <= 48 KB + control block fits
-  rc = plan.launch("umma_selftest", l, stream);
+  rc = plan.launch("umma_selftest", l, stream, nullptr, path);
   cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream);
   plan.release();
   if (a_hi) { cudaFree(a_hi); cudaFree(a_lo); cudaFree(b_hi); cudaFree(b_lo); }
   if (rc != DZ_OK) return rc;
   if (e != cudaSuccess) return fail(DZ_ECUDA, "umma self test: %s", cudaGetErrorString(e));
   return DZ_OK;
+}
+
+extern "C" int dz_test_umma_gemm(const float* d_A, int32_t a_mn_major, const float* d_B, int32_t b_mn_major, int32_t MI, int32_t NJ,
+                                 int32_t R, int32_t convert, const float* d_scale_r, int32_t stages, int32_t epi_rows,
+                                 const float* d_bias, int32_t relu, float* d_C, float* d_hi, float* d_lo, void* stream) {
+  return dz_test_umma_gemm_path(d_A, a_mn_major, d_B, b_mn_major, MI, NJ, R, convert, d_scale_r, stages, epi_rows, d_bias, relu,
+                                d_C, d_hi, d_lo, UM_PATH_AUTO, stream);
 }

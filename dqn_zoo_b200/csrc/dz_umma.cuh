@@ -12,13 +12,15 @@
 //            unit (that is the zero padding of the input-gradient convolutions).
 //   MN-major (row index contiguous in the source, e.g. W[k][n] for y = xW): a stage is [32 r][32 mn] slabs, LBO
 //            apart; the MMA warps' fragment loads do the transposition — no shuffles, no transposed copies.  (This is
-//            why the MMA is the warp-level m16n8k8 one: tf32 wgmma only reads K-major operands from shared memory.)
+//            why these launches use the warp-level m16n8k8 MMA, umma_gemm_kernel: tf32 wgmma only reads K-major
+//            operands from shared memory.  Launches whose operands are all K-major and pre-split run on warpgroup
+//            MMAs that read the staged tiles through shared-memory descriptors, wgmma_gemm_kernel.)
 //
 // Precision: activations are stored ONCE as tf32 hi/lo pairs by the producing epilogue (x = hi + lo, both exactly
 // representable), fp32 weights are split in place in shared memory by converter warps (raw tile -> hi in place, lo
 // in the sibling buffer; the split is position-wise, so it is swizzle-agnostic), D += Al*Bh + Ah*Bl + Ah*Bh.  The
 // tensor core truncates its fp32 accumulator, so each k-step's products are added into the fp32 sums with
-// round-to-nearest adds (dz_tc.cuh, warp_kstep_3xtf32).
+// round-to-nearest adds (dz_tc.cuh, warp_kstep_3xtf32 / wgmma_kstep_3xtf32).
 //
 // The TMA "program" of every CTA (which boxes of which tensor map go where in each stage) is a table built once on
 // the host (dz_umma.cu): the device side is geometry-free.
@@ -204,6 +206,68 @@ __device__ __forceinline__ float4* stage_chunk(uint8_t* base, int r, int c) {
   return reinterpret_cast<float4*>(base + (size_t)r * (NJT * 4) + (size_t)(((c & ~7) | ((c ^ r) & 7)) << 4));
 }
 
+// Cooperative store phase: the fp32 tile staged by stage_chunk<NJT> at stage_base goes out through the row epilogue
+// (bias, ReLU, mask, tf32 hi/lo split; one D row = one output pixel / sample) or the partial epilogue.  tid: 0..383,
+// the thread's index among the 384 threads that take part.
+template <int NJT>
+__device__ __forceinline__ void store_tile(const UmProblem& p, const UmCta& cta, uint8_t* stage_base, int tid) {
+  const int NJ = p.NJ, cpr = NJ >> 2;
+  const int items = 128 * cpr;
+  // idx -> (row, chunk) and row -> (outer, inner) without integer divisions: rows < 128, so a 16-bit reciprocal is exact
+  const uint32_t inv_cpr = (65536u + (uint32_t)cpr - 1u) / (uint32_t)cpr;
+  constexpr int kIters = (128 * (NJT / 4) + 383) / 384;
+  if (p.epi == UM_EPI_ROWS) {
+    const int pw = p.pw;
+    const long long ld = p.out_ld;
+    const bool relu = p.relu != 0;
+    const float* __restrict__ maskp = p.mask;
+    const float* __restrict__ bias = p.bias;
+    float* __restrict__ of = p.out_f32; float* __restrict__ oh = p.out_hi; float* __restrict__ ol = p.out_lo;
+    const uint32_t inv_pw = pw >= 128 ? 0u : (65536u + (uint32_t)pw - 1u) / (uint32_t)pw;
+#pragma unroll
+    for (int j = 0; j < kIters; ++j) {
+      const int idx = tid + j * 384;
+      if (idx >= items) continue;
+      const int r = (int)(((uint32_t)idx * inv_cpr) >> 16), c = idx - r * cpr;
+      const int ro = (int)(((uint32_t)r * inv_pw) >> 16), ri = r - ro * pw;
+      if (ro >= cta.ph_valid || ri >= cta.pw_valid) continue;
+      const long long o = ((long long)cta.row_base + (long long)ro * p.rs_outer + (long long)ri * p.rs_inner) * ld + 4 * c;
+      float4 v = *stage_chunk<NJT>(stage_base, r, c);
+      if (bias) { const float4 b4 = *reinterpret_cast<const float4*>(bias + 4 * c); v.x += b4.x; v.y += b4.y; v.z += b4.z; v.w += b4.w; }
+      if (relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+      if (maskp) {
+        const float4 m4 = *reinterpret_cast<const float4*>(maskp + o);
+        v.x = m4.x > 0.f ? v.x : 0.f; v.y = m4.y > 0.f ? v.y : 0.f; v.z = m4.z > 0.f ? v.z : 0.f; v.w = m4.w > 0.f ? v.w : 0.f;
+      }
+      if (of) *reinterpret_cast<float4*>(of + o) = v;
+      if (oh) {
+        float4 h, l;
+        split_tf32(v, h, l);
+        *reinterpret_cast<float4*>(oh + o) = h;
+        *reinterpret_cast<float4*>(ol + o) = l;
+      }
+    }
+  } else {
+    float* __restrict__ C = p.C + (long long)cta.split * p.split_stride;
+    const float* __restrict__ scale_i = p.scale_i;
+    const long long sc_i = p.sc_i, sc_j = p.sc_j;
+    const bool vec = sc_j == 1 && (sc_i & 3) == 0 && ((reinterpret_cast<uintptr_t>(C) & 15) == 0);
+#pragma unroll
+    for (int j = 0; j < kIters; ++j) {
+      const int idx = tid + j * 384;
+      if (idx >= items) continue;
+      const int r = (int)(((uint32_t)idx * inv_cpr) >> 16), c = idx - r * cpr;
+      const int i = cta.i0 + r;
+      if (i >= p.MI) continue;
+      float4 v = *stage_chunk<NJT>(stage_base, r, c);
+      if (scale_i) { const float s = scale_i[i]; v.x *= s; v.y *= s; v.z *= s; v.w *= s; }
+      float* dst = C + (long long)i * sc_i + (long long)(4 * c) * sc_j;
+      if (vec) *reinterpret_cast<float4*>(dst) = v;
+      else { dst[0] = v.x; dst[sc_j] = v.y; dst[2 * sc_j] = v.z; dst[3 * sc_j] = v.w; }
+    }
+  }
+}
+
 // grid = number of CTA descriptors; dynamic smem = kCtlBytes + stages * stage_bytes + 1024 (alignment slack).
 // Warp roles: 0 TMA producer | 1 barrier set-up | 2-5 MMA (warp 2 + q owns D rows [32q, 32q + 32), all NJT columns, as
 // m16n8k8 fragments read straight from the staged tiles) | 6-13 operand converters.  All twelve warps 2-13 take part in the
@@ -387,64 +451,203 @@ __global__ void __launch_bounds__(kThreadsU, 1)
           }
     }
     bar_sync_coop();
-    const int tid = threadIdx.x - 64;
-    const int NJ = p.NJ, cpr = NJ >> 2;
-    const int items = 128 * cpr;
-    // idx -> (row, chunk) and row -> (outer, inner) without integer divisions: rows < 128, so a 16-bit reciprocal is exact
-    const uint32_t inv_cpr = (65536u + (uint32_t)cpr - 1u) / (uint32_t)cpr;
-    constexpr int kIters = (128 * (NJT / 4) + 383) / 384;
-    if (p.epi == UM_EPI_ROWS) {
-      const int pw = p.pw;
-      const long long ld = p.out_ld;
-      const bool relu = p.relu != 0;
-      const float* __restrict__ maskp = p.mask;
-      const float* __restrict__ bias = p.bias;
-      float* __restrict__ of = p.out_f32; float* __restrict__ oh = p.out_hi; float* __restrict__ ol = p.out_lo;
-      const uint32_t inv_pw = pw >= 128 ? 0u : (65536u + (uint32_t)pw - 1u) / (uint32_t)pw;
-#pragma unroll
-      for (int j = 0; j < kIters; ++j) {
-        const int idx = tid + j * 384;
-        if (idx >= items) continue;
-        const int r = (int)(((uint32_t)idx * inv_cpr) >> 16), c = idx - r * cpr;
-        const int ro = (int)(((uint32_t)r * inv_pw) >> 16), ri = r - ro * pw;
-        if (ro >= cta.ph_valid || ri >= cta.pw_valid) continue;
-        const long long o = ((long long)cta.row_base + (long long)ro * p.rs_outer + (long long)ri * p.rs_inner) * ld + 4 * c;
-        float4 v = *stage_chunk<NJT>(stage_base, r, c);
-        if (bias) { const float4 b4 = *reinterpret_cast<const float4*>(bias + 4 * c); v.x += b4.x; v.y += b4.y; v.z += b4.z; v.w += b4.w; }
-        if (relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
-        if (maskp) {
-          const float4 m4 = *reinterpret_cast<const float4*>(maskp + o);
-          v.x = m4.x > 0.f ? v.x : 0.f; v.y = m4.y > 0.f ? v.y : 0.f; v.z = m4.z > 0.f ? v.z : 0.f; v.w = m4.w > 0.f ? v.w : 0.f;
+    store_tile<NJT>(p, cta, stage_base, threadIdx.x - 64);
+  }
+  if (tr && warp == 2 && lane == 0) trace[321] = clock64();                                         // stores issued
+  if (tr && threadIdx.x == 0) trace[322] = clock64();
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Warpgroup-MMA sibling of umma_gemm_kernel for problems whose operands are both K-major tf32 hi/lo pairs that need no
+// conversion (conv2 / conv3 forward and input gradient): the staged tiles are already in the layout wgmma reads, so
+// the MMAs take their operands straight from shared-memory descriptors, with no fragment loads.  TMA program, stage
+// ring, PDL points, clock stamps and both epilogues are those of umma_gemm_kernel.
+constexpr int kThreadsW = 3 * 128;   // producer warpgroup + two consumer warpgroups
+constexpr int kConsumerWarps = 8;
+
+// Clock stamp *addr = clock64() where `pred` holds, without a branch (see mbar_arrive_if).
+__device__ __forceinline__ void stamp_if(long long* addr, bool pred) {
+  asm volatile("{\n.reg .pred p;\n.reg .b64 c;\nsetp.ne.b32 p, %1, 0;\nmov.u64 c, %%clock64;\n@p st.global.b64 [%0], c;\n}\n" ::"l"(addr),
+               "r"((int)pred)
+               : "memory");
+}
+
+// Rows of the CTA's 128-row tile that reach the output: the tail beyond them (padding, TMA zero fill) is never stored,
+// so an m64 half that lies entirely in it needs no MMAs.
+__device__ __forceinline__ int tile_rows_out(const UmProblem& p, const UmCta& c) {
+  if (p.epi == UM_EPI_ROWS) {
+    if (c.ph_valid <= 0 || c.pw_valid <= 0) return 0;
+    const long long n = (long long)(c.ph_valid - 1) * p.pw + min(c.pw_valid, p.pw);
+    return (int)min(n, 128LL);
+  }
+  return max(0, min(128, p.MI - c.i0));
+}
+
+// grid = number of CTA descriptors; dynamic smem as for umma_gemm_kernel.  Warp roles: 0-3 TMA producers (warp 1 also
+// sets up the barriers) | warpgroup 1 (warps 4-7) D rows [0, 64), warpgroup 2 (warps 8-11) D rows [64, 128), all NJT
+// columns.  All twelve warps take part in the store phase.  A stage holds 32 reduction elements (128-byte K-major
+// rows), i.e. ksteps == 4.
+template <int NJT>
+__global__ void __launch_bounds__(kThreadsW, 1)
+    wgmma_gemm_kernel(const __grid_constant__ UmMaps maps, const UmCta* __restrict__ ctas, const UmProblem* __restrict__ probs,
+                      const UmTmaOp* __restrict__ ops, int nmaps, int stages, uint32_t stage_bytes, long long* __restrict__ trace) {
+  if (threadIdx.x < nmaps) prefetch_tensormap(&maps.m[threadIdx.x]);
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + smem_pad_1024(smem_raw);
+  const bool tr = trace != nullptr && blockIdx.x == 0;
+  const UmCta cta = ctas[blockIdx.x];
+  const int ST = stages;
+  const int nst = (int)cta.nstages;
+
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem);      // [ST] TMA landed
+  uint64_t* empty = full + 2 * kStagesMax;                  // [ST] consumer warps retired every MMA reading the stage
+  UmProblem* p_smem = reinterpret_cast<UmProblem*>(smem + 1024);
+  UmTmaOp* ops_smem = reinterpret_cast<UmTmaOp*>(smem + 2048);
+  uint8_t* stage_base = smem + kCtlBytes;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  {
+    const uint4* src = reinterpret_cast<const uint4*>(probs + cta.prob);
+    uint4* dst = reinterpret_cast<uint4*>(p_smem);
+    for (int i = threadIdx.x; i < (int)(sizeof(UmProblem) / 16); i += kThreadsW) dst[i] = src[i];
+    const int nvec = min(nst * (int)cta.ops_per_stage, kMaxOpsPerCta) * 2;
+    const uint4* osrc = reinterpret_cast<const uint4*>(ops + cta.op0);
+    uint4* odst = reinterpret_cast<uint4*>(ops_smem);
+    for (int i = threadIdx.x; i < nvec; i += kThreadsW) odst[i] = osrc[i];
+  }
+  if (warp == 1 && lane == 0) {
+    for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumerWarps); }
+    fence_mbarrier_init();
+  }
+  __syncthreads();
+  const UmProblem& p = *p_smem;
+  const uint32_t a_bytes = p.A.part_bytes * 2;
+  const bool direct = p.epi == UM_EPI_PARTIAL && p.sc_i == 1;
+  constexpr int NA = NJT / 2;   // accumulator floats per thread of an m64 x NJT tile
+  float sum[NA];
+
+  // consumer warpgroup 0 / 1 (D rows [64 wg, 64 wg + 64)); -1: producer warpgroup.  The values the MMA loop branches on
+  // are broadcast from lane 0 so that ptxas sees them warp-uniform.
+  const int wg = __shfl_sync(0xffffffffu, (warp >> 2) - 1, 0);
+  if (wg < 0) {
+    // TMA producers: the ops of a stage are spread over the producer warpgroup (op q -> warp q % nprod), as in umma_gemm_kernel.
+    const int nops = (int)cta.ops_per_stage;
+    const int nprod = min(nops, 4);
+    if (warp < nprod) {
+      const int pidx = warp;
+      int s = 0;
+      uint32_t ph = 0;
+      uint32_t st_addr = smem_u32(stage_base);
+      int oi = 0;
+      dz::pdl_enter();
+      if (tr && warp == 0 && lane == 0) { trace[323] = clock64(); trace[324] = clock64(); }
+      const int my_ops = (nops - pidx + nprod - 1) / nprod;
+      for (int it = 0; it < nst; ++it) {
+        mbar_wait(&empty[s], ph ^ 1u);
+        if (pidx == 0 && lane == 0) mbar_expect_tx(&full[s], cta.tx_bytes);
+        __syncwarp();
+        if (lane < my_ops) {
+          const int o = oi + pidx + lane * nprod;
+          const UmTmaOp op = o < kMaxOpsPerCta ? ops_smem[o] : ops[cta.op0 + o];
+          tma_load_5d(st_addr + op.smem_off, &maps.m[op.map], &full[s], op.c[0], op.c[1], op.c[2], op.c[3], op.c[4]);
         }
-        if (of) *reinterpret_cast<float4*>(of + o) = v;
-        if (oh) {
-          float4 h, l;
-          split_tf32(v, h, l);
-          *reinterpret_cast<float4*>(oh + o) = h;
-          *reinterpret_cast<float4*>(ol + o) = l;
-        }
+        if (tr && warp == 0 && lane == 0 && it < 64) trace[it] = clock64();                          // [0,64): TMA issued
+        __syncwarp();
+        oi += nops;
+        ++s; st_addr += stage_bytes;
+        if (s == ST) { s = 0; ph ^= 1u; st_addr = smem_u32(stage_base); }
       }
     } else {
-      float* __restrict__ C = p.C + (long long)cta.split * p.split_stride;
-      const float* __restrict__ scale_i = p.scale_i;
-      const long long sc_i = p.sc_i, sc_j = p.sc_j;
-      const bool vec = sc_j == 1 && (sc_i & 3) == 0 && ((reinterpret_cast<uintptr_t>(C) & 15) == 0);
+      dz::pdl_enter();                                      // idle producer warps: first access to global data is in the store phase
+    }
+  } else {
+    // ---------------------------------------------------------------- consumer warpgroups
+    // Every k-step is one wgmma group into a scratch accumulator, acc0 / acc1 alternating: while the tensor cores run
+    // k-step k + 1, k-step k is retired (wgmma_wait<1>) and added into `sum`.  A stage's four k-steps are straight-line
+    // code and its last group is retired before the stage is released to the producers, so no group is in flight
+    // across a branch or a loop edge (ptxas would serialise the MMAs); the other consumer warpgroup keeps the tensor
+    // cores busy across that drain.
+    const bool active = __shfl_sync(0xffffffffu, (int)(64 * wg < tile_rows_out(p, cta)), 0) != 0;
+    const bool lead = warp == 4 && lane == 0;
 #pragma unroll
-      for (int j = 0; j < kIters; ++j) {
-        const int idx = tid + j * 384;
-        if (idx >= items) continue;
-        const int r = (int)(((uint32_t)idx * inv_cpr) >> 16), c = idx - r * cpr;
-        const int i = cta.i0 + r;
+    for (int e = 0; e < NA; ++e) sum[e] = 0.f;
+    float acc0[NA], acc1[NA];
+#pragma unroll
+    for (int e = 0; e < NA; ++e) { acc0[e] = 0.f; acc1[e] = 0.f; }
+    const uint32_t a_lo_off = p.A.part_bytes, b_lo_off = p.B.part_bytes;
+    auto retire = [&](float (&d)[NA]) {
+      wgmma_fence_acc(d);
+#pragma unroll
+      for (int e = 0; e < NA; ++e) sum[e] += d[e];
+    };
+    int s = 0;
+    uint32_t ph = 0;
+    for (int it = 0; it < nst; ++it) {
+      mbar_wait(&full[s], ph);
+      stamp_if(trace + 64 + it, tr && lead && it < 64);                                         // [64,128): stage data ready
+      if (active) {
+        const uint32_t a = smem_u32(stage_base) + (uint32_t)s * stage_bytes + 8192u * (uint32_t)wg;
+        const uint32_t b = smem_u32(stage_base) + (uint32_t)s * stage_bytes + a_bytes;
+        wgmma_kstep_3xtf32(acc0, a, a + a_lo_off, b, b + b_lo_off, 0);
+        wgmma_kstep_3xtf32(acc1, a, a + a_lo_off, b, b + b_lo_off, 8);
+        wgmma_wait<1>();
+        retire(acc0);
+        wgmma_kstep_3xtf32(acc0, a, a + a_lo_off, b, b + b_lo_off, 16);
+        wgmma_wait<1>();
+        retire(acc1);
+        wgmma_kstep_3xtf32(acc1, a, a + a_lo_off, b, b + b_lo_off, 24);
+        wgmma_wait<1>();
+        retire(acc0);
+        wgmma_wait<0>();
+        mbar_arrive_if(&empty[s], lane == 0);
+        retire(acc1);
+      } else {
+        mbar_arrive_if(&empty[s], lane == 0);
+      }
+      stamp_if(trace + 128 + it, tr && lead && it < 64);                                        // [128,192): stage consumed
+      if (++s == ST) { s = 0; ph ^= 1u; }
+    }
+    if (lead) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // the next kernel's set-up overlaps our epilogue
+    dz::pdl_enter();
+    if (tr && lead) trace[320] = clock64();                                                         // store phase starts
+    const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), c0 = 2 * (lane & 3);
+    if (direct) {
+      float* dst = p.C + (long long)cta.split * p.split_stride;
+      const long long sc_j = p.sc_j;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int i = cta.i0 + r0 + 8 * h;
         if (i >= p.MI) continue;
-        float4 v = *stage_chunk<NJT>(stage_base, r, c);
-        if (scale_i) { const float s = scale_i[i]; v.x *= s; v.y *= s; v.z *= s; v.w *= s; }
-        float* dst = C + (long long)i * sc_i + (long long)(4 * c) * sc_j;
-        if (vec) *reinterpret_cast<float4*>(dst) = v;
-        else { dst[0] = v.x; dst[sc_j] = v.y; dst[2 * sc_j] = v.z; dst[3 * sc_j] = v.w; }
+        const float sc = p.scale_i ? p.scale_i[i] : 1.0f;
+#pragma unroll
+        for (int nt = 0; nt < NJT / 8; ++nt)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int j = 8 * nt + c0 + e;
+            if (j < p.NJ) dst[i + (long long)j * sc_j] = sum[4 * nt + 2 * h + e] * sc;
+          }
       }
     }
   }
-  if (tr && warp == 2 && lane == 0) trace[321] = clock64();                                         // stores issued
+  if (!direct) {
+    // ---------------------------------------------------------------- cooperative store phase (all 384 threads)
+    // every consumer warp has retired its last MMA (and with it every TMA write has landed): the stage buffers become the staging tile
+    __syncthreads();
+    if (wg >= 0) {
+      const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+      for (int nt = 0; nt < NJT / 8; ++nt)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = r0 + 8 * h, c = 8 * nt + c0;
+          *reinterpret_cast<float2*>(reinterpret_cast<float*>(stage_chunk<NJT>(stage_base, r, c >> 2)) + (c & 3)) =
+              make_float2(sum[4 * nt + 2 * h], sum[4 * nt + 2 * h + 1]);
+        }
+    }
+    __syncthreads();
+    store_tile<NJT>(p, cta, stage_base, threadIdx.x);
+  }
+  if (tr && warp == 4 && lane == 0) trace[321] = clock64();                                         // stores issued
   if (tr && threadIdx.x == 0) trace[322] = clock64();
 }
 

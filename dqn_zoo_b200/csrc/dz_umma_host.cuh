@@ -7,7 +7,10 @@
 
 namespace dz {
 
-// One launch of umma_gemm_kernel: a contiguous range of CTA descriptors sharing NJT / stage geometry.
+// MMA path of a launch: the warp-level mma.sync kernel (every operand layout) or the wgmma kernel (K-major, pre-split).
+enum : int { UM_PATH_AUTO = 0, UM_PATH_MMA_SYNC = 1, UM_PATH_WGMMA = 2 };
+
+// One launch of umma_gemm_kernel / wgmma_gemm_kernel: a contiguous range of CTA descriptors sharing NJT / stage geometry.
 struct UmLaunch {
   int cta0 = 0, nctas = 0;
   int njt = 64;
@@ -35,7 +38,12 @@ struct UmPlan {
   int localize_maps(UmLaunch& l);
   int upload();          // (re)allocates and copies all four tables
   void release();
-  int launch(const char* tag, const UmLaunch& l, void* stream, long long* d_trace = nullptr) const;   // d_trace: 512 clock stamps of CTA 0 (debug)
+  // d_trace: 512 clock stamps of CTA 0 (debug).  path: UM_PATH_AUTO picks wgmma_gemm_kernel when wgmma_eligible(l), else
+  // umma_gemm_kernel; UM_PATH_MMA_SYNC / UM_PATH_WGMMA force one (forcing wgmma on a launch that is not eligible fails).
+  int launch(const char* tag, const UmLaunch& l, void* stream, long long* d_trace = nullptr, int path = UM_PATH_AUTO) const;
+  // Every CTA of the launch has both operands K-major tf32 hi/lo pairs that need no conversion, four k-steps per stage.
+  bool wgmma_eligible(const UmLaunch& l) const;
+  int path_of(const UmLaunch& l) const { return wgmma_eligible(l) ? UM_PATH_WGMMA : UM_PATH_MMA_SYNC; }
   static int configure();   // one-time kernel attributes (outside any stream capture)
 };
 

@@ -1252,6 +1252,16 @@ int um_net_create(const UmNetDesc& d, char* base, UmNet** out) {
 
 void um_net_trace(UmNet* n, const char* tag, long long* d_trace) { n->trace_tag = tag ? tag : ""; n->trace_ptr = d_trace; }
 
+int um_net_mma_path(UmNet* n, const char* tag) {
+  const std::string t = tag ? tag : "";
+  const UmLaunch* l = t == "conv2_fwd" ? &n->l_conv2 : t == "conv3_fwd" ? &n->l_conv3 : t == "conv3_dgrad" ? &n->l_dconv3
+                    : t == "conv2_dgrad" ? &n->l_dconv2 : (t == "fc1_fwd" || t == "noisy1_fwd") ? &n->l_fc
+                    : (t == "fc1_dgrad" || t == "noisy1_dgrad") ? &n->l_fcd : t == "conv3_wgrad" ? &n->l_wconv3
+                    : t == "conv2_wgrad" ? &n->l_wconv2 : nullptr;
+  if (!l || l->nctas <= 0) return -1;
+  return n->plan.path_of(*l);
+}
+
 void um_net_destroy(UmNet* n) {
   if (!n) return;
   n->plan.release();

@@ -31,6 +31,7 @@ int64_t um_net_workspace_bytes(const UmNetDesc& d);
 int um_net_create(const UmNetDesc& d, char* base, UmNet** out);
 void um_net_destroy(UmNet* n);
 void um_net_trace(UmNet* n, const char* tag, long long* d_trace);   // debug: clock stamps of CTA 0 of the launch `tag`
+int um_net_mma_path(UmNet* n, const char* tag);   // UM_PATH_MMA_SYNC / UM_PATH_WGMMA of the launch `tag`; -1: no such launch
 
 // Buffers the rest of the learner reads / writes (fp32 views of the activations and gradients).
 float* um_act_f32(UmNet* n, int layer, int pass);      // layer 1..3 -> [B][h][w][C] (layers 1, 2: the tf32 hi image)

@@ -348,6 +348,8 @@ int dz_test_learner_buffer(dz_learner* l, const char* name, float** d_ptr, int64
 int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream);   /* device-to-device, tests only */
 /* Debug: the tensor-core launch named `tag` writes the clock stamps of its CTA 0 into d_trace (512 int64). */
 int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace);
+/* Tests: which MMA path the tensor-core launch `tag` (same tags) takes: *path = 1 warp-level mma.sync, 2 wgmma. */
+int dz_test_learner_mma_path(dz_learner* l, const char* tag, int32_t* path);
 /* Debug: every kernel appends (globaltimer ns, gridDim.x << 32 | gridDim.y << 16 | blockDim.x) to d_buf right after its
  * dependencies completed; d_buf[0] (low 32 bits) counts the entries, entries start at d_buf[2].  d_buf: 2 + 2 * 4000
  * uint64, zeroed by the caller; nullptr switches the stamps off.  Works under CUDA-graph replay (tools/step_timeline.py). */
@@ -366,6 +368,11 @@ int dz_test_tc_pgemm(const float* d_A, int32_t a_rows, int32_t a_ld, int32_t a_r
 int dz_test_umma_gemm(const float* d_A, int32_t a_mn_major, const float* d_B, int32_t b_mn_major, int32_t MI, int32_t NJ,
                       int32_t R, int32_t convert, const float* d_scale_r, int32_t stages, int32_t epi_rows,
                       const float* d_bias, int32_t relu, float* d_C, float* d_hi, float* d_lo, void* stream);
+/* The same with the MMA kernel chosen by `path`: 0 automatic (as the learner's launches: wgmma when both operands are
+ * K-major and pre-split), 1 warp-level mma.sync kernel, 2 wgmma kernel (fails for MN-major or converted operands). */
+int dz_test_umma_gemm_path(const float* d_A, int32_t a_mn_major, const float* d_B, int32_t b_mn_major, int32_t MI, int32_t NJ,
+                           int32_t R, int32_t convert, const float* d_scale_r, int32_t stages, int32_t epi_rows,
+                           const float* d_bias, int32_t relu, float* d_C, float* d_hi, float* d_lo, int32_t path, void* stream);
 
 #ifdef __cplusplus
 }
