@@ -298,6 +298,8 @@ class _DeviceAgent(parts.Agent):
     """Raises if a kernel set a sticky error flag (bad priority, root == 0 in the fused path...)."""
     flags = self._replay._distribution._sum_tree._flags if self.PRIORITIZED else self._replay._store.flags
     f = int(flags.item())
+    if f & _lib.DZ_FLAG_FRAME_POOL_FULL:       # sticky: the frame pool stored zeros for planes it had no room for
+      replay_lib._raise_if_pool_full(self._replay._store, flags)
     if f:
       flags.zero_()
       if f & (_lib.DZ_FLAG_BAD_VALUE | _lib.DZ_FLAG_BAD_INDEX):

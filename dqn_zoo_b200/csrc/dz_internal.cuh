@@ -15,12 +15,44 @@ struct BatchExtras {
   float* d_disc;
   float* d_w;
   int fused;
+  // frame-deduplicated replay: the row tables point at [B][2][obs_stride] here, filled by launch_frame_reconstruct
+  const uint8_t* recon;
 };
 
 int launch_sample(const dz_replay_view* view, int prioritized, const dz_sample_inputs* in, const dz_sample_outputs* out,
                   int batch, const BatchExtras& ex, void* stream);
 int launch_update_priorities(const dz_replay_view* view, const int64_t* d_indices, const float* d_priorities, int n,
                              double alpha, int64_t size, void* stream);
+
+// splitmix64 finaliser: the counter hash of the synthetic fills (oracle/replay_oracle.py:_mix64) and the frame hash
+__device__ __forceinline__ uint64_t mix64(uint64_t x) {
+  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+  return x ^ (x >> 31);
+}
+
+// ---- frame-deduplicated replay layout (dz_frames.cu) ----------------------------------------------------------------
+constexpr int kMaxObsChannels = 32;
+// One add: resolves the 2*C planes of (src_tm1, src_t) (device pointers, HWC) into row `slot` (see dz_replay_add).
+int launch_frame_add(const dz_replay_view* view, int64_t slot, int release_row, const uint8_t* src_tm1,
+                     const uint8_t* src_t, void* stream);
+// HWC stacks of rows slots[0..batch): s_tm1 of b at dst_tm1 + b * pitch, s_t at dst_t + b * pitch.
+int launch_frame_reconstruct(const dz_replay_view* view, const int64_t* d_slots, int batch, uint8_t* dst_tm1,
+                             uint8_t* dst_t, int64_t pitch, void* stream);
+int launch_frame_pool_reset(const dz_replay_view* view, void* stream);
+int launch_frame_fill_stacked(const dz_replay_view* view, int64_t n, uint64_t seed, int64_t episode_len, void* stream);
+
+// Word w of frame f of synthetic episode e (dz_replay_fill_synthetic_stacked); words = H*W/8.
+__device__ __forceinline__ uint64_t stacked_frame_word(uint64_t seed, int64_t e, int64_t f, int64_t episode_len,
+                                                       int64_t words, int64_t w) {
+  return mix64(seed * 0x9E3779B97F4A7C15ull + 0x632BE59BD9B4E019ull +
+               (uint64_t)(e * (episode_len + 1) + f) * (uint64_t)words + (uint64_t)w);
+}
+// Frame held by channel c of the stack after frames 0..step (trailing-zero padded while step + 1 < C); -1 = zeros.
+__device__ __forceinline__ int64_t stacked_channel_frame(int64_t step, int c, int C) {
+  if (step + 1 < C) return c <= step ? c : -1;
+  return step - (C - 1) + c;
+}
 
 
 // ---- packed-operand tensor-core GEMM (dz_tcp.cuh / dz_tcp.cu) ------------------------------------------------------

@@ -1202,6 +1202,8 @@ struct dz_learner {
   float *loss_terms, *scalars;              // scalars: [0]=norm, [1]=shared-bias scratch.., [8..]=norm partials
   unsigned int* ticket;
   const uint8_t** rows_sample[2];           // row tables filled by the fused sampler
+  uint8_t* recon = nullptr;                 // frame-deduplicated replay: [B][2][obs_stride] stacks the sampled rows
+  int64_t recon_bytes = 0;                  //   are rebuilt into (allocated by the first, eager, dz_learner_learn)
   const uint8_t** rows_act;                 // 1-entry table for q_values
   int32_t* s_a; float *s_r, *s_d, *s_w;     // sampler-produced batch scalars
   float* q_scratch;
@@ -2426,6 +2428,7 @@ void dz_learner_destroy(dz_learner* l) {
   um_net_destroy(l->um);
   l->side.destroy();
   l->side2.destroy();
+  if (l->recon) cudaFree(l->recon);
   delete l;
 }
 
@@ -2437,6 +2440,21 @@ int dz_learner_learn(dz_learner* l, const dz_replay_view* replay, int32_t priori
   const int B = l->B;
   BatchExtras ex{l->rows_sample[0], l->rows_sample[1], l->s_a, l->s_r, l->s_d, prioritized ? l->s_w : nullptr, 1};
   if (replay->obs_bytes != (int64_t)l->d.H * l->d.W * l->d.C) return fail(DZ_EINVAL, "replay observation size does not match the network");
+  if (replay->d_planes) {
+    const int64_t need = (int64_t)B * 2 * replay->obs_stride;
+    if (need > l->recon_bytes) {
+      cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+      DZ_CUDA_OK(cudaStreamIsCapturing((cudaStream_t)stream, &cs));
+      if (cs != cudaStreamCaptureStatusNone)
+        return fail(DZ_EINVAL, "the first dz_learner_learn on a frame-deduplicated replay must run eagerly, not in a capture");
+      if (l->recon) DZ_CUDA_OK(cudaFree(l->recon));
+      l->recon = nullptr;
+      l->recon_bytes = 0;
+      DZ_CUDA_OK(cudaMalloc(&l->recon, need));
+      l->recon_bytes = need;
+    }
+    ex.recon = l->recon;
+  }
   // conv weight images do not depend on the sampled batch: pack them on the side stream while the sampler runs
   const bool pack_aside = l->um != nullptr;
   if (pack_aside) {
@@ -2444,6 +2462,9 @@ int dz_learner_learn(dz_learner* l, const dz_replay_view* replay, int32_t priori
     DZ_TRY(um_pack_weights(l->um, ws));
   }
   DZ_TRY(launch_sample(replay, prioritized, &io->sample_in, &io->sample_out, B, ex, stream));
+  if (replay->d_planes)
+    DZ_TRY(launch_frame_reconstruct(replay, io->sample_out.d_slots, B, l->recon, l->recon + replay->obs_stride,
+                                    2 * replay->obs_stride, stream));
   dz_batch batch;
   batch.d_s_tm1_rows = l->rows_sample[0];
   batch.d_s_t_rows = l->rows_sample[1];

@@ -291,7 +291,8 @@ __device__ __forceinline__ double is_weight_pow(double x, double beta) {
 }
 
 __device__ void emit_batch_rows(const dz_replay_view& v, const BatchExtras& ex, int b, int64_t slot, double weight) {
-  const uint8_t* row = v.d_obs + slot * 2 * v.obs_stride;
+  // frame-deduplicated replay: the learner reads the stacks launch_frame_reconstruct rebuilds for batch entry b
+  const uint8_t* row = v.d_planes ? ex.recon + (int64_t)b * 2 * v.obs_stride : v.d_obs + slot * 2 * v.obs_stride;
   if (ex.d_s_tm1_rows) ex.d_s_tm1_rows[b] = row;
   if (ex.d_s_t_rows) ex.d_s_t_rows[b] = row + v.obs_stride;
   if (ex.d_a) ex.d_a[b] = v.d_action[slot];
@@ -456,12 +457,6 @@ __global__ void __launch_bounds__(64) apply_add_kernel(dz_replay_view v, dz_add_
   if (rec.tree_index >= 0 && v.d_tree) block_tree_set(v.d_tree, v.first_leaf, s_idx, s_val, 2);
 }
 
-__device__ __forceinline__ uint64_t mix64(uint64_t x) {
-  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-  return x ^ (x >> 31);
-}
-
 __global__ void __launch_bounds__(256) fill_obs_kernel(dz_replay_view v, int64_t row0, int64_t n, uint64_t seed) {
   dz::pdl_enter();
   const int64_t words = v.obs_bytes >> 3;
@@ -490,6 +485,33 @@ __global__ void fill_scalars_kernel(dz_replay_view v, int64_t row0, int64_t n, u
   v.d_reward[row] = u < 0.05 ? -1.0 : (u < 0.95 ? 0.0 : 1.0);
   double u3 = (double)(mix64(base + 2) >> 11) * (1.0 / 9007199254740992.0);
   v.d_discount[row] = u3 < 0.99 ? discount : 0.0;
+}
+
+// Transition-major frame stacks (dz_replay_fill_synthetic_stacked): one thread per 8 pixels of one observation; it
+// interleaves the C channel words into 8*C bytes of the HWC row.
+__global__ void __launch_bounds__(256) fill_stacked_obs_kernel(dz_replay_view v, int64_t n, uint64_t seed,
+                                                               int64_t episode_len, int C) {
+  dz::pdl_enter();
+  const int64_t words = v.obs_bytes / C / 8;
+  const int64_t total = n * 2 * words;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t w = i % words, ro = i / words, row = ro >> 1, o = ro & 1;
+    const int64_t e = row / episode_len, step = row % episode_len + o;
+    uint64_t fw[kMaxObsChannels];
+    for (int c = 0; c < C; ++c) {
+      const int64_t f = stacked_channel_frame(step, c, C);
+      fw[c] = f < 0 ? 0ull : stacked_frame_word(seed, e, f, episode_len, words, w);
+    }
+    uint64_t* dst = reinterpret_cast<uint64_t*>(v.d_obs + (row * 2 + o) * v.obs_stride + w * 8 * C);
+    for (int k = 0; k < C; ++k) {   // output word k holds bytes 8k .. 8k+7 of the 8*C interleaved bytes
+      uint64_t out = 0;
+      for (int j = 0; j < 8; ++j) {
+        const int b = 8 * k + j;
+        out |= ((fw[b % C] >> (8 * (b / C))) & 0xffull) << (8 * j);
+      }
+      dst[k] = out;
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -628,6 +650,21 @@ int dz_replay_add(const dz_replay_view* view, const dz_add_record* rec, const ui
                   void* stream) {
   if (rec->slot < 0 || rec->slot >= view->capacity) return fail(DZ_ERANGE, "slot out of range");
   if (rec->n_patches < 0 || rec->n_patches > 4) return fail(DZ_EINVAL, "at most 4 patches");
+  if (view->d_planes) {
+    if (!h_s_tm1 || !h_s_t) return fail(DZ_EINVAL, "frame-deduplicated add needs both observations");
+    const uint8_t* src[2] = {h_s_tm1, h_s_t};
+    for (int o = 0; o < 2; ++o) {
+      cudaPointerAttributes attr;
+      if (cudaPointerGetAttributes(&attr, src[o]) != cudaSuccess) cudaGetLastError();
+      else if (attr.type == cudaMemoryTypeDevice) continue;   // device source: the add kernel reads it in place
+      uint8_t* stage = view->d_add_staging + o * view->obs_stride;
+      DZ_CUDA_OK(cudaMemcpyAsync(stage, src[o], view->obs_bytes, cudaMemcpyDefault, (cudaStream_t)stream));
+      src[o] = stage;
+    }
+    DZ_TRY(launch_frame_add(view, rec->slot, rec->release_row, src[0], src[1], stream));
+    DZ_LAUNCH(apply_add_kernel, 1, 64, 0, stream, *view, *rec);
+    return DZ_OK;
+  }
   uint8_t* row = view->d_obs + rec->slot * 2 * view->obs_stride;
   // cudaMemcpyDefault: the sources may be host arrays (the reference's add path) or device buffers (frame stacks kept
   // in HBM by the device preprocessing) — the driver infers the direction from the unified address space
@@ -640,6 +677,7 @@ int dz_replay_add(const dz_replay_view* view, const dz_add_record* rec, const ui
 
 int dz_replay_fill_synthetic(const dz_replay_view* view, int64_t row0, int64_t n, uint64_t seed, int32_t num_actions,
                              double discount, void* stream) {
+  if (view->d_planes) return fail(DZ_EINVAL, "iid synthetic rows share no frames: use dz_replay_fill_synthetic_stacked");
   if (view->obs_bytes % 8) return fail(DZ_EINVAL, "obs_bytes must be a multiple of 8 for synthetic fill");
   if (row0 < 0 || row0 + n > view->capacity) return fail(DZ_ERANGE, "rows out of range");
   if (n == 0) return DZ_OK;
@@ -647,6 +685,40 @@ int dz_replay_fill_synthetic(const dz_replay_view* view, int64_t row0, int64_t n
   int grid = (int)(ceil_div(total, 256) < kNumSMs * 32 ? ceil_div(total, 256) : kNumSMs * 32);
   DZ_LAUNCH(fill_obs_kernel, grid, 256, 0, stream, *view, row0, n, seed);
   DZ_LAUNCH(fill_scalars_kernel, (int)ceil_div(n, 256), 256, 0, stream, *view, row0, n, seed, num_actions, discount);
+  return DZ_OK;
+}
+
+int dz_replay_fill_synthetic_stacked(const dz_replay_view* view, int64_t n, uint64_t seed, int64_t episode_len,
+                                     int32_t num_actions, double discount, void* stream) {
+  if (n < 0 || n > view->capacity) return fail(DZ_ERANGE, "rows out of range");
+  if (episode_len < 1) return fail(DZ_EINVAL, "episode_len must be positive");
+  if (num_actions < 1) return fail(DZ_EINVAL, "num_actions must be positive");
+  if (n == 0) return DZ_OK;
+  if (view->d_planes) {
+    DZ_TRY(launch_frame_fill_stacked(view, n, seed, episode_len, stream));
+  } else {
+    const int C = (int)view->obs_channels;
+    if (C < 1 || C > kMaxObsChannels || view->obs_bytes % C || (view->obs_bytes / C) % 8)
+      return fail(DZ_EINVAL, "stacked fill needs obs_channels in [1,32] and H*W a multiple of 8");
+    const int64_t total = n * 2 * (view->obs_bytes / C / 8);
+    const int grid = (int)(ceil_div(total, 256) < kNumSMs * 32 ? ceil_div(total, 256) : kNumSMs * 32);
+    DZ_LAUNCH(fill_stacked_obs_kernel, grid, 256, 0, stream, *view, n, seed, episode_len, C);
+  }
+  DZ_LAUNCH(fill_scalars_kernel, (int)ceil_div(n, 256), 256, 0, stream, *view, (int64_t)0, n, seed, num_actions, discount);
+  return DZ_OK;
+}
+
+int dz_replay_frame_pool_reset(const dz_replay_view* view, void* stream) {
+  if (!view->d_planes) return fail(DZ_EINVAL, "not a frame-deduplicated replay");
+  return launch_frame_pool_reset(view, stream);
+}
+
+int dz_replay_frames_in_use(const dz_replay_view* view, int64_t* h_frames_in_use, void* stream) {
+  if (!view->d_planes) return fail(DZ_EINVAL, "not a frame-deduplicated replay");
+  int64_t top = 0;
+  DZ_CUDA_OK(cudaMemcpyAsync(&top, view->d_pool_counters, sizeof(top), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  DZ_CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream));
+  *h_frames_in_use = view->frame_capacity - top;
   return DZ_OK;
 }
 
@@ -659,6 +731,11 @@ int dz_replay_sample(const dz_replay_view* view, int32_t prioritized, const dz_s
 int dz_replay_gather(const dz_replay_view* view, const int64_t* d_slots, int32_t batch, uint8_t* d_s_tm1, uint8_t* d_s_t,
                      int64_t* d_a, double* d_r, double* d_disc, void* stream) {
   if (batch <= 0) return DZ_OK;
+  if (view->d_planes) {
+    DZ_TRY(launch_frame_reconstruct(view, d_slots, batch, d_s_tm1, d_s_t, view->obs_bytes, stream));
+    DZ_LAUNCH(gather_scalars_kernel, (int)ceil_div(batch, 128), 128, 0, stream, *view, d_slots, batch, d_a, d_r, d_disc);
+    return DZ_OK;
+  }
   int vec16 = (view->obs_bytes % 16 == 0) && ((uintptr_t)d_s_tm1 % 16 == 0) && ((uintptr_t)d_s_t % 16 == 0);
   int64_t work = vec16 ? view->obs_bytes >> 4 : view->obs_bytes;
   int gx = (int)(ceil_div(work, 256) < 8 ? ceil_div(work, 256) : 8);

@@ -8,7 +8,8 @@ generators.  What else differs is where things live:
 
   * transition storage (`OrderedDict` in the reference, `replay.py:140,688`) is a
     transition-major uint8 array in device memory: row = id % capacity holds
-    s_tm1 | s_t back to back (DESIGN.md §3);
+    s_tm1 | s_t back to back (DESIGN.md §3); or, with `frame_dedup=True`, a frame pool
+    that keeps each distinct H*W plane of the stored frame stacks once (`_FramePoolStore`);
   * the float64 sum tree (`replay.py:246-426`) is a device array traversed by a
     warp-cooperative CUDA kernel (csrc/dz_replay.cu);
   * O(1) integer bookkeeping per add (free-slot stack, swap-remove lists,
@@ -271,9 +272,11 @@ class _DeviceList:
 
 
 def _apply_index_record(view, patches, tree_index=-1, leaf_value=0.0, evict_index=-1, size_after=0, slot=0,
-                        action=0, reward=0.0, discount=0.0, h_s_tm1=None, h_s_t=None, d_priority=None, alpha=1.0):
+                        action=0, reward=0.0, discount=0.0, h_s_tm1=None, h_s_t=None, d_priority=None, alpha=1.0,
+                        release_row=False):
   """One dz_replay_add call: <=4 list patches + optional evict/set on the tree (+ optional row write)."""
   rec = _lib.AddRecord()
+  rec.release_row = 1 if release_row else 0
   rec.slot, rec.action, rec.reward, rec.discount = slot, action, reward, discount
   rec.n_patches = len(patches)
   for k, (target, pos, val) in enumerate(patches):
@@ -732,10 +735,137 @@ class _TransitionStore:
       out.extend(type(structure)(*[f[k] for f in tr]) for k in range(len(part)))
     return out
 
+  def storage_bytes(self):
+    """Device bytes this store holds (observations and per-row scalars)."""
+    ts = [t for t in (self.obs, self.action, self.reward, self.discount, self.flags) if t is not None]
+    return sum(t.numel() * t.element_size() for t in ts)
+
   def to_host_transition(self, structure, tensors):
     s_tm1, a, r, d, s_t = [t.cpu().numpy() for t in tensors]
     shape = (len(a),) + self.obs_shape
     return type(structure)(s_tm1.view(self.obs_dtype).reshape(shape), a, r, d, s_t.view(self.obs_dtype).reshape(shape))
+
+
+# Default pool size is 2 * capacity + FRAME_POOL_SLACK planes.  For stacks built as `processors.atari()` builds them
+# (trailing-zero padded, one new frame per step), the live planes of one actor stream are at most
+# transitions + episodes + (stack - 1), and an episode holds at least one transition: 2 * capacity covers the
+# transitions and episodes of every stream together, and the slack covers plane 0 plus the (stack - 1) planes of the
+# oldest, partly evicted episode of up to 21 interleaved 4-deep streams (and the at most one new frame an add brings in
+# before the evicted row releases its planes).
+FRAME_POOL_SLACK = 64
+_POOL_FULL = ('frame pool is full: an add found no free plane and stored zeros instead (frame_capacity=%d is too '
+              'small for these observations; construct the replay with a larger frame_capacity)')
+
+
+class _FramePoolStore(_TransitionStore):
+  """Frame-deduplicated layout (DESIGN.md §3): an observation [H, W, C] uint8 is C planes of H*W bytes; every
+  distinct plane is stored once in a device pool of `frame_capacity` planes and row = id % capacity keeps the 2*C
+  plane ids of s_tm1 | s_t.  Content-addressed inserts and the reconstruction of HWC stacks run in CUDA
+  (csrc/dz_frames.cu); `gather`, `get_rows` and `to_host_transition` return exactly the transition-major bytes."""
+
+  def __init__(self, capacity, frame_capacity=None):
+    super().__init__(capacity)
+    if frame_capacity is not None and not 1 <= int(frame_capacity) < 2 ** 31:
+      raise ValueError('frame_capacity must be in [1, 2**31)')
+    self._requested = None if frame_capacity is None else int(frame_capacity)
+    self.frames = None
+    self.frame_capacity = 0
+
+  def allocate(self, obs_shape, obs_dtype=np.uint8):
+    if self.frames is not None:
+      return
+    shape, dtype = tuple(obs_shape), np.dtype(obs_dtype)
+    if len(shape) != 3 or dtype != np.uint8:
+      raise ValueError('frame_dedup stores 3-D uint8 observations [H, W, C]; got shape %s dtype %s' % (shape, dtype))
+    h, w, c = shape
+    if not 1 <= c <= 32:
+      raise ValueError('frame_dedup supports 1..32 channels, got %d' % c)
+    self.obs_shape, self.obs_dtype = shape, dtype
+    self.obs_bytes = h * w * c
+    self.obs_stride = (self.obs_bytes + 15) // 16 * 16
+    self.channels = c
+    self.frame_bytes = h * w
+    self.frame_stride = (self.frame_bytes + 15) // 16 * 16
+    fc = self._requested if self._requested is not None else 2 * self.capacity + FRAME_POOL_SLACK
+    self.frame_capacity = fc
+    self.table_size = 1 << max(1, (2 * fc - 1).bit_length())
+    dev = self.action.device
+    n = max(self.capacity, 1)
+    self.frames = torch.empty((fc, self.frame_stride), dtype=torch.uint8, device=dev)
+    self.planes = torch.zeros((n, 2 * c), dtype=torch.int32, device=dev)
+    self.refcount = torch.zeros(fc, dtype=torch.int32, device=dev)
+    self.hashes = torch.zeros(fc, dtype=torch.int64, device=dev)
+    self.table = torch.empty(self.table_size, dtype=torch.int32, device=dev)
+    self.free = torch.empty(fc, dtype=torch.int32, device=dev)
+    self.counters = torch.zeros(1, dtype=torch.int64, device=dev)
+    self.staging = torch.zeros(2 * self.obs_stride + 2 * c * self.frame_stride, dtype=torch.uint8, device=dev)
+    self.reset()
+
+  def fill_view(self, v):
+    v.d_action, v.d_reward, v.d_discount = _ptr(self.action), _ptr(self.reward), _ptr(self.discount)
+    v.capacity, v.obs_bytes, v.obs_stride = self.capacity, self.obs_bytes, self.obs_stride
+    v.d_flags = _ptr(self.flags)
+    if self.frames is not None:
+      v.d_frames, v.frame_bytes, v.frame_stride = _ptr(self.frames), self.frame_bytes, self.frame_stride
+      v.obs_channels, v.frame_capacity = self.channels, self.frame_capacity
+      v.d_planes, v.d_refcount, v.d_hashes = _ptr(self.planes), _ptr(self.refcount), _ptr(self.hashes)
+      v.d_table, v.table_size, v.d_free = _ptr(self.table), self.table_size, _ptr(self.free)
+      v.d_pool_counters, v.d_add_staging = _ptr(self.counters), _ptr(self.staging)
+    return v
+
+  def reset(self):
+    """Empties the pool: no row references a plane, the next fresh planes are 1, 2, 3, ..."""
+    if self.frames is not None:
+      _lib.call('dz_replay_frame_pool_reset', C.byref(self.fill_view(_lib.ReplayView())), _stream())
+
+  def frames_in_use(self):
+    """Live planes, plane 0 included (synchronises)."""
+    if self.frames is None:
+      return 0
+    out = C.c_int64()
+    _lib.call('dz_replay_frames_in_use', C.byref(self.fill_view(_lib.ReplayView())), C.byref(out), _stream())
+    return out.value
+
+  def storage_bytes(self):
+    n = super().storage_bytes()
+    if self.frames is not None:
+      n += sum(t.numel() * t.element_size() for t in (self.frames, self.planes, self.refcount, self.hashes, self.table,
+                                                      self.free, self.counters, self.staging))
+    return n
+
+  def check_pool(self, slots):
+    """Each refcount equals its references from the live rows `slots` (+1 for plane 0), and the free stack and the
+    live planes partition the pool."""
+    if self.frames is None:
+      return True, ''
+    fc = self.frame_capacity
+    planes = self.planes[torch.as_tensor(np.asarray(slots, dtype=np.int64), device=self.planes.device)].cpu().numpy()
+    want = np.bincount(planes.reshape(-1), minlength=fc)
+    want[0] += 1
+    ref = self.refcount.cpu().numpy()
+    bad = np.nonzero(ref != want)[0]
+    if bad.size:
+      return False, 'refcount of plane %d is %d, rows reference it %d times.' % (bad[0], ref[bad[0]], want[bad[0]])
+    top = int(self.counters.item())
+    free = self.free[:top].cpu().numpy()
+    live = np.nonzero(ref)[0]
+    if len(free) + len(live) != fc or len(np.union1d(free, live)) != fc:
+      return False, 'free stack and live planes do not partition the frame pool.'
+    return True, ''
+
+
+def _raise_if_pool_full(store, flags):
+  """DZ_FLAG_FRAME_POOL_FULL is sticky: the stored bytes are wrong from that add on, so every sync point raises."""
+  if isinstance(store, _FramePoolStore) and int(flags.item()) & _lib.DZ_FLAG_FRAME_POOL_FULL:
+    raise RuntimeError(_POOL_FULL % store.frame_capacity)
+
+
+def _make_store(capacity, frame_dedup, frame_capacity):
+  if frame_dedup:
+    return _FramePoolStore(capacity, frame_capacity)
+  if frame_capacity is not None:
+    raise ValueError('frame_capacity needs frame_dedup=True')
+  return _TransitionStore(capacity)
 
 
 def _host_obs(x, store):
@@ -774,16 +904,25 @@ def _check_codec(encoder, decoder):
 
 
 class TransitionReplay:
-  """Uniform replay with oldest-out eviction (`replay.py:120-200`), storage in HBM."""
+  """Uniform replay with oldest-out eviction (`replay.py:120-200`), storage in HBM.
 
-  def __init__(self, capacity: int, structure, random_state: np.random.RandomState, encoder=None, decoder=None):
+  `frame_dedup=True` stores each distinct H*W plane of the (3-D uint8) observations once (`_FramePoolStore`,
+  DESIGN.md §3): a reference-sized replay of 84x84x4 frame stacks then takes about a quarter of the HBM.  Everything
+  read back (samples, `get`, `get_state`, learner batches) is byte-identical to the default transition-major layout.
+  `frame_capacity` sizes the pool in planes (default 2 * capacity + FRAME_POOL_SLACK, enough for frame stacks built as
+  `processors.atari()` builds them); running out is a data error, raised as RuntimeError at the next sync point.  The
+  layout is the caller's choice because the replay cannot tell at construction whether its observations are frame
+  stacks, and the pool has to be sized up front."""
+
+  def __init__(self, capacity: int, structure, random_state: np.random.RandomState, encoder=None, decoder=None,
+               frame_dedup: bool = False, frame_capacity: Optional[int] = None):
     self._codec = _check_codec(encoder, decoder)
     self._capacity = capacity
     self._structure = structure
     self._random_state = random_state
     self._distribution = UniformDistribution(random_state=random_state)
     self._distribution._mirror.ensure(capacity)   # fixed address: captured CUDA graphs keep pointing at it
-    self._store = _TransitionStore(capacity)
+    self._store = _make_store(capacity, frame_dedup, frame_capacity)
     self._live_ids = collections.deque()   # ids currently stored, oldest first (keys of the OrderedDict)
     self._t = 0
 
@@ -792,13 +931,18 @@ class TransitionReplay:
     v.d_ids = _ptr(self._distribution.device_ids)
     return v
 
+  def _flags(self):
+    """The sticky device flags the kernels of this replay's view set."""
+    return self._store.flags
+
   def add(self, item) -> None:
     """`replay.py:142-151`."""
     if self._codec is not None:
       item = self._codec(item)
     s_tm1 = _host_obs(item[0], self._store)
     s_t = _host_obs(item[4], self._store)
-    if self.size == self._capacity:
+    full = self.size == self._capacity
+    if full:
       self._distribution.remove([self._live_ids.popleft()])
     item_id = self._t
     self._distribution.add([item_id])
@@ -806,7 +950,7 @@ class TransitionReplay:
     v = self.device_view()
     first = patches[:4]
     _apply_index_record(v, first, slot=item_id % self._capacity, action=int(item[1]), reward=float(item[2]),
-                        discount=float(item[3]), h_s_tm1=s_tm1, h_s_t=s_t)
+                        discount=float(item[3]), h_s_tm1=s_tm1, h_s_t=s_t, release_row=full)
     assert len(patches) <= 4
     self._live_ids.append(item_id)
     self._t += 1
@@ -817,6 +961,7 @@ class TransitionReplay:
     for i in ids:
       if not self._live_ids or not (self._live_ids[0] <= i <= self._live_ids[-1]):
         raise KeyError(i)
+    _raise_if_pool_full(self._store, self._flags())
     return self._store.get_rows(self._structure, np.asarray(ids, dtype=np.int64) % self._capacity)
 
   def sample_device(self, size: int):
@@ -834,6 +979,7 @@ class TransitionReplay:
   def sample(self, size: int):
     """`replay.py:158-165`."""
     _, _, tensors = self.sample_device(size)
+    _raise_if_pool_full(self._store, self._flags())
     return self._store.to_host_transition(self._structure, tensors)
 
   def ids(self) -> Iterable[int]:
@@ -846,6 +992,16 @@ class TransitionReplay:
   @property
   def capacity(self) -> int:
     return self._capacity
+
+  @property
+  def frames_in_use(self) -> int:
+    """Live planes of the frame pool, plane 0 included (a synchronising read; for sizing `frame_capacity`)."""
+    return _frames_in_use(self)
+
+  @property
+  def storage_bytes(self) -> int:
+    """Device bytes of the transition storage (observations or frame pool, plus per-row scalars)."""
+    return self._store.storage_bytes()
 
   def get_state(self) -> Mapping[str, Any]:
     """`replay.py:179-187`: same keys; `storage` is a list of (id, Transition) with host arrays."""
@@ -865,18 +1021,42 @@ class TransitionReplay:
       return False, 't should be >= storage size.'
     if set(self._live_ids) != set(self._distribution.ids()):
       return False, 'IDs in storage and distribution do not match.'
+    ok, msg = _check_pool(self, self._flags())
+    if not ok:
+      return ok, msg
     return self._distribution.check_valid()
 
 
+def _frames_in_use(rep):
+  if not isinstance(rep._store, _FramePoolStore):
+    raise ValueError('frames_in_use needs a replay constructed with frame_dedup=True')
+  return rep._store.frames_in_use()
+
+
+def _check_pool(rep, flags):
+  """check_valid() of a frame-deduplicated replay: the pool-full flag, refcounts and the free-stack partition."""
+  if not isinstance(rep._store, _FramePoolStore):
+    return True, ''
+  _raise_if_pool_full(rep._store, flags)
+  return rep._store.check_pool(np.asarray(list(rep._live_ids), dtype=np.int64) % rep._capacity)
+
+
 def _restore_rows(rep, storage):
-  """Rewrites device rows from a `storage` list of (id, item) (set_state)."""
+  """Rewrites device rows from a `storage` list of (id, item) (set_state).  A frame pool is emptied first and the rows
+  are re-added in id order, so the plane table is the one those adds leave (and either layout loads the other's
+  state)."""
+  pool = isinstance(rep._store, _FramePoolStore)
+  if pool:
+    storage = sorted(storage, key=lambda x: int(x[0]))
+    rep._store.reset()
+    rep._flags().bitwise_and_(~_lib.DZ_FLAG_FRAME_POOL_FULL)   # the emptied pool holds no wrong bytes
   rep._live_ids = collections.deque(int(i) for i, _ in storage)
   v = None
   for i, item in storage:
     s_tm1 = _host_obs(item[0], rep._store)
     s_t = _host_obs(item[4], rep._store)
     if v is None:
-      v = rep._store.fill_view(_lib.ReplayView())
+      v = rep.device_view() if pool else rep._store.fill_view(_lib.ReplayView())
     _apply_index_record(v, [], slot=int(i) % rep._capacity, action=int(item[1]), reward=float(item[2]),
                         discount=float(item[3]), h_s_tm1=s_tm1, h_s_t=s_t)
 
@@ -891,7 +1071,9 @@ class PrioritizedTransitionReplay:
 
   def __init__(self, capacity: int, structure, priority_exponent: float,
                importance_sampling_exponent: Callable[[int], float], uniform_sample_probability: float,
-               normalize_weights: bool, random_state: np.random.RandomState, encoder=None, decoder=None):
+               normalize_weights: bool, random_state: np.random.RandomState, encoder=None, decoder=None,
+               frame_dedup: bool = False, frame_capacity: Optional[int] = None):
+    """`frame_dedup` / `frame_capacity`: the storage layout, as for `TransitionReplay`."""
     self._codec = _check_codec(encoder, decoder)
     self._capacity = capacity
     self._structure = structure
@@ -901,7 +1083,7 @@ class PrioritizedTransitionReplay:
         uniform_sample_probability=uniform_sample_probability, random_state=random_state)
     self._importance_sampling_exponent = importance_sampling_exponent
     self._normalize_weights = normalize_weights
-    self._store = _TransitionStore(capacity)
+    self._store = _make_store(capacity, frame_dedup, frame_capacity)
     self._live_ids = collections.deque()
     self._t = 0
 
@@ -910,6 +1092,9 @@ class PrioritizedTransitionReplay:
     self._store.fill_view(v)
     v.d_flags = _ptr(self._distribution._sum_tree._flags)
     return v
+
+  def _flags(self):
+    return self._distribution._sum_tree._flags
 
   def add(self, item, priority: float) -> None:
     """`replay.py:690-699`: one device call carries the row, the list patches, the evicted
@@ -941,7 +1126,7 @@ class PrioritizedTransitionReplay:
     _apply_index_record(v, patches[:4], tree_index=idx, leaf_value=float(leaf[0]), evict_index=evicted,
                         size_after=dist._sum_tree.size, slot=item_id % self._capacity, action=int(item[1]),
                         reward=float(item[2]), discount=float(item[3]), h_s_tm1=s_tm1, h_s_t=s_t,
-                        d_priority=d_priority, alpha=float(alpha))
+                        d_priority=d_priority, alpha=float(alpha), release_row=evicted >= 0)
     assert len(patches) <= 4
     self._live_ids.append(item_id)
     self._t += 1
@@ -951,6 +1136,7 @@ class PrioritizedTransitionReplay:
     for i in ids:
       if i not in self._distribution._id_to_index:
         raise KeyError(i)
+    _raise_if_pool_full(self._store, self._flags())
     return self._store.get_rows(self._structure, np.asarray(ids, dtype=np.int64) % self._capacity)
 
   def sample_device(self, size: int):
@@ -967,6 +1153,7 @@ class PrioritizedTransitionReplay:
     ids, _, _, _, weights, tensors = self.sample_device(size)
     tr = self._store.to_host_transition(self._structure, tensors)
     w = weights.cpu().numpy()
+    _raise_if_pool_full(self._store, self._flags())
     self._distribution._sum_tree._raise_flags()
     if not np.isfinite(w).all():
       raise ValueError('Weights are not finite: %s.' % w)
@@ -989,6 +1176,16 @@ class PrioritizedTransitionReplay:
     """`replay.py:742-745`."""
     return self._importance_sampling_exponent(self._t)
 
+  @property
+  def frames_in_use(self) -> int:
+    """Live planes of the frame pool, plane 0 included (a synchronising read; for sizing `frame_capacity`)."""
+    return _frames_in_use(self)
+
+  @property
+  def storage_bytes(self) -> int:
+    """Device bytes of the transition storage (observations or frame pool, plus per-row scalars)."""
+    return self._store.storage_bytes()
+
   def get_state(self) -> Mapping[str, Any]:
     """`replay.py:747-754`."""
     ids = list(self._live_ids)
@@ -1007,6 +1204,9 @@ class PrioritizedTransitionReplay:
       return False, 't should be >= storage size.'
     if set(self._live_ids) != set(self._distribution.ids()):
       return False, 'IDs in storage and distribution do not match.'
+    ok, msg = _check_pool(self, self._flags())
+    if not ok:
+      return ok, msg
     return self._distribution.check_valid()
 
 
@@ -1018,10 +1218,36 @@ def bulk_fill_synthetic(rep, obs_shape, seed, num_actions, discount=0.99, priori
   host bookkeeping is written in closed form (allocation order of replay.py:457,499: id i gets
   tree index C-1-i)."""
   assert rep._t == 0 and rep.size == 0
+  if isinstance(rep._store, _FramePoolStore):
+    raise ValueError('bulk_fill_synthetic writes iid rows that share no frames; fill a frame_dedup replay with '
+                     'bulk_fill_synthetic_stacked')
   cap = rep._capacity
   rep._store.allocate(obs_shape, np.uint8)
   v = rep._store.fill_view(_lib.ReplayView())
   _lib.call('dz_replay_fill_synthetic', C.byref(v), 0, cap, int(seed), int(num_actions), float(discount), _stream())
+  _fill_bookkeeping(rep, priority)
+
+
+def bulk_fill_synthetic_stacked(rep, obs_shape, seed, num_actions, episode_len=1000, discount=0.99, priority=1.0):
+  """`bulk_fill_synthetic` with frame stacks instead of iid rows, for either layout: transition i is step
+  i % episode_len of episode i // episode_len, its observations trailing-zero-padded stacks of splitmix frames
+  (dz_replay_fill_synthetic_stacked, byte-identical to oracle/frame_pool_oracle.py:synthetic_stacked_rows).  A
+  frame_dedup replay is left with the plane table, refcounts and free stack that `capacity` sequential adds leave."""
+  assert rep._t == 0 and rep.size == 0
+  if len(obs_shape) != 3:
+    raise ValueError('stacked fill needs [H, W, C] observations')
+  cap = rep._capacity
+  rep._store.allocate(obs_shape, np.uint8)
+  v = rep.device_view()
+  v.obs_channels = int(obs_shape[2])
+  _lib.call('dz_replay_fill_synthetic_stacked', C.byref(v), cap, int(seed), int(episode_len), int(num_actions),
+            float(discount), _stream())
+  _fill_bookkeeping(rep, priority)
+
+
+def _fill_bookkeeping(rep, priority):
+  """Host state (and device mirrors) of `capacity` sequential adds of ids 0..C-1 with priority `priority`."""
+  cap = rep._capacity
   rep._live_ids = collections.deque(range(cap))
   rep._t = cap
   dist = rep._distribution

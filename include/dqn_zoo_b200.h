@@ -79,6 +79,7 @@ int dz_sumtree_get(const double* d_nodes, int64_t first_leaf, int64_t size, cons
 #define DZ_FLAG_BAD_TARGET 4
 #define DZ_FLAG_ROOT_ZERO 8   /* fused PER step met root == 0 (reference would skip an RNG draw) */
 #define DZ_FLAG_NONFINITE_WEIGHT 16
+#define DZ_FLAG_FRAME_POOL_FULL 32  /* an add found no free plane (frame_capacity too small); the plane was mapped to 0 */
 
 /* ------------------------------------------------------------------------------------------
  * R5/R6  Replay storage in HBM (replaces the OrderedDict storage of replay.py:120-200 and
@@ -102,6 +103,23 @@ typedef struct dz_replay_view {
   /* uniform replay only */
   int64_t* d_ids;        /* `UniformDistribution._ids` (replay.py:49): dense list of ids      */
   int32_t* d_flags;      /* sticky error flags (1 int32)                                      */
+  /* frame-deduplicated layout only (d_planes == NULL: transition-major, d_obs holds the rows; DESIGN.md §3).
+   * An observation [H][W][C] uint8 is C planes of H*W bytes; each distinct plane is stored once in d_frames and
+   * row `slot` keeps 2*C plane ids (s_tm1 channels 0..C-1, then s_t channels 0..C-1).  Plane 0 is the reserved
+   * all-zero plane: always live, never freed, its refcount carries one permanent reference. */
+  uint8_t* d_frames;     /* [frame_capacity][frame_stride] planar frame pool; offsets are 64-bit */
+  int64_t frame_bytes;   /* H*W                                                                */
+  int64_t frame_stride;  /* frame_bytes rounded up to 16 (the padding is zero)                 */
+  int64_t obs_channels;  /* C (<= 32); also read by dz_replay_fill_synthetic_stacked in either layout */
+  int64_t frame_capacity;
+  int32_t* d_planes;     /* [capacity][2*C] plane ids                                          */
+  int32_t* d_refcount;   /* [frame_capacity] references from live rows (+1 for plane 0)        */
+  uint64_t* d_hashes;    /* [frame_capacity] 64-bit content hash of each live plane            */
+  int32_t* d_table;      /* [table_size] open-addressing table of live plane ids (-1 = empty)  */
+  int64_t table_size;    /* power of two >= 2 * frame_capacity                                  */
+  int32_t* d_free;       /* [frame_capacity] LIFO free stack (top = d_pool_counters[0])        */
+  int64_t* d_pool_counters; /* [1]: free-stack top; live planes = frame_capacity - top         */
+  uint8_t* d_add_staging;   /* [2][obs_stride] host-source copy + [2*C][frame_stride] planar    */
 } dz_replay_view;
 
 /* One `add` (replay.py:142-151 / :690-699) after the HOST has done the O(1) integer
@@ -126,11 +144,33 @@ typedef struct dz_add_record {
                                 max_seen_priority, rainbow/agent.py:148-149) instead of leaf_value;
                                 leaf = ((double)*d_priority) ** alpha in float64, exact for alpha 0.5 / 1 */
   double alpha;
+  int32_t release_row;       /* frame-deduplicated layout: 1 = row `slot` holds a live transition whose plane
+                                references are released AFTER the new row's planes are resolved and referenced */
 } dz_add_record;
 
-/* s_tm1 / s_t sources may be HOST arrays or DEVICE buffers (cudaMemcpyDefault; NULL = leave the row's bytes). */
+/* s_tm1 / s_t sources may be HOST arrays or DEVICE buffers (cudaMemcpyDefault; NULL = leave the row's bytes).
+ * Frame-deduplicated layout (view->d_planes != NULL): both sources are required; host sources are first copied into
+ * d_add_staging, device sources are read in place.  One CTA hashes the 2*C planes, resolves each (in order, each
+ * seeing the ones before it) to the live plane with identical bytes (hash hit + full byte compare) or to a fresh plane
+ * popped from the free stack, then releases the evicted row (refcount 0 -> back on the free stack).  An empty free
+ * stack sets DZ_FLAG_FRAME_POOL_FULL and maps the plane to plane 0. */
 int dz_replay_add(const dz_replay_view* view, const dz_add_record* rec, const uint8_t* h_s_tm1,
                   const uint8_t* h_s_t, void* stream);
+
+/* Frame-deduplicated layout: empties the pool (every row's plane ids = 0, free stack hands out 1, 2, 3, ... next,
+ * plane 0 zeroed, live and in the table). */
+int dz_replay_frame_pool_reset(const dz_replay_view* view, void* stream);
+/* Frame-deduplicated layout: live planes (plane 0 included) into *h_frames_in_use.  Synchronises `stream`. */
+int dz_replay_frames_in_use(const dz_replay_view* view, int64_t* h_frames_in_use, void* stream);
+
+/* Bulk pre-fill of rows [0, n) of an EMPTY replay with frame stacks, either layout: frame f of episode e is
+ * mix64(seed*0x9E3779B97F4A7C15 + 0x632BE59BD9B4E019 + (e*(episode_len+1) + f)*(H*W/8) + w) per 8-byte word w
+ * (H*W % 8 == 0).  Transition i is step t = i % episode_len of episode e = i / episode_len; its s_tm1 is the stack
+ * after frames 0..t (trailing-zero padded while t + 1 < C: A000, AB00, ...; processors.py:497-504), s_t the stack after
+ * frames 0..t+1.  Scalars as dz_replay_fill_synthetic.  Byte-identical to oracle/frame_pool_oracle.py:synthetic_stacked_rows;
+ * in the deduplicated layout the plane table, refcounts, hash table and free stack are those n sequential adds leave. */
+int dz_replay_fill_synthetic_stacked(const dz_replay_view* view, int64_t n, uint64_t seed, int64_t episode_len,
+                                     int32_t num_actions, double discount, void* stream);
 
 /* Bulk pre-fill for benchmarks/tests: rows [row0,row0+n) get deterministic pseudo-random
  * contents (splitmix64 counter hash; byte-identical to oracle/replay_oracle.py:synthetic_rows):
