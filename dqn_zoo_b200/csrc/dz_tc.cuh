@@ -23,6 +23,34 @@ __device__ __forceinline__ void mma_16x8x8(float (&d)[4], const uint32_t (&a)[4]
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
+// The B fragment loads and MMAs of one k-step of warp_kstep_3xtf32 (below), with the A fragments already in registers
+// (ah / al, element q of m-tile mt = A[m0 + 16 mt + g + 8 (q & 1)][k0 + t + 4 (q >> 1)]); a_has_lo: false when A is
+// exact (al unused).
+template <int MT, int NT, class BOff>
+__device__ __forceinline__ void warp_mma_3xtf32(float (&sum)[MT][NT][4], const uint32_t (&ah)[MT][4], const uint32_t (&al)[MT][4],
+                                                bool a_has_lo, const uint8_t* b_hi, const uint8_t* b_lo, int n0, int k0, BOff b_off) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int nt = 0; nt < NT; ++nt) {
+    uint32_t bh[2], bl[2];
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const uint32_t o = b_off(n0 + nt * 8 + g, k0 + t + q * 4);
+      bh[q] = *reinterpret_cast<const uint32_t*>(b_hi + o);
+      bl[q] = *reinterpret_cast<const uint32_t*>(b_lo + o);
+    }
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) {
+      float p[4] = {0.f, 0.f, 0.f, 0.f};
+      if (a_has_lo) mma_16x8x8(p, al[mt], bh);         // small cross terms first
+      mma_16x8x8(p, ah[mt], bl);
+      mma_16x8x8(p, ah[mt], bh);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) sum[mt][nt][e] += p[e];
+    }
+  }
+}
+
 // One warp's share of one k-step of 8 reduction elements: rows [m0, m0 + 16 MT) x columns [n0, n0 + 8 NT) of
 //     D += Al*Bh + Ah*Bl + Ah*Bh      (Al*Bh skipped when A is exact, i.e. has no lo part: a_lo == nullptr)
 // a_off(m, k) / b_off(n, k): byte offset of an element inside one part (hi or lo) of the staged operand, so any
@@ -44,25 +72,7 @@ __device__ __forceinline__ void warp_kstep_3xtf32(float (&sum)[MT][NT][4], const
       al[mt][q] = a_lo ? *reinterpret_cast<const uint32_t*>(a_lo + o) : 0u;
     }
   }
-#pragma unroll
-  for (int nt = 0; nt < NT; ++nt) {
-    uint32_t bh[2], bl[2];
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      const uint32_t o = b_off(n0 + nt * 8 + g, k0 + t + q * 4);
-      bh[q] = *reinterpret_cast<const uint32_t*>(b_hi + o);
-      bl[q] = *reinterpret_cast<const uint32_t*>(b_lo + o);
-    }
-#pragma unroll
-    for (int mt = 0; mt < MT; ++mt) {
-      float p[4] = {0.f, 0.f, 0.f, 0.f};
-      if (a_lo) mma_16x8x8(p, al[mt], bh);             // small cross terms first
-      mma_16x8x8(p, ah[mt], bl);
-      mma_16x8x8(p, ah[mt], bh);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) sum[mt][nt][e] += p[e];
-    }
-  }
+  warp_mma_3xtf32<MT, NT>(sum, ah, al, a_lo != nullptr, b_hi, b_lo, n0, k0, b_off);
 }
 
 // ---- warpgroup MMA (wgmma, sm_90a) on K-major SWIZZLE_128B operands -----------------------------------------------

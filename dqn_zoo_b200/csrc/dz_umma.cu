@@ -103,6 +103,8 @@ int UmPlan::configure() {
   if (done) return DZ_OK;
   DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_fc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_fc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   DZ_CUDA_OK(cudaFuncSetAttribute(um::wgmma_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   DZ_CUDA_OK(cudaFuncSetAttribute(um::wgmma_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   done = true;
@@ -115,6 +117,26 @@ bool UmPlan::wgmma_eligible(const UmLaunch& l) const {
     for (const UmOperand* o : {&pr.A, &pr.B})
       if (o->mn_major || o->nparts != 2 || o->convert) return false;
     if (pr.ksteps != 4) return false;
+  }
+  return true;
+}
+
+bool UmPlan::fc_eligible(const UmLaunch& l) const {
+  for (int ci = l.cta0; ci < l.cta0 + l.nctas; ++ci) {
+    const UmCta& c = ctas[ci];
+    const int np = c.nprob > 1 ? (int)c.nprob : 1;
+    if (np > um::kFcMaxProbs) return false;
+    for (int q = 0; q < np; ++q) {
+      const UmProblem& pr = probs[c.prob + q];
+      if (!pr.A.mn_major || pr.A.lbo != 4096u || pr.A.part_bytes * (uint32_t)np != 16384u) return false;
+      if (pr.A.convert != 2 && !(pr.A.convert == 1 && pr.A.scale_r == nullptr)) return false;
+      if (pr.B.mn_major || pr.B.nparts != 2 || pr.B.convert) return false;
+      if (pr.ksteps != 4 || pr.red_per_stage != 32 || pr.epi != UM_EPI_PARTIAL || pr.sc_i != 1) return false;
+      if (q > 0 && (pr.A.part_bytes != probs[c.prob].A.part_bytes || pr.A.convert != probs[c.prob].A.convert ||
+                    pr.B.part_bytes != probs[c.prob].B.part_bytes))
+        return false;
+    }
+    if (2 * 16384u / (uint32_t)np + (uint32_t)np * 2u * probs[c.prob].B.part_bytes > l.stage_bytes) return false;
   }
   return true;
 }
@@ -137,7 +159,8 @@ int UmPlan::launch(const char* tag, const UmLaunch& l, void* stream, long long* 
   if ((size_t)stages * l.stage_bytes < (size_t)128 * l.njt * 4) return fail(DZ_EINVAL, "umma launch: stage buffers smaller than the store-phase staging tile");
   const int v = l.njt == 32 ? 0 : 1;
   if (l.njt != 32 && l.njt != 64) return fail(DZ_EINVAL, "umma launch: NJT must be 32 or 64");
-  if (path != UM_PATH_AUTO && path != UM_PATH_MMA_SYNC && path != UM_PATH_WGMMA) return fail(DZ_EINVAL, "umma launch: unknown MMA path");
+  if (path != UM_PATH_AUTO && path != UM_PATH_MMA_SYNC && path != UM_PATH_WGMMA && path != UM_PATH_CONVERTERS)
+    return fail(DZ_EINVAL, "umma launch: unknown MMA path");
   const bool wg = path == UM_PATH_AUTO ? wgmma_eligible(l) : path == UM_PATH_WGMMA;
   if (wg && !wgmma_eligible(l)) return fail(DZ_EINVAL, "umma launch: the wgmma path needs K-major, pre-split operands and four k-steps per stage");
   if (wg)
@@ -156,6 +179,17 @@ int UmPlan::launch(const char* tag, const UmLaunch& l, void* stream, long long* 
                       stages, l.stage_bytes, d_trace);
     return DZ_OK;
   }
+  if (path != UM_PATH_CONVERTERS && fc_eligible(l)) {
+    if (v == 0)
+      DZ_LAUNCH_NAMED(tag, um::umma_fc_kernel<32>, (unsigned)l.nctas, um::kThreadsF, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps,
+                      stages, l.stage_bytes, d_trace);
+    else
+      DZ_LAUNCH_NAMED(tag, um::umma_fc_kernel<64>, (unsigned)l.nctas, um::kThreadsF, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps,
+                      stages, l.stage_bytes, d_trace);
+    return DZ_OK;
+  }
+  for (int ci = l.cta0; ci < l.cta0 + l.nctas; ++ci)
+    if (ctas[ci].nprob > 1) return fail(DZ_EINVAL, "umma launch: CTAs that serve several problems need umma_fc_kernel");
   if (v == 0)
     DZ_LAUNCH_NAMED(tag, um::umma_gemm_kernel<32>, (unsigned)l.nctas, um::kThreadsU, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps, stages,
                     l.stage_bytes, d_trace);

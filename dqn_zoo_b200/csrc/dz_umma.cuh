@@ -18,7 +18,8 @@
 //
 // Precision: activations are stored ONCE as tf32 hi/lo pairs by the producing epilogue (x = hi + lo, both exactly
 // representable), fp32 weights are split in place in shared memory by converter warps (raw tile -> hi in place, lo
-// in the sibling buffer; the split is position-wise, so it is swizzle-agnostic), D += Al*Bh + Ah*Bl + Ah*Bh.  The
+// in the sibling buffer; the split is position-wise, so it is swizzle-agnostic) or, for the fc forward, in the MMA
+// warps' registers (umma_fc_kernel), D += Al*Bh + Ah*Bl + Ah*Bh.  The
 // tensor core truncates its fp32 accumulator, so each k-step's products are added into the fp32 sums with
 // round-to-nearest adds (dz_tc.cuh, warp_kstep_3xtf32 / wgmma_kstep_3xtf32).
 //
@@ -86,7 +87,7 @@ struct UmCta {              // one per CTA
   int32_t split;
   int32_t row_base;         // UM_EPI_ROWS
   int32_t ph_valid, pw_valid;   // valid (r / pw) and (r % pw) extents
-  uint32_t pad;
+  uint32_t nprob;           // umma_fc_kernel: problems prob, prob + 1, ... sharing the staged A tile (0 or 1: one)
 };
 
 namespace um {
@@ -457,6 +458,174 @@ __global__ void __launch_bounds__(kThreadsU, 1)
   if (tr && threadIdx.x == 0) trace[322] = clock64();
 }
 
+// Clock stamp *addr = clock64() where `pred` holds, without a branch (see mbar_arrive_if).
+__device__ __forceinline__ void stamp_if(long long* addr, bool pred) {
+  asm volatile("{\n.reg .pred p;\n.reg .b64 c;\nsetp.ne.b32 p, %1, 0;\nmov.u64 c, %%clock64;\n@p st.global.b64 [%0], c;\n}\n" ::"l"(addr),
+               "r"((int)pred)
+               : "memory");
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Sibling of umma_gemm_kernel for the fc1 / noisy1 forward: A = raw fp32 weights W[k][n], staged MN-major (mu, plus
+// sigma for noisy layers), B = activations, K-major tf32 hi/lo pairs.  There are no converter warps: every MMA warp
+// loads raw mu / sigma fragments from the staged tile at the addresses umma_gemm_kernel reads hi fragments from, forms
+//     w = fmaf(sigma, eps_in[k] * eps_out[n], mu)        (noisy; the operations and their order of convert_part16k)
+// and its tf32 hi/lo split in registers, and issues the k-step of warp_kstep_3xtf32.  Each output element therefore sees
+// the same operands and the same sequence of k-steps as on umma_gemm_kernel: the partials are bit-identical.
+//
+// One CTA serves cta.nprob (1 or 2) consecutive problems that read the same weight tile: the passes of the learner
+// that apply the same parameters (online net on s_tm1 and on s_t) stage each mu / sigma tile once.  The tile spans
+// 128 / nprob D rows; the stage holds the A parts (A.part_bytes each) followed by one B hi/lo pair per problem.
+// Warp roles: 0 TMA producer (and barrier set-up) | 1-8 MMA, 8 / nprob warps per problem, 16 D rows x NJT columns each.
+// Only the direct partial epilogue (UM_EPI_PARTIAL, sc_i == 1) is supported: the warps store from their fragments.
+constexpr int kFcMmaWarps = 8;
+constexpr int kThreadsF = (1 + kFcMmaWarps) * 32;
+constexpr int kFcMaxProbs = 2;
+
+template <int NJT>
+__global__ void __launch_bounds__(kThreadsF, 1)
+    umma_fc_kernel(const __grid_constant__ UmMaps maps, const UmCta* __restrict__ ctas, const UmProblem* __restrict__ probs,
+                   const UmTmaOp* __restrict__ ops, int nmaps, int stages, uint32_t stage_bytes, long long* __restrict__ trace) {
+  if (threadIdx.x < nmaps) prefetch_tensormap(&maps.m[threadIdx.x]);
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + smem_pad_1024(smem_raw);
+  const bool tr = trace != nullptr && blockIdx.x == 0;
+  const UmCta cta = ctas[blockIdx.x];
+  const int ST = stages;
+  const int nst = (int)cta.nstages;
+  const int P = cta.nprob > 1 ? 2 : 1;
+
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem);      // [ST] TMA landed
+  uint64_t* empty = full + 2 * kStagesMax;                  // [ST] MMA warps consumed the stage
+  UmProblem* p_smem = reinterpret_cast<UmProblem*>(smem + 1024);
+  UmTmaOp* ops_smem = reinterpret_cast<UmTmaOp*>(smem + 2048);
+  uint8_t* stage_base = smem + kCtlBytes;
+  static_assert(kFcMaxProbs * sizeof(UmProblem) <= 1024, "problem copies do not fit their slot");
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  {
+    const uint4* src = reinterpret_cast<const uint4*>(probs + cta.prob);
+    uint4* dst = reinterpret_cast<uint4*>(p_smem);
+    for (int i = threadIdx.x; i < P * (int)(sizeof(UmProblem) / 16); i += kThreadsF) dst[i] = src[i];
+    const int nvec = min(nst * (int)cta.ops_per_stage, kMaxOpsPerCta) * 2;
+    const uint4* osrc = reinterpret_cast<const uint4*>(ops + cta.op0);
+    uint4* odst = reinterpret_cast<uint4*>(ops_smem);
+    for (int i = threadIdx.x; i < nvec; i += kThreadsF) odst[i] = osrc[i];
+  }
+  if (warp == 0 && lane == 0) {
+    for (int s = 0; s < ST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kFcMmaWarps); }
+    fence_mbarrier_init();
+  }
+  __syncthreads();
+
+  if (warp == 0) {
+    // ---------------------------------------------------------------- TMA producer (as in umma_gemm_kernel, one warp)
+    const int nops = (int)cta.ops_per_stage;
+    int s = 0;
+    uint32_t ph = 0;
+    uint32_t st_addr = smem_u32(stage_base);
+    int oi = 0;
+    dz::pdl_enter();
+    if (tr && lane == 0) { trace[323] = clock64(); trace[324] = clock64(); }
+    for (int it = 0; it < nst; ++it) {
+      mbar_wait(&empty[s], ph ^ 1u);
+      if (lane == 0) mbar_expect_tx(&full[s], cta.tx_bytes);
+      __syncwarp();
+      if (lane < nops) {
+        const int o = oi + lane;
+        const UmTmaOp op = o < kMaxOpsPerCta ? ops_smem[o] : ops[cta.op0 + o];
+        tma_load_5d(st_addr + op.smem_off, &maps.m[op.map], &full[s], op.c[0], op.c[1], op.c[2], op.c[3], op.c[4]);
+      }
+      if (tr && lane == 0 && it < 64) trace[it] = clock64();                                        // [0,64): TMA issued
+      __syncwarp();
+      oi += nops;
+      ++s; st_addr += stage_bytes;
+      if (s == ST) { s = 0; ph ^= 1u; st_addr = smem_u32(stage_base); }
+    }
+    return;
+  }
+
+  // ---------------------------------------------------------------- MMA warps
+  const int w = warp - 1, wpp = kFcMmaWarps / P;
+  const int q = w / wpp, m0 = 16 * (w - q * wpp);         // problem (pass) of this warp, its first D row in the tile
+  const bool lead = w == 0 && lane == 0;
+  const UmProblem& p = p_smem[q];
+  const int g = lane >> 2, t = lane & 3;
+  const uint32_t a_part = p.A.part_bytes, a_lbo = p.A.lbo;
+  const uint8_t* b_first = stage_base + a_part * 2 + (uint32_t)q * 2u * p.B.part_bytes;
+  const uint32_t b_part = p.B.part_bytes;
+  const bool noisy = p.A.convert == 2;
+  const float* __restrict__ eps_in = p.A.scale_r;
+  constexpr int NT = NJT / 8;
+  float sum[1][NT][4];
+#pragma unroll
+  for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) sum[0][nt][e] = 0.f;
+  auto b_off = [](int n, int k) { return sw128_kmajor(n, k); };
+  dz::pdl_enter();                                          // the noise vectors may come from an earlier kernel
+  // eps_out of the thread's two D rows (g, g + 8): loop invariants
+  float eo[2] = {1.f, 1.f};
+  if (noisy) {
+    eo[0] = p.A.scale_i[cta.i0 + m0 + g];
+    eo[1] = p.A.scale_i[cta.i0 + m0 + g + 8];
+  }
+  int s = 0, r0 = cta.r0;
+  uint32_t ph = 0;
+  for (int it = 0; it < nst; ++it) {
+    mbar_wait(&full[s], ph);
+    stamp_if(trace + 64 + it, tr && lead && it < 64);                                               // [64,128): stage data ready
+    const uint8_t* mu = stage_base + (size_t)s * stage_bytes;
+    const uint8_t* sg = mu + a_part;
+    const uint8_t* bh = b_first + (size_t)s * stage_bytes;
+    // NJT 64: a stage's k-steps unrolled in pairs, so that the loads hoisted ahead of the MMAs fit the 168 registers a
+    // thread of a nine-warp CTA has (three warps share one sub-partition's register file)
+#pragma unroll(NJT == 32 ? 4 : 2)
+    for (int ks = 0; ks < 4; ++ks) {
+      uint32_t ah[1][4], al[1][4];
+      float ei[2] = {1.f, 1.f};              // eps_in of the thread's reduction indices k = 8 ks + t + 4 h
+      if (noisy) { ei[0] = eps_in[r0 + 8 * ks + t]; ei[1] = eps_in[r0 + 8 * ks + t + 4]; }
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const uint32_t o = sw128_mnmajor(m0 + g + (e & 1) * 8, 8 * ks + t + (e >> 1) * 4, a_lbo);
+        float v = *reinterpret_cast<const float*>(mu + o);
+        if (noisy) {
+          const float f = ei[e >> 1] * eo[e & 1];
+          v = fmaf(*reinterpret_cast<const float*>(sg + o), f, v);
+        }
+        float hh, ll;
+        split_tf32(v, hh, ll);
+        ah[0][e] = __float_as_uint(hh);
+        al[0][e] = __float_as_uint(ll);
+      }
+      warp_mma_3xtf32<1, NT>(sum, ah, al, true, bh, bh + b_part, 0, 8 * ks, b_off);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);
+    stamp_if(trace + 128 + it, tr && lead && it < 64);                                              // [128,192): stage consumed
+    r0 += 32;
+    if (++s == ST) { s = 0; ph ^= 1u; }
+  }
+  if (lead) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // the next kernel's set-up overlaps our epilogue
+  if (tr && lead) trace[320] = clock64();                                                           // store phase starts
+  float* dst = p.C + (long long)cta.split * p.split_stride;
+  const long long sc_j = p.sc_j;
+#pragma unroll
+  for (int e = 0; e < 4; e += 2) {
+    const int i = cta.i0 + m0 + frag_row(0, e);
+    if (i >= p.MI) continue;
+    const float sc = p.scale_i ? p.scale_i[i] : 1.0f;
+#pragma unroll
+    for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int j = frag_col(nt, e + h);
+        if (j < p.NJ) dst[i + (long long)j * sc_j] = sum[0][nt][e + h] * sc;
+      }
+  }
+  if (tr && lead) { trace[321] = clock64(); trace[322] = clock64(); }                             // stores issued / exit
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // Warpgroup-MMA sibling of umma_gemm_kernel for problems whose operands are both K-major tf32 hi/lo pairs that need no
 // conversion (conv2 / conv3 forward and input gradient): the staged tiles are already in the layout wgmma reads, so
@@ -464,13 +633,6 @@ __global__ void __launch_bounds__(kThreadsU, 1)
 // ring, PDL points, clock stamps and both epilogues are those of umma_gemm_kernel.
 constexpr int kThreadsW = 3 * 128;   // producer warpgroup + two consumer warpgroups
 constexpr int kConsumerWarps = 8;
-
-// Clock stamp *addr = clock64() where `pred` holds, without a branch (see mbar_arrive_if).
-__device__ __forceinline__ void stamp_if(long long* addr, bool pred) {
-  asm volatile("{\n.reg .pred p;\n.reg .b64 c;\nsetp.ne.b32 p, %1, 0;\nmov.u64 c, %%clock64;\n@p st.global.b64 [%0], c;\n}\n" ::"l"(addr),
-               "r"((int)pred)
-               : "memory");
-}
 
 // Rows of the CTA's 128-row tile that reach the output: the tail beyond them (padding, TMA zero fill) is never stored,
 // so an m64 half that lies entirely in it needs no MMAs.

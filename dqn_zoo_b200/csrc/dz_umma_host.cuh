@@ -7,10 +7,12 @@
 
 namespace dz {
 
-// MMA path of a launch: the warp-level mma.sync kernel (every operand layout) or the wgmma kernel (K-major, pre-split).
-enum : int { UM_PATH_AUTO = 0, UM_PATH_MMA_SYNC = 1, UM_PATH_WGMMA = 2 };
+// MMA path of a launch: the warp-level mma.sync kernels (every operand layout) or the wgmma kernel (K-major, pre-split).
+// On the mma.sync path, launches that fc_eligible() accepts run on umma_fc_kernel, all others on umma_gemm_kernel.
+// UM_PATH_CONVERTERS (tests only) keeps umma_gemm_kernel, with its converter warps, where umma_fc_kernel would run.
+enum : int { UM_PATH_AUTO = 0, UM_PATH_MMA_SYNC = 1, UM_PATH_WGMMA = 2, UM_PATH_CONVERTERS = 3 };
 
-// One launch of umma_gemm_kernel / wgmma_gemm_kernel: a contiguous range of CTA descriptors sharing NJT / stage geometry.
+// One launch of umma_gemm_kernel / umma_fc_kernel / wgmma_gemm_kernel: a contiguous range of CTA descriptors sharing NJT / stage geometry.
 struct UmLaunch {
   int cta0 = 0, nctas = 0;
   int njt = 64;
@@ -39,10 +41,13 @@ struct UmPlan {
   int upload();          // (re)allocates and copies all four tables
   void release();
   // d_trace: 512 clock stamps of CTA 0 (debug).  path: UM_PATH_AUTO picks wgmma_gemm_kernel when wgmma_eligible(l), else
-  // umma_gemm_kernel; UM_PATH_MMA_SYNC / UM_PATH_WGMMA force one (forcing wgmma on a launch that is not eligible fails).
+  // the mma.sync path; UM_PATH_MMA_SYNC / UM_PATH_WGMMA force one (forcing wgmma on a launch that is not eligible fails).
   int launch(const char* tag, const UmLaunch& l, void* stream, long long* d_trace = nullptr, int path = UM_PATH_AUTO) const;
   // Every CTA of the launch has both operands K-major tf32 hi/lo pairs that need no conversion, four k-steps per stage.
   bool wgmma_eligible(const UmLaunch& l) const;
+  // Every CTA has an MN-major raw fp32 A (convert 1 without scale_r, or 2) of 128 / nprob rows and 32 reduction rows per
+  // stage, nprob <= 2, a K-major pre-split B, four k-steps per stage and the direct partial epilogue.
+  bool fc_eligible(const UmLaunch& l) const;
   int path_of(const UmLaunch& l) const { return wgmma_eligible(l) ? UM_PATH_WGMMA : UM_PATH_MMA_SYNC; }
   static int configure();   // one-time kernel attributes (outside any stream capture)
 };

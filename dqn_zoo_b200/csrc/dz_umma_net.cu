@@ -5,7 +5,8 @@
 //
 //   rows (uint8, replay store) --bulk copy--> smem --convert--> conv1 MMA --> act1 {hi,lo,f32} [P*B][h1][w1][32]
 //   act1 --TMA im2col boxes--> conv2 MMA --> act2 [P*B][h2][w2][64] --TMA--> conv3 MMA --> act3 = features [P*B][feat]
-//   W (fp32, [feat][512]) --TMA--> smem --in-place hi/lo split--> MN-major MMA x act3 --> split-K partials --> finish --> h1
+//   W (fp32, [feat][512]) --TMA, once per blob--> smem --hi/lo split in registers--> MN-major MMA x act3 (every pass
+//        applying the blob) --> split-K partials --> finish --> h1
 //   dh1 --> W (K-major) MMA --> partials --> finish (ReLU mask) --> dact3 --TMA (zero-filled halo)--> conv3 dgrad --> dact2
 //        --> conv2 dgrad (4 stride-parity classes) --> dact1
 #include <algorithm>
@@ -42,6 +43,7 @@ struct UmNet {
   std::string trace_tag;                   // debug: the launch with this tag writes CTA 0's clock stamps to trace_ptr
   long long* trace_ptr = nullptr;
   long long* tr(const char* tag) const { return trace_ptr && trace_tag == tag ? trace_ptr : nullptr; }
+  bool fc_per_pass = false;                // tests only: fc forward CTA groups per pass (the umma_gemm_kernel layout)
 };
 
 namespace {
@@ -1066,7 +1068,22 @@ int build_plan(UmNet* n) {
       m_g[part] = pl.add_map(part ? n->dh1_lo : n->dh1_hi, 2, gd, gs, box);
       if (m_x[part] < 0 || m_g[part] < 0) return DZ_EINVAL;
     }
-    // weight maps: [blob][stream][sigma] x {forward box (32 n, 32 k), gradient box (32 n, 128 k)}
+    // Forward CTA groups: the passes that apply the same parameter blob share every staged weight tile (online net on
+    // s_tm1 and s_t), each group's tiles then span 128 / (passes in the group) weight columns, so a CTA does the same
+    // MMA work whether it serves one pass or two.  fc_per_pass (tests only): one group per pass, 128-column tiles.
+    int grp[3][kFcMaxProbs], ngrp = 0, grp_n[3] = {0, 0, 0}, grp_blob[3] = {0, 0, 0};
+    for (int p = 0; p < d.npass; ++p) {
+      const int blob = d.pass_target[p] ? 1 : 0;
+      int gi = -1;
+      if (!n->fc_per_pass)
+        for (int k = 0; k < ngrp; ++k) if (grp_blob[k] == blob) gi = k;
+      if (gi < 0) { gi = ngrp++; grp_blob[gi] = blob; }
+      if (grp_n[gi] == kFcMaxProbs) return fail(DZ_EINVAL, "fc forward: more than two passes apply one parameter blob");
+      grp[gi][grp_n[gi]++] = p;
+    }
+    int fc_rows[2] = {128, 128};   // forward tile columns per blob
+    for (int k = 0; k < ngrp; ++k) fc_rows[grp_blob[k]] = 128 / grp_n[k];
+    // weight maps: [blob][stream][sigma] x {forward box (32 n, 32 k) x fc_rows / 32, gradient box (32 n, 128 k)}
     int m_wf_fc[2][2][2], m_wd_fc[2][2];
     bool wf3d = true;
     for (int blob = 0; blob < 2; ++blob)
@@ -1075,9 +1092,9 @@ int build_plan(UmNet* n) {
           const float* w = (blob ? d.target : d.online) + (sg ? d.off_fc_sw[s] : d.off_fc_w[s]);
           uint64_t dims[2] = {512, (uint64_t)feat}, strides[1] = {2048};
           // MN-major A operand (rows of W are the reduction): W[k][n] viewed as (n % 32, k, n / 32) so that ONE box of
-          // (32, 32, 4) lands as the four [32 k][32 n] slabs of a 128-column tile, slab-major — one TMA op per 16 KB tile
+          // (32, 32, fc_rows / 32) lands as the [32 k][32 n] slabs of a tile, slab-major — one TMA op per tile
           uint64_t dims3[3] = {32, (uint64_t)feat, 16}, strides3[2] = {2048, 128};
-          uint32_t box3[3] = {32, 32, 4};
+          uint32_t box3[3] = {32, 32, (uint32_t)fc_rows[blob] / 32};
           if (wf3d) {
             m_wf_fc[blob][s][sg] = pl.add_map(w, 3, dims3, strides3, box3);
             if (m_wf_fc[blob][s][sg] < 0) wf3d = false;      // driver refused the permuted view: one op per slab instead
@@ -1094,46 +1111,56 @@ int build_plan(UmNet* n) {
             if (m_wd_fc[s][sg] < 0) return DZ_EINVAL;
           }
         }
-    // ---- forward: D[n, m] = sum_k W[k][n] x[m][k];  noisy: W = Wmu + Wsigma * (eps_in[k] * eps_out[n]) formed by the converters
+    // ---- forward: D[n, m] = sum_k W[k][n] x[m][k];  noisy: W = Wmu + Wsigma * (eps_in[k] * eps_out[n]), formed in the
+    // MMA warps (umma_fc_kernel; with fc_per_pass by the converter warps of umma_gemm_kernel)
     {
       UmOperand Bo = um_kmajor(njt, true, false);
       const int nk = feat / 32, S = n->fc_splits, per = (nk + S - 1) / S;
       n->l_fc.cta0 = (int)pl.ctas.size(); n->l_fc.njt = njt;
       n->l_fc.stage_bytes = 2 * 16384 + 2 * Bo.part_bytes;
+      for (int k = 0; k < ngrp; ++k)
+        n->l_fc.stage_bytes = std::max<uint32_t>(n->l_fc.stage_bytes, 2 * 16384 / grp_n[k] + grp_n[k] * 2 * Bo.part_bytes);
       n->l_fc.stages = std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_fc.stage_bytes));
-      for (int p = 0; p < d.npass; ++p) {
-        const int blob = d.pass_target[p] ? 1 : 0;
+      for (int k = 0; k < ngrp; ++k) {
+        const int blob = grp_blob[k], np = grp_n[k], rows = fc_rows[blob], slabs = rows / 32;
+        const UmOperand A = um_mnmajor(rows, 32, true, nullptr);
+        const uint32_t a_bytes = 2 * A.part_bytes;
         for (int s = 0; s < d.nstream; ++s) {
-          const int qi = p * d.nstream + s;
-          UmProblem pr;
-          memset(&pr, 0, sizeof(pr));
-          pr.A = um_mnmajor(128, 32, true, nullptr); pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32;
-          if (d.noisy) pr.A.convert = 2;
-          pr.epi = UM_EPI_PARTIAL; pr.MI = 512; pr.NJ = B;
-          pr.C = n->fc_part + (int64_t)qi * S * B * 512; pr.sc_i = 1; pr.sc_j = 512; pr.split_stride = (long long)B * 512;
-          const int prob = (int)pl.probs.size();
-          pl.probs.push_back(pr);
-          if (d.noisy) {
-            n->patches.push_back({prob, 0, (int64_t)d.noise_apply[p] * d.noise_stride + d.noise_off_in[s]});
-            n->patches.push_back({prob, 2, (int64_t)d.noise_apply[p] * d.noise_stride + d.noise_off_out[s]});
+          const int prob0 = (int)pl.probs.size();
+          for (int gp = 0; gp < np; ++gp) {
+            const int p = grp[k][gp], qi = p * d.nstream + s;
+            UmProblem pr;
+            memset(&pr, 0, sizeof(pr));
+            pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32;
+            if (d.noisy) pr.A.convert = 2;
+            pr.epi = UM_EPI_PARTIAL; pr.MI = 512; pr.NJ = B;
+            pr.C = n->fc_part + (int64_t)qi * S * B * 512; pr.sc_i = 1; pr.sc_j = 512; pr.split_stride = (long long)B * 512;
+            const int prob = (int)pl.probs.size();
+            pl.probs.push_back(pr);
+            if (d.noisy) {
+              n->patches.push_back({prob, 0, (int64_t)d.noise_apply[p] * d.noise_stride + d.noise_off_in[s]});
+              n->patches.push_back({prob, 2, (int64_t)d.noise_apply[p] * d.noise_stride + d.noise_off_out[s]});
+            }
           }
-          // the four 128-column tiles of one k range sit in neighbouring CTAs: together they stream whole 2 KB rows of W
+          // the column tiles of one k range sit in neighbouring CTAs: together they stream whole 2 KB rows of W
           for (int sp = 0; sp < S; ++sp)
-            for (int nt = 0; nt < 4; ++nt) {
+            for (int nt = 0; nt < 512 / rows; ++nt) {
               const int k0 = sp * per, k1 = std::min(nk, k0 + per);
               if (k1 <= k0) continue;
               UmCta c;
               memset(&c, 0, sizeof(c));
-              c.prob = (uint32_t)prob; c.op0 = (uint32_t)pl.ops.size(); c.nstages = (uint32_t)(k1 - k0);
-              c.ops_per_stage = (wf3d ? 1 : 4) * (d.noisy ? 2 : 1) + 2;
-              c.tx_bytes = (uint32_t)((d.noisy ? 32768 : 16384) + 2 * njt * 128);
-              c.r0 = 32 * k0; c.i0 = nt * 128; c.split = sp;
+              c.prob = (uint32_t)prob0; c.nprob = (uint32_t)np; c.op0 = (uint32_t)pl.ops.size(); c.nstages = (uint32_t)(k1 - k0);
+              c.ops_per_stage = (wf3d ? 1 : slabs) * q + 2 * np;
+              c.tx_bytes = (uint32_t)(q * A.part_bytes + np * 2 * njt * 128);
+              c.r0 = 32 * k0; c.i0 = nt * rows; c.split = sp;
               for (int ks = k0; ks < k1; ++ks) {
-                for (int sg = 0; sg < (d.noisy ? 2 : 1); ++sg) {
-                  if (wf3d) push_op(pl, m_wf_fc[blob][s][sg], sg * 16384, 0, 32 * ks, nt * 4, 0, 0);
-                  else for (int sl = 0; sl < 4; ++sl) push_op(pl, m_wf_fc[blob][s][sg], sg * 16384 + sl * 4096, nt * 128 + 32 * sl, 32 * ks, 0, 0, 0);
+                for (int sg = 0; sg < q; ++sg) {
+                  if (wf3d) push_op(pl, m_wf_fc[blob][s][sg], sg * A.part_bytes, 0, 32 * ks, nt * slabs, 0, 0);
+                  else for (int sl = 0; sl < slabs; ++sl) push_op(pl, m_wf_fc[blob][s][sg], sg * A.part_bytes + sl * 4096, nt * rows + 32 * sl, 32 * ks, 0, 0, 0);
                 }
-                for (int part = 0; part < 2; ++part) push_op(pl, m_x[part], 32768 + part * Bo.part_bytes, 32 * ks, p * B, 0, 0, 0);
+                for (int gp = 0; gp < np; ++gp)
+                  for (int part = 0; part < 2; ++part)
+                    push_op(pl, m_x[part], a_bytes + (gp * 2 + part) * Bo.part_bytes, 32 * ks, grp[k][gp] * B, 0, 0, 0);
               }
               pl.ctas.push_back(c);
             }
@@ -1208,10 +1235,12 @@ int64_t um_net_workspace_bytes(const UmNetDesc& d) {
   return carve_net(&tmp, nullptr);
 }
 
-int um_net_create(const UmNetDesc& d, char* base, UmNet** out) {
+namespace {
+int net_create(const UmNetDesc& d, char* base, UmNet** out, bool fc_per_pass) {
   if (!um_net_supported(d)) return fail(DZ_EINVAL, "geometry not supported by the tensor-core path");
   UmNet* n = new UmNet();
   n->d = d;
+  n->fc_per_pass = fc_per_pass;
   carve_net(n, base);
   // conv1 geometry
   const int px = n->h1 * n->w1, m_pass = d.B * px;
@@ -1249,6 +1278,9 @@ int um_net_create(const UmNetDesc& d, char* base, UmNet** out) {
   *out = n;
   return DZ_OK;
 }
+}  // namespace
+
+int um_net_create(const UmNetDesc& d, char* base, UmNet** out) { return net_create(d, base, out, false); }
 
 void um_net_trace(UmNet* n, const char* tag, long long* d_trace) { n->trace_tag = tag ? tag : ""; n->trace_ptr = d_trace; }
 
@@ -1404,3 +1436,58 @@ int um_backward_conv3(UmNet* n, void* stream) { return n->plan.launch("conv3_dgr
 int um_backward_conv2(UmNet* n, void* stream) { return n->plan.launch("conv2_dgrad", n->l_dconv2, stream, n->tr("conv2_dgrad")); }
 
 }  // namespace dz
+
+using namespace dz;
+
+// Test hook: the fc1 / noisy1 forward launch alone, on features x [npass * B][feat] (feat from the H x W observation
+// geometry), with the learner's pass layout for npass 1, 2 or 3 (passes 0 and 1 apply the online blob when npass is 3;
+// otherwise pass 0 is online and pass 1 target).  Stream s reads the weights at online / target + off_w[s] (mu) and
+// + off_sw[s] (sigma, noisy); pass p's noise is apply p: eps_in / eps_out of stream s at noise + p * noise_stride +
+// off_in[s] / off_out[s].  per_pass = 0: the learner's plan on umma_fc_kernel; 1: one CTA group per pass with 128-column
+// tiles on umma_gemm_kernel and its converter warps.  Writes the split partials [npass][nstream][S][B][512] to d_part
+// (room for npass * nstream * 24 * B * 512 floats), S to *splits and the weight-tile bytes the launch stages to
+// *weight_bytes.
+extern "C" int dz_test_fc_forward(int32_t B, int32_t H, int32_t W, int32_t npass, int32_t nstream, int32_t noisy, const float* online,
+                                  const float* target, const int64_t* off_w, const int64_t* off_sw, const float* noise,
+                                  int64_t noise_stride, const int64_t* off_in, const int64_t* off_out, const float* x, int32_t per_pass,
+                                  float* d_part, int32_t* splits, int64_t* weight_bytes, void* stream) {
+  if (nstream < 1 || nstream > 2 || npass < 1 || npass > 3) return fail(DZ_EINVAL, "fc forward test: npass 1..3, nstream 1..2");
+  UmNetDesc d;
+  memset(&d, 0, sizeof(d));
+  d.B = B; d.H = H; d.W = W; d.npass = npass;
+  d.pass_target[0] = 0; d.pass_target[1] = npass == 3 ? 0 : 1; d.pass_target[2] = 1;
+  d.online = online; d.target = target;
+  d.use_fc = 1; d.nstream = nstream; d.noisy = noisy ? 1 : 0;
+  for (int s = 0; s < nstream; ++s) {
+    d.off_fc_w[s] = off_w[s];
+    if (noisy) { d.off_fc_sw[s] = off_sw[s]; d.noise_off_in[s] = off_in[s]; d.noise_off_out[s] = off_out[s]; }
+  }
+  for (int p = 0; p < 3; ++p) d.noise_apply[p] = p;
+  d.noise_stride = noise_stride;
+  if (!um_net_supported(d)) return fail(DZ_EINVAL, "fc forward test: geometry not supported by the tensor-core path");
+  char* ws = nullptr;
+  DZ_CUDA_OK(cudaMalloc(&ws, (size_t)um_net_workspace_bytes(d)));
+  UmNet* n = nullptr;
+  int rc = net_create(d, ws, &n, per_pass != 0);
+  if (rc == DZ_OK) rc = um_split(x, n->act_hi[2], n->act_lo[2], (long long)n->PB * n->feat, stream);
+  if (rc == DZ_OK && noisy) rc = apply_noise(n, noise, stream);
+  if (rc == DZ_OK) rc = n->plan.launch("fc1_fwd", n->l_fc, stream, nullptr, per_pass ? UM_PATH_CONVERTERS : UM_PATH_AUTO);
+  if (rc == DZ_OK) {
+    const size_t bytes = (size_t)npass * nstream * n->fc_splits * B * 512 * sizeof(float);
+    if (cudaMemcpyAsync(d_part, n->fc_part, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream) != cudaSuccess ||
+        cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess)
+      rc = fail(DZ_ECUDA, "fc forward test: %s", cudaGetErrorString(cudaGetLastError()));
+  }
+  if (rc == DZ_OK) {
+    *splits = n->fc_splits;
+    int64_t wb = 0;
+    for (int ci = n->l_fc.cta0; ci < n->l_fc.cta0 + n->l_fc.nctas; ++ci) {
+      const UmCta& c = n->plan.ctas[ci];
+      wb += (int64_t)c.nstages * (noisy ? 2 : 1) * n->plan.probs[c.prob].A.part_bytes;
+    }
+    *weight_bytes = wb;
+  }
+  if (n) um_net_destroy(n);
+  cudaFree(ws);
+  return rc;
+}

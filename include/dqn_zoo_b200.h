@@ -413,6 +413,15 @@ int dz_test_umma_gemm(const float* d_A, int32_t a_mn_major, const float* d_B, in
 int dz_test_umma_gemm_path(const float* d_A, int32_t a_mn_major, const float* d_B, int32_t b_mn_major, int32_t MI, int32_t NJ,
                            int32_t R, int32_t convert, const float* d_scale_r, int32_t stages, int32_t epi_rows,
                            const float* d_bias, int32_t relu, float* d_C, float* d_hi, float* d_lo, int32_t path, void* stream);
+/* The fc1 / noisy1 forward launch alone (split partials [npass][nstream][S][B][512] of features x [npass * B][feat]
+ * against the stream weights at online / target + off_w[s] (mu) and + off_sw[s] (sigma), noise apply p = pass p).
+ * per_pass = 0: the learner's plan (passes that apply one blob share each staged weight tile, umma_fc_kernel); 1: one CTA
+ * group per pass on umma_gemm_kernel with converter warps.  *weight_bytes: weight-tile bytes the launch stages.
+ * d_part holds npass * nstream * 24 * B * 512 floats.  Synchronizes. */
+int dz_test_fc_forward(int32_t B, int32_t H, int32_t W, int32_t npass, int32_t nstream, int32_t noisy, const float* online,
+                       const float* target, const int64_t* off_w, const int64_t* off_sw, const float* noise, int64_t noise_stride,
+                       const int64_t* off_in, const int64_t* off_out, const float* x, int32_t per_pass, float* d_part,
+                       int32_t* splits, int64_t* weight_bytes, void* stream);
 
 #ifdef __cplusplus
 }
