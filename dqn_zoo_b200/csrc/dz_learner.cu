@@ -2581,16 +2581,17 @@ int dz_learner_sync_target(dz_learner* l, void* stream) {
   return DZ_OK;
 }
 
-// Debug hook: the tensor-core launch named `tag` ("conv2_fwd", "conv3_fwd", "fc1_fwd", "fc1_dgrad", "conv3_dgrad", "conv2_dgrad",
-// "conv3_wgrad", "conv2_wgrad") writes the clock stamps of its CTA 0 into d_trace (512 int64); nullptr switches it off.
+// Debug hook: the tensor-core launch named `tag` ("conv1_fwd", "conv2_fwd", "conv3_fwd", "fc1_fwd", "fc1_dgrad", "conv3_dgrad",
+// "conv2_dgrad", "conv3_wgrad", "conv2_wgrad") writes the clock stamps of its CTA 0 into d_trace (512 int64); nullptr switches
+// it off.  conv1_fwd stamps per output tile, the others per shared-memory stage (tools/umma_stage_trace.py reads both).
 int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace) {
   if (!l->um) return fail(DZ_EINVAL, "the tensor-core path is not active for this learner");
   um_net_trace(l->um, tag, d_trace);
   return DZ_OK;
 }
 
-// Test hook: the MMA path of the tensor-core launch named `tag` (the tags of dz_test_learner_trace): 1 warp-level
-// mma.sync kernel, 2 wgmma kernel.
+// Test hook: the MMA path of the tensor-core launch named `tag` (the tags of dz_test_learner_trace, conv1_fwd included):
+// 1 warp-level mma.sync kernel, 2 wgmma kernel.
 int dz_test_learner_mma_path(dz_learner* l, const char* tag, int32_t* path) {
   if (!l->um) return fail(DZ_EINVAL, "the tensor-core path is not active for this learner");
   const int p = um_net_mma_path(l->um, tag);

@@ -137,6 +137,32 @@ __device__ __forceinline__ void wgmma_kstep_3xtf32(float (&d)[NA], uint32_t a_hi
   wgmma_fence_acc(d);
 }
 
+// D (m64 x 32, fp32) = A * B^T (+ D when scale_d != 0) with A from registers: the warp's 16 rows of the warpgroup's
+// 64, a = {A[g][t], A[g + 8][t], A[g][t + 4], A[g + 8][t + 4]} (g = lane / 4, t = lane % 4, the m16n8k8 A layout).
+__device__ __forceinline__ void wgmma_m64k8(float (&d)[16], const uint32_t (&a)[4], uint64_t db, int scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+
+// One k-step of 8 as one wgmma group when A is exact (no lo part) and held in registers:  d = A*Bl, d += A*Bh — the
+// products and order of warp_mma_3xtf32 with a_has_lo = false.  B: K-major SWIZZLE_128B hi/lo tiles at shared
+// addresses b_hi / b_lo, k0: first reduction element.  The caller keeps `a` unchanged until the group is retired.
+__device__ __forceinline__ void wgmma_kstep_exact_a(float (&d)[16], const uint32_t (&a)[4], uint32_t b_hi, uint32_t b_lo, int k0) {
+  const uint32_t ko = (uint32_t)k0 * 4u;
+  const uint64_t bh = wgmma_desc_sw128(b_hi + ko), bl = wgmma_desc_sw128(b_lo + ko);
+  wgmma_fence_acc(d);
+  wgmma_fence();
+  wgmma_m64k8(d, a, bl, 0);
+  wgmma_m64k8(d, a, bh, 1);
+  wgmma_commit();
+  wgmma_fence_acc(d);
+}
+
 // Row / column of D that element e of fragment (mt, nt) of warp_kstep_3xtf32 holds, relative to (m0, n0).
 __device__ __forceinline__ int frag_row(int mt, int e) { return mt * 16 + ((threadIdx.x & 31) >> 2) + (e >> 1) * 8; }
 __device__ __forceinline__ int frag_col(int nt, int e) { return nt * 8 + 2 * (threadIdx.x & 3) + (e & 1); }

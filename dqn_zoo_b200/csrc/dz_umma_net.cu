@@ -102,10 +102,12 @@ __global__ void __launch_bounds__(256) um_pack_conv_kernel(const __grid_constant
 // ------------------------------------------------------------------------------------------------
 // conv1: 8x8 stride 4 over the sampled uint8 observations, read IN PLACE from the replay store (the gather of
 // replay.py:718-722 is this kernel's operand load).  Per 128-pixel output tile: one thread bulk-copies the
-// contiguous input rows the tile needs (cp.async.bulk, <= 4 segments) into a double-buffered staging area;
-// eight converter warps expand the bytes to exact tf32 values in the swizzled K-major A tile (K = 256 = 8 kernel
-// rows x 32); four MMA warps (32 output pixels each) multiply it with the resident weight image (hi/lo), add the
-// bias, ReLU and write act1 as tf32 hi/lo.
+// contiguous input rows the tile needs (cp.async.bulk, <= 4 segments) into a double-buffered staging area; the
+// bytes become exact tf32 values (K = 256 = 8 kernel rows x 32 (kw, c)) that the MMA warps multiply with the resident
+// weight image (hi/lo); the bias, ReLU and tf32 hi/lo split of act1 follow.  conv1_wgmma_kernel (the learner's) forms
+// the A fragments from the staged bytes in the registers of two MMA warpgroups; conv1_umma_kernel, with eight
+// converter warps writing a swizzled A tile for four warps' mma.sync, is kept as the reference it is tested against
+// bit for bit (dz_test_conv1_forward).
 // ------------------------------------------------------------------------------------------------
 struct Conv1Args {
   CUtensorMap wmap[2][2];          // weight image [blob][hi / lo] (grid-constant: descriptor fetch from the constant bank)
@@ -318,6 +320,189 @@ __global__ void __launch_bounds__(kThreadsU, 1) conv1_umma_kernel(const __grid_c
       __syncwarp();
       if (lane == 0) mbar_arrive(&raw_empty[buf]);
     }
+  }
+  if (tr && threadIdx.x == 0) a.trace[322] = clock64();
+}
+
+// Warpgroup-MMA conv1.  Producer (row copies, weight image), weight-image layout, epilogue, PDL points and clock-stamp
+// slots are those of conv1_umma_kernel; there are no converter warps and no A tile in shared memory.  Warp roles:
+// 0 producer | 1 barrier set-up | 2-3 idle | warpgroup 1 (warps 4-7) D rows [0, 64) of the tile, warpgroup 2 (warps
+// 8-11) rows [64, 128), all 32 channels.
+constexpr int kThreadsC1W = 12 * 32;
+// Scratch accumulators a warpgroup rotates through (one MMA group each), as wgmma_gemm_kernel's acc0 / acc1.  Four
+// measured no faster than two in the in-graph tile trace.
+constexpr int kC1Groups = 2;
+
+__global__ void __launch_bounds__(kThreadsC1W, 1) conv1_wgmma_kernel(const __grid_constant__ Conv1Args a) {
+  if (threadIdx.x < 4) prefetch_tensormap(&a.wmap[threadIdx.x >> 1][threadIdx.x & 1]);
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + smem_pad_1024(smem_raw);
+  uint64_t* raw_full = reinterpret_cast<uint64_t*>(smem);   // [2] staged input rows landed
+  uint64_t* raw_empty = raw_full + 2;                        // [2] the 8 MMA warps retired every group of the tile staged there
+  uint64_t* w_full = raw_empty + 2;                          // [1] weight image landed (only reloaded when the pass changes)
+  uint8_t* w_smem = smem + 1024;
+  uint8_t* stag = w_smem + kC1W;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp == 1 && lane == 0) {
+    for (int b = 0; b < 2; ++b) { mbar_init(&raw_full[b], 1); mbar_init(&raw_empty[b], kConsumerWarps); }
+    mbar_init(w_full, 1);
+    fence_mbarrier_init();
+  }
+  __syncthreads();
+  dz::pdl_enter();                        // set-up above overlaps the previous kernel's tail; data accesses start here
+  const bool tr = a.trace != nullptr && blockIdx.x == 0;
+  if (tr && threadIdx.x == 0) { a.trace[323] = clock64(); a.trace[324] = clock64(); }
+
+  const int px = a.oh * a.ow;             // output pixels per image
+  const int row_bytes = a.W * 4;          // one input row of 4-channel pixels
+  const int t_begin = (int)(((long long)blockIdx.x * a.ntiles) / gridDim.x);
+  const int t_end = (int)(((long long)(blockIdx.x + 1) * a.ntiles) / gridDim.x);
+
+  if (warp == 0) {
+    // ---------------------------------------------------------------- producer
+    int cur_pass = -1;
+    for (int tile = t_begin, n = 0; tile < t_end; ++tile, ++n) {
+      const int buf = n & 1;
+      const int pass = tile / a.tiles_per_pass;
+      const int m0 = (tile - pass * a.tiles_per_pass) * 128, m1 = min(m0 + 128, a.m_pass);
+      mbar_wait(&raw_empty[buf], (((uint32_t)n >> 1) & 1u) ^ 1u);
+      if (elect_one()) {
+        conv1_stage_tile(a.rows[pass], m0, m1, px, a.ow, row_bytes, smem_u32(stag + (size_t)buf * a.stag_bytes), &raw_full[buf]);
+        if (tr && n < 64) a.trace[n] = clock64();                                                   // [0,64): row copies issued
+      }
+      __syncwarp();
+      if (pass != cur_pass) {
+        // the previous tile's MMAs are done with the old image
+        if (n > 0) mbar_wait(&raw_empty[(n - 1) & 1], ((uint32_t)(n - 1) >> 1) & 1u);
+        if (elect_one()) {
+          mbar_expect_tx(w_full, (uint32_t)kC1W);
+#pragma unroll
+          for (int q = 0; q < 16; ++q) {
+            const int part = q >> 3, s = q & 7;
+            tma_load_5d(smem_u32(w_smem) + part * 32768 + s * 4096, &a.wmap[a.blob[pass]][part], w_full, 32 * s, 0, 0, 0, 0);
+          }
+        }
+        cur_pass = pass;
+      }
+      __syncwarp();
+    }
+  } else if (warp >= 4) {
+    // ---------------------------------------------------------------- MMA warpgroups + epilogue
+    // Warpgroup wg: D rows [64 wg, 64 wg + 64) of the tile; this warp's rows r0 and r0 + 8 (plus lane / 4).  A comes
+    // from registers: for kernel row kh, thread (g, t) reads the two staged 32-byte kernel rows (8 pixels x 4 channels)
+    // of its output pixels and expands byte t of every pixel to an exact float.  k-step s of kernel row kh covers
+    // (kw, c) = (2s, 0..3), (2s + 1, 0..3), so a = {X[r0][2s][t], X[r0 + 8][2s][t], X[r0][2s + 1][t], X[r0 + 8][2s + 1][t]}:
+    // the wgmma A fragment.  W slab kh = [32 n][32 (kw, c)] at w_smem + 4096 kh, hi | lo 32 KB apart, K-major
+    // SWIZZLE_128B, is read through descriptors.  Every k-step is one group into a scratch accumulator; kC1Groups of them
+    // rotate, and k-step k is retired (wgmma_wait) and added into the sums once k + kC1Groups - 1 has been issued, so
+    // the sums still take the k-steps in order.  The A registers of kernel rows kh and kh + 1 are separate, and every
+    // group of kernel row kh - 1 is retired before row kh + 1 is expanded, so no group in flight reads a register
+    // being written.  A tile's 32 k-steps are straight-line code and its last group is retired
+    // before raw_empty, so no group is in flight across a barrier wait, a branch or a loop edge.  The values the loop
+    // branches on are broadcast from lane 0 so that ptxas sees them warp-uniform.
+    const int wg = __shfl_sync(0xffffffffu, (warp >> 2) - 1, 0);
+    const bool lead = warp == 4 && lane == 0;
+    const uint32_t w_base = smem_u32(w_smem);
+    const int t = lane & 3, c0 = 2 * t;
+    const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    const uint32_t sel = 0x7440u + (uint32_t)t;   // byte t of a word -> low byte of 0x4B0000xx
+    float acc[kC1Groups][16];
+#pragma unroll
+    for (int q = 0; q < kC1Groups; ++q)
+#pragma unroll
+      for (int e = 0; e < 16; ++e) acc[q][e] = 0.f;
+    int cur_pass = -1, wn = 0;
+    for (int tile = t_begin, n = 0; tile < t_end; ++tile, ++n) {
+      const int buf = n & 1;
+      const int pass = tile / a.tiles_per_pass;
+      const int m0 = (tile - pass * a.tiles_per_pass) * 128, m1 = min(m0 + 128, a.m_pass);
+      // an m64 half with no valid pixel issues no MMAs (it still releases the staging buffer)
+      const bool active = __shfl_sync(0xffffffffu, (int)(m0 + 64 * wg < m1), 0) != 0;
+      // staged offsets of this thread's two pixels; a pixel beyond the batch reads offset 0 and is masked to zeros
+      const int ma = m0 + r0, mb = ma + 8;
+      const uint32_t mask_a = ma < m1 ? 0xffffffffu : 0u, mask_b = mb < m1 ? 0xffffffffu : 0u;
+      const int off_a = ma < m1 ? conv1_stage_offset(ma, m0, m1, px, a.ow, row_bytes) : 0;
+      const int off_b = mb < m1 ? conv1_stage_offset(mb, m0, m1, px, a.ow, row_bytes) : 0;
+      if (pass != cur_pass) { mbar_wait(w_full, (uint32_t)wn & 1u); ++wn; cur_pass = pass; }
+      float sum[16];
+      {   // the bias is the initial value of the sums
+        const float* __restrict__ bias = a.bias[pass];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float2 b2 = *reinterpret_cast<const float2*>(bias + 8 * i + c0);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) { sum[4 * i + 2 * h] = b2.x; sum[4 * i + 2 * h + 1] = b2.y; }
+        }
+      }
+      auto retire = [&](float (&d)[16]) {
+        wgmma_fence_acc(d);
+#pragma unroll
+        for (int e = 0; e < 16; ++e) sum[e] += d[e];
+      };
+      mbar_wait(&raw_full[buf], ((uint32_t)n >> 1) & 1u);
+      if (tr && lead && n < 64) a.trace[64 + n] = clock64();                                       // [64,128): input rows landed
+      if (active) {
+        const uint8_t* src_a = stag + (size_t)buf * a.stag_bytes + off_a;
+        const uint8_t* src_b = stag + (size_t)buf * a.stag_bytes + off_b;
+        uint32_t x[2][4][4];   // [kh & 1][k-step][fragment element]
+#pragma unroll
+        for (int kh = 0; kh < 8; ++kh) {
+          const uint4 ua0 = *reinterpret_cast<const uint4*>(src_a + kh * row_bytes);
+          const uint4 ua1 = *reinterpret_cast<const uint4*>(src_a + kh * row_bytes + 16);
+          const uint4 ub0 = *reinterpret_cast<const uint4*>(src_b + kh * row_bytes);
+          const uint4 ub1 = *reinterpret_cast<const uint4*>(src_b + kh * row_bytes + 16);
+          const uint32_t wa[8] = {ua0.x, ua0.y, ua0.z, ua0.w, ua1.x, ua1.y, ua1.z, ua1.w};
+          const uint32_t wb[8] = {ub0.x, ub0.y, ub0.z, ub0.w, ub1.x, ub1.y, ub1.z, ub1.w};
+          // 0x4B000000 | byte = 8388608 + byte exactly; subtracting 2^23 leaves the byte as a float (an exact tf32 number)
+          auto expand = [&](uint32_t w, uint32_t mask) {
+            return __float_as_uint(__uint_as_float(__byte_perm(w & mask, 0x4B000000u, sel)) - 8388608.0f);
+          };
+#pragma unroll
+          for (int s = 0; s < 4; ++s) {
+            x[kh & 1][s][0] = expand(wa[2 * s], mask_a);
+            x[kh & 1][s][1] = expand(wb[2 * s], mask_b);
+            x[kh & 1][s][2] = expand(wa[2 * s + 1], mask_a);
+            x[kh & 1][s][3] = expand(wb[2 * s + 1], mask_b);
+          }
+          const uint32_t w = w_base + 4096u * (uint32_t)kh;
+#pragma unroll
+          for (int s = 0; s < 4; ++s) {
+            const int ks = 4 * kh + s;
+            wgmma_kstep_exact_a(acc[ks % kC1Groups], x[kh & 1][s], w, w + 32768u, 8 * s);
+            if (ks >= kC1Groups - 1) {
+              wgmma_wait<kC1Groups - 1>();
+              retire(acc[(ks + 1) % kC1Groups]);
+            }
+          }
+        }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int ks = 33 - kC1Groups; ks < 32; ++ks) retire(acc[ks % kC1Groups]);
+      }
+      mbar_arrive_if(&raw_empty[buf], lane == 0);
+      if (lead && tile == t_end - 1) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+      if (tr && lead && n < 64) a.trace[192 + n] = clock64();                                      // [192,256): tile's MMAs done
+      // Each store instruction writes eight rows x 32 contiguous bytes of act1 (full sectors).
+      const long long dst0 = ((long long)pass * a.m_pass + m0) * 32;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = r0 + 8 * h;
+        if (m0 + row >= m1) continue;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float v0 = fmaxf(sum[4 * i + 2 * h], 0.f), v1 = fmaxf(sum[4 * i + 2 * h + 1], 0.f);
+          float h0, l0, h1, l1;
+          split_tf32(v0, h0, l0);
+          split_tf32(v1, h1, l1);
+          const long long o = dst0 + row * 32 + 8 * i + c0;
+          *reinterpret_cast<float2*>(a.out_hi + o) = make_float2(h0, h1);
+          *reinterpret_cast<float2*>(a.out_lo + o) = make_float2(l0, l1);
+        }
+      }
+      if (tr && lead && n < 64) a.trace[256 + n] = clock64();                                      // [256,320): tile stored
+    }
+    if (t_begin >= t_end && lead) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   }
   if (tr && threadIdx.x == 0) a.trace[322] = clock64();
 }
@@ -1269,9 +1454,10 @@ int net_create(const UmNetDesc& d, char* base, UmNet** out, bool fc_per_pass) {
   static bool configured = false;
   if (!configured) {
     if (cudaFuncSetAttribute(conv1_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
+        cudaFuncSetAttribute(conv1_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
         cudaFuncSetAttribute(conv1_wgrad_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess) {
       um_net_destroy(n);
-      return fail(DZ_ECUDA, "conv1_umma_kernel shared memory attribute");
+      return fail(DZ_ECUDA, "conv1 kernels: shared memory attribute");
     }
     configured = true;
   }
@@ -1286,6 +1472,7 @@ void um_net_trace(UmNet* n, const char* tag, long long* d_trace) { n->trace_tag 
 
 int um_net_mma_path(UmNet* n, const char* tag) {
   const std::string t = tag ? tag : "";
+  if (t == "conv1_fwd") return UM_PATH_WGMMA;     // conv1_wgmma_kernel (um_forward_torso)
   const UmLaunch* l = t == "conv2_fwd" ? &n->l_conv2 : t == "conv3_fwd" ? &n->l_conv3 : t == "conv3_dgrad" ? &n->l_dconv3
                     : t == "conv2_dgrad" ? &n->l_dconv2 : (t == "fc1_fwd" || t == "noisy1_fwd") ? &n->l_fc
                     : (t == "fc1_dgrad" || t == "noisy1_dgrad") ? &n->l_fcd : t == "conv3_wgrad" ? &n->l_wconv3
@@ -1325,7 +1512,9 @@ int um_pack_weights(UmNet* n, void* stream) {
   return DZ_OK;
 }
 
-int um_forward_torso(UmNet* n, const uint8_t* const* const* rows, void* stream) {
+namespace {
+// conv1 forward into act1 hi / lo; reference: conv1_umma_kernel instead of the learner's conv1_wgmma_kernel (tests only).
+int launch_conv1(UmNet* n, const uint8_t* const* const* rows, void* stream, bool reference) {
   const UmNetDesc& d = n->d;
   Conv1Args a;
   memset(&a, 0, sizeof(a));
@@ -1341,10 +1530,17 @@ int um_forward_torso(UmNet* n, const uint8_t* const* const* rows, void* stream) 
   a.npass = d.npass; a.B = d.B; a.W = d.W; a.oh = n->h1; a.ow = n->w1; a.m_pass = d.B * n->h1 * n->w1;
   a.tiles_per_pass = n->conv1_tiles_per_pass; a.ntiles = a.tiles_per_pass * d.npass; a.stag_bytes = n->conv1_stag_bytes;
   a.trace = n->tr("conv1_fwd");
-  const size_t smem = 2048 + kC1W + kC1A + 2 * (size_t)a.stag_bytes;
+  const size_t smem = 2048 + kC1W + (reference ? kC1A : 0) + 2 * (size_t)a.stag_bytes;   // conv1_wgmma_kernel has no A tile
   if (smem > 227 * 1024) return fail(DZ_EINVAL, "conv1 staging does not fit");
   const unsigned grid = (unsigned)std::min(kNumSMs, a.ntiles);
-  DZ_LAUNCH_NAMED("conv1_fwd", conv1_umma_kernel, grid, kThreadsU, smem, stream, a);
+  if (reference) DZ_LAUNCH_NAMED("conv1_fwd", conv1_umma_kernel, grid, kThreadsU, smem, stream, a);
+  else DZ_LAUNCH_NAMED("conv1_fwd", conv1_wgmma_kernel, grid, kThreadsC1W, smem, stream, a);
+  return DZ_OK;
+}
+}  // namespace
+
+int um_forward_torso(UmNet* n, const uint8_t* const* const* rows, void* stream) {
+  DZ_TRY(launch_conv1(n, rows, stream, false));
   DZ_TRY(n->plan.launch("conv2_fwd", n->l_conv2, stream, n->tr("conv2_fwd")));
   DZ_TRY(n->plan.launch("conv3_fwd", n->l_conv3, stream, n->tr("conv3_fwd")));
   return DZ_OK;
@@ -1486,6 +1682,42 @@ extern "C" int dz_test_fc_forward(int32_t B, int32_t H, int32_t W, int32_t npass
       wb += (int64_t)c.nstages * (noisy ? 2 : 1) * n->plan.probs[c.prob].A.part_bytes;
     }
     *weight_bytes = wb;
+  }
+  if (n) um_net_destroy(n);
+  cudaFree(ws);
+  return rc;
+}
+
+// Test hook: the conv1 forward launch alone, on the uint8 observations of B x H x W x 4 (rows[p]: host array of the
+// npass device row-pointer tables, one observation per pointer), with the pass layout of dz_test_fc_forward (passes 0
+// and 1 apply the online blob when npass is 3; otherwise pass 0 is online and pass 1 target).  The conv weights of
+// both blobs are at off_conv_w[0..2] (all three layers are packed), conv1's bias at off_conv_b1.  path: 2 the
+// learner's conv1_wgmma_kernel, 1 the mma.sync conv1_umma_kernel.  Writes act1 hi / lo [npass * B][h1][w1][32].
+extern "C" int dz_test_conv1_forward(int32_t B, int32_t H, int32_t W, int32_t npass, const float* online, const float* target,
+                                     const int64_t* off_conv_w, int64_t off_conv_b1, const uint8_t* const* const* rows,
+                                     int32_t path, float* d_hi, float* d_lo, void* stream) {
+  if (npass < 1 || npass > 3) return fail(DZ_EINVAL, "conv1 forward test: npass 1..3");
+  if (path != UM_PATH_MMA_SYNC && path != UM_PATH_WGMMA) return fail(DZ_EINVAL, "conv1 forward test: path 1 (mma.sync) or 2 (wgmma)");
+  UmNetDesc d;
+  memset(&d, 0, sizeof(d));
+  d.B = B; d.H = H; d.W = W; d.npass = npass;
+  d.pass_target[0] = 0; d.pass_target[1] = npass == 3 ? 0 : 1; d.pass_target[2] = 1;
+  d.online = online; d.target = target;
+  for (int L = 0; L < 3; ++L) d.off_conv_w[L] = off_conv_w[L];
+  d.off_conv_b[0] = off_conv_b1;
+  if (!um_net_supported(d)) return fail(DZ_EINVAL, "conv1 forward test: geometry not supported by the tensor-core path");
+  char* ws = nullptr;
+  DZ_CUDA_OK(cudaMalloc(&ws, (size_t)um_net_workspace_bytes(d)));
+  UmNet* n = nullptr;
+  int rc = net_create(d, ws, &n, false);
+  if (rc == DZ_OK) rc = um_pack_weights(n, stream);
+  if (rc == DZ_OK) rc = launch_conv1(n, rows, stream, path == UM_PATH_MMA_SYNC);
+  if (rc == DZ_OK) {
+    const size_t bytes = (size_t)npass * B * n->h1 * n->w1 * 32 * sizeof(float);
+    if (cudaMemcpyAsync(d_hi, n->act_hi[0], bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream) != cudaSuccess ||
+        cudaMemcpyAsync(d_lo, n->act_lo[0], bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream) != cudaSuccess ||
+        cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess)
+      rc = fail(DZ_ECUDA, "conv1 forward test: %s", cudaGetErrorString(cudaGetLastError()));
   }
   if (n) um_net_destroy(n);
   cudaFree(ws);

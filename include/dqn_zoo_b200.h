@@ -388,7 +388,8 @@ int dz_test_learner_buffer(dz_learner* l, const char* name, float** d_ptr, int64
 int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream);   /* device-to-device, tests only */
 /* Debug: the tensor-core launch named `tag` writes the clock stamps of its CTA 0 into d_trace (512 int64). */
 int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace);
-/* Tests: which MMA path the tensor-core launch `tag` (same tags) takes: *path = 1 warp-level mma.sync, 2 wgmma. */
+/* Tests: which MMA path the tensor-core launch `tag` (same tags, and "conv1_fwd") takes: *path = 1 warp-level mma.sync,
+ * 2 wgmma. */
 int dz_test_learner_mma_path(dz_learner* l, const char* tag, int32_t* path);
 /* Debug: every kernel appends (globaltimer ns, gridDim.x << 32 | gridDim.y << 16 | blockDim.x) to d_buf right after its
  * dependencies completed; d_buf[0] (low 32 bits) counts the entries, entries start at d_buf[2].  d_buf: 2 + 2 * 4000
@@ -422,6 +423,13 @@ int dz_test_fc_forward(int32_t B, int32_t H, int32_t W, int32_t npass, int32_t n
                        const float* target, const int64_t* off_w, const int64_t* off_sw, const float* noise, int64_t noise_stride,
                        const int64_t* off_in, const int64_t* off_out, const float* x, int32_t per_pass, float* d_part,
                        int32_t* splits, int64_t* weight_bytes, void* stream);
+/* The conv1 forward launch alone: act1 tf32 hi / lo [npass * B][h1][w1][32] (into d_hi / d_lo) of the uint8
+ * observations B x H x W x 4 that rows[p] (host array of npass device tables of B row pointers) point at, pass layout as
+ * in dz_test_fc_forward.  off_conv_w: the three conv weight offsets in both blobs; off_conv_b1: conv1's bias.  path: 2 the
+ * learner's wgmma kernel, 1 the warp-level mma.sync kernel it is checked against.  Synchronizes. */
+int dz_test_conv1_forward(int32_t B, int32_t H, int32_t W, int32_t npass, const float* online, const float* target,
+                          const int64_t* off_conv_w, int64_t off_conv_b1, const uint8_t* const* const* rows, int32_t path,
+                          float* d_hi, float* d_lo, void* stream);
 
 #ifdef __cplusplus
 }

@@ -6,7 +6,12 @@ For every shared-memory stage of the launch's first CTA it prints, in SM clock c
 A launch whose `mma` column dominates is bound by the MMA loop; one whose `wait` column dominates is bound by the
 operand delivery (TMA / L2).
 
-  python tools/umma_stage_trace.py --agent rainbow --tags conv2_fwd,conv3_fwd [--graph] [--steps 8]"""
+conv1_fwd stamps per 128-pixel output tile instead (csrc/dz_umma_net.cu): for every tile of CTA 0
+  wait  = rows landed - row copies issued
+  mma   = tile's MMAs done - rows landed     (includes the byte -> tf32 conversion, which the MMAs wait for)
+  store = tile stored - tile's MMAs done    (ReLU + tf32 hi/lo epilogue)
+
+  python tools/umma_stage_trace.py --agent rainbow --tags conv1_fwd,conv2_fwd,conv3_fwd [--graph] [--steps 8]"""
 
 import argparse
 import os
@@ -21,6 +26,29 @@ import bench  # noqa: E402
 
 # clock-stamp slots written by CTA 0 of the traced launch (csrc/dz_umma.cuh)
 ISSUED, READY, CONSUMED, EPILOGUE, STORED, EXIT, ENTRY = 0, 64, 128, 320, 321, 322, 323
+# conv1_fwd's per-tile slots: row copies issued, rows landed, tile's MMAs done, tile stored (exit / entry as above)
+C1_ISSUED, C1_LANDED, C1_MMA_DONE, C1_STORED = 0, 64, 192, 256
+
+
+def tile_table(t):
+  """Per-tile (issued, landed, MMAs done, stored) stamps of conv1_fwd relative to the kernel entry, plus the exit."""
+  n = int((t[C1_ISSUED:C1_ISSUED + 64] != 0).sum())
+  t0 = int(t[ENTRY])
+  rows = [tuple(int(t[s + i]) - t0 for s in (C1_ISSUED, C1_LANDED, C1_MMA_DONE, C1_STORED)) for i in range(n)]
+  return rows, int(t[EXIT]) - t0
+
+
+def print_tiles(tag, agent, t):
+  rows, exit_ = tile_table(t)
+  if not rows:
+    print('== %s: no stamps' % tag)
+    return
+  print('== %s (%s): %d tiles | exit at %d cycles' % (tag, agent, len(rows), exit_))
+  print('  %5s %9s %9s %9s %9s %8s %8s %8s' % ('tile', 'issued', 'landed', 'mma_done', 'stored', 'wait', 'mma', 'store'))
+  for s, (i, r, m, st) in enumerate(rows):
+    print('  %5d %9d %9d %9d %9d %8d %8d %8d' % (s, i, r, m, st, r - i, m - r, st - m))
+  mma = np.array([r[2] - r[1] for r in rows])
+  print('  median mma %d cycles; first issue -> last store %d cycles' % (int(np.median(mma)), rows[-1][3] - rows[0][0]))
 
 
 def stage_table(t):
@@ -56,6 +84,9 @@ def main():
     _lib.call('dz_test_learner_trace', ag.learner._h, b'', 0)
     if a.graph:
       ag._graph = None
+    if tag == 'conv1_fwd':
+      print_tiles(tag, a.agent, tr.cpu().numpy())
+      continue
     rows, tail = stage_table(tr.cpu().numpy())
     if not rows:
       print('== %s: no stamps (is the tag a TMA-fed tensor-core launch of this agent?)' % tag)
