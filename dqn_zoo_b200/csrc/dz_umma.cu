@@ -53,7 +53,35 @@ int UmPlan::add_map(const void* base, int rank, const uint64_t* dims, const uint
     return -1;
   }
   maps.push_back(m);
+  box_bytes.push_back(bx[0] * bx[1] * bx[2] * bx[3] * bx[4] * 4);
   return (int)maps.size() - 1;
+}
+
+int UmPlan::add_map_pair(const float* hi, const float* lo, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                         const uint32_t* box, int ids[2]) {
+  ids[0] = add_map(hi, rank, dims, strides_bytes, box);
+  ids[1] = ids[0] < 0 ? -1 : add_map(lo, rank, dims, strides_bytes, box);
+  return ids[1] < 0 ? DZ_EINVAL : DZ_OK;
+}
+
+int UmPlan::end_cta() {
+  UmCta& c = ctas.back();
+  const size_t nst = stage_op0.size();
+  c.nstages = (uint32_t)nst;
+  for (size_t s = 0; s < nst; ++s) {
+    const uint32_t o1 = s + 1 < nst ? stage_op0[s + 1] : (uint32_t)ops.size();
+    uint32_t tx = 0;
+    for (uint32_t oi = stage_op0[s]; oi < o1; ++oi) {
+      const uint32_t bytes = box_bytes[ops[oi].map];
+      if (ops[oi].smem_off + bytes > build_stage_bytes) return fail(DZ_EINVAL, "umma plan: a TMA box overruns its stage");
+      tx += bytes;
+    }
+    const uint32_t nops = o1 - stage_op0[s];
+    if (nops > 32) return fail(DZ_EINVAL, "umma plan: more than 32 TMA ops in one stage");
+    if (s == 0) { c.ops_per_stage = nops; c.tx_bytes = tx; }
+    else if (nops != c.ops_per_stage || tx != c.tx_bytes) return fail(DZ_EINVAL, "umma plan: the stages of a CTA differ in TMA ops or bytes");
+  }
+  return DZ_OK;
 }
 
 int UmPlan::localize_maps(UmLaunch& l) {
@@ -151,10 +179,8 @@ int UmPlan::launch(const char* tag, const UmLaunch& l, void* stream, long long* 
     if (pr.A.nparts != 2 || pr.B.nparts != 2 || pr.B.part_bytes != want)
       return fail(DZ_EINVAL, "umma launch: operands must be hi/lo pairs and the B tile must span NJT rows");
   }
-  for (int ci = l.cta0; ci < l.cta0 + l.nctas; ++ci)
-    if (ctas[ci].ops_per_stage > 32) return fail(DZ_EINVAL, "umma launch: more than 32 TMA ops per stage");
   const int stages = l.stages;
-  const size_t smem = 1024 + um::kCtlBytes + (size_t)stages * l.stage_bytes;
+  const size_t smem = um_smem_bytes(stages, l.stage_bytes);
   if (smem > 227 * 1024) return fail(DZ_EINVAL, "umma launch needs too much shared memory");
   if ((size_t)stages * l.stage_bytes < (size_t)128 * l.njt * 4) return fail(DZ_EINVAL, "umma launch: stage buffers smaller than the store-phase staging tile");
   const int v = l.njt == 32 ? 0 : 1;
@@ -164,8 +190,8 @@ int UmPlan::launch(const char* tag, const UmLaunch& l, void* stream, long long* 
   const bool wg = path == UM_PATH_AUTO ? wgmma_eligible(l) : path == UM_PATH_WGMMA;
   if (wg && !wgmma_eligible(l)) return fail(DZ_EINVAL, "umma launch: the wgmma path needs K-major, pre-split operands and four k-steps per stage");
   if (wg)
-    for (int ci = l.cta0; ci < l.cta0 + l.nctas; ++ci)   // both m64 halves of A (hi and lo) are read from inside the stage
-      if (probs[ctas[ci].prob].A.part_bytes + 16384u > l.stage_bytes) return fail(DZ_EINVAL, "umma launch: stage too small for the wgmma A reads");
+    for (int ci = l.cta0; ci < l.cta0 + l.nctas; ++ci)
+      if (um_wgmma_min_stage(probs[ctas[ci].prob].A.part_bytes) > l.stage_bytes) return fail(DZ_EINVAL, "umma launch: stage too small for the wgmma A reads");
   DZ_TRY(configure());
   um::UmMaps lm;
   for (int q = 0; q < l.nmaps; ++q) lm.m[q] = maps[l.map_ids[q]];
@@ -244,17 +270,15 @@ extern "C" int dz_test_umma_gemm_path(const float* d_A, int32_t a_mn_major, cons
     if (rc == DZ_OK) rc = um_split(d_B, b_hi, b_lo, nb, stream);
     if (rc != DZ_OK) return rc;
   }
+  const int nparts = convert ? 1 : 2;   // convert: one raw fp32 map per operand
   auto make_maps = [&](const float* hi, const float* lo, int mn_major, int rows, int tile_rows, int out[2]) -> int {
-    const float* src[2] = {hi, lo};
-    for (int part = 0; part < (convert ? 1 : 2); ++part) {
-      uint64_t dims[2], strides[1];
-      uint32_t box[2];
-      if (!mn_major) { dims[0] = (uint64_t)R; dims[1] = (uint64_t)rows; strides[0] = (uint64_t)R * 4; box[0] = 32; box[1] = (uint32_t)tile_rows; }
-      else { dims[0] = (uint64_t)rows; dims[1] = (uint64_t)R; strides[0] = (uint64_t)rows * 4; box[0] = 32; box[1] = 32; }
-      out[part] = plan.add_map(src[part], 2, dims, strides, box);
-      if (out[part] < 0) return DZ_EINVAL;
-    }
-    return DZ_OK;
+    uint64_t dims[2], strides[1];
+    uint32_t box[2];
+    if (!mn_major) { dims[0] = (uint64_t)R; dims[1] = (uint64_t)rows; strides[0] = (uint64_t)R * 4; box[0] = 32; box[1] = (uint32_t)tile_rows; }
+    else { dims[0] = (uint64_t)rows; dims[1] = (uint64_t)R; strides[0] = (uint64_t)rows * 4; box[0] = 32; box[1] = 32; }
+    if (nparts == 2) return plan.add_map_pair(hi, lo, 2, dims, strides, box, out);
+    out[0] = plan.add_map(hi, 2, dims, strides, box);
+    return out[0] < 0 ? DZ_EINVAL : DZ_OK;
   };
   int ma[2] = {-1, -1}, mb[2] = {-1, -1};
   int rc = make_maps(convert ? d_A : a_hi, a_lo, a_mn_major, MI, 128, ma);
@@ -273,46 +297,35 @@ extern "C" int dz_test_umma_gemm_path(const float* d_A, int32_t a_mn_major, cons
   } else {
     p.epi = UM_EPI_PARTIAL; p.C = d_C; p.sc_i = NJ; p.sc_j = 1; p.split_stride = 0;
   }
-  plan.probs.push_back(p);
+  const int prob = plan.add_problem(p);
   const int nst = (int)ceil_div(R, 32);
   const uint32_t a_bytes = p.A.part_bytes * 2, b_bytes = p.B.part_bytes * 2;
   const int tiles = (int)ceil_div(MI, 128);
-  for (int t = 0; t < tiles; ++t) {
-    UmCta c;
-    memset(&c, 0, sizeof(c));
-    c.prob = 0; c.op0 = (uint32_t)plan.ops.size(); c.nstages = (uint32_t)nst; c.r0 = 0; c.i0 = t * 128; c.split = 0;
-    c.row_base = t * 128; c.ph_valid = 1; c.pw_valid = std::min(128, MI - t * 128);
-    uint32_t tx = 0;
-    int nops = 0;
+  UmLaunch l;
+  plan.begin_launch(l, njt, a_bytes + b_bytes);
+  l.stages = stages > 0 ? stages : 4;   // 4 x <= 48 KB + control block fits
+  for (int t = 0; t < tiles && rc == DZ_OK; ++t) {
+    UmCta& c = plan.begin_cta(prob);
+    c.i0 = t * 128; c.row_base = t * 128; c.ph_valid = 1; c.pw_valid = std::min(128, MI - t * 128);
     for (int s = 0; s < nst; ++s) {
-      nops = 0; tx = 0;
-      auto add = [&](int map, uint32_t off, int c0, int c1, uint32_t bytes) {
-        UmTmaOp o;
-        memset(&o, 0, sizeof(o));
-        o.map = (uint32_t)map; o.smem_off = off; o.c[0] = c0; o.c[1] = c1;
-        plan.ops.push_back(o);
-        ++nops; tx += bytes;
-      };
-      for (int part = 0; part < (convert ? 1 : 2); ++part) {
+      plan.stage();
+      for (int part = 0; part < nparts; ++part) {
         const uint32_t base = part * p.A.part_bytes;
-        if (!a_mn_major) add(ma[part], base, 32 * s, t * 128, 128 * 128);
-        else for (int q = 0; q < 4; ++q) add(ma[part], base + q * 4096, t * 128 + 32 * q, 32 * s, 4096);
+        if (!a_mn_major) plan.op(ma[part], base, 32 * s, t * 128);
+        else for (int q = 0; q < 4; ++q) plan.op(ma[part], base + q * 4096, t * 128 + 32 * q, 32 * s);
       }
-      for (int part = 0; part < (convert ? 1 : 2); ++part) {
+      for (int part = 0; part < nparts; ++part) {
         const uint32_t base = a_bytes + part * p.B.part_bytes;
-        if (!b_mn_major) add(mb[part], base, 32 * s, 0, (uint32_t)njt * 128);
-        else for (int q = 0; q < njt / 32; ++q) add(mb[part], base + q * 4096, 32 * q, 32 * s, 4096);
+        if (!b_mn_major) plan.op(mb[part], base, 32 * s, 0);
+        else for (int q = 0; q < njt / 32; ++q) plan.op(mb[part], base + q * 4096, 32 * q, 32 * s);
       }
     }
-    c.ops_per_stage = (uint32_t)nops; c.tx_bytes = tx;
-    plan.ctas.push_back(c);
+    rc = plan.end_cta();
   }
-  UmLaunch l;
-  l.cta0 = 0; l.nctas = tiles;
-  rc = plan.localize_maps(l);
+  plan.end_launch(l);
+  if (rc == DZ_OK) rc = plan.localize_maps(l);
   if (rc == DZ_OK) rc = plan.upload();
   if (rc != DZ_OK) return rc;
-  l.njt = njt; l.stage_bytes = a_bytes + b_bytes; l.stages = stages > 0 ? stages : 4;   // 4 x <= 48 KB + control block fits
   rc = plan.launch("umma_selftest", l, stream, nullptr, path);
   cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream);
   plan.release();

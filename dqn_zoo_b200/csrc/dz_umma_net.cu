@@ -15,10 +15,22 @@
 
 namespace dz {
 
+// The plan's launches.  tag: the name dz_test_learner_trace and dz_test_learner_mma_path take; noisy: the name the fc
+// launches run under for noisy layers (profiles, timelines), which the MMA-path hook accepts as well.
+enum NetLaunch : int { kConv2Fwd, kConv3Fwd, kConv3Dgrad, kConv2Dgrad, kFcFwd, kFcDgrad, kConv3Wgrad, kConv2Wgrad, kNumNetLaunches };
+struct NetLaunchName { const char* tag; const char* noisy; };
+constexpr NetLaunchName kNetLaunchNames[kNumNetLaunches] = {
+    {"conv2_fwd", nullptr},   {"conv3_fwd", nullptr},    {"conv3_dgrad", nullptr}, {"conv2_dgrad", nullptr},
+    {"fc1_fwd", "noisy1_fwd"}, {"fc1_dgrad", "noisy1_dgrad"}, {"conv3_wgrad", nullptr}, {"conv2_wgrad", nullptr}};
+
+// Conv layers 1..3 as GEMMs: N output channels x K = (kh, kw, input channel) reduction.  um_pack_conv_kernel states the
+// same shapes.  The input-gradient images of conv3 and conv2 are rearrangements of W3 and W2 (as many floats).
+constexpr int kConvN[3] = {32, 64, 64}, kConvK[3] = {256, 512, 576};
+constexpr int kConvFwdFloats = kConvN[0] * kConvK[0] + kConvN[1] * kConvK[1] + kConvN[2] * kConvK[2];   // per blob
+
 struct UmNet {
   UmNetDesc d;
   int h1, w1, h2, w2, h3, w3, feat, PB;
-  int njt_fc;
   UmPlan plan;
   // activations / gradients
   float *act_hi[3], *act_lo[3], *act_f32[3];     // layer 1..3, all passes stacked
@@ -29,7 +41,7 @@ struct UmNet {
   // conv weight images: [blob][layer] K-major [N][K]; dgrad images (online)
   float *wf_hi[2][3], *wf_lo[2][3], *wd3_hi, *wd3_lo, *wd2_hi, *wd2_lo;
   int map_wf1[2][2];                              // [blob][hi/lo] for the conv1 kernel
-  UmLaunch l_conv2, l_conv3, l_dconv3, l_dconv2, l_fc, l_fcd, l_wconv3, l_wconv2;
+  UmLaunch launches[kNumNetLaunches];
   float *wg3_part, *wg2_part, *wg1_part;   // conv3 / conv2 weight-gradient split partials [S][K][64]; conv1: one [256][32] per CTA
   int wg3_splits, wg2_splits, wg1_ctas;
   int map_g1[2];                           // dact1 hi / lo as a flat [B*h1*w1][32] tensor
@@ -796,6 +808,24 @@ int um_split(const float* x, float* hi, float* lo, long long n, void* stream);  
 // Plan
 // ------------------------------------------------------------------------------------------------
 
+namespace {
+// Bytes of one conv1 staging buffer: the input rows of the worst 128-pixel output tile, rounded up to 128.
+int conv1_stag_bytes(int B, int W, int h1, int w1) {
+  const int px = h1 * w1, m_pass = B * px;
+  int worst = 0;
+  for (int m0 = 0; m0 < m_pass; m0 += 128) {
+    const int m1 = std::min(m0 + 128, m_pass);
+    int tot = 0;
+    for (int b = m0 / px; b <= (m1 - 1) / px; ++b) tot += conv1_segment(b, m0, m1, px, w1, W * 4).bytes;
+    worst = std::max(worst, tot);
+  }
+  return (worst + 127) / 128 * 128;
+}
+// Dynamic shared memory of a conv1 kernel whose resident tiles take `resident` bytes: barriers, those tiles and the
+// two staging buffers.
+size_t conv1_smem_bytes(int resident, int stag_bytes) { return 2048 + (size_t)resident + 2 * (size_t)stag_bytes; }
+}  // namespace
+
 bool um_net_supported(const UmNetDesc& d) {
   if (d.B < 1 || d.B > 64 || d.npass < 1 || d.npass > 3) return false;
   if (d.W % 4 || d.H < 36 || d.W < 36) return false;
@@ -806,20 +836,8 @@ bool um_net_supported(const UmNetDesc& d) {
   if (h3 < 1 || w3 < 1) return false;
   if (h2 * w2 > 128 || (h1 / 2) * (w1 / 2) > 128 || h3 * w3 > 128) return false;
   if (h1 * w1 < 64) return false;                      // a 128-pixel conv1 tile spans at most 3 images
-  // conv1 staging: worst case bytes of one tile
-  const int px = h1 * w1, m_pass = d.B * px;
-  int worst = 0;
-  for (int m0 = 0; m0 < m_pass; m0 += 128) {
-    const int m1 = std::min(m0 + 128, m_pass);
-    int tot = 0;
-    for (int b = m0 / px; b <= (m1 - 1) / px; ++b) {
-      const int plo = std::max(m0, b * px) - b * px, phi = std::min(m1, (b + 1) * px) - b * px;
-      tot += (4 * ((phi - 1) / w1 - plo / w1) + 8) * d.W * 4;
-    }
-    worst = std::max(worst, tot);
-  }
-  if (2 * ((worst + 127) / 128 * 128) + 2048 + 65536 + 131072 > 227 * 1024) return false;
-  return true;
+  // the largest conv1 kernel (conv1_umma_kernel: weight image and A tile resident) fits
+  return conv1_smem_bytes(kC1W + kC1A, conv1_stag_bytes(d.B, d.W, h1, w1)) <= 227 * 1024;
 }
 
 namespace {
@@ -856,16 +874,13 @@ int64_t carve_net(UmNet* n, char* base) {
   for (int L = 0; L < 3; ++L) { n->act_hi[L] = c.f(sz[L]); n->act_lo[L] = c.f(sz[L]); n->act_f32[L] = c.f(sz[L]); }
   const int64_t dz_[3] = {(int64_t)d.B * g.h1 * g.w1 * 32, (int64_t)d.B * g.h2 * g.w2 * 64, (int64_t)d.B * g.feat};
   for (int L = 0; L < 3; ++L) { n->dact_hi[L] = c.f(dz_[L]); n->dact_lo[L] = c.f(dz_[L]); n->dact_f32[L] = c.f(dz_[L]); }
-  const int kN[3] = {32, 64, 64}, kK[3] = {256, 512, 576};
   for (int b = 0; b < 2; ++b)
-    for (int L = 0; L < 3; ++L) { n->wf_hi[b][L] = c.f(kN[L] * kK[L]); n->wf_lo[b][L] = c.f(kN[L] * kK[L]); }
-  n->wd3_hi = c.f(64 * 576); n->wd3_lo = c.f(64 * 576);
-  n->wd2_hi = c.f(128 * 256); n->wd2_lo = c.f(128 * 256);
+    for (int L = 0; L < 3; ++L) { n->wf_hi[b][L] = c.f(kConvN[L] * kConvK[L]); n->wf_lo[b][L] = c.f(kConvN[L] * kConvK[L]); }
+  n->wd3_hi = c.f(kConvN[2] * kConvK[2]); n->wd3_lo = c.f(kConvN[2] * kConvK[2]);
+  n->wd2_hi = c.f(kConvN[1] * kConvK[1]); n->wd2_lo = c.f(kConvN[1] * kConvK[1]);
   {
-    const int groups = (d.B + 7) / 8;
     n->wg3_splits = std::max(1, std::min(g.h3, kNumSMs / 5));             // stages = h3 * groups, split over the output rows
     n->wg2_splits = std::max(1, std::min(g.h2, kNumSMs / 8));
-    (void)groups;
     n->wg3_part = c.f((int64_t)n->wg3_splits * 576 * 64);
     n->wg2_part = c.f((int64_t)n->wg2_splits * 512 * 64);
     n->wg1_ctas = std::min(kNumSMs, (d.B * g.h1 * g.w1 + 127) / 128);
@@ -891,129 +906,108 @@ int64_t carve_net(UmNet* n, char* base) {
   return c.used;
 }
 
-void push_op(UmPlan& pl, int map, uint32_t off, int c0, int c1, int c2, int c3, int c4) {
-  UmTmaOp o;
-  memset(&o, 0, sizeof(o));
-  o.map = (uint32_t)map; o.smem_off = off; o.c[0] = c0; o.c[1] = c1; o.c[2] = c2; o.c[3] = c3; o.c[4] = c4;
-  pl.ops.push_back(o);
+// A problem with its operands, k-steps and reduction elements per stage, epilogue and valid extents; the rest zero.
+UmProblem make_problem(const UmOperand& A, const UmOperand& Bo, int ksteps, int red_per_stage, uint32_t epi, int MI, int NJ) {
+  UmProblem pr;
+  memset(&pr, 0, sizeof(pr));
+  pr.A = A; pr.B = Bo; pr.ksteps = (uint32_t)ksteps; pr.red_per_stage = (uint32_t)red_per_stage; pr.epi = epi;
+  pr.MI = MI; pr.NJ = NJ;
+  if (epi == UM_EPI_ROWS) { pr.pw = 1 << 20; pr.rs_outer = 0; pr.rs_inner = 1; }   // tile row r -> dst row row_base + r
+  return pr;
+}
+
+// Stage of a launch whose operands are K-major hi / lo pairs (A, then B): it may run on the wgmma kernel.
+uint32_t kmajor_stage_bytes(const UmOperand& A, const UmOperand& Bo) {
+  return std::max(2 * A.part_bytes + 2 * Bo.part_bytes, um_wgmma_min_stage(A.part_bytes));
 }
 
 int build_plan(UmNet* n) {
   const UmNetDesc& d = n->d;
   UmPlan& pl = n->plan;
   const int B = d.B, PB = n->PB, h1 = n->h1, w1 = n->w1, h2 = n->h2, w2 = n->w2, h3 = n->h3, w3 = n->w3, feat = n->feat;
-  const int kN[3] = {32, 64, 64}, kK[3] = {256, 512, 576};
-#define MAP_OR_FAIL(var, ...) const int var = pl.add_map(__VA_ARGS__); if (var < 0) return DZ_EINVAL;
 
   // ---- weight image maps: [blob][layer][part]; box rows = N tile used by the layer
   int m_wf[2][3][2];
   const uint32_t wf_rows[3] = {32, 64, 32};   // conv1: N 32; conv2: full 64; conv3: halves of 32
   for (int b = 0; b < 2; ++b)
-    for (int L = 0; L < 3; ++L)
-      for (int part = 0; part < 2; ++part) {
-        uint64_t dims[2] = {(uint64_t)kK[L], (uint64_t)kN[L]}, strides[1] = {(uint64_t)kK[L] * 4};
-        uint32_t box[2] = {32, wf_rows[L]};
-        m_wf[b][L][part] = pl.add_map(part ? n->wf_lo[b][L] : n->wf_hi[b][L], 2, dims, strides, box);
-        if (m_wf[b][L][part] < 0) return DZ_EINVAL;
-      }
+    for (int L = 0; L < 3; ++L) {
+      uint64_t dims[2] = {(uint64_t)kConvK[L], (uint64_t)kConvN[L]}, strides[1] = {(uint64_t)kConvK[L] * 4};
+      uint32_t box[2] = {32, wf_rows[L]};
+      DZ_TRY(pl.add_map_pair(n->wf_hi[b][L], n->wf_lo[b][L], 2, dims, strides, box, m_wf[b][L]));
+    }
   for (int b = 0; b < 2; ++b) { n->map_wf1[b][0] = m_wf[b][0][0]; n->map_wf1[b][1] = m_wf[b][0][1]; }
 
   // =========================================================================== conv2 forward
   {
     int m_a[2];
-    for (int part = 0; part < 2; ++part) {
-      uint64_t dims[5] = {64, (uint64_t)w1 / 2, 2, (uint64_t)h1 / 2, (uint64_t)PB};
-      uint64_t strides[4] = {256, (uint64_t)w1 * 128, (uint64_t)2 * w1 * 128, (uint64_t)h1 * w1 * 128};
-      uint32_t box[5] = {32, (uint32_t)w2, 1, (uint32_t)h2, 1};
-      m_a[part] = pl.add_map(part ? n->act_lo[0] : n->act_hi[0], 5, dims, strides, box);
-      if (m_a[part] < 0) return DZ_EINVAL;
-    }
+    uint64_t dims[5] = {64, (uint64_t)w1 / 2, 2, (uint64_t)h1 / 2, (uint64_t)PB};
+    uint64_t strides[4] = {256, (uint64_t)w1 * 128, (uint64_t)2 * w1 * 128, (uint64_t)h1 * w1 * 128};
+    uint32_t box[5] = {32, (uint32_t)w2, 1, (uint32_t)h2, 1};
+    DZ_TRY(pl.add_map_pair(n->act_hi[0], n->act_lo[0], 5, dims, strides, box, m_a));
     const int rows = h2 * w2;
-    UmOperand A = um_kmajor(rows, true, false), Bo = um_kmajor(64, true, false);
+    const UmOperand A = um_kmajor(rows, true, false), Bo = um_kmajor(64, true, false);
     const uint32_t a_bytes = A.part_bytes * 2;
-    n->l_conv2.cta0 = (int)pl.ctas.size(); n->l_conv2.njt = 64; n->l_conv2.stage_bytes = a_bytes + Bo.part_bytes * 2;
-    // the MMA reads 128 rows of every A part: keep the (garbage) tail rows inside the stage
-    n->l_conv2.stage_bytes = std::max<uint32_t>(n->l_conv2.stage_bytes, A.part_bytes + 16384);
-    n->l_conv2.stages = std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_conv2.stage_bytes));
+    UmLaunch& l = n->launches[kConv2Fwd];
+    pl.begin_launch(l, 64, kmajor_stage_bytes(A, Bo));
     for (int p = 0; p < d.npass; ++p) {
       const int blob = d.pass_target[p] ? 1 : 0;
-      UmProblem pr;
-      memset(&pr, 0, sizeof(pr));
-      pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32; pr.epi = UM_EPI_ROWS;
-      pr.MI = rows; pr.NJ = 64;
-      pr.out_hi = n->act_hi[1]; pr.out_lo = n->act_lo[1]; pr.out_f32 = nullptr; pr.out_ld = 64;
+      UmProblem pr = make_problem(A, Bo, 4, 32, UM_EPI_ROWS, rows, 64);
+      pr.out_hi = n->act_hi[1]; pr.out_lo = n->act_lo[1]; pr.out_ld = 64;
       pr.bias = (blob ? d.target : d.online) + d.off_conv_b[1]; pr.relu = 1;
-      pr.pw = 1 << 20; pr.rs_outer = 0; pr.rs_inner = 1;
-      const int prob = (int)pl.probs.size();
-      pl.probs.push_back(pr);
+      const int prob = pl.add_problem(pr);
       for (int b = 0; b < B; ++b) {
         const int img = p * B + b;
-        UmCta c;
-        memset(&c, 0, sizeof(c));
-        c.prob = (uint32_t)prob; c.op0 = (uint32_t)pl.ops.size(); c.nstages = 16; c.ops_per_stage = 4;
-        c.tx_bytes = (uint32_t)(2 * rows * 128 + 2 * 64 * 128);
+        UmCta& c = pl.begin_cta(prob);
         c.row_base = img * rows; c.ph_valid = 1; c.pw_valid = rows;
         for (int kh = 0; kh < 4; ++kh)
           for (int kw = 0; kw < 4; ++kw) {
-            const int s = kh * 4 + kw;
-            for (int part = 0; part < 2; ++part) push_op(pl, m_a[part], part * A.part_bytes, 32 * (kw & 1), kw >> 1, kh & 1, kh >> 1, img);
-            for (int part = 0; part < 2; ++part) push_op(pl, m_wf[blob][1][part], a_bytes + part * Bo.part_bytes, 32 * s, 0, 0, 0, 0);
+            pl.stage();
+            pl.op_pair(m_a, 0, A.part_bytes, 32 * (kw & 1), kw >> 1, kh & 1, kh >> 1, img);
+            pl.op_pair(m_wf[blob][1], a_bytes, Bo.part_bytes, 32 * (kh * 4 + kw));
           }
-        pl.ctas.push_back(c);
+        DZ_TRY(pl.end_cta());
       }
     }
-    n->l_conv2.nctas = (int)pl.ctas.size() - n->l_conv2.cta0;
+    pl.end_launch(l);
   }
 
   // =========================================================================== conv3 forward (two 32-channel halves)
   {
     const int G = (B % 2 == 0 && 2 * h3 * w3 <= 128) ? 2 : 1;
     int m_a[2];
-    for (int part = 0; part < 2; ++part) {
-      uint64_t dims[4] = {64, (uint64_t)w2, (uint64_t)h2, (uint64_t)PB};
-      uint64_t strides[3] = {256, (uint64_t)w2 * 256, (uint64_t)h2 * w2 * 256};
-      uint32_t box[4] = {32, (uint32_t)w3, (uint32_t)h3, (uint32_t)G};
-      m_a[part] = pl.add_map(part ? n->act_lo[1] : n->act_hi[1], 4, dims, strides, box);
-      if (m_a[part] < 0) return DZ_EINVAL;
-    }
+    uint64_t dims[4] = {64, (uint64_t)w2, (uint64_t)h2, (uint64_t)PB};
+    uint64_t strides[3] = {256, (uint64_t)w2 * 256, (uint64_t)h2 * w2 * 256};
+    uint32_t box[4] = {32, (uint32_t)w3, (uint32_t)h3, (uint32_t)G};
+    DZ_TRY(pl.add_map_pair(n->act_hi[1], n->act_lo[1], 4, dims, strides, box, m_a));
     const int rows = G * h3 * w3;
-    UmOperand A = um_kmajor(rows, true, false), Bo = um_kmajor(32, true, false);
+    const UmOperand A = um_kmajor(rows, true, false), Bo = um_kmajor(32, true, false);
     const uint32_t a_bytes = A.part_bytes * 2;
-    n->l_conv3.cta0 = (int)pl.ctas.size(); n->l_conv3.njt = 32;
-    n->l_conv3.stage_bytes = std::max<uint32_t>(a_bytes + Bo.part_bytes * 2, A.part_bytes + 16384);
-    n->l_conv3.stages = std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_conv3.stage_bytes));
+    UmLaunch& l = n->launches[kConv3Fwd];
+    pl.begin_launch(l, 32, kmajor_stage_bytes(A, Bo));
     for (int p = 0; p < d.npass; ++p) {
       const int blob = d.pass_target[p] ? 1 : 0;
       for (int half = 0; half < 2; ++half) {
-        UmProblem pr;
-        memset(&pr, 0, sizeof(pr));
-        pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32; pr.epi = UM_EPI_ROWS;
-        pr.MI = rows; pr.NJ = 32;
+        UmProblem pr = make_problem(A, Bo, 4, 32, UM_EPI_ROWS, rows, 32);
         pr.out_hi = n->act_hi[2] + 32 * half; pr.out_lo = n->act_lo[2] + 32 * half; pr.out_f32 = n->act_f32[2] + 32 * half;
         pr.out_ld = 64;
         pr.bias = (blob ? d.target : d.online) + d.off_conv_b[2] + 32 * half; pr.relu = 1;
-        pr.pw = 1 << 20; pr.rs_outer = 0; pr.rs_inner = 1;
-        const int prob = (int)pl.probs.size();
-        pl.probs.push_back(pr);
+        const int prob = pl.add_problem(pr);
         for (int t = 0; t < B / G; ++t) {
           const int img = p * B + t * G;
-          UmCta c;
-          memset(&c, 0, sizeof(c));
-          c.prob = (uint32_t)prob; c.op0 = (uint32_t)pl.ops.size(); c.nstages = 18; c.ops_per_stage = 4;
-          c.tx_bytes = (uint32_t)(2 * rows * 128 + 2 * 32 * 128);
+          UmCta& c = pl.begin_cta(prob);
           c.row_base = img * h3 * w3; c.ph_valid = 1; c.pw_valid = rows;
           for (int kh = 0; kh < 3; ++kh)
             for (int kw = 0; kw < 3; ++kw)
               for (int ch = 0; ch < 2; ++ch) {
-                const int s = (kh * 3 + kw) * 2 + ch;
-                for (int part = 0; part < 2; ++part) push_op(pl, m_a[part], part * A.part_bytes, 32 * ch, kw, kh, img, 0);
-                for (int part = 0; part < 2; ++part) push_op(pl, m_wf[blob][2][part], a_bytes + part * Bo.part_bytes, 32 * s, 32 * half, 0, 0, 0);
+                pl.stage();
+                pl.op_pair(m_a, 0, A.part_bytes, 32 * ch, kw, kh, img);
+                pl.op_pair(m_wf[blob][2], a_bytes, Bo.part_bytes, 32 * ((kh * 3 + kw) * 2 + ch), 32 * half);
               }
-          pl.ctas.push_back(c);
+          DZ_TRY(pl.end_cta());
         }
       }
     }
-    n->l_conv3.nctas = (int)pl.ctas.size() - n->l_conv3.cta0;
+    pl.end_launch(l);
   }
 
   // =========================================================================== conv3 input gradient
@@ -1033,42 +1027,33 @@ int build_plan(UmNet* n) {
       if (m_a[part] < 0 || m_w[part] < 0) return DZ_EINVAL;
     }
     const int rows = hb * w2;
-    UmOperand A = um_kmajor(rows, true, false), Bo = um_kmajor(32, true, false);
+    const UmOperand A = um_kmajor(rows, true, false), Bo = um_kmajor(32, true, false);
     const uint32_t a_bytes = A.part_bytes * 2;
-    n->l_dconv3.cta0 = (int)pl.ctas.size(); n->l_dconv3.njt = 32;
-    n->l_dconv3.stage_bytes = std::max<uint32_t>(a_bytes + Bo.part_bytes * 2, A.part_bytes + 16384);
-    n->l_dconv3.stages = std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_dconv3.stage_bytes));
+    UmLaunch& l = n->launches[kConv3Dgrad];
+    pl.begin_launch(l, 32, kmajor_stage_bytes(A, Bo));
     for (int half = 0; half < 2; ++half) {
-      UmProblem pr;
-      memset(&pr, 0, sizeof(pr));
-      pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32; pr.epi = UM_EPI_ROWS;
-      pr.MI = rows; pr.NJ = 32;
+      UmProblem pr = make_problem(A, Bo, 4, 32, UM_EPI_ROWS, rows, 32);
       pr.out_hi = n->dact_hi[1] + 32 * half; pr.out_lo = n->dact_lo[1] + 32 * half; pr.out_f32 = n->dact_f32[1] + 32 * half;
       pr.out_ld = 64;
       pr.mask = n->act_hi[1] + 32 * half;                 // pass 0 is the first B images
-      pr.pw = 1 << 20; pr.rs_outer = 0; pr.rs_inner = 1;
-      const int prob = (int)pl.probs.size();
-      pl.probs.push_back(pr);
+      const int prob = pl.add_problem(pr);
       for (int b = 0; b < B; ++b)
         for (int band = 0; band < nb; ++band) {
           const int y0 = band * hb, y1 = std::min(h2, y0 + hb);
           if (y1 <= y0) continue;
-          UmCta c;
-          memset(&c, 0, sizeof(c));
-          c.prob = (uint32_t)prob; c.op0 = (uint32_t)pl.ops.size(); c.nstages = 18; c.ops_per_stage = 4;
-          c.tx_bytes = (uint32_t)(2 * rows * 128 + 2 * 32 * 128);
+          UmCta& c = pl.begin_cta(prob);
           c.row_base = (b * h2 + y0) * w2; c.ph_valid = 1; c.pw_valid = (y1 - y0) * w2;
           for (int kh = 0; kh < 3; ++kh)
             for (int kw = 0; kw < 3; ++kw)
               for (int nh = 0; nh < 2; ++nh) {
-                const int s = (kh * 3 + kw) * 2 + nh;
-                for (int part = 0; part < 2; ++part) push_op(pl, m_a[part], part * A.part_bytes, 32 * nh, -kw, y0 - kh, b, 0);
-                for (int part = 0; part < 2; ++part) push_op(pl, m_w[part], a_bytes + part * Bo.part_bytes, 32 * s, 32 * half, 0, 0, 0);
+                pl.stage();
+                pl.op_pair(m_a, 0, A.part_bytes, 32 * nh, -kw, y0 - kh, b);
+                pl.op_pair(m_w, a_bytes, Bo.part_bytes, 32 * ((kh * 3 + kw) * 2 + nh), 32 * half);
               }
-          pl.ctas.push_back(c);
+          DZ_TRY(pl.end_cta());
         }
     }
-    n->l_dconv3.nctas = (int)pl.ctas.size() - n->l_dconv3.cta0;
+    pl.end_launch(l);
   }
 
   // =========================================================================== conv2 input gradient (4 parity classes)
@@ -1086,45 +1071,36 @@ int build_plan(UmNet* n) {
       if (m_a[part] < 0 || m_w[part] < 0) return DZ_EINVAL;
     }
     const int rows = (h1 / 2) * (w1 / 2);
-    UmOperand A = um_kmajor(rows, true, false), Bo = um_kmajor(32, true, false);
+    const UmOperand A = um_kmajor(rows, true, false), Bo = um_kmajor(32, true, false);
     const uint32_t a_bytes = A.part_bytes * 2;
-    n->l_dconv2.cta0 = (int)pl.ctas.size(); n->l_dconv2.njt = 32;
-    n->l_dconv2.stage_bytes = std::max<uint32_t>(a_bytes + Bo.part_bytes * 2, A.part_bytes + 16384);
-    n->l_dconv2.stages = std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_dconv2.stage_bytes));
-    UmProblem pr;
-    memset(&pr, 0, sizeof(pr));
-    pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32; pr.epi = UM_EPI_ROWS;
-    pr.MI = rows; pr.NJ = 32;
+    UmLaunch& l = n->launches[kConv2Dgrad];
+    pl.begin_launch(l, 32, kmajor_stage_bytes(A, Bo));
+    UmProblem pr = make_problem(A, Bo, 4, 32, UM_EPI_ROWS, rows, 32);
     pr.out_hi = n->dact_hi[0]; pr.out_lo = n->dact_lo[0]; pr.out_f32 = n->dact_f32[0]; pr.out_ld = 32;
     pr.mask = n->act_hi[0];
     pr.pw = w1 / 2; pr.rs_outer = 2 * w1; pr.rs_inner = 2;
-    const int prob = (int)pl.probs.size();
-    pl.probs.push_back(pr);
+    const int prob = pl.add_problem(pr);
     for (int b = 0; b < B; ++b)
       for (int cls = 0; cls < 4; ++cls) {
         const int py = cls >> 1, pxx = cls & 1;
-        UmCta c;
-        memset(&c, 0, sizeof(c));
-        c.prob = (uint32_t)prob; c.op0 = (uint32_t)pl.ops.size(); c.nstages = 8; c.ops_per_stage = 4;
-        c.tx_bytes = (uint32_t)(2 * rows * 128 + 2 * 32 * 128);
+        UmCta& c = pl.begin_cta(prob);
         c.row_base = b * h1 * w1 + py * w1 + pxx; c.ph_valid = h1 / 2; c.pw_valid = w1 / 2;
         for (int ay = 0; ay < 2; ++ay)
           for (int ax = 0; ax < 2; ++ax)
             for (int nh = 0; nh < 2; ++nh) {
-              const int s = (ay * 2 + ax) * 2 + nh;
-              for (int part = 0; part < 2; ++part) push_op(pl, m_a[part], part * A.part_bytes, 32 * nh, -ax, -ay, b, 0);
-              for (int part = 0; part < 2; ++part) push_op(pl, m_w[part], a_bytes + part * Bo.part_bytes, 32 * s, 32 * cls, 0, 0, 0);
+              pl.stage();
+              pl.op_pair(m_a, 0, A.part_bytes, 32 * nh, -ax, -ay, b);
+              pl.op_pair(m_w, a_bytes, Bo.part_bytes, 32 * ((ay * 2 + ax) * 2 + nh), 32 * cls);
             }
-        pl.ctas.push_back(c);
+        DZ_TRY(pl.end_cta());
       }
-    n->l_dconv2.nctas = (int)pl.ctas.size() - n->l_dconv2.cta0;
+    pl.end_launch(l);
   }
 
-  for (int part = 0; part < 2; ++part) {   // conv1 weight gradient: G operand
+  {   // conv1 weight gradient: G operand
     uint64_t dims[2] = {32, (uint64_t)B * h1 * w1}, strides[1] = {128};
     uint32_t box[2] = {32, 128};
-    n->map_g1[part] = pl.add_map(part ? n->dact_lo[0] : n->dact_hi[0], 2, dims, strides, box);
-    if (n->map_g1[part] < 0) return DZ_EINVAL;
+    DZ_TRY(pl.add_map_pair(n->dact_hi[0], n->dact_lo[0], 2, dims, strides, box, n->map_g1));
   }
   // =========================================================================== conv3 / conv2 weight gradients
   // dW[k][n] = sum_m A[m][k] G[m][n]: both operands are read through MN-major (transposing) descriptors straight from the
@@ -1145,43 +1121,35 @@ int build_plan(UmNet* n) {
         if (m_a[part] < 0 || m_g[part] < 0) return DZ_EINVAL;
       }
       const int rows = w3 * 8;                                  // reduction rows per stage (multiple of 8)
-      UmOperand A = um_mnmajor(128, rows, false), Bo = um_mnmajor(64, rows, false);
+      const UmOperand A = um_mnmajor(128, rows, false), Bo = um_mnmajor(64, rows, false);
       const uint32_t a_bytes = A.part_bytes * 2;
-      n->l_wconv3.cta0 = (int)pl.ctas.size(); n->l_wconv3.njt = 64;
-      n->l_wconv3.stage_bytes = (a_bytes + Bo.part_bytes * 2 + 1023) / 1024 * 1024;
-      n->l_wconv3.stages = std::max(1, std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_wconv3.stage_bytes)));
-      UmProblem pr;
-      memset(&pr, 0, sizeof(pr));
-      pr.A = A; pr.B = Bo; pr.ksteps = (uint32_t)(rows / 8); pr.red_per_stage = (uint32_t)rows;
-      pr.epi = UM_EPI_PARTIAL; pr.MI = 576; pr.NJ = 64;
+      UmLaunch& l = n->launches[kConv3Wgrad];
+      pl.begin_launch(l, 64, a_bytes + Bo.part_bytes * 2);
+      UmProblem pr = make_problem(A, Bo, rows / 8, rows, UM_EPI_PARTIAL, 576, 64);
       pr.C = n->wg3_part; pr.sc_i = 64; pr.sc_j = 1; pr.split_stride = 576 * 64;
-      const int prob = (int)pl.probs.size();
-      pl.probs.push_back(pr);
+      const int prob = pl.add_problem(pr);
       const int S = n->wg3_splits, per = (h3 + S - 1) / S;
       for (int kt = 0; kt < 5; ++kt)                            // 18 slabs of 32 reduction... k values: 4,4,4,4,2
         for (int sp = 0; sp < S; ++sp) {
           const int oy0 = sp * per, oy1 = std::min(h3, oy0 + per);
           if (oy1 <= oy0) continue;
-          UmCta c;
-          memset(&c, 0, sizeof(c));
           const int nslab = std::min(4, 18 - kt * 4);
-          c.prob = (uint32_t)prob; c.op0 = (uint32_t)pl.ops.size(); c.nstages = (uint32_t)((oy1 - oy0) * groups);
-          c.ops_per_stage = (uint32_t)(2 * nslab + 4);
-          c.tx_bytes = (uint32_t)((2 * nslab + 4) * rows * 128);
+          UmCta& c = pl.begin_cta(prob);
           c.i0 = kt * 128; c.split = sp;
           for (int oy = oy0; oy < oy1; ++oy)
             for (int gidx = 0; gidx < groups; ++gidx) {
+              pl.stage();
               for (int part = 0; part < 2; ++part)
                 for (int sl = 0; sl < nslab; ++sl) {
                   const int slab = kt * 4 + sl, tap = slab >> 1, ch = slab & 1, kh = tap / 3, kw = tap % 3;
-                  push_op(pl, m_a[part], part * A.part_bytes + sl * A.lbo, 32 * ch, kw, oy + kh, gidx * 8, 0);
+                  pl.op(m_a[part], part * A.part_bytes + sl * A.lbo, 32 * ch, kw, oy + kh, gidx * 8);
                 }
               for (int part = 0; part < 2; ++part)
-                for (int nh = 0; nh < 2; ++nh) push_op(pl, m_g[part], a_bytes + part * Bo.part_bytes + nh * Bo.lbo, 32 * nh, 0, oy, gidx * 8, 0);
+                for (int nh = 0; nh < 2; ++nh) pl.op(m_g[part], a_bytes + part * Bo.part_bytes + nh * Bo.lbo, 32 * nh, 0, oy, gidx * 8);
             }
-          pl.ctas.push_back(c);
+          DZ_TRY(pl.end_cta());
         }
-      n->l_wconv3.nctas = (int)pl.ctas.size() - n->l_wconv3.cta0;
+      pl.end_launch(l);
     }
     // ---- conv2: A = act1 patches through the stride-2 parity view (pass 0), G = dact2; two 32-column halves
     {
@@ -1198,51 +1166,41 @@ int build_plan(UmNet* n) {
         if (m_a[part] < 0 || m_g[part] < 0) return DZ_EINVAL;
       }
       const int rows = w2 * 8;
-      UmOperand A = um_mnmajor(128, rows, false), Bo = um_mnmajor(32, rows, false);
+      const UmOperand A = um_mnmajor(128, rows, false), Bo = um_mnmajor(32, rows, false);
       const uint32_t a_bytes = A.part_bytes * 2;
-      n->l_wconv2.cta0 = (int)pl.ctas.size(); n->l_wconv2.njt = 32;
-      n->l_wconv2.stage_bytes = (a_bytes + Bo.part_bytes * 2 + 1023) / 1024 * 1024;
-      n->l_wconv2.stages = std::max(1, std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_wconv2.stage_bytes)));
+      UmLaunch& l = n->launches[kConv2Wgrad];
+      pl.begin_launch(l, 32, a_bytes + Bo.part_bytes * 2);
       const int S = n->wg2_splits, per = (h2 + S - 1) / S;
       for (int half = 0; half < 2; ++half) {
-        UmProblem pr;
-        memset(&pr, 0, sizeof(pr));
-        pr.A = A; pr.B = Bo; pr.ksteps = (uint32_t)(rows / 8); pr.red_per_stage = (uint32_t)rows;
-        pr.epi = UM_EPI_PARTIAL; pr.MI = 512; pr.NJ = 32;
+        UmProblem pr = make_problem(A, Bo, rows / 8, rows, UM_EPI_PARTIAL, 512, 32);
         pr.C = n->wg2_part + 32 * half; pr.sc_i = 64; pr.sc_j = 1; pr.split_stride = 512 * 64;
-        const int prob = (int)pl.probs.size();
-        pl.probs.push_back(pr);
+        const int prob = pl.add_problem(pr);
         for (int kt = 0; kt < 4; ++kt)
           for (int sp = 0; sp < S; ++sp) {
             const int oy0 = sp * per, oy1 = std::min(h2, oy0 + per);
             if (oy1 <= oy0) continue;
-            UmCta c;
-            memset(&c, 0, sizeof(c));
-            c.prob = (uint32_t)prob; c.op0 = (uint32_t)pl.ops.size(); c.nstages = (uint32_t)((oy1 - oy0) * groups);
-            c.ops_per_stage = 10;
-            c.tx_bytes = (uint32_t)(10 * rows * 128);
+            UmCta& c = pl.begin_cta(prob);
             c.i0 = kt * 128; c.split = sp;
             for (int oy = oy0; oy < oy1; ++oy)
               for (int gidx = 0; gidx < groups; ++gidx) {
+                pl.stage();
                 for (int part = 0; part < 2; ++part)
                   for (int sl = 0; sl < 4; ++sl) {
                     const int tap = kt * 4 + sl, kh = tap >> 2, kw = tap & 3;   // one slab = one (kh, kw) tap x 32 channels
-                    push_op(pl, m_a[part], part * A.part_bytes + sl * A.lbo, 32 * (kw & 1), kw >> 1, kh & 1, oy + (kh >> 1), gidx * 8);
+                    pl.op(m_a[part], part * A.part_bytes + sl * A.lbo, 32 * (kw & 1), kw >> 1, kh & 1, oy + (kh >> 1), gidx * 8);
                   }
-                for (int part = 0; part < 2; ++part) push_op(pl, m_g[part], a_bytes + part * Bo.part_bytes, 32 * half, 0, oy, gidx * 8, 0);
+                pl.op_pair(m_g, a_bytes, Bo.part_bytes, 32 * half, 0, oy, gidx * 8);
               }
-            pl.ctas.push_back(c);
+            DZ_TRY(pl.end_cta());
           }
       }
-      n->l_wconv2.nctas = (int)pl.ctas.size() - n->l_wconv2.cta0;
+      pl.end_launch(l);
     }
   }
 
   // =========================================================================== fc1 / noisy1 forward and input gradient
-  n->l_fc.nctas = 0; n->l_fcd.nctas = 0;
   if (d.use_fc) {
     const int njt = B <= 32 ? 32 : 64;
-    n->njt_fc = njt;
     const int q = d.noisy ? 2 : 1;
     int m_x[2], m_g[2];
     for (int part = 0; part < 2; ++part) {
@@ -1299,13 +1257,12 @@ int build_plan(UmNet* n) {
     // ---- forward: D[n, m] = sum_k W[k][n] x[m][k];  noisy: W = Wmu + Wsigma * (eps_in[k] * eps_out[n]), formed in the
     // MMA warps (umma_fc_kernel; with fc_per_pass by the converter warps of umma_gemm_kernel)
     {
-      UmOperand Bo = um_kmajor(njt, true, false);
+      const UmOperand Bo = um_kmajor(njt, true, false);
       const int nk = feat / 32, S = n->fc_splits, per = (nk + S - 1) / S;
-      n->l_fc.cta0 = (int)pl.ctas.size(); n->l_fc.njt = njt;
-      n->l_fc.stage_bytes = 2 * 16384 + 2 * Bo.part_bytes;
-      for (int k = 0; k < ngrp; ++k)
-        n->l_fc.stage_bytes = std::max<uint32_t>(n->l_fc.stage_bytes, 2 * 16384 / grp_n[k] + grp_n[k] * 2 * Bo.part_bytes);
-      n->l_fc.stages = std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_fc.stage_bytes));
+      uint32_t stage_bytes = 2 * 16384 + 2 * Bo.part_bytes;
+      for (int k = 0; k < ngrp; ++k) stage_bytes = std::max<uint32_t>(stage_bytes, 2 * 16384 / grp_n[k] + grp_n[k] * 2 * Bo.part_bytes);
+      UmLaunch& l = n->launches[kFcFwd];
+      pl.begin_launch(l, njt, stage_bytes);
       for (int k = 0; k < ngrp; ++k) {
         const int blob = grp_blob[k], np = grp_n[k], rows = fc_rows[blob], slabs = rows / 32;
         const UmOperand A = um_mnmajor(rows, 32, true, nullptr);
@@ -1314,14 +1271,10 @@ int build_plan(UmNet* n) {
           const int prob0 = (int)pl.probs.size();
           for (int gp = 0; gp < np; ++gp) {
             const int p = grp[k][gp], qi = p * d.nstream + s;
-            UmProblem pr;
-            memset(&pr, 0, sizeof(pr));
-            pr.A = A; pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32;
+            UmProblem pr = make_problem(A, Bo, 4, 32, UM_EPI_PARTIAL, 512, B);
             if (d.noisy) pr.A.convert = 2;
-            pr.epi = UM_EPI_PARTIAL; pr.MI = 512; pr.NJ = B;
             pr.C = n->fc_part + (int64_t)qi * S * B * 512; pr.sc_i = 1; pr.sc_j = 512; pr.split_stride = (long long)B * 512;
-            const int prob = (int)pl.probs.size();
-            pl.probs.push_back(pr);
+            const int prob = pl.add_problem(pr);
             if (d.noisy) {
               n->patches.push_back({prob, 0, (int64_t)d.noise_apply[p] * d.noise_stride + d.noise_off_in[s]});
               n->patches.push_back({prob, 2, (int64_t)d.noise_apply[p] * d.noise_stride + d.noise_off_out[s]});
@@ -1332,43 +1285,33 @@ int build_plan(UmNet* n) {
             for (int nt = 0; nt < 512 / rows; ++nt) {
               const int k0 = sp * per, k1 = std::min(nk, k0 + per);
               if (k1 <= k0) continue;
-              UmCta c;
-              memset(&c, 0, sizeof(c));
-              c.prob = (uint32_t)prob0; c.nprob = (uint32_t)np; c.op0 = (uint32_t)pl.ops.size(); c.nstages = (uint32_t)(k1 - k0);
-              c.ops_per_stage = (wf3d ? 1 : slabs) * q + 2 * np;
-              c.tx_bytes = (uint32_t)(q * A.part_bytes + np * 2 * njt * 128);
-              c.r0 = 32 * k0; c.i0 = nt * rows; c.split = sp;
+              UmCta& c = pl.begin_cta(prob0);
+              c.nprob = (uint32_t)np; c.r0 = 32 * k0; c.i0 = nt * rows; c.split = sp;
               for (int ks = k0; ks < k1; ++ks) {
+                pl.stage();
                 for (int sg = 0; sg < q; ++sg) {
-                  if (wf3d) push_op(pl, m_wf_fc[blob][s][sg], sg * A.part_bytes, 0, 32 * ks, nt * slabs, 0, 0);
-                  else for (int sl = 0; sl < slabs; ++sl) push_op(pl, m_wf_fc[blob][s][sg], sg * A.part_bytes + sl * 4096, nt * rows + 32 * sl, 32 * ks, 0, 0, 0);
+                  if (wf3d) pl.op(m_wf_fc[blob][s][sg], sg * A.part_bytes, 0, 32 * ks, nt * slabs);
+                  else for (int sl = 0; sl < slabs; ++sl) pl.op(m_wf_fc[blob][s][sg], sg * A.part_bytes + sl * 4096, nt * rows + 32 * sl, 32 * ks);
                 }
-                for (int gp = 0; gp < np; ++gp)
-                  for (int part = 0; part < 2; ++part)
-                    push_op(pl, m_x[part], a_bytes + (gp * 2 + part) * Bo.part_bytes, 32 * ks, grp[k][gp] * B, 0, 0, 0);
+                for (int gp = 0; gp < np; ++gp) pl.op_pair(m_x, a_bytes + gp * 2 * Bo.part_bytes, Bo.part_bytes, 32 * ks, grp[k][gp] * B);
               }
-              pl.ctas.push_back(c);
+              DZ_TRY(pl.end_cta());
             }
         }
       }
-      n->l_fc.nctas = (int)pl.ctas.size() - n->l_fc.cta0;
+      pl.end_launch(l);
     }
     // ---- input gradient: D[k, m] = sum_n W[k][n] g[m][n];  noisy: W = Wmu + Wsigma * (eps_in[k] * eps_out[n]) in the converters
     {
-      UmOperand Bo = um_kmajor(njt, true, false);
+      const UmOperand Bo = um_kmajor(njt, true, false);
       const int S = n->fcd_splits, per = (16 + S - 1) / S, ktiles = (feat + 127) / 128;
-      n->l_fcd.cta0 = (int)pl.ctas.size(); n->l_fcd.njt = njt;
-      n->l_fcd.stage_bytes = 2 * 16384 + 2 * Bo.part_bytes;
-      n->l_fcd.stages = std::min<int>(kStagesMax, (int)((226 * 1024 - 1024 - kCtlBytes) / n->l_fcd.stage_bytes));
+      UmLaunch& l = n->launches[kFcDgrad];
+      pl.begin_launch(l, njt, 2 * 16384 + 2 * Bo.part_bytes);
       for (int s = 0; s < d.nstream; ++s) {
-        UmProblem pr;
-        memset(&pr, 0, sizeof(pr));
-        pr.A = um_kmajor(128, true, true, nullptr); pr.B = Bo; pr.ksteps = 4; pr.red_per_stage = 32;
+        UmProblem pr = make_problem(um_kmajor(128, true, true, nullptr), Bo, 4, 32, UM_EPI_PARTIAL, feat, B);
         if (d.noisy) pr.A.convert = 2;
-        pr.epi = UM_EPI_PARTIAL; pr.MI = feat; pr.NJ = B;
         pr.C = n->fcd_part + (int64_t)s * S * B * feat; pr.sc_i = 1; pr.sc_j = feat; pr.split_stride = (long long)B * feat;
-        const int prob = (int)pl.probs.size();
-        pl.probs.push_back(pr);
+        const int prob = pl.add_problem(pr);
         if (d.noisy) {
           n->patches.push_back({prob, 0, (int64_t)d.noise_apply[0] * d.noise_stride + d.noise_off_out[s]});
           n->patches.push_back({prob, 2, (int64_t)d.noise_apply[0] * d.noise_stride + d.noise_off_in[s]});
@@ -1377,21 +1320,18 @@ int build_plan(UmNet* n) {
           for (int sp = 0; sp < S; ++sp) {
             const int n0 = sp * per, n1 = std::min(16, n0 + per);
             if (n1 <= n0) continue;
-            UmCta c;
-            memset(&c, 0, sizeof(c));
-            c.prob = (uint32_t)prob; c.op0 = (uint32_t)pl.ops.size(); c.nstages = (uint32_t)(n1 - n0);
-            c.ops_per_stage = d.noisy ? 4 : 3;
-            c.tx_bytes = (uint32_t)((d.noisy ? 32768 : 16384) + 2 * njt * 128);
+            UmCta& c = pl.begin_cta(prob);
             c.r0 = 32 * n0; c.i0 = kt * 128; c.split = sp;
             for (int ns = n0; ns < n1; ++ns) {
-              push_op(pl, m_wd_fc[s][0], 0, 32 * ns, kt * 128, 0, 0, 0);
-              if (d.noisy) push_op(pl, m_wd_fc[s][1], 16384, 32 * ns, kt * 128, 0, 0, 0);
-              for (int part = 0; part < 2; ++part) push_op(pl, m_g[part], 32768 + part * Bo.part_bytes, 32 * ns, s * B, 0, 0, 0);
+              pl.stage();
+              pl.op(m_wd_fc[s][0], 0, 32 * ns, kt * 128);
+              if (d.noisy) pl.op(m_wd_fc[s][1], 16384, 32 * ns, kt * 128);
+              pl.op_pair(m_g, 32768, Bo.part_bytes, 32 * ns, s * B);
             }
-            pl.ctas.push_back(c);
+            DZ_TRY(pl.end_cta());
           }
       }
-      n->l_fcd.nctas = (int)pl.ctas.size() - n->l_fcd.cta0;
+      pl.end_launch(l);
     }
   }
   return DZ_OK;
@@ -1427,17 +1367,8 @@ int net_create(const UmNetDesc& d, char* base, UmNet** out, bool fc_per_pass) {
   n->d = d;
   n->fc_per_pass = fc_per_pass;
   carve_net(n, base);
-  // conv1 geometry
-  const int px = n->h1 * n->w1, m_pass = d.B * px;
-  n->conv1_tiles_per_pass = (m_pass + 127) / 128;
-  int worst = 0;
-  for (int m0 = 0; m0 < m_pass; m0 += 128) {
-    const int m1 = std::min(m0 + 128, m_pass);
-    int tot = 0;
-    for (int b = m0 / px; b <= (m1 - 1) / px; ++b) tot += conv1_segment(b, m0, m1, px, n->w1, d.W * 4).bytes;
-    worst = std::max(worst, tot);
-  }
-  n->conv1_stag_bytes = (worst + 127) / 128 * 128;
+  n->conv1_tiles_per_pass = (d.B * n->h1 * n->w1 + 127) / 128;
+  n->conv1_stag_bytes = conv1_stag_bytes(d.B, d.W, n->h1, n->w1);
   cudaMemset(n->wg_ticket, 0, 64 * 4);
   // gradient buffers start as zeros (hi/lo pairs of layers whose producer has not run yet are never NaN)
   for (int L = 0; L < 3; ++L) {
@@ -1445,9 +1376,8 @@ int net_create(const UmNetDesc& d, char* base, UmNet** out, bool fc_per_pass) {
     cudaMemset(n->dact_hi[L], 0, cnt[L] * 4); cudaMemset(n->dact_lo[L], 0, cnt[L] * 4); cudaMemset(n->dact_f32[L], 0, cnt[L] * 4);
   }
   int rc = build_plan(n);
-  UmLaunch* all[8] = {&n->l_conv2, &n->l_conv3, &n->l_dconv3, &n->l_dconv2, &n->l_fc, &n->l_fcd, &n->l_wconv3, &n->l_wconv2};
-  for (int i = 0; i < 8 && rc == DZ_OK; ++i)
-    if (all[i]->nctas > 0) rc = n->plan.localize_maps(*all[i]);
+  for (int i = 0; i < kNumNetLaunches && rc == DZ_OK; ++i)
+    if (n->launches[i].nctas > 0) rc = n->plan.localize_maps(n->launches[i]);
   if (rc == DZ_OK) rc = n->plan.upload();
   if (rc == DZ_OK) rc = UmPlan::configure();
   if (rc != DZ_OK) { um_net_destroy(n); return rc; }
@@ -1473,12 +1403,11 @@ void um_net_trace(UmNet* n, const char* tag, long long* d_trace) { n->trace_tag 
 int um_net_mma_path(UmNet* n, const char* tag) {
   const std::string t = tag ? tag : "";
   if (t == "conv1_fwd") return UM_PATH_WGMMA;     // conv1_wgmma_kernel (um_forward_torso)
-  const UmLaunch* l = t == "conv2_fwd" ? &n->l_conv2 : t == "conv3_fwd" ? &n->l_conv3 : t == "conv3_dgrad" ? &n->l_dconv3
-                    : t == "conv2_dgrad" ? &n->l_dconv2 : (t == "fc1_fwd" || t == "noisy1_fwd") ? &n->l_fc
-                    : (t == "fc1_dgrad" || t == "noisy1_dgrad") ? &n->l_fcd : t == "conv3_wgrad" ? &n->l_wconv3
-                    : t == "conv2_wgrad" ? &n->l_wconv2 : nullptr;
-  if (!l || l->nctas <= 0) return -1;
-  return n->plan.path_of(*l);
+  for (int i = 0; i < kNumNetLaunches; ++i) {
+    const NetLaunchName& nm = kNetLaunchNames[i];
+    if (t == nm.tag || (nm.noisy && t == nm.noisy)) return n->launches[i].nctas > 0 ? n->plan.path_of(n->launches[i]) : -1;
+  }
+  return -1;
 }
 
 void um_net_destroy(UmNet* n) {
@@ -1507,7 +1436,7 @@ int um_pack_weights(UmNet* n, void* stream) {
   for (int b = 0; b < 2; ++b)
     for (int L = 0; L < 3; ++L) { a.wf_hi[b][L] = n->wf_hi[b][L]; a.wf_lo[b][L] = n->wf_lo[b][L]; }
   a.wd3_hi = n->wd3_hi; a.wd3_lo = n->wd3_lo; a.wd2_hi = n->wd2_hi; a.wd2_lo = n->wd2_lo;
-  const int total = 2 * 77824 + 64 * 576 + 128 * 256;
+  const int total = 2 * kConvFwdFloats + kConvN[2] * kConvK[2] + kConvN[1] * kConvK[1];
   DZ_LAUNCH_NAMED("conv_pack", um_pack_conv_kernel, (unsigned)ceil_div(total, 256), 256, 0, stream, a);
   return DZ_OK;
 }
@@ -1530,19 +1459,25 @@ int launch_conv1(UmNet* n, const uint8_t* const* const* rows, void* stream, bool
   a.npass = d.npass; a.B = d.B; a.W = d.W; a.oh = n->h1; a.ow = n->w1; a.m_pass = d.B * n->h1 * n->w1;
   a.tiles_per_pass = n->conv1_tiles_per_pass; a.ntiles = a.tiles_per_pass * d.npass; a.stag_bytes = n->conv1_stag_bytes;
   a.trace = n->tr("conv1_fwd");
-  const size_t smem = 2048 + kC1W + (reference ? kC1A : 0) + 2 * (size_t)a.stag_bytes;   // conv1_wgmma_kernel has no A tile
+  const size_t smem = conv1_smem_bytes(kC1W + (reference ? kC1A : 0), a.stag_bytes);   // conv1_wgmma_kernel has no A tile
   if (smem > 227 * 1024) return fail(DZ_EINVAL, "conv1 staging does not fit");
   const unsigned grid = (unsigned)std::min(kNumSMs, a.ntiles);
   if (reference) DZ_LAUNCH_NAMED("conv1_fwd", conv1_umma_kernel, grid, kThreadsU, smem, stream, a);
   else DZ_LAUNCH_NAMED("conv1_fwd", conv1_wgmma_kernel, grid, kThreadsC1W, smem, stream, a);
   return DZ_OK;
 }
+
+// Launch `id` of the plan under its name; it writes CTA 0's clock stamps when the trace is set on its tag.
+int run_launch(UmNet* n, NetLaunch id, void* stream) {
+  const NetLaunchName& nm = kNetLaunchNames[id];
+  return n->plan.launch(n->d.noisy && nm.noisy ? nm.noisy : nm.tag, n->launches[id], stream, n->tr(nm.tag));
+}
 }  // namespace
 
 int um_forward_torso(UmNet* n, const uint8_t* const* const* rows, void* stream) {
   DZ_TRY(launch_conv1(n, rows, stream, false));
-  DZ_TRY(n->plan.launch("conv2_fwd", n->l_conv2, stream, n->tr("conv2_fwd")));
-  DZ_TRY(n->plan.launch("conv3_fwd", n->l_conv3, stream, n->tr("conv3_fwd")));
+  DZ_TRY(run_launch(n, kConv2Fwd, stream));
+  DZ_TRY(run_launch(n, kConv3Fwd, stream));
   return DZ_OK;
 }
 
@@ -1550,7 +1485,7 @@ int um_forward_fc(UmNet* n, const float* noise, void* stream) {
   const UmNetDesc& d = n->d;
   if (!d.use_fc) return fail(DZ_EINVAL, "fc layers are not on the tensor-core path for this agent");
   if (d.noisy) DZ_TRY(apply_noise(n, noise, stream));
-  DZ_TRY(n->plan.launch(d.noisy ? "noisy1_fwd" : "fc1_fwd", n->l_fc, stream, n->tr("fc1_fwd")));
+  DZ_TRY(run_launch(n, kFcFwd, stream));
   FcFinishArgs a;
   memset(&a, 0, sizeof(a));
   a.part = n->fc_part; a.S = n->fc_splits; a.B = d.B; a.nstream = d.nstream; a.noisy = d.noisy; a.npass = d.npass; a.h1 = n->h1_buf;
@@ -1576,7 +1511,7 @@ int um_backward_fc(UmNet* n, const float* noise, void* stream) {
   const UmNetDesc& d = n->d;
   if (!d.use_fc) return fail(DZ_EINVAL, "fc layers are not on the tensor-core path for this agent");
   if (d.noisy) DZ_TRY(apply_noise(n, noise, stream));
-  DZ_TRY(n->plan.launch(d.noisy ? "noisy1_dgrad" : "fc1_dgrad", n->l_fcd, stream, n->tr("fc1_dgrad")));
+  DZ_TRY(run_launch(n, kFcDgrad, stream));
   const long long total = (long long)d.B * n->feat;
   DZ_LAUNCH_NAMED("fcd_finish", um_fcd_finish_kernel, (unsigned)std::min<long long>(ceil_div(total / 4, 256), kNumSMs * 4), 256, 0, stream,
                   n->fcd_part, n->fcd_nsrc * n->fcd_splits, total, n->act_hi[2], n->dact_f32[2], n->dact_hi[2], n->dact_lo[2], total / 4);
@@ -1594,18 +1529,18 @@ int um_wgrad_conv1(UmNet* n, const uint8_t* const* rows0, void* stream) {
   a.rows = rows0; a.gmap[0] = n->plan.maps[n->map_g1[0]]; a.gmap[1] = n->plan.maps[n->map_g1[1]]; a.partial = n->wg1_part;
   a.B = d.B; a.W = d.W; a.oh = n->h1; a.ow = n->w1; a.m_pass = d.B * n->h1 * n->w1;
   a.ntiles = (a.m_pass + 127) / 128; a.stag_bytes = n->conv1_stag_bytes;
-  const size_t smem = 2048 + kC1G + kC1A + 2 * (size_t)a.stag_bytes;
+  const size_t smem = conv1_smem_bytes(kC1G + kC1A, a.stag_bytes);
   if (smem > 227 * 1024) return fail(DZ_EINVAL, "conv1 wgrad staging does not fit");
   DZ_LAUNCH_NAMED("conv1_wgrad", conv1_wgrad_umma_kernel, (unsigned)n->wg1_ctas, kThreadsU, smem, stream, a);
   return DZ_OK;
 }
 
-int um_wgrad_conv3(UmNet* n, void* stream) { return n->plan.launch("conv3_wgrad", n->l_wconv3, stream, n->tr("conv3_wgrad")); }
-int um_wgrad_conv2(UmNet* n, void* stream) { return n->plan.launch("conv2_wgrad", n->l_wconv2, stream, n->tr("conv2_wgrad")); }
+int um_wgrad_conv3(UmNet* n, void* stream) { return run_launch(n, kConv3Wgrad, stream); }
+int um_wgrad_conv2(UmNet* n, void* stream) { return run_launch(n, kConv2Wgrad, stream); }
 
 // dW / db of conv3 and conv2 from the split partials (+ optionally conv1's FMA partials in the same launch).
 namespace {
-int wg_sum_blocks(int layer) { const int KN[3] = {256 * 32, 512 * 64, 576 * 64}; return (KN[layer - 1] / 4 + 31) / 32; }
+int wg_sum_blocks(int layer) { return (kConvN[layer - 1] * kConvK[layer - 1] / 4 + 31) / 32; }
 int wg_slot_base(int layer) { int b = 0; for (int L = 3; L > layer; --L) b += wg_sum_blocks(L) + 1; return b; }
 }  // namespace
 
@@ -1628,8 +1563,8 @@ int um_wgrad_finish_layer(UmNet* n, int layer, float* dW, float* db, float* norm
   return DZ_OK;
 }
 
-int um_backward_conv3(UmNet* n, void* stream) { return n->plan.launch("conv3_dgrad", n->l_dconv3, stream, n->tr("conv3_dgrad")); }
-int um_backward_conv2(UmNet* n, void* stream) { return n->plan.launch("conv2_dgrad", n->l_dconv2, stream, n->tr("conv2_dgrad")); }
+int um_backward_conv3(UmNet* n, void* stream) { return run_launch(n, kConv3Dgrad, stream); }
+int um_backward_conv2(UmNet* n, void* stream) { return run_launch(n, kConv2Dgrad, stream); }
 
 }  // namespace dz
 
@@ -1667,7 +1602,7 @@ extern "C" int dz_test_fc_forward(int32_t B, int32_t H, int32_t W, int32_t npass
   int rc = net_create(d, ws, &n, per_pass != 0);
   if (rc == DZ_OK) rc = um_split(x, n->act_hi[2], n->act_lo[2], (long long)n->PB * n->feat, stream);
   if (rc == DZ_OK && noisy) rc = apply_noise(n, noise, stream);
-  if (rc == DZ_OK) rc = n->plan.launch("fc1_fwd", n->l_fc, stream, nullptr, per_pass ? UM_PATH_CONVERTERS : UM_PATH_AUTO);
+  if (rc == DZ_OK) rc = n->plan.launch("fc1_fwd", n->launches[kFcFwd], stream, nullptr, per_pass ? UM_PATH_CONVERTERS : UM_PATH_AUTO);
   if (rc == DZ_OK) {
     const size_t bytes = (size_t)npass * nstream * n->fc_splits * B * 512 * sizeof(float);
     if (cudaMemcpyAsync(d_part, n->fc_part, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream) != cudaSuccess ||
@@ -1677,7 +1612,8 @@ extern "C" int dz_test_fc_forward(int32_t B, int32_t H, int32_t W, int32_t npass
   if (rc == DZ_OK) {
     *splits = n->fc_splits;
     int64_t wb = 0;
-    for (int ci = n->l_fc.cta0; ci < n->l_fc.cta0 + n->l_fc.nctas; ++ci) {
+    const UmLaunch& l = n->launches[kFcFwd];
+    for (int ci = l.cta0; ci < l.cta0 + l.nctas; ++ci) {
       const UmCta& c = n->plan.ctas[ci];
       wb += (int64_t)c.nstages * (noisy ? 2 : 1) * n->plan.probs[c.prob].A.part_bytes;
     }
