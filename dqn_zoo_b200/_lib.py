@@ -35,6 +35,13 @@ class AddRecord(C.Structure):
               ('release_row', i32)]
 
 
+class AddBatch(C.Structure):   # struct dz_add_batch
+  _fields_ = [('count', i32), ('first_slot', i64), ('d_action', vp), ('d_reward', vp), ('d_discount', vp),
+              ('d_release_row', vp), ('d_tree_index', vp), ('d_evict_index', vp), ('d_leaf_value', vp),
+              ('d_priority', vp), ('alpha', f64), ('n_patches', i32), ('d_patch_pos', vp), ('d_patch_val', vp),
+              ('d_patch_target', vp), ('s_tm1', vp), ('s_t', vp), ('src_pitch', i64)]
+
+
 class SampleInputs(C.Structure):
   _fields_ = [('d_rand_pos', vp), ('d_u_tree', vp), ('d_u_mix', vp), ('d_scalars', vp)]
 
@@ -97,6 +104,8 @@ _SIGNATURES = {
     'dz_sumtree_query': (i32, [vp, i64, vp, i64, vp, vp, vp]),
     'dz_sumtree_get': (i32, [vp, i64, i64, vp, i64, vp, vp, vp]),
     'dz_replay_add': (i32, [C.POINTER(ReplayView), C.POINTER(AddRecord), vp, vp, vp]),
+    'dz_replay_add_batch_workspace': (i32, [C.POINTER(ReplayView), C.POINTER(i32), C.POINTER(i64)]),
+    'dz_replay_add_batch': (i32, [C.POINTER(ReplayView), C.POINTER(AddBatch), vp, i64, vp]),
     'dz_replay_fill_synthetic': (i32, [C.POINTER(ReplayView), i64, i64, u64, i32, f64, vp]),
     'dz_replay_fill_synthetic_stacked': (i32, [C.POINTER(ReplayView), i64, u64, i64, i32, f64, vp]),
     'dz_replay_frame_pool_reset': (i32, [C.POINTER(ReplayView), vp]),

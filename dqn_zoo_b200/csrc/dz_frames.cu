@@ -153,6 +153,244 @@ __global__ void __launch_bounds__(512) frame_add_kernel(dz_replay_view v, int64_
   }
 }
 
+// ---- batched add (dz_replay_add_batch) -------------------------------------------------------------------------------
+// The K adds of a batch have N = K * P planes, plane q = k * P + p.  Phases:
+//   1. frame_batch_planes_kernel (a CTA per observation): de-interleave into the planar workspace, hash each plane; gather
+//      the plane ids of the rows the batch overwrites.
+//   2. frame_batch_match_kernel (a warp per plane): rep[q] = the first plane of the batch with the same bytes, and for
+//      each such representative the plane live at batch start with the same bytes.  The only phase that compares bytes.
+//   3. frame_batch_resolve_kernel (one CTA, one thread for the rules): replays the pool rules of the K adds on integers in
+//      shared memory, then writes rows, refcounts, the free stack and erases the freed planes from the table.
+//   4. frame_batch_insert_kernel (a warp per popped plane): bytes, hash and table entry of every plane that ends the
+//      batch holding new content.
+// Every plane id the batch touches gets a local slot ("loc") in phase 3: [0, N) the batch-start matches, [N, 2N) the ids
+// of the overwritten rows, [2N, 3N) the top N entries of the free stack, 3N plane 0.  id_loc[id] (workspace, indexed by
+// plane id, written by phases 1-2 and read in phase 3 only) picks one canonical loc per id: any writer may win.
+
+struct FrameBatchWs {
+  uint8_t* planar;    // [N][frame_stride]
+  uint64_t* hash;     // [N]
+  int32_t* rep;       // [N]
+  int32_t* match;     // [N] (representatives only; -1 = no live plane with these bytes)
+  int32_t* old;       // [N] plane ids of the overwritten rows at batch start
+  int32_t* pop_id;    // [N] planes popped by phase 3, in pop order
+  int32_t* pop_cls;   // [N] the representative plane whose bytes each popped plane takes
+  int32_t* counts;    // [1] pops
+  int32_t* id_loc;    // [frame_capacity]
+};
+
+static int64_t align256(int64_t x) { return (x + 255) / 256 * 256; }
+
+static FrameBatchWs frame_batch_ws(const dz_replay_view* v, int64_t max_count, uint8_t* base, int64_t* total) {
+  const int64_t N = max_count * 2 * v->obs_channels;
+  FrameBatchWs w{};
+  int64_t off = 0;
+  auto take = [&](int64_t bytes) { uint8_t* p = base ? base + off : nullptr; off += align256(bytes); return p; };
+  w.planar = take(N * v->frame_stride);
+  w.hash = reinterpret_cast<uint64_t*>(take(N * 8));
+  w.rep = reinterpret_cast<int32_t*>(take(N * 4));
+  w.match = reinterpret_cast<int32_t*>(take(N * 4));
+  w.old = reinterpret_cast<int32_t*>(take(N * 4));
+  w.pop_id = reinterpret_cast<int32_t*>(take(N * 4));
+  w.pop_cls = reinterpret_cast<int32_t*>(take(N * 4));
+  w.counts = reinterpret_cast<int32_t*>(take(4));
+  w.id_loc = reinterpret_cast<int32_t*>(take(v->frame_capacity * 4));
+  if (total) *total = off;
+  return w;
+}
+
+static __device__ __forceinline__ bool warp_planes_equal(const uint8_t* a, const uint8_t* b, int64_t frame_stride) {
+  const uint4* x = reinterpret_cast<const uint4*>(a);
+  const uint4* y = reinterpret_cast<const uint4*>(b);
+  int diff = 0;
+  for (int64_t i = threadIdx.x & 31; i < (frame_stride >> 4); i += 32) {
+    const uint4 u = x[i], w = y[i];
+    diff |= (u.x != w.x) | (u.y != w.y) | (u.z != w.z) | (u.w != w.w);
+  }
+  return !__any_sync(0xffffffffu, diff);
+}
+
+__global__ void __launch_bounds__(256) frame_batch_planes_kernel(dz_replay_view v, dz_add_batch b,
+                                                                 const uint8_t* __restrict__ src_tm1,
+                                                                 const uint8_t* __restrict__ src_t, int64_t pitch,
+                                                                 FrameBatchWs w) {
+  dz::pdl_enter();
+  const int C = (int)v.obs_channels, P = 2 * C;
+  const int k = blockIdx.x >> 1, o = blockIdx.x & 1;
+  const int64_t N = (int64_t)b.count * P, fb = v.frame_bytes, fs = v.frame_stride;
+  const uint8_t* src = (o ? src_t : src_tm1) + k * pitch;
+  const int64_t q0 = (int64_t)k * P + o * C;
+  uint8_t* dst = w.planar + q0 * fs;
+  for (int64_t i = threadIdx.x; i < fs; i += blockDim.x)
+    for (int c = 0; c < C; ++c) dst[c * fs + i] = i < fb ? src[i * C + c] : 0;
+  __syncthreads();
+  for (int c = threadIdx.x >> 5; c < C; c += blockDim.x >> 5) {
+    const uint64_t h = plane_hash_warp(dst + c * fs, fs);
+    if ((threadIdx.x & 31) == 0) w.hash[q0 + c] = h;
+  }
+  if (o == 0 && threadIdx.x < P) {
+    const int64_t slot = (b.first_slot + k) % v.capacity;
+    const int32_t id = v.d_planes[slot * P + threadIdx.x];
+    w.old[(int64_t)k * P + threadIdx.x] = id;
+    if (b.d_release_row[k] && id > 0) w.id_loc[id] = (int32_t)(N + (int64_t)k * P + threadIdx.x);
+  }
+  if (blockIdx.x == 0) {
+    const int64_t top = v.d_pool_counters[0];
+    for (int64_t j = threadIdx.x; j < N && j < top; j += blockDim.x) w.id_loc[v.d_free[top - 1 - j]] = (int32_t)(2 * N + j);
+  }
+}
+
+__global__ void __launch_bounds__(256) frame_batch_match_kernel(dz_replay_view v, int32_t N, FrameBatchWs w) {
+  dz::pdl_enter();
+  const int q = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5);
+  if (q >= N) return;
+  const int lane = threadIdx.x & 31;
+  const int64_t fs = v.frame_stride;
+  const uint64_t h = w.hash[q];
+  const uint8_t* mine = w.planar + (int64_t)q * fs;
+  int rep = q;
+  for (int base = 0; base < q && rep == q; base += 32) {
+    const int c = base + lane;
+    unsigned m = __ballot_sync(0xffffffffu, c < q && w.hash[c] == h);
+    while (m) {
+      const int cand = base + __ffs((int)m) - 1;
+      if (warp_planes_equal(w.planar + (int64_t)cand * fs, mine, fs)) { rep = cand; break; }
+      m &= m - 1;
+    }
+  }
+  if (lane == 0) w.rep[q] = rep;
+  if (rep != q) return;
+  const int64_t mask = v.table_size - 1;
+  int32_t found = -1;
+  for (int64_t t = (int64_t)(h & (uint64_t)mask);; t = (t + 1) & mask) {
+    const int32_t cand = v.d_table[t];
+    if (cand < 0) break;
+    if (v.d_hashes[cand] == h && warp_planes_equal(pool_plane(v, cand), mine, fs)) { found = cand; break; }
+  }
+  if (lane == 0) {
+    w.match[q] = found;
+    if (found > 0) w.id_loc[found] = q;
+  }
+}
+
+__global__ void __launch_bounds__(512) frame_batch_resolve_kernel(dz_replay_view v, dz_add_batch b, FrameBatchWs w) {
+  dz::pdl_enter();
+  const int C = (int)v.obs_channels, P = 2 * C, K = b.count, N = K * P, L = 3 * N + 1;
+  extern __shared__ int32_t sm[];
+  int32_t* ref = sm;               // [L] refcount of each loc
+  int32_t* cls_of = ref + L;       // [L] representative plane whose bytes the loc holds (-1: none in this batch)
+  int32_t* loc2id = cls_of + L;    // [L] plane id of the loc (-1: not a canonical loc)
+  int32_t* cls_loc = loc2id + L;   // [N] loc holding the bytes of representative q, -1 = none live
+  int32_t* rep = cls_loc + N;      // [N]
+  int32_t* loc_old = rep + N;      // [N] loc of the plane the overwritten row held (-1: row not released)
+  int32_t* new_loc = loc_old + N;  // [N]
+  int32_t* pushed = new_loc + N;   // [N] locs pushed onto the free stack by this batch, bottom first
+  int32_t* freed = pushed + N;     // [N]
+  int32_t* release = freed + N;    // [K]
+  __shared__ int s_pops_init, s_pushed;
+  const int64_t top0 = v.d_pool_counters[0];
+  auto loc_of = [&](int32_t id) { return id == 0 ? 3 * N : w.id_loc[id]; };
+  for (int k = threadIdx.x; k < K; k += blockDim.x) release[k] = b.d_release_row[k];
+  __syncthreads();
+  for (int e = threadIdx.x; e < L; e += blockDim.x) {
+    int32_t id = -1;
+    if (e == 3 * N) id = 0;
+    else if (e >= 2 * N) id = e - 2 * N < top0 ? v.d_free[top0 - 1 - (e - 2 * N)] : -1;
+    else if (e >= N) id = release[(e - N) / P] ? w.old[e - N] : -1;
+    else if (w.rep[e] == e) id = w.match[e];
+    const bool canonical = id == 0 ? e == 3 * N : (id > 0 && (e >= 2 * N || w.id_loc[id] == e));
+    loc2id[e] = canonical ? id : -1;
+    ref[e] = canonical && e < 2 * N ? v.d_refcount[id] : (e == 3 * N ? v.d_refcount[0] : 0);
+    cls_of[e] = -1;
+  }
+  __syncthreads();
+  for (int q = threadIdx.x; q < N; q += blockDim.x) {
+    const int r = w.rep[q];
+    rep[q] = r;
+    loc_old[q] = release[q / P] ? loc_of(w.old[q]) : -1;
+    cls_loc[q] = -1;
+    if (r == q && w.match[q] >= 0) {
+      const int loc = loc_of(w.match[q]);
+      cls_loc[q] = loc;
+      if (loc != 3 * N) cls_of[loc] = q;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    // the pool rules of frame_add_kernel, add after add: resolve, reference, then release the overwritten row
+    int pops_init = 0, npush = 0, nfreed = 0, npop = 0;
+    bool full = false;
+    for (int k = 0; k < K; ++k) {
+      for (int q = k * P; q < (k + 1) * P; ++q) {
+        const int c = rep[q];
+        int loc = cls_loc[c];
+        if (loc < 0) {
+          if (npush > 0) loc = pushed[--npush];
+          else if (pops_init < top0) loc = 2 * N + pops_init++;
+          if (loc < 0) {
+            full = true;
+            loc = 3 * N;
+          } else {
+            ref[loc] = 0;
+            cls_loc[c] = loc;
+            cls_of[loc] = c;
+            w.pop_id[npop] = loc2id[loc];
+            w.pop_cls[npop] = c;
+            ++npop;
+          }
+        }
+        ref[loc] += 1;
+        new_loc[q] = loc;
+      }
+      if (release[k]) {
+        for (int q = k * P; q < (k + 1) * P; ++q) {
+          const int loc = loc_old[q];
+          if (--ref[loc] == 0) {
+            pushed[npush++] = loc;
+            freed[nfreed++] = loc;
+            const int c = cls_of[loc];
+            if (c >= 0 && cls_loc[c] == loc) cls_loc[c] = -1;
+          }
+        }
+      }
+    }
+    // every freed plane was live at batch start, so it is in the table under its old hash
+    for (int i = 0; i < nfreed; ++i) table_erase(v, loc2id[freed[i]]);
+    if (full && v.d_flags) atomicOr(v.d_flags, DZ_FLAG_FRAME_POOL_FULL);
+    w.counts[0] = npop;
+    s_pops_init = pops_init;
+    s_pushed = npush;
+  }
+  __syncthreads();
+  const int pops_init = s_pops_init, npush = s_pushed;
+  for (int e = threadIdx.x; e < L; e += blockDim.x)
+    if (loc2id[e] >= 0 && (e < 2 * N || e == 3 * N || e - 2 * N < pops_init)) v.d_refcount[loc2id[e]] = ref[e];
+  for (int i = threadIdx.x; i < npush; i += blockDim.x) v.d_free[top0 - pops_init + i] = loc2id[pushed[i]];
+  if (threadIdx.x == 0) v.d_pool_counters[0] = top0 - pops_init + npush;
+  for (int q = threadIdx.x; q < N; q += blockDim.x) {
+    const int64_t slot = (b.first_slot + q / P) % v.capacity;
+    v.d_planes[slot * P + q % P] = loc2id[new_loc[q]];
+  }
+}
+
+__global__ void __launch_bounds__(256) frame_batch_insert_kernel(dz_replay_view v, int32_t N, FrameBatchWs w) {
+  dz::pdl_enter();
+  const int i = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5);
+  if (i >= N || i >= w.counts[0]) return;
+  const int32_t id = w.pop_id[i];
+  const int c = w.pop_cls[i];
+  const uint4* src = reinterpret_cast<const uint4*>(w.planar + (int64_t)c * v.frame_stride);
+  uint4* dst = reinterpret_cast<uint4*>(const_cast<uint8_t*>(pool_plane(v, id)));
+  for (int64_t j = threadIdx.x & 31; j < (v.frame_stride >> 4); j += 32) dst[j] = src[j];
+  if ((threadIdx.x & 31) == 0) {
+    const uint64_t h = w.hash[c];
+    v.d_hashes[id] = h;
+    const int64_t mask = v.table_size - 1;
+    int64_t t = (int64_t)(h & (uint64_t)mask);
+    while (atomicCAS(&v.d_table[t], -1, id) != -1) t = (t + 1) & mask;
+  }
+}
+
 // Plane ids -> HWC stacks.  blockIdx.x = 2 * b + which (s_tm1 / s_t of batch entry b), blockIdx.y splits the row.
 // C == 4 with 4-byte planes and a 16-byte aligned destination: each thread reads 4 pixels of each plane (one 32-bit
 // word per plane) and writes their 16 interleaved bytes as one uint4 (a 4x4 byte transpose with prmt).
@@ -278,6 +516,34 @@ int launch_frame_add(const dz_replay_view* view, int64_t slot, int release_row, 
                      const uint8_t* src_t, void* stream) {
   DZ_TRY(check_pool_view(view));
   DZ_LAUNCH(frame_add_kernel, 1, 512, 0, stream, *view, slot, release_row, src_tm1, src_t);
+  return DZ_OK;
+}
+
+int64_t frame_add_batch_workspace(const dz_replay_view* view, int64_t max_count) {
+  int64_t total = 0;
+  frame_batch_ws(view, max_count, nullptr, &total);
+  return total;
+}
+
+static size_t resolve_smem_bytes(int64_t N, int64_t K) { return (size_t)(3 * (3 * N + 1) + 6 * N + K) * 4; }
+
+int launch_frame_add_batch(const dz_replay_view* view, const dz_add_batch* b, const uint8_t* src_tm1,
+                           const uint8_t* src_t, int64_t pitch, uint8_t* ws, void* stream) {
+  DZ_TRY(check_pool_view(view));
+  const int64_t K = b->count, N = K * 2 * view->obs_channels;
+  if (N > kMaxBatchPlanes) return fail(DZ_EINVAL, "frame-deduplicated batch has more than kMaxBatchPlanes planes");
+  static bool smem_set = false;
+  if (!smem_set) {
+    DZ_CUDA_OK(cudaFuncSetAttribute(frame_batch_resolve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)resolve_smem_bytes(kMaxBatchPlanes, kMaxAddBatch)));
+    smem_set = true;
+  }
+  const FrameBatchWs w = frame_batch_ws(view, K, ws, nullptr);
+  const int warp_grid = (int)ceil_div(N * 32, 256);
+  DZ_LAUNCH(frame_batch_planes_kernel, (int)(2 * K), 256, 0, stream, *view, *b, src_tm1, src_t, pitch, w);
+  DZ_LAUNCH(frame_batch_match_kernel, warp_grid, 256, 0, stream, *view, (int32_t)N, w);
+  DZ_LAUNCH(frame_batch_resolve_kernel, 1, 512, resolve_smem_bytes(N, K), stream, *view, *b, w);
+  DZ_LAUNCH(frame_batch_insert_kernel, warp_grid, 256, 0, stream, *view, (int32_t)N, w);
   return DZ_OK;
 }
 

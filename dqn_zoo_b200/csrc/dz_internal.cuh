@@ -39,6 +39,15 @@ int launch_frame_add(const dz_replay_view* view, int64_t slot, int release_row, 
 // HWC stacks of rows slots[0..batch): s_tm1 of b at dst_tm1 + b * pitch, s_t at dst_t + b * pitch.
 int launch_frame_reconstruct(const dz_replay_view* view, const int64_t* d_slots, int batch, uint8_t* dst_tm1,
                              uint8_t* dst_t, int64_t pitch, void* stream);
+// Batched add (dz_replay_add_batch): at most kMaxAddBatch adds per call (2 * K leaf writes in one block_tree_set), and
+// in the frame-deduplicated layout at most kMaxBatchPlanes = K * 2 * C planes (the resolve kernel's shared memory).
+constexpr int kMaxAddBatch = 512;
+constexpr int kMaxBatchPlanes = 2048;
+// Workspace bytes of the frame pool's part of a batch of up to max_count adds (the planar planes and the match results).
+int64_t frame_add_batch_workspace(const dz_replay_view* view, int64_t max_count);
+// Plane ids of the rows of `b` (observations at src_tm1 / src_t + k * pitch, device memory); ws: frame_add_batch_workspace bytes.
+int launch_frame_add_batch(const dz_replay_view* view, const dz_add_batch* b, const uint8_t* src_tm1,
+                           const uint8_t* src_t, int64_t pitch, uint8_t* ws, void* stream);
 int launch_frame_pool_reset(const dz_replay_view* view, void* stream);
 int launch_frame_fill_stacked(const dz_replay_view* view, int64_t n, uint64_t seed, int64_t episode_len, void* stream);
 

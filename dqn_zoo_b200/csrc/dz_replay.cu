@@ -457,6 +457,71 @@ __global__ void __launch_bounds__(64) apply_add_kernel(dz_replay_view v, dz_add_
   if (rec.tree_index >= 0 && v.d_tree) block_tree_set(v.d_tree, v.first_leaf, s_idx, s_val, 2);
 }
 
+// Batched add (dz_replay_add_batch).  Blocks 0 .. 2K-1 (transition-major layout only) copy observation (k, o) into its
+// row; the last block writes the scalars, applies the list patches in order on one thread, and sets the 2K leaves
+// (evict_k, 0), (tree_k, leaf_k) in k order: last write wins, and every ancestor is resummed from the final leaves, which
+// is what K sequential apply_add_kernel calls leave.
+__global__ void __launch_bounds__(256) apply_add_batch_kernel(dz_replay_view v, dz_add_batch b,
+                                                              const uint8_t* __restrict__ src_tm1,
+                                                              const uint8_t* __restrict__ src_t, int64_t pitch,
+                                                              int vec16) {
+  dz::pdl_enter();
+  const int K = b.count;
+  if (blockIdx.x + 1 < gridDim.x) {
+    const int k = blockIdx.x >> 1, o = blockIdx.x & 1;
+    const int64_t slot = (b.first_slot + k) % v.capacity;
+    const uint8_t* src = (o ? src_t : src_tm1) + k * pitch;
+    uint8_t* dst = v.d_obs + (slot * 2 + o) * v.obs_stride;
+    if (vec16) {
+      const uint4* s4 = reinterpret_cast<const uint4*>(src);
+      uint4* d4 = reinterpret_cast<uint4*>(dst);
+      for (int64_t i = threadIdx.x; i < (v.obs_bytes >> 4); i += blockDim.x) d4[i] = s4[i];
+    } else {
+      for (int64_t i = threadIdx.x; i < v.obs_bytes; i += blockDim.x) dst[i] = src[i];
+    }
+    return;
+  }
+  __shared__ int64_t s_idx[2 * kMaxAddBatch];
+  __shared__ double s_val[2 * kMaxAddBatch];
+  __shared__ double s_dev_leaf;
+  for (int k = threadIdx.x; k < K; k += blockDim.x) {
+    const int64_t slot = (b.first_slot + k) % v.capacity;
+    v.d_action[slot] = b.d_action[k];
+    v.d_reward[slot] = b.d_reward[k];
+    v.d_discount[slot] = b.d_discount[k];
+  }
+  if (threadIdx.x == 0) {
+    for (int p = 0; p < b.n_patches; ++p) {
+      int64_t* dst = b.d_patch_target[p] == 0 ? v.d_live : (b.d_patch_target[p] == 1 ? v.d_id_at : v.d_ids);
+      dst[b.d_patch_pos[p]] = b.d_patch_val[p];
+    }
+    if (b.d_priority) {  // as apply_add_kernel: one device priority shared by the K adds
+      double pr = (double)b.d_priority[0];
+      if (!finite_nonneg(pr)) {
+        if (v.d_flags) atomicOr(v.d_flags, DZ_FLAG_BAD_VALUE);
+        pr = 0.0;
+      }
+      s_dev_leaf = pr == 0.0 ? 0.0 : (b.alpha == 0.5 ? __dsqrt_rn(pr) : (b.alpha == 1.0 ? pr : pow(pr, b.alpha)));
+    }
+  }
+  if (!b.d_tree_index || !v.d_tree) return;
+  __syncthreads();
+  for (int k = threadIdx.x; k < K; k += blockDim.x) {
+    int64_t ev = b.d_evict_index[k], ti = b.d_tree_index[k];
+    if (ev >= v.first_leaf || ti >= v.first_leaf) {
+      if (v.d_flags) atomicOr(v.d_flags, DZ_FLAG_BAD_INDEX);
+      ev = ev >= v.first_leaf ? -1 : ev;
+      ti = ti >= v.first_leaf ? -1 : ti;
+    }
+    s_idx[2 * k] = ev;
+    s_val[2 * k] = 0.0;
+    s_idx[2 * k + 1] = ti;
+    s_val[2 * k + 1] = b.d_priority ? s_dev_leaf : b.d_leaf_value[k];
+  }
+  __syncthreads();
+  block_tree_set(v.d_tree, v.first_leaf, s_idx, s_val, 2 * K);
+}
+
 __global__ void __launch_bounds__(256) fill_obs_kernel(dz_replay_view v, int64_t row0, int64_t n, uint64_t seed) {
   dz::pdl_enter();
   const int64_t words = v.obs_bytes >> 3;
@@ -672,6 +737,79 @@ int dz_replay_add(const dz_replay_view* view, const dz_add_record* rec, const ui
   if (h_s_t)
     DZ_CUDA_OK(cudaMemcpyAsync(row + view->obs_stride, h_s_t, view->obs_bytes, cudaMemcpyDefault, (cudaStream_t)stream));
   DZ_LAUNCH(apply_add_kernel, 1, 64, 0, stream, *view, *rec);
+  return DZ_OK;
+}
+
+// Workspace of dz_replay_add_batch: [max_count][2][obs_stride] host-source copies, then the frame pool's part.
+static int64_t add_batch_stage_bytes(const dz_replay_view* view, int64_t max_count) {
+  return (max_count * 2 * view->obs_stride + 255) / 256 * 256;
+}
+
+static int64_t add_batch_bytes(const dz_replay_view* view, int64_t max_count) {
+  return add_batch_stage_bytes(view, max_count) + (view->d_planes ? frame_add_batch_workspace(view, max_count) : 0);
+}
+
+int dz_replay_add_batch_workspace(const dz_replay_view* view, int32_t* max_count, int64_t* bytes) {
+  if (*max_count < 1) return fail(DZ_EINVAL, "max_count must be positive");
+  if (view->obs_bytes <= 0 || view->obs_stride < view->obs_bytes) return fail(DZ_EINVAL, "observation layout not set");
+  int64_t m = *max_count < kMaxAddBatch ? *max_count : kMaxAddBatch;
+  if (view->d_planes) {
+    if (view->obs_channels < 1 || view->obs_channels > kMaxObsChannels) return fail(DZ_EINVAL, "obs_channels must be in [1,32]");
+    const int64_t planes_max = kMaxBatchPlanes / (2 * view->obs_channels);
+    m = m < planes_max ? m : planes_max;
+  }
+  *max_count = (int32_t)m;
+  *bytes = add_batch_bytes(view, m);
+  return DZ_OK;
+}
+
+int dz_replay_add_batch(const dz_replay_view* view, const dz_add_batch* b, void* d_workspace, int64_t workspace_bytes,
+                        void* stream) {
+  const int64_t K = b->count;
+  if (K < 0) return fail(DZ_EINVAL, "count must be >= 0");
+  if (K == 0) return DZ_OK;
+  if (K > view->capacity) return fail(DZ_ERANGE, "count exceeds the capacity");
+  if (b->first_slot < 0 || b->first_slot >= view->capacity) return fail(DZ_ERANGE, "first_slot out of range");
+  int32_t most = (int32_t)(K < INT32_MAX ? K : INT32_MAX);
+  int64_t need = 0;
+  DZ_TRY(dz_replay_add_batch_workspace(view, &most, &need));
+  if (most < K || need > workspace_bytes || !d_workspace) return fail(DZ_EINVAL, "count exceeds the workspace");
+  if (b->n_patches < 0 || b->n_patches > 4 * K) return fail(DZ_EINVAL, "at most 4 patches per add");
+  if (b->n_patches && (!b->d_patch_pos || !b->d_patch_val || !b->d_patch_target)) return fail(DZ_EINVAL, "patch arrays missing");
+  if (!b->d_action || !b->d_reward || !b->d_discount || !b->d_release_row) return fail(DZ_EINVAL, "scalar arrays missing");
+  if (b->d_tree_index && (!b->d_evict_index || (!b->d_leaf_value && !b->d_priority)))
+    return fail(DZ_EINVAL, "prioritized add needs evict indices and leaf values");
+  if (!b->s_tm1 || !b->s_t) return fail(DZ_EINVAL, "both observations are required");
+  if (b->src_pitch < view->obs_bytes) return fail(DZ_EINVAL, "src_pitch < obs_bytes");
+  // host sources: one 2-D copy per observation field into [K][2][obs_stride]; device sources are read in place
+  uint8_t* stage = static_cast<uint8_t*>(d_workspace);
+  const uint8_t* src[2] = {b->s_tm1, b->s_t};
+  int64_t pitch[2] = {b->src_pitch, b->src_pitch};
+  for (int o = 0; o < 2; ++o) {
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, src[o]) != cudaSuccess) cudaGetLastError();
+    else if (attr.type == cudaMemoryTypeDevice) continue;
+    DZ_CUDA_OK(cudaMemcpy2DAsync(stage + o * view->obs_stride, 2 * view->obs_stride, src[o], b->src_pitch,
+                                 view->obs_bytes, K, cudaMemcpyDefault, (cudaStream_t)stream));
+    src[o] = stage + o * view->obs_stride;
+    pitch[o] = 2 * view->obs_stride;
+  }
+  // both fields share one pitch in the kernels: a mixed host/device pair reads the device field through the stage too
+  if (pitch[0] != pitch[1]) {
+    const int o = pitch[0] == b->src_pitch ? 0 : 1;
+    DZ_CUDA_OK(cudaMemcpy2DAsync(stage + o * view->obs_stride, 2 * view->obs_stride, src[o], b->src_pitch,
+                                 view->obs_bytes, K, cudaMemcpyDefault, (cudaStream_t)stream));
+    src[o] = stage + o * view->obs_stride;
+    pitch[o] = 2 * view->obs_stride;
+  }
+  if (view->d_planes) {
+    DZ_TRY(launch_frame_add_batch(view, b, src[0], src[1], pitch[0], stage + add_batch_stage_bytes(view, K), stream));
+    DZ_LAUNCH(apply_add_batch_kernel, 1, 256, 0, stream, *view, *b, src[0], src[1], pitch[0], 0);
+    return DZ_OK;
+  }
+  const int vec16 = view->obs_bytes % 16 == 0 && pitch[0] % 16 == 0 && (uintptr_t)src[0] % 16 == 0 &&
+                    (uintptr_t)src[1] % 16 == 0;
+  DZ_LAUNCH(apply_add_batch_kernel, (int)(2 * K + 1), 256, 0, stream, *view, *b, src[0], src[1], pitch[0], vec16);
   return DZ_OK;
 }
 

@@ -695,6 +695,17 @@ class _TransitionStore:
     self.flags = torch.zeros(1, dtype=torch.int32, device=dev)
     self.obs_bytes = 0
     self.obs_stride = 0
+    self._batch = None
+
+  def add_batch_buffers(self, view):
+    """(records, workspace, adds per call) of dz_replay_add_batch, allocated on first use: the workspace is sized by
+    dz_replay_add_batch_workspace for min(capacity, ADD_BATCH_MAX) adds, lowered to what one call takes."""
+    if self._batch is None:
+      most, nbytes = C.c_int32(max(1, min(self.capacity, ADD_BATCH_MAX))), C.c_int64()
+      _lib.call('dz_replay_add_batch_workspace', C.byref(view), C.byref(most), C.byref(nbytes))
+      ws = torch.empty(nbytes.value, dtype=torch.uint8, device=self.action.device)
+      self._batch = (_AddBatchRecords(most.value, self.action.device), ws, most.value)
+    return self._batch
 
   def allocate(self, obs_shape, obs_dtype=np.uint8):
     if self.obs is not None:
@@ -886,6 +897,127 @@ def _host_obs(x, store):
   return arr.view(np.uint8).reshape(-1)
 
 
+ADD_BATCH_MAX = 256   # adds per dz_replay_add_batch call (the workspace holds two host-source copies per add)
+
+
+class _AddBatchRecords:
+  """The [K] record arrays of dz_add_batch as one pinned host block (numpy views, filled per call) and its device twin,
+  shipped with one copy per call.  The host block is rewritten only after the previous copy out of it has completed."""
+
+  _FIELDS = (('tree_index', np.int64, 1), ('evict_index', np.int64, 1), ('patch_pos', np.int64, 4),
+             ('patch_val', np.int64, 4), ('reward', np.float64, 1), ('discount', np.float64, 1), ('leaf', np.float64, 1),
+             ('action', np.int32, 1), ('release', np.int32, 1), ('patch_target', np.int32, 4))
+
+  def __init__(self, max_count, device):
+    offsets, off = {}, 0
+    for name, dtype, per in self._FIELDS:
+      offsets[name] = off
+      off += per * max_count * np.dtype(dtype).itemsize
+    self.host = torch.empty(off, dtype=torch.uint8).pin_memory()
+    self.dev = torch.empty(off, dtype=torch.uint8, device=device)
+    raw = self.host.numpy()
+    self.h = {name: raw[offsets[name]:offsets[name] + per * max_count * np.dtype(dt).itemsize].view(dt)
+              for name, dt, per in self._FIELDS}
+    self.d = {name: self.dev.data_ptr() + offsets[name] for name in offsets}
+    self._copied = torch.cuda.Event()
+    self._pending = False
+
+  def writable(self):
+    if self._pending:
+      self._copied.synchronize()
+      self._pending = False
+    return self.h
+
+  def ship(self):
+    self.dev.copy_(self.host, non_blocking=True)
+    self._copied.record()
+    self._pending = True
+
+
+def _batch_obs(x, store, count):
+  """`_host_obs` for a [K, *obs_shape] batch: (array or CUDA tensor kept alive for the call, address, bytes per item)."""
+  if isinstance(x, torch.Tensor) and x.is_cuda:
+    t = x.contiguous()
+    dtype = np.dtype(str(t.dtype).replace('torch.', ''))
+    shape, addr = tuple(t.shape), t.data_ptr()
+  else:
+    t = np.ascontiguousarray(x)
+    dtype, shape, addr = t.dtype, t.shape, t.ctypes.data
+  if len(shape) < 1 or shape[0] != count:
+    raise ValueError('observations must have a leading axis of length %d, got shape %s' % (count, shape))
+  store.allocate(shape[1:], dtype)
+  if shape[1:] != store.obs_shape or dtype != store.obs_dtype:
+    raise ValueError('observation shape/dtype changed: %s %s' % (shape[1:], dtype))
+  return t, addr
+
+
+def _batch_vector(x, count, dtype, name):
+  if isinstance(x, torch.Tensor):
+    x = x.detach().cpu().numpy()
+  v = np.asarray(x)
+  if v.shape != (count,):
+    raise ValueError('%s must have shape (%d,), got %s' % (name, count, v.shape))
+  return v.astype(dtype)
+
+
+def _batch_items(items, codec, store):
+  """Validates a batch `items` (Transition with a leading K axis) before anything changes: returns K, the observation
+  sources (s_tm1, s_t) and the scalars as host arrays (action int32, reward / discount float64)."""
+  count = len(items[1])
+  if codec is not None:
+    coded = [codec(type(items)(*[f[k] for f in items])) for k in range(count)]
+    items = type(items)(*[np.stack([np.asarray(c[i]) for c in coded]) if count else np.asarray(items[i])
+                          for i in range(5)])
+  s_tm1 = _batch_obs(items[0], store, count)
+  s_t = _batch_obs(items[4], store, count)
+  # int(a) into an int32 record, float(r) into a double, as `add` does
+  a = _batch_vector(items[1], count, np.int64, 'a_tm1').astype(np.int32)
+  r = _batch_vector(items[2], count, np.float64, 'r_t')
+  d = _batch_vector(items[3], count, np.float64, 'discount_t')
+  return count, s_tm1, s_t, a, r, d
+
+
+def _add_batch(rep, items, book, leaves=None, d_priority=None, alpha=1.0):
+  """Shared body of `add_batch` on a validated batch (`_batch_items`): chunks of at most min(capacity, adds per call)
+  transitions, so no call evicts a row it wrote itself.  `book()` runs one add's host bookkeeping (the same calls, in
+  the same order, as `add`) and returns (release_row, evict_index, tree_index, patches)."""
+  count, (o_tm1, p_tm1), (o_t, p_t), a, r, d = items
+  store = rep._store
+  v = rep.device_view()
+  recs, ws, most = store.add_batch_buffers(v)
+  chunk = min(rep._capacity, most)
+  obs_bytes = store.obs_bytes
+  for lo in range(0, count, chunk):
+    k = min(chunk, count - lo)
+    h = recs.writable()
+    first_slot = rep._t % rep._capacity
+    patches = []
+    for j in range(k):
+      release, evict, tree, p = book()
+      h['release'][j], h['evict_index'][j], h['tree_index'][j] = release, evict, tree
+      patches.extend(p)
+    n = len(patches)
+    if n:
+      pt = np.asarray(patches, dtype=np.int64)
+      h['patch_target'][:n], h['patch_pos'][:n], h['patch_val'][:n] = pt[:, 0], pt[:, 1], pt[:, 2]
+    h['action'][:k], h['reward'][:k], h['discount'][:k] = a[lo:lo + k], r[lo:lo + k], d[lo:lo + k]
+    if leaves is not None:
+      h['leaf'][:k] = leaves[lo:lo + k]
+    recs.ship()
+    b = _lib.AddBatch()
+    b.count, b.first_slot = k, first_slot
+    b.d_action, b.d_reward, b.d_discount = recs.d['action'], recs.d['reward'], recs.d['discount']
+    b.d_release_row = recs.d['release']
+    if leaves is not None:
+      b.d_tree_index, b.d_evict_index, b.d_leaf_value = recs.d['tree_index'], recs.d['evict_index'], recs.d['leaf']
+    b.d_priority = None if d_priority is None else d_priority.data_ptr()
+    b.alpha = alpha
+    b.n_patches = n
+    b.d_patch_pos, b.d_patch_val, b.d_patch_target = recs.d['patch_pos'], recs.d['patch_val'], recs.d['patch_target']
+    b.s_tm1, b.s_t, b.src_pitch = p_tm1 + lo * obs_bytes, p_t + lo * obs_bytes, obs_bytes
+    _lib.call('dz_replay_add_batch', C.byref(v), C.byref(b), ws.data_ptr(), ws.numel(), _stream())
+
+
 def _check_codec(encoder, decoder):
   """The reference stores `encoder(item)` and returns `decoder(stored)` (`replay.py:148,155`; every run_atari.py passes
   the snappy pair of `replay.py:895-904` so that 1M x 56 KB fits in host RAM).  HBM holds raw observations, so a codec
@@ -954,6 +1086,27 @@ class TransitionReplay:
     assert len(patches) <= 4
     self._live_ids.append(item_id)
     self._t += 1
+
+  def add_batch(self, items) -> None:
+    """K transitions at once: `items` is a Transition whose fields have a leading K axis (observations [K, *obs_shape]
+    as a numpy array or a CUDA tensor; a_tm1, r_t, discount_t of length K).  The replay afterwards equals the replay
+    after `for k in range(K): add(item_k)`.  Unlike that loop, the whole batch is validated first: a shape or dtype
+    mismatch raises what `add` raises and leaves the replay unchanged."""
+    batch = _batch_items(items, self._codec, self._store)
+    if batch[0] == 0:
+      return
+    dist = self._distribution
+
+    def book():
+      full = self.size == self._capacity
+      if full:
+        dist.remove([self._live_ids.popleft()])
+      dist.add([self._t])
+      self._live_ids.append(self._t)
+      self._t += 1
+      return full, -1, -1, dist.take_patches()
+
+    _add_batch(self, batch, book)
 
   def get(self, ids: Sequence[int]):
     """`replay.py:153-156`."""
@@ -1130,6 +1283,45 @@ class PrioritizedTransitionReplay:
     assert len(patches) <= 4
     self._live_ids.append(item_id)
     self._t += 1
+
+  def add_batch(self, items, priorities) -> None:
+    """K transitions at once (`items` as for `TransitionReplay.add_batch`).  `priorities`: a float, a length-K sequence
+    or array, or a device float32 scalar tensor (the agent's max_seen_priority, taken on the device for alpha in
+    {0.5, 1} as `add` does).  The replay afterwards equals the replay after `for k: add(item_k, priority_k)`.  Unlike
+    that loop, the whole batch is validated first: a bad priority or a shape or dtype mismatch raises what `add` raises
+    and leaves the replay unchanged."""
+    batch = _batch_items(items, self._codec, self._store)
+    count = batch[0]
+    dist = self._distribution
+    alpha = dist._priority_exponent
+    d_priority = None
+    if isinstance(priorities, torch.Tensor) and priorities.numel() == 1 and priorities.is_cuda \
+        and priorities.dtype == torch.float32 and alpha in (0.5, 1.0):
+      d_priority, pri = priorities, np.ones(count)
+    else:
+      if isinstance(priorities, torch.Tensor):
+        priorities = priorities.detach().cpu().numpy()
+      pri = np.asarray(priorities, dtype=np.float64)
+      if pri.ndim == 0:
+        pri = np.full(count, float(pri))
+      elif pri.shape != (count,):
+        raise ValueError('priorities must be a scalar or have shape (%d,), got %s' % (count, pri.shape))
+    leaves = np.asarray(_power(pri, alpha), dtype=np.float64)
+    if not np.isfinite(leaves).all() or (leaves < 0.0).any():
+      raise ValueError('value must be finite and positive.')
+    if count == 0:
+      return
+
+    def book():
+      evicted = -1
+      if self.size == self._capacity:
+        (evicted,) = dist._host_remove([self._live_ids.popleft()])
+      (idx,) = dist._host_add([self._t])
+      self._live_ids.append(self._t)
+      self._t += 1
+      return evicted >= 0, evicted, idx, dist.take_patches()
+
+    _add_batch(self, batch, book, leaves=leaves, d_priority=d_priority, alpha=float(alpha))
 
   def get(self, ids: Sequence[int]):
     ids = [int(i) for i in ids]
@@ -1316,6 +1508,100 @@ class NStepTransitionAccumulator:
     self._transitions.clear()
     self._timestep_tm1 = None
     self._a_tm1 = None
+
+
+class VectorNStepAccumulator:
+  """`num_streams` independent `NStepTransitionAccumulator`s as array code: the insert-side counterpart of
+  `processors.VectorScalars`, fed the struct-of-arrays timesteps of `VectorizedAtariPreprocessor.step_arrays` and
+  emitting one Transition with a leading K axis for `add_batch`.
+
+  The emitting streams' observations are copied into a device ring [E][n + 1][*obs_shape] (the caller's stacks are
+  overwritten in place on later ticks); the returned s_tm1 / s_t are gathered from it into fresh [K] tensors.  Returns
+  and discounts are folded in float64 as `_fold_n_steps` does, one numpy multiply and one add per step, which round as
+  the Python floats do."""
+
+  FIRST, MID, LAST = 0, 1, 2
+
+  def __init__(self, num_streams: int, n: int, device='cuda'):
+    if num_streams < 1 or n < 1:
+      raise ValueError('num_streams and n must be positive')
+    self._E, self._n = int(num_streams), int(n)
+    self._device = torch.device(device)
+    self._ring = None
+    self._len = np.zeros(self._E, np.int64)      # transitions in each stream's window
+    self._pos = np.zeros(self._E, np.int64)      # ring slot of each stream's latest observation
+    self._has_tm1 = np.zeros(self._E, bool)
+    self._a_tm1 = np.zeros(self._E, np.int64)
+    self._r = np.zeros((self._E, self._n))       # window of each stream, oldest transition first
+    self._d = np.zeros((self._E, self._n))
+    self._a = np.zeros((self._E, self._n), np.int64)
+
+  def reset(self, stream: Optional[int] = None) -> None:
+    sel = slice(None) if stream is None else stream
+    self._len[sel] = 0
+    self._has_tm1[sel] = False
+
+  def step(self, emit, step_type, reward, discount, observations, actions) -> Optional[Transition]:
+    """emit: bool [E], the streams with a new timestep; step_type / reward / discount: [E] (NaN = None); observations:
+    [E, *obs_shape] (e.g. `VectorizedAtariPreprocessor.stacks`); actions: [E], the a_t chosen on this timestep.
+    Returns the transitions completed this tick in stream-major order, or None."""
+    e = np.nonzero(np.asarray(emit, bool))[0]
+    if e.size == 0:
+      return None
+    st = np.asarray(step_type)[e].astype(np.int64)
+    first = st == self.FIRST
+    bad = ~first & ~self._has_tm1[e]
+    if bad.any():
+      k = int(np.argmax(bad))
+      raise ValueError('Expected FIRST timestep, got step_type %d on stream %d.' % (st[k], e[k]))
+    if isinstance(actions, torch.Tensor):
+      actions = actions.detach().cpu().numpy()
+    act = np.asarray(actions)[e].astype(np.int64)
+    rw = np.asarray(reward, np.float64)[e]
+    dc = np.asarray(discount, np.float64)[e]
+    n, ring_n = self._n, self._n + 1
+    if isinstance(observations, torch.Tensor):
+      obs = observations.index_select(0, torch.as_tensor(e, device=observations.device)).to(self._device)
+    else:
+      obs = torch.as_tensor(np.asarray(observations)[e], device=self._device)
+    if self._ring is None:
+      self._ring = torch.zeros((self._E * ring_n,) + tuple(obs.shape[1:]), dtype=obs.dtype, device=self._device)
+    pos = np.where(first, 0, (self._pos[e] + 1) % ring_n)
+    self._ring[torch.as_tensor(e * ring_n + pos, device=self._device)] = obs
+    # FIRST resets the stream; every other timestep appends (s_tm1, a_tm1, r_t, discount_t, s_t) to its window
+    self._len[e[first]] = 0
+    app = e[~first]
+    L = self._len[app]
+    full = app[L == n]
+    if full.size:
+      for w in (self._r, self._d, self._a):
+        w[full, :-1] = w[full, 1:]
+    L = np.minimum(L, n - 1)
+    self._r[app, L], self._d[app, L], self._a[app, L] = rw[~first], dc[~first], self._a_tm1[app]
+    self._len[app] = L + 1
+    self._pos[e], self._a_tm1[e], self._has_tm1[e] = pos, act, True
+    # LAST: the n, n-1, ..., 1-step windows ending at s_T; otherwise the full window
+    last = st == self.LAST
+    L = self._len[e]
+    count = np.where(last, L, (L == n).astype(np.int64))
+    total = int(count.sum())
+    self._len[e[last]] = 0
+    if total == 0:
+      return None
+    rows = np.repeat(e, count)
+    start = np.arange(total) - np.repeat(np.cumsum(count) - count, count)
+    end = np.repeat(L, count)
+    ret, disc = np.zeros(total), np.ones(total)
+    with np.errstate(all='ignore'):
+      for j in range(n):
+        m = (start <= j) & (j < end)
+        ret = np.where(m, ret + disc * self._r[rows, j], ret)
+        disc = np.where(m, disc * self._d[rows, j], disc)
+    latest = self._pos[rows]
+    tm1 = (latest - (end - start)) % ring_n
+    s_tm1 = self._ring[torch.as_tensor(rows * ring_n + tm1, device=self._device)]
+    s_t = self._ring[torch.as_tensor(rows * ring_n + latest, device=self._device)]
+    return Transition(s_tm1=s_tm1, a_tm1=self._a[rows, start], r_t=ret, discount_t=disc, s_t=s_t)
 
 
 class TransitionAccumulator(NStepTransitionAccumulator):

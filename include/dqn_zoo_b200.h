@@ -157,6 +157,47 @@ typedef struct dz_add_record {
 int dz_replay_add(const dz_replay_view* view, const dz_add_record* rec, const uint8_t* h_s_tm1,
                   const uint8_t* h_s_t, void* stream);
 
+/* K = `count` adds in one call, leaving the replay exactly as K dz_replay_add calls in order k = 0..K-1 would: the
+ * same rows, scalars, list patches, sum tree (a pure function of its leaves) and, in the frame-deduplicated layout,
+ * the same plane ids, refcounts, free stack (order included), plane bytes and hashes of every live plane, and the same
+ * sticky DZ_FLAG_FRAME_POOL_FULL.  The plane table then holds exactly the live planes; its slot layout may differ.
+ * Transition k goes to row (first_slot + k) % capacity, so K <= capacity rows are distinct.  The [K] arrays are DEVICE
+ * arrays (the Python host fills them with one H2D copy of a pinned block per call). */
+typedef struct dz_add_batch {
+  int32_t count;
+  int64_t first_slot;
+  const int32_t* d_action;          /* [K] */
+  const double* d_reward;           /* [K] */
+  const double* d_discount;         /* [K] */
+  const int32_t* d_release_row;     /* [K] as dz_add_record.release_row */
+  const int64_t* d_tree_index;      /* [K] prioritized replay; NULL for uniform */
+  const int64_t* d_evict_index;     /* [K] -1 = nothing evicted */
+  const double* d_leaf_value;       /* [K] priority**alpha in float64 (host), unless d_priority */
+  const float* d_priority;          /* optional, shared by the K adds: as dz_add_record.d_priority */
+  double alpha;
+  int32_t n_patches;                /* list patches of all K adds, applied in order (positions can repeat) */
+  const int64_t* d_patch_pos;       /* [n_patches] */
+  const int64_t* d_patch_val;       /* [n_patches] */
+  const int32_t* d_patch_target;    /* [n_patches] 0 = d_live, 1 = d_id_at, 2 = d_ids */
+  const uint8_t* s_tm1;             /* observation k at s_tm1 + k * src_pitch; host or device memory */
+  const uint8_t* s_t;
+  int64_t src_pitch;
+} dz_add_batch;
+
+/* Bytes of the workspace dz_replay_add_batch needs for up to *max_count adds per call.  *max_count is lowered to the
+ * most one call takes for this view (the sum-tree update and, in the frame-deduplicated layout, the plane resolution
+ * keep their state on chip). */
+int dz_replay_add_batch_workspace(const dz_replay_view* view, int32_t* max_count, int64_t* bytes);
+
+/* Host observations are copied H2D once per call, for the whole batch, into the workspace; device observations are
+ * read in place.  Argument errors (count above the workspace's or the capacity, first_slot out of range) return
+ * DZ_EINVAL / DZ_ERANGE before anything is enqueued.  Frame-deduplicated layout: the planes of the batch are hashed
+ * and matched (against the planes live at batch start and against earlier planes of the batch, every hash hit
+ * confirmed by a byte compare) in parallel; one thread then replays the pool rules of K sequential adds on integers
+ * only; the bytes of the planes that end the batch holding new content are copied in parallel. */
+int dz_replay_add_batch(const dz_replay_view* view, const dz_add_batch* batch, void* d_workspace,
+                        int64_t workspace_bytes, void* stream);
+
 /* Frame-deduplicated layout: empties the pool (every row's plane ids = 0, free stack hands out 1, 2, 3, ... next,
  * plane 0 zeroed, live and in the table). */
 int dz_replay_frame_pool_reset(const dz_replay_view* view, void* stream);
