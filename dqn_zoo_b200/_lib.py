@@ -124,6 +124,9 @@ _SIGNATURES = {
     'dz_learner_generate_randomness_async': (i32, [vp, u64, vp, vp, vp]),
     'dz_learner_q_values': (i32, [vp, vp, vp, vp, vp, vp]),
     'dz_learner_act_batch': (i32, [vp, vp, i32, vp, vp, vp, f32, vp, vp, vp]),
+    'dz_learner_act_batch_stream_noise': (i32, [vp, vp, i32, vp, vp, f32, vp, vp, vp]),
+    'dz_learner_noise_stride': (i32, [C.POINTER(LearnerConfig), C.POINTER(i64)]),
+    'dz_learner_generate_stream_noise': (i32, [vp, u64, i32, vp, vp]),
     'dz_learner_sync_target': (i32, [vp, vp]),
     'dz_test_u8_to_unit': (i32, [vp, vp]),
     'dz_atari_preprocess': (i32, [vp, vp, i32, vp, vp, vp, vp, i32, vp, i32, vp]),

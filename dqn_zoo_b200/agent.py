@@ -541,13 +541,19 @@ class BatchedEpsilonGreedyActor:
 
   `learner` is the training agent's `Learner` (shared parameters, as the reference's actors read the learner's online
   params) or any `Learner` whose batch size is >= E.  Exploration uniforms come from a host RandomState seeded from
-  `rng_key` (2E floats per tick; the reference draws with the JAX PRNG per actor).  Rainbow: one noise sample per tick is
-  shared by the E streams; IQN: every stream gets its own tau samples."""
+  `rng_key` (2E floats per tick; the reference draws with the JAX PRNG per actor).  IQN: every stream gets its own tau
+  samples.  Rainbow explores only through its noisy layers: by default one noise sample per tick is shared by the E
+  streams, so they explore in lockstep; `per_stream_noise=True` draws E samples per tick and gives stream e its own, as
+  the reference's actors each draw theirs (rainbow/agent.py:125-133)."""
 
-  def __init__(self, learner: learner_lib.Learner, num_streams: int, exploration_epsilon, rng_key):
+  def __init__(self, learner: learner_lib.Learner, num_streams: int, exploration_epsilon, rng_key,
+               per_stream_noise: bool = False):
     if num_streams < 1 or num_streams > learner.batch_size:
       raise ValueError('num_streams must be in [1, learner.batch_size]')
+    if per_stream_noise and learner.net.kind != 'rainbow':
+      raise ValueError('per_stream_noise needs a rainbow learner')
     self._learner = learner
+    self._per_stream_noise = bool(per_stream_noise)
     self._E = int(num_streams)
     self._epsilon = exploration_epsilon
     seed = int(np.asarray(rng_key).reshape(-1)[-1]) & 0x7FFFFFFF
@@ -569,15 +575,18 @@ class BatchedEpsilonGreedyActor:
       self._explore_host.copy_(torch.from_numpy(self._rng.uniform(size=(2, self._E)).astype(np.float32)))
       self._explore_dev.copy_(self._explore_host, non_blocking=True)
       explore = self._explore_dev
-    taus = noise = None
+    taus = noise = stream_noise = None
     kind = L.net.kind
-    if kind in ('iqn', 'rainbow'):
+    if self._per_stream_noise:
+      stream_noise = L.generate_stream_noise(self._seed, self._E)
+    elif kind in ('iqn', 'rainbow'):
       L.generate_randomness(self._seed)
       if kind == 'iqn':
         taus = L.taus[:self._E * L.net.tau_samples_policy] if hasattr(L.net, 'tau_samples_policy') else L.taus
       else:
         noise = L.noise
-    actions, self.q_values = L.act_batch(observations, epsilon=eps, explore=explore, taus=taus, noise=noise)
+    actions, self.q_values = L.act_batch(observations, epsilon=eps, explore=explore, taus=taus, noise=noise,
+                                         stream_noise=stream_noise)
     self._actions_host.copy_(actions, non_blocking=True)
     torch.cuda.current_stream().synchronize()
     self._t += 1

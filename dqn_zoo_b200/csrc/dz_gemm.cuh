@@ -319,6 +319,150 @@ __global__ void __launch_bounds__((BM / TM) * (BN / TN)) gemm_nn_kernel(const __
 }
 
 // ---------------------------------------------------------------------------------------------
+// NN noisy layer with one noise apply per row (batched acting: actor stream m draws its own noise):
+// C[m,n] = x[m,:] (Wmu + Wsigma . (eps_in[m] (x) eps_out[m]))[:,n], with row m's vectors at a_scale / c_scale +
+// m * noise_ld.  Each mu / sigma tile is staged once per CTA for all BM rows and each row's weight is formed in
+// registers with the operations and order of gemm_nn_kernel<DUAL> (t = eps_in * eps_out, w = fmaf(sigma, t, mu),
+// acc = fmaf(x, w, acc)), over the same BK chunks, split boundaries and partial layout: rows that carry the same apply
+// get that kernel's results bit for bit.  Plain A rows only.  grid = (tiles_n, tiles_m * splits, problems)
+// ---------------------------------------------------------------------------------------------
+template <int BM, int BN, int BK, int TM, int TN>
+__global__ void __launch_bounds__((BM / TM) * (BN / TN))
+    gemm_nn_rownoise_kernel(const __grid_constant__ GemmBatch batch, const long long noise_ld) {
+  dz::pdl_enter();
+  constexpr int NT = (BM / TM) * (BN / TN);
+  const GemmProblem& p = batch.p[blockIdx.z];
+  const int tiles_m = (p.M + BM - 1) / BM;
+  const int tile_m = blockIdx.y % tiles_m, split = blockIdx.y / tiles_m;
+  const int m0 = tile_m * BM, n0 = blockIdx.x * BN;
+  if (blockIdx.y >= tiles_m * p.splits || n0 >= p.N) return;
+  const int kchunks = (p.K + BK - 1) / BK;
+  const int per = (kchunks + p.splits - 1) / p.splits;
+  const int kc0 = split * per, kc1 = min(kchunks, kc0 + per);
+
+  __shared__ __align__(16) float As[2][BK][BM + kPad];   // x
+  __shared__ __align__(16) float Es[2][BK][BM + kPad];   // eps_in of each row
+  __shared__ __align__(16) float Bs[2][BK][BN + kPad];   // mu
+  __shared__ __align__(16) float Ss[2][BK][BN + kPad];   // sigma
+
+  const int tid = threadIdx.x, tx = tid % (BN / TN), ty = tid / (BN / TN);
+  constexpr int A_VEC = BM * BK / 4, B_VEC = BK * BN / 4;
+  constexpr int A_PER = (A_VEC + NT - 1) / NT, B_PER = (B_VEC + NT - 1) / NT;
+  ARow rows[A_PER];
+  const float* ein[A_PER];
+#pragma unroll
+  for (int i = 0; i < A_PER; ++i) {
+    int v = tid + i * NT;
+    int m = (v < A_VEC) ? m0 + v / (BK / 4) : p.M;
+    rows[i] = a_row_base(p, m);
+    ein[i] = m < p.M ? p.a_scale + (long long)m * noise_ld : nullptr;
+  }
+  const bool vecB = (p.ldb % 4 == 0) && (((reinterpret_cast<uintptr_t>(p.B) | reinterpret_cast<uintptr_t>(p.B2)) & 15) == 0);
+  const bool vecE = (noise_ld % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.a_scale) & 15) == 0);
+  float eo[TM][TN];   // eps_out of this thread's rows and columns (fixed over k)
+#pragma unroll
+  for (int i = 0; i < TM; ++i)
+#pragma unroll
+    for (int j = 0; j < TN; ++j) {
+      int m = m0 + ty * TM + i, n = n0 + tx * TN + j;
+      eo[i][j] = (m < p.M && n < p.N) ? p.c_scale[(long long)m * noise_ld + n] : 0.f;
+    }
+  Acc<TM, TN> acc;
+  acc.clear();
+
+  float4 ra[A_PER], re[A_PER], rb[B_PER], rs[B_PER];
+  auto gload = [&](int kc) {
+    const int k0 = kc * BK;
+#pragma unroll
+    for (int i = 0; i < A_PER; ++i) {
+      int v = tid + i * NT;
+      if (v < A_VEC) {
+        int k = k0 + (v % (BK / 4)) * 4;
+        ra[i] = a_load4(p, rows[i], k);
+        re[i] = (ein[i] && k < p.K) ? ld4_guard(ein[i] + k, k, p.K, vecE) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < B_PER; ++i) {
+      int v = tid + i * NT;
+      if (v < B_VEC) {
+        int k = k0 + v / (BN / 4), n = n0 + (v % (BN / 4)) * 4;
+        rb[i] = rs[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (k < p.K) {
+          rb[i] = ld4_guard(p.B + (long long)k * p.ldb + n, n, p.N, vecB);
+          rs[i] = ld4_guard(p.B2 + (long long)k * p.ldb + n, n, p.N, vecB);
+        }
+      }
+    }
+  };
+  auto sstore = [&](int buf) {
+#pragma unroll
+    for (int i = 0; i < A_PER; ++i) {
+      int v = tid + i * NT;
+      if (v < A_VEC) {
+        int r = v / (BK / 4), kq = (v % (BK / 4)) * 4;
+        As[buf][kq + 0][r] = ra[i].x; As[buf][kq + 1][r] = ra[i].y; As[buf][kq + 2][r] = ra[i].z; As[buf][kq + 3][r] = ra[i].w;
+        Es[buf][kq + 0][r] = re[i].x; Es[buf][kq + 1][r] = re[i].y; Es[buf][kq + 2][r] = re[i].z; Es[buf][kq + 3][r] = re[i].w;
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < B_PER; ++i) {
+      int v = tid + i * NT;
+      if (v < B_VEC) {
+        *reinterpret_cast<float4*>(&Bs[buf][v / (BN / 4)][(v % (BN / 4)) * 4]) = rb[i];
+        *reinterpret_cast<float4*>(&Ss[buf][v / (BN / 4)][(v % (BN / 4)) * 4]) = rs[i];
+      }
+    }
+  };
+
+  if (kc0 < kc1) { gload(kc0); sstore(0); }
+  __syncthreads();
+  for (int kc = kc0; kc < kc1; ++kc) {
+    const int cur = (kc - kc0) & 1;
+    const bool more = kc + 1 < kc1;
+    if (more) gload(kc + 1);
+#pragma unroll
+    for (int k = 0; k < BK; ++k) {
+      float a[TM], e[TM], mu[TN], sg[TN];
+      lds_vec<TM>(&As[cur][k][ty * TM], a);
+      lds_vec<TM>(&Es[cur][k][ty * TM], e);
+      lds_vec<TN>(&Bs[cur][k][tx * TN], mu);
+      lds_vec<TN>(&Ss[cur][k][tx * TN], sg);
+#pragma unroll
+      for (int i = 0; i < TM; ++i)
+#pragma unroll
+        for (int j = 0; j < TN; ++j) {
+          const float w = fmaf(sg[j], e[i] * eo[i][j], mu[j]);
+          acc.v[i][j] = fmaf(a[i], w, acc.v[i][j]);
+        }
+    }
+    if (more) sstore(cur ^ 1);
+    __syncthreads();
+  }
+
+  // epilogue (gemm_nn_kernel's, with row m's eps_out on the sigma bias)
+#pragma unroll
+  for (int i = 0; i < TM; ++i) {
+    int m = m0 + ty * TM + i;
+    if (m >= p.M) continue;
+#pragma unroll
+    for (int j = 0; j < TN; ++j) {
+      int n = n0 + tx * TN + j;
+      if (n >= p.N) continue;
+      if (p.splits > 1) {
+        p.C[(long long)split * p.split_stride + (long long)m * p.ldc + n] = acc.v[i][j];
+        continue;
+      }
+      float v = acc.v[i][j];
+      if (p.bias) v += p.bias[n];
+      if (p.bias2) v = fmaf(p.bias2[n], eo[i][j], v);
+      if (p.relu) v = fmaxf(v, 0.f);
+      p.C[(long long)m * p.ldc + n] = v;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // TN (weight gradient): C[K,N] = sum_m A[m,K]^T G[m,N].  Row K (one past the weights) accumulates
 // the bias gradient (A treated as 1).  grid = (tiles_n, tiles_k * splits, problems); splits over m.
 // ---------------------------------------------------------------------------------------------

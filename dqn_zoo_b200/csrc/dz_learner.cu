@@ -197,8 +197,9 @@ struct FinishNN {  // split-K partials of an NN problem -> bias / noisy combine 
 };
 struct FinishNNBatch { FinishNN f[kMaxProblems]; int n; };
 
-__global__ void __launch_bounds__(256) finish_nn_kernel(const __grid_constant__ FinishNNBatch b) {
-  dz::pdl_enter();
+// ROW_NOISE: row m of a noisy layer carries its own noise apply, its eps_out at c_scale + m * c_ld.
+template <bool ROW_NOISE>
+__device__ __forceinline__ void finish_nn_body(const FinishNNBatch& b, long long c_ld) {
   const FinishNN& f = b.f[blockIdx.y];
   long long total = (long long)f.M * f.N;
   if ((f.N & 3) == 0 && ((reinterpret_cast<uintptr_t>(f.partial) | reinterpret_cast<uintptr_t>(f.out) | (uintptr_t)(f.stride * 4)) & 15) == 0) {
@@ -217,8 +218,9 @@ __global__ void __launch_bounds__(256) finish_nn_kernel(const __grid_constant__ 
         else { v.x += f.bias[n]; v.y += f.bias[n + 1]; v.z += f.bias[n + 2]; v.w += f.bias[n + 3]; }
       }
       if (f.dual && f.bias2) {
-        v.x = fmaf(f.bias2[n], f.c_scale[n], v.x); v.y = fmaf(f.bias2[n + 1], f.c_scale[n + 1], v.y);
-        v.z = fmaf(f.bias2[n + 2], f.c_scale[n + 2], v.z); v.w = fmaf(f.bias2[n + 3], f.c_scale[n + 3], v.w);
+        const float* eo = ROW_NOISE ? f.c_scale + (i / f.N) * c_ld : f.c_scale;
+        v.x = fmaf(f.bias2[n], eo[n], v.x); v.y = fmaf(f.bias2[n + 1], eo[n + 1], v.y);
+        v.z = fmaf(f.bias2[n + 2], eo[n + 2], v.z); v.w = fmaf(f.bias2[n + 3], eo[n + 3], v.w);
       }
       if (f.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
       *reinterpret_cast<float4*>(f.out + i) = v;
@@ -230,10 +232,23 @@ __global__ void __launch_bounds__(256) finish_nn_kernel(const __grid_constant__ 
     float v = 0.f;
     for (int k = 0; k < f.splits; ++k) v += f.partial[k * f.stride + i];
     if (f.bias) v += f.bias_shared ? f.bias[0] : f.bias[n];
-    if (f.dual && f.bias2) v = fmaf(f.bias2[n], f.c_scale[n], v);   // sigma bias of the noisy layer
+    if (f.dual && f.bias2) {   // sigma bias of the noisy layer
+      const float* eo = ROW_NOISE ? f.c_scale + (i / f.N) * c_ld : f.c_scale;
+      v = fmaf(f.bias2[n], eo[n], v);
+    }
     if (f.relu) v = fmaxf(v, 0.f);
     f.out[i] = v;
   }
+}
+
+__global__ void __launch_bounds__(256) finish_nn_kernel(const __grid_constant__ FinishNNBatch b) {
+  dz::pdl_enter();
+  finish_nn_body<false>(b, 0);
+}
+
+__global__ void __launch_bounds__(256) finish_nn_rownoise_kernel(const __grid_constant__ FinishNNBatch b, long long c_ld) {
+  dz::pdl_enter();
+  finish_nn_body<true>(b, c_ld);
 }
 
 struct FinishTN {  // split partials [Kext][N] of a TN problem -> weight / bias gradients
@@ -1487,7 +1502,23 @@ int run_nt(const char* tag, GemmBatch& gb, bool dual, void* stream) {
   return launch_batch(tag, gemm_nt_kernel<64, 64, 16, 4, 4, false>, gb, grid, 256, stream);
 }
 
-int finish_nn(const GemmBatch& gb, float* const* outs, bool dual, void* stream) {
+// One noise apply per row of a noisy layer (rows of a batched-acting tick): same launch shape as run_nn's M <= 32 case,
+// tiles of 32 rows.  noise_ld: floats between the noise applies of consecutive rows.
+int run_nn_rownoise(const char* tag, GemmBatch& gb, long long noise_ld, void* stream) {
+  int maxM = 0, maxN = 0, maxS = 1;
+  for (int i = 0; i < gb.n; ++i) {
+    if (gb.p[i].a_mode != A_PLAIN || !gb.p[i].B2 || !gb.p[i].a_scale || !gb.p[i].c_scale)
+      return fail(DZ_EINVAL, "%s: per-row noise needs a plain noisy problem", tag);
+    maxM = gb.p[i].M > maxM ? gb.p[i].M : maxM;
+    maxN = gb.p[i].N > maxN ? gb.p[i].N : maxN;
+    maxS = gb.p[i].splits > maxS ? gb.p[i].splits : maxS;
+  }
+  dim3 grid((unsigned)ceil_div(maxN, 64), (unsigned)(ceil_div(maxM, 32) * maxS), gb.n);
+  DZ_LAUNCH_NAMED(tag, (gemm_nn_rownoise_kernel<32, 64, 16, 2, 4>), grid, 256, 0, stream, gb, noise_ld);
+  return DZ_OK;
+}
+
+int finish_nn(const GemmBatch& gb, float* const* outs, bool dual, void* stream, long long noise_ld = 0) {
   FinishNNBatch fb;
   fb.n = gb.n;
   long long mx = 0;
@@ -1498,7 +1529,8 @@ int finish_nn(const GemmBatch& gb, float* const* outs, bool dual, void* stream) 
     mx = t > mx ? t : mx;
   }
   dim3 grid((unsigned)std::min<long long>(ceil_div(mx, 256), kNumSMs * 8), gb.n);   // grid-stride kernels
-  DZ_LAUNCH(finish_nn_kernel, grid, 256, 0, stream, fb);
+  if (noise_ld) DZ_LAUNCH(finish_nn_rownoise_kernel, grid, 256, 0, stream, fb, noise_ld);
+  else DZ_LAUNCH(finish_nn_kernel, grid, 256, 0, stream, fb);
   return DZ_OK;
 }
 
@@ -1600,12 +1632,18 @@ int forward_heads_plain(dz_learner* l, const Pass* passes, int np, int nimg, voi
   return DZ_OK;
 }
 
-// Rainbow: two noisy streams (networks.py:224-261, :137-178).
-int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, const float* noise, void* stream, bool fc1_done = false) {
+// Rainbow: two noisy streams (networks.py:224-261, :137-178).  noise_ld > 0: image m of the pass uses its own noise
+// apply at noise + m * noise_ld (one pass only); 0: every image uses the pass's apply.
+int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, const float* noise, void* stream, bool fc1_done = false,
+                          long long noise_ld = 0) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
   if (2 * np > kMaxProblems) return fail(DZ_EINVAL, "too many rainbow passes");
+  if (noise_ld && (np != 1 || fc1_done)) return fail(DZ_EINVAL, "per-row noise: one pass with its own fc1");
+  auto run = [&](const char* tag, GemmBatch& b) {
+    return noise_ld ? run_nn_rownoise(tag, b, noise_ld, stream) : run_nn(tag, b, true, stream);
+  };
   GemmBatch gb;
   gb.n = 2 * np;
   float* outs[kMaxProblems];
@@ -1631,8 +1669,8 @@ int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, c
     }
   }
   if (!fc1_done) {
-    DZ_TRY(run_nn("noisy1_fwd", gb, true, stream));
-    if (splits > 1) DZ_TRY(finish_nn(gb, outs, true, stream));
+    DZ_TRY(run("noisy1_fwd", gb));
+    if (splits > 1) DZ_TRY(finish_nn(gb, outs, true, stream, noise_ld));
   }
   for (int i = 0; i < np; ++i) {
     NoiseVecs nz = noise_of(c, d, noise, passes[i].apply);
@@ -1656,8 +1694,8 @@ int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, c
       gb.p[q] = p;
     }
   }
-  DZ_TRY(run_nn("noisy2_fwd", gb, true, stream));
-  if (nimg <= 32) DZ_TRY(finish_nn(gb, outs, true, stream));
+  DZ_TRY(run("noisy2_fwd", gb));
+  if (nimg <= 32) DZ_TRY(finish_nn(gb, outs, true, stream, noise_ld));
   return DZ_OK;
 }
 
@@ -2529,10 +2567,11 @@ int dz_learner_q_values(dz_learner* l, const uint8_t* d_obs, const float* d_taus
 // in one enqueue, q-values [E][A], and the epsilon-greedy choice on the device — one D2H of E actions per tick instead of a
 // D2H sync per decision.  d_obs: E contiguous observations (H*W*C bytes each).  d_explore: [2][E] uniforms in [0,1) or
 // NULL (greedy): action = u0 < epsilon ? floor(u1 * A) : argmax (first maximum, as np.argmax).  IQN: d_taus is
-// [E][tau_samples_policy]; rainbow: ONE noise apply shared by the E streams of the tick (the reference's actors each draw
-// their own: statistically the same exploration, not the same sample path).
-int dz_learner_act_batch(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* d_taus, const float* d_noise,
-                         const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
+// [E][tau_samples_policy]; rainbow: ONE noise apply shared by the E streams of the tick, so the streams explore in
+// lockstep.  dz_learner_act_batch_stream_noise gives stream e its own apply, as the reference's actors each draw their own.
+namespace {
+int act_batch_impl(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* d_taus, const float* d_noise, long long noise_ld,
+                   const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
   const dz_learner_config& c = l->cfg;
   const float* on = l->buf.d_online;
   if (E < 1 || E > l->B) return fail(DZ_EINVAL, "act_batch: 1 <= E <= learner batch");
@@ -2551,7 +2590,7 @@ int dz_learner_act_batch(dz_learner* l, const uint8_t* d_obs, int32_t E, const f
     nq = c.tau_samples_policy;
   } else if (c.kind == DZ_RAINBOW) {
     if (!d_noise) return fail(DZ_EINVAL, "rainbow act_batch needs one apply of noise");
-    DZ_TRY(forward_heads_rainbow(l, &pass, 1, E, d_noise, stream));
+    DZ_TRY(forward_heads_rainbow(l, &pass, 1, E, d_noise, stream, false, noise_ld));
   } else {
     DZ_TRY(forward_heads_plain(l, &pass, 1, E, stream));
     nq = c.num_quantiles;
@@ -2559,6 +2598,44 @@ int dz_learner_act_batch(dz_learner* l, const uint8_t* d_obs, int32_t E, const f
   size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
   DZ_LAUNCH(q_values_kernel, (unsigned)E, 128, smem, stream, c.kind, c.num_actions, c.num_atoms, nq, c.vmax, l->out[1], l->out[1], l->outv[1], d_q_out);
   DZ_LAUNCH(act_select_kernel, (unsigned)ceil_div(E, 128), 128, 0, stream, (const float*)d_q_out, c.num_actions, (int)E, d_explore, epsilon, d_actions);
+  return DZ_OK;
+}
+}  // namespace
+
+int dz_learner_act_batch(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* d_taus, const float* d_noise,
+                         const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
+  return act_batch_impl(l, d_obs, E, d_taus, d_noise, 0, d_explore, epsilon, d_q_out, d_actions, stream);
+}
+
+// Rainbow only: stream e's forward uses noise apply e of d_noise ([E][noise stride], dz_learner_noise_stride), so each
+// stream explores with its own draw as in the reference.  Stream e gets exactly what dz_learner_act_batch gives it
+// when every stream carries that apply: the per-row kernels form the weights in the same order over the same splits.
+int dz_learner_act_batch_stream_noise(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* d_noise,
+                                      const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
+  if (l->cfg.kind != DZ_RAINBOW) return fail(DZ_EINVAL, "act_batch_stream_noise: only rainbow has noisy layers");
+  if (E < 1 || E > l->B) return fail(DZ_EINVAL, "act_batch_stream_noise: 1 <= E <= learner batch");
+  if (!d_noise) return fail(DZ_EINVAL, "act_batch_stream_noise needs noise[E][stride]");
+  return act_batch_impl(l, d_obs, E, nullptr, d_noise, noise_layout(l->cfg, l->d).stride, d_explore, epsilon, d_q_out,
+                        d_actions, stream);
+}
+
+int dz_learner_noise_stride(const dz_learner_config* cfg, int64_t* out) {
+  DZ_TRY(validate(*cfg));
+  if (cfg->kind != DZ_RAINBOW) return fail(DZ_EINVAL, "noise_stride: only rainbow has noisy layers");
+  *out = noise_layout(*cfg, make_dims(*cfg)).stride;
+  return DZ_OK;
+}
+
+// E noise applies for dz_learner_act_batch_stream_noise: the generator of dz_learner_generate_randomness (Philox keyed by
+// element index, counter d_counters[1] and stream id 2) over E * stride floats, so the first three applies equal what that
+// call writes for the same seed and counter.  Advances the counter once.
+int dz_learner_generate_stream_noise(dz_learner* l, uint64_t seed, int32_t E, float* d_noise, void* stream) {
+  if (l->cfg.kind != DZ_RAINBOW) return fail(DZ_EINVAL, "generate_stream_noise: only rainbow has noisy layers");
+  if (E < 1 || E > l->B) return fail(DZ_EINVAL, "generate_stream_noise: 1 <= E <= learner batch");
+  if (!d_noise) return fail(DZ_EINVAL, "generate_stream_noise: null buffer");
+  const long long n = (long long)E * noise_layout(l->cfg, l->d).stride;
+  DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_noise, n, seed, l->buf.d_counters, 1, 2u);
+  DZ_LAUNCH(bump_counter_kernel, 1, 1, 0, stream, l->buf.d_counters, 1);
   return DZ_OK;
 }
 

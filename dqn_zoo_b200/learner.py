@@ -149,6 +149,12 @@ class Learner:
     self.counters = torch.zeros(4, dtype=torch.int64, device=dev)
     self.taus = torch.zeros(max(plan.tau_floats, 1), dtype=torch.float32, device=dev)
     self.noise = torch.zeros(max(plan.noise_floats, 1), dtype=torch.float32, device=dev)
+    self.noise_stride = 0          # floats of one noise apply (rainbow)
+    if net.kind == 'rainbow':
+      stride = C.c_int64()
+      _lib.call('dz_learner_noise_stride', C.byref(cfg), C.byref(stride))
+      self.noise_stride = stride.value
+    self._stream_noise = None      # [batch_size, noise_stride], allocated by the first generate_stream_noise
     self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
     self.per_example = torch.zeros(batch_size, dtype=torch.float32, device=dev)
     self.priorities = torch.zeros(batch_size, dtype=torch.float32, device=dev)
@@ -277,6 +283,17 @@ class Learner:
     _lib.call('dz_learner_generate_randomness_async' if beside_sampler else 'dz_learner_generate_randomness', self._h, seed,
               self.taus.data_ptr(), self.noise.data_ptr(), _cstream())
 
+  def generate_stream_noise(self, seed: int, num_streams: int) -> torch.Tensor:
+    """Rainbow: one noise apply per actor stream, `[num_streams, noise_stride]` float32 on the device, for
+    `act_batch(..., stream_noise=...)`.  Same generator and counter as `generate_randomness` (which it advances); the
+    returned view is overwritten by the next call."""
+    if self._stream_noise is None and self.kind == 'rainbow':
+      self._stream_noise = torch.zeros((self.batch_size, self.noise_stride), dtype=torch.float32, device=self.device)
+    buf = self._stream_noise
+    _lib.call('dz_learner_generate_stream_noise', self._h, seed, int(num_streams), 0 if buf is None else buf.data_ptr(),
+              _cstream())
+    return buf[:num_streams]
+
   def q_values(self, obs_u8: torch.Tensor, taus=None, noise=None) -> torch.Tensor:
     """Online-network Q-values for one observation (the network half of select_action)."""
     obs = torch.as_tensor(obs_u8, device=self.device).contiguous().view(-1)
@@ -287,18 +304,30 @@ class Learner:
     self._keep_q = (obs, t, n)
     return self.q_out[:self.net.num_actions]
 
-  def act_batch(self, obs_u8: torch.Tensor, epsilon: float = 0.0, explore=None, taus=None, noise=None):
+  def act_batch(self, obs_u8: torch.Tensor, epsilon: float = 0.0, explore=None, taus=None, noise=None, stream_noise=None):
     """Batched select_action for E <= batch_size environment streams in ONE enqueue: `obs_u8` is [E, H, W, C] uint8 (device
-    or host), `explore` a float32 [2, E] tensor of uniforms in [0, 1) (None: greedy).  Returns (actions int32 [E],
-    q_values float32 [E, num_actions]) as device tensors — the caller does one D2H of the actions per tick."""
+    or host), `explore` a float32 [2, E] tensor of uniforms in [0, 1) (None: greedy).  Rainbow takes either `noise` (one
+    apply shared by the E streams) or `stream_noise`, a [E, noise_stride] tensor whose row e is stream e's own apply
+    (`generate_stream_noise`).  Returns (actions int32 [E], q_values float32 [E, num_actions]) as device tensors — the
+    caller does one D2H of the actions per tick."""
     obs = torch.as_tensor(obs_u8, device=self.device).contiguous()
     E = int(obs.shape[0])
     if not hasattr(self, '_act_q') or self._act_q.shape[0] < E:
       self._act_q = torch.zeros((self.batch_size, self.net.num_actions), dtype=torch.float32, device=self.device)
       self._act_a = torch.zeros(self.batch_size, dtype=torch.int32, device=self.device)
+    x = None if explore is None else torch.as_tensor(explore, device=self.device).to(torch.float32).contiguous()
+    if stream_noise is not None:
+      if noise is not None or taus is not None:
+        raise ValueError('stream_noise replaces noise / taus')
+      n = torch.as_tensor(stream_noise, device=self.device).to(torch.float32).contiguous()
+      if n.dim() != 2 or n.shape[0] != E or n.shape[1] != self.noise_stride:
+        raise ValueError('stream_noise must be [E, noise_stride] = [%d, %d], got %s' % (E, self.noise_stride, tuple(n.shape)))
+      _lib.call('dz_learner_act_batch_stream_noise', self._h, obs.data_ptr(), E, n.data_ptr(),
+                0 if x is None else x.data_ptr(), float(epsilon), self._act_q.data_ptr(), self._act_a.data_ptr(), _cstream())
+      self._keep_act = (obs, n, x)
+      return self._act_a[:E], self._act_q[:E]
     t = None if taus is None else torch.as_tensor(taus, device=self.device).to(torch.float32).contiguous()
     n = None if noise is None else torch.as_tensor(noise, device=self.device).to(torch.float32).contiguous()
-    x = None if explore is None else torch.as_tensor(explore, device=self.device).to(torch.float32).contiguous()
     _lib.call('dz_learner_act_batch', self._h, obs.data_ptr(), E, 0 if t is None else t.data_ptr(),
               0 if n is None else n.data_ptr(), 0 if x is None else x.data_ptr(), float(epsilon), self._act_q.data_ptr(),
               self._act_a.data_ptr(), _cstream())

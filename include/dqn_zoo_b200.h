@@ -373,10 +373,26 @@ int dz_learner_q_values(dz_learner* l, const uint8_t* d_obs, const float* d_taus
  * epsilon-greedy choice on the device, so a tick costs ONE device-to-host copy of E int32 actions.
  *   d_obs      E contiguous uint8 observations (obs_h*obs_w*obs_c bytes each), device memory
  *   d_taus     iqn: [E][tau_samples_policy];  d_noise  rainbow: one noise apply, shared by the E streams of the tick
+ *              (the streams explore in lockstep; dz_learner_act_batch_stream_noise gives each stream its own apply)
  *   d_explore  [2][E] float32 uniforms in [0,1) (device) or NULL for greedy acting:
  *              action = u0[e] < epsilon ? min(floor(u1[e] * num_actions), num_actions - 1) : first argmax of q[e] */
 int dz_learner_act_batch(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* d_taus, const float* d_noise,
                          const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream);
+
+/* Rainbow batched acting with one noise apply per stream (rainbow/agent.py:125-133 run by E actors, each drawing its own
+ * noise): as dz_learner_act_batch, but stream e's noisy layers use apply e of d_noise, which is [E][stride] floats with
+ * stride from dz_learner_noise_stride.  When every row carries the same apply, the q-values and actions equal
+ * dz_learner_act_batch's with that apply bit for bit.  DZ_EINVAL for a non-rainbow learner, E outside [1, batch] or a
+ * NULL buffer. */
+int dz_learner_act_batch_stream_noise(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* d_noise,
+                                      const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions,
+                                      void* stream);
+/* Floats of ONE rainbow noise apply (the 8 factorised-noise vectors, each padded to 4 floats); DZ_EINVAL for other kinds. */
+int dz_learner_noise_stride(const dz_learner_config* cfg, int64_t* out);
+/* E noise applies ([E][stride] floats) for dz_learner_act_batch_stream_noise from the generator of
+ * dz_learner_generate_randomness (same seed and counter: the first min(E, 3) applies equal what it writes); advances
+ * d_counters[1] once.  DZ_EINVAL for a non-rainbow learner, E outside [1, batch] or a NULL buffer. */
+int dz_learner_generate_stream_noise(dz_learner* l, uint64_t seed, int32_t E, float* d_noise, void* stream);
 
 /* target <- online (dqn/agent.py:155-156): device-to-device copy of the blob. */
 int dz_learner_sync_target(dz_learner* l, void* stream);

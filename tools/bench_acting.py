@@ -1,11 +1,16 @@
 """Batched acting throughput: E environment streams per tick through BatchedEpsilonGreedyActor (one network evaluation and
 ONE device-to-host copy of E actions per tick) versus the single-observation path (one D2H sync per decision).
   python tools/bench_acting.py --agent dqn --streams 32 [--ticks 300]
+Rainbow's two noise modes, alternated in one run (decisions/s of each round), then kernel times in a separate run:
+  python tools/bench_acting.py --agent rainbow --per-stream-noise [--rounds 3]
+  python tools/bench_acting.py --agent rainbow --per-stream-noise --profile OUT_DIR
 Observations are device-resident frame stacks (what processors.BatchedAtariPreprocessor hands out)."""
 
 import argparse
+import collections
 import json
 import os
+import subprocess
 import sys
 import time
 
@@ -15,12 +20,92 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 
+def card():
+  """Name and power limit of the device the numbers were measured on."""
+  out = {'gpu': torch.cuda.get_device_name()}
+  try:
+    q = subprocess.run(['nvidia-smi', '--query-gpu=power.limit,clocks.max.sm', '--format=csv,noheader', '-i',
+                        str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
+    out['power_limit'], out['max_sm_clock'] = [s.strip() for s in q.split(',')][:2]
+  except (OSError, ValueError, subprocess.SubprocessError):
+    out['power_limit'] = 'unknown'
+  return out
+
+
+def decisions_per_s(actor, obs, ticks):
+  torch.cuda.synchronize()
+  t0 = time.perf_counter()
+  for _ in range(ticks):
+    actor.step(obs)
+  torch.cuda.synchronize()
+  return obs.shape[0] * ticks / (time.perf_counter() - t0)
+
+
+def noise_modes(L, E, obs, a):
+  """Rainbow decisions/s with one noise apply shared by the tick's streams and with one apply per stream, alternated."""
+  from dqn_zoo_b200 import agent as agent_lib
+  actors = {mode: agent_lib.BatchedEpsilonGreedyActor(L, E, exploration_epsilon=0.01, rng_key=[0, 3],
+                                                      per_stream_noise=mode == 'per_stream')
+            for mode in ('shared', 'per_stream')}
+  for actor in actors.values():
+    for _ in range(20):
+      actor.step(obs)
+  if a.profile:
+    return profile_modes(actors, obs, a)
+  rates = {mode: [] for mode in actors}
+  for _ in range(a.rounds):
+    for mode, actor in actors.items():
+      rates[mode].append(round(decisions_per_s(actor, obs, a.ticks), 1))
+  print(json.dumps(dict({'metric': 'rainbow acting decisions per second by noise mode (device-resident observations)',
+                         'streams': E, 'ticks_per_round': a.ticks, 'shared_noise_decisions_per_s': rates['shared'],
+                         'per_stream_noise_decisions_per_s': rates['per_stream']}, **card())))
+
+
+def profile_modes(actors, obs, a):
+  """Kernel times per tick of each mode from torch.profiler CUDA activity (a run of its own: tracing slows the host).
+  noisy1_fwd is the noisy GEMM launch with 512 / 64 = 8 column tiles, noisy2_fwd the one with ceil(A * atoms / 64)."""
+  os.makedirs(a.profile, exist_ok=True)
+  result = dict({'metric': 'rainbow acting kernel time per tick (us), torch.profiler', 'streams': obs.shape[0],
+                 'ticks': a.ticks}, **card())
+  for mode, actor in actors.items():
+    path = os.path.join(a.profile, 'acting_%s.json' % mode)
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+      for _ in range(a.ticks):
+        actor.step(obs)
+      torch.cuda.synchronize()
+    prof.export_chrome_trace(path)
+    per_kernel = collections.defaultdict(float)
+    layers = collections.defaultdict(float)
+    with open(path) as f:
+      events = json.load(f)['traceEvents']
+    for ev in events:
+      if ev.get('cat') != 'kernel':
+        continue
+      name = ev['name']
+      short = name.replace('(anonymous namespace)::', '').replace('void ', '').split('(')[0].split('<')[0].split('::')[-1]
+      per_kernel[short] += ev['dur'] / a.ticks
+      if short == 'gemm_nn_rownoise_kernel' or (short == 'gemm_nn_kernel' and 'true>' in name):
+        layers['noisy1_fwd' if ev['args']['grid'][0] == 8 else 'noisy2_fwd'] += ev['dur'] / a.ticks
+    result[mode] = {'noisy1_fwd_us': round(layers['noisy1_fwd'], 2), 'noisy2_fwd_us': round(layers['noisy2_fwd'], 2),
+                    'kernels_us': {k: round(v, 2) for k, v in sorted(per_kernel.items(), key=lambda kv: -kv[1])}}
+  print(json.dumps(result))
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--agent', default='dqn')
   ap.add_argument('--streams', type=int, default=32)
   ap.add_argument('--ticks', type=int, default=300)
+  ap.add_argument('--per-stream-noise', action='store_true',
+                  help='rainbow: compare one noise apply per tick with one apply per stream, alternated')
+  ap.add_argument('--rounds', type=int, default=3)
+  ap.add_argument('--profile', default=None, help='with --per-stream-noise: kernel times from torch.profiler, traces here')
   a = ap.parse_args()
+  if a.per_stream_noise and a.agent != 'rainbow':
+    ap.error('--per-stream-noise needs --agent rainbow')
+  if not torch.cuda.is_available():
+    raise SystemExit('bench_acting.py needs a CUDA device')
   from dqn_zoo_b200 import agent as agent_lib
   from dqn_zoo_b200 import learner as dl
   from oracle import learner_oracle as lo
@@ -28,15 +113,12 @@ def main():
   L.set_params(lo.init_params(lo.NetSpec(a.agent, 6), 2), also_target=True)
   E = a.streams
   obs = torch.randint(0, 256, (E, 84, 84, 4), dtype=torch.uint8, device='cuda')
+  if a.per_stream_noise:
+    return noise_modes(L, E, obs, a)
   actor = agent_lib.BatchedEpsilonGreedyActor(L, E, exploration_epsilon=0.01, rng_key=[0, 3])
   for _ in range(20):
     actor.step(obs)
-  torch.cuda.synchronize()
-  t0 = time.perf_counter()
-  for _ in range(a.ticks):
-    actor.step(obs)
-  torch.cuda.synchronize()
-  batched = E * a.ticks / (time.perf_counter() - t0)
+  batched = decisions_per_s(actor, obs, a.ticks)
   # single-observation path: q_values + D2H per decision
   noise = taus = None
   if a.agent == 'rainbow':
