@@ -2668,8 +2668,17 @@ int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace) {
 }
 
 // Test hook: the MMA path of the tensor-core launch named `tag` (the tags of dz_test_learner_trace, conv1_fwd included):
-// 1 warp-level mma.sync kernel, 2 wgmma kernel.
+// 1 warp-level mma.sync kernel, 2 wgmma kernel.  The IQN update's launches "iqn_embed_fwd", "iqn_fc1_fwd",
+// "iqn_fc1_wgrad", "iqn_fc1_dgrad" and "iqn_embed_wgrad" answer 1 when they run on the packed-operand GEMM
+// (tc_pgemm_kernel) and DZ_EINVAL when they run on the fp32-FMA kernels, whatever path the torso takes.
 int dz_test_learner_mma_path(dz_learner* l, const char* tag, int32_t* path) {
+  const std::string t = tag ? tag : "";
+  if (t == "iqn_embed_fwd" || t == "iqn_fc1_fwd" || t == "iqn_fc1_wgrad" || t == "iqn_fc1_dgrad" || t == "iqn_embed_wgrad") {
+    const bool packed = l->pk_on && (t != "iqn_embed_wgrad" || l->pk_embed_bwd);
+    if (!packed) return fail(DZ_EINVAL, "'%s' does not run on the packed tensor-core GEMM in this learner", tag);
+    *path = UM_PATH_MMA_SYNC;
+    return DZ_OK;
+  }
   if (!l->um) return fail(DZ_EINVAL, "the tensor-core path is not active for this learner");
   const int p = um_net_mma_path(l->um, tag);
   if (p < 0) return fail(DZ_EINVAL, "no tensor-core launch '%s' in this learner", tag ? tag : "");

@@ -402,11 +402,6 @@ int dz_learner_sync_target(dz_learner* l, void* stream);
 int dz_test_u8_to_unit(float* d_out256, void* stream);
 
 
-/* Self-test of the packed-operand tensor-core GEMM (csrc/dz_tcp.cuh; the IQN 3136->512 layer's kernels): packs
- * A (a_rows x red) and B (b_rows x red) from plain fp32 matrices (x_red_contig = 1: element (row, r) at
- * x[row*ld + r]; 0: at x[r*ld + row]) into hi/lo TF32 tile images inside d_work (dz_test_tc_pgemm_work floats),
- * then D[i,j] = sum_r A(i,r) B(j,r).  a_ones_row = a_rows appends a row of ones to A (bias-gradient row), -1: none.
- * splits == 1: + d_bias[j] and ReLU are applied if given; otherwise raw partials at d_C + s*split_stride. */
 /* ---- Atari frame preprocessing (SURVEY §8(f) #3) ---------------------------------------------------------------
  * Replaces the observation branch of processors.atari() — np.max over the pooled frame pair, rgb2y, PIL bilinear
  * resize, frame stack (dqn_zoo/processors.py:367-388, 482-501) — for n_env environment streams per launch.
@@ -446,12 +441,19 @@ int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream);  
 /* Debug: the tensor-core launch named `tag` writes the clock stamps of its CTA 0 into d_trace (512 int64). */
 int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace);
 /* Tests: which MMA path the tensor-core launch `tag` (same tags, and "conv1_fwd") takes: *path = 1 warp-level mma.sync,
- * 2 wgmma. */
+ * 2 wgmma.  The IQN update's "iqn_embed_fwd", "iqn_fc1_fwd", "iqn_fc1_wgrad", "iqn_fc1_dgrad" and "iqn_embed_wgrad"
+ * give 1 when the launch runs on the packed-operand GEMM (csrc/dz_tcp.cuh) and DZ_EINVAL when it runs on the fp32-FMA
+ * kernels, independently of the torso's path. */
 int dz_test_learner_mma_path(dz_learner* l, const char* tag, int32_t* path);
 /* Debug: every kernel appends (globaltimer ns, gridDim.x << 32 | gridDim.y << 16 | blockDim.x) to d_buf right after its
  * dependencies completed; d_buf[0] (low 32 bits) counts the entries, entries start at d_buf[2].  d_buf: 2 + 2 * 4000
  * uint64, zeroed by the caller; nullptr switches the stamps off.  Works under CUDA-graph replay (tools/step_timeline.py). */
 int dz_debug_timeline(unsigned long long* d_buf);
+/* Self-test of the packed-operand tensor-core GEMM (csrc/dz_tcp.cuh; the IQN 3136->512 layer's kernels): packs
+ * A (a_rows x red) and B (b_rows x red) from plain fp32 matrices (x_red_contig = 1: element (row, r) at
+ * x[row*ld + r]; 0: at x[r*ld + row]) into hi/lo TF32 tile images inside d_work (dz_test_tc_pgemm_work floats),
+ * then D[i,j] = sum_r A(i,r) B(j,r).  a_ones_row = a_rows appends a row of ones to A (bias-gradient row), -1: none.
+ * splits == 1: + d_bias[j] and ReLU are applied if given; otherwise raw partials at d_C + s*split_stride. */
 int64_t dz_test_tc_pgemm_work(int32_t a_rows, int32_t b_rows, int32_t red);
 int dz_test_tc_pgemm(const float* d_A, int32_t a_rows, int32_t a_ld, int32_t a_red_contig, const float* d_B,
                      int32_t b_rows, int32_t b_ld, int32_t b_red_contig, int32_t red, int32_t a_ones_row,

@@ -45,8 +45,9 @@ class NetSpec(NamedTuple):
   num_quantiles: int = 201     # qrdqn (`qrdqn/run_atari.py:83`)
   latent_dim: int = 64         # iqn (`iqn/run_atari.py:56`)
   noisy_sigma0: float = 0.1    # rainbow (`rainbow/run_atari.py:99`)
-  obs_hw: int = 84
+  obs_hw: int = 84             # observation height (and width, unless obs_w is given)
   obs_c: int = 4
+  obs_w: Optional[int] = None  # observation width of a non-square observation; None: obs_hw
 
 
 def conv_out(n, k, s):
@@ -55,7 +56,8 @@ def conv_out(n, k, s):
 
 def feature_dim(spec):
   h = conv_out(conv_out(conv_out(spec.obs_hw, 8, 4), 4, 2), 3, 1)
-  return h * h * 64
+  w = conv_out(conv_out(conv_out(spec.obs_hw if spec.obs_w is None else spec.obs_w, 8, 4), 4, 2), 3, 1)
+  return h * w * 64
 
 
 def head_out(spec):

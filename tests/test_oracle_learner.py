@@ -24,14 +24,15 @@ from oracle import learner_oracle as lo
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'learner_hand_vectors.json')
 
 
-def tiny_case(kind, seed=0, B=3):
-  spec = lo.NetSpec(kind, 4, num_atoms=7, num_quantiles=5, latent_dim=16, obs_hw=44)
+def tiny_case(kind, seed=0, B=3, hw=(44, 44)):
+  H, W = hw
+  spec = lo.NetSpec(kind, 4, num_atoms=7, num_quantiles=5, latent_dim=16, obs_hw=H, obs_w=W)
   rs = np.random.RandomState(seed)
   # larger-than-default weights so that every head has O(1) outputs and the loss is well away from flat regions
   online = {k: (v * 3.0).astype(np.float64) for k, v in lo.init_params(spec, seed).items()}
   target = {k: (v * 3.0).astype(np.float64) for k, v in lo.init_params(spec, seed + 1).items()}
-  s_tm1 = rs.randint(0, 256, (B, 44, 44, 4)).astype(np.uint8)
-  s_t = rs.randint(0, 256, (B, 44, 44, 4)).astype(np.uint8)
+  s_tm1 = rs.randint(0, 256, (B, H, W, 4)).astype(np.uint8)
+  s_t = rs.randint(0, 256, (B, H, W, 4)).astype(np.uint8)
   batch = lo.batch_from_numpy(s_tm1, rs.randint(0, 4, B), rs.choice([-1.0, 0.5, 1.0], B), rs.choice([0.0, 0.99], B), s_t)
   w = torch.tensor(rs.uniform(0.2, 1.0, B)) if kind in ('rainbow', 'prioritized') else None
   taus = [torch.tensor(rs.uniform(size=(B, n)).astype(np.float32)) for n in (6, 4, 5)] if kind == 'iqn' else None
@@ -56,7 +57,20 @@ def loss_value(spec, online_np, target_np, batch, w, taus, noise, bound):
 
 @pytest.mark.parametrize('kind', lo.AGENT_KINDS)
 def test_autograd_gradients_equal_finite_differences(kind):
-  spec, online, target, batch, w, taus, noise = tiny_case(kind)
+  check_finite_differences(kind, (44, 44))
+
+
+@pytest.mark.parametrize('kind,hw', [('dqn', (36, 52)), ('rainbow', (52, 36)), ('iqn', (52, 36))])
+def test_non_square_observation_gradients_equal_finite_differences(kind, hw):
+  """A non-square observation (conv3 output 1x3 or 3x1): the feature size follows obs_hw x obs_w, so the fc1 / embed /
+  noise shapes of the spec must match what the torso produces, and the gradients still equal finite differences."""
+  assert lo.feature_dim(lo.NetSpec(kind, 4, obs_hw=hw[0], obs_w=hw[1])) == 64 * 3
+  assert lo.feature_dim(lo.NetSpec(kind, 4, obs_hw=hw[0])) == 64 * (1 if hw[0] == 36 else 9)   # obs_w defaults to obs_hw
+  check_finite_differences(kind, hw)
+
+
+def check_finite_differences(kind, hw):
+  spec, online, target, batch, w, taus, noise = tiny_case(kind, hw=hw)
   bound = 1e9   # clip_gradient inactive: the gradient is the derivative of the loss
   on = {k: torch.tensor(v, dtype=torch.float64, requires_grad=True) for k, v in online.items()}
   tg = {k: torch.tensor(v, dtype=torch.float64) for k, v in target.items()}
