@@ -144,6 +144,7 @@ _SIGNATURES = {
     'dz_test_umma_gemm_path': (i32, [vp, i32, vp, i32, i32, i32, i32, i32, vp, i32, i32, vp, i32, vp, vp, vp, i32, vp]),
     'dz_test_fc_forward': (i32, [i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp, vp, vp, i32, vp, C.POINTER(i32),
                                  C.POINTER(i64), vp]),
+    'dz_test_fc_dgrad': (i32, [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, i32, vp, C.POINTER(i32), vp]),
     'dz_test_conv1_forward': (i32, [i32, i32, i32, i32, vp, vp, vp, i64, vp, i32, vp, vp, vp]),
 }
 

@@ -1234,8 +1234,11 @@ struct dz_learner {
   // second stream for work that is off the critical path of the backward pass (weight gradients, priority
   // write-back, noise generation)
   SideStream side;
-  // third branch: the FC part of the split gradient norm and the conv2 weight gradient run beside the first side stream
+  // third branch: the conv2 weight gradient runs beside the first side stream
   SideStream side2;
+  // fourth branch: the conv3 and conv1 weight gradients.  They need only the main stream's input gradients, so they
+  // do not queue behind the FC / head weight gradients and the FC norm on the first side stream.
+  SideStream side3;
   float* norm_parts;                        // split-norm slots written by the conv weight-gradient finish kernels
   // TMA-fed tensor-core path of the batch-sized step (dz_umma_net.cu): torso + 3136 -> 512 layer(s), forward and input gradients
   UmNet* um;
@@ -1882,8 +1885,8 @@ int backward_torso(dz_learner* l, const uint8_t* const* rows0, void* stream) {
   if (l->um && l->cfg.kind == DZ_IQN) DZ_TRY(um_split_dact3(l->um, stream));   // dact3 came from the Hadamard kernel (fp32)
   // conv3 wgrad
   float* norm_parts = split_norm_active(l) ? l->norm_parts : nullptr;
-  if (l->um) {   // conv3 weight gradient + its finish (partial sums, bias gradient, split-norm partials) on the side stream
-    void* ws = l->side.fork(stream, stream);
+  if (l->um) {   // conv3 weight gradient + its finish (partial sums, bias gradient, split-norm partials) on a side stream
+    void* ws = l->side3.fork(stream, stream);
     DZ_TRY(um_wgrad_conv3(l->um, ws));
     DZ_TRY(um_wgrad_finish_layer(l->um, 3, G + o.conv_w[2], G + o.conv_b[2], norm_parts, ws));
   } else {
@@ -1941,9 +1944,10 @@ int backward_torso(dz_learner* l, const uint8_t* const* rows0, void* stream) {
   }
   // conv1 wgrad (A = uint8 rows in place)
   if (l->um) {
-    void* ws = l->side.fork(stream, stream);
+    void* ws = l->side3.fork(stream, stream);
     DZ_TRY(um_wgrad_conv1(l->um, rows0, ws));
     DZ_TRY(um_wgrad_finish_layer(l->um, 1, G + o.conv_w[0], G + o.conv_b[0], norm_parts, ws));
+    DZ_TRY(l->side3.join(stream));
     DZ_TRY(l->side2.join(stream));
     return l->side.join(stream);
   } else {
@@ -2347,7 +2351,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   else if (c.kind == DZ_IQN) DZ_TRY(backward_iqn(l, stream));
   else DZ_TRY(backward_plain(l, stream));
   if (split_norm_active(l)) {   // every gradient behind the conv tensors is final once the side stream's FC / head wgrads are done
-    DZ_TRY(norm_fc_range(l, apply_update != 0, l->side2.fork(l->side.tail(stream), stream)));
+    DZ_TRY(norm_fc_range(l, apply_update != 0, l->side.tail(stream)));
   }
   DZ_TRY(backward_torso(l, batch->d_s_tm1_rows, stream));
 
@@ -2431,6 +2435,7 @@ int dz_learner_create(const dz_learner_config* cfg, const dz_learner_buffers* bu
   }
   cudaError_t se = l->side.create();
   if (se == cudaSuccess) se = l->side2.create();
+  if (se == cudaSuccess) se = l->side3.create();
   if (se != cudaSuccess) { dz_learner_destroy(l); return fail(DZ_ECUDA, "side streams: %s", cudaGetErrorString(se)); }
   // The categorical loss needs more than the default 48 KB of dynamic shared memory at large num_actions x num_atoms.
   // The attribute is per device: set it for the device this learner is created on.
@@ -2466,6 +2471,7 @@ void dz_learner_destroy(dz_learner* l) {
   um_net_destroy(l->um);
   l->side.destroy();
   l->side2.destroy();
+  l->side3.destroy();
   if (l->recon) cudaFree(l->recon);
   delete l;
 }

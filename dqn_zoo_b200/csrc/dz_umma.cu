@@ -131,8 +131,10 @@ int UmPlan::configure() {
   if (done) return DZ_OK;
   DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-  DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_fc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-  DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_fc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_fc_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_fc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_fc_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  DZ_CUDA_OK(cudaFuncSetAttribute(um::umma_fc_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   DZ_CUDA_OK(cudaFuncSetAttribute(um::wgmma_gemm_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   DZ_CUDA_OK(cudaFuncSetAttribute(um::wgmma_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   done = true;
@@ -156,7 +158,9 @@ bool UmPlan::fc_eligible(const UmLaunch& l) const {
     if (np > um::kFcMaxProbs) return false;
     for (int q = 0; q < np; ++q) {
       const UmProblem& pr = probs[c.prob + q];
-      if (!pr.A.mn_major || pr.A.lbo != 4096u || pr.A.part_bytes * (uint32_t)np != 16384u) return false;
+      if (pr.A.mn_major != probs[ctas[l.cta0].prob].A.mn_major) return false;   // one A layout per launch
+      if (pr.A.mn_major ? pr.A.lbo != 4096u : np != 1) return false;
+      if (pr.A.part_bytes * (uint32_t)np != 16384u) return false;
       if (pr.A.convert != 2 && !(pr.A.convert == 1 && pr.A.scale_r == nullptr)) return false;
       if (pr.B.mn_major || pr.B.nparts != 2 || pr.B.convert) return false;
       if (pr.ksteps != 4 || pr.red_per_stage != 32 || pr.epi != UM_EPI_PARTIAL || pr.sc_i != 1) return false;
@@ -206,12 +210,11 @@ int UmPlan::launch(const char* tag, const UmLaunch& l, void* stream, long long* 
     return DZ_OK;
   }
   if (path != UM_PATH_CONVERTERS && fc_eligible(l)) {
-    if (v == 0)
-      DZ_LAUNCH_NAMED(tag, um::umma_fc_kernel<32>, (unsigned)l.nctas, um::kThreadsF, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps,
-                      stages, l.stage_bytes, d_trace);
-    else
-      DZ_LAUNCH_NAMED(tag, um::umma_fc_kernel<64>, (unsigned)l.nctas, um::kThreadsF, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps,
-                      stages, l.stage_bytes, d_trace);
+    const bool ak = !probs[ctas[l.cta0].prob].A.mn_major;
+    auto kern = v == 0 ? (ak ? um::umma_fc_kernel<32, true> : um::umma_fc_kernel<32, false>)
+                       : (ak ? um::umma_fc_kernel<64, true> : um::umma_fc_kernel<64, false>);
+    DZ_LAUNCH_NAMED(tag, kern, (unsigned)l.nctas, um::kThreadsF, smem, stream, lm, d_ctas + l.cta0, d_probs, d_ops, l.nmaps, stages,
+                    l.stage_bytes, d_trace);
     return DZ_OK;
   }
   for (int ci = l.cta0; ci < l.cta0 + l.nctas; ++ci)

@@ -18,8 +18,8 @@
 //
 // Precision: activations are stored ONCE as tf32 hi/lo pairs by the producing epilogue (x = hi + lo, both exactly
 // representable), fp32 weights are split in place in shared memory by converter warps (raw tile -> hi in place, lo
-// in the sibling buffer; the split is position-wise, so it is swizzle-agnostic) or, for the fc forward, in the MMA
-// warps' registers (umma_fc_kernel), D += Al*Bh + Ah*Bl + Ah*Bh.  The
+// in the sibling buffer; the split is position-wise, so it is swizzle-agnostic) or, for the fc forward and input
+// gradient, in the MMA warps' registers (umma_fc_kernel), D += Al*Bh + Ah*Bl + Ah*Bh.  The
 // tensor core truncates its fp32 accumulator, so each k-step's products are added into the fp32 sums with
 // round-to-nearest adds (dz_tc.cuh, warp_kstep_3xtf32 / wgmma_kstep_3xtf32).
 //
@@ -466,10 +466,13 @@ __device__ __forceinline__ void stamp_if(long long* addr, bool pred) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Sibling of umma_gemm_kernel for the fc1 / noisy1 forward: A = raw fp32 weights W[k][n], staged MN-major (mu, plus
-// sigma for noisy layers), B = activations, K-major tf32 hi/lo pairs.  There are no converter warps: every MMA warp
-// loads raw mu / sigma fragments from the staged tile at the addresses umma_gemm_kernel reads hi fragments from, forms
-//     w = fmaf(sigma, eps_in[k] * eps_out[n], mu)        (noisy; the operations and their order of convert_part16k)
+// Sibling of umma_gemm_kernel for the fc1 / noisy1 forward and input gradient: A = raw fp32 weights W[k][n] (mu, plus
+// sigma for noisy layers), B = activations / output gradients, K-major tf32 hi/lo pairs.  The forward stages A
+// MN-major (D row = n, reduction = k), the input gradient K-major (AK: D row = k, reduction = n; W's rows are
+// contiguous in n).  There are no converter warps: every MMA warp loads raw mu / sigma fragments from the staged tile
+// at the addresses umma_gemm_kernel reads hi fragments from, forms
+//     w = fmaf(sigma, scale_r[r] * scale_i[i], mu)       (noisy; the operations and their order of convert_part16k)
+// (scale_r: the noise factor of the reduction index, scale_i: that of the D row; eps_in[k] * eps_out[n] either way)
 // and its tf32 hi/lo split in registers, and issues the k-step of warp_kstep_3xtf32.  Each output element therefore sees
 // the same operands and the same sequence of k-steps as on umma_gemm_kernel: the partials are bit-identical.
 //
@@ -482,7 +485,7 @@ constexpr int kFcMmaWarps = 8;
 constexpr int kThreadsF = (1 + kFcMmaWarps) * 32;
 constexpr int kFcMaxProbs = 2;
 
-template <int NJT>
+template <int NJT, bool AK>
 __global__ void __launch_bounds__(kThreadsF, 1)
     umma_fc_kernel(const __grid_constant__ UmMaps maps, const UmCta* __restrict__ ctas, const UmProblem* __restrict__ probs,
                    const UmTmaOp* __restrict__ ops, int nmaps, int stages, uint32_t stage_bytes, long long* __restrict__ trace) {
@@ -555,7 +558,7 @@ __global__ void __launch_bounds__(kThreadsF, 1)
   const uint8_t* b_first = stage_base + a_part * 2 + (uint32_t)q * 2u * p.B.part_bytes;
   const uint32_t b_part = p.B.part_bytes;
   const bool noisy = p.A.convert == 2;
-  const float* __restrict__ eps_in = p.A.scale_r;
+  const float* __restrict__ eps_r = p.A.scale_r;
   constexpr int NT = NJT / 8;
   float sum[1][NT][4];
 #pragma unroll
@@ -564,15 +567,22 @@ __global__ void __launch_bounds__(kThreadsF, 1)
     for (int e = 0; e < 4; ++e) sum[0][nt][e] = 0.f;
   auto b_off = [](int n, int k) { return sw128_kmajor(n, k); };
   dz::pdl_enter();                                          // the noise vectors may come from an earlier kernel
-  // eps_out of the thread's two D rows (g, g + 8): loop invariants
+  // noise factor of the thread's two D rows (g, g + 8): loop invariants.  Rows past MI (the zero-filled tail of the
+  // input gradient's last tile, never stored) read the last row's factor, as the converters do.
   float eo[2] = {1.f, 1.f};
   if (noisy) {
-    eo[0] = p.A.scale_i[cta.i0 + m0 + g];
-    eo[1] = p.A.scale_i[cta.i0 + m0 + g + 8];
+    eo[0] = p.A.scale_i[min(cta.i0 + m0 + g, p.MI - 1)];
+    eo[1] = p.A.scale_i[min(cta.i0 + m0 + g + 8, p.MI - 1)];
   }
+  // Noise factors of a stage's 32 reduction indices: lane L holds the one of index r0 + L and the k-steps take theirs
+  // by shuffle.  The next stage's load is issued before the current stage's barrier wait, so its global-load latency
+  // is hidden behind a stage of MMAs instead of sitting at the head of every stage's dependency chain.
+  float er_next = noisy ? eps_r[cta.r0 + lane] : 1.f;
   int s = 0, r0 = cta.r0;
   uint32_t ph = 0;
   for (int it = 0; it < nst; ++it) {
+    const float er = er_next;
+    if (noisy && it + 1 < nst) er_next = eps_r[r0 + 32 + lane];
     mbar_wait(&full[s], ph);
     stamp_if(trace + 64 + it, tr && lead && it < 64);                                               // [64,128): stage data ready
     const uint8_t* mu = stage_base + (size_t)s * stage_bytes;
@@ -583,11 +593,13 @@ __global__ void __launch_bounds__(kThreadsF, 1)
 #pragma unroll(NJT == 32 ? 4 : 2)
     for (int ks = 0; ks < 4; ++ks) {
       uint32_t ah[1][4], al[1][4];
-      float ei[2] = {1.f, 1.f};              // eps_in of the thread's reduction indices k = 8 ks + t + 4 h
-      if (noisy) { ei[0] = eps_in[r0 + 8 * ks + t]; ei[1] = eps_in[r0 + 8 * ks + t + 4]; }
+      // noise factors of the thread's reduction indices r0 + 8 ks + t + 4 h; shuffled unconditionally (1 on plain
+      // layers), so that no branch splits the stage's straight-line k-steps
+      const float ei[2] = {__shfl_sync(0xffffffffu, er, 8 * ks + t), __shfl_sync(0xffffffffu, er, 8 * ks + t + 4)};
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const uint32_t o = sw128_mnmajor(m0 + g + (e & 1) * 8, 8 * ks + t + (e >> 1) * 4, a_lbo);
+        const int m = m0 + g + (e & 1) * 8, k = 8 * ks + t + (e >> 1) * 4;
+        const uint32_t o = AK ? sw128_kmajor(m, k) : sw128_mnmajor(m, k, a_lbo);
         float v = *reinterpret_cast<const float*>(mu + o);
         if (noisy) {
           const float f = ei[e >> 1] * eo[e & 1];

@@ -87,8 +87,9 @@ struct UmPlan {
   int launch(const char* tag, const UmLaunch& l, void* stream, long long* d_trace = nullptr, int path = UM_PATH_AUTO) const;
   // Every CTA of the launch has both operands K-major tf32 hi/lo pairs that need no conversion, four k-steps per stage.
   bool wgmma_eligible(const UmLaunch& l) const;
-  // Every CTA has an MN-major raw fp32 A (convert 1 without scale_r, or 2) of 128 / nprob rows and 32 reduction rows per
-  // stage, nprob <= 2, a K-major pre-split B, four k-steps per stage and the direct partial epilogue.
+  // Every CTA has a raw fp32 A (convert 1 without scale_r, or 2), either MN-major of 128 / nprob rows and 32 reduction
+  // rows per stage, nprob <= 2, or K-major of 128 rows, nprob 1 (the same layout in every CTA of the launch), a K-major
+  // pre-split B, four k-steps per stage and the direct partial epilogue.
   bool fc_eligible(const UmLaunch& l) const;
   int path_of(const UmLaunch& l) const { return wgmma_eligible(l) ? UM_PATH_WGMMA : UM_PATH_MMA_SYNC; }
   static int configure();   // one-time kernel attributes (outside any stream capture)

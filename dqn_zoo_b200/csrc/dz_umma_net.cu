@@ -1301,7 +1301,8 @@ int build_plan(UmNet* n) {
       }
       pl.end_launch(l);
     }
-    // ---- input gradient: D[k, m] = sum_n W[k][n] g[m][n];  noisy: W = Wmu + Wsigma * (eps_in[k] * eps_out[n]) in the converters
+    // ---- input gradient: D[k, m] = sum_n W[k][n] g[m][n];  noisy: W = Wmu + Wsigma * (eps_in[k] * eps_out[n]), formed in the
+    // MMA warps (umma_fc_kernel on the K-major tile; with UM_PATH_CONVERTERS by the converter warps of umma_gemm_kernel)
     {
       const UmOperand Bo = um_kmajor(njt, true, false);
       const int S = n->fcd_splits, per = (16 + S - 1) / S, ktiles = (feat + 127) / 128;
@@ -1619,6 +1620,44 @@ extern "C" int dz_test_fc_forward(int32_t B, int32_t H, int32_t W, int32_t npass
     }
     *weight_bytes = wb;
   }
+  if (n) um_net_destroy(n);
+  cudaFree(ws);
+  return rc;
+}
+
+// Test hook: the fc1 / noisy1 input-gradient launch alone, on the output gradients g [nstream][B][512] (feat from the
+// H x W observation geometry).  Stream s reads the online weights at online + off_w[s] (mu) and + off_sw[s] (sigma,
+// noisy); its noise is eps_in / eps_out at noise + off_in[s] / off_out[s].  converters = 0: the learner's launch on
+// umma_fc_kernel; 1: umma_gemm_kernel and its converter warps.  Writes the split partials [nstream][S][B][feat] to d_part
+// (room for nstream * 8 * B * feat floats) and S to *splits.
+extern "C" int dz_test_fc_dgrad(int32_t B, int32_t H, int32_t W, int32_t nstream, int32_t noisy, const float* online, const int64_t* off_w,
+                                const int64_t* off_sw, const float* noise, const int64_t* off_in, const int64_t* off_out, const float* g,
+                                int32_t converters, float* d_part, int32_t* splits, void* stream) {
+  if (nstream < 1 || nstream > 2) return fail(DZ_EINVAL, "fc input-gradient test: nstream 1..2");
+  UmNetDesc d;
+  memset(&d, 0, sizeof(d));
+  d.B = B; d.H = H; d.W = W; d.npass = 1;
+  d.online = online; d.target = online;
+  d.use_fc = 1; d.nstream = nstream; d.noisy = noisy ? 1 : 0;
+  for (int s = 0; s < nstream; ++s) {
+    d.off_fc_w[s] = off_w[s];
+    if (noisy) { d.off_fc_sw[s] = off_sw[s]; d.noise_off_in[s] = off_in[s]; d.noise_off_out[s] = off_out[s]; }
+  }
+  if (!um_net_supported(d)) return fail(DZ_EINVAL, "fc input-gradient test: geometry not supported by the tensor-core path");
+  char* ws = nullptr;
+  DZ_CUDA_OK(cudaMalloc(&ws, (size_t)um_net_workspace_bytes(d)));
+  UmNet* n = nullptr;
+  int rc = net_create(d, ws, &n, false);
+  if (rc == DZ_OK) rc = um_split(g, n->dh1_hi, n->dh1_lo, (long long)nstream * B * 512, stream);
+  if (rc == DZ_OK && noisy) rc = apply_noise(n, noise, stream);
+  if (rc == DZ_OK) rc = n->plan.launch("fc1_dgrad", n->launches[kFcDgrad], stream, nullptr, converters ? UM_PATH_CONVERTERS : UM_PATH_AUTO);
+  if (rc == DZ_OK) {
+    const size_t bytes = (size_t)nstream * n->fcd_splits * B * n->feat * sizeof(float);
+    if (cudaMemcpyAsync(d_part, n->fcd_part, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream) != cudaSuccess ||
+        cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess)
+      rc = fail(DZ_ECUDA, "fc input-gradient test: %s", cudaGetErrorString(cudaGetLastError()));
+  }
+  if (rc == DZ_OK) *splits = n->fcd_splits;
   if (n) um_net_destroy(n);
   cudaFree(ws);
   return rc;

@@ -482,6 +482,13 @@ int dz_test_fc_forward(int32_t B, int32_t H, int32_t W, int32_t npass, int32_t n
                        const float* target, const int64_t* off_w, const int64_t* off_sw, const float* noise, int64_t noise_stride,
                        const int64_t* off_in, const int64_t* off_out, const float* x, int32_t per_pass, float* d_part,
                        int32_t* splits, int64_t* weight_bytes, void* stream);
+/* The fc1 / noisy1 input-gradient launch alone (split partials [nstream][S][B][feat] of the output gradients
+ * g [nstream][B][512] against the stream weights at online + off_w[s] (mu) and + off_sw[s] (sigma), noise eps_in /
+ * eps_out at noise + off_in[s] / off_out[s]).  converters = 0: the learner's umma_fc_kernel; 1: umma_gemm_kernel with
+ * converter warps.  d_part holds nstream * 8 * B * feat floats.  Synchronizes. */
+int dz_test_fc_dgrad(int32_t B, int32_t H, int32_t W, int32_t nstream, int32_t noisy, const float* online, const int64_t* off_w,
+                     const int64_t* off_sw, const float* noise, const int64_t* off_in, const int64_t* off_out, const float* g,
+                     int32_t converters, float* d_part, int32_t* splits, void* stream);
 /* The conv1 forward launch alone: act1 tf32 hi / lo [npass * B][h1][w1][32] (into d_hi / d_lo) of the uint8
  * observations B x H x W x 4 that rows[p] (host array of npass device tables of B row pointers) point at, pass layout as
  * in dz_test_fc_forward.  off_conv_w: the three conv weight offsets in both blobs; off_conv_b1: conv1's bias.  path: 2 the
