@@ -127,6 +127,13 @@ _SIGNATURES = {
     'dz_learner_act_batch_stream_noise': (i32, [vp, vp, i32, vp, vp, f32, vp, vp, vp]),
     'dz_learner_noise_stride': (i32, [C.POINTER(LearnerConfig), C.POINTER(i64)]),
     'dz_learner_generate_stream_noise': (i32, [vp, u64, i32, vp, vp]),
+    'dz_actor_plan_query': (i32, [C.POINTER(LearnerConfig), i32, C.POINTER(i64)]),
+    'dz_actor_create': (i32, [vp, i32, vp, C.POINTER(vp)]),
+    'dz_actor_destroy': (None, [vp]),
+    'dz_actor_act': (i32, [vp, vp, vp, vp, i64, vp, f32, vp, vp, vp]),
+    'dz_actor_generate_randomness': (i32, [vp, u64, i32, vp, vp]),
+    'dz_test_actor_mma_path': (i32, [vp, C.c_char_p, C.POINTER(i32)]),
+    'dz_test_actor_buffer': (i32, [vp, C.c_char_p, vp, vp]),
     'dz_learner_sync_target': (i32, [vp, vp]),
     'dz_test_u8_to_unit': (i32, [vp, vp]),
     'dz_atari_preprocess': (i32, [vp, vp, i32, vp, vp, vp, vp, i32, vp, i32, vp]),

@@ -540,7 +540,8 @@ class BatchedEpsilonGreedyActor:
   q-values and the epsilon-greedy choice on the device) -> one device-to-host copy of E actions.
 
   `learner` is the training agent's `Learner` (shared parameters, as the reference's actors read the learner's online
-  params) or any `Learner` whose batch size is >= E.  Exploration uniforms come from a host RandomState seeded from
+  params).  Up to its batch size the tick runs on `Learner.act_batch`; beyond it, on a `learner_lib.Actor` sized for the
+  E streams (up to 1024), over the same live parameters.  Exploration uniforms come from a host RandomState seeded from
   `rng_key` (2E floats per tick; the reference draws with the JAX PRNG per actor).  IQN: every stream gets its own tau
   samples.  Rainbow explores only through its noisy layers: by default one noise sample per tick is shared by the E
   streams, so they explore in lockstep; `per_stream_noise=True` draws E samples per tick and gives stream e its own, as
@@ -548,10 +549,12 @@ class BatchedEpsilonGreedyActor:
 
   def __init__(self, learner: learner_lib.Learner, num_streams: int, exploration_epsilon, rng_key,
                per_stream_noise: bool = False):
-    if num_streams < 1 or num_streams > learner.batch_size:
-      raise ValueError('num_streams must be in [1, learner.batch_size]')
+    if num_streams < 1:
+      raise ValueError('num_streams must be >= 1')
     if per_stream_noise and learner.net.kind != 'rainbow':
       raise ValueError('per_stream_noise needs a rainbow learner')
+    # beyond the learner's batch the tick needs buffers of its own size
+    self._actor = learner.actor(num_streams) if num_streams > learner.batch_size else None
     self._learner = learner
     self._per_stream_noise = bool(per_stream_noise)
     self._E = int(num_streams)
@@ -577,16 +580,26 @@ class BatchedEpsilonGreedyActor:
       explore = self._explore_dev
     taus = noise = stream_noise = None
     kind = L.net.kind
-    if self._per_stream_noise:
-      stream_noise = L.generate_stream_noise(self._seed, self._E)
-    elif kind in ('iqn', 'rainbow'):
-      L.generate_randomness(self._seed)
-      if kind == 'iqn':
-        taus = L.taus[:self._E * L.net.tau_samples_policy] if hasattr(L.net, 'tau_samples_policy') else L.taus
-      else:
-        noise = L.noise
-    actions, self.q_values = L.act_batch(observations, epsilon=eps, explore=explore, taus=taus, noise=noise,
-                                         stream_noise=stream_noise)
+    if self._actor is not None:
+      if self._per_stream_noise:
+        stream_noise = self._actor.generate_randomness(self._seed, per_stream=True)
+      elif kind == 'iqn':
+        taus = self._actor.generate_randomness(self._seed)
+      elif kind == 'rainbow':
+        noise = self._actor.generate_randomness(self._seed)
+      actions, self.q_values = self._actor.act(observations, epsilon=eps, explore=explore, taus=taus, noise=noise,
+                                               stream_noise=stream_noise)
+    else:
+      if self._per_stream_noise:
+        stream_noise = L.generate_stream_noise(self._seed, self._E)
+      elif kind in ('iqn', 'rainbow'):
+        L.generate_randomness(self._seed)
+        if kind == 'iqn':
+          taus = L.taus[:self._E * L.net.tau_samples_policy] if hasattr(L.net, 'tau_samples_policy') else L.taus
+        else:
+          noise = L.noise
+      actions, self.q_values = L.act_batch(observations, epsilon=eps, explore=explore, taus=taus, noise=noise,
+                                           stream_noise=stream_noise)
     self._actions_host.copy_(actions, non_blocking=True)
     torch.cuda.current_stream().synchronize()
     self._t += 1

@@ -1546,9 +1546,33 @@ struct Pass {        // one network.apply
 
 // ---- forward -----------------------------------------------------------------------------------
 
+// The buffers a forward pass writes: torso activation sets [set], head outputs [head pass] (indices as in Pass), and
+// the split-K partials of the fp32-FMA GEMMs.  The learner passes its own; an actor passes buffers sized for its streams.
+struct NetBufs {
+  float *act1[3], *act2[3], *act3[3];
+  float *h1[3][2], *out[3], *outv[3];
+  float *cosf[3], *hi[3];
+  float* nn_partial;
+  float* conv_partial;
+  int split_rows;      // the fp32 fc1 / head GEMMs split K (into nn_partial) when the pass has at most this many images
+};
+
+NetBufs learner_bufs(const dz_learner* l) {
+  NetBufs b;
+  for (int p = 0; p < 3; ++p) {
+    b.act1[p] = l->act1[p]; b.act2[p] = l->act2[p]; b.act3[p] = l->act3[p];
+    b.h1[p][0] = l->h1[p][0]; b.h1[p][1] = l->h1[p][1]; b.out[p] = l->out[p]; b.outv[p] = l->outv[p];
+    b.cosf[p] = l->cosf[p]; b.hi[p] = l->hi[p];
+  }
+  b.nn_partial = l->nn_partial;
+  b.conv_partial = l->conv_partial;
+  b.split_rows = 32;
+  return b;
+}
+
 struct TorsoJob { const float* params; const uint8_t* const* rows; int set; };
 
-int forward_torso(dz_learner* l, const TorsoJob* jobs, int njobs, int nimg, void* stream) {
+int forward_torso(dz_learner* l, const NetBufs& nb, const TorsoJob* jobs, int njobs, int nimg, void* stream) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
   GemmBatch gb;
@@ -1559,7 +1583,7 @@ int forward_torso(dz_learner* l, const TorsoJob* jobs, int njobs, int nimg, void
     GemmProblem p = zero_problem();
     set_conv(p, A_CONV_U8, jobs[i].rows, nimg, d.H, d.W, d.C, 8, 8, 4);
     p.B = jobs[i].params + o.conv_w[0]; p.bias = jobs[i].params + o.conv_b[0];
-    p.N = 32; p.ldb = 32; p.ldc = 32; p.relu = 1; p.C = l->act1[jobs[i].set];
+    p.N = 32; p.ldb = 32; p.ldc = 32; p.relu = 1; p.C = nb.act1[jobs[i].set];
     gb.p[i] = p;
   }
   DZ_TRY(run_nn("conv1_fwd", gb, false, stream));
@@ -1570,17 +1594,17 @@ int forward_torso(dz_learner* l, const TorsoJob* jobs, int njobs, int nimg, void
     for (int i = 0; i < njobs; ++i) {
       GemmProblem p = zero_problem();
       if (layer == 2) {
-        set_conv(p, A_CONV_F32, l->act1[jobs[i].set], nimg, d.h1, d.w1, 32, 4, 4, 2);
+        set_conv(p, A_CONV_F32, nb.act1[jobs[i].set], nimg, d.h1, d.w1, 32, 4, 4, 2);
         p.B = jobs[i].params + o.conv_w[1]; p.bias = jobs[i].params + o.conv_b[1];
-        outs[i] = l->act2[jobs[i].set];
+        outs[i] = nb.act2[jobs[i].set];
       } else {
-        set_conv(p, A_CONV_F32, l->act2[jobs[i].set], nimg, d.h2, d.w2, 64, 3, 3, 1);
+        set_conv(p, A_CONV_F32, nb.act2[jobs[i].set], nimg, d.h2, d.w2, 64, 3, 3, 1);
         p.B = jobs[i].params + o.conv_w[2]; p.bias = jobs[i].params + o.conv_b[2];
-        outs[i] = l->act3[jobs[i].set];
+        outs[i] = nb.act3[jobs[i].set];
       }
       p.N = 64; p.ldb = 64; p.ldc = 64; p.relu = 1;
       p.splits = l->conv_splits; p.split_stride = (long long)p.M * 64;
-      p.C = l->conv_partial + (long long)i * p.splits * p.split_stride;
+      p.C = nb.conv_partial + (long long)i * p.splits * p.split_stride;
       gb.p[i] = p;
     }
     DZ_TRY(run_nn(layer == 2 ? "conv2_fwd" : "conv3_fwd", gb, false, stream));
@@ -1590,23 +1614,23 @@ int forward_torso(dz_learner* l, const TorsoJob* jobs, int njobs, int nimg, void
 }
 
 // Heads for the dqn / double_q / prioritized / c51 / qrdqn family.
-int forward_heads_plain(dz_learner* l, const Pass* passes, int np, int nimg, void* stream, bool fc1_done = false) {
+int forward_heads_plain(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, void* stream, bool fc1_done = false) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
   GemmBatch gb;
   gb.n = np;
   float* outs[kMaxProblems];
   const bool shared = l->cfg.kind == DZ_DOUBLE_Q || l->cfg.kind == DZ_PRIORITIZED;
-  const int splits = nimg <= 32 ? l->fc_splits : 1;
+  const int splits = nimg <= nb.split_rows ? l->fc_splits : 1;
   for (int i = 0; i < np && !fc1_done; ++i) {
     GemmProblem p = zero_problem();
-    p.a_mode = A_PLAIN; p.A = l->act3[passes[i].set]; p.lda = d.feat; p.M = nimg; p.K = d.feat;
+    p.a_mode = A_PLAIN; p.A = nb.act3[passes[i].set]; p.lda = d.feat; p.M = nimg; p.K = d.feat;
     p.B = passes[i].params + o.w1[0]; p.N = 512; p.ldb = 512; p.ldc = 512;
     p.bias = passes[i].params + o.b1[0]; p.relu = 1;
-    outs[i] = l->h1[passes[i].head][0];
+    outs[i] = nb.h1[passes[i].head][0];
     if (splits > 1) {
       p.splits = splits; p.split_stride = (long long)nimg * 512;
-      p.C = l->nn_partial + (long long)i * splits * p.split_stride;
+      p.C = nb.nn_partial + (long long)i * splits * p.split_stride;
     } else {
       p.C = outs[i];
     }
@@ -1618,26 +1642,26 @@ int forward_heads_plain(dz_learner* l, const Pass* passes, int np, int nimg, voi
   }
   for (int i = 0; i < np; ++i) {
     GemmProblem p = zero_problem();
-    p.a_mode = A_PLAIN; p.A = l->h1[passes[i].head][0]; p.lda = 512; p.M = nimg; p.K = 512;
+    p.a_mode = A_PLAIN; p.A = nb.h1[passes[i].head][0]; p.lda = 512; p.M = nimg; p.K = 512;
     p.B = passes[i].params + o.w2[0]; p.N = d.out; p.ldb = d.out; p.ldc = d.out;
     p.bias = passes[i].params + o.b2[0]; p.bias_shared = shared ? 1 : 0;
-    outs[i] = l->out[passes[i].head];
-    if (nimg <= 32) {
+    outs[i] = nb.out[passes[i].head];
+    if (nimg <= nb.split_rows) {
       p.splits = l->head_splits; p.split_stride = (long long)nimg * d.out;
-      p.C = l->nn_partial + (long long)i * p.splits * p.split_stride;
+      p.C = nb.nn_partial + (long long)i * p.splits * p.split_stride;
     } else {
       p.C = outs[i];
     }
     gb.p[i] = p;
   }
   DZ_TRY(run_nn("head_fwd", gb, false, stream));
-  if (nimg <= 32) DZ_TRY(finish_nn(gb, outs, false, stream));
+  if (nimg <= nb.split_rows) DZ_TRY(finish_nn(gb, outs, false, stream));
   return DZ_OK;
 }
 
 // Rainbow: two noisy streams (networks.py:224-261, :137-178).  noise_ld > 0: image m of the pass uses its own noise
 // apply at noise + m * noise_ld (one pass only); 0: every image uses the pass's apply.
-int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, const float* noise, void* stream, bool fc1_done = false,
+int forward_heads_rainbow(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, const float* noise, void* stream, bool fc1_done = false,
                           long long noise_ld = 0) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
@@ -1650,21 +1674,21 @@ int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, c
   GemmBatch gb;
   gb.n = 2 * np;
   float* outs[kMaxProblems];
-  const int splits = nimg <= 32 ? l->fc_splits : 1;
+  const int splits = nimg <= nb.split_rows ? l->fc_splits : 1;
   for (int i = 0; i < np && !fc1_done; ++i) {
     NoiseVecs nz = noise_of(c, d, noise, passes[i].apply);
     for (int s = 0; s < 2; ++s) {
       GemmProblem p = zero_problem();
-      p.a_mode = A_PLAIN; p.A = l->act3[passes[i].set]; p.lda = d.feat; p.M = nimg; p.K = d.feat;
+      p.a_mode = A_PLAIN; p.A = nb.act3[passes[i].set]; p.lda = d.feat; p.M = nimg; p.K = d.feat;
       p.B = passes[i].params + o.w1[s]; p.B2 = passes[i].params + o.sw1[s];
       p.N = 512; p.ldb = 512; p.ldc = 512;
       p.bias = passes[i].params + o.b1[s]; p.bias2 = passes[i].params + o.sb1[s];
       p.a_scale = s == 0 ? nz.a1i : nz.v1i; p.c_scale = s == 0 ? nz.a1o : nz.v1o; p.relu = 1;
       int q = 2 * i + s;
-      outs[q] = l->h1[passes[i].head][s];
+      outs[q] = nb.h1[passes[i].head][s];
       if (splits > 1) {
         p.splits = splits; p.split_stride = (long long)2 * nimg * 512;
-        p.C = l->nn_partial + (long long)q * splits * p.split_stride;
+        p.C = nb.nn_partial + (long long)q * splits * p.split_stride;
       } else {
         p.C = outs[q];
       }
@@ -1680,17 +1704,17 @@ int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, c
     for (int s = 0; s < 2; ++s) {
       int n_out = s == 0 ? c.num_actions * c.num_atoms : c.num_atoms;
       GemmProblem p = zero_problem();
-      p.a_mode = A_PLAIN; p.A = l->h1[passes[i].head][s]; p.lda = 512; p.M = nimg; p.K = 512;
+      p.a_mode = A_PLAIN; p.A = nb.h1[passes[i].head][s]; p.lda = 512; p.M = nimg; p.K = 512;
       p.B = passes[i].params + o.w2[s]; p.B2 = passes[i].params + o.sw2[s];
       p.N = n_out; p.ldb = n_out; p.ldc = n_out;
       p.bias = nullptr; p.bias2 = passes[i].params + o.sb2[s];   // with_bias=False: mu has no bias
       p.a_scale = s == 0 ? nz.a2i : nz.v2i; p.c_scale = s == 0 ? nz.a2o : nz.v2o;
       int q = 2 * i + s;
-      outs[q] = s == 0 ? l->out[passes[i].head] : l->outv[passes[i].head];
-      if (nimg <= 32) {
+      outs[q] = s == 0 ? nb.out[passes[i].head] : nb.outv[passes[i].head];
+      if (nimg <= nb.split_rows) {
         int64_t head_n = (int64_t)c.num_actions * c.num_atoms;
         p.splits = l->head_splits; p.split_stride = (long long)2 * nimg * n_out;
-        p.C = l->nn_partial + (long long)q * l->head_splits * 2 * nimg * head_n;
+        p.C = nb.nn_partial + (long long)q * l->head_splits * 2 * nimg * head_n;
       } else {
         p.C = outs[q];
       }
@@ -1698,7 +1722,7 @@ int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, c
     }
   }
   DZ_TRY(run("noisy2_fwd", gb));
-  if (nimg <= 32) DZ_TRY(finish_nn(gb, outs, true, stream, noise_ld));
+  if (nimg <= nb.split_rows) DZ_TRY(finish_nn(gb, outs, true, stream, noise_ld));
   return DZ_OK;
 }
 
@@ -1706,7 +1730,7 @@ int forward_heads_rainbow(dz_learner* l, const Pass* passes, int np, int nimg, c
 // one update on the packed-operand tensor-core kernels: one pack launch (cosine features + every weight operand of
 // this step), the embedding GEMM whose epilogue writes the hi/lo tile images of the next GEMMs directly (the fp32
 // `hi` tensors are never materialised), the split fc1 GEMM, one finish (bias + ReLU).
-int iqn_embed_fc1_forward_packed(dz_learner* l, const Pass* passes, const GemmBatch& fc1, bool keep_E0, void* stream) {
+int iqn_embed_fc1_forward_packed(dz_learner* l, const NetBufs& nb, const Pass* passes, const GemmBatch& fc1, bool keep_E0, void* stream) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
@@ -1721,7 +1745,7 @@ int iqn_embed_fc1_forward_packed(dz_learner* l, const Pass* passes, const GemmBa
     blob[k] = passes[i].params; widx[i] = k;
     int hp = passes[i].head;
     const dz_learner::PkImg& im = l->pk_cos[hp];
-    DZ_TRY(pk_add_job(pb, l->cosf[hp], c.latent_dim, 1, fc1.p[i].M, c.latent_dim, im.rows_pad, im.red_pad, -1, im.hi, im.lo));
+    DZ_TRY(pk_add_job(pb, nb.cosf[hp], c.latent_dim, 1, fc1.p[i].M, c.latent_dim, im.rows_pad, im.red_pad, -1, im.hi, im.lo));
   }
   for (int k = 0; k < 2; ++k) {
     if (!blob[k]) continue;
@@ -1744,7 +1768,7 @@ int iqn_embed_fc1_forward_packed(dz_learner* l, const Pass* passes, const GemmBa
     p.B = PkOperand{l->pk_weT[widx[i]].hi, l->pk_weT[widx[i]].lo, l->pk_weT[widx[i]].rows_pad / 8};
     p.MI = fc1.p[i].M; p.NJ = d.feat; p.nkb = l->pk_cos[hp].red_pad / kPkKB; p.splits = 1;
     p.bias_j = passes[i].params + o.embed_b;
-    p.mul = l->act3[passes[i].set]; p.mul_div = l->n_head[hp]; p.mul_ld = d.feat;
+    p.mul = nb.act3[passes[i].set]; p.mul_div = l->n_head[hp]; p.mul_ld = d.feat;
     p.e0 = (keep_E0 && hp == 0) ? l->E0 : nullptr; p.e0_ld = d.feat;
     p.img_hi = l->pk_act[hp].hi; p.img_lo = l->pk_act[hp].lo; p.img_rg = l->pk_act[hp].rows_pad / 8;
     if (keep_E0 && hp == 0) { p.imgT_hi = l->pk_actT.hi; p.imgT_lo = l->pk_actT.lo; p.imgT_rg = l->pk_actT.rows_pad / 8; }
@@ -1779,7 +1803,7 @@ int iqn_embed_fc1_forward_packed(dz_learner* l, const Pass* passes, const GemmBa
 }
 
 // IQN (networks.py:264-292): cosine embedding -> linear -> relu -> * state embedding -> value head.
-int forward_heads_iqn(dz_learner* l, const Pass* passes, int np, int nimg, const float* const* taus, bool keep_E0, void* stream) {
+int forward_heads_iqn(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, const float* const* taus, bool keep_E0, void* stream) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
@@ -1787,7 +1811,7 @@ int forward_heads_iqn(dz_learner* l, const Pass* passes, int np, int nimg, const
   gb.n = np;
   for (int i = 0; i < np; ++i) {
     long long rows = (long long)nimg * l->n_head[passes[i].head];
-    DZ_LAUNCH(iqn_cos_kernel, (unsigned)ceil_div(rows * c.latent_dim, 256), 256, 0, stream, taus[i], l->cosf[passes[i].head],
+    DZ_LAUNCH(iqn_cos_kernel, (unsigned)ceil_div(rows * c.latent_dim, 256), 256, 0, stream, taus[i], nb.cosf[passes[i].head],
               rows, c.latent_dim);
   }
   const bool packed = l->pk_on && nimg == l->B && np == 3;
@@ -1795,11 +1819,11 @@ int forward_heads_iqn(dz_learner* l, const Pass* passes, int np, int nimg, const
     for (int i = 0; i < np; ++i) {
       int hp = passes[i].head;
       GemmProblem p = zero_problem();
-      p.a_mode = A_PLAIN; p.A = l->cosf[hp]; p.lda = c.latent_dim; p.M = nimg * l->n_head[hp]; p.K = c.latent_dim;
+      p.a_mode = A_PLAIN; p.A = nb.cosf[hp]; p.lda = c.latent_dim; p.M = nimg * l->n_head[hp]; p.K = c.latent_dim;
       p.B = passes[i].params + o.embed_w; p.N = d.feat; p.ldb = d.feat; p.ldc = d.feat;
       p.bias = passes[i].params + o.embed_b; p.relu = 1;
-      p.mul = l->act3[passes[i].set]; p.mul_div = l->n_head[hp];
-      p.C = l->hi[hp]; p.C2 = (keep_E0 && hp == 0) ? l->E0 : nullptr;
+      p.mul = nb.act3[passes[i].set]; p.mul_div = l->n_head[hp];
+      p.C = nb.hi[hp]; p.C2 = (keep_E0 && hp == 0) ? l->E0 : nullptr;
       gb.p[i] = p;
     }
     DZ_TRY(run_nn("iqn_embed_fwd", gb, false, stream));
@@ -1807,14 +1831,14 @@ int forward_heads_iqn(dz_learner* l, const Pass* passes, int np, int nimg, const
   for (int i = 0; i < np; ++i) {
     int hp = passes[i].head;
     GemmProblem p = zero_problem();
-    p.a_mode = A_PLAIN; p.A = l->hi[hp]; p.lda = d.feat; p.M = nimg * l->n_head[hp]; p.K = d.feat;
+    p.a_mode = A_PLAIN; p.A = nb.hi[hp]; p.lda = d.feat; p.M = nimg * l->n_head[hp]; p.K = d.feat;
     p.B = passes[i].params + o.w1[0]; p.N = 512; p.ldb = 512; p.ldc = 512;
-    p.bias = passes[i].params + o.b1[0]; p.relu = 1; p.C = l->h1[hp][0];
+    p.bias = passes[i].params + o.b1[0]; p.relu = 1; p.C = nb.h1[hp][0];
     gb.p[i] = p;
   }
   // M can be small when acting (1 x tau_samples_policy rows): same kernel family handles it
   if (packed) {
-    DZ_TRY(iqn_embed_fc1_forward_packed(l, passes, gb, keep_E0, stream));
+    DZ_TRY(iqn_embed_fc1_forward_packed(l, nb, passes, gb, keep_E0, stream));
   } else {
     DZ_TRY(run_nn("iqn_fc1_fwd", gb, false, stream));
   }
@@ -1825,8 +1849,8 @@ int forward_heads_iqn(dz_learner* l, const Pass* passes, int np, int nimg, const
     int maxM = 0;
     for (int i = 0; i < np; ++i) {
       int hp = passes[i].head;
-      h.A[i] = l->h1[hp][0]; h.W[i] = passes[i].params + o.w2[0]; h.bias[i] = passes[i].params + o.b2[0];
-      h.out[i] = l->out[hp]; h.M[i] = nimg * l->n_head[hp];
+      h.A[i] = nb.h1[hp][0]; h.W[i] = passes[i].params + o.w2[0]; h.bias[i] = passes[i].params + o.b2[0];
+      h.out[i] = nb.out[hp]; h.M[i] = nimg * l->n_head[hp];
       maxM = std::max(maxM, h.M[i]);
     }
     dim3 grid((unsigned)std::min<int64_t>(ceil_div(maxM, 8), kNumSMs * 2), (unsigned)np);
@@ -1836,9 +1860,9 @@ int forward_heads_iqn(dz_learner* l, const Pass* passes, int np, int nimg, const
   for (int i = 0; i < np; ++i) {
     int hp = passes[i].head;
     GemmProblem p = zero_problem();
-    p.a_mode = A_PLAIN; p.A = l->h1[hp][0]; p.lda = 512; p.M = nimg * l->n_head[hp]; p.K = 512;
+    p.a_mode = A_PLAIN; p.A = nb.h1[hp][0]; p.lda = 512; p.M = nimg * l->n_head[hp]; p.K = 512;
     p.B = passes[i].params + o.w2[0]; p.N = d.out; p.ldb = d.out; p.ldc = d.out;
-    p.bias = passes[i].params + o.b2[0]; p.C = l->out[hp];
+    p.bias = passes[i].params + o.b2[0]; p.C = nb.out[hp];
     gb.p[i] = p;
   }
   DZ_TRY(run_nn("iqn_head_fwd", gb, false, stream));
@@ -2295,7 +2319,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     DZ_TRY(l->side.join(stream));
     if (c.kind != DZ_IQN) DZ_TRY(um_forward_fc(l->um, batch->d_noise, stream));
   } else {
-    DZ_TRY(forward_torso(l, jobs, nj, B, stream));
+    DZ_TRY(forward_torso(l, learner_bufs(l), jobs, nj, B, stream));
   }
 
   if (c.kind == DZ_IQN) {
@@ -2305,17 +2329,17 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     const float* t1 = t0 + (long long)B * c.tau_samples_s_tm1;
     const float* t2 = t1 + (long long)B * c.tau_samples_policy;
     const float* taus[3] = {t0, t1, t2};
-    DZ_TRY(forward_heads_iqn(l, passes, 3, B, taus, true, stream));
+    DZ_TRY(forward_heads_iqn(l, learner_bufs(l), passes, 3, B, taus, true, stream));
   } else if (c.kind == DZ_RAINBOW) {
     Pass passes[3] = {{on, 0, 0, 0}, {on, 1, 1, 1}, {tg, 2, 2, 2}};
-    DZ_TRY(forward_heads_rainbow(l, passes, 3, B, batch->d_noise, stream, um));
+    DZ_TRY(forward_heads_rainbow(l, learner_bufs(l), passes, 3, B, batch->d_noise, stream, um));
   } else {
     Pass passes[3];
     int np = 0;
     passes[np++] = Pass{on, 0, 0, 0};
     if (needs_online_st) passes[np++] = Pass{on, 1, 1, 0};
     passes[np++] = Pass{tg, 2, 2, 0};
-    DZ_TRY(forward_heads_plain(l, passes, np, B, stream, um));
+    DZ_TRY(forward_heads_plain(l, learner_bufs(l), passes, np, B, stream, um));
   }
 
   // ---- loss + gradient wrt the pass-0 head outputs
@@ -2549,19 +2573,19 @@ int dz_learner_q_values(dz_learner* l, const uint8_t* d_obs, const float* d_taus
   DZ_TRY(l->side.join(stream));   // pending side-stream work (asynchronous randomness)
   DZ_LAUNCH(make_row_table_kernel, 1, 32, 0, stream, d_obs, (long long)0, 1, l->rows_act);
   TorsoJob job{on, l->rows_act, 1};   // use activation set 1 so a pending backward's set-0 buffers stay intact
-  DZ_TRY(forward_torso(l, &job, 1, 1, stream));
+  DZ_TRY(forward_torso(l, learner_bufs(l), &job, 1, 1, stream));
   Pass pass{on, 1, 1, 0};
   int nq = 1;
   if (c.kind == DZ_IQN) {
     if (!d_taus) return fail(DZ_EINVAL, "iqn q_values needs taus[tau_samples_policy]");
     const float* taus[1] = {d_taus};
-    DZ_TRY(forward_heads_iqn(l, &pass, 1, 1, taus, false, stream));
+    DZ_TRY(forward_heads_iqn(l, learner_bufs(l), &pass, 1, 1, taus, false, stream));
     nq = c.tau_samples_policy;
   } else if (c.kind == DZ_RAINBOW) {
     if (!d_noise) return fail(DZ_EINVAL, "rainbow q_values needs one apply of noise");
-    DZ_TRY(forward_heads_rainbow(l, &pass, 1, 1, d_noise, stream));
+    DZ_TRY(forward_heads_rainbow(l, learner_bufs(l), &pass, 1, 1, d_noise, stream));
   } else {
-    DZ_TRY(forward_heads_plain(l, &pass, 1, 1, stream));
+    DZ_TRY(forward_heads_plain(l, learner_bufs(l), &pass, 1, 1, stream));
     nq = c.num_quantiles;
   }
   size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
@@ -2586,19 +2610,19 @@ int act_batch_impl(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* 
   const long long obs_bytes = (long long)l->d.H * l->d.W * l->d.C;
   DZ_LAUNCH(make_row_table_kernel, (unsigned)ceil_div(E, 64), 64, 0, stream, d_obs, obs_bytes, (int)E, l->rows_act);
   TorsoJob job{on, l->rows_act, 1};
-  DZ_TRY(forward_torso(l, &job, 1, E, stream));
+  DZ_TRY(forward_torso(l, learner_bufs(l), &job, 1, E, stream));
   Pass pass{on, 1, 1, 0};
   int nq = 1;
   if (c.kind == DZ_IQN) {
     if (!d_taus) return fail(DZ_EINVAL, "iqn act_batch needs taus[E][tau_samples_policy]");
     const float* taus[1] = {d_taus};
-    DZ_TRY(forward_heads_iqn(l, &pass, 1, E, taus, false, stream));
+    DZ_TRY(forward_heads_iqn(l, learner_bufs(l), &pass, 1, E, taus, false, stream));
     nq = c.tau_samples_policy;
   } else if (c.kind == DZ_RAINBOW) {
     if (!d_noise) return fail(DZ_EINVAL, "rainbow act_batch needs one apply of noise");
-    DZ_TRY(forward_heads_rainbow(l, &pass, 1, E, d_noise, stream, false, noise_ld));
+    DZ_TRY(forward_heads_rainbow(l, learner_bufs(l), &pass, 1, E, d_noise, stream, false, noise_ld));
   } else {
-    DZ_TRY(forward_heads_plain(l, &pass, 1, E, stream));
+    DZ_TRY(forward_heads_plain(l, learner_bufs(l), &pass, 1, E, stream));
     nq = c.num_quantiles;
   }
   size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
@@ -2642,6 +2666,207 @@ int dz_learner_generate_stream_noise(dz_learner* l, uint64_t seed, int32_t E, fl
   const long long n = (long long)E * noise_layout(l->cfg, l->d).stride;
   DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_noise, n, seed, l->buf.d_counters, 1, 2u);
   DZ_LAUNCH(bump_counter_kernel, 1, 1, 0, stream, l->buf.d_counters, 1);
+  return DZ_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Acting context: batched acting for up to kActorMaxStreams streams over the learner's online parameters, read in
+// place (an act enqueued after a learner step on the same stream sees that step's parameters).  Its buffers are sized
+// for its stream count; the torso and the 3136 -> 512 layer run on a forward-only tensor-core plan where the geometry
+// allows it.
+// ------------------------------------------------------------------------------------------------
+
+struct dz_actor {
+  dz_learner* l;
+  int E;                       // streams
+  NetBufs b;                   // activation set / head pass 1, as the learner's act_batch
+  const uint8_t** rows;        // [E] observation row table
+  float* noise;                // rainbow: the apply the tensor-core noisy1 reads (a copy of the caller's shared apply)
+  UmNet* um;                   // forward-only tensor-core plan (nullptr: fp32-FMA torso)
+  char* um_ws;
+};
+
+namespace {
+
+constexpr int kActorMaxStreams = 1024, kActorMaxIqnRows = 16384;
+
+int actor_check(const dz_learner_config& c, int E) {
+  if (E < 1 || E > kActorMaxStreams) return fail(DZ_EINVAL, "actor: num_streams must be in [1, 1024]");
+  if (c.kind == DZ_IQN && (int64_t)E * c.tau_samples_policy > kActorMaxIqnRows)
+    return fail(DZ_EINVAL, "actor: num_streams * tau_samples_policy must be <= 16384");
+  return DZ_OK;
+}
+
+UmNetDesc actor_um_desc(const dz_learner* l, int E) {
+  UmNetDesc u = make_um_desc(l);
+  u.B = E; u.npass = 1; u.fwd_only = 1;
+  u.pass_target[0] = 0; u.target = nullptr;
+  for (int p = 0; p < 3; ++p) u.noise_apply[p] = 0;
+  return u;
+}
+
+// Carves the actor's buffers (sizes only when base is NULL); the tensor-core plan's own buffers come from um_ws.
+int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
+  const dz_learner_config& c = l->cfg;
+  const Dims& d = l->d;
+  const int E = a->E;
+  const bool rb = c.kind == DZ_RAINBOW, iqn = c.kind == DZ_IQN;
+  Bump w{base};
+  NetBufs& b = a->b;
+  memset(&b, 0, sizeof(b));   // split_rows 0: the fp32 GEMMs never split K, so row e's sums do not depend on E
+  const UmNetDesc ud = actor_um_desc(l, E);
+  const bool um = um_net_supported(ud);
+  a->um_ws = um ? w.take<char>(um_net_workspace_bytes(ud)) : nullptr;
+  if (!um) {
+    b.act1[1] = w.take<float>((int64_t)E * d.h1 * d.w1 * 32);
+    b.act2[1] = w.take<float>((int64_t)E * d.h2 * d.w2 * 64);
+    b.act3[1] = w.take<float>((int64_t)E * d.feat);
+    b.conv_partial = w.take<float>((int64_t)l->conv_splits * E * d.h2 * d.w2 * 64);
+  }
+  const int64_t rows = (int64_t)E * (iqn ? c.tau_samples_policy : 1);
+  if (!um || iqn) {                      // otherwise h1 is the tensor-core plan's
+    b.h1[1][0] = w.take<float>(rows * 512);
+    b.h1[1][1] = rb ? w.take<float>(rows * 512) : nullptr;
+  }
+  b.out[1] = w.take<float>(rows * d.out);
+  b.outv[1] = rb ? w.take<float>((int64_t)E * c.num_atoms) : nullptr;
+  b.cosf[1] = iqn ? w.take<float>(rows * c.latent_dim) : nullptr;
+  b.hi[1] = iqn ? w.take<float>(rows * d.feat) : nullptr;
+  a->rows = w.take<const uint8_t*>(E);
+  a->noise = rb ? w.take<float>(noise_layout(c, d).stride) : nullptr;
+  return w.used;
+}
+
+}  // namespace
+
+int dz_actor_plan_query(const dz_learner_config* cfg, int32_t num_streams, int64_t* workspace_bytes) {
+  if (!cfg || !workspace_bytes) return fail(DZ_EINVAL, "actor plan query: null argument");
+  DZ_TRY(validate(*cfg));
+  DZ_TRY(actor_check(*cfg, num_streams));
+  dz_learner tmp;
+  tmp.um = nullptr;
+  memset(&tmp.buf, 0, sizeof(tmp.buf));
+  tmp.cfg = *cfg;
+  tmp.lay = make_layout(*cfg);
+  DZ_TRY(param_offsets(*cfg, tmp.lay, &tmp.po));
+  tmp.d = make_dims(*cfg);
+  tmp.B = cfg->batch;
+  carve(&tmp, nullptr);                  // the learner's split counts, which the actor's fp32 GEMMs share
+  dz_actor a;
+  a.E = num_streams;
+  *workspace_bytes = carve_actor(&a, &tmp, nullptr);
+  return DZ_OK;
+}
+
+int dz_actor_create(dz_learner* l, int32_t num_streams, void* d_workspace, dz_actor** out) {
+  if (!l || !d_workspace || !out) return fail(DZ_EINVAL, "actor create: null argument");
+  DZ_TRY(actor_check(l->cfg, num_streams));
+  dz_actor* a = new dz_actor();
+  a->l = l;
+  a->E = num_streams;
+  carve_actor(a, l, static_cast<char*>(d_workspace));
+  if (a->um_ws) {
+    int rc = um_net_create(actor_um_desc(l, num_streams), a->um_ws, &a->um);
+    if (rc == DZ_OK && a->noise) rc = um_bind_noise(a->um, a->noise);
+    if (rc != DZ_OK) { dz_actor_destroy(a); return rc; }
+    for (int L = 1; L <= 3; ++L) (L == 1 ? a->b.act1 : L == 2 ? a->b.act2 : a->b.act3)[1] = um_act_f32(a->um, L, 0);
+    if (l->cfg.kind != DZ_IQN)
+      for (int s = 0; s < (l->cfg.kind == DZ_RAINBOW ? 2 : 1); ++s) a->b.h1[1][s] = um_h1_f32(a->um, 0, s);
+  }
+  *out = a;
+  return DZ_OK;
+}
+
+void dz_actor_destroy(dz_actor* a) {
+  if (!a) return;
+  um_net_destroy(a->um);
+  delete a;
+}
+
+// dz_learner_act_batch's contract for the actor's num_streams observations.  noise_ld (rainbow): 0, d_noise is one
+// apply shared by every stream (noisy1 on the tensor cores when the torso is); the noise stride, d_noise is [E][stride]
+// and stream e uses apply e (noisy layers on the per-row fp32 kernels).
+int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const float* d_noise, int64_t noise_ld,
+                 const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
+  if (!a) return fail(DZ_EINVAL, "actor: null handle");
+  dz_learner* l = a->l;
+  const dz_learner_config& c = l->cfg;
+  const int E = a->E;
+  const bool rb = c.kind == DZ_RAINBOW;
+  if (!d_obs || !d_q_out || !d_actions) return fail(DZ_EINVAL, "actor: null buffer");
+  if (c.kind == DZ_IQN && !d_taus) return fail(DZ_EINVAL, "iqn actor needs taus[E][tau_samples_policy]");
+  if (rb && !d_noise) return fail(DZ_EINVAL, "rainbow actor needs noise");
+  const int64_t stride = rb ? noise_layout(c, l->d).stride : 0;
+  if (noise_ld != 0 && (!rb || noise_ld != stride))
+    return fail(DZ_EINVAL, "actor: noise_ld must be 0 (one shared apply) or the noise stride (rainbow, one apply per stream)");
+  const float* on = l->buf.d_online;
+  const long long obs_bytes = (long long)l->d.H * l->d.W * l->d.C;
+  DZ_LAUNCH(make_row_table_kernel, (unsigned)ceil_div(E, 64), 64, 0, stream, d_obs, obs_bytes, E, a->rows);
+  const bool fc_done = a->um && c.kind != DZ_IQN && noise_ld == 0;
+  if (a->um) {
+    const uint8_t* const* rows[3] = {a->rows, nullptr, nullptr};
+    DZ_TRY(um_pack_weights(a->um, stream));
+    DZ_TRY(um_forward_torso(a->um, rows, stream));
+    if (fc_done) {
+      if (rb) DZ_CUDA_OK(cudaMemcpyAsync(a->noise, d_noise, stride * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+      DZ_TRY(um_forward_fc(a->um, a->noise, stream));
+    }
+  } else {
+    TorsoJob job{on, a->rows, 1};
+    DZ_TRY(forward_torso(l, a->b, &job, 1, E, stream));
+  }
+  Pass pass{on, 1, 1, 0};
+  int nq = 1;
+  if (c.kind == DZ_IQN) {
+    const float* taus[1] = {d_taus};
+    DZ_TRY(forward_heads_iqn(l, a->b, &pass, 1, E, taus, false, stream));
+    nq = c.tau_samples_policy;
+  } else if (rb) {
+    DZ_TRY(forward_heads_rainbow(l, a->b, &pass, 1, E, d_noise, stream, fc_done, noise_ld));
+  } else {
+    DZ_TRY(forward_heads_plain(l, a->b, &pass, 1, E, stream, fc_done));
+    nq = c.num_quantiles;
+  }
+  size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
+  DZ_LAUNCH(q_values_kernel, (unsigned)E, 128, smem, stream, c.kind, c.num_actions, c.num_atoms, nq, c.vmax, a->b.out[1], a->b.out[1],
+            a->b.outv[1], d_q_out);
+  DZ_LAUNCH(act_select_kernel, (unsigned)ceil_div(E, 128), 128, 0, stream, (const float*)d_q_out, c.num_actions, E, d_explore, epsilon,
+            d_actions);
+  return DZ_OK;
+}
+
+// The actor's randomness from the learner's generator and counter: iqn taus [E][tau_samples_policy] (the stream id of
+// dz_learner_generate_randomness's taus); rainbow one noise apply, or E applies when per_stream is set (the stream id of
+// its noise and of dz_learner_generate_stream_noise).  Advances d_counters[1] once.
+int dz_actor_generate_randomness(dz_actor* a, uint64_t seed, int32_t per_stream, float* d_out, void* stream) {
+  if (!a || !d_out) return fail(DZ_EINVAL, "actor randomness: null argument");
+  const dz_learner_config& c = a->l->cfg;
+  long long n;
+  if (c.kind == DZ_IQN && !per_stream) n = (long long)a->E * c.tau_samples_policy;
+  else if (c.kind == DZ_RAINBOW) n = (per_stream ? (long long)a->E : 1LL) * noise_layout(c, a->l->d).stride;
+  else return fail(DZ_EINVAL, "actor randomness: iqn draws taus, rainbow noise (per_stream: rainbow only); other kinds draw nothing");
+  const int kind = c.kind == DZ_IQN ? 0 : 1;
+  DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_out, n, seed, a->l->buf.d_counters, kind,
+            c.kind == DZ_IQN ? 1u : 2u);
+  DZ_LAUNCH(bump_counter_kernel, 1, 1, 0, stream, a->l->buf.d_counters, 1);
+  return DZ_OK;
+}
+
+// Test hook: the MMA path of the actor's tensor-core launch `tag` (the tags of dz_test_learner_mma_path's torso and fc
+// launches).  DZ_EINVAL when the actor runs on the fp32-FMA kernels or has no such launch.
+int dz_test_actor_mma_path(dz_actor* a, const char* tag, int32_t* path) {
+  if (!a->um) return fail(DZ_EINVAL, "the actor runs on the fp32-FMA kernels (geometry outside the tensor-core path)");
+  const int p = um_net_mma_path(a->um, tag);
+  if (p < 0) return fail(DZ_EINVAL, "no tensor-core launch '%s' in this actor", tag ? tag : "");
+  *path = p;
+  return DZ_OK;
+}
+
+// Test hook: device pointer + element count of the actor's conv3 output "act3" ([E][feat], written by the last act).
+int dz_test_actor_buffer(dz_actor* a, const char* name, float** d_ptr, int64_t* count) {
+  if (std::string(name ? name : "") != "act3") return fail(DZ_EINVAL, "unknown actor buffer '%s'", name ? name : "");
+  *d_ptr = a->b.act3[1];
+  *count = (int64_t)a->E * a->l->d.feat;
   return DZ_OK;
 }
 

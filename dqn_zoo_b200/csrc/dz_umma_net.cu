@@ -827,7 +827,7 @@ size_t conv1_smem_bytes(int resident, int stag_bytes) { return 2048 + (size_t)re
 }  // namespace
 
 bool um_net_supported(const UmNetDesc& d) {
-  if (d.B < 1 || d.B > 64 || d.npass < 1 || d.npass > 3) return false;
+  if (d.fwd_only ? (d.B < 1 || d.npass != 1) : (d.B < 1 || d.B > 64 || d.npass < 1 || d.npass > 3)) return false;
   if (d.W % 4 || d.H < 36 || d.W < 36) return false;
   const int h1 = conv_out(d.H, 8, 4), w1 = conv_out(d.W, 8, 4);
   if ((h1 & 1) || (w1 & 1)) return false;              // stride-2 parity view of act1
@@ -864,6 +864,9 @@ struct Carver {
 
 int fc_splits_for(int nprob, int nk) { return std::max(1, std::min(std::min(kNumSMs / (nprob * 4), 24), nk)); }
 
+// Forward-only plans: rows of the fc x operand per problem (one NJT 64 tile).
+constexpr int kFwdFcRows = 64;
+
 int64_t carve_net(UmNet* n, char* base) {
   const UmNetDesc& d = n->d;
   const Geo g = geo_of(d);
@@ -872,6 +875,17 @@ int64_t carve_net(UmNet* n, char* base) {
   const int64_t a1 = (int64_t)g.PB * g.h1 * g.w1 * 32, a2 = (int64_t)g.PB * g.h2 * g.w2 * 64, a3 = (int64_t)g.PB * g.feat;
   const int64_t sz[3] = {a1, a2, a3};
   for (int L = 0; L < 3; ++L) { n->act_hi[L] = c.f(sz[L]); n->act_lo[L] = c.f(sz[L]); n->act_f32[L] = c.f(sz[L]); }
+  if (d.fwd_only) {
+    for (int L = 0; L < 3; ++L) { n->wf_hi[0][L] = c.f(kConvN[L] * kConvK[L]); n->wf_lo[0][L] = c.f(kConvN[L] * kConvK[L]); }
+    n->fc_nprob = n->fcd_nsrc = 0; n->fc_splits = n->fcd_splits = 1;
+    if (d.use_fc) {
+      n->fc_nprob = d.nstream;
+      n->fc_splits = fc_splits_for(d.nstream, g.feat / 32);   // as for one 64-row chunk, whatever B is
+      n->h1_buf = c.f((int64_t)d.nstream * d.B * 512);
+      n->fc_part = c.f((int64_t)d.nstream * n->fc_splits * d.B * 512);
+    }
+    return c.used;
+  }
   const int64_t dz_[3] = {(int64_t)d.B * g.h1 * g.w1 * 32, (int64_t)d.B * g.h2 * g.w2 * 64, (int64_t)d.B * g.feat};
   for (int L = 0; L < 3; ++L) { n->dact_hi[L] = c.f(dz_[L]); n->dact_lo[L] = c.f(dz_[L]); n->dact_f32[L] = c.f(dz_[L]); }
   for (int b = 0; b < 2; ++b)
@@ -928,14 +942,15 @@ int build_plan(UmNet* n) {
 
   // ---- weight image maps: [blob][layer][part]; box rows = N tile used by the layer
   int m_wf[2][3][2];
+  const int nblob = d.fwd_only ? 1 : 2;
   const uint32_t wf_rows[3] = {32, 64, 32};   // conv1: N 32; conv2: full 64; conv3: halves of 32
-  for (int b = 0; b < 2; ++b)
+  for (int b = 0; b < nblob; ++b)
     for (int L = 0; L < 3; ++L) {
       uint64_t dims[2] = {(uint64_t)kConvK[L], (uint64_t)kConvN[L]}, strides[1] = {(uint64_t)kConvK[L] * 4};
       uint32_t box[2] = {32, wf_rows[L]};
       DZ_TRY(pl.add_map_pair(n->wf_hi[b][L], n->wf_lo[b][L], 2, dims, strides, box, m_wf[b][L]));
     }
-  for (int b = 0; b < 2; ++b) { n->map_wf1[b][0] = m_wf[b][0][0]; n->map_wf1[b][1] = m_wf[b][0][1]; }
+  for (int b = 0; b < 2; ++b) { n->map_wf1[b][0] = m_wf[b % nblob][0][0]; n->map_wf1[b][1] = m_wf[b % nblob][0][1]; }
 
   // =========================================================================== conv2 forward
   {
@@ -973,7 +988,9 @@ int build_plan(UmNet* n) {
 
   // =========================================================================== conv3 forward (two 32-channel halves)
   {
-    const int G = (B % 2 == 0 && 2 * h3 * w3 <= 128) ? 2 : 1;
+    // Image pairs per CTA.  A forward-only plan pairs odd B too: its last CTA's second image lies beyond the single
+    // pass's B images, where the TMA unit reads zeros, and stores only its first image's rows.
+    const int G = ((B % 2 == 0 || d.fwd_only) && 2 * h3 * w3 <= 128) ? 2 : 1;
     int m_a[2];
     uint64_t dims[4] = {64, (uint64_t)w2, (uint64_t)h2, (uint64_t)PB};
     uint64_t strides[3] = {256, (uint64_t)w2 * 256, (uint64_t)h2 * w2 * 256};
@@ -992,10 +1009,10 @@ int build_plan(UmNet* n) {
         pr.out_ld = 64;
         pr.bias = (blob ? d.target : d.online) + d.off_conv_b[2] + 32 * half; pr.relu = 1;
         const int prob = pl.add_problem(pr);
-        for (int t = 0; t < B / G; ++t) {
+        for (int t = 0; t < (B + G - 1) / G; ++t) {
           const int img = p * B + t * G;
           UmCta& c = pl.begin_cta(prob);
-          c.row_base = img * h3 * w3; c.ph_valid = 1; c.pw_valid = rows;
+          c.row_base = img * h3 * w3; c.ph_valid = 1; c.pw_valid = std::min(G, B - t * G) * h3 * w3;
           for (int kh = 0; kh < 3; ++kh)
             for (int kw = 0; kw < 3; ++kw)
               for (int ch = 0; ch < 2; ++ch) {
@@ -1012,7 +1029,7 @@ int build_plan(UmNet* n) {
 
   // =========================================================================== conv3 input gradient
   // dact2[b,y,x,c] = [act2 > 0] * sum_{kh,kw,n} dact3[b, y-kh, x-kw, n] * W3[kh,kw,c,n]; halo zero-filled by the TMA unit
-  {
+  if (!d.fwd_only) {
     const int nb = 2;                                     // row bands per image
     const int hb = (h2 + nb - 1) / nb;
     int m_a[2], m_w[2];
@@ -1058,7 +1075,7 @@ int build_plan(UmNet* n) {
 
   // =========================================================================== conv2 input gradient (4 parity classes)
   // dact1[b, 2i+py, 2j+px, c] = [act1 > 0] * sum_{ay,ax,n} dact2[b, i-ay, j-ax, n] * W2[py+2ay, px+2ax, c, n]
-  {
+  if (!d.fwd_only) {
     int m_a[2], m_w[2];
     for (int part = 0; part < 2; ++part) {
       uint64_t dims[4] = {64, (uint64_t)w2, (uint64_t)h2, (uint64_t)B};
@@ -1097,7 +1114,7 @@ int build_plan(UmNet* n) {
     pl.end_launch(l);
   }
 
-  {   // conv1 weight gradient: G operand
+  if (!d.fwd_only) {   // conv1 weight gradient: G operand
     uint64_t dims[2] = {32, (uint64_t)B * h1 * w1}, strides[1] = {128};
     uint32_t box[2] = {32, 128};
     DZ_TRY(pl.add_map_pair(n->dact_hi[0], n->dact_lo[0], 2, dims, strides, box, n->map_g1));
@@ -1105,7 +1122,7 @@ int build_plan(UmNet* n) {
   // =========================================================================== conv3 / conv2 weight gradients
   // dW[k][n] = sum_m A[m][k] G[m][n]: both operands are read through MN-major (transposing) descriptors straight from the
   // NHWC tensors — the same im2col boxes as the forward pass, with the reduction running over (output row, 8 images).
-  {
+  if (!d.fwd_only) {
     const int groups = (B + 7) / 8;
     // ---- conv3: A = act2 patches (pass 0), G = dact3
     {
@@ -1200,36 +1217,47 @@ int build_plan(UmNet* n) {
 
   // =========================================================================== fc1 / noisy1 forward and input gradient
   if (d.use_fc) {
-    const int njt = B <= 32 ? 32 : 64;
+    const int njt = d.fwd_only || B > 32 ? 64 : 32;
     const int q = d.noisy ? 2 : 1;
-    int m_x[2], m_g[2];
+    int m_x[2], m_g[2] = {0, 0};
     for (int part = 0; part < 2; ++part) {
       uint64_t dims[2] = {(uint64_t)feat, (uint64_t)PB}, strides[1] = {(uint64_t)feat * 4};
       uint32_t box[2] = {32, (uint32_t)njt};
       m_x[part] = pl.add_map(part ? n->act_lo[2] : n->act_hi[2], 2, dims, strides, box);
-      uint64_t gd[2] = {512, (uint64_t)d.nstream * B}, gs[1] = {2048};
-      m_g[part] = pl.add_map(part ? n->dh1_lo : n->dh1_hi, 2, gd, gs, box);
+      if (!d.fwd_only) {
+        uint64_t gd[2] = {512, (uint64_t)d.nstream * B}, gs[1] = {2048};
+        m_g[part] = pl.add_map(part ? n->dh1_lo : n->dh1_hi, 2, gd, gs, box);
+      }
       if (m_x[part] < 0 || m_g[part] < 0) return DZ_EINVAL;
     }
     // Forward CTA groups: the passes that apply the same parameter blob share every staged weight tile (online net on
     // s_tm1 and s_t), each group's tiles then span 128 / (passes in the group) weight columns, so a CTA does the same
     // MMA work whether it serves one pass or two.  fc_per_pass (tests only): one group per pass, 128-column tiles.
-    int grp[3][kFcMaxProbs], ngrp = 0, grp_n[3] = {0, 0, 0}, grp_blob[3] = {0, 0, 0};
-    for (int p = 0; p < d.npass; ++p) {
-      const int blob = d.pass_target[p] ? 1 : 0;
-      int gi = -1;
-      if (!n->fc_per_pass)
-        for (int k = 0; k < ngrp; ++k) if (grp_blob[k] == blob) gi = k;
-      if (gi < 0) { gi = ngrp++; grp_blob[gi] = blob; }
-      if (grp_n[gi] == kFcMaxProbs) return fail(DZ_EINVAL, "fc forward: more than two passes apply one parameter blob");
-      grp[gi][grp_n[gi]++] = p;
+    // A group member is the x rows [row0, row0 + rows) of one pass: all B of them, or in a forward-only plan one
+    // chunk of at most kFwdFcRows, each chunk a group of its own (the same CTAs and reduction order for every row).
+    struct FcMember { int pass, row0, rows; };
+    std::vector<std::vector<FcMember>> grp;
+    std::vector<int> grp_blob;
+    if (d.fwd_only) {
+      for (int r0 = 0; r0 < B; r0 += kFwdFcRows) { grp.push_back({{0, r0, std::min(kFwdFcRows, B - r0)}}); grp_blob.push_back(0); }
+    } else {
+      for (int p = 0; p < d.npass; ++p) {
+        const int blob = d.pass_target[p] ? 1 : 0;
+        int gi = -1;
+        if (!n->fc_per_pass)
+          for (int k = 0; k < (int)grp.size(); ++k) if (grp_blob[k] == blob) gi = k;
+        if (gi < 0) { gi = (int)grp.size(); grp.emplace_back(); grp_blob.push_back(blob); }
+        if ((int)grp[gi].size() == kFcMaxProbs) return fail(DZ_EINVAL, "fc forward: more than two passes apply one parameter blob");
+        grp[gi].push_back({p, p * B, B});
+      }
     }
+    const int ngrp = (int)grp.size();
     int fc_rows[2] = {128, 128};   // forward tile columns per blob
-    for (int k = 0; k < ngrp; ++k) fc_rows[grp_blob[k]] = 128 / grp_n[k];
+    for (int k = 0; k < ngrp; ++k) fc_rows[grp_blob[k]] = 128 / (int)grp[k].size();
     // weight maps: [blob][stream][sigma] x {forward box (32 n, 32 k) x fc_rows / 32, gradient box (32 n, 128 k)}
     int m_wf_fc[2][2][2], m_wd_fc[2][2];
     bool wf3d = true;
-    for (int blob = 0; blob < 2; ++blob)
+    for (int blob = 0; blob < nblob; ++blob)
       for (int s = 0; s < d.nstream; ++s)
         for (int sg = 0; sg < q; ++sg) {
           const float* w = (blob ? d.target : d.online) + (sg ? d.off_fc_sw[s] : d.off_fc_w[s]);
@@ -1248,7 +1276,7 @@ int build_plan(UmNet* n) {
             m_wf_fc[blob][s][sg] = pl.add_map(w, 2, dims, strides, box2);
           }
           if (m_wf_fc[blob][s][sg] < 0) return DZ_EINVAL;
-          if (blob == 0) {
+          if (blob == 0 && !d.fwd_only) {
             uint32_t boxd[2] = {32, 128};
             m_wd_fc[s][sg] = pl.add_map(w, 2, dims, strides, boxd);
             if (m_wd_fc[s][sg] < 0) return DZ_EINVAL;
@@ -1260,20 +1288,25 @@ int build_plan(UmNet* n) {
       const UmOperand Bo = um_kmajor(njt, true, false);
       const int nk = feat / 32, S = n->fc_splits, per = (nk + S - 1) / S;
       uint32_t stage_bytes = 2 * 16384 + 2 * Bo.part_bytes;
-      for (int k = 0; k < ngrp; ++k) stage_bytes = std::max<uint32_t>(stage_bytes, 2 * 16384 / grp_n[k] + grp_n[k] * 2 * Bo.part_bytes);
+      for (int k = 0; k < ngrp; ++k) {
+        const int np = (int)grp[k].size();
+        stage_bytes = std::max<uint32_t>(stage_bytes, 2 * 16384 / np + np * 2 * Bo.part_bytes);
+      }
       UmLaunch& l = n->launches[kFcFwd];
       pl.begin_launch(l, njt, stage_bytes);
       for (int k = 0; k < ngrp; ++k) {
-        const int blob = grp_blob[k], np = grp_n[k], rows = fc_rows[blob], slabs = rows / 32;
+        const int blob = grp_blob[k], np = (int)grp[k].size(), rows = fc_rows[blob], slabs = rows / 32;
         const UmOperand A = um_mnmajor(rows, 32, true, nullptr);
         const uint32_t a_bytes = 2 * A.part_bytes;
         for (int s = 0; s < d.nstream; ++s) {
           const int prob0 = (int)pl.probs.size();
           for (int gp = 0; gp < np; ++gp) {
-            const int p = grp[k][gp], qi = p * d.nstream + s;
-            UmProblem pr = make_problem(A, Bo, 4, 32, UM_EPI_PARTIAL, 512, B);
+            const FcMember& m = grp[k][gp];
+            const int p = m.pass, qi = p * d.nstream + s;
+            UmProblem pr = make_problem(A, Bo, 4, 32, UM_EPI_PARTIAL, 512, m.rows);
             if (d.noisy) pr.A.convert = 2;
-            pr.C = n->fc_part + (int64_t)qi * S * B * 512; pr.sc_i = 1; pr.sc_j = 512; pr.split_stride = (long long)B * 512;
+            pr.C = n->fc_part + (int64_t)qi * S * B * 512 + (int64_t)(m.row0 - p * B) * 512;
+            pr.sc_i = 1; pr.sc_j = 512; pr.split_stride = (long long)B * 512;
             const int prob = pl.add_problem(pr);
             if (d.noisy) {
               n->patches.push_back({prob, 0, (int64_t)d.noise_apply[p] * d.noise_stride + d.noise_off_in[s]});
@@ -1293,7 +1326,7 @@ int build_plan(UmNet* n) {
                   if (wf3d) pl.op(m_wf_fc[blob][s][sg], sg * A.part_bytes, 0, 32 * ks, nt * slabs);
                   else for (int sl = 0; sl < slabs; ++sl) pl.op(m_wf_fc[blob][s][sg], sg * A.part_bytes + sl * 4096, nt * rows + 32 * sl, 32 * ks);
                 }
-                for (int gp = 0; gp < np; ++gp) pl.op_pair(m_x, a_bytes + gp * 2 * Bo.part_bytes, Bo.part_bytes, 32 * ks, grp[k][gp] * B);
+                for (int gp = 0; gp < np; ++gp) pl.op_pair(m_x, a_bytes + gp * 2 * Bo.part_bytes, Bo.part_bytes, 32 * ks, grp[k][gp].row0);
               }
               DZ_TRY(pl.end_cta());
             }
@@ -1303,7 +1336,7 @@ int build_plan(UmNet* n) {
     }
     // ---- input gradient: D[k, m] = sum_n W[k][n] g[m][n];  noisy: W = Wmu + Wsigma * (eps_in[k] * eps_out[n]), formed in the
     // MMA warps (umma_fc_kernel on the K-major tile; with UM_PATH_CONVERTERS by the converter warps of umma_gemm_kernel)
-    {
+    if (!d.fwd_only) {
       const UmOperand Bo = um_kmajor(njt, true, false);
       const int S = n->fcd_splits, per = (16 + S - 1) / S, ktiles = (feat + 127) / 128;
       UmLaunch& l = n->launches[kFcDgrad];
@@ -1370,9 +1403,9 @@ int net_create(const UmNetDesc& d, char* base, UmNet** out, bool fc_per_pass) {
   carve_net(n, base);
   n->conv1_tiles_per_pass = (d.B * n->h1 * n->w1 + 127) / 128;
   n->conv1_stag_bytes = conv1_stag_bytes(d.B, d.W, n->h1, n->w1);
-  cudaMemset(n->wg_ticket, 0, 64 * 4);
   // gradient buffers start as zeros (hi/lo pairs of layers whose producer has not run yet are never NaN)
-  for (int L = 0; L < 3; ++L) {
+  if (!d.fwd_only) cudaMemset(n->wg_ticket, 0, 64 * 4);
+  for (int L = 0; L < 3 && !d.fwd_only; ++L) {
     const int64_t cnt[3] = {(int64_t)d.B * n->h1 * n->w1 * 32, (int64_t)d.B * n->h2 * n->w2 * 64, (int64_t)d.B * n->feat};
     cudaMemset(n->dact_hi[L], 0, cnt[L] * 4); cudaMemset(n->dact_lo[L], 0, cnt[L] * 4); cudaMemset(n->dact_f32[L], 0, cnt[L] * 4);
   }
@@ -1437,7 +1470,8 @@ int um_pack_weights(UmNet* n, void* stream) {
   for (int b = 0; b < 2; ++b)
     for (int L = 0; L < 3; ++L) { a.wf_hi[b][L] = n->wf_hi[b][L]; a.wf_lo[b][L] = n->wf_lo[b][L]; }
   a.wd3_hi = n->wd3_hi; a.wd3_lo = n->wd3_lo; a.wd2_hi = n->wd2_hi; a.wd2_lo = n->wd2_lo;
-  const int total = 2 * kConvFwdFloats + kConvN[2] * kConvK[2] + kConvN[1] * kConvK[1];
+  // the kernel's elements run online forward images first: a forward-only plan launches just those
+  const int total = n->d.fwd_only ? kConvFwdFloats : 2 * kConvFwdFloats + kConvN[2] * kConvK[2] + kConvN[1] * kConvK[1];
   DZ_LAUNCH_NAMED("conv_pack", um_pack_conv_kernel, (unsigned)ceil_div(total, 256), 256, 0, stream, a);
   return DZ_OK;
 }
@@ -1503,6 +1537,8 @@ int um_forward_fc(UmNet* n, const float* noise, void* stream) {
   DZ_LAUNCH_NAMED("fc_finish", um_fc_finish_kernel, grid, 256, 0, stream, a);
   return DZ_OK;
 }
+
+int um_bind_noise(UmNet* n, const float* noise) { return apply_noise(n, noise, nullptr); }
 
 int um_split_dh1(UmNet* n, void* stream) {
   return um_split(n->dh1_f32, n->dh1_hi, n->dh1_lo, (long long)n->d.nstream * n->d.B * 512, stream);

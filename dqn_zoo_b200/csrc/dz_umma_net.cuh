@@ -20,11 +20,16 @@ struct UmNetDesc {
   int noise_apply[3];                // rainbow: noise apply index of each pass
   int64_t noise_stride;              // floats per apply
   int64_t noise_off_in[2], noise_off_out[2];   // offsets of eps_in[feat] / eps_out[512] of stream s inside one apply
+  // 1: forward-only plan for acting (npass 1 on the online blob, any B up to the actor's cap): forward buffers and
+  // launches only, the fc x operand in row chunks of 64 and split counts that depend on the geometry alone, so that
+  // every row's arithmetic is the same at every B.
+  int fwd_only;
 };
 
 struct UmNet;
 
-// Geometry the path supports (else the learner keeps the fp32-FMA kernels).
+// Geometry the path supports (else the learner keeps the fp32-FMA kernels).  The learner's plans take B <= 64;
+// forward-only plans any B >= 1.
 bool um_net_supported(const UmNetDesc& d);
 int64_t um_net_workspace_bytes(const UmNetDesc& d);
 // `base` may be nullptr (size query through carve); buffers are carved from it in a fixed order.
@@ -42,7 +47,10 @@ float* um_dh1_hi(UmNet* n, int stream);               // tf32 hi / lo of dh1 (wr
 float* um_dh1_lo(UmNet* n, int stream);
 
 // One launch each unless noted.  rows[p]: row-pointer table of pass p (uint8 observations, gathered in place).
-int um_pack_weights(UmNet* n, void* stream);                                   // conv weight images (both nets)
+int um_pack_weights(UmNet* n, void* stream);                                   // conv weight images (both nets;
+                                                                               // forward-only: online forward images)
+int um_bind_noise(UmNet* n, const float* noise);                               // noisy fc: the noise buffer um_forward_fc
+                                                                               // will read (synchronous; outside captures)
 int um_forward_torso(UmNet* n, const uint8_t* const* const* rows, void* stream);   // conv1, conv2, conv3
 int um_forward_fc(UmNet* n, const float* noise, void* stream);                 // fc1 / noisy1 + finish -> h1
 int um_split_dh1(UmNet* n, void* stream);                                      // dh1 fp32 -> hi/lo (if the producer wrote fp32 only)

@@ -334,6 +334,10 @@ class Learner:
     self._keep_act = (obs, t, n, x)
     return self._act_a[:E], self._act_q[:E]
 
+  def actor(self, num_streams: int) -> 'Actor':
+    """An acting context for `num_streams` streams (not capped by batch_size) over this learner's online parameters."""
+    return Actor(self, num_streams)
+
   # -- fused sample -> update -> priority write-back -------------------------------------------------
   def make_learn_io(self, stage: torch.Tensor, prioritized: bool, priority_exponent: float):
     """Binds the per-step staging buffer (float64 view: [pos(int64) B | u_tree B | u_mix B | scalars 4])
@@ -370,3 +374,88 @@ class Learner:
   @property
   def sampled_weights(self):
     return self.s_f64[self.batch_size:]
+
+
+class Actor:
+  """Batched acting for a fixed number of streams (1 to 1024; IQN: num_streams * tau_samples_policy <= 16384) in one
+  call, over the learner's online parameters read in place: an act enqueued after `learn()` / `update()` on the stream
+  sees their parameters, with no copy.  Its buffers are sized for its streams, so one learner of any batch size can act
+  for many environments.  On the tensor-core geometries (84x84x4 among them) the torso and the 3136 -> 512 layer run
+  on the learner's sm_90a tensor-core kernels.  Row e's result does not depend on num_streams."""
+
+  def __init__(self, learner: Learner, num_streams: int):
+    E = int(num_streams)
+    nbytes = C.c_int64()
+    _lib.call('dz_actor_plan_query', C.byref(learner.cfg), E, C.byref(nbytes))
+    self.learner = learner          # the actor reads the learner's parameters: keep it alive for the actor's lifetime
+    self.num_streams = E
+    dev = learner.device
+    net = learner.net
+    self.workspace = torch.zeros(nbytes.value, dtype=torch.uint8, device=dev)
+    self.q = torch.zeros((E, net.num_actions), dtype=torch.float32, device=dev)
+    self.actions = torch.zeros(E, dtype=torch.int32, device=dev)
+    self.taus = torch.zeros((E, net.tau_samples_policy), dtype=torch.float32, device=dev) if net.kind == 'iqn' else None
+    rb = net.kind == 'rainbow'
+    self.noise = torch.zeros(learner.noise_stride, dtype=torch.float32, device=dev) if rb else None
+    self.stream_noise = torch.zeros((E, learner.noise_stride), dtype=torch.float32, device=dev) if rb else None
+    handle = C.c_void_p()
+    _lib.call('dz_actor_create', learner._h, E, self.workspace.data_ptr(), C.byref(handle))
+    self._h = handle
+
+  def __del__(self):
+    h, self._h = getattr(self, '_h', None), None
+    if h:
+      _lib.lib.dz_actor_destroy(h)
+
+  def generate_randomness(self, seed: int, per_stream: bool = False) -> torch.Tensor:
+    """Fills and returns `.taus` (IQN, [E, tau_samples_policy]), `.noise` (rainbow, one apply) or, with `per_stream`,
+    `.stream_noise` (rainbow, [E, noise_stride]) from the learner's generator, advancing its counter once.  For E <=
+    batch_size the draws equal `Learner.generate_randomness` / `generate_stream_noise` at the same seed and counter."""
+    kind = self.learner.kind
+    if per_stream and kind != 'rainbow':
+      raise ValueError('per_stream randomness needs a rainbow learner')
+    if kind not in ('iqn', 'rainbow'):
+      raise ValueError('%s acting draws no randomness' % kind)
+    buf = self.taus if kind == 'iqn' else (self.stream_noise if per_stream else self.noise)
+    _lib.call('dz_actor_generate_randomness', self._h, seed, 1 if per_stream else 0, buf.data_ptr(), _cstream())
+    return buf
+
+  def act(self, obs_u8, epsilon: float = 0.0, explore=None, taus=None, noise=None, stream_noise=None):
+    """`Learner.act_batch` for exactly num_streams observations: `obs_u8` [E, H, W, C] uint8, `explore` float32 [2, E]
+    uniforms (None: greedy), IQN `taus` [E, tau_samples_policy], rainbow `noise` (one apply shared by the streams) or
+    `stream_noise` [E, noise_stride].  Returns (actions int32 [E], q_values float32 [E, num_actions]) device tensors,
+    overwritten by the next call."""
+    L = self.learner
+    E = self.num_streams
+    obs = torch.as_tensor(obs_u8, device=L.device).contiguous()
+    if obs.dtype != torch.uint8 or obs.dim() < 1 or obs.shape[0] != E or obs[0].numel() != L.obs_bytes:
+      raise ValueError('obs must be uint8 [%d, %s], got %s %s' % (E, ', '.join(map(str, L.net.obs_shape)), obs.dtype,
+                                                                  tuple(obs.shape)))
+    x = None if explore is None else torch.as_tensor(explore, device=L.device).to(torch.float32).contiguous()
+    if x is not None and x.numel() != 2 * E:
+      raise ValueError('explore must be [2, %d], got %s' % (E, tuple(x.shape)))
+    t = n = None
+    noise_ld = 0
+    if stream_noise is not None:
+      if noise is not None or taus is not None:
+        raise ValueError('stream_noise replaces noise / taus')
+      if L.kind != 'rainbow':
+        raise ValueError('stream_noise needs a rainbow learner')
+      n = torch.as_tensor(stream_noise, device=L.device).to(torch.float32).contiguous()
+      if n.dim() != 2 or n.shape[0] != E or n.shape[1] != L.noise_stride:
+        raise ValueError('stream_noise must be [E, noise_stride] = [%d, %d], got %s' % (E, L.noise_stride, tuple(n.shape)))
+      noise_ld = L.noise_stride
+    else:
+      if taus is not None:
+        t = torch.as_tensor(taus, device=L.device).to(torch.float32).contiguous()
+        if L.kind == 'iqn' and t.numel() != E * L.net.tau_samples_policy:
+          raise ValueError('taus must be [%d, %d], got %s' % (E, L.net.tau_samples_policy, tuple(t.shape)))
+      if noise is not None:
+        n = torch.as_tensor(noise, device=L.device).to(torch.float32).contiguous()
+        if L.kind == 'rainbow' and n.numel() < L.noise_stride:
+          raise ValueError('noise must hold one apply (%d floats), got %d' % (L.noise_stride, n.numel()))
+    _lib.call('dz_actor_act', self._h, obs.data_ptr(), 0 if t is None else t.data_ptr(), 0 if n is None else n.data_ptr(),
+              noise_ld, 0 if x is None else x.data_ptr(), float(epsilon), self.q.data_ptr(), self.actions.data_ptr(),
+              _cstream())
+    self._keep = (obs, t, n, x)
+    return self.actions, self.q

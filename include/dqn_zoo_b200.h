@@ -394,6 +394,29 @@ int dz_learner_noise_stride(const dz_learner_config* cfg, int64_t* out);
  * d_counters[1] once.  DZ_EINVAL for a non-rainbow learner, E outside [1, batch] or a NULL buffer. */
 int dz_learner_generate_stream_noise(dz_learner* l, uint64_t seed, int32_t E, float* d_noise, void* stream);
 
+/* ---- Acting context (SURVEY §8(f) #3: many actor streams per GPU) ----------------------------------------------
+ * Batched acting for num_streams in [1, 1024] streams per call (iqn: also num_streams * tau_samples_policy <= 16384)
+ * over the learner's ONLINE parameters, read in place: an act enqueued on the stream after a learner step sees that
+ * step's parameters.  The actor keeps the learner handle (destroy the actor first) and owns only buffers sized for its
+ * streams.  On the tensor-core geometries the torso and the 3136 -> 512 layer (rainbow: with one shared noise apply)
+ * run on the learner's sm_90a tensor-core kernels; the heads, and rainbow's per-stream noisy layers, on the fp32-FMA
+ * kernels.  Row e's result does not depend on num_streams. */
+typedef struct dz_actor dz_actor;
+/* Device workspace bytes of an actor for num_streams streams.  DZ_EINVAL outside the caps. */
+int dz_actor_plan_query(const dz_learner_config* cfg, int32_t num_streams, int64_t* workspace_bytes);
+int dz_actor_create(dz_learner* l, int32_t num_streams, void* d_workspace, dz_actor** out);
+void dz_actor_destroy(dz_actor* a);
+/* dz_learner_act_batch's contract for exactly num_streams observations (E below).  Rainbow: noise_ld = 0, d_noise is
+ * one apply shared by the streams; noise_ld = dz_learner_noise_stride, d_noise is [E][stride] and stream e uses apply e.
+ * DZ_EINVAL for a NULL buffer, a missing taus / noise or another noise_ld. */
+int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const float* d_noise, int64_t noise_ld,
+                 const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream);
+/* The learner's generator and counter (d_counters[1], advanced once): iqn taus [E][tau_samples_policy] with the stream
+ * of dz_learner_generate_randomness's taus; rainbow one noise apply, or E applies when per_stream is set, with the
+ * stream of its noise (so for E <= batch the draws equal those calls' for the same seed and counter).  DZ_EINVAL for
+ * other kinds, per_stream on iqn or a NULL buffer. */
+int dz_actor_generate_randomness(dz_actor* a, uint64_t seed, int32_t per_stream, float* d_out, void* stream);
+
 /* target <- online (dqn/agent.py:155-156): device-to-device copy of the blob. */
 int dz_learner_sync_target(dz_learner* l, void* stream);
 
@@ -445,6 +468,11 @@ int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace);
  * give 1 when the launch runs on the packed-operand GEMM (csrc/dz_tcp.cuh) and DZ_EINVAL when it runs on the fp32-FMA
  * kernels, independently of the torso's path. */
 int dz_test_learner_mma_path(dz_learner* l, const char* tag, int32_t* path);
+/* Tests: the same for the actor's forward launches ("conv1_fwd", "conv2_fwd", "conv3_fwd", "fc1_fwd" / "noisy1_fwd");
+ * DZ_EINVAL when the actor runs on the fp32-FMA kernels. */
+int dz_test_actor_mma_path(dz_actor* a, const char* tag, int32_t* path);
+/* Tests: device pointer + element count of the actor's conv3 output "act3" ([E][feat], written by the last act). */
+int dz_test_actor_buffer(dz_actor* a, const char* name, float** d_ptr, int64_t* count);
 /* Debug: every kernel appends (globaltimer ns, gridDim.x << 32 | gridDim.y << 16 | blockDim.x) to d_buf right after its
  * dependencies completed; d_buf[0] (low 32 bits) counts the entries, entries start at d_buf[2].  d_buf: 2 + 2 * 4000
  * uint64, zeroed by the caller; nullptr switches the stamps off.  Works under CUDA-graph replay (tools/step_timeline.py). */

@@ -4,6 +4,9 @@ ONE device-to-host copy of E actions per tick) versus the single-observation pat
 Rainbow's two noise modes, alternated in one run (decisions/s of each round), then kernel times in a separate run:
   python tools/bench_acting.py --agent rainbow --per-stream-noise [--rounds 3]
   python tools/bench_acting.py --agent rainbow --per-stream-noise --profile OUT_DIR
+The acting context against act_batch on a learner of batch E (the only single-call option without it), alternated per
+stream count, then kernel times per tick in a separate run:
+  python tools/bench_acting.py --agent dqn --compare-actor --streams 32,128,256,512 [--rounds 3] [--profile OUT_DIR]
 Observations are device-resident frame stacks (what processors.BatchedAtariPreprocessor hands out)."""
 
 import argparse
@@ -92,20 +95,109 @@ def profile_modes(actors, obs, a):
   print(json.dumps(result))
 
 
+def kernel_times(fn, ticks, path):
+  """Kernel time per tick (us) by kernel name, from torch.profiler CUDA activity written to `path`."""
+  torch.cuda.synchronize()
+  with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+    for _ in range(ticks):
+      fn()
+    torch.cuda.synchronize()
+  prof.export_chrome_trace(path)
+  per_kernel = collections.defaultdict(float)
+  with open(path) as f:
+    for ev in json.load(f)['traceEvents']:
+      if ev.get('cat') == 'kernel':
+        short = ev['name'].replace('(anonymous namespace)::', '').replace('void ', '').split('(')[0].split('<')[0].split('::')[-1]
+        per_kernel[short] += ev['dur'] / ticks
+  return {'total_us': round(sum(per_kernel.values()), 2),
+          'kernels_us': {k: round(v, 2) for k, v in sorted(per_kernel.items(), key=lambda kv: -kv[1])}}
+
+
+def compare_actor(a, streams):
+  """Per stream count E, alternated within each round: (a) the acting context of a batch-32 learner, (b) act_batch on
+  a learner of batch E, and at E = 32 also (c) act_batch on the batch-32 learner.  A tick is one act call (greedy
+  for half the streams: epsilon 0.5 with device uniforms) and the D2H of its E actions.  Rainbow: one shared noise
+  apply; IQN: one tau row per stream.  Randomness is drawn once, outside the timed ticks."""
+  from dqn_zoo_b200 import learner as dl
+  from oracle import learner_oracle as lo
+  net = dl.NetworkSpec(a.agent, 6)
+  params = lo.init_params(lo.NetSpec(a.agent, 6), 2)
+
+  def learner(batch):
+    L = dl.Learner(net, batch_size=batch)
+    L.set_params(params, also_target=True)
+    return L
+
+  L32 = learner(32)
+  rs = np.random.RandomState(0)
+  ticks = {}
+  keep = []
+  for E in streams:
+    obs = torch.randint(0, 256, (E, 84, 84, 4), dtype=torch.uint8, device='cuda')
+    explore = torch.as_tensor(rs.uniform(size=(2, E)).astype(np.float32), device='cuda')
+    kw = {}
+    if a.agent == 'iqn':
+      kw['taus'] = torch.as_tensor(rs.uniform(size=(E, net.tau_samples_policy)).astype(np.float32), device='cuda')
+    if a.agent == 'rainbow':
+      L32.generate_randomness(1)
+      kw['noise'] = L32.noise[:L32.noise_stride].clone()
+    actor = L32.actor(E)
+    LE = L32 if E == 32 else learner(E)
+    keep += [actor, LE]
+
+    def tick(act, obs=obs, explore=explore, kw=kw):
+      actions, _ = act(obs, epsilon=0.5, explore=explore, **kw)
+      actions.cpu()
+    ticks[(E, 'actor_on_batch32_learner')] = lambda tick=tick, actor=actor: tick(actor.act)
+    ticks[(E, 'act_batch_on_batch%d_learner' % E)] = lambda tick=tick, LE=LE: tick(LE.act_batch)
+  for fn in ticks.values():
+    for _ in range(20):
+      fn()
+  result = dict({'metric': 'acting decisions per second: acting context vs act_batch (device-resident observations)',
+                 'agent': a.agent, 'ticks_per_round': a.ticks, 'rounds': a.rounds}, **card())
+  if a.profile:
+    os.makedirs(a.profile, exist_ok=True)
+    result['metric'] = 'acting kernel time per tick (us), torch.profiler'
+    result['kernel_times'] = {'E=%d %s' % k: kernel_times(fn, a.ticks, os.path.join(a.profile, 'acting_E%d_%s.json' % k))
+                              for k, fn in ticks.items()}
+    print(json.dumps(result))
+    return
+  rates = collections.defaultdict(list)
+  for _ in range(a.rounds):
+    for (E, mode), fn in ticks.items():
+      torch.cuda.synchronize()
+      t0 = time.perf_counter()
+      for _ in range(a.ticks):
+        fn()
+      torch.cuda.synchronize()
+      rates['E=%d %s' % (E, mode)].append(round(E * a.ticks / (time.perf_counter() - t0), 1))
+  result['decisions_per_s'] = dict(rates)
+  print(json.dumps(result))
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--agent', default='dqn')
-  ap.add_argument('--streams', type=int, default=32)
+  ap.add_argument('--streams', default='32', help='streams per tick; with --compare-actor a comma-separated list')
   ap.add_argument('--ticks', type=int, default=300)
   ap.add_argument('--per-stream-noise', action='store_true',
                   help='rainbow: compare one noise apply per tick with one apply per stream, alternated')
   ap.add_argument('--rounds', type=int, default=3)
-  ap.add_argument('--profile', default=None, help='with --per-stream-noise: kernel times from torch.profiler, traces here')
+  ap.add_argument('--compare-actor', action='store_true',
+                  help='the acting context of a batch-32 learner vs act_batch on a learner of batch E, alternated')
+  ap.add_argument('--profile', default=None,
+                  help='with --per-stream-noise or --compare-actor: kernel times from torch.profiler, traces here')
   a = ap.parse_args()
   if a.per_stream_noise and a.agent != 'rainbow':
     ap.error('--per-stream-noise needs --agent rainbow')
+  streams = [int(x) for x in str(a.streams).split(',')]
+  if len(streams) > 1 and not a.compare_actor:
+    ap.error('a list of stream counts needs --compare-actor')
   if not torch.cuda.is_available():
     raise SystemExit('bench_acting.py needs a CUDA device')
+  if a.compare_actor:
+    return compare_actor(a, streams)
+  a.streams = streams[0]
   from dqn_zoo_b200 import agent as agent_lib
   from dqn_zoo_b200 import learner as dl
   from oracle import learner_oracle as lo
