@@ -28,6 +28,7 @@ from dqn_zoo_b200 import _lib
 from dqn_zoo_b200 import jax_prng
 from dqn_zoo_b200 import learner as learner_lib
 from dqn_zoo_b200 import parts
+from dqn_zoo_b200 import processors
 from dqn_zoo_b200 import replay as replay_lib
 
 NetworkSpec = learner_lib.NetworkSpec
@@ -568,11 +569,15 @@ class BatchedEpsilonGreedyActor:
     self._actions_host = torch.zeros(self._E, dtype=torch.int32).pin_memory()
     self.q_values = None
 
-  def step(self, observations) -> np.ndarray:
+  def step(self, observations, epsilon: Optional[float] = None) -> np.ndarray:
     """observations: [E, H, W, C] uint8 (device tensor, e.g. the stacks of processors.BatchedAtariPreprocessor, or host
-    array).  Returns the E actions as a host int32 array."""
+    array).  `epsilon` overrides the actor's own schedule for this tick (`VectorTrainer` evaluates the training agent's
+    schedule at its frame count).  Returns the E actions as a host int32 array."""
     L = self._learner
-    eps = self._epsilon(self._t) if callable(self._epsilon) else float(self._epsilon)
+    if epsilon is not None:
+      eps = float(epsilon)
+    else:
+      eps = self._epsilon(self._t) if callable(self._epsilon) else float(self._epsilon)
     explore = None
     if eps > 0.0:
       self._explore_host.copy_(torch.from_numpy(self._rng.uniform(size=(2, self._E)).astype(np.float32)))
@@ -605,3 +610,242 @@ class BatchedEpsilonGreedyActor:
     self._t += 1
     return self._actions_host.numpy().copy()
 
+
+
+# The acting context's limits (`learner_lib.Actor`), checked when a trainer acts beyond its learner's batch.
+ACTOR_MAX_STREAMS = 1024
+ACTOR_MAX_IQN_ROWS = 16384
+
+
+def _due(lo: int, hi: int, period: int) -> range:
+  """The frames f in [lo, hi] with f % period == 0."""
+  return range(lo + (-lo) % period, hi + 1, period)
+
+
+class VectorTrainer:
+  """Trains one agent from E environment streams: dqn/agent.py:133-158 generalised to a tick of E timesteps, over the
+  batched device paths (`VectorizedAtariPreprocessor.step_arrays`, `BatchedEpsilonGreedyActor`,
+  `replay.VectorNStepAccumulator` + `add_batch`, the agent's CUDA-graph learner step).
+
+  The trainer wraps a training agent (any of `AGENTS`) and uses its state in place: learner and replay, the host
+  RandomState draws of `_learn`, the CUDA graph, `min_replay_capacity`, `learn_period`, `target_network_update_period`
+  and the exploration schedule.  It owns a `VectorizedAtariPreprocessor(E, device_observations=True)`, a
+  `VectorNStepAccumulator(E, n)` (n read from the agent's transition accumulator) and a `BatchedEpsilonGreedyActor` over
+  the agent's learner, whose exploration uniforms (and acting randomness seed) come from `rng_key`.
+
+  Tick contract.  `frame_t` is the agent's frame counter (-1 before the first step, as for `step`).  With t0 = frame_t
+  before the tick, stream e's timestep is frame f = t0 + 1 + e, and the tick leaves frame_t = t0 + E.  In order:
+    1. preprocess: `step_arrays` on the E raw timesteps;
+    2. act: if any stream emits a timestep, ONE act call for all E streams at epsilon = schedule(t0 + 1); emitting
+       streams take the new action, the others repeat their last one (RuntimeError if a stream has none yet); the
+       actions reach the host in one copy;
+    3. insert: `acc.step`, then `replay.add_batch` (prioritized agents at the learner's max_seen_priority);
+    4. gate: if replay.size < min_replay_capacity, return the actions (no learn step, no target sync);
+    5. learn and sync: for the frames f of the tick in increasing order, one `_learn()` where f % learn_period == 0,
+       then `sync_target()` + `check_device_flags()` where f % target_network_update_period == 0;
+    6. return the actions without waiting for the learn steps: the next tick's act is ordered after them on the stream.
+  With E = 1 this is `step`'s control flow.  The tick synchronises with the device once, for the actions, plus the flag
+  reads at target syncs."""
+
+  def __init__(self, train_agent: _DeviceAgent, num_streams: int, rng_key, per_stream_noise: bool = False,
+               preprocessor_kwargs: Optional[Mapping[str, Any]] = None):
+    if not isinstance(train_agent, _DeviceAgent):
+      raise TypeError('train_agent must be one of the training agents (%s)' % ', '.join(sorted(AGENTS)))
+    E = int(num_streams)
+    L = train_agent.learner
+    if E < 1:
+      raise ValueError('num_streams must be >= 1')
+    if E > L.batch_size:                       # acted through an acting context: its limits apply
+      if E > ACTOR_MAX_STREAMS:
+        raise ValueError('num_streams %d exceeds the acting limit of %d streams' % (E, ACTOR_MAX_STREAMS))
+      if L.kind == 'iqn' and E * L.net.tau_samples_policy > ACTOR_MAX_IQN_ROWS:
+        raise ValueError('iqn acting needs num_streams * tau_samples_policy <= %d, got %d * %d'
+                         % (ACTOR_MAX_IQN_ROWS, E, L.net.tau_samples_policy))
+    acc = train_agent._transition_accumulator
+    if not isinstance(acc, replay_lib.NStepTransitionAccumulator):
+      raise ValueError('the agent needs a TransitionAccumulator or NStepTransitionAccumulator')
+    kwargs = dict(preprocessor_kwargs or {})
+    if not kwargs.pop('device_observations', True):
+      raise ValueError('the trainer keeps its frame stacks on the device: device_observations must be True')
+    kwargs.setdefault('device', L.device)
+    self._agent = train_agent
+    self._E = E
+    self._pre = processors.VectorizedAtariPreprocessor(E, device_observations=True, **kwargs)
+    self._acc = replay_lib.VectorNStepAccumulator(E, acc._transitions.maxlen, device=L.device)
+    self._actor = BatchedEpsilonGreedyActor(L, E, exploration_epsilon=0.0, rng_key=rng_key,
+                                            per_stream_noise=per_stream_noise)
+    self._actions = np.zeros(E, np.int32)
+    self._has_action = np.zeros(E, bool)
+    self._learn_steps = 0
+    self._q_host = torch.zeros((E, L.net.num_actions), dtype=torch.float32).pin_memory()
+    self._q_pending = None                     # (event, acting streams) of the last act's q-value copy
+    self._statistics = {'state_value': np.nan}
+    self._episode_return = np.zeros(E)
+    self._episode_length = np.zeros(E, np.int64)
+    self._num_episodes = np.zeros(E, np.int64)
+
+  # -- one tick ------------------------------------------------------------------------------------
+  def step(self, frames, step_type, reward, discount, lives) -> np.ndarray:
+    """frames: uint8 [E, H, W, 3] raw RGB (device tensor, or host array: one H2D copy); step_type int [E]; reward /
+    discount float [E] with NaN for None (FIRST timesteps); lives int [E].  Returns the E actions, int32 [E]."""
+    step_type, reward, discount, lives = self._check(frames, step_type, reward, discount, lives)
+    ag = self._agent
+    E = self._E
+    t0 = ag._frame_t
+    ag._frame_t = t0 + E
+    out = self._pre.step_arrays(frames, step_type, reward, discount, lives)
+    self._track_episodes(step_type, reward)
+    emit = out['emit']
+    if np.any(~emit & ~self._has_action):
+      raise RuntimeError('Cannot repeat if action has never been selected.')
+    if emit.any():
+      new = self._actor.step(self._pre.stacks, epsilon=self._epsilon_at(t0 + 1))
+      self._actions = np.where(emit, new, self._actions).astype(np.int32)
+      self._has_action |= emit
+      self._q_host.copy_(self._actor.q_values, non_blocking=True)
+      ev = torch.cuda.Event()
+      ev.record()
+      self._q_pending = (ev, emit.copy())
+      batch = self._acc.step(emit, out['step_type'], out['reward'], out['discount'], self._pre.stacks, self._actions)
+      if batch is not None:
+        if ag.PRIORITIZED:
+          ag._replay.add_batch(batch, ag._learner.max_seen_priority)
+        else:
+          ag._replay.add_batch(batch)
+    actions = self._actions.copy()
+    if ag._replay.size < ag._min_replay_capacity:
+      return actions
+    lo, hi = t0 + 1, t0 + E
+    due = sorted([(f, 0) for f in _due(lo, hi, ag._learn_period)] +
+                 [(f, 1) for f in _due(lo, hi, ag._target_network_update_period)])
+    for _, sync in due:                        # at a frame due for both, the learn step comes first
+      if sync:
+        ag._learner.sync_target()
+        ag.check_device_flags()
+      else:
+        ag._learn()
+        self._learn_steps += 1
+    return actions
+
+  def _check(self, frames, step_type, reward, discount, lives):
+    E = self._E
+    shape = tuple(frames.shape)
+    dtype_ok = frames.dtype == torch.uint8 if isinstance(frames, torch.Tensor) else np.asarray(frames).dtype == np.uint8
+    if len(shape) != 4 or shape[0] != E or shape[3] != 3 or not dtype_ok:
+      raise ValueError('frames must be uint8 [%d, H, W, 3], got %s %s' % (E, frames.dtype, shape))
+    if self._pre._in_shape is not None and shape[1:] != self._pre._in_shape:
+      raise ValueError('frame shape changed: %s vs %s' % (shape[1:], self._pre._in_shape))
+    arrays = (np.asarray(step_type, np.int64), np.asarray(reward, np.float64), np.asarray(discount, np.float64),
+              np.asarray(lives, np.int64))
+    for name, a in zip(('step_type', 'reward', 'discount', 'lives'), arrays):
+      if a.shape != (E,):
+        raise ValueError('%s must have shape (%d,), got %s' % (name, E, a.shape))
+    return arrays
+
+  def _epsilon_at(self, t: int) -> float:
+    ag = self._agent
+    return 0.0 if ag.GREEDY or ag._exploration_epsilon is None else float(ag._exploration_epsilon(t))
+
+  def _track_episodes(self, step_type, reward):
+    first = step_type == int(parts.StepType.FIRST)
+    self._episode_return[first] = 0.0
+    self._episode_length[first] = 0
+    self._episode_return += np.where(first | np.isnan(reward), 0.0, reward)
+    self._episode_length += 1
+    self._num_episodes += step_type == int(parts.StepType.LAST)
+
+  def reset(self, stream=None) -> None:
+    """`Agent.reset` (which `run_loop` calls before every episode) for every stream, or for one stream or a sequence of
+    streams, e.g. those whose last timestep was LAST: their preprocessor and accumulator state and their last action."""
+    if stream is None:
+      self._pre.reset()
+      self._acc.reset()
+      self._has_action[:] = False
+      return
+    for e in np.atleast_1d(np.asarray(stream, np.int64)):    # the streams ending an episode, not every stream
+      self._pre.reset(int(e))
+      self._acc.reset(int(e))
+      self._has_action[e] = False
+
+  # -- surface ------------------------------------------------------------------------------------------------------
+  @property
+  def num_streams(self) -> int:
+    return self._E
+
+  @property
+  def agent(self) -> _DeviceAgent:
+    return self._agent
+
+  @property
+  def frame_t(self) -> int:
+    return self._agent._frame_t
+
+  @property
+  def learn_steps(self) -> int:
+    """Learner steps this trainer has run."""
+    return self._learn_steps
+
+  @property
+  def exploration_epsilon(self) -> float:
+    return self._agent.exploration_epsilon
+
+  @property
+  def statistics(self) -> Mapping[str, float]:
+    """`state_value`: the mean over the streams that acted in the last acting tick of their max q-value."""
+    if self._q_pending is not None:
+      ev, acted = self._q_pending
+      ev.synchronize()
+      self._statistics['state_value'] = float(self._q_host.numpy()[acted].max(axis=1).mean())
+      self._q_pending = None
+    return self._statistics
+
+  @property
+  def episode_return(self) -> np.ndarray:
+    """Per stream: the summed raw rewards of its current episode (after a LAST timestep: of the episode it ended)."""
+    return self._episode_return.copy()
+
+  @property
+  def episode_length(self) -> np.ndarray:
+    """Per stream: the timesteps of its current episode, FIRST included (after LAST: of the episode it ended)."""
+    return self._episode_length.copy()
+
+  @property
+  def num_episodes(self) -> np.ndarray:
+    """Per stream: the episodes it has completed (LAST timesteps seen)."""
+    return self._num_episodes.copy()
+
+  def get_state(self) -> Mapping[str, Any]:
+    return {
+        'agent': self._agent.get_state(),
+        'frame_t': self._agent._frame_t,
+        'actions': self._actions.copy(),
+        'has_action': self._has_action.copy(),
+        'learn_steps': self._learn_steps,
+        # the replay draws its samples from a RandomState the agent's state leaves to the run (as the reference does)
+        'replay_rng': self._agent._replay._random_state.get_state(),
+        'actor_rng': self._actor._rng.get_state(),
+        'actor_t': self._actor._t,
+        'preprocessor': self._pre.get_state(),
+        'accumulator': self._acc.get_state(),
+        'statistics': dict(self.statistics),
+        'episodes': (self._episode_return.copy(), self._episode_length.copy(), self._num_episodes.copy()),
+    }
+
+  def set_state(self, state: Mapping[str, Any]) -> None:
+    if np.shape(state['actions']) != (self._E,):
+      raise ValueError('state is for %d streams, this trainer has %d' % (len(state['actions']), self._E))
+    self._agent.set_state(state['agent'])
+    self._agent._frame_t = state['frame_t']
+    self._actions = np.array(state['actions'], np.int32)
+    self._has_action = np.array(state['has_action'], bool)
+    self._learn_steps = int(state['learn_steps'])
+    self._agent._replay._random_state.set_state(state['replay_rng'])
+    self._actor._rng.set_state(state['actor_rng'])
+    self._actor._t = int(state['actor_t'])
+    self._pre.set_state(state['preprocessor'])
+    self._acc.set_state(state['accumulator'])
+    self._statistics = dict(state['statistics'])
+    self._q_pending = None
+    ret, length, count = state['episodes']
+    self._episode_return, self._episode_length, self._num_episodes = (np.array(ret), np.array(length),
+                                                                      np.array(count))

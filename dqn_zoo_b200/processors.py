@@ -13,7 +13,7 @@ There is no CPU fallback: without the CUDA library the import of `dqn_zoo_b200._
 
 import ctypes as C
 import math
-from typing import Any, List, Optional, Sequence, Tuple
+from typing import Any, List, Mapping, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -413,6 +413,33 @@ class VectorizedAtariPreprocessor(BatchedAtariPreprocessor):
     self._vs.reset(None if stream is None else [stream])
     if self._in_shape is not None:
       (self._stacks if stream is None else self._stacks[stream]).zero_()
+
+  def get_state(self) -> Mapping[str, Any]:
+    """The scalar state machine's arrays and, once frames have arrived, the device frame stacks and the two pooled raw
+    frames of every stream, copied to the host."""
+    state = {'scalars': {k: v.copy() for k, v in vars(self._vs).items() if isinstance(v, np.ndarray)},
+             'in_shape': self._in_shape}
+    if self._in_shape is not None:
+      state['stacks'] = self._stacks.cpu().numpy()
+      state['raw'] = self._raw.cpu().numpy()
+    return state
+
+  def set_state(self, state: Mapping[str, Any]) -> None:
+    """Restores `get_state()` of a preprocessor with the same options and stream count."""
+    scalars = state['scalars']
+    if scalars['index'].shape != (self._n,):
+      raise ValueError('state is for %d streams, this preprocessor has %d' % (scalars['index'].shape[0], self._n))
+    for k, v in scalars.items():
+      setattr(self._vs, k, np.array(v, copy=True))
+    if state['in_shape'] is None:
+      return
+    shape = tuple(state['in_shape'])
+    if self._in_shape is None:
+      self._allocate(shape)
+    elif self._in_shape != shape:
+      raise ValueError('frame shape of the state %s != %s' % (shape, self._in_shape))
+    self._stacks.copy_(torch.as_tensor(state['stacks']))
+    self._raw.copy_(torch.as_tensor(state['raw']))
 
   def step_arrays(self, frames, step_type, reward, discount, lives, active=None):
     """frames: uint8 [n, H, W, 3] (device tensor, or a host array -> one H2D copy); step_type int [n]; reward / discount

@@ -1541,6 +1541,22 @@ class VectorNStepAccumulator:
     self._len[sel] = 0
     self._has_tm1[sel] = False
 
+  _STATE_ARRAYS = ('_len', '_pos', '_has_tm1', '_a_tm1', '_r', '_d', '_a')
+
+  def get_state(self) -> Mapping[str, Any]:
+    """The pending windows of every stream, with the observation ring copied to the host."""
+    state = {k.lstrip('_'): getattr(self, k).copy() for k in self._STATE_ARRAYS}
+    state['ring'] = None if self._ring is None else self._ring.cpu().numpy()
+    return state
+
+  def set_state(self, state: Mapping[str, Any]) -> None:
+    """Restores `get_state()` of an accumulator with the same stream count and n."""
+    if np.shape(state['r']) != (self._E, self._n):
+      raise ValueError('state is for [streams, n] = %s, this accumulator is %s' % (np.shape(state['r']), (self._E, self._n)))
+    for k in self._STATE_ARRAYS:
+      setattr(self, k, np.array(state[k.lstrip('_')], copy=True))
+    self._ring = None if state['ring'] is None else torch.as_tensor(state['ring']).to(self._device)
+
   def step(self, emit, step_type, reward, discount, observations, actions) -> Optional[Transition]:
     """emit: bool [E], the streams with a new timestep; step_type / reward / discount: [E] (NaN = None); observations:
     [E, *obs_shape] (e.g. `VectorizedAtariPreprocessor.stacks`); actions: [E], the a_t chosen on this timestep.

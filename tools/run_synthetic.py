@@ -7,12 +7,18 @@ sequence of calls is what tests/test_gpu_agent.py::test_train_eval_iteration_wit
 
   python tools/run_synthetic.py --agent rainbow --num_iterations 3 --num_train_frames 2000 --num_eval_frames 500 \
       --results_csv_path /tmp/results.csv --checkpoint_path /tmp/ck.pkl
+
+`--num_streams E` (E > 1) trains from E environments at once through `agent.VectorTrainer`: each tick stages the E raw
+frames in pinned memory, sends them to the device in one copy and makes one trainer step; `--num_train_frames` then
+counts the frames of all streams.  Evaluation, CSV rows and checkpoints are as with one stream.
 """
 import argparse
 import collections
 import itertools
+import math
 import os
 import sys
+import timeit
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
@@ -87,6 +93,62 @@ def build_train_agent(args, random_state, preprocessor):
   return agent_lib.AGENTS[kind](exploration_epsilon=epsilon, grad_error_bound=1.0 / 32, **common), network
 
 
+def train_streams(trainer, envs, num_frames, max_frames_per_episode):
+  """`num_frames` frames (rounded up to whole ticks) of E environments through `trainer`; returns the keys of
+  `reporting.EpisodeTracker` / `StepRateTracker` the CSV row reads, plus the mean `state_value` of the acting ticks.
+  The raw frames go to the device in one copy per tick, staged in pinned memory (double-buffered, so the staging of
+  tick t + 1 overlaps the copy of tick t)."""
+  import torch
+  from dqn_zoo_b200 import parts
+  E = len(envs)
+  first = [env.reset() for env in envs]
+  shape = first[0].observation[0].shape
+  stage = [torch.zeros((E,) + shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
+  frames = [torch.zeros((E,) + shape, dtype=torch.uint8, device='cuda') for _ in range(2)]
+  copied = [None, None]
+  trainer.reset()
+  timesteps = first
+  steps = np.zeros(E, np.int64)
+  returns, values = [], []
+  ticks = -(-num_frames // E)
+  t0 = timeit.default_timer()
+  for tick in range(ticks):
+    slot = tick % 2
+    if copied[slot] is not None:
+      copied[slot].synchronize()                 # the copy out of this staging buffer has finished
+    host = stage[slot].numpy()
+    for e, ts in enumerate(timesteps):
+      host[e] = ts.observation[0]
+    step_type = np.array([int(ts.step_type) for ts in timesteps], np.int64)
+    reward = np.array([np.nan if ts.reward is None else ts.reward for ts in timesteps])
+    discount = np.array([np.nan if ts.discount is None else ts.discount for ts in timesteps])
+    lives = np.array([ts.observation[1] for ts in timesteps], np.int64)
+    steps = np.where(step_type == int(parts.StepType.FIRST), 0, steps) + 1
+    if max_frames_per_episode > 0:               # run_loop's truncation: relabel the timestep LAST
+      step_type[steps > max_frames_per_episode] = int(parts.StepType.LAST)
+    frames[slot].copy_(stage[slot], non_blocking=True)
+    copied[slot] = torch.cuda.Event()
+    copied[slot].record()
+    actions = trainer.step(frames[slot], step_type, reward, discount, lives)
+    value = trainer.statistics['state_value']
+    if not math.isnan(value):
+      values.append(value)
+    last = step_type == int(parts.StepType.LAST)
+    if last.any():
+      returns.extend(trainer.episode_return[last].tolist())
+      trainer.reset(np.nonzero(last)[0])
+    timesteps = [envs[e].reset() if last[e] else envs[e].step(int(actions[e])) for e in range(E)]
+  duration = timeit.default_timer() - t0
+  running = float(trainer.episode_return.mean())
+  frames_done = ticks * E
+  return {
+      'episode_return': float(np.mean(returns)) if returns else (running if frames_done else math.nan),
+      'num_episodes': len(returns),
+      'step_rate': frames_done / duration if frames_done else math.nan,
+      'state_value': float(np.mean(values)) if values else math.nan,
+  }
+
+
 def main():
   ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
   ap.add_argument('--agent', default='dqn', choices=['dqn', 'double_q', 'prioritized', 'c51', 'qrdqn', 'rainbow', 'iqn'])
@@ -102,7 +164,10 @@ def main():
   ap.add_argument('--seed', type=int, default=1)
   ap.add_argument('--results_csv_path', default='')
   ap.add_argument('--checkpoint_path', default='')
+  ap.add_argument('--num_streams', type=int, default=1, help='E > 1: train from E environments with agent.VectorTrainer')
   args = ap.parse_args()
+  if args.num_streams < 1:
+    ap.error('--num_streams must be >= 1')
 
   import torch
   if not torch.cuda.is_available():
@@ -122,6 +187,10 @@ def main():
     return processors.atari(device_observations=True)
 
   train_agent, network = build_train_agent(args, random_state, preprocessor_builder())
+  trainer = None
+  if args.num_streams > 1:
+    trainer = agent_lib.VectorTrainer(train_agent, num_streams=args.num_streams,
+                                      rng_key=[0, int(random_state.randint(1, 2 ** 31))])
   eval_agent = agent_lib.EpsilonGreedyActor(preprocessor=preprocessor_builder(), network=network,
                                             exploration_epsilon=args.eval_exploration_epsilon,
                                             rng_key=[0, int(random_state.randint(1, 2 ** 31))])
@@ -129,7 +198,7 @@ def main():
   checkpoint = reporting.FileCheckpoint(args.checkpoint_path) if args.checkpoint_path else reporting.NullCheckpoint()
   state = checkpoint.state
   state.iteration = 0
-  state.train_agent = train_agent
+  state.train_agent = train_agent if trainer is None else trainer
   state.eval_agent = eval_agent
   state.random_state = random_state
   state.writer = writer
@@ -138,10 +207,14 @@ def main():
 
   while state.iteration <= args.num_iterations:
     env = environment_builder()          # a new environment per iteration: deterministic after a restore
-    train_seq = parts.run_loop(train_agent, env, args.max_frames_per_episode)
     num_train_frames = 0 if state.iteration == 0 else args.num_train_frames
-    train_stats = reporting.generate_statistics(reporting.make_default_trackers(train_agent),
-                                                itertools.islice(train_seq, num_train_frames))
+    if trainer is None:
+      train_seq = parts.run_loop(train_agent, env, args.max_frames_per_episode)
+      train_stats = reporting.generate_statistics(reporting.make_default_trackers(train_agent),
+                                                  itertools.islice(train_seq, num_train_frames))
+    else:
+      envs = [env] + [environment_builder() for _ in range(args.num_streams - 1)]
+      train_stats = train_streams(trainer, envs, num_train_frames, args.max_frames_per_episode)
     eval_agent.network_params = train_agent.learner      # device-to-device copy of the online parameters
     eval_seq = parts.run_loop(eval_agent, env, args.max_frames_per_episode)
     eval_stats = reporting.generate_statistics(reporting.make_default_trackers(eval_agent),
