@@ -132,6 +132,12 @@ _SIGNATURES = {
     'dz_actor_destroy': (None, [vp]),
     'dz_actor_act': (i32, [vp, vp, vp, vp, i64, vp, f32, vp, vp, vp]),
     'dz_actor_generate_randomness': (i32, [vp, u64, i32, vp, vp]),
+    'dz_actor_frozen_plan_query': (i32, [C.POINTER(LearnerConfig), i32, C.POINTER(i64)]),
+    'dz_actor_create_frozen': (i32, [vp, i32, vp, C.POINTER(vp)]),
+    'dz_actor_load_params': (i32, [vp, vp, vp]),
+    'dz_actor_get_params': (i32, [vp, vp, vp]),
+    'dz_actor_get_counter': (i32, [vp, C.POINTER(i64), vp]),
+    'dz_actor_set_counter': (i32, [vp, i64, vp]),
     'dz_test_actor_mma_path': (i32, [vp, C.c_char_p, C.POINTER(i32)]),
     'dz_test_actor_buffer': (i32, [vp, C.c_char_p, vp, vp]),
     'dz_learner_sync_target': (i32, [vp, vp]),

@@ -18,6 +18,7 @@ write-back], optionally replayed as a CUDA graph.  Nothing is read back per lear
 
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 from typing import Any, Callable, Mapping, Optional
 
@@ -846,6 +847,227 @@ class VectorTrainer:
     self._acc.set_state(state['accumulator'])
     self._statistics = dict(state['statistics'])
     self._q_pending = None
+    ret, length, count = state['episodes']
+    self._episode_return, self._episode_length, self._num_episodes = (np.array(ret), np.array(length),
+                                                                      np.array(count))
+
+
+class VectorEvaluator:
+  """Evaluates an agent on E environment streams: the evaluation phase of the run drivers (`eval_agent.network_params =
+  train_agent.online_params` + an epsilon-greedy actor, dqn/run_atari.py:250-290) as one tick of E timesteps, over a
+  frozen parameter snapshot.
+
+  `network_or_learner` is a `NetworkSpec` or a `Learner` with the network to evaluate; either only shapes the evaluator
+  (a learner's parameters are not read until `network_params` is set).  The evaluator owns a
+  `VectorizedAtariPreprocessor(E, device_observations=True)` and a frozen acting context (`Learner.actor(E,
+  frozen=True)`): its own parameter snapshot, weight images and generator counter, so evaluating neither reads the
+  training learner's live parameters nor shifts its noise or tau draws, and it may run beside training.  It always acts
+  through that context, at any E in [1, 1024] (IQN: E * tau_samples_policy <= 16384).
+
+  Tick contract (`step`): preprocess the E raw timesteps; if any stream emits a timestep, ONE act call for all E streams
+  at `exploration_epsilon`, with 2E host uniforms from a RandomState seeded by `rng_key` (as `BatchedEpsilonGreedyActor`)
+  when epsilon > 0; emitting streams take the new action, the others repeat their last one (RuntimeError if a stream
+  has none yet).  IQN draws E x tau_samples_policy taus and rainbow one noise apply (or, with `per_stream_noise`, one
+  per stream) per acting tick from the actor's counter.  The tick waits for its actions only.
+
+  `stream`: a `torch.cuda.Stream` on which all of the evaluator's device work is enqueued (e.g. to evaluate one
+  iteration while the next one trains on the default stream).  Setting `network_params` then enqueues the snapshot copy
+  on the caller's current stream, ordered after both the caller's earlier work and the evaluator's earlier acts, and
+  makes the evaluator's stream wait for it through an event."""
+
+  # the trainer's input checks and episode bookkeeping (they read only _E, _pre and the episode arrays)
+  _check = VectorTrainer._check
+  _track_episodes = VectorTrainer._track_episodes
+
+  def __init__(self, network_or_learner, num_streams: int, exploration_epsilon: float, rng_key,
+               per_stream_noise: bool = False, preprocessor_kwargs: Optional[Mapping[str, Any]] = None, stream=None):
+    E = int(num_streams)
+    if E < 1 or E > ACTOR_MAX_STREAMS:
+      raise ValueError('num_streams must be in [1, %d], got %d' % (ACTOR_MAX_STREAMS, E))
+    if isinstance(network_or_learner, learner_lib.Learner):
+      shape_learner = network_or_learner
+    elif isinstance(network_or_learner, NetworkSpec):
+      shape_learner = None
+    else:
+      raise TypeError('network_or_learner must be a NetworkSpec or a Learner')
+    net = network_or_learner.net if shape_learner is not None else network_or_learner
+    if net.kind == 'iqn' and E * net.tau_samples_policy > ACTOR_MAX_IQN_ROWS:
+      raise ValueError('iqn acting needs num_streams * tau_samples_policy <= %d, got %d * %d'
+                       % (ACTOR_MAX_IQN_ROWS, E, net.tau_samples_policy))
+    if per_stream_noise and net.kind != 'rainbow':
+      raise ValueError('per_stream_noise needs a rainbow network')
+    kwargs = dict(preprocessor_kwargs or {})
+    if not kwargs.pop('device_observations', True):
+      raise ValueError('the evaluator keeps its frame stacks on the device: device_observations must be True')
+    self._stream = stream
+    self._E = E
+    self._net = net
+    self._epsilon = float(exploration_epsilon)
+    self._per_stream_noise = bool(per_stream_noise)
+    seed = int(np.asarray(rng_key).reshape(-1)[-1]) & 0x7FFFFFFF
+    self._rng = np.random.RandomState(seed)
+    self._seed = seed
+    with self._on_stream():
+      if shape_learner is None:            # the frozen actor takes only the configuration; the learner is dropped
+        shape_learner = learner_lib.Learner(net)
+      kwargs.setdefault('device', shape_learner.device)
+      self._actor = shape_learner.actor(E, frozen=True)
+      self._pre = processors.VectorizedAtariPreprocessor(E, device_observations=True, **kwargs)
+      self._explore_host = torch.zeros((2, E), dtype=torch.float32).pin_memory()
+      self._explore_dev = torch.zeros((2, E), dtype=torch.float32, device=shape_learner.device)
+      self._actions_host = torch.zeros(E, dtype=torch.int32).pin_memory()
+    del shape_learner
+    self._actions = np.zeros(E, np.int32)
+    self._has_action = np.zeros(E, bool)
+    self._episode_return = np.zeros(E)
+    self._episode_length = np.zeros(E, np.int64)
+    self._num_episodes = np.zeros(E, np.int64)
+
+  def _on_stream(self):
+    return torch.cuda.stream(self._stream) if self._stream is not None else contextlib.nullcontext()
+
+  # -- the snapshot ---------------------------------------------------------------------------------------------------
+  @property
+  def network_params(self):
+    """The snapshot as an `hk.Params`-shaped dict of host arrays (None before it is set)."""
+    if not self._actor.loaded:
+      return None
+    with self._on_stream():
+      flat = self._actor.get_params()
+    out = {}
+    for name, value in flat.items():
+      mod, leaf = learner_lib.haiku_name(name, self._net.kind)
+      out.setdefault(mod, {})[leaf] = value
+    return out
+
+  @network_params.setter
+  def network_params(self, params) -> None:
+    """`EpsilonGreedyActor.network_params`'s inputs: a `Learner` (one device-to-device copy of its online parameters),
+    an `hk.Params`-shaped dict or a flat {canonical_name: array} dict.  None leaves the evaluator without parameters."""
+    if params is None:
+      self._actor.loaded = False
+      return
+    if self._stream is None:
+      self._actor.load_params(params)
+      return
+    caller = torch.cuda.current_stream()
+    caller.wait_stream(self._stream)       # the evaluator's enqueued acts read the previous snapshot
+    self._actor.load_params(params)
+    done = torch.cuda.Event()
+    done.record(caller)
+    self._stream.wait_event(done)
+
+  # -- one tick -------------------------------------------------------------------------------------------------------
+  def step(self, frames, step_type, reward, discount, lives) -> np.ndarray:
+    """`VectorTrainer.step`'s arguments: frames uint8 [E, H, W, 3] raw RGB (device tensor, or host array: one H2D copy);
+    step_type int [E]; reward / discount float [E] with NaN for None (FIRST timesteps); lives int [E].  Returns the E
+    actions, int32 [E]."""
+    if not self._actor.loaded:
+      raise RuntimeError('network_params have not been set.')
+    step_type, reward, discount, lives = self._check(frames, step_type, reward, discount, lives)
+    with self._on_stream():
+      out = self._pre.step_arrays(frames, step_type, reward, discount, lives)
+      self._track_episodes(step_type, reward)
+      emit = out['emit']
+      if np.any(~emit & ~self._has_action):
+        raise RuntimeError('Cannot repeat if action has never been selected.')
+      if emit.any():
+        new = self._act()
+        self._actions = np.where(emit, new, self._actions).astype(np.int32)
+        self._has_action |= emit
+    return self._actions.copy()
+
+  def _act(self) -> np.ndarray:
+    A = self._actor
+    explore = None
+    if self._epsilon > 0.0:
+      self._explore_host.copy_(torch.from_numpy(self._rng.uniform(size=(2, self._E)).astype(np.float32)))
+      self._explore_dev.copy_(self._explore_host, non_blocking=True)
+      explore = self._explore_dev
+    taus = noise = stream_noise = None
+    if self._per_stream_noise:
+      stream_noise = A.generate_randomness(self._seed, per_stream=True)
+    elif self._net.kind == 'iqn':
+      taus = A.generate_randomness(self._seed)
+    elif self._net.kind == 'rainbow':
+      noise = A.generate_randomness(self._seed)
+    actions, _ = A.act(self._pre.stacks, epsilon=self._epsilon, explore=explore, taus=taus, noise=noise,
+                       stream_noise=stream_noise)
+    self._actions_host.copy_(actions, non_blocking=True)
+    torch.cuda.current_stream().synchronize()   # also frees the pinned uniforms for the next tick
+    return self._actions_host.numpy().copy()
+
+  def reset(self, streams=None) -> None:
+    """`Agent.reset` for every stream, or for one stream or a sequence of streams (e.g. those whose last timestep was
+    LAST): their preprocessor state and their last action."""
+    with self._on_stream():
+      if streams is None:
+        self._pre.reset()
+        self._has_action[:] = False
+        return
+      for e in np.atleast_1d(np.asarray(streams, np.int64)):
+        self._pre.reset(int(e))
+        self._has_action[e] = False
+
+  # -- surface --------------------------------------------------------------------------------------------------------
+  @property
+  def num_streams(self) -> int:
+    return self._E
+
+  @property
+  def actor(self) -> learner_lib.Actor:
+    """The frozen acting context."""
+    return self._actor
+
+  @property
+  def stream(self):
+    return self._stream
+
+  @property
+  def statistics(self) -> Mapping[str, float]:
+    return {}
+
+  @property
+  def episode_return(self) -> np.ndarray:
+    """Per stream: the summed raw rewards of its current episode (after a LAST timestep: of the episode it ended)."""
+    return self._episode_return.copy()
+
+  @property
+  def episode_length(self) -> np.ndarray:
+    """Per stream: the timesteps of its current episode, FIRST included (after LAST: of the episode it ended)."""
+    return self._episode_length.copy()
+
+  @property
+  def num_episodes(self) -> np.ndarray:
+    """Per stream: the episodes it has completed (LAST timesteps seen)."""
+    return self._num_episodes.copy()
+
+  def get_state(self) -> Mapping[str, Any]:
+    """The snapshot, the actor's generator counter, the exploration RandomState, the preprocessor, the last actions and
+    the episode statistics: a restored evaluator continues bit for bit."""
+    with self._on_stream():
+      return {
+          'network_params': self._actor.get_params() if self._actor.loaded else None,
+          'counter': self._actor.counter,
+          'rng': self._rng.get_state(),
+          'seed': self._seed,
+          'preprocessor': self._pre.get_state(),
+          'actions': self._actions.copy(),
+          'has_action': self._has_action.copy(),
+          'episodes': (self._episode_return.copy(), self._episode_length.copy(), self._num_episodes.copy()),
+      }
+
+  def set_state(self, state: Mapping[str, Any]) -> None:
+    if np.shape(state['actions']) != (self._E,):
+      raise ValueError('state is for %d streams, this evaluator has %d' % (len(state['actions']), self._E))
+    self.network_params = state['network_params']
+    with self._on_stream():
+      self._actor.counter = int(state['counter'])
+      self._pre.set_state(state['preprocessor'])
+    self._rng.set_state(state['rng'])
+    self._seed = int(state['seed'])
+    self._actions = np.array(state['actions'], np.int32)
+    self._has_action = np.array(state['has_action'], bool)
     ret, length, count = state['episodes']
     self._episode_return, self._episode_length, self._num_episodes = (np.array(ret), np.array(length),
                                                                       np.array(count))

@@ -2674,16 +2674,26 @@ int dz_learner_generate_stream_noise(dz_learner* l, uint64_t seed, int32_t E, fl
 // place (an act enqueued after a learner step on the same stream sees that step's parameters).  Its buffers are sized
 // for its stream count; the torso and the 3136 -> 512 layer run on a forward-only tensor-core plan where the geometry
 // allows it.
+//
+// A frozen actor (dz_actor_create_frozen) acts on a parameter snapshot of its own instead: P floats in the learner's
+// layout inside its workspace, loaded by dz_actor_load_params, which also packs the conv weight images once.  It draws
+// its randomness from a counter of its own, and its `l` is a shape-only learner (configuration, layout, offsets, dims
+// and split counts; every device pointer NULL), so its act and randomness paths read and write nothing but its
+// workspace, the caller's buffers and its plan's constant tables.
 // ------------------------------------------------------------------------------------------------
 
 struct dz_actor {
-  dz_learner* l;
+  dz_learner* l;               // live: the learner; frozen: a shape-only learner the actor owns
   int E;                       // streams
   NetBufs b;                   // activation set / head pass 1, as the learner's act_batch
   const uint8_t** rows;        // [E] observation row table
   float* noise;                // rainbow: the apply the tensor-core noisy1 reads (a copy of the caller's shared apply)
   UmNet* um;                   // forward-only tensor-core plan (nullptr: fp32-FMA torso)
   char* um_ws;
+  bool frozen = false;
+  bool loaded = false;         // frozen: dz_actor_load_params has run
+  float* params = nullptr;     // frozen: the parameter snapshot, [P] in the learner's layout
+  int64_t* counters = nullptr; // frozen: [2]; [1] is the generator counter (the slot randomness_kernel reads)
 };
 
 namespace {
@@ -2697,9 +2707,11 @@ int actor_check(const dz_learner_config& c, int E) {
   return DZ_OK;
 }
 
-UmNetDesc actor_um_desc(const dz_learner* l, int E) {
+// online: the parameter blob the plan's conv / fc tensor maps, bias reads and weight packing use.
+UmNetDesc actor_um_desc(const dz_learner* l, int E, const float* online) {
   UmNetDesc u = make_um_desc(l);
   u.B = E; u.npass = 1; u.fwd_only = 1;
+  u.online = online;
   u.pass_target[0] = 0; u.target = nullptr;
   for (int p = 0; p < 3; ++p) u.noise_apply[p] = 0;
   return u;
@@ -2714,7 +2726,7 @@ int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
   Bump w{base};
   NetBufs& b = a->b;
   memset(&b, 0, sizeof(b));   // split_rows 0: the fp32 GEMMs never split K, so row e's sums do not depend on E
-  const UmNetDesc ud = actor_um_desc(l, E);
+  const UmNetDesc ud = actor_um_desc(l, E, nullptr);   // sizes only
   const bool um = um_net_supported(ud);
   a->um_ws = um ? w.take<char>(um_net_workspace_bytes(ud)) : nullptr;
   if (!um) {
@@ -2734,39 +2746,54 @@ int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
   b.hi[1] = iqn ? w.take<float>(rows * d.feat) : nullptr;
   a->rows = w.take<const uint8_t*>(E);
   a->noise = rb ? w.take<float>(noise_layout(c, d).stride) : nullptr;
+  if (a->frozen) {
+    a->params = w.take<float>(l->lay.total);
+    a->counters = w.take<int64_t>(2);
+  }
   return w.used;
 }
 
-}  // namespace
+// A learner with cfg's configuration, layout, parameter offsets, dims and split counts and no device state: carve()
+// without a base leaves every workspace pointer NULL.
+int init_shape_learner(dz_learner* t, const dz_learner_config& cfg) {
+  t->um = nullptr;
+  memset(&t->buf, 0, sizeof(t->buf));
+  t->cfg = cfg;
+  t->lay = make_layout(cfg);
+  DZ_TRY(param_offsets(cfg, t->lay, &t->po));
+  t->d = make_dims(cfg);
+  t->B = cfg.batch;
+  carve(t, nullptr);                     // the learner's split counts, which the actor's fp32 GEMMs share
+  return DZ_OK;
+}
 
-int dz_actor_plan_query(const dz_learner_config* cfg, int32_t num_streams, int64_t* workspace_bytes) {
+int actor_plan_bytes(const dz_learner_config* cfg, int32_t num_streams, bool frozen, int64_t* workspace_bytes) {
   if (!cfg || !workspace_bytes) return fail(DZ_EINVAL, "actor plan query: null argument");
   DZ_TRY(validate(*cfg));
   DZ_TRY(actor_check(*cfg, num_streams));
   dz_learner tmp;
-  tmp.um = nullptr;
-  memset(&tmp.buf, 0, sizeof(tmp.buf));
-  tmp.cfg = *cfg;
-  tmp.lay = make_layout(*cfg);
-  DZ_TRY(param_offsets(*cfg, tmp.lay, &tmp.po));
-  tmp.d = make_dims(*cfg);
-  tmp.B = cfg->batch;
-  carve(&tmp, nullptr);                  // the learner's split counts, which the actor's fp32 GEMMs share
+  DZ_TRY(init_shape_learner(&tmp, *cfg));
   dz_actor a;
   a.E = num_streams;
+  a.frozen = frozen;
   *workspace_bytes = carve_actor(&a, &tmp, nullptr);
   return DZ_OK;
 }
 
-int dz_actor_create(dz_learner* l, int32_t num_streams, void* d_workspace, dz_actor** out) {
-  if (!l || !d_workspace || !out) return fail(DZ_EINVAL, "actor create: null argument");
-  DZ_TRY(actor_check(l->cfg, num_streams));
+// l: the learner (live) or a shape-only learner the actor takes over (frozen).
+int actor_create(dz_learner* l, bool frozen, int32_t num_streams, void* d_workspace, dz_actor** out) {
   dz_actor* a = new dz_actor();
   a->l = l;
   a->E = num_streams;
+  a->frozen = frozen;
   carve_actor(a, l, static_cast<char*>(d_workspace));
+  if (frozen) {
+    cudaError_t e = cudaMemsetAsync(a->counters, 0, 2 * sizeof(int64_t), 0);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(0);
+    if (e != cudaSuccess) { dz_actor_destroy(a); return fail(DZ_ECUDA, "frozen actor: counter init: %s", cudaGetErrorString(e)); }
+  }
   if (a->um_ws) {
-    int rc = um_net_create(actor_um_desc(l, num_streams), a->um_ws, &a->um);
+    int rc = um_net_create(actor_um_desc(l, num_streams, frozen ? a->params : l->buf.d_online), a->um_ws, &a->um);
     if (rc == DZ_OK && a->noise) rc = um_bind_noise(a->um, a->noise);
     if (rc != DZ_OK) { dz_actor_destroy(a); return rc; }
     for (int L = 1; L <= 3; ++L) (L == 1 ? a->b.act1 : L == 2 ? a->b.act2 : a->b.act3)[1] = um_act_f32(a->um, L, 0);
@@ -2777,10 +2804,75 @@ int dz_actor_create(dz_learner* l, int32_t num_streams, void* d_workspace, dz_ac
   return DZ_OK;
 }
 
+}  // namespace
+
+int dz_actor_plan_query(const dz_learner_config* cfg, int32_t num_streams, int64_t* workspace_bytes) {
+  return actor_plan_bytes(cfg, num_streams, false, workspace_bytes);
+}
+
+int dz_actor_frozen_plan_query(const dz_learner_config* cfg, int32_t num_streams, int64_t* workspace_bytes) {
+  return actor_plan_bytes(cfg, num_streams, true, workspace_bytes);
+}
+
+int dz_actor_create(dz_learner* l, int32_t num_streams, void* d_workspace, dz_actor** out) {
+  if (!l || !d_workspace || !out) return fail(DZ_EINVAL, "actor create: null argument");
+  DZ_TRY(actor_check(l->cfg, num_streams));
+  return actor_create(l, false, num_streams, d_workspace, out);
+}
+
+int dz_actor_create_frozen(dz_learner* l, int32_t num_streams, void* d_workspace, dz_actor** out) {
+  if (!l || !d_workspace || !out) return fail(DZ_EINVAL, "frozen actor create: null argument");
+  DZ_TRY(actor_check(l->cfg, num_streams));
+  dz_learner* shape = new dz_learner();
+  const int rc = init_shape_learner(shape, l->cfg);
+  if (rc != DZ_OK) { delete shape; return rc; }
+  return actor_create(shape, true, num_streams, d_workspace, out);   // on failure the actor's destroy frees shape
+}
+
 void dz_actor_destroy(dz_actor* a) {
   if (!a) return;
   um_net_destroy(a->um);
+  if (a->frozen) delete a->l;
   delete a;
+}
+
+// Frozen actor: snapshot <- d_src (a full parameter blob in the learner's layout, e.g. its online blob), then the conv
+// weight images of the tensor-core plan are packed from the snapshot, once.  Both are enqueued on `stream`.
+int dz_actor_load_params(dz_actor* a, const float* d_src, void* stream) {
+  if (!a || !d_src) return fail(DZ_EINVAL, "actor load_params: null argument");
+  if (!a->frozen) return fail(DZ_EINVAL, "load_params: a live actor reads the learner's parameters in place (create a frozen actor)");
+  DZ_CUDA_OK(cudaMemcpyAsync(a->params, d_src, a->l->lay.total * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  if (a->um) DZ_TRY(um_pack_weights(a->um, stream));
+  a->loaded = true;
+  return DZ_OK;
+}
+
+// Frozen actor: d_dst <- the snapshot (P floats), enqueued on `stream`.
+int dz_actor_get_params(dz_actor* a, float* d_dst, void* stream) {
+  if (!a || !d_dst) return fail(DZ_EINVAL, "actor get_params: null argument");
+  if (!a->frozen || !a->loaded) return fail(DZ_EINVAL, "get_params: the actor holds no parameter snapshot");
+  DZ_CUDA_OK(cudaMemcpyAsync(d_dst, a->params, a->l->lay.total * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return DZ_OK;
+}
+
+// Frozen actor: its generator counter, read after the work enqueued on `stream` (which this call waits for).
+int dz_actor_get_counter(dz_actor* a, int64_t* out, void* stream) {
+  if (!a || !out) return fail(DZ_EINVAL, "actor get_counter: null argument");
+  if (!a->frozen) return fail(DZ_EINVAL, "get_counter: a live actor advances the learner's counter");
+  int64_t v = 0;
+  DZ_CUDA_OK(cudaMemcpyAsync(&v, a->counters + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  DZ_CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream));
+  *out = v;
+  return DZ_OK;
+}
+
+// Frozen actor: sets its generator counter, ordered on `stream` (the call returns once the value is staged).
+int dz_actor_set_counter(dz_actor* a, int64_t value, void* stream) {
+  if (!a) return fail(DZ_EINVAL, "actor set_counter: null handle");
+  if (!a->frozen) return fail(DZ_EINVAL, "set_counter: a live actor advances the learner's counter");
+  DZ_CUDA_OK(cudaMemcpyAsync(a->counters + 1, &value, sizeof(int64_t), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  DZ_CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream));
+  return DZ_OK;
 }
 
 // dz_learner_act_batch's contract for the actor's num_streams observations.  noise_ld (rainbow): 0, d_noise is one
@@ -2799,13 +2891,14 @@ int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const f
   const int64_t stride = rb ? noise_layout(c, l->d).stride : 0;
   if (noise_ld != 0 && (!rb || noise_ld != stride))
     return fail(DZ_EINVAL, "actor: noise_ld must be 0 (one shared apply) or the noise stride (rainbow, one apply per stream)");
-  const float* on = l->buf.d_online;
+  if (a->frozen && !a->loaded) return fail(DZ_EINVAL, "frozen actor: no parameters loaded (dz_actor_load_params)");
+  const float* on = a->frozen ? a->params : l->buf.d_online;
   const long long obs_bytes = (long long)l->d.H * l->d.W * l->d.C;
   DZ_LAUNCH(make_row_table_kernel, (unsigned)ceil_div(E, 64), 64, 0, stream, d_obs, obs_bytes, E, a->rows);
   const bool fc_done = a->um && c.kind != DZ_IQN && noise_ld == 0;
   if (a->um) {
     const uint8_t* const* rows[3] = {a->rows, nullptr, nullptr};
-    DZ_TRY(um_pack_weights(a->um, stream));
+    if (!a->frozen) DZ_TRY(um_pack_weights(a->um, stream));   // frozen: packed by load_params
     DZ_TRY(um_forward_torso(a->um, rows, stream));
     if (fc_done) {
       if (rb) DZ_CUDA_OK(cudaMemcpyAsync(a->noise, d_noise, stride * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
@@ -2837,7 +2930,8 @@ int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const f
 
 // The actor's randomness from the learner's generator and counter: iqn taus [E][tau_samples_policy] (the stream id of
 // dz_learner_generate_randomness's taus); rainbow one noise apply, or E applies when per_stream is set (the stream id of
-// its noise and of dz_learner_generate_stream_noise).  Advances d_counters[1] once.
+// its noise and of dz_learner_generate_stream_noise).  Advances d_counters[1] once.  A frozen actor draws the same way
+// from its own counter and never touches the learner's.
 int dz_actor_generate_randomness(dz_actor* a, uint64_t seed, int32_t per_stream, float* d_out, void* stream) {
   if (!a || !d_out) return fail(DZ_EINVAL, "actor randomness: null argument");
   const dz_learner_config& c = a->l->cfg;
@@ -2846,9 +2940,10 @@ int dz_actor_generate_randomness(dz_actor* a, uint64_t seed, int32_t per_stream,
   else if (c.kind == DZ_RAINBOW) n = (per_stream ? (long long)a->E : 1LL) * noise_layout(c, a->l->d).stride;
   else return fail(DZ_EINVAL, "actor randomness: iqn draws taus, rainbow noise (per_stream: rainbow only); other kinds draw nothing");
   const int kind = c.kind == DZ_IQN ? 0 : 1;
-  DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_out, n, seed, a->l->buf.d_counters, kind,
+  int64_t* counters = a->frozen ? a->counters : a->l->buf.d_counters;
+  DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_out, n, seed, counters, kind,
             c.kind == DZ_IQN ? 1u : 2u);
-  DZ_LAUNCH(bump_counter_kernel, 1, 1, 0, stream, a->l->buf.d_counters, 1);
+  DZ_LAUNCH(bump_counter_kernel, 1, 1, 0, stream, counters, 1);
   return DZ_OK;
 }
 

@@ -334,9 +334,11 @@ class Learner:
     self._keep_act = (obs, t, n, x)
     return self._act_a[:E], self._act_q[:E]
 
-  def actor(self, num_streams: int) -> 'Actor':
-    """An acting context for `num_streams` streams (not capped by batch_size) over this learner's online parameters."""
-    return Actor(self, num_streams)
+  def actor(self, num_streams: int, frozen: bool = False) -> 'Actor':
+    """An acting context for `num_streams` streams (not capped by batch_size) over this learner's online parameters.
+    `frozen=True`: over a parameter snapshot of its own (`Actor.load_params`) with a generator counter of its own; it
+    touches no device state of this learner."""
+    return Actor(self, num_streams, frozen=frozen)
 
   # -- fused sample -> update -> priority write-back -------------------------------------------------
   def make_learn_io(self, stage: torch.Tensor, prioritized: bool, priority_exponent: float):
@@ -381,25 +383,43 @@ class Actor:
   call, over the learner's online parameters read in place: an act enqueued after `learn()` / `update()` on the stream
   sees their parameters, with no copy.  Its buffers are sized for its streams, so one learner of any batch size can act
   for many environments.  On the tensor-core geometries (84x84x4 among them) the torso and the 3136 -> 512 layer run
-  on the learner's sm_90a tensor-core kernels.  Row e's result does not depend on num_streams."""
+  on the learner's sm_90a tensor-core kernels.  Row e's result does not depend on num_streams.
 
-  def __init__(self, learner: Learner, num_streams: int):
+  A frozen actor (`Learner.actor(E, frozen=True)`) acts on a snapshot of its own instead, taken by `load_params` (which
+  also packs the tensor-core weight images once), and draws its randomness from a counter of its own (`counter`).  It
+  keeps no reference to the learner and touches none of its device state, so it can act on another CUDA stream while
+  the learner trains, and the learner's next draws do not depend on it.  For the same parameters and randomness inputs
+  its outputs equal a live actor's bit for bit."""
+
+  def __init__(self, learner: Learner, num_streams: int, frozen: bool = False):
     E = int(num_streams)
+    self.frozen = bool(frozen)
     nbytes = C.c_int64()
-    _lib.call('dz_actor_plan_query', C.byref(learner.cfg), E, C.byref(nbytes))
-    self.learner = learner          # the actor reads the learner's parameters: keep it alive for the actor's lifetime
+    _lib.call('dz_actor_frozen_plan_query' if self.frozen else 'dz_actor_plan_query', C.byref(learner.cfg), E,
+              C.byref(nbytes))
+    # a live actor reads the learner's parameters: keep it alive for the actor's lifetime
+    self.learner = None if self.frozen else learner
     self.num_streams = E
+    self.net, self.kind, self.device = learner.net, learner.kind, learner.device
+    self.obs_bytes, self.noise_stride = learner.obs_bytes, learner.noise_stride
+    self.tensors = dict(learner.tensors)
+    self.param_count = int(learner.plan.param_count)
     dev = learner.device
     net = learner.net
+    # zero-filled: the tensor-core plan reads padding rows of its operand images that no launch writes
     self.workspace = torch.zeros(nbytes.value, dtype=torch.uint8, device=dev)
+    if self.frozen:
+      torch.cuda.current_stream().synchronize()   # create zeroes the counter on the legacy stream: after the fill
     self.q = torch.zeros((E, net.num_actions), dtype=torch.float32, device=dev)
     self.actions = torch.zeros(E, dtype=torch.int32, device=dev)
     self.taus = torch.zeros((E, net.tau_samples_policy), dtype=torch.float32, device=dev) if net.kind == 'iqn' else None
     rb = net.kind == 'rainbow'
     self.noise = torch.zeros(learner.noise_stride, dtype=torch.float32, device=dev) if rb else None
     self.stream_noise = torch.zeros((E, learner.noise_stride), dtype=torch.float32, device=dev) if rb else None
+    self.loaded = False
     handle = C.c_void_p()
-    _lib.call('dz_actor_create', learner._h, E, self.workspace.data_ptr(), C.byref(handle))
+    _lib.call('dz_actor_create_frozen' if self.frozen else 'dz_actor_create', learner._h, E, self.workspace.data_ptr(),
+              C.byref(handle))
     self._h = handle
 
   def __del__(self):
@@ -407,11 +427,83 @@ class Actor:
     if h:
       _lib.lib.dz_actor_destroy(h)
 
+  # -- frozen actors: the parameter snapshot and the generator counter ------------------------------------------------
+  def _need_frozen(self, what):
+    if not self.frozen:
+      raise ValueError('%s needs a frozen actor (Learner.actor(E, frozen=True)); a live actor reads the learner in place'
+                       % what)
+
+  def flat_params(self, params) -> Dict[str, np.ndarray]:
+    """An `hk.Params`-shaped {module: {leaf: array}} or flat {canonical_name: array} dict as a flat dict."""
+    flat = {}
+    for key, value in params.items():
+      if isinstance(value, Mapping):
+        for leaf, arr in value.items():
+          names = [n for n in self.tensors if haiku_name(n, self.kind) == (key, leaf)]
+          if not names:
+            raise KeyError('unknown parameter %s/%s' % (key, leaf))
+          flat[names[0]] = arr
+      else:
+        flat[key] = value
+    return flat
+
+  def load_params(self, source) -> None:
+    """Takes a snapshot: `source` is a `Learner` with this network (one device-to-device copy of its online blob, ordered
+    after the work already enqueued on the current stream), an `hk.Params`-shaped dict or a flat {canonical_name: array}
+    dict naming every tensor.  Enqueued on the current stream, with the packing of the tensor-core weight images."""
+    self._need_frozen('load_params')
+    if isinstance(source, Learner):
+      if source.kind != self.kind or source.tensors != self.tensors or source.net.obs_shape != self.net.obs_shape:
+        raise ValueError('the learner\'s network does not match this actor\'s')
+      src = source.online
+    else:
+      flat = self.flat_params(source)
+      missing = sorted(set(self.tensors) - set(flat))
+      if missing:
+        raise KeyError('parameters missing: %s' % ', '.join(missing))
+      blob = np.zeros(self.param_count, np.float32)
+      for name, (off, shape) in self.tensors.items():
+        value = np.asarray(flat[name], dtype=np.float32)
+        if value.shape != tuple(shape):
+          raise ValueError('%s has shape %s, expected %s' % (name, value.shape, tuple(shape)))
+        blob[off:off + value.size] = value.reshape(-1)
+      src = torch.from_numpy(blob).to(self.device)
+    _lib.call('dz_actor_load_params', self._h, src.data_ptr(), _cstream())
+    self._keep_load = src
+    self.loaded = True
+
+  def params(self) -> torch.Tensor:
+    """A device copy of the snapshot ([P] float32 in the learner's layout), made on the current stream."""
+    self._need_frozen('params')
+    out = torch.empty(self.param_count, dtype=torch.float32, device=self.device)
+    _lib.call('dz_actor_get_params', self._h, out.data_ptr(), _cstream())
+    return out
+
+  def get_params(self) -> Dict[str, np.ndarray]:
+    """The snapshot as a flat {canonical_name: array} dict of host arrays."""
+    blob = self.params().cpu().numpy()
+    return {name: blob[off:off + int(np.prod(shape))].reshape(shape).copy() for name, (off, shape) in self.tensors.items()}
+
+  @property
+  def counter(self) -> int:
+    """A frozen actor's generator counter (0 at creation; each `generate_randomness` advances it by one), read after
+    the work enqueued on the current stream."""
+    self._need_frozen('counter')
+    v = C.c_int64()
+    _lib.call('dz_actor_get_counter', self._h, C.byref(v), _cstream())
+    return int(v.value)
+
+  @counter.setter
+  def counter(self, value: int) -> None:
+    self._need_frozen('counter')
+    _lib.call('dz_actor_set_counter', self._h, int(value), _cstream())
+
   def generate_randomness(self, seed: int, per_stream: bool = False) -> torch.Tensor:
     """Fills and returns `.taus` (IQN, [E, tau_samples_policy]), `.noise` (rainbow, one apply) or, with `per_stream`,
-    `.stream_noise` (rainbow, [E, noise_stride]) from the learner's generator, advancing its counter once.  For E <=
-    batch_size the draws equal `Learner.generate_randomness` / `generate_stream_noise` at the same seed and counter."""
-    kind = self.learner.kind
+    `.stream_noise` (rainbow, [E, noise_stride]) from the learner's generator, advancing its counter once (a frozen
+    actor: its own counter).  For E <= batch_size the draws equal `Learner.generate_randomness` /
+    `generate_stream_noise` at the same seed and counter."""
+    kind = self.kind
     if per_stream and kind != 'rainbow':
       raise ValueError('per_stream randomness needs a rainbow learner')
     if kind not in ('iqn', 'rainbow'):
@@ -425,12 +517,14 @@ class Actor:
     uniforms (None: greedy), IQN `taus` [E, tau_samples_policy], rainbow `noise` (one apply shared by the streams) or
     `stream_noise` [E, noise_stride].  Returns (actions int32 [E], q_values float32 [E, num_actions]) device tensors,
     overwritten by the next call."""
-    L = self.learner
+    L = self                        # network shape and device, as the learner's
     E = self.num_streams
     obs = torch.as_tensor(obs_u8, device=L.device).contiguous()
     if obs.dtype != torch.uint8 or obs.dim() < 1 or obs.shape[0] != E or obs[0].numel() != L.obs_bytes:
       raise ValueError('obs must be uint8 [%d, %s], got %s %s' % (E, ', '.join(map(str, L.net.obs_shape)), obs.dtype,
                                                                   tuple(obs.shape)))
+    if self.frozen and not self.loaded:
+      raise RuntimeError('the frozen actor has no parameters: call load_params first')
     x = None if explore is None else torch.as_tensor(explore, device=L.device).to(torch.float32).contiguous()
     if x is not None and x.numel() != 2 * E:
       raise ValueError('explore must be [2, %d], got %s' % (E, tuple(x.shape)))

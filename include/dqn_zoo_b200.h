@@ -417,6 +417,27 @@ int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const f
  * other kinds, per_stream on iqn or a NULL buffer. */
 int dz_actor_generate_randomness(dz_actor* a, uint64_t seed, int32_t per_stream, float* d_out, void* stream);
 
+/* ---- Frozen acting context (evaluation over a parameter snapshot) -------------------------------------------------
+ * The acting context above with its own state: a snapshot of P parameter floats in the learner's layout and a generator
+ * counter, both inside its workspace.  The learner handle supplies only the configuration, layout, dims and split
+ * counts (the actor keeps a copy of them, not the handle: the learner may be destroyed first).  Acting, randomness and
+ * loading read and write only the actor's workspace, the caller's buffers and constant tables, never a learner's device
+ * state, so a frozen actor can act on another CUDA stream while a learner trains.  dz_actor_act and
+ * dz_actor_generate_randomness take a frozen actor with the same contract; act fails (DZ_EINVAL) before the first
+ * load_params.  The live-only calls below fail on a live actor. */
+/* Device workspace bytes of a frozen actor; the workspace must be zero-filled before dz_actor_create_frozen, as a live
+ * actor's. */
+int dz_actor_frozen_plan_query(const dz_learner_config* cfg, int32_t num_streams, int64_t* workspace_bytes);
+int dz_actor_create_frozen(dz_learner* l, int32_t num_streams, void* d_workspace, dz_actor** out);
+/* snapshot <- d_src (P floats, e.g. a learner's online blob), then the conv weight images are packed once; on stream. */
+int dz_actor_load_params(dz_actor* a, const float* d_src, void* stream);
+/* d_dst <- the snapshot (P floats), on stream.  DZ_EINVAL before the first load_params. */
+int dz_actor_get_params(dz_actor* a, float* d_dst, void* stream);
+/* The generator counter (0 at creation; each generate_randomness advances it once), ordered on stream (both calls
+ * synchronise with it). */
+int dz_actor_get_counter(dz_actor* a, int64_t* out, void* stream);
+int dz_actor_set_counter(dz_actor* a, int64_t value, void* stream);
+
 /* target <- online (dqn/agent.py:155-156): device-to-device copy of the blob. */
 int dz_learner_sync_target(dz_learner* l, void* stream);
 

@@ -10,7 +10,13 @@ sequence of calls is what tests/test_gpu_agent.py::test_train_eval_iteration_wit
 
 `--num_streams E` (E > 1) trains from E environments at once through `agent.VectorTrainer`: each tick stages the E raw
 frames in pinned memory, sends them to the device in one copy and makes one trainer step; `--num_train_frames` then
-counts the frames of all streams.  Evaluation, CSV rows and checkpoints are as with one stream.
+counts the frames of all streams.
+
+`--num_eval_streams E` evaluates on E environments of their own through `agent.VectorEvaluator` (a frozen parameter
+snapshot taken after each training phase); `--num_eval_frames` then counts the frames of all evaluation streams.  Both
+phases share `StreamLoop`'s truncation and episode bookkeeping.  `--overlap_eval` (with `--num_streams` > 1) runs
+iteration i's evaluation on its own CUDA stream, one tick after each training tick of iteration i + 1; every column of
+the CSV rows but the rates is as without it.  CSV columns and checkpoints are otherwise as with one stream.
 """
 import argparse
 import collections
@@ -93,63 +99,122 @@ def build_train_agent(args, random_state, preprocessor):
   return agent_lib.AGENTS[kind](exploration_epsilon=epsilon, grad_error_bound=1.0 / 32, **common), network
 
 
-def train_streams(trainer, envs, num_frames, max_frames_per_episode):
-  """`num_frames` frames (rounded up to whole ticks) of E environments through `trainer`; returns the keys of
-  `reporting.EpisodeTracker` / `StepRateTracker` the CSV row reads, plus the mean `state_value` of the acting ticks.
-  The raw frames go to the device in one copy per tick, staged in pinned memory (double-buffered, so the staging of
-  tick t + 1 overlaps the copy of tick t)."""
-  import torch
-  from dqn_zoo_b200 import parts
-  E = len(envs)
-  first = [env.reset() for env in envs]
-  shape = first[0].observation[0].shape
-  stage = [torch.zeros((E,) + shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
-  frames = [torch.zeros((E,) + shape, dtype=torch.uint8, device='cuda') for _ in range(2)]
-  copied = [None, None]
-  trainer.reset()
-  timesteps = first
-  steps = np.zeros(E, np.int64)
-  returns, values = [], []
-  ticks = -(-num_frames // E)
-  t0 = timeit.default_timer()
-  for tick in range(ticks):
-    slot = tick % 2
-    if copied[slot] is not None:
-      copied[slot].synchronize()                 # the copy out of this staging buffer has finished
-    host = stage[slot].numpy()
+class StreamLoop:
+  """E environments stepped through a vectorised agent (`agent.VectorTrainer` or `agent.VectorEvaluator`) for
+  `num_frames` frames (rounded up to whole ticks), with `parts.run_loop`'s truncation at `max_frames_per_episode` and the
+  episode bookkeeping the CSV row reads.  One `tick()` per call, so an evaluation loop can be interleaved tick by tick
+  with a training loop; `stats()` gives the keys of `reporting.EpisodeTracker` / `StepRateTracker` plus the mean
+  `state_value` of the acting ticks.  The raw frames go to the device in one copy per tick, staged in pinned memory
+  (double-buffered, so the staging of tick t + 1 overlaps the copy of tick t), on `stream` when one is given."""
+
+  def __init__(self, agent, envs, num_frames, max_frames_per_episode, stream=None):
+    import torch
+    self._torch = torch
+    self._agent, self._envs, self._max = agent, envs, max_frames_per_episode
+    self._stream = stream
+    E = len(envs)
+    self._E = E
+    first = [env.reset() for env in envs]
+    shape = first[0].observation[0].shape
+    with self._on_stream():
+      self._stage = [torch.zeros((E,) + shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
+      self._frames = [torch.zeros((E,) + shape, dtype=torch.uint8, device='cuda') for _ in range(2)]
+    self._copied = [None, None]
+    agent.reset()
+    self._timesteps = first
+    self._steps = np.zeros(E, np.int64)
+    self._returns, self._values = [], []
+    self._ticks = -(-num_frames // E)
+    self._tick = 0
+    self._duration = 0.0
+
+  def _on_stream(self):
+    import contextlib
+    return self._torch.cuda.stream(self._stream) if self._stream is not None else contextlib.nullcontext()
+
+  @property
+  def done(self) -> bool:
+    return self._tick >= self._ticks
+
+  def tick(self) -> None:
+    from dqn_zoo_b200 import parts
+    torch = self._torch
+    t0 = timeit.default_timer()
+    E, agent, envs = self._E, self._agent, self._envs
+    slot = self._tick % 2
+    if self._copied[slot] is not None:
+      self._copied[slot].synchronize()           # the copy out of this staging buffer has finished
+    host = self._stage[slot].numpy()
+    timesteps = self._timesteps
     for e, ts in enumerate(timesteps):
       host[e] = ts.observation[0]
     step_type = np.array([int(ts.step_type) for ts in timesteps], np.int64)
     reward = np.array([np.nan if ts.reward is None else ts.reward for ts in timesteps])
     discount = np.array([np.nan if ts.discount is None else ts.discount for ts in timesteps])
     lives = np.array([ts.observation[1] for ts in timesteps], np.int64)
-    steps = np.where(step_type == int(parts.StepType.FIRST), 0, steps) + 1
-    if max_frames_per_episode > 0:               # run_loop's truncation: relabel the timestep LAST
-      step_type[steps > max_frames_per_episode] = int(parts.StepType.LAST)
-    frames[slot].copy_(stage[slot], non_blocking=True)
-    copied[slot] = torch.cuda.Event()
-    copied[slot].record()
-    actions = trainer.step(frames[slot], step_type, reward, discount, lives)
-    value = trainer.statistics['state_value']
+    self._steps = np.where(step_type == int(parts.StepType.FIRST), 0, self._steps) + 1
+    if self._max > 0:                            # run_loop's truncation: relabel the timestep LAST
+      step_type[self._steps > self._max] = int(parts.StepType.LAST)
+    with self._on_stream():
+      self._frames[slot].copy_(self._stage[slot], non_blocking=True)
+      self._copied[slot] = torch.cuda.Event()
+      self._copied[slot].record()
+    actions = agent.step(self._frames[slot], step_type, reward, discount, lives)
+    value = agent.statistics.get('state_value', math.nan)
     if not math.isnan(value):
-      values.append(value)
+      self._values.append(value)
     last = step_type == int(parts.StepType.LAST)
     if last.any():
-      returns.extend(trainer.episode_return[last].tolist())
-      trainer.reset(np.nonzero(last)[0])
-    timesteps = [envs[e].reset() if last[e] else envs[e].step(int(actions[e])) for e in range(E)]
-  duration = timeit.default_timer() - t0
-  running = float(trainer.episode_return.mean())
-  frames_done = ticks * E
-  return {
-      'episode_return': float(np.mean(returns)) if returns else (running if frames_done else math.nan),
-      'num_episodes': len(returns),
-      'step_rate': frames_done / duration if frames_done else math.nan,
-      'state_value': float(np.mean(values)) if values else math.nan,
-  }
+      self._returns.extend(agent.episode_return[last].tolist())
+      agent.reset(np.nonzero(last)[0])
+    self._timesteps = [envs[e].reset() if last[e] else envs[e].step(int(actions[e])) for e in range(E)]
+    self._tick += 1
+    self._duration += timeit.default_timer() - t0
+
+  def run(self):
+    while not self.done:
+      self.tick()
+    return self.stats()
+
+  def stats(self):
+    running = float(self._agent.episode_return.mean())
+    frames_done = self._tick * self._E
+    return {
+        'episode_return': float(np.mean(self._returns)) if self._returns else (running if frames_done else math.nan),
+        'num_episodes': len(self._returns),
+        'step_rate': frames_done / self._duration if frames_done else math.nan,
+        'state_value': float(np.mean(self._values)) if self._values else math.nan,
+    }
 
 
-def main():
+def train_streams(trainer, envs, num_frames, max_frames_per_episode):
+  """`num_frames` frames (rounded up to whole ticks) of E environments through `trainer` (a `StreamLoop` run to the
+  end); returns its statistics."""
+  return StreamLoop(trainer, envs, num_frames, max_frames_per_episode).run()
+
+
+def eval_streams(evaluator, envs, num_frames, max_frames_per_episode):
+  """The evaluation phase on E environments through an `agent.VectorEvaluator`, on the evaluator's CUDA stream."""
+  return StreamLoop(evaluator, envs, num_frames, max_frames_per_episode, stream=evaluator.stream).run()
+
+
+def iteration_row(iteration, args, train_stats, eval_stats, train_epsilon):
+  """The CSV row of one iteration (the column names and order of the reference's run_atari)."""
+  return [
+      ('iteration', iteration, '%3d'),
+      ('frame', iteration * args.num_train_frames, '%5d'),
+      ('eval_episode_return', eval_stats['episode_return'], '% 2.2f'),
+      ('train_episode_return', train_stats['episode_return'], '% 2.2f'),
+      ('eval_num_episodes', eval_stats['num_episodes'], '%3d'),
+      ('train_num_episodes', train_stats['num_episodes'], '%3d'),
+      ('eval_frame_rate', eval_stats['step_rate'], '%4.0f'),
+      ('train_frame_rate', train_stats['step_rate'], '%4.0f'),
+      ('train_exploration_epsilon', train_epsilon, '%.3f'),
+      ('train_state_value', train_stats['state_value'], '%.3f'),
+  ]
+
+
+def parse_args(argv=None):
   ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
   ap.add_argument('--agent', default='dqn', choices=['dqn', 'double_q', 'prioritized', 'c51', 'qrdqn', 'rainbow', 'iqn'])
   ap.add_argument('--num_actions', type=int, default=6)
@@ -165,10 +230,26 @@ def main():
   ap.add_argument('--results_csv_path', default='')
   ap.add_argument('--checkpoint_path', default='')
   ap.add_argument('--num_streams', type=int, default=1, help='E > 1: train from E environments with agent.VectorTrainer')
-  args = ap.parse_args()
+  ap.add_argument('--num_eval_streams', type=int, default=0,
+                  help='E >= 1: evaluate on E environments of their own with agent.VectorEvaluator')
+  ap.add_argument('--overlap_eval', action='store_true',
+                  help="run iteration i's evaluation on its own CUDA stream, interleaved tick by tick with iteration "
+                       "i + 1's training (needs --num_streams > 1 and --num_eval_streams; rows are written one "
+                       "iteration late)")
+  args = ap.parse_args(argv)
   if args.num_streams < 1:
     ap.error('--num_streams must be >= 1')
+  if args.num_eval_streams < 0:
+    ap.error('--num_eval_streams must be >= 0')
+  if args.overlap_eval and (args.num_streams < 2 or args.num_eval_streams < 1):
+    ap.error('--overlap_eval needs --num_streams > 1 and --num_eval_streams >= 1')
+  if args.overlap_eval and args.checkpoint_path:
+    ap.error('--overlap_eval does not checkpoint: an iteration ends while the previous evaluation is still running')
+  return args
 
+
+def run(args):
+  """The iterations of the run driver; returns the CSV rows (OrderedDicts) in order."""
   import torch
   if not torch.cuda.is_available():
     raise SystemExit('run_synthetic.py needs a CUDA device (the package has no CPU fallback)')
@@ -191,9 +272,13 @@ def main():
   if args.num_streams > 1:
     trainer = agent_lib.VectorTrainer(train_agent, num_streams=args.num_streams,
                                       rng_key=[0, int(random_state.randint(1, 2 ** 31))])
-  eval_agent = agent_lib.EpsilonGreedyActor(preprocessor=preprocessor_builder(), network=network,
-                                            exploration_epsilon=args.eval_exploration_epsilon,
-                                            rng_key=[0, int(random_state.randint(1, 2 ** 31))])
+  eval_key = [0, int(random_state.randint(1, 2 ** 31))]
+  if args.num_eval_streams:
+    eval_agent = agent_lib.VectorEvaluator(network, args.num_eval_streams, args.eval_exploration_epsilon, eval_key,
+                                           stream=torch.cuda.Stream() if args.overlap_eval else None)
+  else:
+    eval_agent = agent_lib.EpsilonGreedyActor(preprocessor=preprocessor_builder(), network=network,
+                                              exploration_epsilon=args.eval_exploration_epsilon, rng_key=eval_key)
 
   checkpoint = reporting.FileCheckpoint(args.checkpoint_path) if args.checkpoint_path else reporting.NullCheckpoint()
   state = checkpoint.state
@@ -205,6 +290,16 @@ def main():
   if checkpoint.can_be_restored():
     checkpoint.restore()
 
+  rows = []
+
+  def write(iteration, train_stats, eval_stats, train_epsilon):
+    log_output = iteration_row(iteration, args, train_stats, eval_stats, train_epsilon)
+    print(', '.join(('%s: ' + f) % (n, v) for n, v, f in log_output), flush=True)
+    row = collections.OrderedDict((n, v) for n, v, _ in log_output)
+    writer.write(row)
+    rows.append(row)
+
+  pending = None                         # overlap: (iteration, train stats, epsilon, evaluation loop) still evaluating
   while state.iteration <= args.num_iterations:
     env = environment_builder()          # a new environment per iteration: deterministic after a restore
     num_train_frames = 0 if state.iteration == 0 else args.num_train_frames
@@ -212,30 +307,44 @@ def main():
       train_seq = parts.run_loop(train_agent, env, args.max_frames_per_episode)
       train_stats = reporting.generate_statistics(reporting.make_default_trackers(train_agent),
                                                   itertools.islice(train_seq, num_train_frames))
+      eval_envs = [environment_builder() for _ in range(args.num_eval_streams)]
     else:
       envs = [env] + [environment_builder() for _ in range(args.num_streams - 1)]
-      train_stats = train_streams(trainer, envs, num_train_frames, args.max_frames_per_episode)
+      eval_envs = [environment_builder() for _ in range(args.num_eval_streams)]
+      train_loop = StreamLoop(trainer, envs, num_train_frames, args.max_frames_per_episode)
+      while not train_loop.done:
+        train_loop.tick()
+        if pending is not None and not pending[3].done:
+          pending[3].tick()              # the previous iteration's evaluation, on the evaluator's stream
+      train_stats = train_loop.stats()
+    if pending is not None:
+      write(pending[0], pending[1], pending[3].run(), pending[2])
+      pending = None
+    train_epsilon = train_agent.exploration_epsilon
     eval_agent.network_params = train_agent.learner      # device-to-device copy of the online parameters
-    eval_seq = parts.run_loop(eval_agent, env, args.max_frames_per_episode)
-    eval_stats = reporting.generate_statistics(reporting.make_default_trackers(eval_agent),
-                                               itertools.islice(eval_seq, args.num_eval_frames))
-    log_output = [
-        ('iteration', state.iteration, '%3d'),
-        ('frame', state.iteration * args.num_train_frames, '%5d'),
-        ('eval_episode_return', eval_stats['episode_return'], '% 2.2f'),
-        ('train_episode_return', train_stats['episode_return'], '% 2.2f'),
-        ('eval_num_episodes', eval_stats['num_episodes'], '%3d'),
-        ('train_num_episodes', train_stats['num_episodes'], '%3d'),
-        ('eval_frame_rate', eval_stats['step_rate'], '%4.0f'),
-        ('train_frame_rate', train_stats['step_rate'], '%4.0f'),
-        ('train_exploration_epsilon', train_agent.exploration_epsilon, '%.3f'),
-        ('train_state_value', train_stats['state_value'], '%.3f'),
-    ]
-    print(', '.join(('%s: ' + f) % (n, v) for n, v, f in log_output), flush=True)
-    writer.write(collections.OrderedDict((n, v) for n, v, _ in log_output))
+    if args.num_eval_streams:
+      eval_loop = StreamLoop(eval_agent, eval_envs, args.num_eval_frames, args.max_frames_per_episode,
+                             stream=eval_agent.stream)
+      if args.overlap_eval:
+        pending = (state.iteration, train_stats, train_epsilon, eval_loop)
+        state.iteration += 1
+        continue
+      eval_stats = eval_loop.run()
+    else:
+      eval_seq = parts.run_loop(eval_agent, env, args.max_frames_per_episode)
+      eval_stats = reporting.generate_statistics(reporting.make_default_trackers(eval_agent),
+                                                 itertools.islice(eval_seq, args.num_eval_frames))
+    write(state.iteration, train_stats, eval_stats, train_epsilon)
     state.iteration += 1
     checkpoint.save()
+  if pending is not None:
+    write(pending[0], pending[1], pending[3].run(), pending[2])
   writer.close()
+  return rows
+
+
+def main():
+  run(parse_args())
 
 
 if __name__ == '__main__':
