@@ -14,6 +14,7 @@ vp = C.c_void_p
 
 DZ_FLAG_BAD_VALUE, DZ_FLAG_BAD_INDEX, DZ_FLAG_BAD_TARGET, DZ_FLAG_ROOT_ZERO, DZ_FLAG_NONFINITE_WEIGHT = 1, 2, 4, 8, 16
 DZ_FLAG_FRAME_POOL_FULL = 32
+DZ_CKPT_BAD_PLANE_ID, DZ_CKPT_UNREFERENCED_PLANE, DZ_CKPT_HASH_MISMATCH, DZ_CKPT_BAD_FREE_STACK = 1, 2, 4, 8
 AGENT_KINDS = {'dqn': 0, 'double_q': 1, 'prioritized': 2, 'c51': 3, 'qrdqn': 4, 'rainbow': 5, 'iqn': 6}
 OPTIMIZERS = {'adam': 0, 'rmsprop': 1}
 
@@ -113,6 +114,13 @@ _SIGNATURES = {
     'dz_replay_sample': (i32, [C.POINTER(ReplayView), i32, C.POINTER(SampleInputs), C.POINTER(SampleOutputs), i32, vp]),
     'dz_replay_gather': (i32, [C.POINTER(ReplayView), vp, i32, vp, vp, vp, vp, vp, vp]),
     'dz_replay_update_priorities': (i32, [C.POINTER(ReplayView), vp, vp, i32, f64, i64, vp]),
+    'dz_ckpt_digest': (i32, [vp, i64, vp, vp]),
+    'dz_ckpt_digest_host': (i32, [vp, i64, C.POINTER(u64)]),
+    'dz_ckpt_pool_live': (i32, [C.POINTER(ReplayView), vp, vp, vp, vp]),
+    'dz_ckpt_pool_gather': (i32, [C.POINTER(ReplayView), vp, i64, vp, vp]),
+    'dz_ckpt_pool_scatter': (i32, [C.POINTER(ReplayView), vp, i64, vp, vp, vp]),
+    'dz_ckpt_pool_rebuild': (i32, [C.POINTER(ReplayView), vp, i64, vp, vp, i64, i64, vp, vp]),
+    'dz_ckpt_rows': (i32, [C.POINTER(ReplayView), i64, i64, vp, i32, vp]),
     'dz_learner_plan_query': (i32, [C.POINTER(LearnerConfig), C.POINTER(LearnerPlan)]),
     'dz_learner_tensor_info': (i32, [C.POINTER(LearnerConfig), i32, C.c_char_p, C.POINTER(i64), C.POINTER(i32),
                                      C.POINTER(i64)]),

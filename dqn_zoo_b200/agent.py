@@ -20,6 +20,8 @@ from __future__ import annotations
 
 import contextlib
 import ctypes as C
+import os
+import pickle
 from typing import Any, Callable, Mapping, Optional
 
 import numpy as np
@@ -171,6 +173,62 @@ class _DeviceAgent(parts.Agent):
     if self.PRIORITIZED:
       self._learner.max_seen_priority.fill_(float(state['max_seen_priority']))
     self._graph = None  # device pointers of the replay may have changed
+
+  _CHECKPOINT_BLOBS = ('online', 'target', 'opt_state', 'counters', 'max_seen_priority')
+
+  def save_checkpoint(self, directory: str) -> None:
+    """Writes the agent into `directory` (DESIGN.md §9): the raw online, target and optimizer-state blobs, the learner
+    counters and max_seen_priority as .npy files, the host RandomState, seed, IQN jax key and frame_t in a small
+    pickle, and the replay (`save_checkpoint`) in `replay/`.  The replay's RandomState belongs to the run, as for
+    `get_state`."""
+    from dqn_zoo_b200 import checkpoint as ck
+    os.makedirs(directory, exist_ok=True)
+    L = self._learner
+    digests = {}
+    for name in self._CHECKPOINT_BLOBS:
+      a = getattr(L, name).cpu().numpy()
+      np.save(os.path.join(directory, name + '.npy'), a)
+      digests[name] = ck.digest_host(a)
+    state = {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'param_count': L.plan.param_count,
+             'opt_state_floats': L.plan.opt_state_floats, 'host_rng': self._host_rng.get_state(), 'seed': self._seed,
+             'jax_key': None if getattr(self, '_jax_key', None) is None else self._jax_key.copy(),
+             'frame_t': self._frame_t, 'digests': digests}
+    with open(os.path.join(directory, 'agent.pkl'), 'wb') as f:
+      pickle.dump(state, f, protocol=pickle.HIGHEST_PROTOCOL)
+    self._replay.save_checkpoint(os.path.join(directory, 'replay'))
+
+  def load_checkpoint(self, directory: str) -> None:
+    """Restores `save_checkpoint` of an agent of the same kind and network.  ValueError (agent and replay untouched)
+    for a checkpoint of another kind, network size or replay geometry; RuntimeError for a file that fails its
+    digest.  Drops the CUDA graph, as `set_state` does."""
+    from dqn_zoo_b200 import checkpoint as ck
+    try:
+      with open(os.path.join(directory, 'agent.pkl'), 'rb') as f:
+        state = pickle.load(f)
+    except (OSError, pickle.UnpicklingError, EOFError) as e:
+      raise ValueError('%s is not a readable agent checkpoint: %s' % (directory, e)) from e
+    L = self._learner
+    ck.validate(state, {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND,
+                        'param_count': L.plan.param_count, 'opt_state_floats': L.plan.opt_state_floats}, directory)
+    blobs = {}
+    for name in self._CHECKPOINT_BLOBS:
+      path = os.path.join(directory, name + '.npy')
+      try:
+        a = np.load(path)
+      except (OSError, ValueError) as e:
+        raise RuntimeError('%s: %s' % (path, e)) from e
+      if a.shape != tuple(getattr(L, name).shape) or ck.digest_host(a) != state['digests'][name]:
+        raise RuntimeError('%s: shape or digest differs from the checkpoint\'s record' % path)
+      blobs[name] = a
+    self._replay.load_checkpoint(os.path.join(directory, 'replay'))
+    for name, a in blobs.items():
+      getattr(L, name).copy_(torch.from_numpy(a))
+    self._host_rng.set_state(state['host_rng'])
+    self._seed = state['seed']
+    if state['jax_key'] is not None:
+      self._jax_key = np.asarray(state['jax_key'], dtype=np.uint32).copy()
+    self._frame_t = state['frame_t']
+    self._graph = None
 
   # -- acting (dqn/agent.py:121-131,169-177) --------------------------------------------------------------
   def _act(self, timestep) -> parts.Action:
@@ -816,8 +874,38 @@ class VectorTrainer:
     return self._num_episodes.copy()
 
   def get_state(self) -> Mapping[str, Any]:
+    return dict(self._stream_state(), agent=self._agent.get_state())
+
+  def set_state(self, state: Mapping[str, Any]) -> None:
+    self._check_streams(state)
+    self._agent.set_state(state['agent'])
+    self._set_stream_state(state)
+
+  def save_checkpoint(self, directory: str) -> None:
+    """The agent's checkpoint directory (`_DeviceAgent.save_checkpoint`) in `agent/`, plus the per-stream state of
+    `get_state` (actions, RandomStates, preprocessor, accumulator, episode statistics) pickled in `trainer.pkl`."""
+    os.makedirs(directory, exist_ok=True)
+    self._agent.save_checkpoint(os.path.join(directory, 'agent'))
+    with open(os.path.join(directory, 'trainer.pkl'), 'wb') as f:
+      pickle.dump(self._stream_state(), f, protocol=pickle.HIGHEST_PROTOCOL)
+
+  def load_checkpoint(self, directory: str) -> None:
+    """Restores `save_checkpoint` of a trainer with the same stream count over the same kind of agent."""
+    try:
+      with open(os.path.join(directory, 'trainer.pkl'), 'rb') as f:
+        state = pickle.load(f)
+    except (OSError, pickle.UnpicklingError, EOFError) as e:
+      raise ValueError('%s is not a readable trainer checkpoint: %s' % (directory, e)) from e
+    self._check_streams(state)
+    self._agent.load_checkpoint(os.path.join(directory, 'agent'))
+    self._set_stream_state(state)
+
+  def _check_streams(self, state):
+    if np.shape(state['actions']) != (self._E,):
+      raise ValueError('state is for %d streams, this trainer has %d' % (len(state['actions']), self._E))
+
+  def _stream_state(self) -> Mapping[str, Any]:
     return {
-        'agent': self._agent.get_state(),
         'frame_t': self._agent._frame_t,
         'actions': self._actions.copy(),
         'has_action': self._has_action.copy(),
@@ -832,10 +920,7 @@ class VectorTrainer:
         'episodes': (self._episode_return.copy(), self._episode_length.copy(), self._num_episodes.copy()),
     }
 
-  def set_state(self, state: Mapping[str, Any]) -> None:
-    if np.shape(state['actions']) != (self._E,):
-      raise ValueError('state is for %d streams, this trainer has %d' % (len(state['actions']), self._E))
-    self._agent.set_state(state['agent'])
+  def _set_stream_state(self, state: Mapping[str, Any]) -> None:
     self._agent._frame_t = state['frame_t']
     self._actions = np.array(state['actions'], np.int32)
     self._has_action = np.array(state['has_action'], bool)

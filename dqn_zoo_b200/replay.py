@@ -27,6 +27,7 @@ from __future__ import annotations
 
 import collections
 import ctypes as C
+import os
 from typing import Any, Callable, Iterable, List, Mapping, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
@@ -1168,6 +1169,20 @@ class TransitionReplay:
     self._t = state['t']
     self._distribution.set_state(state['distribution'])
 
+  def save_checkpoint(self, directory: str) -> None:
+    """Writes the replay into `directory` (DESIGN.md §9): device arrays streamed through a fixed staging ring with a
+    digest per chunk, the host bookkeeping as int64 arrays, a JSON manifest.  Host memory stays bounded by the ring
+    plus the O(capacity) integer bookkeeping.  The RandomState is not saved (as for `get_state`)."""
+    _save_checkpoint(self, directory)
+
+  def load_checkpoint(self, directory: str) -> None:
+    """Restores `save_checkpoint` of a replay of the same class, layout, capacity, observation shape and
+    frame_capacity: afterwards every device array and host list equals the saved replay's, the frame pool's plane
+    ids and free stack included, so later adds and samples are those the saved replay would make.  A mismatch of
+    those raises ValueError before anything changes; a digest, size or pool-consistency failure raises RuntimeError
+    naming the file (and chunk) and leaves the replay empty."""
+    _load_checkpoint(self, directory)
+
   def check_valid(self) -> Tuple[bool, str]:
     """`replay.py:195-200`."""
     if self._t < self.size:
@@ -1192,6 +1207,256 @@ def _check_pool(rep, flags):
     return True, ''
   _raise_if_pool_full(rep._store, flags)
   return rep._store.check_pool(np.asarray(list(rep._live_ids), dtype=np.int64) % rep._capacity)
+
+
+# ------------------------------------------------------------------------------------------------
+# Checkpoint directories (DESIGN.md §9)
+# ------------------------------------------------------------------------------------------------
+
+REPLAY_FORMAT = 'dqn_zoo_b200.replay'
+REPLAY_FORMAT_VERSION = 1
+
+
+def _pool_capacity(store):
+  """frame_capacity the store has or will allocate (None: transition-major)."""
+  if not isinstance(store, _FramePoolStore):
+    return None
+  if store.frames is not None:
+    return store.frame_capacity
+  return store._requested if store._requested is not None else 2 * store.capacity + FRAME_POOL_SLACK
+
+
+def _checkpoint_header(rep):
+  return {'version': REPLAY_FORMAT_VERSION, 'kind': type(rep).__name__,
+          'layout': 'frames' if isinstance(rep._store, _FramePoolStore) else 'rows', 'capacity': rep._capacity,
+          'frame_capacity': _pool_capacity(rep._store)}
+
+
+def _bytes_of(t):
+  return t.reshape(-1).view(torch.uint8)
+
+
+def _dict_array(d):
+  return np.fromiter((x for kv in d.items() for x in kv), dtype=np.int64, count=2 * len(d)).reshape(-1, 2)
+
+
+def _array_dict(a):
+  return dict(zip(a[:, 0].tolist(), a[:, 1].tolist()))
+
+
+def _slot_runs(slots):
+  """(first slot, count, position) of each run of consecutive slots."""
+  if not len(slots):
+    return []
+  cut = np.nonzero(np.diff(slots) != 1)[0] + 1
+  starts = np.concatenate([[0], cut])
+  ends = np.concatenate([cut, [len(slots)]])
+  return [(int(slots[s]), int(e - s), int(s)) for s, e in zip(starts, ends)]
+
+
+def _row_copier(rep, live, to_replay):
+  """`Transfer` callback moving packed rows (live ids in order, 2 * obs_bytes each) between the staging buffer and
+  the transition-major rows: with FIFO eviction the live slots are at most two runs, each one pitched copy."""
+  st = rep._store
+  row = 2 * st.obs_bytes
+  v = st.fill_view(_lib.ReplayView())
+
+  def copy(off, n, staging):
+    r0 = off // row
+    for first, count, pos in _slot_runs(live[r0:r0 + n // row] % rep._capacity):
+      _lib.call('dz_ckpt_rows', C.byref(v), first, count, staging.data_ptr() + pos * row, int(to_replay), _stream())
+    return staging
+  return copy
+
+
+def _save_checkpoint(rep, directory):
+  from dqn_zoo_b200 import checkpoint as ck
+  st, dist = rep._store, rep._distribution
+  _raise_if_pool_full(st, rep._flags())
+  os.makedirs(directory, exist_ok=True)
+  dist.flush()                                    # device mirrors up to date with the host lists
+  xfer = ck.Transfer(st.action.device)
+  files = {}
+  path = lambda name: os.path.join(directory, name + '.bin')
+
+  def dev(name, nbytes, produce, chunk=None):
+    files[name] = xfer.save_device(path(name), nbytes, produce, chunk)
+
+  def host(name, array):
+    files[name] = ck.Transfer.save_host(path(name), array)
+
+  live = np.fromiter(rep._live_ids, dtype=np.int64, count=len(rep._live_ids))
+  host('live_ids', live)
+  extra = {}
+  if isinstance(dist, UniformDistribution):
+    host('ids', np.asarray(dist._ids, dtype=np.int64))
+    host('id_to_index', _dict_array(dist._id_to_index))
+    dev('ids_mirror', dist._mirror.t.numel() * 8, _bytes_of(dist._mirror.t))
+  else:
+    host('id_to_index', _dict_array(dist._id_to_index))
+    host('index_to_id', _dict_array(dist._index_to_id))
+    host('inactive_indices', np.asarray(dist._inactive_indices, dtype=np.int64))
+    host('active_indices', np.asarray(dist._active_indices, dtype=np.int64))
+    host('active_indices_location', _dict_array(dist._active_indices_location))
+    tree = dist._sum_tree
+    dev('sum_tree', tree._nodes.numel() * 8, _bytes_of(tree._nodes))
+    dev('live_mirror', dist._live_dev.t.numel() * 8, _bytes_of(dist._live_dev.t))
+    dev('id_at_mirror', dist._id_at_dev.t.numel() * 8, _bytes_of(dist._id_at_dev.t))
+    extra.update(tree_size=tree.size, tree_first_leaf=tree.capacity)
+  allocated = st.obs_shape is not None
+  if allocated:
+    for name in ('action', 'reward', 'discount'):
+      t = getattr(st, name)
+      dev(name, t.numel() * t.element_size(), _bytes_of(t))
+    if isinstance(st, _FramePoolStore):
+      v = st.fill_view(_lib.ReplayView())
+      fc = st.frame_capacity
+      ids = torch.empty(fc, dtype=torch.int32, device=st.frames.device)
+      hashes = torch.empty(fc, dtype=torch.int64, device=st.frames.device)
+      count = torch.zeros(1, dtype=torch.int64, device=st.frames.device)
+      _lib.call('dz_ckpt_pool_live', C.byref(v), _ptr(ids), _ptr(hashes), _ptr(count), _stream())
+      n, top = int(count.item()), int(st.counters.item())
+      fb = st.frame_bytes
+
+      def gather(off, nb, staging):
+        _lib.call('dz_ckpt_pool_gather', C.byref(v), _ptr(ids) + 4 * (off // fb), nb // fb, staging.data_ptr(), _stream())
+        return staging
+      dev('planes', st.planes.numel() * 4, _bytes_of(st.planes))
+      dev('free', top * 4, _bytes_of(st.free[:top]))
+      dev('pool_ids', n * 4, _bytes_of(ids[:n]))
+      dev('pool_hashes', n * 8, _bytes_of(hashes[:n]))
+      dev('frames', n * fb, gather, chunk=max(1, ck.CHUNK_BYTES // fb) * fb)
+      extra.update(pool_top=top, pool_planes=n)
+    else:
+      row = 2 * st.obs_bytes
+      dev('rows', len(live) * row, _row_copier(rep, live, False), chunk=max(1, ck.CHUNK_BYTES // row) * row)
+  manifest = dict(_checkpoint_header(rep), format=REPLAY_FORMAT, t=rep._t, files=files,
+                  obs_shape=list(st.obs_shape) if allocated else None,
+                  obs_dtype=st.obs_dtype.str if allocated else None, **extra)
+  ck.write_json(os.path.join(directory, ck.MANIFEST), manifest)
+
+
+def _reset_empty(rep):
+  """A replay that failed to load: empty, with the host lists, mirrors' meaning, sum tree and pool of a new one."""
+  rep._live_ids = collections.deque()
+  rep._t = 0
+  dist = rep._distribution
+  if isinstance(dist, UniformDistribution):
+    dist._ids, dist._id_to_index, dist._pending = [], {}, []
+  else:
+    dist._id_to_index, dist._index_to_id, dist._pending = {}, {}, []
+    dist._inactive_indices = list(range(rep._capacity))
+    dist._active_indices, dist._active_indices_location = [], {}
+    dist._sum_tree._nodes.zero_()
+    dist._sum_tree._size = rep._capacity
+  if isinstance(rep._store, _FramePoolStore):
+    rep._store.reset()
+  rep._flags().zero_()
+
+
+def _load_checkpoint(rep, directory):
+  from dqn_zoo_b200 import checkpoint as ck
+  m = ck.read_manifest(directory, REPLAY_FORMAT)
+  ck.validate(m, _checkpoint_header(rep), directory)
+  st = rep._store
+  saved_shape = None if m.get('obs_shape') is None else (tuple(m['obs_shape']), np.dtype(m['obs_dtype']))
+  if saved_shape is not None and st.obs_shape is not None and saved_shape != (st.obs_shape, st.obs_dtype):
+    raise ValueError('%s: checkpoint has observations %s %s, this replay stores %s %s'
+                     % (directory, saved_shape[0], saved_shape[1], st.obs_shape, st.obs_dtype))
+  try:
+    _restore_checkpoint(rep, directory, m, saved_shape, ck)
+  except BaseException as e:
+    _reset_empty(rep)
+    if isinstance(e, RuntimeError):
+      raise
+    raise RuntimeError('%s: checkpoint data is inconsistent (%s: %s); the replay was reset to empty'
+                       % (directory, type(e).__name__, e)) from e
+
+
+def _restore_checkpoint(rep, directory, m, saved_shape, ck):
+  st, dist = rep._store, rep._distribution
+  files = m['files']
+  path = lambda name: os.path.join(directory, name + '.bin')
+  host = {name: ck.Transfer.load_host(path(name), e) for name, e in files.items() if 'dtype' in e}
+  live = host['live_ids']
+  rep._flags().zero_()
+  xfer = ck.Transfer(st.action.device)
+
+  def dev(name, consume):
+    xfer.load_device(path(name), files[name], consume)
+
+  if isinstance(dist, UniformDistribution):
+    dev('ids_mirror', _bytes_of(dist._mirror.t))
+  else:
+    tree = dist._sum_tree
+    if (m['tree_first_leaf'], m['tree_size']) != (tree.capacity, tree.size):
+      raise RuntimeError('%s: sum tree of %d leaves (size %d) in the manifest, %d (size %d) here'
+                         % (directory, m['tree_first_leaf'], m['tree_size'], tree.capacity, tree.size))
+    dev('sum_tree', _bytes_of(tree._nodes))
+    dev('live_mirror', _bytes_of(dist._live_dev.t))
+    dev('id_at_mirror', _bytes_of(dist._id_at_dev.t))
+  if saved_shape is not None:
+    st.allocate(*saved_shape)
+    for name in ('action', 'reward', 'discount'):
+      dev(name, _bytes_of(getattr(st, name)))
+    if isinstance(st, _FramePoolStore):
+      _restore_pool(rep, directory, m, live, dev)
+    else:
+      dev('rows', _row_copier(rep, live, True))
+  # host bookkeeping last: the same containers, filled in the saved insertion order
+  rep._live_ids = collections.deque(live.tolist())
+  rep._t = int(m['t'])
+  if isinstance(dist, UniformDistribution):
+    dist._ids = host['ids'].tolist()
+    dist._id_to_index = _array_dict(host['id_to_index'])
+  else:
+    dist._id_to_index = _array_dict(host['id_to_index'])
+    dist._index_to_id = _array_dict(host['index_to_id'])
+    dist._inactive_indices = host['inactive_indices'].tolist()
+    dist._active_indices = host['active_indices'].tolist()
+    dist._active_indices_location = _array_dict(host['active_indices_location'])
+  dist._pending = []
+
+
+def _restore_pool(rep, directory, m, live, dev):
+  """Plane table, plane bytes and free stack from the files; refcounts, hashes and the lookup table rebuilt on the
+  device and checked against the saved live list and hashes."""
+  st = rep._store
+  fc, n, top = st.frame_capacity, int(m['pool_planes']), int(m['pool_top'])
+  if not (0 <= n < fc and 0 <= top < fc and n + 1 + top == fc):
+    raise RuntimeError('%s: %d live planes and a free stack of %d do not partition a pool of %d planes'
+                       % (directory, n, top, fc))
+  device = st.frames.device
+  st.reset()
+  dev('planes', _bytes_of(st.planes))
+  ids = torch.empty(max(n, 1), dtype=torch.int32, device=device)
+  hashes = torch.empty(max(n, 1), dtype=torch.int64, device=device)
+  dev('pool_ids', _bytes_of(ids)[:4 * n])
+  dev('pool_hashes', _bytes_of(hashes)[:8 * n])
+  bad = torch.zeros(4, dtype=torch.int32, device=device)
+  v = st.fill_view(_lib.ReplayView())
+  fb = st.frame_bytes
+
+  def scatter(off, nb, staging):
+    _lib.call('dz_ckpt_pool_scatter', C.byref(v), _ptr(ids) + 4 * (off // fb), nb // fb, staging.data_ptr(), _ptr(bad),
+              _stream())
+  dev('frames', scatter)
+  dev('free', _bytes_of(st.free)[:4 * top])
+  st.counters.fill_(top)
+  slots = torch.as_tensor(live % rep._capacity, device=device)
+  _lib.call('dz_ckpt_pool_rebuild', C.byref(v), _ptr(slots), len(live), _ptr(ids), _ptr(hashes), n, top, _ptr(bad),
+            _stream())
+  got = bad.cpu().numpy()
+  flags, referenced = int(got[0]), int(got.view(np.uint64)[1])
+  if flags or referenced != n + 1:
+    what = [text for bit, text in ((_lib.DZ_CKPT_BAD_PLANE_ID, 'a plane id out of range or an unsorted live list'),
+                                   (_lib.DZ_CKPT_UNREFERENCED_PLANE, 'a listed plane no live row references'),
+                                   (_lib.DZ_CKPT_HASH_MISMATCH, 'a plane whose bytes do not match its saved hash'),
+                                   (_lib.DZ_CKPT_BAD_FREE_STACK, 'a free-stack entry naming a referenced plane'))
+            if flags & bit]
+    if referenced != n + 1:
+      what.append('%d referenced planes for %d listed (+ plane 0)' % (referenced, n))
+    raise RuntimeError('%s: frame pool is inconsistent: %s' % (directory, '; '.join(what)))
 
 
 def _restore_rows(rep, storage):
@@ -1389,6 +1654,14 @@ class PrioritizedTransitionReplay:
     _restore_rows(self, state['storage'])
     self._t = state['t']
     self._distribution.set_state(state['distribution'])
+
+  def save_checkpoint(self, directory: str) -> None:
+    """As `TransitionReplay.save_checkpoint`; the raw sum-tree nodes are written bit for bit."""
+    _save_checkpoint(self, directory)
+
+  def load_checkpoint(self, directory: str) -> None:
+    """As `TransitionReplay.load_checkpoint`."""
+    _load_checkpoint(self, directory)
 
   def check_valid(self) -> Tuple[bool, str]:
     """`replay.py:762-768`."""

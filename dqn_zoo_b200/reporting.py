@@ -12,7 +12,8 @@ Behavioural contract kept from the reference so that its plotting notebook and r
     trick on `agent.statistics`).
   * `CsvWriter` / `NullWriter` — parts.py:448-504: one header row from the first dict's keys, append mode, resumable.
   * `NullCheckpoint` / `AttributeDict` — parts.py:507-541.  `FileCheckpoint` is the working implementation behind the
-    same three methods (`save`, `can_be_restored`, `restore`) that the reference leaves as a placeholder.
+    same three methods (`save`, `can_be_restored`, `restore`) that the reference leaves as a placeholder;
+    `DirectoryCheckpoint` is the same surface over a directory, for agents and replays too large to pickle.
 
 Everything here is host-side bookkeeping; nothing touches the GPU."""
 
@@ -21,6 +22,7 @@ import csv
 import math
 import os
 import pickle
+import shutil
 import tempfile
 import timeit
 from typing import Any, Iterable, Mapping, Optional, Sequence
@@ -260,10 +262,100 @@ class FileCheckpoint:
   def restore(self) -> None:
     with open(self._path, 'rb') as f:
       payload = pickle.load(f)
+    _apply(self.state, payload)
+
+
+def _fsync(path):
+  fd = os.open(path, os.O_RDONLY)
+  try:
+    os.fsync(fd)
+  finally:
+    os.close(fd)
+
+
+def _apply(state, payload):
+  for key, (kind, value) in payload.items():
+    if kind == 'stateful':
+      if key not in state:
+        raise KeyError('checkpoint entry %r has no registered object to restore into' % key)
+      state[key].set_state(value)
+    else:
+      state[key] = value
+
+
+class DirectoryCheckpoint:
+  """Checkpoint directory behind NullCheckpoint's interface, for state too large to pickle in one piece (DESIGN.md §9).
+
+  Entries of `state` with `save_checkpoint` / `load_checkpoint` (agents, replays, `VectorTrainer`) write into a
+  subdirectory of their own; every other entry is pickled as `FileCheckpoint` pickles it, into `state.pkl`.  Each
+  `save()` writes a new generation directory `gen-<n>` and fsyncs it, then switches the `LATEST` file to it by
+  write-and-rename, and only then removes the older generations: a save interrupted at any point leaves the previous
+  checkpoint restorable."""
+
+  LATEST = 'LATEST'
+
+  def __init__(self, path: str):
+    self._path = path
+    self.state = AttributeDict()
+
+  def _latest(self) -> Optional[str]:
+    try:
+      with open(os.path.join(self._path, self.LATEST)) as f:
+        name = f.read().strip()
+    except OSError:
+      return None
+    return name if name and os.path.isdir(os.path.join(self._path, name)) else None
+
+  def save(self) -> None:
+    os.makedirs(self._path, exist_ok=True)
+    gen = self._write_generation()
+    self._publish(gen)
+    for name in os.listdir(self._path):
+      if name.startswith('gen-') and name != gen:
+        shutil.rmtree(os.path.join(self._path, name), ignore_errors=True)
+
+  def _write_generation(self) -> str:
+    taken = [int(n[4:]) for n in os.listdir(self._path) if n.startswith('gen-') and n[4:].isdigit()]
+    gen = 'gen-%06d' % (max(taken, default=0) + 1)
+    folder = os.path.join(self._path, gen)
+    os.makedirs(folder)
+    payload = {}
+    for key, value in self.state.items():
+      if hasattr(value, 'save_checkpoint') and hasattr(value, 'load_checkpoint'):
+        value.save_checkpoint(os.path.join(folder, key))
+        payload[key] = ('directory', key)
+      else:
+        payload[key] = FileCheckpoint._snapshot(value)
+    with open(os.path.join(folder, 'state.pkl'), 'wb') as f:
+      pickle.dump(payload, f, protocol=pickle.HIGHEST_PROTOCOL)
+    for root, _, names in os.walk(folder):
+      for name in names:
+        _fsync(os.path.join(root, name))
+      _fsync(root)
+    return gen
+
+  def _publish(self, gen: str) -> None:
+    tmp = os.path.join(self._path, self.LATEST + '.tmp')
+    with open(tmp, 'w') as f:
+      f.write(gen + '\n')
+      f.flush()
+      os.fsync(f.fileno())
+    os.replace(tmp, os.path.join(self._path, self.LATEST))
+    _fsync(self._path)
+
+  def can_be_restored(self) -> bool:
+    return self._latest() is not None
+
+  def restore(self) -> None:
+    gen = self._latest()
+    if gen is None:
+      raise FileNotFoundError('no checkpoint generation under %s' % self._path)
+    folder = os.path.join(self._path, gen)
+    with open(os.path.join(folder, 'state.pkl'), 'rb') as f:
+      payload = pickle.load(f)
     for key, (kind, value) in payload.items():
-      if kind == 'stateful':
+      if kind == 'directory':
         if key not in self.state:
           raise KeyError('checkpoint entry %r has no registered object to restore into' % key)
-        self.state[key].set_state(value)
-      else:
-        self.state[key] = value
+        self.state[key].load_checkpoint(os.path.join(folder, value))
+    _apply(self.state, {k: v for k, v in payload.items() if v[0] != 'directory'})

@@ -213,6 +213,46 @@ int dz_replay_frames_in_use(const dz_replay_view* view, int64_t* h_frames_in_use
 int dz_replay_fill_synthetic_stacked(const dz_replay_view* view, int64_t n, uint64_t seed, int64_t episode_len,
                                      int32_t num_actions, double discount, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Checkpoint transfers (DESIGN.md §9; dz_checkpoint.cu).  A checkpoint streams device arrays
+ * through a fixed staging ring in chunks; every chunk is digested on the device before its D2H
+ * copy on save and after its H2D copy on load.
+ * ---------------------------------------------------------------------------------------- */
+
+/* 64-bit digest of `bytes` bytes at d_src (8-byte aligned): 8-byte little-endian words w_i (the last
+ * zero padded), digest = mix64(S ^ bytes), S = sum_i mix64(w_i ^ ((i+1) * 0x9E3779B97F4A7C15)) mod 2^64,
+ * mix64 the splitmix64 finaliser.  Wrapping adds make S independent of the reduction order.  Writes
+ * the digest to the DEVICE uint64 *d_out. */
+int dz_ckpt_digest(const void* d_src, int64_t bytes, uint64_t* d_out, void* stream);
+/* The same digest of a HOST range, computed on the CPU. */
+int dz_ckpt_digest_host(const void* h_src, int64_t bytes, uint64_t* h_out);
+
+/* Frame-deduplicated layout.  Live planes (refcount > 0, plane 0 excluded) in increasing id order into
+ * d_ids[0..*d_count) with their hashes into d_hashes (both sized frame_capacity); *d_count is a DEVICE int64. */
+int dz_ckpt_pool_live(const dz_replay_view* view, int32_t* d_ids, uint64_t* d_hashes, int64_t* d_count, void* stream);
+/* Planes d_ids[0..n) -> d_dst, packed at frame_bytes per plane (no stride padding). */
+int dz_ckpt_pool_gather(const dz_replay_view* view, const int32_t* d_ids, int64_t n, uint8_t* d_dst, void* stream);
+/* Packed planes d_src -> planes d_ids[0..n), stride padding zeroed.  An id outside [1, frame_capacity) sets
+ * DZ_CKPT_BAD_PLANE_ID in d_bad[0] and is skipped. */
+int dz_ckpt_pool_scatter(const dz_replay_view* view, const int32_t* d_ids, int64_t n, const uint8_t* d_src,
+                         int32_t* d_bad, void* stream);
+/* After dz_replay_frame_pool_reset, the plane-id table, the planes' bytes and the free stack [0, top): adds one
+ * reference per plane id of the live rows d_live_slots[0..n_live); recomputes the hash of each listed plane
+ * d_ids[0..n_ids) (strictly increasing), compares it with d_saved_hashes and inserts the plane into the table.
+ * d_bad is a zeroed DEVICE int32[4]: d_bad[0] collects DZ_CKPT_* bits, d_bad[2..3] the uint64 count of planes with
+ * refcount > 0 (plane 0 included), which the caller checks against n_ids + 1. */
+int dz_ckpt_pool_rebuild(const dz_replay_view* view, const int64_t* d_live_slots, int64_t n_live, const int32_t* d_ids,
+                         const uint64_t* d_saved_hashes, int64_t n_ids, int64_t top, int32_t* d_bad, void* stream);
+#define DZ_CKPT_BAD_PLANE_ID 1        /* a row or the live list names a plane outside the pool, or the list is unsorted */
+#define DZ_CKPT_UNREFERENCED_PLANE 2  /* a listed plane has no reference from a live row */
+#define DZ_CKPT_HASH_MISMATCH 4       /* a listed plane's bytes do not hash to the saved hash */
+#define DZ_CKPT_BAD_FREE_STACK 8      /* a free-stack entry is out of range or names a referenced plane */
+
+/* Transition-major layout: rows [first_slot, first_slot + n) <-> d_buf packed at obs_bytes per observation
+ * (s_tm1 then s_t of each row), one pitched device-to-device copy.  to_replay = 0: replay -> d_buf. */
+int dz_ckpt_rows(const dz_replay_view* view, int64_t first_slot, int64_t n, uint8_t* d_buf, int32_t to_replay,
+                 void* stream);
+
 /* Bulk pre-fill for benchmarks/tests: rows [row0,row0+n) get deterministic pseudo-random
  * contents (splitmix64 counter hash; byte-identical to oracle/replay_oracle.py:synthetic_rows):
  * uint8 observations iid uniform, action uniform, reward in {-1,0,1} w.p. .05/.9/.05, discount_t =

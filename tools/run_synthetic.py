@@ -228,7 +228,10 @@ def parse_args(argv=None):
   ap.add_argument('--eval_exploration_epsilon', type=float, default=0.01)
   ap.add_argument('--seed', type=int, default=1)
   ap.add_argument('--results_csv_path', default='')
-  ap.add_argument('--checkpoint_path', default='')
+  ap.add_argument('--checkpoint_path', default='', help='pickle the whole run state into one file (FileCheckpoint)')
+  ap.add_argument('--checkpoint_dir', default='',
+                  help='checkpoint into a directory (DirectoryCheckpoint): the agent and its replay are streamed to '
+                       'files with bounded host memory')
   ap.add_argument('--num_streams', type=int, default=1, help='E > 1: train from E environments with agent.VectorTrainer')
   ap.add_argument('--num_eval_streams', type=int, default=0,
                   help='E >= 1: evaluate on E environments of their own with agent.VectorEvaluator')
@@ -243,8 +246,10 @@ def parse_args(argv=None):
     ap.error('--num_eval_streams must be >= 0')
   if args.overlap_eval and (args.num_streams < 2 or args.num_eval_streams < 1):
     ap.error('--overlap_eval needs --num_streams > 1 and --num_eval_streams >= 1')
-  if args.overlap_eval and args.checkpoint_path:
+  if args.overlap_eval and (args.checkpoint_path or args.checkpoint_dir):
     ap.error('--overlap_eval does not checkpoint: an iteration ends while the previous evaluation is still running')
+  if args.checkpoint_path and args.checkpoint_dir:
+    ap.error('give --checkpoint_path or --checkpoint_dir, not both')
   return args
 
 
@@ -280,7 +285,12 @@ def run(args):
     eval_agent = agent_lib.EpsilonGreedyActor(preprocessor=preprocessor_builder(), network=network,
                                               exploration_epsilon=args.eval_exploration_epsilon, rng_key=eval_key)
 
-  checkpoint = reporting.FileCheckpoint(args.checkpoint_path) if args.checkpoint_path else reporting.NullCheckpoint()
+  if args.checkpoint_dir:
+    checkpoint = reporting.DirectoryCheckpoint(args.checkpoint_dir)
+  elif args.checkpoint_path:
+    checkpoint = reporting.FileCheckpoint(args.checkpoint_path)
+  else:
+    checkpoint = reporting.NullCheckpoint()
   state = checkpoint.state
   state.iteration = 0
   state.train_agent = train_agent if trainer is None else trainer
