@@ -88,6 +88,16 @@ class LearnIO(C.Structure):
               ('update_out', UpdateOutputs), ('d_max_seen_priority', vp), ('priority_exponent', f64)]
 
 
+class CatchConfig(C.Structure):   # struct dz_catch_config
+  _fields_ = [('num_streams', i32), ('num_actions', i32), ('min_noop_steps', i32), ('max_noop_steps', i32),
+              ('seed', C.c_uint32), ('stream_offset', C.c_uint32)]
+
+
+CATCH_STATE_FIELDS = ('paddle_x', 'ball_x', 'ball_y', 'ball_dx', 'lives', 'balls_left', 'counter', 'noops', 'over')
+CATCH_MAX_STREAMS = 4096
+CATCH_MAX_NOOP_STEPS = 89
+
+
 class DzError(RuntimeError):
   pass
 
@@ -154,6 +164,9 @@ _SIGNATURES = {
     'dz_atari_preprocess_band_rows': (i32, []),
     'dz_jax_uniform': (i32, [vp, vp, i32, vp, vp]),
     'dz_test_threefry2x32': (i32, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, vp]),
+    'dz_catch_step': (i32, [C.POINTER(CatchConfig), vp, vp, vp, vp, vp, vp, vp]),
+    'dz_catch_render': (i32, [C.POINTER(CatchConfig), vp, vp, vp]),
+    'dz_test_catch_step': (i32, [C.POINTER(CatchConfig), vp, i32, i32, vp, vp]),
     'dz_test_learner_buffer': (i32, [vp, C.c_char_p, vp, vp]),
     'dz_test_copy': (i32, [vp, vp, i64, vp]),
     'dz_test_learner_trace': (i32, [vp, C.c_char_p, vp]),

@@ -11,30 +11,9 @@
 // (ffffffff.. ; ffffffff..) = 1cb996fc bb002be7; (13198a2e 03707344; 243f6a88 85a308d3) = c4923a9c 483df7a0;
 // split(PRNGKey(0)) = [[4146024105, 967050713], [2718843009, 1272950319]]; uniform(PRNGKey(0)) = 0.41845703.
 #include "dz_common.cuh"
+#include "dz_threefry.cuh"
 
 namespace dz {
-
-__host__ __device__ __forceinline__ uint32_t rotl32(uint32_t x, int r) { return (x << r) | (x >> (32 - r)); }
-
-// Threefry-2x32, 20 rounds (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3").
-__host__ __device__ inline void threefry2x32(uint32_t k0, uint32_t k1, uint32_t c0, uint32_t c1, uint32_t* o0, uint32_t* o1) {
-  const uint32_t ks[3] = {k0, k1, k0 ^ k1 ^ 0x1BD11BDAu};
-  const int rot[2][4] = {{13, 15, 26, 6}, {17, 29, 16, 24}};
-  uint32_t x0 = c0 + ks[0], x1 = c1 + ks[1];
-#pragma unroll
-  for (int i = 0; i < 5; ++i) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      x0 += x1;
-      x1 = rotl32(x1, rot[i & 1][j]);
-      x1 ^= x0;
-    }
-    x0 += ks[(i + 1) % 3];
-    x1 += ks[(i + 2) % 3] + (uint32_t)(i + 1);
-  }
-  *o0 = x0;
-  *o1 = x1;
-}
 
 namespace {
 

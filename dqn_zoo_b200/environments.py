@@ -1,0 +1,169 @@
+"""Catch at Atari geometry, simulated and rendered on the device (csrc/dz_env.cu; rules in DESIGN.md §10).
+
+`VectorCatch` steps E streams of the game with one kernel launch per tick and leaves their 210x160x3 RGB frames in a
+device tensor, where `agent.VectorTrainer.step` / `agent.VectorEvaluator.step` read them in place: the whole loop
+(environment -> preprocess -> act -> insert -> learn) stays on the GPU but for the actions and a small per-stream
+record.  `Catch` is one stream with the reference's dm_env surface, for `parts.run_loop` and the one-stream agents.
+"""
+
+import ctypes as C
+from typing import Any, Mapping, Optional
+
+import numpy as np
+import torch
+
+from dqn_zoo_b200 import _lib
+from dqn_zoo_b200 import parts
+
+HEIGHT, WIDTH = 210, 160
+
+
+class VectorCatch:
+  """E streams of Catch on the device.
+
+  `reset()` starts a new episode in every stream; `step(actions, reset=None)` applies stream e's action, or starts a
+  new episode in the streams where `reset` is true (a stream whose last step was LAST starts one too, as a dm_env
+  environment does).  Both return `(frames, step_type, reward, discount, lives)`: `frames` is the device tensor uint8
+  [E, 210, 160, 3] that every tick overwrites in place (clone it to keep a frame); step_type int64, reward / discount
+  float64 with NaN on FIRST, lives int64, all host arrays [E].  That is the form `VectorTrainer.step` takes.
+
+  A reset simulates k no-op frames, k uniform in [min_noop_steps, max_noop_steps], and its FIRST timestep carries the
+  last of them (the reference's `RandomNoopsEnvironmentWrapper`).  Stream e's trajectory depends only on `seed`,
+  `stream_offset + e` and its own actions and resets, not on E.  A tick is one pinned host-to-device copy of the actions
+  and reset flags, one kernel, one device-to-host copy of the record, and one synchronisation, all on `stream` (default:
+  the current CUDA stream)."""
+
+  def __init__(self, num_streams: int, seed: int, num_actions: int = 6, min_noop_steps: int = 1,
+               max_noop_steps: int = 30, stream_offset: int = 0, device='cuda'):
+    E = int(num_streams)
+    if not 1 <= E <= _lib.CATCH_MAX_STREAMS:
+      raise ValueError('num_streams must be in [1, %d], got %d' % (_lib.CATCH_MAX_STREAMS, E))
+    if not 3 <= num_actions <= 18:
+      raise ValueError('num_actions must be in [3, 18], got %d' % num_actions)
+    if not 0 <= min_noop_steps <= max_noop_steps:
+      raise ValueError('need 0 <= min_noop_steps <= max_noop_steps, got %d, %d' % (min_noop_steps, max_noop_steps))
+    if max_noop_steps > _lib.CATCH_MAX_NOOP_STEPS:
+      raise ValueError('max_noop_steps %d > %d: a ball could land during the no-op frames of a reset'
+                       % (max_noop_steps, _lib.CATCH_MAX_NOOP_STEPS))
+    if not 0 <= seed < 2 ** 32:
+      raise ValueError('seed must be in [0, 2^32)')
+    if stream_offset < 0 or stream_offset + E > 2 ** 32:
+      raise ValueError('stream_offset + num_streams must be in [0, 2^32]')
+    self._cfg = _lib.CatchConfig(E, num_actions, min_noop_steps, max_noop_steps, seed, stream_offset)
+    self._E = E
+    self._device = torch.device(device)
+    F = len(_lib.CATCH_STATE_FIELDS)
+    self._state = torch.zeros((F, E), dtype=torch.int32, device=self._device)
+    self._state[_lib.CATCH_STATE_FIELDS.index('over')] = 1     # the first tick of every stream is a reset
+    self._frames = torch.zeros((E, HEIGHT, WIDTH, 3), dtype=torch.uint8, device=self._device)
+    self._control = torch.zeros((2, E), dtype=torch.int32, device=self._device)
+    self._record = torch.zeros((4, E), dtype=torch.int32, device=self._device)
+    self._control_host = torch.zeros((2, E), dtype=torch.int32).pin_memory()
+    self._record_host = torch.zeros((4, E), dtype=torch.int32).pin_memory()
+
+  def reset(self, stream=None):
+    """A new episode in every stream."""
+    control = self._control_host.numpy()
+    control[0] = 0
+    control[1] = 1
+    return self._tick(stream)
+
+  def step(self, actions, reset=None, stream=None):
+    """actions: int [E] in [0, num_actions) (ignored for the streams that reset); reset: bool [E] or None."""
+    actions = np.asarray(actions)
+    if actions.shape != (self._E,):
+      raise ValueError('actions must have shape (%d,), got %s' % (self._E, actions.shape))
+    control = self._control_host.numpy()
+    control[0] = actions
+    if reset is None:
+      control[1] = 0
+    else:
+      reset = np.asarray(reset, bool)
+      if reset.shape != (self._E,):
+        raise ValueError('reset must have shape (%d,), got %s' % (self._E, reset.shape))
+      control[1] = reset
+    return self._tick(stream)
+
+  def _tick(self, stream):
+    s = torch.cuda.current_stream(self._device) if stream is None else stream
+    _lib.call('dz_catch_step', C.byref(self._cfg), self._state.data_ptr(), self._control_host.data_ptr(),
+              self._control.data_ptr(), self._frames.data_ptr(), self._record.data_ptr(), self._record_host.data_ptr(),
+              s.cuda_stream)
+    s.synchronize()
+    rec = self._record_host.numpy()
+    step_type = rec[0].astype(np.int64)
+    first = step_type == int(parts.StepType.FIRST)
+    reward = np.where(first, np.nan, rec[1].astype(np.float64))
+    discount = np.where(first, np.nan, rec[2].astype(np.float64))
+    return self._frames, step_type, reward, discount, rec[3].astype(np.int64)
+
+  @property
+  def num_streams(self) -> int:
+    return self._E
+
+  @property
+  def num_actions(self) -> int:
+    return self._cfg.num_actions
+
+  @property
+  def frames(self) -> torch.Tensor:
+    """The device frames of the last tick, uint8 [E, 210, 160, 3]."""
+    return self._frames
+
+  def _config(self):
+    c = self._cfg
+    return (c.num_streams, c.num_actions, c.min_noop_steps, c.max_noop_steps, c.seed, c.stream_offset)
+
+  def get_state(self, stream=None) -> Mapping[str, Any]:
+    """The configuration and the device state arrays (one int32 [E] array per field of
+    `_lib.CATCH_STATE_FIELDS`), copied to the host."""
+    s = torch.cuda.current_stream(self._device) if stream is None else stream
+    with torch.cuda.stream(s):
+      state = self._state.cpu().numpy()
+    return {'config': self._config(), 'fields': {k: state[i].copy() for i, k in enumerate(_lib.CATCH_STATE_FIELDS)}}
+
+  def set_state(self, state: Mapping[str, Any], stream=None) -> None:
+    """Restores `get_state()` of an environment with the same configuration and re-renders every stream's frame from
+    it: the environment continues bit for bit."""
+    if tuple(state['config']) != self._config():
+      raise ValueError('state is for the configuration %s, this environment has %s'
+                       % (tuple(state['config']), self._config()))
+    arrays = np.stack([np.asarray(state['fields'][k], np.int32) for k in _lib.CATCH_STATE_FIELDS])
+    s = torch.cuda.current_stream(self._device) if stream is None else stream
+    with torch.cuda.stream(s):
+      self._state.copy_(torch.from_numpy(arrays))
+      _lib.call('dz_catch_render', C.byref(self._cfg), self._state.data_ptr(), self._frames.data_ptr(), s.cuda_stream)
+
+
+class Catch:
+  """One stream of Catch with the reference's dm_env surface: `reset()` / `step(action)` return a `parts.TimeStep`
+  whose observation is (rgb uint8 [210, 160, 3] host array, lives).  Backed by `VectorCatch(1)`; its trajectory is
+  stream 0 of a `VectorCatch` with the same arguments."""
+
+  def __init__(self, seed: int, num_actions: int = 6, min_noop_steps: int = 1, max_noop_steps: int = 30,
+               stream_offset: int = 0, device='cuda'):
+    self._env = VectorCatch(1, seed, num_actions, min_noop_steps, max_noop_steps, stream_offset, device)
+
+  @staticmethod
+  def _timestep(out):
+    frames, step_type, reward, discount, lives = out
+    st = parts.StepType(int(step_type[0]))
+    first = st == parts.StepType.FIRST
+    return parts.TimeStep(st, None if first else float(reward[0]), None if first else float(discount[0]),
+                          (frames[0].cpu().numpy(), int(lives[0])))
+
+  def reset(self) -> parts.TimeStep:
+    return self._timestep(self._env.reset())
+
+  def step(self, action) -> parts.TimeStep:
+    return self._timestep(self._env.step(np.array([int(action)])))
+
+  @property
+  def num_actions(self) -> int:
+    return self._env.num_actions
+
+  def get_state(self) -> Mapping[str, Any]:
+    return self._env.get_state()
+
+  def set_state(self, state: Mapping[str, Any]) -> None:
+    self._env.set_state(state)

@@ -517,6 +517,41 @@ int dz_jax_uniform(const uint32_t* d_keys, const int64_t* counts, int32_t nblock
 /* threefry2x32 (20 rounds) evaluated on the HOST by the same source the kernel compiles; tests only. */
 int dz_test_threefry2x32(uint32_t k0, uint32_t k1, uint32_t c0, uint32_t c1, uint32_t* out2);
 
+/* ---- Catch at Atari geometry on the device (DESIGN.md §10) ------------------------------------------------------
+ * E streams of the game, each simulated and rendered as a 210x160x3 uint8 RGB frame in HBM.  State: int32
+ * [DZ_CATCH_STATE_FIELDS][E] device array (fields paddle_x, ball_x, ball_y, ball_dx, lives, balls_left, counter, noops,
+ * over); a new state is all 0 but over = 1, so that the first tick of every stream is a reset.  Stream e's randomness:
+ * key = threefry2x32((0, seed), (stream_offset + e, 0)). */
+#define DZ_CATCH_HEIGHT 210
+#define DZ_CATCH_WIDTH 160
+#define DZ_CATCH_STATE_FIELDS 9
+#define DZ_CATCH_RECORD_FIELDS 4
+#define DZ_CATCH_MAX_STREAMS 4096
+#define DZ_CATCH_MAX_NOOP_STEPS 89   /* the first ball lands on the 90th frame after a reset */
+typedef struct dz_catch_config {
+  int32_t num_streams;      /* E in [1, 4096] */
+  int32_t num_actions;      /* A in [3, 18]: 0 stay, 1 left, 2 right, 3.. stay */
+  int32_t min_noop_steps;   /* 0 <= min <= max <= DZ_CATCH_MAX_NOOP_STEPS */
+  int32_t max_noop_steps;
+  uint32_t seed;
+  uint32_t stream_offset;   /* stream_offset + E <= 2^32 */
+} dz_catch_config;
+/* One tick of all E streams.  h_control: PINNED int32 [2][E] (row 0 actions, row 1 reset flags: non-zero starts a new
+ * episode instead of stepping; so does stepping a stream whose last step was LAST), checked on the host (an action
+ * outside [0, A) of a stream that is not reset is DZ_EINVAL) and copied into d_control (device int32 [2][E]).  The
+ * kernel updates d_state, writes every stream's frame into d_frames (device uint8 [E][210][160][3], 16-byte aligned)
+ * and d_record (device int32 [DZ_CATCH_RECORD_FIELDS][E]: step_type 0 FIRST / 1 MID / 2 LAST, reward, discount,
+ * lives; reward and discount are 0 on FIRST), which is copied to h_record (PINNED, same shape).  All on `stream`;
+ * the caller synchronises before reading h_record or reusing h_control. */
+int dz_catch_step(const dz_catch_config* cfg, int32_t* d_state, const int32_t* h_control, int32_t* d_control,
+                  uint8_t* d_frames, int32_t* d_record, int32_t* h_record, void* stream);
+/* Renders every stream's frame from d_state (e.g. after the state was restored); the state is not changed. */
+int dz_catch_render(const dz_catch_config* cfg, int32_t* d_state, uint8_t* d_frames, void* stream);
+/* The kernel's tick and picture evaluated on the HOST by the same source: stream id cfg->stream_offset, state int32
+ * [DZ_CATCH_STATE_FIELDS] updated in place, frame (NULL: not rendered) 210*160*3 bytes, record int32 [4]; tests only. */
+int dz_test_catch_step(const dz_catch_config* cfg, int32_t* state, int32_t action, int32_t reset, uint8_t* frame,
+                       int32_t* record);
+
 /* Device pointer + element count of an internal learner buffer of the last update (pass 0: "act1", "act2", "act3",
  * "h1", "h1_val", "dh1", "iqn_e0", "iqn_hi", "iqn_dhi");
  * tests/tools only. */

@@ -17,6 +17,11 @@ snapshot taken after each training phase); `--num_eval_frames` then counts the f
 phases share `StreamLoop`'s truncation and episode bookkeeping.  `--overlap_eval` (with `--num_streams` > 1) runs
 iteration i's evaluation on its own CUDA stream, one tick after each training tick of iteration i + 1; every column of
 the CSV rows but the rates is as without it.  CSV columns and checkpoints are otherwise as with one stream.
+
+`--env catch` plays Catch (`dqn_zoo_b200.environments`, DESIGN.md §10) instead of the synthetic frames: a game that is
+simulated and rendered on the device, so its returns measure learning.  With E > 1 streams each phase steps one
+`VectorCatch` whose frames tensor goes to the trainer or evaluator as it is, with no host staging; with one stream the
+phases play `Catch` through `parts.run_loop`.
 """
 import argparse
 import collections
@@ -105,21 +110,30 @@ class StreamLoop:
   episode bookkeeping the CSV row reads.  One `tick()` per call, so an evaluation loop can be interleaved tick by tick
   with a training loop; `stats()` gives the keys of `reporting.EpisodeTracker` / `StepRateTracker` plus the mean
   `state_value` of the acting ticks.  The raw frames go to the device in one copy per tick, staged in pinned memory
-  (double-buffered, so the staging of tick t + 1 overlaps the copy of tick t), on `stream` when one is given."""
+  (double-buffered, so the staging of tick t + 1 overlaps the copy of tick t), on `stream` when one is given.
+
+  `envs` is a list of E dm_env-style environments, or one vectorised device environment (`environments.VectorCatch`)
+  whose frames tensor the agent reads in place, stepped on `stream`."""
 
   def __init__(self, agent, envs, num_frames, max_frames_per_episode, stream=None):
     import torch
     self._torch = torch
     self._agent, self._envs, self._max = agent, envs, max_frames_per_episode
     self._stream = stream
-    E = len(envs)
+    self._vector = not isinstance(envs, (list, tuple))
+    if self._vector:
+      E = envs.num_streams
+      with self._on_stream():
+        first = envs.reset()
+    else:
+      E = len(envs)
+      first = [env.reset() for env in envs]
+      shape = first[0].observation[0].shape
+      with self._on_stream():
+        self._stage = [torch.zeros((E,) + shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self._frames = [torch.zeros((E,) + shape, dtype=torch.uint8, device='cuda') for _ in range(2)]
+      self._copied = [None, None]
     self._E = E
-    first = [env.reset() for env in envs]
-    shape = first[0].observation[0].shape
-    with self._on_stream():
-      self._stage = [torch.zeros((E,) + shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
-      self._frames = [torch.zeros((E,) + shape, dtype=torch.uint8, device='cuda') for _ in range(2)]
-    self._copied = [None, None]
     agent.reset()
     self._timesteps = first
     self._steps = np.zeros(E, np.int64)
@@ -141,6 +155,33 @@ class StreamLoop:
     torch = self._torch
     t0 = timeit.default_timer()
     E, agent, envs = self._E, self._agent, self._envs
+    if self._vector:
+      frames, step_type, reward, discount, lives = self._timesteps
+      step_type = step_type.copy()
+    else:
+      frames, step_type, reward, discount, lives = self._stage_timesteps()
+    self._steps = np.where(step_type == int(parts.StepType.FIRST), 0, self._steps) + 1
+    if self._max > 0:                            # run_loop's truncation: relabel the timestep LAST
+      step_type[self._steps > self._max] = int(parts.StepType.LAST)
+    actions = agent.step(frames, step_type, reward, discount, lives)
+    value = agent.statistics.get('state_value', math.nan)
+    if not math.isnan(value):
+      self._values.append(value)
+    last = step_type == int(parts.StepType.LAST)
+    if last.any():
+      self._returns.extend(agent.episode_return[last].tolist())
+      agent.reset(np.nonzero(last)[0])
+    if self._vector:
+      with self._on_stream():
+        self._timesteps = envs.step(actions, reset=last)
+    else:
+      self._timesteps = [envs[e].reset() if last[e] else envs[e].step(int(actions[e])) for e in range(E)]
+    self._tick += 1
+    self._duration += timeit.default_timer() - t0
+
+  def _stage_timesteps(self):
+    """The E host timesteps as struct-of-arrays, their frames sent to the device in one staged copy."""
+    torch = self._torch
     slot = self._tick % 2
     if self._copied[slot] is not None:
       self._copied[slot].synchronize()           # the copy out of this staging buffer has finished
@@ -152,24 +193,11 @@ class StreamLoop:
     reward = np.array([np.nan if ts.reward is None else ts.reward for ts in timesteps])
     discount = np.array([np.nan if ts.discount is None else ts.discount for ts in timesteps])
     lives = np.array([ts.observation[1] for ts in timesteps], np.int64)
-    self._steps = np.where(step_type == int(parts.StepType.FIRST), 0, self._steps) + 1
-    if self._max > 0:                            # run_loop's truncation: relabel the timestep LAST
-      step_type[self._steps > self._max] = int(parts.StepType.LAST)
     with self._on_stream():
       self._frames[slot].copy_(self._stage[slot], non_blocking=True)
       self._copied[slot] = torch.cuda.Event()
       self._copied[slot].record()
-    actions = agent.step(self._frames[slot], step_type, reward, discount, lives)
-    value = agent.statistics.get('state_value', math.nan)
-    if not math.isnan(value):
-      self._values.append(value)
-    last = step_type == int(parts.StepType.LAST)
-    if last.any():
-      self._returns.extend(agent.episode_return[last].tolist())
-      agent.reset(np.nonzero(last)[0])
-    self._timesteps = [envs[e].reset() if last[e] else envs[e].step(int(actions[e])) for e in range(E)]
-    self._tick += 1
-    self._duration += timeit.default_timer() - t0
+    return self._frames[slot], step_type, reward, discount, lives
 
   def run(self):
     while not self.done:
@@ -216,6 +244,8 @@ def iteration_row(iteration, args, train_stats, eval_stats, train_epsilon):
 
 def parse_args(argv=None):
   ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+  ap.add_argument('--env', default='synthetic', choices=['synthetic', 'catch'],
+                  help='synthetic: random host frames; catch: the device Catch game (dqn_zoo_b200.environments)')
   ap.add_argument('--agent', default='dqn', choices=['dqn', 'double_q', 'prioritized', 'c51', 'qrdqn', 'rainbow', 'iqn'])
   ap.add_argument('--num_actions', type=int, default=6)
   ap.add_argument('--replay_capacity', type=int, default=20000)
@@ -248,6 +278,8 @@ def parse_args(argv=None):
     ap.error('--overlap_eval needs --num_streams > 1 and --num_eval_streams >= 1')
   if args.overlap_eval and (args.checkpoint_path or args.checkpoint_dir):
     ap.error('--overlap_eval does not checkpoint: an iteration ends while the previous evaluation is still running')
+  if args.env == 'catch' and not 3 <= args.num_actions <= 18:
+    ap.error('--env catch needs --num_actions in [3, 18]')
   if args.checkpoint_path and args.checkpoint_dir:
     ap.error('give --checkpoint_path or --checkpoint_dir, not both')
   return args
@@ -259,6 +291,7 @@ def run(args):
   if not torch.cuda.is_available():
     raise SystemExit('run_synthetic.py needs a CUDA device (the package has no CPU fallback)')
   from dqn_zoo_b200 import agent as agent_lib
+  from dqn_zoo_b200 import environments
   from dqn_zoo_b200 import parts
   from dqn_zoo_b200 import processors
   from dqn_zoo_b200 import reporting
@@ -266,8 +299,14 @@ def run(args):
   random_state = np.random.RandomState(args.seed)
   writer = reporting.CsvWriter(args.results_csv_path) if args.results_csv_path else reporting.NullWriter()
 
-  def environment_builder():
-    return SyntheticAtari(seed=int(random_state.randint(1, 2 ** 31)), num_actions=args.num_actions)
+  def environment_builder(num_streams=0):
+    """A new environment seeded from the run's RandomState; with --env catch and num_streams > 0, one VectorCatch."""
+    seed = int(random_state.randint(1, 2 ** 31))
+    if args.env == 'catch':
+      if num_streams:
+        return environments.VectorCatch(num_streams, seed, num_actions=args.num_actions)
+      return environments.Catch(seed, num_actions=args.num_actions)
+    return SyntheticAtari(seed=seed, num_actions=args.num_actions)
 
   def preprocessor_builder():
     return processors.atari(device_observations=True)
@@ -310,17 +349,30 @@ def run(args):
     rows.append(row)
 
   pending = None                         # overlap: (iteration, train stats, epsilon, evaluation loop) still evaluating
+  vector_catch = args.env == 'catch' and trainer is not None
   while state.iteration <= args.num_iterations:
-    env = environment_builder()          # a new environment per iteration: deterministic after a restore
+    # a new environment per iteration: deterministic after a restore
+    env = environment_builder(args.num_streams if vector_catch else 0)
+    eval_env = env                       # the one-stream evaluation (no --num_eval_streams) plays the first stream
     num_train_frames = 0 if state.iteration == 0 else args.num_train_frames
     if trainer is None:
       train_seq = parts.run_loop(train_agent, env, args.max_frames_per_episode)
       train_stats = reporting.generate_statistics(reporting.make_default_trackers(train_agent),
                                                   itertools.islice(train_seq, num_train_frames))
-      eval_envs = [environment_builder() for _ in range(args.num_eval_streams)]
+      if args.env == 'catch' and args.num_eval_streams:
+        eval_envs = environment_builder(args.num_eval_streams)
+      else:
+        eval_envs = [environment_builder() for _ in range(args.num_eval_streams)]
     else:
-      envs = [env] + [environment_builder() for _ in range(args.num_streams - 1)]
-      eval_envs = [environment_builder() for _ in range(args.num_eval_streams)]
+      if vector_catch:
+        envs = env
+        if args.num_eval_streams:
+          eval_envs = environment_builder(args.num_eval_streams)
+        else:
+          eval_env = environment_builder()
+      else:
+        envs = [env] + [environment_builder() for _ in range(args.num_streams - 1)]
+        eval_envs = [environment_builder() for _ in range(args.num_eval_streams)]
       train_loop = StreamLoop(trainer, envs, num_train_frames, args.max_frames_per_episode)
       while not train_loop.done:
         train_loop.tick()
@@ -341,7 +393,7 @@ def run(args):
         continue
       eval_stats = eval_loop.run()
     else:
-      eval_seq = parts.run_loop(eval_agent, env, args.max_frames_per_episode)
+      eval_seq = parts.run_loop(eval_agent, eval_env, args.max_frames_per_episode)
       eval_stats = reporting.generate_statistics(reporting.make_default_trackers(eval_agent),
                                                  itertools.islice(eval_seq, args.num_eval_frames))
     write(state.iteration, train_stats, eval_stats, train_epsilon)
