@@ -98,6 +98,17 @@ CATCH_MAX_STREAMS = 4096
 CATCH_MAX_NOOP_STEPS = 89
 
 
+class BreakoutConfig(C.Structure):   # struct dz_breakout_config
+  _fields_ = [('num_streams', i32), ('num_actions', i32), ('min_noop_steps', i32), ('max_noop_steps', i32),
+              ('seed', C.c_uint32), ('stream_offset', C.c_uint32)]
+
+
+BREAKOUT_STATE_FIELDS = ('paddle_x', 'ball_x', 'ball_y', 'ball_dx', 'ball_dy', 'in_play', 'serve_timer', 'lives',
+                         'row0', 'row1', 'row2', 'row3', 'row4', 'row5', 'counter', 'noops', 'over')
+BREAKOUT_MAX_STREAMS = 4096
+BREAKOUT_MAX_NOOP_STEPS = 63
+
+
 class DzError(RuntimeError):
   pass
 
@@ -167,6 +178,9 @@ _SIGNATURES = {
     'dz_catch_step': (i32, [C.POINTER(CatchConfig), vp, vp, vp, vp, vp, vp, vp]),
     'dz_catch_render': (i32, [C.POINTER(CatchConfig), vp, vp, vp]),
     'dz_test_catch_step': (i32, [C.POINTER(CatchConfig), vp, i32, i32, vp, vp]),
+    'dz_breakout_step': (i32, [C.POINTER(BreakoutConfig), vp, vp, vp, vp, vp, vp, vp]),
+    'dz_breakout_render': (i32, [C.POINTER(BreakoutConfig), vp, vp, vp]),
+    'dz_test_breakout_step': (i32, [C.POINTER(BreakoutConfig), vp, i32, i32, vp, vp]),
     'dz_test_learner_buffer': (i32, [vp, C.c_char_p, vp, vp]),
     'dz_test_copy': (i32, [vp, vp, i64, vp]),
     'dz_test_learner_trace': (i32, [vp, C.c_char_p, vp]),

@@ -1,5 +1,6 @@
-"""The device Catch environment (`environments.VectorCatch`, DESIGN.md §10) alone and in the loop.  One JSON line per
-point:
+"""A device game (`--game catch`: `environments.VectorCatch`, DESIGN.md §10, the default; `--game breakout`:
+`environments.VectorBreakout`, §11) alone and in the loop.  One JSON line per point (with `--game breakout` each carries
+`game`):
 
   * env_step: E in {32, 256, 1024}.  device_us_per_tick: CUDA events around back-to-back ticks (actions copy, kernel,
     record copy) without host synchronisation; store_GBps: the E x 100,800 frame bytes a tick writes over that time;
@@ -7,14 +8,15 @@ point:
   * env_train / env_eval: E in {32, 256}, `VectorCatch.step` + `VectorTrainer.step` (dqn, rainbow; replay prefilled so
     the learner runs every 16 frames) or + `VectorEvaluator.step`, frames per second over the host clock, beside
     bench_train.py / bench_eval.py's device-pool figures;
-  * driver: `tools/run_synthetic.py --env catch --num_streams 64 --num_eval_streams 64`, with and without
+  * driver: `tools/run_synthetic.py --env <game> --num_streams 64 --num_eval_streams 64`, with and without
     `--overlap_eval`, wall time of the whole run;
-  * learning (`--learning FRAMES`): the learning curve of the GPU learning test (tests/test_gpu_catch.py): dqn, E = 32,
-    evaluated with epsilon 0.01 on 64 streams every `--eval_every` frames.
+  * learning (`--learning FRAMES`): the learning curve of the GPU learning tests (tests/test_gpu_catch.py,
+    tests/test_gpu_breakout.py): `--agent` (dqn; also rainbow), E = 32, evaluated with epsilon 0.01 on 64 streams every
+    `--eval_every` frames (`evaluate` says what an evaluation episode is).
 
 The card's name and power limit are read in the same run.
 
-  python tools/bench_env.py [--parts env,train,eval,driver] [--learning 0]"""
+  python tools/bench_env.py [--game catch] [--parts env,train,eval,driver] [--learning 0] [--agent dqn]"""
 
 import argparse
 import json
@@ -32,17 +34,31 @@ import torch  # noqa: E402
 import bench_train  # noqa: E402
 
 FRAME_BYTES = 210 * 160 * 3
+# Breakout evaluation: episodes are truncated at this many frames, and every stream plays one frame more than that, so
+# each completes at least one episode (a good policy can keep the ball alive far longer).
+BREAKOUT_EVAL_FRAMES = 4500
+
+
+def make_env(game, num_streams, seed, num_actions=6):
+  """`VectorCatch` or `VectorBreakout` (whose actions 4.. do nothing, so 6-action agents drive both)."""
+  from dqn_zoo_b200 import environments
+  if game == 'breakout':
+    return environments.VectorBreakout(num_streams, seed, num_actions=num_actions)
+  return environments.VectorCatch(num_streams, seed, num_actions=num_actions)
+
+
+def _tag(game):
+  return {} if game == 'catch' else {'game': game}
 
 
 def emit(**kw):
   print(json.dumps(kw), flush=True)
 
 
-def bench_env_step(E, ticks=400):
+def bench_env_step(E, ticks=400, game='catch'):
   import ctypes as C
   from dqn_zoo_b200 import _lib
-  from dqn_zoo_b200 import environments
-  env = environments.VectorCatch(E, seed=1)
+  env = make_env(game, E, seed=1)
   env.reset()
   rs = np.random.RandomState(0)
   for _ in range(20):
@@ -53,7 +69,7 @@ def bench_env_step(E, ticks=400):
   start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
   start.record()
   for _ in range(ticks):
-    _lib.call('dz_catch_step', *args, s.cuda_stream)
+    _lib.call(env._STEP, *args, s.cuda_stream)
   end.record()
   end.synchronize()
   device_s = start.elapsed_time(end) / 1e3 / ticks
@@ -62,7 +78,7 @@ def bench_env_step(E, ticks=400):
   for t in range(ticks):
     env.step(actions[t % 16])
   host_s = (time.perf_counter() - t0) / ticks
-  emit(metric='env_step', streams=E, device_us_per_tick=round(device_s * 1e6, 2),
+  emit(metric='env_step', **_tag(game), streams=E, device_us_per_tick=round(device_s * 1e6, 2),
        store_GBps=round(E * FRAME_BYTES / device_s / 1e9, 1), frames_per_sec=round(E / host_s, 1),
        host_us_per_step=round(host_s * 1e6, 2), ticks=ticks)
 
@@ -79,11 +95,10 @@ def _loop(agent, env, ticks):
     frames, st, rw, dc, lv = env.step(actions, reset=last)
 
 
-def bench_env_agent(what, kind, E, frames_target, repeats=2):
+def bench_env_agent(what, kind, E, frames_target, repeats=2, game='catch'):
   from dqn_zoo_b200 import agent as ag
-  from dqn_zoo_b200 import environments
   from dqn_zoo_b200 import learner as dl
-  env = environments.VectorCatch(E, seed=2)
+  env = make_env(game, E, seed=2)
   if what == 'train':
     agent = bench_train.make_agent(kind, 100000)
     runner = ag.VectorTrainer(agent, num_streams=E, rng_key=[0, 3])
@@ -99,12 +114,12 @@ def bench_env_agent(what, kind, E, frames_target, repeats=2):
     _loop(runner, env, ticks)
     torch.cuda.synchronize()
     dt = time.perf_counter() - t0
-    emit(metric='env_' + what, agent=kind, streams=E, repeat=r, frames_per_sec=round(ticks * E / dt, 1), ticks=ticks)
+    emit(metric='env_' + what, **_tag(game), agent=kind, streams=E, repeat=r, frames_per_sec=round(ticks * E / dt, 1), ticks=ticks)
 
 
-def bench_driver():
+def bench_driver(game='catch'):
   import run_synthetic
-  base = ['--env', 'catch', '--num_streams', '64', '--num_eval_streams', '64', '--num_iterations', '2',
+  base = ['--env', game, '--num_streams', '64', '--num_eval_streams', '64', '--num_iterations', '2',
           '--num_train_frames', '65536', '--num_eval_frames', '32768', '--replay_capacity', '20000',
           '--min_replay_capacity_fraction', '0.05']
   for overlap in (False, True, False, True):
@@ -112,59 +127,76 @@ def bench_driver():
     t0 = time.perf_counter()
     rows = run_synthetic.run(run_synthetic.parse_args(argv))
     dt = time.perf_counter() - t0
-    emit(metric='driver', overlap_eval=overlap, wall_s=round(dt, 2),
+    emit(metric='driver', **_tag(game), overlap_eval=overlap, wall_s=round(dt, 2),
          train_frame_rate=[round(r['train_frame_rate'], 1) for r in rows],
          eval_frame_rate=[round(r['eval_frame_rate'], 1) for r in rows])
 
 
 # -- learning ----------------------------------------------------------------------------------------------------------
-def learning_agent(seed, train_frames):
+def learning_agent(seed, train_frames, kind='dqn', num_actions=6):
   """dqn at the reference's hyper-parameters but for a faster schedule: replay of 100k transitions, learning from 10k,
-  epsilon 1 -> 0.01 over the first quarter of the frames, target sync every 8000 frames."""
+  epsilon 1 -> 0.01 over the first quarter of the frames, target sync every 8000 frames.  `kind='rainbow'`: the same
+  schedule with rainbow's prioritized replay (exponent 0.5, importance exponent 0.4 -> 1 over the run), 3-step returns,
+  noisy greedy acting and its 51-atom support on [-10, 10]."""
   from dqn_zoo_b200 import agent as ag
   from dqn_zoo_b200 import learner as dl
   from dqn_zoo_b200 import parts
   from dqn_zoo_b200 import replay as dr
   rs = np.random.RandomState(seed)
   capacity, min_fill = 100000, 10000
-  rep = dr.TransitionReplay(capacity, dr.Transition(None, None, None, None, None), rs, frame_dedup=True)
+  structure = dr.Transition(None, None, None, None, None)
+  common = dict(preprocessor=None, sample_network_input=None, network=dl.NetworkSpec(kind, num_actions),
+                optimizer=None, batch_size=32, min_replay_capacity_fraction=min_fill / capacity, learn_period=16,
+                target_network_update_period=8000, rng_key=[0, seed + 1])
+  if kind == 'rainbow':
+    importance = parts.LinearSchedule(begin_t=min_fill, decay_steps=max(train_frames, 1), begin_value=0.4,
+                                      end_value=1.0)
+    rep = dr.PrioritizedTransitionReplay(capacity, structure, 0.5, importance, 1e-3, True, rs, frame_dedup=True)
+    return ag.Rainbow(support=np.linspace(-10, 10, 51), transition_accumulator=dr.NStepTransitionAccumulator(3),
+                      replay=rep, **common)
+  rep = dr.TransitionReplay(capacity, structure, rs, frame_dedup=True)
   epsilon = parts.LinearSchedule(begin_t=4 * min_fill, decay_steps=max(train_frames // 4, 1), begin_value=1.0,
                                  end_value=0.01)
-  return ag.Dqn(preprocessor=None, sample_network_input=None, network=dl.NetworkSpec('dqn', 6), optimizer=None,
-                transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep, batch_size=32,
-                min_replay_capacity_fraction=min_fill / capacity, learn_period=16, target_network_update_period=8000,
-                rng_key=[0, seed + 1], exploration_epsilon=epsilon, grad_error_bound=1.0 / 32)
+  return ag.Dqn(transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep, exploration_epsilon=epsilon,
+                grad_error_bound=1.0 / 32, **common)
 
 
-def evaluate(learner, seed, num_streams=64):
-  """Mean return of the episodes that `num_streams` Catch streams complete in 1,900 ticks (every stream completes at
-  least one: an episode is at most 20 x 91 + 30 frames) at epsilon 0.01, and their number."""
+def evaluate(learner, seed, num_streams=64, game='catch', num_actions=6):
+  """Mean return of the episodes that `num_streams` streams complete at epsilon 0.01, and their number.  Catch: 1,900
+  ticks, no truncation (every stream completes at least one episode: one is at most 20 x 91 + 30 frames).  Breakout:
+  an episode runs from its FIRST step to its LAST step or to its BREAKOUT_EVAL_FRAMES-th frame, where it is
+  truncated; every stream plays BREAKOUT_EVAL_FRAMES + 1 ticks, so it completes at least one, and the episodes still
+  running at the end are not counted."""
   import run_synthetic
   from dqn_zoo_b200 import agent as ag
-  from dqn_zoo_b200 import environments
   ev = ag.VectorEvaluator(learner, num_streams, 0.01, [0, seed + 2])
   ev.network_params = learner
-  env = environments.VectorCatch(num_streams, seed + 3)
-  stats = run_synthetic.StreamLoop(ev, env, 1900 * num_streams, 0).run()
+  env = make_env(game, num_streams, seed + 3, num_actions)
+  if game == 'breakout':
+    loop = run_synthetic.StreamLoop(ev, env, (BREAKOUT_EVAL_FRAMES + 1) * num_streams, BREAKOUT_EVAL_FRAMES)
+  else:
+    loop = run_synthetic.StreamLoop(ev, env, 1900 * num_streams, 0)
+  stats = loop.run()
   return stats['episode_return'], stats['num_episodes']
 
 
-def learning_run(train_frames, seed=0, num_streams=32, eval_every=0, log=None):
-  """Trains `learning_agent` from `num_streams` Catch streams for `train_frames` frames; evaluates every `eval_every`
-  frames (0: at the end only).  Returns [(frames, mean eval return, eval episodes, train episode return)]."""
+def learning_run(train_frames, seed=0, num_streams=32, eval_every=0, log=None, game='catch', num_actions=6,
+                 kind='dqn'):
+  """Trains `learning_agent` from `num_streams` streams of `game` for `train_frames` frames (training episodes are not
+  truncated); evaluates every `eval_every` frames (0: at the end only).  Returns [(frames, mean eval return, eval
+  episodes, train episode return)]."""
   import run_synthetic
   from dqn_zoo_b200 import agent as ag
-  from dqn_zoo_b200 import environments
-  agent = learning_agent(seed, train_frames)
+  agent = learning_agent(seed, train_frames, kind, num_actions)
   trainer = ag.VectorTrainer(agent, num_streams=num_streams, rng_key=[0, seed + 4])
-  env = environments.VectorCatch(num_streams, seed + 5)
+  env = make_env(game, num_streams, seed + 5, num_actions)
   loop = run_synthetic.StreamLoop(trainer, env, train_frames, 0)
   curve = []
   every = max(eval_every // num_streams, 1) if eval_every else None
   while not loop.done:
     loop.tick()
     if (every and loop._tick % every == 0) or loop.done:
-      ret, n = evaluate(agent.learner, seed)
+      ret, n = evaluate(agent.learner, seed, game=game, num_actions=num_actions)
       curve.append((loop._tick * num_streams, ret, n, loop.stats()['episode_return']))
       if log:
         log(frames=curve[-1][0], eval_return=round(ret, 3), eval_episodes=n, train_return=round(curve[-1][3], 3))
@@ -173,6 +205,8 @@ def learning_run(train_frames, seed=0, num_streams=32, eval_every=0, log=None):
 
 def main():
   ap = argparse.ArgumentParser()
+  ap.add_argument('--game', default='catch', choices=['catch', 'breakout'])
+  ap.add_argument('--agent', default='dqn', choices=['dqn', 'rainbow'], help='the agent of the learning curve')
   ap.add_argument('--parts', default='env,train,eval,driver')
   ap.add_argument('--frames', type=int, default=65536, help='frames per timed window of env_train / env_eval')
   ap.add_argument('--learning', type=int, default=0, help='frames of the learning curve (0: none)')
@@ -186,18 +220,20 @@ def main():
   parts = a.parts.split(',') if a.parts else []
   if 'env' in parts:
     for E in (32, 256, 1024):
-      bench_env_step(E)
+      bench_env_step(E, game=a.game)
   for what in ('train', 'eval'):
     if what in parts:
       for kind in ('dqn', 'rainbow'):
         for E in (32, 256):
-          bench_env_agent(what, kind, E, a.frames)
+          bench_env_agent(what, kind, E, a.frames, game=a.game)
   if 'driver' in parts:
-    bench_driver()
+    bench_driver(a.game)
   if a.learning:
     t0 = time.perf_counter()
-    learning_run(a.learning, a.seed, eval_every=a.eval_every,
-                 log=lambda **kw: emit(metric='learning', seed=a.seed, wall_s=round(time.perf_counter() - t0, 1), **kw))
+    learning_run(a.learning, a.seed, eval_every=a.eval_every, game=a.game, kind=a.agent,
+                 log=lambda **kw: emit(metric='learning', **_tag(a.game), **({} if a.agent == 'dqn' else
+                                                                              {'agent': a.agent}),
+                                       seed=a.seed, wall_s=round(time.perf_counter() - t0, 1), **kw))
   emit(metric='device_after', **bench_train.device_info())
 
 

@@ -21,7 +21,9 @@ the CSV rows but the rates is as without it.  CSV columns and checkpoints are ot
 `--env catch` plays Catch (`dqn_zoo_b200.environments`, DESIGN.md §10) instead of the synthetic frames: a game that is
 simulated and rendered on the device, so its returns measure learning.  With E > 1 streams each phase steps one
 `VectorCatch` whose frames tensor goes to the trainer or evaluator as it is, with no host staging; with one stream the
-phases play `Catch` through `parts.run_loop`.
+phases play `Catch` through `parts.run_loop`.  `--env breakout` does the same with the device Breakout (DESIGN.md §11;
+`VectorBreakout` / `Breakout`, `--num_actions` in [4, 18]).  Breakout has no frame limit of its own:
+`--max_frames_per_episode` truncates its episodes.
 """
 import argparse
 import collections
@@ -244,8 +246,9 @@ def iteration_row(iteration, args, train_stats, eval_stats, train_epsilon):
 
 def parse_args(argv=None):
   ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
-  ap.add_argument('--env', default='synthetic', choices=['synthetic', 'catch'],
-                  help='synthetic: random host frames; catch: the device Catch game (dqn_zoo_b200.environments)')
+  ap.add_argument('--env', default='synthetic', choices=['synthetic', 'catch', 'breakout'],
+                  help='synthetic: random host frames; catch / breakout: a game simulated and rendered on the device '
+                       '(dqn_zoo_b200.environments)')
   ap.add_argument('--agent', default='dqn', choices=['dqn', 'double_q', 'prioritized', 'c51', 'qrdqn', 'rainbow', 'iqn'])
   ap.add_argument('--num_actions', type=int, default=6)
   ap.add_argument('--replay_capacity', type=int, default=20000)
@@ -280,6 +283,8 @@ def parse_args(argv=None):
     ap.error('--overlap_eval does not checkpoint: an iteration ends while the previous evaluation is still running')
   if args.env == 'catch' and not 3 <= args.num_actions <= 18:
     ap.error('--env catch needs --num_actions in [3, 18]')
+  if args.env == 'breakout' and not 4 <= args.num_actions <= 18:
+    ap.error('--env breakout needs --num_actions in [4, 18]')
   if args.checkpoint_path and args.checkpoint_dir:
     ap.error('give --checkpoint_path or --checkpoint_dir, not both')
   return args
@@ -300,12 +305,17 @@ def run(args):
   writer = reporting.CsvWriter(args.results_csv_path) if args.results_csv_path else reporting.NullWriter()
 
   def environment_builder(num_streams=0):
-    """A new environment seeded from the run's RandomState; with --env catch and num_streams > 0, one VectorCatch."""
+    """A new environment seeded from the run's RandomState; with a device game and num_streams > 0, its vectorised
+    form (VectorCatch, VectorBreakout)."""
     seed = int(random_state.randint(1, 2 ** 31))
     if args.env == 'catch':
       if num_streams:
         return environments.VectorCatch(num_streams, seed, num_actions=args.num_actions)
       return environments.Catch(seed, num_actions=args.num_actions)
+    if args.env == 'breakout':
+      if num_streams:
+        return environments.VectorBreakout(num_streams, seed, num_actions=args.num_actions)
+      return environments.Breakout(seed, num_actions=args.num_actions)
     return SyntheticAtari(seed=seed, num_actions=args.num_actions)
 
   def preprocessor_builder():
@@ -349,22 +359,23 @@ def run(args):
     rows.append(row)
 
   pending = None                         # overlap: (iteration, train stats, epsilon, evaluation loop) still evaluating
-  vector_catch = args.env == 'catch' and trainer is not None
+  device_game = args.env in ('catch', 'breakout')
+  vector_game = device_game and trainer is not None
   while state.iteration <= args.num_iterations:
     # a new environment per iteration: deterministic after a restore
-    env = environment_builder(args.num_streams if vector_catch else 0)
+    env = environment_builder(args.num_streams if vector_game else 0)
     eval_env = env                       # the one-stream evaluation (no --num_eval_streams) plays the first stream
     num_train_frames = 0 if state.iteration == 0 else args.num_train_frames
     if trainer is None:
       train_seq = parts.run_loop(train_agent, env, args.max_frames_per_episode)
       train_stats = reporting.generate_statistics(reporting.make_default_trackers(train_agent),
                                                   itertools.islice(train_seq, num_train_frames))
-      if args.env == 'catch' and args.num_eval_streams:
+      if device_game and args.num_eval_streams:
         eval_envs = environment_builder(args.num_eval_streams)
       else:
         eval_envs = [environment_builder() for _ in range(args.num_eval_streams)]
     else:
-      if vector_catch:
+      if vector_game:
         envs = env
         if args.num_eval_streams:
           eval_envs = environment_builder(args.num_eval_streams)
