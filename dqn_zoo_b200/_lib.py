@@ -109,6 +109,17 @@ BREAKOUT_MAX_STREAMS = 4096
 BREAKOUT_MAX_NOOP_STEPS = 63
 
 
+class PongConfig(C.Structure):   # struct dz_pong_config
+  _fields_ = [('num_streams', i32), ('num_actions', i32), ('min_noop_steps', i32), ('max_noop_steps', i32),
+              ('seed', C.c_uint32), ('stream_offset', C.c_uint32)]
+
+
+PONG_STATE_FIELDS = ('paddle_y', 'opponent_y', 'ball_x', 'ball_y', 'ball_dx', 'ball_dy', 'in_play', 'serve_timer',
+                     'agent_score', 'opponent_score', 'counter', 'noops', 'over')
+PONG_MAX_STREAMS = 4096
+PONG_MAX_NOOP_STEPS = 63
+
+
 class DzError(RuntimeError):
   pass
 
@@ -181,6 +192,9 @@ _SIGNATURES = {
     'dz_breakout_step': (i32, [C.POINTER(BreakoutConfig), vp, vp, vp, vp, vp, vp, vp]),
     'dz_breakout_render': (i32, [C.POINTER(BreakoutConfig), vp, vp, vp]),
     'dz_test_breakout_step': (i32, [C.POINTER(BreakoutConfig), vp, i32, i32, vp, vp]),
+    'dz_pong_step': (i32, [C.POINTER(PongConfig), vp, vp, vp, vp, vp, vp, vp]),
+    'dz_pong_render': (i32, [C.POINTER(PongConfig), vp, vp, vp]),
+    'dz_test_pong_step': (i32, [C.POINTER(PongConfig), vp, i32, i32, vp, vp]),
     'dz_test_learner_buffer': (i32, [vp, C.c_char_p, vp, vp]),
     'dz_test_copy': (i32, [vp, vp, i64, vp]),
     'dz_test_learner_trace': (i32, [vp, C.c_char_p, vp]),

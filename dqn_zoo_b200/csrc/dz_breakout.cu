@@ -12,7 +12,7 @@
 // threefry2x32((0, seed), (stream_offset + e, 1)) (the 1 tags the game: Catch keys with 0); a reset draws its no-op
 // count from threefry2x32(key, (counter, 0)) and a serve its x and dx from threefry2x32(key, (counter, 1)), each
 // advancing counter.
-#include "dz_common.cuh"
+#include "dz_game.cuh"
 #include "dz_threefry.cuh"
 
 namespace dz {
@@ -58,11 +58,6 @@ struct BreakoutState {   // the field order of the state arrays
 static_assert(sizeof(BreakoutState) == DZ_BREAKOUT_STATE_FIELDS * sizeof(int32_t), "one int32 per field");
 
 struct Step { int32_t step_type, reward, discount, lives; };
-
-// floor(u * n / 2^32): a uniform draw in [0, n) from 32 random bits.
-__host__ __device__ __forceinline__ int32_t below(uint32_t u, uint32_t n) {
-  return (int32_t)(((uint64_t)u * n) >> 32);
-}
 
 __host__ __device__ __forceinline__ void breakout_serve(BreakoutState& s, uint32_t k0, uint32_t k1) {
   uint32_t o0, o1;
@@ -188,20 +183,6 @@ __host__ __device__ __forceinline__ uint32_t breakout_rgb(const BreakoutState& s
   return kBackground;
 }
 
-__device__ __forceinline__ BreakoutState load_state(const int32_t* st, int E, int e) {
-  BreakoutState s;
-  int32_t* f = reinterpret_cast<int32_t*>(&s);
-#pragma unroll
-  for (int i = 0; i < DZ_BREAKOUT_STATE_FIELDS; ++i) f[i] = st[i * E + e];
-  return s;
-}
-
-__device__ __forceinline__ void store_state(const BreakoutState& s, int32_t* st, int E, int e) {
-  const int32_t* f = reinterpret_cast<const int32_t*>(&s);
-#pragma unroll
-  for (int i = 0; i < DZ_BREAKOUT_STATE_FIELDS; ++i) st[i * E + e] = f[i];
-}
-
 // Can an object touch pixels [xa, xb] of row y?  Conservative: false means background.  In the wall's rows the test is
 // against the row's brick mask, so the cleared part of the wall is written as background.
 __device__ __forceinline__ bool span_has_object(const BreakoutState& s, int y, int xa, int xb) {
@@ -218,15 +199,6 @@ __device__ __forceinline__ bool span_has_object(const BreakoutState& s, int y, i
          xa < kLivesX + (s.lives - 1) * kLivesPitch + kLivesW;
 }
 
-// The 16 bytes of a word whose first byte is channel K of pixel 0 of rgb[0..5].
-template <int K>
-__device__ __forceinline__ uint4 pack_word(const uint32_t (&rgb)[6]) {
-  uint32_t w[4] = {0, 0, 0, 0};
-#pragma unroll
-  for (int b = 0; b < 16; ++b) w[b >> 2] |= ((rgb[(K + b) / 3] >> (8 * ((K + b) % 3))) & 0xFFu) << (8 * (b & 3));
-  return make_uint4(w[0], w[1], w[2], w[3]);
-}
-
 template <bool kStep>
 __global__ void __launch_bounds__(kThreads) breakout_kernel(const dz_breakout_config cfg, int32_t* __restrict__ state,
                                                             const int32_t* __restrict__ control,
@@ -236,7 +208,7 @@ __global__ void __launch_bounds__(kThreads) breakout_kernel(const dz_breakout_co
   __shared__ BreakoutState s_state;
   const int E = cfg.num_streams, e = blockIdx.x;
   if (threadIdx.x == 0) {
-    BreakoutState s = load_state(state, E, e);
+    BreakoutState s = load_state<BreakoutState>(state, E, e);
     if (kStep) {
       const Step r = breakout_tick(s, cfg, cfg.stream_offset + (uint32_t)e, control[e], control[E + e] != 0);
       store_state(s, state, E, e);
@@ -266,17 +238,7 @@ __global__ void __launch_bounds__(kThreads) breakout_kernel(const dz_breakout_co
 }
 
 int check_config(const dz_breakout_config* cfg) {
-  if (!cfg) return fail(DZ_EINVAL, "dz_breakout: null config");
-  if (cfg->num_streams < 1 || cfg->num_streams > DZ_BREAKOUT_MAX_STREAMS)
-    return fail(DZ_EINVAL, "dz_breakout: num_streams must be in [1, 4096]");
-  if (cfg->num_actions < 4 || cfg->num_actions > 18)
-    return fail(DZ_EINVAL, "dz_breakout: num_actions must be in [4, 18]");
-  if (cfg->min_noop_steps < 0 || cfg->min_noop_steps > cfg->max_noop_steps ||
-      cfg->max_noop_steps > DZ_BREAKOUT_MAX_NOOP_STEPS)
-    return fail(DZ_EINVAL, "dz_breakout: no-op steps must satisfy 0 <= min <= max <= 63");
-  if ((uint64_t)cfg->stream_offset + (uint64_t)cfg->num_streams > (1ull << 32))
-    return fail(DZ_EINVAL, "dz_breakout: stream_offset + num_streams must be <= 2^32");
-  return DZ_OK;
+  return check_game_config(cfg, "dz_breakout", DZ_BREAKOUT_MAX_STREAMS, 4, DZ_BREAKOUT_MAX_NOOP_STEPS);
 }
 
 }  // namespace

@@ -1,10 +1,10 @@
-"""Games at Atari geometry, simulated and rendered on the device: Catch (csrc/dz_env.cu; rules in DESIGN.md §10) and
-Breakout (csrc/dz_breakout.cu; DESIGN.md §11).
+"""Games at Atari geometry, simulated and rendered on the device: Catch (csrc/dz_env.cu; rules in DESIGN.md §10),
+Breakout (csrc/dz_breakout.cu; DESIGN.md §11) and Pong (csrc/dz_pong.cu; DESIGN.md §12).
 
-`VectorCatch` / `VectorBreakout` step E streams of a game with one kernel launch per tick and leave their 210x160x3 RGB
+`VectorCatch` / `VectorBreakout` / `VectorPong` step E streams of a game with one kernel launch per tick and leave their 210x160x3 RGB
 frames in a device tensor, where `agent.VectorTrainer.step` / `agent.VectorEvaluator.step` read them in place: the
 whole loop (environment -> preprocess -> act -> insert -> learn) stays on the GPU but for the actions and a small
-per-stream record.  `Catch` / `Breakout` are one stream with the reference's dm_env surface, for `parts.run_loop` and
+per-stream record.  `Catch` / `Breakout` / `Pong` are one stream with the reference's dm_env surface, for `parts.run_loop` and
 the one-stream agents.
 """
 
@@ -116,7 +116,7 @@ class _VectorGame:
 
   def get_state(self, stream=None) -> Mapping[str, Any]:
     """The configuration and the device state arrays (one int32 [E] array per field of the game's
-    `_lib.CATCH_STATE_FIELDS` / `_lib.BREAKOUT_STATE_FIELDS`), copied to the host."""
+    `_lib.CATCH_STATE_FIELDS` / `_lib.BREAKOUT_STATE_FIELDS` / `_lib.PONG_STATE_FIELDS`), copied to the host."""
     s = torch.cuda.current_stream(self._device) if stream is None else stream
     with torch.cuda.stream(s):
       state = self._state.cpu().numpy()
@@ -227,3 +227,34 @@ class Breakout(_OneStream):
   def __init__(self, seed: int, num_actions: int = 4, min_noop_steps: int = 1, max_noop_steps: int = 30,
                stream_offset: int = 0, device='cuda'):
     self._env = VectorBreakout(1, seed, num_actions, min_noop_steps, max_noop_steps, stream_offset, device)
+
+
+class VectorPong(_VectorGame):
+  """E streams of Pong on the device (the project's own game, DESIGN.md §12, not ALE Pong).
+
+  The surface is `VectorCatch`'s: `reset()` and `step(actions, reset=None, stream=None)` return `(frames, step_type,
+  reward, discount, lives)` with `frames` the device tensor uint8 [E, 210, 160, 3] that every tick overwrites, and
+  `get_state` / `set_state` restore the state and re-render the frames.  Actions: 0 NOOP, 1 FIRE, 2 RIGHT (paddle up),
+  3 LEFT (paddle down), 4 RIGHTFIRE, 5 LEFTFIRE (the order of ALE's minimal Pong set); 6 .. num_actions - 1 do nothing.
+  The agent's paddle is on the right, a scripted opponent's on the left; a point is +1 or -1, lives are always 0, and
+  the episode ends (LAST) when either side reaches 21.  A reset simulates k no-op frames, k uniform in
+  [min_noop_steps, max_noop_steps] with max <= 63, below the 64-frame serve delay, so no ball is served during them.
+  The game has no frame limit: a driver truncates."""
+
+  _STEP, _RENDER, _FIELDS = 'dz_pong_step', 'dz_pong_render', _lib.PONG_STATE_FIELDS
+
+  def __init__(self, num_streams: int, seed: int, num_actions: int = 6, min_noop_steps: int = 1,
+               max_noop_steps: int = 30, stream_offset: int = 0, device='cuda'):
+    E = _check_arguments(num_streams, seed, num_actions, min_noop_steps, max_noop_steps, stream_offset,
+                         _lib.PONG_MAX_STREAMS, 6, _lib.PONG_MAX_NOOP_STEPS, 'a ball could be served')
+    self._setup(_lib.PongConfig(E, num_actions, min_noop_steps, max_noop_steps, seed, stream_offset), device)
+
+
+class Pong(_OneStream):
+  """One stream of Pong with the reference's dm_env surface: `reset()` / `step(action)` return a `parts.TimeStep`
+  whose observation is (rgb uint8 [210, 160, 3] host array, lives).  Backed by `VectorPong(1)`; its trajectory is
+  stream 0 of a `VectorPong` with the same arguments."""
+
+  def __init__(self, seed: int, num_actions: int = 6, min_noop_steps: int = 1, max_noop_steps: int = 30,
+               stream_offset: int = 0, device='cuda'):
+    self._env = VectorPong(1, seed, num_actions, min_noop_steps, max_noop_steps, stream_offset, device)

@@ -588,6 +588,40 @@ int dz_breakout_render(const dz_breakout_config* cfg, int32_t* d_state, uint8_t*
 int dz_test_breakout_step(const dz_breakout_config* cfg, int32_t* state, int32_t action, int32_t reset, uint8_t* frame,
                           int32_t* record);
 
+/* ---- Pong at Atari geometry on the device (DESIGN.md §12) -------------------------------------------------------
+ * The project's own Pong (not ALE's): E streams against a scripted opponent, each simulated and rendered as a
+ * 210x160x3 uint8 RGB frame in HBM.  State: int32 [DZ_PONG_STATE_FIELDS][E] device array (fields paddle_y, opponent_y,
+ * ball_x, ball_y, ball_dx, ball_dy, in_play, serve_timer, agent_score, opponent_score, counter, noops, over); a new
+ * state is all 0 but over = 1, so that the first tick of every stream is a reset.  Stream e's randomness:
+ * key = threefry2x32((0, seed), (stream_offset + e, 2)). */
+#define DZ_PONG_HEIGHT 210
+#define DZ_PONG_WIDTH 160
+#define DZ_PONG_STATE_FIELDS 13
+#define DZ_PONG_RECORD_FIELDS 4
+#define DZ_PONG_MAX_STREAMS 4096
+#define DZ_PONG_MAX_NOOP_STEPS 63   /* below the 64-frame serve delay: no ball is served during the no-ops */
+typedef struct dz_pong_config {
+  int32_t num_streams;      /* E in [1, 4096] */
+  int32_t num_actions;      /* A in [6, 18]: 0 no-op, 1 fire, 2 up, 3 down, 4 up + fire, 5 down + fire, 6.. no-op */
+  int32_t min_noop_steps;   /* 0 <= min <= max <= DZ_PONG_MAX_NOOP_STEPS */
+  int32_t max_noop_steps;
+  uint32_t seed;
+  uint32_t stream_offset;   /* stream_offset + E <= 2^32 */
+} dz_pong_config;
+/* One tick of all E streams, with dz_catch_step's conventions: h_control PINNED int32 [2][E] (actions, reset flags),
+ * checked on the host and copied into d_control; d_state updated, d_frames (device uint8 [E][210][160][3], 16-byte
+ * aligned) rewritten, d_record (device int32 [DZ_PONG_RECORD_FIELDS][E]: step_type, reward, discount, lives)
+ * copied to h_record (PINNED).  All on `stream`; the caller synchronises before reading h_record. */
+int dz_pong_step(const dz_pong_config* cfg, int32_t* d_state, const int32_t* h_control, int32_t* d_control,
+                 uint8_t* d_frames, int32_t* d_record, int32_t* h_record, void* stream);
+/* Renders every stream's frame from d_state (e.g. after the state was restored); the state is not changed. */
+int dz_pong_render(const dz_pong_config* cfg, int32_t* d_state, uint8_t* d_frames, void* stream);
+/* The kernel's tick and picture evaluated on the HOST by the same source: stream id cfg->stream_offset, state int32
+ * [DZ_PONG_STATE_FIELDS] updated in place, frame (NULL: not rendered) 210*160*3 bytes, record int32 [4]; tests
+ * only. */
+int dz_test_pong_step(const dz_pong_config* cfg, int32_t* state, int32_t action, int32_t reset, uint8_t* frame,
+                      int32_t* record);
+
 /* Device pointer + element count of an internal learner buffer of the last update (pass 0: "act1", "act2", "act3",
  * "h1", "h1_val", "dh1", "iqn_e0", "iqn_hi", "iqn_dhi");
  * tests/tools only. */

@@ -1,6 +1,6 @@
 """A device game (`--game catch`: `environments.VectorCatch`, DESIGN.md §10, the default; `--game breakout`:
-`environments.VectorBreakout`, §11) alone and in the loop.  One JSON line per point (with `--game breakout` each carries
-`game`):
+`environments.VectorBreakout`, §11; `--game pong`: `environments.VectorPong`, §12) alone and in the loop.  One JSON line
+per point (with `--game breakout` or `pong` each carries `game`):
 
   * env_step: E in {32, 256, 1024}.  device_us_per_tick: CUDA events around back-to-back ticks (actions copy, kernel,
     record copy) without host synchronisation; store_GBps: the E x 100,800 frame bytes a tick writes over that time;
@@ -11,7 +11,7 @@
   * driver: `tools/run_synthetic.py --env <game> --num_streams 64 --num_eval_streams 64`, with and without
     `--overlap_eval`, wall time of the whole run;
   * learning (`--learning FRAMES`): the learning curve of the GPU learning tests (tests/test_gpu_catch.py,
-    tests/test_gpu_breakout.py): `--agent` (dqn; also rainbow), E = 32, evaluated with epsilon 0.01 on 64 streams every
+    tests/test_gpu_breakout.py, tests/test_gpu_pong.py): `--agent` (dqn; also rainbow), E = 32, evaluated with epsilon 0.01 on 64 streams every
     `--eval_every` frames (`evaluate` says what an evaluation episode is).
 
 The card's name and power limit are read in the same run.
@@ -37,13 +37,18 @@ FRAME_BYTES = 210 * 160 * 3
 # Breakout evaluation: episodes are truncated at this many frames, and every stream plays one frame more than that, so
 # each completes at least one episode (a good policy can keep the ball alive far longer).
 BREAKOUT_EVAL_FRAMES = 4500
+# Pong evaluation, the same way: a game of a random policy lasts about 2,000 frames, and one whose rallies go on can
+# last far longer.
+PONG_EVAL_FRAMES = 6000
 
 
 def make_env(game, num_streams, seed, num_actions=6):
-  """`VectorCatch` or `VectorBreakout` (whose actions 4.. do nothing, so 6-action agents drive both)."""
+  """`VectorCatch`, `VectorBreakout` (whose actions 4.. do nothing, so 6-action agents drive it) or `VectorPong`."""
   from dqn_zoo_b200 import environments
   if game == 'breakout':
     return environments.VectorBreakout(num_streams, seed, num_actions=num_actions)
+  if game == 'pong':
+    return environments.VectorPong(num_streams, seed, num_actions=num_actions)
   return environments.VectorCatch(num_streams, seed, num_actions=num_actions)
 
 
@@ -166,14 +171,15 @@ def evaluate(learner, seed, num_streams=64, game='catch', num_actions=6):
   ticks, no truncation (every stream completes at least one episode: one is at most 20 x 91 + 30 frames).  Breakout:
   an episode runs from its FIRST step to its LAST step or to its BREAKOUT_EVAL_FRAMES-th frame, where it is
   truncated; every stream plays BREAKOUT_EVAL_FRAMES + 1 ticks, so it completes at least one, and the episodes still
-  running at the end are not counted."""
+  running at the end are not counted.  Pong: the same with PONG_EVAL_FRAMES."""
   import run_synthetic
   from dqn_zoo_b200 import agent as ag
   ev = ag.VectorEvaluator(learner, num_streams, 0.01, [0, seed + 2])
   ev.network_params = learner
   env = make_env(game, num_streams, seed + 3, num_actions)
-  if game == 'breakout':
-    loop = run_synthetic.StreamLoop(ev, env, (BREAKOUT_EVAL_FRAMES + 1) * num_streams, BREAKOUT_EVAL_FRAMES)
+  if game in ('breakout', 'pong'):
+    limit = BREAKOUT_EVAL_FRAMES if game == 'breakout' else PONG_EVAL_FRAMES
+    loop = run_synthetic.StreamLoop(ev, env, (limit + 1) * num_streams, limit)
   else:
     loop = run_synthetic.StreamLoop(ev, env, 1900 * num_streams, 0)
   stats = loop.run()
@@ -205,7 +211,7 @@ def learning_run(train_frames, seed=0, num_streams=32, eval_every=0, log=None, g
 
 def main():
   ap = argparse.ArgumentParser()
-  ap.add_argument('--game', default='catch', choices=['catch', 'breakout'])
+  ap.add_argument('--game', default='catch', choices=['catch', 'breakout', 'pong'])
   ap.add_argument('--agent', default='dqn', choices=['dqn', 'rainbow'], help='the agent of the learning curve')
   ap.add_argument('--parts', default='env,train,eval,driver')
   ap.add_argument('--frames', type=int, default=65536, help='frames per timed window of env_train / env_eval')

@@ -23,7 +23,8 @@ simulated and rendered on the device, so its returns measure learning.  With E >
 `VectorCatch` whose frames tensor goes to the trainer or evaluator as it is, with no host staging; with one stream the
 phases play `Catch` through `parts.run_loop`.  `--env breakout` does the same with the device Breakout (DESIGN.md §11;
 `VectorBreakout` / `Breakout`, `--num_actions` in [4, 18]).  Breakout has no frame limit of its own:
-`--max_frames_per_episode` truncates its episodes.
+`--max_frames_per_episode` truncates its episodes.  `--env pong` plays the device Pong against a scripted opponent
+(DESIGN.md §12; `VectorPong` / `Pong`, `--num_actions` in [6, 18]), which has no frame limit either.
 """
 import argparse
 import collections
@@ -246,8 +247,8 @@ def iteration_row(iteration, args, train_stats, eval_stats, train_epsilon):
 
 def parse_args(argv=None):
   ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
-  ap.add_argument('--env', default='synthetic', choices=['synthetic', 'catch', 'breakout'],
-                  help='synthetic: random host frames; catch / breakout: a game simulated and rendered on the device '
+  ap.add_argument('--env', default='synthetic', choices=['synthetic', 'catch', 'breakout', 'pong'],
+                  help='synthetic: random host frames; catch / breakout / pong: a game simulated and rendered on the device '
                        '(dqn_zoo_b200.environments)')
   ap.add_argument('--agent', default='dqn', choices=['dqn', 'double_q', 'prioritized', 'c51', 'qrdqn', 'rainbow', 'iqn'])
   ap.add_argument('--num_actions', type=int, default=6)
@@ -285,6 +286,8 @@ def parse_args(argv=None):
     ap.error('--env catch needs --num_actions in [3, 18]')
   if args.env == 'breakout' and not 4 <= args.num_actions <= 18:
     ap.error('--env breakout needs --num_actions in [4, 18]')
+  if args.env == 'pong' and not 6 <= args.num_actions <= 18:
+    ap.error('--env pong needs --num_actions in [6, 18]')
   if args.checkpoint_path and args.checkpoint_dir:
     ap.error('give --checkpoint_path or --checkpoint_dir, not both')
   return args
@@ -306,7 +309,7 @@ def run(args):
 
   def environment_builder(num_streams=0):
     """A new environment seeded from the run's RandomState; with a device game and num_streams > 0, its vectorised
-    form (VectorCatch, VectorBreakout)."""
+    form (VectorCatch, VectorBreakout, VectorPong)."""
     seed = int(random_state.randint(1, 2 ** 31))
     if args.env == 'catch':
       if num_streams:
@@ -316,6 +319,10 @@ def run(args):
       if num_streams:
         return environments.VectorBreakout(num_streams, seed, num_actions=args.num_actions)
       return environments.Breakout(seed, num_actions=args.num_actions)
+    if args.env == 'pong':
+      if num_streams:
+        return environments.VectorPong(num_streams, seed, num_actions=args.num_actions)
+      return environments.Pong(seed, num_actions=args.num_actions)
     return SyntheticAtari(seed=seed, num_actions=args.num_actions)
 
   def preprocessor_builder():
@@ -359,7 +366,7 @@ def run(args):
     rows.append(row)
 
   pending = None                         # overlap: (iteration, train stats, epsilon, evaluation loop) still evaluating
-  device_game = args.env in ('catch', 'breakout')
+  device_game = args.env in ('catch', 'breakout', 'pong')
   vector_game = device_game and trainer is not None
   while state.iteration <= args.num_iterations:
     # a new environment per iteration: deterministic after a restore
