@@ -149,7 +149,7 @@ _SIGNATURES = {
     'dz_ckpt_digest': (i32, [vp, i64, vp, vp]),
     'dz_ckpt_digest_host': (i32, [vp, i64, C.POINTER(u64)]),
     'dz_ckpt_pool_live': (i32, [C.POINTER(ReplayView), vp, vp, vp, vp]),
-    'dz_ckpt_pool_gather': (i32, [C.POINTER(ReplayView), vp, i64, vp, vp]),
+    'dz_ckpt_snapshot': (i32, [C.POINTER(ReplayView), vp, i64, vp, i64, vp, vp]),
     'dz_ckpt_pool_scatter': (i32, [C.POINTER(ReplayView), vp, i64, vp, vp, vp]),
     'dz_ckpt_pool_rebuild': (i32, [C.POINTER(ReplayView), vp, i64, vp, vp, i64, i64, vp, vp]),
     'dz_ckpt_rows': (i32, [C.POINTER(ReplayView), i64, i64, vp, i32, vp]),

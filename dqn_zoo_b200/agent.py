@@ -182,20 +182,54 @@ class _DeviceAgent(parts.Agent):
     pickle, and the replay (`save_checkpoint`) in `replay/`.  The replay's RandomState belongs to the run, as for
     `get_state`."""
     from dqn_zoo_b200 import checkpoint as ck
-    os.makedirs(directory, exist_ok=True)
+    write = self._checkpoint_writer(snapshot=False)
+    write(directory, ck.Transfer(self._learner.device))
+
+  def snapshot_checkpoint(self):
+    """A `checkpoint.Snapshot` of the agent at the current point of the CUDA stream, after the learn steps already
+    enqueued: device copies of the blobs `save_checkpoint` writes, copies of the host RandomState, seed, IQN jax key
+    and frame_t, and the replay's `snapshot_checkpoint`.  Its `write(directory)` gives the files `save_checkpoint`
+    would give now, byte for byte, while training goes on."""
+    from dqn_zoo_b200 import checkpoint as ck
+    held = []
+    return ck.Snapshot(self._checkpoint_writer(snapshot=True, held=held), held, self._learner.device)
+
+  def snapshot_checkpoint_bytes(self) -> int:
+    """An upper bound of the device memory `snapshot_checkpoint()` takes now."""
     L = self._learner
-    digests = {}
+    return (sum(getattr(L, name).numel() * getattr(L, name).element_size() for name in self._CHECKPOINT_BLOBS) +
+            self._replay.snapshot_checkpoint_bytes())
+
+  def _checkpoint_writer(self, snapshot, held=None):
+    """(directory, xfer) -> None writing the agent's checkpoint directory: the one definition of its files, fed by
+    the live blobs (snapshot=False) or by copies taken now on the current stream (appended to `held`)."""
+    from dqn_zoo_b200 import checkpoint as ck
+    from dqn_zoo_b200 import replay as replay_lib
+    L = self._learner
+    blobs = {}
     for name in self._CHECKPOINT_BLOBS:
-      a = getattr(L, name).cpu().numpy()
-      np.save(os.path.join(directory, name + '.npy'), a)
-      digests[name] = ck.digest_host(a)
+      t = getattr(L, name)
+      if snapshot:
+        t = t.clone()
+        held.append(t)
+      blobs[name] = t
     state = {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'param_count': L.plan.param_count,
              'opt_state_floats': L.plan.opt_state_floats, 'host_rng': self._host_rng.get_state(), 'seed': self._seed,
              'jax_key': None if getattr(self, '_jax_key', None) is None else self._jax_key.copy(),
-             'frame_t': self._frame_t, 'digests': digests}
-    with open(os.path.join(directory, 'agent.pkl'), 'wb') as f:
-      pickle.dump(state, f, protocol=pickle.HIGHEST_PROTOCOL)
-    self._replay.save_checkpoint(os.path.join(directory, 'replay'))
+             'frame_t': self._frame_t}
+    replay_files = replay_lib._replay_files(self._replay, snapshot, held)
+
+    def write(directory, xfer):
+      os.makedirs(directory, exist_ok=True)
+      digests = {}
+      for name, t in blobs.items():
+        a = t.cpu().numpy()
+        np.save(os.path.join(directory, name + '.npy'), a)
+        digests[name] = ck.digest_host(a)
+      ck.write_bytes(os.path.join(directory, 'agent.pkl'),
+                     pickle.dumps(dict(state, digests=digests), protocol=pickle.HIGHEST_PROTOCOL))
+      replay_files.write(os.path.join(directory, 'replay'), xfer)
+    return write
 
   def load_checkpoint(self, directory: str) -> None:
     """Restores `save_checkpoint` of an agent of the same kind and network.  ValueError (agent and replay untouched)
@@ -884,10 +918,31 @@ class VectorTrainer:
   def save_checkpoint(self, directory: str) -> None:
     """The agent's checkpoint directory (`_DeviceAgent.save_checkpoint`) in `agent/`, plus the per-stream state of
     `get_state` (actions, RandomStates, preprocessor, accumulator, episode statistics) pickled in `trainer.pkl`."""
-    os.makedirs(directory, exist_ok=True)
-    self._agent.save_checkpoint(os.path.join(directory, 'agent'))
-    with open(os.path.join(directory, 'trainer.pkl'), 'wb') as f:
-      pickle.dump(self._stream_state(), f, protocol=pickle.HIGHEST_PROTOCOL)
+    from dqn_zoo_b200 import checkpoint as ck
+    self._checkpoint_writer(snapshot=False)(directory, ck.Transfer(self._agent.learner.device))
+
+  def snapshot_checkpoint(self):
+    """A `checkpoint.Snapshot` of the trainer after the learn steps of the ticks so far (`_DeviceAgent.
+    snapshot_checkpoint`), with the per-stream state pickled now.  Its `write(directory)` gives the files
+    `save_checkpoint` would give now, byte for byte, while later ticks run."""
+    from dqn_zoo_b200 import checkpoint as ck
+    held = []
+    return ck.Snapshot(self._checkpoint_writer(snapshot=True, held=held), held, self._agent.learner.device)
+
+  def snapshot_checkpoint_bytes(self) -> int:
+    """An upper bound of the device memory `snapshot_checkpoint()` takes now."""
+    return self._agent.snapshot_checkpoint_bytes()
+
+  def _checkpoint_writer(self, snapshot, held=None):
+    from dqn_zoo_b200 import checkpoint as ck
+    streams = pickle.dumps(self._stream_state(), protocol=pickle.HIGHEST_PROTOCOL)
+    agent = self._agent._checkpoint_writer(snapshot, held)
+
+    def write(directory, xfer):
+      os.makedirs(directory, exist_ok=True)
+      agent(os.path.join(directory, 'agent'), xfer)
+      ck.write_bytes(os.path.join(directory, 'trainer.pkl'), streams)
+    return write
 
   def load_checkpoint(self, directory: str) -> None:
     """Restores `save_checkpoint` of a trainer with the same stream count over the same kind of agent."""

@@ -1,4 +1,5 @@
-// Checkpoint transfers (DESIGN.md §9): the chunk digest, the frame pool's export (live-plane list, plane gather) and
+// Checkpoint transfers (DESIGN.md §9): the chunk digest, the frame pool's export (live-plane list), the snapshot pass
+// that packs either layout's bulk records and digests them per chunk in one read, the pool's
 // import (plane scatter, refcount / hash / table rebuild with consistency checks), and the pitched row copies of the
 // transition-major layout.
 //
@@ -107,25 +108,120 @@ __global__ void __launch_bounds__(kCompactThreads) pool_compact_kernel(dz_replay
   if (threadIdx.x == 0) *count = s_base;
 }
 
-// Planes ids[0..n) <-> a packed buffer of n * frame_bytes bytes (no stride padding); a warp per plane.  On import the
-// padding bytes [frame_bytes, frame_stride) are zeroed, as every add leaves them.
-__global__ void __launch_bounds__(256) pool_gather_kernel(dz_replay_view v, const int32_t* __restrict__ ids, int64_t n,
-                                                          uint8_t* __restrict__ dst) {
+// The snapshot pass: records ids[0..n) of the replay's bulk storage packed into dst in file order, and the digest sum S
+// of every chunk of that packed stream, in one read of the source.  Record q is `units` pieces of unit_bytes, piece u
+// at base + (ids[q] * units + u) * unit_pitch: one plane of the frame pool (units = 1, pitch frame_stride) or the
+// s_tm1 | s_t observations of one transition-major row (units = 2, pitch obs_stride).  Chunks hold whole records, so a
+// record lies in one chunk; a word may still straddle two records when the record size is not a multiple of 8.
+struct SnapSource {
+  const uint8_t* base;
+  const int32_t* ids;
+  int64_t unit_bytes, unit_pitch;
+  int units;
+};
+
+__device__ __forceinline__ const uint8_t* snap_piece(const SnapSource& s, int64_t q, int u) {
+  return s.base + ((int64_t)s.ids[q] * s.units + u) * s.unit_pitch;
+}
+
+__device__ __forceinline__ void snap_flush(uint64_t acc, int64_t chunk, unsigned long long* sums) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0 && acc) atomicAdd(&sums[chunk], (unsigned long long)acc);
+}
+
+// unit_bytes % 16 == 0 and 16-byte aligned base and dst: a warp per record with 16-byte loads and stores, each warp
+// over a contiguous range of records, so it flushes its partial sum once per chunk it touches.
+constexpr int kSnapUnroll = 4;
+__global__ void __launch_bounds__(256, 4) snapshot_vec_kernel(SnapSource s, int64_t n, uint8_t* __restrict__ dst,
+                                                              int64_t recs_per_chunk, unsigned long long* sums) {
   dz::pdl_enter();
-  const int64_t q = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
-  if (q >= n) return;
-  const uint8_t* src = pool_plane(v, ids[q]);
-  uint8_t* out = dst + q * v.frame_bytes;
   const int lane = threadIdx.x & 31;
-  if ((v.frame_bytes & 15) == 0) {
-    const uint4* s4 = reinterpret_cast<const uint4*>(src);
-    uint4* d4 = reinterpret_cast<uint4*>(out);
-    for (int64_t i = lane; i < (v.frame_bytes >> 4); i += 32) d4[i] = s4[i];
-  } else {
-    for (int64_t i = lane; i < v.frame_bytes; i += 32) out[i] = src[i];
+  const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const int64_t per = (n + warps - 1) / warps;
+  const int64_t q0 = warp * per, q1 = q0 + per < n ? q0 + per : n;
+  const int64_t vecs = s.unit_bytes >> 4;                 // 16-byte vectors per piece
+  const int64_t rec_words = 2 * vecs * s.units;           // 8-byte words per record
+  uint64_t acc = 0;
+  int64_t chunk = q0 < q1 ? q0 / recs_per_chunk : 0;
+  for (int64_t q = q0; q < q1; ++q) {
+    const int64_t k = q / recs_per_chunk;
+    if (k != chunk) {
+      snap_flush(acc, chunk, sums);
+      acc = 0;
+      chunk = k;
+    }
+    uint4* out = reinterpret_cast<uint4*>(dst) + q * vecs * s.units;
+    const int64_t w_rec = (q - k * recs_per_chunk) * rec_words;   // the record's first word within its chunk
+    for (int u = 0; u < s.units; ++u) {
+      const uint4* in = reinterpret_cast<const uint4*>(snap_piece(s, q, u));
+      for (int64_t v0 = lane; v0 < vecs; v0 += 32 * kSnapUnroll) {
+        uint4 x[kSnapUnroll];
+#pragma unroll
+        for (int j = 0; j < kSnapUnroll; ++j)
+          if (v0 + 32 * j < vecs) x[j] = __ldcs(in + v0 + 32 * j);
+#pragma unroll
+        for (int j = 0; j < kSnapUnroll; ++j) {
+          const int64_t v = v0 + 32 * j;
+          if (v < vecs) {
+            __stcs(out + u * vecs + v, x[j]);
+            const int64_t w = w_rec + 2 * (u * vecs + v);
+            acc += ckpt_word_hash((uint64_t)x[j].x | (uint64_t)x[j].y << 32, w) +
+                   ckpt_word_hash((uint64_t)x[j].z | (uint64_t)x[j].w << 32, w + 1);
+          }
+        }
+      }
+    }
+  }
+  if (q0 < q1) snap_flush(acc, chunk, sums);
+}
+
+// Any geometry: a thread per 8-byte word of a chunk, byte by byte (a word may take bytes of two records and of both
+// pieces of a row; the last word of a chunk is zero padded).  Partial sums are flushed when a thread changes chunk.
+__global__ void __launch_bounds__(256) snapshot_word_kernel(SnapSource s, int64_t n, uint8_t* __restrict__ dst,
+                                                            int64_t chunk_bytes, unsigned long long* sums) {
+  dz::pdl_enter();
+  const int64_t rec = s.unit_bytes * s.units, total = n * rec;
+  const int64_t words_per_chunk = (chunk_bytes + 7) >> 3;
+  const int64_t last = (total - 1) / chunk_bytes;
+  const int64_t words = last * words_per_chunk + ((total - last * chunk_bytes + 7) >> 3);
+  uint64_t acc = 0;
+  int64_t chunk = -1;
+  for (int64_t g = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; g < words; g += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t k = g / words_per_chunk, i = g - k * words_per_chunk;
+    if (k != chunk) {
+      if (chunk >= 0 && acc) atomicAdd(&sums[chunk], (unsigned long long)acc);
+      acc = 0;
+      chunk = k;
+    }
+    const int64_t c0 = k * chunk_bytes;
+    const int64_t end = total - c0 < chunk_bytes ? total - c0 : chunk_bytes;
+    uint64_t w = 0;
+    for (int64_t b = 8 * i; b < 8 * i + 8 && b < end; ++b) {
+      const int64_t p = c0 + b, q = p / rec, r = p - q * rec;
+      const int u = (int)(r / s.unit_bytes);
+      const uint8_t x = snap_piece(s, q, u)[r - u * s.unit_bytes];
+      dst[p] = x;
+      w |= (uint64_t)x << (8 * (b - 8 * i));
+    }
+    acc += ckpt_word_hash(w, i);
+  }
+  if (chunk >= 0 && acc) atomicAdd(&sums[chunk], (unsigned long long)acc);
+}
+
+// digest_k = mix64(S_k ^ bytes of chunk k)
+__global__ void __launch_bounds__(256) snapshot_final_kernel(unsigned long long* sums, int64_t nchunks,
+                                                             int64_t chunk_bytes, int64_t total) {
+  dz::pdl_enter();
+  for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < nchunks; k += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t nk = total - k * chunk_bytes < chunk_bytes ? total - k * chunk_bytes : chunk_bytes;
+    sums[k] = ckpt_mix64(sums[k] ^ (uint64_t)nk);
   }
 }
 
+// Packed planes -> planes ids[0..n); a warp per plane.  The padding bytes [frame_bytes, frame_stride) are zeroed, as
+// every add leaves them.
 __global__ void __launch_bounds__(256) pool_scatter_kernel(dz_replay_view v, const int32_t* __restrict__ ids, int64_t n,
                                                            const uint8_t* __restrict__ src, int32_t* bad) {
   dz::pdl_enter();
@@ -275,12 +371,35 @@ int dz_ckpt_pool_live(const dz_replay_view* view, int32_t* d_ids, uint64_t* d_ha
   return DZ_OK;
 }
 
-int dz_ckpt_pool_gather(const dz_replay_view* view, const int32_t* d_ids, int64_t n, uint8_t* d_dst, void* stream) {
-  DZ_TRY(check_pool(view));
+int dz_ckpt_snapshot(const dz_replay_view* view, const int32_t* d_ids, int64_t n, uint8_t* d_dst, int64_t chunk_bytes,
+                     uint64_t* d_digests, void* stream) {
+  SnapSource s{};
+  if (view->d_planes) {
+    DZ_TRY(check_pool(view));
+    s = SnapSource{view->d_frames, d_ids, view->frame_bytes, view->frame_stride, 1};
+  } else {
+    if (!view->d_obs || view->obs_bytes < 1 || view->obs_stride < view->obs_bytes)
+      return fail(DZ_EINVAL, "neither a frame-deduplicated nor an allocated transition-major replay view");
+    s = SnapSource{view->d_obs, d_ids, view->obs_bytes, view->obs_stride, 2};
+  }
+  const int64_t rec = s.unit_bytes * s.units;
   if (n < 0) return fail(DZ_EINVAL, "n must be >= 0");
+  if (chunk_bytes < rec || chunk_bytes % rec) return fail(DZ_EINVAL, "chunk_bytes must be a positive multiple of the record size");
   if (n == 0) return DZ_OK;
-  if ((view->frame_bytes & 15) == 0 && (uintptr_t)d_dst % 16) return fail(DZ_EINVAL, "d_dst must be 16-byte aligned");
-  DZ_LAUNCH(pool_gather_kernel, (int)ceil_div(n * 32, 256), 256, 0, stream, *view, d_ids, n, d_dst);
+  if (!d_ids || !d_dst || !d_digests) return fail(DZ_EINVAL, "null pointer");
+  if ((uintptr_t)d_digests % 8) return fail(DZ_EINVAL, "d_digests must be 8-byte aligned");
+  const int64_t total = n * rec, nchunks = ceil_div(total, chunk_bytes);
+  unsigned long long* sums = reinterpret_cast<unsigned long long*>(d_digests);
+  DZ_CUDA_OK(cudaMemsetAsync(d_digests, 0, nchunks * sizeof(uint64_t), (cudaStream_t)stream));
+  const bool vec = s.unit_bytes % 16 == 0 && s.unit_pitch % 16 == 0 && (uintptr_t)s.base % 16 == 0 &&
+                   (uintptr_t)d_dst % 16 == 0;
+  if (vec) {
+    const int grid = (int)std::min<int64_t>(ceil_div(n * 32, 256), kNumSMs * 4);
+    DZ_LAUNCH(snapshot_vec_kernel, grid, 256, 0, stream, s, n, d_dst, chunk_bytes / rec, sums);
+  } else {
+    DZ_LAUNCH(snapshot_word_kernel, grid_for(ceil_div(total, 8), 256), 256, 0, stream, s, n, d_dst, chunk_bytes, sums);
+  }
+  DZ_LAUNCH(snapshot_final_kernel, grid_for(nchunks, 256), 256, 0, stream, sums, nchunks, chunk_bytes, total);
   return DZ_OK;
 }
 

@@ -26,6 +26,7 @@ No CPU fallback: every numeric result returned by `sample()` is computed on the 
 from __future__ import annotations
 
 import collections
+import copy
 import ctypes as C
 import os
 from typing import Any, Callable, Iterable, List, Mapping, NamedTuple, Optional, Sequence, Tuple
@@ -1183,6 +1184,18 @@ class TransitionReplay:
     naming the file (and chunk) and leaves the replay empty."""
     _load_checkpoint(self, directory)
 
+  def snapshot_checkpoint(self):
+    """A `checkpoint.Snapshot` of the replay at the current point of the CUDA stream (DESIGN.md §9): device copies of
+    the per-row scalars, the sum tree or id mirror, the plane table, the free stack and the live planes' ids and
+    hashes, the observation bytes of the live rows packed and digested in one pass, and copies of the host
+    bookkeeping.  Its `write(directory)` gives the files `save_checkpoint(directory)` would give now, byte for byte,
+    while the replay goes on changing."""
+    return _snapshot_checkpoint(self)
+
+  def snapshot_checkpoint_bytes(self) -> int:
+    """An upper bound of the device memory `snapshot_checkpoint()` takes now (a synchronising read)."""
+    return _snapshot_bytes(self)
+
   def check_valid(self) -> Tuple[bool, str]:
     """`replay.py:195-200`."""
     if self._t < self.size:
@@ -1255,8 +1268,8 @@ def _slot_runs(slots):
 
 
 def _row_copier(rep, live, to_replay):
-  """`Transfer` callback moving packed rows (live ids in order, 2 * obs_bytes each) between the staging buffer and
-  the transition-major rows: with FIFO eviction the live slots are at most two runs, each one pitched copy."""
+  """`Transfer` callback moving packed rows (live ids in order, 2 * obs_bytes each) from the staging buffer to the
+  transition-major rows: with FIFO eviction the live slots are at most two runs, each one pitched copy."""
   st = rep._store
   row = 2 * st.obs_bytes
   v = st.fill_view(_lib.ReplayView())
@@ -1269,71 +1282,121 @@ def _row_copier(rep, live, to_replay):
   return copy
 
 
-def _save_checkpoint(rep, directory):
+def _replay_files(rep, snapshot, held=None):
+  """The files and manifest of the replay's checkpoint directory (`checkpoint.Files`), ordered on the current stream
+  after the work already enqueued there.  snapshot=False: the live arrays, read by the write that follows (the blocking
+  save: host memory bounded by the staging ring).  snapshot=True: device copies (appended to `held`) and copies of the
+  host containers, with the bulk records packed and digested per chunk by one `dz_ckpt_snapshot` pass, so the replay
+  may change before the files are written."""
   from dqn_zoo_b200 import checkpoint as ck
   st, dist = rep._store, rep._distribution
   _raise_if_pool_full(st, rep._flags())
-  os.makedirs(directory, exist_ok=True)
   dist.flush()                                    # device mirrors up to date with the host lists
-  xfer = ck.Transfer(st.action.device)
-  files = {}
-  path = lambda name: os.path.join(directory, name + '.bin')
 
-  def dev(name, nbytes, produce, chunk=None):
-    files[name] = xfer.save_device(path(name), nbytes, produce, chunk)
-
-  def host(name, array):
-    files[name] = ck.Transfer.save_host(path(name), array)
-
+  def dev(t):
+    b = _bytes_of(t)
+    if snapshot:
+      b = b.clone()
+      held.append(b)
+    return b
+  keep = copy.copy if snapshot else (lambda x: x)
+  files = ck.Files()
   live = np.fromiter(rep._live_ids, dtype=np.int64, count=len(rep._live_ids))
-  host('live_ids', live)
+  files.host['live_ids'] = lambda: live
   extra = {}
   if isinstance(dist, UniformDistribution):
-    host('ids', np.asarray(dist._ids, dtype=np.int64))
-    host('id_to_index', _dict_array(dist._id_to_index))
-    dev('ids_mirror', dist._mirror.t.numel() * 8, _bytes_of(dist._mirror.t))
+    ids, id_to_index = keep(dist._ids), keep(dist._id_to_index)
+    files.host['ids'] = lambda: np.asarray(ids, dtype=np.int64)
+    files.host['id_to_index'] = lambda: _dict_array(id_to_index)
+    files.dev['ids_mirror'] = dev(dist._mirror.t)
   else:
-    host('id_to_index', _dict_array(dist._id_to_index))
-    host('index_to_id', _dict_array(dist._index_to_id))
-    host('inactive_indices', np.asarray(dist._inactive_indices, dtype=np.int64))
-    host('active_indices', np.asarray(dist._active_indices, dtype=np.int64))
-    host('active_indices_location', _dict_array(dist._active_indices_location))
+    id_to_index, index_to_id = keep(dist._id_to_index), keep(dist._index_to_id)
+    inactive, active = keep(dist._inactive_indices), keep(dist._active_indices)
+    location = keep(dist._active_indices_location)
+    files.host['id_to_index'] = lambda: _dict_array(id_to_index)
+    files.host['index_to_id'] = lambda: _dict_array(index_to_id)
+    files.host['inactive_indices'] = lambda: np.asarray(inactive, dtype=np.int64)
+    files.host['active_indices'] = lambda: np.asarray(active, dtype=np.int64)
+    files.host['active_indices_location'] = lambda: _dict_array(location)
     tree = dist._sum_tree
-    dev('sum_tree', tree._nodes.numel() * 8, _bytes_of(tree._nodes))
-    dev('live_mirror', dist._live_dev.t.numel() * 8, _bytes_of(dist._live_dev.t))
-    dev('id_at_mirror', dist._id_at_dev.t.numel() * 8, _bytes_of(dist._id_at_dev.t))
+    files.dev['sum_tree'] = dev(tree._nodes)
+    files.dev['live_mirror'] = dev(dist._live_dev.t)
+    files.dev['id_at_mirror'] = dev(dist._id_at_dev.t)
     extra.update(tree_size=tree.size, tree_first_leaf=tree.capacity)
   allocated = st.obs_shape is not None
   if allocated:
     for name in ('action', 'reward', 'discount'):
-      t = getattr(st, name)
-      dev(name, t.numel() * t.element_size(), _bytes_of(t))
+      files.dev[name] = dev(getattr(st, name))
+    device = st.action.device
+    v = st.fill_view(_lib.ReplayView())
     if isinstance(st, _FramePoolStore):
-      v = st.fill_view(_lib.ReplayView())
       fc = st.frame_capacity
-      ids = torch.empty(fc, dtype=torch.int32, device=st.frames.device)
-      hashes = torch.empty(fc, dtype=torch.int64, device=st.frames.device)
-      count = torch.zeros(1, dtype=torch.int64, device=st.frames.device)
-      _lib.call('dz_ckpt_pool_live', C.byref(v), _ptr(ids), _ptr(hashes), _ptr(count), _stream())
+      records = torch.empty(fc, dtype=torch.int32, device=device)    # the live plane ids
+      hashes = torch.empty(fc, dtype=torch.int64, device=device)
+      count = torch.zeros(1, dtype=torch.int64, device=device)
+      _lib.call('dz_ckpt_pool_live', C.byref(v), _ptr(records), _ptr(hashes), _ptr(count), _stream())
       n, top = int(count.item()), int(st.counters.item())
-      fb = st.frame_bytes
-
-      def gather(off, nb, staging):
-        _lib.call('dz_ckpt_pool_gather', C.byref(v), _ptr(ids) + 4 * (off // fb), nb // fb, staging.data_ptr(), _stream())
-        return staging
-      dev('planes', st.planes.numel() * 4, _bytes_of(st.planes))
-      dev('free', top * 4, _bytes_of(st.free[:top]))
-      dev('pool_ids', n * 4, _bytes_of(ids[:n]))
-      dev('pool_hashes', n * 8, _bytes_of(hashes[:n]))
-      dev('frames', n * fb, gather, chunk=max(1, ck.CHUNK_BYTES // fb) * fb)
+      files.dev['planes'] = dev(st.planes)
+      files.dev['free'] = dev(st.free[:top])
+      files.dev['pool_ids'] = dev(records[:n])
+      files.dev['pool_hashes'] = dev(hashes[:n])
+      name, record = 'frames', st.frame_bytes
       extra.update(pool_top=top, pool_planes=n)
     else:
-      row = 2 * st.obs_bytes
-      dev('rows', len(live) * row, _row_copier(rep, live, False), chunk=max(1, ck.CHUNK_BYTES // row) * row)
-  manifest = dict(_checkpoint_header(rep), format=REPLAY_FORMAT, t=rep._t, files=files,
-                  obs_shape=list(st.obs_shape) if allocated else None,
-                  obs_dtype=st.obs_dtype.str if allocated else None, **extra)
-  ck.write_json(os.path.join(directory, ck.MANIFEST), manifest)
+      n = len(live)
+      records = torch.as_tensor((live % rep._capacity).astype(np.int32), device=device)   # the live rows' slots
+      name, record = 'rows', 2 * st.obs_bytes
+    chunk = max(1, ck.CHUNK_BYTES // record) * record
+    if snapshot:
+      packed = torch.empty(max(n * record, 1), dtype=torch.uint8, device=device)
+      digests = torch.empty(max(-(-n * record // chunk), 1), dtype=torch.int64, device=device)
+      _lib.call('dz_ckpt_snapshot', C.byref(v), _ptr(records), n, _ptr(packed), chunk, _ptr(digests), _stream())
+      held.extend([packed, digests])
+      files.bulk = (name, n * record, packed, chunk, digests)
+    else:
+      def pack(off, nb, staging, digest):
+        _lib.call('dz_ckpt_snapshot', C.byref(v), _ptr(records) + 4 * (off // record), nb // record, staging.data_ptr(),
+                  chunk, digest, _stream())
+        return staging
+      files.bulk = (name, n * record, pack, chunk, None)
+  files.manifest = dict(_checkpoint_header(rep), format=REPLAY_FORMAT, t=rep._t,
+                        obs_shape=list(st.obs_shape) if allocated else None,
+                        obs_dtype=st.obs_dtype.str if allocated else None, **extra)
+  return files
+
+
+def _save_checkpoint(rep, directory):
+  from dqn_zoo_b200 import checkpoint as ck
+  _replay_files(rep, False).write(directory, ck.Transfer(rep._store.action.device))
+
+
+def _snapshot_bytes(rep):
+  """An upper bound of the device bytes `_replay_files(rep, True)` allocates, transient buffers included (the frame
+  pool's live count is a synchronising read)."""
+  st, dist = rep._store, rep._distribution
+  mirrors = [dist._mirror.t] if isinstance(dist, UniformDistribution) else [dist._sum_tree._nodes, dist._live_dev.t,
+                                                                            dist._id_at_dev.t]
+  n = sum(t.numel() * t.element_size() for t in mirrors)
+  if st.obs_shape is None:
+    return n
+  n += sum(getattr(st, k).numel() * getattr(st, k).element_size() for k in ('action', 'reward', 'discount'))
+  if isinstance(st, _FramePoolStore):
+    live = st.frame_capacity - int(st.counters.item()) - 1
+    n += st.planes.numel() * 4 + 4 * st.frame_capacity + 24 * st.frame_capacity + live * st.frame_bytes
+    record = st.frame_bytes
+  else:
+    live = len(rep._live_ids)
+    n += live * (4 + 2 * st.obs_bytes)
+    record = 2 * st.obs_bytes
+  from dqn_zoo_b200 import checkpoint as ck
+  return n + 8 * (live * record // max(1, ck.CHUNK_BYTES // record * record) + 1) + 4096
+
+
+def _snapshot_checkpoint(rep):
+  from dqn_zoo_b200 import checkpoint as ck
+  held = []
+  files = _replay_files(rep, True, held)
+  return ck.Snapshot(files.write, held, rep._store.action.device)
 
 
 def _reset_empty(rep):
@@ -1662,6 +1725,14 @@ class PrioritizedTransitionReplay:
   def load_checkpoint(self, directory: str) -> None:
     """As `TransitionReplay.load_checkpoint`."""
     _load_checkpoint(self, directory)
+
+  def snapshot_checkpoint(self):
+    """As `TransitionReplay.snapshot_checkpoint`."""
+    return _snapshot_checkpoint(self)
+
+  def snapshot_checkpoint_bytes(self) -> int:
+    """As `TransitionReplay.snapshot_checkpoint_bytes`."""
+    return _snapshot_bytes(self)
 
   def check_valid(self) -> Tuple[bool, str]:
     """`replay.py:762-768`."""

@@ -15,7 +15,8 @@ Behavioural contract kept from the reference so that its plotting notebook and r
     same three methods (`save`, `can_be_restored`, `restore`) that the reference leaves as a placeholder;
     `DirectoryCheckpoint` is the same surface over a directory, for agents and replays too large to pickle.
 
-Everything here is host-side bookkeeping; nothing touches the GPU."""
+Everything here is host-side bookkeeping; the GPU is touched only through the registered objects, and to read the free
+device memory when `DirectoryCheckpoint.save(blocking=False)` has no explicit budget."""
 
 import collections
 import csv
@@ -24,7 +25,9 @@ import os
 import pickle
 import shutil
 import tempfile
+import threading
 import timeit
+import traceback
 from typing import Any, Iterable, Mapping, Optional, Sequence
 
 
@@ -290,13 +293,26 @@ class DirectoryCheckpoint:
   subdirectory of their own; every other entry is pickled as `FileCheckpoint` pickles it, into `state.pkl`.  Each
   `save()` writes a new generation directory `gen-<n>` and fsyncs it, then switches the `LATEST` file to it by
   write-and-rename, and only then removes the older generations: a save interrupted at any point leaves the previous
-  checkpoint restorable."""
+  checkpoint restorable.
+
+  `save(blocking=False)` snapshots instead: every directory entry's `snapshot_checkpoint()` (device copies taken on the
+  current CUDA stream) and the pickle of the other entries are taken at the call, which then returns; one background
+  thread (not a daemon, so interpreter exit waits for it) writes the generation from the snapshots, fsyncs it,
+  switches `LATEST` and prunes, in the blocking save's order.  One save is in flight at a time: `save`, `restore` and
+  `wait` first wait for it, and re-raise its exception if it failed (its partial generation is removed; `LATEST`
+  still names the previous one).  When the snapshots would not fit in `snapshot_budget` bytes of device memory
+  (default: the free device memory plus what the caching allocator holds unused, less `SNAPSHOT_MARGIN`), or an
+  entry can save but not snapshot, that save is blocking."""
 
   LATEST = 'LATEST'
+  SNAPSHOT_MARGIN = 2 << 30
 
-  def __init__(self, path: str):
+  def __init__(self, path: str, snapshot_budget: Optional[int] = None):
     self._path = path
     self.state = AttributeDict()
+    self.snapshot_budget = snapshot_budget
+    self._writer = None            # the background save's thread
+    self._error = None             # its exception, re-raised by the next wait()
 
   def _latest(self) -> Optional[str]:
     try:
@@ -306,17 +322,55 @@ class DirectoryCheckpoint:
       return None
     return name if name and os.path.isdir(os.path.join(self._path, name)) else None
 
-  def save(self) -> None:
+  def save(self, blocking: bool = True) -> str:
+    """Writes a new generation; returns 'blocking' or 'background', the mode used (see the class)."""
+    self.wait()
     os.makedirs(self._path, exist_ok=True)
+    if not blocking and self._can_snapshot():
+      self._save_background()
+      return 'background'
     gen = self._write_generation()
     self._publish(gen)
+    self._prune(gen)
+    return 'blocking'
+
+  def wait(self) -> None:
+    """Returns when no save is in flight; raises the exception of a background save that failed."""
+    if self._writer is not None:
+      self._writer.join()
+      self._writer = None
+    if self._error is not None:
+      error, self._error = self._error, None
+      raise error
+
+  def _directory_entries(self):
+    return {k: v for k, v in self.state.items() if hasattr(v, 'save_checkpoint') and hasattr(v, 'load_checkpoint')}
+
+  def _can_snapshot(self) -> bool:
+    entries = self._directory_entries()
+    if not all(hasattr(v, 'snapshot_checkpoint') for v in entries.values()):
+      return False
+    need = sum(int(v.snapshot_checkpoint_bytes()) for v in entries.values())
+    return need <= self._snapshot_budget()
+
+  def _snapshot_budget(self) -> int:
+    if self.snapshot_budget is not None:
+      return int(self.snapshot_budget)
+    import torch
+    free, _ = torch.cuda.mem_get_info()
+    return free + torch.cuda.memory_reserved() - torch.cuda.memory_allocated() - self.SNAPSHOT_MARGIN
+
+  def _next_generation(self) -> str:
+    taken = [int(n[4:]) for n in os.listdir(self._path) if n.startswith('gen-') and n[4:].isdigit()]
+    return 'gen-%06d' % (max(taken, default=0) + 1)
+
+  def _prune(self, gen: str) -> None:
     for name in os.listdir(self._path):
       if name.startswith('gen-') and name != gen:
         shutil.rmtree(os.path.join(self._path, name), ignore_errors=True)
 
   def _write_generation(self) -> str:
-    taken = [int(n[4:]) for n in os.listdir(self._path) if n.startswith('gen-') and n[4:].isdigit()]
-    gen = 'gen-%06d' % (max(taken, default=0) + 1)
+    gen = self._next_generation()
     folder = os.path.join(self._path, gen)
     os.makedirs(folder)
     payload = {}
@@ -326,13 +380,53 @@ class DirectoryCheckpoint:
         payload[key] = ('directory', key)
       else:
         payload[key] = FileCheckpoint._snapshot(value)
+    self._finish(folder, pickle.dumps(payload, protocol=pickle.HIGHEST_PROTOCOL))
+    return gen
+
+  @staticmethod
+  def _finish(folder: str, payload: bytes) -> None:
     with open(os.path.join(folder, 'state.pkl'), 'wb') as f:
-      pickle.dump(payload, f, protocol=pickle.HIGHEST_PROTOCOL)
+      f.write(payload)
     for root, _, names in os.walk(folder):
       for name in names:
         _fsync(os.path.join(root, name))
       _fsync(root)
-    return gen
+
+  def _save_background(self) -> None:
+    snapshots, payload = {}, {}
+    try:
+      for key, value in self.state.items():
+        if key in self._directory_entries():
+          snapshots[key] = value.snapshot_checkpoint()
+          payload[key] = ('directory', key)
+        else:
+          payload[key] = FileCheckpoint._snapshot(value)
+      blob = pickle.dumps(payload, protocol=pickle.HIGHEST_PROTOCOL)
+    except BaseException:
+      for snap in snapshots.values():
+        snap.release()
+      raise
+    self._writer = threading.Thread(target=self._write_background, args=(self._next_generation(), snapshots, blob),
+                                    name='DirectoryCheckpoint-writer', daemon=False)
+    self._writer.start()
+
+  def _write_background(self, gen, snapshots, blob) -> None:
+    folder = os.path.join(self._path, gen)
+    try:
+      os.makedirs(folder)
+      for key, snap in snapshots.items():
+        snap.write(os.path.join(folder, key))
+      self._finish(folder, blob)
+      self._publish(gen)
+      self._prune(gen)
+    except BaseException as e:     # kept for the next wait(); the previous generation stays the latest
+      if self._latest() != gen:
+        shutil.rmtree(folder, ignore_errors=True)
+      traceback.clear_frames(e.__traceback__)      # the frames' locals would keep the snapshot's buffers alive
+      self._error = e
+    finally:
+      for snap in snapshots.values():
+        snap.release()
 
   def _publish(self, gen: str) -> None:
     tmp = os.path.join(self._path, self.LATEST + '.tmp')
@@ -347,6 +441,7 @@ class DirectoryCheckpoint:
     return self._latest() is not None
 
   def restore(self) -> None:
+    self.wait()
     gen = self._latest()
     if gen is None:
       raise FileNotFoundError('no checkpoint generation under %s' % self._path)

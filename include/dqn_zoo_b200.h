@@ -230,8 +230,15 @@ int dz_ckpt_digest_host(const void* h_src, int64_t bytes, uint64_t* h_out);
 /* Frame-deduplicated layout.  Live planes (refcount > 0, plane 0 excluded) in increasing id order into
  * d_ids[0..*d_count) with their hashes into d_hashes (both sized frame_capacity); *d_count is a DEVICE int64. */
 int dz_ckpt_pool_live(const dz_replay_view* view, int32_t* d_ids, uint64_t* d_hashes, int64_t* d_count, void* stream);
-/* Planes d_ids[0..n) -> d_dst, packed at frame_bytes per plane (no stride padding). */
-int dz_ckpt_pool_gather(const dz_replay_view* view, const int32_t* d_ids, int64_t n, uint8_t* d_dst, void* stream);
+/* Either layout: records d_ids[0..n) packed into d_dst in file order, and the digest of each chunk of
+ * chunk_bytes (a positive multiple of the record size) of the packed bytes into the DEVICE uint64
+ * d_digests[0..ceil(n * record / chunk_bytes)), each equal to dz_ckpt_digest of that chunk, in one read of
+ * the replay.  Frame-deduplicated view: record q is plane d_ids[q] (frame_bytes, no stride padding).
+ * Transition-major view: record q is row slot d_ids[q], s_tm1 then s_t (2 * obs_bytes).  The ids must name
+ * planes / rows of the view; offsets are 64-bit.  16-byte loads and stores when frame_bytes / obs_bytes is a
+ * multiple of 16 and d_dst is 16-byte aligned.  n = 0 enqueues nothing. */
+int dz_ckpt_snapshot(const dz_replay_view* view, const int32_t* d_ids, int64_t n, uint8_t* d_dst, int64_t chunk_bytes,
+                     uint64_t* d_digests, void* stream);
 /* Packed planes d_src -> planes d_ids[0..n), stride padding zeroed.  An id outside [1, frame_capacity) sets
  * DZ_CKPT_BAD_PLANE_ID in d_bad[0] and is skipped. */
 int dz_ckpt_pool_scatter(const dz_replay_view* view, const int32_t* d_ids, int64_t n, const uint8_t* d_src,

@@ -25,6 +25,11 @@ phases play `Catch` through `parts.run_loop`.  `--env breakout` does the same wi
 `VectorBreakout` / `Breakout`, `--num_actions` in [4, 18]).  Breakout has no frame limit of its own:
 `--max_frames_per_episode` truncates its episodes.  `--env pong` plays the device Pong against a scripted opponent
 (DESIGN.md §12; `VectorPong` / `Pong`, `--num_actions` in [6, 18]), which has no frame limit either.
+
+`--checkpoint_dir D --background_checkpoint` ends each iteration with `DirectoryCheckpoint.save(blocking=False)`: the
+agent and its replay are snapshotted in device memory and the generation is written by a background thread while the
+next iteration trains (DESIGN.md §9); the run waits for the last write before it returns.  The rows are those of the
+blocking saves.
 """
 import argparse
 import collections
@@ -266,6 +271,9 @@ def parse_args(argv=None):
   ap.add_argument('--checkpoint_dir', default='',
                   help='checkpoint into a directory (DirectoryCheckpoint): the agent and its replay are streamed to '
                        'files with bounded host memory')
+  ap.add_argument('--background_checkpoint', action='store_true',
+                  help='with --checkpoint_dir: snapshot the agent and its replay in device memory at the end of each '
+                       'iteration and write the directory on a background thread while training goes on')
   ap.add_argument('--num_streams', type=int, default=1, help='E > 1: train from E environments with agent.VectorTrainer')
   ap.add_argument('--num_eval_streams', type=int, default=0,
                   help='E >= 1: evaluate on E environments of their own with agent.VectorEvaluator')
@@ -290,6 +298,8 @@ def parse_args(argv=None):
     ap.error('--env pong needs --num_actions in [6, 18]')
   if args.checkpoint_path and args.checkpoint_dir:
     ap.error('give --checkpoint_path or --checkpoint_dir, not both')
+  if args.background_checkpoint and not args.checkpoint_dir:
+    ap.error('--background_checkpoint needs --checkpoint_dir')
   return args
 
 
@@ -416,9 +426,14 @@ def run(args):
                                                  itertools.islice(eval_seq, args.num_eval_frames))
     write(state.iteration, train_stats, eval_stats, train_epsilon)
     state.iteration += 1
-    checkpoint.save()
+    if args.background_checkpoint:
+      checkpoint.save(blocking=False)   # a snapshot; the directory is written while the next iteration trains
+    else:
+      checkpoint.save()
   if pending is not None:
     write(pending[0], pending[1], pending[3].run(), pending[2])
+  if args.background_checkpoint:
+    checkpoint.wait()
   writer.close()
   return rows
 
