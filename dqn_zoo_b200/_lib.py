@@ -15,7 +15,7 @@ vp = C.c_void_p
 DZ_FLAG_BAD_VALUE, DZ_FLAG_BAD_INDEX, DZ_FLAG_BAD_TARGET, DZ_FLAG_ROOT_ZERO, DZ_FLAG_NONFINITE_WEIGHT = 1, 2, 4, 8, 16
 DZ_FLAG_FRAME_POOL_FULL = 32
 DZ_CKPT_BAD_PLANE_ID, DZ_CKPT_UNREFERENCED_PLANE, DZ_CKPT_HASH_MISMATCH, DZ_CKPT_BAD_FREE_STACK = 1, 2, 4, 8
-AGENT_KINDS = {'dqn': 0, 'double_q': 1, 'prioritized': 2, 'c51': 3, 'qrdqn': 4, 'rainbow': 5, 'iqn': 6}
+AGENT_KINDS = {'dqn': 0, 'double_q': 1, 'prioritized': 2, 'c51': 3, 'qrdqn': 4, 'rainbow': 5, 'iqn': 6, 'munchausen': 7}
 OPTIMIZERS = {'adam': 0, 'rmsprop': 1}
 
 
@@ -56,7 +56,8 @@ class LearnerConfig(C.Structure):
               ('tau_samples_s_tm1', i32), ('tau_samples_policy', i32), ('tau_samples_s_t', i32), ('batch', i32),
               ('obs_h', i32), ('obs_w', i32), ('obs_c', i32), ('vmax', f32), ('grad_error_bound', f32),
               ('huber_param', f32), ('optimizer', i32), ('learning_rate', f32), ('opt_eps', f32), ('rms_decay', f32),
-              ('adam_b1', f32), ('adam_b2', f32), ('max_global_grad_norm', f32)]
+              ('adam_b1', f32), ('adam_b2', f32), ('max_global_grad_norm', f32), ('munchausen_alpha', f32),
+              ('entropy_temperature', f32), ('log_policy_clip', f32)]
 
 
 class LearnerPlan(C.Structure):
@@ -196,6 +197,7 @@ _SIGNATURES = {
     'dz_pong_render': (i32, [C.POINTER(PongConfig), vp, vp, vp]),
     'dz_test_pong_step': (i32, [C.POINTER(PongConfig), vp, i32, i32, vp, vp]),
     'dz_test_learner_buffer': (i32, [vp, C.c_char_p, vp, vp]),
+    'dz_test_munchausen_example': (i32, [vp, vp, vp, i32, i32, f32, f32, f32, f32, f32, vp]),
     'dz_test_copy': (i32, [vp, vp, i64, vp]),
     'dz_test_learner_trace': (i32, [vp, C.c_char_p, vp]),
     'dz_test_learner_mma_path': (i32, [vp, C.c_char_p, C.POINTER(i32)]),

@@ -1,5 +1,5 @@
-"""The seven dqn_zoo agents behind the reference's `parts.Agent` surface, running on the
-CUDA replay + learner.
+"""The seven dqn_zoo agents, and Munchausen DQN beside them, behind the reference's `parts.Agent`
+surface, running on the CUDA replay + learner.
 
 Each class keeps the reference constructor's argument names and the `step / reset /
 get_state / set_state / statistics` behaviour (dqn/agent.py:133-229, rainbow/agent.py:135-245,
@@ -56,7 +56,7 @@ class _DeviceAgent(parts.Agent):
   def _setup(self, preprocessor, sample_network_input, network: NetworkSpec, optimizer: Optional[OptimizerSpec],
              transition_accumulator, replay, batch_size, exploration_epsilon, min_replay_capacity_fraction,
              learn_period, target_network_update_period, rng_key, grad_error_bound=1.0 / 32, huber_param=1.0,
-             use_cuda_graph=True):
+             use_cuda_graph=True, **munchausen):
     if network.kind != self.KIND:
       raise ValueError('network spec kind %r does not match agent %r' % (network.kind, self.KIND))
     if sample_network_input is not None and tuple(np.asarray(sample_network_input).shape) != tuple(network.obs_shape):
@@ -73,7 +73,7 @@ class _DeviceAgent(parts.Agent):
     self._seed = _seed_of(rng_key)
     self._host_rng = np.random.RandomState(self._seed % (1 << 32))
     self._learner = learner_lib.Learner(network, batch_size=batch_size, optimizer=optimizer,
-                                        grad_error_bound=grad_error_bound, huber_param=huber_param)
+                                        grad_error_bound=grad_error_bound, huber_param=huber_param, **munchausen)
     self._learner.init_params(seed=self._seed % (1 << 31))      # network.init + target = online
     self._action = None
     self._frame_t = -1
@@ -420,6 +420,23 @@ class DoubleQ(Dqn):
   KIND = 'double_q'
 
 
+class Munchausen(_DeviceAgent):
+  """Munchausen DQN (Vieillard, Pietquin & Geist, NeurIPS 2020; DESIGN.md §13): dqn's constructor, network, uniform
+  replay and epsilon-greedy acting, with the soft target r + alpha clip(tau log pi(a_tm1|s_tm1), l0, 0) +
+  discount sum_a pi(a|s_t) (q(s_t, a) - tau log pi(a|s_t)) of the target network's softmax policy pi.  The defaults
+  of `munchausen_alpha`, `entropy_temperature` (tau) and `log_policy_clip` (l0) are the paper's Atari values."""
+  KIND = 'munchausen'
+
+  def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
+               batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
+               target_network_update_period, grad_error_bound, rng_key, use_cuda_graph=True, munchausen_alpha=0.9,
+               entropy_temperature=0.03, log_policy_clip=-1.0):
+    self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
+                exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
+                grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph, munchausen_alpha=munchausen_alpha,
+                entropy_temperature=entropy_temperature, log_policy_clip=log_policy_clip)
+
+
 class PrioritizedDqn(_DeviceAgent):
   """prioritized/agent.py:40-258."""
   KIND = 'prioritized'
@@ -625,7 +642,7 @@ class EpsilonGreedyActor(parts.Agent):
 
 
 AGENTS = {'dqn': Dqn, 'double_q': DoubleQ, 'prioritized': PrioritizedDqn, 'c51': C51, 'qrdqn': QrDqn,
-          'rainbow': Rainbow, 'iqn': Iqn}
+          'rainbow': Rainbow, 'iqn': Iqn, 'munchausen': Munchausen}
 
 
 class BatchedEpsilonGreedyActor:

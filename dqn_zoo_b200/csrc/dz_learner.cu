@@ -7,6 +7,8 @@
 //                 categorical_[double_]q_learning, quantile_q_learning (restated; SURVEY §8(c))
 //   optax 0.1.2   adam, rmsprop(centered), clip_by_global_norm, apply_updates
 //   _learn glue   rainbow/agent.py:181-198, prioritized/agent.py:187-206
+//   munchausen    Munchausen DQN (Vieillard, Pietquin & Geist, NeurIPS 2020), the one agent outside the
+//                 reference: dqn's network with online(s_tm1) | target(s_tm1) | target(s_t) (DESIGN.md §13)
 //
 // Gradients flow only through online(s_tm1).  All forward passes of a layer are one grouped
 // launch (dz_gemm.cuh); the replay gather is fused into conv1's operand load.
@@ -162,8 +164,36 @@ struct Bump {
   }
 };
 
+// ---- Munchausen DQN per-example arithmetic (DESIGN.md §13), shared by loss_munchausen_kernel and its host twin
+// dz_test_munchausen_example.  Each softmax over the target network's A action values enters through two reductions,
+// v = max_a qbar(s, a) and S = sum_a exp((qbar(s, a) - v) / tau), which the kernel forms with warp shuffles and the
+// host twin with the same xor butterfly over an array.  tau log pi(a|s) = qbar(s, a) - v - tau log S, and the bootstrap
+// sum_a pi(a|s_t) (qbar(s_t, a) - tau log pi(a|s_t)) equals v_t + tau log S_t for every a; that form is evaluated: it
+// needs no third reduction and has no cancellation.  Explicit fmaf keeps the host and device roundings the same.
+constexpr int kMunchausenMaxActions = 18;
+
+inline bool munchausen_params_ok(float alpha, float tau, float l0) {
+  return std::isfinite(alpha) && std::isfinite(tau) && std::isfinite(l0) && tau > 0.f && alpha >= 0.f && l0 <= 0.f;
+}
+
+__host__ __device__ inline float munchausen_exp(float qbar, float v, float tau) { return expf((qbar - v) / tau); }
+
+struct MunchausenTarget { float target, bonus; };
+
+__host__ __device__ inline MunchausenTarget munchausen_target(float r, float disc, float qbar_tm1_a, float v_tm1, float s_tm1,
+                                                              float v_t, float s_t, float alpha, float tau, float l0) {
+  const float tau_log_pi = fmaf(-tau, logf(s_tm1), qbar_tm1_a - v_tm1);     // tau log pi(a_tm1 | s_tm1)
+  const float bonus = alpha * fminf(fmaxf(tau_log_pi, l0), 0.f);
+  const float boot = fmaf(tau, logf(s_t), v_t);
+  return MunchausenTarget{fmaf(disc, boot, r + bonus), bonus};
+}
+
 static int validate(const dz_learner_config& c) {
-  if (c.kind < 0 || c.kind > DZ_IQN) return fail(DZ_EINVAL, "unknown agent kind");
+  if (c.kind < 0 || c.kind > DZ_MUNCHAUSEN) return fail(DZ_EINVAL, "unknown agent kind");
+  if (c.kind == DZ_MUNCHAUSEN && !munchausen_params_ok(c.munchausen_alpha, c.entropy_temperature, c.log_policy_clip))
+    return fail(DZ_EINVAL, "munchausen needs finite alpha >= 0, entropy_temperature > 0 and log_policy_clip <= 0");
+  if (c.kind == DZ_MUNCHAUSEN && c.num_actions > kMunchausenMaxActions)
+    return fail(DZ_EINVAL, "munchausen: num_actions must be in [1,18] (one warp lane per action)");
   if (c.batch <= 0 || c.batch > 1024) return fail(DZ_EINVAL, "batch must be in [1,1024]");
   if (c.obs_c != 4) return fail(DZ_EINVAL, "obs_c must be 4 (stacked frames; conv1 reads uchar4 pixels)");
   if (c.obs_w % 4) return fail(DZ_EINVAL, "obs_w must be a multiple of 4");
@@ -619,6 +649,36 @@ __global__ void __launch_bounds__(64) loss_q_kernel(LossArgs L) {
   L.per_example[b] = td;
   if (L.priorities) L.priorities[b] = fabsf(td);                   // prioritized/agent.py:201
   L.loss_terms[b] = w * 0.5f * td * td;
+}
+
+// munchausen: one warp per example, lane a holding action a of the target network's passes on s_tm1 (out1) and s_t
+// (out2); the target of DESIGN.md §13, then dqn's clip_gradient + l2_loss on td = target - q(s_tm1, a_tm1).  The
+// per-example value is the loss 0.5 td^2.
+__global__ void __launch_bounds__(128) loss_munchausen_kernel(LossArgs L, float alpha, float tau, float l0) {
+  dz::pdl_enter();
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= L.B) return;   // the whole warp leaves together
+  const int A = L.A;
+  const long long row = (long long)b * A;
+  const bool act = lane < A;
+  const float qbar_tm1 = act ? L.out1[row + lane] : -INFINITY;
+  const float qbar_t = act ? L.out2[row + lane] : -INFINITY;
+  const float v_tm1 = warp_max(qbar_tm1), v_t = warp_max(qbar_t);
+  const float s_tm1 = warp_sum(act ? munchausen_exp(qbar_tm1, v_tm1, tau) : 0.f);
+  const float s_t = warp_sum(act ? munchausen_exp(qbar_t, v_t, tau) : 0.f);
+  const int at = L.a[b];
+  const float qbar_a = __shfl_sync(0xffffffffu, qbar_tm1, at);
+  const MunchausenTarget m = munchausen_target(L.r[b], L.disc[b], qbar_a, v_tm1, s_tm1, v_t, s_t, alpha, tau, l0);
+  const float td = m.target - L.out0[row + at];
+  const float w = L.w ? L.w[b] : 1.0f;
+  const float g = fminf(fmaxf(w * td / (float)L.B, -L.bound), L.bound);   // cotangent reaching clip_gradient
+  if (act) L.dout[row + lane] = lane == at ? -g : 0.f;
+  if (lane == 0) {
+    const float loss = 0.5f * td * td;
+    L.per_example[b] = loss;
+    L.loss_terms[b] = w * loss;
+  }
 }
 
 // c51 / rainbow: categorical_[double_]q_learning with categorical_l2_project + cross entropy.
@@ -1402,7 +1462,8 @@ UmNetDesc make_um_desc(const dz_learner* l) {
   memset(&u, 0, sizeof(u));
   const bool needs_online_st = c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED || c.kind == DZ_RAINBOW;
   u.B = c.batch; u.H = d.H; u.W = d.W;
-  u.npass = needs_online_st ? 3 : 2;
+  const bool mdqn = c.kind == DZ_MUNCHAUSEN;   // online(s_tm1) | target(s_tm1) | target(s_t)
+  u.npass = needs_online_st || mdqn ? 3 : 2;
   u.pass_target[0] = 0; u.pass_target[1] = needs_online_st ? 0 : 1; u.pass_target[2] = 1;
   u.online = l->buf.d_online; u.target = l->buf.d_target;
   for (int i = 0; i < 3; ++i) { u.off_conv_w[i] = o.conv_w[i]; u.off_conv_b[i] = o.conv_b[i]; }
@@ -2305,8 +2366,10 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   // ---- forward: every network.apply of loss_fn in grouped launches
   TorsoJob jobs[3];
   int nj = 0;
+  const bool mdqn = c.kind == DZ_MUNCHAUSEN;   // the target network also applies to s_tm1 (the log-policy bonus)
   jobs[nj++] = TorsoJob{on, batch->d_s_tm1_rows, 0};
   if (needs_online_st) jobs[nj++] = TorsoJob{on, batch->d_s_t_rows, 1};
+  if (mdqn) jobs[nj++] = TorsoJob{tg, batch->d_s_tm1_rows, 1};
   jobs[nj++] = TorsoJob{tg, batch->d_s_t_rows, 2};
   const bool um = l->um != nullptr;
   if (um) {
@@ -2338,6 +2401,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     int np = 0;
     passes[np++] = Pass{on, 0, 0, 0};
     if (needs_online_st) passes[np++] = Pass{on, 1, 1, 0};
+    if (mdqn) passes[np++] = Pass{tg, 1, 1, 0};
     passes[np++] = Pass{tg, 2, 2, 0};
     DZ_TRY(forward_heads_plain(l, learner_bufs(l), passes, np, B, stream, um));
   }
@@ -2355,6 +2419,9 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   L.priorities = (c.kind == DZ_RAINBOW || c.kind == DZ_PRIORITIZED) ? out->d_priorities : nullptr;
   if (c.kind == DZ_DQN || c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED) {
     DZ_LAUNCH(loss_q_kernel, B, 64, 0, stream, L);
+  } else if (mdqn) {
+    DZ_LAUNCH(loss_munchausen_kernel, (B + 3) / 4, 128, 0, stream, L, c.munchausen_alpha, c.entropy_temperature,
+              c.log_policy_clip);
   } else if (c.kind == DZ_C51 || c.kind == DZ_RAINBOW) {
     DZ_LAUNCH_NAMED("loss_categorical_kernel", loss_categorical_staged_kernel, B, 128, categorical_loss_smem(c), stream, L);
   } else {
@@ -3015,6 +3082,38 @@ int dz_test_learner_mma_path(dz_learner* l, const char* tag, int32_t* path) {
 // Test hook: device-to-device copy out of an internal buffer (tests hold only the raw pointer).
 int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream) {
   DZ_CUDA_OK(cudaMemcpyAsync(d_dst, d_src, (size_t)bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return DZ_OK;
+}
+
+// Host twin of loss_munchausen_kernel's per-example arithmetic: the warp's xor-butterfly reductions over an array of 32
+// lanes, then the same munchausen_exp / munchausen_target (tests only).
+int dz_test_munchausen_example(const float* q_tm1, const float* qbar_tm1, const float* qbar_t, int32_t A, int32_t a_tm1,
+                               float r_t, float discount_t, float alpha, float tau, float l0, float* out) {
+  if (!q_tm1 || !qbar_tm1 || !qbar_t || !out) return fail(DZ_EINVAL, "munchausen example: NULL buffer");
+  if (A < 1 || A > kMunchausenMaxActions || a_tm1 < 0 || a_tm1 >= A) return fail(DZ_EINVAL, "munchausen example: A or a_tm1 out of range");
+  if (!munchausen_params_ok(alpha, tau, l0)) return fail(DZ_EINVAL, "munchausen example: bad alpha / tau / l0");
+  auto butterfly = [](float* v, bool is_max) {
+    for (int o = 16; o > 0; o >>= 1) {
+      float t[32];
+      for (int i = 0; i < 32; ++i) t[i] = is_max ? fmaxf(v[i], v[i ^ o]) : v[i] + v[i ^ o];
+      for (int i = 0; i < 32; ++i) v[i] = t[i];
+    }
+    return v[0];
+  };
+  float red[2][2];   // [s_tm1, s_t][max, sum]
+  const float* q[2] = {qbar_tm1, qbar_t};
+  for (int s = 0; s < 2; ++s) {
+    float v[32];
+    for (int i = 0; i < 32; ++i) v[i] = i < A ? q[s][i] : -INFINITY;
+    red[s][0] = butterfly(v, true);
+    for (int i = 0; i < 32; ++i) v[i] = i < A ? munchausen_exp(q[s][i], red[s][0], tau) : 0.f;
+    red[s][1] = butterfly(v, false);
+  }
+  const MunchausenTarget m = munchausen_target(r_t, discount_t, qbar_tm1[a_tm1], red[0][0], red[0][1], red[1][0], red[1][1],
+                                               alpha, tau, l0);
+  out[0] = m.target;
+  out[1] = m.target - q_tm1[a_tm1];
+  out[2] = m.bonus;
   return DZ_OK;
 }
 

@@ -46,6 +46,8 @@ def default_optimizer(kind: str) -> OptimizerSpec:
     return OptimizerSpec('adam', 0.0000625, 0.005 / 32, max_global_grad_norm=10.0)  # rainbow/run_atari.py:229-235
   if kind == 'iqn':
     return OptimizerSpec('adam', 0.00005, 0.01 / 32)
+  if kind == 'munchausen':
+    return OptimizerSpec('adam', 0.00005, 0.01 / 32)   # the M-DQN paper's Atari values; no run_atari pins them
   raise ValueError(kind)
 
 
@@ -116,7 +118,11 @@ class Learner:
   """Device-resident parameters, optimizer state and workspace + the fused update."""
 
   def __init__(self, net: NetworkSpec, batch_size: int = 32, optimizer: Optional[OptimizerSpec] = None,
-               grad_error_bound: float = 1.0 / 32, huber_param: float = 1.0, device=None):
+               grad_error_bound: float = 1.0 / 32, huber_param: float = 1.0, munchausen_alpha: float = 0.9,
+               entropy_temperature: float = 0.03, log_policy_clip: float = -1.0, device=None):
+    """`munchausen_alpha`, `entropy_temperature` (tau) and `log_policy_clip` (l0) are Munchausen DQN's (DESIGN.md §13,
+    defaults the paper's Atari values); the library rejects tau <= 0, alpha < 0, l0 > 0 and non-finite values for that
+    kind, and the other kinds ignore them."""
     if not torch.cuda.is_available():
       raise RuntimeError('dqn_zoo_b200.learner needs a CUDA device (there is no CPU fallback)')
     self.net = net
@@ -134,6 +140,7 @@ class Learner:
     cfg.optimizer = _lib.OPTIMIZERS[self.opt.name]
     cfg.learning_rate, cfg.opt_eps, cfg.rms_decay = self.opt.learning_rate, self.opt.eps, self.opt.decay
     cfg.adam_b1, cfg.adam_b2, cfg.max_global_grad_norm = self.opt.b1, self.opt.b2, self.opt.max_global_grad_norm
+    cfg.munchausen_alpha, cfg.entropy_temperature, cfg.log_policy_clip = munchausen_alpha, entropy_temperature, log_policy_clip
     self.cfg = cfg
     plan = _lib.LearnerPlan()
     _lib.call('dz_learner_plan_query', C.byref(cfg), C.byref(plan))

@@ -309,7 +309,10 @@ int dz_replay_update_priorities(const dz_replay_view* view, const int64_t* d_ind
  * iqn/agent.py:178-226; networks: networks.py:58-363)
  * ---------------------------------------------------------------------------------------- */
 
-enum dz_agent_kind { DZ_DQN = 0, DZ_DOUBLE_Q = 1, DZ_PRIORITIZED = 2, DZ_C51 = 3, DZ_QRDQN = 4, DZ_RAINBOW = 5, DZ_IQN = 6 };
+/* DZ_MUNCHAUSEN: Munchausen DQN (Vieillard, Pietquin & Geist, NeurIPS 2020), the one agent outside the reference tree:
+ * dqn's network, parameter layout and acting, with the soft, log-policy-augmented target of DESIGN.md §13. */
+enum dz_agent_kind { DZ_DQN = 0, DZ_DOUBLE_Q = 1, DZ_PRIORITIZED = 2, DZ_C51 = 3, DZ_QRDQN = 4, DZ_RAINBOW = 5, DZ_IQN = 6,
+                     DZ_MUNCHAUSEN = 7 };
 enum dz_optimizer_kind { DZ_ADAM = 0, DZ_RMSPROP_CENTERED = 1 };
 
 typedef struct dz_learner_config {
@@ -327,6 +330,11 @@ typedef struct dz_learner_config {
   int32_t optimizer;         /* dz_optimizer_kind */
   float learning_rate, opt_eps, rms_decay, adam_b1, adam_b2;
   float max_global_grad_norm; /* 0 = off (optax.clip_by_global_norm) */
+  /* munchausen only (other kinds ignore them, so a zero-filled tail is valid there); dz_learner_create and
+   * dz_learner_plan_query return DZ_EINVAL unless all three are finite, tau > 0, alpha >= 0 and l0 <= 0 */
+  float munchausen_alpha;    /* scale of the log-policy bonus: 0.9 */
+  float entropy_temperature; /* tau of the softmax policy of the target network: 0.03 */
+  float log_policy_clip;     /* l0, the lower clip of tau * log pi: -1 */
 } dz_learner_config;
 
 typedef struct dz_learner_plan {
@@ -633,6 +641,12 @@ int dz_test_pong_step(const dz_pong_config* cfg, int32_t* state, int32_t action,
  * "h1", "h1_val", "dh1", "iqn_e0", "iqn_hi", "iqn_dhi");
  * tests/tools only. */
 int dz_test_learner_buffer(dz_learner* l, const char* name, float** d_ptr, int64_t* count);
+/* The per-example arithmetic of the munchausen loss kernel evaluated on the HOST by the same source (fp32, expf / logf):
+ * q_tm1 = online(s_tm1), qbar_tm1 = target(s_tm1), qbar_t = target(s_t), each [A] (1 <= A <= 18).  Writes the target
+ * out[0], td out[1] and the log-policy bonus alpha * clip(tau * log pi(a_tm1 | s_tm1), l0, 0) out[2].  DZ_EINVAL for
+ * A or a_tm1 out of range and for the hyperparameters dz_learner_create rejects; tests only. */
+int dz_test_munchausen_example(const float* q_tm1, const float* qbar_tm1, const float* qbar_t, int32_t A, int32_t a_tm1,
+                               float r_t, float discount_t, float alpha, float tau, float l0, float* out);
 int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream);   /* device-to-device, tests only */
 /* Debug: the tensor-core launch named `tag` writes the clock stamps of its CTA 0 into d_trace (512 int64). */
 int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace);

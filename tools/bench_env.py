@@ -162,8 +162,9 @@ def learning_agent(seed, train_frames, kind='dqn', num_actions=6):
   rep = dr.TransitionReplay(capacity, structure, rs, frame_dedup=True)
   epsilon = parts.LinearSchedule(begin_t=4 * min_fill, decay_steps=max(train_frames // 4, 1), begin_value=1.0,
                                  end_value=0.01)
-  return ag.Dqn(transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep, exploration_epsilon=epsilon,
-                grad_error_bound=1.0 / 32, **common)
+  agent_cls = ag.Munchausen if kind == 'munchausen' else ag.Dqn   # munchausen: dqn's schedule, the paper's alpha / tau / l0
+  return agent_cls(transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep, exploration_epsilon=epsilon,
+                   grad_error_bound=1.0 / 32, **common)
 
 
 def evaluate(learner, seed, num_streams=64, game='catch', num_actions=6):
@@ -212,7 +213,8 @@ def learning_run(train_frames, seed=0, num_streams=32, eval_every=0, log=None, g
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--game', default='catch', choices=['catch', 'breakout', 'pong'])
-  ap.add_argument('--agent', default='dqn', choices=['dqn', 'rainbow'], help='the agent of the learning curve')
+  ap.add_argument('--agent', default='dqn', choices=['dqn', 'rainbow', 'munchausen'],
+                  help='the agent of the learning curve')
   ap.add_argument('--parts', default='env,train,eval,driver')
   ap.add_argument('--frames', type=int, default=65536, help='frames per timed window of env_train / env_eval')
   ap.add_argument('--learning', type=int, default=0, help='frames of the learning curve (0: none)')

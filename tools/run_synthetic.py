@@ -255,7 +255,8 @@ def parse_args(argv=None):
   ap.add_argument('--env', default='synthetic', choices=['synthetic', 'catch', 'breakout', 'pong'],
                   help='synthetic: random host frames; catch / breakout / pong: a game simulated and rendered on the device '
                        '(dqn_zoo_b200.environments)')
-  ap.add_argument('--agent', default='dqn', choices=['dqn', 'double_q', 'prioritized', 'c51', 'qrdqn', 'rainbow', 'iqn'])
+  ap.add_argument('--agent', default='dqn',
+                  choices=['dqn', 'double_q', 'prioritized', 'c51', 'qrdqn', 'rainbow', 'iqn', 'munchausen'])
   ap.add_argument('--num_actions', type=int, default=6)
   ap.add_argument('--replay_capacity', type=int, default=20000)
   ap.add_argument('--min_replay_capacity_fraction', type=float, default=0.05)
