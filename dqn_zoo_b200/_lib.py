@@ -15,7 +15,8 @@ vp = C.c_void_p
 DZ_FLAG_BAD_VALUE, DZ_FLAG_BAD_INDEX, DZ_FLAG_BAD_TARGET, DZ_FLAG_ROOT_ZERO, DZ_FLAG_NONFINITE_WEIGHT = 1, 2, 4, 8, 16
 DZ_FLAG_FRAME_POOL_FULL = 32
 DZ_CKPT_BAD_PLANE_ID, DZ_CKPT_UNREFERENCED_PLANE, DZ_CKPT_HASH_MISMATCH, DZ_CKPT_BAD_FREE_STACK = 1, 2, 4, 8
-AGENT_KINDS = {'dqn': 0, 'double_q': 1, 'prioritized': 2, 'c51': 3, 'qrdqn': 4, 'rainbow': 5, 'iqn': 6, 'munchausen': 7}
+AGENT_KINDS = {'dqn': 0, 'double_q': 1, 'prioritized': 2, 'c51': 3, 'qrdqn': 4, 'rainbow': 5, 'iqn': 6, 'munchausen': 7,
+               'munchausen_iqn': 8}
 OPTIMIZERS = {'adam': 0, 'rmsprop': 1}
 
 
@@ -198,6 +199,7 @@ _SIGNATURES = {
     'dz_test_pong_step': (i32, [C.POINTER(PongConfig), vp, i32, i32, vp, vp]),
     'dz_test_learner_buffer': (i32, [vp, C.c_char_p, vp, vp]),
     'dz_test_munchausen_example': (i32, [vp, vp, vp, i32, i32, f32, f32, f32, f32, f32, vp]),
+    'dz_test_munchausen_iqn_example': (i32, [vp, vp, i32, i32, i32, i32, f32, f32, f32, f32, f32, vp]),
     'dz_test_copy': (i32, [vp, vp, i64, vp]),
     'dz_test_learner_trace': (i32, [vp, C.c_char_p, vp]),
     'dz_test_learner_mma_path': (i32, [vp, C.c_char_p, C.POINTER(i32)]),

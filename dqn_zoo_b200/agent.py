@@ -1,5 +1,5 @@
-"""The seven dqn_zoo agents, and Munchausen DQN beside them, behind the reference's `parts.Agent`
-surface, running on the CUDA replay + learner.
+"""The seven dqn_zoo agents, and Munchausen DQN and Munchausen-IQN beside them, behind the reference's
+`parts.Agent` surface, running on the CUDA replay + learner.
 
 Each class keeps the reference constructor's argument names and the `step / reset /
 get_state / set_state / statistics` behaviour (dqn/agent.py:133-229, rainbow/agent.py:135-245,
@@ -36,6 +36,7 @@ from dqn_zoo_b200 import replay as replay_lib
 
 NetworkSpec = learner_lib.NetworkSpec
 OptimizerSpec = learner_lib.OptimizerSpec
+_iqn_net = learner_lib.uses_iqn_network
 
 
 def _seed_of(rng_key) -> int:
@@ -279,9 +280,9 @@ class _DeviceAgent(parts.Agent):
       self._jax_act.set_keys(sample)
       self._jax_act.launch(L.taus)
       taus = L.taus
-    elif self.KIND in ('iqn', 'rainbow'):
+    elif _iqn_net(self.KIND) or self.KIND == 'rainbow':
       L.generate_randomness(self._seed)
-      taus = L.taus if self.KIND == 'iqn' else None
+      taus = L.taus if _iqn_net(self.KIND) else None
       noise = L.noise if self.KIND == 'rainbow' else None
     q = L.q_values(self._obs_dev, taus=taus, noise=noise).cpu().numpy()   # D2H sync, as jax.device_get
     eps = 0.0 if self.GREEDY else self.exploration_epsilon
@@ -384,7 +385,7 @@ class _DeviceAgent(parts.Agent):
     L = self._learner
     if getattr(self, '_jax_key', None) is not None:
       self._jax_learn.launch(L.taus)            # jax.random.uniform draws from the keys staged by _learn()
-    elif self.KIND in ('iqn', 'rainbow'):
+    elif _iqn_net(self.KIND) or self.KIND == 'rainbow':
       L.generate_randomness(self._seed, beside_sampler=True)
     L.learn(self._view, self.PRIORITIZED, self._io)
 
@@ -539,6 +540,28 @@ class Iqn(_DeviceAgent):
       self._jax_act = jax_prng.DeviceUniform([tau_samples_policy], dev)
 
 
+class MunchausenIqn(_DeviceAgent):
+  """Munchausen-IQN (Vieillard, Pietquin & Geist, NeurIPS 2020; DESIGN.md §14): Iqn's constructor (without
+  `jax_prng_taus`: no reference key chain pins this agent's taus), network, taus, uniform replay and epsilon-greedy
+  acting, with the soft quantile targets y_j = r + alpha clip(tau log pi(a_tm1|s_tm1), l0, 0) +
+  discount sum_a pi(a|s_t) (zbar_j(s_t, a) - tau log pi(a|s_t)) of the target network's softmax policy pi over its
+  mean quantiles.  The defaults of `munchausen_alpha`, `entropy_temperature` (tau) and `log_policy_clip` (l0) are the
+  paper's Atari values."""
+  KIND = 'munchausen_iqn'
+
+  def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
+               batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
+               target_network_update_period, huber_param, tau_samples_policy, tau_samples_s_tm1, tau_samples_s_t,
+               rng_key, use_cuda_graph=True, munchausen_alpha=0.9, entropy_temperature=0.03, log_policy_clip=-1.0):
+    if (network.tau_samples_policy, network.tau_samples_s_tm1, network.tau_samples_s_t) != (
+        tau_samples_policy, tau_samples_s_tm1, tau_samples_s_t):
+      raise ValueError('tau sample counts must match the NetworkSpec')
+    self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
+                exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
+                huber_param=huber_param, use_cuda_graph=use_cuda_graph, munchausen_alpha=munchausen_alpha,
+                entropy_temperature=entropy_temperature, log_policy_clip=log_policy_clip)
+
+
 def _check_support(support, network):
   s = np.asarray(support, dtype=np.float64)
   want = np.linspace(-network.vmax, network.vmax, network.num_atoms)
@@ -610,10 +633,10 @@ class EpsilonGreedyActor(parts.Agent):
       self._obs_dev.copy_(torch.from_numpy(np.ascontiguousarray(obs).reshape(-1)))
     L = self._learner
     taus = noise = None
-    if L.kind in ('iqn', 'rainbow'):
+    if _iqn_net(L.kind) or L.kind == 'rainbow':
       self._seed += 1
       L.generate_randomness(self._seed)
-      taus = L.taus if L.kind == 'iqn' else None
+      taus = L.taus if _iqn_net(L.kind) else None
       noise = L.noise if L.kind == 'rainbow' else None
     q = L.q_values(self._obs_dev, taus=taus, noise=noise).cpu().numpy()
     if self._epsilon > 0.0 and self._rng.uniform() < self._epsilon:
@@ -642,7 +665,7 @@ class EpsilonGreedyActor(parts.Agent):
 
 
 AGENTS = {'dqn': Dqn, 'double_q': DoubleQ, 'prioritized': PrioritizedDqn, 'c51': C51, 'qrdqn': QrDqn,
-          'rainbow': Rainbow, 'iqn': Iqn, 'munchausen': Munchausen}
+          'rainbow': Rainbow, 'iqn': Iqn, 'munchausen': Munchausen, 'munchausen_iqn': MunchausenIqn}
 
 
 class BatchedEpsilonGreedyActor:
@@ -698,7 +721,7 @@ class BatchedEpsilonGreedyActor:
     if self._actor is not None:
       if self._per_stream_noise:
         stream_noise = self._actor.generate_randomness(self._seed, per_stream=True)
-      elif kind == 'iqn':
+      elif _iqn_net(kind):
         taus = self._actor.generate_randomness(self._seed)
       elif kind == 'rainbow':
         noise = self._actor.generate_randomness(self._seed)
@@ -707,9 +730,9 @@ class BatchedEpsilonGreedyActor:
     else:
       if self._per_stream_noise:
         stream_noise = L.generate_stream_noise(self._seed, self._E)
-      elif kind in ('iqn', 'rainbow'):
+      elif _iqn_net(kind) or kind == 'rainbow':
         L.generate_randomness(self._seed)
-        if kind == 'iqn':
+        if _iqn_net(kind):
           taus = L.taus[:self._E * L.net.tau_samples_policy] if hasattr(L.net, 'tau_samples_policy') else L.taus
         else:
           noise = L.noise
@@ -768,7 +791,7 @@ class VectorTrainer:
     if E > L.batch_size:                       # acted through an acting context: its limits apply
       if E > ACTOR_MAX_STREAMS:
         raise ValueError('num_streams %d exceeds the acting limit of %d streams' % (E, ACTOR_MAX_STREAMS))
-      if L.kind == 'iqn' and E * L.net.tau_samples_policy > ACTOR_MAX_IQN_ROWS:
+      if _iqn_net(L.kind) and E * L.net.tau_samples_policy > ACTOR_MAX_IQN_ROWS:
         raise ValueError('iqn acting needs num_streams * tau_samples_policy <= %d, got %d * %d'
                          % (ACTOR_MAX_IQN_ROWS, E, L.net.tau_samples_policy))
     acc = train_agent._transition_accumulator
@@ -1048,7 +1071,7 @@ class VectorEvaluator:
     else:
       raise TypeError('network_or_learner must be a NetworkSpec or a Learner')
     net = network_or_learner.net if shape_learner is not None else network_or_learner
-    if net.kind == 'iqn' and E * net.tau_samples_policy > ACTOR_MAX_IQN_ROWS:
+    if _iqn_net(net.kind) and E * net.tau_samples_policy > ACTOR_MAX_IQN_ROWS:
       raise ValueError('iqn acting needs num_streams * tau_samples_policy <= %d, got %d * %d'
                        % (ACTOR_MAX_IQN_ROWS, E, net.tau_samples_policy))
     if per_stream_noise and net.kind != 'rainbow':
@@ -1144,7 +1167,7 @@ class VectorEvaluator:
     taus = noise = stream_noise = None
     if self._per_stream_noise:
       stream_noise = A.generate_randomness(self._seed, per_stream=True)
-    elif self._net.kind == 'iqn':
+    elif _iqn_net(self._net.kind):
       taus = A.generate_randomness(self._seed)
     elif self._net.kind == 'rainbow':
       noise = A.generate_randomness(self._seed)

@@ -7,8 +7,8 @@
 //                 categorical_[double_]q_learning, quantile_q_learning (restated; SURVEY §8(c))
 //   optax 0.1.2   adam, rmsprop(centered), clip_by_global_norm, apply_updates
 //   _learn glue   rainbow/agent.py:181-198, prioritized/agent.py:187-206
-//   munchausen    Munchausen DQN (Vieillard, Pietquin & Geist, NeurIPS 2020), the one agent outside the
-//                 reference: dqn's network with online(s_tm1) | target(s_tm1) | target(s_t) (DESIGN.md §13)
+//   munchausen    Munchausen DQN and Munchausen-IQN (Vieillard, Pietquin & Geist, NeurIPS 2020), outside the
+//                 reference: dqn's / iqn's network with online(s_tm1) | target(s_tm1) | target(s_t) (DESIGN.md §13, §14)
 //
 // Gradients flow only through online(s_tm1).  All forward passes of a layer are one grouped
 // launch (dz_gemm.cuh); the replay gather is fused into conv1's operand load.
@@ -24,6 +24,16 @@
 #include "dz_umma_net.cuh"
 
 namespace dz {
+
+// The network an agent kind applies: munchausen_iqn runs iqn's network, munchausen dqn's.  Every network-structure
+// decision (layout, carving, tensor-core plan, randomness, tau counts, acting) goes through these two predicates; the
+// loss launch is the only place that tells a Munchausen kind from the kind whose network it uses.
+__host__ __device__ constexpr bool uses_iqn_net(int kind) { return kind == DZ_IQN || kind == DZ_MUNCHAUSEN_IQN; }
+__host__ __device__ constexpr bool uses_dqn_net(int kind) { return kind == DZ_DQN || kind == DZ_MUNCHAUSEN; }
+// The kind given to the device kernels that branch on the network (q_values_kernel).
+constexpr int net_kind(int kind) { return uses_iqn_net(kind) ? DZ_IQN : uses_dqn_net(kind) ? DZ_DQN : kind; }
+// The Munchausen kinds: alpha / tau / l0 are validated, and the target network also applies to s_tm1.
+constexpr bool is_munchausen(int kind) { return kind == DZ_MUNCHAUSEN || kind == DZ_MUNCHAUSEN_IQN; }
 
 // ------------------------------------------------------------------------------------------------
 // Parameter layout (canonical names; haiku layouts) — must match oracle/learner_oracle.py:param_shapes
@@ -99,7 +109,7 @@ static Layout make_layout(const dz_learner_config& c) {
     }
     return L;
   }
-  if (c.kind == DZ_IQN) { L.add("embed/w", {c.latent_dim, d.feat}); L.add("embed/b", {d.feat}); }
+  if (uses_iqn_net(c.kind)) { L.add("embed/w", {c.latent_dim, d.feat}); L.add("embed/b", {d.feat}); }
   L.add("fc1/w", {d.feat, 512}); L.add("fc1/b", {512});
   L.add("head/w", {512, d.out});
   bool shared = c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED;
@@ -145,9 +155,9 @@ static int param_offsets(const dz_learner_config& c, const Layout& L, ParamOffse
   } else {
     o.w1[0] = need("fc1/w"); o.b1[0] = need("fc1/b");
     o.w2[0] = need("head/w"); o.b2[0] = need("head/b");
-    if (c.kind == DZ_IQN) { o.embed_w = need("embed/w"); o.embed_b = need("embed/b"); }
+    if (uses_iqn_net(c.kind)) { o.embed_w = need("embed/w"); o.embed_b = need("embed/b"); }
   }
-  o.fc_begin = c.kind == DZ_IQN ? o.embed_w : o.w1[0];
+  o.fc_begin = uses_iqn_net(c.kind) ? o.embed_w : o.w1[0];
   if (missing) return fail(DZ_EINVAL, "parameter layout lacks a tensor of this agent kind");
   *out = o;
   return DZ_OK;
@@ -180,19 +190,45 @@ __host__ __device__ inline float munchausen_exp(float qbar, float v, float tau) 
 
 struct MunchausenTarget { float target, bonus; };
 
+// alpha clip(tau log pi(a_tm1 | s_tm1), l0, 0)
+__host__ __device__ inline float munchausen_bonus(float qbar_tm1_a, float v_tm1, float s_tm1, float alpha, float tau, float l0) {
+  const float tau_log_pi = fmaf(-tau, logf(s_tm1), qbar_tm1_a - v_tm1);     // tau log pi(a_tm1 | s_tm1)
+  return alpha * fminf(fmaxf(tau_log_pi, l0), 0.f);
+}
+
 __host__ __device__ inline MunchausenTarget munchausen_target(float r, float disc, float qbar_tm1_a, float v_tm1, float s_tm1,
                                                               float v_t, float s_t, float alpha, float tau, float l0) {
-  const float tau_log_pi = fmaf(-tau, logf(s_tm1), qbar_tm1_a - v_tm1);     // tau log pi(a_tm1 | s_tm1)
-  const float bonus = alpha * fminf(fmaxf(tau_log_pi, l0), 0.f);
+  const float bonus = munchausen_bonus(qbar_tm1_a, v_tm1, s_tm1, alpha, tau, l0);
   const float boot = fmaf(tau, logf(s_t), v_t);
   return MunchausenTarget{fmaf(disc, boot, r + bonus), bonus};
 }
 
+// ---- Munchausen-IQN per-example target arithmetic (DESIGN.md §14), shared by loss_munchausen_iqn_kernel and its host
+// twin dz_test_munchausen_iqn_example.  qbar(s, a) is the mean of the target network's quantile samples of that pass,
+// summed in row order; the softmax reductions are the warp's (the host twin's butterfly), as for munchausen above.
+// The bootstrap of sample j is sum_a pi(a|s_t) (zbar_j(s_t, a) + h(a)) with h(a) = v + tau log S - qbar(a) =
+// -tau log pi(a|s_t) >= 0, evaluated as sum_a pi zbar_j + E with the entropy term E = sum_a pi h a sum of non-negative
+// terms: no cancellation at large qbar (sum pi qbar - tau logsumexp would cancel).
+__host__ __device__ inline float miqn_mean(const float* z, int rows, int A, int a) {
+  float s = 0.f;
+  for (int j = 0; j < rows; ++j) s += z[(long long)j * A + a];
+  return s / (float)rows;
+}
+
+__host__ __device__ inline float miqn_h(float qbar, float v, float s, float tau) { return fmaf(tau, logf(s), v - qbar); }
+
+// y_j = r + bonus + disc (sum_a pi(a) zbar_j(a) + E); rb = r + bonus
+__host__ __device__ inline float miqn_target(const float* zbar_j, const float* pi, int A, float rb, float disc, float ent) {
+  float s = 0.f;
+  for (int a = 0; a < A; ++a) s = fmaf(pi[a], zbar_j[a], s);
+  return fmaf(disc, s + ent, rb);
+}
+
 static int validate(const dz_learner_config& c) {
-  if (c.kind < 0 || c.kind > DZ_MUNCHAUSEN) return fail(DZ_EINVAL, "unknown agent kind");
-  if (c.kind == DZ_MUNCHAUSEN && !munchausen_params_ok(c.munchausen_alpha, c.entropy_temperature, c.log_policy_clip))
+  if (c.kind < 0 || c.kind > DZ_MUNCHAUSEN_IQN) return fail(DZ_EINVAL, "unknown agent kind");
+  if (is_munchausen(c.kind) && !munchausen_params_ok(c.munchausen_alpha, c.entropy_temperature, c.log_policy_clip))
     return fail(DZ_EINVAL, "munchausen needs finite alpha >= 0, entropy_temperature > 0 and log_policy_clip <= 0");
-  if (c.kind == DZ_MUNCHAUSEN && c.num_actions > kMunchausenMaxActions)
+  if (is_munchausen(c.kind) && c.num_actions > kMunchausenMaxActions)
     return fail(DZ_EINVAL, "munchausen: num_actions must be in [1,18] (one warp lane per action)");
   if (c.batch <= 0 || c.batch > 1024) return fail(DZ_EINVAL, "batch must be in [1,1024]");
   if (c.obs_c != 4) return fail(DZ_EINVAL, "obs_c must be 4 (stacked frames; conv1 reads uchar4 pixels)");
@@ -201,7 +237,7 @@ static int validate(const dz_learner_config& c) {
   if (c.num_actions <= 0 || c.num_actions > 64) return fail(DZ_EINVAL, "num_actions must be in [1,64]");
   if ((c.kind == DZ_C51 || c.kind == DZ_RAINBOW) && (c.num_atoms < 2 || c.num_atoms > 128)) return fail(DZ_EINVAL, "num_atoms must be in [2,128]");
   if (c.kind == DZ_QRDQN && (c.num_quantiles < 1 || c.num_quantiles > 256)) return fail(DZ_EINVAL, "num_quantiles must be in [1,256]");
-  if (c.kind == DZ_IQN) {
+  if (uses_iqn_net(c.kind)) {
     if (c.latent_dim <= 0 || c.latent_dim % 16) return fail(DZ_EINVAL, "latent_dim must be a positive multiple of 16");
     int mx = c.tau_samples_s_tm1 > c.tau_samples_s_t ? c.tau_samples_s_tm1 : c.tau_samples_s_t;
     mx = mx > c.tau_samples_policy ? mx : c.tau_samples_policy;
@@ -842,6 +878,45 @@ size_t categorical_loss_smem(const dz_learner_config& c) {
   return (6 * K + A + 4 + K + 3 * A * K + 3 * K) * sizeof(float);
 }
 
+// rlax.quantile_regression_loss of example b's N source quantiles src (at taus tau) against its Nt targets tgt, all in
+// shared memory, and the gradient wrt the pass-0 head outputs in IQN's layout (nonzero at a_tm1 only): the tail of
+// loss_quantile_kernel, which keeps its own inline copy so that its code generation stays as it was.
+__device__ __forceinline__ void quantile_huber_tail(const LossArgs& L, int b, int at, int N, int Nt, const float* tgt,
+                                                    const float* src, const float* tau, float* red) {
+  const int A = L.A, tid = threadIdx.x;
+  const float kappa = L.kappa;
+  const float w = L.w ? L.w[b] : 1.0f;
+  const float cot = w / (float)L.B;
+  float total = 0.f;
+  for (int i = tid; i < N; i += blockDim.x) {
+    float acc = 0.f, gacc = 0.f;
+    for (int j = 0; j < Nt; ++j) {
+      float delta = tgt[j] - src[i];
+      float wt = fabsf(tau[i] - (delta < 0.f ? 1.0f : 0.0f));
+      float ad = fabsf(delta);
+      float l, dl;
+      if (kappa > 0.f) {
+        float q = fminf(ad, kappa);
+        l = 0.5f * q * q + kappa * (ad - q);
+        dl = fminf(fmaxf(delta, -kappa), kappa);
+      } else {
+        l = ad;
+        dl = delta > 0.f ? 1.0f : (delta < 0.f ? -1.0f : 0.0f);
+      }
+      acc += wt * l;
+      gacc += wt * dl;
+    }
+    total += acc / (float)Nt;
+    float g = -cot * gacc / (float)Nt;  // d loss / d src_i  (delta = target - src)
+    for (int a = 0; a < A; ++a) L.dout[((long long)b * N + i) * A + a] = (a == at) ? g : 0.f;
+  }
+  total = block_sum(total, red);
+  if (tid == 0) {
+    L.per_example[b] = total;
+    L.loss_terms[b] = w * total;
+  }
+}
+
 // qrdqn / iqn: rlax.quantile_q_learning with quantile_regression_loss (Huber kappa).
 // Layouts: qrdqn out[b, q*A + a] (networks.py:308), iqn out[(b*N + n)*A + a] (networks.py:286-287).
 __global__ void __launch_bounds__(256) loss_quantile_kernel(LossArgs L) {
@@ -909,6 +984,59 @@ __global__ void __launch_bounds__(256) loss_quantile_kernel(LossArgs L) {
     L.per_example[b] = total;
     L.loss_terms[b] = w * total;
   }
+}
+
+// munchausen_iqn (DESIGN.md §14): one CTA per example.  (1) qbar of target(s_tm1) over its K policy samples (out1) and
+// of target(s_t) over its N' samples (out2), one thread per (pass, action), in row order; (2) one warp, lane a holding
+// action a: both softmaxes, the log-policy bonus and the entropy term E = sum_a pi(a|s_t) h(a); (3) the N' targets
+// y_j = r + bonus + disc (sum_a pi(a|s_t) zbar_j(s_t, a) + E); (4) IQN's quantile-Huber term of online(s_tm1)'s N
+// samples at a_tm1 against them and (5) dout in IQN's layout (quantile_huber_tail).  The per-example value is the loss.
+__global__ void __launch_bounds__(256) loss_munchausen_iqn_kernel(LossArgs L, float alpha, float tau_e, float l0) {
+  dz::pdl_enter();
+  extern __shared__ float sm[];
+  const int b = blockIdx.x, A = L.A, tid = threadIdx.x;
+  const int N = L.N, K = L.Ksel, Nt = L.Nt;
+  float* red = sm;            // [32]
+  float* qbar = sm + 32;      // [2][A]: s_tm1, s_t
+  float* pi = qbar + 2 * A;   // [A]: pi(a|s_t)
+  float* scal = pi + A;       // [2]: bonus, E
+  float* tgt = scal + 2;      // [Nt]
+  float* src = tgt + Nt;      // [N]
+  float* tau = src + N;       // [N]
+  const float* zbar_tm1 = L.out1 + (long long)b * K * A;
+  const float* zbar_t = L.out2 + (long long)b * Nt * A;
+  if (tid < 2 * A) {
+    const bool t = tid >= A;
+    qbar[tid] = miqn_mean(t ? zbar_t : zbar_tm1, t ? Nt : K, A, t ? tid - A : tid);
+  }
+  __syncthreads();
+  const int at = L.a[b];
+  if (tid < 32) {
+    const bool act = tid < A;
+    const float q1 = act ? qbar[tid] : -INFINITY, q2 = act ? qbar[A + tid] : -INFINITY;
+    const float v1 = warp_max(q1), v2 = warp_max(q2);
+    const float s1 = warp_sum(act ? munchausen_exp(q1, v1, tau_e) : 0.f);
+    const float e2 = act ? munchausen_exp(q2, v2, tau_e) : 0.f;
+    const float s2 = warp_sum(e2);
+    const float p2 = e2 / s2;
+    const float ent = warp_sum(act ? p2 * miqn_h(q2, v2, s2, tau_e) : 0.f);
+    if (act) pi[tid] = p2;
+    if (tid == 0) { scal[0] = munchausen_bonus(qbar[at], v1, s1, alpha, tau_e, l0); scal[1] = ent; }
+  }
+  __syncthreads();
+  const float rb = L.r[b] + scal[0], dsc = L.disc[b], ent = scal[1];
+  for (int j = tid; j < Nt; j += blockDim.x) tgt[j] = miqn_target(zbar_t + (long long)j * A, pi, A, rb, dsc, ent);
+  const float* dist_s = L.out0 + (long long)b * N * A;
+  for (int i = tid; i < N; i += blockDim.x) {
+    src[i] = dist_s[(long long)i * A + at];
+    tau[i] = L.taus0[(long long)b * N + i];
+  }
+  __syncthreads();
+  quantile_huber_tail(L, b, at, N, Nt, tgt, src, tau, red);
+}
+
+size_t munchausen_iqn_loss_smem(const dz_learner_config& c) {
+  return (32 + 3 * (size_t)c.num_actions + 2 + c.tau_samples_s_t + 2 * (size_t)c.tau_samples_s_tm1) * sizeof(float);
 }
 
 __global__ void loss_mean_kernel(const float* __restrict__ terms, int B, float* loss, float* max_seen, const float* priorities) {
@@ -1333,7 +1461,7 @@ int64_t carve(dz_learner* l, char* base) {
   const Dims& d = l->d;
   const int B = c.batch;
   Bump w{base};
-  const bool rb = c.kind == DZ_RAINBOW, iqn = c.kind == DZ_IQN;
+  const bool rb = c.kind == DZ_RAINBOW, iqn = uses_iqn_net(c.kind);
   int nh[3] = {1, 1, 1};
   if (iqn) { nh[0] = c.tau_samples_s_tm1; nh[1] = c.tau_samples_policy; nh[2] = c.tau_samples_s_t; }
   for (int p = 0; p < 3; ++p) l->n_head[p] = nh[p];
@@ -1462,12 +1590,12 @@ UmNetDesc make_um_desc(const dz_learner* l) {
   memset(&u, 0, sizeof(u));
   const bool needs_online_st = c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED || c.kind == DZ_RAINBOW;
   u.B = c.batch; u.H = d.H; u.W = d.W;
-  const bool mdqn = c.kind == DZ_MUNCHAUSEN;   // online(s_tm1) | target(s_tm1) | target(s_t)
-  u.npass = needs_online_st || mdqn ? 3 : 2;
+  const bool target_stm1 = is_munchausen(c.kind);   // online(s_tm1) | target(s_tm1) | target(s_t)
+  u.npass = needs_online_st || target_stm1 ? 3 : 2;
   u.pass_target[0] = 0; u.pass_target[1] = needs_online_st ? 0 : 1; u.pass_target[2] = 1;
   u.online = l->buf.d_online; u.target = l->buf.d_target;
   for (int i = 0; i < 3; ++i) { u.off_conv_w[i] = o.conv_w[i]; u.off_conv_b[i] = o.conv_b[i]; }
-  u.use_fc = c.kind != DZ_IQN;
+  u.use_fc = !uses_iqn_net(c.kind);
   u.nstream = c.kind == DZ_RAINBOW ? 2 : 1;
   u.noisy = c.kind == DZ_RAINBOW ? 1 : 0;
   if (c.kind == DZ_RAINBOW) {
@@ -1967,7 +2095,7 @@ int backward_torso(dz_learner* l, const uint8_t* const* rows0, void* stream) {
   FinishTNBatch fb;
   fb.n = 0;
   GemmBatch gb;
-  if (l->um && l->cfg.kind == DZ_IQN) DZ_TRY(um_split_dact3(l->um, stream));   // dact3 came from the Hadamard kernel (fp32)
+  if (l->um && uses_iqn_net(l->cfg.kind)) DZ_TRY(um_split_dact3(l->um, stream));   // dact3 came from the Hadamard kernel (fp32)
   // conv3 wgrad
   float* norm_parts = split_norm_active(l) ? l->norm_parts : nullptr;
   if (l->um) {   // conv3 weight gradient + its finish (partial sums, bias gradient, split-norm partials) on a side stream
@@ -2310,7 +2438,7 @@ int backward_iqn(dz_learner* l, void* stream) {
 // Split global norm (tensor-core path, every agent but IQN): the sum of squares of everything behind the conv tensors is taken
 // on the second side stream as soon as the last FC / head weight gradient is written (norm_fc_range), the conv tensors'
 // partials come from the per-layer weight-gradient finish kernels, and the optimizer (or norm_finalize_kernel) combines them.
-bool split_norm_active(const dz_learner* l) { return l->um != nullptr && l->cfg.kind != DZ_IQN; }
+bool split_norm_active(const dz_learner* l) { return l->um != nullptr && !uses_iqn_net(l->cfg.kind); }
 
 int norm_fc_range(dz_learner* l, bool apply, void* stream) {
   const long long begin = l->po.fc_begin;
@@ -2359,17 +2487,18 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   const float* tg = l->buf.d_target;
   const bool needs_online_st = c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED || c.kind == DZ_RAINBOW;
   if (c.kind == DZ_RAINBOW && !batch->d_noise) return fail(DZ_EINVAL, "rainbow update needs d_noise");
-  if (c.kind == DZ_IQN && !batch->d_taus) return fail(DZ_EINVAL, "iqn update needs d_taus");
+  if (uses_iqn_net(c.kind) && !batch->d_taus) return fail(DZ_EINVAL, "iqn update needs d_taus");
   if (!out || !out->d_loss || !out->d_per_example) return fail(DZ_EINVAL, "update outputs d_loss and d_per_example are required");
   if (!(weights_packed && l->um != nullptr)) DZ_TRY(l->side.join(stream));   // pending side-stream work (asynchronous randomness)
 
   // ---- forward: every network.apply of loss_fn in grouped launches
   TorsoJob jobs[3];
   int nj = 0;
-  const bool mdqn = c.kind == DZ_MUNCHAUSEN;   // the target network also applies to s_tm1 (the log-policy bonus)
+  const bool target_stm1 = is_munchausen(c.kind);   // the target network also applies to s_tm1 (the log-policy bonus)
+  const bool iqn = uses_iqn_net(c.kind);
   jobs[nj++] = TorsoJob{on, batch->d_s_tm1_rows, 0};
   if (needs_online_st) jobs[nj++] = TorsoJob{on, batch->d_s_t_rows, 1};
-  if (mdqn) jobs[nj++] = TorsoJob{tg, batch->d_s_tm1_rows, 1};
+  if (target_stm1) jobs[nj++] = TorsoJob{tg, batch->d_s_tm1_rows, 1};
   jobs[nj++] = TorsoJob{tg, batch->d_s_t_rows, 2};
   const bool um = l->um != nullptr;
   if (um) {
@@ -2380,14 +2509,15 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     else DZ_TRY(um_pack_weights(l->um, stream));
     DZ_TRY(um_forward_torso(l->um, rows, stream));
     DZ_TRY(l->side.join(stream));
-    if (c.kind != DZ_IQN) DZ_TRY(um_forward_fc(l->um, batch->d_noise, stream));
+    if (!iqn) DZ_TRY(um_forward_fc(l->um, batch->d_noise, stream));
   } else {
     DZ_TRY(forward_torso(l, learner_bufs(l), jobs, nj, B, stream));
   }
 
-  if (c.kind == DZ_IQN) {
-    // online(s_tm1, tau_tm1) | target(s_t, tau_selector) | target(s_t, tau_t)   (iqn/agent.py:192-203)
-    Pass passes[3] = {{on, 0, 0, 0}, {tg, 2, 1, 0}, {tg, 2, 2, 0}};
+  if (iqn) {
+    // iqn: online(s_tm1, tau_tm1) | target(s_t, tau_selector) | target(s_t, tau_t)   (iqn/agent.py:192-203)
+    // munchausen_iqn: online(s_tm1, tau_tm1) | target(s_tm1, tau_policy) | target(s_t, tau_t), three torso sets
+    Pass passes[3] = {{on, 0, 0, 0}, {tg, target_stm1 ? 1 : 2, 1, 0}, {tg, 2, 2, 0}};
     const float* t0 = batch->d_taus;
     const float* t1 = t0 + (long long)B * c.tau_samples_s_tm1;
     const float* t2 = t1 + (long long)B * c.tau_samples_policy;
@@ -2401,7 +2531,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     int np = 0;
     passes[np++] = Pass{on, 0, 0, 0};
     if (needs_online_st) passes[np++] = Pass{on, 1, 1, 0};
-    if (mdqn) passes[np++] = Pass{tg, 1, 1, 0};
+    if (target_stm1) passes[np++] = Pass{tg, 1, 1, 0};
     passes[np++] = Pass{tg, 2, 2, 0};
     DZ_TRY(forward_heads_plain(l, learner_bufs(l), passes, np, B, stream, um));
   }
@@ -2419,11 +2549,15 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   L.priorities = (c.kind == DZ_RAINBOW || c.kind == DZ_PRIORITIZED) ? out->d_priorities : nullptr;
   if (c.kind == DZ_DQN || c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED) {
     DZ_LAUNCH(loss_q_kernel, B, 64, 0, stream, L);
-  } else if (mdqn) {
+  } else if (c.kind == DZ_MUNCHAUSEN) {
     DZ_LAUNCH(loss_munchausen_kernel, (B + 3) / 4, 128, 0, stream, L, c.munchausen_alpha, c.entropy_temperature,
               c.log_policy_clip);
   } else if (c.kind == DZ_C51 || c.kind == DZ_RAINBOW) {
     DZ_LAUNCH_NAMED("loss_categorical_kernel", loss_categorical_staged_kernel, B, 128, categorical_loss_smem(c), stream, L);
+  } else if (c.kind == DZ_MUNCHAUSEN_IQN) {
+    L.N = c.tau_samples_s_tm1; L.Ksel = c.tau_samples_policy; L.Nt = c.tau_samples_s_t;
+    DZ_LAUNCH(loss_munchausen_iqn_kernel, B, 256, munchausen_iqn_loss_smem(c), stream, L, c.munchausen_alpha,
+              c.entropy_temperature, c.log_policy_clip);
   } else {
     if (c.kind == DZ_QRDQN) { L.N = c.num_quantiles; L.Ksel = c.num_quantiles; L.Nt = c.num_quantiles; }
     else { L.N = c.tau_samples_s_tm1; L.Ksel = c.tau_samples_policy; L.Nt = c.tau_samples_s_t; }
@@ -2439,7 +2573,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
 
   // ---- backward through online(s_tm1)
   if (c.kind == DZ_RAINBOW) DZ_TRY(backward_rainbow(l, batch->d_noise, stream));
-  else if (c.kind == DZ_IQN) DZ_TRY(backward_iqn(l, stream));
+  else if (iqn) DZ_TRY(backward_iqn(l, stream));
   else DZ_TRY(backward_plain(l, stream));
   if (split_norm_active(l)) {   // every gradient behind the conv tensors is final once the side stream's FC / head wgrads are done
     DZ_TRY(norm_fc_range(l, apply_update != 0, l->side.tail(stream)));
@@ -2476,7 +2610,7 @@ int dz_learner_plan_query(const dz_learner_config* cfg, dz_learner_plan* out) {
   out->opt_state_floats = 2 * tmp.lay.total;
   out->workspace_bytes = carve(&tmp, nullptr);
   out->noise_floats = cfg->kind == DZ_RAINBOW ? 3 * noise_layout(*cfg, tmp.d).stride : 0;
-  out->tau_floats = cfg->kind == DZ_IQN
+  out->tau_floats = uses_iqn_net(cfg->kind)
                         ? (int64_t)cfg->batch * (cfg->tau_samples_s_tm1 + cfg->tau_samples_policy + cfg->tau_samples_s_t)
                         : 0;
   return DZ_OK;
@@ -2622,7 +2756,7 @@ int dz_learner_generate_randomness_async(dz_learner* l, uint64_t seed, float* d_
 
 int dz_learner_generate_randomness(dz_learner* l, uint64_t seed, float* d_taus, float* d_noise, void* stream) {
   const dz_learner_config& c = l->cfg;
-  if (c.kind == DZ_IQN && d_taus) {
+  if (uses_iqn_net(c.kind) && d_taus) {
     long long n = (long long)c.batch * (c.tau_samples_s_tm1 + c.tau_samples_policy + c.tau_samples_s_t);
     DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_taus, n, seed, l->buf.d_counters, 0, 1u);
   }
@@ -2643,7 +2777,7 @@ int dz_learner_q_values(dz_learner* l, const uint8_t* d_obs, const float* d_taus
   DZ_TRY(forward_torso(l, learner_bufs(l), &job, 1, 1, stream));
   Pass pass{on, 1, 1, 0};
   int nq = 1;
-  if (c.kind == DZ_IQN) {
+  if (uses_iqn_net(c.kind)) {
     if (!d_taus) return fail(DZ_EINVAL, "iqn q_values needs taus[tau_samples_policy]");
     const float* taus[1] = {d_taus};
     DZ_TRY(forward_heads_iqn(l, learner_bufs(l), &pass, 1, 1, taus, false, stream));
@@ -2656,7 +2790,7 @@ int dz_learner_q_values(dz_learner* l, const uint8_t* d_obs, const float* d_taus
     nq = c.num_quantiles;
   }
   size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
-  DZ_LAUNCH(q_values_kernel, 1, 128, smem, stream, c.kind, c.num_actions, c.num_atoms, nq, c.vmax, l->out[1], l->out[1], l->outv[1], d_q_out);
+  DZ_LAUNCH(q_values_kernel, 1, 128, smem, stream, net_kind(c.kind), c.num_actions, c.num_atoms, nq, c.vmax, l->out[1], l->out[1], l->outv[1], d_q_out);
   return DZ_OK;
 }
 
@@ -2680,7 +2814,7 @@ int act_batch_impl(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* 
   DZ_TRY(forward_torso(l, learner_bufs(l), &job, 1, E, stream));
   Pass pass{on, 1, 1, 0};
   int nq = 1;
-  if (c.kind == DZ_IQN) {
+  if (uses_iqn_net(c.kind)) {
     if (!d_taus) return fail(DZ_EINVAL, "iqn act_batch needs taus[E][tau_samples_policy]");
     const float* taus[1] = {d_taus};
     DZ_TRY(forward_heads_iqn(l, learner_bufs(l), &pass, 1, E, taus, false, stream));
@@ -2693,7 +2827,7 @@ int act_batch_impl(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* 
     nq = c.num_quantiles;
   }
   size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
-  DZ_LAUNCH(q_values_kernel, (unsigned)E, 128, smem, stream, c.kind, c.num_actions, c.num_atoms, nq, c.vmax, l->out[1], l->out[1], l->outv[1], d_q_out);
+  DZ_LAUNCH(q_values_kernel, (unsigned)E, 128, smem, stream, net_kind(c.kind), c.num_actions, c.num_atoms, nq, c.vmax, l->out[1], l->out[1], l->outv[1], d_q_out);
   DZ_LAUNCH(act_select_kernel, (unsigned)ceil_div(E, 128), 128, 0, stream, (const float*)d_q_out, c.num_actions, (int)E, d_explore, epsilon, d_actions);
   return DZ_OK;
 }
@@ -2769,7 +2903,7 @@ constexpr int kActorMaxStreams = 1024, kActorMaxIqnRows = 16384;
 
 int actor_check(const dz_learner_config& c, int E) {
   if (E < 1 || E > kActorMaxStreams) return fail(DZ_EINVAL, "actor: num_streams must be in [1, 1024]");
-  if (c.kind == DZ_IQN && (int64_t)E * c.tau_samples_policy > kActorMaxIqnRows)
+  if (uses_iqn_net(c.kind) && (int64_t)E * c.tau_samples_policy > kActorMaxIqnRows)
     return fail(DZ_EINVAL, "actor: num_streams * tau_samples_policy must be <= 16384");
   return DZ_OK;
 }
@@ -2789,7 +2923,7 @@ int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
   const dz_learner_config& c = l->cfg;
   const Dims& d = l->d;
   const int E = a->E;
-  const bool rb = c.kind == DZ_RAINBOW, iqn = c.kind == DZ_IQN;
+  const bool rb = c.kind == DZ_RAINBOW, iqn = uses_iqn_net(c.kind);
   Bump w{base};
   NetBufs& b = a->b;
   memset(&b, 0, sizeof(b));   // split_rows 0: the fp32 GEMMs never split K, so row e's sums do not depend on E
@@ -2864,7 +2998,7 @@ int actor_create(dz_learner* l, bool frozen, int32_t num_streams, void* d_worksp
     if (rc == DZ_OK && a->noise) rc = um_bind_noise(a->um, a->noise);
     if (rc != DZ_OK) { dz_actor_destroy(a); return rc; }
     for (int L = 1; L <= 3; ++L) (L == 1 ? a->b.act1 : L == 2 ? a->b.act2 : a->b.act3)[1] = um_act_f32(a->um, L, 0);
-    if (l->cfg.kind != DZ_IQN)
+    if (!uses_iqn_net(l->cfg.kind))
       for (int s = 0; s < (l->cfg.kind == DZ_RAINBOW ? 2 : 1); ++s) a->b.h1[1][s] = um_h1_f32(a->um, 0, s);
   }
   *out = a;
@@ -2953,7 +3087,7 @@ int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const f
   const int E = a->E;
   const bool rb = c.kind == DZ_RAINBOW;
   if (!d_obs || !d_q_out || !d_actions) return fail(DZ_EINVAL, "actor: null buffer");
-  if (c.kind == DZ_IQN && !d_taus) return fail(DZ_EINVAL, "iqn actor needs taus[E][tau_samples_policy]");
+  if (uses_iqn_net(c.kind) && !d_taus) return fail(DZ_EINVAL, "iqn actor needs taus[E][tau_samples_policy]");
   if (rb && !d_noise) return fail(DZ_EINVAL, "rainbow actor needs noise");
   const int64_t stride = rb ? noise_layout(c, l->d).stride : 0;
   if (noise_ld != 0 && (!rb || noise_ld != stride))
@@ -2962,7 +3096,7 @@ int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const f
   const float* on = a->frozen ? a->params : l->buf.d_online;
   const long long obs_bytes = (long long)l->d.H * l->d.W * l->d.C;
   DZ_LAUNCH(make_row_table_kernel, (unsigned)ceil_div(E, 64), 64, 0, stream, d_obs, obs_bytes, E, a->rows);
-  const bool fc_done = a->um && c.kind != DZ_IQN && noise_ld == 0;
+  const bool fc_done = a->um && !uses_iqn_net(c.kind) && noise_ld == 0;
   if (a->um) {
     const uint8_t* const* rows[3] = {a->rows, nullptr, nullptr};
     if (!a->frozen) DZ_TRY(um_pack_weights(a->um, stream));   // frozen: packed by load_params
@@ -2977,7 +3111,7 @@ int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const f
   }
   Pass pass{on, 1, 1, 0};
   int nq = 1;
-  if (c.kind == DZ_IQN) {
+  if (uses_iqn_net(c.kind)) {
     const float* taus[1] = {d_taus};
     DZ_TRY(forward_heads_iqn(l, a->b, &pass, 1, E, taus, false, stream));
     nq = c.tau_samples_policy;
@@ -2988,7 +3122,7 @@ int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const f
     nq = c.num_quantiles;
   }
   size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
-  DZ_LAUNCH(q_values_kernel, (unsigned)E, 128, smem, stream, c.kind, c.num_actions, c.num_atoms, nq, c.vmax, a->b.out[1], a->b.out[1],
+  DZ_LAUNCH(q_values_kernel, (unsigned)E, 128, smem, stream, net_kind(c.kind), c.num_actions, c.num_atoms, nq, c.vmax, a->b.out[1], a->b.out[1],
             a->b.outv[1], d_q_out);
   DZ_LAUNCH(act_select_kernel, (unsigned)ceil_div(E, 128), 128, 0, stream, (const float*)d_q_out, c.num_actions, E, d_explore, epsilon,
             d_actions);
@@ -3003,13 +3137,14 @@ int dz_actor_generate_randomness(dz_actor* a, uint64_t seed, int32_t per_stream,
   if (!a || !d_out) return fail(DZ_EINVAL, "actor randomness: null argument");
   const dz_learner_config& c = a->l->cfg;
   long long n;
-  if (c.kind == DZ_IQN && !per_stream) n = (long long)a->E * c.tau_samples_policy;
+  const bool iqn = uses_iqn_net(c.kind);
+  if (iqn && !per_stream) n = (long long)a->E * c.tau_samples_policy;
   else if (c.kind == DZ_RAINBOW) n = (per_stream ? (long long)a->E : 1LL) * noise_layout(c, a->l->d).stride;
   else return fail(DZ_EINVAL, "actor randomness: iqn draws taus, rainbow noise (per_stream: rainbow only); other kinds draw nothing");
-  const int kind = c.kind == DZ_IQN ? 0 : 1;
+  const int kind = iqn ? 0 : 1;
   int64_t* counters = a->frozen ? a->counters : a->l->buf.d_counters;
   DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_out, n, seed, counters, kind,
-            c.kind == DZ_IQN ? 1u : 2u);
+            iqn ? 1u : 2u);
   DZ_LAUNCH(bump_counter_kernel, 1, 1, 0, stream, counters, 1);
   return DZ_OK;
 }
@@ -3114,6 +3249,46 @@ int dz_test_munchausen_example(const float* q_tm1, const float* qbar_tm1, const 
   out[0] = m.target;
   out[1] = m.target - q_tm1[a_tm1];
   out[2] = m.bonus;
+  return DZ_OK;
+}
+
+// Host twin of loss_munchausen_iqn_kernel's per-example target arithmetic: the same miqn_mean sums, the warp's
+// xor-butterfly reductions over an array of 32 lanes, then the same munchausen_exp / miqn_h / munchausen_bonus /
+// miqn_target (tests only).
+int dz_test_munchausen_iqn_example(const float* zbar_tm1, const float* zbar_t, int32_t A, int32_t K, int32_t Nt,
+                                   int32_t a_tm1, float r_t, float discount_t, float alpha, float tau, float l0, float* out) {
+  if (!zbar_tm1 || !zbar_t || !out) return fail(DZ_EINVAL, "munchausen_iqn example: NULL buffer");
+  if (A < 1 || A > kMunchausenMaxActions || a_tm1 < 0 || a_tm1 >= A || K < 1 || K > 256 || Nt < 1 || Nt > 256)
+    return fail(DZ_EINVAL, "munchausen_iqn example: A, K, Nt or a_tm1 out of range");
+  if (!munchausen_params_ok(alpha, tau, l0)) return fail(DZ_EINVAL, "munchausen_iqn example: bad alpha / tau / l0");
+  auto butterfly = [](const float* in, bool is_max) {
+    float v[32];
+    for (int i = 0; i < 32; ++i) v[i] = in[i];
+    for (int o = 16; o > 0; o >>= 1) {
+      float t[32];
+      for (int i = 0; i < 32; ++i) t[i] = is_max ? fmaxf(v[i], v[i ^ o]) : v[i] + v[i ^ o];
+      for (int i = 0; i < 32; ++i) v[i] = t[i];
+    }
+    return v[0];
+  };
+  float q[2][32], lane[32];
+  for (int a = 0; a < 32; ++a) {
+    q[0][a] = a < A ? miqn_mean(zbar_tm1, K, A, a) : -INFINITY;
+    q[1][a] = a < A ? miqn_mean(zbar_t, Nt, A, a) : -INFINITY;
+  }
+  const float v1 = butterfly(q[0], true), v2 = butterfly(q[1], true);
+  for (int a = 0; a < 32; ++a) lane[a] = a < A ? munchausen_exp(q[0][a], v1, tau) : 0.f;
+  const float s1 = butterfly(lane, false);
+  float e2[32], pi[32];
+  for (int a = 0; a < 32; ++a) e2[a] = a < A ? munchausen_exp(q[1][a], v2, tau) : 0.f;
+  const float s2 = butterfly(e2, false);
+  for (int a = 0; a < 32; ++a) pi[a] = e2[a] / s2;
+  for (int a = 0; a < 32; ++a) lane[a] = a < A ? pi[a] * miqn_h(q[1][a], v2, s2, tau) : 0.f;
+  const float ent = butterfly(lane, false);
+  const float bonus = munchausen_bonus(q[0][a_tm1], v1, s1, alpha, tau, l0);
+  for (int j = 0; j < Nt; ++j) out[j] = miqn_target(zbar_t + (long long)j * A, pi, A, r_t + bonus, discount_t, ent);
+  out[Nt] = bonus;
+  out[Nt + 1] = ent;
   return DZ_OK;
 }
 

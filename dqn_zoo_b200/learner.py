@@ -44,11 +44,17 @@ def default_optimizer(kind: str) -> OptimizerSpec:
     return OptimizerSpec('adam', 0.00005, 0.01 / 32, max_global_grad_norm=10.0)
   if kind == 'rainbow':
     return OptimizerSpec('adam', 0.0000625, 0.005 / 32, max_global_grad_norm=10.0)  # rainbow/run_atari.py:229-235
-  if kind == 'iqn':
-    return OptimizerSpec('adam', 0.00005, 0.01 / 32)
+  if uses_iqn_network(kind):
+    return OptimizerSpec('adam', 0.00005, 0.01 / 32)   # munchausen_iqn: iqn's, as the M-IQN paper's Atari values
   if kind == 'munchausen':
     return OptimizerSpec('adam', 0.00005, 0.01 / 32)   # the M-DQN paper's Atari values; no run_atari pins them
   raise ValueError(kind)
+
+
+def uses_iqn_network(kind: str) -> bool:
+  """Whether the agent kind applies IQN's network (cosine tau embedding, quantile samples, taus drawn per step):
+  iqn, and munchausen_iqn (DESIGN.md §14), which shares its parameters, taus and acting."""
+  return kind in ('iqn', 'munchausen_iqn')
 
 
 class NetworkSpec(NamedTuple):
@@ -77,7 +83,7 @@ def haiku_name(canonical: str, kind: str):
   if kind == 'rainbow':
     idx = {'adv1': '', 'adv2': '_1', 'val1': '_2', 'val2': '_3'}[parts[0]]
     return 'noisy_linear%s/%s' % (idx, parts[1]), leaf
-  if kind == 'iqn':
+  if uses_iqn_network(kind):
     return {'embed': 'batch_apply/linear', 'fc1': 'batch_apply_1/sequential/linear',
             'head': 'batch_apply_1/sequential/linear_1'}[parts[0]], leaf
   return {'fc1': 'sequential/sequential_1/linear', 'head': 'sequential/sequential_1/linear_1'}[parts[0]], leaf
@@ -120,9 +126,9 @@ class Learner:
   def __init__(self, net: NetworkSpec, batch_size: int = 32, optimizer: Optional[OptimizerSpec] = None,
                grad_error_bound: float = 1.0 / 32, huber_param: float = 1.0, munchausen_alpha: float = 0.9,
                entropy_temperature: float = 0.03, log_policy_clip: float = -1.0, device=None):
-    """`munchausen_alpha`, `entropy_temperature` (tau) and `log_policy_clip` (l0) are Munchausen DQN's (DESIGN.md §13,
-    defaults the paper's Atari values); the library rejects tau <= 0, alpha < 0, l0 > 0 and non-finite values for that
-    kind, and the other kinds ignore them."""
+    """`munchausen_alpha`, `entropy_temperature` (tau) and `log_policy_clip` (l0) are Munchausen DQN's and
+    Munchausen-IQN's (DESIGN.md §13, §14, defaults the paper's Atari values); the library rejects tau <= 0, alpha < 0,
+    l0 > 0 and non-finite values for those kinds, and the other kinds ignore them."""
     if not torch.cuda.is_available():
       raise RuntimeError('dqn_zoo_b200.learner needs a CUDA device (there is no CPU fallback)')
     self.net = net
@@ -277,7 +283,7 @@ class Learner:
       self.noise[:flat.numel()].copy_(flat)
     batch = _lib.Batch(keep[2].data_ptr(), keep[3].data_ptr(), keep[4].data_ptr(), keep[5].data_ptr(),
                        keep[6].data_ptr(), 0 if w is None else w.data_ptr(),
-                       self.taus.data_ptr() if self.kind == 'iqn' else 0,
+                       self.taus.data_ptr() if uses_iqn_network(self.kind) else 0,
                        self.noise.data_ptr() if self.kind == 'rainbow' else 0)
     out = _lib.UpdateOutputs(self.loss.data_ptr(), self.per_example.data_ptr(), self.priorities.data_ptr(),
                              self.grad_norm.data_ptr())
@@ -360,7 +366,7 @@ class Learner:
     io.sample_in = _lib.SampleInputs(base, base + 8 * B, base + 16 * B, base + 24 * B)
     sp, fp = self.s_ids.data_ptr(), self.s_f64.data_ptr()
     io.sample_out = _lib.SampleOutputs(sp, sp + 8 * B, sp + 16 * B, fp, fp + 8 * B)
-    io.d_taus = self.taus.data_ptr() if self.kind == 'iqn' else 0
+    io.d_taus = self.taus.data_ptr() if uses_iqn_network(self.kind) else 0
     io.d_noise = self.noise.data_ptr() if self.kind == 'rainbow' else 0
     io.update_out = _lib.UpdateOutputs(self.loss.data_ptr(), self.per_example.data_ptr(), self.priorities.data_ptr(),
                                        self.grad_norm.data_ptr())
@@ -419,7 +425,7 @@ class Actor:
       torch.cuda.current_stream().synchronize()   # create zeroes the counter on the legacy stream: after the fill
     self.q = torch.zeros((E, net.num_actions), dtype=torch.float32, device=dev)
     self.actions = torch.zeros(E, dtype=torch.int32, device=dev)
-    self.taus = torch.zeros((E, net.tau_samples_policy), dtype=torch.float32, device=dev) if net.kind == 'iqn' else None
+    self.taus = torch.zeros((E, net.tau_samples_policy), dtype=torch.float32, device=dev) if uses_iqn_network(net.kind) else None
     rb = net.kind == 'rainbow'
     self.noise = torch.zeros(learner.noise_stride, dtype=torch.float32, device=dev) if rb else None
     self.stream_noise = torch.zeros((E, learner.noise_stride), dtype=torch.float32, device=dev) if rb else None
@@ -513,9 +519,9 @@ class Actor:
     kind = self.kind
     if per_stream and kind != 'rainbow':
       raise ValueError('per_stream randomness needs a rainbow learner')
-    if kind not in ('iqn', 'rainbow'):
+    if not uses_iqn_network(kind) and kind != 'rainbow':
       raise ValueError('%s acting draws no randomness' % kind)
-    buf = self.taus if kind == 'iqn' else (self.stream_noise if per_stream else self.noise)
+    buf = self.taus if uses_iqn_network(kind) else (self.stream_noise if per_stream else self.noise)
     _lib.call('dz_actor_generate_randomness', self._h, seed, 1 if per_stream else 0, buf.data_ptr(), _cstream())
     return buf
 
@@ -549,7 +555,7 @@ class Actor:
     else:
       if taus is not None:
         t = torch.as_tensor(taus, device=L.device).to(torch.float32).contiguous()
-        if L.kind == 'iqn' and t.numel() != E * L.net.tau_samples_policy:
+        if uses_iqn_network(L.kind) and t.numel() != E * L.net.tau_samples_policy:
           raise ValueError('taus must be [%d, %d], got %s' % (E, L.net.tau_samples_policy, tuple(t.shape)))
       if noise is not None:
         n = torch.as_tensor(noise, device=L.device).to(torch.float32).contiguous()

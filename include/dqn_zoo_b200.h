@@ -309,10 +309,12 @@ int dz_replay_update_priorities(const dz_replay_view* view, const int64_t* d_ind
  * iqn/agent.py:178-226; networks: networks.py:58-363)
  * ---------------------------------------------------------------------------------------- */
 
-/* DZ_MUNCHAUSEN: Munchausen DQN (Vieillard, Pietquin & Geist, NeurIPS 2020), the one agent outside the reference tree:
- * dqn's network, parameter layout and acting, with the soft, log-policy-augmented target of DESIGN.md §13. */
+/* DZ_MUNCHAUSEN: Munchausen DQN (Vieillard, Pietquin & Geist, NeurIPS 2020), outside the reference tree: dqn's
+ * network, parameter layout and acting, with the soft, log-policy-augmented target of DESIGN.md §13.
+ * DZ_MUNCHAUSEN_IQN: Munchausen-IQN from the same paper: iqn's network, parameter layout, taus and acting, with the
+ * soft target over quantile samples of DESIGN.md §14. */
 enum dz_agent_kind { DZ_DQN = 0, DZ_DOUBLE_Q = 1, DZ_PRIORITIZED = 2, DZ_C51 = 3, DZ_QRDQN = 4, DZ_RAINBOW = 5, DZ_IQN = 6,
-                     DZ_MUNCHAUSEN = 7 };
+                     DZ_MUNCHAUSEN = 7, DZ_MUNCHAUSEN_IQN = 8 };
 enum dz_optimizer_kind { DZ_ADAM = 0, DZ_RMSPROP_CENTERED = 1 };
 
 typedef struct dz_learner_config {
@@ -320,8 +322,8 @@ typedef struct dz_learner_config {
   int32_t num_actions;
   int32_t num_atoms;         /* c51 / rainbow: 51 */
   int32_t num_quantiles;     /* qrdqn: 201 */
-  int32_t latent_dim;        /* iqn: 64 */
-  int32_t tau_samples_s_tm1, tau_samples_policy, tau_samples_s_t; /* iqn: N, K, N' */
+  int32_t latent_dim;        /* iqn / munchausen_iqn: 64 */
+  int32_t tau_samples_s_tm1, tau_samples_policy, tau_samples_s_t; /* iqn / munchausen_iqn: N, K, N' */
   int32_t batch;             /* 32 */
   int32_t obs_h, obs_w, obs_c; /* 84,84,4 */
   float vmax;                /* c51 / rainbow support is linspace(-vmax, vmax, atoms) */
@@ -330,8 +332,9 @@ typedef struct dz_learner_config {
   int32_t optimizer;         /* dz_optimizer_kind */
   float learning_rate, opt_eps, rms_decay, adam_b1, adam_b2;
   float max_global_grad_norm; /* 0 = off (optax.clip_by_global_norm) */
-  /* munchausen only (other kinds ignore them, so a zero-filled tail is valid there); dz_learner_create and
-   * dz_learner_plan_query return DZ_EINVAL unless all three are finite, tau > 0, alpha >= 0 and l0 <= 0 */
+  /* munchausen and munchausen_iqn only (other kinds ignore them, so a zero-filled tail is valid there);
+   * dz_learner_create and dz_learner_plan_query return DZ_EINVAL unless all three are finite, tau > 0, alpha >= 0
+   * and l0 <= 0 */
   float munchausen_alpha;    /* scale of the log-policy bonus: 0.9 */
   float entropy_temperature; /* tau of the softmax policy of the target network: 0.03 */
   float log_policy_clip;     /* l0, the lower clip of tau * log pi: -1 */
@@ -647,6 +650,13 @@ int dz_test_learner_buffer(dz_learner* l, const char* name, float** d_ptr, int64
  * A or a_tm1 out of range and for the hyperparameters dz_learner_create rejects; tests only. */
 int dz_test_munchausen_example(const float* q_tm1, const float* qbar_tm1, const float* qbar_t, int32_t A, int32_t a_tm1,
                                float r_t, float discount_t, float alpha, float tau, float l0, float* out);
+/* The per-example target arithmetic of the munchausen_iqn loss kernel evaluated on the HOST by the same source (fp32,
+ * expf / logf): zbar_tm1 = target(s_tm1) at the K policy taus [K][A], zbar_t = target(s_t) at the N' taus [Nt][A]
+ * (1 <= A <= 18, 1 <= K, Nt <= 256).  Writes the targets y_j to out[0 .. Nt), the log-policy bonus
+ * alpha * clip(tau * log pi(a_tm1 | s_tm1), l0, 0) to out[Nt] and the entropy term sum_a pi(a|s_t) h_t(a) to out[Nt + 1].
+ * DZ_EINVAL for sizes or a_tm1 out of range and for the hyperparameters dz_learner_create rejects; tests only. */
+int dz_test_munchausen_iqn_example(const float* zbar_tm1, const float* zbar_t, int32_t A, int32_t K, int32_t Nt,
+                                   int32_t a_tm1, float r_t, float discount_t, float alpha, float tau, float l0, float* out);
 int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream);   /* device-to-device, tests only */
 /* Debug: the tensor-core launch named `tag` writes the clock stamps of its CTA 0 into d_trace (512 int64). */
 int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace);

@@ -136,7 +136,7 @@ def compare_actor(a, streams):
     obs = torch.randint(0, 256, (E, 84, 84, 4), dtype=torch.uint8, device='cuda')
     explore = torch.as_tensor(rs.uniform(size=(2, E)).astype(np.float32), device='cuda')
     kw = {}
-    if a.agent == 'iqn':
+    if dl.uses_iqn_network(a.agent):
       kw['taus'] = torch.as_tensor(rs.uniform(size=(E, net.tau_samples_policy)).astype(np.float32), device='cuda')
     if a.agent == 'rainbow':
       L32.generate_randomness(1)
@@ -215,7 +215,7 @@ def main():
   noise = taus = None
   if a.agent == 'rainbow':
     noise = L.noise
-  if a.agent == 'iqn':
+  if dl.uses_iqn_network(a.agent):
     taus = L.taus[:64]
   for _ in range(20):
     L.q_values(obs[0], taus=taus, noise=noise).cpu()

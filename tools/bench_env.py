@@ -162,6 +162,10 @@ def learning_agent(seed, train_frames, kind='dqn', num_actions=6):
   rep = dr.TransitionReplay(capacity, structure, rs, frame_dedup=True)
   epsilon = parts.LinearSchedule(begin_t=4 * min_fill, decay_steps=max(train_frames // 4, 1), begin_value=1.0,
                                  end_value=0.01)
+  if dl.uses_iqn_network(kind):   # iqn / munchausen_iqn: dqn's schedule, iqn's 64 / 64 / 64 taus and kappa 1
+    return ag.AGENTS[kind](transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep,
+                           exploration_epsilon=epsilon, huber_param=1.0, tau_samples_policy=64, tau_samples_s_tm1=64,
+                           tau_samples_s_t=64, **common)
   agent_cls = ag.Munchausen if kind == 'munchausen' else ag.Dqn   # munchausen: dqn's schedule, the paper's alpha / tau / l0
   return agent_cls(transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep, exploration_epsilon=epsilon,
                    grad_error_bound=1.0 / 32, **common)
@@ -213,7 +217,7 @@ def learning_run(train_frames, seed=0, num_streams=32, eval_every=0, log=None, g
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--game', default='catch', choices=['catch', 'breakout', 'pong'])
-  ap.add_argument('--agent', default='dqn', choices=['dqn', 'rainbow', 'munchausen'],
+  ap.add_argument('--agent', default='dqn', choices=['dqn', 'rainbow', 'munchausen', 'iqn', 'munchausen_iqn'],
                   help='the agent of the learning curve')
   ap.add_argument('--parts', default='env,train,eval,driver')
   ap.add_argument('--frames', type=int, default=65536, help='frames per timed window of env_train / env_eval')

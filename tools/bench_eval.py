@@ -116,7 +116,7 @@ def act_time(kind, E, acts, frozen):
     actor.load_params(L)
   obs = torch.randint(0, 256, (E, 84, 84, 4), dtype=torch.uint8, device='cuda')
   kw = {}
-  if kind == 'iqn':
+  if dl.uses_iqn_network(kind):
     kw['taus'] = actor.generate_randomness(1)
   elif kind == 'rainbow':
     kw['noise'] = actor.generate_randomness(1)

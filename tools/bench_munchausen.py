@@ -2,7 +2,10 @@
 84x84x4, batch 32, 6 actions, on a synthetic uniform replay, the three agents alternated over `--rounds` rounds in one
 process so that they share the machine's state.  Then one eager profiled pass of each (per-launch CUDA events,
 dz_profile_begin / end) for the loss kernels' times.  One JSON line per result.
-  python tools/bench_munchausen.py [--steps 2000] [--rounds 3]
+  python tools/bench_munchausen.py [--steps 2000] [--rounds 3] [--kinds munchausen,double_q,dqn]
+
+`--kinds munchausen_iqn,iqn` times Munchausen-IQN beside iqn (64 / 64 / 64 taus drawn on the device each step): it adds
+a third torso pass, target(s_tm1), to iqn's two, so its step should cost iqn's plus about one torso pass.
 
 The expectation this checks: munchausen applies three networks per step like double_q (online(s_tm1) with
 target(s_tm1) and target(s_t) instead of online(s_t) and target(s_t)), the two target passes sharing each staged fc1
@@ -23,6 +26,7 @@ import torch  # noqa: E402
 import bench_train  # noqa: E402
 
 KINDS = ('munchausen', 'double_q', 'dqn')
+ALL_KINDS = KINDS + ('munchausen_iqn', 'iqn')
 
 
 def emit(**kw):
@@ -41,6 +45,9 @@ def make_agent(kind, capacity=65536, seed=1):
                 transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep, batch_size=32,
                 min_replay_capacity_fraction=0.02, learn_period=16, target_network_update_period=32000,
                 rng_key=[0, seed])
+  if dl.uses_iqn_network(kind):
+    return ag.AGENTS[kind](exploration_epsilon=lambda t: 0.01, huber_param=1.0, tau_samples_policy=64,
+                           tau_samples_s_tm1=64, tau_samples_s_t=64, **common)
   return ag.AGENTS[kind](exploration_epsilon=lambda t: 0.01, grad_error_bound=1.0 / 32, **common)
 
 
@@ -75,25 +82,29 @@ def main():
   ap.add_argument('--steps', type=int, default=2000)
   ap.add_argument('--warmup', type=int, default=200)
   ap.add_argument('--rounds', type=int, default=3)
+  ap.add_argument('--kinds', default=','.join(KINDS), help='comma-separated agent kinds, alternated in this order')
   a = ap.parse_args()
+  kinds = tuple(a.kinds.split(','))
+  if not kinds or any(k not in ALL_KINDS for k in kinds):
+    raise SystemExit('--kinds: choose from %s' % ', '.join(ALL_KINDS))
   if not torch.cuda.is_available():
     raise SystemExit('bench_munchausen.py needs a CUDA device')
   torch.cuda.set_device(0)
   emit(metric='device', **bench_train.device_info())
-  agents = {k: make_agent(k) for k in KINDS}
+  agents = {k: make_agent(k) for k in kinds}
   for k, ag in agents.items():
     for _ in range(a.warmup):
       ag.learn()
-  times = {k: [] for k in KINDS}
+  times = {k: [] for k in kinds}
   for r in range(a.rounds):
-    for k in KINDS:
+    for k in kinds:
       us = time_steps(agents[k], a.steps)
       times[k].append(us)
       emit(metric='learn_step_us', agent=k, round=r, steps=a.steps, us=round(us, 2))
-  for k in KINDS:
+  for k in kinds:
     emit(metric='learn_step_us_summary', agent=k, median=round(float(np.median(times[k])), 2),
          min=round(min(times[k]), 2), max=round(max(times[k]), 2))
-  for k in KINDS:
+  for k in kinds:
     prof = profile_step(agents[k])
     loss = {t: v for t, v in prof.items() if t.startswith('loss_')}
     emit(metric='loss_kernel_us', agent=k, kernels={t: v[0] for t, v in loss.items()})

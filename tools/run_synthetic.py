@@ -106,8 +106,8 @@ def build_train_agent(args, random_state, preprocessor):
     return agent_lib.C51(support=np.linspace(-10, 10, 51), exploration_epsilon=epsilon, **common), network
   if kind == 'qrdqn':
     return agent_lib.QrDqn(quantiles=(np.arange(201) + 0.5) / 201, exploration_epsilon=epsilon, huber_param=1.0, **common), network
-  if kind == 'iqn':
-    return agent_lib.Iqn(exploration_epsilon=epsilon, huber_param=1.0, tau_samples_policy=64, tau_samples_s_tm1=64,
+  if learner_lib.uses_iqn_network(kind):
+    return agent_lib.AGENTS[kind](exploration_epsilon=epsilon, huber_param=1.0, tau_samples_policy=64, tau_samples_s_tm1=64,
                          tau_samples_s_t=64, **common), network
   return agent_lib.AGENTS[kind](exploration_epsilon=epsilon, grad_error_bound=1.0 / 32, **common), network
 
@@ -256,7 +256,8 @@ def parse_args(argv=None):
                   help='synthetic: random host frames; catch / breakout / pong: a game simulated and rendered on the device '
                        '(dqn_zoo_b200.environments)')
   ap.add_argument('--agent', default='dqn',
-                  choices=['dqn', 'double_q', 'prioritized', 'c51', 'qrdqn', 'rainbow', 'iqn', 'munchausen'])
+                  choices=['dqn', 'double_q', 'prioritized', 'c51', 'qrdqn', 'rainbow', 'iqn', 'munchausen',
+                           'munchausen_iqn'])
   ap.add_argument('--num_actions', type=int, default=6)
   ap.add_argument('--replay_capacity', type=int, default=20000)
   ap.add_argument('--min_replay_capacity_fraction', type=float, default=0.05)
