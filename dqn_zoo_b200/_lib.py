@@ -60,6 +60,10 @@ class LearnerConfig(C.Structure):
               ('adam_b1', f32), ('adam_b2', f32), ('max_global_grad_norm', f32), ('munchausen_alpha', f32),
               ('entropy_temperature', f32), ('log_policy_clip', f32)]
 
+  def __init__(self, **fields):
+    # the loss hyperparameters start at the reference's values instead of 0, which the library rejects for vmax
+    super().__init__(**dict(dict(vmax=10.0, grad_error_bound=1.0 / 32, huber_param=1.0), **fields))
+
 
 class LearnerPlan(C.Structure):
   _fields_ = [('param_count', i64), ('num_tensors', i32), ('opt_state_floats', i64), ('workspace_bytes', i64),
@@ -200,6 +204,9 @@ _SIGNATURES = {
     'dz_test_learner_buffer': (i32, [vp, C.c_char_p, vp, vp]),
     'dz_test_munchausen_example': (i32, [vp, vp, vp, i32, i32, f32, f32, f32, f32, f32, vp]),
     'dz_test_munchausen_iqn_example': (i32, [vp, vp, i32, i32, i32, i32, f32, f32, f32, f32, f32, vp]),
+    'dz_test_loss': (i32, [C.POINTER(LearnerConfig), i32, C.POINTER(vp), C.POINTER(vp), vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                           vp, vp, vp, vp]),
+    'dz_test_q_values': (i32, [C.POINTER(LearnerConfig), i32, vp, vp, vp, f32, vp, vp, vp]),
     'dz_test_copy': (i32, [vp, vp, i64, vp]),
     'dz_test_learner_trace': (i32, [vp, C.c_char_p, vp]),
     'dz_test_learner_mma_path': (i32, [vp, C.c_char_p, C.POINTER(i32)]),

@@ -230,6 +230,12 @@ static int validate(const dz_learner_config& c) {
     return fail(DZ_EINVAL, "munchausen needs finite alpha >= 0, entropy_temperature > 0 and log_policy_clip <= 0");
   if (is_munchausen(c.kind) && c.num_actions > kMunchausenMaxActions)
     return fail(DZ_EINVAL, "munchausen: num_actions must be in [1,18] (one warp lane per action)");
+  // The loss hyperparameters of every kind: the kernels take them as given, so a NaN or a sign error would train on
+  // silently wrong targets (a support of -vmax..vmax turned inside out, a negative clip range or Huber width).
+  if (!std::isfinite(c.vmax) || !(c.vmax > 0.f)) return fail(DZ_EINVAL, "vmax must be finite and > 0");
+  if (!std::isfinite(c.huber_param) || c.huber_param < 0.f) return fail(DZ_EINVAL, "huber_param must be finite and >= 0");
+  if (!std::isfinite(c.grad_error_bound) || c.grad_error_bound < 0.f)
+    return fail(DZ_EINVAL, "grad_error_bound must be finite and >= 0");
   if (c.batch <= 0 || c.batch > 1024) return fail(DZ_EINVAL, "batch must be in [1,1024]");
   if (c.obs_c != 4) return fail(DZ_EINVAL, "obs_c must be 4 (stacked frames; conv1 reads uchar4 pixels)");
   if (c.obs_w % 4) return fail(DZ_EINVAL, "obs_w must be a multiple of 4");
@@ -2477,6 +2483,59 @@ int run_optimizer(dz_learner* l, float* user_norm, bool apply, void* stream) {
   return DZ_OK;
 }
 
+// The loss section of a learner step: the agent kind's loss kernel on `stream`, then loss_mean_kernel (the scalar loss,
+// and rainbow's running max priority when max_seen is given).  L carries the buffers: head outputs, batch, outputs and
+// loss_terms; every field that follows from the configuration (sizes, vmax, bound, kappa, whether priorities are
+// written) is set here.  With `side`, loss_mean_kernel runs on the side stream forked after the loss kernel and
+// *mean_stream receives it; without, everything runs on `stream`.  dz_test_loss runs this same function.
+int launch_loss(const dz_learner_config& c, LossArgs& L, int B, void* stream, SideStream* side, float* d_loss, float* max_seen,
+                void** mean_stream) {
+  L.kind = c.kind; L.B = B; L.A = c.num_actions; L.atoms = c.num_atoms;
+  L.vmax = c.vmax; L.bound = c.grad_error_bound; L.kappa = c.huber_param;
+  if (!(c.kind == DZ_RAINBOW || c.kind == DZ_PRIORITIZED)) L.priorities = nullptr;
+  if (c.kind == DZ_DQN || c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED) {
+    DZ_LAUNCH(loss_q_kernel, B, 64, 0, stream, L);
+  } else if (c.kind == DZ_MUNCHAUSEN) {
+    DZ_LAUNCH(loss_munchausen_kernel, (B + 3) / 4, 128, 0, stream, L, c.munchausen_alpha, c.entropy_temperature,
+              c.log_policy_clip);
+  } else if (c.kind == DZ_C51 || c.kind == DZ_RAINBOW) {
+    // More than the default 48 KB of dynamic shared memory at large num_actions x num_atoms; the attribute is per
+    // device, so it is set for the current one.
+    const size_t smem = categorical_loss_smem(c);
+    if (smem > 48 * 1024)
+      DZ_CUDA_OK(cudaFuncSetAttribute(loss_categorical_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    DZ_LAUNCH_NAMED("loss_categorical_kernel", loss_categorical_staged_kernel, B, 128, smem, stream, L);
+  } else if (c.kind == DZ_MUNCHAUSEN_IQN) {
+    L.N = c.tau_samples_s_tm1; L.Ksel = c.tau_samples_policy; L.Nt = c.tau_samples_s_t;
+    DZ_LAUNCH(loss_munchausen_iqn_kernel, B, 256, munchausen_iqn_loss_smem(c), stream, L, c.munchausen_alpha,
+              c.entropy_temperature, c.log_policy_clip);
+  } else {
+    if (c.kind == DZ_QRDQN) { L.N = c.num_quantiles; L.Ksel = c.num_quantiles; L.Nt = c.num_quantiles; }
+    else { L.N = c.tau_samples_s_tm1; L.Ksel = c.tau_samples_policy; L.Nt = c.tau_samples_s_t; }
+    size_t smem = (32 + c.num_actions + L.Nt + 2 * L.N) * sizeof(float);
+    DZ_LAUNCH(loss_quantile_kernel, B, 256, smem, stream, L);
+  }
+  void* ms = side ? side->fork(stream, stream) : stream;
+  DZ_LAUNCH(loss_mean_kernel, 1, 32, 0, ms, L.loss_terms, B, d_loss, max_seen, L.priorities);
+  if (mean_stream) *mean_stream = ms;
+  return DZ_OK;
+}
+
+// The acting tail of a head pass over E observations: q-values [E][A] (q_values_kernel) and, when `actions` is given,
+// the epsilon-greedy choice (act_select_kernel).  out: the head outputs of the pass (rainbow: the advantage stream),
+// val: rainbow's value stream.  dz_learner_q_values, batched acting, the actor and dz_test_q_values run this function.
+int launch_q_values(const dz_learner_config& c, int E, const float* out, const float* val, const float* explore, float epsilon,
+                    float* q, int32_t* actions, void* stream) {
+  const int nq = uses_iqn_net(c.kind) ? c.tau_samples_policy : c.num_quantiles;
+  const size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
+  DZ_LAUNCH(q_values_kernel, (unsigned)E, 128, smem, stream, net_kind(c.kind), c.num_actions, c.num_atoms, nq, c.vmax, out, out,
+            val, q);
+  if (actions)
+    DZ_LAUNCH(act_select_kernel, (unsigned)ceil_div(E, 128), 128, 0, stream, (const float*)q, c.num_actions, E, explore, epsilon,
+              actions);
+  return DZ_OK;
+}
+
 struct WriteBack { const dz_replay_view* view; const int64_t* indices; const float* priorities; double alpha; };
 
 int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* out, int apply_update, float* max_seen,
@@ -2539,35 +2598,15 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   // ---- loss + gradient wrt the pass-0 head outputs
   LossArgs L;
   memset(&L, 0, sizeof(L));
-  L.kind = c.kind; L.B = B; L.A = c.num_actions; L.atoms = c.num_atoms;
   L.out0 = l->out[0]; L.out1 = l->out[1]; L.out2 = l->out[2];
   L.adv0 = l->out[0]; L.val0 = l->outv[0]; L.adv1 = l->out[1]; L.val1 = l->outv[1]; L.adv2 = l->out[2]; L.val2 = l->outv[2];
   L.a = batch->d_a_tm1; L.r = batch->d_r_t; L.disc = batch->d_discount_t; L.w = batch->d_weights; L.taus0 = batch->d_taus;
-  L.vmax = c.vmax; L.bound = c.grad_error_bound; L.kappa = c.huber_param;
   L.dout = l->dout; L.dadv = l->dout; L.dval = l->doutv;
-  L.per_example = out->d_per_example; L.loss_terms = l->loss_terms;
-  L.priorities = (c.kind == DZ_RAINBOW || c.kind == DZ_PRIORITIZED) ? out->d_priorities : nullptr;
-  if (c.kind == DZ_DQN || c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED) {
-    DZ_LAUNCH(loss_q_kernel, B, 64, 0, stream, L);
-  } else if (c.kind == DZ_MUNCHAUSEN) {
-    DZ_LAUNCH(loss_munchausen_kernel, (B + 3) / 4, 128, 0, stream, L, c.munchausen_alpha, c.entropy_temperature,
-              c.log_policy_clip);
-  } else if (c.kind == DZ_C51 || c.kind == DZ_RAINBOW) {
-    DZ_LAUNCH_NAMED("loss_categorical_kernel", loss_categorical_staged_kernel, B, 128, categorical_loss_smem(c), stream, L);
-  } else if (c.kind == DZ_MUNCHAUSEN_IQN) {
-    L.N = c.tau_samples_s_tm1; L.Ksel = c.tau_samples_policy; L.Nt = c.tau_samples_s_t;
-    DZ_LAUNCH(loss_munchausen_iqn_kernel, B, 256, munchausen_iqn_loss_smem(c), stream, L, c.munchausen_alpha,
-              c.entropy_temperature, c.log_policy_clip);
-  } else {
-    if (c.kind == DZ_QRDQN) { L.N = c.num_quantiles; L.Ksel = c.num_quantiles; L.Nt = c.num_quantiles; }
-    else { L.N = c.tau_samples_s_tm1; L.Ksel = c.tau_samples_policy; L.Nt = c.tau_samples_s_t; }
-    size_t smem = (32 + c.num_actions + L.Nt + 2 * L.N) * sizeof(float);
-    DZ_LAUNCH(loss_quantile_kernel, B, 256, smem, stream, L);
-  }
+  L.per_example = out->d_per_example; L.loss_terms = l->loss_terms; L.priorities = out->d_priorities;
   {   // the scalar loss / running max priority and replay.update_priorities(ids, priorities) (rainbow/agent.py:198) are
       // independent of the backward pass: both leave the critical path for the side stream
-    void* ls = l->side.fork(stream, stream);
-    DZ_LAUNCH(loss_mean_kernel, 1, 32, 0, ls, l->loss_terms, B, out->d_loss, max_seen, L.priorities);
+    void* ls = stream;
+    DZ_TRY(launch_loss(c, L, B, stream, &l->side, out->d_loss, max_seen, &ls));
     if (wb) DZ_TRY(launch_update_priorities(wb->view, wb->indices, wb->priorities, B, wb->alpha, wb->view->capacity, ls));
   }
 
@@ -2662,13 +2701,6 @@ int dz_learner_create(const dz_learner_config* cfg, const dz_learner_buffers* bu
   if (se == cudaSuccess) se = l->side2.create();
   if (se == cudaSuccess) se = l->side3.create();
   if (se != cudaSuccess) { dz_learner_destroy(l); return fail(DZ_ECUDA, "side streams: %s", cudaGetErrorString(se)); }
-  // The categorical loss needs more than the default 48 KB of dynamic shared memory at large num_actions x num_atoms.
-  // The attribute is per device: set it for the device this learner is created on.
-  const size_t loss_smem = categorical_loss_smem(*cfg);
-  if ((cfg->kind == DZ_C51 || cfg->kind == DZ_RAINBOW) && loss_smem > 48 * 1024) {
-    se = cudaFuncSetAttribute(loss_categorical_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)loss_smem);
-    if (se != cudaSuccess) { dz_learner_destroy(l); return fail(DZ_ECUDA, "kernel attributes: %s", cudaGetErrorString(se)); }
-  }
   if (l->pk_on) {
     // fused epilogues only write the valid region of these images: zero the padding once, and set the constant
     // row of ones (bias-gradient row) of the transposed activation image
@@ -2776,22 +2808,17 @@ int dz_learner_q_values(dz_learner* l, const uint8_t* d_obs, const float* d_taus
   TorsoJob job{on, l->rows_act, 1};   // use activation set 1 so a pending backward's set-0 buffers stay intact
   DZ_TRY(forward_torso(l, learner_bufs(l), &job, 1, 1, stream));
   Pass pass{on, 1, 1, 0};
-  int nq = 1;
   if (uses_iqn_net(c.kind)) {
     if (!d_taus) return fail(DZ_EINVAL, "iqn q_values needs taus[tau_samples_policy]");
     const float* taus[1] = {d_taus};
     DZ_TRY(forward_heads_iqn(l, learner_bufs(l), &pass, 1, 1, taus, false, stream));
-    nq = c.tau_samples_policy;
   } else if (c.kind == DZ_RAINBOW) {
     if (!d_noise) return fail(DZ_EINVAL, "rainbow q_values needs one apply of noise");
     DZ_TRY(forward_heads_rainbow(l, learner_bufs(l), &pass, 1, 1, d_noise, stream));
   } else {
     DZ_TRY(forward_heads_plain(l, learner_bufs(l), &pass, 1, 1, stream));
-    nq = c.num_quantiles;
   }
-  size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
-  DZ_LAUNCH(q_values_kernel, 1, 128, smem, stream, net_kind(c.kind), c.num_actions, c.num_atoms, nq, c.vmax, l->out[1], l->out[1], l->outv[1], d_q_out);
-  return DZ_OK;
+  return launch_q_values(c, 1, l->out[1], l->outv[1], nullptr, 0.f, d_q_out, nullptr, stream);
 }
 
 // Batched acting (parts.py:342-411 with many actors; dqn/agent.py:121-131,169-177): online forward on E <= batch observations
@@ -2813,23 +2840,17 @@ int act_batch_impl(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* 
   TorsoJob job{on, l->rows_act, 1};
   DZ_TRY(forward_torso(l, learner_bufs(l), &job, 1, E, stream));
   Pass pass{on, 1, 1, 0};
-  int nq = 1;
   if (uses_iqn_net(c.kind)) {
     if (!d_taus) return fail(DZ_EINVAL, "iqn act_batch needs taus[E][tau_samples_policy]");
     const float* taus[1] = {d_taus};
     DZ_TRY(forward_heads_iqn(l, learner_bufs(l), &pass, 1, E, taus, false, stream));
-    nq = c.tau_samples_policy;
   } else if (c.kind == DZ_RAINBOW) {
     if (!d_noise) return fail(DZ_EINVAL, "rainbow act_batch needs one apply of noise");
     DZ_TRY(forward_heads_rainbow(l, learner_bufs(l), &pass, 1, E, d_noise, stream, false, noise_ld));
   } else {
     DZ_TRY(forward_heads_plain(l, learner_bufs(l), &pass, 1, E, stream));
-    nq = c.num_quantiles;
   }
-  size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
-  DZ_LAUNCH(q_values_kernel, (unsigned)E, 128, smem, stream, net_kind(c.kind), c.num_actions, c.num_atoms, nq, c.vmax, l->out[1], l->out[1], l->outv[1], d_q_out);
-  DZ_LAUNCH(act_select_kernel, (unsigned)ceil_div(E, 128), 128, 0, stream, (const float*)d_q_out, c.num_actions, (int)E, d_explore, epsilon, d_actions);
-  return DZ_OK;
+  return launch_q_values(c, E, l->out[1], l->outv[1], d_explore, epsilon, d_q_out, d_actions, stream);
 }
 }  // namespace
 
@@ -3110,23 +3131,15 @@ int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const f
     DZ_TRY(forward_torso(l, a->b, &job, 1, E, stream));
   }
   Pass pass{on, 1, 1, 0};
-  int nq = 1;
   if (uses_iqn_net(c.kind)) {
     const float* taus[1] = {d_taus};
     DZ_TRY(forward_heads_iqn(l, a->b, &pass, 1, E, taus, false, stream));
-    nq = c.tau_samples_policy;
   } else if (rb) {
     DZ_TRY(forward_heads_rainbow(l, a->b, &pass, 1, E, d_noise, stream, fc_done, noise_ld));
   } else {
     DZ_TRY(forward_heads_plain(l, a->b, &pass, 1, E, stream, fc_done));
-    nq = c.num_quantiles;
   }
-  size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
-  DZ_LAUNCH(q_values_kernel, (unsigned)E, 128, smem, stream, net_kind(c.kind), c.num_actions, c.num_atoms, nq, c.vmax, a->b.out[1], a->b.out[1],
-            a->b.outv[1], d_q_out);
-  DZ_LAUNCH(act_select_kernel, (unsigned)ceil_div(E, 128), 128, 0, stream, (const float*)d_q_out, c.num_actions, E, d_explore, epsilon,
-            d_actions);
-  return DZ_OK;
+  return launch_q_values(c, E, a->b.out[1], a->b.outv[1], d_explore, epsilon, d_q_out, d_actions, stream);
 }
 
 // The actor's randomness from the learner's generator and counter: iqn taus [E][tau_samples_policy] (the stream id of
@@ -3290,6 +3303,46 @@ int dz_test_munchausen_iqn_example(const float* zbar_tm1, const float* zbar_t, i
   out[Nt] = bonus;
   out[Nt + 1] = ent;
   return DZ_OK;
+}
+
+// Test hook: the learner's loss section (launch_loss) on caller-owned head outputs, batch and output buffers, all on
+// `stream`.  The observation fields of cfg play no part; they are replaced by a legal geometry before validate().
+int dz_test_loss(const dz_learner_config* cfg, int32_t B, const float* const* d_out, const float* const* d_val,
+                 const int32_t* d_a_tm1, const float* d_r_t, const float* d_discount_t, const float* d_weights,
+                 const float* d_taus, float* d_dout, float* d_dval, float* d_per_example, float* d_priorities,
+                 float* d_loss_terms, float* d_loss, float* d_max_seen, void* stream) {
+  if (!cfg || !d_out) return fail(DZ_EINVAL, "test_loss: NULL argument");
+  dz_learner_config c = *cfg;
+  c.batch = B; c.obs_h = 84; c.obs_w = 84; c.obs_c = 4;
+  DZ_TRY(validate(c));
+  const bool rb = c.kind == DZ_RAINBOW;
+  if (!d_out[0] || !d_out[1] || !d_out[2] || (rb && (!d_val || !d_val[0] || !d_val[1] || !d_val[2] || !d_dval)))
+    return fail(DZ_EINVAL, "test_loss: head outputs of three passes are required (rainbow: and value streams)");
+  if (!d_a_tm1 || !d_r_t || !d_discount_t || !d_dout || !d_per_example || !d_loss_terms || !d_loss)
+    return fail(DZ_EINVAL, "test_loss: NULL buffer");
+  if (uses_iqn_net(c.kind) && !d_taus) return fail(DZ_EINVAL, "test_loss: iqn needs taus[B][tau_samples_s_tm1]");
+  if ((rb || c.kind == DZ_PRIORITIZED) && !d_priorities) return fail(DZ_EINVAL, "test_loss: this kind writes priorities");
+  LossArgs L;
+  memset(&L, 0, sizeof(L));
+  L.out0 = d_out[0]; L.out1 = d_out[1]; L.out2 = d_out[2];
+  L.adv0 = d_out[0]; L.adv1 = d_out[1]; L.adv2 = d_out[2];
+  if (rb) { L.val0 = d_val[0]; L.val1 = d_val[1]; L.val2 = d_val[2]; }
+  L.a = d_a_tm1; L.r = d_r_t; L.disc = d_discount_t; L.w = d_weights; L.taus0 = d_taus;
+  L.dout = d_dout; L.dadv = d_dout; L.dval = d_dval;
+  L.per_example = d_per_example; L.loss_terms = d_loss_terms; L.priorities = d_priorities;
+  return launch_loss(c, L, B, stream, nullptr, d_loss, d_max_seen, nullptr);
+}
+
+// Test hook: the acting tail (launch_q_values) on caller-owned head outputs of E observations.
+int dz_test_q_values(const dz_learner_config* cfg, int32_t E, const float* d_out, const float* d_val, const float* d_explore,
+                     float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
+  if (!cfg) return fail(DZ_EINVAL, "test_q_values: NULL config");
+  dz_learner_config c = *cfg;
+  c.obs_h = 84; c.obs_w = 84; c.obs_c = 4;
+  DZ_TRY(validate(c));
+  if (E < 1) return fail(DZ_EINVAL, "test_q_values: E must be >= 1");
+  if (!d_out || !d_q_out || (c.kind == DZ_RAINBOW && !d_val)) return fail(DZ_EINVAL, "test_q_values: NULL buffer");
+  return launch_q_values(c, E, d_out, d_val, d_explore, epsilon, d_q_out, d_actions, stream);
 }
 
 // Test hook: device pointer + element count of an internal activation / gradient buffer (tests and tools only).

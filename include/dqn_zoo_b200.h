@@ -326,6 +326,7 @@ typedef struct dz_learner_config {
   int32_t tau_samples_s_tm1, tau_samples_policy, tau_samples_s_t; /* iqn / munchausen_iqn: N, K, N' */
   int32_t batch;             /* 32 */
   int32_t obs_h, obs_w, obs_c; /* 84,84,4 */
+  /* loss hyperparameters, validated for every kind: finite, vmax > 0, grad_error_bound >= 0, huber_param >= 0 */
   float vmax;                /* c51 / rainbow support is linspace(-vmax, vmax, atoms) */
   float grad_error_bound;    /* dqn family: 1/32 (dqn/run_atari.py:79) */
   float huber_param;         /* qrdqn / iqn: 1.0 */
@@ -657,6 +658,26 @@ int dz_test_munchausen_example(const float* q_tm1, const float* qbar_tm1, const 
  * DZ_EINVAL for sizes or a_tm1 out of range and for the hyperparameters dz_learner_create rejects; tests only. */
 int dz_test_munchausen_iqn_example(const float* zbar_tm1, const float* zbar_t, int32_t A, int32_t K, int32_t Nt,
                                    int32_t a_tm1, float r_t, float discount_t, float alpha, float tau, float l0, float* out);
+/* The loss section of a learner step (the agent kind's loss kernel, then the scalar loss and rainbow's running max
+ * priority) on caller-owned device buffers, all enqueued on `stream`; tests only.  cfg is validated as
+ * dz_learner_create does, with batch = B and its observation fields replaced by a legal geometry.  d_out[p]: the head
+ * outputs of pass p (0 online(s_tm1); dqn: 2 target(s_t) is also the selector; double_q / prioritized: 1 online(s_t)
+ * selects; c51: [B][A][K] logits, 2 is target(s_t) and selects; rainbow: advantages [B][A][K] with d_val[p] the value
+ * streams [B][K], for online(s_tm1), online(s_t), target(s_t); qrdqn: [B][N][A]; iqn: [B][N_tm1 | N_policy | N_t][A];
+ * munchausen / munchausen_iqn: 1 is target(s_tm1)).  d_weights: importance weights [B] or NULL; d_taus: the s_tm1
+ * taus [B][N_tm1] (iqn, munchausen_iqn).  Writes d_dout (the gradient wrt pass 0; rainbow: advantages, with d_dval the
+ * value stream), d_per_example, d_priorities (prioritized, rainbow), d_loss_terms [B], d_loss [1] and, when d_max_seen
+ * is given for rainbow, the running max priority. */
+int dz_test_loss(const dz_learner_config* cfg, int32_t B, const float* const* d_out, const float* const* d_val,
+                 const int32_t* d_a_tm1, const float* d_r_t, const float* d_discount_t, const float* d_weights,
+                 const float* d_taus, float* d_dout, float* d_dval, float* d_per_example, float* d_priorities,
+                 float* d_loss_terms, float* d_loss, float* d_max_seen, void* stream);
+/* The acting tail of every acting entry point on caller-owned device buffers; tests only.  d_out: the head outputs of
+ * E observations in the layout of d_out[p] above (iqn: tau_samples_policy samples; rainbow: advantages, d_val the value
+ * streams).  Writes the q-values d_q_out [E][A] and, when d_actions is given, the epsilon-greedy actions as
+ * dz_learner_act_batch does (d_explore: [2][E] uniforms or NULL). */
+int dz_test_q_values(const dz_learner_config* cfg, int32_t E, const float* d_out, const float* d_val, const float* d_explore,
+                     float epsilon, float* d_q_out, int32_t* d_actions, void* stream);
 int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream);   /* device-to-device, tests only */
 /* Debug: the tensor-core launch named `tag` writes the clock stamps of its CTA 0 into d_trace (512 int64). */
 int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace);

@@ -145,6 +145,11 @@ def noise_shapes(spec):
 # ----------------------------------------------------------------------------
 
 
+def dueling(adv, val):
+  """`networks.py:251`: logits [B,A,K] of advantages [B,A,K] and values [B,K]."""
+  return val[:, None, :] + adv - adv.mean(dim=1, keepdim=True)
+
+
 def _conv(x, w, b, stride):
   """hk.Conv2D VALID, NHWC activations, HWIO weights (`networks.py:82-103`)."""
   y = F.conv2d(x.permute(0, 3, 1, 2), w.permute(3, 2, 0, 1), b, stride=stride)
@@ -204,10 +209,10 @@ def apply_net(spec, p, obs_u8, dtype, taus=None, noise=None, tap=None):
     adv = _noisy(p, 'adv2', adv, n['adv2/in'], n['adv2/out'], False).reshape(-1, a, k)
     val = _relu(_noisy(p, 'val1', feat, n['val1/in'], n['val1/out'], True), tap, 'val1')
     val = _noisy(p, 'val2', val, n['val2/in'], n['val2/out'], False).reshape(-1, 1, k)
-    logits = val + adv - adv.mean(dim=1, keepdim=True)          # `networks.py:251`
+    logits = dueling(adv, val[:, 0, :])
     support = support_atoms(spec, dtype)
     q = (F.softmax(logits, dim=-1) * support).sum(-1).detach()
-    return {'q_logits': logits, 'q_values': q}
+    return {'q_logits': logits, 'q_values': q, 'adv': adv, 'val': val[:, 0, :]}
   if kind == 'iqn':
     # `networks.py:264-292`
     latent = spec.latent_dim
@@ -302,69 +307,116 @@ def loss_fn(spec, online, target, batch, dtype, weights=None, taus=None, noise=N
   iqn `iqn/agent.py:178-214`."""
   kind = spec.kind
   s_tm1, s_t = batch['s_tm1'], batch['s_t']
-  a_tm1 = batch['a_tm1'].long()
-  r = batch['r_t'].to(torch.float32).to(dtype)
-  disc = batch['discount_t'].to(torch.float32).to(dtype)
-  rows = torch.arange(s_tm1.shape[0])
+  if kind in ('dqn', 'double_q', 'prioritized', 'c51', 'qrdqn'):
+    heads = [apply_net(spec, online, s_tm1, dtype, tap=tap), None, apply_net(spec, target, s_t, dtype)]
+    if kind in ('double_q', 'prioritized'):
+      heads[1] = apply_net(spec, online, s_t, dtype)
+  elif kind == 'rainbow':
+    nz = noise or [None, None, None]
+    heads = [apply_net(spec, online, s_tm1, dtype, noise=nz[0], tap=tap), apply_net(spec, online, s_t, dtype, noise=nz[1]),
+             apply_net(spec, target, s_t, dtype, noise=nz[2])]
+  elif kind == 'iqn':
+    heads = [apply_net(spec, online, s_tm1, dtype, taus=taus[0], tap=tap), apply_net(spec, target, s_t, dtype, taus=taus[1]),
+             apply_net(spec, target, s_t, dtype, taus=taus[2])]
+  else:
+    raise ValueError(kind)
+  field = {'c51': 'q_logits', 'qrdqn': 'q_dist', 'iqn': 'q_dist'}.get(kind, 'q_values')
+  if kind == 'rainbow':
+    heads = [(h['adv'], h['val']) for h in heads]
+  else:
+    heads = [None if h is None else h[field] for h in heads]
+  loss, aux = head_loss(kind, heads, batch['a_tm1'], batch['r_t'], batch['discount_t'], weights,
+                        None if taus is None else taus[0], vmax=spec.vmax, grad_error_bound=grad_error_bound,
+                        huber_param=huber_param, grad=False)
+  return loss, aux
+
+
+def head_loss(kind, heads, a_tm1, r_t, discount_t, weights=None, taus=None, *, vmax=10.0, grad_error_bound=1.0 / 32,
+              huber_param=1.0, grad=True):
+  """The loss of each agent from its head outputs: everything `loss_fn` does after the network applies.
+
+  heads: the three passes (online(s_tm1), selector, target(s_t)) in `dtype`, as the device lays them out:
+    dqn [B,A] with heads[1] unused (None); double_q / prioritized [B,A], heads[1] online(s_t);
+    c51 [B,A,K] logits, heads[1] unused (the target pass selects); rainbow (adv [B,A,K], val [B,K]) per pass,
+    heads[1] online(s_t); qrdqn [B,N,A], heads[1] unused; iqn [B,N,A] at (tau_tm1, tau_policy, tau_t).
+  taus: iqn's s_tm1 taus [B,N].  r_t / discount_t / weights are rounded to float32 first, as the reference feeds float32.
+  Returns (scalar loss, aux): aux 'losses' [B], 'per_example' (td for the dqn family, the loss otherwise),
+  'priorities' (prioritized |td|, rainbow clip(|loss|, 0, 100)), 'a_star' (the selected action; dqn: argmax of the
+  target pass) and, with grad=True, 'grad': the gradient of the loss wrt the pass-0 head outputs (rainbow: a tuple
+  (d adv, d val)), by autograd.  grad=False leaves the pass-0 tensors in the caller's graph (loss_fn)."""
+  dtype = (heads[0][0] if kind == 'rainbow' else heads[0]).dtype
+  a_tm1 = torch.as_tensor(a_tm1).long()
+  r = torch.as_tensor(r_t).to(torch.float32).to(dtype)
+  disc = torch.as_tensor(discount_t).to(torch.float32).to(dtype)
+  pass0 = list(heads[0]) if kind == 'rainbow' else [heads[0]]
+  if grad:
+    pass0 = [x.detach().clone().requires_grad_(True) for x in pass0]
+  rows = torch.arange(a_tm1.shape[0])
   aux = {}
   if kind in ('dqn', 'double_q', 'prioritized'):
-    q_tm1 = apply_net(spec, online, s_tm1, dtype, tap=tap)['q_values']
-    q_target = apply_net(spec, target, s_t, dtype)['q_values'].detach()
-    if kind == 'dqn':
-      boot = q_target.max(dim=1).values
-    else:
-      sel = apply_net(spec, online, s_t, dtype)['q_values'].detach()
-      boot = q_target[rows, sel.argmax(dim=1)]
+    q_tm1 = pass0[0]
+    q_target = heads[2].detach()
+    sel = q_target if kind == 'dqn' else heads[1].detach()
+    a_star = sel.argmax(dim=1)                 # first maximum, as jnp.argmax
+    boot = q_target.max(dim=1).values if kind == 'dqn' else q_target[rows, a_star]
     td = (r + disc * boot).detach() - q_tm1[rows, a_tm1]
     aux['td_errors'] = td.detach()
     td_c = _ClipGrad.apply(td, -grad_error_bound, grad_error_bound)
     losses = 0.5 * td_c * td_c
     aux['q_tm1'] = q_tm1.detach()
   elif kind in ('c51', 'rainbow'):
-    k = spec.num_atoms
-    support = support_atoms(spec, dtype)
-    nz = noise or [None, None, None]
     if kind == 'rainbow':
-      out_tm1 = apply_net(spec, online, s_tm1, dtype, noise=nz[0], tap=tap)
-      sel_q = apply_net(spec, online, s_t, dtype, noise=nz[1])['q_values'].detach()
-      tgt = apply_net(spec, target, s_t, dtype, noise=nz[2])
+      logits_tm1 = dueling(*pass0)
+      sel_logits = dueling(*[x.detach() for x in heads[1]])
+      tgt_logits = dueling(*[x.detach() for x in heads[2]])
     else:
-      out_tm1 = apply_net(spec, online, s_tm1, dtype, tap=tap)
-      tgt = apply_net(spec, target, s_t, dtype)
-      sel_q = tgt['q_values'].detach()
+      logits_tm1, tgt_logits = pass0[0], heads[2].detach()
+      sel_logits = tgt_logits
+    support = torch.tensor(np.linspace(-vmax, vmax, logits_tm1.shape[-1]).astype(np.float32)).to(dtype)
+    sel_q = (F.softmax(sel_logits, dim=-1) * support).sum(-1)
     a_star = sel_q.argmax(dim=1)
-    p_target = F.softmax(tgt['q_logits'].detach()[rows, a_star], dim=-1)
+    p_target = F.softmax(tgt_logits[rows, a_star], dim=-1)
     target_z = r[:, None] + disc[:, None] * support[None, :]
     proj = categorical_l2_project(target_z, p_target, support).detach()
-    logit_qa = out_tm1['q_logits'][rows, a_tm1]
+    logit_qa = logits_tm1[rows, a_tm1]
     losses = -(proj * F.log_softmax(logit_qa, dim=-1)).sum(-1)
-    aux['logits_tm1'] = out_tm1['q_logits'].detach()
+    aux['logits_tm1'] = logits_tm1.detach()
     aux['target_probs'] = proj
-  elif kind == 'qrdqn':
-    n = spec.num_quantiles
-    quantiles = ((torch.arange(0, n, dtype=torch.float32) + 0.5) / float(n)).to(dtype)   # `qrdqn/run_atari.py:136-137`
-    dist_tm1 = apply_net(spec, online, s_tm1, dtype, tap=tap)['q_dist']
-    dist_t = apply_net(spec, target, s_t, dtype)['q_dist'].detach()
-    a_star = dist_t.mean(dim=1).argmax(dim=1)
+    aux['p_target'] = p_target
+  elif kind in ('qrdqn', 'iqn'):
+    dist_tm1, dist_t = pass0[0], heads[2].detach()
+    if kind == 'qrdqn':
+      n = dist_tm1.shape[1]
+      tau_src = ((torch.arange(0, n, dtype=torch.float32) + 0.5) / float(n)).to(dtype)   # `qrdqn/run_atari.py:136-137`
+      sel = dist_t
+    else:
+      tau_src = torch.as_tensor(taus).to(dtype)
+      sel = heads[1].detach()
+    a_star = sel.mean(dim=1).argmax(dim=1)
     tgt = (r[:, None] + disc[:, None] * dist_t[rows, :, a_star]).detach()
-    losses = quantile_regression_loss(dist_tm1[rows, :, a_tm1], quantiles, tgt, huber_param)
+    losses = quantile_regression_loss(dist_tm1[rows, :, a_tm1], tau_src, tgt, huber_param)
     aux['dist_tm1'] = dist_tm1.detach()
-  elif kind == 'iqn':
-    tau_tm1, tau_sel, tau_t = taus
-    dist_tm1 = apply_net(spec, online, s_tm1, dtype, taus=tau_tm1, tap=tap)['q_dist']
-    dist_sel = apply_net(spec, target, s_t, dtype, taus=tau_sel)['q_dist'].detach()
-    dist_t = apply_net(spec, target, s_t, dtype, taus=tau_t)['q_dist'].detach()
-    a_star = dist_sel.mean(dim=1).argmax(dim=1)
-    tgt = (r[:, None] + disc[:, None] * dist_t[rows, :, a_star]).detach()
-    losses = quantile_regression_loss(dist_tm1[rows, :, a_tm1], tau_tm1.to(dtype), tgt, huber_param)
-    aux['dist_tm1'] = dist_tm1.detach()
+    aux['targets'] = tgt
   else:
     raise ValueError(kind)
+  return _finish(kind, losses, weights, pass0, grad, dict(aux, a_star=a_star))
+
+
+def _finish(kind, losses, weights, pass0, grad, aux):
+  """The weighted mean, the per-example values and priorities of `head_loss` and, with grad, its pass-0 gradient."""
+  dtype = losses.dtype
   aux['losses'] = losses.detach()
-  if weights is not None:
-    loss = (losses * weights.to(torch.float32).to(dtype)).mean()
-  else:
-    loss = losses.mean()
+  w = None if weights is None else torch.as_tensor(weights).to(torch.float32).to(dtype)
+  loss = losses.mean() if w is None else (losses * w).mean()
+  aux['per_example'] = aux['td_errors'] if kind in ('dqn', 'double_q', 'prioritized') else aux['losses']
+  if kind == 'rainbow':
+    aux['priorities'] = aux['losses'].abs().clamp(0.0, 100.0)       # `rainbow/agent.py:194`
+  elif kind == 'prioritized':
+    aux['priorities'] = aux['td_errors'].abs()                       # `prioritized/agent.py:201`
+  if grad:
+    g = torch.autograd.grad(loss, pass0, allow_unused=True)
+    g = [torch.zeros_like(x) if gi is None else gi for x, gi in zip(pass0, g)]
+    aux['grad'] = tuple(g) if kind == 'rainbow' else g[0]
   return loss, aux
 
 
@@ -442,16 +494,18 @@ def optimizer_step(opt, params, grads, state):
 class Learner:
   """Holds params/opt-state as torch tensors in `dtype`; `update()` is one jit(update)."""
 
-  def __init__(self, spec, params_np, opt=None, dtype=torch.float64):
+  def __init__(self, spec, params_np, opt=None, dtype=torch.float64, grad_error_bound=1.0 / 32, huber_param=1.0):
     self.spec, self.dtype = spec, dtype
     self.opt = opt or default_opt(spec.kind)
+    self.grad_error_bound, self.huber_param = grad_error_bound, huber_param
     self.online = {k: torch.tensor(v, dtype=dtype) for k, v in params_np.items()}
     self.target = {k: v.clone() for k, v in self.online.items()}
     self.state = init_opt_state(self.opt, self.online)
 
   def grads(self, batch, weights=None, taus=None, noise=None, tap=None):
     p = {k: v.clone().requires_grad_(True) for k, v in self.online.items()}
-    loss, aux = loss_fn(self.spec, p, self.target, batch, self.dtype, weights, taus, noise, tap=tap)
+    loss, aux = loss_fn(self.spec, p, self.target, batch, self.dtype, weights, taus, noise,
+                        grad_error_bound=self.grad_error_bound, huber_param=self.huber_param, tap=tap)
     loss.backward()
     g = {k: (v.grad if v.grad is not None else torch.zeros_like(v)) for k, v in p.items()}
     return loss.detach(), aux, g

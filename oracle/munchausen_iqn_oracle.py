@@ -87,18 +87,34 @@ def loss_fn(spec, online, target_params, batch, dtype, taus, weights=None, huber
   a_tm1 = batch['a_tm1'].long()
   r = batch['r_t'].to(torch.float32).to(dtype)
   disc = batch['discount_t'].to(torch.float32).to(dtype)
-  rows = torch.arange(s_tm1.shape[0])
   tau_tm1, tau_pol, tau_t = taus
   dist_tm1 = apply_net(spec, online, s_tm1, dtype, tau_tm1, tap=tap)['q_dist']
   zbar_tm1 = apply_net(spec, target_params, s_tm1, dtype, tau_pol)['q_dist'].detach()
   zbar_t = apply_net(spec, target_params, s_t, dtype, tau_t)['q_dist'].detach()
+  return head_loss((dist_tm1, zbar_tm1, zbar_t), a_tm1, r, disc, tau_tm1, weights, huber_param=huber_param, hyper=hyper,
+                   grad=False)
+
+
+def head_loss(heads, a_tm1, r_t, discount_t, taus, weights=None, *, huber_param=1.0, hyper=Hyper(), grad=True):
+  """learner_oracle.head_loss for this agent: heads = (online(s_tm1) [B, N, A], target(s_tm1) at the policy taus
+  [B, K, A], target(s_t) [B, N', A]); taus: the s_tm1 taus [B, N].  aux 'per_example' is the loss."""
+  dist_tm1 = heads[0].detach().clone().requires_grad_(True) if grad else heads[0]
+  dtype = dist_tm1.dtype
+  a_tm1 = torch.as_tensor(a_tm1).long()
+  r = torch.as_tensor(r_t).to(torch.float32).to(dtype)
+  disc = torch.as_tensor(discount_t).to(torch.float32).to(dtype)
+  rows = torch.arange(a_tm1.shape[0])
+  zbar_tm1, zbar_t = heads[1].detach(), heads[2].detach()
   y, bonus, ent = target(zbar_tm1, zbar_t, a_tm1, r, disc, hyper)
-  losses = lo.quantile_regression_loss(dist_tm1[rows, :, a_tm1], tau_tm1.to(dtype), y.detach(), huber_param)
+  losses = lo.quantile_regression_loss(dist_tm1[rows, :, a_tm1], torch.as_tensor(taus).to(dtype), y.detach(), huber_param)
   aux = {'losses': losses.detach(), 'targets': y.detach(), 'bonus': bonus.detach(), 'entropy': ent.detach(),
          'dist_tm1': dist_tm1.detach(), 'qbar_tm1': zbar_tm1.mean(dim=1), 'qbar_t': zbar_t.mean(dim=1)}
-  if weights is not None:
-    return (losses * weights.to(torch.float32).to(dtype)).mean(), aux
-  return losses.mean(), aux
+  w = None if weights is None else torch.as_tensor(weights).to(torch.float32).to(dtype)
+  loss = losses.mean() if w is None else (losses * w).mean()
+  aux['per_example'] = aux['losses']
+  if grad:
+    aux['grad'] = torch.autograd.grad(loss, dist_tm1)[0]
+  return loss, aux
 
 
 class Learner(lo.Learner):

@@ -80,19 +80,35 @@ def loss_fn(spec, online, target_params, batch, dtype, weights=None, grad_error_
   a_tm1 = batch['a_tm1'].long()
   r = batch['r_t'].to(torch.float32).to(dtype)
   disc = batch['discount_t'].to(torch.float32).to(dtype)
-  rows = torch.arange(s_tm1.shape[0])
   q_tm1 = apply_net(spec, online, s_tm1, dtype, tap=tap)['q_values']
   qbar_tm1 = apply_net(spec, target_params, s_tm1, dtype)['q_values'].detach()
   qbar_t = apply_net(spec, target_params, s_t, dtype)['q_values'].detach()
+  return head_loss((q_tm1, qbar_tm1, qbar_t), a_tm1, r, disc, weights, grad_error_bound=grad_error_bound, hyper=hyper,
+                   grad=False)
+
+
+def head_loss(heads, a_tm1, r_t, discount_t, weights=None, *, grad_error_bound=1.0 / 32, hyper=Hyper(), grad=True):
+  """learner_oracle.head_loss for this agent: heads = (online(s_tm1), target(s_tm1), target(s_t)), each [B, A].
+  aux 'per_example' is the loss 0.5 td^2, as the device writes it."""
+  q_tm1 = heads[0].detach().clone().requires_grad_(True) if grad else heads[0]
+  dtype = q_tm1.dtype
+  a_tm1 = torch.as_tensor(a_tm1).long()
+  r = torch.as_tensor(r_t).to(torch.float32).to(dtype)
+  disc = torch.as_tensor(discount_t).to(torch.float32).to(dtype)
+  rows = torch.arange(a_tm1.shape[0])
+  qbar_tm1, qbar_t = heads[1].detach(), heads[2].detach()
   tgt, bonus = target(qbar_tm1, qbar_t, a_tm1, r, disc, hyper)
   td = tgt.detach() - q_tm1[rows, a_tm1]
   td_c = lo._ClipGrad.apply(td, -grad_error_bound, grad_error_bound)
   losses = 0.5 * td_c * td_c
   aux = {'losses': losses.detach(), 'td_errors': td.detach(), 'q_tm1': q_tm1.detach(), 'targets': tgt.detach(),
          'bonus': bonus.detach(), 'qbar_tm1': qbar_tm1, 'qbar_t': qbar_t}
-  if weights is not None:
-    return (losses * weights.to(torch.float32).to(dtype)).mean(), aux
-  return losses.mean(), aux
+  w = None if weights is None else torch.as_tensor(weights).to(torch.float32).to(dtype)
+  loss = losses.mean() if w is None else (losses * w).mean()
+  aux['per_example'] = aux['losses']
+  if grad:
+    aux['grad'] = torch.autograd.grad(loss, q_tm1)[0]
+  return loss, aux
 
 
 class Learner(lo.Learner):

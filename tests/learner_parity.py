@@ -20,9 +20,11 @@ def _hw(hw):
   return (hw, hw) if isinstance(hw, int) else tuple(hw)
 
 
-def make_case(kind, B, hw, seed, num_actions=6, num_atoms=None, num_quantiles=None, latent_dim=64, taus=None):
+def make_case(kind, B, hw, seed, num_actions=6, num_atoms=None, num_quantiles=None, latent_dim=64, taus=None, vmax=10.0,
+              grad_error_bound=1.0 / 32, huber_param=1.0):
   """hw: side of a square observation, or (H, W).  taus: (s_tm1, policy, s_t) sample counts of IQN.  Unset head sizes
-  and tau counts take the full-size values at 84x84 and small ones elsewhere."""
+  and tau counts take the full-size values at 84x84 and small ones elsewhere.  vmax, grad_error_bound and huber_param
+  go to both the device learner and the oracle."""
   from dqn_zoo_b200 import learner as dl
   H, W = _hw(hw)
   full = (H, W) == (84, 84)
@@ -34,15 +36,15 @@ def make_case(kind, B, hw, seed, num_actions=6, num_atoms=None, num_quantiles=No
     heads['num_quantiles'] = num_quantiles
   if taus is None:
     taus = (64, 64, 64) if full else (8, 5, 7)
-  spec = lo.NetSpec(kind, num_actions, obs_hw=H, obs_w=W, **heads)
+  spec = lo.NetSpec(kind, num_actions, obs_hw=H, obs_w=W, vmax=vmax, **heads)
   net = dl.NetworkSpec(kind, num_actions, obs_shape=(H, W, 4), tau_samples_s_tm1=taus[0], tau_samples_policy=taus[1],
-                       tau_samples_s_t=taus[2], **heads)
+                       tau_samples_s_t=taus[2], vmax=vmax, **heads)
   online = lo.init_params(spec, seed)
   target = lo.init_params(spec, seed + 1)
-  L = dl.Learner(net, batch_size=B)
+  L = dl.Learner(net, batch_size=B, grad_error_bound=grad_error_bound, huber_param=huber_param)
   L.set_params(online)
   L.set_params(target, blob='target')
-  O = lo.Learner(spec, online, dtype=torch.float64)
+  O = lo.Learner(spec, online, dtype=torch.float64, grad_error_bound=grad_error_bound, huber_param=huber_param)
   O.target = {k: torch.tensor(v, dtype=torch.float64) for k, v in target.items()}
   return spec, net, L, O, rs
 

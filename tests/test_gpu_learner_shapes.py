@@ -90,6 +90,25 @@ def test_head_widths(kind, case, B):
   check(kind, 44, B, True, **case)
 
 
+# ---- loss hyperparameters other than the defaults ----------------------------------------------------------------------
+# vmax, grad_error_bound and huber_param travel from the learner's configuration to the loss kernels; a value dropped or
+# hard-coded on the way runs the default (10, 1/32, 1) and fails these bars.
+
+@pytest.mark.parametrize('kind,case', [
+    ('c51', dict(vmax=3.0)), ('c51', dict(vmax=50.0)), ('rainbow', dict(vmax=3.0)), ('rainbow', dict(vmax=50.0)),
+    ('qrdqn', dict(huber_param=0.0)), ('qrdqn', dict(huber_param=3.0)),
+    ('iqn', dict(huber_param=0.0)), ('iqn', dict(huber_param=3.0)),
+    ('dqn', dict(grad_error_bound=1.0)), ('dqn', dict(grad_error_bound=1.0 / 1024)),
+    ('prioritized', dict(grad_error_bound=1.0)), ('prioritized', dict(grad_error_bound=1.0 / 1024)),
+], ids=lambda x: '-'.join('%s%g' % kv for kv in x.items()) if isinstance(x, dict) else x)
+def test_non_default_loss_hyperparameters(kind, case):
+  check(kind, 44, 32, True, **case)
+
+
+def test_three_optimizer_steps_with_a_non_default_support():
+  check_three_optimizer_steps('c51', 44, 32, vmax=3.0)
+
+
 # ---- optimizer steps -------------------------------------------------------------------------------------------------
 
 @pytest.mark.parametrize('hw,B', [(84, 64), ((84, 92), 32)])

@@ -101,6 +101,34 @@ def test_c_abi_library_exports_every_declared_symbol():
     _lib.call('dz_learner_plan_query', ctypes.byref(cfg), ctypes.byref(plan))
 
 
+def test_loss_hyperparameters_are_validated_for_every_kind():
+  """vmax, grad_error_bound and huber_param reach the loss kernels as given: non-finite values, vmax <= 0 and a
+  negative bound or Huber width are refused by validate() (here through dz_learner_plan_query, which does no device
+  work), for every kind; the defaults and the boundary values 0 of the bound and the width pass."""
+  from dqn_zoo_b200 import _lib
+  plan = _lib.LearnerPlan()
+
+  def cfg(kind, **fields):
+    c = _lib.LearnerConfig(**fields)
+    c.kind = _lib.AGENT_KINDS[kind]
+    c.num_actions, c.num_atoms, c.num_quantiles, c.latent_dim = 6, 51, 201, 64
+    c.tau_samples_s_tm1 = c.tau_samples_policy = c.tau_samples_s_t = 64
+    c.batch, c.obs_h, c.obs_w, c.obs_c = 32, 84, 84, 4
+    c.munchausen_alpha, c.entropy_temperature, c.log_policy_clip = 0.9, 0.03, -1.0
+    return c
+
+  nan, inf = float('nan'), float('inf')
+  bad = [('vmax', 0.0), ('vmax', -1.0), ('vmax', nan), ('vmax', inf), ('huber_param', -1e-3), ('huber_param', nan),
+         ('huber_param', inf), ('grad_error_bound', -1.0 / 32), ('grad_error_bound', nan), ('grad_error_bound', -inf)]
+  for kind in _lib.AGENT_KINDS:
+    _lib.call('dz_learner_plan_query', ctypes.byref(cfg(kind)), ctypes.byref(plan))
+    _lib.call('dz_learner_plan_query', ctypes.byref(cfg(kind, grad_error_bound=0.0, huber_param=0.0, vmax=1e-3)),
+              ctypes.byref(plan))
+    for field, value in bad:
+      with pytest.raises(ValueError, match=field):
+        _lib.call('dz_learner_plan_query', ctypes.byref(cfg(kind, **{field: value})), ctypes.byref(plan))
+
+
 def test_parameter_layout_matches_the_oracle_shapes():
   from dqn_zoo_b200 import _lib
   from oracle import learner_oracle as lo

@@ -205,6 +205,61 @@ def test_noisy_linear_and_dueling_hand_vectors(hand):
   np.testing.assert_allclose(logits, duel['expected'], rtol=0, atol=1e-15)
 
 
+def test_autograd_conventions_at_the_kinks_are_jaxs():
+  """The GPU loss-kernel tests compare against head_loss's autograd exactly at the kinks, so its conventions there are
+  pinned here, each against the JAX rule it restates."""
+  # abs'(0) = sign(0) = 0 (jax.lax.abs_p's jvp multiplies by sign(x)).
+  x = torch.zeros(1, dtype=torch.float64, requires_grad=True)
+  x.abs().sum().backward()
+  assert float(x.grad) == 0.0
+  # rlax.huber_loss at |x| = k: jnp.minimum's tie sends half the cotangent to each operand, so
+  # d/dx [0.5 q^2 + k (|x| - q)] = 0.5 (k * 1) + k (1 - 0.5) = k; torch.clamp(max=k) passes all of it through q
+  # (d/dx = k * 1 + k * (1 - 1) = k): both give k, and the device's clamp(delta, -k, k) gives k too.
+  for k in (0.5, 1.0, 3.0):
+    for sgn in (1.0, -1.0):
+      x = torch.tensor([sgn * k], dtype=torch.float64, requires_grad=True)
+      lo.huber(x, k).sum().backward()
+      assert float(x.grad) == sgn * k, (k, sgn)
+  # quantile_regression_loss at delta = 0: the weight's 1[delta < 0] is 0 (tau, not 1 - tau) and the Huber slope is 0,
+  # so a source quantile equal to its target contributes neither loss nor gradient, at k > 0 and at k = 0.
+  for k in (0.0, 1.0):
+    src = torch.tensor([[0.5]], dtype=torch.float64, requires_grad=True)
+    loss = lo.quantile_regression_loss(src, torch.tensor([0.25], dtype=torch.float64), torch.tensor([[0.5]], dtype=torch.float64), k)
+    loss.sum().backward()
+    assert float(loss.detach()) == 0.0 and float(src.grad) == 0.0
+  # jnp.argmax and torch.argmax both return the first maximum.
+  assert int(torch.tensor([1.0, 3.0, 3.0, 2.0]).argmax()) == 1
+  assert int(torch.tensor([[0.0, 0.0]]).argmax(dim=1)) == 0
+  # rlax.clip_gradient at exactly the bound: the clipped cotangent is the bound itself.
+  x = torch.tensor([2.0], dtype=torch.float64, requires_grad=True)
+  (lo._ClipGrad.apply(x, -0.25, 0.25) * 0.25).sum().backward()
+  assert float(x.grad) == 0.25
+
+
+def test_head_loss_is_loss_fn_after_the_networks():
+  """head_loss on the head outputs loss_fn's networks produce gives loss_fn's loss, and its pass-0 gradient is the
+  autograd gradient of that loss wrt those outputs, for every reference kind (rainbow: advantages and values)."""
+  for kind in lo.AGENT_KINDS:
+    spec, online, target, batch, w, taus, noise = tiny_case(kind)
+    on = {k: torch.tensor(v, dtype=torch.float64) for k, v in online.items()}
+    tg = {k: torch.tensor(v, dtype=torch.float64) for k, v in target.items()}
+    loss, aux = lo.loss_fn(spec, on, tg, batch, torch.float64, w, taus, noise, grad_error_bound=0.05, huber_param=0.5)
+    nz = noise or [None] * 3
+    tau3 = taus or [None] * 3
+    nets = [(on, batch['s_tm1']), (on if kind in ('double_q', 'prioritized', 'rainbow') else tg, batch['s_t']),
+            (tg, batch['s_t'])]
+    outs = [lo.apply_net(spec, p, s, torch.float64, taus=tau3[i], noise=nz[i]) for i, (p, s) in enumerate(nets)]
+    field = {'c51': 'q_logits', 'qrdqn': 'q_dist', 'iqn': 'q_dist'}.get(kind, 'q_values')
+    heads = [(o['adv'], o['val']) if kind == 'rainbow' else o[field] for o in outs]
+    hl, haux = lo.head_loss(kind, heads, batch['a_tm1'], batch['r_t'], batch['discount_t'], w, tau3[0], vmax=spec.vmax,
+                            grad_error_bound=0.05, huber_param=0.5)
+    assert float(hl.detach()) == float(loss.detach()), kind
+    np.testing.assert_array_equal(haux['losses'].numpy(), aux['losses'].numpy())
+    grads = haux['grad'] if kind == 'rainbow' else (haux['grad'],)
+    assert [g.shape for g in grads] == [x.shape for x in (heads[0] if kind == 'rainbow' else (heads[0],))]
+    assert float(sum(g.abs().sum() for g in grads)) > 0 and haux['per_example'].shape == (3,)
+
+
 def test_device_loss_formulas_are_the_hand_vectors_formulas(hand):
   """The same vectors again through `loss_fn`-level code paths of the oracle that the CUDA kernels are compared with:
   a 3-atom C51 head reduced to the projection + cross entropy above."""
