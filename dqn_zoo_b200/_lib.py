@@ -16,7 +16,7 @@ DZ_FLAG_BAD_VALUE, DZ_FLAG_BAD_INDEX, DZ_FLAG_BAD_TARGET, DZ_FLAG_ROOT_ZERO, DZ_
 DZ_FLAG_FRAME_POOL_FULL = 32
 DZ_CKPT_BAD_PLANE_ID, DZ_CKPT_UNREFERENCED_PLANE, DZ_CKPT_HASH_MISMATCH, DZ_CKPT_BAD_FREE_STACK = 1, 2, 4, 8
 AGENT_KINDS = {'dqn': 0, 'double_q': 1, 'prioritized': 2, 'c51': 3, 'qrdqn': 4, 'rainbow': 5, 'iqn': 6, 'munchausen': 7,
-               'munchausen_iqn': 8}
+               'munchausen_iqn': 8, 'fqf': 9}
 OPTIMIZERS = {'adam': 0, 'rmsprop': 1}
 
 
@@ -58,11 +58,14 @@ class LearnerConfig(C.Structure):
               ('obs_h', i32), ('obs_w', i32), ('obs_c', i32), ('vmax', f32), ('grad_error_bound', f32),
               ('huber_param', f32), ('optimizer', i32), ('learning_rate', f32), ('opt_eps', f32), ('rms_decay', f32),
               ('adam_b1', f32), ('adam_b2', f32), ('max_global_grad_norm', f32), ('munchausen_alpha', f32),
-              ('entropy_temperature', f32), ('log_policy_clip', f32)]
+              ('entropy_temperature', f32), ('log_policy_clip', f32), ('num_fractions', i32),
+              ('fraction_learning_rate', f32), ('fraction_opt_eps', f32), ('fraction_rms_decay', f32)]
 
   def __init__(self, **fields):
-    # the loss hyperparameters start at the reference's values instead of 0, which the library rejects for vmax
-    super().__init__(**dict(dict(vmax=10.0, grad_error_bound=1.0 / 32, huber_param=1.0), **fields))
+    # the loss hyperparameters start at the reference's values instead of 0, which the library rejects for vmax, and
+    # fqf's fraction fields at its defaults (DESIGN.md §15), which the library rejects at 0 for that kind
+    super().__init__(**dict(dict(vmax=10.0, grad_error_bound=1.0 / 32, huber_param=1.0, num_fractions=32,
+                                 fraction_learning_rate=2.5e-9, fraction_opt_eps=1e-5, fraction_rms_decay=0.95), **fields))
 
 
 class LearnerPlan(C.Structure):
@@ -204,6 +207,7 @@ _SIGNATURES = {
     'dz_test_learner_buffer': (i32, [vp, C.c_char_p, vp, vp]),
     'dz_test_munchausen_example': (i32, [vp, vp, vp, i32, i32, f32, f32, f32, f32, f32, vp]),
     'dz_test_munchausen_iqn_example': (i32, [vp, vp, i32, i32, i32, i32, f32, f32, f32, f32, f32, vp]),
+    'dz_test_fqf_example': (i32, [vp, vp, vp, i32, f32, vp]),
     'dz_test_loss': (i32, [C.POINTER(LearnerConfig), i32, C.POINTER(vp), C.POINTER(vp), vp, vp, vp, vp, vp, vp, vp, vp, vp,
                            vp, vp, vp, vp]),
     'dz_test_q_values': (i32, [C.POINTER(LearnerConfig), i32, vp, vp, vp, f32, vp, vp, vp]),

@@ -37,6 +37,21 @@ from dqn_zoo_b200 import replay as replay_lib
 NetworkSpec = learner_lib.NetworkSpec
 OptimizerSpec = learner_lib.OptimizerSpec
 _iqn_net = learner_lib.uses_iqn_network
+_draws_taus = learner_lib.draws_taus
+
+
+def _acting_rows_error(net, E):
+  """The acting context's row limit of IQN's network (E x its rows per observation <= ACTOR_MAX_IQN_ROWS) as a
+  message, or None within it: iqn / munchausen_iqn act on tau_samples_policy rows, fqf on its num_fractions."""
+  if not _iqn_net(net.kind):
+    return None
+  if _draws_taus(net.kind):
+    if E * net.tau_samples_policy > ACTOR_MAX_IQN_ROWS:
+      return 'iqn acting needs num_streams * tau_samples_policy <= %d, got %d * %d' % (ACTOR_MAX_IQN_ROWS, E,
+                                                                                       net.tau_samples_policy)
+  elif E * net.num_fractions > ACTOR_MAX_IQN_ROWS:
+    return 'fqf acting needs num_streams * num_fractions <= %d, got %d * %d' % (ACTOR_MAX_IQN_ROWS, E, net.num_fractions)
+  return None
 
 
 def _seed_of(rng_key) -> int:
@@ -280,9 +295,9 @@ class _DeviceAgent(parts.Agent):
       self._jax_act.set_keys(sample)
       self._jax_act.launch(L.taus)
       taus = L.taus
-    elif _iqn_net(self.KIND) or self.KIND == 'rainbow':
+    elif _draws_taus(self.KIND) or self.KIND == 'rainbow':
       L.generate_randomness(self._seed)
-      taus = L.taus if _iqn_net(self.KIND) else None
+      taus = L.taus if _draws_taus(self.KIND) else None
       noise = L.noise if self.KIND == 'rainbow' else None
     q = L.q_values(self._obs_dev, taus=taus, noise=noise).cpu().numpy()   # D2H sync, as jax.device_get
     eps = 0.0 if self.GREEDY else self.exploration_epsilon
@@ -385,7 +400,7 @@ class _DeviceAgent(parts.Agent):
     L = self._learner
     if getattr(self, '_jax_key', None) is not None:
       self._jax_learn.launch(L.taus)            # jax.random.uniform draws from the keys staged by _learn()
-    elif _iqn_net(self.KIND) or self.KIND == 'rainbow':
+    elif _draws_taus(self.KIND) or self.KIND == 'rainbow':
       L.generate_randomness(self._seed, beside_sampler=True)
     L.learn(self._view, self.PRIORITIZED, self._io)
 
@@ -562,6 +577,27 @@ class MunchausenIqn(_DeviceAgent):
                 entropy_temperature=entropy_temperature, log_policy_clip=log_policy_clip)
 
 
+class Fqf(_DeviceAgent):
+  """FQF, the Fully parameterized Quantile Function (Yang et al., NeurIPS 2019; DESIGN.md §15): Iqn's constructor without
+  the tau sample counts and `jax_prng_taus` (its taus are not drawn: a fraction proposal layer computes N fractions from
+  the torso features inside every step and every action selection), plus `num_fractions` (which must match the
+  NetworkSpec's) and the fraction layer's centred RMSProp (`fraction_learning_rate`, `fraction_opt_eps`,
+  `fraction_rms_decay`).  `optimizer` covers every other tensor (default: Adam at lr 5e-5, eps 0.01 / 32).  Uniform
+  replay and epsilon-greedy acting on Q(s, a) = sum_i w_i Z(s, a, tau_hat_i)."""
+  KIND = 'fqf'
+
+  def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
+               batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
+               target_network_update_period, huber_param, rng_key, use_cuda_graph=True, num_fractions=32,
+               fraction_learning_rate=2.5e-9, fraction_opt_eps=1e-5, fraction_rms_decay=0.95):
+    if network.num_fractions != num_fractions:
+      raise ValueError('num_fractions must match the NetworkSpec')
+    self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
+                exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
+                huber_param=huber_param, use_cuda_graph=use_cuda_graph, fraction_learning_rate=fraction_learning_rate,
+                fraction_opt_eps=fraction_opt_eps, fraction_rms_decay=fraction_rms_decay)
+
+
 def _check_support(support, network):
   s = np.asarray(support, dtype=np.float64)
   want = np.linspace(-network.vmax, network.vmax, network.num_atoms)
@@ -633,10 +669,10 @@ class EpsilonGreedyActor(parts.Agent):
       self._obs_dev.copy_(torch.from_numpy(np.ascontiguousarray(obs).reshape(-1)))
     L = self._learner
     taus = noise = None
-    if _iqn_net(L.kind) or L.kind == 'rainbow':
+    if _draws_taus(L.kind) or L.kind == 'rainbow':
       self._seed += 1
       L.generate_randomness(self._seed)
-      taus = L.taus if _iqn_net(L.kind) else None
+      taus = L.taus if _draws_taus(L.kind) else None
       noise = L.noise if L.kind == 'rainbow' else None
     q = L.q_values(self._obs_dev, taus=taus, noise=noise).cpu().numpy()
     if self._epsilon > 0.0 and self._rng.uniform() < self._epsilon:
@@ -665,7 +701,7 @@ class EpsilonGreedyActor(parts.Agent):
 
 
 AGENTS = {'dqn': Dqn, 'double_q': DoubleQ, 'prioritized': PrioritizedDqn, 'c51': C51, 'qrdqn': QrDqn,
-          'rainbow': Rainbow, 'iqn': Iqn, 'munchausen': Munchausen, 'munchausen_iqn': MunchausenIqn}
+          'rainbow': Rainbow, 'iqn': Iqn, 'munchausen': Munchausen, 'munchausen_iqn': MunchausenIqn, 'fqf': Fqf}
 
 
 class BatchedEpsilonGreedyActor:
@@ -721,7 +757,7 @@ class BatchedEpsilonGreedyActor:
     if self._actor is not None:
       if self._per_stream_noise:
         stream_noise = self._actor.generate_randomness(self._seed, per_stream=True)
-      elif _iqn_net(kind):
+      elif _draws_taus(kind):
         taus = self._actor.generate_randomness(self._seed)
       elif kind == 'rainbow':
         noise = self._actor.generate_randomness(self._seed)
@@ -730,9 +766,9 @@ class BatchedEpsilonGreedyActor:
     else:
       if self._per_stream_noise:
         stream_noise = L.generate_stream_noise(self._seed, self._E)
-      elif _iqn_net(kind) or kind == 'rainbow':
+      elif _draws_taus(kind) or kind == 'rainbow':
         L.generate_randomness(self._seed)
-        if _iqn_net(kind):
+        if _draws_taus(kind):
           taus = L.taus[:self._E * L.net.tau_samples_policy] if hasattr(L.net, 'tau_samples_policy') else L.taus
         else:
           noise = L.noise
@@ -791,9 +827,9 @@ class VectorTrainer:
     if E > L.batch_size:                       # acted through an acting context: its limits apply
       if E > ACTOR_MAX_STREAMS:
         raise ValueError('num_streams %d exceeds the acting limit of %d streams' % (E, ACTOR_MAX_STREAMS))
-      if _iqn_net(L.kind) and E * L.net.tau_samples_policy > ACTOR_MAX_IQN_ROWS:
-        raise ValueError('iqn acting needs num_streams * tau_samples_policy <= %d, got %d * %d'
-                         % (ACTOR_MAX_IQN_ROWS, E, L.net.tau_samples_policy))
+      err = _acting_rows_error(L.net, E)
+      if err:
+        raise ValueError(err)
     acc = train_agent._transition_accumulator
     if not isinstance(acc, replay_lib.NStepTransitionAccumulator):
       raise ValueError('the agent needs a TransitionAccumulator or NStepTransitionAccumulator')
@@ -1071,9 +1107,9 @@ class VectorEvaluator:
     else:
       raise TypeError('network_or_learner must be a NetworkSpec or a Learner')
     net = network_or_learner.net if shape_learner is not None else network_or_learner
-    if _iqn_net(net.kind) and E * net.tau_samples_policy > ACTOR_MAX_IQN_ROWS:
-      raise ValueError('iqn acting needs num_streams * tau_samples_policy <= %d, got %d * %d'
-                       % (ACTOR_MAX_IQN_ROWS, E, net.tau_samples_policy))
+    err = _acting_rows_error(net, E)
+    if err:
+      raise ValueError(err)
     if per_stream_noise and net.kind != 'rainbow':
       raise ValueError('per_stream_noise needs a rainbow network')
     kwargs = dict(preprocessor_kwargs or {})
@@ -1167,7 +1203,7 @@ class VectorEvaluator:
     taus = noise = stream_noise = None
     if self._per_stream_noise:
       stream_noise = A.generate_randomness(self._seed, per_stream=True)
-    elif _iqn_net(self._net.kind):
+    elif _draws_taus(self._net.kind):
       taus = A.generate_randomness(self._seed)
     elif self._net.kind == 'rainbow':
       noise = A.generate_randomness(self._seed)

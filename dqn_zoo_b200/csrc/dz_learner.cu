@@ -9,6 +9,9 @@
 //   _learn glue   rainbow/agent.py:181-198, prioritized/agent.py:187-206
 //   munchausen    Munchausen DQN and Munchausen-IQN (Vieillard, Pietquin & Geist, NeurIPS 2020), outside the
 //                 reference: dqn's / iqn's network with online(s_tm1) | target(s_tm1) | target(s_t) (DESIGN.md §13, §14)
+//   fqf           Fully parameterized Quantile Function (Yang et al., NeurIPS 2019), outside the reference: iqn's
+//                 network at taus a fraction proposal layer computes in the step, its own loss kernel and a second
+//                 (RMSProp) optimizer launch over the fraction layer (DESIGN.md §15)
 //
 // Gradients flow only through online(s_tm1).  All forward passes of a layer are one grouped
 // launch (dz_gemm.cuh); the replay gather is fused into conv1's operand load.
@@ -25,10 +28,16 @@
 
 namespace dz {
 
-// The network an agent kind applies: munchausen_iqn runs iqn's network, munchausen dqn's.  Every network-structure
+// The network an agent kind applies: munchausen_iqn and fqf run iqn's network, munchausen dqn's.  Every network-structure
 // decision (layout, carving, tensor-core plan, randomness, tau counts, acting) goes through these two predicates; the
 // loss launch is the only place that tells a Munchausen kind from the kind whose network it uses.
-__host__ __device__ constexpr bool uses_iqn_net(int kind) { return kind == DZ_IQN || kind == DZ_MUNCHAUSEN_IQN; }
+__host__ __device__ constexpr bool uses_iqn_net(int kind) { return kind == DZ_IQN || kind == DZ_MUNCHAUSEN_IQN || kind == DZ_FQF; }
+// fqf (DESIGN.md §15) carries every decision in which it differs from iqn: its taus are proposed in the step from the
+// torso features (no draws, no tau inputs, nothing for the randomness calls to generate), its Q-values weight the
+// quantiles by the interval widths, and the fraction layer at the end of the blob gets its own optimizer launch.
+constexpr bool proposes_fractions(int kind) { return kind == DZ_FQF; }
+// iqn's network with taus drawn per step and passed in by the caller (iqn, munchausen_iqn)
+constexpr bool draws_taus(int kind) { return uses_iqn_net(kind) && !proposes_fractions(kind); }
 __host__ __device__ constexpr bool uses_dqn_net(int kind) { return kind == DZ_DQN || kind == DZ_MUNCHAUSEN; }
 // The kind given to the device kernels that branch on the network (q_values_kernel).
 constexpr int net_kind(int kind) { return uses_iqn_net(kind) ? DZ_IQN : uses_dqn_net(kind) ? DZ_DQN : kind; }
@@ -114,6 +123,8 @@ static Layout make_layout(const dz_learner_config& c) {
   L.add("head/w", {512, d.out});
   bool shared = c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED;
   L.add("head/b", {shared ? 1 : d.out});
+  // fqf: the fraction proposal layer, last, so that it is one contiguous tail of the blob for its optimizer launch
+  if (proposes_fractions(c.kind)) { L.add("fraction/w", {d.feat, c.num_fractions}); L.add("fraction/b", {c.num_fractions}); }
   return L;
 }
 
@@ -125,6 +136,7 @@ struct ParamOffsets {
   int64_t w1[2], b1[2], sw1[2], sb1[2];
   int64_t w2[2], b2[2], sw2[2], sb2[2];
   int64_t embed_w, embed_b;
+  int64_t frac_w, frac_b;   // fqf's fraction layer; frac_w is also where the fraction tail of the blob begins
   int64_t fc_begin;   // first offset after the conv tensors
 };
 
@@ -145,6 +157,7 @@ static int param_offsets(const dz_learner_config& c, const Layout& L, ParamOffse
     o.w2[s] = o.b2[s] = o.sw2[s] = o.sb2[s] = -1;
   }
   o.embed_w = o.embed_b = -1;
+  o.frac_w = o.frac_b = -1;
   if (c.kind == DZ_RAINBOW) {
     const char* streams[2] = {"adv", "val"};
     for (int s = 0; s < 2; ++s) {
@@ -156,6 +169,7 @@ static int param_offsets(const dz_learner_config& c, const Layout& L, ParamOffse
     o.w1[0] = need("fc1/w"); o.b1[0] = need("fc1/b");
     o.w2[0] = need("head/w"); o.b2[0] = need("head/b");
     if (uses_iqn_net(c.kind)) { o.embed_w = need("embed/w"); o.embed_b = need("embed/b"); }
+    if (proposes_fractions(c.kind)) { o.frac_w = need("fraction/w"); o.frac_b = need("fraction/b"); }
   }
   o.fc_begin = uses_iqn_net(c.kind) ? o.embed_w : o.w1[0];
   if (missing) return fail(DZ_EINVAL, "parameter layout lacks a tensor of this agent kind");
@@ -224,8 +238,55 @@ __host__ __device__ inline float miqn_target(const float* zbar_j, const float* p
   return fmaf(disc, s + ent, rb);
 }
 
+// ---- FQF per-example fraction arithmetic (DESIGN.md §15), shared by fraction_forward_kernel / loss_fqf_kernel and
+// their host twin dz_test_fqf_example.  Every sum runs serially in index order, so the host and the device add in the
+// same order, and the result of example e does not depend on how many examples a launch holds.
+constexpr int kFqfMaxFractions = 128;   // pass 2 holds 2N rows per example: within the 256 rows of the IQN tau limit
+
+// logits [N] -> q = softmax(logits), tau_0 = 0, tau_i = sum_{k<i} q_k, tau_N = 1, tau_hat_i = (tau_i + tau_{i+1}) / 2 and
+// the interval weights w_i = tau_{i+1} - tau_i.  tau has N + 1 entries; any output may alias nothing else.
+__host__ __device__ inline void fqf_fractions(const float* logits, int N, float* q, float* tau, float* tau_hat, float* w) {
+  float m = logits[0];
+  for (int i = 1; i < N; ++i) m = fmaxf(m, logits[i]);
+  float s = 0.f;
+  for (int i = 0; i < N; ++i) { q[i] = expf(logits[i] - m); s += q[i]; }
+  for (int i = 0; i < N; ++i) q[i] = q[i] / s;
+  tau[0] = 0.f;
+  for (int i = 1; i < N; ++i) tau[i] = tau[i - 1] + q[i - 1];
+  tau[N] = 1.f;
+  for (int i = 0; i < N; ++i) {
+    tau_hat[i] = (tau[i] + tau[i + 1]) * 0.5f;
+    w[i] = tau[i + 1] - tau[i];
+  }
+}
+
+// The fraction gradient (the paper's Proposition 1) of one example, chained to the logits: with F(tau) =
+// Z(s_tm1, a_tm1, tau), dW1/dtau_i = 2 F(tau_i) - F(tau_hat_i) - F(tau_hat_{i-1}) for i = 1..N-1; tau_i = sum_{k<i} q_k
+// gives dq_k = sum_{i>k} dW1/dtau_i, and the softmax dlogit_k = q_k (dq_k - sum_j q_j dq_j).  F_tau[i] = F(tau_i)
+// (entries 1..N-1 are read), F_hat[i] = F(tau_hat_i); cot = w_b / B scales the result.  dlogits [N] is also the dq scratch.
+__host__ __device__ inline void fqf_dlogits(const float* F_tau, const float* F_hat, const float* q, int N, float cot,
+                                            float* dlogits) {
+  float acc = 0.f;
+  dlogits[N - 1] = 0.f;
+  for (int k = N - 2; k >= 0; --k) {
+    const int i = k + 1;
+    acc += (2.f * F_tau[i] - F_hat[i]) - F_hat[i - 1];
+    dlogits[k] = acc;
+  }
+  float dot = 0.f;
+  for (int j = 0; j < N; ++j) dot = fmaf(q[j], dlogits[j], dot);
+  for (int k = 0; k < N; ++k) dlogits[k] = cot * (q[k] * (dlogits[k] - dot));
+}
+
+// Q(s, a) = sum_i w_i Z(s, a, tau_hat_i) over N quantile rows z [N][A]: fqf's selection in the loss and its acting.
+__host__ __device__ inline float fqf_weighted_q(const float* z, const float* w, int N, int A, int a) {
+  float s = 0.f;
+  for (int i = 0; i < N; ++i) s = fmaf(w[i], z[(long long)i * A + a], s);
+  return s;
+}
+
 static int validate(const dz_learner_config& c) {
-  if (c.kind < 0 || c.kind > DZ_MUNCHAUSEN_IQN) return fail(DZ_EINVAL, "unknown agent kind");
+  if (c.kind < 0 || c.kind > DZ_FQF) return fail(DZ_EINVAL, "unknown agent kind");
   if (is_munchausen(c.kind) && !munchausen_params_ok(c.munchausen_alpha, c.entropy_temperature, c.log_policy_clip))
     return fail(DZ_EINVAL, "munchausen needs finite alpha >= 0, entropy_temperature > 0 and log_policy_clip <= 0");
   if (is_munchausen(c.kind) && c.num_actions > kMunchausenMaxActions)
@@ -243,8 +304,19 @@ static int validate(const dz_learner_config& c) {
   if (c.num_actions <= 0 || c.num_actions > 64) return fail(DZ_EINVAL, "num_actions must be in [1,64]");
   if ((c.kind == DZ_C51 || c.kind == DZ_RAINBOW) && (c.num_atoms < 2 || c.num_atoms > 128)) return fail(DZ_EINVAL, "num_atoms must be in [2,128]");
   if (c.kind == DZ_QRDQN && (c.num_quantiles < 1 || c.num_quantiles > 256)) return fail(DZ_EINVAL, "num_quantiles must be in [1,256]");
+  if (proposes_fractions(c.kind)) {
+    if (c.num_fractions < 2 || c.num_fractions > kFqfMaxFractions) return fail(DZ_EINVAL, "fqf: num_fractions must be in [2,128]");
+    if (!std::isfinite(c.fraction_learning_rate) || c.fraction_learning_rate < 0.f)
+      return fail(DZ_EINVAL, "fqf: fraction_learning_rate must be finite and >= 0");
+    if (!std::isfinite(c.fraction_opt_eps) || !(c.fraction_opt_eps > 0.f))
+      return fail(DZ_EINVAL, "fqf: fraction_opt_eps must be finite and > 0");
+    if (!(c.fraction_rms_decay >= 0.f && c.fraction_rms_decay < 1.f))
+      return fail(DZ_EINVAL, "fqf: fraction_rms_decay must be in [0,1)");
+  }
   if (uses_iqn_net(c.kind)) {
     if (c.latent_dim <= 0 || c.latent_dim % 16) return fail(DZ_EINVAL, "latent_dim must be a positive multiple of 16");
+  }
+  if (draws_taus(c.kind)) {
     int mx = c.tau_samples_s_tm1 > c.tau_samples_s_t ? c.tau_samples_s_tm1 : c.tau_samples_s_t;
     mx = mx > c.tau_samples_policy ? mx : c.tau_samples_policy;
     if (c.tau_samples_s_tm1 <= 0 || c.tau_samples_s_t <= 0 || c.tau_samples_policy <= 0 || mx > 256)
@@ -1045,6 +1117,116 @@ size_t munchausen_iqn_loss_smem(const dz_learner_config& c) {
   return (32 + 3 * (size_t)c.num_actions + 2 + c.tau_samples_s_t + 2 * (size_t)c.tau_samples_s_tm1) * sizeof(float);
 }
 
+// ---- fqf (DESIGN.md §15) ------------------------------------------------------------------------
+
+// The fraction proposal layer on the torso features of E examples and up to two applications (blockIdx.y), one CTA per
+// (example, application): logits = feat . W + b with W = fraction/w [D][N], then fqf_fractions.  Each of the 8 warps
+// takes every 8th feature row in order and the partials are added in warp order, so example e's bits do not depend on
+// E.  Every output may be NULL.  The learner's two pass inputs are written here too: pass1 = tau_1..tau_N of
+// application 0 (online(s_tm1), no gradient; row N-1 is tau_N = 1, which no loss term reads) and pass2 = [tau_hat of
+// application 1 | tau_hat of application 0] (target(s_t): the selection rows, then the target rows).
+struct FracArgs {
+  const float* feat[2];               // [E][D] torso features of each application
+  const float* W; const float* bias;  // the online blob's fraction layer
+  int N, D;
+  float* tau[2];       // [E][N + 1]
+  float* tau_hat[2];   // [E][N]
+  float* w[2];         // [E][N]
+  float* q[2];         // [E][N]
+  float* pass1;        // [E][N]
+  float* pass2;        // [E][2N]
+};
+
+__global__ void __launch_bounds__(256) fraction_forward_kernel(const __grid_constant__ FracArgs f) {
+  dz::pdl_enter();
+  constexpr int kMax = kFqfMaxFractions;
+  __shared__ float part[8][kMax];
+  __shared__ float logits[kMax], q[kMax], tau[kMax + 1], hat[kMax], w[kMax];
+  const int e = blockIdx.x, app = blockIdx.y, N = f.N, D = f.D, tid = threadIdx.x;
+  const int warp = tid >> 5, lane = tid & 31;
+  const float* __restrict__ x = f.feat[app] + (long long)e * D;
+  for (int c0 = 0; c0 < N; c0 += 32) {
+    const int col = c0 + lane;
+    if (col >= N) continue;
+    float acc = 0.f;
+#pragma unroll 4
+    for (int k = warp; k < D; k += 8) acc = fmaf(x[k], f.W[(long long)k * N + col], acc);
+    part[warp][col] = acc;
+  }
+  __syncthreads();
+  if (tid < N) {
+    float s = 0.f;
+#pragma unroll
+    for (int r = 0; r < 8; ++r) s += part[r][tid];
+    logits[tid] = s + f.bias[tid];
+  }
+  __syncthreads();
+  if (tid == 0) fqf_fractions(logits, N, q, tau, hat, w);
+  __syncthreads();
+  const long long row = (long long)e * N;
+  for (int i = tid; i <= N; i += blockDim.x) {
+    if (f.tau[app]) f.tau[app][(long long)e * (N + 1) + i] = tau[i];
+    if (i == N) continue;
+    if (f.tau_hat[app]) f.tau_hat[app][row + i] = hat[i];
+    if (f.w[app]) f.w[app][row + i] = w[i];
+    if (f.q[app]) f.q[app][row + i] = q[i];
+    if (app == 0 && f.pass1) f.pass1[row + i] = tau[i + 1];
+    if (f.pass2) f.pass2[2 * row + (app == 0 ? N : 0) + i] = hat[i];
+  }
+}
+
+struct FqfLossArgs {
+  const float* w_t;     // [B][N] interval weights of the proposal on target(s_t)'s features (application 1)
+  const float* q_tm1;   // [B][N] softmax of the proposal on online(s_tm1)'s features (application 0)
+  float* dlogits;       // [B][N] gradient of the weighted fraction loss wrt the fraction logits of application 0
+};
+
+// fqf: one CTA per example.  out0 = online(s_tm1) at tau_hat (N rows), out1 = online(s_tm1) at tau_1..tau_N (N rows, no
+// gradient), out2 = target(s_t) at [tau_hat' | tau_hat] (2N rows); taus0 = tau_hat.  (1) the selection a* = argmax_a
+// sum_i w'_i Zbar(s_t, a, tau_hat'_i), one thread per action, first maximum; (2) the targets y_j = r + discount
+// Zbar(s_t, a*, tau_hat_j); (3) the fraction gradient at a_tm1 chained to dlogits (fqf_dlogits, thread 0); (4) IQN's
+// quantile-Huber term of online(s_tm1)'s N samples at a_tm1 against the targets and dout in IQN's layout
+// (quantile_huber_tail).  The per-example value is the quantile loss.
+__global__ void __launch_bounds__(256) loss_fqf_kernel(LossArgs L, FqfLossArgs f) {
+  dz::pdl_enter();
+  extern __shared__ float sm[];
+  const int b = blockIdx.x, A = L.A, N = L.N, tid = threadIdx.x;
+  float* red = sm;           // [32]
+  float* qsel = red + 32;    // [A]
+  float* tgt = qsel + A;     // [N]
+  float* src = tgt + N;      // [N] F(tau_hat_i)
+  float* tau = src + N;      // [N] tau_hat_i
+  float* ftau = tau + N;     // [N] F(tau_i), i >= 1
+  float* q = ftau + N;       // [N]
+  float* dl = q + N;         // [N]
+  const float* zsel = L.out2 + (long long)b * 2 * N * A;
+  if (tid < A) qsel[tid] = fqf_weighted_q(zsel, f.w_t + (long long)b * N, N, A, tid);
+  const int at = L.a[b];
+  const float* z0 = L.out0 + (long long)b * N * A;
+  const float* z1 = L.out1 + (long long)b * N * A;
+  for (int i = tid; i < N; i += blockDim.x) {
+    src[i] = z0[(long long)i * A + at];
+    tau[i] = L.taus0[(long long)b * N + i];
+    ftau[i] = i > 0 ? z1[(long long)(i - 1) * A + at] : 0.f;
+    q[i] = f.q_tm1[(long long)b * N + i];
+  }
+  __syncthreads();
+  int best = 0;
+  for (int a = 1; a < A; ++a)
+    if (qsel[a] > qsel[best]) best = a;
+  const float r = L.r[b], dsc = L.disc[b];
+  const float* ztgt = zsel + (long long)N * A;
+  for (int j = tid; j < N; j += blockDim.x) tgt[j] = r + dsc * ztgt[(long long)j * A + best];
+  if (tid == 0) fqf_dlogits(ftau, src, q, N, (L.w ? L.w[b] : 1.0f) / (float)L.B, dl);
+  __syncthreads();
+  for (int k = tid; k < N; k += blockDim.x) f.dlogits[(long long)b * N + k] = dl[k];
+  quantile_huber_tail(L, b, at, N, N, tgt, src, tau, red);
+}
+
+size_t fqf_loss_smem(const dz_learner_config& c) {
+  return (32 + (size_t)c.num_actions + 6 * (size_t)c.num_fractions) * sizeof(float);
+}
+
 __global__ void loss_mean_kernel(const float* __restrict__ terms, int B, float* loss, float* max_seen, const float* priorities) {
   dz::pdl_enter();
   if (threadIdx.x == 0 && blockIdx.x == 0) {
@@ -1110,6 +1292,15 @@ __global__ void __launch_bounds__(128) q_values_kernel(int kind, int A, int atom
     if (tid == 0) q[a] = res;
     __syncthreads();
   }
+}
+
+// fqf's q-values of one N-row head pass per observation (blockIdx.x): Q(s, a) = sum_i w_i Z(s, a, tau_hat_i), the
+// weighting of the loss kernel's selection (fqf_weighted_q); out [E][N][A], w [E][N].
+__global__ void __launch_bounds__(64) q_values_fqf_kernel(int A, int N, const float* __restrict__ out, const float* __restrict__ w,
+                                                          float* __restrict__ q) {
+  dz::pdl_enter();
+  const long long e = blockIdx.x;
+  for (int a = threadIdx.x; a < A; a += blockDim.x) q[e * A + a] = fqf_weighted_q(out + e * N * A, w + e * N, N, A, a);
 }
 
 // ---- optimizer ---------------------------------------------------------------------------------
@@ -1403,6 +1594,10 @@ struct dz_learner {
   float *act1[3], *act2[3], *act3[3];
   float *h1[3][2], *out[3], *outv[3];      // rainbow: h1[p][0]=adv stream, [1]=val stream; out=adv, outv=val
   float *cosf[3], *hi[3], *E0;             // iqn
+  // fqf: the step's proposals (application 0 = online(s_tm1)'s features, 1 = target(s_t)'s): fq_tau [2][B][N+1],
+  // fq_hat / fq_w / fq_q [2][B][N]; the head passes' tau inputs fq_pass1 [B][N] and fq_pass2 [B][2N] (pass 0 reads
+  // fq_hat[0]); the fraction logits' gradient fq_dlogits [B][N]; acting's tau_hat / w, fq_act_hat / fq_act_w [B][N]
+  float *fq_tau, *fq_hat, *fq_w, *fq_q, *fq_pass1, *fq_pass2, *fq_dlogits, *fq_act_hat, *fq_act_w;
   float* nn_partial;                        // split-K partials for the M=batch FC layers and heads
   float* conv_partial;                      // split-K partials for conv2/conv3 forward
   float* nt_partial;                        // split partials of the input-gradient (NT) GEMMs
@@ -1469,7 +1664,9 @@ int64_t carve(dz_learner* l, char* base) {
   Bump w{base};
   const bool rb = c.kind == DZ_RAINBOW, iqn = uses_iqn_net(c.kind);
   int nh[3] = {1, 1, 1};
-  if (iqn) { nh[0] = c.tau_samples_s_tm1; nh[1] = c.tau_samples_policy; nh[2] = c.tau_samples_s_t; }
+  if (draws_taus(c.kind)) { nh[0] = c.tau_samples_s_tm1; nh[1] = c.tau_samples_policy; nh[2] = c.tau_samples_s_t; }
+  // fqf: online(s_tm1) at tau_hat | online(s_tm1) at tau_1..tau_N | target(s_t) at [tau_hat' | tau_hat]; acting uses pass 1
+  if (proposes_fractions(c.kind)) { nh[0] = c.num_fractions; nh[1] = c.num_fractions; nh[2] = 2 * c.num_fractions; }
   for (int p = 0; p < 3; ++p) l->n_head[p] = nh[p];
   for (int p = 0; p < 3; ++p) {
     l->act1[p] = w.take<float>((int64_t)B * d.h1 * d.w1 * 32);
@@ -1484,6 +1681,19 @@ int64_t carve(dz_learner* l, char* base) {
     l->hi[p] = iqn ? w.take<float>(rows * d.feat) : nullptr;
   }
   l->E0 = iqn ? w.take<float>((int64_t)B * nh[0] * d.feat) : nullptr;
+  {
+    const bool fq = proposes_fractions(c.kind);
+    const int64_t n = fq ? (int64_t)B * c.num_fractions : 0;
+    l->fq_tau = fq ? w.take<float>(2 * (n + B)) : nullptr;
+    l->fq_hat = fq ? w.take<float>(2 * n) : nullptr;
+    l->fq_w = fq ? w.take<float>(2 * n) : nullptr;
+    l->fq_q = fq ? w.take<float>(2 * n) : nullptr;
+    l->fq_pass1 = fq ? w.take<float>(n) : nullptr;
+    l->fq_pass2 = fq ? w.take<float>(2 * n) : nullptr;
+    l->fq_dlogits = fq ? w.take<float>(n) : nullptr;
+    l->fq_act_hat = fq ? w.take<float>(n) : nullptr;
+    l->fq_act_w = fq ? w.take<float>(n) : nullptr;
+  }
   l->fc_splits = 14; l->head_splits = 8; l->conv_splits = 4; l->nt_splits = 8;
   {
     int64_t head_n = std::max<int64_t>(d.out, c.num_atoms);
@@ -1997,8 +2207,11 @@ int iqn_embed_fc1_forward_packed(dz_learner* l, const NetBufs& nb, const Pass* p
   return DZ_OK;
 }
 
-// IQN (networks.py:264-292): cosine embedding -> linear -> relu -> * state embedding -> value head.
-int forward_heads_iqn(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, const float* const* taus, bool keep_E0, void* stream) {
+// IQN (networks.py:264-292): cosine embedding -> linear -> relu -> * state embedding -> value head.  `row_invariant`: the
+// value head takes the one-warp-per-row kernel at any row count (where the head is narrow enough), so that a row's
+// bits do not depend on how many rows the call holds (fqf's acting; the fp32 GEMMs before it never split K here).
+int forward_heads_iqn(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, const float* const* taus, bool keep_E0, void* stream,
+                      bool row_invariant = false) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
@@ -2037,7 +2250,7 @@ int forward_heads_iqn(dz_learner* l, const NetBufs& nb, const Pass* passes, int 
   } else {
     DZ_TRY(run_nn("iqn_fc1_fwd", gb, false, stream));
   }
-  if ((long long)nimg * l->n_head[passes[0].head] >= 512 && d.out <= kSkinnyMaxN && np <= 3) {
+  if (((long long)nimg * l->n_head[passes[0].head] >= 512 || row_invariant) && d.out <= kSkinnyMaxN && np <= 3) {
     SkinnyHead h;
     memset(&h, 0, sizeof(h));
     h.n = np;
@@ -2441,6 +2654,44 @@ int backward_iqn(dz_learner* l, void* stream) {
   return DZ_OK;
 }
 
+// fqf: fraction_forward_kernel over E examples of `napp` applications (grid E x napp), reading the fraction layer of
+// `params` (the online blob, or a frozen actor's snapshot).
+int launch_fraction_forward(const dz_learner* l, FracArgs f, const float* params, int E, int napp, void* stream) {
+  f.W = params + l->po.frac_w; f.bias = params + l->po.frac_b;
+  f.N = l->cfg.num_fractions; f.D = l->d.feat;
+  DZ_LAUNCH(fraction_forward_kernel, dim3((unsigned)E, (unsigned)napp), 256, 0, stream, f);
+  return DZ_OK;
+}
+
+// fqf's acting forward on set 1 of `nb` (the torso has run): the fraction layer of `params` on act3, then one N-row
+// IQN pass at tau_hat; the interval weights land in `w` for the q-values.
+int fqf_act_heads(dz_learner* l, const NetBufs& nb, const float* params, int E, float* hat, float* w, void* stream) {
+  FracArgs f;
+  memset(&f, 0, sizeof(f));
+  f.feat[0] = nb.act3[1]; f.tau_hat[0] = hat; f.w[0] = w;
+  DZ_TRY(launch_fraction_forward(l, f, params, E, 1, stream));
+  Pass pass{params, 1, 1, 0};
+  const float* taus[1] = {hat};
+  return forward_heads_iqn(l, nb, &pass, 1, E, taus, false, stream, true);
+}
+
+// fqf: the fraction layer's gradient, dW_f = act3(s_tm1)^T dlogits ([feat][N], rank B) and db_f = sum_b dlogits, on the
+// fp32 TN GEMM on the side stream (the features are stop-gradient: nothing flows back into the torso).
+int backward_fraction(dz_learner* l, void* stream) {
+  const Dims& d = l->d;
+  const ParamOffsets& o = l->po;
+  const int N = l->cfg.num_fractions;
+  float* G = l->buf.d_grads;
+  GemmBatch gb;
+  gb.n = 1;
+  GemmProblem p = zero_problem();
+  p.a_mode = A_PLAIN; p.A = l->act3[0]; p.lda = d.feat; p.M = l->B; p.K = d.feat;
+  p.B = l->fq_dlogits; p.N = N; p.ldb = N; p.ldc = N;
+  p.C = G + o.frac_w; p.Cb = G + o.frac_b;
+  gb.p[0] = p;
+  return run_tn("fqf_fraction_wgrad", gb, l->side.fork(stream, stream));
+}
+
 // Split global norm (tensor-core path, every agent but IQN): the sum of squares of everything behind the conv tensors is taken
 // on the second side stream as soon as the last FC / head weight gradient is written (norm_fc_range), the conv tensors'
 // partials come from the per-layer weight-gradient finish kernels, and the optimizer (or norm_finalize_kernel) combines them.
@@ -2457,29 +2708,44 @@ int norm_fc_range(dz_learner* l, bool apply, void* stream) {
 int run_optimizer(dz_learner* l, float* user_norm, bool apply, void* stream) {
   const dz_learner_config& c = l->cfg;
   long long n = l->lay.total;
+  // fqf: the norm, the clip and the configured optimizer cover [0, frac_w); the fraction tail gets its own launch below
+  const bool frac = proposes_fractions(c.kind);
+  const long long n_main = frac ? l->po.frac_w : n;
   float* norm = l->scalars;
   const bool split = split_norm_active(l);
   const float* parts = split ? l->norm_parts : nullptr;
   const int nparts = split ? um_norm_slots(l->um) : 0;
   if (!split) {
-    DZ_LAUNCH(grad_norm_kernel, kNormBlocks, 256, 0, stream, l->buf.d_grads, n, l->scalars + 8, l->ticket, norm,
+    DZ_LAUNCH(grad_norm_kernel, kNormBlocks, 256, 0, stream, l->buf.d_grads, n_main, l->scalars + 8, l->ticket, norm,
               apply ? l->buf.d_counters : l->buf.d_counters + 3, user_norm, 0);
   } else if (!apply) {
     DZ_LAUNCH(norm_finalize_kernel, 1, 256, 0, stream, parts, nparts, l->scalars + 1, norm, user_norm);
   }
   if (!apply) return DZ_OK;
   OptArgs o{c.optimizer, c.learning_rate, c.opt_eps, c.rms_decay, c.adam_b1, c.adam_b2, c.max_global_grad_norm,
-            l->buf.d_online, l->buf.d_grads, l->buf.d_opt_state, l->buf.d_opt_state + n, n, norm, l->buf.d_counters,
+            l->buf.d_online, l->buf.d_grads, l->buf.d_opt_state, l->buf.d_opt_state + n, n_main, norm, l->buf.d_counters,
             parts, nparts, l->scalars + 1, norm, user_norm};
   o.stages = kOptRingStages;
   const OptKernel kernel = optimizer_kernel_for(c.optimizer);
+  const OptKernel frac_kernel = optimizer_kernel_for(DZ_RMSPROP_CENTERED);
   if (!l->opt_smem_set) {
     DZ_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptSmem));
+    if (frac) DZ_CUDA_OK(cudaFuncSetAttribute(frac_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kOptSmem));
     l->opt_smem_set = true;
   }
-  const long long nchunks = ((o.n >> 2) + kOptChunk - 1) / kOptChunk;
-  const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>((long long)kNumSMs * kOptBlocksPerSM, nchunks));
-  DZ_LAUNCH_NAMED("optimizer_kernel", kernel, grid, kOptThreads, kOptSmem, stream, o);
+  auto grid_of = [](long long count) {
+    const long long nchunks = ((count >> 2) + kOptChunk - 1) / kOptChunk;
+    return (unsigned)std::max<long long>(1, std::min<long long>((long long)kNumSMs * kOptBlocksPerSM, nchunks));
+  };
+  DZ_LAUNCH_NAMED("optimizer_kernel", kernel, grid_of(o.n), kOptThreads, kOptSmem, stream, o);
+  if (frac) {   // centred RMSProp over the fraction layer, without a clip, on the same moment buffers at the same offsets
+    const long long fb = l->po.frac_w;
+    OptArgs f{DZ_RMSPROP_CENTERED, c.fraction_learning_rate, c.fraction_opt_eps, c.fraction_rms_decay, c.adam_b1, c.adam_b2,
+              0.f, l->buf.d_online + fb, l->buf.d_grads + fb, l->buf.d_opt_state + fb, l->buf.d_opt_state + n + fb, n - fb,
+              norm, l->buf.d_counters, nullptr, 0, nullptr, nullptr, nullptr};
+    f.stages = kOptRingStages;
+    DZ_LAUNCH_NAMED("fqf_fraction_optimizer", frac_kernel, grid_of(f.n), kOptThreads, kOptSmem, stream, f);
+  }
   return DZ_OK;
 }
 
@@ -2489,7 +2755,7 @@ int run_optimizer(dz_learner* l, float* user_norm, bool apply, void* stream) {
 // written) is set here.  With `side`, loss_mean_kernel runs on the side stream forked after the loss kernel and
 // *mean_stream receives it; without, everything runs on `stream`.  dz_test_loss runs this same function.
 int launch_loss(const dz_learner_config& c, LossArgs& L, int B, void* stream, SideStream* side, float* d_loss, float* max_seen,
-                void** mean_stream) {
+                void** mean_stream, const FqfLossArgs* fqf = nullptr) {
   L.kind = c.kind; L.B = B; L.A = c.num_actions; L.atoms = c.num_atoms;
   L.vmax = c.vmax; L.bound = c.grad_error_bound; L.kappa = c.huber_param;
   if (!(c.kind == DZ_RAINBOW || c.kind == DZ_PRIORITIZED)) L.priorities = nullptr;
@@ -2505,6 +2771,10 @@ int launch_loss(const dz_learner_config& c, LossArgs& L, int B, void* stream, Si
     if (smem > 48 * 1024)
       DZ_CUDA_OK(cudaFuncSetAttribute(loss_categorical_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     DZ_LAUNCH_NAMED("loss_categorical_kernel", loss_categorical_staged_kernel, B, 128, smem, stream, L);
+  } else if (proposes_fractions(c.kind)) {
+    if (!fqf) return fail(DZ_EINVAL, "fqf's loss needs the fraction buffers of a learner step");
+    L.N = c.num_fractions; L.Ksel = c.num_fractions; L.Nt = c.num_fractions;
+    DZ_LAUNCH(loss_fqf_kernel, B, 256, fqf_loss_smem(c), stream, L, *fqf);
   } else if (c.kind == DZ_MUNCHAUSEN_IQN) {
     L.N = c.tau_samples_s_tm1; L.Ksel = c.tau_samples_policy; L.Nt = c.tau_samples_s_t;
     DZ_LAUNCH(loss_munchausen_iqn_kernel, B, 256, munchausen_iqn_loss_smem(c), stream, L, c.munchausen_alpha,
@@ -2524,12 +2794,18 @@ int launch_loss(const dz_learner_config& c, LossArgs& L, int B, void* stream, Si
 // The acting tail of a head pass over E observations: q-values [E][A] (q_values_kernel) and, when `actions` is given,
 // the epsilon-greedy choice (act_select_kernel).  out: the head outputs of the pass (rainbow: the advantage stream),
 // val: rainbow's value stream.  dz_learner_q_values, batched acting, the actor and dz_test_q_values run this function.
+// fqf: `frac_w` holds the interval weights [E][N] of the pass's proposals (q_values_fqf_kernel).
 int launch_q_values(const dz_learner_config& c, int E, const float* out, const float* val, const float* explore, float epsilon,
-                    float* q, int32_t* actions, void* stream) {
-  const int nq = uses_iqn_net(c.kind) ? c.tau_samples_policy : c.num_quantiles;
-  const size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
-  DZ_LAUNCH(q_values_kernel, (unsigned)E, 128, smem, stream, net_kind(c.kind), c.num_actions, c.num_atoms, nq, c.vmax, out, out,
-            val, q);
+                    float* q, int32_t* actions, void* stream, const float* frac_w = nullptr) {
+  if (proposes_fractions(c.kind)) {
+    if (!frac_w) return fail(DZ_EINVAL, "fqf's q-values need the interval weights of the acting pass's proposals");
+    DZ_LAUNCH(q_values_fqf_kernel, (unsigned)E, 64, 0, stream, c.num_actions, c.num_fractions, out, frac_w, q);
+  } else {
+    const int nq = uses_iqn_net(c.kind) ? c.tau_samples_policy : c.num_quantiles;
+    const size_t smem = (32 + c.num_atoms + 8) * sizeof(float);
+    DZ_LAUNCH(q_values_kernel, (unsigned)E, 128, smem, stream, net_kind(c.kind), c.num_actions, c.num_atoms, nq, c.vmax, out,
+              out, val, q);
+  }
   if (actions)
     DZ_LAUNCH(act_select_kernel, (unsigned)ceil_div(E, 128), 128, 0, stream, (const float*)q, c.num_actions, E, explore, epsilon,
               actions);
@@ -2546,7 +2822,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   const float* tg = l->buf.d_target;
   const bool needs_online_st = c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED || c.kind == DZ_RAINBOW;
   if (c.kind == DZ_RAINBOW && !batch->d_noise) return fail(DZ_EINVAL, "rainbow update needs d_noise");
-  if (uses_iqn_net(c.kind) && !batch->d_taus) return fail(DZ_EINVAL, "iqn update needs d_taus");
+  if (draws_taus(c.kind) && !batch->d_taus) return fail(DZ_EINVAL, "iqn update needs d_taus");
   if (!out || !out->d_loss || !out->d_per_example) return fail(DZ_EINVAL, "update outputs d_loss and d_per_example are required");
   if (!(weights_packed && l->um != nullptr)) DZ_TRY(l->side.join(stream));   // pending side-stream work (asynchronous randomness)
 
@@ -2573,7 +2849,23 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     DZ_TRY(forward_torso(l, learner_bufs(l), jobs, nj, B, stream));
   }
 
-  if (iqn) {
+  const bool fqf = proposes_fractions(c.kind);
+  if (fqf) {
+    // fqf: the fraction layer on online(s_tm1)'s and target(s_t)'s features, then online(s_tm1, tau_hat) |
+    // online(s_tm1, tau_1..tau_N) (no gradient) | target(s_t, [tau_hat' | tau_hat])   (DESIGN.md §15)
+    const long long n = (long long)B * c.num_fractions;
+    FracArgs f;
+    memset(&f, 0, sizeof(f));
+    f.feat[0] = l->act3[0]; f.feat[1] = l->act3[2];
+    for (int a = 0; a < 2; ++a) {
+      f.tau[a] = l->fq_tau + a * (n + B); f.tau_hat[a] = l->fq_hat + a * n; f.w[a] = l->fq_w + a * n; f.q[a] = l->fq_q + a * n;
+    }
+    f.pass1 = l->fq_pass1; f.pass2 = l->fq_pass2;
+    DZ_TRY(launch_fraction_forward(l, f, on, B, 2, stream));
+    Pass passes[3] = {{on, 0, 0, 0}, {on, 0, 1, 0}, {tg, 2, 2, 0}};
+    const float* taus[3] = {l->fq_hat, l->fq_pass1, l->fq_pass2};
+    DZ_TRY(forward_heads_iqn(l, learner_bufs(l), passes, 3, B, taus, true, stream));
+  } else if (iqn) {
     // iqn: online(s_tm1, tau_tm1) | target(s_t, tau_selector) | target(s_t, tau_t)   (iqn/agent.py:192-203)
     // munchausen_iqn: online(s_tm1, tau_tm1) | target(s_tm1, tau_policy) | target(s_t, tau_t), three torso sets
     Pass passes[3] = {{on, 0, 0, 0}, {tg, target_stm1 ? 1 : 2, 1, 0}, {tg, 2, 2, 0}};
@@ -2600,13 +2892,15 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   memset(&L, 0, sizeof(L));
   L.out0 = l->out[0]; L.out1 = l->out[1]; L.out2 = l->out[2];
   L.adv0 = l->out[0]; L.val0 = l->outv[0]; L.adv1 = l->out[1]; L.val1 = l->outv[1]; L.adv2 = l->out[2]; L.val2 = l->outv[2];
-  L.a = batch->d_a_tm1; L.r = batch->d_r_t; L.disc = batch->d_discount_t; L.w = batch->d_weights; L.taus0 = batch->d_taus;
+  L.a = batch->d_a_tm1; L.r = batch->d_r_t; L.disc = batch->d_discount_t; L.w = batch->d_weights;
+  L.taus0 = fqf ? l->fq_hat : batch->d_taus;
   L.dout = l->dout; L.dadv = l->dout; L.dval = l->doutv;
   L.per_example = out->d_per_example; L.loss_terms = l->loss_terms; L.priorities = out->d_priorities;
+  const FqfLossArgs fl{l->fq_w + (fqf ? (long long)B * c.num_fractions : 0), l->fq_q, l->fq_dlogits};
   {   // the scalar loss / running max priority and replay.update_priorities(ids, priorities) (rainbow/agent.py:198) are
       // independent of the backward pass: both leave the critical path for the side stream
     void* ls = stream;
-    DZ_TRY(launch_loss(c, L, B, stream, &l->side, out->d_loss, max_seen, &ls));
+    DZ_TRY(launch_loss(c, L, B, stream, &l->side, out->d_loss, max_seen, &ls, fqf ? &fl : nullptr));
     if (wb) DZ_TRY(launch_update_priorities(wb->view, wb->indices, wb->priorities, B, wb->alpha, wb->view->capacity, ls));
   }
 
@@ -2614,6 +2908,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   if (c.kind == DZ_RAINBOW) DZ_TRY(backward_rainbow(l, batch->d_noise, stream));
   else if (iqn) DZ_TRY(backward_iqn(l, stream));
   else DZ_TRY(backward_plain(l, stream));
+  if (fqf) DZ_TRY(backward_fraction(l, stream));
   if (split_norm_active(l)) {   // every gradient behind the conv tensors is final once the side stream's FC / head wgrads are done
     DZ_TRY(norm_fc_range(l, apply_update != 0, l->side.tail(stream)));
   }
@@ -2649,7 +2944,7 @@ int dz_learner_plan_query(const dz_learner_config* cfg, dz_learner_plan* out) {
   out->opt_state_floats = 2 * tmp.lay.total;
   out->workspace_bytes = carve(&tmp, nullptr);
   out->noise_floats = cfg->kind == DZ_RAINBOW ? 3 * noise_layout(*cfg, tmp.d).stride : 0;
-  out->tau_floats = uses_iqn_net(cfg->kind)
+  out->tau_floats = draws_taus(cfg->kind)
                         ? (int64_t)cfg->batch * (cfg->tau_samples_s_tm1 + cfg->tau_samples_policy + cfg->tau_samples_s_t)
                         : 0;
   return DZ_OK;
@@ -2788,7 +3083,7 @@ int dz_learner_generate_randomness_async(dz_learner* l, uint64_t seed, float* d_
 
 int dz_learner_generate_randomness(dz_learner* l, uint64_t seed, float* d_taus, float* d_noise, void* stream) {
   const dz_learner_config& c = l->cfg;
-  if (uses_iqn_net(c.kind) && d_taus) {
+  if (draws_taus(c.kind) && d_taus) {
     long long n = (long long)c.batch * (c.tau_samples_s_tm1 + c.tau_samples_policy + c.tau_samples_s_t);
     DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_taus, n, seed, l->buf.d_counters, 0, 1u);
   }
@@ -2808,7 +3103,9 @@ int dz_learner_q_values(dz_learner* l, const uint8_t* d_obs, const float* d_taus
   TorsoJob job{on, l->rows_act, 1};   // use activation set 1 so a pending backward's set-0 buffers stay intact
   DZ_TRY(forward_torso(l, learner_bufs(l), &job, 1, 1, stream));
   Pass pass{on, 1, 1, 0};
-  if (uses_iqn_net(c.kind)) {
+  if (proposes_fractions(c.kind)) {
+    DZ_TRY(fqf_act_heads(l, learner_bufs(l), on, 1, l->fq_act_hat, l->fq_act_w, stream));
+  } else if (uses_iqn_net(c.kind)) {
     if (!d_taus) return fail(DZ_EINVAL, "iqn q_values needs taus[tau_samples_policy]");
     const float* taus[1] = {d_taus};
     DZ_TRY(forward_heads_iqn(l, learner_bufs(l), &pass, 1, 1, taus, false, stream));
@@ -2818,7 +3115,7 @@ int dz_learner_q_values(dz_learner* l, const uint8_t* d_obs, const float* d_taus
   } else {
     DZ_TRY(forward_heads_plain(l, learner_bufs(l), &pass, 1, 1, stream));
   }
-  return launch_q_values(c, 1, l->out[1], l->outv[1], nullptr, 0.f, d_q_out, nullptr, stream);
+  return launch_q_values(c, 1, l->out[1], l->outv[1], nullptr, 0.f, d_q_out, nullptr, stream, l->fq_act_w);
 }
 
 // Batched acting (parts.py:342-411 with many actors; dqn/agent.py:121-131,169-177): online forward on E <= batch observations
@@ -2840,7 +3137,9 @@ int act_batch_impl(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* 
   TorsoJob job{on, l->rows_act, 1};
   DZ_TRY(forward_torso(l, learner_bufs(l), &job, 1, E, stream));
   Pass pass{on, 1, 1, 0};
-  if (uses_iqn_net(c.kind)) {
+  if (proposes_fractions(c.kind)) {
+    DZ_TRY(fqf_act_heads(l, learner_bufs(l), on, E, l->fq_act_hat, l->fq_act_w, stream));
+  } else if (uses_iqn_net(c.kind)) {
     if (!d_taus) return fail(DZ_EINVAL, "iqn act_batch needs taus[E][tau_samples_policy]");
     const float* taus[1] = {d_taus};
     DZ_TRY(forward_heads_iqn(l, learner_bufs(l), &pass, 1, E, taus, false, stream));
@@ -2850,7 +3149,7 @@ int act_batch_impl(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* 
   } else {
     DZ_TRY(forward_heads_plain(l, learner_bufs(l), &pass, 1, E, stream));
   }
-  return launch_q_values(c, E, l->out[1], l->outv[1], d_explore, epsilon, d_q_out, d_actions, stream);
+  return launch_q_values(c, E, l->out[1], l->outv[1], d_explore, epsilon, d_q_out, d_actions, stream, l->fq_act_w);
 }
 }  // namespace
 
@@ -2915,6 +3214,8 @@ struct dz_actor {
   bool frozen = false;
   bool loaded = false;         // frozen: dz_actor_load_params has run
   float* params = nullptr;     // frozen: the parameter snapshot, [P] in the learner's layout
+  float* frac_hat = nullptr;   // fqf: the acting pass's tau_hat and interval weights, [E][N] each
+  float* frac_w = nullptr;
   int64_t* counters = nullptr; // frozen: [2]; [1] is the generator counter (the slot randomness_kernel reads)
 };
 
@@ -2922,10 +3223,15 @@ namespace {
 
 constexpr int kActorMaxStreams = 1024, kActorMaxIqnRows = 16384;
 
+// Rows per observation of the acting pass of iqn's network: the policy taus, or fqf's N fractions.
+int acting_samples(const dz_learner_config& c) { return proposes_fractions(c.kind) ? c.num_fractions : c.tau_samples_policy; }
+
 int actor_check(const dz_learner_config& c, int E) {
   if (E < 1 || E > kActorMaxStreams) return fail(DZ_EINVAL, "actor: num_streams must be in [1, 1024]");
-  if (uses_iqn_net(c.kind) && (int64_t)E * c.tau_samples_policy > kActorMaxIqnRows)
+  if (draws_taus(c.kind) && (int64_t)E * c.tau_samples_policy > kActorMaxIqnRows)
     return fail(DZ_EINVAL, "actor: num_streams * tau_samples_policy must be <= 16384");
+  if (proposes_fractions(c.kind) && (int64_t)E * c.num_fractions > kActorMaxIqnRows)
+    return fail(DZ_EINVAL, "actor: num_streams * num_fractions must be <= 16384");
   return DZ_OK;
 }
 
@@ -2957,7 +3263,7 @@ int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
     b.act3[1] = w.take<float>((int64_t)E * d.feat);
     b.conv_partial = w.take<float>((int64_t)l->conv_splits * E * d.h2 * d.w2 * 64);
   }
-  const int64_t rows = (int64_t)E * (iqn ? c.tau_samples_policy : 1);
+  const int64_t rows = (int64_t)E * (iqn ? acting_samples(c) : 1);
   if (!um || iqn) {                      // otherwise h1 is the tensor-core plan's
     b.h1[1][0] = w.take<float>(rows * 512);
     b.h1[1][1] = rb ? w.take<float>(rows * 512) : nullptr;
@@ -2968,6 +3274,8 @@ int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
   b.hi[1] = iqn ? w.take<float>(rows * d.feat) : nullptr;
   a->rows = w.take<const uint8_t*>(E);
   a->noise = rb ? w.take<float>(noise_layout(c, d).stride) : nullptr;
+  a->frac_hat = proposes_fractions(c.kind) ? w.take<float>((int64_t)E * c.num_fractions) : nullptr;
+  a->frac_w = proposes_fractions(c.kind) ? w.take<float>((int64_t)E * c.num_fractions) : nullptr;
   if (a->frozen) {
     a->params = w.take<float>(l->lay.total);
     a->counters = w.take<int64_t>(2);
@@ -3108,7 +3416,7 @@ int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const f
   const int E = a->E;
   const bool rb = c.kind == DZ_RAINBOW;
   if (!d_obs || !d_q_out || !d_actions) return fail(DZ_EINVAL, "actor: null buffer");
-  if (uses_iqn_net(c.kind) && !d_taus) return fail(DZ_EINVAL, "iqn actor needs taus[E][tau_samples_policy]");
+  if (draws_taus(c.kind) && !d_taus) return fail(DZ_EINVAL, "iqn actor needs taus[E][tau_samples_policy]");
   if (rb && !d_noise) return fail(DZ_EINVAL, "rainbow actor needs noise");
   const int64_t stride = rb ? noise_layout(c, l->d).stride : 0;
   if (noise_ld != 0 && (!rb || noise_ld != stride))
@@ -3131,7 +3439,9 @@ int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const f
     DZ_TRY(forward_torso(l, a->b, &job, 1, E, stream));
   }
   Pass pass{on, 1, 1, 0};
-  if (uses_iqn_net(c.kind)) {
+  if (proposes_fractions(c.kind)) {
+    DZ_TRY(fqf_act_heads(l, a->b, on, E, a->frac_hat, a->frac_w, stream));
+  } else if (uses_iqn_net(c.kind)) {
     const float* taus[1] = {d_taus};
     DZ_TRY(forward_heads_iqn(l, a->b, &pass, 1, E, taus, false, stream));
   } else if (rb) {
@@ -3139,7 +3449,7 @@ int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const f
   } else {
     DZ_TRY(forward_heads_plain(l, a->b, &pass, 1, E, stream, fc_done));
   }
-  return launch_q_values(c, E, a->b.out[1], a->b.outv[1], d_explore, epsilon, d_q_out, d_actions, stream);
+  return launch_q_values(c, E, a->b.out[1], a->b.outv[1], d_explore, epsilon, d_q_out, d_actions, stream, a->frac_w);
 }
 
 // The actor's randomness from the learner's generator and counter: iqn taus [E][tau_samples_policy] (the stream id of
@@ -3150,7 +3460,7 @@ int dz_actor_generate_randomness(dz_actor* a, uint64_t seed, int32_t per_stream,
   if (!a || !d_out) return fail(DZ_EINVAL, "actor randomness: null argument");
   const dz_learner_config& c = a->l->cfg;
   long long n;
-  const bool iqn = uses_iqn_net(c.kind);
+  const bool iqn = draws_taus(c.kind);
   if (iqn && !per_stream) n = (long long)a->E * c.tau_samples_policy;
   else if (c.kind == DZ_RAINBOW) n = (per_stream ? (long long)a->E : 1LL) * noise_layout(c, a->l->d).stride;
   else return fail(DZ_EINVAL, "actor randomness: iqn draws taus, rainbow noise (per_stream: rainbow only); other kinds draw nothing");
@@ -3305,6 +3615,21 @@ int dz_test_munchausen_iqn_example(const float* zbar_tm1, const float* zbar_t, i
   return DZ_OK;
 }
 
+// Host twin of fqf's per-example fraction arithmetic: fqf_fractions and fqf_dlogits, the functions the fraction and
+// loss kernels run (tests only).
+int dz_test_fqf_example(const float* logits, const float* F_tau, const float* F_hat, int32_t N, float cot, float* out) {
+  if (!logits || !F_tau || !F_hat || !out) return fail(DZ_EINVAL, "fqf example: NULL buffer");
+  if (N < 2 || N > kFqfMaxFractions) return fail(DZ_EINVAL, "fqf example: N must be in [2,128]");
+  float* q = out;
+  float* tau = q + N;
+  float* hat = tau + N + 1;
+  float* w = hat + N;
+  float* dl = w + N;
+  fqf_fractions(logits, N, q, tau, hat, w);
+  fqf_dlogits(F_tau, F_hat, q, N, cot, dl);
+  return DZ_OK;
+}
+
 // Test hook: the learner's loss section (launch_loss) on caller-owned head outputs, batch and output buffers, all on
 // `stream`.  The observation fields of cfg play no part; they are replaced by a legal geometry before validate().
 int dz_test_loss(const dz_learner_config* cfg, int32_t B, const float* const* d_out, const float* const* d_val,
@@ -3320,7 +3645,7 @@ int dz_test_loss(const dz_learner_config* cfg, int32_t B, const float* const* d_
     return fail(DZ_EINVAL, "test_loss: head outputs of three passes are required (rainbow: and value streams)");
   if (!d_a_tm1 || !d_r_t || !d_discount_t || !d_dout || !d_per_example || !d_loss_terms || !d_loss)
     return fail(DZ_EINVAL, "test_loss: NULL buffer");
-  if (uses_iqn_net(c.kind) && !d_taus) return fail(DZ_EINVAL, "test_loss: iqn needs taus[B][tau_samples_s_tm1]");
+  if (draws_taus(c.kind) && !d_taus) return fail(DZ_EINVAL, "test_loss: iqn needs taus[B][tau_samples_s_tm1]");
   if ((rb || c.kind == DZ_PRIORITIZED) && !d_priorities) return fail(DZ_EINVAL, "test_loss: this kind writes priorities");
   LossArgs L;
   memset(&L, 0, sizeof(L));
@@ -3361,6 +3686,9 @@ int dz_test_learner_buffer(dz_learner* l, const char* name, float** d_ptr, int64
     *d_ptr = l->hi[0]; *count = l->hi[0] ? rows0 * l->d.feat : 0;
   }
   else if (n == "iqn_dhi") { *d_ptr = l->dhi; *count = l->dhi ? rows0 * l->d.feat : 0; }
+  else if (n == "fqf_tau") { *d_ptr = l->fq_tau; *count = (int64_t)2 * l->B * (l->cfg.num_fractions + 1); }
+  else if (n == "fqf_tau_hat") { *d_ptr = l->fq_hat; *count = (int64_t)2 * l->B * l->cfg.num_fractions; }
+  else if (n == "fqf_dlogits") { *d_ptr = l->fq_dlogits; *count = (int64_t)l->B * l->cfg.num_fractions; }
   else return fail(DZ_EINVAL, "unknown buffer '%s'", name);
   if (!*d_ptr) return fail(DZ_EINVAL, "buffer '%s' is not used by this agent kind", name);
   return DZ_OK;

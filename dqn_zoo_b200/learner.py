@@ -45,16 +45,24 @@ def default_optimizer(kind: str) -> OptimizerSpec:
   if kind == 'rainbow':
     return OptimizerSpec('adam', 0.0000625, 0.005 / 32, max_global_grad_norm=10.0)  # rainbow/run_atari.py:229-235
   if uses_iqn_network(kind):
-    return OptimizerSpec('adam', 0.00005, 0.01 / 32)   # munchausen_iqn: iqn's, as the M-IQN paper's Atari values
+    # munchausen_iqn: iqn's, as the M-IQN paper's Atari values; fqf: the same Adam over every tensor but the fraction
+    # layer, which has its own RMSProp (Learner's fraction_* keywords, DESIGN.md §15)
+    return OptimizerSpec('adam', 0.00005, 0.01 / 32)
   if kind == 'munchausen':
     return OptimizerSpec('adam', 0.00005, 0.01 / 32)   # the M-DQN paper's Atari values; no run_atari pins them
   raise ValueError(kind)
 
 
 def uses_iqn_network(kind: str) -> bool:
-  """Whether the agent kind applies IQN's network (cosine tau embedding, quantile samples, taus drawn per step):
-  iqn, and munchausen_iqn (DESIGN.md §14), which shares its parameters, taus and acting."""
-  return kind in ('iqn', 'munchausen_iqn')
+  """Whether the agent kind applies IQN's network (cosine tau embedding, quantile samples): iqn, munchausen_iqn
+  (DESIGN.md §14), which shares its parameters, taus and acting, and fqf (DESIGN.md §15), which adds a fraction layer."""
+  return kind in ('iqn', 'munchausen_iqn', 'fqf')
+
+
+def draws_taus(kind: str) -> bool:
+  """Whether the agent kind's steps and acting take taus drawn by the caller: IQN's network except fqf, whose fraction
+  layer proposes them from the torso features.  Every place that allocates, draws or passes taus asks this."""
+  return uses_iqn_network(kind) and kind != 'fqf'
 
 
 class NetworkSpec(NamedTuple):
@@ -70,6 +78,7 @@ class NetworkSpec(NamedTuple):
   tau_samples_policy: int = 64
   tau_samples_s_t: int = 64
   obs_shape: tuple = (84, 84, 4)
+  num_fractions: int = 32              # fqf: N, the number of proposed quantile fractions
 
 
 # canonical name -> haiku-style module path (the nested "sequential/..." prefixes are
@@ -83,9 +92,9 @@ def haiku_name(canonical: str, kind: str):
   if kind == 'rainbow':
     idx = {'adv1': '', 'adv2': '_1', 'val1': '_2', 'val2': '_3'}[parts[0]]
     return 'noisy_linear%s/%s' % (idx, parts[1]), leaf
-  if uses_iqn_network(kind):
+  if uses_iqn_network(kind):   # fqf's fraction layer: a linear module of its own beside the quantile network
     return {'embed': 'batch_apply/linear', 'fc1': 'batch_apply_1/sequential/linear',
-            'head': 'batch_apply_1/sequential/linear_1'}[parts[0]], leaf
+            'head': 'batch_apply_1/sequential/linear_1', 'fraction': 'fraction_proposal/linear'}[parts[0]], leaf
   return {'fc1': 'sequential/sequential_1/linear', 'head': 'sequential/sequential_1/linear_1'}[parts[0]], leaf
 
 
@@ -125,10 +134,13 @@ class Learner:
 
   def __init__(self, net: NetworkSpec, batch_size: int = 32, optimizer: Optional[OptimizerSpec] = None,
                grad_error_bound: float = 1.0 / 32, huber_param: float = 1.0, munchausen_alpha: float = 0.9,
-               entropy_temperature: float = 0.03, log_policy_clip: float = -1.0, device=None):
+               entropy_temperature: float = 0.03, log_policy_clip: float = -1.0, fraction_learning_rate: float = 2.5e-9,
+               fraction_opt_eps: float = 1e-5, fraction_rms_decay: float = 0.95, device=None):
     """`munchausen_alpha`, `entropy_temperature` (tau) and `log_policy_clip` (l0) are Munchausen DQN's and
     Munchausen-IQN's (DESIGN.md §13, §14, defaults the paper's Atari values); the library rejects tau <= 0, alpha < 0,
-    l0 > 0 and non-finite values for those kinds, and the other kinds ignore them."""
+    l0 > 0 and non-finite values for those kinds, and the other kinds ignore them.  `fraction_learning_rate`,
+    `fraction_opt_eps` and `fraction_rms_decay` are fqf's centred RMSProp over its fraction layer (DESIGN.md §15); the
+    library rejects a negative or non-finite rate, eps <= 0 and a decay outside [0, 1) for fqf."""
     if not torch.cuda.is_available():
       raise RuntimeError('dqn_zoo_b200.learner needs a CUDA device (there is no CPU fallback)')
     self.net = net
@@ -147,6 +159,9 @@ class Learner:
     cfg.learning_rate, cfg.opt_eps, cfg.rms_decay = self.opt.learning_rate, self.opt.eps, self.opt.decay
     cfg.adam_b1, cfg.adam_b2, cfg.max_global_grad_norm = self.opt.b1, self.opt.b2, self.opt.max_global_grad_norm
     cfg.munchausen_alpha, cfg.entropy_temperature, cfg.log_policy_clip = munchausen_alpha, entropy_temperature, log_policy_clip
+    cfg.num_fractions = net.num_fractions
+    cfg.fraction_learning_rate, cfg.fraction_opt_eps, cfg.fraction_rms_decay = (fraction_learning_rate, fraction_opt_eps,
+                                                                                fraction_rms_decay)
     self.cfg = cfg
     plan = _lib.LearnerPlan()
     _lib.call('dz_learner_plan_query', C.byref(cfg), C.byref(plan))
@@ -202,13 +217,18 @@ class Learner:
 
   def init_params(self, seed: int) -> None:
     """Legacy U(+-1/sqrt(fan_in)) init for weights AND biases (networks.py:58-79); noisy sigma =
-    sigma0/sqrt(in) (networks.py:156-166).  numpy RandomState stream — not the JAX PRNG."""
+    sigma0/sqrt(in) (networks.py:156-166); fqf's fraction layer U(+-0.01/sqrt(fan_in)) weights and zero biases, so the
+    first fractions are uniform to within about 1e-2.  numpy RandomState stream — not the JAX PRNG."""
     rs = np.random.RandomState(seed)
     params = {}
     for name, (_, shape) in self.tensors.items():
       layer = name.rsplit('/', 1)[0]
       n_in = int(np.prod(self.tensors[layer + '/w'][1][:-1]))
-      if '/sigma/' in name:
+      if name == 'fraction/w':
+        params[name] = rs.uniform(-0.01 / math.sqrt(n_in), 0.01 / math.sqrt(n_in), size=shape).astype(np.float32)
+      elif name == 'fraction/b':
+        params[name] = np.zeros(shape, np.float32)
+      elif '/sigma/' in name:
         params[name] = np.full(shape, self.net.noisy_weight_init / math.sqrt(n_in), dtype=np.float32)
       else:
         bound = math.sqrt(1.0 / n_in)
@@ -283,7 +303,7 @@ class Learner:
       self.noise[:flat.numel()].copy_(flat)
     batch = _lib.Batch(keep[2].data_ptr(), keep[3].data_ptr(), keep[4].data_ptr(), keep[5].data_ptr(),
                        keep[6].data_ptr(), 0 if w is None else w.data_ptr(),
-                       self.taus.data_ptr() if uses_iqn_network(self.kind) else 0,
+                       self.taus.data_ptr() if draws_taus(self.kind) else 0,
                        self.noise.data_ptr() if self.kind == 'rainbow' else 0)
     out = _lib.UpdateOutputs(self.loss.data_ptr(), self.per_example.data_ptr(), self.priorities.data_ptr(),
                              self.grad_norm.data_ptr())
@@ -366,7 +386,7 @@ class Learner:
     io.sample_in = _lib.SampleInputs(base, base + 8 * B, base + 16 * B, base + 24 * B)
     sp, fp = self.s_ids.data_ptr(), self.s_f64.data_ptr()
     io.sample_out = _lib.SampleOutputs(sp, sp + 8 * B, sp + 16 * B, fp, fp + 8 * B)
-    io.d_taus = self.taus.data_ptr() if uses_iqn_network(self.kind) else 0
+    io.d_taus = self.taus.data_ptr() if draws_taus(self.kind) else 0
     io.d_noise = self.noise.data_ptr() if self.kind == 'rainbow' else 0
     io.update_out = _lib.UpdateOutputs(self.loss.data_ptr(), self.per_example.data_ptr(), self.priorities.data_ptr(),
                                        self.grad_norm.data_ptr())
@@ -425,7 +445,7 @@ class Actor:
       torch.cuda.current_stream().synchronize()   # create zeroes the counter on the legacy stream: after the fill
     self.q = torch.zeros((E, net.num_actions), dtype=torch.float32, device=dev)
     self.actions = torch.zeros(E, dtype=torch.int32, device=dev)
-    self.taus = torch.zeros((E, net.tau_samples_policy), dtype=torch.float32, device=dev) if uses_iqn_network(net.kind) else None
+    self.taus = torch.zeros((E, net.tau_samples_policy), dtype=torch.float32, device=dev) if draws_taus(net.kind) else None
     rb = net.kind == 'rainbow'
     self.noise = torch.zeros(learner.noise_stride, dtype=torch.float32, device=dev) if rb else None
     self.stream_noise = torch.zeros((E, learner.noise_stride), dtype=torch.float32, device=dev) if rb else None
@@ -519,9 +539,9 @@ class Actor:
     kind = self.kind
     if per_stream and kind != 'rainbow':
       raise ValueError('per_stream randomness needs a rainbow learner')
-    if not uses_iqn_network(kind) and kind != 'rainbow':
+    if not draws_taus(kind) and kind != 'rainbow':
       raise ValueError('%s acting draws no randomness' % kind)
-    buf = self.taus if uses_iqn_network(kind) else (self.stream_noise if per_stream else self.noise)
+    buf = self.taus if draws_taus(kind) else (self.stream_noise if per_stream else self.noise)
     _lib.call('dz_actor_generate_randomness', self._h, seed, 1 if per_stream else 0, buf.data_ptr(), _cstream())
     return buf
 
@@ -555,7 +575,7 @@ class Actor:
     else:
       if taus is not None:
         t = torch.as_tensor(taus, device=L.device).to(torch.float32).contiguous()
-        if uses_iqn_network(L.kind) and t.numel() != E * L.net.tau_samples_policy:
+        if draws_taus(L.kind) and t.numel() != E * L.net.tau_samples_policy:
           raise ValueError('taus must be [%d, %d], got %s' % (E, L.net.tau_samples_policy, tuple(t.shape)))
       if noise is not None:
         n = torch.as_tensor(noise, device=L.device).to(torch.float32).contiguous()

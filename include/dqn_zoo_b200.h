@@ -312,9 +312,12 @@ int dz_replay_update_priorities(const dz_replay_view* view, const int64_t* d_ind
 /* DZ_MUNCHAUSEN: Munchausen DQN (Vieillard, Pietquin & Geist, NeurIPS 2020), outside the reference tree: dqn's
  * network, parameter layout and acting, with the soft, log-policy-augmented target of DESIGN.md §13.
  * DZ_MUNCHAUSEN_IQN: Munchausen-IQN from the same paper: iqn's network, parameter layout, taus and acting, with the
- * soft target over quantile samples of DESIGN.md §14. */
+ * soft target over quantile samples of DESIGN.md §14.
+ * DZ_FQF: the Fully parameterized Quantile Function (Yang et al., NeurIPS 2019): iqn's network, whose taus a fraction
+ * proposal layer computes from the torso features inside the step instead of drawing them (DESIGN.md §15).  Its
+ * parameter layout is iqn's followed by "fraction/w" [feat][N] and "fraction/b" [N]; it takes no taus anywhere. */
 enum dz_agent_kind { DZ_DQN = 0, DZ_DOUBLE_Q = 1, DZ_PRIORITIZED = 2, DZ_C51 = 3, DZ_QRDQN = 4, DZ_RAINBOW = 5, DZ_IQN = 6,
-                     DZ_MUNCHAUSEN = 7, DZ_MUNCHAUSEN_IQN = 8 };
+                     DZ_MUNCHAUSEN = 7, DZ_MUNCHAUSEN_IQN = 8, DZ_FQF = 9 };
 enum dz_optimizer_kind { DZ_ADAM = 0, DZ_RMSPROP_CENTERED = 1 };
 
 typedef struct dz_learner_config {
@@ -322,8 +325,8 @@ typedef struct dz_learner_config {
   int32_t num_actions;
   int32_t num_atoms;         /* c51 / rainbow: 51 */
   int32_t num_quantiles;     /* qrdqn: 201 */
-  int32_t latent_dim;        /* iqn / munchausen_iqn: 64 */
-  int32_t tau_samples_s_tm1, tau_samples_policy, tau_samples_s_t; /* iqn / munchausen_iqn: N, K, N' */
+  int32_t latent_dim;        /* iqn / munchausen_iqn / fqf: 64 */
+  int32_t tau_samples_s_tm1, tau_samples_policy, tau_samples_s_t; /* iqn / munchausen_iqn: N, K, N' (fqf ignores them) */
   int32_t batch;             /* 32 */
   int32_t obs_h, obs_w, obs_c; /* 84,84,4 */
   /* loss hyperparameters, validated for every kind: finite, vmax > 0, grad_error_bound >= 0, huber_param >= 0 */
@@ -339,6 +342,14 @@ typedef struct dz_learner_config {
   float munchausen_alpha;    /* scale of the log-policy bonus: 0.9 */
   float entropy_temperature; /* tau of the softmax policy of the target network: 0.03 */
   float log_policy_clip;     /* l0, the lower clip of tau * log pi: -1 */
+  /* fqf only (other kinds ignore them, so a zero-filled tail is valid there); DZ_EINVAL unless num_fractions is in
+   * [2, 128], the learning rate finite and >= 0, eps finite and > 0 and the decay in [0, 1).  The fraction layer is
+   * updated by centred RMSProp with these values; the optimizer fields above cover every other tensor, and the clip
+   * (when set) and the reported grad norm cover those same tensors. */
+  int32_t num_fractions;         /* N: 32 */
+  float fraction_learning_rate;  /* 2.5e-9 */
+  float fraction_opt_eps;        /* 1e-5 */
+  float fraction_rms_decay;      /* 0.95 */
 } dz_learner_config;
 
 typedef struct dz_learner_plan {
@@ -347,7 +358,7 @@ typedef struct dz_learner_plan {
   int64_t opt_state_floats;  /* 2*param_count (adam: mu,nu; rmsprop: mu,nu) */
   int64_t workspace_bytes;
   int64_t noise_floats;      /* rainbow: floats of factorised noise for ONE update (3 applies) */
-  int64_t tau_floats;        /* iqn: batch*(N+K+N') */
+  int64_t tau_floats;        /* iqn / munchausen_iqn: batch*(N+K+N'); fqf: 0 (its taus live in the workspace) */
 } dz_learner_plan;
 
 int dz_learner_plan_query(const dz_learner_config* cfg, dz_learner_plan* out);
@@ -380,7 +391,7 @@ typedef struct dz_batch {
   const float* d_r_t;                  /* [B] float32, as inside jit */
   const float* d_discount_t;           /* [B] */
   const float* d_weights;              /* [B] importance weights (float32) or NULL -> 1 */
-  const float* d_taus;                 /* iqn: [B*N | B*K | B*N'] in U[0,1)  (iqn/agent.py:182-190) or NULL */
+  const float* d_taus;                 /* iqn: [B*N | B*K | B*N'] in U[0,1)  (iqn/agent.py:182-190) or NULL; fqf: unused */
   const float* d_noise;                /* rainbow: 3 applies x 8 vectors in the order of networks.py:235-248 (adv1 in/out,
                                           adv2 in/out, val1 in/out, val2 in/out), each padded to a multiple of 4 floats; or NULL */
 } dz_batch;
@@ -431,7 +442,7 @@ int dz_learner_q_values(dz_learner* l, const uint8_t* d_obs, const float* d_taus
  * dqn/agent.py:121-131,169-177): online forward on E observations in one enqueue, q-values [E][num_actions] and the
  * epsilon-greedy choice on the device, so a tick costs ONE device-to-host copy of E int32 actions.
  *   d_obs      E contiguous uint8 observations (obs_h*obs_w*obs_c bytes each), device memory
- *   d_taus     iqn: [E][tau_samples_policy];  d_noise  rainbow: one noise apply, shared by the E streams of the tick
+ *   d_taus     iqn: [E][tau_samples_policy] (fqf: NULL, its fractions are proposed from the torso features);  d_noise  rainbow: one noise apply, shared by the E streams of the tick
  *              (the streams explore in lockstep; dz_learner_act_batch_stream_noise gives each stream its own apply)
  *   d_explore  [2][E] float32 uniforms in [0,1) (device) or NULL for greedy acting:
  *              action = u0[e] < epsilon ? min(floor(u1[e] * num_actions), num_actions - 1) : first argmax of q[e] */
@@ -454,7 +465,8 @@ int dz_learner_noise_stride(const dz_learner_config* cfg, int64_t* out);
 int dz_learner_generate_stream_noise(dz_learner* l, uint64_t seed, int32_t E, float* d_noise, void* stream);
 
 /* ---- Acting context (SURVEY §8(f) #3: many actor streams per GPU) ----------------------------------------------
- * Batched acting for num_streams in [1, 1024] streams per call (iqn: also num_streams * tau_samples_policy <= 16384)
+ * Batched acting for num_streams in [1, 1024] streams per call (iqn: also num_streams * tau_samples_policy <= 16384;
+ * fqf: num_streams * num_fractions <= 16384)
  * over the learner's ONLINE parameters, read in place: an act enqueued on the stream after a learner step sees that
  * step's parameters.  The actor keeps the learner handle (destroy the actor first) and owns only buffers sized for its
  * streams.  On the tensor-core geometries the torso and the 3136 -> 512 layer (rainbow: with one shared noise apply)
@@ -473,7 +485,7 @@ int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const f
 /* The learner's generator and counter (d_counters[1], advanced once): iqn taus [E][tau_samples_policy] with the stream
  * of dz_learner_generate_randomness's taus; rainbow one noise apply, or E applies when per_stream is set, with the
  * stream of its noise (so for E <= batch the draws equal those calls' for the same seed and counter).  DZ_EINVAL for
- * other kinds, per_stream on iqn or a NULL buffer. */
+ * other kinds (fqf included: it draws nothing), per_stream on iqn or a NULL buffer. */
 int dz_actor_generate_randomness(dz_actor* a, uint64_t seed, int32_t per_stream, float* d_out, void* stream);
 
 /* ---- Frozen acting context (evaluation over a parameter snapshot) -------------------------------------------------
@@ -642,7 +654,8 @@ int dz_test_pong_step(const dz_pong_config* cfg, int32_t* state, int32_t action,
                       int32_t* record);
 
 /* Device pointer + element count of an internal learner buffer of the last update (pass 0: "act1", "act2", "act3",
- * "h1", "h1_val", "dh1", "iqn_e0", "iqn_hi", "iqn_dhi");
+ * "h1", "h1_val", "dh1", "iqn_e0", "iqn_hi", "iqn_dhi"; fqf's proposals: "fqf_tau" [2][B][N+1] and "fqf_tau_hat"
+ * [2][B][N], application 0 from online(s_tm1)'s features and 1 from target(s_t)'s, and "fqf_dlogits" [B][N]);
  * tests/tools only. */
 int dz_test_learner_buffer(dz_learner* l, const char* name, float** d_ptr, int64_t* count);
 /* The per-example arithmetic of the munchausen loss kernel evaluated on the HOST by the same source (fp32, expf / logf):
@@ -658,6 +671,13 @@ int dz_test_munchausen_example(const float* q_tm1, const float* qbar_tm1, const 
  * DZ_EINVAL for sizes or a_tm1 out of range and for the hyperparameters dz_learner_create rejects; tests only. */
 int dz_test_munchausen_iqn_example(const float* zbar_tm1, const float* zbar_t, int32_t A, int32_t K, int32_t Nt,
                                    int32_t a_tm1, float r_t, float discount_t, float alpha, float tau, float l0, float* out);
+/* The per-example fraction arithmetic of fqf's fraction and loss kernels evaluated on the HOST by the same source
+ * (fp32, expf): logits [N] (2 <= N <= 128) -> q = softmax, tau_0..tau_N, tau_hat and the interval weights w; then the
+ * fraction gradient from F_tau [N] (F_tau[i] = Z(s_tm1, a_tm1, tau_i), entries 1..N-1 read) and F_hat [N]
+ * (Z(s_tm1, a_tm1, tau_hat_i)), chained through the cumulative sum and the softmax and scaled by cot (w_b / B).  Writes
+ * q to out[0, N), tau to out[N, 2N+1), tau_hat to out[2N+1, 3N+1), w to out[3N+1, 4N+1) and dlogits to
+ * out[4N+1, 5N+1).  DZ_EINVAL for N out of range or a NULL buffer; tests only. */
+int dz_test_fqf_example(const float* logits, const float* F_tau, const float* F_hat, int32_t N, float cot, float* out);
 /* The loss section of a learner step (the agent kind's loss kernel, then the scalar loss and rainbow's running max
  * priority) on caller-owned device buffers, all enqueued on `stream`; tests only.  cfg is validated as
  * dz_learner_create does, with batch = B and its observation fields replaced by a legal geometry.  d_out[p]: the head

@@ -162,6 +162,9 @@ def learning_agent(seed, train_frames, kind='dqn', num_actions=6):
   rep = dr.TransitionReplay(capacity, structure, rs, frame_dedup=True)
   epsilon = parts.LinearSchedule(begin_t=4 * min_fill, decay_steps=max(train_frames // 4, 1), begin_value=1.0,
                                  end_value=0.01)
+  if kind == 'fqf':   # dqn's schedule, 32 fractions, kappa 1 and the fraction layer's default RMSProp
+    return ag.Fqf(transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep, exploration_epsilon=epsilon,
+                  huber_param=1.0, **common)
   if dl.uses_iqn_network(kind):   # iqn / munchausen_iqn: dqn's schedule, iqn's 64 / 64 / 64 taus and kappa 1
     return ag.AGENTS[kind](transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep,
                            exploration_epsilon=epsilon, huber_param=1.0, tau_samples_policy=64, tau_samples_s_tm1=64,
@@ -217,7 +220,7 @@ def learning_run(train_frames, seed=0, num_streams=32, eval_every=0, log=None, g
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--game', default='catch', choices=['catch', 'breakout', 'pong'])
-  ap.add_argument('--agent', default='dqn', choices=['dqn', 'rainbow', 'munchausen', 'iqn', 'munchausen_iqn'],
+  ap.add_argument('--agent', default='dqn', choices=['dqn', 'rainbow', 'munchausen', 'iqn', 'munchausen_iqn', 'fqf'],
                   help='the agent of the learning curve')
   ap.add_argument('--parts', default='env,train,eval,driver')
   ap.add_argument('--frames', type=int, default=65536, help='frames per timed window of env_train / env_eval')

@@ -7,6 +7,11 @@ dz_profile_begin / end) for the loss kernels' times.  One JSON line per result.
 `--kinds munchausen_iqn,iqn` times Munchausen-IQN beside iqn (64 / 64 / 64 taus drawn on the device each step): it adds
 a third torso pass, target(s_tm1), to iqn's two, so its step should cost iqn's plus about one torso pass.
 
+`--kinds fqf,iqn` times FQF (32 proposed fractions) beside iqn: FQF sends fewer rows through the embedding and fc1
+(4096 against 6144 forward, 1024 against 2048 backward) but runs the fraction layer between the torso and the
+embedding, where iqn's taus are drawn beforehand; which effect wins is what this measures.  The profiled pass then also
+times fraction_forward_kernel and the fraction layer's optimizer launch.
+
 The expectation this checks: munchausen applies three networks per step like double_q (online(s_tm1) with
 target(s_tm1) and target(s_t) instead of online(s_t) and target(s_t)), the two target passes sharing each staged fc1
 weight tile as double_q's two online passes do, so its step should cost about what double_q's does."""
@@ -26,7 +31,7 @@ import torch  # noqa: E402
 import bench_train  # noqa: E402
 
 KINDS = ('munchausen', 'double_q', 'dqn')
-ALL_KINDS = KINDS + ('munchausen_iqn', 'iqn')
+ALL_KINDS = KINDS + ('munchausen_iqn', 'iqn', 'fqf')
 
 
 def emit(**kw):
@@ -45,6 +50,8 @@ def make_agent(kind, capacity=65536, seed=1):
                 transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep, batch_size=32,
                 min_replay_capacity_fraction=0.02, learn_period=16, target_network_update_period=32000,
                 rng_key=[0, seed])
+  if kind == 'fqf':
+    return ag.Fqf(exploration_epsilon=lambda t: 0.01, huber_param=1.0, **common)
   if dl.uses_iqn_network(kind):
     return ag.AGENTS[kind](exploration_epsilon=lambda t: 0.01, huber_param=1.0, tau_samples_policy=64,
                            tau_samples_s_tm1=64, tau_samples_s_t=64, **common)
@@ -108,6 +115,9 @@ def main():
     prof = profile_step(agents[k])
     loss = {t: v for t, v in prof.items() if t.startswith('loss_')}
     emit(metric='loss_kernel_us', agent=k, kernels={t: v[0] for t, v in loss.items()})
+    if k == 'fqf':   # the launches fqf adds to iqn's step
+      emit(metric='fqf_kernel_us', agent=k, kernels={t: v[0] for t, v in prof.items()
+                                                     if t.startswith('fraction_') or t.startswith('fqf_')})
     emit(metric='launches', agent=k, launches={t: [v[1], list(v[2])] for t, v in prof.items()})
   emit(metric='device_after', **bench_train.device_info())
 

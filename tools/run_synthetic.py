@@ -106,6 +106,8 @@ def build_train_agent(args, random_state, preprocessor):
     return agent_lib.C51(support=np.linspace(-10, 10, 51), exploration_epsilon=epsilon, **common), network
   if kind == 'qrdqn':
     return agent_lib.QrDqn(quantiles=(np.arange(201) + 0.5) / 201, exploration_epsilon=epsilon, huber_param=1.0, **common), network
+  if kind == 'fqf':
+    return agent_lib.Fqf(exploration_epsilon=epsilon, huber_param=1.0, **common), network
   if learner_lib.uses_iqn_network(kind):
     return agent_lib.AGENTS[kind](exploration_epsilon=epsilon, huber_param=1.0, tau_samples_policy=64, tau_samples_s_tm1=64,
                          tau_samples_s_t=64, **common), network
@@ -257,7 +259,7 @@ def parse_args(argv=None):
                        '(dqn_zoo_b200.environments)')
   ap.add_argument('--agent', default='dqn',
                   choices=['dqn', 'double_q', 'prioritized', 'c51', 'qrdqn', 'rainbow', 'iqn', 'munchausen',
-                           'munchausen_iqn'])
+                           'munchausen_iqn', 'fqf'])
   ap.add_argument('--num_actions', type=int, default=6)
   ap.add_argument('--replay_capacity', type=int, default=20000)
   ap.add_argument('--min_replay_capacity_fraction', type=float, default=0.05)
