@@ -171,9 +171,7 @@ _SIGNATURES = {
     'dz_learner_learn': (i32, [vp, C.POINTER(ReplayView), i32, C.POINTER(LearnIO), vp]),
     'dz_learner_generate_randomness': (i32, [vp, u64, vp, vp, vp]),
     'dz_learner_generate_randomness_async': (i32, [vp, u64, vp, vp, vp]),
-    'dz_learner_q_values': (i32, [vp, vp, vp, vp, vp, vp]),
-    'dz_learner_act_batch': (i32, [vp, vp, i32, vp, vp, vp, f32, vp, vp, vp]),
-    'dz_learner_act_batch_stream_noise': (i32, [vp, vp, i32, vp, vp, f32, vp, vp, vp]),
+    'dz_learner_act_batch': (i32, [vp, vp, i32, vp, vp, i64, vp, f32, vp, vp, vp]),
     'dz_learner_noise_stride': (i32, [C.POINTER(LearnerConfig), C.POINTER(i64)]),
     'dz_learner_generate_stream_noise': (i32, [vp, u64, i32, vp, vp]),
     'dz_actor_plan_query': (i32, [C.POINTER(LearnerConfig), i32, C.POINTER(i64)]),

@@ -54,6 +54,27 @@ def _acting_rows_error(net, E):
   return None
 
 
+def _acting_randomness(source, seed, per_stream=False, num_streams=1):
+  """The randomness of one act on `source` (a `Learner` or a `learner_lib.Actor`), drawn from its generator with one
+  counter step, as the keyword argument of `Learner.q_values` / `Learner.act_batch` / `Actor.act`: rainbow's own apply
+  per stream (`per_stream`, num_streams of them), IQN's taus or rainbow's one shared apply.  The other kinds act
+  without randomness (fqf proposes its fractions) and draw nothing: {}."""
+  if per_stream:
+    what = 'stream_noise'
+  elif _draws_taus(source.kind):
+    what = 'taus'
+  elif source.kind == 'rainbow':
+    what = 'noise'
+  else:
+    return {}
+  if isinstance(source, learner_lib.Actor):
+    return {what: source.generate_randomness(seed, per_stream=per_stream)}
+  if per_stream:
+    return {what: source.generate_stream_noise(seed, num_streams)}
+  source.generate_randomness(seed)
+  return {what: getattr(source, what)}
+
+
 def _seed_of(rng_key) -> int:
   arr = np.asarray(rng_key).astype(np.uint64).reshape(-1)
   seed = 0
@@ -288,18 +309,15 @@ class _DeviceAgent(parts.Agent):
     else:
       self._obs_dev.copy_(torch.from_numpy(np.ascontiguousarray(obs).reshape(-1)))
     L = self._learner
-    taus = noise = None
     if getattr(self, '_jax_key', None) is not None:
       # iqn/agent.py:220-222: rng_key, sample_key, apply_key, policy_key = split(rng_key, 4); tau_t = uniform(sample_key)
       self._jax_key, sample = jax_prng.iqn_act_keys(self._jax_key)
       self._jax_act.set_keys(sample)
       self._jax_act.launch(L.taus)
-      taus = L.taus
-    elif _draws_taus(self.KIND) or self.KIND == 'rainbow':
-      L.generate_randomness(self._seed)
-      taus = L.taus if _draws_taus(self.KIND) else None
-      noise = L.noise if self.KIND == 'rainbow' else None
-    q = L.q_values(self._obs_dev, taus=taus, noise=noise).cpu().numpy()   # D2H sync, as jax.device_get
+      randomness = {'taus': L.taus}
+    else:
+      randomness = _acting_randomness(L, self._seed)
+    q = L.q_values(self._obs_dev, **randomness).cpu().numpy()   # D2H sync, as jax.device_get
     eps = 0.0 if self.GREEDY else self.exploration_epsilon
     if eps > 0.0 and self._host_rng.uniform() < eps:
       a_t = int(self._host_rng.randint(len(q)))
@@ -668,13 +686,10 @@ class EpsilonGreedyActor(parts.Agent):
     else:
       self._obs_dev.copy_(torch.from_numpy(np.ascontiguousarray(obs).reshape(-1)))
     L = self._learner
-    taus = noise = None
-    if _draws_taus(L.kind) or L.kind == 'rainbow':
-      self._seed += 1
-      L.generate_randomness(self._seed)
-      taus = L.taus if _draws_taus(L.kind) else None
-      noise = L.noise if L.kind == 'rainbow' else None
-    q = L.q_values(self._obs_dev, taus=taus, noise=noise).cpu().numpy()
+    randomness = _acting_randomness(L, self._seed + 1)
+    if randomness:
+      self._seed += 1                       # a new seed for every act that draws
+    q = L.q_values(self._obs_dev, **randomness).cpu().numpy()
     if self._epsilon > 0.0 and self._rng.uniform() < self._epsilon:
       self._action = parts.Action(int(self._rng.randint(len(q))))
     else:
@@ -747,37 +762,25 @@ class BatchedEpsilonGreedyActor:
       eps = float(epsilon)
     else:
       eps = self._epsilon(self._t) if callable(self._epsilon) else float(self._epsilon)
+    actions, self.q_values = self._tick(L if self._actor is None else self._actor, observations, eps)
+    self._t += 1
+    return actions
+
+  def _tick(self, source, observations, eps):
+    """One acting tick of the E streams on `source` (a `Learner`, or a `learner_lib.Actor` for E streams): 2E host
+    uniforms when eps > 0, the kind's acting randomness, the act, one pinned device-to-host copy of the actions and a
+    synchronise.  Returns (host actions, device q-values)."""
     explore = None
     if eps > 0.0:
       self._explore_host.copy_(torch.from_numpy(self._rng.uniform(size=(2, self._E)).astype(np.float32)))
       self._explore_dev.copy_(self._explore_host, non_blocking=True)
       explore = self._explore_dev
-    taus = noise = stream_noise = None
-    kind = L.net.kind
-    if self._actor is not None:
-      if self._per_stream_noise:
-        stream_noise = self._actor.generate_randomness(self._seed, per_stream=True)
-      elif _draws_taus(kind):
-        taus = self._actor.generate_randomness(self._seed)
-      elif kind == 'rainbow':
-        noise = self._actor.generate_randomness(self._seed)
-      actions, self.q_values = self._actor.act(observations, epsilon=eps, explore=explore, taus=taus, noise=noise,
-                                               stream_noise=stream_noise)
-    else:
-      if self._per_stream_noise:
-        stream_noise = L.generate_stream_noise(self._seed, self._E)
-      elif _draws_taus(kind) or kind == 'rainbow':
-        L.generate_randomness(self._seed)
-        if _draws_taus(kind):
-          taus = L.taus[:self._E * L.net.tau_samples_policy] if hasattr(L.net, 'tau_samples_policy') else L.taus
-        else:
-          noise = L.noise
-      actions, self.q_values = L.act_batch(observations, epsilon=eps, explore=explore, taus=taus, noise=noise,
-                                           stream_noise=stream_noise)
+    randomness = _acting_randomness(source, self._seed, self._per_stream_noise, self._E)
+    act = source.act if isinstance(source, learner_lib.Actor) else source.act_batch
+    actions, q = act(observations, epsilon=eps, explore=explore, **randomness)
     self._actions_host.copy_(actions, non_blocking=True)
-    torch.cuda.current_stream().synchronize()
-    self._t += 1
-    return self._actions_host.numpy().copy()
+    torch.cuda.current_stream().synchronize()   # also frees the pinned uniforms for the next tick
+    return self._actions_host.numpy().copy(), q
 
 
 
@@ -1094,6 +1097,8 @@ class VectorEvaluator:
   # the trainer's input checks and episode bookkeeping (they read only _E, _pre and the episode arrays)
   _check = VectorTrainer._check
   _track_episodes = VectorTrainer._track_episodes
+  # the batched actor's acting tick (it reads only _E, _rng, _seed, _per_stream_noise and the staging buffers)
+  _tick = BatchedEpsilonGreedyActor._tick
 
   def __init__(self, network_or_learner, num_streams: int, exploration_epsilon: float, rng_key,
                per_stream_noise: bool = False, preprocessor_kwargs: Optional[Mapping[str, Any]] = None, stream=None):
@@ -1194,24 +1199,7 @@ class VectorEvaluator:
     return self._actions.copy()
 
   def _act(self) -> np.ndarray:
-    A = self._actor
-    explore = None
-    if self._epsilon > 0.0:
-      self._explore_host.copy_(torch.from_numpy(self._rng.uniform(size=(2, self._E)).astype(np.float32)))
-      self._explore_dev.copy_(self._explore_host, non_blocking=True)
-      explore = self._explore_dev
-    taus = noise = stream_noise = None
-    if self._per_stream_noise:
-      stream_noise = A.generate_randomness(self._seed, per_stream=True)
-    elif _draws_taus(self._net.kind):
-      taus = A.generate_randomness(self._seed)
-    elif self._net.kind == 'rainbow':
-      noise = A.generate_randomness(self._seed)
-    actions, _ = A.act(self._pre.stacks, epsilon=self._epsilon, explore=explore, taus=taus, noise=noise,
-                       stream_noise=stream_noise)
-    self._actions_host.copy_(actions, non_blocking=True)
-    torch.cuda.current_stream().synchronize()   # also frees the pinned uniforms for the next tick
-    return self._actions_host.numpy().copy()
+    return self._tick(self._actor, self._pre.stacks, self._epsilon)[0]
 
   def reset(self, streams=None) -> None:
     """`Agent.reset` for every stream, or for one stream or a sequence of streams (e.g. those whose last timestep was

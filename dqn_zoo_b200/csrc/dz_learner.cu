@@ -1608,7 +1608,7 @@ struct dz_learner {
   const uint8_t** rows_sample[2];           // row tables filled by the fused sampler
   uint8_t* recon = nullptr;                 // frame-deduplicated replay: [B][2][obs_stride] stacks the sampled rows
   int64_t recon_bytes = 0;                  //   are rebuilt into (allocated by the first, eager, dz_learner_learn)
-  const uint8_t** rows_act;                 // 1-entry table for q_values
+  const uint8_t** rows_act;                 // [batch] observation row table of the learner's acting
   int32_t* s_a; float *s_r, *s_d, *s_w;     // sampler-produced batch scalars
   float* q_scratch;
   int fc_splits, head_splits, conv_splits, nt_splits;
@@ -2793,7 +2793,7 @@ int launch_loss(const dz_learner_config& c, LossArgs& L, int B, void* stream, Si
 
 // The acting tail of a head pass over E observations: q-values [E][A] (q_values_kernel) and, when `actions` is given,
 // the epsilon-greedy choice (act_select_kernel).  out: the head outputs of the pass (rainbow: the advantage stream),
-// val: rainbow's value stream.  dz_learner_q_values, batched acting, the actor and dz_test_q_values run this function.
+// val: rainbow's value stream.  The acting body (the learner's and the actor's) and dz_test_q_values run this function.
 // fqf: `frac_w` holds the interval weights [E][N] of the pass's proposals (q_values_fqf_kernel).
 int launch_q_values(const dz_learner_config& c, int E, const float* out, const float* val, const float* explore, float epsilon,
                     float* q, int32_t* actions, void* stream, const float* frac_w = nullptr) {
@@ -2809,6 +2809,72 @@ int launch_q_values(const dz_learner_config& c, int E, const float* out, const f
   if (actions)
     DZ_LAUNCH(act_select_kernel, (unsigned)ceil_div(E, 128), 128, 0, stream, (const float*)q, c.num_actions, E, explore, epsilon,
               actions);
+  return DZ_OK;
+}
+
+// What one act reads and writes.  The learner's acting fills it with its own fp32 buffers (split-K up to 32 rows), its
+// row table and fqf buffers, and no plan; an actor with buffers sized for its streams and, where the geometry allows,
+// its forward-only tensor-core plan.
+struct ActTarget {
+  dz_learner* l;              // configuration, layout, offsets, dims and split counts (a frozen actor's: shape only)
+  const float* params;        // the online blob or a frozen snapshot
+  NetBufs nb;                 // activation set / head pass 1
+  const uint8_t** rows;       // [E] observation row table
+  UmNet* um;                  // forward-only tensor-core plan (nullptr: fp32-FMA torso)
+  bool pack;                  // pack the plan's weight images on every act (a live actor; frozen: packed by load_params)
+  float* noise;               // rainbow on the plan: the copy of the caller's shared apply that noisy1 reads
+  float *frac_hat, *frac_w;   // fqf: the acting pass's tau_hat and interval weights, [E][N] each
+};
+
+// The acting body of dz_learner_act_batch and dz_actor_act: row table, torso, heads by kind, q-values and, when
+// d_actions is given, the epsilon-greedy choice.
+int act(const ActTarget& t, int E, const uint8_t* d_obs, const float* d_taus, const float* d_noise, int64_t noise_ld,
+        const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
+  dz_learner* l = t.l;
+  const dz_learner_config& c = l->cfg;
+  const bool rb = c.kind == DZ_RAINBOW;
+  if (!d_obs || !d_q_out) return fail(DZ_EINVAL, "act: null buffer");
+  if (draws_taus(c.kind) && !d_taus) return fail(DZ_EINVAL, "iqn acting needs taus[E][tau_samples_policy]");
+  if (rb && !d_noise) return fail(DZ_EINVAL, "rainbow acting needs noise");
+  const int64_t stride = rb ? noise_layout(c, l->d).stride : 0;
+  if (noise_ld != 0 && (!rb || noise_ld != stride))
+    return fail(DZ_EINVAL, "act: noise_ld must be 0 (one shared apply) or the noise stride (rainbow, one apply per stream)");
+  const float* on = t.params;
+  const long long obs_bytes = (long long)l->d.H * l->d.W * l->d.C;
+  DZ_LAUNCH(make_row_table_kernel, (unsigned)ceil_div(E, 64), 64, 0, stream, d_obs, obs_bytes, E, t.rows);
+  const bool fc_done = t.um && !uses_iqn_net(c.kind) && noise_ld == 0;
+  if (t.um) {
+    const uint8_t* const* rows[3] = {t.rows, nullptr, nullptr};
+    if (t.pack) DZ_TRY(um_pack_weights(t.um, stream));
+    DZ_TRY(um_forward_torso(t.um, rows, stream));
+    if (fc_done) {
+      if (rb) DZ_CUDA_OK(cudaMemcpyAsync(t.noise, d_noise, stride * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+      DZ_TRY(um_forward_fc(t.um, t.noise, stream));
+    }
+  } else {
+    TorsoJob job{on, t.rows, 1};   // activation set 1, so a pending backward's set-0 buffers stay intact
+    DZ_TRY(forward_torso(l, t.nb, &job, 1, E, stream));
+  }
+  Pass pass{on, 1, 1, 0};
+  if (proposes_fractions(c.kind)) {
+    DZ_TRY(fqf_act_heads(l, t.nb, on, E, t.frac_hat, t.frac_w, stream));
+  } else if (uses_iqn_net(c.kind)) {
+    const float* taus[1] = {d_taus};
+    DZ_TRY(forward_heads_iqn(l, t.nb, &pass, 1, E, taus, false, stream));
+  } else if (rb) {
+    DZ_TRY(forward_heads_rainbow(l, t.nb, &pass, 1, E, d_noise, stream, fc_done, noise_ld));
+  } else {
+    DZ_TRY(forward_heads_plain(l, t.nb, &pass, 1, E, stream, fc_done));
+  }
+  return launch_q_values(c, E, t.nb.out[1], t.nb.outv[1], d_explore, epsilon, d_q_out, d_actions, stream, t.frac_w);
+}
+
+// One draw of acting randomness: n floats from the generator of dz_learner_generate_randomness (Philox keyed by element
+// index, counter counters[1] and the stream id of its taus or of its noise), then one counter step.
+int launch_acting_draw(float* d_out, long long n, bool taus, uint64_t seed, int64_t* counters, void* stream) {
+  DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_out, n, seed, counters, taus ? 0 : 1,
+            taus ? 1u : 2u);
+  DZ_LAUNCH(bump_counter_kernel, 1, 1, 0, stream, counters, 1);
   return DZ_OK;
 }
 
@@ -3075,7 +3141,7 @@ int dz_learner_learn(dz_learner* l, const dz_replay_view* replay, int32_t priori
 
 // Same as dz_learner_generate_randomness, but enqueued on the learner's side stream (when it has one): the draws do not
 // depend on the sampled batch, so they run beside the sampler instead of in front of it.  Ordered after everything already
-// enqueued on `stream` and before the next dz_learner_learn / dz_learner_update / dz_learner_q_values on `stream`; any
+// enqueued on `stream` and before the next dz_learner_learn / dz_learner_update / dz_learner_act_batch on `stream`; any
 // other consumer of the buffers must synchronise the device first.
 int dz_learner_generate_randomness_async(dz_learner* l, uint64_t seed, float* d_taus, float* d_noise, void* stream) {
   return dz_learner_generate_randomness(l, seed, d_taus, d_noise, l->side.fork(stream, stream));
@@ -3095,79 +3161,16 @@ int dz_learner_generate_randomness(dz_learner* l, uint64_t seed, float* d_taus, 
   return DZ_OK;
 }
 
-int dz_learner_q_values(dz_learner* l, const uint8_t* d_obs, const float* d_taus, const float* d_noise, float* d_q_out, void* stream) {
-  const dz_learner_config& c = l->cfg;
-  const float* on = l->buf.d_online;
-  DZ_TRY(l->side.join(stream));   // pending side-stream work (asynchronous randomness)
-  DZ_LAUNCH(make_row_table_kernel, 1, 32, 0, stream, d_obs, (long long)0, 1, l->rows_act);
-  TorsoJob job{on, l->rows_act, 1};   // use activation set 1 so a pending backward's set-0 buffers stay intact
-  DZ_TRY(forward_torso(l, learner_bufs(l), &job, 1, 1, stream));
-  Pass pass{on, 1, 1, 0};
-  if (proposes_fractions(c.kind)) {
-    DZ_TRY(fqf_act_heads(l, learner_bufs(l), on, 1, l->fq_act_hat, l->fq_act_w, stream));
-  } else if (uses_iqn_net(c.kind)) {
-    if (!d_taus) return fail(DZ_EINVAL, "iqn q_values needs taus[tau_samples_policy]");
-    const float* taus[1] = {d_taus};
-    DZ_TRY(forward_heads_iqn(l, learner_bufs(l), &pass, 1, 1, taus, false, stream));
-  } else if (c.kind == DZ_RAINBOW) {
-    if (!d_noise) return fail(DZ_EINVAL, "rainbow q_values needs one apply of noise");
-    DZ_TRY(forward_heads_rainbow(l, learner_bufs(l), &pass, 1, 1, d_noise, stream));
-  } else {
-    DZ_TRY(forward_heads_plain(l, learner_bufs(l), &pass, 1, 1, stream));
-  }
-  return launch_q_values(c, 1, l->out[1], l->outv[1], nullptr, 0.f, d_q_out, nullptr, stream, l->fq_act_w);
-}
-
 // Batched acting (parts.py:342-411 with many actors; dqn/agent.py:121-131,169-177): online forward on E <= batch observations
 // in one enqueue, q-values [E][A], and the epsilon-greedy choice on the device — one D2H of E actions per tick instead of a
-// D2H sync per decision.  d_obs: E contiguous observations (H*W*C bytes each).  d_explore: [2][E] uniforms in [0,1) or
-// NULL (greedy): action = u0 < epsilon ? floor(u1 * A) : argmax (first maximum, as np.argmax).  IQN: d_taus is
-// [E][tau_samples_policy]; rainbow: ONE noise apply shared by the E streams of the tick, so the streams explore in
-// lockstep.  dz_learner_act_batch_stream_noise gives stream e its own apply, as the reference's actors each draw their own.
-namespace {
-int act_batch_impl(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* d_taus, const float* d_noise, long long noise_ld,
-                   const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
-  const dz_learner_config& c = l->cfg;
-  const float* on = l->buf.d_online;
-  if (E < 1 || E > l->B) return fail(DZ_EINVAL, "act_batch: 1 <= E <= learner batch");
-  if (!d_obs || !d_q_out || !d_actions) return fail(DZ_EINVAL, "act_batch: null buffer");
-  DZ_TRY(l->side.join(stream));
-  const long long obs_bytes = (long long)l->d.H * l->d.W * l->d.C;
-  DZ_LAUNCH(make_row_table_kernel, (unsigned)ceil_div(E, 64), 64, 0, stream, d_obs, obs_bytes, (int)E, l->rows_act);
-  TorsoJob job{on, l->rows_act, 1};
-  DZ_TRY(forward_torso(l, learner_bufs(l), &job, 1, E, stream));
-  Pass pass{on, 1, 1, 0};
-  if (proposes_fractions(c.kind)) {
-    DZ_TRY(fqf_act_heads(l, learner_bufs(l), on, E, l->fq_act_hat, l->fq_act_w, stream));
-  } else if (uses_iqn_net(c.kind)) {
-    if (!d_taus) return fail(DZ_EINVAL, "iqn act_batch needs taus[E][tau_samples_policy]");
-    const float* taus[1] = {d_taus};
-    DZ_TRY(forward_heads_iqn(l, learner_bufs(l), &pass, 1, E, taus, false, stream));
-  } else if (c.kind == DZ_RAINBOW) {
-    if (!d_noise) return fail(DZ_EINVAL, "rainbow act_batch needs one apply of noise");
-    DZ_TRY(forward_heads_rainbow(l, learner_bufs(l), &pass, 1, E, d_noise, stream, false, noise_ld));
-  } else {
-    DZ_TRY(forward_heads_plain(l, learner_bufs(l), &pass, 1, E, stream));
-  }
-  return launch_q_values(c, E, l->out[1], l->outv[1], d_explore, epsilon, d_q_out, d_actions, stream, l->fq_act_w);
-}
-}  // namespace
-
+// D2H sync per decision.  E = 1 with d_actions NULL is select_action's network half.
 int dz_learner_act_batch(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* d_taus, const float* d_noise,
-                         const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
-  return act_batch_impl(l, d_obs, E, d_taus, d_noise, 0, d_explore, epsilon, d_q_out, d_actions, stream);
-}
-
-// Rainbow only: stream e's forward uses noise apply e of d_noise ([E][noise stride], dz_learner_noise_stride), so each
-// stream explores with its own draw as in the reference.  Stream e gets exactly what dz_learner_act_batch gives it
-// when every stream carries that apply: the per-row kernels form the weights in the same order over the same splits.
-int dz_learner_act_batch_stream_noise(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* d_noise,
-                                      const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
-  if (l->cfg.kind != DZ_RAINBOW) return fail(DZ_EINVAL, "act_batch_stream_noise: only rainbow has noisy layers");
-  if (E < 1 || E > l->B) return fail(DZ_EINVAL, "act_batch_stream_noise: 1 <= E <= learner batch");
-  if (!d_noise) return fail(DZ_EINVAL, "act_batch_stream_noise needs noise[E][stride]");
-  return act_batch_impl(l, d_obs, E, nullptr, d_noise, noise_layout(l->cfg, l->d).stride, d_explore, epsilon, d_q_out,
-                        d_actions, stream);
+                         int64_t noise_ld, const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions,
+                         void* stream) {
+  if (E < 1 || E > l->B) return fail(DZ_EINVAL, "act_batch: 1 <= E <= learner batch");
+  DZ_TRY(l->side.join(stream));   // pending side-stream work (asynchronous randomness)
+  const ActTarget t{l, l->buf.d_online, learner_bufs(l), l->rows_act, nullptr, false, nullptr, l->fq_act_hat, l->fq_act_w};
+  return act(t, E, d_obs, d_taus, d_noise, noise_ld, d_explore, epsilon, d_q_out, d_actions, stream);
 }
 
 int dz_learner_noise_stride(const dz_learner_config* cfg, int64_t* out) {
@@ -3177,17 +3180,14 @@ int dz_learner_noise_stride(const dz_learner_config* cfg, int64_t* out) {
   return DZ_OK;
 }
 
-// E noise applies for dz_learner_act_batch_stream_noise: the generator of dz_learner_generate_randomness (Philox keyed by
-// element index, counter d_counters[1] and stream id 2) over E * stride floats, so the first three applies equal what that
-// call writes for the same seed and counter.  Advances the counter once.
+// E noise applies for dz_learner_act_batch's per-stream noise: the generator of dz_learner_generate_randomness over
+// E * stride floats, so the first three applies equal what that call writes for the same seed and counter.  Advances
+// the counter once.
 int dz_learner_generate_stream_noise(dz_learner* l, uint64_t seed, int32_t E, float* d_noise, void* stream) {
   if (l->cfg.kind != DZ_RAINBOW) return fail(DZ_EINVAL, "generate_stream_noise: only rainbow has noisy layers");
   if (E < 1 || E > l->B) return fail(DZ_EINVAL, "generate_stream_noise: 1 <= E <= learner batch");
   if (!d_noise) return fail(DZ_EINVAL, "generate_stream_noise: null buffer");
-  const long long n = (long long)E * noise_layout(l->cfg, l->d).stride;
-  DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_noise, n, seed, l->buf.d_counters, 1, 2u);
-  DZ_LAUNCH(bump_counter_kernel, 1, 1, 0, stream, l->buf.d_counters, 1);
-  return DZ_OK;
+  return launch_acting_draw(d_noise, (long long)E * noise_layout(l->cfg, l->d).stride, false, seed, l->buf.d_counters, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -3411,45 +3411,11 @@ int dz_actor_set_counter(dz_actor* a, int64_t value, void* stream) {
 int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const float* d_noise, int64_t noise_ld,
                  const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
   if (!a) return fail(DZ_EINVAL, "actor: null handle");
-  dz_learner* l = a->l;
-  const dz_learner_config& c = l->cfg;
-  const int E = a->E;
-  const bool rb = c.kind == DZ_RAINBOW;
-  if (!d_obs || !d_q_out || !d_actions) return fail(DZ_EINVAL, "actor: null buffer");
-  if (draws_taus(c.kind) && !d_taus) return fail(DZ_EINVAL, "iqn actor needs taus[E][tau_samples_policy]");
-  if (rb && !d_noise) return fail(DZ_EINVAL, "rainbow actor needs noise");
-  const int64_t stride = rb ? noise_layout(c, l->d).stride : 0;
-  if (noise_ld != 0 && (!rb || noise_ld != stride))
-    return fail(DZ_EINVAL, "actor: noise_ld must be 0 (one shared apply) or the noise stride (rainbow, one apply per stream)");
+  if (!d_actions) return fail(DZ_EINVAL, "actor: null buffer");
   if (a->frozen && !a->loaded) return fail(DZ_EINVAL, "frozen actor: no parameters loaded (dz_actor_load_params)");
-  const float* on = a->frozen ? a->params : l->buf.d_online;
-  const long long obs_bytes = (long long)l->d.H * l->d.W * l->d.C;
-  DZ_LAUNCH(make_row_table_kernel, (unsigned)ceil_div(E, 64), 64, 0, stream, d_obs, obs_bytes, E, a->rows);
-  const bool fc_done = a->um && !uses_iqn_net(c.kind) && noise_ld == 0;
-  if (a->um) {
-    const uint8_t* const* rows[3] = {a->rows, nullptr, nullptr};
-    if (!a->frozen) DZ_TRY(um_pack_weights(a->um, stream));   // frozen: packed by load_params
-    DZ_TRY(um_forward_torso(a->um, rows, stream));
-    if (fc_done) {
-      if (rb) DZ_CUDA_OK(cudaMemcpyAsync(a->noise, d_noise, stride * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-      DZ_TRY(um_forward_fc(a->um, a->noise, stream));
-    }
-  } else {
-    TorsoJob job{on, a->rows, 1};
-    DZ_TRY(forward_torso(l, a->b, &job, 1, E, stream));
-  }
-  Pass pass{on, 1, 1, 0};
-  if (proposes_fractions(c.kind)) {
-    DZ_TRY(fqf_act_heads(l, a->b, on, E, a->frac_hat, a->frac_w, stream));
-  } else if (uses_iqn_net(c.kind)) {
-    const float* taus[1] = {d_taus};
-    DZ_TRY(forward_heads_iqn(l, a->b, &pass, 1, E, taus, false, stream));
-  } else if (rb) {
-    DZ_TRY(forward_heads_rainbow(l, a->b, &pass, 1, E, d_noise, stream, fc_done, noise_ld));
-  } else {
-    DZ_TRY(forward_heads_plain(l, a->b, &pass, 1, E, stream, fc_done));
-  }
-  return launch_q_values(c, E, a->b.out[1], a->b.outv[1], d_explore, epsilon, d_q_out, d_actions, stream, a->frac_w);
+  const ActTarget t{a->l, a->frozen ? a->params : a->l->buf.d_online, a->b, a->rows, a->um, !a->frozen, a->noise,
+                    a->frac_hat, a->frac_w};
+  return act(t, a->E, d_obs, d_taus, d_noise, noise_ld, d_explore, epsilon, d_q_out, d_actions, stream);
 }
 
 // The actor's randomness from the learner's generator and counter: iqn taus [E][tau_samples_policy] (the stream id of
@@ -3464,12 +3430,7 @@ int dz_actor_generate_randomness(dz_actor* a, uint64_t seed, int32_t per_stream,
   if (iqn && !per_stream) n = (long long)a->E * c.tau_samples_policy;
   else if (c.kind == DZ_RAINBOW) n = (per_stream ? (long long)a->E : 1LL) * noise_layout(c, a->l->d).stride;
   else return fail(DZ_EINVAL, "actor randomness: iqn draws taus, rainbow noise (per_stream: rainbow only); other kinds draw nothing");
-  const int kind = iqn ? 0 : 1;
-  int64_t* counters = a->frozen ? a->counters : a->l->buf.d_counters;
-  DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_out, n, seed, counters, kind,
-            iqn ? 1u : 2u);
-  DZ_LAUNCH(bump_counter_kernel, 1, 1, 0, stream, counters, 1);
-  return DZ_OK;
+  return launch_acting_draw(d_out, n, iqn, seed, a->frozen ? a->counters : a->l->buf.d_counters, stream);
 }
 
 // Test hook: the MMA path of the actor's tensor-core launch `tag` (the tags of dz_test_learner_mma_path's torso and fc

@@ -129,6 +129,32 @@ def _cstream():
   return torch.cuda.current_stream().cuda_stream
 
 
+def _f32(x, device):
+  """`x` as a contiguous float32 tensor on `device`; None stays None."""
+  return None if x is None else torch.as_tensor(x, device=device).to(torch.float32).contiguous()
+
+
+def _ptr(t):
+  return 0 if t is None else t.data_ptr()
+
+
+def _act_inputs(owner, E, explore, taus, noise, stream_noise):
+  """The exploration and randomness inputs of one act of E streams on `owner` (a `Learner` or an `Actor`) as device
+  tensors: (explore, taus, noise, noise_ld).  `stream_noise` is rainbow's [E, noise_stride] block whose row e is stream
+  e's own apply; it replaces noise / taus and sets noise_ld to the stride (0: one apply shared by the streams)."""
+  x = _f32(explore, owner.device)
+  if stream_noise is None:
+    return x, _f32(taus, owner.device), _f32(noise, owner.device), 0
+  if noise is not None or taus is not None:
+    raise ValueError('stream_noise replaces noise / taus')
+  if owner.kind != 'rainbow':
+    raise ValueError('stream_noise needs a rainbow learner')
+  n = _f32(stream_noise, owner.device)
+  if n.dim() != 2 or n.shape[0] != E or n.shape[1] != owner.noise_stride:
+    raise ValueError('stream_noise must be [E, noise_stride] = [%d, %d], got %s' % (E, owner.noise_stride, tuple(n.shape)))
+  return x, None, n, owner.noise_stride
+
+
 class Learner:
   """Device-resident parameters, optimizer state and workspace + the fused update."""
 
@@ -330,10 +356,9 @@ class Learner:
   def q_values(self, obs_u8: torch.Tensor, taus=None, noise=None) -> torch.Tensor:
     """Online-network Q-values for one observation (the network half of select_action)."""
     obs = torch.as_tensor(obs_u8, device=self.device).contiguous().view(-1)
-    t = None if taus is None else torch.as_tensor(taus, device=self.device).to(torch.float32).contiguous()
-    n = None if noise is None else torch.as_tensor(noise, device=self.device).to(torch.float32).contiguous()
-    _lib.call('dz_learner_q_values', self._h, obs.data_ptr(), 0 if t is None else t.data_ptr(),
-              0 if n is None else n.data_ptr(), self.q_out.data_ptr(), _cstream())
+    t, n = _f32(taus, self.device), _f32(noise, self.device)
+    _lib.call('dz_learner_act_batch', self._h, obs.data_ptr(), 1, _ptr(t), _ptr(n), 0, 0, 0.0, self.q_out.data_ptr(), 0,
+              _cstream())
     self._keep_q = (obs, t, n)
     return self.q_out[:self.net.num_actions]
 
@@ -348,22 +373,9 @@ class Learner:
     if not hasattr(self, '_act_q') or self._act_q.shape[0] < E:
       self._act_q = torch.zeros((self.batch_size, self.net.num_actions), dtype=torch.float32, device=self.device)
       self._act_a = torch.zeros(self.batch_size, dtype=torch.int32, device=self.device)
-    x = None if explore is None else torch.as_tensor(explore, device=self.device).to(torch.float32).contiguous()
-    if stream_noise is not None:
-      if noise is not None or taus is not None:
-        raise ValueError('stream_noise replaces noise / taus')
-      n = torch.as_tensor(stream_noise, device=self.device).to(torch.float32).contiguous()
-      if n.dim() != 2 or n.shape[0] != E or n.shape[1] != self.noise_stride:
-        raise ValueError('stream_noise must be [E, noise_stride] = [%d, %d], got %s' % (E, self.noise_stride, tuple(n.shape)))
-      _lib.call('dz_learner_act_batch_stream_noise', self._h, obs.data_ptr(), E, n.data_ptr(),
-                0 if x is None else x.data_ptr(), float(epsilon), self._act_q.data_ptr(), self._act_a.data_ptr(), _cstream())
-      self._keep_act = (obs, n, x)
-      return self._act_a[:E], self._act_q[:E]
-    t = None if taus is None else torch.as_tensor(taus, device=self.device).to(torch.float32).contiguous()
-    n = None if noise is None else torch.as_tensor(noise, device=self.device).to(torch.float32).contiguous()
-    _lib.call('dz_learner_act_batch', self._h, obs.data_ptr(), E, 0 if t is None else t.data_ptr(),
-              0 if n is None else n.data_ptr(), 0 if x is None else x.data_ptr(), float(epsilon), self._act_q.data_ptr(),
-              self._act_a.data_ptr(), _cstream())
+    x, t, n, noise_ld = _act_inputs(self, E, explore, taus, noise, stream_noise)
+    _lib.call('dz_learner_act_batch', self._h, obs.data_ptr(), E, _ptr(t), _ptr(n), noise_ld, _ptr(x), float(epsilon),
+              self._act_q.data_ptr(), self._act_a.data_ptr(), _cstream())
     self._keep_act = (obs, t, n, x)
     return self._act_a[:E], self._act_q[:E]
 
@@ -558,31 +570,14 @@ class Actor:
                                                                   tuple(obs.shape)))
     if self.frozen and not self.loaded:
       raise RuntimeError('the frozen actor has no parameters: call load_params first')
-    x = None if explore is None else torch.as_tensor(explore, device=L.device).to(torch.float32).contiguous()
+    x, t, n, noise_ld = _act_inputs(self, E, explore, taus, noise, stream_noise)
     if x is not None and x.numel() != 2 * E:
       raise ValueError('explore must be [2, %d], got %s' % (E, tuple(x.shape)))
-    t = n = None
-    noise_ld = 0
-    if stream_noise is not None:
-      if noise is not None or taus is not None:
-        raise ValueError('stream_noise replaces noise / taus')
-      if L.kind != 'rainbow':
-        raise ValueError('stream_noise needs a rainbow learner')
-      n = torch.as_tensor(stream_noise, device=L.device).to(torch.float32).contiguous()
-      if n.dim() != 2 or n.shape[0] != E or n.shape[1] != L.noise_stride:
-        raise ValueError('stream_noise must be [E, noise_stride] = [%d, %d], got %s' % (E, L.noise_stride, tuple(n.shape)))
-      noise_ld = L.noise_stride
-    else:
-      if taus is not None:
-        t = torch.as_tensor(taus, device=L.device).to(torch.float32).contiguous()
-        if draws_taus(L.kind) and t.numel() != E * L.net.tau_samples_policy:
-          raise ValueError('taus must be [%d, %d], got %s' % (E, L.net.tau_samples_policy, tuple(t.shape)))
-      if noise is not None:
-        n = torch.as_tensor(noise, device=L.device).to(torch.float32).contiguous()
-        if L.kind == 'rainbow' and n.numel() < L.noise_stride:
-          raise ValueError('noise must hold one apply (%d floats), got %d' % (L.noise_stride, n.numel()))
-    _lib.call('dz_actor_act', self._h, obs.data_ptr(), 0 if t is None else t.data_ptr(), 0 if n is None else n.data_ptr(),
-              noise_ld, 0 if x is None else x.data_ptr(), float(epsilon), self.q.data_ptr(), self.actions.data_ptr(),
-              _cstream())
+    if t is not None and draws_taus(L.kind) and t.numel() != E * L.net.tau_samples_policy:
+      raise ValueError('taus must be [%d, %d], got %s' % (E, L.net.tau_samples_policy, tuple(t.shape)))
+    if noise_ld == 0 and n is not None and L.kind == 'rainbow' and n.numel() < L.noise_stride:
+      raise ValueError('noise must hold one apply (%d floats), got %d' % (L.noise_stride, n.numel()))
+    _lib.call('dz_actor_act', self._h, obs.data_ptr(), _ptr(t), _ptr(n), noise_ld, _ptr(x), float(epsilon), self.q.data_ptr(),
+              self.actions.data_ptr(), _cstream())
     self._keep = (obs, t, n, x)
     return self.actions, self.q

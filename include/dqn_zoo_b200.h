@@ -429,37 +429,32 @@ int dz_learner_learn(dz_learner* l, const dz_replay_view* replay, int32_t priori
  * sign(n)*sqrt(|n|), n ~ TruncNormal(-2,2) (networks.py:142-144).  NOT the JAX threefry stream. */
 int dz_learner_generate_randomness(dz_learner* l, uint64_t seed, float* d_taus, float* d_noise, void* stream);
 /* Same draws, enqueued on the learner's side stream: ordered after the work already on `stream` and before the next
- * dz_learner_learn / dz_learner_update / dz_learner_q_values on `stream` (they run beside the sampler instead of in
+ * dz_learner_learn / dz_learner_update / dz_learner_act_batch on `stream` (they run beside the sampler instead of in
  * front of it).  Any other reader of d_taus / d_noise must synchronise the device first. */
 int dz_learner_generate_randomness_async(dz_learner* l, uint64_t seed, float* d_taus, float* d_noise, void* stream);
 
-/* select_action's network part (dqn/agent.py:121-131; rainbow/agent.py:125-133; iqn/agent.py:228-243):
- * online forward on ONE observation -> q_values[num_actions] on device.  The epsilon-greedy draw stays on the host. */
-int dz_learner_q_values(dz_learner* l, const uint8_t* d_obs, const float* d_taus, const float* d_noise,
-                        float* d_q_out, void* stream);
-
 /* Batched acting for E <= batch independent environment streams (parts.py:342-411 run over many actors;
  * dqn/agent.py:121-131,169-177): online forward on E observations in one enqueue, q-values [E][num_actions] and the
- * epsilon-greedy choice on the device, so a tick costs ONE device-to-host copy of E int32 actions.
+ * epsilon-greedy choice on the device, so a tick costs ONE device-to-host copy of E int32 actions.  E = 1 with
+ * d_actions NULL is select_action's network part (rainbow/agent.py:125-133; iqn/agent.py:228-243), the epsilon-greedy
+ * draw left to the host.
  *   d_obs      E contiguous uint8 observations (obs_h*obs_w*obs_c bytes each), device memory
- *   d_taus     iqn: [E][tau_samples_policy] (fqf: NULL, its fractions are proposed from the torso features);  d_noise  rainbow: one noise apply, shared by the E streams of the tick
- *              (the streams explore in lockstep; dz_learner_act_batch_stream_noise gives each stream its own apply)
+ *   d_taus     iqn: [E][tau_samples_policy] (fqf: NULL, its fractions are proposed from the torso features)
+ *   d_noise    rainbow: noise_ld = 0, ONE apply shared by the E streams of the tick (they explore in lockstep);
+ *              noise_ld = dz_learner_noise_stride, [E][stride] and stream e uses apply e (rainbow/agent.py:125-133 run
+ *              by E actors, each drawing its own noise).  When every row carries the same apply the q-values and
+ *              actions equal the shared mode's bit for bit.  Other kinds: noise_ld = 0.
  *   d_explore  [2][E] float32 uniforms in [0,1) (device) or NULL for greedy acting:
- *              action = u0[e] < epsilon ? min(floor(u1[e] * num_actions), num_actions - 1) : first argmax of q[e] */
+ *              action = u0[e] < epsilon ? min(floor(u1[e] * num_actions), num_actions - 1) : first argmax of q[e]
+ *   d_actions  [E] int32, or NULL for q-values only
+ * DZ_EINVAL for E outside [1, batch], a NULL d_obs / d_q_out, missing taus / noise or another noise_ld. */
 int dz_learner_act_batch(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* d_taus, const float* d_noise,
-                         const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream);
+                         int64_t noise_ld, const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions,
+                         void* stream);
 
-/* Rainbow batched acting with one noise apply per stream (rainbow/agent.py:125-133 run by E actors, each drawing its own
- * noise): as dz_learner_act_batch, but stream e's noisy layers use apply e of d_noise, which is [E][stride] floats with
- * stride from dz_learner_noise_stride.  When every row carries the same apply, the q-values and actions equal
- * dz_learner_act_batch's with that apply bit for bit.  DZ_EINVAL for a non-rainbow learner, E outside [1, batch] or a
- * NULL buffer. */
-int dz_learner_act_batch_stream_noise(dz_learner* l, const uint8_t* d_obs, int32_t E, const float* d_noise,
-                                      const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions,
-                                      void* stream);
 /* Floats of ONE rainbow noise apply (the 8 factorised-noise vectors, each padded to 4 floats); DZ_EINVAL for other kinds. */
 int dz_learner_noise_stride(const dz_learner_config* cfg, int64_t* out);
-/* E noise applies ([E][stride] floats) for dz_learner_act_batch_stream_noise from the generator of
+/* E noise applies ([E][stride] floats) for dz_learner_act_batch's per-stream noise from the generator of
  * dz_learner_generate_randomness (same seed and counter: the first min(E, 3) applies equal what it writes); advances
  * d_counters[1] once.  DZ_EINVAL for a non-rainbow learner, E outside [1, batch] or a NULL buffer. */
 int dz_learner_generate_stream_noise(dz_learner* l, uint64_t seed, int32_t E, float* d_noise, void* stream);

@@ -1,4 +1,4 @@
-"""GPU: rainbow batched acting with one noise apply per actor stream (`dz_learner_act_batch_stream_noise`,
+"""GPU: rainbow batched acting with one noise apply per actor stream (`dz_learner_act_batch` with noise_ld = stride,
 `Learner.act_batch(..., stream_noise=...)`, `Learner.generate_stream_noise`, `BatchedEpsilonGreedyActor(per_stream_noise=True)`)
 against the shared-noise mode, the single-observation path and the float64 oracle."""
 
@@ -154,7 +154,7 @@ def test_actor_with_per_stream_noise_explores_each_stream_independently():
   assert a3.min() >= 0 and a3.max() < A
 
 
-def test_errors_raise_value_error_through_the_shim():
+def test_per_stream_errors_raise_value_error_through_act_batch():
   from dqn_zoo_b200 import _lib
   from dqn_zoo_b200 import agent as agent_lib
   from dqn_zoo_b200 import learner as dl
@@ -166,11 +166,11 @@ def test_errors_raise_value_error_through_the_shim():
   act = torch.zeros(B + 1, dtype=torch.int32, device='cuda')
   stream = torch.cuda.current_stream().cuda_stream
 
-  def call(h, E, noise_ptr):
-    _lib.call('dz_learner_act_batch_stream_noise', h, obs.data_ptr(), E, noise_ptr, 0, 0.0, q.data_ptr(), act.data_ptr(),
-              stream)
+  def call(h, E, noise_ptr, noise_ld=S, actions=act.data_ptr()):
+    _lib.call('dz_learner_act_batch', h, obs.data_ptr(), E, 0, noise_ptr, noise_ld, 0, 0.0, q.data_ptr(), actions, stream)
 
   call(L._h, 3, noise.data_ptr())                  # valid call for reference
+  call(L._h, 3, noise.data_ptr(), actions=0)       # q-values only
   for E in (0, B + 1):
     with pytest.raises(ValueError):
       call(L._h, E, noise.data_ptr())
@@ -178,6 +178,8 @@ def test_errors_raise_value_error_through_the_shim():
       _lib.call('dz_learner_generate_stream_noise', L._h, 1, E, noise.data_ptr(), stream)
   with pytest.raises(ValueError):
     call(L._h, 3, 0)
+  with pytest.raises(ValueError):
+    call(L._h, 3, noise.data_ptr(), noise_ld=S + 4)   # neither one shared apply nor one per stream
   with pytest.raises(ValueError):
     _lib.call('dz_learner_generate_stream_noise', L._h, 1, 3, 0, stream)
   with pytest.raises(ValueError):
