@@ -59,7 +59,7 @@ class LearnerConfig(C.Structure):
               ('huber_param', f32), ('optimizer', i32), ('learning_rate', f32), ('opt_eps', f32), ('rms_decay', f32),
               ('adam_b1', f32), ('adam_b2', f32), ('max_global_grad_norm', f32), ('munchausen_alpha', f32),
               ('entropy_temperature', f32), ('log_policy_clip', f32), ('num_fractions', i32),
-              ('fraction_learning_rate', f32), ('fraction_opt_eps', f32), ('fraction_rms_decay', f32)]
+              ('fraction_learning_rate', f32), ('fraction_opt_eps', f32), ('fraction_rms_decay', f32), ('dueling', i32)]
 
   def __init__(self, **fields):
     # the loss hyperparameters start at the reference's values instead of 0, which the library rejects for vmax, and
@@ -206,6 +206,7 @@ _SIGNATURES = {
     'dz_test_munchausen_example': (i32, [vp, vp, vp, i32, i32, f32, f32, f32, f32, f32, vp]),
     'dz_test_munchausen_iqn_example': (i32, [vp, vp, i32, i32, i32, i32, f32, f32, f32, f32, f32, vp]),
     'dz_test_fqf_example': (i32, [vp, vp, vp, i32, f32, vp]),
+    'dz_test_dueling_example': (i32, [vp, f32, vp, i32, vp]),
     'dz_test_loss': (i32, [C.POINTER(LearnerConfig), i32, C.POINTER(vp), C.POINTER(vp), vp, vp, vp, vp, vp, vp, vp, vp, vp,
                            vp, vp, vp, vp]),
     'dz_test_q_values': (i32, [C.POINTER(LearnerConfig), i32, vp, vp, vp, f32, vp, vp, vp]),

@@ -250,7 +250,8 @@ class _DeviceAgent(parts.Agent):
         t = t.clone()
         held.append(t)
       blobs[name] = t
-    state = {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'param_count': L.plan.param_count,
+    state = {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'dueling': bool(L.net.dueling),
+             'param_count': L.plan.param_count,
              'opt_state_floats': L.plan.opt_state_floats, 'host_rng': self._host_rng.get_state(), 'seed': self._seed,
              'jax_key': None if getattr(self, '_jax_key', None) is None else self._jax_key.copy(),
              'frame_t': self._frame_t}
@@ -279,8 +280,10 @@ class _DeviceAgent(parts.Agent):
     except (OSError, pickle.UnpicklingError, EOFError) as e:
       raise ValueError('%s is not a readable agent checkpoint: %s' % (directory, e)) from e
     L = self._learner
-    ck.validate(state, {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND,
-                        'param_count': L.plan.param_count, 'opt_state_floats': L.plan.opt_state_floats}, directory)
+    # checkpoints written before the dueling network existed have no 'dueling' key: they hold the plain network
+    ck.validate(dict({'dueling': False}, **state),
+                {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'dueling': bool(L.net.dueling),
+                 'param_count': L.plan.param_count, 'opt_state_floats': L.plan.opt_state_floats}, directory)
     blobs = {}
     for name in self._CHECKPOINT_BLOBS:
       path = os.path.join(directory, name + '.npy')

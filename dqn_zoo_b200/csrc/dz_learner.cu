@@ -43,6 +43,15 @@ __host__ __device__ constexpr bool uses_dqn_net(int kind) { return kind == DZ_DQ
 constexpr int net_kind(int kind) { return uses_iqn_net(kind) ? DZ_IQN : uses_dqn_net(kind) ? DZ_DQN : kind; }
 // The Munchausen kinds: alpha / tau / l0 are validated, and the target network also applies to s_tm1.
 constexpr bool is_munchausen(int kind) { return kind == DZ_MUNCHAUSEN || kind == DZ_MUNCHAUSEN_IQN; }
+// The kinds that may take the dueling network (DESIGN.md §16): their losses read one scalar q per action.
+constexpr bool dueling_allowed(int kind) {
+  return kind == DZ_DQN || kind == DZ_DOUBLE_Q || kind == DZ_PRIORITIZED || kind == DZ_MUNCHAUSEN;
+}
+// After validate(): the network has two 512-wide streams after the torso (rainbow's noisy pair, the dueling network's
+// plain pair), and its layers are noisy (rainbow).  Every decision about the second stream's buffers, plan and launches
+// asks the first; every decision about noise asks the second.
+inline bool two_streams(const dz_learner_config& c) { return c.kind == DZ_RAINBOW || c.dueling != 0; }
+inline bool noisy_net(const dz_learner_config& c) { return c.kind == DZ_RAINBOW; }
 
 // ------------------------------------------------------------------------------------------------
 // Parameter layout (canonical names; haiku layouts) — must match oracle/learner_oracle.py:param_shapes
@@ -118,6 +127,16 @@ static Layout make_layout(const dz_learner_config& c) {
     }
     return L;
   }
+  if (c.dueling) {   // advantage stream first, as rainbow's, so that stream index s means the same in both networks
+    const char* streams[2] = {"adv", "val"};
+    for (int s = 0; s < 2; ++s) {
+      const std::string p = streams[s];
+      const int64_t n_out = s == 0 ? c.num_actions : 1;
+      L.add(p + "1/w", {d.feat, 512}); L.add(p + "1/b", {512});
+      L.add(p + "2/w", {512, n_out}); L.add(p + "2/b", {n_out});
+    }
+    return L;
+  }
   if (uses_iqn_net(c.kind)) { L.add("embed/w", {c.latent_dim, d.feat}); L.add("embed/b", {d.feat}); }
   L.add("fc1/w", {d.feat, 512}); L.add("fc1/b", {512});
   L.add("head/w", {512, d.out});
@@ -164,6 +183,12 @@ static int param_offsets(const dz_learner_config& c, const Layout& L, ParamOffse
       const std::string p = streams[s];
       o.w1[s] = need(p + "1/mu/w"); o.b1[s] = need(p + "1/mu/b"); o.sw1[s] = need(p + "1/sigma/w"); o.sb1[s] = need(p + "1/sigma/b");
       o.w2[s] = need(p + "2/mu/w"); o.sw2[s] = need(p + "2/sigma/w"); o.sb2[s] = need(p + "2/sigma/b");
+    }
+  } else if (c.dueling) {
+    const char* streams[2] = {"adv", "val"};
+    for (int s = 0; s < 2; ++s) {
+      const std::string p = streams[s];
+      o.w1[s] = need(p + "1/w"); o.b1[s] = need(p + "1/b"); o.w2[s] = need(p + "2/w"); o.b2[s] = need(p + "2/b");
     }
   } else {
     o.w1[0] = need("fc1/w"); o.b1[0] = need("fc1/b");
@@ -285,8 +310,33 @@ __host__ __device__ inline float fqf_weighted_q(const float* z, const float* w, 
   return s;
 }
 
+// ---- Dueling head per-row arithmetic (DESIGN.md §16), shared by dueling_head_fwd_kernel / dueling_head_bwd_kernel and
+// their host twin dz_test_dueling_example.  Both sums run serially in action order; at A = 1 the mean is adv itself, so
+// q = v and dadv = 0 exactly.
+constexpr int kDuelingMaxActions = 64;
+
+// q_a = v + (adv_a - m), m = (sum_a adv_a) / A.  q may alias adv.
+__host__ __device__ inline void dueling_aggregate(const float* adv, float v, int A, float* q) {
+  float s = 0.f;
+  for (int a = 0; a < A; ++a) s += adv[a];
+  const float m = s / (float)A;
+  for (int a = 0; a < A; ++a) q[a] = v + (adv[a] - m);
+}
+
+// The aggregation's transpose: dadv_a = dq_a - (sum_a dq_a) / A; returns dval = sum_a dq_a.  dadv may alias dq.
+__host__ __device__ inline float dueling_transpose(const float* dq, int A, float* dadv) {
+  float s = 0.f;
+  for (int a = 0; a < A; ++a) s += dq[a];
+  const float m = s / (float)A;
+  for (int a = 0; a < A; ++a) dadv[a] = dq[a] - m;
+  return s;
+}
+
 static int validate(const dz_learner_config& c) {
   if (c.kind < 0 || c.kind > DZ_FQF) return fail(DZ_EINVAL, "unknown agent kind");
+  if (c.dueling != 0 && c.dueling != 1) return fail(DZ_EINVAL, "dueling must be 0 or 1");
+  if (c.dueling && !dueling_allowed(c.kind))
+    return fail(DZ_EINVAL, "dueling: only dqn, double_q, prioritized and munchausen take the dueling network");
   if (is_munchausen(c.kind) && !munchausen_params_ok(c.munchausen_alpha, c.entropy_temperature, c.log_policy_clip))
     return fail(DZ_EINVAL, "munchausen needs finite alpha >= 0, entropy_temperature > 0 and log_policy_clip <= 0");
   if (is_munchausen(c.kind) && c.num_actions > kMunchausenMaxActions)
@@ -1517,6 +1567,126 @@ OptKernel optimizer_kernel_for(int kind) {
   return kind == DZ_ADAM ? optimizer_bulk_kernel<DZ_ADAM> : optimizer_bulk_kernel<DZ_RMSPROP_CENTERED>;
 }
 
+// The dueling head of up to three passes (blockIdx.y): one warp per row forms the advantages adv = h1_adv adv2/w +
+// adv2/b and the value v = h1_val val2/w + val2/b, and writes q = dueling_aggregate(adv, v) to out.  Lane l owns the
+// inputs k = l + 32 j (j = 0..15) and sums its 16 terms of each output in j order; an xor butterfly then adds the 32
+// lanes' partials in a fixed order, which leaves every lane with the same bits.  No sum depends on how many rows the
+// launch holds.  The advantages go four at a time, so that the 64 weight loads of four outputs are in flight together
+// (the 8 warps of a block apply the same pass, so its weights are read from L1 after the first row).
+struct DuelingFwdArgs {
+  const float* h1[3][2];    // [rows][512] of each pass's advantage / value stream
+  const float* params[3];   // each pass's parameter blob
+  float* out[3];            // q [rows][A]
+  long long off_w[2], off_b[2];
+  int rows, A;
+};
+
+__device__ __forceinline__ float warp_sum_xor(float s) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  return s;
+}
+
+__global__ void __launch_bounds__(256) dueling_head_fwd_kernel(const __grid_constant__ DuelingFwdArgs h) {
+  dz::pdl_enter();
+  __shared__ float adv_s[8][kDuelingMaxActions];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, p = blockIdx.y, A = h.A;
+  const long long r = (long long)blockIdx.x * 8 + warp;
+  if (r >= h.rows) return;
+  const float* __restrict__ xa = h.h1[p][0] + r * 512;
+  const float* __restrict__ xv = h.h1[p][1] + r * 512;
+  const float* __restrict__ P = h.params[p];
+  const float* __restrict__ Wa = P + h.off_w[0];
+  const float* __restrict__ Wv = P + h.off_w[1];
+  float x[16];
+  float sv = 0.f;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    x[j] = xa[lane + 32 * j];
+    sv = fmaf(xv[lane + 32 * j], Wv[lane + 32 * j], sv);
+  }
+  const float v = warp_sum_xor(sv) + P[h.off_b[1]];
+  for (int a0 = 0; a0 < A; a0 += 4) {
+    const int na = A - a0 < 4 ? A - a0 : 4;
+    float s[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const float* __restrict__ w = Wa + (long long)(lane + 32 * j) * A + a0;
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        if (c < na) s[c] = fmaf(x[j], w[c], s[c]);
+    }
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const float t = warp_sum_xor(s[c]);
+      if (lane == 0 && c < na) adv_s[warp][a0 + c] = t + P[h.off_b[0] + a0 + c];
+    }
+  }
+  __syncwarp();
+  if (lane == 0) dueling_aggregate(adv_s[warp], v, A, adv_s[warp]);
+  __syncwarp();
+  for (int a = lane; a < A; a += 32) h.out[p][r * A + a] = adv_s[warp][a];
+}
+
+// The dueling head's backward of online(s_tm1), one warp per row: dadv and dval from dq (dueling_transpose; dadv
+// overwrites dq in place and dval goes to its own [B] buffer, both for the head weight gradients), then both streams'
+// dh1: dh1_adv = dadv adv2/w^T and dh1_val = dval val2/w^T, each masked by its own h1 > 0.  Lane l owns inputs
+// k = l + 32 j; dh1_adv[k] sums serially over the actions, the 16 inputs of a lane side by side so that their weight
+// loads are in flight together.  With hi / lo set it also writes the tf32 hi/lo pair of both streams that the
+// tensor-core input gradient reads.
+struct DuelingBwdArgs {
+  float* dq;                 // [B][A]: in dq, out dadv
+  float* dval;               // [B]
+  const float* h1[2];        // [B][512] post-ReLU activations of online(s_tm1), the masks
+  const float* W[2];         // adv2/w [512][A], val2/w [512][1] of the online blob
+  float* dh1[2];             // [B][512]
+  float *hi[2], *lo[2];      // optional tf32 images of dh1, same layout
+  int B, A;
+};
+
+__global__ void __launch_bounds__(256) dueling_head_bwd_kernel(const __grid_constant__ DuelingBwdArgs g) {
+  dz::pdl_enter();
+  __shared__ float d_s[8][kDuelingMaxActions + 1];   // per warp: [0, A) dadv, [kDuelingMaxActions] dval
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, A = g.A;
+  const long long r = (long long)blockIdx.x * 8 + warp;
+  if (r >= g.B) return;
+  float* __restrict__ d = d_s[warp];
+  for (int a = lane; a < A; a += 32) d[a] = g.dq[r * A + a];
+  __syncwarp();
+  if (lane == 0) d[kDuelingMaxActions] = dueling_transpose(d, A, d);
+  __syncwarp();
+  for (int a = lane; a < A; a += 32) g.dq[r * A + a] = d[a];
+  const float dval = d[kDuelingMaxActions];
+  if (lane == 0) g.dval[r] = dval;
+  const float* __restrict__ Wa = g.W[0];
+  const float* __restrict__ Wv = g.W[1];
+  float acc[16];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) acc[j] = 0.f;
+#pragma unroll 2
+  for (int a = 0; a < A; ++a) {
+    const float da = d[a];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) acc[j] = fmaf(da, Wa[(long long)(lane + 32 * j) * A + a], acc[j]);
+  }
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int k = lane + 32 * j;
+    const long long i = r * 512 + k;
+    const float va = g.h1[0][i] > 0.f ? acc[j] : 0.f;
+    const float vv = g.h1[1][i] > 0.f ? dval * Wv[k] : 0.f;
+    g.dh1[0][i] = va;
+    g.dh1[1][i] = vv;
+    if (g.hi[0]) {
+      float hi, lo;
+      tc::split_tf32(va, hi, lo);
+      g.hi[0][i] = hi; g.lo[0][i] = lo;
+      tc::split_tf32(vv, hi, lo);
+      g.hi[1][i] = hi; g.lo[1][i] = lo;
+    }
+  }
+}
+
 // epsilon-greedy over q[E][A] (dqn/agent.py:121-127): first maximum wins, as np.argmax / jnp.argmax.
 __global__ void act_select_kernel(const float* __restrict__ q, int A, int E, const float* __restrict__ explore, float eps,
                                   int32_t* __restrict__ actions) {
@@ -1662,7 +1832,7 @@ int64_t carve(dz_learner* l, char* base) {
   const Dims& d = l->d;
   const int B = c.batch;
   Bump w{base};
-  const bool rb = c.kind == DZ_RAINBOW, iqn = uses_iqn_net(c.kind);
+  const bool rb = noisy_net(c), two = two_streams(c), iqn = uses_iqn_net(c.kind);
   int nh[3] = {1, 1, 1};
   if (draws_taus(c.kind)) { nh[0] = c.tau_samples_s_tm1; nh[1] = c.tau_samples_policy; nh[2] = c.tau_samples_s_t; }
   // fqf: online(s_tm1) at tau_hat | online(s_tm1) at tau_1..tau_N | target(s_t) at [tau_hat' | tau_hat]; acting uses pass 1
@@ -1674,7 +1844,7 @@ int64_t carve(dz_learner* l, char* base) {
     l->act3[p] = w.take<float>((int64_t)B * d.feat);
     int64_t rows = (int64_t)B * nh[p];
     l->h1[p][0] = w.take<float>(rows * 512);
-    l->h1[p][1] = rb ? w.take<float>(rows * 512) : nullptr;
+    l->h1[p][1] = two ? w.take<float>(rows * 512) : nullptr;
     l->out[p] = w.take<float>(rows * d.out);
     l->outv[p] = rb ? w.take<float>((int64_t)B * c.num_atoms) : nullptr;
     l->cosf[p] = iqn ? w.take<float>(rows * c.latent_dim) : nullptr;
@@ -1705,9 +1875,10 @@ int64_t carve(dz_learner* l, char* base) {
   }
   int64_t rows0 = (int64_t)B * nh[0];
   l->dout = w.take<float>(rows0 * d.out);
-  l->doutv = rb ? w.take<float>((int64_t)B * c.num_atoms) : nullptr;
+  // the value stream's output gradient: rainbow's [B][atoms], the dueling network's dval [B]
+  l->doutv = two ? w.take<float>((int64_t)B * (rb ? c.num_atoms : 1)) : nullptr;
   l->dh1[0] = w.take<float>(rows0 * 512);
-  l->dh1[1] = rb ? w.take<float>(rows0 * 512) : nullptr;
+  l->dh1[1] = two ? w.take<float>(rows0 * 512) : nullptr;
   l->dact3 = w.take<float>((int64_t)B * d.feat);
   l->dtmp[0] = rb ? w.take<float>((int64_t)B * d.feat) : nullptr;
   l->dtmp[1] = rb ? w.take<float>((int64_t)B * d.feat) : nullptr;
@@ -1812,20 +1983,17 @@ UmNetDesc make_um_desc(const dz_learner* l) {
   u.online = l->buf.d_online; u.target = l->buf.d_target;
   for (int i = 0; i < 3; ++i) { u.off_conv_w[i] = o.conv_w[i]; u.off_conv_b[i] = o.conv_b[i]; }
   u.use_fc = !uses_iqn_net(c.kind);
-  u.nstream = c.kind == DZ_RAINBOW ? 2 : 1;
-  u.noisy = c.kind == DZ_RAINBOW ? 1 : 0;
-  if (c.kind == DZ_RAINBOW) {
-    for (int s = 0; s < 2; ++s) {
-      u.off_fc_w[s] = o.w1[s]; u.off_fc_b[s] = o.b1[s];
-      u.off_fc_sw[s] = o.sw1[s]; u.off_fc_sb[s] = o.sb1[s];
-    }
+  u.nstream = two_streams(c) ? 2 : 1;
+  u.noisy = noisy_net(c) ? 1 : 0;
+  if (u.use_fc)
+    for (int s = 0; s < u.nstream; ++s) { u.off_fc_w[s] = o.w1[s]; u.off_fc_b[s] = o.b1[s]; }
+  if (u.noisy) {
+    for (int s = 0; s < 2; ++s) { u.off_fc_sw[s] = o.sw1[s]; u.off_fc_sb[s] = o.sb1[s]; }
     const NoiseLayout nl = noise_layout(c, d);
     u.noise_stride = nl.stride;
     u.noise_off_in[0] = nl.a1i; u.noise_off_out[0] = nl.a1o;
     u.noise_off_in[1] = nl.v1i; u.noise_off_out[1] = nl.v1o;
     for (int p = 0; p < 3; ++p) u.noise_apply[p] = p;
-  } else if (u.use_fc) {
-    u.off_fc_w[0] = o.w1[0]; u.off_fc_b[0] = o.b1[0];
   }
   return u;
 }
@@ -2128,6 +2296,50 @@ int forward_heads_rainbow(dz_learner* l, const NetBufs& nb, const Pass* passes, 
   }
   DZ_TRY(run("noisy2_fwd", gb));
   if (nimg <= nb.split_rows) DZ_TRY(finish_nn(gb, outs, true, stream, noise_ld));
+  return DZ_OK;
+}
+
+// The dueling network's heads (DESIGN.md §16): both streams' 3136 -> 512 layers (on the fp32-FMA path one grouped
+// launch of 2 np problems, split over K as forward_heads_plain's fc1), then one dueling_head_fwd_kernel for every pass,
+// which writes each pass's aggregated q to out[head].
+int forward_heads_dueling(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, void* stream, bool fc1_done = false) {
+  const Dims& d = l->d;
+  const ParamOffsets& o = l->po;
+  if (2 * np > kMaxProblems) return fail(DZ_EINVAL, "too many dueling passes");
+  if (!fc1_done) {
+    GemmBatch gb;
+    gb.n = 2 * np;
+    float* outs[kMaxProblems];
+    const int splits = nimg <= nb.split_rows ? l->fc_splits : 1;
+    for (int i = 0; i < np; ++i)
+      for (int s = 0; s < 2; ++s) {
+        GemmProblem p = zero_problem();
+        p.a_mode = A_PLAIN; p.A = nb.act3[passes[i].set]; p.lda = d.feat; p.M = nimg; p.K = d.feat;
+        p.B = passes[i].params + o.w1[s]; p.N = 512; p.ldb = 512; p.ldc = 512;
+        p.bias = passes[i].params + o.b1[s]; p.relu = 1;
+        const int q = 2 * i + s;
+        outs[q] = nb.h1[passes[i].head][s];
+        if (splits > 1) {
+          p.splits = splits; p.split_stride = (long long)nimg * 512;
+          p.C = nb.nn_partial + (long long)q * splits * p.split_stride;
+        } else {
+          p.C = outs[q];
+        }
+        gb.p[q] = p;
+      }
+    DZ_TRY(run_nn("fc1_fwd", gb, false, stream));
+    if (splits > 1) DZ_TRY(finish_nn(gb, outs, false, stream));
+  }
+  DuelingFwdArgs h;
+  memset(&h, 0, sizeof(h));
+  for (int i = 0; i < np; ++i) {
+    const int hp = passes[i].head;
+    h.h1[i][0] = nb.h1[hp][0]; h.h1[i][1] = nb.h1[hp][1];
+    h.params[i] = passes[i].params; h.out[i] = nb.out[hp];
+  }
+  for (int s = 0; s < 2; ++s) { h.off_w[s] = o.w2[s]; h.off_b[s] = o.b2[s]; }
+  h.rows = nimg; h.A = l->cfg.num_actions;
+  DZ_LAUNCH_NAMED("dueling_head_fwd", dueling_head_fwd_kernel, dim3((unsigned)ceil_div(nimg, 8), (unsigned)np), 256, 0, stream, h);
   return DZ_OK;
 }
 
@@ -2531,6 +2743,57 @@ int backward_rainbow(dz_learner* l, const float* noise, void* stream) {
   return DZ_OK;
 }
 
+// The dueling network's backward (DESIGN.md §16): dueling_head_bwd_kernel turns dout into dadv (in place) and dval and
+// writes both streams' dh1 (and, on the tensor-core path, their tf32 hi/lo pair); the head and 3136 -> 512 weight
+// gradients of both streams run as two-problem launches on the side stream; dact3 sums both streams' input gradients.
+int backward_dueling(dz_learner* l, void* stream) {
+  const Dims& d = l->d;
+  const ParamOffsets& o = l->po;
+  const int B = l->B, A = l->cfg.num_actions;
+  float* G = l->buf.d_grads;
+  const float* P = l->buf.d_online;
+  {
+    DuelingBwdArgs a;
+    memset(&a, 0, sizeof(a));
+    a.dq = l->dout; a.dval = l->doutv; a.B = B; a.A = A;
+    for (int s = 0; s < 2; ++s) {
+      a.h1[s] = l->h1[0][s]; a.W[s] = P + o.w2[s]; a.dh1[s] = l->dh1[s];
+      if (l->um) { a.hi[s] = um_dh1_hi(l->um, s); a.lo[s] = um_dh1_lo(l->um, s); }
+    }
+    DZ_LAUNCH_NAMED("dueling_head_bwd", dueling_head_bwd_kernel, (unsigned)ceil_div(B, 8), 256, 0, stream, a);
+  }
+  GemmBatch gb;
+  gb.n = 2;
+  for (int s = 0; s < 2; ++s) {  // adv2 / val2 weight and bias gradients
+    const int n_out = s == 0 ? A : 1;
+    GemmProblem p = zero_problem();
+    p.a_mode = A_PLAIN; p.A = l->h1[0][s]; p.lda = 512; p.M = B; p.K = 512;
+    p.B = s == 0 ? l->dout : l->doutv; p.N = n_out; p.ldb = n_out; p.ldc = n_out;
+    p.C = G + o.w2[s]; p.Cb = G + o.b2[s];
+    gb.p[s] = p;
+  }
+  DZ_TRY(run_tn("head_wgrad", gb, l->side.fork(stream, stream)));
+  for (int s = 0; s < 2; ++s) {  // adv1 / val1 weight and bias gradients
+    GemmProblem p = zero_problem();
+    p.a_mode = A_PLAIN; p.A = l->act3[0]; p.lda = d.feat; p.M = B; p.K = d.feat;
+    p.B = l->dh1[s]; p.N = 512; p.ldb = 512; p.ldc = 512;
+    p.C = G + o.w1[s]; p.Cb = G + o.b1[s];
+    gb.p[s] = p;
+  }
+  DZ_TRY(run_tn("fc1_wgrad", gb, l->side.fork(stream, stream)));
+  if (l->um) return um_backward_fc(l->um, nullptr, stream);   // dh1 hi/lo came from dueling_head_bwd_kernel
+  for (int s = 0; s < 2; ++s) {  // dact3 contributions
+    GemmProblem p = zero_problem();
+    p.A = l->dh1[s]; p.lda = 512; p.M = B; p.N = 512; p.K = d.feat;
+    p.B = P + o.w1[s]; p.ldb = 512; p.ldc = d.feat;
+    p.splits = l->nt_splits; p.split_stride = (long long)B * d.feat;
+    p.C = l->nt_partial + (long long)s * l->nt_splits * p.split_stride;
+    gb.p[s] = p;
+  }
+  DZ_TRY(run_nt("fc1_dgrad", gb, false, stream));
+  return finish_nt(gb.p, 2, l->act3[0], l->dact3, false, stream);
+}
+
 int backward_iqn(dz_learner* l, void* stream) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
@@ -2832,7 +3095,7 @@ int act(const ActTarget& t, int E, const uint8_t* d_obs, const float* d_taus, co
         const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
   dz_learner* l = t.l;
   const dz_learner_config& c = l->cfg;
-  const bool rb = c.kind == DZ_RAINBOW;
+  const bool rb = noisy_net(c);
   if (!d_obs || !d_q_out) return fail(DZ_EINVAL, "act: null buffer");
   if (draws_taus(c.kind) && !d_taus) return fail(DZ_EINVAL, "iqn acting needs taus[E][tau_samples_policy]");
   if (rb && !d_noise) return fail(DZ_EINVAL, "rainbow acting needs noise");
@@ -2863,6 +3126,8 @@ int act(const ActTarget& t, int E, const uint8_t* d_obs, const float* d_taus, co
     DZ_TRY(forward_heads_iqn(l, t.nb, &pass, 1, E, taus, false, stream));
   } else if (rb) {
     DZ_TRY(forward_heads_rainbow(l, t.nb, &pass, 1, E, d_noise, stream, fc_done, noise_ld));
+  } else if (two_streams(c)) {
+    DZ_TRY(forward_heads_dueling(l, t.nb, &pass, 1, E, stream, fc_done));
   } else {
     DZ_TRY(forward_heads_plain(l, t.nb, &pass, 1, E, stream, fc_done));
   }
@@ -2940,7 +3205,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     const float* t2 = t1 + (long long)B * c.tau_samples_policy;
     const float* taus[3] = {t0, t1, t2};
     DZ_TRY(forward_heads_iqn(l, learner_bufs(l), passes, 3, B, taus, true, stream));
-  } else if (c.kind == DZ_RAINBOW) {
+  } else if (noisy_net(c)) {
     Pass passes[3] = {{on, 0, 0, 0}, {on, 1, 1, 1}, {tg, 2, 2, 2}};
     DZ_TRY(forward_heads_rainbow(l, learner_bufs(l), passes, 3, B, batch->d_noise, stream, um));
   } else {
@@ -2950,7 +3215,8 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     if (needs_online_st) passes[np++] = Pass{on, 1, 1, 0};
     if (target_stm1) passes[np++] = Pass{tg, 1, 1, 0};
     passes[np++] = Pass{tg, 2, 2, 0};
-    DZ_TRY(forward_heads_plain(l, learner_bufs(l), passes, np, B, stream, um));
+    if (two_streams(c)) DZ_TRY(forward_heads_dueling(l, learner_bufs(l), passes, np, B, stream, um));
+    else DZ_TRY(forward_heads_plain(l, learner_bufs(l), passes, np, B, stream, um));
   }
 
   // ---- loss + gradient wrt the pass-0 head outputs
@@ -2971,7 +3237,8 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   }
 
   // ---- backward through online(s_tm1)
-  if (c.kind == DZ_RAINBOW) DZ_TRY(backward_rainbow(l, batch->d_noise, stream));
+  if (noisy_net(c)) DZ_TRY(backward_rainbow(l, batch->d_noise, stream));
+  else if (two_streams(c)) DZ_TRY(backward_dueling(l, stream));
   else if (iqn) DZ_TRY(backward_iqn(l, stream));
   else DZ_TRY(backward_plain(l, stream));
   if (fqf) DZ_TRY(backward_fraction(l, stream));
@@ -3250,7 +3517,7 @@ int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
   const dz_learner_config& c = l->cfg;
   const Dims& d = l->d;
   const int E = a->E;
-  const bool rb = c.kind == DZ_RAINBOW, iqn = uses_iqn_net(c.kind);
+  const bool rb = noisy_net(c), two = two_streams(c), iqn = uses_iqn_net(c.kind);
   Bump w{base};
   NetBufs& b = a->b;
   memset(&b, 0, sizeof(b));   // split_rows 0: the fp32 GEMMs never split K, so row e's sums do not depend on E
@@ -3266,7 +3533,7 @@ int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
   const int64_t rows = (int64_t)E * (iqn ? acting_samples(c) : 1);
   if (!um || iqn) {                      // otherwise h1 is the tensor-core plan's
     b.h1[1][0] = w.take<float>(rows * 512);
-    b.h1[1][1] = rb ? w.take<float>(rows * 512) : nullptr;
+    b.h1[1][1] = two ? w.take<float>(rows * 512) : nullptr;
   }
   b.out[1] = w.take<float>(rows * d.out);
   b.outv[1] = rb ? w.take<float>((int64_t)E * c.num_atoms) : nullptr;
@@ -3328,7 +3595,7 @@ int actor_create(dz_learner* l, bool frozen, int32_t num_streams, void* d_worksp
     if (rc != DZ_OK) { dz_actor_destroy(a); return rc; }
     for (int L = 1; L <= 3; ++L) (L == 1 ? a->b.act1 : L == 2 ? a->b.act2 : a->b.act3)[1] = um_act_f32(a->um, L, 0);
     if (!uses_iqn_net(l->cfg.kind))
-      for (int s = 0; s < (l->cfg.kind == DZ_RAINBOW ? 2 : 1); ++s) a->b.h1[1][s] = um_h1_f32(a->um, 0, s);
+      for (int s = 0; s < (two_streams(l->cfg) ? 2 : 1); ++s) a->b.h1[1][s] = um_h1_f32(a->um, 0, s);
   }
   *out = a;
   return DZ_OK;
@@ -3588,6 +3855,16 @@ int dz_test_fqf_example(const float* logits, const float* F_tau, const float* F_
   float* dl = w + N;
   fqf_fractions(logits, N, q, tau, hat, w);
   fqf_dlogits(F_tau, F_hat, q, N, cot, dl);
+  return DZ_OK;
+}
+
+// Host twin of the dueling head's per-row arithmetic: dueling_aggregate and dueling_transpose, the functions
+// dueling_head_fwd_kernel and dueling_head_bwd_kernel run (tests only).
+int dz_test_dueling_example(const float* adv, float v, const float* dq, int32_t A, float* out) {
+  if (!adv || !dq || !out) return fail(DZ_EINVAL, "dueling example: NULL buffer");
+  if (A < 1 || A > kDuelingMaxActions) return fail(DZ_EINVAL, "dueling example: A must be in [1,64]");
+  dueling_aggregate(adv, v, A, out);
+  out[2 * A] = dueling_transpose(dq, A, out + A);
   return DZ_OK;
 }
 

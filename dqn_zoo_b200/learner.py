@@ -79,6 +79,16 @@ class NetworkSpec(NamedTuple):
   tau_samples_s_t: int = 64
   obs_shape: tuple = (84, 84, 4)
   num_fractions: int = 32              # fqf: N, the number of proposed quantile fractions
+  dueling: bool = False                # the dueling network (DESIGN.md §16): dqn, double_q, prioritized, munchausen
+
+
+# The kinds that take NetworkSpec(dueling=True); rainbow's network is dueling already.
+DUELING_KINDS = ('dqn', 'double_q', 'prioritized', 'munchausen')
+
+# The dueling network's linear modules.  The reference has no plain dueling network, so these module paths are the
+# project's own, kept stable for hk.Params-shaped dicts.
+_DUELING_MODULES = {'adv1': 'dueling/advantage/linear', 'adv2': 'dueling/advantage/linear_1',
+                    'val1': 'dueling/value/linear', 'val2': 'dueling/value/linear_1'}
 
 
 # canonical name -> haiku-style module path (the nested "sequential/..." prefixes are
@@ -89,6 +99,8 @@ def haiku_name(canonical: str, kind: str):
   conv = {'conv1': 'conv2_d', 'conv2': 'conv2_d_1', 'conv3': 'conv2_d_2'}
   if parts[0] in conv:
     return 'sequential/sequential/' + conv[parts[0]], leaf
+  if kind != 'rainbow' and parts[0] in _DUELING_MODULES:   # the tensor names identify the dueling network
+    return _DUELING_MODULES[parts[0]], leaf
   if kind == 'rainbow':
     idx = {'adv1': '', 'adv2': '_1', 'val1': '_2', 'val2': '_3'}[parts[0]]
     return 'noisy_linear%s/%s' % (idx, parts[1]), leaf
@@ -96,6 +108,13 @@ def haiku_name(canonical: str, kind: str):
     return {'embed': 'batch_apply/linear', 'fc1': 'batch_apply_1/sequential/linear',
             'head': 'batch_apply_1/sequential/linear_1', 'fraction': 'fraction_proposal/linear'}[parts[0]], leaf
   return {'fc1': 'sequential/sequential_1/linear', 'head': 'sequential/sequential_1/linear_1'}[parts[0]], leaf
+
+
+def check_network(net: NetworkSpec) -> None:
+  """ValueError for a NetworkSpec no learner can build: dueling=True on a kind outside DUELING_KINDS."""
+  if net.dueling and net.kind not in DUELING_KINDS:
+    raise ValueError('dueling=True needs one of %s, got %r%s' % (', '.join(DUELING_KINDS), net.kind,
+                                                                 ' (its network is dueling already)' if net.kind == 'rainbow' else ''))
 
 
 def noise_vector_sizes(net: NetworkSpec):
@@ -167,6 +186,7 @@ class Learner:
     l0 > 0 and non-finite values for those kinds, and the other kinds ignore them.  `fraction_learning_rate`,
     `fraction_opt_eps` and `fraction_rms_decay` are fqf's centred RMSProp over its fraction layer (DESIGN.md §15); the
     library rejects a negative or non-finite rate, eps <= 0 and a decay outside [0, 1) for fqf."""
+    check_network(net)
     if not torch.cuda.is_available():
       raise RuntimeError('dqn_zoo_b200.learner needs a CUDA device (there is no CPU fallback)')
     self.net = net
@@ -188,6 +208,7 @@ class Learner:
     cfg.num_fractions = net.num_fractions
     cfg.fraction_learning_rate, cfg.fraction_opt_eps, cfg.fraction_rms_decay = (fraction_learning_rate, fraction_opt_eps,
                                                                                 fraction_rms_decay)
+    cfg.dueling = 1 if net.dueling else 0
     self.cfg = cfg
     plan = _lib.LearnerPlan()
     _lib.call('dz_learner_plan_query', C.byref(cfg), C.byref(plan))

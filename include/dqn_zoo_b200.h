@@ -350,6 +350,12 @@ typedef struct dz_learner_config {
   float fraction_learning_rate;  /* 2.5e-9 */
   float fraction_opt_eps;        /* 1e-5 */
   float fraction_rms_decay;      /* 0.95 */
+  /* 1: the dueling network (Wang et al., ICML 2016; DESIGN.md §16) in place of the fc1 / head layers, valid for dqn,
+   * double_q, prioritized and munchausen (DZ_EINVAL for any other kind; rainbow's network is dueling already).  0, as a
+   * zero-filled tail leaves it: the plain network.  The parameter layout after the conv tensors is "adv1/w" [feat][512],
+   * "adv1/b" [512], "adv2/w" [512][A], "adv2/b" [A], "val1/w" [feat][512], "val1/b" [512], "val2/w" [512][1],
+   * "val2/b" [1], and the head outputs q_a = v + (adv_a - mean_a adv) in every place the plain network's are read. */
+  int32_t dueling;
 } dz_learner_config;
 
 typedef struct dz_learner_plan {
@@ -673,6 +679,11 @@ int dz_test_munchausen_iqn_example(const float* zbar_tm1, const float* zbar_t, i
  * q to out[0, N), tau to out[N, 2N+1), tau_hat to out[2N+1, 3N+1), w to out[3N+1, 4N+1) and dlogits to
  * out[4N+1, 5N+1).  DZ_EINVAL for N out of range or a NULL buffer; tests only. */
 int dz_test_fqf_example(const float* logits, const float* F_tau, const float* F_hat, int32_t N, float cot, float* out);
+/* Host twin of the dueling head's per-row arithmetic (dueling_head_fwd_kernel / dueling_head_bwd_kernel; DESIGN.md
+ * §16), the functions those kernels run: from the advantages adv [A], the value v and the q gradient dq [A] it writes
+ * q_a = v + (adv_a - m) with m = (sum_a adv_a) / A to out[0, A), dadv_a = dq_a - (sum_a dq_a) / A to out[A, 2A) and
+ * dval = sum_a dq_a to out[2A].  Sums run in action order.  DZ_EINVAL for A outside [1, 64] or a NULL buffer; tests only. */
+int dz_test_dueling_example(const float* adv, float v, const float* dq, int32_t A, float* out);
 /* The loss section of a learner step (the agent kind's loss kernel, then the scalar loss and rainbow's running max
  * priority) on caller-owned device buffers, all enqueued on `stream`; tests only.  cfg is validated as
  * dz_learner_create does, with batch = B and its observation fields replaced by a legal geometry.  d_out[p]: the head

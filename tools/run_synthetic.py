@@ -92,7 +92,7 @@ def build_train_agent(args, random_state, preprocessor):
                                                     1e-3, True, random_state)
   else:
     replay = replay_lib.TransitionReplay(args.replay_capacity, structure, random_state)
-  network = learner_lib.NetworkSpec(kind, args.num_actions)
+  network = learner_lib.NetworkSpec(kind, args.num_actions, dueling=args.dueling)
   epsilon = parts.LinearSchedule(begin_t=int(args.min_replay_capacity_fraction * args.replay_capacity * 4),
                                  decay_steps=max(args.num_train_frames, 1), begin_value=1.0, end_value=0.01)
   common = dict(preprocessor=preprocessor, sample_network_input=np.zeros((84, 84, 4), np.uint8), network=network, optimizer=None,
@@ -260,6 +260,8 @@ def parse_args(argv=None):
   ap.add_argument('--agent', default='dqn',
                   choices=['dqn', 'double_q', 'prioritized', 'c51', 'qrdqn', 'rainbow', 'iqn', 'munchausen',
                            'munchausen_iqn', 'fqf'])
+  ap.add_argument('--dueling', action='store_true',
+                  help='the dueling network (DESIGN.md §16): dqn, double_q, prioritized and munchausen only')
   ap.add_argument('--num_actions', type=int, default=6)
   ap.add_argument('--replay_capacity', type=int, default=20000)
   ap.add_argument('--min_replay_capacity_fraction', type=float, default=0.05)
