@@ -56,14 +56,15 @@ def _acting_rows_error(net, E):
 
 def _acting_randomness(source, seed, per_stream=False, num_streams=1):
   """The randomness of one act on `source` (a `Learner` or a `learner_lib.Actor`), drawn from its generator with one
-  counter step, as the keyword argument of `Learner.q_values` / `Learner.act_batch` / `Actor.act`: rainbow's own apply
-  per stream (`per_stream`, num_streams of them), IQN's taus or rainbow's one shared apply.  The other kinds act
-  without randomness (fqf proposes its fractions) and draw nothing: {}."""
+  counter step, as the keyword argument of `Learner.q_values` / `Learner.act_batch` / `Actor.act`: a noisy network's
+  own apply per stream (`per_stream`, num_streams of them), IQN's taus or a noisy network's one shared apply (rainbow,
+  and NetworkSpec(noisy=True)).  The other networks act without randomness (fqf proposes its fractions) and draw
+  nothing: {}."""
   if per_stream:
     what = 'stream_noise'
   elif _draws_taus(source.kind):
     what = 'taus'
-  elif source.kind == 'rainbow':
+  elif learner_lib.noisy_layers(source.net):
     what = 'noise'
   else:
     return {}
@@ -251,7 +252,7 @@ class _DeviceAgent(parts.Agent):
         held.append(t)
       blobs[name] = t
     state = {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'dueling': bool(L.net.dueling),
-             'param_count': L.plan.param_count,
+             'noisy': bool(L.net.noisy), 'param_count': L.plan.param_count,
              'opt_state_floats': L.plan.opt_state_floats, 'host_rng': self._host_rng.get_state(), 'seed': self._seed,
              'jax_key': None if getattr(self, '_jax_key', None) is None else self._jax_key.copy(),
              'frame_t': self._frame_t}
@@ -280,10 +281,11 @@ class _DeviceAgent(parts.Agent):
     except (OSError, pickle.UnpicklingError, EOFError) as e:
       raise ValueError('%s is not a readable agent checkpoint: %s' % (directory, e)) from e
     L = self._learner
-    # checkpoints written before the dueling network existed have no 'dueling' key: they hold the plain network
-    ck.validate(dict({'dueling': False}, **state),
+    # checkpoints written before the dueling network or noisy networks existed have no 'dueling' / 'noisy' key: they
+    # hold the plain network
+    ck.validate(dict({'dueling': False, 'noisy': False}, **state),
                 {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'dueling': bool(L.net.dueling),
-                 'param_count': L.plan.param_count, 'opt_state_floats': L.plan.opt_state_floats}, directory)
+                 'noisy': bool(L.net.noisy), 'param_count': L.plan.param_count, 'opt_state_floats': L.plan.opt_state_floats}, directory)
     blobs = {}
     for name in self._CHECKPOINT_BLOBS:
       path = os.path.join(directory, name + '.npy')
@@ -421,7 +423,7 @@ class _DeviceAgent(parts.Agent):
     L = self._learner
     if getattr(self, '_jax_key', None) is not None:
       self._jax_learn.launch(L.taus)            # jax.random.uniform draws from the keys staged by _learn()
-    elif _draws_taus(self.KIND) or self.KIND == 'rainbow':
+    elif _draws_taus(self.KIND) or learner_lib.noisy_layers(L.net):
       L.generate_randomness(self._seed, beside_sampler=True)
     L.learn(self._view, self.PRIORITIZED, self._io)
 
@@ -441,7 +443,10 @@ class _DeviceAgent(parts.Agent):
 
 
 class Dqn(_DeviceAgent):
-  """dqn/agent.py:40-229."""
+  """dqn/agent.py:40-229.  It takes the network it is given: with NetworkSpec(noisy=True) (DESIGN.md §17) it draws
+  the noise of its noisy layers every step and every act, and still acts epsilon-greedily on the
+  `exploration_epsilon` schedule, so NoisyNet-DQN (Fortunato et al., ICLR 2018) is this agent on the noisy network
+  with a schedule that is zero throughout.  DoubleQ, PrioritizedDqn and Munchausen take noisy networks the same way."""
   KIND = 'dqn'
 
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
@@ -739,8 +744,8 @@ class BatchedEpsilonGreedyActor:
                per_stream_noise: bool = False):
     if num_streams < 1:
       raise ValueError('num_streams must be >= 1')
-    if per_stream_noise and learner.net.kind != 'rainbow':
-      raise ValueError('per_stream_noise needs a rainbow learner')
+    if per_stream_noise and not learner_lib.noisy_layers(learner.net):
+      raise ValueError('per_stream_noise needs a learner with noisy layers')
     # beyond the learner's batch the tick needs buffers of its own size
     self._actor = learner.actor(num_streams) if num_streams > learner.batch_size else None
     self._learner = learner
@@ -1118,8 +1123,8 @@ class VectorEvaluator:
     err = _acting_rows_error(net, E)
     if err:
       raise ValueError(err)
-    if per_stream_noise and net.kind != 'rainbow':
-      raise ValueError('per_stream_noise needs a rainbow network')
+    if per_stream_noise and not learner_lib.noisy_layers(net):
+      raise ValueError('per_stream_noise needs a network with noisy layers')
     kwargs = dict(preprocessor_kwargs or {})
     if not kwargs.pop('device_observations', True):
       raise ValueError('the evaluator keeps its frame stacks on the device: device_observations must be True')

@@ -12,6 +12,9 @@
 //   fqf           Fully parameterized Quantile Function (Yang et al., NeurIPS 2019), outside the reference: iqn's
 //                 network at taus a fraction proposal layer computes in the step, its own loss kernel and a second
 //                 (RMSProp) optimizer launch over the fraction layer (DESIGN.md §15)
+//   dueling,      network options of dqn / double_q / prioritized / munchausen, outside the reference: the dueling
+//   noisy         network (Wang et al., ICML 2016; DESIGN.md §16) and factorised-noise layers with a mu bias
+//                 (Fortunato et al., ICLR 2018; networks.py:137-178 with_bias=True; DESIGN.md §17), alone or together
 //
 // Gradients flow only through online(s_tm1).  All forward passes of a layer are one grouped
 // launch (dz_gemm.cuh); the replay gather is fused into conv1's operand load.
@@ -43,15 +46,16 @@ __host__ __device__ constexpr bool uses_dqn_net(int kind) { return kind == DZ_DQ
 constexpr int net_kind(int kind) { return uses_iqn_net(kind) ? DZ_IQN : uses_dqn_net(kind) ? DZ_DQN : kind; }
 // The Munchausen kinds: alpha / tau / l0 are validated, and the target network also applies to s_tm1.
 constexpr bool is_munchausen(int kind) { return kind == DZ_MUNCHAUSEN || kind == DZ_MUNCHAUSEN_IQN; }
-// The kinds that may take the dueling network (DESIGN.md §16): their losses read one scalar q per action.
+// The kinds that may take the dueling network (DESIGN.md §16) and noisy layers (§17): their losses read one scalar q per
+// action.
 constexpr bool dueling_allowed(int kind) {
   return kind == DZ_DQN || kind == DZ_DOUBLE_Q || kind == DZ_PRIORITIZED || kind == DZ_MUNCHAUSEN;
 }
 // After validate(): the network has two 512-wide streams after the torso (rainbow's noisy pair, the dueling network's
-// plain pair), and its layers are noisy (rainbow).  Every decision about the second stream's buffers, plan and launches
-// asks the first; every decision about noise asks the second.
+// pair), and its layers are noisy (rainbow, noisy networks).  Every decision about the second stream's buffers, plan and
+// launches asks the first; every decision about noise asks the second.
 inline bool two_streams(const dz_learner_config& c) { return c.kind == DZ_RAINBOW || c.dueling != 0; }
-inline bool noisy_net(const dz_learner_config& c) { return c.kind == DZ_RAINBOW; }
+inline bool noisy_net(const dz_learner_config& c) { return c.kind == DZ_RAINBOW || c.noisy != 0; }
 
 // ------------------------------------------------------------------------------------------------
 // Parameter layout (canonical names; haiku layouts) — must match oracle/learner_oracle.py:param_shapes
@@ -127,6 +131,17 @@ static Layout make_layout(const dz_learner_config& c) {
     }
     return L;
   }
+  if (c.noisy) {   // DESIGN.md §17: mu w, mu b, sigma w, sigma b of each layer; dueling: the advantage stream first
+    const char* plain[2] = {"fc1", "head"};
+    const char* dueling[4] = {"adv1", "adv2", "val1", "val2"};
+    for (int i = 0; i < (c.dueling ? 4 : 2); ++i) {
+      const std::string p = c.dueling ? dueling[i] : plain[i];
+      const int64_t n_in = i % 2 ? 512 : d.feat, n_out = i % 2 == 0 ? 512 : i == 1 ? c.num_actions : 1;
+      L.add(p + "/mu/w", {n_in, n_out}); L.add(p + "/mu/b", {n_out});
+      L.add(p + "/sigma/w", {n_in, n_out}); L.add(p + "/sigma/b", {n_out});
+    }
+    return L;
+  }
   if (c.dueling) {   // advantage stream first, as rainbow's, so that stream index s means the same in both networks
     const char* streams[2] = {"adv", "val"};
     for (int s = 0; s < 2; ++s) {
@@ -148,7 +163,7 @@ static Layout make_layout(const dz_learner_config& c) {
 }
 
 // Offsets into a parameter blob of every tensor the step's launches address; -1 where the agent kind has no such tensor.
-// Stream s = 0 is fc1 (rainbow: the advantage stream), s = 1 rainbow's value stream.  Layer 1 is the 512-wide layer,
+// Stream s = 0 is fc1 (two streams: the advantage stream), s = 1 the value stream.  Layer 1 is the 512-wide layer,
 // layer 2 the head (plain heads: head/w, head/b; rainbow's mu has no bias).  sw / sb: noisy sigma weight / bias.
 struct ParamOffsets {
   int64_t conv_w[3], conv_b[3];
@@ -183,6 +198,14 @@ static int param_offsets(const dz_learner_config& c, const Layout& L, ParamOffse
       const std::string p = streams[s];
       o.w1[s] = need(p + "1/mu/w"); o.b1[s] = need(p + "1/mu/b"); o.sw1[s] = need(p + "1/sigma/w"); o.sb1[s] = need(p + "1/sigma/b");
       o.w2[s] = need(p + "2/mu/w"); o.sw2[s] = need(p + "2/sigma/w"); o.sb2[s] = need(p + "2/sigma/b");
+    }
+  } else if (c.noisy) {
+    const char* streams[2] = {"adv", "val"};
+    for (int s = 0; s < (c.dueling ? 2 : 1); ++s) {
+      const std::string p1 = c.dueling ? std::string(streams[s]) + "1" : "fc1";
+      const std::string p2 = c.dueling ? std::string(streams[s]) + "2" : "head";
+      o.w1[s] = need(p1 + "/mu/w"); o.b1[s] = need(p1 + "/mu/b"); o.sw1[s] = need(p1 + "/sigma/w"); o.sb1[s] = need(p1 + "/sigma/b");
+      o.w2[s] = need(p2 + "/mu/w"); o.b2[s] = need(p2 + "/mu/b"); o.sw2[s] = need(p2 + "/sigma/w"); o.sb2[s] = need(p2 + "/sigma/b");
     }
   } else if (c.dueling) {
     const char* streams[2] = {"adv", "val"};
@@ -337,6 +360,10 @@ static int validate(const dz_learner_config& c) {
   if (c.dueling != 0 && c.dueling != 1) return fail(DZ_EINVAL, "dueling must be 0 or 1");
   if (c.dueling && !dueling_allowed(c.kind))
     return fail(DZ_EINVAL, "dueling: only dqn, double_q, prioritized and munchausen take the dueling network");
+  if (c.noisy != 0 && c.noisy != 1) return fail(DZ_EINVAL, "noisy must be 0 or 1");
+  if (c.noisy && c.kind == DZ_RAINBOW) return fail(DZ_EINVAL, "noisy: rainbow's network is noisy already");
+  if (c.noisy && !dueling_allowed(c.kind))
+    return fail(DZ_EINVAL, "noisy: only dqn, double_q, prioritized and munchausen take noisy layers");
   if (is_munchausen(c.kind) && !munchausen_params_ok(c.munchausen_alpha, c.entropy_temperature, c.log_policy_clip))
     return fail(DZ_EINVAL, "munchausen needs finite alpha >= 0, entropy_temperature > 0 and log_policy_clip <= 0");
   if (is_munchausen(c.kind) && c.num_actions > kMunchausenMaxActions)
@@ -1581,14 +1608,25 @@ struct DuelingFwdArgs {
   int rows, A;
 };
 
+// The noisy dueling head (DESIGN.md §17): the same launch with each weight formed in registers as
+// w = fmaf(sigma_w, eps_in_k * eps_out_a, mu_w) (the operations of gemm_nn_kernel<DUAL>) and each bias as
+// b = fmaf(sigma_b, eps_out_a, mu_b), where mu_b is added before the sigma term as in its epilogue.
+struct NoisyDuelingFwdArgs {
+  DuelingFwdArgs h;
+  long long off_sw[2], off_sb[2];
+  const float* noise[3];    // each pass's noise apply
+  long long noise_ld;       // floats between the applies of consecutive rows (per-stream acting); 0: one apply per pass
+  long long off_in[2], off_out[2];   // offsets in an apply of each stream's head eps_in [512] / eps_out
+};
+
 __device__ __forceinline__ float warp_sum_xor(float s) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   return s;
 }
 
-__global__ void __launch_bounds__(256) dueling_head_fwd_kernel(const __grid_constant__ DuelingFwdArgs h) {
-  dz::pdl_enter();
+template <bool NOISY>
+__device__ __forceinline__ void dueling_head_fwd(const DuelingFwdArgs& h, const NoisyDuelingFwdArgs* n) {
   __shared__ float adv_s[8][kDuelingMaxActions];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, p = blockIdx.y, A = h.A;
   const long long r = (long long)blockIdx.x * 8 + warp;
@@ -1598,34 +1636,75 @@ __global__ void __launch_bounds__(256) dueling_head_fwd_kernel(const __grid_cons
   const float* __restrict__ P = h.params[p];
   const float* __restrict__ Wa = P + h.off_w[0];
   const float* __restrict__ Wv = P + h.off_w[1];
+  const float *Sa = nullptr, *Sv = nullptr, *eia = nullptr, *eoa = nullptr, *eiv = nullptr;
+  float eov = 0.f;
+  if constexpr (NOISY) {
+    const float* nz = n->noise[p] + r * n->noise_ld;
+    Sa = P + n->off_sw[0]; Sv = P + n->off_sw[1];
+    eia = nz + n->off_in[0]; eoa = nz + n->off_out[0]; eiv = nz + n->off_in[1]; eov = nz[n->off_out[1]];
+  }
   float x[16];
+  float ei[NOISY ? 16 : 1];
   float sv = 0.f;
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     x[j] = xa[lane + 32 * j];
-    sv = fmaf(xv[lane + 32 * j], Wv[lane + 32 * j], sv);
+    if constexpr (NOISY) {
+      const int k = lane + 32 * j;
+      ei[j] = eia[k];
+      sv = fmaf(xv[k], fmaf(Sv[k], eiv[k] * eov, Wv[k]), sv);
+    } else {
+      sv = fmaf(xv[lane + 32 * j], Wv[lane + 32 * j], sv);
+    }
   }
-  const float v = warp_sum_xor(sv) + P[h.off_b[1]];
+  float v = warp_sum_xor(sv) + P[h.off_b[1]];
+  if constexpr (NOISY) v = fmaf(P[n->off_sb[1]], eov, v);
   for (int a0 = 0; a0 < A; a0 += 4) {
     const int na = A - a0 < 4 ? A - a0 : 4;
     float s[4] = {0.f, 0.f, 0.f, 0.f};
+    float eo[NOISY ? 4 : 1];
+    if constexpr (NOISY) {
+#pragma unroll
+      for (int c = 0; c < 4; ++c) eo[c] = c < na ? eoa[a0 + c] : 0.f;
+    }
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       const float* __restrict__ w = Wa + (long long)(lane + 32 * j) * A + a0;
+      if constexpr (NOISY) {
+        const float* __restrict__ sg = Sa + (long long)(lane + 32 * j) * A + a0;
 #pragma unroll
-      for (int c = 0; c < 4; ++c)
-        if (c < na) s[c] = fmaf(x[j], w[c], s[c]);
+        for (int c = 0; c < 4; ++c)
+          if (c < na) s[c] = fmaf(x[j], fmaf(sg[c], ei[j] * eo[c], w[c]), s[c]);
+      } else {
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          if (c < na) s[c] = fmaf(x[j], w[c], s[c]);
+      }
     }
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
       const float t = warp_sum_xor(s[c]);
-      if (lane == 0 && c < na) adv_s[warp][a0 + c] = t + P[h.off_b[0] + a0 + c];
+      if constexpr (NOISY) {
+        if (lane == 0 && c < na) adv_s[warp][a0 + c] = fmaf(P[n->off_sb[0] + a0 + c], eo[c], t + P[h.off_b[0] + a0 + c]);
+      } else {
+        if (lane == 0 && c < na) adv_s[warp][a0 + c] = t + P[h.off_b[0] + a0 + c];
+      }
     }
   }
   __syncwarp();
   if (lane == 0) dueling_aggregate(adv_s[warp], v, A, adv_s[warp]);
   __syncwarp();
   for (int a = lane; a < A; a += 32) h.out[p][r * A + a] = adv_s[warp][a];
+}
+
+__global__ void __launch_bounds__(256) dueling_head_fwd_kernel(const __grid_constant__ DuelingFwdArgs h) {
+  dz::pdl_enter();
+  dueling_head_fwd<false>(h, nullptr);
+}
+
+__global__ void __launch_bounds__(256) noisy_dueling_head_fwd_kernel(const __grid_constant__ NoisyDuelingFwdArgs n) {
+  dz::pdl_enter();
+  dueling_head_fwd<true>(n.h, &n);
 }
 
 // The dueling head's backward of online(s_tm1), one warp per row: dadv and dval from dq (dueling_transpose; dadv
@@ -1644,8 +1723,15 @@ struct DuelingBwdArgs {
   int B, A;
 };
 
-__global__ void __launch_bounds__(256) dueling_head_bwd_kernel(const __grid_constant__ DuelingBwdArgs g) {
-  dz::pdl_enter();
+// The noisy dueling head's backward: the same launch through the weights the forward formed (noise apply 0).
+struct NoisyDuelingBwdArgs {
+  DuelingBwdArgs g;
+  const float* S[2];                    // adv2/sigma/w, val2/sigma/w of the online blob
+  const float *ein[2], *eout[2];        // each stream's head eps_in [512] / eps_out
+};
+
+template <bool NOISY>
+__device__ __forceinline__ void dueling_head_bwd(const DuelingBwdArgs& g, const NoisyDuelingBwdArgs* n) {
   __shared__ float d_s[8][kDuelingMaxActions + 1];   // per warp: [0, A) dadv, [kDuelingMaxActions] dval
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, A = g.A;
   const long long r = (long long)blockIdx.x * 8 + warp;
@@ -1661,20 +1747,36 @@ __global__ void __launch_bounds__(256) dueling_head_bwd_kernel(const __grid_cons
   const float* __restrict__ Wa = g.W[0];
   const float* __restrict__ Wv = g.W[1];
   float acc[16];
+  float ei[NOISY ? 16 : 1];
 #pragma unroll
   for (int j = 0; j < 16; ++j) acc[j] = 0.f;
+  if constexpr (NOISY) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) ei[j] = n->ein[0][lane + 32 * j];
+  }
 #pragma unroll 2
   for (int a = 0; a < A; ++a) {
     const float da = d[a];
+    if constexpr (NOISY) {
+      const float eo = n->eout[0][a];
 #pragma unroll
-    for (int j = 0; j < 16; ++j) acc[j] = fmaf(da, Wa[(long long)(lane + 32 * j) * A + a], acc[j]);
+      for (int j = 0; j < 16; ++j) {
+        const long long i = (long long)(lane + 32 * j) * A + a;
+        acc[j] = fmaf(da, fmaf(n->S[0][i], ei[j] * eo, Wa[i]), acc[j]);
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) acc[j] = fmaf(da, Wa[(long long)(lane + 32 * j) * A + a], acc[j]);
+    }
   }
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const int k = lane + 32 * j;
     const long long i = r * 512 + k;
     const float va = g.h1[0][i] > 0.f ? acc[j] : 0.f;
-    const float vv = g.h1[1][i] > 0.f ? dval * Wv[k] : 0.f;
+    float vv;
+    if constexpr (NOISY) vv = g.h1[1][i] > 0.f ? dval * fmaf(n->S[1][k], n->ein[1][k] * n->eout[1][0], Wv[k]) : 0.f;
+    else vv = g.h1[1][i] > 0.f ? dval * Wv[k] : 0.f;
     g.dh1[0][i] = va;
     g.dh1[1][i] = vv;
     if (g.hi[0]) {
@@ -1685,6 +1787,16 @@ __global__ void __launch_bounds__(256) dueling_head_bwd_kernel(const __grid_cons
       g.hi[1][i] = hi; g.lo[1][i] = lo;
     }
   }
+}
+
+__global__ void __launch_bounds__(256) dueling_head_bwd_kernel(const __grid_constant__ DuelingBwdArgs g) {
+  dz::pdl_enter();
+  dueling_head_bwd<false>(g, nullptr);
+}
+
+__global__ void __launch_bounds__(256) noisy_dueling_head_bwd_kernel(const __grid_constant__ NoisyDuelingBwdArgs n) {
+  dz::pdl_enter();
+  dueling_head_bwd<true>(n.g, &n);
 }
 
 // epsilon-greedy over q[E][A] (dqn/agent.py:121-127): first maximum wins, as np.argmax / jnp.argmax.
@@ -1832,7 +1944,7 @@ int64_t carve(dz_learner* l, char* base) {
   const Dims& d = l->d;
   const int B = c.batch;
   Bump w{base};
-  const bool rb = noisy_net(c), two = two_streams(c), iqn = uses_iqn_net(c.kind);
+  const bool rb = c.kind == DZ_RAINBOW, two = two_streams(c), iqn = uses_iqn_net(c.kind);
   int nh[3] = {1, 1, 1};
   if (draws_taus(c.kind)) { nh[0] = c.tau_samples_s_tm1; nh[1] = c.tau_samples_policy; nh[2] = c.tau_samples_s_t; }
   // fqf: online(s_tm1) at tau_hat | online(s_tm1) at tau_1..tau_N | target(s_t) at [tau_hat' | tau_hat]; acting uses pass 1
@@ -1947,8 +2059,10 @@ int64_t carve(dz_learner* l, char* base) {
   return w.used;
 }
 
-// Rainbow noise of ONE apply, in this order: adv1_in[feat] adv1_out[512] adv2_in[512] adv2_out[A*atoms] val1_in[feat]
-// val1_out[512] val2_in[512] val2_out[atoms]; every vector starts on a 4-float boundary.  Offsets in floats.
+// Noise of ONE apply, in this order: adv1_in[feat] adv1_out[512] adv2_in[512] adv2_out[A*atoms] val1_in[feat]
+// val1_out[512] val2_in[512] val2_out[atoms]; every vector starts on a 4-float boundary.  Offsets in floats.  Rainbow;
+// the noisy dueling network with one atom; the noisy plain network has only the first four (fc1 in / out, head in /
+// out; the value stream's offsets are then those of the next apply and never read).
 struct NoiseLayout {
   int64_t stride;   // floats per apply
   int64_t a1i, a1o, a2i, a2o, v1i, v1o, v2i, v2o;
@@ -1957,9 +2071,11 @@ NoiseLayout noise_layout(const dz_learner_config& c, const Dims& d) {
   NoiseLayout n;
   int64_t end = 0;
   auto next = [&](int64_t len) { const int64_t at = end; end += (len + 3) / 4 * 4; return at; };
-  n.a1i = next(d.feat); n.a1o = next(512); n.a2i = next(512); n.a2o = next((int64_t)c.num_actions * c.num_atoms);
-  n.v1i = next(d.feat); n.v1o = next(512); n.v2i = next(512); n.v2o = next(c.num_atoms);
-  n.stride = end;
+  const int64_t atoms = c.kind == DZ_RAINBOW ? c.num_atoms : 1;
+  n.a1i = next(d.feat); n.a1o = next(512); n.a2i = next(512); n.a2o = next((int64_t)c.num_actions * atoms);
+  const int64_t one = end;
+  n.v1i = next(d.feat); n.v1o = next(512); n.v2i = next(512); n.v2o = next(atoms);
+  n.stride = two_streams(c) ? end : one;
   return n;
 }
 struct NoiseVecs { const float *a1i, *a1o, *a2i, *a2o, *v1i, *v1o, *v2i, *v2o; };
@@ -1988,12 +2104,15 @@ UmNetDesc make_um_desc(const dz_learner* l) {
   if (u.use_fc)
     for (int s = 0; s < u.nstream; ++s) { u.off_fc_w[s] = o.w1[s]; u.off_fc_b[s] = o.b1[s]; }
   if (u.noisy) {
-    for (int s = 0; s < 2; ++s) { u.off_fc_sw[s] = o.sw1[s]; u.off_fc_sb[s] = o.sb1[s]; }
     const NoiseLayout nl = noise_layout(c, d);
+    const int64_t in[2] = {nl.a1i, nl.v1i}, out[2] = {nl.a1o, nl.v1o};
+    for (int s = 0; s < u.nstream; ++s) {
+      u.off_fc_sw[s] = o.sw1[s]; u.off_fc_sb[s] = o.sb1[s];
+      u.noise_off_in[s] = in[s]; u.noise_off_out[s] = out[s];
+    }
     u.noise_stride = nl.stride;
-    u.noise_off_in[0] = nl.a1i; u.noise_off_out[0] = nl.a1o;
-    u.noise_off_in[1] = nl.v1i; u.noise_off_out[1] = nl.v1o;
-    for (int p = 0; p < 3; ++p) u.noise_apply[p] = p;
+    // apply p is noise slot p: online(s_tm1) | the middle pass | target(s_t); dqn's two passes read slots 0 and 2
+    for (int p = 0; p < 3; ++p) u.noise_apply[p] = u.npass == 2 && p == 1 ? 2 : p;
   }
   return u;
 }
@@ -2114,7 +2233,7 @@ struct Pass {        // one network.apply
   const float* params;     // online or target blob
   int set;                 // torso activation set index (0..2)
   int head;                // head pass index (0..2)
-  int apply;               // noise apply index (rainbow)
+  int apply;               // noise apply index (noisy layers): the step's slot 0 / 1 / 2
 };
 
 // ---- forward -----------------------------------------------------------------------------------
@@ -2232,32 +2351,36 @@ int forward_heads_plain(dz_learner* l, const NetBufs& nb, const Pass* passes, in
   return DZ_OK;
 }
 
-// Rainbow: two noisy streams (networks.py:224-261, :137-178).  noise_ld > 0: image m of the pass uses its own noise
-// apply at noise + m * noise_ld (one pass only); 0: every image uses the pass's apply.
-int forward_heads_rainbow(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, const float* noise, void* stream, bool fc1_done = false,
-                          long long noise_ld = 0) {
+// Noisy layers (networks.py:137-178): rainbow's two streams (:224-261), the noisy plain network's one and the noisy
+// dueling network's two (DESIGN.md §17).  The 3136 -> 512 layers are one grouped noisy launch; the heads are one
+// grouped noisy launch (rainbow's mu has no bias, the noisy networks' has), or for the noisy dueling network one
+// noisy_dueling_head_fwd_kernel.  noise_ld > 0: image m of the pass uses its own noise apply at noise + m * noise_ld
+// (one pass only); 0: every image uses the pass's apply.
+int forward_heads_noisy(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, const float* noise, void* stream, bool fc1_done = false,
+                        long long noise_ld = 0) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
-  if (2 * np > kMaxProblems) return fail(DZ_EINVAL, "too many rainbow passes");
+  const int ns = two_streams(c) ? 2 : 1;
+  if (ns * np > kMaxProblems) return fail(DZ_EINVAL, "too many noisy passes");
   if (noise_ld && (np != 1 || fc1_done)) return fail(DZ_EINVAL, "per-row noise: one pass with its own fc1");
   auto run = [&](const char* tag, GemmBatch& b) {
     return noise_ld ? run_nn_rownoise(tag, b, noise_ld, stream) : run_nn(tag, b, true, stream);
   };
   GemmBatch gb;
-  gb.n = 2 * np;
+  gb.n = ns * np;
   float* outs[kMaxProblems];
   const int splits = nimg <= nb.split_rows ? l->fc_splits : 1;
   for (int i = 0; i < np && !fc1_done; ++i) {
     NoiseVecs nz = noise_of(c, d, noise, passes[i].apply);
-    for (int s = 0; s < 2; ++s) {
+    for (int s = 0; s < ns; ++s) {
       GemmProblem p = zero_problem();
       p.a_mode = A_PLAIN; p.A = nb.act3[passes[i].set]; p.lda = d.feat; p.M = nimg; p.K = d.feat;
       p.B = passes[i].params + o.w1[s]; p.B2 = passes[i].params + o.sw1[s];
       p.N = 512; p.ldb = 512; p.ldc = 512;
       p.bias = passes[i].params + o.b1[s]; p.bias2 = passes[i].params + o.sb1[s];
       p.a_scale = s == 0 ? nz.a1i : nz.v1i; p.c_scale = s == 0 ? nz.a1o : nz.v1o; p.relu = 1;
-      int q = 2 * i + s;
+      int q = ns * i + s;
       outs[q] = nb.h1[passes[i].head][s];
       if (splits > 1) {
         p.splits = splits; p.split_stride = (long long)2 * nimg * 512;
@@ -2272,22 +2395,40 @@ int forward_heads_rainbow(dz_learner* l, const NetBufs& nb, const Pass* passes, 
     DZ_TRY(run("noisy1_fwd", gb));
     if (splits > 1) DZ_TRY(finish_nn(gb, outs, true, stream, noise_ld));
   }
+  if (c.kind != DZ_RAINBOW && ns == 2) {
+    NoisyDuelingFwdArgs a;
+    memset(&a, 0, sizeof(a));
+    const NoiseLayout nl = noise_layout(c, d);
+    for (int i = 0; i < np; ++i) {
+      const int hp = passes[i].head;
+      a.h.h1[i][0] = nb.h1[hp][0]; a.h.h1[i][1] = nb.h1[hp][1];
+      a.h.params[i] = passes[i].params; a.h.out[i] = nb.out[hp];
+      a.noise[i] = noise + (int64_t)passes[i].apply * nl.stride;
+    }
+    for (int s = 0; s < 2; ++s) { a.h.off_w[s] = o.w2[s]; a.h.off_b[s] = o.b2[s]; a.off_sw[s] = o.sw2[s]; a.off_sb[s] = o.sb2[s]; }
+    a.off_in[0] = nl.a2i; a.off_out[0] = nl.a2o; a.off_in[1] = nl.v2i; a.off_out[1] = nl.v2o;
+    a.noise_ld = noise_ld;
+    a.h.rows = nimg; a.h.A = c.num_actions;
+    DZ_LAUNCH_NAMED("noisy_dueling_head_fwd", noisy_dueling_head_fwd_kernel, dim3((unsigned)ceil_div(nimg, 8), (unsigned)np), 256, 0,
+                    stream, a);
+    return DZ_OK;
+  }
   for (int i = 0; i < np; ++i) {
     NoiseVecs nz = noise_of(c, d, noise, passes[i].apply);
-    for (int s = 0; s < 2; ++s) {
-      int n_out = s == 0 ? c.num_actions * c.num_atoms : c.num_atoms;
+    for (int s = 0; s < ns; ++s) {
+      int n_out = s == 0 ? d.out : c.num_atoms;
       GemmProblem p = zero_problem();
       p.a_mode = A_PLAIN; p.A = nb.h1[passes[i].head][s]; p.lda = 512; p.M = nimg; p.K = 512;
       p.B = passes[i].params + o.w2[s]; p.B2 = passes[i].params + o.sw2[s];
       p.N = n_out; p.ldb = n_out; p.ldc = n_out;
-      p.bias = nullptr; p.bias2 = passes[i].params + o.sb2[s];   // with_bias=False: mu has no bias
+      // rainbow's mu has no bias (with_bias=False); the noisy plain head's has
+      p.bias = o.b2[s] < 0 ? nullptr : passes[i].params + o.b2[s]; p.bias2 = passes[i].params + o.sb2[s];
       p.a_scale = s == 0 ? nz.a2i : nz.v2i; p.c_scale = s == 0 ? nz.a2o : nz.v2o;
-      int q = 2 * i + s;
+      int q = ns * i + s;
       outs[q] = s == 0 ? nb.out[passes[i].head] : nb.outv[passes[i].head];
       if (nimg <= nb.split_rows) {
-        int64_t head_n = (int64_t)c.num_actions * c.num_atoms;
         p.splits = l->head_splits; p.split_stride = (long long)2 * nimg * n_out;
-        p.C = nb.nn_partial + (long long)q * l->head_splits * 2 * nimg * head_n;
+        p.C = nb.nn_partial + (long long)q * l->head_splits * 2 * nimg * d.out;
       } else {
         p.C = outs[q];
       }
@@ -2675,46 +2816,66 @@ int backward_plain(dz_learner* l, void* stream) {
   return DZ_OK;
 }
 
-int backward_rainbow(dz_learner* l, const float* noise, void* stream) {
+// The backward of forward_heads_noisy's networks through online(s_tm1) (noise apply 0).  The heads: rainbow's and the
+// noisy plain network's input gradient is a noisy run_nt and a finish that masks dh1 (and, on the tensor-core path,
+// writes its tf32 hi/lo pair); the noisy dueling network's is noisy_dueling_head_bwd_kernel.  Every weight gradient is a
+// noisy run_tn on the side stream that fills the mu and sigma gradients together.
+int backward_noisy(dz_learner* l, const float* noise, void* stream) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
   const int B = l->B;
+  const int ns = two_streams(c) ? 2 : 1;
+  const bool dueling_head = c.kind != DZ_RAINBOW && ns == 2;
+  const int n_val = c.kind == DZ_RAINBOW ? c.num_atoms : 1;   // value-stream outputs
   float* G = l->buf.d_grads;
   const float* P = l->buf.d_online;
   NoiseVecs nz = noise_of(c, d, noise, 0);
+  if (dueling_head) {   // dout -> dadv in place, dval -> doutv, both streams' dh1
+    NoisyDuelingBwdArgs a;
+    memset(&a, 0, sizeof(a));
+    a.g.dq = l->dout; a.g.dval = l->doutv; a.g.B = B; a.g.A = c.num_actions;
+    for (int s = 0; s < 2; ++s) {
+      a.g.h1[s] = l->h1[0][s]; a.g.W[s] = P + o.w2[s]; a.g.dh1[s] = l->dh1[s];
+      if (l->um) { a.g.hi[s] = um_dh1_hi(l->um, s); a.g.lo[s] = um_dh1_lo(l->um, s); }
+      a.S[s] = P + o.sw2[s];
+    }
+    a.ein[0] = nz.a2i; a.eout[0] = nz.a2o; a.ein[1] = nz.v2i; a.eout[1] = nz.v2o;
+    DZ_LAUNCH_NAMED("noisy_dueling_head_bwd", noisy_dueling_head_bwd_kernel, (unsigned)ceil_div(B, 8), 256, 0, stream, a);
+  }
   GemmBatch gb;
-  gb.n = 2;
-  for (int s = 0; s < 2; ++s) {  // second noisy layer weight grads
-    int n_out = s == 0 ? c.num_actions * c.num_atoms : c.num_atoms;
+  gb.n = ns;
+  for (int s = 0; s < ns; ++s) {  // second noisy layer weight grads
+    int n_out = s == 0 ? d.out : n_val;
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->h1[0][s]; p.lda = 512; p.M = B; p.K = 512;
     p.B = s == 0 ? l->dout : l->doutv; p.N = n_out; p.ldb = n_out; p.ldc = n_out;
-    p.C = G + o.w2[s]; p.C2 = G + o.sw2[s]; p.Cb = nullptr; p.Cb2 = G + o.sb2[s];
+    p.C = G + o.w2[s]; p.C2 = G + o.sw2[s]; p.Cb = o.b2[s] < 0 ? nullptr : G + o.b2[s]; p.Cb2 = G + o.sb2[s];
     p.a_scale = s == 0 ? nz.a2i : nz.v2i; p.c_scale = s == 0 ? nz.a2o : nz.v2o;
     gb.p[s] = p;
   }
   DZ_TRY(run_tn("noisy2_wgrad", gb, l->side.fork(stream, stream)));
-  for (int s = 0; s < 2; ++s) {  // dh1_s
-    int n_out = s == 0 ? c.num_actions * c.num_atoms : c.num_atoms;
-    GemmProblem p = zero_problem();
-    p.A = s == 0 ? l->dout : l->doutv; p.lda = n_out; p.M = B; p.N = n_out; p.K = 512;
-    p.B = P + o.w2[s]; p.B2 = P + o.sw2[s]; p.ldb = n_out;
-    p.a_scale = s == 0 ? nz.a2i : nz.v2i; p.c_scale = s == 0 ? nz.a2o : nz.v2o;
-    p.ldc = 512;
-    p.splits = 4; p.split_stride = (long long)2 * B * 512;
-    p.C = l->nt_partial + (long long)s * 4 * p.split_stride;
-    gb.p[s] = p;
-  }
-  DZ_TRY(run_nt("noisy2_dgrad", gb, true, stream));
-  {   // both streams' dh1 in one launch; on the tensor-core path it also writes the tf32 hi/lo pair noisy1_dgrad reads
+  if (!dueling_head) {
+    for (int s = 0; s < ns; ++s) {  // dh1_s
+      int n_out = s == 0 ? d.out : n_val;
+      GemmProblem p = zero_problem();
+      p.A = s == 0 ? l->dout : l->doutv; p.lda = n_out; p.M = B; p.N = n_out; p.K = 512;
+      p.B = P + o.w2[s]; p.B2 = P + o.sw2[s]; p.ldb = n_out;
+      p.a_scale = s == 0 ? nz.a2i : nz.v2i; p.c_scale = s == 0 ? nz.a2o : nz.v2o;
+      p.ldc = 512;
+      p.splits = 4; p.split_stride = (long long)2 * B * 512;
+      p.C = l->nt_partial + (long long)s * 4 * p.split_stride;
+      gb.p[s] = p;
+    }
+    DZ_TRY(run_nt("noisy2_dgrad", gb, true, stream));
+    // every stream's dh1 in one launch; on the tensor-core path it also writes the tf32 hi/lo pair noisy1_dgrad reads
     FinishNT jobs[2];
-    for (int s = 0; s < 2; ++s)
+    for (int s = 0; s < ns; ++s)
       jobs[s] = make_finish_nt(&gb.p[s], 1, l->h1[0][s], l->dh1[s], true, l->um ? um_dh1_hi(l->um, s) : nullptr,
                                l->um ? um_dh1_lo(l->um, s) : nullptr);
-    DZ_TRY(finish_nt_batch(jobs, 2, stream));
+    DZ_TRY(finish_nt_batch(jobs, ns, stream));
   }
-  for (int s = 0; s < 2; ++s) {  // first noisy layer weight grads
+  for (int s = 0; s < ns; ++s) {  // first noisy layer weight grads
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->act3[0]; p.lda = d.feat; p.M = B; p.K = d.feat;
     p.B = l->dh1[s]; p.N = 512; p.ldb = 512; p.ldc = 512;
@@ -2724,10 +2885,10 @@ int backward_rainbow(dz_learner* l, const float* noise, void* stream) {
   }
   DZ_TRY(run_tn("noisy1_wgrad", gb, l->side.fork(stream, stream)));
   if (l->um) {
-    DZ_TRY(um_backward_fc(l->um, noise, stream));   // dh1 hi/lo came from the finish kernel above
+    DZ_TRY(um_backward_fc(l->um, noise, stream));   // dh1 hi/lo came from the head's input gradient above
     return DZ_OK;
   }
-  for (int s = 0; s < 2; ++s) {  // dact3 contributions
+  for (int s = 0; s < ns; ++s) {  // dact3 contributions
     GemmProblem p = zero_problem();
     p.A = l->dh1[s]; p.lda = 512; p.M = B; p.N = 512; p.K = d.feat;
     p.B = P + o.w1[s]; p.B2 = P + o.sw1[s]; p.ldb = 512;
@@ -2738,8 +2899,8 @@ int backward_rainbow(dz_learner* l, const float* noise, void* stream) {
     gb.p[s] = p;
   }
   DZ_TRY(run_nt("noisy1_dgrad", gb, true, stream));
-  // dact3 = (adv-stream + val-stream contributions) * [act3 > 0], summed from the split partials
-  DZ_TRY(finish_nt(gb.p, 2, l->act3[0], l->dact3, true, stream));
+  // dact3 = (sum of the streams' contributions) * [act3 > 0], summed from the split partials
+  DZ_TRY(finish_nt(gb.p, ns, l->act3[0], l->dact3, true, stream));
   return DZ_OK;
 }
 
@@ -3098,10 +3259,10 @@ int act(const ActTarget& t, int E, const uint8_t* d_obs, const float* d_taus, co
   const bool rb = noisy_net(c);
   if (!d_obs || !d_q_out) return fail(DZ_EINVAL, "act: null buffer");
   if (draws_taus(c.kind) && !d_taus) return fail(DZ_EINVAL, "iqn acting needs taus[E][tau_samples_policy]");
-  if (rb && !d_noise) return fail(DZ_EINVAL, "rainbow acting needs noise");
+  if (rb && !d_noise) return fail(DZ_EINVAL, "acting a noisy network needs noise");
   const int64_t stride = rb ? noise_layout(c, l->d).stride : 0;
   if (noise_ld != 0 && (!rb || noise_ld != stride))
-    return fail(DZ_EINVAL, "act: noise_ld must be 0 (one shared apply) or the noise stride (rainbow, one apply per stream)");
+    return fail(DZ_EINVAL, "act: noise_ld must be 0 (one shared apply) or the noise stride (noisy layers, one apply per stream)");
   const float* on = t.params;
   const long long obs_bytes = (long long)l->d.H * l->d.W * l->d.C;
   DZ_LAUNCH(make_row_table_kernel, (unsigned)ceil_div(E, 64), 64, 0, stream, d_obs, obs_bytes, E, t.rows);
@@ -3125,7 +3286,7 @@ int act(const ActTarget& t, int E, const uint8_t* d_obs, const float* d_taus, co
     const float* taus[1] = {d_taus};
     DZ_TRY(forward_heads_iqn(l, t.nb, &pass, 1, E, taus, false, stream));
   } else if (rb) {
-    DZ_TRY(forward_heads_rainbow(l, t.nb, &pass, 1, E, d_noise, stream, fc_done, noise_ld));
+    DZ_TRY(forward_heads_noisy(l, t.nb, &pass, 1, E, d_noise, stream, fc_done, noise_ld));
   } else if (two_streams(c)) {
     DZ_TRY(forward_heads_dueling(l, t.nb, &pass, 1, E, stream, fc_done));
   } else {
@@ -3152,7 +3313,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   const float* on = l->buf.d_online;
   const float* tg = l->buf.d_target;
   const bool needs_online_st = c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED || c.kind == DZ_RAINBOW;
-  if (c.kind == DZ_RAINBOW && !batch->d_noise) return fail(DZ_EINVAL, "rainbow update needs d_noise");
+  if (noisy_net(c) && !batch->d_noise) return fail(DZ_EINVAL, "a noisy network's update needs d_noise");
   if (draws_taus(c.kind) && !batch->d_taus) return fail(DZ_EINVAL, "iqn update needs d_taus");
   if (!out || !out->d_loss || !out->d_per_example) return fail(DZ_EINVAL, "update outputs d_loss and d_per_example are required");
   if (!(weights_packed && l->um != nullptr)) DZ_TRY(l->side.join(stream));   // pending side-stream work (asynchronous randomness)
@@ -3205,17 +3366,19 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     const float* t2 = t1 + (long long)B * c.tau_samples_policy;
     const float* taus[3] = {t0, t1, t2};
     DZ_TRY(forward_heads_iqn(l, learner_bufs(l), passes, 3, B, taus, true, stream));
-  } else if (noisy_net(c)) {
+  } else if (c.kind == DZ_RAINBOW) {
     Pass passes[3] = {{on, 0, 0, 0}, {on, 1, 1, 1}, {tg, 2, 2, 2}};
-    DZ_TRY(forward_heads_rainbow(l, learner_bufs(l), passes, 3, B, batch->d_noise, stream, um));
+    DZ_TRY(forward_heads_noisy(l, learner_bufs(l), passes, 3, B, batch->d_noise, stream, um));
   } else {
+    // noise slot = head pass (noisy networks, DESIGN.md §17): online(s_tm1) | the middle pass | target(s_t)
     Pass passes[3];
     int np = 0;
     passes[np++] = Pass{on, 0, 0, 0};
-    if (needs_online_st) passes[np++] = Pass{on, 1, 1, 0};
-    if (target_stm1) passes[np++] = Pass{tg, 1, 1, 0};
-    passes[np++] = Pass{tg, 2, 2, 0};
-    if (two_streams(c)) DZ_TRY(forward_heads_dueling(l, learner_bufs(l), passes, np, B, stream, um));
+    if (needs_online_st) passes[np++] = Pass{on, 1, 1, 1};
+    if (target_stm1) passes[np++] = Pass{tg, 1, 1, 1};
+    passes[np++] = Pass{tg, 2, 2, 2};
+    if (noisy_net(c)) DZ_TRY(forward_heads_noisy(l, learner_bufs(l), passes, np, B, batch->d_noise, stream, um));
+    else if (two_streams(c)) DZ_TRY(forward_heads_dueling(l, learner_bufs(l), passes, np, B, stream, um));
     else DZ_TRY(forward_heads_plain(l, learner_bufs(l), passes, np, B, stream, um));
   }
 
@@ -3237,7 +3400,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   }
 
   // ---- backward through online(s_tm1)
-  if (noisy_net(c)) DZ_TRY(backward_rainbow(l, batch->d_noise, stream));
+  if (noisy_net(c)) DZ_TRY(backward_noisy(l, batch->d_noise, stream));
   else if (two_streams(c)) DZ_TRY(backward_dueling(l, stream));
   else if (iqn) DZ_TRY(backward_iqn(l, stream));
   else DZ_TRY(backward_plain(l, stream));
@@ -3276,7 +3439,7 @@ int dz_learner_plan_query(const dz_learner_config* cfg, dz_learner_plan* out) {
   out->num_tensors = (int32_t)tmp.lay.t.size();
   out->opt_state_floats = 2 * tmp.lay.total;
   out->workspace_bytes = carve(&tmp, nullptr);
-  out->noise_floats = cfg->kind == DZ_RAINBOW ? 3 * noise_layout(*cfg, tmp.d).stride : 0;
+  out->noise_floats = noisy_net(*cfg) ? 3 * noise_layout(*cfg, tmp.d).stride : 0;
   out->tau_floats = draws_taus(cfg->kind)
                         ? (int64_t)cfg->batch * (cfg->tau_samples_s_tm1 + cfg->tau_samples_policy + cfg->tau_samples_s_t)
                         : 0;
@@ -3420,7 +3583,7 @@ int dz_learner_generate_randomness(dz_learner* l, uint64_t seed, float* d_taus, 
     long long n = (long long)c.batch * (c.tau_samples_s_tm1 + c.tau_samples_policy + c.tau_samples_s_t);
     DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_taus, n, seed, l->buf.d_counters, 0, 1u);
   }
-  if (c.kind == DZ_RAINBOW && d_noise) {
+  if (noisy_net(c) && d_noise) {
     long long n = 3 * noise_layout(c, l->d).stride;
     DZ_LAUNCH(randomness_kernel, (unsigned)ceil_div(ceil_div(n, 4), 256), 256, 0, stream, d_noise, n, seed, l->buf.d_counters, 1, 2u);
   }
@@ -3442,7 +3605,7 @@ int dz_learner_act_batch(dz_learner* l, const uint8_t* d_obs, int32_t E, const f
 
 int dz_learner_noise_stride(const dz_learner_config* cfg, int64_t* out) {
   DZ_TRY(validate(*cfg));
-  if (cfg->kind != DZ_RAINBOW) return fail(DZ_EINVAL, "noise_stride: only rainbow has noisy layers");
+  if (!noisy_net(*cfg)) return fail(DZ_EINVAL, "noise_stride: only rainbow and noisy networks have noisy layers");
   *out = noise_layout(*cfg, make_dims(*cfg)).stride;
   return DZ_OK;
 }
@@ -3451,7 +3614,7 @@ int dz_learner_noise_stride(const dz_learner_config* cfg, int64_t* out) {
 // E * stride floats, so the first three applies equal what that call writes for the same seed and counter.  Advances
 // the counter once.
 int dz_learner_generate_stream_noise(dz_learner* l, uint64_t seed, int32_t E, float* d_noise, void* stream) {
-  if (l->cfg.kind != DZ_RAINBOW) return fail(DZ_EINVAL, "generate_stream_noise: only rainbow has noisy layers");
+  if (!noisy_net(l->cfg)) return fail(DZ_EINVAL, "generate_stream_noise: only rainbow and noisy networks have noisy layers");
   if (E < 1 || E > l->B) return fail(DZ_EINVAL, "generate_stream_noise: 1 <= E <= learner batch");
   if (!d_noise) return fail(DZ_EINVAL, "generate_stream_noise: null buffer");
   return launch_acting_draw(d_noise, (long long)E * noise_layout(l->cfg, l->d).stride, false, seed, l->buf.d_counters, stream);
@@ -3517,7 +3680,7 @@ int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
   const dz_learner_config& c = l->cfg;
   const Dims& d = l->d;
   const int E = a->E;
-  const bool rb = noisy_net(c), two = two_streams(c), iqn = uses_iqn_net(c.kind);
+  const bool rb = c.kind == DZ_RAINBOW, two = two_streams(c), iqn = uses_iqn_net(c.kind);
   Bump w{base};
   NetBufs& b = a->b;
   memset(&b, 0, sizeof(b));   // split_rows 0: the fp32 GEMMs never split K, so row e's sums do not depend on E
@@ -3540,7 +3703,7 @@ int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
   b.cosf[1] = iqn ? w.take<float>(rows * c.latent_dim) : nullptr;
   b.hi[1] = iqn ? w.take<float>(rows * d.feat) : nullptr;
   a->rows = w.take<const uint8_t*>(E);
-  a->noise = rb ? w.take<float>(noise_layout(c, d).stride) : nullptr;
+  a->noise = noisy_net(c) ? w.take<float>(noise_layout(c, d).stride) : nullptr;
   a->frac_hat = proposes_fractions(c.kind) ? w.take<float>((int64_t)E * c.num_fractions) : nullptr;
   a->frac_w = proposes_fractions(c.kind) ? w.take<float>((int64_t)E * c.num_fractions) : nullptr;
   if (a->frozen) {
@@ -3695,8 +3858,8 @@ int dz_actor_generate_randomness(dz_actor* a, uint64_t seed, int32_t per_stream,
   long long n;
   const bool iqn = draws_taus(c.kind);
   if (iqn && !per_stream) n = (long long)a->E * c.tau_samples_policy;
-  else if (c.kind == DZ_RAINBOW) n = (per_stream ? (long long)a->E : 1LL) * noise_layout(c, a->l->d).stride;
-  else return fail(DZ_EINVAL, "actor randomness: iqn draws taus, rainbow noise (per_stream: rainbow only); other kinds draw nothing");
+  else if (noisy_net(c)) n = (per_stream ? (long long)a->E : 1LL) * noise_layout(c, a->l->d).stride;
+  else return fail(DZ_EINVAL, "actor randomness: iqn draws taus, noisy layers noise (per_stream: noise only); other kinds draw nothing");
   return launch_acting_draw(d_out, n, iqn, seed, a->frozen ? a->counters : a->l->buf.d_counters, stream);
 }
 
@@ -3918,6 +4081,10 @@ int dz_test_learner_buffer(dz_learner* l, const char* name, float** d_ptr, int64
   else if (n == "h1_val") { *d_ptr = l->h1[0][1]; *count = l->h1[0][1] ? rows0 * 512 : 0; }
   else if (n == "iqn_e0") { *d_ptr = l->E0; *count = l->E0 ? rows0 * l->d.feat : 0; }
   else if (n == "h1") { *d_ptr = l->h1[0][0]; *count = rows0 * 512; }
+  else if (n == "out0" || n == "out1" || n == "out2") {   // head pass p's outputs
+    const int p = n[3] - '0';
+    *d_ptr = l->out[p]; *count = (int64_t)l->B * l->n_head[p] * l->d.out;
+  }
   else if (n == "dh1") { *d_ptr = l->dh1[0]; *count = rows0 * 512; }
   else if (n == "iqn_hi") {
     if (l->pk_on) return fail(DZ_EINVAL, "iqn_hi is not materialised on the packed tensor-core path");

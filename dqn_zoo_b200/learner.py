@@ -80,10 +80,18 @@ class NetworkSpec(NamedTuple):
   obs_shape: tuple = (84, 84, 4)
   num_fractions: int = 32              # fqf: N, the number of proposed quantile fractions
   dueling: bool = False                # the dueling network (DESIGN.md §16): dqn, double_q, prioritized, munchausen
+  noisy: bool = False                  # noisy networks (DESIGN.md §17): the same kinds, plain or dueling
 
 
-# The kinds that take NetworkSpec(dueling=True); rainbow's network is dueling already.
+# The kinds that take NetworkSpec(dueling=True) and NetworkSpec(noisy=True); rainbow's network is dueling and noisy already.
 DUELING_KINDS = ('dqn', 'double_q', 'prioritized', 'munchausen')
+NOISY_KINDS = DUELING_KINDS
+
+
+def noisy_layers(net: NetworkSpec) -> bool:
+  """Whether the network has factorised-noise layers (rainbow, and NetworkSpec(noisy=True)): every place that allocates,
+  draws or passes noise asks this."""
+  return net.kind == 'rainbow' or bool(net.noisy)
 
 # The dueling network's linear modules.  The reference has no plain dueling network, so these module paths are the
 # project's own, kept stable for hk.Params-shaped dicts.
@@ -99,6 +107,10 @@ def haiku_name(canonical: str, kind: str):
   conv = {'conv1': 'conv2_d', 'conv2': 'conv2_d_1', 'conv3': 'conv2_d_2'}
   if parts[0] in conv:
     return 'sequential/sequential/' + conv[parts[0]], leaf
+  if kind != 'rainbow' and len(parts) == 3:   # noisy networks (DESIGN.md §17): '<layer>/{mu,sigma}/{w,b}'
+    module = _DUELING_MODULES.get(parts[0]) or {'fc1': 'sequential/sequential_1/linear',
+                                               'head': 'sequential/sequential_1/linear_1'}[parts[0]]
+    return module.replace('linear', 'noisy_linear') + '/' + parts[1], leaf
   if kind != 'rainbow' and parts[0] in _DUELING_MODULES:   # the tensor names identify the dueling network
     return _DUELING_MODULES[parts[0]], leaf
   if kind == 'rainbow':
@@ -111,15 +123,20 @@ def haiku_name(canonical: str, kind: str):
 
 
 def check_network(net: NetworkSpec) -> None:
-  """ValueError for a NetworkSpec no learner can build: dueling=True on a kind outside DUELING_KINDS."""
+  """ValueError for a NetworkSpec no learner can build: dueling=True on a kind outside DUELING_KINDS, noisy=True on a
+  kind outside NOISY_KINDS."""
   if net.dueling and net.kind not in DUELING_KINDS:
     raise ValueError('dueling=True needs one of %s, got %r%s' % (', '.join(DUELING_KINDS), net.kind,
                                                                  ' (its network is dueling already)' if net.kind == 'rainbow' else ''))
+  if net.noisy and net.kind not in NOISY_KINDS:
+    raise ValueError('noisy=True needs one of %s, got %r%s' % (', '.join(NOISY_KINDS), net.kind,
+                                                               ' (its network is noisy already)' if net.kind == 'rainbow' else ''))
 
 
 def noise_vector_sizes(net: NetworkSpec):
-  """(name, length) of the 8 factorised-noise vectors of ONE `network.apply`, in
-  `hk.next_rng_key()` order (networks.py:169-170, :235-248)."""
+  """(name, length) of the factorised-noise vectors of ONE `network.apply`: rainbow's 8 in `hk.next_rng_key()` order
+  (networks.py:169-170, :235-248); a noisy network's (DESIGN.md §17) fc1 in / out and head in / out, or dueling,
+  rainbow's 8 with one atom."""
   h = net.obs_shape[0]
   for k, s in ((8, 4), (4, 2), (3, 1)):
     h = (h - k) // s + 1
@@ -128,6 +145,10 @@ def noise_vector_sizes(net: NetworkSpec):
     w = (w - k) // s + 1
   d = h * w * 64
   a, k = net.num_actions, net.num_atoms
+  if net.kind != 'rainbow':
+    if not net.dueling:
+      return [('fc1/in', d), ('fc1/out', 512), ('head/in', 512), ('head/out', a)]
+    k = 1
   return [('adv1/in', d), ('adv1/out', 512), ('adv2/in', 512), ('adv2/out', a * k),
           ('val1/in', d), ('val1/out', 512), ('val2/in', 512), ('val2/out', k)]
 
@@ -159,15 +180,15 @@ def _ptr(t):
 
 def _act_inputs(owner, E, explore, taus, noise, stream_noise):
   """The exploration and randomness inputs of one act of E streams on `owner` (a `Learner` or an `Actor`) as device
-  tensors: (explore, taus, noise, noise_ld).  `stream_noise` is rainbow's [E, noise_stride] block whose row e is stream
+  tensors: (explore, taus, noise, noise_ld).  `stream_noise` is a noisy network's [E, noise_stride] block whose row e is stream
   e's own apply; it replaces noise / taus and sets noise_ld to the stride (0: one apply shared by the streams)."""
   x = _f32(explore, owner.device)
   if stream_noise is None:
     return x, _f32(taus, owner.device), _f32(noise, owner.device), 0
   if noise is not None or taus is not None:
     raise ValueError('stream_noise replaces noise / taus')
-  if owner.kind != 'rainbow':
-    raise ValueError('stream_noise needs a rainbow learner')
+  if not noisy_layers(owner.net):
+    raise ValueError('stream_noise needs a learner with noisy layers')
   n = _f32(stream_noise, owner.device)
   if n.dim() != 2 or n.shape[0] != E or n.shape[1] != owner.noise_stride:
     raise ValueError('stream_noise must be [E, noise_stride] = [%d, %d], got %s' % (E, owner.noise_stride, tuple(n.shape)))
@@ -209,6 +230,7 @@ class Learner:
     cfg.fraction_learning_rate, cfg.fraction_opt_eps, cfg.fraction_rms_decay = (fraction_learning_rate, fraction_opt_eps,
                                                                                 fraction_rms_decay)
     cfg.dueling = 1 if net.dueling else 0
+    cfg.noisy = 1 if net.noisy else 0
     self.cfg = cfg
     plan = _lib.LearnerPlan()
     _lib.call('dz_learner_plan_query', C.byref(cfg), C.byref(plan))
@@ -224,8 +246,8 @@ class Learner:
     self.counters = torch.zeros(4, dtype=torch.int64, device=dev)
     self.taus = torch.zeros(max(plan.tau_floats, 1), dtype=torch.float32, device=dev)
     self.noise = torch.zeros(max(plan.noise_floats, 1), dtype=torch.float32, device=dev)
-    self.noise_stride = 0          # floats of one noise apply (rainbow)
-    if net.kind == 'rainbow':
+    self.noise_stride = 0          # floats of one noise apply (noisy layers)
+    if noisy_layers(net):
       stride = C.c_int64()
       _lib.call('dz_learner_noise_stride', C.byref(cfg), C.byref(stride))
       self.noise_stride = stride.value
@@ -351,7 +373,7 @@ class Learner:
     batch = _lib.Batch(keep[2].data_ptr(), keep[3].data_ptr(), keep[4].data_ptr(), keep[5].data_ptr(),
                        keep[6].data_ptr(), 0 if w is None else w.data_ptr(),
                        self.taus.data_ptr() if draws_taus(self.kind) else 0,
-                       self.noise.data_ptr() if self.kind == 'rainbow' else 0)
+                       self.noise.data_ptr() if noisy_layers(self.net) else 0)
     out = _lib.UpdateOutputs(self.loss.data_ptr(), self.per_example.data_ptr(), self.priorities.data_ptr(),
                              self.grad_norm.data_ptr())
     _lib.call('dz_learner_update', self._h, C.byref(batch), C.byref(out), 1 if apply_update else 0, _cstream())
@@ -364,10 +386,10 @@ class Learner:
               self.taus.data_ptr(), self.noise.data_ptr(), _cstream())
 
   def generate_stream_noise(self, seed: int, num_streams: int) -> torch.Tensor:
-    """Rainbow: one noise apply per actor stream, `[num_streams, noise_stride]` float32 on the device, for
+    """Noisy layers: one noise apply per actor stream, `[num_streams, noise_stride]` float32 on the device, for
     `act_batch(..., stream_noise=...)`.  Same generator and counter as `generate_randomness` (which it advances); the
     returned view is overwritten by the next call."""
-    if self._stream_noise is None and self.kind == 'rainbow':
+    if self._stream_noise is None and noisy_layers(self.net):
       self._stream_noise = torch.zeros((self.batch_size, self.noise_stride), dtype=torch.float32, device=self.device)
     buf = self._stream_noise
     _lib.call('dz_learner_generate_stream_noise', self._h, seed, int(num_streams), 0 if buf is None else buf.data_ptr(),
@@ -420,7 +442,7 @@ class Learner:
     sp, fp = self.s_ids.data_ptr(), self.s_f64.data_ptr()
     io.sample_out = _lib.SampleOutputs(sp, sp + 8 * B, sp + 16 * B, fp, fp + 8 * B)
     io.d_taus = self.taus.data_ptr() if draws_taus(self.kind) else 0
-    io.d_noise = self.noise.data_ptr() if self.kind == 'rainbow' else 0
+    io.d_noise = self.noise.data_ptr() if noisy_layers(self.net) else 0
     io.update_out = _lib.UpdateOutputs(self.loss.data_ptr(), self.per_example.data_ptr(), self.priorities.data_ptr(),
                                        self.grad_norm.data_ptr())
     io.d_max_seen_priority = self.max_seen_priority.data_ptr()
@@ -479,7 +501,7 @@ class Actor:
     self.q = torch.zeros((E, net.num_actions), dtype=torch.float32, device=dev)
     self.actions = torch.zeros(E, dtype=torch.int32, device=dev)
     self.taus = torch.zeros((E, net.tau_samples_policy), dtype=torch.float32, device=dev) if draws_taus(net.kind) else None
-    rb = net.kind == 'rainbow'
+    rb = noisy_layers(net)
     self.noise = torch.zeros(learner.noise_stride, dtype=torch.float32, device=dev) if rb else None
     self.stream_noise = torch.zeros((E, learner.noise_stride), dtype=torch.float32, device=dev) if rb else None
     self.loaded = False
@@ -570,9 +592,9 @@ class Actor:
     actor: its own counter).  For E <= batch_size the draws equal `Learner.generate_randomness` /
     `generate_stream_noise` at the same seed and counter."""
     kind = self.kind
-    if per_stream and kind != 'rainbow':
-      raise ValueError('per_stream randomness needs a rainbow learner')
-    if not draws_taus(kind) and kind != 'rainbow':
+    if per_stream and not noisy_layers(self.net):
+      raise ValueError('per_stream randomness needs a learner with noisy layers')
+    if not draws_taus(kind) and not noisy_layers(self.net):
       raise ValueError('%s acting draws no randomness' % kind)
     buf = self.taus if draws_taus(kind) else (self.stream_noise if per_stream else self.noise)
     _lib.call('dz_actor_generate_randomness', self._h, seed, 1 if per_stream else 0, buf.data_ptr(), _cstream())
@@ -596,7 +618,7 @@ class Actor:
       raise ValueError('explore must be [2, %d], got %s' % (E, tuple(x.shape)))
     if t is not None and draws_taus(L.kind) and t.numel() != E * L.net.tau_samples_policy:
       raise ValueError('taus must be [%d, %d], got %s' % (E, L.net.tau_samples_policy, tuple(t.shape)))
-    if noise_ld == 0 and n is not None and L.kind == 'rainbow' and n.numel() < L.noise_stride:
+    if noise_ld == 0 and n is not None and noisy_layers(L.net) and n.numel() < L.noise_stride:
       raise ValueError('noise must hold one apply (%d floats), got %d' % (L.noise_stride, n.numel()))
     _lib.call('dz_actor_act', self._h, obs.data_ptr(), _ptr(t), _ptr(n), noise_ld, _ptr(x), float(epsilon), self.q.data_ptr(),
               self.actions.data_ptr(), _cstream())

@@ -356,6 +356,14 @@ typedef struct dz_learner_config {
    * "adv1/b" [512], "adv2/w" [512][A], "adv2/b" [A], "val1/w" [feat][512], "val1/b" [512], "val2/w" [512][1],
    * "val2/b" [1], and the head outputs q_a = v + (adv_a - mean_a adv) in every place the plain network's are read. */
   int32_t dueling;
+  /* 1: noisy networks (Fortunato et al., ICLR 2018; DESIGN.md §17): every layer after the torso is a factorised-noise
+   * layer y = x mu_w + mu_b + ((x * f(eps_in)) sigma_w + sigma_b) * f(eps_out), plain or (with dueling = 1) dueling.
+   * Valid for dqn, double_q, prioritized and munchausen (DZ_EINVAL for any other kind; rainbow's network is noisy
+   * already).  0, as a zero-filled tail leaves it: no noise.  Each layer L of the network ("fc1", "head"; dueling:
+   * "adv1", "adv2", "val1", "val2") holds "L/mu/w", "L/mu/b", "L/sigma/w", "L/sigma/b" in that order after the conv
+   * tensors.  The learner then takes noise exactly as rainbow does: noise_floats = 3 applies, dz_learner_noise_stride,
+   * per-stream acting noise and the actor's draws. */
+  int32_t noisy;
 } dz_learner_config;
 
 typedef struct dz_learner_plan {
@@ -363,7 +371,7 @@ typedef struct dz_learner_plan {
   int32_t num_tensors;
   int64_t opt_state_floats;  /* 2*param_count (adam: mu,nu; rmsprop: mu,nu) */
   int64_t workspace_bytes;
-  int64_t noise_floats;      /* rainbow: floats of factorised noise for ONE update (3 applies) */
+  int64_t noise_floats;      /* rainbow and noisy networks: floats of factorised noise for ONE update (3 applies) */
   int64_t tau_floats;        /* iqn / munchausen_iqn: batch*(N+K+N'); fqf: 0 (its taus live in the workspace) */
 } dz_learner_plan;
 
@@ -399,7 +407,9 @@ typedef struct dz_batch {
   const float* d_weights;              /* [B] importance weights (float32) or NULL -> 1 */
   const float* d_taus;                 /* iqn: [B*N | B*K | B*N'] in U[0,1)  (iqn/agent.py:182-190) or NULL; fqf: unused */
   const float* d_noise;                /* rainbow: 3 applies x 8 vectors in the order of networks.py:235-248 (adv1 in/out,
-                                          adv2 in/out, val1 in/out, val2 in/out), each padded to a multiple of 4 floats; or NULL */
+                                          adv2 in/out, val1 in/out, val2 in/out), each padded to a multiple of 4 floats; or NULL.
+                                          noisy networks: the same 3 applies (online(s_tm1) | the middle pass | target(s_t)),
+                                          each fc1 in/out, head in/out (dueling: rainbow's 8 vectors with one atom) */
 } dz_batch;
 
 typedef struct dz_update_outputs {
@@ -446,7 +456,7 @@ int dz_learner_generate_randomness_async(dz_learner* l, uint64_t seed, float* d_
  * draw left to the host.
  *   d_obs      E contiguous uint8 observations (obs_h*obs_w*obs_c bytes each), device memory
  *   d_taus     iqn: [E][tau_samples_policy] (fqf: NULL, its fractions are proposed from the torso features)
- *   d_noise    rainbow: noise_ld = 0, ONE apply shared by the E streams of the tick (they explore in lockstep);
+ *   d_noise    rainbow and noisy networks: noise_ld = 0, ONE apply shared by the E streams of the tick (they explore in lockstep);
  *              noise_ld = dz_learner_noise_stride, [E][stride] and stream e uses apply e (rainbow/agent.py:125-133 run
  *              by E actors, each drawing its own noise).  When every row carries the same apply the q-values and
  *              actions equal the shared mode's bit for bit.  Other kinds: noise_ld = 0.
@@ -458,11 +468,12 @@ int dz_learner_act_batch(dz_learner* l, const uint8_t* d_obs, int32_t E, const f
                          int64_t noise_ld, const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions,
                          void* stream);
 
-/* Floats of ONE rainbow noise apply (the 8 factorised-noise vectors, each padded to 4 floats); DZ_EINVAL for other kinds. */
+/* Floats of ONE noise apply (rainbow: the 8 factorised-noise vectors; a noisy network: its 4 or 8; each padded to 4
+ * floats); DZ_EINVAL for a network without noisy layers. */
 int dz_learner_noise_stride(const dz_learner_config* cfg, int64_t* out);
 /* E noise applies ([E][stride] floats) for dz_learner_act_batch's per-stream noise from the generator of
  * dz_learner_generate_randomness (same seed and counter: the first min(E, 3) applies equal what it writes); advances
- * d_counters[1] once.  DZ_EINVAL for a non-rainbow learner, E outside [1, batch] or a NULL buffer. */
+ * d_counters[1] once.  DZ_EINVAL for a learner without noisy layers, E outside [1, batch] or a NULL buffer. */
 int dz_learner_generate_stream_noise(dz_learner* l, uint64_t seed, int32_t E, float* d_noise, void* stream);
 
 /* ---- Acting context (SURVEY §8(f) #3: many actor streams per GPU) ----------------------------------------------
@@ -470,21 +481,21 @@ int dz_learner_generate_stream_noise(dz_learner* l, uint64_t seed, int32_t E, fl
  * fqf: num_streams * num_fractions <= 16384)
  * over the learner's ONLINE parameters, read in place: an act enqueued on the stream after a learner step sees that
  * step's parameters.  The actor keeps the learner handle (destroy the actor first) and owns only buffers sized for its
- * streams.  On the tensor-core geometries the torso and the 3136 -> 512 layer (rainbow: with one shared noise apply)
- * run on the learner's sm_90a tensor-core kernels; the heads, and rainbow's per-stream noisy layers, on the fp32-FMA
+ * streams.  On the tensor-core geometries the torso and the 3136 -> 512 layer (noisy layers: with one shared noise
+ * apply) run on the learner's sm_90a tensor-core kernels; the heads, and per-stream noisy layers, on the fp32-FMA
  * kernels.  Row e's result does not depend on num_streams. */
 typedef struct dz_actor dz_actor;
 /* Device workspace bytes of an actor for num_streams streams.  DZ_EINVAL outside the caps. */
 int dz_actor_plan_query(const dz_learner_config* cfg, int32_t num_streams, int64_t* workspace_bytes);
 int dz_actor_create(dz_learner* l, int32_t num_streams, void* d_workspace, dz_actor** out);
 void dz_actor_destroy(dz_actor* a);
-/* dz_learner_act_batch's contract for exactly num_streams observations (E below).  Rainbow: noise_ld = 0, d_noise is
+/* dz_learner_act_batch's contract for exactly num_streams observations (E below).  Noisy layers: noise_ld = 0, d_noise is
  * one apply shared by the streams; noise_ld = dz_learner_noise_stride, d_noise is [E][stride] and stream e uses apply e.
  * DZ_EINVAL for a NULL buffer, a missing taus / noise or another noise_ld. */
 int dz_actor_act(dz_actor* a, const uint8_t* d_obs, const float* d_taus, const float* d_noise, int64_t noise_ld,
                  const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream);
 /* The learner's generator and counter (d_counters[1], advanced once): iqn taus [E][tau_samples_policy] with the stream
- * of dz_learner_generate_randomness's taus; rainbow one noise apply, or E applies when per_stream is set, with the
+ * of dz_learner_generate_randomness's taus; rainbow and noisy networks one noise apply, or E applies when per_stream is set, with the
  * stream of its noise (so for E <= batch the draws equal those calls' for the same seed and counter).  DZ_EINVAL for
  * other kinds (fqf included: it draws nothing), per_stream on iqn or a NULL buffer. */
 int dz_actor_generate_randomness(dz_actor* a, uint64_t seed, int32_t per_stream, float* d_out, void* stream);

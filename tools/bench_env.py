@@ -138,12 +138,14 @@ def bench_driver(game='catch'):
 
 
 # -- learning ----------------------------------------------------------------------------------------------------------
-def learning_agent(seed, train_frames, kind='dqn', num_actions=6, dueling=False):
+def learning_agent(seed, train_frames, kind='dqn', num_actions=6, dueling=False, noisy=False):
   """dqn at the reference's hyper-parameters but for a faster schedule: replay of 100k transitions, learning from 10k,
   epsilon 1 -> 0.01 over the first quarter of the frames, target sync every 8000 frames.  `kind='rainbow'`: the same
   schedule with rainbow's prioritized replay (exponent 0.5, importance exponent 0.4 -> 1 over the run), 3-step returns,
   noisy greedy acting and its 51-atom support on [-10, 10].  `kind='double_q'`: dqn's schedule with the double Q-learning
-  target.  `dueling`: the dueling network (DESIGN.md §16) in place of dqn's fc1 / head."""
+  target.  `dueling`: the dueling network (DESIGN.md §16) in place of dqn's fc1 / head.  `noisy`: noisy networks
+  (DESIGN.md §17) with an epsilon schedule that is zero throughout, so that the agent explores through its noise alone
+  (NoisyNet-DQN for dqn)."""
   from dqn_zoo_b200 import agent as ag
   from dqn_zoo_b200 import learner as dl
   from dqn_zoo_b200 import parts
@@ -151,7 +153,8 @@ def learning_agent(seed, train_frames, kind='dqn', num_actions=6, dueling=False)
   rs = np.random.RandomState(seed)
   capacity, min_fill = 100000, 10000
   structure = dr.Transition(None, None, None, None, None)
-  common = dict(preprocessor=None, sample_network_input=None, network=dl.NetworkSpec(kind, num_actions, dueling=dueling),
+  common = dict(preprocessor=None, sample_network_input=None, network=dl.NetworkSpec(kind, num_actions, dueling=dueling,
+                                                                                          noisy=noisy),
                 optimizer=None, batch_size=32, min_replay_capacity_fraction=min_fill / capacity, learn_period=16,
                 target_network_update_period=8000, rng_key=[0, seed + 1])
   if kind == 'rainbow':
@@ -163,6 +166,8 @@ def learning_agent(seed, train_frames, kind='dqn', num_actions=6, dueling=False)
   rep = dr.TransitionReplay(capacity, structure, rs, frame_dedup=True)
   epsilon = parts.LinearSchedule(begin_t=4 * min_fill, decay_steps=max(train_frames // 4, 1), begin_value=1.0,
                                  end_value=0.01)
+  if noisy:
+    epsilon = lambda t: 0.0
   if kind == 'fqf':   # dqn's schedule, 32 fractions, kappa 1 and the fraction layer's default RMSProp
     return ag.Fqf(transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep, exploration_epsilon=epsilon,
                   huber_param=1.0, **common)
@@ -197,13 +202,13 @@ def evaluate(learner, seed, num_streams=64, game='catch', num_actions=6):
 
 
 def learning_run(train_frames, seed=0, num_streams=32, eval_every=0, log=None, game='catch', num_actions=6,
-                 kind='dqn', dueling=False):
-  """Trains `learning_agent` (of `kind`, on the dueling network with `dueling`) from `num_streams` streams of `game` for `train_frames` frames (training episodes are not
+                 kind='dqn', dueling=False, noisy=False):
+  """Trains `learning_agent` (of `kind`, on the dueling network with `dueling`, with noisy layers with `noisy`) from `num_streams` streams of `game` for `train_frames` frames (training episodes are not
   truncated); evaluates every `eval_every` frames (0: at the end only).  Returns [(frames, mean eval return, eval
   episodes, train episode return)]."""
   import run_synthetic
   from dqn_zoo_b200 import agent as ag
-  agent = learning_agent(seed, train_frames, kind, num_actions, dueling)
+  agent = learning_agent(seed, train_frames, kind, num_actions, dueling, noisy)
   trainer = ag.VectorTrainer(agent, num_streams=num_streams, rng_key=[0, seed + 4])
   env = make_env(game, num_streams, seed + 5, num_actions)
   loop = run_synthetic.StreamLoop(trainer, env, train_frames, 0)
@@ -225,6 +230,8 @@ def main():
   ap.add_argument('--agent', default='dqn', choices=['dqn', 'double_q', 'rainbow', 'munchausen', 'iqn', 'munchausen_iqn', 'fqf'],
                   help='the agent of the learning curve')
   ap.add_argument('--dueling', action='store_true', help='the learning curve on the dueling network (DESIGN.md §16)')
+  ap.add_argument('--noisy', action='store_true',
+                  help='the learning curve on noisy networks with a zero epsilon schedule (DESIGN.md §17)')
   ap.add_argument('--parts', default='env,train,eval,driver')
   ap.add_argument('--frames', type=int, default=65536, help='frames per timed window of env_train / env_eval')
   ap.add_argument('--learning', type=int, default=0, help='frames of the learning curve (0: none)')
@@ -249,9 +256,10 @@ def main():
   if a.learning:
     t0 = time.perf_counter()
     learning_run(a.learning, a.seed, eval_every=a.eval_every, game=a.game, kind=a.agent, dueling=a.dueling,
-                 log=lambda **kw: emit(metric='learning', **_tag(a.game), **({} if a.agent == 'dqn' else
+                 noisy=a.noisy, log=lambda **kw: emit(metric='learning', **_tag(a.game), **({} if a.agent == 'dqn' else
                                                                               {'agent': a.agent}),
                                        **({'dueling': True} if a.dueling else {}),
+                                       **({'noisy': True} if a.noisy else {}),
                                        seed=a.seed, wall_s=round(time.perf_counter() - t0, 1), **kw))
   emit(metric='device_after', **bench_train.device_info())
 

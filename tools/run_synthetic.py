@@ -92,9 +92,11 @@ def build_train_agent(args, random_state, preprocessor):
                                                     1e-3, True, random_state)
   else:
     replay = replay_lib.TransitionReplay(args.replay_capacity, structure, random_state)
-  network = learner_lib.NetworkSpec(kind, args.num_actions, dueling=args.dueling)
+  network = learner_lib.NetworkSpec(kind, args.num_actions, dueling=args.dueling, noisy=args.noisy)
   epsilon = parts.LinearSchedule(begin_t=int(args.min_replay_capacity_fraction * args.replay_capacity * 4),
                                  decay_steps=max(args.num_train_frames, 1), begin_value=1.0, end_value=0.01)
+  if args.noisy:   # noisy networks explore through their noise: a zero schedule (NoisyNet-DQN for dqn)
+    epsilon = lambda t: 0.0
   common = dict(preprocessor=preprocessor, sample_network_input=np.zeros((84, 84, 4), np.uint8), network=network, optimizer=None,
                 transition_accumulator=replay_lib.NStepTransitionAccumulator(n_step), replay=replay, batch_size=32,
                 min_replay_capacity_fraction=args.min_replay_capacity_fraction, learn_period=16,
@@ -262,6 +264,9 @@ def parse_args(argv=None):
                            'munchausen_iqn', 'fqf'])
   ap.add_argument('--dueling', action='store_true',
                   help='the dueling network (DESIGN.md §16): dqn, double_q, prioritized and munchausen only')
+  ap.add_argument('--noisy', action='store_true',
+                  help='noisy networks (DESIGN.md §17) with a zero epsilon schedule: dqn, double_q, prioritized and '
+                       'munchausen only; combines with --dueling')
   ap.add_argument('--num_actions', type=int, default=6)
   ap.add_argument('--replay_capacity', type=int, default=20000)
   ap.add_argument('--min_replay_capacity_fraction', type=float, default=0.05)
