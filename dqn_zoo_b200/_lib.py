@@ -210,7 +210,15 @@ _SIGNATURES = {
     'dz_test_dueling_example': (i32, [vp, f32, vp, i32, vp]),
     'dz_test_loss': (i32, [C.POINTER(LearnerConfig), i32, C.POINTER(vp), C.POINTER(vp), vp, vp, vp, vp, vp, vp, vp, vp, vp,
                            vp, vp, vp, vp]),
+    'dz_test_loss_fqf': (i32, [C.POINTER(LearnerConfig), i32, C.POINTER(vp), vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                               vp]),
     'dz_test_q_values': (i32, [C.POINTER(LearnerConfig), i32, vp, vp, vp, f32, vp, vp, vp]),
+    'dz_test_q_values_fqf': (i32, [C.POINTER(LearnerConfig), i32, vp, vp, vp, f32, vp, vp, vp]),
+    'dz_test_fraction_forward': (i32, [vp, i32, i32, C.POINTER(vp), vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
+                                       C.POINTER(vp), vp, vp, vp]),
+    'dz_test_dueling_head_fwd': (i32, [vp, i32, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), i64, C.POINTER(vp), vp]),
+    'dz_test_dueling_head_bwd': (i32, [vp, i32, vp, vp, C.POINTER(vp), vp, vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
+                                       vp]),
     'dz_test_copy': (i32, [vp, vp, i64, vp]),
     'dz_test_learner_trace': (i32, [vp, C.c_char_p, vp]),
     'dz_test_learner_mma_path': (i32, [vp, C.c_char_p, C.POINTER(i32)]),

@@ -291,8 +291,10 @@ __host__ __device__ inline float miqn_target(const float* zbar_j, const float* p
 // same order, and the result of example e does not depend on how many examples a launch holds.
 constexpr int kFqfMaxFractions = 128;   // pass 2 holds 2N rows per example: within the 256 rows of the IQN tau limit
 
-// logits [N] -> q = softmax(logits), tau_0 = 0, tau_i = sum_{k<i} q_k, tau_N = 1, tau_hat_i = (tau_i + tau_{i+1}) / 2 and
-// the interval weights w_i = tau_{i+1} - tau_i.  tau has N + 1 entries; any output may alias nothing else.
+// logits [N] -> q = softmax(logits), tau_0 = 0, tau_i = min(sum_{k<i} q_k, 1), tau_N = 1, tau_hat_i = (tau_i +
+// tau_{i+1}) / 2 and the interval weights w_i = tau_{i+1} - tau_i.  The float32 prefix sum can round above 1 when the
+// last fractions are small; the clamp keeps 0 <= tau_i <= tau_{i+1} <= 1, so w_i >= 0 and tau_i <= tau_hat_i <= tau_{i+1}
+// hold exactly.  tau has N + 1 entries; any output may alias nothing else.
 __host__ __device__ inline void fqf_fractions(const float* logits, int N, float* q, float* tau, float* tau_hat, float* w) {
   float m = logits[0];
   for (int i = 1; i < N; ++i) m = fmaxf(m, logits[i]);
@@ -300,7 +302,7 @@ __host__ __device__ inline void fqf_fractions(const float* logits, int N, float*
   for (int i = 0; i < N; ++i) { q[i] = expf(logits[i] - m); s += q[i]; }
   for (int i = 0; i < N; ++i) q[i] = q[i] / s;
   tau[0] = 0.f;
-  for (int i = 1; i < N; ++i) tau[i] = tau[i - 1] + q[i - 1];
+  for (int i = 1; i < N; ++i) tau[i] = fminf(tau[i - 1] + q[i - 1], 1.f);
   tau[N] = 1.f;
   for (int i = 0; i < N; ++i) {
     tau_hat[i] = (tau[i] + tau[i + 1]) * 0.5f;
@@ -2351,6 +2353,62 @@ int forward_heads_plain(dz_learner* l, const NetBufs& nb, const Pass* passes, in
   return DZ_OK;
 }
 
+// The dueling head of `np` passes over `rows` rows: dueling_head_fwd_kernel, or for the noisy dueling network
+// noisy_dueling_head_fwd_kernel.  Pass i reads h1[i][0] / h1[i][1] (advantage / value stream [rows][512]) and the head
+// of params[i], and writes q [rows][A] to out[i]; noisy: through noise apply noise[i], or with noise_ld > 0 row r's
+// apply at noise[i] + r * noise_ld.  The learner's forwards and dz_test_dueling_head_fwd run this function.
+int launch_dueling_head_fwd(const dz_learner* l, int rows, int np, const float* const (*h1)[2], const float* const* params,
+                            float* const* out, const float* const* noise, long long noise_ld, void* stream) {
+  const ParamOffsets& o = l->po;
+  const dz_learner_config& c = l->cfg;
+  NoisyDuelingFwdArgs a;
+  memset(&a, 0, sizeof(a));
+  for (int i = 0; i < np; ++i) {
+    a.h.h1[i][0] = h1[i][0]; a.h.h1[i][1] = h1[i][1];
+    a.h.params[i] = params[i]; a.h.out[i] = out[i];
+  }
+  for (int s = 0; s < 2; ++s) { a.h.off_w[s] = o.w2[s]; a.h.off_b[s] = o.b2[s]; }
+  a.h.rows = rows; a.h.A = c.num_actions;
+  const dim3 grid((unsigned)ceil_div(rows, 8), (unsigned)np);
+  if (!noisy_net(c)) {
+    DZ_LAUNCH_NAMED("dueling_head_fwd", dueling_head_fwd_kernel, grid, 256, 0, stream, a.h);
+    return DZ_OK;
+  }
+  const NoiseLayout nl = noise_layout(c, l->d);
+  for (int i = 0; i < np; ++i) a.noise[i] = noise[i];
+  for (int s = 0; s < 2; ++s) { a.off_sw[s] = o.sw2[s]; a.off_sb[s] = o.sb2[s]; }
+  a.off_in[0] = nl.a2i; a.off_out[0] = nl.a2o; a.off_in[1] = nl.v2i; a.off_out[1] = nl.v2o;
+  a.noise_ld = noise_ld;
+  DZ_LAUNCH_NAMED("noisy_dueling_head_fwd", noisy_dueling_head_fwd_kernel, grid, 256, 0, stream, a);
+  return DZ_OK;
+}
+
+// The dueling head's backward over `rows` rows of online(s_tm1): dueling_head_bwd_kernel, or for the noisy dueling
+// network noisy_dueling_head_bwd_kernel through noise apply `noise`.  dq [rows][A] becomes dadv in place, dval [rows]
+// is written, and both streams' dh1 [rows][512] from the head of `params`, masked by h1 > 0; with hi / lo (NULL: none)
+// also their tf32 hi/lo pair.  The learner's backwards and dz_test_dueling_head_bwd run this function.
+int launch_dueling_head_bwd(const dz_learner* l, int rows, float* dq, float* dval, const float* const* h1, const float* params,
+                            float* const* dh1, float* const* hi, float* const* lo, const float* noise, void* stream) {
+  const ParamOffsets& o = l->po;
+  const dz_learner_config& c = l->cfg;
+  NoisyDuelingBwdArgs a;
+  memset(&a, 0, sizeof(a));
+  a.g.dq = dq; a.g.dval = dval; a.g.B = rows; a.g.A = c.num_actions;
+  for (int s = 0; s < 2; ++s) {
+    a.g.h1[s] = h1[s]; a.g.W[s] = params + o.w2[s]; a.g.dh1[s] = dh1[s];
+    if (hi) { a.g.hi[s] = hi[s]; a.g.lo[s] = lo[s]; }
+  }
+  if (!noisy_net(c)) {
+    DZ_LAUNCH_NAMED("dueling_head_bwd", dueling_head_bwd_kernel, (unsigned)ceil_div(rows, 8), 256, 0, stream, a.g);
+    return DZ_OK;
+  }
+  const NoiseVecs nz = noise_of(c, l->d, noise, 0);
+  for (int s = 0; s < 2; ++s) a.S[s] = params + o.sw2[s];
+  a.ein[0] = nz.a2i; a.eout[0] = nz.a2o; a.ein[1] = nz.v2i; a.eout[1] = nz.v2o;
+  DZ_LAUNCH_NAMED("noisy_dueling_head_bwd", noisy_dueling_head_bwd_kernel, (unsigned)ceil_div(rows, 8), 256, 0, stream, a);
+  return DZ_OK;
+}
+
 // Noisy layers (networks.py:137-178): rainbow's two streams (:224-261), the noisy plain network's one and the noisy
 // dueling network's two (DESIGN.md §17).  The 3136 -> 512 layers are one grouped noisy launch; the heads are one
 // grouped noisy launch (rainbow's mu has no bias, the noisy networks' has), or for the noisy dueling network one
@@ -2396,22 +2454,18 @@ int forward_heads_noisy(dz_learner* l, const NetBufs& nb, const Pass* passes, in
     if (splits > 1) DZ_TRY(finish_nn(gb, outs, true, stream, noise_ld));
   }
   if (c.kind != DZ_RAINBOW && ns == 2) {
-    NoisyDuelingFwdArgs a;
-    memset(&a, 0, sizeof(a));
-    const NoiseLayout nl = noise_layout(c, d);
+    const float* h1[3][2];
+    const float* prm[3];
+    float* out[3];
+    const float* noise_at[3];
+    const int64_t stride = noise_layout(c, d).stride;
     for (int i = 0; i < np; ++i) {
       const int hp = passes[i].head;
-      a.h.h1[i][0] = nb.h1[hp][0]; a.h.h1[i][1] = nb.h1[hp][1];
-      a.h.params[i] = passes[i].params; a.h.out[i] = nb.out[hp];
-      a.noise[i] = noise + (int64_t)passes[i].apply * nl.stride;
+      h1[i][0] = nb.h1[hp][0]; h1[i][1] = nb.h1[hp][1];
+      prm[i] = passes[i].params; out[i] = nb.out[hp];
+      noise_at[i] = noise + (int64_t)passes[i].apply * stride;
     }
-    for (int s = 0; s < 2; ++s) { a.h.off_w[s] = o.w2[s]; a.h.off_b[s] = o.b2[s]; a.off_sw[s] = o.sw2[s]; a.off_sb[s] = o.sb2[s]; }
-    a.off_in[0] = nl.a2i; a.off_out[0] = nl.a2o; a.off_in[1] = nl.v2i; a.off_out[1] = nl.v2o;
-    a.noise_ld = noise_ld;
-    a.h.rows = nimg; a.h.A = c.num_actions;
-    DZ_LAUNCH_NAMED("noisy_dueling_head_fwd", noisy_dueling_head_fwd_kernel, dim3((unsigned)ceil_div(nimg, 8), (unsigned)np), 256, 0,
-                    stream, a);
-    return DZ_OK;
+    return launch_dueling_head_fwd(l, nimg, np, h1, prm, out, noise_at, noise_ld, stream);
   }
   for (int i = 0; i < np; ++i) {
     NoiseVecs nz = noise_of(c, d, noise, passes[i].apply);
@@ -2471,17 +2525,15 @@ int forward_heads_dueling(dz_learner* l, const NetBufs& nb, const Pass* passes, 
     DZ_TRY(run_nn("fc1_fwd", gb, false, stream));
     if (splits > 1) DZ_TRY(finish_nn(gb, outs, false, stream));
   }
-  DuelingFwdArgs h;
-  memset(&h, 0, sizeof(h));
+  const float* h1[3][2];
+  const float* prm[3];
+  float* out[3];
   for (int i = 0; i < np; ++i) {
     const int hp = passes[i].head;
-    h.h1[i][0] = nb.h1[hp][0]; h.h1[i][1] = nb.h1[hp][1];
-    h.params[i] = passes[i].params; h.out[i] = nb.out[hp];
+    h1[i][0] = nb.h1[hp][0]; h1[i][1] = nb.h1[hp][1];
+    prm[i] = passes[i].params; out[i] = nb.out[hp];
   }
-  for (int s = 0; s < 2; ++s) { h.off_w[s] = o.w2[s]; h.off_b[s] = o.b2[s]; }
-  h.rows = nimg; h.A = l->cfg.num_actions;
-  DZ_LAUNCH_NAMED("dueling_head_fwd", dueling_head_fwd_kernel, dim3((unsigned)ceil_div(nimg, 8), (unsigned)np), 256, 0, stream, h);
-  return DZ_OK;
+  return launch_dueling_head_fwd(l, nimg, np, h1, prm, out, nullptr, 0, stream);
 }
 
 // IQN embedding (latent -> 3136, ReLU, * state embedding) and 3136 -> 512 layer of the three network applies of
@@ -2816,6 +2868,17 @@ int backward_plain(dz_learner* l, void* stream) {
   return DZ_OK;
 }
 
+// The dueling head's backward on the learner's buffers (noise apply 0 of `noise` for the noisy dueling network):
+// dout -> dadv in place, dval -> doutv, both streams' dh1 and, on the tensor-core path, their tf32 hi/lo pair.
+int dueling_head_bwd_of(dz_learner* l, const float* noise, void* stream) {
+  const float* h1[2] = {l->h1[0][0], l->h1[0][1]};
+  float* hi[2] = {nullptr, nullptr};
+  float* lo[2] = {nullptr, nullptr};
+  if (l->um)
+    for (int s = 0; s < 2; ++s) { hi[s] = um_dh1_hi(l->um, s); lo[s] = um_dh1_lo(l->um, s); }
+  return launch_dueling_head_bwd(l, l->B, l->dout, l->doutv, h1, l->buf.d_online, l->dh1, hi, lo, noise, stream);
+}
+
 // The backward of forward_heads_noisy's networks through online(s_tm1) (noise apply 0).  The heads: rainbow's and the
 // noisy plain network's input gradient is a noisy run_nt and a finish that masks dh1 (and, on the tensor-core path,
 // writes its tf32 hi/lo pair); the noisy dueling network's is noisy_dueling_head_bwd_kernel.  Every weight gradient is a
@@ -2831,18 +2894,7 @@ int backward_noisy(dz_learner* l, const float* noise, void* stream) {
   float* G = l->buf.d_grads;
   const float* P = l->buf.d_online;
   NoiseVecs nz = noise_of(c, d, noise, 0);
-  if (dueling_head) {   // dout -> dadv in place, dval -> doutv, both streams' dh1
-    NoisyDuelingBwdArgs a;
-    memset(&a, 0, sizeof(a));
-    a.g.dq = l->dout; a.g.dval = l->doutv; a.g.B = B; a.g.A = c.num_actions;
-    for (int s = 0; s < 2; ++s) {
-      a.g.h1[s] = l->h1[0][s]; a.g.W[s] = P + o.w2[s]; a.g.dh1[s] = l->dh1[s];
-      if (l->um) { a.g.hi[s] = um_dh1_hi(l->um, s); a.g.lo[s] = um_dh1_lo(l->um, s); }
-      a.S[s] = P + o.sw2[s];
-    }
-    a.ein[0] = nz.a2i; a.eout[0] = nz.a2o; a.ein[1] = nz.v2i; a.eout[1] = nz.v2o;
-    DZ_LAUNCH_NAMED("noisy_dueling_head_bwd", noisy_dueling_head_bwd_kernel, (unsigned)ceil_div(B, 8), 256, 0, stream, a);
-  }
+  if (dueling_head) DZ_TRY(dueling_head_bwd_of(l, noise, stream));   // dout -> dadv in place, dval -> doutv, both dh1
   GemmBatch gb;
   gb.n = ns;
   for (int s = 0; s < ns; ++s) {  // second noisy layer weight grads
@@ -2913,16 +2965,7 @@ int backward_dueling(dz_learner* l, void* stream) {
   const int B = l->B, A = l->cfg.num_actions;
   float* G = l->buf.d_grads;
   const float* P = l->buf.d_online;
-  {
-    DuelingBwdArgs a;
-    memset(&a, 0, sizeof(a));
-    a.dq = l->dout; a.dval = l->doutv; a.B = B; a.A = A;
-    for (int s = 0; s < 2; ++s) {
-      a.h1[s] = l->h1[0][s]; a.W[s] = P + o.w2[s]; a.dh1[s] = l->dh1[s];
-      if (l->um) { a.hi[s] = um_dh1_hi(l->um, s); a.lo[s] = um_dh1_lo(l->um, s); }
-    }
-    DZ_LAUNCH_NAMED("dueling_head_bwd", dueling_head_bwd_kernel, (unsigned)ceil_div(B, 8), 256, 0, stream, a);
-  }
+  DZ_TRY(dueling_head_bwd_of(l, nullptr, stream));
   GemmBatch gb;
   gb.n = 2;
   for (int s = 0; s < 2; ++s) {  // adv2 / val2 weight and bias gradients
@@ -3177,7 +3220,8 @@ int run_optimizer(dz_learner* l, float* user_norm, bool apply, void* stream) {
 // and rainbow's running max priority when max_seen is given).  L carries the buffers: head outputs, batch, outputs and
 // loss_terms; every field that follows from the configuration (sizes, vmax, bound, kappa, whether priorities are
 // written) is set here.  With `side`, loss_mean_kernel runs on the side stream forked after the loss kernel and
-// *mean_stream receives it; without, everything runs on `stream`.  dz_test_loss runs this same function.
+// *mean_stream receives it; without, everything runs on `stream`.  dz_test_loss and dz_test_loss_fqf run this same
+// function.
 int launch_loss(const dz_learner_config& c, LossArgs& L, int B, void* stream, SideStream* side, float* d_loss, float* max_seen,
                 void** mean_stream, const FqfLossArgs* fqf = nullptr) {
   L.kind = c.kind; L.B = B; L.A = c.num_actions; L.atoms = c.num_atoms;
@@ -3217,7 +3261,8 @@ int launch_loss(const dz_learner_config& c, LossArgs& L, int B, void* stream, Si
 
 // The acting tail of a head pass over E observations: q-values [E][A] (q_values_kernel) and, when `actions` is given,
 // the epsilon-greedy choice (act_select_kernel).  out: the head outputs of the pass (rainbow: the advantage stream),
-// val: rainbow's value stream.  The acting body (the learner's and the actor's) and dz_test_q_values run this function.
+// val: rainbow's value stream.  The acting body (the learner's and the actor's), dz_test_q_values and
+// dz_test_q_values_fqf run this function.
 // fqf: `frac_w` holds the interval weights [E][N] of the pass's proposals (q_values_fqf_kernel).
 int launch_q_values(const dz_learner_config& c, int E, const float* out, const float* val, const float* explore, float epsilon,
                     float* q, int32_t* actions, void* stream, const float* frac_w = nullptr) {
@@ -4031,12 +4076,13 @@ int dz_test_dueling_example(const float* adv, float v, const float* dq, int32_t 
   return DZ_OK;
 }
 
-// Test hook: the learner's loss section (launch_loss) on caller-owned head outputs, batch and output buffers, all on
-// `stream`.  The observation fields of cfg play no part; they are replaced by a legal geometry before validate().
-int dz_test_loss(const dz_learner_config* cfg, int32_t B, const float* const* d_out, const float* const* d_val,
-                 const int32_t* d_a_tm1, const float* d_r_t, const float* d_discount_t, const float* d_weights,
-                 const float* d_taus, float* d_dout, float* d_dval, float* d_per_example, float* d_priorities,
-                 float* d_loss_terms, float* d_loss, float* d_max_seen, void* stream) {
+// The body of dz_test_loss and dz_test_loss_fqf: the learner's loss section (launch_loss) on caller-owned head outputs,
+// batch and output buffers, all on `stream`; fqf: its fraction buffers.  The observation fields of cfg play no part;
+// they are replaced by a legal geometry before validate().
+static int test_loss_section(const dz_learner_config* cfg, int32_t B, const float* const* d_out, const float* const* d_val,
+                             const int32_t* d_a_tm1, const float* d_r_t, const float* d_discount_t, const float* d_weights,
+                             const float* d_taus, float* d_dout, float* d_dval, float* d_per_example, float* d_priorities,
+                             float* d_loss_terms, float* d_loss, float* d_max_seen, const FqfLossArgs* fqf, void* stream) {
   if (!cfg || !d_out) return fail(DZ_EINVAL, "test_loss: NULL argument");
   dz_learner_config c = *cfg;
   c.batch = B; c.obs_h = 84; c.obs_w = 84; c.obs_c = 4;
@@ -4056,19 +4102,109 @@ int dz_test_loss(const dz_learner_config* cfg, int32_t B, const float* const* d_
   L.a = d_a_tm1; L.r = d_r_t; L.disc = d_discount_t; L.w = d_weights; L.taus0 = d_taus;
   L.dout = d_dout; L.dadv = d_dout; L.dval = d_dval;
   L.per_example = d_per_example; L.loss_terms = d_loss_terms; L.priorities = d_priorities;
-  return launch_loss(c, L, B, stream, nullptr, d_loss, d_max_seen, nullptr);
+  return launch_loss(c, L, B, stream, nullptr, d_loss, d_max_seen, nullptr, fqf);
 }
 
-// Test hook: the acting tail (launch_q_values) on caller-owned head outputs of E observations.
-int dz_test_q_values(const dz_learner_config* cfg, int32_t E, const float* d_out, const float* d_val, const float* d_explore,
-                     float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
+// Test hook: the loss section of every kind but fqf, whose loss needs the fraction buffers of dz_test_loss_fqf.
+int dz_test_loss(const dz_learner_config* cfg, int32_t B, const float* const* d_out, const float* const* d_val,
+                 const int32_t* d_a_tm1, const float* d_r_t, const float* d_discount_t, const float* d_weights,
+                 const float* d_taus, float* d_dout, float* d_dval, float* d_per_example, float* d_priorities,
+                 float* d_loss_terms, float* d_loss, float* d_max_seen, void* stream) {
+  return test_loss_section(cfg, B, d_out, d_val, d_a_tm1, d_r_t, d_discount_t, d_weights, d_taus, d_dout, d_dval,
+                           d_per_example, d_priorities, d_loss_terms, d_loss, d_max_seen, nullptr, stream);
+}
+
+// Test hook: fqf's loss section (loss_fqf_kernel, then loss_mean_kernel) with the fraction buffers.
+int dz_test_loss_fqf(const dz_learner_config* cfg, int32_t B, const float* const* d_out, const int32_t* d_a_tm1,
+                     const float* d_r_t, const float* d_discount_t, const float* d_weights, const float* d_tau_hat,
+                     const float* d_w_t, const float* d_q_tm1, float* d_dout, float* d_dlogits, float* d_per_example,
+                     float* d_loss_terms, float* d_loss, void* stream) {
+  if (!cfg || !proposes_fractions(cfg->kind)) return fail(DZ_EINVAL, "test_loss_fqf: the configuration is not fqf");
+  if (!d_tau_hat || !d_w_t || !d_q_tm1 || !d_dlogits)
+    return fail(DZ_EINVAL, "test_loss_fqf: tau_hat, w_t, q_tm1 and dlogits [B][num_fractions] are required");
+  const FqfLossArgs fl{d_w_t, d_q_tm1, d_dlogits};
+  return test_loss_section(cfg, B, d_out, nullptr, d_a_tm1, d_r_t, d_discount_t, d_weights, d_tau_hat, d_dout, nullptr,
+                           d_per_example, nullptr, d_loss_terms, d_loss, nullptr, &fl, stream);
+}
+
+// The body of dz_test_q_values and dz_test_q_values_fqf: the acting tail (launch_q_values) on caller-owned head outputs
+// of E observations; fqf: with the interval weights frac_w.
+static int test_q_values_tail(const dz_learner_config* cfg, int32_t E, const float* d_out, const float* d_val,
+                              const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions,
+                              const float* d_frac_w, void* stream) {
   if (!cfg) return fail(DZ_EINVAL, "test_q_values: NULL config");
   dz_learner_config c = *cfg;
   c.obs_h = 84; c.obs_w = 84; c.obs_c = 4;
   DZ_TRY(validate(c));
   if (E < 1) return fail(DZ_EINVAL, "test_q_values: E must be >= 1");
   if (!d_out || !d_q_out || (c.kind == DZ_RAINBOW && !d_val)) return fail(DZ_EINVAL, "test_q_values: NULL buffer");
-  return launch_q_values(c, E, d_out, d_val, d_explore, epsilon, d_q_out, d_actions, stream);
+  return launch_q_values(c, E, d_out, d_val, d_explore, epsilon, d_q_out, d_actions, stream, d_frac_w);
+}
+
+// Test hook: the acting tail of every kind but fqf (dz_test_q_values_fqf).
+int dz_test_q_values(const dz_learner_config* cfg, int32_t E, const float* d_out, const float* d_val, const float* d_explore,
+                     float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
+  return test_q_values_tail(cfg, E, d_out, d_val, d_explore, epsilon, d_q_out, d_actions, nullptr, stream);
+}
+
+// Test hook: fqf's acting tail (q_values_fqf_kernel, act_select_kernel) with the interval weights.
+int dz_test_q_values_fqf(const dz_learner_config* cfg, int32_t E, const float* d_out, const float* d_frac_w,
+                         const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream) {
+  if (!cfg || !proposes_fractions(cfg->kind)) return fail(DZ_EINVAL, "test_q_values_fqf: the configuration is not fqf");
+  if (!d_frac_w) return fail(DZ_EINVAL, "test_q_values_fqf: NULL interval weights");
+  return test_q_values_tail(cfg, E, d_out, nullptr, d_explore, epsilon, d_q_out, d_actions, d_frac_w, stream);
+}
+
+// Test hook: the fraction proposal (launch_fraction_forward) of an fqf learner's layout on caller-owned buffers.
+int dz_test_fraction_forward(dz_learner* l, int32_t E, int32_t napp, const float* const* d_feat, const float* d_params,
+                             float* const* d_tau, float* const* d_tau_hat, float* const* d_w, float* const* d_q,
+                             float* d_pass1, float* d_pass2, void* stream) {
+  if (!l || !d_feat || !d_params) return fail(DZ_EINVAL, "test_fraction_forward: NULL argument");
+  if (!proposes_fractions(l->cfg.kind)) return fail(DZ_EINVAL, "test_fraction_forward: the learner is not fqf");
+  if (E < 1 || napp < 1 || napp > 2) return fail(DZ_EINVAL, "test_fraction_forward: E >= 1 and napp in {1, 2}");
+  FracArgs f;
+  memset(&f, 0, sizeof(f));
+  for (int a = 0; a < napp; ++a) {
+    if (!d_feat[a]) return fail(DZ_EINVAL, "test_fraction_forward: NULL features");
+    f.feat[a] = d_feat[a];
+    if (d_tau) f.tau[a] = d_tau[a];
+    if (d_tau_hat) f.tau_hat[a] = d_tau_hat[a];
+    if (d_w) f.w[a] = d_w[a];
+    if (d_q) f.q[a] = d_q[a];
+  }
+  f.pass1 = d_pass1; f.pass2 = d_pass2;
+  return launch_fraction_forward(l, f, d_params, E, napp, stream);
+}
+
+// Test hook: the dueling head forward (launch_dueling_head_fwd) of a dueling learner's layout on caller-owned buffers.
+int dz_test_dueling_head_fwd(dz_learner* l, int32_t rows, int32_t np, const float* const* d_h1, const float* const* d_params,
+                             const float* const* d_noise, int64_t noise_ld, float* const* d_out, void* stream) {
+  if (!l || !d_h1 || !d_params || !d_out) return fail(DZ_EINVAL, "test_dueling_head_fwd: NULL argument");
+  const dz_learner_config& c = l->cfg;
+  if (!two_streams(c) || c.kind == DZ_RAINBOW) return fail(DZ_EINVAL, "test_dueling_head_fwd: the learner is not dueling");
+  if (rows < 1 || np < 1 || np > 3 || noise_ld < 0) return fail(DZ_EINVAL, "test_dueling_head_fwd: rows, np or noise_ld out of range");
+  if (noisy_net(c) ? !d_noise : noise_ld != 0) return fail(DZ_EINVAL, "test_dueling_head_fwd: noise only for the noisy network");
+  const float* h1[3][2];
+  for (int i = 0; i < np; ++i) {
+    h1[i][0] = d_h1[2 * i]; h1[i][1] = d_h1[2 * i + 1];
+    if (!h1[i][0] || !h1[i][1] || !d_params[i] || !d_out[i] || (d_noise && !d_noise[i]))
+      return fail(DZ_EINVAL, "test_dueling_head_fwd: NULL buffer");
+  }
+  return launch_dueling_head_fwd(l, rows, np, h1, d_params, d_out, d_noise, noise_ld, stream);
+}
+
+// Test hook: the dueling head backward (launch_dueling_head_bwd) of a dueling learner's layout on caller-owned buffers.
+int dz_test_dueling_head_bwd(dz_learner* l, int32_t rows, float* d_dq, float* d_dval, const float* const* d_h1,
+                             const float* d_params, const float* d_noise, float* const* d_dh1, float* const* d_hi,
+                             float* const* d_lo, void* stream) {
+  if (!l || !d_dq || !d_dval || !d_h1 || !d_params || !d_dh1) return fail(DZ_EINVAL, "test_dueling_head_bwd: NULL argument");
+  const dz_learner_config& c = l->cfg;
+  if (!two_streams(c) || c.kind == DZ_RAINBOW) return fail(DZ_EINVAL, "test_dueling_head_bwd: the learner is not dueling");
+  if (rows < 1) return fail(DZ_EINVAL, "test_dueling_head_bwd: rows must be >= 1");
+  if (noisy_net(c) && !d_noise) return fail(DZ_EINVAL, "test_dueling_head_bwd: the noisy network needs its noise apply");
+  if (!d_h1[0] || !d_h1[1] || !d_dh1[0] || !d_dh1[1] || (!d_hi != !d_lo) || (d_hi && (!d_hi[0] || !d_hi[1] || !d_lo[0] || !d_lo[1])))
+    return fail(DZ_EINVAL, "test_dueling_head_bwd: NULL buffer");
+  return launch_dueling_head_bwd(l, rows, d_dq, d_dval, d_h1, d_params, d_dh1, d_hi, d_lo, d_noise, stream);
 }
 
 // Test hook: device pointer + element count of an internal activation / gradient buffer (tests and tools only).

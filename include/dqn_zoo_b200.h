@@ -704,17 +704,48 @@ int dz_test_dueling_example(const float* adv, float v, const float* dq, int32_t 
  * munchausen / munchausen_iqn: 1 is target(s_tm1)).  d_weights: importance weights [B] or NULL; d_taus: the s_tm1
  * taus [B][N_tm1] (iqn, munchausen_iqn).  Writes d_dout (the gradient wrt pass 0; rainbow: advantages, with d_dval the
  * value stream), d_per_example, d_priorities (prioritized, rainbow), d_loss_terms [B], d_loss [1] and, when d_max_seen
- * is given for rainbow, the running max priority. */
+ * is given for rainbow, the running max priority.  fqf's loss needs its fraction buffers: dz_test_loss_fqf. */
 int dz_test_loss(const dz_learner_config* cfg, int32_t B, const float* const* d_out, const float* const* d_val,
                  const int32_t* d_a_tm1, const float* d_r_t, const float* d_discount_t, const float* d_weights,
                  const float* d_taus, float* d_dout, float* d_dval, float* d_per_example, float* d_priorities,
                  float* d_loss_terms, float* d_loss, float* d_max_seen, void* stream);
+/* fqf's loss section on caller-owned device buffers, as dz_test_loss; tests only.  N = num_fractions: d_out[0]
+ * online(s_tm1) at tau_hat [B][N][A], d_out[1] online(s_tm1) at tau_1..tau_N [B][N][A] (the last row, tau_N = 1, is not
+ * read), d_out[2] target(s_t) at [tau_hat' | tau_hat] [B][2N][A]; d_tau_hat [B][N], d_w_t the interval weights of
+ * s_t's proposal [B][N], d_q_tm1 the fractions of s_tm1's [B][N].  Writes d_dout [B][N][A], d_dlogits [B][N],
+ * d_per_example, d_loss_terms [B] and d_loss [1]. */
+int dz_test_loss_fqf(const dz_learner_config* cfg, int32_t B, const float* const* d_out, const int32_t* d_a_tm1,
+                     const float* d_r_t, const float* d_discount_t, const float* d_weights, const float* d_tau_hat,
+                     const float* d_w_t, const float* d_q_tm1, float* d_dout, float* d_dlogits, float* d_per_example,
+                     float* d_loss_terms, float* d_loss, void* stream);
 /* The acting tail of every acting entry point on caller-owned device buffers; tests only.  d_out: the head outputs of
  * E observations in the layout of d_out[p] above (iqn: tau_samples_policy samples; rainbow: advantages, d_val the value
  * streams).  Writes the q-values d_q_out [E][A] and, when d_actions is given, the epsilon-greedy actions as
- * dz_learner_act_batch does (d_explore: [2][E] uniforms or NULL). */
+ * dz_learner_act_batch does (d_explore: [2][E] uniforms or NULL).  fqf: dz_test_q_values_fqf. */
 int dz_test_q_values(const dz_learner_config* cfg, int32_t E, const float* d_out, const float* d_val, const float* d_explore,
                      float epsilon, float* d_q_out, int32_t* d_actions, void* stream);
+/* fqf's acting tail, as dz_test_q_values: d_out [E][N][A] at tau_hat and d_frac_w the interval weights [E][N]. */
+int dz_test_q_values_fqf(const dz_learner_config* cfg, int32_t E, const float* d_out, const float* d_frac_w,
+                         const float* d_explore, float epsilon, float* d_q_out, int32_t* d_actions, void* stream);
+/* fqf's fraction proposal of learner l's layout (num_fractions N, feature width D, the fraction layer of d_params) on
+ * caller-owned buffers; tests only.  d_feat: host array of napp (1 or 2) device features [E][D].  d_tau [E][N + 1],
+ * d_tau_hat, d_w, d_q [E][N]: host arrays of 2 device pointers, any of them (or the array) NULL; d_pass1 [E][N] and
+ * d_pass2 [E][2N] (the learner's pass inputs) may be NULL. */
+int dz_test_fraction_forward(dz_learner* l, int32_t E, int32_t napp, const float* const* d_feat, const float* d_params,
+                             float* const* d_tau, float* const* d_tau_hat, float* const* d_w, float* const* d_q,
+                             float* d_pass1, float* d_pass2, void* stream);
+/* The dueling head forward of dueling learner l's layout (plain or noisy) on caller-owned buffers; tests only.  np in
+ * 1..3 passes of `rows` rows: d_h1 host array [np][2] of device [rows][512] (advantage, value stream), d_params[i] a
+ * parameter blob, d_out[i] q [rows][A].  Noisy: d_noise[i] the pass's noise apply (noise_ld > 0: row r's apply at
+ * d_noise[i] + r * noise_ld); NULL and 0 for the plain network. */
+int dz_test_dueling_head_fwd(dz_learner* l, int32_t rows, int32_t np, const float* const* d_h1, const float* const* d_params,
+                             const float* const* d_noise, int64_t noise_ld, float* const* d_out, void* stream);
+/* The dueling head backward of dueling learner l's layout on caller-owned buffers; tests only.  d_dq [rows][A] becomes
+ * dadv in place; writes d_dval [rows] and d_dh1[s] [rows][512] (host array of 2) masked by d_h1[s] > 0 and, when d_hi /
+ * d_lo (host arrays of 2, or NULL) are given, the tf32 hi/lo pair of each dh1.  Noisy: d_noise is the noise apply. */
+int dz_test_dueling_head_bwd(dz_learner* l, int32_t rows, float* d_dq, float* d_dval, const float* const* d_h1,
+                             const float* d_params, const float* d_noise, float* const* d_dh1, float* const* d_hi,
+                             float* const* d_lo, void* stream);
 int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream);   /* device-to-device, tests only */
 /* Debug: the tensor-core launch named `tag` writes the clock stamps of its CTA 0 into d_trace (512 int64). */
 int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace);

@@ -234,6 +234,45 @@ def test_host_twin_within_the_float32_budget(N):
   print('fqf host twin N=%d: worst error / budget %.3f' % (N, worst))
 
 
+def assert_fraction_invariant(tau, hat, w, N):
+  """0 = tau_0 <= tau_1 <= ... <= tau_N = 1, w_i = tau_{i+1} - tau_i >= 0 and tau_i <= tau_hat_i <= tau_{i+1}, exactly in
+  float32 (tau [..., N + 1], hat and w [..., N])."""
+  tau, hat, w = (np.asarray(x, np.float32) for x in (tau, hat, w))
+  assert (tau[..., 0] == 0).all() and (tau[..., N] == 1).all()
+  assert (np.diff(tau, axis=-1) >= 0).all() and (tau <= 1).all(), tau.max()
+  assert (w >= 0).all() and (w == tau[..., 1:] - tau[..., :-1]).all()
+  assert (tau[..., :-1] <= hat).all() and (hat <= tau[..., 1:]).all() and (hat <= 1).all()
+
+
+@pytest.mark.parametrize('N', [2, 3, 11, 19, 27, 31, 32, 127, 128])
+def test_host_twin_fractions_stay_ordered_inside_0_1(N):
+  """A saturated last logit leaves the float32 prefix sum of the other N - 1 fractions free to round above 1 (at N = 11
+  with logits (0, ..., 0, -30) it gives 1 + 2^-23); the fractions are clamped to 1 so that the invariant holds."""
+  from dqn_zoo_b200 import _lib
+  rs = np.random.RandomState(100 + N)
+  cases = [np.concatenate([np.zeros(N - 1), [-30.0]])]
+  for _ in range(60):
+    lg = rs.standard_normal(N)
+    lg[-1] = -rs.uniform(20, 90)   # the last fraction's share is below float32's rounding of the others' sum
+    cases.append(lg)
+  for lead in (0, N // 2):         # one fraction takes every other's mass
+    lg = np.full(N, -100.0)
+    lg[lead] = 0.0
+    cases.append(lg)
+  cases.append(np.linspace(-80, 80, N))
+  z = np.zeros(N, np.float32)
+  for lg in cases:
+    lg = lg.astype(np.float32)
+    out = np.zeros(5 * N + 1, np.float32)
+    _lib.call('dz_test_fqf_example', lg.ctypes.data, z.ctypes.data, z.ctypes.data, N, 1.0, out.ctypes.data)
+    tau, hat, w = out[N:2 * N + 1], out[2 * N + 1:3 * N + 1], out[3 * N + 1:4 * N + 1]
+    assert_fraction_invariant(tau, hat, w, N)
+    p = fo.proposal(torch.tensor(lg.astype(np.float64))[None])
+    R = float(np.abs(lg.astype(np.float64) - lg.max()).max())
+    T = (2 * N + 4 + 2 * R) * U   # the clamp only moves a tau that rounded above 1 back towards the float64 value
+    assert np.abs(tau - p['tau'][0].numpy()).max() <= T
+
+
 # ---- configuration checks and the Python surface ---------------------------------------------------------------------
 
 def _cfg(kind, **fields):
@@ -276,6 +315,14 @@ def test_library_validates_the_fraction_configuration():
   x = np.zeros(129, np.float32)
   with pytest.raises(ValueError):
     _lib.call('dz_test_fqf_example', x.ctypes.data, x.ctypes.data, x.ctypes.data, 129, 1.0, out.ctypes.data)
+  # fqf's loss and acting hooks take only an fqf configuration and its fraction buffers
+  heads = (ctypes.c_void_p * 3)(1, 1, 1)
+  for kind, w in (('iqn', 1), ('fqf', None)):
+    with pytest.raises(ValueError, match='test_loss_fqf'):
+      _lib.call('dz_test_loss_fqf', ctypes.byref(_cfg(kind)), 32, heads, 1, 1, 1, None, 1, w, 1, 1, 1, 1, 1, 1, None)
+    if w:
+      with pytest.raises(ValueError, match='test_q_values_fqf'):
+        _lib.call('dz_test_q_values_fqf', ctypes.byref(_cfg(kind)), 4, 1, 1, None, 0.0, 1, None, None)
 
 
 def test_parameter_layout_and_python_surface():
