@@ -20,7 +20,7 @@
 // launch (dz_gemm.cuh); the replay gather is fused into conv1's operand load.
 #include <algorithm>
 #include <cmath>
-#include <map>
+#include <string>
 #include <vector>
 
 #include "dz_async.cuh"
@@ -46,6 +46,8 @@ __host__ __device__ constexpr bool uses_dqn_net(int kind) { return kind == DZ_DQ
 constexpr int net_kind(int kind) { return uses_iqn_net(kind) ? DZ_IQN : uses_dqn_net(kind) ? DZ_DQN : kind; }
 // The Munchausen kinds: alpha / tau / l0 are validated, and the target network also applies to s_tm1.
 constexpr bool is_munchausen(int kind) { return kind == DZ_MUNCHAUSEN || kind == DZ_MUNCHAUSEN_IQN; }
+// The kinds whose online network also applies to s_t (double-Q action selection): online(s_tm1) | online(s_t) | target(s_t).
+constexpr bool online_applies_to_s_t(int kind) { return kind == DZ_DOUBLE_Q || kind == DZ_PRIORITIZED || kind == DZ_RAINBOW; }
 // The kinds that may take the dueling network (DESIGN.md §16) and noisy layers (§17): their losses read one scalar q per
 // action.
 constexpr bool dueling_allowed(int kind) {
@@ -91,80 +93,33 @@ static Dims make_dims(const dz_learner_config& c) {
   return d;
 }
 
-struct Layout {
-  std::vector<TensorInfo> t;
-  std::map<std::string, int> index;
-  int64_t total = 0;
-  void add(const std::string& name, std::initializer_list<int64_t> shape) {
-    TensorInfo ti;
-    ti.name = name;
-    ti.ndim = (int)shape.size();
-    ti.count = 1;
-    int i = 0;
-    for (auto s : shape) { ti.shape[i++] = s; ti.count *= s; }
-    for (; i < 4; ++i) ti.shape[i] = 1;
-    ti.offset = total;
-    total += (ti.count + 3) / 4 * 4;  // keep every tensor 16-byte aligned for float4 loads
-    index[name] = (int)t.size();
-    t.push_back(ti);
-  }
-  int64_t off(const std::string& name) const {   // -1: no such tensor
-    auto it = index.find(name);
-    return it == index.end() ? -1 : t[it->second].offset;
-  }
+// The layers after the torso of every network but IQN's (which has stream 0 only, with plain layers): one or two
+// streams (two: the advantage stream s = 0, then the value stream), each a 3136 -> 512 layer and a head, plain or noisy.
+// Rainbow's streams are noisy with GEMM heads; the dueling network's head is one kernel over both streams.
+struct FcNet {
+  int ns;               // streams
+  bool noisy;           // factorised-noise layers: mu and sigma tensors, noise vectors, dual GEMMs
+  bool dueling_head;    // the head is dueling_head_fwd/bwd_kernel (or its noisy variant); else a grouped GEMM per stream
+  int64_t out[2];       // each stream's head width: d.out; the value stream's num_atoms for rainbow, 1 for dueling
+  bool head_mu_bias;    // the head has a mu bias (rainbow's has none: with_bias=False)
+  bool shared_bias;     // head/b has shape {1} (plain double_q / prioritized)
 };
 
-static Layout make_layout(const dz_learner_config& c) {
-  Layout L;
-  Dims d = make_dims(c);
-  L.add("conv1/w", {8, 8, d.C, 32}); L.add("conv1/b", {32});
-  L.add("conv2/w", {4, 4, 32, 64});  L.add("conv2/b", {64});
-  L.add("conv3/w", {3, 3, 64, 64});  L.add("conv3/b", {64});
-  if (c.kind == DZ_RAINBOW) {
-    const char* streams[2] = {"adv", "val"};
-    for (int s = 0; s < 2; ++s) {
-      std::string p = streams[s];
-      int64_t n_out = s == 0 ? (int64_t)c.num_actions * c.num_atoms : c.num_atoms;
-      L.add(p + "1/mu/w", {d.feat, 512}); L.add(p + "1/mu/b", {512});
-      L.add(p + "1/sigma/w", {d.feat, 512}); L.add(p + "1/sigma/b", {512});
-      L.add(p + "2/mu/w", {512, n_out}); L.add(p + "2/sigma/w", {512, n_out}); L.add(p + "2/sigma/b", {n_out});
-    }
-    return L;
-  }
-  if (c.noisy) {   // DESIGN.md §17: mu w, mu b, sigma w, sigma b of each layer; dueling: the advantage stream first
-    const char* plain[2] = {"fc1", "head"};
-    const char* dueling[4] = {"adv1", "adv2", "val1", "val2"};
-    for (int i = 0; i < (c.dueling ? 4 : 2); ++i) {
-      const std::string p = c.dueling ? dueling[i] : plain[i];
-      const int64_t n_in = i % 2 ? 512 : d.feat, n_out = i % 2 == 0 ? 512 : i == 1 ? c.num_actions : 1;
-      L.add(p + "/mu/w", {n_in, n_out}); L.add(p + "/mu/b", {n_out});
-      L.add(p + "/sigma/w", {n_in, n_out}); L.add(p + "/sigma/b", {n_out});
-    }
-    return L;
-  }
-  if (c.dueling) {   // advantage stream first, as rainbow's, so that stream index s means the same in both networks
-    const char* streams[2] = {"adv", "val"};
-    for (int s = 0; s < 2; ++s) {
-      const std::string p = streams[s];
-      const int64_t n_out = s == 0 ? c.num_actions : 1;
-      L.add(p + "1/w", {d.feat, 512}); L.add(p + "1/b", {512});
-      L.add(p + "2/w", {512, n_out}); L.add(p + "2/b", {n_out});
-    }
-    return L;
-  }
-  if (uses_iqn_net(c.kind)) { L.add("embed/w", {c.latent_dim, d.feat}); L.add("embed/b", {d.feat}); }
-  L.add("fc1/w", {d.feat, 512}); L.add("fc1/b", {512});
-  L.add("head/w", {512, d.out});
-  bool shared = c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED;
-  L.add("head/b", {shared ? 1 : d.out});
-  // fqf: the fraction proposal layer, last, so that it is one contiguous tail of the blob for its optimizer launch
-  if (proposes_fractions(c.kind)) { L.add("fraction/w", {d.feat, c.num_fractions}); L.add("fraction/b", {c.num_fractions}); }
-  return L;
+static FcNet fc_net(const dz_learner_config& c, const Dims& d) {
+  const bool rb = c.kind == DZ_RAINBOW;
+  FcNet f;
+  f.ns = two_streams(c) ? 2 : 1;
+  f.noisy = noisy_net(c);
+  f.dueling_head = f.ns == 2 && !rb;
+  f.out[0] = d.out;
+  f.out[1] = f.ns == 2 ? (rb ? c.num_atoms : 1) : 0;
+  f.head_mu_bias = !rb;
+  f.shared_bias = f.ns == 1 && !f.noisy && (c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED);
+  return f;
 }
 
 // Offsets into a parameter blob of every tensor the step's launches address; -1 where the agent kind has no such tensor.
-// Stream s = 0 is fc1 (two streams: the advantage stream), s = 1 the value stream.  Layer 1 is the 512-wide layer,
-// layer 2 the head (plain heads: head/w, head/b; rainbow's mu has no bias).  sw / sb: noisy sigma weight / bias.
+// Stream s as in FcNet.  Layer 1 is the 512-wide layer, layer 2 the head; w / b are plain or mu, sw / sb noisy sigma.
 struct ParamOffsets {
   int64_t conv_w[3], conv_b[3];
   int64_t w1[2], b1[2], sw1[2], sb1[2];
@@ -174,55 +129,69 @@ struct ParamOffsets {
   int64_t fc_begin;   // first offset after the conv tensors
 };
 
-static int param_offsets(const dz_learner_config& c, const Layout& L, ParamOffsets* out) {
-  ParamOffsets o;
-  bool missing = false;
-  auto need = [&](const std::string& name) {
-    const int64_t off = L.off(name);
-    missing |= off < 0;
-    return off;
-  };
-  for (int i = 0; i < 3; ++i) {
-    const std::string conv = "conv" + std::to_string(i + 1);
-    o.conv_w[i] = need(conv + "/w"); o.conv_b[i] = need(conv + "/b");
+struct Layout {
+  std::vector<TensorInfo> t;
+  int64_t total = 0;
+  int64_t add(const std::string& name, std::initializer_list<int64_t> shape) {
+    TensorInfo ti;
+    ti.name = name;
+    ti.ndim = (int)shape.size();
+    ti.count = 1;
+    int i = 0;
+    for (auto s : shape) { ti.shape[i++] = s; ti.count *= s; }
+    for (; i < 4; ++i) ti.shape[i] = 1;
+    ti.offset = total;
+    total += (ti.count + 3) / 4 * 4;  // keep every tensor 16-byte aligned for float4 loads
+    t.push_back(ti);
+    return ti.offset;
   }
+};
+
+// The parameter layout of cfg's network, and in *po (when given) the offset of every tensor the step addresses.  After
+// the conv tensors: iqn's embedding, the layers of FcNet stream by stream (advantage stream first, so that stream index
+// s means the same in rainbow and the dueling network), then fqf's fraction layer.  A plain layer is w, b; a noisy one
+// (DESIGN.md §17) mu/w, mu/b, sigma/w, sigma/b.  One stream names its layers fc1 / head, two streams adv1 / adv2 and
+// val1 / val2.
+static Layout make_layout(const dz_learner_config& c, ParamOffsets* po = nullptr) {
+  Layout L;
+  ParamOffsets o;
+  const Dims d = make_dims(c);
+  const FcNet f = fc_net(c, d);
+  o.conv_w[0] = L.add("conv1/w", {8, 8, d.C, 32}); o.conv_b[0] = L.add("conv1/b", {32});
+  o.conv_w[1] = L.add("conv2/w", {4, 4, 32, 64});  o.conv_b[1] = L.add("conv2/b", {64});
+  o.conv_w[2] = L.add("conv3/w", {3, 3, 64, 64});  o.conv_b[2] = L.add("conv3/b", {64});
   for (int s = 0; s < 2; ++s) {
     o.w1[s] = o.b1[s] = o.sw1[s] = o.sb1[s] = -1;
     o.w2[s] = o.b2[s] = o.sw2[s] = o.sb2[s] = -1;
   }
   o.embed_w = o.embed_b = -1;
   o.frac_w = o.frac_b = -1;
-  if (c.kind == DZ_RAINBOW) {
-    const char* streams[2] = {"adv", "val"};
-    for (int s = 0; s < 2; ++s) {
-      const std::string p = streams[s];
-      o.w1[s] = need(p + "1/mu/w"); o.b1[s] = need(p + "1/mu/b"); o.sw1[s] = need(p + "1/sigma/w"); o.sb1[s] = need(p + "1/sigma/b");
-      o.w2[s] = need(p + "2/mu/w"); o.sw2[s] = need(p + "2/sigma/w"); o.sb2[s] = need(p + "2/sigma/b");
+  if (uses_iqn_net(c.kind)) { o.embed_w = L.add("embed/w", {c.latent_dim, d.feat}); o.embed_b = L.add("embed/b", {d.feat}); }
+  const char* streams[2] = {"adv", "val"};
+  for (int s = 0; s < f.ns; ++s)
+    for (int layer = 1; layer <= 2; ++layer) {
+      const std::string p = f.ns == 2 ? streams[s] + std::to_string(layer) : layer == 1 ? "fc1" : "head";
+      const bool head = layer == 2;
+      const int64_t n_in = head ? 512 : d.feat, n_out = head ? f.out[s] : 512;
+      int64_t* w = head ? o.w2 : o.w1;
+      int64_t* b = head ? o.b2 : o.b1;
+      if (!f.noisy) {
+        w[s] = L.add(p + "/w", {n_in, n_out});
+        b[s] = L.add(p + "/b", {head && f.shared_bias ? 1 : n_out});
+        continue;
+      }
+      w[s] = L.add(p + "/mu/w", {n_in, n_out});
+      if (!head || f.head_mu_bias) b[s] = L.add(p + "/mu/b", {n_out});
+      (head ? o.sw2 : o.sw1)[s] = L.add(p + "/sigma/w", {n_in, n_out});
+      (head ? o.sb2 : o.sb1)[s] = L.add(p + "/sigma/b", {n_out});
     }
-  } else if (c.noisy) {
-    const char* streams[2] = {"adv", "val"};
-    for (int s = 0; s < (c.dueling ? 2 : 1); ++s) {
-      const std::string p1 = c.dueling ? std::string(streams[s]) + "1" : "fc1";
-      const std::string p2 = c.dueling ? std::string(streams[s]) + "2" : "head";
-      o.w1[s] = need(p1 + "/mu/w"); o.b1[s] = need(p1 + "/mu/b"); o.sw1[s] = need(p1 + "/sigma/w"); o.sb1[s] = need(p1 + "/sigma/b");
-      o.w2[s] = need(p2 + "/mu/w"); o.b2[s] = need(p2 + "/mu/b"); o.sw2[s] = need(p2 + "/sigma/w"); o.sb2[s] = need(p2 + "/sigma/b");
-    }
-  } else if (c.dueling) {
-    const char* streams[2] = {"adv", "val"};
-    for (int s = 0; s < 2; ++s) {
-      const std::string p = streams[s];
-      o.w1[s] = need(p + "1/w"); o.b1[s] = need(p + "1/b"); o.w2[s] = need(p + "2/w"); o.b2[s] = need(p + "2/b");
-    }
-  } else {
-    o.w1[0] = need("fc1/w"); o.b1[0] = need("fc1/b");
-    o.w2[0] = need("head/w"); o.b2[0] = need("head/b");
-    if (uses_iqn_net(c.kind)) { o.embed_w = need("embed/w"); o.embed_b = need("embed/b"); }
-    if (proposes_fractions(c.kind)) { o.frac_w = need("fraction/w"); o.frac_b = need("fraction/b"); }
+  // fqf: the fraction proposal layer, last, so that it is one contiguous tail of the blob for its optimizer launch
+  if (proposes_fractions(c.kind)) {
+    o.frac_w = L.add("fraction/w", {d.feat, c.num_fractions}); o.frac_b = L.add("fraction/b", {c.num_fractions});
   }
   o.fc_begin = uses_iqn_net(c.kind) ? o.embed_w : o.w1[0];
-  if (missing) return fail(DZ_EINVAL, "parameter layout lacks a tensor of this agent kind");
-  *out = o;
-  return DZ_OK;
+  if (po) *po = o;
+  return L;
 }
 
 struct Bump {
@@ -1872,6 +1841,7 @@ struct dz_learner {
   Layout lay;
   ParamOffsets po;
   Dims d;
+  FcNet fc;        // the layers after the torso
   int B;           // train batch
   int n_head[3];   // rows per image in the head stage for pass 0/1/2 (IQN: tau samples; others 1)
   // workspace (floats unless noted)
@@ -1885,7 +1855,7 @@ struct dz_learner {
   float* nn_partial;                        // split-K partials for the M=batch FC layers and heads
   float* conv_partial;                      // split-K partials for conv2/conv3 forward
   float* nt_partial;                        // split partials of the input-gradient (NT) GEMMs
-  float *dout, *doutv, *dh1[2], *dact3, *dtmp[2], *dcol, *dact2, *dact1, *dhi;
+  float *dout, *doutv, *dh1[2], *dact3, *dcol, *dact2, *dact1, *dhi;
   float* tn_partial[4];                     // conv1/2/3 wgrad partials, [3] = iqn head/embed partial
   float *loss_terms, *scalars;              // scalars: [0]=norm, [1]=shared-bias scratch.., [8..]=norm partials
   unsigned int* ticket;
@@ -1946,7 +1916,8 @@ int64_t carve(dz_learner* l, char* base) {
   const Dims& d = l->d;
   const int B = c.batch;
   Bump w{base};
-  const bool rb = c.kind == DZ_RAINBOW, two = two_streams(c), iqn = uses_iqn_net(c.kind);
+  const FcNet& f = l->fc;
+  const bool two = f.ns == 2, gemm_val = two && !f.dueling_head, iqn = uses_iqn_net(c.kind);
   int nh[3] = {1, 1, 1};
   if (draws_taus(c.kind)) { nh[0] = c.tau_samples_s_tm1; nh[1] = c.tau_samples_policy; nh[2] = c.tau_samples_s_t; }
   // fqf: online(s_tm1) at tau_hat | online(s_tm1) at tau_1..tau_N | target(s_t) at [tau_hat' | tau_hat]; acting uses pass 1
@@ -1960,7 +1931,7 @@ int64_t carve(dz_learner* l, char* base) {
     l->h1[p][0] = w.take<float>(rows * 512);
     l->h1[p][1] = two ? w.take<float>(rows * 512) : nullptr;
     l->out[p] = w.take<float>(rows * d.out);
-    l->outv[p] = rb ? w.take<float>((int64_t)B * c.num_atoms) : nullptr;
+    l->outv[p] = gemm_val ? w.take<float>((int64_t)B * f.out[1]) : nullptr;
     l->cosf[p] = iqn ? w.take<float>(rows * c.latent_dim) : nullptr;
     l->hi[p] = iqn ? w.take<float>(rows * d.feat) : nullptr;
   }
@@ -1990,12 +1961,10 @@ int64_t carve(dz_learner* l, char* base) {
   int64_t rows0 = (int64_t)B * nh[0];
   l->dout = w.take<float>(rows0 * d.out);
   // the value stream's output gradient: rainbow's [B][atoms], the dueling network's dval [B]
-  l->doutv = two ? w.take<float>((int64_t)B * (rb ? c.num_atoms : 1)) : nullptr;
+  l->doutv = two ? w.take<float>((int64_t)B * f.out[1]) : nullptr;
   l->dh1[0] = w.take<float>(rows0 * 512);
   l->dh1[1] = two ? w.take<float>(rows0 * 512) : nullptr;
   l->dact3 = w.take<float>((int64_t)B * d.feat);
-  l->dtmp[0] = rb ? w.take<float>((int64_t)B * d.feat) : nullptr;
-  l->dtmp[1] = rb ? w.take<float>((int64_t)B * d.feat) : nullptr;
   int64_t col2 = (int64_t)B * d.h2 * d.w2 * 512, col3 = (int64_t)B * d.h3 * d.w3 * 576;
   l->dcol = w.take<float>(col2 > col3 ? col2 : col3);
   l->dact2 = w.take<float>((int64_t)B * d.h2 * d.w2 * 64);
@@ -2061,6 +2030,19 @@ int64_t carve(dz_learner* l, char* base) {
   return w.used;
 }
 
+// A learner with cfg's configuration, layout, parameter offsets, network description, dims and split counts and no
+// device state: carve() without a base leaves every workspace pointer NULL.  Returns the workspace bytes.
+int64_t init_shape_learner(dz_learner* t, const dz_learner_config& cfg) {
+  t->um = nullptr;
+  memset(&t->buf, 0, sizeof(t->buf));
+  t->cfg = cfg;
+  t->lay = make_layout(cfg, &t->po);
+  t->d = make_dims(cfg);
+  t->fc = fc_net(cfg, t->d);
+  t->B = cfg.batch;
+  return carve(t, nullptr);   // the learner's split counts, which the actor's fp32 GEMMs share
+}
+
 // Noise of ONE apply, in this order: adv1_in[feat] adv1_out[512] adv2_in[512] adv2_out[A*atoms] val1_in[feat]
 // val1_out[512] val2_in[512] val2_out[atoms]; every vector starts on a 4-float boundary.  Offsets in floats.  Rainbow;
 // the noisy dueling network with one atom; the noisy plain network has only the first four (fc1 in / out, head in /
@@ -2093,11 +2075,11 @@ UmNetDesc make_um_desc(const dz_learner* l) {
   const ParamOffsets& o = l->po;
   UmNetDesc u;
   memset(&u, 0, sizeof(u));
-  const bool needs_online_st = c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED || c.kind == DZ_RAINBOW;
+  const bool online_st = online_applies_to_s_t(c.kind);
   u.B = c.batch; u.H = d.H; u.W = d.W;
   const bool target_stm1 = is_munchausen(c.kind);   // online(s_tm1) | target(s_tm1) | target(s_t)
-  u.npass = needs_online_st || target_stm1 ? 3 : 2;
-  u.pass_target[0] = 0; u.pass_target[1] = needs_online_st ? 0 : 1; u.pass_target[2] = 1;
+  u.npass = online_st || target_stm1 ? 3 : 2;
+  u.pass_target[0] = 0; u.pass_target[1] = online_st ? 0 : 1; u.pass_target[2] = 1;
   u.online = l->buf.d_online; u.target = l->buf.d_target;
   for (int i = 0; i < 3; ++i) { u.off_conv_w[i] = o.conv_w[i]; u.off_conv_b[i] = o.conv_b[i]; }
   u.use_fc = !uses_iqn_net(c.kind);
@@ -2307,52 +2289,6 @@ int forward_torso(dz_learner* l, const NetBufs& nb, const TorsoJob* jobs, int nj
   return DZ_OK;
 }
 
-// Heads for the dqn / double_q / prioritized / c51 / qrdqn family.
-int forward_heads_plain(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, void* stream, bool fc1_done = false) {
-  const Dims& d = l->d;
-  const ParamOffsets& o = l->po;
-  GemmBatch gb;
-  gb.n = np;
-  float* outs[kMaxProblems];
-  const bool shared = l->cfg.kind == DZ_DOUBLE_Q || l->cfg.kind == DZ_PRIORITIZED;
-  const int splits = nimg <= nb.split_rows ? l->fc_splits : 1;
-  for (int i = 0; i < np && !fc1_done; ++i) {
-    GemmProblem p = zero_problem();
-    p.a_mode = A_PLAIN; p.A = nb.act3[passes[i].set]; p.lda = d.feat; p.M = nimg; p.K = d.feat;
-    p.B = passes[i].params + o.w1[0]; p.N = 512; p.ldb = 512; p.ldc = 512;
-    p.bias = passes[i].params + o.b1[0]; p.relu = 1;
-    outs[i] = nb.h1[passes[i].head][0];
-    if (splits > 1) {
-      p.splits = splits; p.split_stride = (long long)nimg * 512;
-      p.C = nb.nn_partial + (long long)i * splits * p.split_stride;
-    } else {
-      p.C = outs[i];
-    }
-    gb.p[i] = p;
-  }
-  if (!fc1_done) {
-    DZ_TRY(run_nn("fc1_fwd", gb, false, stream));
-    if (splits > 1) DZ_TRY(finish_nn(gb, outs, false, stream));
-  }
-  for (int i = 0; i < np; ++i) {
-    GemmProblem p = zero_problem();
-    p.a_mode = A_PLAIN; p.A = nb.h1[passes[i].head][0]; p.lda = 512; p.M = nimg; p.K = 512;
-    p.B = passes[i].params + o.w2[0]; p.N = d.out; p.ldb = d.out; p.ldc = d.out;
-    p.bias = passes[i].params + o.b2[0]; p.bias_shared = shared ? 1 : 0;
-    outs[i] = nb.out[passes[i].head];
-    if (nimg <= nb.split_rows) {
-      p.splits = l->head_splits; p.split_stride = (long long)nimg * d.out;
-      p.C = nb.nn_partial + (long long)i * p.splits * p.split_stride;
-    } else {
-      p.C = outs[i];
-    }
-    gb.p[i] = p;
-  }
-  DZ_TRY(run_nn("head_fwd", gb, false, stream));
-  if (nimg <= nb.split_rows) DZ_TRY(finish_nn(gb, outs, false, stream));
-  return DZ_OK;
-}
-
 // The dueling head of `np` passes over `rows` rows: dueling_head_fwd_kernel, or for the noisy dueling network
 // noisy_dueling_head_fwd_kernel.  Pass i reads h1[i][0] / h1[i][1] (advantage / value stream [rows][512]) and the head
 // of params[i], and writes q [rows][A] to out[i]; noisy: through noise apply noise[i], or with noise_ld > 0 row r's
@@ -2409,39 +2345,45 @@ int launch_dueling_head_bwd(const dz_learner* l, int rows, float* dq, float* dva
   return DZ_OK;
 }
 
-// Noisy layers (networks.py:137-178): rainbow's two streams (:224-261), the noisy plain network's one and the noisy
-// dueling network's two (DESIGN.md §17).  The 3136 -> 512 layers are one grouped noisy launch; the heads are one
-// grouped noisy launch (rainbow's mu has no bias, the noisy networks' has), or for the noisy dueling network one
-// noisy_dueling_head_fwd_kernel.  noise_ld > 0: image m of the pass uses its own noise apply at noise + m * noise_ld
-// (one pass only); 0: every image uses the pass's apply.
-int forward_heads_noisy(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, const float* noise, void* stream, bool fc1_done = false,
-                        long long noise_ld = 0) {
+// The layers after the torso (FcNet) of `np` passes over `nimg` images: rainbow's and the noisy networks' noisy layers
+// (networks.py:137-178, DESIGN.md §17), the dueling network's streams (§16) and the plain network.  The 3136 -> 512
+// layers of every pass and stream are one grouped launch (skipped with fc1_done: the tensor-core plan wrote h1), then
+// the heads are one dueling head launch or one grouped launch; both GEMM stages split K into nn_partial when the pass
+// has at most split_rows images.  Noisy layers read noise apply passes[i].apply of `noise`; with noise_ld > 0 (one pass
+// only) image m uses its own apply at noise + m * noise_ld.
+int forward_heads_fc(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, const float* noise, void* stream,
+                     bool fc1_done = false, long long noise_ld = 0) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
-  const int ns = two_streams(c) ? 2 : 1;
-  if (ns * np > kMaxProblems) return fail(DZ_EINVAL, "too many noisy passes");
+  const FcNet& f = l->fc;
+  const int ns = f.ns;
+  const int halves = f.noisy ? 2 : 1;   // a noisy problem's split partials carry a second (sigma) half
+  if (ns * np > kMaxProblems) return fail(DZ_EINVAL, "too many passes for one grouped launch");
   if (noise_ld && (np != 1 || fc1_done)) return fail(DZ_EINVAL, "per-row noise: one pass with its own fc1");
   auto run = [&](const char* tag, GemmBatch& b) {
-    return noise_ld ? run_nn_rownoise(tag, b, noise_ld, stream) : run_nn(tag, b, true, stream);
+    return noise_ld ? run_nn_rownoise(tag, b, noise_ld, stream) : run_nn(tag, b, f.noisy, stream);
   };
   GemmBatch gb;
   gb.n = ns * np;
   float* outs[kMaxProblems];
   const int splits = nimg <= nb.split_rows ? l->fc_splits : 1;
   for (int i = 0; i < np && !fc1_done; ++i) {
-    NoiseVecs nz = noise_of(c, d, noise, passes[i].apply);
+    const float* prm = passes[i].params;
+    const NoiseVecs nz = f.noisy ? noise_of(c, d, noise, passes[i].apply) : NoiseVecs{};
     for (int s = 0; s < ns; ++s) {
       GemmProblem p = zero_problem();
       p.a_mode = A_PLAIN; p.A = nb.act3[passes[i].set]; p.lda = d.feat; p.M = nimg; p.K = d.feat;
-      p.B = passes[i].params + o.w1[s]; p.B2 = passes[i].params + o.sw1[s];
-      p.N = 512; p.ldb = 512; p.ldc = 512;
-      p.bias = passes[i].params + o.b1[s]; p.bias2 = passes[i].params + o.sb1[s];
-      p.a_scale = s == 0 ? nz.a1i : nz.v1i; p.c_scale = s == 0 ? nz.a1o : nz.v1o; p.relu = 1;
-      int q = ns * i + s;
+      p.B = prm + o.w1[s]; p.N = 512; p.ldb = 512; p.ldc = 512;
+      p.bias = prm + o.b1[s]; p.relu = 1;
+      if (f.noisy) {
+        p.B2 = prm + o.sw1[s]; p.bias2 = prm + o.sb1[s];
+        p.a_scale = s == 0 ? nz.a1i : nz.v1i; p.c_scale = s == 0 ? nz.a1o : nz.v1o;
+      }
+      const int q = ns * i + s;
       outs[q] = nb.h1[passes[i].head][s];
       if (splits > 1) {
-        p.splits = splits; p.split_stride = (long long)2 * nimg * 512;
+        p.splits = splits; p.split_stride = (long long)halves * nimg * 512;
         p.C = nb.nn_partial + (long long)q * splits * p.split_stride;
       } else {
         p.C = outs[q];
@@ -2450,90 +2392,50 @@ int forward_heads_noisy(dz_learner* l, const NetBufs& nb, const Pass* passes, in
     }
   }
   if (!fc1_done) {
-    DZ_TRY(run("noisy1_fwd", gb));
-    if (splits > 1) DZ_TRY(finish_nn(gb, outs, true, stream, noise_ld));
+    DZ_TRY(run(f.noisy ? "noisy1_fwd" : "fc1_fwd", gb));
+    if (splits > 1) DZ_TRY(finish_nn(gb, outs, f.noisy, stream, noise_ld));
   }
-  if (c.kind != DZ_RAINBOW && ns == 2) {
+  if (f.dueling_head) {
     const float* h1[3][2];
     const float* prm[3];
     float* out[3];
     const float* noise_at[3];
-    const int64_t stride = noise_layout(c, d).stride;
     for (int i = 0; i < np; ++i) {
       const int hp = passes[i].head;
       h1[i][0] = nb.h1[hp][0]; h1[i][1] = nb.h1[hp][1];
       prm[i] = passes[i].params; out[i] = nb.out[hp];
-      noise_at[i] = noise + (int64_t)passes[i].apply * stride;
+      noise_at[i] = f.noisy ? noise + (int64_t)passes[i].apply * noise_layout(c, d).stride : nullptr;
     }
     return launch_dueling_head_fwd(l, nimg, np, h1, prm, out, noise_at, noise_ld, stream);
   }
+  const bool split_head = nimg <= nb.split_rows;
   for (int i = 0; i < np; ++i) {
-    NoiseVecs nz = noise_of(c, d, noise, passes[i].apply);
+    const float* prm = passes[i].params;
+    const NoiseVecs nz = f.noisy ? noise_of(c, d, noise, passes[i].apply) : NoiseVecs{};
     for (int s = 0; s < ns; ++s) {
-      int n_out = s == 0 ? d.out : c.num_atoms;
+      const int n_out = (int)f.out[s];
       GemmProblem p = zero_problem();
       p.a_mode = A_PLAIN; p.A = nb.h1[passes[i].head][s]; p.lda = 512; p.M = nimg; p.K = 512;
-      p.B = passes[i].params + o.w2[s]; p.B2 = passes[i].params + o.sw2[s];
-      p.N = n_out; p.ldb = n_out; p.ldc = n_out;
-      // rainbow's mu has no bias (with_bias=False); the noisy plain head's has
-      p.bias = o.b2[s] < 0 ? nullptr : passes[i].params + o.b2[s]; p.bias2 = passes[i].params + o.sb2[s];
-      p.a_scale = s == 0 ? nz.a2i : nz.v2i; p.c_scale = s == 0 ? nz.a2o : nz.v2o;
-      int q = ns * i + s;
+      p.B = prm + o.w2[s]; p.N = n_out; p.ldb = n_out; p.ldc = n_out;
+      p.bias = o.b2[s] < 0 ? nullptr : prm + o.b2[s]; p.bias_shared = f.shared_bias ? 1 : 0;
+      if (f.noisy) {
+        p.B2 = prm + o.sw2[s]; p.bias2 = prm + o.sb2[s];
+        p.a_scale = s == 0 ? nz.a2i : nz.v2i; p.c_scale = s == 0 ? nz.a2o : nz.v2o;
+      }
+      const int q = ns * i + s;
       outs[q] = s == 0 ? nb.out[passes[i].head] : nb.outv[passes[i].head];
-      if (nimg <= nb.split_rows) {
-        p.splits = l->head_splits; p.split_stride = (long long)2 * nimg * n_out;
-        p.C = nb.nn_partial + (long long)q * l->head_splits * 2 * nimg * d.out;
+      if (split_head) {   // every problem's partials sized for the widest head, stream 0's
+        p.splits = l->head_splits; p.split_stride = (long long)halves * nimg * n_out;
+        p.C = nb.nn_partial + (long long)q * l->head_splits * halves * nimg * f.out[0];
       } else {
         p.C = outs[q];
       }
       gb.p[q] = p;
     }
   }
-  DZ_TRY(run("noisy2_fwd", gb));
-  if (nimg <= nb.split_rows) DZ_TRY(finish_nn(gb, outs, true, stream, noise_ld));
+  DZ_TRY(run(f.noisy ? "noisy2_fwd" : "head_fwd", gb));
+  if (split_head) DZ_TRY(finish_nn(gb, outs, f.noisy, stream, noise_ld));
   return DZ_OK;
-}
-
-// The dueling network's heads (DESIGN.md §16): both streams' 3136 -> 512 layers (on the fp32-FMA path one grouped
-// launch of 2 np problems, split over K as forward_heads_plain's fc1), then one dueling_head_fwd_kernel for every pass,
-// which writes each pass's aggregated q to out[head].
-int forward_heads_dueling(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, void* stream, bool fc1_done = false) {
-  const Dims& d = l->d;
-  const ParamOffsets& o = l->po;
-  if (2 * np > kMaxProblems) return fail(DZ_EINVAL, "too many dueling passes");
-  if (!fc1_done) {
-    GemmBatch gb;
-    gb.n = 2 * np;
-    float* outs[kMaxProblems];
-    const int splits = nimg <= nb.split_rows ? l->fc_splits : 1;
-    for (int i = 0; i < np; ++i)
-      for (int s = 0; s < 2; ++s) {
-        GemmProblem p = zero_problem();
-        p.a_mode = A_PLAIN; p.A = nb.act3[passes[i].set]; p.lda = d.feat; p.M = nimg; p.K = d.feat;
-        p.B = passes[i].params + o.w1[s]; p.N = 512; p.ldb = 512; p.ldc = 512;
-        p.bias = passes[i].params + o.b1[s]; p.relu = 1;
-        const int q = 2 * i + s;
-        outs[q] = nb.h1[passes[i].head][s];
-        if (splits > 1) {
-          p.splits = splits; p.split_stride = (long long)nimg * 512;
-          p.C = nb.nn_partial + (long long)q * splits * p.split_stride;
-        } else {
-          p.C = outs[q];
-        }
-        gb.p[q] = p;
-      }
-    DZ_TRY(run_nn("fc1_fwd", gb, false, stream));
-    if (splits > 1) DZ_TRY(finish_nn(gb, outs, false, stream));
-  }
-  const float* h1[3][2];
-  const float* prm[3];
-  float* out[3];
-  for (int i = 0; i < np; ++i) {
-    const int hp = passes[i].head;
-    h1[i][0] = nb.h1[hp][0]; h1[i][1] = nb.h1[hp][1];
-    prm[i] = passes[i].params; out[i] = nb.out[hp];
-  }
-  return launch_dueling_head_fwd(l, nimg, np, h1, prm, out, nullptr, 0, stream);
 }
 
 // IQN embedding (latent -> 3136, ReLU, * state embedding) and 3136 -> 512 layer of the three network applies of
@@ -2804,198 +2706,102 @@ int backward_torso(dz_learner* l, const uint8_t* const* rows0, void* stream) {
   return l->side.join(stream);
 }
 
-int backward_plain(dz_learner* l, void* stream) {
+// The backward of forward_heads_fc through online(s_tm1), noise apply 0 of `noise` for noisy layers: the dueling head
+// kernel (dout -> dadv in place, dval -> doutv, both streams' dh1), the head and 3136 -> 512 weight gradients on the
+// side stream (a noisy one fills the mu and sigma gradients together), the GEMM heads' input gradient, and dact3, which
+// sums every stream's input gradient.  On the tensor-core path fc1's input gradient reads dh1 as a tf32 hi/lo pair,
+// written by the dueling head kernel or by a split head input gradient's finish, else by um_split_dh1.
+int backward_fc(dz_learner* l, const float* noise, void* stream) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
-  const int B = l->B;
+  const FcNet& f = l->fc;
+  const int B = l->B, ns = f.ns;
+  const int halves = f.noisy ? 2 : 1;   // a noisy problem's split partials carry a second (sigma) half
   float* G = l->buf.d_grads;
   const float* P = l->buf.d_online;
-  const bool shared = l->cfg.kind == DZ_DOUBLE_Q || l->cfg.kind == DZ_PRIORITIZED;
-  GemmBatch gb;
-  gb.n = 1;
-  {  // head wgrad
-    GemmProblem p = zero_problem();
-    p.a_mode = A_PLAIN; p.A = l->h1[0][0]; p.lda = 512; p.M = B; p.K = 512;
-    p.B = l->dout; p.N = d.out; p.ldb = d.out; p.ldc = d.out;
-    p.C = G + o.w2[0]; p.Cb = shared ? l->scalars + 8 + kNormBlocks : G + o.b2[0];
-    gb.p[0] = p;
-    DZ_TRY(run_tn("head_wgrad", gb, l->side.fork(stream, stream)));
-    if (shared) DZ_LAUNCH(sum_to_scalar_kernel, 1, 128, 0, l->side.tail(stream), l->scalars + 8 + kNormBlocks, d.out, G + o.b2[0]);
-  }
-  bool dh1_split_done = false;
-  {  // dh1 = dout * Wh^T, masked by h1 > 0
-    GemmProblem p = zero_problem();
-    p.A = l->dout; p.lda = d.out; p.M = B; p.N = d.out; p.K = 512;
-    p.B = P + o.w2[0]; p.ldb = d.out; p.C = l->dh1[0]; p.ldc = 512; p.mask = l->h1[0][0];
-    // Wide heads (c51: 306 outputs, qr-dqn: 1206): with one CTA column per 64 outputs of dh1 the reduction over the head
-    // width is a serial chain (measured 24 / 65 us); split it and let the finish kernel apply the mask (and, on the tensor-core
-    // path, write the tf32 hi/lo pair fc1_dgrad reads, which saves the separate split launch).
-    const int splits = d.out > 64 ? (int)std::min<int64_t>(16, ceil_div(d.out, 96)) : 1;
-    if (splits > 1) {
-      p.splits = splits; p.split_stride = (long long)B * 512; p.C = l->nt_partial; p.mask = nullptr;
-      gb.p[0] = p;
-      DZ_TRY(run_nt("head_dgrad", gb, false, stream));
-      FinishNT job = make_finish_nt(&gb.p[0], 1, l->h1[0][0], l->dh1[0], false, l->um ? um_dh1_hi(l->um, 0) : nullptr,
-                                    l->um ? um_dh1_lo(l->um, 0) : nullptr);
-      DZ_TRY(finish_nt_batch(&job, 1, stream));
-      dh1_split_done = l->um != nullptr;
-    } else {
-      gb.p[0] = p;
-      DZ_TRY(run_nt("head_dgrad", gb, false, stream));
-    }
-  }
-  {  // fc1 wgrad
-    GemmProblem p = zero_problem();
-    p.a_mode = A_PLAIN; p.A = l->act3[0]; p.lda = d.feat; p.M = B; p.K = d.feat;
-    p.B = l->dh1[0]; p.N = 512; p.ldb = 512; p.ldc = 512;
-    p.C = G + o.w1[0]; p.Cb = G + o.b1[0];
-    gb.p[0] = p;
-    DZ_TRY(run_tn("fc1_wgrad", gb, l->side.fork(stream, stream)));
-  }
-  if (l->um) {   // dact3 on the tensor-core path: dh1 -> tf32 hi/lo, W streamed once through TMA, split partials + masked finish
-    if (!dh1_split_done) DZ_TRY(um_split_dh1(l->um, stream));
-    DZ_TRY(um_backward_fc(l->um, nullptr, stream));
-  } else {  // dact3 = dh1 * Wf^T, masked by act3 > 0
-    GemmProblem p = zero_problem();
-    p.A = l->dh1[0]; p.lda = 512; p.M = B; p.N = 512; p.K = d.feat;
-    p.B = P + o.w1[0]; p.ldb = 512; p.ldc = d.feat;
-    // weight-streaming GEMM with a 32-row output: split the reduction so ~400 CTAs keep HBM busy
-    p.splits = l->nt_splits; p.split_stride = (long long)B * d.feat; p.C = l->nt_partial;
-    gb.p[0] = p;
-    DZ_TRY(run_nt("fc1_dgrad", gb, false, stream));
-    DZ_TRY(finish_nt(gb.p, 1, l->act3[0], l->dact3, false, stream));
-  }
-  return DZ_OK;
-}
-
-// The dueling head's backward on the learner's buffers (noise apply 0 of `noise` for the noisy dueling network):
-// dout -> dadv in place, dval -> doutv, both streams' dh1 and, on the tensor-core path, their tf32 hi/lo pair.
-int dueling_head_bwd_of(dz_learner* l, const float* noise, void* stream) {
-  const float* h1[2] = {l->h1[0][0], l->h1[0][1]};
+  const NoiseVecs nz = f.noisy ? noise_of(l->cfg, d, noise, 0) : NoiseVecs{};
+  const float* in1[2] = {nz.a1i, nz.v1i};
+  const float* out1[2] = {nz.a1o, nz.v1o};
+  const float* in2[2] = {nz.a2i, nz.v2i};
+  const float* out2[2] = {nz.a2o, nz.v2o};
+  float* dout[2] = {l->dout, l->doutv};
   float* hi[2] = {nullptr, nullptr};
   float* lo[2] = {nullptr, nullptr};
   if (l->um)
-    for (int s = 0; s < 2; ++s) { hi[s] = um_dh1_hi(l->um, s); lo[s] = um_dh1_lo(l->um, s); }
-  return launch_dueling_head_bwd(l, l->B, l->dout, l->doutv, h1, l->buf.d_online, l->dh1, hi, lo, noise, stream);
-}
-
-// The backward of forward_heads_noisy's networks through online(s_tm1) (noise apply 0).  The heads: rainbow's and the
-// noisy plain network's input gradient is a noisy run_nt and a finish that masks dh1 (and, on the tensor-core path,
-// writes its tf32 hi/lo pair); the noisy dueling network's is noisy_dueling_head_bwd_kernel.  Every weight gradient is a
-// noisy run_tn on the side stream that fills the mu and sigma gradients together.
-int backward_noisy(dz_learner* l, const float* noise, void* stream) {
-  const Dims& d = l->d;
-  const ParamOffsets& o = l->po;
-  const dz_learner_config& c = l->cfg;
-  const int B = l->B;
-  const int ns = two_streams(c) ? 2 : 1;
-  const bool dueling_head = c.kind != DZ_RAINBOW && ns == 2;
-  const int n_val = c.kind == DZ_RAINBOW ? c.num_atoms : 1;   // value-stream outputs
-  float* G = l->buf.d_grads;
-  const float* P = l->buf.d_online;
-  NoiseVecs nz = noise_of(c, d, noise, 0);
-  if (dueling_head) DZ_TRY(dueling_head_bwd_of(l, noise, stream));   // dout -> dadv in place, dval -> doutv, both dh1
+    for (int s = 0; s < ns; ++s) { hi[s] = um_dh1_hi(l->um, s); lo[s] = um_dh1_lo(l->um, s); }
+  bool hilo_done = false;
+  if (f.dueling_head) {
+    const float* h1[2] = {l->h1[0][0], l->h1[0][1]};
+    DZ_TRY(launch_dueling_head_bwd(l, B, l->dout, l->doutv, h1, P, l->dh1, hi, lo, noise, stream));
+    hilo_done = true;
+  }
   GemmBatch gb;
   gb.n = ns;
-  for (int s = 0; s < ns; ++s) {  // second noisy layer weight grads
-    int n_out = s == 0 ? d.out : n_val;
+  float* bias_terms = l->scalars + 8 + kNormBlocks;   // a shared bias: the per-output terms sum_to_scalar_kernel adds
+  for (int s = 0; s < ns; ++s) {  // head weight and bias gradients
+    const int n_out = (int)f.out[s];
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->h1[0][s]; p.lda = 512; p.M = B; p.K = 512;
-    p.B = s == 0 ? l->dout : l->doutv; p.N = n_out; p.ldb = n_out; p.ldc = n_out;
-    p.C = G + o.w2[s]; p.C2 = G + o.sw2[s]; p.Cb = o.b2[s] < 0 ? nullptr : G + o.b2[s]; p.Cb2 = G + o.sb2[s];
-    p.a_scale = s == 0 ? nz.a2i : nz.v2i; p.c_scale = s == 0 ? nz.a2o : nz.v2o;
+    p.B = dout[s]; p.N = n_out; p.ldb = n_out; p.ldc = n_out;
+    p.C = G + o.w2[s]; p.Cb = f.shared_bias ? bias_terms : o.b2[s] < 0 ? nullptr : G + o.b2[s];
+    if (f.noisy) { p.C2 = G + o.sw2[s]; p.Cb2 = G + o.sb2[s]; p.a_scale = in2[s]; p.c_scale = out2[s]; }
     gb.p[s] = p;
   }
-  DZ_TRY(run_tn("noisy2_wgrad", gb, l->side.fork(stream, stream)));
-  if (!dueling_head) {
-    for (int s = 0; s < ns; ++s) {  // dh1_s
-      int n_out = s == 0 ? d.out : n_val;
+  DZ_TRY(run_tn(f.noisy ? "noisy2_wgrad" : "head_wgrad", gb, l->side.fork(stream, stream)));
+  if (f.shared_bias) DZ_LAUNCH(sum_to_scalar_kernel, 1, 128, 0, l->side.tail(stream), bias_terms, d.out, G + o.b2[0]);
+  if (!f.dueling_head) {  // dh1_s = dout_s * W2_s^T, masked by h1_s > 0
+    // Noisy heads split the reduction 4 ways.  Wide plain heads (c51: 306 outputs, qr-dqn: 1206): with one CTA column
+    // per 64 outputs of dh1 the reduction over the head width is a serial chain (measured 24 / 65 us); split it.  The
+    // finish of the split partials applies the mask and, on the tensor-core path, writes the tf32 hi/lo pair, which
+    // saves the separate split launch; unsplit, the GEMM applies the mask.
+    const int splits = f.noisy ? 4 : d.out > 64 ? (int)std::min<int64_t>(16, ceil_div(d.out, 96)) : 1;
+    for (int s = 0; s < ns; ++s) {
+      const int n_out = (int)f.out[s];
       GemmProblem p = zero_problem();
-      p.A = s == 0 ? l->dout : l->doutv; p.lda = n_out; p.M = B; p.N = n_out; p.K = 512;
-      p.B = P + o.w2[s]; p.B2 = P + o.sw2[s]; p.ldb = n_out;
-      p.a_scale = s == 0 ? nz.a2i : nz.v2i; p.c_scale = s == 0 ? nz.a2o : nz.v2o;
-      p.ldc = 512;
-      p.splits = 4; p.split_stride = (long long)2 * B * 512;
-      p.C = l->nt_partial + (long long)s * 4 * p.split_stride;
+      p.A = dout[s]; p.lda = n_out; p.M = B; p.N = n_out; p.K = 512;
+      p.B = P + o.w2[s]; p.ldb = n_out; p.ldc = 512;
+      if (f.noisy) { p.B2 = P + o.sw2[s]; p.a_scale = in2[s]; p.c_scale = out2[s]; }
+      if (splits > 1) {
+        p.splits = splits; p.split_stride = (long long)halves * B * 512;
+        p.C = l->nt_partial + (long long)s * splits * p.split_stride;
+      } else {
+        p.C = l->dh1[s]; p.mask = l->h1[0][s];
+      }
       gb.p[s] = p;
     }
-    DZ_TRY(run_nt("noisy2_dgrad", gb, true, stream));
-    // every stream's dh1 in one launch; on the tensor-core path it also writes the tf32 hi/lo pair noisy1_dgrad reads
-    FinishNT jobs[2];
-    for (int s = 0; s < ns; ++s)
-      jobs[s] = make_finish_nt(&gb.p[s], 1, l->h1[0][s], l->dh1[s], true, l->um ? um_dh1_hi(l->um, s) : nullptr,
-                               l->um ? um_dh1_lo(l->um, s) : nullptr);
-    DZ_TRY(finish_nt_batch(jobs, ns, stream));
+    DZ_TRY(run_nt(f.noisy ? "noisy2_dgrad" : "head_dgrad", gb, f.noisy, stream));
+    if (splits > 1) {   // every stream's dh1 in one launch
+      FinishNT jobs[2];
+      for (int s = 0; s < ns; ++s) jobs[s] = make_finish_nt(&gb.p[s], 1, l->h1[0][s], l->dh1[s], f.noisy, hi[s], lo[s]);
+      DZ_TRY(finish_nt_batch(jobs, ns, stream));
+      hilo_done = true;
+    }
   }
-  for (int s = 0; s < ns; ++s) {  // first noisy layer weight grads
-    GemmProblem p = zero_problem();
-    p.a_mode = A_PLAIN; p.A = l->act3[0]; p.lda = d.feat; p.M = B; p.K = d.feat;
-    p.B = l->dh1[s]; p.N = 512; p.ldb = 512; p.ldc = 512;
-    p.C = G + o.w1[s]; p.C2 = G + o.sw1[s]; p.Cb = G + o.b1[s]; p.Cb2 = G + o.sb1[s];
-    p.a_scale = s == 0 ? nz.a1i : nz.v1i; p.c_scale = s == 0 ? nz.a1o : nz.v1o;
-    gb.p[s] = p;
-  }
-  DZ_TRY(run_tn("noisy1_wgrad", gb, l->side.fork(stream, stream)));
-  if (l->um) {
-    DZ_TRY(um_backward_fc(l->um, noise, stream));   // dh1 hi/lo came from the head's input gradient above
-    return DZ_OK;
-  }
-  for (int s = 0; s < ns; ++s) {  // dact3 contributions
-    GemmProblem p = zero_problem();
-    p.A = l->dh1[s]; p.lda = 512; p.M = B; p.N = 512; p.K = d.feat;
-    p.B = P + o.w1[s]; p.B2 = P + o.sw1[s]; p.ldb = 512;
-    p.a_scale = s == 0 ? nz.a1i : nz.v1i; p.c_scale = s == 0 ? nz.a1o : nz.v1o;
-    p.ldc = d.feat;
-    p.splits = l->nt_splits; p.split_stride = (long long)2 * B * d.feat;
-    p.C = l->nt_partial + (long long)s * l->nt_splits * p.split_stride;
-    gb.p[s] = p;
-  }
-  DZ_TRY(run_nt("noisy1_dgrad", gb, true, stream));
-  // dact3 = (sum of the streams' contributions) * [act3 > 0], summed from the split partials
-  DZ_TRY(finish_nt(gb.p, ns, l->act3[0], l->dact3, true, stream));
-  return DZ_OK;
-}
-
-// The dueling network's backward (DESIGN.md §16): dueling_head_bwd_kernel turns dout into dadv (in place) and dval and
-// writes both streams' dh1 (and, on the tensor-core path, their tf32 hi/lo pair); the head and 3136 -> 512 weight
-// gradients of both streams run as two-problem launches on the side stream; dact3 sums both streams' input gradients.
-int backward_dueling(dz_learner* l, void* stream) {
-  const Dims& d = l->d;
-  const ParamOffsets& o = l->po;
-  const int B = l->B, A = l->cfg.num_actions;
-  float* G = l->buf.d_grads;
-  const float* P = l->buf.d_online;
-  DZ_TRY(dueling_head_bwd_of(l, nullptr, stream));
-  GemmBatch gb;
-  gb.n = 2;
-  for (int s = 0; s < 2; ++s) {  // adv2 / val2 weight and bias gradients
-    const int n_out = s == 0 ? A : 1;
-    GemmProblem p = zero_problem();
-    p.a_mode = A_PLAIN; p.A = l->h1[0][s]; p.lda = 512; p.M = B; p.K = 512;
-    p.B = s == 0 ? l->dout : l->doutv; p.N = n_out; p.ldb = n_out; p.ldc = n_out;
-    p.C = G + o.w2[s]; p.Cb = G + o.b2[s];
-    gb.p[s] = p;
-  }
-  DZ_TRY(run_tn("head_wgrad", gb, l->side.fork(stream, stream)));
-  for (int s = 0; s < 2; ++s) {  // adv1 / val1 weight and bias gradients
+  for (int s = 0; s < ns; ++s) {  // 3136 -> 512 weight and bias gradients
     GemmProblem p = zero_problem();
     p.a_mode = A_PLAIN; p.A = l->act3[0]; p.lda = d.feat; p.M = B; p.K = d.feat;
     p.B = l->dh1[s]; p.N = 512; p.ldb = 512; p.ldc = 512;
     p.C = G + o.w1[s]; p.Cb = G + o.b1[s];
+    if (f.noisy) { p.C2 = G + o.sw1[s]; p.Cb2 = G + o.sb1[s]; p.a_scale = in1[s]; p.c_scale = out1[s]; }
     gb.p[s] = p;
   }
-  DZ_TRY(run_tn("fc1_wgrad", gb, l->side.fork(stream, stream)));
-  if (l->um) return um_backward_fc(l->um, nullptr, stream);   // dh1 hi/lo came from dueling_head_bwd_kernel
-  for (int s = 0; s < 2; ++s) {  // dact3 contributions
+  DZ_TRY(run_tn(f.noisy ? "noisy1_wgrad" : "fc1_wgrad", gb, l->side.fork(stream, stream)));
+  if (l->um) {   // dact3 on the tensor-core path: W streamed once through TMA, split partials + masked finish
+    if (!hilo_done) DZ_TRY(um_split_dh1(l->um, stream));
+    return um_backward_fc(l->um, f.noisy ? noise : nullptr, stream);
+  }
+  for (int s = 0; s < ns; ++s) {  // dact3 = (sum over streams of dh1_s * W1_s^T) * [act3 > 0]
     GemmProblem p = zero_problem();
     p.A = l->dh1[s]; p.lda = 512; p.M = B; p.N = 512; p.K = d.feat;
     p.B = P + o.w1[s]; p.ldb = 512; p.ldc = d.feat;
-    p.splits = l->nt_splits; p.split_stride = (long long)B * d.feat;
+    if (f.noisy) { p.B2 = P + o.sw1[s]; p.a_scale = in1[s]; p.c_scale = out1[s]; }
+    // weight-streaming GEMM with a 32-row output: split the reduction so ~400 CTAs keep HBM busy
+    p.splits = l->nt_splits; p.split_stride = (long long)halves * B * d.feat;
     p.C = l->nt_partial + (long long)s * l->nt_splits * p.split_stride;
     gb.p[s] = p;
   }
-  DZ_TRY(run_nt("fc1_dgrad", gb, false, stream));
-  return finish_nt(gb.p, 2, l->act3[0], l->dact3, false, stream);
+  DZ_TRY(run_nt(f.noisy ? "noisy1_dgrad" : "fc1_dgrad", gb, f.noisy, stream));
+  return finish_nt(gb.p, ns, l->act3[0], l->dact3, f.noisy, stream);
 }
 
 int backward_iqn(dz_learner* l, void* stream) {
@@ -3330,12 +3136,8 @@ int act(const ActTarget& t, int E, const uint8_t* d_obs, const float* d_taus, co
   } else if (uses_iqn_net(c.kind)) {
     const float* taus[1] = {d_taus};
     DZ_TRY(forward_heads_iqn(l, t.nb, &pass, 1, E, taus, false, stream));
-  } else if (rb) {
-    DZ_TRY(forward_heads_noisy(l, t.nb, &pass, 1, E, d_noise, stream, fc_done, noise_ld));
-  } else if (two_streams(c)) {
-    DZ_TRY(forward_heads_dueling(l, t.nb, &pass, 1, E, stream, fc_done));
   } else {
-    DZ_TRY(forward_heads_plain(l, t.nb, &pass, 1, E, stream, fc_done));
+    DZ_TRY(forward_heads_fc(l, t.nb, &pass, 1, E, d_noise, stream, fc_done, noise_ld));
   }
   return launch_q_values(c, E, t.nb.out[1], t.nb.outv[1], d_explore, epsilon, d_q_out, d_actions, stream, t.frac_w);
 }
@@ -3357,7 +3159,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   const int B = l->B;
   const float* on = l->buf.d_online;
   const float* tg = l->buf.d_target;
-  const bool needs_online_st = c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED || c.kind == DZ_RAINBOW;
+  const bool online_st = online_applies_to_s_t(c.kind);
   if (noisy_net(c) && !batch->d_noise) return fail(DZ_EINVAL, "a noisy network's update needs d_noise");
   if (draws_taus(c.kind) && !batch->d_taus) return fail(DZ_EINVAL, "iqn update needs d_taus");
   if (!out || !out->d_loss || !out->d_per_example) return fail(DZ_EINVAL, "update outputs d_loss and d_per_example are required");
@@ -3369,7 +3171,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   const bool target_stm1 = is_munchausen(c.kind);   // the target network also applies to s_tm1 (the log-policy bonus)
   const bool iqn = uses_iqn_net(c.kind);
   jobs[nj++] = TorsoJob{on, batch->d_s_tm1_rows, 0};
-  if (needs_online_st) jobs[nj++] = TorsoJob{on, batch->d_s_t_rows, 1};
+  if (online_st) jobs[nj++] = TorsoJob{on, batch->d_s_t_rows, 1};
   if (target_stm1) jobs[nj++] = TorsoJob{tg, batch->d_s_tm1_rows, 1};
   jobs[nj++] = TorsoJob{tg, batch->d_s_t_rows, 2};
   const bool um = l->um != nullptr;
@@ -3411,20 +3213,15 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     const float* t2 = t1 + (long long)B * c.tau_samples_policy;
     const float* taus[3] = {t0, t1, t2};
     DZ_TRY(forward_heads_iqn(l, learner_bufs(l), passes, 3, B, taus, true, stream));
-  } else if (c.kind == DZ_RAINBOW) {
-    Pass passes[3] = {{on, 0, 0, 0}, {on, 1, 1, 1}, {tg, 2, 2, 2}};
-    DZ_TRY(forward_heads_noisy(l, learner_bufs(l), passes, 3, B, batch->d_noise, stream, um));
   } else {
-    // noise slot = head pass (noisy networks, DESIGN.md §17): online(s_tm1) | the middle pass | target(s_t)
+    // noise slot = head pass (rainbow, noisy networks, DESIGN.md §17): online(s_tm1) | the middle pass | target(s_t)
     Pass passes[3];
     int np = 0;
     passes[np++] = Pass{on, 0, 0, 0};
-    if (needs_online_st) passes[np++] = Pass{on, 1, 1, 1};
+    if (online_st) passes[np++] = Pass{on, 1, 1, 1};
     if (target_stm1) passes[np++] = Pass{tg, 1, 1, 1};
     passes[np++] = Pass{tg, 2, 2, 2};
-    if (noisy_net(c)) DZ_TRY(forward_heads_noisy(l, learner_bufs(l), passes, np, B, batch->d_noise, stream, um));
-    else if (two_streams(c)) DZ_TRY(forward_heads_dueling(l, learner_bufs(l), passes, np, B, stream, um));
-    else DZ_TRY(forward_heads_plain(l, learner_bufs(l), passes, np, B, stream, um));
+    DZ_TRY(forward_heads_fc(l, learner_bufs(l), passes, np, B, batch->d_noise, stream, um));
   }
 
   // ---- loss + gradient wrt the pass-0 head outputs
@@ -3445,10 +3242,8 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   }
 
   // ---- backward through online(s_tm1)
-  if (noisy_net(c)) DZ_TRY(backward_noisy(l, batch->d_noise, stream));
-  else if (two_streams(c)) DZ_TRY(backward_dueling(l, stream));
-  else if (iqn) DZ_TRY(backward_iqn(l, stream));
-  else DZ_TRY(backward_plain(l, stream));
+  if (iqn) DZ_TRY(backward_iqn(l, stream));
+  else DZ_TRY(backward_fc(l, batch->d_noise, stream));
   if (fqf) DZ_TRY(backward_fraction(l, stream));
   if (split_norm_active(l)) {   // every gradient behind the conv tensors is final once the side stream's FC / head wgrads are done
     DZ_TRY(norm_fc_range(l, apply_update != 0, l->side.tail(stream)));
@@ -3473,17 +3268,10 @@ extern "C" {
 int dz_learner_plan_query(const dz_learner_config* cfg, dz_learner_plan* out) {
   DZ_TRY(validate(*cfg));
   dz_learner tmp;
-  tmp.um = nullptr;
-  memset(&tmp.buf, 0, sizeof(tmp.buf));
-  tmp.cfg = *cfg;
-  tmp.lay = make_layout(*cfg);
-  DZ_TRY(param_offsets(*cfg, tmp.lay, &tmp.po));
-  tmp.d = make_dims(*cfg);
-  tmp.B = cfg->batch;
+  out->workspace_bytes = init_shape_learner(&tmp, *cfg);
   out->param_count = tmp.lay.total;
   out->num_tensors = (int32_t)tmp.lay.t.size();
   out->opt_state_floats = 2 * tmp.lay.total;
-  out->workspace_bytes = carve(&tmp, nullptr);
   out->noise_floats = noisy_net(*cfg) ? 3 * noise_layout(*cfg, tmp.d).stride : 0;
   out->tau_floats = draws_taus(cfg->kind)
                         ? (int64_t)cfg->batch * (cfg->tau_samples_s_tm1 + cfg->tau_samples_policy + cfg->tau_samples_s_t)
@@ -3508,18 +3296,12 @@ int dz_learner_create(const dz_learner_config* cfg, const dz_learner_buffers* bu
   if (!buf->d_online || !buf->d_target || !buf->d_grads || !buf->d_opt_state || !buf->d_workspace || !buf->d_counters)
     return fail(DZ_EINVAL, "all learner buffers are required");
   dz_learner* l = new dz_learner();
-  l->cfg = *cfg;
+  init_shape_learner(l, *cfg);
   l->buf = *buf;
-  l->lay = make_layout(*cfg);
-  l->d = make_dims(*cfg);
-  l->B = cfg->batch;
-  l->um = nullptr;
-  int rc = param_offsets(*cfg, l->lay, &l->po);
-  if (rc != DZ_OK) { delete l; return rc; }
   carve(l, static_cast<char*>(buf->d_workspace));
   if (l->um_ws) {
     UmNetDesc ud = make_um_desc(l);
-    rc = um_net_create(ud, l->um_ws, &l->um);
+    const int rc = um_net_create(ud, l->um_ws, &l->um);
     if (rc != DZ_OK) { delete l; return rc; }
     l->um_npass = ud.npass;
     const int um_set[3] = {0, ud.npass == 3 ? 1 : 2, 2};   // torso activation set of each tensor-core pass
@@ -3725,7 +3507,8 @@ int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
   const dz_learner_config& c = l->cfg;
   const Dims& d = l->d;
   const int E = a->E;
-  const bool rb = c.kind == DZ_RAINBOW, two = two_streams(c), iqn = uses_iqn_net(c.kind);
+  const FcNet& f = l->fc;
+  const bool iqn = uses_iqn_net(c.kind);
   Bump w{base};
   NetBufs& b = a->b;
   memset(&b, 0, sizeof(b));   // split_rows 0: the fp32 GEMMs never split K, so row e's sums do not depend on E
@@ -3741,10 +3524,10 @@ int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
   const int64_t rows = (int64_t)E * (iqn ? acting_samples(c) : 1);
   if (!um || iqn) {                      // otherwise h1 is the tensor-core plan's
     b.h1[1][0] = w.take<float>(rows * 512);
-    b.h1[1][1] = two ? w.take<float>(rows * 512) : nullptr;
+    b.h1[1][1] = f.ns == 2 ? w.take<float>(rows * 512) : nullptr;
   }
   b.out[1] = w.take<float>(rows * d.out);
-  b.outv[1] = rb ? w.take<float>((int64_t)E * c.num_atoms) : nullptr;
+  b.outv[1] = f.ns == 2 && !f.dueling_head ? w.take<float>((int64_t)E * f.out[1]) : nullptr;
   b.cosf[1] = iqn ? w.take<float>(rows * c.latent_dim) : nullptr;
   b.hi[1] = iqn ? w.take<float>(rows * d.feat) : nullptr;
   a->rows = w.take<const uint8_t*>(E);
@@ -3758,26 +3541,12 @@ int64_t carve_actor(dz_actor* a, const dz_learner* l, char* base) {
   return w.used;
 }
 
-// A learner with cfg's configuration, layout, parameter offsets, dims and split counts and no device state: carve()
-// without a base leaves every workspace pointer NULL.
-int init_shape_learner(dz_learner* t, const dz_learner_config& cfg) {
-  t->um = nullptr;
-  memset(&t->buf, 0, sizeof(t->buf));
-  t->cfg = cfg;
-  t->lay = make_layout(cfg);
-  DZ_TRY(param_offsets(cfg, t->lay, &t->po));
-  t->d = make_dims(cfg);
-  t->B = cfg.batch;
-  carve(t, nullptr);                     // the learner's split counts, which the actor's fp32 GEMMs share
-  return DZ_OK;
-}
-
 int actor_plan_bytes(const dz_learner_config* cfg, int32_t num_streams, bool frozen, int64_t* workspace_bytes) {
   if (!cfg || !workspace_bytes) return fail(DZ_EINVAL, "actor plan query: null argument");
   DZ_TRY(validate(*cfg));
   DZ_TRY(actor_check(*cfg, num_streams));
   dz_learner tmp;
-  DZ_TRY(init_shape_learner(&tmp, *cfg));
+  init_shape_learner(&tmp, *cfg);
   dz_actor a;
   a.E = num_streams;
   a.frozen = frozen;
@@ -3803,7 +3572,7 @@ int actor_create(dz_learner* l, bool frozen, int32_t num_streams, void* d_worksp
     if (rc != DZ_OK) { dz_actor_destroy(a); return rc; }
     for (int L = 1; L <= 3; ++L) (L == 1 ? a->b.act1 : L == 2 ? a->b.act2 : a->b.act3)[1] = um_act_f32(a->um, L, 0);
     if (!uses_iqn_net(l->cfg.kind))
-      for (int s = 0; s < (two_streams(l->cfg) ? 2 : 1); ++s) a->b.h1[1][s] = um_h1_f32(a->um, 0, s);
+      for (int s = 0; s < l->fc.ns; ++s) a->b.h1[1][s] = um_h1_f32(a->um, 0, s);
   }
   *out = a;
   return DZ_OK;
@@ -3829,8 +3598,7 @@ int dz_actor_create_frozen(dz_learner* l, int32_t num_streams, void* d_workspace
   if (!l || !d_workspace || !out) return fail(DZ_EINVAL, "frozen actor create: null argument");
   DZ_TRY(actor_check(l->cfg, num_streams));
   dz_learner* shape = new dz_learner();
-  const int rc = init_shape_learner(shape, l->cfg);
-  if (rc != DZ_OK) { delete shape; return rc; }
+  init_shape_learner(shape, l->cfg);
   return actor_create(shape, true, num_streams, d_workspace, out);   // on failure the actor's destroy frees shape
 }
 
@@ -4181,7 +3949,7 @@ int dz_test_dueling_head_fwd(dz_learner* l, int32_t rows, int32_t np, const floa
                              const float* const* d_noise, int64_t noise_ld, float* const* d_out, void* stream) {
   if (!l || !d_h1 || !d_params || !d_out) return fail(DZ_EINVAL, "test_dueling_head_fwd: NULL argument");
   const dz_learner_config& c = l->cfg;
-  if (!two_streams(c) || c.kind == DZ_RAINBOW) return fail(DZ_EINVAL, "test_dueling_head_fwd: the learner is not dueling");
+  if (!l->fc.dueling_head) return fail(DZ_EINVAL, "test_dueling_head_fwd: the learner is not dueling");
   if (rows < 1 || np < 1 || np > 3 || noise_ld < 0) return fail(DZ_EINVAL, "test_dueling_head_fwd: rows, np or noise_ld out of range");
   if (noisy_net(c) ? !d_noise : noise_ld != 0) return fail(DZ_EINVAL, "test_dueling_head_fwd: noise only for the noisy network");
   const float* h1[3][2];
@@ -4199,7 +3967,7 @@ int dz_test_dueling_head_bwd(dz_learner* l, int32_t rows, float* d_dq, float* d_
                              float* const* d_lo, void* stream) {
   if (!l || !d_dq || !d_dval || !d_h1 || !d_params || !d_dh1) return fail(DZ_EINVAL, "test_dueling_head_bwd: NULL argument");
   const dz_learner_config& c = l->cfg;
-  if (!two_streams(c) || c.kind == DZ_RAINBOW) return fail(DZ_EINVAL, "test_dueling_head_bwd: the learner is not dueling");
+  if (!l->fc.dueling_head) return fail(DZ_EINVAL, "test_dueling_head_bwd: the learner is not dueling");
   if (rows < 1) return fail(DZ_EINVAL, "test_dueling_head_bwd: rows must be >= 1");
   if (noisy_net(c) && !d_noise) return fail(DZ_EINVAL, "test_dueling_head_bwd: the noisy network needs its noise apply");
   if (!d_h1[0] || !d_h1[1] || !d_dh1[0] || !d_dh1[1] || (!d_hi != !d_lo) || (d_hi && (!d_hi[0] || !d_hi[1] || !d_lo[0] || !d_lo[1])))
