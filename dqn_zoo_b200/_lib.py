@@ -219,12 +219,17 @@ _SIGNATURES = {
     'dz_test_dueling_head_fwd': (i32, [vp, i32, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), i64, C.POINTER(vp), vp]),
     'dz_test_dueling_head_bwd': (i32, [vp, i32, vp, vp, C.POINTER(vp), vp, vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
                                        vp]),
+    'dz_test_iqn_cos': (i32, [vp, i64, i32, vp, vp]),
+    'dz_test_iqn_head_fwd': (i32, [vp, i32, C.POINTER(i32), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), vp]),
+    'dz_test_iqn_head_dgrad': (i32, [vp, i32, vp, vp, vp, vp, vp]),
+    'dz_test_iqn_hadamard_bwd': (i32, [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, i32, vp]),
     'dz_test_copy': (i32, [vp, vp, i64, vp]),
     'dz_test_learner_trace': (i32, [vp, C.c_char_p, vp]),
     'dz_test_learner_mma_path': (i32, [vp, C.c_char_p, C.POINTER(i32)]),
     'dz_debug_timeline': (i32, [vp]),
     'dz_test_tc_pgemm_work': (i64, [i32, i32, i32]),
     'dz_test_tc_pgemm': (i32, [vp, i32, i32, i32, vp, i32, i32, i32, i32, i32, vp, vp, i64, i64, i32, i64, vp, i32, vp]),
+    'dz_test_iqn_embed_packed': (i32, [vp, i32, i32, vp, i32, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]),
     'dz_test_umma_gemm': (i32, [vp, i32, vp, i32, i32, i32, i32, i32, vp, i32, i32, vp, i32, vp, vp, vp, vp]),
     'dz_test_umma_gemm_path': (i32, [vp, i32, vp, i32, i32, i32, i32, i32, vp, i32, i32, vp, i32, vp, vp, vp, i32, vp]),
     'dz_test_fc_forward': (i32, [i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp, vp, vp, i32, vp, C.POINTER(i32),

@@ -119,5 +119,13 @@ int pk_add_job(PackBatch& pb, const float* src, int ld, int red_contig, int rows
 int launch_pack(const char* tag, const PackBatch& pb, void* stream);
 int pk_set_ones_row(float* hi, int rows_pad, int row, int red, void* stream);   // image element (row, r < red) = 1
 int launch_pgemm(const char* tag, const PkBatch& kb, void* stream, int epi = 0);
+// A tile image an epilogue writes: rg = rows_pad / 8; hi == nullptr: none.
+struct PkTarget { float* hi; float* lo; int rg; };
+// The EPI 1 problem (IQN embedding, dz_tcp.cuh) of one network apply: rows i < M of the cosine image `cos` against the
+// embedding weight image `weT` (rows j < D), nkb k-blocks; v = relu(acc + bias[j]) -> e0 [M][D] (optional), h = v *
+// mul[(i / mul_div) * mul_ld + j] -> img (rows i) and imgT (rows j, optional).  The learner's forward and
+// dz_test_iqn_embed_packed build their problem with this function.
+PkProblem pk_embed_problem(const PkOperand& cos, const PkOperand& weT, int M, int D, int nkb, const float* bias,
+                           const float* mul, int mul_div, int mul_ld, float* e0, const PkTarget& img, const PkTarget& imgT);
 
 }  // namespace dz

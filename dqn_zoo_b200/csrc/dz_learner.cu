@@ -2438,6 +2438,57 @@ int forward_heads_fc(dz_learner* l, const NetBufs& nb, const Pass* passes, int n
   return DZ_OK;
 }
 
+// The cosine features out [rows][latent] of `rows` taus (iqn_cos_kernel).  forward_heads_iqn and dz_test_iqn_cos run
+// this function.
+int launch_iqn_cos(const float* taus, float* out, long long rows, int latent, void* stream) {
+  DZ_LAUNCH(iqn_cos_kernel, (unsigned)ceil_div(rows * latent, 256), 256, 0, stream, taus, out, rows, latent);
+  return DZ_OK;
+}
+
+// IQN's value head (iqn_head_fwd_kernel, A = num_actions <= kSkinnyMaxN) of `np` (<= 3) applies: apply i reads h1[i]
+// [M[i]][512] and the head of params[i], and writes out[i] [M[i]][A].  forward_heads_iqn and dz_test_iqn_head_fwd run
+// this function.
+int launch_iqn_head_fwd(const dz_learner* l, int np, const float* const* h1, const float* const* params, float* const* out,
+                        const int* M, void* stream) {
+  const ParamOffsets& o = l->po;
+  SkinnyHead h;
+  memset(&h, 0, sizeof(h));
+  h.n = np;
+  int maxM = 0;
+  for (int i = 0; i < np; ++i) {
+    h.A[i] = h1[i]; h.W[i] = params[i] + o.w2[0]; h.bias[i] = params[i] + o.b2[0];
+    h.out[i] = out[i]; h.M[i] = M[i];
+    maxM = std::max(maxM, h.M[i]);
+  }
+  dim3 grid((unsigned)std::min<int64_t>(ceil_div(maxM, 8), kNumSMs * 2), (unsigned)np);
+  DZ_LAUNCH_NAMED("iqn_head_fwd", iqn_head_fwd_kernel, grid, 256, 0, stream, h, l->d.out);
+  return DZ_OK;
+}
+
+// The value head's input gradient dh1 [M][512] = [h1 > 0] dout W^T from dout [M][A] and the head of `params`
+// (iqn_head_dgrad_kernel, A <= kSkinnyMaxN).  backward_iqn and dz_test_iqn_head_dgrad run this function.
+int launch_iqn_head_dgrad(const dz_learner* l, const float* dout, const float* params, const float* h1, float* dh1, int M,
+                          void* stream) {
+  DZ_LAUNCH_NAMED("iqn_head_dgrad", iqn_head_dgrad_kernel, (unsigned)std::min<int64_t>(ceil_div((long long)M * 128, 256), kNumSMs * 8),
+                  256, 0, stream, dout, params + l->po.w2[0], h1, dh1, M, l->d.out);
+  return DZ_OK;
+}
+
+// The backward of E * F (E [B][N][D] the embedding after its ReLU, F [B][D] the state features): dfeat [B][D] and dE,
+// in place in dhi (iqn_hadamard_bwd_kernel) or, packed, only as the transposed tf32 hi/lo image with rows k and
+// reduction b * N + n (iqn_hadamard_bwd_packed_kernel: N == 64, D % 64 == 0; rg_total = the image's rows_pad / 8).
+// backward_iqn and dz_test_iqn_hadamard_bwd run this function.
+int launch_iqn_hadamard_bwd(bool packed, float* dhi, const float* E, const float* F, float* dfeat, float* img_hi, float* img_lo,
+                            int rg_total, int B, int N, int D, void* stream) {
+  if (packed) {
+    dim3 hgrid((unsigned)(D / 64), (unsigned)B);
+    DZ_LAUNCH(iqn_hadamard_bwd_packed_kernel, hgrid, 256, 0, stream, dhi, E, F, dfeat, img_hi, img_lo, rg_total, D);
+  } else {
+    DZ_LAUNCH(iqn_hadamard_bwd_kernel, (unsigned)ceil_div((long long)B * D, 256), 256, 0, stream, dhi, E, F, dfeat, B, N, D);
+  }
+  return DZ_OK;
+}
+
 // IQN embedding (latent -> 3136, ReLU, * state embedding) and 3136 -> 512 layer of the three network applies of
 // one update on the packed-operand tensor-core kernels: one pack launch (cosine features + every weight operand of
 // this step), the embedding GEMM whose epilogue writes the hi/lo tile images of the next GEMMs directly (the fp32
@@ -2475,15 +2526,13 @@ int iqn_embed_fc1_forward_packed(dz_learner* l, const NetBufs& nb, const Pass* p
   eb.n = 3;
   for (int i = 0; i < 3; ++i) {
     int hp = passes[i].head;
-    PkProblem& p = eb.p[i];
-    p.A = PkOperand{l->pk_cos[hp].hi, l->pk_cos[hp].lo, l->pk_cos[hp].rows_pad / 8};
-    p.B = PkOperand{l->pk_weT[widx[i]].hi, l->pk_weT[widx[i]].lo, l->pk_weT[widx[i]].rows_pad / 8};
-    p.MI = fc1.p[i].M; p.NJ = d.feat; p.nkb = l->pk_cos[hp].red_pad / kPkKB; p.splits = 1;
-    p.bias_j = passes[i].params + o.embed_b;
-    p.mul = nb.act3[passes[i].set]; p.mul_div = l->n_head[hp]; p.mul_ld = d.feat;
-    p.e0 = (keep_E0 && hp == 0) ? l->E0 : nullptr; p.e0_ld = d.feat;
-    p.img_hi = l->pk_act[hp].hi; p.img_lo = l->pk_act[hp].lo; p.img_rg = l->pk_act[hp].rows_pad / 8;
-    if (keep_E0 && hp == 0) { p.imgT_hi = l->pk_actT.hi; p.imgT_lo = l->pk_actT.lo; p.imgT_rg = l->pk_actT.rows_pad / 8; }
+    const bool keep = keep_E0 && hp == 0;
+    const dz_learner::PkImg &cs = l->pk_cos[hp], &we = l->pk_weT[widx[i]], &im = l->pk_act[hp];
+    const PkTarget img{im.hi, im.lo, im.rows_pad / 8};
+    const PkTarget imgT = keep ? PkTarget{l->pk_actT.hi, l->pk_actT.lo, l->pk_actT.rows_pad / 8} : PkTarget{nullptr, nullptr, 0};
+    eb.p[i] = pk_embed_problem(PkOperand{cs.hi, cs.lo, cs.rows_pad / 8}, PkOperand{we.hi, we.lo, we.rows_pad / 8}, fc1.p[i].M,
+                               d.feat, cs.red_pad / kPkKB, passes[i].params + o.embed_b, nb.act3[passes[i].set], l->n_head[hp],
+                               d.feat, keep ? l->E0 : nullptr, img, imgT);
   }
   DZ_TRY(launch_pgemm("iqn_embed_fwd", eb, stream, 1));
 
@@ -2524,11 +2573,8 @@ int forward_heads_iqn(dz_learner* l, const NetBufs& nb, const Pass* passes, int 
   const dz_learner_config& c = l->cfg;
   GemmBatch gb;
   gb.n = np;
-  for (int i = 0; i < np; ++i) {
-    long long rows = (long long)nimg * l->n_head[passes[i].head];
-    DZ_LAUNCH(iqn_cos_kernel, (unsigned)ceil_div(rows * c.latent_dim, 256), 256, 0, stream, taus[i], nb.cosf[passes[i].head],
-              rows, c.latent_dim);
-  }
+  for (int i = 0; i < np; ++i)
+    DZ_TRY(launch_iqn_cos(taus[i], nb.cosf[passes[i].head], (long long)nimg * l->n_head[passes[i].head], c.latent_dim, stream));
   const bool packed = l->pk_on && nimg == l->B && np == 3;
   if (!packed) {
     for (int i = 0; i < np; ++i) {
@@ -2558,19 +2604,15 @@ int forward_heads_iqn(dz_learner* l, const NetBufs& nb, const Pass* passes, int 
     DZ_TRY(run_nn("iqn_fc1_fwd", gb, false, stream));
   }
   if (((long long)nimg * l->n_head[passes[0].head] >= 512 || row_invariant) && d.out <= kSkinnyMaxN && np <= 3) {
-    SkinnyHead h;
-    memset(&h, 0, sizeof(h));
-    h.n = np;
-    int maxM = 0;
+    const float* h1[3];
+    const float* prm[3];
+    float* out[3];
+    int M[3];
     for (int i = 0; i < np; ++i) {
       int hp = passes[i].head;
-      h.A[i] = nb.h1[hp][0]; h.W[i] = passes[i].params + o.w2[0]; h.bias[i] = passes[i].params + o.b2[0];
-      h.out[i] = nb.out[hp]; h.M[i] = nimg * l->n_head[hp];
-      maxM = std::max(maxM, h.M[i]);
+      h1[i] = nb.h1[hp][0]; prm[i] = passes[i].params; out[i] = nb.out[hp]; M[i] = nimg * l->n_head[hp];
     }
-    dim3 grid((unsigned)std::min<int64_t>(ceil_div(maxM, 8), kNumSMs * 2), (unsigned)np);
-    DZ_LAUNCH_NAMED("iqn_head_fwd", iqn_head_fwd_kernel, grid, 256, 0, stream, h, d.out);
-    return DZ_OK;
+    return launch_iqn_head_fwd(l, np, h1, prm, out, M, stream);
   }
   for (int i = 0; i < np; ++i) {
     int hp = passes[i].head;
@@ -2834,8 +2876,7 @@ int backward_iqn(dz_learner* l, void* stream) {
     p.B = P + o.w2[0]; p.ldb = d.out; p.C = l->dh1[0]; p.ldc = 512; p.mask = l->h1[0][0];
     gb.p[0] = p;
     if (M >= 512 && d.out <= kSkinnyMaxN) {
-      DZ_LAUNCH_NAMED("iqn_head_dgrad", iqn_head_dgrad_kernel, (unsigned)std::min<int64_t>(ceil_div((long long)M * 128, 256), kNumSMs * 8),
-                      256, 0, stream, l->dout, P + o.w2[0], l->h1[0][0], l->dh1[0], M, d.out);
+      DZ_TRY(launch_iqn_head_dgrad(l, l->dout, P, l->h1[0][0], l->dh1[0], M, stream));
     } else {
       DZ_TRY(run_nt("iqn_head_dgrad", gb, false, stream));
     }
@@ -2890,9 +2931,8 @@ int backward_iqn(dz_learner* l, void* stream) {
   }
   }
   if (l->pk_embed_bwd) {
-    dim3 hgrid((unsigned)(d.feat / 64), (unsigned)B);
-    DZ_LAUNCH(iqn_hadamard_bwd_packed_kernel, hgrid, 256, 0, stream, l->dhi, l->E0, l->act3[0], l->dact3, l->pk_dET.hi,
-              l->pk_dET.lo, l->pk_dET.rows_pad / 8, d.feat);
+    DZ_TRY(launch_iqn_hadamard_bwd(true, l->dhi, l->E0, l->act3[0], l->dact3, l->pk_dET.hi, l->pk_dET.lo, l->pk_dET.rows_pad / 8,
+                                   B, N, d.feat, stream));
     // embed wgrad: [feat, latent + 1 (bias column)] = dE^T * [cos | 1], stored transposed into the [latent + 1, feat] partials
     PkBatch kb;
     memset(&kb, 0, sizeof(kb));
@@ -2906,8 +2946,7 @@ int backward_iqn(dz_learner* l, void* stream) {
     DZ_TRY(launch_pgemm("iqn_embed_wgrad", kb, l->side.fork(stream, stream)));
     fb.f[fb.n++] = FinishTN{p.C, p.splits, p.split_stride, c.latent_dim, d.feat, G + o.embed_w, nullptr, G + o.embed_b, nullptr, nullptr, nullptr};
   } else {
-  DZ_LAUNCH(iqn_hadamard_bwd_kernel, (unsigned)ceil_div((long long)B * d.feat, 256), 256, 0, stream, l->dhi, l->E0, l->act3[0],
-              l->dact3, B, N, d.feat);
+    DZ_TRY(launch_iqn_hadamard_bwd(false, l->dhi, l->E0, l->act3[0], l->dact3, nullptr, nullptr, 0, B, N, d.feat, stream));
     {  // embed wgrad: [latent, feat] = cos^T * dE
       GemmProblem p = zero_problem();
       p.a_mode = A_PLAIN; p.A = l->cosf[0]; p.lda = c.latent_dim; p.M = M; p.K = c.latent_dim;
@@ -3973,6 +4012,58 @@ int dz_test_dueling_head_bwd(dz_learner* l, int32_t rows, float* d_dq, float* d_
   if (!d_h1[0] || !d_h1[1] || !d_dh1[0] || !d_dh1[1] || (!d_hi != !d_lo) || (d_hi && (!d_hi[0] || !d_hi[1] || !d_lo[0] || !d_lo[1])))
     return fail(DZ_EINVAL, "test_dueling_head_bwd: NULL buffer");
   return launch_dueling_head_bwd(l, rows, d_dq, d_dval, d_h1, d_params, d_dh1, d_hi, d_lo, d_noise, stream);
+}
+
+// Test hook: IQN's cosine features (launch_iqn_cos) on caller-owned buffers.
+int dz_test_iqn_cos(const float* d_taus, int64_t rows, int32_t latent, float* d_out, void* stream) {
+  if (!d_taus || !d_out) return fail(DZ_EINVAL, "test_iqn_cos: NULL buffer");
+  if (rows < 1 || latent < 1) return fail(DZ_EINVAL, "test_iqn_cos: rows and latent must be >= 1");
+  return launch_iqn_cos(d_taus, d_out, rows, latent, stream);
+}
+
+static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+
+// Test hook: IQN's value head (launch_iqn_head_fwd) of an IQN-network learner's layout on caller-owned buffers.
+int dz_test_iqn_head_fwd(dz_learner* l, int32_t np, const int32_t* M, const float* const* d_h1, const float* const* d_params,
+                         float* const* d_out, void* stream) {
+  if (!l || !M || !d_h1 || !d_params || !d_out) return fail(DZ_EINVAL, "test_iqn_head_fwd: NULL argument");
+  if (!uses_iqn_net(l->cfg.kind)) return fail(DZ_EINVAL, "test_iqn_head_fwd: the learner has no IQN network");
+  if (l->d.out > kSkinnyMaxN) return fail(DZ_EINVAL, "test_iqn_head_fwd: the one-warp-per-row head takes at most 18 actions");
+  if (np < 1 || np > 3) return fail(DZ_EINVAL, "test_iqn_head_fwd: np must be in [1, 3]");
+  int m[3];
+  for (int i = 0; i < np; ++i) {
+    if (M[i] < 1) return fail(DZ_EINVAL, "test_iqn_head_fwd: M must be >= 1");
+    if (!d_h1[i] || !d_params[i] || !d_out[i]) return fail(DZ_EINVAL, "test_iqn_head_fwd: NULL buffer");
+    if (misaligned16(d_h1[i])) return fail(DZ_EINVAL, "test_iqn_head_fwd: h1 rows are read as float4");
+    m[i] = M[i];
+  }
+  return launch_iqn_head_fwd(l, np, d_h1, d_params, d_out, m, stream);
+}
+
+// Test hook: the value head's input gradient (launch_iqn_head_dgrad) of an IQN-network learner's layout.
+int dz_test_iqn_head_dgrad(dz_learner* l, int32_t M, const float* d_dout, const float* d_params, const float* d_h1,
+                           float* d_dh1, void* stream) {
+  if (!l || !d_dout || !d_params || !d_h1 || !d_dh1) return fail(DZ_EINVAL, "test_iqn_head_dgrad: NULL argument");
+  if (!uses_iqn_net(l->cfg.kind)) return fail(DZ_EINVAL, "test_iqn_head_dgrad: the learner has no IQN network");
+  if (l->d.out > kSkinnyMaxN) return fail(DZ_EINVAL, "test_iqn_head_dgrad: the kernel takes at most 18 actions");
+  if (M < 1) return fail(DZ_EINVAL, "test_iqn_head_dgrad: M must be >= 1");
+  if (misaligned16(d_h1) || misaligned16(d_dh1)) return fail(DZ_EINVAL, "test_iqn_head_dgrad: h1 and dh1 are accessed as float4");
+  return launch_iqn_head_dgrad(l, d_dout, d_params, d_h1, d_dh1, M, stream);
+}
+
+// Test hook: the backward of IQN's Hadamard product (launch_iqn_hadamard_bwd), unpacked or packed.
+int dz_test_iqn_hadamard_bwd(int32_t packed, int32_t B, int32_t N, int32_t D, float* d_dhi, const float* d_E, const float* d_F,
+                             float* d_dfeat, float* d_img_hi, float* d_img_lo, int32_t img_rows_pad, void* stream) {
+  if (!d_dhi || !d_E || !d_F || !d_dfeat) return fail(DZ_EINVAL, "test_iqn_hadamard_bwd: NULL buffer");
+  if (B < 1 || N < 1 || D < 1) return fail(DZ_EINVAL, "test_iqn_hadamard_bwd: B, N and D must be >= 1");
+  if (packed) {
+    if (N != 64 || D % 64) return fail(DZ_EINVAL, "test_iqn_hadamard_bwd: the packed kernel needs N = 64 and D % 64 = 0");
+    if (!d_img_hi || !d_img_lo || img_rows_pad % 128 || img_rows_pad < D)
+      return fail(DZ_EINVAL, "test_iqn_hadamard_bwd: the packed kernel writes a [rows_pad >= D][B * 64] image");
+    if (misaligned16(d_dhi) || misaligned16(d_E) || misaligned16(d_F) || misaligned16(d_img_hi) || misaligned16(d_img_lo))
+      return fail(DZ_EINVAL, "test_iqn_hadamard_bwd: the packed kernel accesses its buffers as float4");
+  }
+  return launch_iqn_hadamard_bwd(packed != 0, d_dhi, d_E, d_F, d_dfeat, d_img_hi, d_img_lo, img_rows_pad / 8, B, N, D, stream);
 }
 
 // Test hook: device pointer + element count of an internal activation / gradient buffer (tests and tools only).

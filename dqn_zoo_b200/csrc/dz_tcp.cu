@@ -68,6 +68,20 @@ int launch_pgemm(const char* tag, const PkBatch& kb, void* stream, int epi) {
   return epi ? launch_pgemm_t<1>(tag, kb, stream) : launch_pgemm_t<0>(tag, kb, stream);
 }
 
+PkProblem pk_embed_problem(const PkOperand& cos, const PkOperand& weT, int M, int D, int nkb, const float* bias,
+                           const float* mul, int mul_div, int mul_ld, float* e0, const PkTarget& img, const PkTarget& imgT) {
+  PkProblem p;
+  memset(&p, 0, sizeof(p));
+  p.A = cos; p.B = weT;
+  p.MI = M; p.NJ = D; p.nkb = nkb; p.splits = 1;
+  p.bias_j = bias;
+  p.mul = mul; p.mul_div = mul_div; p.mul_ld = mul_ld;
+  p.e0 = e0; p.e0_ld = D;
+  p.img_hi = img.hi; p.img_lo = img.lo; p.img_rg = img.rg;
+  if (imgT.hi) { p.imgT_hi = imgT.hi; p.imgT_lo = imgT.lo; p.imgT_rg = imgT.rg; }
+  return p;
+}
+
 }  // namespace dz
 
 using namespace dz;
@@ -104,4 +118,37 @@ extern "C" int dz_test_tc_pgemm(const float* d_A, int32_t a_rows, int32_t a_ld, 
   p.MI = a_rows + (a_ones_row >= 0 ? 1 : 0); p.NJ = b_rows; p.nkb = rp / kPkKB;
   p.C = d_C; p.sc_i = sc_i; p.sc_j = sc_j; p.splits = splits; p.split_stride = split_stride; p.bias_j = d_bias; p.relu = relu;
   return launch_pgemm("tc_pgemm_selftest", kb, stream);
+}
+
+// Self test of the IQN embedding epilogue (EPI 1): packs cos [M][latent] and embed_w [latent][D] as the learner's
+// forward does, then runs the embedding problem of pk_embed_problem into the caller's images.
+extern "C" int dz_test_iqn_embed_packed(const float* d_cos, int32_t M, int32_t latent, const float* d_embed_w, int32_t D,
+                                        const float* d_bias, const float* d_mul, int32_t mul_div, int32_t mul_ld,
+                                        float* d_work, float* d_e0, float* d_img_hi, float* d_img_lo, float* d_imgT_hi,
+                                        float* d_imgT_lo, void* stream) {
+  if (!d_cos || !d_embed_w || !d_bias || !d_mul || !d_work || !d_img_hi || !d_img_lo || (!d_imgT_hi != !d_imgT_lo))
+    return fail(DZ_EINVAL, "test_iqn_embed_packed: NULL buffer");
+  if (latent < 1 || latent > 8 * kPkKB) return fail(DZ_EINVAL, "test_iqn_embed_packed: latent must be in [1, 128]");
+  if (M < 4 || M % 4 || D < 4 || D % 4) return fail(DZ_EINVAL, "test_iqn_embed_packed: M and D must be positive multiples of 4");
+  if (mul_div < 1 || mul_ld < D || mul_ld % 4) return fail(DZ_EINVAL, "test_iqn_embed_packed: mul_div >= 1, mul_ld >= D and a multiple of 4");
+  auto misaligned = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) != 0; };
+  if (misaligned(d_bias) || misaligned(d_mul) || (d_e0 && misaligned(d_e0)))
+    return fail(DZ_EINVAL, "test_iqn_embed_packed: bias, mul and e0 are read and written as float4");
+  const int ar = (int)(ceil_div(M, 128) * 128), br = (int)(ceil_div(D, 256) * 256);
+  const int rp = (int)(ceil_div(latent, kPkKB) * kPkKB);
+  float* c_hi = d_work; float* c_lo = c_hi + (int64_t)ar * rp;
+  float* w_hi = c_lo + (int64_t)ar * rp; float* w_lo = w_hi + (int64_t)br * rp;
+  PackBatch pb;
+  memset(&pb, 0, sizeof(pb));
+  DZ_TRY(pk_add_job(pb, d_cos, latent, 1, M, latent, ar, rp, -1, c_hi, c_lo));
+  DZ_TRY(pk_add_job(pb, d_embed_w, D, 0, D, latent, br, rp, -1, w_hi, w_lo));
+  DZ_TRY(launch_pack("iqn_pack_selftest", pb, stream));
+  PkBatch kb;
+  memset(&kb, 0, sizeof(kb));
+  kb.n = 1;
+  const PkTarget img{d_img_hi, d_img_lo, ar / 8};
+  const PkTarget imgT{d_imgT_hi, d_imgT_lo, (int)(ceil_div(D + 1, 128) * 128) / 8};
+  kb.p[0] = pk_embed_problem(PkOperand{c_hi, c_lo, ar / 8}, PkOperand{w_hi, w_lo, br / 8}, M, D, rp / kPkKB, d_bias, d_mul,
+                             mul_div, mul_ld, d_e0, img, imgT);
+  return launch_pgemm("iqn_embed_selftest", kb, stream, 1);
 }

@@ -746,6 +746,24 @@ int dz_test_dueling_head_fwd(dz_learner* l, int32_t rows, int32_t np, const floa
 int dz_test_dueling_head_bwd(dz_learner* l, int32_t rows, float* d_dq, float* d_dval, const float* const* d_h1,
                              const float* d_params, const float* d_noise, float* const* d_dh1, float* const* d_hi,
                              float* const* d_lo, void* stream);
+/* IQN's cosine features on caller-owned buffers; tests only: d_out [rows][latent] = cos(fl(fl((j + 1) pi_f) tau_r)) of
+ * d_taus [rows]. */
+int dz_test_iqn_cos(const float* d_taus, int64_t rows, int32_t latent, float* d_out, void* stream);
+/* IQN's value head of IQN-network learner l's layout (A = num_actions <= 18) on caller-owned buffers; tests only.  np in
+ * 1..3 applies in one launch: apply i reads d_h1[i] [M[i]][512] (16-byte aligned) and the head of the parameter blob
+ * d_params[i], and writes d_out[i] [M[i]][A].  M: host array of np row counts. */
+int dz_test_iqn_head_fwd(dz_learner* l, int32_t np, const int32_t* M, const float* const* d_h1, const float* const* d_params,
+                         float* const* d_out, void* stream);
+/* The value head's input gradient of learner l's layout; tests only: d_dh1 [M][512] = [d_h1 > 0] d_dout W^T with d_dout
+ * [M][A] and W the head of d_params (A <= 18). */
+int dz_test_iqn_head_dgrad(dz_learner* l, int32_t M, const float* d_dout, const float* d_params, const float* d_h1,
+                           float* d_dh1, void* stream);
+/* The backward of IQN's Hadamard product E * F; tests only.  d_E, d_dhi [B][N][D], d_F, d_dfeat [B][D]: d_dfeat = [F > 0]
+ * sum_n dhi E, dE = [E > 0] dhi F.  packed = 0: dE replaces d_dhi in place (the image arguments are unused).  packed = 1
+ * (N = 64, D % 64 = 0): d_dhi is read only and dE is written as the hi/lo tf32 tile image of rows k < D and reduction
+ * b * 64 + n into d_img_hi / d_img_lo ([img_rows_pad][B * 64], img_rows_pad a multiple of 128). */
+int dz_test_iqn_hadamard_bwd(int32_t packed, int32_t B, int32_t N, int32_t D, float* d_dhi, const float* d_E, const float* d_F,
+                             float* d_dfeat, float* d_img_hi, float* d_img_lo, int32_t img_rows_pad, void* stream);
 int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream);   /* device-to-device, tests only */
 /* Debug: the tensor-core launch named `tag` writes the clock stamps of its CTA 0 into d_trace (512 int64). */
 int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace);
@@ -773,6 +791,16 @@ int dz_test_tc_pgemm(const float* d_A, int32_t a_rows, int32_t a_ld, int32_t a_r
                      int32_t b_rows, int32_t b_ld, int32_t b_red_contig, int32_t red, int32_t a_ones_row,
                      float* d_work, float* d_C, int64_t sc_i, int64_t sc_j, int32_t splits, int64_t split_stride,
                      const float* d_bias, int32_t relu, void* stream);
+/* Self-test of the IQN embedding epilogue of the packed-operand GEMM (the learner's embedding forward): packs d_cos
+ * [M][latent] and d_embed_w [latent][D] into d_work (dz_test_tc_pgemm_work(M, D, latent) floats), then with
+ * v = relu(cos W + d_bias[j]) writes v to d_e0 [M][D] (or nothing when NULL) and h = v * d_mul[(i / mul_div) * mul_ld + j]
+ * as the hi/lo tf32 tile images d_img_hi / d_img_lo (rows i, [ceil(M / 128) 128][ceil(D / 16) 16]) and, when given,
+ * d_imgT_hi / d_imgT_lo (rows j, [ceil((D + 1) / 128) 128][ceil(M / 16) 16]).  Only the valid elements of the images
+ * are written.  latent <= 128; M, D, mul_ld multiples of 4; mul_ld >= D; d_bias, d_mul, d_e0 16-byte aligned. */
+int dz_test_iqn_embed_packed(const float* d_cos, int32_t M, int32_t latent, const float* d_embed_w, int32_t D,
+                             const float* d_bias, const float* d_mul, int32_t mul_div, int32_t mul_ld, float* d_work,
+                             float* d_e0, float* d_img_hi, float* d_img_lo, float* d_imgT_hi, float* d_imgT_lo,
+                             void* stream);
 /* Self-test of the TMA-fed tensor-core GEMM family (csrc/dz_umma.cuh; conv / FC layers of the batch-32 step):
  * C[MI][NJ] = sum_r A(i,r) B(j,r), NJ <= 64.  x_mn_major = 0: the operand is stored [rows][R]; 1: [R][rows] (the
  * MMA warps' fragment loads transpose).  convert = 0: operands pre-split into tf32 hi/lo arrays (activation path);
