@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB_DIR = os.path.join(HERE, 'lib')
 LIB_PATH = os.path.join(LIB_DIR, 'libdqnzoo_b200.so')
-SOURCES = ['dz_replay.cu', 'dz_frames.cu', 'dz_learner.cu', 'dz_tcp.cu', 'dz_umma.cu', 'dz_umma_net.cu', 'dz_preprocess.cu', 'dz_jaxprng.cu', 'dz_checkpoint.cu', 'dz_env.cu', 'dz_breakout.cu', 'dz_pong.cu']
+SOURCES = ['dz_replay.cu', 'dz_frames.cu', 'dz_learner.cu', 'dz_tcp.cu', 'dz_umma.cu', 'dz_umma_net.cu', 'dz_preprocess.cu', 'dz_jaxprng.cu', 'dz_checkpoint.cu', 'dz_catch.cu', 'dz_breakout.cu', 'dz_pong.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 

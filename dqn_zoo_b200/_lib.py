@@ -98,30 +98,22 @@ class LearnIO(C.Structure):
               ('update_out', UpdateOutputs), ('d_max_seen_priority', vp), ('priority_exponent', f64)]
 
 
-class CatchConfig(C.Structure):   # struct dz_catch_config
+class GameConfig(C.Structure):   # struct dz_game_config: dz_catch_config, dz_breakout_config, dz_pong_config
   _fields_ = [('num_streams', i32), ('num_actions', i32), ('min_noop_steps', i32), ('max_noop_steps', i32),
               ('seed', C.c_uint32), ('stream_offset', C.c_uint32)]
 
+
+CatchConfig = BreakoutConfig = PongConfig = GameConfig
 
 CATCH_STATE_FIELDS = ('paddle_x', 'ball_x', 'ball_y', 'ball_dx', 'lives', 'balls_left', 'counter', 'noops', 'over')
 CATCH_MAX_STREAMS = 4096
 CATCH_MAX_NOOP_STEPS = 89
 
 
-class BreakoutConfig(C.Structure):   # struct dz_breakout_config
-  _fields_ = [('num_streams', i32), ('num_actions', i32), ('min_noop_steps', i32), ('max_noop_steps', i32),
-              ('seed', C.c_uint32), ('stream_offset', C.c_uint32)]
-
-
 BREAKOUT_STATE_FIELDS = ('paddle_x', 'ball_x', 'ball_y', 'ball_dx', 'ball_dy', 'in_play', 'serve_timer', 'lives',
                          'row0', 'row1', 'row2', 'row3', 'row4', 'row5', 'counter', 'noops', 'over')
 BREAKOUT_MAX_STREAMS = 4096
 BREAKOUT_MAX_NOOP_STEPS = 63
-
-
-class PongConfig(C.Structure):   # struct dz_pong_config
-  _fields_ = [('num_streams', i32), ('num_actions', i32), ('min_noop_steps', i32), ('max_noop_steps', i32),
-              ('seed', C.c_uint32), ('stream_offset', C.c_uint32)]
 
 
 PONG_STATE_FIELDS = ('paddle_y', 'opponent_y', 'ball_x', 'ball_y', 'ball_dx', 'ball_dy', 'in_play', 'serve_timer',

@@ -1,5 +1,5 @@
 // Threefry-2x32, 20 rounds (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3"): the counter-based generator
-// behind jax.random at the pinned jax 0.3.10 (dz_jaxprng.cu) and the randomness of the device Catch game (dz_env.cu).
+// behind jax.random at the pinned jax 0.3.10 (dz_jaxprng.cu) and the randomness of the device games (dz_game.cuh).
 // One definition, compiled for the host and the device; its known answers are in dz_jaxprng.cu.
 #pragma once
 #include <stdint.h>

@@ -1,4 +1,4 @@
-"""Games at Atari geometry, simulated and rendered on the device: Catch (csrc/dz_env.cu; rules in DESIGN.md §10),
+"""Games at Atari geometry, simulated and rendered on the device: Catch (csrc/dz_catch.cu; rules in DESIGN.md §10),
 Breakout (csrc/dz_breakout.cu; DESIGN.md §11) and Pong (csrc/dz_pong.cu; DESIGN.md §12).
 
 `VectorCatch` / `VectorBreakout` / `VectorPong` step E streams of a game with one kernel launch per tick and leave their 210x160x3 RGB

@@ -560,47 +560,52 @@ int dz_jax_uniform(const uint32_t* d_keys, const int64_t* counts, int32_t nblock
 /* threefry2x32 (20 rounds) evaluated on the HOST by the same source the kernel compiles; tests only. */
 int dz_test_threefry2x32(uint32_t k0, uint32_t k1, uint32_t c0, uint32_t c1, uint32_t* out2);
 
-/* ---- Catch at Atari geometry on the device (DESIGN.md §10) ------------------------------------------------------
- * E streams of the game, each simulated and rendered as a 210x160x3 uint8 RGB frame in HBM.  State: int32
- * [DZ_CATCH_STATE_FIELDS][E] device array (fields paddle_x, ball_x, ball_y, ball_dx, lives, balls_left, counter, noops,
- * over); a new state is all 0 but over = 1, so that the first tick of every stream is a reset.  Stream e's randomness:
- * key = threefry2x32((0, seed), (stream_offset + e, 0)). */
+/* ---- Games at Atari geometry on the device (DESIGN.md §10-§12) -------------------------------------------------
+ * Catch, Breakout and Pong run E streams each, every stream simulated and rendered as a 210x160x3 uint8 RGB frame in
+ * HBM, and share one configuration and one calling convention.  State: int32 [DZ_<GAME>_STATE_FIELDS][E] device array
+ * (the fields are listed per game below); a new state is all 0 but over = 1, so that the first tick of every stream is
+ * a reset.  Stream e's randomness: key = threefry2x32((0, seed), (stream_offset + e, tag)), tag 0 for Catch, 1 for
+ * Breakout, 2 for Pong.
+ *
+ * dz_<game>_step: one tick of all E streams.  h_control: PINNED int32 [2][E] (row 0 actions, row 1 reset flags:
+ * non-zero starts a new episode instead of stepping; so does stepping a stream whose last step was LAST), checked on
+ * the host (an action outside [0, A) of a stream that is not reset is DZ_EINVAL) and copied into d_control (device
+ * int32 [2][E]).  The kernel updates d_state, writes every stream's frame into d_frames (device uint8 [E][210][160][3],
+ * 16-byte aligned) and d_record (device int32 [DZ_<GAME>_RECORD_FIELDS][E]: step_type 0 FIRST / 1 MID / 2 LAST,
+ * reward, discount, lives; reward and discount are 0 on FIRST), which is copied to h_record (PINNED, same shape).  All
+ * on `stream`; the caller synchronises before reading h_record or reusing h_control.
+ * dz_<game>_render: renders every stream's frame from d_state (e.g. after the state was restored); the state is not
+ * changed.
+ * dz_test_<game>_step: the kernel's tick and picture evaluated on the HOST by the same source: stream id
+ * cfg->stream_offset, state int32 [DZ_<GAME>_STATE_FIELDS] updated in place, frame (NULL: not rendered) 210*160*3
+ * bytes, record int32 [4]; tests only. */
+typedef struct dz_game_config {
+  int32_t num_streams;      /* E in [1, DZ_<GAME>_MAX_STREAMS] */
+  int32_t num_actions;      /* A in [the game's minimum, 18] */
+  int32_t min_noop_steps;   /* 0 <= min <= max <= DZ_<GAME>_MAX_NOOP_STEPS */
+  int32_t max_noop_steps;
+  uint32_t seed;
+  uint32_t stream_offset;   /* stream_offset + E <= 2^32 */
+} dz_game_config;
+
+/* Catch (DESIGN.md §10).  State fields paddle_x, ball_x, ball_y, ball_dx, lives, balls_left, counter, noops, over.
+ * Actions: A in [3, 18]: 0 stay, 1 left, 2 right, 3.. stay. */
 #define DZ_CATCH_HEIGHT 210
 #define DZ_CATCH_WIDTH 160
 #define DZ_CATCH_STATE_FIELDS 9
 #define DZ_CATCH_RECORD_FIELDS 4
 #define DZ_CATCH_MAX_STREAMS 4096
 #define DZ_CATCH_MAX_NOOP_STEPS 89   /* the first ball lands on the 90th frame after a reset */
-typedef struct dz_catch_config {
-  int32_t num_streams;      /* E in [1, 4096] */
-  int32_t num_actions;      /* A in [3, 18]: 0 stay, 1 left, 2 right, 3.. stay */
-  int32_t min_noop_steps;   /* 0 <= min <= max <= DZ_CATCH_MAX_NOOP_STEPS */
-  int32_t max_noop_steps;
-  uint32_t seed;
-  uint32_t stream_offset;   /* stream_offset + E <= 2^32 */
-} dz_catch_config;
-/* One tick of all E streams.  h_control: PINNED int32 [2][E] (row 0 actions, row 1 reset flags: non-zero starts a new
- * episode instead of stepping; so does stepping a stream whose last step was LAST), checked on the host (an action
- * outside [0, A) of a stream that is not reset is DZ_EINVAL) and copied into d_control (device int32 [2][E]).  The
- * kernel updates d_state, writes every stream's frame into d_frames (device uint8 [E][210][160][3], 16-byte aligned)
- * and d_record (device int32 [DZ_CATCH_RECORD_FIELDS][E]: step_type 0 FIRST / 1 MID / 2 LAST, reward, discount,
- * lives; reward and discount are 0 on FIRST), which is copied to h_record (PINNED, same shape).  All on `stream`;
- * the caller synchronises before reading h_record or reusing h_control. */
+typedef dz_game_config dz_catch_config;
 int dz_catch_step(const dz_catch_config* cfg, int32_t* d_state, const int32_t* h_control, int32_t* d_control,
                   uint8_t* d_frames, int32_t* d_record, int32_t* h_record, void* stream);
-/* Renders every stream's frame from d_state (e.g. after the state was restored); the state is not changed. */
 int dz_catch_render(const dz_catch_config* cfg, int32_t* d_state, uint8_t* d_frames, void* stream);
-/* The kernel's tick and picture evaluated on the HOST by the same source: stream id cfg->stream_offset, state int32
- * [DZ_CATCH_STATE_FIELDS] updated in place, frame (NULL: not rendered) 210*160*3 bytes, record int32 [4]; tests only. */
 int dz_test_catch_step(const dz_catch_config* cfg, int32_t* state, int32_t action, int32_t reset, uint8_t* frame,
                        int32_t* record);
 
-/* ---- Breakout at Atari geometry on the device (DESIGN.md §11) ---------------------------------------------------
- * The project's own Breakout (not ALE's): E streams, each simulated and rendered as a 210x160x3 uint8 RGB frame in
- * HBM.  State: int32 [DZ_BREAKOUT_STATE_FIELDS][E] device array (fields paddle_x, ball_x, ball_y, ball_dx, ball_dy,
- * in_play, serve_timer, lives, row0..row5 (18-bit brick masks, bit c = brick (r, c) is there), counter, noops, over);
- * a new state is all 0 but over = 1, so that the first tick of every stream is a reset.  Stream e's randomness:
- * key = threefry2x32((0, seed), (stream_offset + e, 1)). */
+/* The project's own Breakout (not ALE's; DESIGN.md §11).  State fields paddle_x, ball_x, ball_y, ball_dx, ball_dy,
+ * in_play, serve_timer, lives, row0..row5 (18-bit brick masks, bit c = brick (r, c) is there), counter, noops, over.
+ * Actions: A in [4, 18]: 0 no-op, 1 fire, 2 right, 3 left, 4.. no-op. */
 #define DZ_BREAKOUT_HEIGHT 210
 #define DZ_BREAKOUT_WIDTH 160
 #define DZ_BREAKOUT_BRICK_ROWS 6
@@ -609,59 +614,26 @@ int dz_test_catch_step(const dz_catch_config* cfg, int32_t* state, int32_t actio
 #define DZ_BREAKOUT_RECORD_FIELDS 4
 #define DZ_BREAKOUT_MAX_STREAMS 4096
 #define DZ_BREAKOUT_MAX_NOOP_STEPS 63   /* below the 64-frame serve delay: no ball is served during the no-ops */
-typedef struct dz_breakout_config {
-  int32_t num_streams;      /* E in [1, 4096] */
-  int32_t num_actions;      /* A in [4, 18]: 0 no-op, 1 fire, 2 right, 3 left, 4.. no-op */
-  int32_t min_noop_steps;   /* 0 <= min <= max <= DZ_BREAKOUT_MAX_NOOP_STEPS */
-  int32_t max_noop_steps;
-  uint32_t seed;
-  uint32_t stream_offset;   /* stream_offset + E <= 2^32 */
-} dz_breakout_config;
-/* One tick of all E streams, with dz_catch_step's conventions: h_control PINNED int32 [2][E] (actions, reset flags),
- * checked on the host and copied into d_control; d_state updated, d_frames (device uint8 [E][210][160][3], 16-byte
- * aligned) rewritten, d_record (device int32 [DZ_BREAKOUT_RECORD_FIELDS][E]: step_type, reward, discount, lives)
- * copied to h_record (PINNED).  All on `stream`; the caller synchronises before reading h_record. */
+typedef dz_game_config dz_breakout_config;
 int dz_breakout_step(const dz_breakout_config* cfg, int32_t* d_state, const int32_t* h_control, int32_t* d_control,
                      uint8_t* d_frames, int32_t* d_record, int32_t* h_record, void* stream);
-/* Renders every stream's frame from d_state (e.g. after the state was restored); the state is not changed. */
 int dz_breakout_render(const dz_breakout_config* cfg, int32_t* d_state, uint8_t* d_frames, void* stream);
-/* The kernel's tick and picture evaluated on the HOST by the same source: stream id cfg->stream_offset, state int32
- * [DZ_BREAKOUT_STATE_FIELDS] updated in place, frame (NULL: not rendered) 210*160*3 bytes, record int32 [4]; tests
- * only. */
 int dz_test_breakout_step(const dz_breakout_config* cfg, int32_t* state, int32_t action, int32_t reset, uint8_t* frame,
                           int32_t* record);
 
-/* ---- Pong at Atari geometry on the device (DESIGN.md §12) -------------------------------------------------------
- * The project's own Pong (not ALE's): E streams against a scripted opponent, each simulated and rendered as a
- * 210x160x3 uint8 RGB frame in HBM.  State: int32 [DZ_PONG_STATE_FIELDS][E] device array (fields paddle_y, opponent_y,
- * ball_x, ball_y, ball_dx, ball_dy, in_play, serve_timer, agent_score, opponent_score, counter, noops, over); a new
- * state is all 0 but over = 1, so that the first tick of every stream is a reset.  Stream e's randomness:
- * key = threefry2x32((0, seed), (stream_offset + e, 2)). */
+/* The project's own Pong (not ALE's; DESIGN.md §12), against a scripted opponent.  State fields paddle_y, opponent_y,
+ * ball_x, ball_y, ball_dx, ball_dy, in_play, serve_timer, agent_score, opponent_score, counter, noops, over.
+ * Actions: A in [6, 18]: 0 no-op, 1 fire, 2 up, 3 down, 4 up + fire, 5 down + fire, 6.. no-op. */
 #define DZ_PONG_HEIGHT 210
 #define DZ_PONG_WIDTH 160
 #define DZ_PONG_STATE_FIELDS 13
 #define DZ_PONG_RECORD_FIELDS 4
 #define DZ_PONG_MAX_STREAMS 4096
 #define DZ_PONG_MAX_NOOP_STEPS 63   /* below the 64-frame serve delay: no ball is served during the no-ops */
-typedef struct dz_pong_config {
-  int32_t num_streams;      /* E in [1, 4096] */
-  int32_t num_actions;      /* A in [6, 18]: 0 no-op, 1 fire, 2 up, 3 down, 4 up + fire, 5 down + fire, 6.. no-op */
-  int32_t min_noop_steps;   /* 0 <= min <= max <= DZ_PONG_MAX_NOOP_STEPS */
-  int32_t max_noop_steps;
-  uint32_t seed;
-  uint32_t stream_offset;   /* stream_offset + E <= 2^32 */
-} dz_pong_config;
-/* One tick of all E streams, with dz_catch_step's conventions: h_control PINNED int32 [2][E] (actions, reset flags),
- * checked on the host and copied into d_control; d_state updated, d_frames (device uint8 [E][210][160][3], 16-byte
- * aligned) rewritten, d_record (device int32 [DZ_PONG_RECORD_FIELDS][E]: step_type, reward, discount, lives)
- * copied to h_record (PINNED).  All on `stream`; the caller synchronises before reading h_record. */
+typedef dz_game_config dz_pong_config;
 int dz_pong_step(const dz_pong_config* cfg, int32_t* d_state, const int32_t* h_control, int32_t* d_control,
                  uint8_t* d_frames, int32_t* d_record, int32_t* h_record, void* stream);
-/* Renders every stream's frame from d_state (e.g. after the state was restored); the state is not changed. */
 int dz_pong_render(const dz_pong_config* cfg, int32_t* d_state, uint8_t* d_frames, void* stream);
-/* The kernel's tick and picture evaluated on the HOST by the same source: stream id cfg->stream_offset, state int32
- * [DZ_PONG_STATE_FIELDS] updated in place, frame (NULL: not rendered) 210*160*3 bytes, record int32 [4]; tests
- * only. */
 int dz_test_pong_step(const dz_pong_config* cfg, int32_t* state, int32_t action, int32_t reset, uint8_t* frame,
                       int32_t* record);
 
