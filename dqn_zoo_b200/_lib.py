@@ -60,7 +60,7 @@ class LearnerConfig(C.Structure):
               ('adam_b1', f32), ('adam_b2', f32), ('max_global_grad_norm', f32), ('munchausen_alpha', f32),
               ('entropy_temperature', f32), ('log_policy_clip', f32), ('num_fractions', i32),
               ('fraction_learning_rate', f32), ('fraction_opt_eps', f32), ('fraction_rms_decay', f32), ('dueling', i32),
-              ('noisy', i32)]
+              ('noisy', i32), ('random_shift_pad', i32)]
 
   def __init__(self, **fields):
     # the loss hyperparameters start at the reference's values instead of 0, which the library rejects for vmax, and
@@ -81,7 +81,7 @@ class LearnerBuffers(C.Structure):
 
 class Batch(C.Structure):
   _fields_ = [('d_s_tm1_rows', vp), ('d_s_t_rows', vp), ('d_a_tm1', vp), ('d_r_t', vp), ('d_discount_t', vp),
-              ('d_weights', vp), ('d_taus', vp), ('d_noise', vp)]
+              ('d_weights', vp), ('d_taus', vp), ('d_noise', vp), ('d_shifts', vp)]
 
 
 class UpdateOutputs(C.Structure):
@@ -95,7 +95,7 @@ class ResampleAxis(C.Structure):   # struct dz_resample_axis
 
 class LearnIO(C.Structure):
   _fields_ = [('sample_in', SampleInputs), ('sample_out', SampleOutputs), ('d_taus', vp), ('d_noise', vp),
-              ('update_out', UpdateOutputs), ('d_max_seen_priority', vp), ('priority_exponent', f64)]
+              ('update_out', UpdateOutputs), ('d_max_seen_priority', vp), ('priority_exponent', f64), ('d_shifts', vp)]
 
 
 class GameConfig(C.Structure):   # struct dz_game_config: dz_catch_config, dz_breakout_config, dz_pong_config
@@ -164,6 +164,7 @@ _SIGNATURES = {
     'dz_learner_learn': (i32, [vp, C.POINTER(ReplayView), i32, C.POINTER(LearnIO), vp]),
     'dz_learner_generate_randomness': (i32, [vp, u64, vp, vp, vp]),
     'dz_learner_generate_randomness_async': (i32, [vp, u64, vp, vp, vp]),
+    'dz_learner_generate_shifts': (i32, [vp, u64, vp, vp]),
     'dz_learner_act_batch': (i32, [vp, vp, i32, vp, vp, i64, vp, f32, vp, vp, vp]),
     'dz_learner_noise_stride': (i32, [C.POINTER(LearnerConfig), C.POINTER(i64)]),
     'dz_learner_generate_stream_noise': (i32, [vp, u64, i32, vp, vp]),
@@ -216,6 +217,7 @@ _SIGNATURES = {
     'dz_test_iqn_head_dgrad': (i32, [vp, i32, vp, vp, vp, vp, vp]),
     'dz_test_iqn_hadamard_bwd': (i32, [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, i32, vp]),
     'dz_test_copy': (i32, [vp, vp, i64, vp]),
+    'dz_test_random_shift': (i32, [vp, vp, vp, i32, i32, i32, i32, i32, vp, i64, vp]),
     'dz_test_learner_trace': (i32, [vp, C.c_char_p, vp]),
     'dz_test_learner_mma_path': (i32, [vp, C.c_char_p, C.POINTER(i32)]),
     'dz_debug_timeline': (i32, [vp]),

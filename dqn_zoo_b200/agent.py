@@ -94,7 +94,7 @@ class _DeviceAgent(parts.Agent):
   def _setup(self, preprocessor, sample_network_input, network: NetworkSpec, optimizer: Optional[OptimizerSpec],
              transition_accumulator, replay, batch_size, exploration_epsilon, min_replay_capacity_fraction,
              learn_period, target_network_update_period, rng_key, grad_error_bound=1.0 / 32, huber_param=1.0,
-             use_cuda_graph=True, **munchausen):
+             use_cuda_graph=True, random_shift_pad=0, **munchausen):
     if network.kind != self.KIND:
       raise ValueError('network spec kind %r does not match agent %r' % (network.kind, self.KIND))
     if sample_network_input is not None and tuple(np.asarray(sample_network_input).shape) != tuple(network.obs_shape):
@@ -111,7 +111,8 @@ class _DeviceAgent(parts.Agent):
     self._seed = _seed_of(rng_key)
     self._host_rng = np.random.RandomState(self._seed % (1 << 32))
     self._learner = learner_lib.Learner(network, batch_size=batch_size, optimizer=optimizer,
-                                        grad_error_bound=grad_error_bound, huber_param=huber_param, **munchausen)
+                                        grad_error_bound=grad_error_bound, huber_param=huber_param,
+                                        random_shift_pad=random_shift_pad, **munchausen)
     self._learner.init_params(seed=self._seed % (1 << 31))      # network.init + target = online
     self._action = None
     self._frame_t = -1
@@ -252,7 +253,7 @@ class _DeviceAgent(parts.Agent):
         held.append(t)
       blobs[name] = t
     state = {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'dueling': bool(L.net.dueling),
-             'noisy': bool(L.net.noisy), 'param_count': L.plan.param_count,
+             'noisy': bool(L.net.noisy), 'random_shift_pad': L.random_shift_pad, 'param_count': L.plan.param_count,
              'opt_state_floats': L.plan.opt_state_floats, 'host_rng': self._host_rng.get_state(), 'seed': self._seed,
              'jax_key': None if getattr(self, '_jax_key', None) is None else self._jax_key.copy(),
              'frame_t': self._frame_t}
@@ -281,11 +282,12 @@ class _DeviceAgent(parts.Agent):
     except (OSError, pickle.UnpicklingError, EOFError) as e:
       raise ValueError('%s is not a readable agent checkpoint: %s' % (directory, e)) from e
     L = self._learner
-    # checkpoints written before the dueling network or noisy networks existed have no 'dueling' / 'noisy' key: they
-    # hold the plain network
-    ck.validate(dict({'dueling': False, 'noisy': False}, **state),
+    # checkpoints written before the dueling network, noisy networks or random-shift augmentation existed have no
+    # 'dueling' / 'noisy' / 'random_shift_pad' key: they hold the plain network, trained without augmentation
+    ck.validate(dict({'dueling': False, 'noisy': False, 'random_shift_pad': 0}, **state),
                 {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'dueling': bool(L.net.dueling),
-                 'noisy': bool(L.net.noisy), 'param_count': L.plan.param_count, 'opt_state_floats': L.plan.opt_state_floats}, directory)
+                 'noisy': bool(L.net.noisy), 'random_shift_pad': L.random_shift_pad, 'param_count': L.plan.param_count,
+                 'opt_state_floats': L.plan.opt_state_floats}, directory)
     blobs = {}
     for name in self._CHECKPOINT_BLOBS:
       path = os.path.join(directory, name + '.npy')
@@ -422,8 +424,10 @@ class _DeviceAgent(parts.Agent):
   def _enqueue(self):
     L = self._learner
     if getattr(self, '_jax_key', None) is not None:
+      if L.random_shift_pad:
+        L.generate_randomness(self._seed)       # the shifts and one counter step; the jax taus below replace its taus
       self._jax_learn.launch(L.taus)            # jax.random.uniform draws from the keys staged by _learn()
-    elif _draws_taus(self.KIND) or learner_lib.noisy_layers(L.net):
+    elif _draws_taus(self.KIND) or learner_lib.noisy_layers(L.net) or L.random_shift_pad:
       L.generate_randomness(self._seed, beside_sampler=True)
     L.learn(self._view, self.PRIORITIZED, self._io)
 
@@ -451,10 +455,10 @@ class Dqn(_DeviceAgent):
 
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
                batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
-               target_network_update_period, grad_error_bound, rng_key, use_cuda_graph=True):
+               target_network_update_period, grad_error_bound, rng_key, use_cuda_graph=True, random_shift_pad=0):
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph)
+                grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
 
 
 class DoubleQ(Dqn):
@@ -472,11 +476,11 @@ class Munchausen(_DeviceAgent):
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
                batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
                target_network_update_period, grad_error_bound, rng_key, use_cuda_graph=True, munchausen_alpha=0.9,
-               entropy_temperature=0.03, log_policy_clip=-1.0):
+               entropy_temperature=0.03, log_policy_clip=-1.0, random_shift_pad=0):
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph, munchausen_alpha=munchausen_alpha,
-                entropy_temperature=entropy_temperature, log_policy_clip=log_policy_clip)
+                grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad,
+                munchausen_alpha=munchausen_alpha, entropy_temperature=entropy_temperature, log_policy_clip=log_policy_clip)
 
 
 class PrioritizedDqn(_DeviceAgent):
@@ -486,10 +490,10 @@ class PrioritizedDqn(_DeviceAgent):
 
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
                batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
-               target_network_update_period, grad_error_bound, rng_key, use_cuda_graph=True):
+               target_network_update_period, grad_error_bound, rng_key, use_cuda_graph=True, random_shift_pad=0):
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph)
+                grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
 
   @property
   def importance_sampling_exponent(self) -> float:
@@ -506,11 +510,11 @@ class C51(_DeviceAgent):
 
   def __init__(self, preprocessor, sample_network_input, network, support, optimizer, transition_accumulator,
                replay, batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
-               target_network_update_period, rng_key, use_cuda_graph=True):
+               target_network_update_period, rng_key, use_cuda_graph=True, random_shift_pad=0):
     _check_support(support, network)
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                use_cuda_graph=use_cuda_graph)
+                use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
 
 
 class QrDqn(_DeviceAgent):
@@ -519,14 +523,14 @@ class QrDqn(_DeviceAgent):
 
   def __init__(self, preprocessor, sample_network_input, network, quantiles, optimizer, transition_accumulator,
                replay, batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
-               target_network_update_period, huber_param, rng_key, use_cuda_graph=True):
+               target_network_update_period, huber_param, rng_key, use_cuda_graph=True, random_shift_pad=0):
     q = np.asarray(quantiles, dtype=np.float64)
     n = network.num_quantiles
     if len(q) != n or not np.allclose(q, (np.arange(n) + 0.5) / n, rtol=0, atol=1e-6):
       raise ValueError('quantiles must be the %d midpoints (i + 0.5) / n' % n)
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                huber_param=huber_param, use_cuda_graph=use_cuda_graph)
+                huber_param=huber_param, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
 
 
 class Rainbow(_DeviceAgent):
@@ -537,11 +541,11 @@ class Rainbow(_DeviceAgent):
 
   def __init__(self, preprocessor, sample_network_input, network, support, optimizer, transition_accumulator,
                replay, batch_size, min_replay_capacity_fraction, learn_period, target_network_update_period,
-               rng_key, use_cuda_graph=True):
+               rng_key, use_cuda_graph=True, random_shift_pad=0):
     _check_support(support, network)
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 None, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                use_cuda_graph=use_cuda_graph)
+                use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
 
   @property
   def importance_sampling_exponent(self) -> float:
@@ -559,7 +563,7 @@ class Iqn(_DeviceAgent):
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
                batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
                target_network_update_period, huber_param, tau_samples_policy, tau_samples_s_tm1, tau_samples_s_t,
-               rng_key, use_cuda_graph=True, jax_prng_taus=False):
+               rng_key, use_cuda_graph=True, jax_prng_taus=False, random_shift_pad=0):
     """`jax_prng_taus=True`: `rng_key` is treated as a jax PRNG key (`jax.random.PRNGKey(seed)` = [0, seed]) and the tau
     samples of every update and every action selection follow the reference's key chain bit for bit
     (iqn/agent.py:182-190, 207, 220-222; threefry2x32 + jax.random.split/uniform, csrc/dz_jaxprng.cu).  The default keeps
@@ -569,7 +573,7 @@ class Iqn(_DeviceAgent):
       raise ValueError('tau sample counts must match the NetworkSpec')
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                huber_param=huber_param, use_cuda_graph=use_cuda_graph)
+                huber_param=huber_param, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
     if jax_prng_taus:
       key = np.asarray(rng_key, dtype=np.uint32).reshape(-1)
       if key.size != 2:
@@ -593,14 +597,15 @@ class MunchausenIqn(_DeviceAgent):
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
                batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
                target_network_update_period, huber_param, tau_samples_policy, tau_samples_s_tm1, tau_samples_s_t,
-               rng_key, use_cuda_graph=True, munchausen_alpha=0.9, entropy_temperature=0.03, log_policy_clip=-1.0):
+               rng_key, use_cuda_graph=True, munchausen_alpha=0.9, entropy_temperature=0.03, log_policy_clip=-1.0,
+               random_shift_pad=0):
     if (network.tau_samples_policy, network.tau_samples_s_tm1, network.tau_samples_s_t) != (
         tau_samples_policy, tau_samples_s_tm1, tau_samples_s_t):
       raise ValueError('tau sample counts must match the NetworkSpec')
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                huber_param=huber_param, use_cuda_graph=use_cuda_graph, munchausen_alpha=munchausen_alpha,
-                entropy_temperature=entropy_temperature, log_policy_clip=log_policy_clip)
+                huber_param=huber_param, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad,
+                munchausen_alpha=munchausen_alpha, entropy_temperature=entropy_temperature, log_policy_clip=log_policy_clip)
 
 
 class Fqf(_DeviceAgent):
@@ -615,13 +620,14 @@ class Fqf(_DeviceAgent):
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
                batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
                target_network_update_period, huber_param, rng_key, use_cuda_graph=True, num_fractions=32,
-               fraction_learning_rate=2.5e-9, fraction_opt_eps=1e-5, fraction_rms_decay=0.95):
+               fraction_learning_rate=2.5e-9, fraction_opt_eps=1e-5, fraction_rms_decay=0.95, random_shift_pad=0):
     if network.num_fractions != num_fractions:
       raise ValueError('num_fractions must match the NetworkSpec')
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                huber_param=huber_param, use_cuda_graph=use_cuda_graph, fraction_learning_rate=fraction_learning_rate,
-                fraction_opt_eps=fraction_opt_eps, fraction_rms_decay=fraction_rms_decay)
+                huber_param=huber_param, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad,
+                fraction_learning_rate=fraction_learning_rate, fraction_opt_eps=fraction_opt_eps,
+                fraction_rms_decay=fraction_rms_decay)
 
 
 def _check_support(support, network):

@@ -326,6 +326,11 @@ __host__ __device__ inline float dueling_transpose(const float* dq, int A, float
   return s;
 }
 
+// ---- random-shift augmentation (DESIGN.md §18): the largest pad, and the shared-memory stage of random_shift_kernel,
+// which holds the source rows of one band of output rows (84x84x4 and 84x92x4 observations: one band)
+constexpr int kShiftMaxPad = 16;
+constexpr int kShiftStageBytes = 32768;
+
 static int validate(const dz_learner_config& c) {
   if (c.kind < 0 || c.kind > DZ_FQF) return fail(DZ_EINVAL, "unknown agent kind");
   if (c.dueling != 0 && c.dueling != 1) return fail(DZ_EINVAL, "dueling must be 0 or 1");
@@ -349,6 +354,10 @@ static int validate(const dz_learner_config& c) {
   if (c.obs_c != 4) return fail(DZ_EINVAL, "obs_c must be 4 (stacked frames; conv1 reads uchar4 pixels)");
   if (c.obs_w % 4) return fail(DZ_EINVAL, "obs_w must be a multiple of 4");
   if (c.obs_h < 36 || c.obs_w < 36) return fail(DZ_EINVAL, "observation too small for the Nature-CNN torso");
+  if (c.random_shift_pad < 0 || c.random_shift_pad > kShiftMaxPad) return fail(DZ_EINVAL, "random_shift_pad must be in [0,16]");
+  if (c.random_shift_pad >= std::min(c.obs_h, c.obs_w)) return fail(DZ_EINVAL, "random_shift_pad must be less than min(obs_h, obs_w)");
+  if (c.random_shift_pad && (int64_t)c.obs_w * c.obs_c > kShiftStageBytes)
+    return fail(DZ_EINVAL, "random_shift_pad: an observation row (obs_w * obs_c bytes) must be at most 32768 bytes");
   if (c.num_actions <= 0 || c.num_actions > 64) return fail(DZ_EINVAL, "num_actions must be in [1,64]");
   if ((c.kind == DZ_C51 || c.kind == DZ_RAINBOW) && (c.num_atoms < 2 || c.num_atoms > 128)) return fail(DZ_EINVAL, "num_atoms must be in [2,128]");
   if (c.kind == DZ_QRDQN && (c.num_quantiles < 1 || c.num_quantiles > 256)) return fail(DZ_EINVAL, "num_quantiles must be in [1,256]");
@@ -751,6 +760,77 @@ __global__ void randomness_kernel(float* __restrict__ out, long long n, uint64_t
 
 __global__ void bump_counter_kernel(int64_t* counters, int which) {
   dz::pdl_enter(); counters[which] += 1; }
+
+// ---- random-shift augmentation (DESIGN.md §18) ---------------------------------------------------
+
+// The shifts of one update: example b takes the Philox block at counter (b, 0, ctr low, ctr high ^ (3 << 24)) and its
+// words w give (dy0, dx0, dy1, dx1) = floor(w (2p + 1) / 2^32).  Reads the counter, does not advance it.
+__global__ void shift_draw_kernel(int32_t* __restrict__ out, int B, int pad, uint64_t seed, const int64_t* counters) {
+  dz::pdl_enter();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const uint64_t ctr = (uint64_t)counters[1];
+  uint32_t r[4];
+  philox4x32_10((uint32_t)b, 0u, (uint32_t)ctr, (uint32_t)(ctr >> 32) ^ (3u << 24), (uint32_t)seed, (uint32_t)(seed >> 32), r);
+  const uint32_t span = 2u * (uint32_t)pad + 1u;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) out[4 * b + j] = (int32_t)__umulhi(r[j], span);
+}
+
+struct ShiftArgs {
+  const uint8_t* const* src[2];   // [B] row tables of s_tm1 and s_t, [H][W][C] each
+  const int32_t* shifts;          // [B][4]: (dy0, dx0, dy1, dx1)
+  uint8_t* out;                   // [B][2][stride]
+  long long stride;               // a multiple of 16, >= H * W * C
+  const uint8_t** rows[2];        // when set, rows[i][b] <- the shifted observation (the tables the torso then reads)
+  int H, W, C, pad;
+};
+
+constexpr int kShiftThreads = 256;
+
+// One CTA per (observation i = s_tm1 | s_t, example b): out[y][x][c] = in[clamp(y + dy - p)][clamp(x + dx - p)][c].  The
+// source rows of a band of output rows are contiguous: they are staged through shared memory with 16-byte loads, and
+// each output 16-byte word is gathered from the stage in 32-bit pixel words (C % 4 == 0) and stored whole.
+__global__ void __launch_bounds__(kShiftThreads) random_shift_kernel(const __grid_constant__ ShiftArgs a) {
+  __shared__ uint4 stage[kShiftStageBytes / 16];
+  dz::pdl_enter();
+  const int i = blockIdx.x, b = blockIdx.y, p = a.pad;
+  const int dy = min(max(a.shifts[4 * b + 2 * i], 0), 2 * p) - p;
+  const int dx = min(max(a.shifts[4 * b + 2 * i + 1], 0), 2 * p) - p;
+  const int rw = a.W * a.C / 16;   // 16-byte words per row
+  const int cw = a.C / 4;          // 32-bit words per pixel
+  const uint4* src = reinterpret_cast<const uint4*>(a.src[i][b]);
+  uint4* dst = reinterpret_cast<uint4*>(a.out + ((long long)b * 2 + i) * a.stride);
+  if (a.rows[i] != nullptr && threadIdx.x == 0) a.rows[i][b] = reinterpret_cast<const uint8_t*>(dst);
+  const uint32_t* st = reinterpret_cast<const uint32_t*>(stage);
+  const int band = kShiftStageBytes / 16 / rw;
+  for (int y0 = 0; y0 < a.H; y0 += band) {
+    const int y1 = min(a.H, y0 + band);
+    // clamp is monotone and 1-Lipschitz: the band's source rows s0..s1 are at most y1 - y0
+    const int s0 = min(max(y0 + dy, 0), a.H - 1), s1 = min(max(y1 - 1 + dy, 0), a.H - 1);
+    const int n = (s1 - s0 + 1) * rw;
+    const uint4* from = src + (long long)s0 * rw;
+#pragma unroll 4
+    for (int k = threadIdx.x; k < n; k += kShiftThreads) stage[k] = __ldg(from + k);
+    __syncthreads();
+    const int m = (y1 - y0) * rw;
+    for (int k = threadIdx.x; k < m; k += kShiftThreads) {
+      const int yy = k / rw, kw = k - yy * rw;
+      const uint32_t* row = st + (min(max(y0 + yy + dy, 0), a.H - 1) - s0) * rw * 4;
+      uint32_t v[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int wd = 4 * kw + j;
+        const int px = cw == 1 ? wd : wd / cw;
+        v[j] = row[min(max(px + dx, 0), a.W - 1) * cw + (wd - px * cw)];
+      }
+      dst[(long long)(y0 + yy) * rw + kw] = make_uint4(v[0], v[1], v[2], v[3]);
+    }
+    __syncthreads();
+  }
+  const long long obs16 = (long long)a.H * rw, tail16 = a.stride / 16 - obs16;   // the row's stride padding is zero
+  for (long long k = threadIdx.x; k < tail16; k += kShiftThreads) dst[obs16 + k] = make_uint4(0u, 0u, 0u, 0u);
+}
 
 // ---- losses ------------------------------------------------------------------------------------
 
@@ -1862,6 +1942,10 @@ struct dz_learner {
   const uint8_t** rows_sample[2];           // row tables filled by the fused sampler
   uint8_t* recon = nullptr;                 // frame-deduplicated replay: [B][2][obs_stride] stacks the sampled rows
   int64_t recon_bytes = 0;                  //   are rebuilt into (allocated by the first, eager, dz_learner_learn)
+  // random_shift_pad > 0 (DESIGN.md §18): the step's shifted observations [B][2][obs_bytes] and the row tables of
+  // s_tm1 / s_t into them, which the torso reads in place of the sampler's or the caller's
+  uint8_t* shift_obs;
+  const uint8_t** rows_shift[2];
   const uint8_t** rows_act;                 // [batch] observation row table of the learner's acting
   int32_t* s_a; float *s_r, *s_d, *s_w;     // sampler-produced batch scalars
   float* q_scratch;
@@ -2027,6 +2111,11 @@ int64_t carve(dz_learner* l, char* base) {
     l->um_ws = w.take<char>(bytes);
     if (!base) l->um_ws = reinterpret_cast<char*>(1);   // size query: "enabled" marker only
   }
+  // last, so that with the pad at 0 the workspace and every offset in it are what they are without augmentation
+  const bool shift = c.random_shift_pad > 0;
+  l->shift_obs = shift ? w.take<uint8_t>((int64_t)B * 2 * d.H * d.W * d.C) : nullptr;   // H*W*C: a multiple of 16
+  l->rows_shift[0] = shift ? w.take<const uint8_t*>(B) : nullptr;
+  l->rows_shift[1] = shift ? w.take<const uint8_t*>(B) : nullptr;
   return w.used;
 }
 
@@ -3190,6 +3279,24 @@ int launch_acting_draw(float* d_out, long long n, bool taus, uint64_t seed, int6
   return DZ_OK;
 }
 
+// random_shift_kernel over B examples: d_out [B][2][stride]; rows_tm1 / rows_t (or NULL) are pointed at the results.
+int launch_random_shift(const uint8_t* const* src_tm1, const uint8_t* const* src_t, const int32_t* shifts, int B, int H, int W,
+                        int C, int pad, uint8_t* out, long long stride, const uint8_t** rows_tm1, const uint8_t** rows_t,
+                        void* stream) {
+  const ShiftArgs a{{src_tm1, src_t}, shifts, out, stride, {rows_tm1, rows_t}, H, W, C, pad};
+  DZ_LAUNCH(random_shift_kernel, dim3(2, (unsigned)B), kShiftThreads, 0, stream, a);
+  return DZ_OK;
+}
+
+// The step's shifted observations (DESIGN.md §18): the batch's row tables, whatever the sampler or the caller pointed
+// them at (replay rows, the frame-deduplicated reconstruction, dense arrays), into l->shift_obs and l->rows_shift.
+int launch_learner_shift(dz_learner* l, const dz_batch* batch, void* stream) {
+  const Dims& d = l->d;
+  const long long obs = (long long)d.H * d.W * d.C;
+  return launch_random_shift(batch->d_s_tm1_rows, batch->d_s_t_rows, batch->d_shifts, l->B, d.H, d.W, d.C,
+                             l->cfg.random_shift_pad, l->shift_obs, obs, l->rows_shift[0], l->rows_shift[1], stream);
+}
+
 struct WriteBack { const dz_replay_view* view; const int64_t* indices; const float* priorities; double alpha; };
 
 int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* out, int apply_update, float* max_seen,
@@ -3202,17 +3309,22 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   if (noisy_net(c) && !batch->d_noise) return fail(DZ_EINVAL, "a noisy network's update needs d_noise");
   if (draws_taus(c.kind) && !batch->d_taus) return fail(DZ_EINVAL, "iqn update needs d_taus");
   if (!out || !out->d_loss || !out->d_per_example) return fail(DZ_EINVAL, "update outputs d_loss and d_per_example are required");
+  const bool shift = c.random_shift_pad > 0;
+  if (shift && !batch->d_shifts) return fail(DZ_EINVAL, "an update with random_shift_pad > 0 needs d_shifts");
   if (!(weights_packed && l->um != nullptr)) DZ_TRY(l->side.join(stream));   // pending side-stream work (asynchronous randomness)
 
-  // ---- forward: every network.apply of loss_fn in grouped launches
+  // ---- forward: every network.apply of loss_fn in grouped launches.  With augmentation every pass over s_tm1 reads
+  // the one shifted s_tm1 and every pass over s_t the one shifted s_t (DESIGN.md §18).
+  const uint8_t* const* s_tm1 = shift ? l->rows_shift[0] : batch->d_s_tm1_rows;
+  const uint8_t* const* s_t = shift ? l->rows_shift[1] : batch->d_s_t_rows;
   TorsoJob jobs[3];
   int nj = 0;
   const bool target_stm1 = is_munchausen(c.kind);   // the target network also applies to s_tm1 (the log-policy bonus)
   const bool iqn = uses_iqn_net(c.kind);
-  jobs[nj++] = TorsoJob{on, batch->d_s_tm1_rows, 0};
-  if (online_st) jobs[nj++] = TorsoJob{on, batch->d_s_t_rows, 1};
-  if (target_stm1) jobs[nj++] = TorsoJob{tg, batch->d_s_tm1_rows, 1};
-  jobs[nj++] = TorsoJob{tg, batch->d_s_t_rows, 2};
+  jobs[nj++] = TorsoJob{on, s_tm1, 0};
+  if (online_st) jobs[nj++] = TorsoJob{on, s_t, 1};
+  if (target_stm1) jobs[nj++] = TorsoJob{tg, s_tm1, 1};
+  jobs[nj++] = TorsoJob{tg, s_t, 2};
   const bool um = l->um != nullptr;
   if (um) {
     if (nj != l->um_npass) return fail(DZ_EINVAL, "tensor-core path: pass count mismatch");
@@ -3220,10 +3332,12 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     for (int i = 0; i < nj; ++i) rows[i] = jobs[i].rows;
     if (weights_packed) DZ_TRY(l->side.join(stream));   // packed on the side stream, concurrently with the sampler
     else DZ_TRY(um_pack_weights(l->um, stream));
+    if (shift) DZ_TRY(launch_learner_shift(l, batch, stream));   // after the join: the shifts may be drawn beside the sampler
     DZ_TRY(um_forward_torso(l->um, rows, stream));
     DZ_TRY(l->side.join(stream));
     if (!iqn) DZ_TRY(um_forward_fc(l->um, batch->d_noise, stream));
   } else {
+    if (shift) DZ_TRY(launch_learner_shift(l, batch, stream));
     DZ_TRY(forward_torso(l, learner_bufs(l), jobs, nj, B, stream));
   }
 
@@ -3287,7 +3401,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   if (split_norm_active(l)) {   // every gradient behind the conv tensors is final once the side stream's FC / head wgrads are done
     DZ_TRY(norm_fc_range(l, apply_update != 0, l->side.tail(stream)));
   }
-  DZ_TRY(backward_torso(l, batch->d_s_tm1_rows, stream));
+  DZ_TRY(backward_torso(l, s_tm1, stream));
 
   // ---- clip_by_global_norm + adam / rmsprop + apply_updates
   DZ_TRY(l->side2.join(stream));
@@ -3429,6 +3543,7 @@ int dz_learner_learn(dz_learner* l, const dz_replay_view* replay, int32_t priori
   batch.d_a_tm1 = l->s_a; batch.d_r_t = l->s_r; batch.d_discount_t = l->s_d;
   batch.d_weights = prioritized ? l->s_w : nullptr;
   batch.d_taus = io->d_taus; batch.d_noise = io->d_noise;
+  batch.d_shifts = l->cfg.random_shift_pad ? io->d_shifts : nullptr;   // the field is not read with the pad at 0
   WriteBack wb{replay, io->sample_out.d_indices, io->update_out.d_priorities, io->priority_exponent};
   if (prioritized && !io->update_out.d_priorities) return fail(DZ_EINVAL, "prioritized learn needs update_out.d_priorities");
   DZ_TRY(update_impl(l, &batch, &io->update_out, 1, io->d_max_seen_priority, prioritized ? &wb : nullptr, stream, pack_aside));
@@ -3441,6 +3556,16 @@ int dz_learner_learn(dz_learner* l, const dz_replay_view* replay, int32_t priori
 // other consumer of the buffers must synchronise the device first.
 int dz_learner_generate_randomness_async(dz_learner* l, uint64_t seed, float* d_taus, float* d_noise, void* stream) {
   return dz_learner_generate_randomness(l, seed, d_taus, d_noise, l->side.fork(stream, stream));
+}
+
+// The shifts of the next update at the current counter; the dz_learner_generate_randomness enqueued after it makes the
+// step's one counter step.
+int dz_learner_generate_shifts(dz_learner* l, uint64_t seed, int32_t* d_shifts, void* stream) {
+  if (l->cfg.random_shift_pad == 0) return fail(DZ_EINVAL, "generate_shifts: the learner's random_shift_pad is 0");
+  if (!d_shifts) return fail(DZ_EINVAL, "generate_shifts: null buffer");
+  DZ_LAUNCH(shift_draw_kernel, (unsigned)ceil_div(l->B, 128), 128, 0, stream, d_shifts, l->B, l->cfg.random_shift_pad, seed,
+            l->buf.d_counters);
+  return DZ_OK;
 }
 
 int dz_learner_generate_randomness(dz_learner* l, uint64_t seed, float* d_taus, float* d_noise, void* stream) {
@@ -3784,6 +3909,19 @@ int dz_test_learner_mma_path(dz_learner* l, const char* tag, int32_t* path) {
 int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream) {
   DZ_CUDA_OK(cudaMemcpyAsync(d_dst, d_src, (size_t)bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return DZ_OK;
+}
+
+int dz_test_random_shift(const uint8_t* const* d_rows_tm1, const uint8_t* const* d_rows_t, const int32_t* d_shifts,
+                         int32_t B, int32_t H, int32_t W, int32_t C, int32_t pad, uint8_t* d_out, int64_t out_stride,
+                         void* stream) {
+  if (!d_rows_tm1 || !d_rows_t || !d_shifts || !d_out) return fail(DZ_EINVAL, "random_shift: null buffer");
+  if (B < 1 || B > 65535 || H < 1 || W < 1 || C < 4 || C % 4) return fail(DZ_EINVAL, "random_shift: bad B / H / W / C");
+  if (pad < 0 || pad > kShiftMaxPad || pad >= std::min(H, W)) return fail(DZ_EINVAL, "random_shift: pad must be in [0,16] and < min(H, W)");
+  const int64_t row = (int64_t)W * C;
+  if (row % 16 || row > kShiftStageBytes) return fail(DZ_EINVAL, "random_shift: W * C must be a multiple of 16 and at most 32768");
+  if (out_stride < row * H || out_stride % 16 || (reinterpret_cast<uintptr_t>(d_out) & 15))
+    return fail(DZ_EINVAL, "random_shift: out_stride must be >= H*W*C and a multiple of 16, d_out 16-byte aligned");
+  return launch_random_shift(d_rows_tm1, d_rows_t, d_shifts, B, H, W, C, pad, d_out, out_stride, nullptr, nullptr, stream);
 }
 
 // Host twin of loss_munchausen_kernel's per-example arithmetic: the warp's xor-butterfly reductions over an array of 32

@@ -133,6 +133,22 @@ def check_network(net: NetworkSpec) -> None:
                                                                ' (its network is noisy already)' if net.kind == 'rainbow' else ''))
 
 
+MAX_RANDOM_SHIFT_PAD = 16
+
+
+def check_random_shift_pad(pad, obs_shape) -> int:
+  """The random-shift pad (DESIGN.md §18) as an int; ValueError unless it is an integer in [0, 16] and less than
+  min(H, W)."""
+  if isinstance(pad, (bool, np.bool_)) or not isinstance(pad, (int, np.integer)):
+    raise ValueError('random_shift_pad must be an integer, got %r' % (pad,))
+  pad = int(pad)
+  if not 0 <= pad <= MAX_RANDOM_SHIFT_PAD:
+    raise ValueError('random_shift_pad must be in [0, %d], got %d' % (MAX_RANDOM_SHIFT_PAD, pad))
+  if pad >= min(obs_shape[0], obs_shape[1]):
+    raise ValueError('random_shift_pad must be less than min(H, W) = %d, got %d' % (min(obs_shape[0], obs_shape[1]), pad))
+  return pad
+
+
 def noise_vector_sizes(net: NetworkSpec):
   """(name, length) of the factorised-noise vectors of ONE `network.apply`: rainbow's 8 in `hk.next_rng_key()` order
   (networks.py:169-170, :235-248); a noisy network's (DESIGN.md §17) fc1 in / out and head in / out, or dueling,
@@ -201,13 +217,17 @@ class Learner:
   def __init__(self, net: NetworkSpec, batch_size: int = 32, optimizer: Optional[OptimizerSpec] = None,
                grad_error_bound: float = 1.0 / 32, huber_param: float = 1.0, munchausen_alpha: float = 0.9,
                entropy_temperature: float = 0.03, log_policy_clip: float = -1.0, fraction_learning_rate: float = 2.5e-9,
-               fraction_opt_eps: float = 1e-5, fraction_rms_decay: float = 0.95, device=None):
+               fraction_opt_eps: float = 1e-5, fraction_rms_decay: float = 0.95, device=None, random_shift_pad: int = 0):
     """`munchausen_alpha`, `entropy_temperature` (tau) and `log_policy_clip` (l0) are Munchausen DQN's and
     Munchausen-IQN's (DESIGN.md §13, §14, defaults the paper's Atari values); the library rejects tau <= 0, alpha < 0,
     l0 > 0 and non-finite values for those kinds, and the other kinds ignore them.  `fraction_learning_rate`,
     `fraction_opt_eps` and `fraction_rms_decay` are fqf's centred RMSProp over its fraction layer (DESIGN.md §15); the
-    library rejects a negative or non-finite rate, eps <= 0 and a decay outside [0, 1) for fqf."""
+    library rejects a negative or non-finite rate, eps <= 0 and a decay outside [0, 1) for fqf.  `random_shift_pad` p > 0
+    turns on random-shift augmentation of the update (DrQ; DESIGN.md §18): every update reads s_tm1 and s_t shifted by
+    the [B, 4] int32 `shifts`, which `generate_randomness` draws; acting never sees a shift.  ValueError unless p is an
+    integer in [0, 16] and less than min(H, W)."""
     check_network(net)
+    random_shift_pad = check_random_shift_pad(random_shift_pad, net.obs_shape)
     if not torch.cuda.is_available():
       raise RuntimeError('dqn_zoo_b200.learner needs a CUDA device (there is no CPU fallback)')
     self.net = net
@@ -231,6 +251,8 @@ class Learner:
                                                                                 fraction_rms_decay)
     cfg.dueling = 1 if net.dueling else 0
     cfg.noisy = 1 if net.noisy else 0
+    cfg.random_shift_pad = random_shift_pad
+    self.random_shift_pad = random_shift_pad
     self.cfg = cfg
     plan = _lib.LearnerPlan()
     _lib.call('dz_learner_plan_query', C.byref(cfg), C.byref(plan))
@@ -252,6 +274,8 @@ class Learner:
       _lib.call('dz_learner_noise_stride', C.byref(cfg), C.byref(stride))
       self.noise_stride = stride.value
     self._stream_noise = None      # [batch_size, noise_stride], allocated by the first generate_stream_noise
+    # random_shift_pad > 0: (dy0, dx0, dy1, dx1) of each example of the next update
+    self.shifts = torch.zeros((batch_size, 4), dtype=torch.int32, device=dev)
     self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
     self.per_example = torch.zeros(batch_size, dtype=torch.float32, device=dev)
     self.priorities = torch.zeros(batch_size, dtype=torch.float32, device=dev)
@@ -350,10 +374,12 @@ class Learner:
     stride = dense.stride(0) * dense.element_size()
     return dense.data_ptr() + torch.arange(n, dtype=torch.int64, device=self.device) * stride
 
-  def update(self, s_tm1, a_tm1, r_t, discount_t, s_t, weights=None, taus=None, noise=None, apply_update=True):
+  def update(self, s_tm1, a_tm1, r_t, discount_t, s_t, weights=None, taus=None, noise=None, apply_update=True,
+             shifts=None):
     """`jit(update)` on an explicit batch of device tensors (uint8 [B,H,W,C], int, float, float,
-    uint8).  r/discount/weights are rounded to float32 as at the jit boundary.  Returns nothing;
-    results are in `.loss`, `.per_example`, `.priorities`, `.grad_norm`, `.grads`."""
+    uint8).  r/discount/weights are rounded to float32 as at the jit boundary.  `shifts` ([B, 4] int, random_shift_pad
+    > 0) replaces `.shifts`, as `taus` / `noise` replace theirs.  Returns nothing; results are in `.loss`,
+    `.per_example`, `.priorities`, `.grad_norm`, `.grads`."""
     dev = self.device
     B = self.batch_size
     s_tm1 = torch.as_tensor(s_tm1, device=dev).contiguous().view(B, -1)
@@ -370,18 +396,28 @@ class Learner:
     if noise is not None:
       flat = torch.as_tensor(noise, device=dev).to(torch.float32).reshape(-1)
       self.noise[:flat.numel()].copy_(flat)
+    if shifts is not None:
+      if not self.random_shift_pad:
+        raise ValueError('shifts need a learner with random_shift_pad > 0')
+      self.shifts.copy_(torch.as_tensor(shifts, device=dev).to(torch.int32).reshape(B, 4))
     batch = _lib.Batch(keep[2].data_ptr(), keep[3].data_ptr(), keep[4].data_ptr(), keep[5].data_ptr(),
                        keep[6].data_ptr(), 0 if w is None else w.data_ptr(),
                        self.taus.data_ptr() if draws_taus(self.kind) else 0,
-                       self.noise.data_ptr() if noisy_layers(self.net) else 0)
+                       self.noise.data_ptr() if noisy_layers(self.net) else 0, self._shifts_ptr())
     out = _lib.UpdateOutputs(self.loss.data_ptr(), self.per_example.data_ptr(), self.priorities.data_ptr(),
                              self.grad_norm.data_ptr())
     _lib.call('dz_learner_update', self._h, C.byref(batch), C.byref(out), 1 if apply_update else 0, _cstream())
     self._keep = (keep, w)
 
+  def _shifts_ptr(self):
+    return self.shifts.data_ptr() if self.random_shift_pad else 0
+
   def generate_randomness(self, seed: int, beside_sampler: bool = False) -> None:
     """Fills `.taus` / `.noise` for the next update from the device generator (Philox).  `beside_sampler`: enqueue on
-    the learner's side stream (ordered before the next learn()/update()/q_values() only)."""
+    the learner's side stream (ordered before the next learn()/update()/q_values() only).  With random_shift_pad > 0 it
+    first fills `.shifts` on the current stream, at the same counter; the counter still advances once."""
+    if self.random_shift_pad:
+      _lib.call('dz_learner_generate_shifts', self._h, seed, self.shifts.data_ptr(), _cstream())
     _lib.call('dz_learner_generate_randomness_async' if beside_sampler else 'dz_learner_generate_randomness', self._h, seed,
               self.taus.data_ptr(), self.noise.data_ptr(), _cstream())
 
@@ -447,6 +483,7 @@ class Learner:
                                        self.grad_norm.data_ptr())
     io.d_max_seen_priority = self.max_seen_priority.data_ptr()
     io.priority_exponent = float(priority_exponent)
+    io.d_shifts = self._shifts_ptr()
     return io
 
   def learn(self, replay_view, prioritized: bool, io) -> None:

@@ -364,6 +364,14 @@ typedef struct dz_learner_config {
    * tensors.  The learner then takes noise exactly as rainbow does: noise_floats = 3 applies, dz_learner_noise_stride,
    * per-stream acting noise and the actor's draws. */
   int32_t noisy;
+  /* Random-shift image augmentation of the learner step (DrQ, Kostrikov, Yarats & Fergus, ICLR 2021; DESIGN.md §18),
+   * valid for every kind and network option.  p in [0, 16] and p < min(obs_h, obs_w) (DZ_EINVAL otherwise); 0, as a
+   * zero-filled tail leaves it: off, and the step is what it is without the field.  p > 0: each update reads s_tm1
+   * and s_t of example b shifted by (dy0, dx0) and (dy1, dx1) = d_shifts[b][0..3], each in [0, 2p]:
+   * out[y][x][c] = in[clamp(y + dy - p, 0, H - 1)][clamp(x + dx - p, 0, W - 1)][c], the observation edge-padded by
+   * p and cropped back to H x W.  Every pass over s_tm1 reads the one shifted s_tm1 and every pass over s_t the one
+   * shifted s_t; acting never sees a shift. */
+  int32_t random_shift_pad;
 } dz_learner_config;
 
 typedef struct dz_learner_plan {
@@ -410,6 +418,9 @@ typedef struct dz_batch {
                                           adv2 in/out, val1 in/out, val2 in/out), each padded to a multiple of 4 floats; or NULL.
                                           noisy networks: the same 3 applies (online(s_tm1) | the middle pass | target(s_t)),
                                           each fc1 in/out, head in/out (dueling: rainbow's 8 vectors with one atom) */
+  const int32_t* d_shifts;             /* random_shift_pad > 0: [B][4] (dy0, dx0, dy1, dx1), each in [0, 2p]
+                                          (dz_learner_generate_shifts); required then (DZ_EINVAL when NULL) and
+                                          ignored when the pad is 0 */
 } dz_batch;
 
 typedef struct dz_update_outputs {
@@ -436,6 +447,7 @@ typedef struct dz_learn_io {
   dz_update_outputs update_out;
   float* d_max_seen_priority;
   double priority_exponent;  /* alpha */
+  const int32_t* d_shifts;   /* as dz_batch.d_shifts */
 } dz_learn_io;
 int dz_learner_learn(dz_learner* l, const dz_replay_view* replay, int32_t prioritized, const dz_learn_io* io,
                      void* stream);
@@ -448,6 +460,12 @@ int dz_learner_generate_randomness(dz_learner* l, uint64_t seed, float* d_taus, 
  * dz_learner_learn / dz_learner_update / dz_learner_act_batch on `stream` (they run beside the sampler instead of in
  * front of it).  Any other reader of d_taus / d_noise must synchronise the device first. */
 int dz_learner_generate_randomness_async(dz_learner* l, uint64_t seed, float* d_taus, float* d_noise, void* stream);
+/* random_shift_pad > 0: the shifts of one update, d_shifts [batch][4] int32, from the same generator at the current
+ * counter d_counters[1] on stream id 3, WITHOUT advancing it: example b takes the Philox4x32-10 block at counter
+ * (b, 0, ctr low, ctr high ^ (3 << 24)), key = seed, and its words w give (dy0, dx0, dy1, dx1) = floor(w (2p + 1) / 2^32).
+ * Enqueue it before the dz_learner_generate_randomness (or _async) of the same step, whose counter step then covers
+ * both.  DZ_EINVAL for a learner with the pad at 0 or a NULL buffer. */
+int dz_learner_generate_shifts(dz_learner* l, uint64_t seed, int32_t* d_shifts, void* stream);
 
 /* Batched acting for E <= batch independent environment streams (parts.py:342-411 run over many actors;
  * dqn/agent.py:121-131,169-177): online forward on E observations in one enqueue, q-values [E][num_actions] and the
@@ -737,6 +755,14 @@ int dz_test_iqn_head_dgrad(dz_learner* l, int32_t M, const float* d_dout, const 
 int dz_test_iqn_hadamard_bwd(int32_t packed, int32_t B, int32_t N, int32_t D, float* d_dhi, const float* d_E, const float* d_F,
                              float* d_dfeat, float* d_img_hi, float* d_img_lo, int32_t img_rows_pad, void* stream);
 int dz_test_copy(void* d_dst, const void* d_src, int64_t bytes, void* stream);   /* device-to-device, tests only */
+/* The learner's random-shift kernel alone, tests only: observations [H][W][C] at d_rows_tm1[b] / d_rows_t[b] shifted by
+ * d_shifts[b] (dz_batch.d_shifts; components clamped to [0, 2p]) into d_out [B][2][out_stride] (s_tm1, then s_t), with
+ * the out_stride - H*W*C padding bytes of each row zeroed.  DZ_EINVAL unless pad is in [0, 16] and < min(H, W), C % 4 == 0,
+ * W * C is a multiple of 16 and at most 32768, out_stride >= H*W*C is a multiple of 16 and d_out is 16-byte aligned;
+ * the source rows must be 16-byte aligned. */
+int dz_test_random_shift(const uint8_t* const* d_rows_tm1, const uint8_t* const* d_rows_t, const int32_t* d_shifts,
+                         int32_t B, int32_t H, int32_t W, int32_t C, int32_t pad, uint8_t* d_out, int64_t out_stride,
+                         void* stream);
 /* Debug: the tensor-core launch named `tag` writes the clock stamps of its CTA 0 into d_trace (512 int64). */
 int dz_test_learner_trace(dz_learner* l, const char* tag, long long* d_trace);
 /* Tests: which MMA path the tensor-core launch `tag` (same tags, and "conv1_fwd") takes: *path = 1 warp-level mma.sync,

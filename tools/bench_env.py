@@ -138,14 +138,15 @@ def bench_driver(game='catch'):
 
 
 # -- learning ----------------------------------------------------------------------------------------------------------
-def learning_agent(seed, train_frames, kind='dqn', num_actions=6, dueling=False, noisy=False):
+def learning_agent(seed, train_frames, kind='dqn', num_actions=6, dueling=False, noisy=False, random_shift_pad=0):
   """dqn at the reference's hyper-parameters but for a faster schedule: replay of 100k transitions, learning from 10k,
   epsilon 1 -> 0.01 over the first quarter of the frames, target sync every 8000 frames.  `kind='rainbow'`: the same
   schedule with rainbow's prioritized replay (exponent 0.5, importance exponent 0.4 -> 1 over the run), 3-step returns,
   noisy greedy acting and its 51-atom support on [-10, 10].  `kind='double_q'`: dqn's schedule with the double Q-learning
   target.  `dueling`: the dueling network (DESIGN.md §16) in place of dqn's fc1 / head.  `noisy`: noisy networks
   (DESIGN.md §17) with an epsilon schedule that is zero throughout, so that the agent explores through its noise alone
-  (NoisyNet-DQN for dqn)."""
+  (NoisyNet-DQN for dqn).  `random_shift_pad`: random-shift augmentation of every learner step (DESIGN.md §18); with
+  kind='double_q' and `dueling` that is DrQ-epsilon's agent on this schedule."""
   from dqn_zoo_b200 import agent as ag
   from dqn_zoo_b200 import learner as dl
   from dqn_zoo_b200 import parts
@@ -156,7 +157,7 @@ def learning_agent(seed, train_frames, kind='dqn', num_actions=6, dueling=False,
   common = dict(preprocessor=None, sample_network_input=None, network=dl.NetworkSpec(kind, num_actions, dueling=dueling,
                                                                                           noisy=noisy),
                 optimizer=None, batch_size=32, min_replay_capacity_fraction=min_fill / capacity, learn_period=16,
-                target_network_update_period=8000, rng_key=[0, seed + 1])
+                target_network_update_period=8000, rng_key=[0, seed + 1], random_shift_pad=random_shift_pad)
   if kind == 'rainbow':
     importance = parts.LinearSchedule(begin_t=min_fill, decay_steps=max(train_frames, 1), begin_value=0.4,
                                       end_value=1.0)
@@ -202,13 +203,13 @@ def evaluate(learner, seed, num_streams=64, game='catch', num_actions=6):
 
 
 def learning_run(train_frames, seed=0, num_streams=32, eval_every=0, log=None, game='catch', num_actions=6,
-                 kind='dqn', dueling=False, noisy=False):
+                 kind='dqn', dueling=False, noisy=False, random_shift_pad=0):
   """Trains `learning_agent` (of `kind`, on the dueling network with `dueling`, with noisy layers with `noisy`) from `num_streams` streams of `game` for `train_frames` frames (training episodes are not
   truncated); evaluates every `eval_every` frames (0: at the end only).  Returns [(frames, mean eval return, eval
   episodes, train episode return)]."""
   import run_synthetic
   from dqn_zoo_b200 import agent as ag
-  agent = learning_agent(seed, train_frames, kind, num_actions, dueling, noisy)
+  agent = learning_agent(seed, train_frames, kind, num_actions, dueling, noisy, random_shift_pad)
   trainer = ag.VectorTrainer(agent, num_streams=num_streams, rng_key=[0, seed + 4])
   env = make_env(game, num_streams, seed + 5, num_actions)
   loop = run_synthetic.StreamLoop(trainer, env, train_frames, 0)
@@ -232,6 +233,8 @@ def main():
   ap.add_argument('--dueling', action='store_true', help='the learning curve on the dueling network (DESIGN.md §16)')
   ap.add_argument('--noisy', action='store_true',
                   help='the learning curve on noisy networks with a zero epsilon schedule (DESIGN.md §17)')
+  ap.add_argument('--random_shift_pad', type=int, default=0,
+                  help='the learning curve with random-shift augmentation at pad N (DESIGN.md §18)')
   ap.add_argument('--parts', default='env,train,eval,driver')
   ap.add_argument('--frames', type=int, default=65536, help='frames per timed window of env_train / env_eval')
   ap.add_argument('--learning', type=int, default=0, help='frames of the learning curve (0: none)')
@@ -256,10 +259,11 @@ def main():
   if a.learning:
     t0 = time.perf_counter()
     learning_run(a.learning, a.seed, eval_every=a.eval_every, game=a.game, kind=a.agent, dueling=a.dueling,
-                 noisy=a.noisy, log=lambda **kw: emit(metric='learning', **_tag(a.game), **({} if a.agent == 'dqn' else
+                 noisy=a.noisy, random_shift_pad=a.random_shift_pad, log=lambda **kw: emit(metric='learning', **_tag(a.game), **({} if a.agent == 'dqn' else
                                                                               {'agent': a.agent}),
                                        **({'dueling': True} if a.dueling else {}),
                                        **({'noisy': True} if a.noisy else {}),
+                                       **({'random_shift_pad': a.random_shift_pad} if a.random_shift_pad else {}),
                                        seed=a.seed, wall_s=round(time.perf_counter() - t0, 1), **kw))
   emit(metric='device_after', **bench_train.device_info())
 

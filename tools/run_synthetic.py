@@ -101,7 +101,7 @@ def build_train_agent(args, random_state, preprocessor):
                 transition_accumulator=replay_lib.NStepTransitionAccumulator(n_step), replay=replay, batch_size=32,
                 min_replay_capacity_fraction=args.min_replay_capacity_fraction, learn_period=16,
                 target_network_update_period=args.target_network_update_period,
-                rng_key=[0, int(random_state.randint(1, 2 ** 31))])
+                rng_key=[0, int(random_state.randint(1, 2 ** 31))], random_shift_pad=args.random_shift_pad)
   if kind == 'rainbow':
     return agent_lib.Rainbow(support=np.linspace(-10, 10, 51), **common), network
   if kind == 'c51':
@@ -267,6 +267,8 @@ def parse_args(argv=None):
   ap.add_argument('--noisy', action='store_true',
                   help='noisy networks (DESIGN.md §17) with a zero epsilon schedule: dqn, double_q, prioritized and '
                        'munchausen only; combines with --dueling')
+  ap.add_argument('--random_shift_pad', type=int, default=0,
+                  help='random-shift augmentation of every learner step at pad N in [0, 16] (DESIGN.md §18); 0: off')
   ap.add_argument('--num_actions', type=int, default=6)
   ap.add_argument('--replay_capacity', type=int, default=20000)
   ap.add_argument('--min_replay_capacity_fraction', type=float, default=0.05)
