@@ -346,13 +346,12 @@ class _DeviceAgent(parts.Agent):
     """Host RandomState draws in the reference's order (replay.py:551-567 / :78)."""
     rs = self._replay._random_state
     B = self._batch_size
-    size = self._replay.size
     slot = self._ring[self._ring_pos]
     ev = self._ring_events[self._ring_pos]
     if ev is not None:
       ev.synchronize()
     host = slot.numpy()
-    host[:B].view(np.int64)[:] = rs.randint(size, size=B)
+    host[:B].view(np.int64)[:] = rs.randint(self._replay.size, size=B)
     if self.PRIORITIZED:
       # Scaled by the root on the device.  KNOWN DIVERGENCE: the reference skips this draw when the root is 0
       # (replay.py:556-560); the root lives on the device here and is not read back per step, so the draw is always
@@ -360,11 +359,7 @@ class _DeviceAgent(parts.Agent):
       # cadence).  A zero root needs every stored priority to be 0, which the agents' priority rule never produces.
       host[B:2 * B] = rs.uniform(size=B)
       host[2 * B:3 * B] = rs.uniform(size=B)
-      dist = self._replay._distribution
-      host[3 * B:] = (float(size), float(self._replay.importance_sampling_exponent),
-                      float(dist._uniform_sample_probability), 1.0 if self._replay._normalize_weights else 0.0)
-    else:
-      host[3 * B:] = (float(size), 1.0, 0.0, 0.0)
+    host[3 * B:] = self._replay._sample_constants()
     return slot
 
   def _learn(self) -> None:
@@ -397,16 +392,14 @@ class _DeviceAgent(parts.Agent):
 
   def _launch(self) -> None:
     L = self._learner
-    if self.PRIORITIZED:
-      self._replay._distribution.flush()
+    self._replay._flush()
     self._view = self._replay.device_view()
     key = bytes(self._view)
     if self._graph is not None and key != self._graph_key:
       self._graph = None                     # a device array moved (growth / set_state): recapture
     self._graph_key = key
     if self._io is None:
-      alpha = self._replay._distribution._priority_exponent if self.PRIORITIZED else 1.0
-      self._io = L.make_learn_io(self._stage_dev, self.PRIORITIZED, alpha)
+      self._io = L.make_learn_io(self._stage_dev, self.PRIORITIZED, self._replay._alpha())
     if self._use_graph:
       if self._graph is None:
         self._enqueue()                      # first step runs eagerly (also the warm-up for capture)
@@ -433,10 +426,10 @@ class _DeviceAgent(parts.Agent):
 
   def check_device_flags(self):
     """Raises if a kernel set a sticky error flag (bad priority, root == 0 in the fused path...)."""
-    flags = self._replay._distribution._sum_tree._flags if self.PRIORITIZED else self._replay._store.flags
+    flags = self._replay._flags()
     f = int(flags.item())
     if f & _lib.DZ_FLAG_FRAME_POOL_FULL:       # sticky: the frame pool stored zeros for planes it had no room for
-      replay_lib._raise_if_pool_full(self._replay._store, flags)
+      self._replay._raise_if_pool_full()
     if f:
       flags.zero_()
       if f & (_lib.DZ_FLAG_BAD_VALUE | _lib.DZ_FLAG_BAD_INDEX):
@@ -1059,7 +1052,7 @@ class VectorTrainer:
         'has_action': self._has_action.copy(),
         'learn_steps': self._learn_steps,
         # the replay draws its samples from a RandomState the agent's state leaves to the run (as the reference does)
-        'replay_rng': self._agent._replay._random_state.get_state(),
+        'replay_rng': self._agent._replay._rng_state(),
         'actor_rng': self._actor._rng.get_state(),
         'actor_t': self._actor._t,
         'preprocessor': self._pre.get_state(),
@@ -1073,7 +1066,7 @@ class VectorTrainer:
     self._actions = np.array(state['actions'], np.int32)
     self._has_action = np.array(state['has_action'], bool)
     self._learn_steps = int(state['learn_steps'])
-    self._agent._replay._random_state.set_state(state['replay_rng'])
+    self._agent._replay._set_rng_state(state['replay_rng'])
     self._actor._rng.set_state(state['actor_rng'])
     self._actor._t = int(state['actor_t'])
     self._pre.set_state(state['preprocessor'])

@@ -293,13 +293,41 @@ def _apply_index_record(view, patches, tree_index=-1, leaf_value=0.0, evict_inde
   _lib.call('dz_replay_add', C.byref(view), C.byref(rec), addr(h_s_tm1), addr(h_s_t), _stream())
 
 
+class _MirroredIndex:
+  """The device mirrors of a distribution's host lists, kept equal to them through (target, position, value) patches.
+  A distribution says how many pending patches are cheaper to `_upload` as whole lists (`_BULK`), which host lists and
+  device mirrors a checkpoint holds (`_HOST_LISTS`, `_device_mirrors`, `_manifest`), and how a replay's add, reset and
+  synthetic fill change its lists (`_insert`, `_reset`, `_fill`)."""
+
+  _scratch = None
+
+  def flush(self):
+    """Pushes pending patches to the device mirrors."""
+    patches = self.take_patches()
+    if not patches:
+      return
+    if len(patches) > self._BULK:
+      self._upload()
+      return
+    v = self.device_view()
+    # dz_replay_add also writes the row scalars; give it a scratch row.
+    if self._scratch is None:
+      self._scratch = torch.zeros(8, dtype=torch.float64, device=_device())
+    v.d_action, v.d_reward, v.d_discount, v.d_obs = (_ptr(self._scratch),) * 4
+    for k in range(0, len(patches), 4):
+      _apply_index_record(v, patches[k:k + 4])
+
+
 # ------------------------------------------------------------------------------------------------
 # R6: UniformDistribution
 # ------------------------------------------------------------------------------------------------
 
 
-class UniformDistribution:
+class UniformDistribution(_MirroredIndex):
   """`replay.py:44-117`.  Host swap-remove list + device mirror for in-kernel lookups."""
+
+  _BULK = 16
+  _HOST_LISTS = {'ids': list, 'id_to_index': dict}
 
   def __init__(self, random_state: np.random.RandomState):
     self._random_state = random_state
@@ -336,26 +364,35 @@ class UniformDistribution:
     self._mirror.ensure(len(self._ids))
     return p
 
-  def flush(self, view=None):
-    """Pushes pending patches to the device mirror."""
-    patches = self.take_patches()
-    if not patches:
-      return
-    if len(patches) > 16:
-      self._mirror.upload(self._ids)
-      return
-    v = view if view is not None else self.device_view()
-    for k in range(0, len(patches), 4):
-      _apply_index_record(v, patches[k:k + 4])
+  def _upload(self):
+    self._mirror.upload(self._ids)
+
+  def _insert(self, item_id, evicted_id=None):
+    """One replay add: removes `evicted_id` (if any), adds `item_id`.  No tree: (evict_index, tree_index) = (-1, -1)."""
+    if evicted_id is not None:
+      self.remove([evicted_id])
+    self.add([item_id])
+    return -1, -1
+
+  def _reset(self, capacity):
+    self._ids, self._id_to_index, self._pending = [], {}, []
+
+  def _fill(self, capacity, priority):
+    self._ids = list(range(capacity))
+    self._id_to_index = {i: i for i in range(capacity)}
+    self._pending = []
+    self._mirror.upload(self._ids)
+
+  def _device_mirrors(self):
+    return {'ids_mirror': self._mirror.t}
+
+  def _manifest(self):
+    return {}
 
   def device_view(self):
     v = _lib.ReplayView()
     v.capacity = 1
     v.d_ids = _ptr(self._mirror.t)
-    # dz_replay_add also writes the row scalars; give it a scratch row.
-    if not hasattr(self, '_scratch'):
-      self._scratch = torch.zeros(8, dtype=torch.float64, device=self._mirror.t.device)
-    v.d_action, v.d_reward, v.d_discount, v.d_obs = (_ptr(self._scratch),) * 4
     return v
 
   def sample(self, size: int) -> np.ndarray:
@@ -413,8 +450,12 @@ class UniformDistribution:
 # ------------------------------------------------------------------------------------------------
 
 
-class PrioritizedDistribution:
+class PrioritizedDistribution(_MirroredIndex):
   """`replay.py:429-651`: host id/index bookkeeping, device sum tree and sampling."""
+
+  _BULK = 32
+  _HOST_LISTS = {'id_to_index': dict, 'index_to_id': dict, 'inactive_indices': list, 'active_indices': list,
+                 'active_indices_location': dict}
 
   def __init__(self, priority_exponent: float, uniform_sample_probability: float,
                random_state: np.random.RandomState, min_capacity: int = 0, max_capacity: Optional[int] = None):
@@ -498,6 +539,49 @@ class PrioritizedDistribution:
     p, self._pending = self._pending, []
     return p
 
+  def _upload(self):
+    self._live_dev.upload(self._active_indices)
+    dense = np.zeros(max(self._sum_tree.size, 1), dtype=np.int64)
+    if self._index_to_id:
+      k = np.fromiter(self._index_to_id.keys(), dtype=np.int64, count=len(self._index_to_id))
+      dense[k] = np.fromiter(self._index_to_id.values(), dtype=np.int64, count=len(self._index_to_id))
+    self._id_at_dev.upload(dense)
+
+  def _insert(self, item_id, evicted_id=None):
+    """One replay add: removes `evicted_id` (if any), adds `item_id`; returns their (evict_index, tree_index), -1 for
+    no eviction."""
+    evict_index = -1
+    if evicted_id is not None:
+      (evict_index,) = self._host_remove([evicted_id])
+    (tree_index,) = self._host_add([item_id])
+    return evict_index, tree_index
+
+  def _reset(self, capacity):
+    self._id_to_index, self._index_to_id, self._pending = {}, {}, []
+    self._inactive_indices = list(range(capacity))
+    self._active_indices, self._active_indices_location = [], {}
+    self._sum_tree._nodes.zero_()
+    self._sum_tree._size = capacity
+
+  def _fill(self, capacity, priority):
+    idx = np.arange(capacity - 1, -1, -1, dtype=np.int64)          # id i -> index C-1-i
+    self._id_to_index = dict(zip(range(capacity), idx.tolist()))
+    self._index_to_id = dict(zip(idx.tolist(), range(capacity)))
+    self._inactive_indices = []
+    self._active_indices = idx.tolist()
+    self._active_indices_location = dict(zip(idx.tolist(), range(capacity)))
+    self._pending = []
+    self._live_dev.upload(idx)
+    self._id_at_dev.upload(idx)                                     # id_at[index] = C-1-index
+    leaf = float(_power([priority], self._priority_exponent)[0])
+    self._sum_tree.set_all(np.full(capacity, leaf, dtype=np.float64))
+
+  def _device_mirrors(self):
+    return {'sum_tree': self._sum_tree._nodes, 'live_mirror': self._live_dev.t, 'id_at_mirror': self._id_at_dev.t}
+
+  def _manifest(self):
+    return {'tree_size': self._sum_tree.size, 'tree_first_leaf': self._sum_tree.capacity}
+
   def device_view(self):
     v = _lib.ReplayView()
     v.capacity = 1
@@ -506,26 +590,7 @@ class PrioritizedDistribution:
     v.d_live = _ptr(self._live_dev.t)
     v.d_id_at = _ptr(self._id_at_dev.t)
     v.d_flags = _ptr(self._sum_tree._flags)
-    if not hasattr(self, '_scratch'):
-      self._scratch = torch.zeros(8, dtype=torch.float64, device=self._live_dev.t.device)
-    v.d_action, v.d_reward, v.d_discount, v.d_obs = (_ptr(self._scratch),) * 4
     return v
-
-  def flush(self):
-    patches = self.take_patches()
-    if not patches:
-      return
-    if len(patches) > 32:
-      self._live_dev.upload(self._active_indices)
-      dense = np.zeros(max(self._sum_tree.size, 1), dtype=np.int64)
-      if self._index_to_id:
-        k = np.fromiter(self._index_to_id.keys(), dtype=np.int64, count=len(self._index_to_id))
-        dense[k] = np.fromiter(self._index_to_id.values(), dtype=np.int64, count=len(self._index_to_id))
-      self._id_at_dev.upload(dense)
-      return
-    v = self.device_view()
-    for k in range(0, len(patches), 4):
-      _apply_index_record(v, patches[k:k + 4])
 
   # -- reference surface ---------------------------------------------------------------------------
   def add_priorities(self, ids: Sequence[int], priorities: Sequence[float]) -> None:
@@ -867,12 +932,6 @@ class _FramePoolStore(_TransitionStore):
     return True, ''
 
 
-def _raise_if_pool_full(store, flags):
-  """DZ_FLAG_FRAME_POOL_FULL is sticky: the stored bytes are wrong from that add on, so every sync point raises."""
-  if isinstance(store, _FramePoolStore) and int(flags.item()) & _lib.DZ_FLAG_FRAME_POOL_FULL:
-    raise RuntimeError(_POOL_FULL % store.frame_capacity)
-
-
 def _make_store(capacity, frame_dedup, frame_capacity):
   if frame_dedup:
     return _FramePoolStore(capacity, frame_capacity)
@@ -979,11 +1038,13 @@ def _batch_items(items, codec, store):
   return count, s_tm1, s_t, a, r, d
 
 
-def _add_batch(rep, items, book, leaves=None, d_priority=None, alpha=1.0):
+def _add_batch(rep, items, leaves=None, d_priority=None, alpha=1.0):
   """Shared body of `add_batch` on a validated batch (`_batch_items`): chunks of at most min(capacity, adds per call)
-  transitions, so no call evicts a row it wrote itself.  `book()` runs one add's host bookkeeping (the same calls, in
-  the same order, as `add`) and returns (release_row, evict_index, tree_index, patches)."""
+  transitions, so no call evicts a row it wrote itself, each add's host bookkeeping done by `rep._book()` as `add`
+  does it."""
   count, (o_tm1, p_tm1), (o_t, p_t), a, r, d = items
+  if count == 0:
+    return
   store = rep._store
   v = rep.device_view()
   recs, ws, most = store.add_batch_buffers(v)
@@ -995,7 +1056,7 @@ def _add_batch(rep, items, book, leaves=None, d_priority=None, alpha=1.0):
     first_slot = rep._t % rep._capacity
     patches = []
     for j in range(k):
-      release, evict, tree, p = book()
+      release, evict, tree, p = rep._book()
       h['release'][j], h['evict_index'][j], h['tree_index'][j] = release, evict, tree
       patches.extend(p)
     n = len(patches)
@@ -1033,11 +1094,185 @@ def _check_codec(encoder, decoder):
 
 
 # ------------------------------------------------------------------------------------------------
+# The body of both replays
+# ------------------------------------------------------------------------------------------------
+
+
+class _Replay:
+  """What `TransitionReplay` and `PrioritizedTransitionReplay` share: the codec, the transition store, the ids stored
+  oldest first, the add bookkeeping, state, checkpoints and checks.  A subclass builds its index distribution and
+  defines the device view, the sticky flags, the id check of `get` (`_stored`), how a priority becomes a leaf in `add`
+  and `add_batch`, and sampling."""
+
+  def __init__(self, codec, capacity, structure, random_state, distribution, frame_dedup, frame_capacity):
+    self._codec = codec
+    self._capacity = capacity
+    self._structure = structure
+    self._random_state = random_state
+    self._distribution = distribution
+    self._store = _make_store(capacity, frame_dedup, frame_capacity)
+    self._live_ids = collections.deque()   # ids currently stored, oldest first (keys of the OrderedDict)
+    self._t = 0
+
+  def _observations(self, item):
+    """The codec round trip of one added item and its flat observations: (item, s_tm1, s_t)."""
+    if self._codec is not None:
+      item = self._codec(item)
+    return item, _host_obs(item[0], self._store), _host_obs(item[4], self._store)
+
+  def _book(self):
+    """The host bookkeeping of one add, in `add` and `add_batch` alike: evicts the oldest id when the replay is full
+    and registers id `_t`.  Returns (release_row, evict_index, tree_index, patches) of the add's device record."""
+    evicted = self._live_ids.popleft() if self.size == self._capacity else None
+    evict_index, tree_index = self._distribution._insert(self._t, evicted)
+    self._live_ids.append(self._t)
+    self._t += 1
+    return evicted is not None, evict_index, tree_index, self._distribution.take_patches()
+
+  def _add(self, item, s_tm1, s_t, **leaf):
+    """`add` after `_observations`: the bookkeeping, then one dz_replay_add call carrying the row, the list patches
+    and, for a prioritized add, the sum-tree fields `leaf`."""
+    slot = self._t % self._capacity
+    release, evict, tree, patches = self._book()
+    assert len(patches) <= 4
+    _apply_index_record(self.device_view(), patches, tree_index=tree, evict_index=evict, slot=slot,
+                        action=int(item[1]), reward=float(item[2]), discount=float(item[3]), h_s_tm1=s_tm1, h_s_t=s_t,
+                        release_row=release, **leaf)
+
+  def get(self, ids: Sequence[int]):
+    """`replay.py:153-156`."""
+    ids = [int(i) for i in ids]
+    for i in ids:
+      if not self._stored(i):
+        raise KeyError(i)
+    self._raise_if_pool_full()
+    return self._store.get_rows(self._structure, np.asarray(ids, dtype=np.int64) % self._capacity)
+
+  @property
+  def size(self) -> int:
+    return len(self._live_ids)
+
+  @property
+  def capacity(self) -> int:
+    return self._capacity
+
+  @property
+  def frames_in_use(self) -> int:
+    """Live planes of the frame pool, plane 0 included (a synchronising read; for sizing `frame_capacity`)."""
+    if not isinstance(self._store, _FramePoolStore):
+      raise ValueError('frames_in_use needs a replay constructed with frame_dedup=True')
+    return self._store.frames_in_use()
+
+  @property
+  def storage_bytes(self) -> int:
+    """Device bytes of the transition storage (observations or frame pool, plus per-row scalars)."""
+    return self._store.storage_bytes()
+
+  def get_state(self) -> Mapping[str, Any]:
+    """`replay.py:179-187` / `:747-754`: same keys; `storage` is a list of (id, Transition) with host arrays."""
+    ids = list(self._live_ids)
+    return {'storage': list(zip(ids, self.get(ids))) if ids else [], 't': self._t,
+            'distribution': self._distribution.get_state()}
+
+  def set_state(self, state: Mapping[str, Any]) -> None:
+    """`replay.py:189-193` / `:756-760`."""
+    _restore_rows(self, state['storage'])
+    self._t = state['t']
+    self._distribution.set_state(state['distribution'])
+
+  def save_checkpoint(self, directory: str) -> None:
+    """Writes the replay into `directory` (DESIGN.md §9): device arrays streamed through a fixed staging ring with a
+    digest per chunk, the host bookkeeping as int64 arrays, a JSON manifest.  Host memory stays bounded by the ring
+    plus the O(capacity) integer bookkeeping.  The RandomState is not saved (as for `get_state`).  The raw sum-tree
+    nodes of a prioritized replay are written bit for bit."""
+    from dqn_zoo_b200 import checkpoint as ck
+    _replay_files(self, False).write(directory, ck.Transfer(self._store.action.device))
+
+  def load_checkpoint(self, directory: str) -> None:
+    """Restores `save_checkpoint` of a replay of the same class, layout, capacity, observation shape and
+    frame_capacity: afterwards every device array and host list equals the saved replay's, the frame pool's plane
+    ids and free stack included, so later adds and samples are those the saved replay would make.  A mismatch of
+    those raises ValueError before anything changes; a digest, size or pool-consistency failure raises RuntimeError
+    naming the file (and chunk) and leaves the replay empty."""
+    from dqn_zoo_b200 import checkpoint as ck
+    m = ck.read_manifest(directory, REPLAY_FORMAT)
+    ck.validate(m, _checkpoint_header(self), directory)
+    st = self._store
+    saved_shape = None if m.get('obs_shape') is None else (tuple(m['obs_shape']), np.dtype(m['obs_dtype']))
+    if saved_shape is not None and st.obs_shape is not None and saved_shape != (st.obs_shape, st.obs_dtype):
+      raise ValueError('%s: checkpoint has observations %s %s, this replay stores %s %s'
+                       % (directory, saved_shape[0], saved_shape[1], st.obs_shape, st.obs_dtype))
+    try:
+      _restore_checkpoint(self, directory, m, saved_shape, ck)
+    except BaseException as e:
+      _reset_empty(self)
+      if isinstance(e, RuntimeError):
+        raise
+      raise RuntimeError('%s: checkpoint data is inconsistent (%s: %s); the replay was reset to empty'
+                         % (directory, type(e).__name__, e)) from e
+
+  def snapshot_checkpoint(self):
+    """A `checkpoint.Snapshot` of the replay at the current point of the CUDA stream (DESIGN.md §9): device copies of
+    the per-row scalars, the sum tree or id mirror, the plane table, the free stack and the live planes' ids and
+    hashes, the observation bytes of the live rows packed and digested in one pass, and copies of the host
+    bookkeeping.  Its `write(directory)` gives the files `save_checkpoint(directory)` would give now, byte for byte,
+    while the replay goes on changing."""
+    from dqn_zoo_b200 import checkpoint as ck
+    held = []
+    files = _replay_files(self, True, held)
+    return ck.Snapshot(files.write, held, self._store.action.device)
+
+  def snapshot_checkpoint_bytes(self) -> int:
+    """An upper bound of the device memory `snapshot_checkpoint()` takes now (a synchronising read)."""
+    return _snapshot_bytes(self)
+
+  def check_valid(self) -> Tuple[bool, str]:
+    """`replay.py:195-200` / `:762-768`, plus for a frame pool: the pool-full flag, refcounts and the free-stack
+    partition."""
+    if self._t < self.size:
+      return False, 't should be >= storage size.'
+    if set(self._live_ids) != set(self._distribution.ids()):
+      return False, 'IDs in storage and distribution do not match.'
+    if isinstance(self._store, _FramePoolStore):
+      self._raise_if_pool_full()
+      ok, msg = self._store.check_pool(np.asarray(list(self._live_ids), dtype=np.int64) % self._capacity)
+      if not ok:
+        return ok, msg
+    return self._distribution.check_valid()
+
+  def _raise_if_pool_full(self):
+    """DZ_FLAG_FRAME_POOL_FULL is sticky: the stored bytes are wrong from that add on, so every sync point raises."""
+    if isinstance(self._store, _FramePoolStore) and int(self._flags().item()) & _lib.DZ_FLAG_FRAME_POOL_FULL:
+      raise RuntimeError(_POOL_FULL % self._store.frame_capacity)
+
+  # -- what a learner step reads of the replay -----------------------------------------------------------------------
+  def _flush(self):
+    """Brings the device mirrors up to date with the host lists (before a learner step is captured)."""
+    self._distribution.flush()
+
+  def _alpha(self) -> float:
+    """The priority exponent of the learner's priority write-back (1 for a replay without priorities)."""
+    return 1.0
+
+  def _sample_constants(self) -> Tuple[float, float, float, float]:
+    """The last four words of the learner's staging record: size, importance-sampling exponent, uniform sample
+    probability and normalize weights (1 or 0)."""
+    return float(self.size), 1.0, 0.0, 0.0
+
+  def _rng_state(self):
+    """The state of the RandomState the samples are drawn from (which `get_state` leaves to the run)."""
+    return self._random_state.get_state()
+
+  def _set_rng_state(self, state) -> None:
+    self._random_state.set_state(state)
+
+
+# ------------------------------------------------------------------------------------------------
 # R6: TransitionReplay
 # ------------------------------------------------------------------------------------------------
 
 
-class TransitionReplay:
+class TransitionReplay(_Replay):
   """Uniform replay with oldest-out eviction (`replay.py:120-200`), storage in HBM.
 
   `frame_dedup=True` stores each distinct H*W plane of the (3-D uint8) observations once (`_FramePoolStore`,
@@ -1050,15 +1285,9 @@ class TransitionReplay:
 
   def __init__(self, capacity: int, structure, random_state: np.random.RandomState, encoder=None, decoder=None,
                frame_dedup: bool = False, frame_capacity: Optional[int] = None):
-    self._codec = _check_codec(encoder, decoder)
-    self._capacity = capacity
-    self._structure = structure
-    self._random_state = random_state
-    self._distribution = UniformDistribution(random_state=random_state)
+    super().__init__(_check_codec(encoder, decoder), capacity, structure, random_state,
+                     UniformDistribution(random_state=random_state), frame_dedup, frame_capacity)
     self._distribution._mirror.ensure(capacity)   # fixed address: captured CUDA graphs keep pointing at it
-    self._store = _make_store(capacity, frame_dedup, frame_capacity)
-    self._live_ids = collections.deque()   # ids currently stored, oldest first (keys of the OrderedDict)
-    self._t = 0
 
   def device_view(self):
     v = self._store.fill_view(_lib.ReplayView())
@@ -1069,55 +1298,19 @@ class TransitionReplay:
     """The sticky device flags the kernels of this replay's view set."""
     return self._store.flags
 
+  def _stored(self, i):
+    return bool(self._live_ids) and self._live_ids[0] <= i <= self._live_ids[-1]
+
   def add(self, item) -> None:
     """`replay.py:142-151`."""
-    if self._codec is not None:
-      item = self._codec(item)
-    s_tm1 = _host_obs(item[0], self._store)
-    s_t = _host_obs(item[4], self._store)
-    full = self.size == self._capacity
-    if full:
-      self._distribution.remove([self._live_ids.popleft()])
-    item_id = self._t
-    self._distribution.add([item_id])
-    patches = self._distribution.take_patches()
-    v = self.device_view()
-    first = patches[:4]
-    _apply_index_record(v, first, slot=item_id % self._capacity, action=int(item[1]), reward=float(item[2]),
-                        discount=float(item[3]), h_s_tm1=s_tm1, h_s_t=s_t, release_row=full)
-    assert len(patches) <= 4
-    self._live_ids.append(item_id)
-    self._t += 1
+    self._add(*self._observations(item))
 
   def add_batch(self, items) -> None:
     """K transitions at once: `items` is a Transition whose fields have a leading K axis (observations [K, *obs_shape]
     as a numpy array or a CUDA tensor; a_tm1, r_t, discount_t of length K).  The replay afterwards equals the replay
     after `for k in range(K): add(item_k)`.  Unlike that loop, the whole batch is validated first: a shape or dtype
     mismatch raises what `add` raises and leaves the replay unchanged."""
-    batch = _batch_items(items, self._codec, self._store)
-    if batch[0] == 0:
-      return
-    dist = self._distribution
-
-    def book():
-      full = self.size == self._capacity
-      if full:
-        dist.remove([self._live_ids.popleft()])
-      dist.add([self._t])
-      self._live_ids.append(self._t)
-      self._t += 1
-      return full, -1, -1, dist.take_patches()
-
-    _add_batch(self, batch, book)
-
-  def get(self, ids: Sequence[int]):
-    """`replay.py:153-156`."""
-    ids = [int(i) for i in ids]
-    for i in ids:
-      if not self._live_ids or not (self._live_ids[0] <= i <= self._live_ids[-1]):
-        raise KeyError(i)
-    _raise_if_pool_full(self._store, self._flags())
-    return self._store.get_rows(self._structure, np.asarray(ids, dtype=np.int64) % self._capacity)
+    _add_batch(self, _batch_items(items, self._codec, self._store))
 
   def sample_device(self, size: int):
     """Host randint draw (`replay.py:78`), device id lookup + gather; returns device tensors."""
@@ -1134,92 +1327,11 @@ class TransitionReplay:
   def sample(self, size: int):
     """`replay.py:158-165`."""
     _, _, tensors = self.sample_device(size)
-    _raise_if_pool_full(self._store, self._flags())
+    self._raise_if_pool_full()
     return self._store.to_host_transition(self._structure, tensors)
 
   def ids(self) -> Iterable[int]:
     return list(self._live_ids)
-
-  @property
-  def size(self) -> int:
-    return len(self._live_ids)
-
-  @property
-  def capacity(self) -> int:
-    return self._capacity
-
-  @property
-  def frames_in_use(self) -> int:
-    """Live planes of the frame pool, plane 0 included (a synchronising read; for sizing `frame_capacity`)."""
-    return _frames_in_use(self)
-
-  @property
-  def storage_bytes(self) -> int:
-    """Device bytes of the transition storage (observations or frame pool, plus per-row scalars)."""
-    return self._store.storage_bytes()
-
-  def get_state(self) -> Mapping[str, Any]:
-    """`replay.py:179-187`: same keys; `storage` is a list of (id, Transition) with host arrays."""
-    ids = list(self._live_ids)
-    return {'storage': list(zip(ids, self.get(ids))) if ids else [], 't': self._t,
-            'distribution': self._distribution.get_state()}
-
-  def set_state(self, state: Mapping[str, Any]) -> None:
-    """`replay.py:189-193`."""
-    _restore_rows(self, state['storage'])
-    self._t = state['t']
-    self._distribution.set_state(state['distribution'])
-
-  def save_checkpoint(self, directory: str) -> None:
-    """Writes the replay into `directory` (DESIGN.md §9): device arrays streamed through a fixed staging ring with a
-    digest per chunk, the host bookkeeping as int64 arrays, a JSON manifest.  Host memory stays bounded by the ring
-    plus the O(capacity) integer bookkeeping.  The RandomState is not saved (as for `get_state`)."""
-    _save_checkpoint(self, directory)
-
-  def load_checkpoint(self, directory: str) -> None:
-    """Restores `save_checkpoint` of a replay of the same class, layout, capacity, observation shape and
-    frame_capacity: afterwards every device array and host list equals the saved replay's, the frame pool's plane
-    ids and free stack included, so later adds and samples are those the saved replay would make.  A mismatch of
-    those raises ValueError before anything changes; a digest, size or pool-consistency failure raises RuntimeError
-    naming the file (and chunk) and leaves the replay empty."""
-    _load_checkpoint(self, directory)
-
-  def snapshot_checkpoint(self):
-    """A `checkpoint.Snapshot` of the replay at the current point of the CUDA stream (DESIGN.md §9): device copies of
-    the per-row scalars, the sum tree or id mirror, the plane table, the free stack and the live planes' ids and
-    hashes, the observation bytes of the live rows packed and digested in one pass, and copies of the host
-    bookkeeping.  Its `write(directory)` gives the files `save_checkpoint(directory)` would give now, byte for byte,
-    while the replay goes on changing."""
-    return _snapshot_checkpoint(self)
-
-  def snapshot_checkpoint_bytes(self) -> int:
-    """An upper bound of the device memory `snapshot_checkpoint()` takes now (a synchronising read)."""
-    return _snapshot_bytes(self)
-
-  def check_valid(self) -> Tuple[bool, str]:
-    """`replay.py:195-200`."""
-    if self._t < self.size:
-      return False, 't should be >= storage size.'
-    if set(self._live_ids) != set(self._distribution.ids()):
-      return False, 'IDs in storage and distribution do not match.'
-    ok, msg = _check_pool(self, self._flags())
-    if not ok:
-      return ok, msg
-    return self._distribution.check_valid()
-
-
-def _frames_in_use(rep):
-  if not isinstance(rep._store, _FramePoolStore):
-    raise ValueError('frames_in_use needs a replay constructed with frame_dedup=True')
-  return rep._store.frames_in_use()
-
-
-def _check_pool(rep, flags):
-  """check_valid() of a frame-deduplicated replay: the pool-full flag, refcounts and the free-stack partition."""
-  if not isinstance(rep._store, _FramePoolStore):
-    return True, ''
-  _raise_if_pool_full(rep._store, flags)
-  return rep._store.check_pool(np.asarray(list(rep._live_ids), dtype=np.int64) % rep._capacity)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1290,7 +1402,7 @@ def _replay_files(rep, snapshot, held=None):
   may change before the files are written."""
   from dqn_zoo_b200 import checkpoint as ck
   st, dist = rep._store, rep._distribution
-  _raise_if_pool_full(st, rep._flags())
+  rep._raise_if_pool_full()
   dist.flush()                                    # device mirrors up to date with the host lists
 
   def dev(t):
@@ -1303,26 +1415,12 @@ def _replay_files(rep, snapshot, held=None):
   files = ck.Files()
   live = np.fromiter(rep._live_ids, dtype=np.int64, count=len(rep._live_ids))
   files.host['live_ids'] = lambda: live
-  extra = {}
-  if isinstance(dist, UniformDistribution):
-    ids, id_to_index = keep(dist._ids), keep(dist._id_to_index)
-    files.host['ids'] = lambda: np.asarray(ids, dtype=np.int64)
-    files.host['id_to_index'] = lambda: _dict_array(id_to_index)
-    files.dev['ids_mirror'] = dev(dist._mirror.t)
-  else:
-    id_to_index, index_to_id = keep(dist._id_to_index), keep(dist._index_to_id)
-    inactive, active = keep(dist._inactive_indices), keep(dist._active_indices)
-    location = keep(dist._active_indices_location)
-    files.host['id_to_index'] = lambda: _dict_array(id_to_index)
-    files.host['index_to_id'] = lambda: _dict_array(index_to_id)
-    files.host['inactive_indices'] = lambda: np.asarray(inactive, dtype=np.int64)
-    files.host['active_indices'] = lambda: np.asarray(active, dtype=np.int64)
-    files.host['active_indices_location'] = lambda: _dict_array(location)
-    tree = dist._sum_tree
-    files.dev['sum_tree'] = dev(tree._nodes)
-    files.dev['live_mirror'] = dev(dist._live_dev.t)
-    files.dev['id_at_mirror'] = dev(dist._id_at_dev.t)
-    extra.update(tree_size=tree.size, tree_first_leaf=tree.capacity)
+  for name, kind in dist._HOST_LISTS.items():
+    x = keep(getattr(dist, '_' + name))
+    files.host[name] = (lambda x=x: _dict_array(x)) if kind is dict else (lambda x=x: np.asarray(x, dtype=np.int64))
+  for name, t in dist._device_mirrors().items():
+    files.dev[name] = dev(t)
+  extra = dist._manifest()
   allocated = st.obs_shape is not None
   if allocated:
     for name in ('action', 'reward', 'discount'):
@@ -1365,18 +1463,11 @@ def _replay_files(rep, snapshot, held=None):
   return files
 
 
-def _save_checkpoint(rep, directory):
-  from dqn_zoo_b200 import checkpoint as ck
-  _replay_files(rep, False).write(directory, ck.Transfer(rep._store.action.device))
-
-
 def _snapshot_bytes(rep):
   """An upper bound of the device bytes `_replay_files(rep, True)` allocates, transient buffers included (the frame
   pool's live count is a synchronising read)."""
-  st, dist = rep._store, rep._distribution
-  mirrors = [dist._mirror.t] if isinstance(dist, UniformDistribution) else [dist._sum_tree._nodes, dist._live_dev.t,
-                                                                            dist._id_at_dev.t]
-  n = sum(t.numel() * t.element_size() for t in mirrors)
+  st = rep._store
+  n = sum(t.numel() * t.element_size() for t in rep._distribution._device_mirrors().values())
   if st.obs_shape is None:
     return n
   n += sum(getattr(st, k).numel() * getattr(st, k).element_size() for k in ('action', 'reward', 'discount'))
@@ -1392,48 +1483,14 @@ def _snapshot_bytes(rep):
   return n + 8 * (live * record // max(1, ck.CHUNK_BYTES // record * record) + 1) + 4096
 
 
-def _snapshot_checkpoint(rep):
-  from dqn_zoo_b200 import checkpoint as ck
-  held = []
-  files = _replay_files(rep, True, held)
-  return ck.Snapshot(files.write, held, rep._store.action.device)
-
-
 def _reset_empty(rep):
   """A replay that failed to load: empty, with the host lists, mirrors' meaning, sum tree and pool of a new one."""
   rep._live_ids = collections.deque()
   rep._t = 0
-  dist = rep._distribution
-  if isinstance(dist, UniformDistribution):
-    dist._ids, dist._id_to_index, dist._pending = [], {}, []
-  else:
-    dist._id_to_index, dist._index_to_id, dist._pending = {}, {}, []
-    dist._inactive_indices = list(range(rep._capacity))
-    dist._active_indices, dist._active_indices_location = [], {}
-    dist._sum_tree._nodes.zero_()
-    dist._sum_tree._size = rep._capacity
+  rep._distribution._reset(rep._capacity)
   if isinstance(rep._store, _FramePoolStore):
     rep._store.reset()
   rep._flags().zero_()
-
-
-def _load_checkpoint(rep, directory):
-  from dqn_zoo_b200 import checkpoint as ck
-  m = ck.read_manifest(directory, REPLAY_FORMAT)
-  ck.validate(m, _checkpoint_header(rep), directory)
-  st = rep._store
-  saved_shape = None if m.get('obs_shape') is None else (tuple(m['obs_shape']), np.dtype(m['obs_dtype']))
-  if saved_shape is not None and st.obs_shape is not None and saved_shape != (st.obs_shape, st.obs_dtype):
-    raise ValueError('%s: checkpoint has observations %s %s, this replay stores %s %s'
-                     % (directory, saved_shape[0], saved_shape[1], st.obs_shape, st.obs_dtype))
-  try:
-    _restore_checkpoint(rep, directory, m, saved_shape, ck)
-  except BaseException as e:
-    _reset_empty(rep)
-    if isinstance(e, RuntimeError):
-      raise
-    raise RuntimeError('%s: checkpoint data is inconsistent (%s: %s); the replay was reset to empty'
-                       % (directory, type(e).__name__, e)) from e
 
 
 def _restore_checkpoint(rep, directory, m, saved_shape, ck):
@@ -1448,16 +1505,11 @@ def _restore_checkpoint(rep, directory, m, saved_shape, ck):
   def dev(name, consume):
     xfer.load_device(path(name), files[name], consume)
 
-  if isinstance(dist, UniformDistribution):
-    dev('ids_mirror', _bytes_of(dist._mirror.t))
-  else:
-    tree = dist._sum_tree
-    if (m['tree_first_leaf'], m['tree_size']) != (tree.capacity, tree.size):
-      raise RuntimeError('%s: sum tree of %d leaves (size %d) in the manifest, %d (size %d) here'
-                         % (directory, m['tree_first_leaf'], m['tree_size'], tree.capacity, tree.size))
-    dev('sum_tree', _bytes_of(tree._nodes))
-    dev('live_mirror', _bytes_of(dist._live_dev.t))
-    dev('id_at_mirror', _bytes_of(dist._id_at_dev.t))
+  for key, value in dist._manifest().items():
+    if m.get(key) != value:
+      raise RuntimeError('%s: the manifest has %s = %r, this replay has %r' % (directory, key, m.get(key), value))
+  for name, t in dist._device_mirrors().items():
+    dev(name, _bytes_of(t))
   if saved_shape is not None:
     st.allocate(*saved_shape)
     for name in ('action', 'reward', 'discount'):
@@ -1469,15 +1521,8 @@ def _restore_checkpoint(rep, directory, m, saved_shape, ck):
   # host bookkeeping last: the same containers, filled in the saved insertion order
   rep._live_ids = collections.deque(live.tolist())
   rep._t = int(m['t'])
-  if isinstance(dist, UniformDistribution):
-    dist._ids = host['ids'].tolist()
-    dist._id_to_index = _array_dict(host['id_to_index'])
-  else:
-    dist._id_to_index = _array_dict(host['id_to_index'])
-    dist._index_to_id = _array_dict(host['index_to_id'])
-    dist._inactive_indices = host['inactive_indices'].tolist()
-    dist._active_indices = host['active_indices'].tolist()
-    dist._active_indices_location = _array_dict(host['active_indices_location'])
+  for name, kind in dist._HOST_LISTS.items():
+    setattr(dist, '_' + name, _array_dict(host[name]) if kind is dict else host[name].tolist())
   dist._pending = []
 
 
@@ -1526,8 +1571,7 @@ def _restore_rows(rep, storage):
   """Rewrites device rows from a `storage` list of (id, item) (set_state).  A frame pool is emptied first and the rows
   are re-added in id order, so the plane table is the one those adds leave (and either layout loads the other's
   state)."""
-  pool = isinstance(rep._store, _FramePoolStore)
-  if pool:
+  if isinstance(rep._store, _FramePoolStore):
     storage = sorted(storage, key=lambda x: int(x[0]))
     rep._store.reset()
     rep._flags().bitwise_and_(~_lib.DZ_FLAG_FRAME_POOL_FULL)   # the emptied pool holds no wrong bytes
@@ -1537,7 +1581,7 @@ def _restore_rows(rep, storage):
     s_tm1 = _host_obs(item[0], rep._store)
     s_t = _host_obs(item[4], rep._store)
     if v is None:
-      v = rep.device_view() if pool else rep._store.fill_view(_lib.ReplayView())
+      v = rep.device_view()
     _apply_index_record(v, [], slot=int(i) % rep._capacity, action=int(item[1]), reward=float(item[2]),
                         discount=float(item[3]), h_s_tm1=s_tm1, h_s_t=s_t)
 
@@ -1547,7 +1591,7 @@ def _restore_rows(rep, storage):
 # ------------------------------------------------------------------------------------------------
 
 
-class PrioritizedTransitionReplay:
+class PrioritizedTransitionReplay(_Replay):
   """Proportional prioritized replay (`replay.py:654-768`), storage + sum tree in HBM."""
 
   def __init__(self, capacity: int, structure, priority_exponent: float,
@@ -1555,18 +1599,11 @@ class PrioritizedTransitionReplay:
                normalize_weights: bool, random_state: np.random.RandomState, encoder=None, decoder=None,
                frame_dedup: bool = False, frame_capacity: Optional[int] = None):
     """`frame_dedup` / `frame_capacity`: the storage layout, as for `TransitionReplay`."""
-    self._codec = _check_codec(encoder, decoder)
-    self._capacity = capacity
-    self._structure = structure
-    self._random_state = random_state
-    self._distribution = PrioritizedDistribution(
+    super().__init__(_check_codec(encoder, decoder), capacity, structure, random_state, PrioritizedDistribution(
         min_capacity=capacity, max_capacity=capacity, priority_exponent=priority_exponent,
-        uniform_sample_probability=uniform_sample_probability, random_state=random_state)
+        uniform_sample_probability=uniform_sample_probability, random_state=random_state), frame_dedup, frame_capacity)
     self._importance_sampling_exponent = importance_sampling_exponent
     self._normalize_weights = normalize_weights
-    self._store = _make_store(capacity, frame_dedup, frame_capacity)
-    self._live_ids = collections.deque()
-    self._t = 0
 
   def device_view(self):
     v = self._distribution.device_view()
@@ -1577,16 +1614,15 @@ class PrioritizedTransitionReplay:
   def _flags(self):
     return self._distribution._sum_tree._flags
 
+  def _stored(self, i):
+    return i in self._distribution._id_to_index
+
   def add(self, item, priority: float) -> None:
     """`replay.py:690-699`: one device call carries the row, the list patches, the evicted
     leaf's zeroing and the new leaf (= priority**alpha evaluated in float64 on the host, as
     `replay.py:507` does)."""
-    if self._codec is not None:
-      item = self._codec(item)
-    s_tm1 = _host_obs(item[0], self._store)
-    s_t = _host_obs(item[4], self._store)
-    dist = self._distribution
-    alpha = dist._priority_exponent
+    item, s_tm1, s_t = self._observations(item)
+    alpha = self._distribution._priority_exponent
     d_priority = None
     if isinstance(priority, torch.Tensor):
       # priority kept on the device by the agent (max_seen_priority); exact for alpha in {0.5, 1}
@@ -1597,20 +1633,8 @@ class PrioritizedTransitionReplay:
     leaf = np.asarray(_power([priority], alpha))
     if not np.isfinite(leaf).all() or (leaf < 0.0).any():
       raise ValueError('value must be finite and positive.')
-    evicted = -1
-    if self.size == self._capacity:
-      (evicted,) = dist._host_remove([self._live_ids.popleft()])
-    item_id = self._t
-    (idx,) = dist._host_add([item_id])
-    patches = dist.take_patches()
-    v = self.device_view()
-    _apply_index_record(v, patches[:4], tree_index=idx, leaf_value=float(leaf[0]), evict_index=evicted,
-                        size_after=dist._sum_tree.size, slot=item_id % self._capacity, action=int(item[1]),
-                        reward=float(item[2]), discount=float(item[3]), h_s_tm1=s_tm1, h_s_t=s_t,
-                        d_priority=d_priority, alpha=float(alpha), release_row=evicted >= 0)
-    assert len(patches) <= 4
-    self._live_ids.append(item_id)
-    self._t += 1
+    self._add(item, s_tm1, s_t, leaf_value=float(leaf[0]), size_after=self._distribution._sum_tree.size,
+              d_priority=d_priority, alpha=float(alpha))
 
   def add_batch(self, items, priorities) -> None:
     """K transitions at once (`items` as for `TransitionReplay.add_batch`).  `priorities`: a float, a length-K sequence
@@ -1620,8 +1644,7 @@ class PrioritizedTransitionReplay:
     and leaves the replay unchanged."""
     batch = _batch_items(items, self._codec, self._store)
     count = batch[0]
-    dist = self._distribution
-    alpha = dist._priority_exponent
+    alpha = self._distribution._priority_exponent
     d_priority = None
     if isinstance(priorities, torch.Tensor) and priorities.numel() == 1 and priorities.is_cuda \
         and priorities.dtype == torch.float32 and alpha in (0.5, 1.0):
@@ -1637,27 +1660,7 @@ class PrioritizedTransitionReplay:
     leaves = np.asarray(_power(pri, alpha), dtype=np.float64)
     if not np.isfinite(leaves).all() or (leaves < 0.0).any():
       raise ValueError('value must be finite and positive.')
-    if count == 0:
-      return
-
-    def book():
-      evicted = -1
-      if self.size == self._capacity:
-        (evicted,) = dist._host_remove([self._live_ids.popleft()])
-      (idx,) = dist._host_add([self._t])
-      self._live_ids.append(self._t)
-      self._t += 1
-      return evicted >= 0, evicted, idx, dist.take_patches()
-
-    _add_batch(self, batch, book, leaves=leaves, d_priority=d_priority, alpha=float(alpha))
-
-  def get(self, ids: Sequence[int]):
-    ids = [int(i) for i in ids]
-    for i in ids:
-      if i not in self._distribution._id_to_index:
-        raise KeyError(i)
-    _raise_if_pool_full(self._store, self._flags())
-    return self._store.get_rows(self._structure, np.asarray(ids, dtype=np.int64) % self._capacity)
+    _add_batch(self, batch, leaves=leaves, d_priority=d_priority, alpha=float(alpha))
 
   def sample_device(self, size: int):
     """Sampling + gather, everything left on the device: (ids, indices, slots, probs, weights, batch)."""
@@ -1673,7 +1676,7 @@ class PrioritizedTransitionReplay:
     ids, _, _, _, weights, tensors = self.sample_device(size)
     tr = self._store.to_host_transition(self._structure, tensors)
     w = weights.cpu().numpy()
-    _raise_if_pool_full(self._store, self._flags())
+    self._raise_if_pool_full()
     self._distribution._sum_tree._raise_flags()
     if not np.isfinite(w).all():
       raise ValueError('Weights are not finite: %s.' % w)
@@ -1684,66 +1687,16 @@ class PrioritizedTransitionReplay:
     self._distribution.update_priorities(ids, np.asarray(priorities))
 
   @property
-  def size(self) -> int:
-    return len(self._live_ids)
-
-  @property
-  def capacity(self) -> int:
-    return self._capacity
-
-  @property
   def importance_sampling_exponent(self):
     """`replay.py:742-745`."""
     return self._importance_sampling_exponent(self._t)
 
-  @property
-  def frames_in_use(self) -> int:
-    """Live planes of the frame pool, plane 0 included (a synchronising read; for sizing `frame_capacity`)."""
-    return _frames_in_use(self)
+  def _alpha(self):
+    return self._distribution._priority_exponent
 
-  @property
-  def storage_bytes(self) -> int:
-    """Device bytes of the transition storage (observations or frame pool, plus per-row scalars)."""
-    return self._store.storage_bytes()
-
-  def get_state(self) -> Mapping[str, Any]:
-    """`replay.py:747-754`."""
-    ids = list(self._live_ids)
-    return {'storage': list(zip(ids, self.get(ids))) if ids else [], 't': self._t,
-            'distribution': self._distribution.get_state()}
-
-  def set_state(self, state: Mapping[str, Any]) -> None:
-    """`replay.py:756-760`."""
-    _restore_rows(self, state['storage'])
-    self._t = state['t']
-    self._distribution.set_state(state['distribution'])
-
-  def save_checkpoint(self, directory: str) -> None:
-    """As `TransitionReplay.save_checkpoint`; the raw sum-tree nodes are written bit for bit."""
-    _save_checkpoint(self, directory)
-
-  def load_checkpoint(self, directory: str) -> None:
-    """As `TransitionReplay.load_checkpoint`."""
-    _load_checkpoint(self, directory)
-
-  def snapshot_checkpoint(self):
-    """As `TransitionReplay.snapshot_checkpoint`."""
-    return _snapshot_checkpoint(self)
-
-  def snapshot_checkpoint_bytes(self) -> int:
-    """As `TransitionReplay.snapshot_checkpoint_bytes`."""
-    return _snapshot_bytes(self)
-
-  def check_valid(self) -> Tuple[bool, str]:
-    """`replay.py:762-768`."""
-    if self._t < self.size:
-      return False, 't should be >= storage size.'
-    if set(self._live_ids) != set(self._distribution.ids()):
-      return False, 'IDs in storage and distribution do not match.'
-    ok, msg = _check_pool(self, self._flags())
-    if not ok:
-      return ok, msg
-    return self._distribution.check_valid()
+  def _sample_constants(self):
+    return (float(self.size), float(self.importance_sampling_exponent),
+            float(self._distribution._uniform_sample_probability), 1.0 if self._normalize_weights else 0.0)
 
 
 def bulk_fill_synthetic(rep, obs_shape, seed, num_actions, discount=0.99, priority=1.0):
@@ -1786,24 +1739,7 @@ def _fill_bookkeeping(rep, priority):
   cap = rep._capacity
   rep._live_ids = collections.deque(range(cap))
   rep._t = cap
-  dist = rep._distribution
-  if isinstance(dist, UniformDistribution):
-    dist._ids = list(range(cap))
-    dist._id_to_index = {i: i for i in range(cap)}
-    dist._pending = []
-    dist._mirror.upload(dist._ids)
-    return
-  idx = np.arange(cap - 1, -1, -1, dtype=np.int64)          # id i -> index C-1-i
-  dist._id_to_index = dict(zip(range(cap), idx.tolist()))
-  dist._index_to_id = dict(zip(idx.tolist(), range(cap)))
-  dist._inactive_indices = []
-  dist._active_indices = idx.tolist()
-  dist._active_indices_location = dict(zip(idx.tolist(), range(cap)))
-  dist._pending = []
-  dist._live_dev.upload(idx)
-  dist._id_at_dev.upload(idx)                                  # id_at[index] = C-1-index
-  leaf = float(_power([priority], dist._priority_exponent)[0])
-  dist._sum_tree.set_all(np.full(cap, leaf, dtype=np.float64))
+  rep._distribution._fill(cap, priority)
 
 
 # ------------------------------------------------------------------------------------------------
