@@ -212,6 +212,9 @@ _SIGNATURES = {
     'dz_test_dueling_head_fwd': (i32, [vp, i32, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), i64, C.POINTER(vp), vp]),
     'dz_test_dueling_head_bwd': (i32, [vp, i32, vp, vp, C.POINTER(vp), vp, vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
                                        vp]),
+    'dz_test_noisy_head_fwd': (i32, [vp, i32, i32, C.POINTER(vp), C.POINTER(vp), vp, C.POINTER(vp), vp]),
+    'dz_test_noisy_head_bwd': (i32, [vp, i32, C.POINTER(vp), vp, vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
+                                     C.POINTER(vp), vp]),
     'dz_test_iqn_cos': (i32, [vp, i64, i32, vp, vp]),
     'dz_test_iqn_head_fwd': (i32, [vp, i32, C.POINTER(i32), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), vp]),
     'dz_test_iqn_head_dgrad': (i32, [vp, i32, vp, vp, vp, vp, vp]),

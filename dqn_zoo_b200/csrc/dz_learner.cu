@@ -1850,6 +1850,256 @@ __global__ void __launch_bounds__(256) noisy_dueling_head_bwd_kernel(const __gri
   dueling_head_bwd<true>(n.g, &n);
 }
 
+// ---- Rainbow's noisy head (DESIGN.md §7): two streams (advantage 512 -> A * atoms, value 512 -> atoms) without a split
+// reduction or a finish launch.  Each weight is formed as fmaf(sigma_w, eps_in_k * eps_out_n, mu_w), the operations of
+// gemm_nn_kernel<DUAL> / gemm_nt_kernel<DUAL>.
+
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem));
+}
+__device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem));
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+constexpr int kNhTile = 8;       // forward: output columns of one stream per CTA
+constexpr int kNhRows = 32;      // forward: rows (images) per pass
+constexpr int kNhLd = 68;        // forward: x row stride in shared memory, 17 16-byte units (odd: conflict-free float4 reads)
+constexpr int kNhKc = 4;         // backward: dh1 columns per CTA
+constexpr size_t kMaxDynSmem = 227 * 1024;   // the most dynamic shared memory one CTA may opt in to
+constexpr size_t kNhFwdSmem = (size_t)(8 * 2 * kNhRows * kNhLd + 8 * 2 * 64 * kNhTile) * sizeof(float);
+
+// Forward.  blockIdx.y is a group of one or two passes that apply the same parameter blob (online on s_tm1 and s_t,
+// target on s_t): the group's CTAs read each mu / sigma tile once and form it with every member's noise.  blockIdx.x
+// is a kNhTile-column tile of stream 0's outputs, then of stream 1's.  Warp w reduces k in [64 w, 64 w + 64) for all
+// rows, columns and members in ascending k order; the eight warp sums are then added in warp order, then mu_b (if any)
+// and fmaf(sigma_b, eps_out, .) as finish_nn_body does.  The order depends on nothing but k.
+struct NoisyHeadFwdArgs {
+  const float* x[2][2][2];        // [group][member][stream]: h1 [rows][512]
+  float* out[2][2][2];            // [group][member][stream]: [rows][N[stream]]
+  const float* ein[2][2][2];      // [group][member][stream]: eps_in [512]
+  const float* eout[2][2][2];     // [group][member][stream]: eps_out [N[stream]]
+  const float* mu[2][2];          // [group][stream]: [512][N]
+  const float* sigma[2][2];
+  const float* bias[2][2];        // mu bias [N] (or [1] with bias_shared), nullptr without one
+  const float* sbias[2][2];       // sigma bias [N]
+  int members[2];
+  int N[2], tiles0;               // stream widths; tiles of stream 0
+  int rows, bias_shared;
+};
+
+template <int P>
+__device__ __forceinline__ void noisy_head_fwd(const NoisyHeadFwdArgs& a) {
+  extern __shared__ __align__(16) float nh_smem[];
+  const int g = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int s = (int)blockIdx.x < a.tiles0 ? 0 : 1;
+  const int n0 = (s == 0 ? (int)blockIdx.x : (int)blockIdx.x - a.tiles0) * kNhTile, N = a.N[s];
+  const int k0 = warp * 64;
+  float* xs = nh_smem + warp * (2 * kNhRows * kNhLd);                      // [P][rows][kNhLd]: this warp's k slice
+  float* ws = nh_smem + 8 * 2 * kNhRows * kNhLd + warp * (2 * 64 * kNhTile);  // [P][64][kNhTile]: formed weights
+  // this thread's bias terms in the final sums (column n0 + threadIdx.x % kNhTile, member q), loaded up front
+  const int ne = n0 + (int)(threadIdx.x % kNhTile);
+  float bias_e = 0.f, sb_e = 0.f, eo_e[P];
+  if (ne < N) {
+    const float* b = a.bias[g][s];
+    if (b) bias_e = a.bias_shared ? b[0] : b[ne];
+    sb_e = a.sbias[g][s][ne];
+  }
+#pragma unroll
+  for (int q = 0; q < P; ++q) eo_e[q] = ne < N ? a.eout[g][q][s][ne] : 0.f;
+  for (int p = 0; p < P; ++p) {
+    const float* x = a.x[g][p][s];
+    for (int i = lane; i < kNhRows * 16; i += 32) {
+      const int m = i >> 4, q = (i & 15) * 4;
+      float* dst = xs + (p * kNhRows + m) * kNhLd + q;
+      if (m < a.rows) cp_async16(dst, x + (long long)m * 512 + k0 + q);
+      else *reinterpret_cast<float4*>(dst) = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  }
+  {
+    // every load of the tile is issued before any is used: the weights come from HBM, and a loop that waited for
+    // them a few rows at a time paid their latency once per few rows
+    const int c = lane & 7, n = n0 + c, kr = lane >> 3;
+    const bool ok = n < N;
+    const float* __restrict__ mu = a.mu[g][s];
+    const float* __restrict__ sg = a.sigma[g][s];
+    float m_[16], s_[16], ei[P][16], eo[P];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int k = k0 + kr + 4 * i;
+      m_[i] = ok ? mu[(long long)k * N + n] : 0.f;
+      s_[i] = ok ? sg[(long long)k * N + n] : 0.f;
+#pragma unroll
+      for (int p = 0; p < P; ++p) ei[p][i] = a.ein[g][p][s][k];
+    }
+#pragma unroll
+    for (int p = 0; p < P; ++p) eo[p] = ok ? a.eout[g][p][s][n] : 0.f;
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+#pragma unroll
+      for (int p = 0; p < P; ++p) ws[(p * 64 + kr + 4 * i) * kNhTile + c] = fmaf(s_[i], ei[p][i] * eo[p], m_[i]);
+  }
+  cp_async_wait_all();
+  __syncwarp();
+  // lane: row group rg (rows rg + RG i), column quad cq, member p
+  constexpr int RM = 2 * P, RG = kNhRows / RM;
+  const int rg = lane % RG, cq = (lane / RG) & 1, p = lane / (2 * RG);
+  float acc[RM][4];
+#pragma unroll
+  for (int i = 0; i < RM; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+  const float* xp = xs + (p * kNhRows + rg) * kNhLd;
+  const float* wp = ws + p * 64 * kNhTile + cq * 4;
+#pragma unroll 4
+  for (int kq = 0; kq < 64; kq += 4) {
+    float4 xv[RM];
+#pragma unroll
+    for (int i = 0; i < RM; ++i) xv[i] = *reinterpret_cast<const float4*>(xp + i * RG * kNhLd + kq);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float4 w = *reinterpret_cast<const float4*>(wp + (kq + e) * kNhTile);
+#pragma unroll
+      for (int i = 0; i < RM; ++i) {
+        const float xe = e == 0 ? xv[i].x : e == 1 ? xv[i].y : e == 2 ? xv[i].z : xv[i].w;
+        acc[i][0] = fmaf(xe, w.x, acc[i][0]); acc[i][1] = fmaf(xe, w.y, acc[i][1]);
+        acc[i][2] = fmaf(xe, w.z, acc[i][2]); acc[i][3] = fmaf(xe, w.w, acc[i][3]);
+      }
+    }
+  }
+  __syncwarp();
+  float* red = xs;   // [P][rows][kNhTile] warp sums, over this warp's own x slice
+#pragma unroll
+  for (int i = 0; i < RM; ++i)
+    *reinterpret_cast<float4*>(red + (p * kNhRows + rg + i * RG) * kNhTile + cq * 4) =
+        make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+  __syncthreads();
+#pragma unroll
+  for (int q = 0; q < P; ++q) {   // 256 threads: t = q * 256 + threadIdx.x covers [P][rows][kNhTile]
+    const int t = q * kNhRows * kNhTile + (int)threadIdx.x, m = (int)threadIdx.x / kNhTile;
+    if (m >= a.rows || ne >= N) continue;
+    float v = nh_smem[t];
+#pragma unroll
+    for (int w = 1; w < 8; ++w) v += nh_smem[w * (2 * kNhRows * kNhLd) + t];
+    if (a.bias[g][s]) v += bias_e;
+    v = fmaf(sb_e, eo_e[q], v);
+    a.out[g][q][s][(long long)m * N + ne] = v;
+  }
+}
+
+// Both head kernels let the next kernel launch as soon as every CTA is resident: its launch and set-up overlap this
+// kernel, and its griddepcontrol.wait (every kernel's first step) still waits for this grid to complete.
+__device__ __forceinline__ void noisy_head_enter() {
+  dz::pdl_enter();
+  if (threadIdx.x == 0) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+}
+
+__global__ void __launch_bounds__(256) noisy_head_fwd_kernel(const __grid_constant__ NoisyHeadFwdArgs a) {
+  noisy_head_enter();
+  if (a.members[blockIdx.y] == 2) noisy_head_fwd<2>(a);
+  else noisy_head_fwd<1>(a);
+}
+
+// Input gradient through online(s_tm1)'s head (noise apply 0): dh1_s[m][k] = sum_n dout_s[m][n] W_s[k][n], masked by
+// h1_s > 0, for both streams; CTA j owns k in [kNhKc j, kNhKc j + kNhKc).  The CTA stages every row of dout and forms
+// its weights in shared memory; each warp then takes four rows at a time: lane l sums n = l + 32 i in ascending i for
+// the 32 outputs (4 rows x 2 streams x kNhKc columns), and a halving butterfly leaves output l's total in lane l.  The
+// order depends on nothing but n.  With hi / lo set it also writes the tf32 hi/lo pair the tensor-core fc1 input
+// gradient reads, as finish_nt_kernel does.
+struct NoisyHeadBwdArgs {
+  const float* dout[2];           // [B][N[s]]
+  const float* mu[2];             // [512][N[s]] of the online blob
+  const float* sigma[2];
+  const float* ein[2];            // eps_in [512]
+  const float* eout[2];           // eps_out [N[s]]
+  const float* h1[2];             // [B][512], the masks
+  float* dh1[2];                  // [B][512]
+  float *hi[2], *lo[2];           // optional tf32 images of dh1
+  int N[2], B;
+};
+
+// acc[r * 8 + S * kNhKc + kl] += sum over lane's n of d[m0 + r][n] w[kl][n] (stream S: d [B][N], w row stride NT).
+template <int S>
+__device__ __forceinline__ void noisy_head_bwd_sum(float (&acc)[32], const float* d, const float* w, int N, int NT, int B,
+                                                   int m0, int lane) {
+  for (int n = lane; n < N; n += 32) {
+    float wk[kNhKc];
+#pragma unroll
+    for (int kl = 0; kl < kNhKc; ++kl) wk[kl] = w[kl * NT + n];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const float dv = m0 + r < B ? d[(m0 + r) * N + n] : 0.f;
+#pragma unroll
+      for (int kl = 0; kl < kNhKc; ++kl) acc[r * 8 + S * kNhKc + kl] = fmaf(dv, wk[kl], acc[r * 8 + S * kNhKc + kl]);
+    }
+  }
+}
+
+// One step of the halving butterfly: lanes with bit H set keep outputs [H, 2H) of acc, the others [0, H); each adds its
+// partner's partial sums of the half it keeps.
+template <int H>
+__device__ __forceinline__ void noisy_head_halve(float (&acc)[32], int lane) {
+  const bool up = (lane & H) != 0;
+#pragma unroll
+  for (int o = 0; o < H; ++o) {
+    const float a0 = acc[o], a1 = acc[o + H];
+    acc[o] = (up ? a1 : a0) + __shfl_xor_sync(0xffffffffu, up ? a0 : a1, H);
+  }
+}
+
+__global__ void __launch_bounds__(256) noisy_head_bwd_kernel(const __grid_constant__ NoisyHeadBwdArgs a) {
+  noisy_head_enter();
+  extern __shared__ __align__(16) float nh_smem[];
+  const int N0 = a.N[0], N1 = a.N[1], NT = N0 + N1, B = a.B;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, k0 = blockIdx.x * kNhKc;
+  float* ds = nh_smem;                  // [B][N0] then [B][N1]
+  float* ws = nh_smem + (long long)B * NT;   // [kNhKc][N0 + N1]: stream 0's columns, then stream 1's
+  for (int i = threadIdx.x; i < B * N0; i += blockDim.x) cp_async4(ds + i, a.dout[0] + i);
+  for (int i = threadIdx.x; i < B * N1; i += blockDim.x) cp_async4(ds + B * N0 + i, a.dout[1] + i);
+  // the weights come from HBM: eight of each thread's elements are loaded before any is used, so that their latency
+  // is paid once per 8 x 256 elements (rainbow: 4 x 357, once)
+  for (int i0 = threadIdx.x; i0 < kNhKc * NT; i0 += 8 * 256) {
+    float m_[8], s_[8], e_[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int i = i0 + j * 256;
+      m_[j] = s_[j] = e_[j] = 0.f;
+      if (i < kNhKc * NT) {
+        const int kl = i / NT, c = i % NT, s = c < N0 ? 0 : 1, n = s ? c - N0 : c, k = k0 + kl;
+        const long long wi = (long long)k * a.N[s] + n;
+        m_[j] = a.mu[s][wi]; s_[j] = a.sigma[s][wi]; e_[j] = a.ein[s][k] * a.eout[s][n];
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      if (i0 + j * 256 < kNhKc * NT) ws[i0 + j * 256] = fmaf(s_[j], e_[j], m_[j]);
+  }
+  cp_async_wait_all();
+  __syncthreads();
+  for (int m0 = warp * 4; m0 < B; m0 += 32) {
+    float acc[32];   // acc[r * 8 + s * kNhKc + kl]
+#pragma unroll
+    for (int o = 0; o < 32; ++o) acc[o] = 0.f;
+    noisy_head_bwd_sum<0>(acc, ds, ws, N0, NT, B, m0, lane);
+    noisy_head_bwd_sum<1>(acc, ds + B * N0, ws + N0, N1, NT, B, m0, lane);
+    // halving butterfly: after the step of width H, lane l holds in acc[0 .. H) the partial sums of the outputs whose
+    // bit H matches l's
+    noisy_head_halve<16>(acc, lane); noisy_head_halve<8>(acc, lane); noisy_head_halve<4>(acc, lane);
+    noisy_head_halve<2>(acc, lane); noisy_head_halve<1>(acc, lane);
+    const int r = lane >> 3, s = (lane >> 2) & 1, kl = lane & 3, m = m0 + r, k = k0 + kl;
+    if (m < B) {
+      const long long i = (long long)m * 512 + k;
+      const float v = a.h1[s][i] > 0.f ? acc[0] : 0.f;
+      a.dh1[s][i] = v;
+      if (a.hi[s]) {
+        float hi, lo;
+        tc::split_tf32(v, hi, lo);
+        a.hi[s][i] = hi; a.lo[s][i] = lo;
+      }
+    }
+  }
+}
+
 // epsilon-greedy over q[E][A] (dqn/agent.py:121-127): first maximum wins, as np.argmax / jnp.argmax.
 __global__ void act_select_kernel(const float* __restrict__ q, int A, int E, const float* __restrict__ explore, float eps,
                                   int32_t* __restrict__ actions) {
@@ -2434,14 +2684,88 @@ int launch_dueling_head_bwd(const dz_learner* l, int rows, float* dq, float* dva
   return DZ_OK;
 }
 
+// Rainbow's noisy head of `np` passes over `nimg` <= kNhRows images in one launch (noisy_head_fwd_kernel): the passes
+// that apply one parameter blob form a group, at most two passes each.  Pass i reads nb.h1[passes[i].head] and noise
+// apply passes[i].apply, and writes nb.out / nb.outv of its head pass.  The learner step and dz_test_noisy_head_fwd
+// run this function.
+int launch_noisy_head_fwd(const dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, const float* noise,
+                          void* stream) {
+  const ParamOffsets& o = l->po;
+  const FcNet& f = l->fc;
+  if (f.ns != 2 || !f.noisy || f.dueling_head || nimg < 1 || nimg > kNhRows)
+    return fail(DZ_EINVAL, "noisy head: a two-stream noisy GEMM head over 1..32 images");
+  NoisyHeadFwdArgs a;
+  memset(&a, 0, sizeof(a));
+  const float* blob[2] = {nullptr, nullptr};
+  int ng = 0;
+  for (int i = 0; i < np; ++i) {
+    int g = 0;
+    while (g < ng && !(blob[g] == passes[i].params && a.members[g] < 2)) ++g;
+    if (g == 2) return fail(DZ_EINVAL, "noisy head: more than two groups of passes");
+    if (g == ng) { blob[ng++] = passes[i].params; }
+    const int q = a.members[g]++;
+    const NoiseVecs nz = noise_of(l->cfg, l->d, noise, passes[i].apply);
+    const int hp = passes[i].head;
+    for (int s = 0; s < 2; ++s) {
+      a.x[g][q][s] = nb.h1[hp][s];
+      if ((reinterpret_cast<uintptr_t>(a.x[g][q][s]) & 15) != 0) return fail(DZ_EINVAL, "noisy head: h1 not 16-byte aligned");
+      a.out[g][q][s] = s == 0 ? nb.out[hp] : nb.outv[hp];
+      a.ein[g][q][s] = s == 0 ? nz.a2i : nz.v2i;
+      a.eout[g][q][s] = s == 0 ? nz.a2o : nz.v2o;
+    }
+  }
+  for (int g = 0; g < ng; ++g)
+    for (int s = 0; s < 2; ++s) {
+      a.mu[g][s] = blob[g] + o.w2[s]; a.sigma[g][s] = blob[g] + o.sw2[s];
+      a.bias[g][s] = o.b2[s] < 0 ? nullptr : blob[g] + o.b2[s]; a.sbias[g][s] = blob[g] + o.sb2[s];
+    }
+  a.N[0] = (int)f.out[0]; a.N[1] = (int)f.out[1];
+  a.tiles0 = (int)ceil_div(a.N[0], kNhTile);
+  a.rows = nimg; a.bias_shared = f.shared_bias ? 1 : 0;
+  DZ_CUDA_OK(cudaFuncSetAttribute(noisy_head_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kNhFwdSmem));
+  const dim3 grid((unsigned)(a.tiles0 + ceil_div(a.N[1], kNhTile)), (unsigned)ng);
+  DZ_LAUNCH_NAMED("noisy2_fwd", noisy_head_fwd_kernel, grid, 256, kNhFwdSmem, stream, a);
+  return DZ_OK;
+}
+
+// Dynamic shared memory of noisy_head_bwd_kernel at B rows: every row of dout and the CTA's formed weights.
+size_t noisy_head_bwd_smem(const FcNet& f, int B) { return (size_t)(B + kNhKc) * (f.out[0] + f.out[1]) * sizeof(float); }
+
+// Rainbow's head input gradient through online(s_tm1) (noisy_head_bwd_kernel): dh1 of both streams from dout / doutv,
+// and with hi / lo set their tf32 hi/lo pairs.  backward_fc and dz_test_noisy_head_bwd run this function.
+int launch_noisy_head_bwd(const dz_learner* l, int B, const float* const* dout, const float* params, const float* noise,
+                          const float* const* h1, float* const* dh1, float* const* hi, float* const* lo, void* stream) {
+  const ParamOffsets& o = l->po;
+  const FcNet& f = l->fc;
+  if (f.ns != 2 || !f.noisy || f.dueling_head || B < 1 || B > kNhRows)
+    return fail(DZ_EINVAL, "noisy head: a two-stream noisy GEMM head over 1..32 images");
+  const NoiseVecs nz = noise_of(l->cfg, l->d, noise, 0);
+  NoisyHeadBwdArgs a;
+  memset(&a, 0, sizeof(a));
+  for (int s = 0; s < 2; ++s) {
+    a.dout[s] = dout[s]; a.mu[s] = params + o.w2[s]; a.sigma[s] = params + o.sw2[s];
+    a.h1[s] = h1[s]; a.dh1[s] = dh1[s]; a.hi[s] = hi[s]; a.lo[s] = lo[s];
+    a.N[s] = (int)f.out[s];
+  }
+  a.ein[0] = nz.a2i; a.eout[0] = nz.a2o; a.ein[1] = nz.v2i; a.eout[1] = nz.v2o;
+  a.B = B;
+  const size_t smem = noisy_head_bwd_smem(f, B);
+  if (smem > kMaxDynSmem) return fail(DZ_EINVAL, "noisy head: the input gradient needs more than 227 KB of shared memory");
+  if (smem > 48 * 1024)
+    DZ_CUDA_OK(cudaFuncSetAttribute(noisy_head_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  DZ_LAUNCH_NAMED("noisy2_dgrad", noisy_head_bwd_kernel, (unsigned)(512 / kNhKc), 256, smem, stream, a);
+  return DZ_OK;
+}
+
 // The layers after the torso (FcNet) of `np` passes over `nimg` images: rainbow's and the noisy networks' noisy layers
 // (networks.py:137-178, DESIGN.md §17), the dueling network's streams (§16) and the plain network.  The 3136 -> 512
 // layers of every pass and stream are one grouped launch (skipped with fc1_done: the tensor-core plan wrote h1), then
 // the heads are one dueling head launch or one grouped launch; both GEMM stages split K into nn_partial when the pass
 // has at most split_rows images.  Noisy layers read noise apply passes[i].apply of `noise`; with noise_ld > 0 (one pass
-// only) image m uses its own apply at noise + m * noise_ld.
+// only) image m uses its own apply at noise + m * noise_ld.  With noisy_head, rainbow's head of at most kNhRows images
+// per pass is one launch_noisy_head_fwd instead (the learner step; acting keeps the grouped launch).
 int forward_heads_fc(dz_learner* l, const NetBufs& nb, const Pass* passes, int np, int nimg, const float* noise, void* stream,
-                     bool fc1_done = false, long long noise_ld = 0) {
+                     bool fc1_done = false, long long noise_ld = 0, bool noisy_head = false) {
   const Dims& d = l->d;
   const ParamOffsets& o = l->po;
   const dz_learner_config& c = l->cfg;
@@ -2497,6 +2821,8 @@ int forward_heads_fc(dz_learner* l, const NetBufs& nb, const Pass* passes, int n
     }
     return launch_dueling_head_fwd(l, nimg, np, h1, prm, out, noise_at, noise_ld, stream);
   }
+  if (noisy_head && f.noisy && f.ns == 2 && !noise_ld && nimg <= kNhRows)
+    return launch_noisy_head_fwd(l, nb, passes, np, nimg, noise, stream);
   const bool split_head = nimg <= nb.split_rows;
   for (int i = 0; i < np; ++i) {
     const float* prm = passes[i].params;
@@ -2880,7 +3206,13 @@ int backward_fc(dz_learner* l, const float* noise, void* stream) {
   }
   DZ_TRY(run_tn(f.noisy ? "noisy2_wgrad" : "head_wgrad", gb, l->side.fork(stream, stream)));
   if (f.shared_bias) DZ_LAUNCH(sum_to_scalar_kernel, 1, 128, 0, l->side.tail(stream), bias_terms, d.out, G + o.b2[0]);
-  if (!f.dueling_head) {  // dh1_s = dout_s * W2_s^T, masked by h1_s > 0
+  // rainbow: one launch without split partials, when every row of dout fits in shared memory (not at the widest heads,
+  // e.g. 64 actions x 128 atoms, which keep the split input gradient below)
+  if (!f.dueling_head && f.noisy && ns == 2 && B <= kNhRows && noisy_head_bwd_smem(f, B) <= kMaxDynSmem) {
+    const float* h1[2] = {l->h1[0][0], l->h1[0][1]};
+    DZ_TRY(launch_noisy_head_bwd(l, B, dout, P, noise, h1, l->dh1, hi, lo, stream));
+    hilo_done = true;
+  } else if (!f.dueling_head) {  // dh1_s = dout_s * W2_s^T, masked by h1_s > 0
     // Noisy heads split the reduction 4 ways.  Wide plain heads (c51: 306 outputs, qr-dqn: 1206): with one CTA column
     // per 64 outputs of dh1 the reduction over the head width is a serial chain (measured 24 / 65 us); split it.  The
     // finish of the split partials applies the mask and, on the tensor-core path, writes the tf32 hi/lo pair, which
@@ -3374,7 +3706,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
     if (online_st) passes[np++] = Pass{on, 1, 1, 1};
     if (target_stm1) passes[np++] = Pass{tg, 1, 1, 1};
     passes[np++] = Pass{tg, 2, 2, 2};
-    DZ_TRY(forward_heads_fc(l, learner_bufs(l), passes, np, B, batch->d_noise, stream, um));
+    DZ_TRY(forward_heads_fc(l, learner_bufs(l), passes, np, B, batch->d_noise, stream, um, 0, true));
   }
 
   // ---- loss + gradient wrt the pass-0 head outputs
@@ -4150,6 +4482,33 @@ int dz_test_dueling_head_bwd(dz_learner* l, int32_t rows, float* d_dq, float* d_
   if (!d_h1[0] || !d_h1[1] || !d_dh1[0] || !d_dh1[1] || (!d_hi != !d_lo) || (d_hi && (!d_hi[0] || !d_hi[1] || !d_lo[0] || !d_lo[1])))
     return fail(DZ_EINVAL, "test_dueling_head_bwd: NULL buffer");
   return launch_dueling_head_bwd(l, rows, d_dq, d_dval, d_h1, d_params, d_dh1, d_hi, d_lo, d_noise, stream);
+}
+
+// Test hook: rainbow's noisy head forward (launch_noisy_head_fwd) of a rainbow learner's layout on caller-owned buffers.
+int dz_test_noisy_head_fwd(dz_learner* l, int32_t rows, int32_t np, const float* const* d_h1, const float* const* d_params,
+                           const float* d_noise, float* const* d_out, void* stream) {
+  if (!l || !d_h1 || !d_params || !d_noise || !d_out) return fail(DZ_EINVAL, "test_noisy_head_fwd: NULL argument");
+  if (np < 1 || np > 3) return fail(DZ_EINVAL, "test_noisy_head_fwd: np must be in 1..3");
+  NetBufs nb;
+  memset(&nb, 0, sizeof(nb));
+  Pass passes[3];
+  for (int i = 0; i < np; ++i) {
+    if (!d_h1[2 * i] || !d_h1[2 * i + 1] || !d_params[i] || !d_out[2 * i] || !d_out[2 * i + 1])
+      return fail(DZ_EINVAL, "test_noisy_head_fwd: NULL buffer");
+    nb.h1[i][0] = const_cast<float*>(d_h1[2 * i]); nb.h1[i][1] = const_cast<float*>(d_h1[2 * i + 1]);
+    nb.out[i] = d_out[2 * i]; nb.outv[i] = d_out[2 * i + 1];
+    passes[i] = Pass{d_params[i], 0, i, i};
+  }
+  return launch_noisy_head_fwd(l, nb, passes, np, rows, d_noise, stream);
+}
+
+// Test hook: rainbow's noisy head input gradient (launch_noisy_head_bwd) on caller-owned buffers.
+int dz_test_noisy_head_bwd(dz_learner* l, int32_t rows, const float* const* d_dout, const float* d_params, const float* d_noise,
+                           const float* const* d_h1, float* const* d_dh1, float* const* d_hi, float* const* d_lo, void* stream) {
+  if (!l || !d_dout || !d_params || !d_noise || !d_h1 || !d_dh1) return fail(DZ_EINVAL, "test_noisy_head_bwd: NULL argument");
+  if ((!d_hi != !d_lo)) return fail(DZ_EINVAL, "test_noisy_head_bwd: hi and lo go together");
+  float* none[2] = {nullptr, nullptr};
+  return launch_noisy_head_bwd(l, rows, d_dout, d_params, d_noise, d_h1, d_dh1, d_hi ? d_hi : none, d_lo ? d_lo : none, stream);
 }
 
 // Test hook: IQN's cosine features (launch_iqn_cos) on caller-owned buffers.

@@ -736,6 +736,17 @@ int dz_test_dueling_head_fwd(dz_learner* l, int32_t rows, int32_t np, const floa
 int dz_test_dueling_head_bwd(dz_learner* l, int32_t rows, float* d_dq, float* d_dval, const float* const* d_h1,
                              const float* d_params, const float* d_noise, float* const* d_dh1, float* const* d_hi,
                              float* const* d_lo, void* stream);
+/* Rainbow's noisy head forward of rainbow learner l's layout on caller-owned buffers; tests only.  np in 1..3 passes of
+ * `rows` <= 32 rows: d_h1 host array [np][2] of device [rows][512] (advantage, value stream; 16-byte aligned),
+ * d_params[i] a parameter blob (passes with the same blob share its weight tiles), pass i's noise apply at apply i of
+ * d_noise, d_out host array [np][2] of device [rows][A * atoms] and [rows][atoms]. */
+int dz_test_noisy_head_fwd(dz_learner* l, int32_t rows, int32_t np, const float* const* d_h1, const float* const* d_params,
+                           const float* d_noise, float* const* d_out, void* stream);
+/* Rainbow's noisy head input gradient on caller-owned buffers; tests only.  d_dout host array of 2 ([rows][A * atoms],
+ * [rows][atoms]), the head of d_params through noise apply 0 of d_noise; writes d_dh1[s] [rows][512] masked by
+ * d_h1[s] > 0 and, when d_hi / d_lo (host arrays of 2, or NULL) are given, the tf32 hi/lo pair of each dh1. */
+int dz_test_noisy_head_bwd(dz_learner* l, int32_t rows, const float* const* d_dout, const float* d_params, const float* d_noise,
+                           const float* const* d_h1, float* const* d_dh1, float* const* d_hi, float* const* d_lo, void* stream);
 /* IQN's cosine features on caller-owned buffers; tests only: d_out [rows][latent] = cos(fl(fl((j + 1) pi_f) tau_r)) of
  * d_taus [rows]. */
 int dz_test_iqn_cos(const float* d_taus, int64_t rows, int32_t latent, float* d_out, void* stream);
