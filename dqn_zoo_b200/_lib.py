@@ -60,7 +60,7 @@ class LearnerConfig(C.Structure):
               ('adam_b1', f32), ('adam_b2', f32), ('max_global_grad_norm', f32), ('munchausen_alpha', f32),
               ('entropy_temperature', f32), ('log_policy_clip', f32), ('num_fractions', i32),
               ('fraction_learning_rate', f32), ('fraction_opt_eps', f32), ('fraction_rms_decay', f32), ('dueling', i32),
-              ('noisy', i32), ('random_shift_pad', i32)]
+              ('noisy', i32), ('random_shift_pad', i32), ('prioritized', i32)]
 
   def __init__(self, **fields):
     # the loss hyperparameters start at the reference's values instead of 0, which the library rejects for vmax, and

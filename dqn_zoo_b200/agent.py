@@ -85,7 +85,8 @@ def _seed_of(rng_key) -> int:
 
 
 class _DeviceAgent(parts.Agent):
-  """Shared machinery; subclasses set KIND / PRIORITIZED and mirror the reference constructors."""
+  """Shared machinery; subclasses set KIND and mirror the reference constructors.  PRIORITIZED is True for
+  PrioritizedDqn and Rainbow; any other agent takes it from its replay's `prioritized` (DESIGN.md §19)."""
 
   KIND = 'dqn'
   PRIORITIZED = False
@@ -102,6 +103,8 @@ class _DeviceAgent(parts.Agent):
                        % (np.asarray(sample_network_input).shape, network.obs_shape))
     self._preprocessor = preprocessor
     self._replay = replay
+    # on a prioritized replay every agent adds at max_seen_priority and learns by priority (DESIGN.md §19)
+    self.PRIORITIZED = type(self).PRIORITIZED or bool(replay.prioritized)
     self._transition_accumulator = transition_accumulator
     self._batch_size = batch_size
     self._exploration_epsilon = exploration_epsilon
@@ -112,7 +115,7 @@ class _DeviceAgent(parts.Agent):
     self._host_rng = np.random.RandomState(self._seed % (1 << 32))
     self._learner = learner_lib.Learner(network, batch_size=batch_size, optimizer=optimizer,
                                         grad_error_bound=grad_error_bound, huber_param=huber_param,
-                                        random_shift_pad=random_shift_pad, **munchausen)
+                                        random_shift_pad=random_shift_pad, prioritized=self.PRIORITIZED, **munchausen)
     self._learner.init_params(seed=self._seed % (1 << 31))      # network.init + target = online
     self._action = None
     self._frame_t = -1
@@ -179,6 +182,23 @@ class _DeviceAgent(parts.Agent):
   @property
   def learner(self) -> learner_lib.Learner:
     return self._learner
+
+  @property
+  def importance_sampling_exponent(self) -> float:
+    """The prioritized replay's importance-sampling exponent at its current step; AttributeError on a uniform one."""
+    self._need_prioritized('importance_sampling_exponent')
+    return self._replay.importance_sampling_exponent
+
+  @property
+  def max_seen_priority(self) -> float:
+    """The largest priority the learner has written (new transitions take it; a synchronising read); AttributeError on
+    a uniform replay."""
+    self._need_prioritized('max_seen_priority')
+    return float(self._learner.max_seen_priority.item())
+
+  def _need_prioritized(self, what):
+    if not self.PRIORITIZED:
+      raise AttributeError('%s needs an agent on a prioritized replay' % what)
 
   def get_state(self) -> Mapping[str, Any]:
     """dqn/agent.py:210-220 / rainbow/agent.py:224-235: same keys."""
@@ -253,8 +273,9 @@ class _DeviceAgent(parts.Agent):
         held.append(t)
       blobs[name] = t
     state = {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'dueling': bool(L.net.dueling),
-             'noisy': bool(L.net.noisy), 'random_shift_pad': L.random_shift_pad, 'param_count': L.plan.param_count,
-             'opt_state_floats': L.plan.opt_state_floats, 'host_rng': self._host_rng.get_state(), 'seed': self._seed,
+             'noisy': bool(L.net.noisy), 'random_shift_pad': L.random_shift_pad, 'prioritized': self.PRIORITIZED,
+             'param_count': L.plan.param_count, 'opt_state_floats': L.plan.opt_state_floats,
+             'host_rng': self._host_rng.get_state(), 'seed': self._seed,
              'jax_key': None if getattr(self, '_jax_key', None) is None else self._jax_key.copy(),
              'frame_t': self._frame_t}
     replay_files = replay_lib._replay_files(self._replay, snapshot, held)
@@ -282,12 +303,14 @@ class _DeviceAgent(parts.Agent):
     except (OSError, pickle.UnpicklingError, EOFError) as e:
       raise ValueError('%s is not a readable agent checkpoint: %s' % (directory, e)) from e
     L = self._learner
-    # checkpoints written before the dueling network, noisy networks or random-shift augmentation existed have no
-    # 'dueling' / 'noisy' / 'random_shift_pad' key: they hold the plain network, trained without augmentation
-    ck.validate(dict({'dueling': False, 'noisy': False, 'random_shift_pad': 0}, **state),
+    # checkpoints written before the dueling network, noisy networks, random-shift augmentation or prioritized replay
+    # for every kind existed have no 'dueling' / 'noisy' / 'random_shift_pad' / 'prioritized' key: they hold the plain
+    # network, trained without augmentation, on the replay of the kind (prioritized for prioritized and rainbow only)
+    ck.validate(dict({'dueling': False, 'noisy': False, 'random_shift_pad': 0,
+                      'prioritized': type(self).PRIORITIZED}, **state),
                 {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'dueling': bool(L.net.dueling),
-                 'noisy': bool(L.net.noisy), 'random_shift_pad': L.random_shift_pad, 'param_count': L.plan.param_count,
-                 'opt_state_floats': L.plan.opt_state_floats}, directory)
+                 'noisy': bool(L.net.noisy), 'random_shift_pad': L.random_shift_pad, 'prioritized': self.PRIORITIZED,
+                 'param_count': L.plan.param_count, 'opt_state_floats': L.plan.opt_state_floats}, directory)
     blobs = {}
     for name in self._CHECKPOINT_BLOBS:
       path = os.path.join(directory, name + '.npy')
@@ -460,8 +483,8 @@ class DoubleQ(Dqn):
 
 
 class Munchausen(_DeviceAgent):
-  """Munchausen DQN (Vieillard, Pietquin & Geist, NeurIPS 2020; DESIGN.md §13): dqn's constructor, network, uniform
-  replay and epsilon-greedy acting, with the soft target r + alpha clip(tau log pi(a_tm1|s_tm1), l0, 0) +
+  """Munchausen DQN (Vieillard, Pietquin & Geist, NeurIPS 2020; DESIGN.md §13): dqn's constructor, network, replay
+  and epsilon-greedy acting, with the soft target r + alpha clip(tau log pi(a_tm1|s_tm1), l0, 0) +
   discount sum_a pi(a|s_t) (q(s_t, a) - tau log pi(a|s_t)) of the target network's softmax policy pi.  The defaults
   of `munchausen_alpha`, `entropy_temperature` (tau) and `log_policy_clip` (l0) are the paper's Atari values."""
   KIND = 'munchausen'
@@ -487,14 +510,6 @@ class PrioritizedDqn(_DeviceAgent):
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
                 grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
-
-  @property
-  def importance_sampling_exponent(self) -> float:
-    return self._replay.importance_sampling_exponent
-
-  @property
-  def max_seen_priority(self) -> float:
-    return float(self._learner.max_seen_priority.item())
 
 
 class C51(_DeviceAgent):
@@ -540,14 +555,6 @@ class Rainbow(_DeviceAgent):
                 None, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
                 use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
 
-  @property
-  def importance_sampling_exponent(self) -> float:
-    return self._replay.importance_sampling_exponent
-
-  @property
-  def max_seen_priority(self) -> float:
-    return float(self._learner.max_seen_priority.item())
-
 
 class Iqn(_DeviceAgent):
   """iqn/agent.py:133-340."""
@@ -580,7 +587,7 @@ class Iqn(_DeviceAgent):
 
 class MunchausenIqn(_DeviceAgent):
   """Munchausen-IQN (Vieillard, Pietquin & Geist, NeurIPS 2020; DESIGN.md §14): Iqn's constructor (without
-  `jax_prng_taus`: no reference key chain pins this agent's taus), network, taus, uniform replay and epsilon-greedy
+  `jax_prng_taus`: no reference key chain pins this agent's taus), network, taus, replay and epsilon-greedy
   acting, with the soft quantile targets y_j = r + alpha clip(tau log pi(a_tm1|s_tm1), l0, 0) +
   discount sum_a pi(a|s_t) (zbar_j(s_t, a) - tau log pi(a|s_t)) of the target network's softmax policy pi over its
   mean quantiles.  The defaults of `munchausen_alpha`, `entropy_temperature` (tau) and `log_policy_clip` (l0) are the
@@ -606,8 +613,8 @@ class Fqf(_DeviceAgent):
   the tau sample counts and `jax_prng_taus` (its taus are not drawn: a fraction proposal layer computes N fractions from
   the torso features inside every step and every action selection), plus `num_fractions` (which must match the
   NetworkSpec's) and the fraction layer's centred RMSProp (`fraction_learning_rate`, `fraction_opt_eps`,
-  `fraction_rms_decay`).  `optimizer` covers every other tensor (default: Adam at lr 5e-5, eps 0.01 / 32).  Uniform
-  replay and epsilon-greedy acting on Q(s, a) = sum_i w_i Z(s, a, tau_hat_i)."""
+  `fraction_rms_decay`).  `optimizer` covers every other tensor (default: Adam at lr 5e-5, eps 0.01 / 32).
+  Epsilon-greedy acting on Q(s, a) = sum_i w_i Z(s, a, tau_hat_i)."""
   KIND = 'fqf'
 
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,

@@ -58,6 +58,11 @@ constexpr bool dueling_allowed(int kind) {
 // launches asks the first; every decision about noise asks the second.
 inline bool two_streams(const dz_learner_config& c) { return c.kind == DZ_RAINBOW || c.dueling != 0; }
 inline bool noisy_net(const dz_learner_config& c) { return c.kind == DZ_RAINBOW || c.noisy != 0; }
+// Whether the loss section writes priorities and keeps the running max-seen priority (DESIGN.md §19): prioritized and
+// rainbow always, any other kind with the config's prioritized field set.
+inline bool writes_priorities(const dz_learner_config& c) {
+  return c.kind == DZ_PRIORITIZED || c.kind == DZ_RAINBOW || c.prioritized != 0;
+}
 
 // ------------------------------------------------------------------------------------------------
 // Parameter layout (canonical names; haiku layouts) — must match oracle/learner_oracle.py:param_shapes
@@ -337,6 +342,7 @@ static int validate(const dz_learner_config& c) {
   if (c.dueling && !dueling_allowed(c.kind))
     return fail(DZ_EINVAL, "dueling: only dqn, double_q, prioritized and munchausen take the dueling network");
   if (c.noisy != 0 && c.noisy != 1) return fail(DZ_EINVAL, "noisy must be 0 or 1");
+  if (c.prioritized != 0 && c.prioritized != 1) return fail(DZ_EINVAL, "prioritized must be 0 or 1");
   if (c.noisy && c.kind == DZ_RAINBOW) return fail(DZ_EINVAL, "noisy: rainbow's network is noisy already");
   if (c.noisy && !dueling_allowed(c.kind))
     return fail(DZ_EINVAL, "noisy: only dqn, double_q, prioritized and munchausen take noisy layers");
@@ -895,7 +901,7 @@ __global__ void __launch_bounds__(64) loss_q_kernel(LossArgs L) {
 
 // munchausen: one warp per example, lane a holding action a of the target network's passes on s_tm1 (out1) and s_t
 // (out2); the target of DESIGN.md §13, then dqn's clip_gradient + l2_loss on td = target - q(s_tm1, a_tm1).  The
-// per-example value is the loss 0.5 td^2.
+// per-example value is the loss 0.5 td^2; the priority is |td|, the dqn family's rule on the soft target.
 __global__ void __launch_bounds__(128) loss_munchausen_kernel(LossArgs L, float alpha, float tau, float l0) {
   dz::pdl_enter();
   const int lane = threadIdx.x & 31;
@@ -919,6 +925,7 @@ __global__ void __launch_bounds__(128) loss_munchausen_kernel(LossArgs L, float 
   if (lane == 0) {
     const float loss = 0.5f * td * td;
     L.per_example[b] = loss;
+    if (L.priorities) L.priorities[b] = fabsf(td);
     L.loss_terms[b] = w * loss;
   }
 }
@@ -1119,6 +1126,7 @@ __device__ __forceinline__ void quantile_huber_tail(const LossArgs& L, int b, in
   total = block_sum(total, red);
   if (tid == 0) {
     L.per_example[b] = total;
+    if (L.priorities) L.priorities[b] = fminf(fmaxf(fabsf(total), 0.f), 100.f);   // rainbow's rule, DESIGN.md §19
     L.loss_terms[b] = w * total;
   }
 }
@@ -1188,6 +1196,7 @@ __global__ void __launch_bounds__(256) loss_quantile_kernel(LossArgs L) {
   total = block_sum(total, red);
   if (tid == 0) {
     L.per_example[b] = total;
+    if (L.priorities) L.priorities[b] = fminf(fmaxf(fabsf(total), 0.f), 100.f);   // rainbow's rule, DESIGN.md §19
     L.loss_terms[b] = w * total;
   }
 }
@@ -1314,7 +1323,7 @@ struct FqfLossArgs {
 // sum_i w'_i Zbar(s_t, a, tau_hat'_i), one thread per action, first maximum; (2) the targets y_j = r + discount
 // Zbar(s_t, a*, tau_hat_j); (3) the fraction gradient at a_tm1 chained to dlogits (fqf_dlogits, thread 0); (4) IQN's
 // quantile-Huber term of online(s_tm1)'s N samples at a_tm1 against the targets and dout in IQN's layout
-// (quantile_huber_tail).  The per-example value is the quantile loss.
+// (quantile_huber_tail).  The per-example value, and the priority's source, is the quantile loss.
 __global__ void __launch_bounds__(256) loss_fqf_kernel(LossArgs L, FqfLossArgs f) {
   dz::pdl_enter();
   extern __shared__ float sm[];
@@ -3483,16 +3492,16 @@ int run_optimizer(dz_learner* l, float* user_norm, bool apply, void* stream) {
 }
 
 // The loss section of a learner step: the agent kind's loss kernel on `stream`, then loss_mean_kernel (the scalar loss,
-// and rainbow's running max priority when max_seen is given).  L carries the buffers: head outputs, batch, outputs and
-// loss_terms; every field that follows from the configuration (sizes, vmax, bound, kappa, whether priorities are
-// written) is set here.  With `side`, loss_mean_kernel runs on the side stream forked after the loss kernel and
+// and the running max priority when max_seen is given and the learner writes priorities).  L carries the buffers: head
+// outputs, batch, outputs and loss_terms; every field that follows from the configuration (sizes, vmax, bound, kappa,
+// whether priorities are written: writes_priorities) is set here.  With `side`, loss_mean_kernel runs on the side stream forked after the loss kernel and
 // *mean_stream receives it; without, everything runs on `stream`.  dz_test_loss and dz_test_loss_fqf run this same
 // function.
 int launch_loss(const dz_learner_config& c, LossArgs& L, int B, void* stream, SideStream* side, float* d_loss, float* max_seen,
                 void** mean_stream, const FqfLossArgs* fqf = nullptr) {
   L.kind = c.kind; L.B = B; L.A = c.num_actions; L.atoms = c.num_atoms;
   L.vmax = c.vmax; L.bound = c.grad_error_bound; L.kappa = c.huber_param;
-  if (!(c.kind == DZ_RAINBOW || c.kind == DZ_PRIORITIZED)) L.priorities = nullptr;
+  if (!writes_priorities(c)) L.priorities = nullptr;
   if (c.kind == DZ_DQN || c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED) {
     DZ_LAUNCH(loss_q_kernel, B, 64, 0, stream, L);
   } else if (c.kind == DZ_MUNCHAUSEN) {
@@ -3842,6 +3851,9 @@ int dz_learner_update(dz_learner* l, const dz_batch* batch, const dz_update_outp
 
 int dz_learner_learn(dz_learner* l, const dz_replay_view* replay, int32_t prioritized, const dz_learn_io* io, void* stream) {
   const int B = l->B;
+  if (prioritized && !writes_priorities(l->cfg))
+    return fail(DZ_EINVAL, "prioritized learn needs a learner that writes priorities (prioritized, rainbow, or "
+                           "dz_learner_config.prioritized = 1)");
   BatchExtras ex{l->rows_sample[0], l->rows_sample[1], l->s_a, l->s_r, l->s_d, prioritized ? l->s_w : nullptr, 1};
   if (replay->obs_bytes != (int64_t)l->d.H * l->d.W * l->d.C) return fail(DZ_EINVAL, "replay observation size does not match the network");
   if (replay->d_planes) {
@@ -4370,7 +4382,7 @@ static int test_loss_section(const dz_learner_config* cfg, int32_t B, const floa
   if (!d_a_tm1 || !d_r_t || !d_discount_t || !d_dout || !d_per_example || !d_loss_terms || !d_loss)
     return fail(DZ_EINVAL, "test_loss: NULL buffer");
   if (draws_taus(c.kind) && !d_taus) return fail(DZ_EINVAL, "test_loss: iqn needs taus[B][tau_samples_s_tm1]");
-  if ((rb || c.kind == DZ_PRIORITIZED) && !d_priorities) return fail(DZ_EINVAL, "test_loss: this kind writes priorities");
+  if (writes_priorities(c) && !d_priorities) return fail(DZ_EINVAL, "test_loss: this learner writes priorities");
   LossArgs L;
   memset(&L, 0, sizeof(L));
   L.out0 = d_out[0]; L.out1 = d_out[1]; L.out2 = d_out[2];

@@ -217,7 +217,8 @@ class Learner:
   def __init__(self, net: NetworkSpec, batch_size: int = 32, optimizer: Optional[OptimizerSpec] = None,
                grad_error_bound: float = 1.0 / 32, huber_param: float = 1.0, munchausen_alpha: float = 0.9,
                entropy_temperature: float = 0.03, log_policy_clip: float = -1.0, fraction_learning_rate: float = 2.5e-9,
-               fraction_opt_eps: float = 1e-5, fraction_rms_decay: float = 0.95, device=None, random_shift_pad: int = 0):
+               fraction_opt_eps: float = 1e-5, fraction_rms_decay: float = 0.95, device=None, random_shift_pad: int = 0,
+               prioritized: bool = False):
     """`munchausen_alpha`, `entropy_temperature` (tau) and `log_policy_clip` (l0) are Munchausen DQN's and
     Munchausen-IQN's (DESIGN.md §13, §14, defaults the paper's Atari values); the library rejects tau <= 0, alpha < 0,
     l0 > 0 and non-finite values for those kinds, and the other kinds ignore them.  `fraction_learning_rate`,
@@ -225,7 +226,9 @@ class Learner:
     library rejects a negative or non-finite rate, eps <= 0 and a decay outside [0, 1) for fqf.  `random_shift_pad` p > 0
     turns on random-shift augmentation of the update (DrQ; DESIGN.md §18): every update reads s_tm1 and s_t shifted by
     the [B, 4] int32 `shifts`, which `generate_randomness` draws; acting never sees a shift.  ValueError unless p is an
-    integer in [0, 16] and less than min(H, W)."""
+    integer in [0, 16] and less than min(H, W).  `prioritized=True` makes every update fill `.priorities` by the kind's
+    rule and lets `learn` sample by priority and write them back (DESIGN.md §19); prioritized and rainbow do so
+    whatever it says."""
     check_network(net)
     random_shift_pad = check_random_shift_pad(random_shift_pad, net.obs_shape)
     if not torch.cuda.is_available():
@@ -252,6 +255,7 @@ class Learner:
     cfg.dueling = 1 if net.dueling else 0
     cfg.noisy = 1 if net.noisy else 0
     cfg.random_shift_pad = random_shift_pad
+    cfg.prioritized = 1 if prioritized else 0
     self.random_shift_pad = random_shift_pad
     self.cfg = cfg
     plan = _lib.LearnerPlan()

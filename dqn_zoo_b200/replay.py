@@ -1283,6 +1283,8 @@ class TransitionReplay(_Replay):
   layout is the caller's choice because the replay cannot tell at construction whether its observations are frame
   stacks, and the pool has to be sized up front."""
 
+  prioritized = False   # whether an agent adds with priorities and learns by them from this replay
+
   def __init__(self, capacity: int, structure, random_state: np.random.RandomState, encoder=None, decoder=None,
                frame_dedup: bool = False, frame_capacity: Optional[int] = None):
     super().__init__(_check_codec(encoder, decoder), capacity, structure, random_state,
@@ -1593,6 +1595,8 @@ def _restore_rows(rep, storage):
 
 class PrioritizedTransitionReplay(_Replay):
   """Proportional prioritized replay (`replay.py:654-768`), storage + sum tree in HBM."""
+
+  prioritized = True    # as TransitionReplay.prioritized
 
   def __init__(self, capacity: int, structure, priority_exponent: float,
                importance_sampling_exponent: Callable[[int], float], uniform_sample_probability: float,

@@ -372,6 +372,20 @@ typedef struct dz_learner_config {
    * p and cropped back to H x W.  Every pass over s_tm1 reads the one shifted s_tm1 and every pass over s_t the one
    * shifted s_t; acting never sees a shift. */
   int32_t random_shift_pad;
+  /* Prioritized experience replay (Schaul et al., ICLR 2016; DESIGN.md §19) for any kind and network option: 0 or 1
+   * (DZ_EINVAL otherwise).  1: every update writes dz_update_outputs.d_priorities and, in dz_learner_learn, updates
+   * d_max_seen_priority as max(old, batch max).  0, as a zero-filled tail leaves it: a learner of any kind but
+   * prioritized and rainbow writes no priorities, and dz_learner_learn(prioritized = 1) on it returns DZ_EINVAL.
+   * DZ_PRIORITIZED and DZ_RAINBOW write them whatever the field says.  The priority of example b, from its UNWEIGHTED
+   * loss:
+   *   dqn, double_q, prioritized   |td|
+   *   munchausen                   |td| against its soft target (not the per-example 0.5 td^2)
+   *   c51, rainbow                 clip(|cross entropy|, 0, 100)
+   *   qrdqn, iqn, munchausen_iqn,  clip(|quantile Huber loss|, 0, 100), the per-example value (fqf: the quantile
+   *   fqf                          loss at the proposed fractions, not the fraction loss)
+   * The importance weights d_weights scale each example's loss term and its gradient (fqf: the fraction loss's too)
+   * whatever the field says. */
+  int32_t prioritized;
 } dz_learner_config;
 
 typedef struct dz_learner_plan {
@@ -427,7 +441,9 @@ typedef struct dz_update_outputs {
   float* d_loss;         /* [1] scalar loss (mean of weighted per-example losses) */
   float* d_per_example;  /* [B] per-example losses (c51/rainbow/qr/iqn) or td errors (dqn family) */
   float* d_priorities;   /* [B] new priorities: rainbow clip(|loss|,0,100) (rainbow/agent.py:194),
-                                prioritized |td| (prioritized/agent.py:201); else untouched; may be NULL */
+                                prioritized |td| (prioritized/agent.py:201), any other kind with
+                                dz_learner_config.prioritized = 1 by the rule table there; else untouched;
+                                may be NULL */
   float* d_grad_norm;    /* [1] global gradient norm before clipping; may be NULL */
 } dz_update_outputs;
 
@@ -438,7 +454,9 @@ int dz_learner_update(dz_learner* l, const dz_batch* batch, const dz_update_outp
 
 /* The whole `_learn()` (rainbow/agent.py:181-198) in one enqueue: sample -> (rows addressed in
  * place) -> update -> priority write-back.  `d_max_seen_priority` ([1] float32, device) is
- * updated as max(old, batch max) (rainbow/agent.py:196-197). */
+ * updated as max(old, batch max) (rainbow/agent.py:196-197) by a learner that writes priorities.
+ * `prioritized` = 1 needs such a learner (prioritized, rainbow, or dz_learner_config.prioritized = 1;
+ * DZ_EINVAL otherwise, before anything is enqueued) and update_out.d_priorities. */
 typedef struct dz_learn_io {
   dz_sample_inputs sample_in;
   dz_sample_outputs sample_out;
@@ -685,16 +703,17 @@ int dz_test_fqf_example(const float* logits, const float* F_tau, const float* F_
  * q_a = v + (adv_a - m) with m = (sum_a adv_a) / A to out[0, A), dadv_a = dq_a - (sum_a dq_a) / A to out[A, 2A) and
  * dval = sum_a dq_a to out[2A].  Sums run in action order.  DZ_EINVAL for A outside [1, 64] or a NULL buffer; tests only. */
 int dz_test_dueling_example(const float* adv, float v, const float* dq, int32_t A, float* out);
-/* The loss section of a learner step (the agent kind's loss kernel, then the scalar loss and rainbow's running max
- * priority) on caller-owned device buffers, all enqueued on `stream`; tests only.  cfg is validated as
+/* The loss section of a learner step (the agent kind's loss kernel, then the scalar loss and the running max priority)
+ * on caller-owned device buffers, all enqueued on `stream`; tests only.  cfg is validated as
  * dz_learner_create does, with batch = B and its observation fields replaced by a legal geometry.  d_out[p]: the head
  * outputs of pass p (0 online(s_tm1); dqn: 2 target(s_t) is also the selector; double_q / prioritized: 1 online(s_t)
  * selects; c51: [B][A][K] logits, 2 is target(s_t) and selects; rainbow: advantages [B][A][K] with d_val[p] the value
  * streams [B][K], for online(s_tm1), online(s_t), target(s_t); qrdqn: [B][N][A]; iqn: [B][N_tm1 | N_policy | N_t][A];
  * munchausen / munchausen_iqn: 1 is target(s_tm1)).  d_weights: importance weights [B] or NULL; d_taus: the s_tm1
  * taus [B][N_tm1] (iqn, munchausen_iqn).  Writes d_dout (the gradient wrt pass 0; rainbow: advantages, with d_dval the
- * value stream), d_per_example, d_priorities (prioritized, rainbow), d_loss_terms [B], d_loss [1] and, when d_max_seen
- * is given for rainbow, the running max priority.  fqf's loss needs its fraction buffers: dz_test_loss_fqf. */
+ * value stream), d_per_example, d_priorities (required from a configuration that writes priorities: prioritized,
+ * rainbow, or cfg->prioritized = 1), d_loss_terms [B], d_loss [1] and, when d_max_seen is given to such a
+ * configuration, the running max priority.  fqf's loss needs its fraction buffers: dz_test_loss_fqf. */
 int dz_test_loss(const dz_learner_config* cfg, int32_t B, const float* const* d_out, const float* const* d_val,
                  const int32_t* d_a_tm1, const float* d_r_t, const float* d_discount_t, const float* d_weights,
                  const float* d_taus, float* d_dout, float* d_dval, float* d_per_example, float* d_priorities,
@@ -703,7 +722,8 @@ int dz_test_loss(const dz_learner_config* cfg, int32_t B, const float* const* d_
  * online(s_tm1) at tau_hat [B][N][A], d_out[1] online(s_tm1) at tau_1..tau_N [B][N][A] (the last row, tau_N = 1, is not
  * read), d_out[2] target(s_t) at [tau_hat' | tau_hat] [B][2N][A]; d_tau_hat [B][N], d_w_t the interval weights of
  * s_t's proposal [B][N], d_q_tm1 the fractions of s_tm1's [B][N].  Writes d_dout [B][N][A], d_dlogits [B][N],
- * d_per_example, d_loss_terms [B] and d_loss [1]. */
+ * d_per_example, d_loss_terms [B] and d_loss [1].  It takes no priority buffer, so by dz_test_loss's rule a cfg with
+ * prioritized = 1 is DZ_EINVAL here; fqf's priorities are those of a learner step (dz_learner_update). */
 int dz_test_loss_fqf(const dz_learner_config* cfg, int32_t B, const float* const* d_out, const int32_t* d_a_tm1,
                      const float* d_r_t, const float* d_discount_t, const float* d_weights, const float* d_tau_hat,
                      const float* d_w_t, const float* d_q_tm1, float* d_dout, float* d_dlogits, float* d_per_example,

@@ -138,7 +138,8 @@ def bench_driver(game='catch'):
 
 
 # -- learning ----------------------------------------------------------------------------------------------------------
-def learning_agent(seed, train_frames, kind='dqn', num_actions=6, dueling=False, noisy=False, random_shift_pad=0):
+def learning_agent(seed, train_frames, kind='dqn', num_actions=6, dueling=False, noisy=False, random_shift_pad=0,
+                   prioritized=False, n_step=None):
   """dqn at the reference's hyper-parameters but for a faster schedule: replay of 100k transitions, learning from 10k,
   epsilon 1 -> 0.01 over the first quarter of the frames, target sync every 8000 frames.  `kind='rainbow'`: the same
   schedule with rainbow's prioritized replay (exponent 0.5, importance exponent 0.4 -> 1 over the run), 3-step returns,
@@ -146,7 +147,8 @@ def learning_agent(seed, train_frames, kind='dqn', num_actions=6, dueling=False,
   target.  `dueling`: the dueling network (DESIGN.md §16) in place of dqn's fc1 / head.  `noisy`: noisy networks
   (DESIGN.md §17) with an epsilon schedule that is zero throughout, so that the agent explores through its noise alone
   (NoisyNet-DQN for dqn).  `random_shift_pad`: random-shift augmentation of every learner step (DESIGN.md §18); with
-  kind='double_q' and `dueling` that is DrQ-epsilon's agent on this schedule."""
+  kind='double_q' and `dueling` that is DrQ-epsilon's agent on this schedule.  `prioritized`: any kind on rainbow's
+  prioritized replay (DESIGN.md §19).  `n_step`: the returns' step count (None: 3 for rainbow, 1 otherwise)."""
   from dqn_zoo_b200 import agent as ag
   from dqn_zoo_b200 import learner as dl
   from dqn_zoo_b200 import parts
@@ -158,28 +160,35 @@ def learning_agent(seed, train_frames, kind='dqn', num_actions=6, dueling=False,
                                                                                           noisy=noisy),
                 optimizer=None, batch_size=32, min_replay_capacity_fraction=min_fill / capacity, learn_period=16,
                 target_network_update_period=8000, rng_key=[0, seed + 1], random_shift_pad=random_shift_pad)
-  if kind == 'rainbow':
+  n = dr.NStepTransitionAccumulator(n_step or (3 if kind == 'rainbow' else 1))
+  if kind == 'rainbow' or prioritized:
     importance = parts.LinearSchedule(begin_t=min_fill, decay_steps=max(train_frames, 1), begin_value=0.4,
                                       end_value=1.0)
     rep = dr.PrioritizedTransitionReplay(capacity, structure, 0.5, importance, 1e-3, True, rs, frame_dedup=True)
-    return ag.Rainbow(support=np.linspace(-10, 10, 51), transition_accumulator=dr.NStepTransitionAccumulator(3),
-                      replay=rep, **common)
-  rep = dr.TransitionReplay(capacity, structure, rs, frame_dedup=True)
+  else:
+    rep = dr.TransitionReplay(capacity, structure, rs, frame_dedup=True)
+  if kind == 'rainbow':
+    return ag.Rainbow(support=np.linspace(-10, 10, 51), transition_accumulator=n, replay=rep, **common)
   epsilon = parts.LinearSchedule(begin_t=4 * min_fill, decay_steps=max(train_frames // 4, 1), begin_value=1.0,
                                  end_value=0.01)
   if noisy:
     epsilon = lambda t: 0.0
   if kind == 'fqf':   # dqn's schedule, 32 fractions, kappa 1 and the fraction layer's default RMSProp
-    return ag.Fqf(transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep, exploration_epsilon=epsilon,
+    return ag.Fqf(transition_accumulator=n, replay=rep, exploration_epsilon=epsilon,
                   huber_param=1.0, **common)
   if dl.uses_iqn_network(kind):   # iqn / munchausen_iqn: dqn's schedule, iqn's 64 / 64 / 64 taus and kappa 1
-    return ag.AGENTS[kind](transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep,
-                           exploration_epsilon=epsilon, huber_param=1.0, tau_samples_policy=64, tau_samples_s_tm1=64,
+    return ag.AGENTS[kind](transition_accumulator=n, replay=rep, exploration_epsilon=epsilon, huber_param=1.0, tau_samples_policy=64, tau_samples_s_tm1=64,
                            tau_samples_s_t=64, **common)
+  if kind == 'c51':   # dqn's schedule, 51 atoms on [-10, 10]
+    return ag.C51(support=np.linspace(-10, 10, 51), transition_accumulator=n, replay=rep, exploration_epsilon=epsilon,
+                  **common)
+  if kind == 'qrdqn':   # dqn's schedule, 201 quantiles, kappa 1
+    return ag.QrDqn(quantiles=(np.arange(201) + 0.5) / 201, transition_accumulator=n, replay=rep,
+                    exploration_epsilon=epsilon, huber_param=1.0, **common)
   # munchausen: dqn's schedule, the paper's alpha / tau / l0; double_q: dqn's schedule
   agent_cls = {'munchausen': ag.Munchausen, 'double_q': ag.DoubleQ}.get(kind, ag.Dqn)
-  return agent_cls(transition_accumulator=dr.NStepTransitionAccumulator(1), replay=rep, exploration_epsilon=epsilon,
-                   grad_error_bound=1.0 / 32, **common)
+  return agent_cls(transition_accumulator=n, replay=rep, exploration_epsilon=epsilon, grad_error_bound=1.0 / 32,
+                   **common)
 
 
 def evaluate(learner, seed, num_streams=64, game='catch', num_actions=6):
@@ -203,13 +212,13 @@ def evaluate(learner, seed, num_streams=64, game='catch', num_actions=6):
 
 
 def learning_run(train_frames, seed=0, num_streams=32, eval_every=0, log=None, game='catch', num_actions=6,
-                 kind='dqn', dueling=False, noisy=False, random_shift_pad=0):
+                 kind='dqn', dueling=False, noisy=False, random_shift_pad=0, prioritized=False, n_step=None):
   """Trains `learning_agent` (of `kind`, on the dueling network with `dueling`, with noisy layers with `noisy`) from `num_streams` streams of `game` for `train_frames` frames (training episodes are not
   truncated); evaluates every `eval_every` frames (0: at the end only).  Returns [(frames, mean eval return, eval
   episodes, train episode return)]."""
   import run_synthetic
   from dqn_zoo_b200 import agent as ag
-  agent = learning_agent(seed, train_frames, kind, num_actions, dueling, noisy, random_shift_pad)
+  agent = learning_agent(seed, train_frames, kind, num_actions, dueling, noisy, random_shift_pad, prioritized, n_step)
   trainer = ag.VectorTrainer(agent, num_streams=num_streams, rng_key=[0, seed + 4])
   env = make_env(game, num_streams, seed + 5, num_actions)
   loop = run_synthetic.StreamLoop(trainer, env, train_frames, 0)
@@ -228,13 +237,17 @@ def learning_run(train_frames, seed=0, num_streams=32, eval_every=0, log=None, g
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--game', default='catch', choices=['catch', 'breakout', 'pong'])
-  ap.add_argument('--agent', default='dqn', choices=['dqn', 'double_q', 'rainbow', 'munchausen', 'iqn', 'munchausen_iqn', 'fqf'],
+  ap.add_argument('--agent', default='dqn', choices=['dqn', 'double_q', 'c51', 'qrdqn', 'rainbow', 'munchausen', 'iqn',
+                                                       'munchausen_iqn', 'fqf'],
                   help='the agent of the learning curve')
   ap.add_argument('--dueling', action='store_true', help='the learning curve on the dueling network (DESIGN.md §16)')
   ap.add_argument('--noisy', action='store_true',
                   help='the learning curve on noisy networks with a zero epsilon schedule (DESIGN.md §17)')
   ap.add_argument('--random_shift_pad', type=int, default=0,
                   help='the learning curve with random-shift augmentation at pad N (DESIGN.md §18)')
+  ap.add_argument('--prioritized', action='store_true',
+                  help='the learning curve on rainbow\'s prioritized replay, for any agent (DESIGN.md §19)')
+  ap.add_argument('--n_step', type=int, default=None, help='the returns\' step count (default: 3 for rainbow, else 1)')
   ap.add_argument('--parts', default='env,train,eval,driver')
   ap.add_argument('--frames', type=int, default=65536, help='frames per timed window of env_train / env_eval')
   ap.add_argument('--learning', type=int, default=0, help='frames of the learning curve (0: none)')
@@ -259,11 +272,13 @@ def main():
   if a.learning:
     t0 = time.perf_counter()
     learning_run(a.learning, a.seed, eval_every=a.eval_every, game=a.game, kind=a.agent, dueling=a.dueling,
-                 noisy=a.noisy, random_shift_pad=a.random_shift_pad, log=lambda **kw: emit(metric='learning', **_tag(a.game), **({} if a.agent == 'dqn' else
+                 noisy=a.noisy, random_shift_pad=a.random_shift_pad, prioritized=a.prioritized, n_step=a.n_step, log=lambda **kw: emit(metric='learning', **_tag(a.game), **({} if a.agent == 'dqn' else
                                                                               {'agent': a.agent}),
                                        **({'dueling': True} if a.dueling else {}),
                                        **({'noisy': True} if a.noisy else {}),
                                        **({'random_shift_pad': a.random_shift_pad} if a.random_shift_pad else {}),
+                                       **({'prioritized': True} if a.prioritized else {}),
+                                       **({'n_step': a.n_step} if a.n_step else {}),
                                        seed=a.seed, wall_s=round(time.perf_counter() - t0, 1), **kw))
   emit(metric='device_after', **bench_train.device_info())
 

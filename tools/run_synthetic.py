@@ -81,14 +81,14 @@ def build_train_agent(args, random_state, preprocessor):
   from dqn_zoo_b200 import parts
   from dqn_zoo_b200 import replay as replay_lib
   kind = args.agent
-  prioritized = kind in ('prioritized', 'rainbow')
+  prioritized = kind in ('prioritized', 'rainbow') or args.prioritized
   n_step = 3 if kind == 'rainbow' else 1
   structure = replay_lib.Transition(None, None, None, None, None)
   if prioritized:
     schedule = parts.LinearSchedule(begin_t=int(args.min_replay_capacity_fraction * args.replay_capacity),
                                     decay_steps=max(args.num_iterations * args.num_train_frames // 4, 1), begin_value=0.4,
                                     end_value=1.0)
-    replay = replay_lib.PrioritizedTransitionReplay(args.replay_capacity, structure, 0.5 if kind == 'rainbow' else 0.6, schedule,
+    replay = replay_lib.PrioritizedTransitionReplay(args.replay_capacity, structure, 0.6 if kind == 'prioritized' else 0.5, schedule,
                                                     1e-3, True, random_state)
   else:
     replay = replay_lib.TransitionReplay(args.replay_capacity, structure, random_state)
@@ -269,6 +269,9 @@ def parse_args(argv=None):
                        'munchausen only; combines with --dueling')
   ap.add_argument('--random_shift_pad', type=int, default=0,
                   help='random-shift augmentation of every learner step at pad N in [0, 16] (DESIGN.md §18); 0: off')
+  ap.add_argument('--prioritized', action='store_true',
+                  help='prioritized replay for any agent (DESIGN.md §19): rainbow\'s exponent 0.5, importance exponent '
+                       '0.4 -> 1 and uniform-sample probability 1e-3; prioritized and rainbow always use it')
   ap.add_argument('--num_actions', type=int, default=6)
   ap.add_argument('--replay_capacity', type=int, default=20000)
   ap.add_argument('--min_replay_capacity_fraction', type=float, default=0.05)
