@@ -60,7 +60,7 @@ class LearnerConfig(C.Structure):
               ('adam_b1', f32), ('adam_b2', f32), ('max_global_grad_norm', f32), ('munchausen_alpha', f32),
               ('entropy_temperature', f32), ('log_policy_clip', f32), ('num_fractions', i32),
               ('fraction_learning_rate', f32), ('fraction_opt_eps', f32), ('fraction_rms_decay', f32), ('dueling', i32),
-              ('noisy', i32), ('random_shift_pad', i32), ('prioritized', i32)]
+              ('noisy', i32), ('random_shift_pad', i32), ('prioritized', i32), ('cql_alpha', f32)]
 
   def __init__(self, **fields):
     # the loss hyperparameters start at the reference's values instead of 0, which the library rejects for vmax, and
@@ -85,7 +85,8 @@ class Batch(C.Structure):
 
 
 class UpdateOutputs(C.Structure):
-  _fields_ = [('d_loss', vp), ('d_per_example', vp), ('d_priorities', vp), ('d_grad_norm', vp)]
+  # d_regularizer last, so that positional UpdateOutputs(loss, per_example, priorities, grad_norm) leaves it NULL
+  _fields_ = [('d_loss', vp), ('d_per_example', vp), ('d_priorities', vp), ('d_grad_norm', vp), ('d_regularizer', vp)]
 
 
 class ResampleAxis(C.Structure):   # struct dz_resample_axis
@@ -201,6 +202,7 @@ _SIGNATURES = {
     'dz_test_munchausen_iqn_example': (i32, [vp, vp, i32, i32, i32, i32, f32, f32, f32, f32, f32, vp]),
     'dz_test_fqf_example': (i32, [vp, vp, vp, i32, f32, vp]),
     'dz_test_dueling_example': (i32, [vp, f32, vp, i32, vp]),
+    'dz_test_cql_example': (i32, [vp, i32, i32, f32, vp]),
     'dz_test_loss': (i32, [C.POINTER(LearnerConfig), i32, C.POINTER(vp), C.POINTER(vp), vp, vp, vp, vp, vp, vp, vp, vp, vp,
                            vp, vp, vp, vp]),
     'dz_test_loss_fqf': (i32, [C.POINTER(LearnerConfig), i32, C.POINTER(vp), vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,

@@ -95,7 +95,7 @@ class _DeviceAgent(parts.Agent):
   def _setup(self, preprocessor, sample_network_input, network: NetworkSpec, optimizer: Optional[OptimizerSpec],
              transition_accumulator, replay, batch_size, exploration_epsilon, min_replay_capacity_fraction,
              learn_period, target_network_update_period, rng_key, grad_error_bound=1.0 / 32, huber_param=1.0,
-             use_cuda_graph=True, random_shift_pad=0, **munchausen):
+             use_cuda_graph=True, random_shift_pad=0, cql_alpha=0.0, **munchausen):
     if network.kind != self.KIND:
       raise ValueError('network spec kind %r does not match agent %r' % (network.kind, self.KIND))
     if sample_network_input is not None and tuple(np.asarray(sample_network_input).shape) != tuple(network.obs_shape):
@@ -115,7 +115,8 @@ class _DeviceAgent(parts.Agent):
     self._host_rng = np.random.RandomState(self._seed % (1 << 32))
     self._learner = learner_lib.Learner(network, batch_size=batch_size, optimizer=optimizer,
                                         grad_error_bound=grad_error_bound, huber_param=huber_param,
-                                        random_shift_pad=random_shift_pad, prioritized=self.PRIORITIZED, **munchausen)
+                                        random_shift_pad=random_shift_pad, prioritized=self.PRIORITIZED,
+                                        cql_alpha=cql_alpha, **munchausen)
     self._learner.init_params(seed=self._seed % (1 << 31))      # network.init + target = online
     self._action = None
     self._frame_t = -1
@@ -274,7 +275,7 @@ class _DeviceAgent(parts.Agent):
       blobs[name] = t
     state = {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'dueling': bool(L.net.dueling),
              'noisy': bool(L.net.noisy), 'random_shift_pad': L.random_shift_pad, 'prioritized': self.PRIORITIZED,
-             'param_count': L.plan.param_count, 'opt_state_floats': L.plan.opt_state_floats,
+             'cql_alpha': L.cql_alpha, 'param_count': L.plan.param_count, 'opt_state_floats': L.plan.opt_state_floats,
              'host_rng': self._host_rng.get_state(), 'seed': self._seed,
              'jax_key': None if getattr(self, '_jax_key', None) is None else self._jax_key.copy(),
              'frame_t': self._frame_t}
@@ -305,12 +306,13 @@ class _DeviceAgent(parts.Agent):
     L = self._learner
     # checkpoints written before the dueling network, noisy networks, random-shift augmentation or prioritized replay
     # for every kind existed have no 'dueling' / 'noisy' / 'random_shift_pad' / 'prioritized' key: they hold the plain
-    # network, trained without augmentation, on the replay of the kind (prioritized for prioritized and rainbow only)
+    # network, trained without augmentation, on the replay of the kind (prioritized for prioritized and rainbow only);
+    # those written before the CQL term (DESIGN.md §20) have no 'cql_alpha' key: they were trained without it
     ck.validate(dict({'dueling': False, 'noisy': False, 'random_shift_pad': 0,
-                      'prioritized': type(self).PRIORITIZED}, **state),
+                      'prioritized': type(self).PRIORITIZED, 'cql_alpha': 0.0}, **state),
                 {'format': 'dqn_zoo_b200.agent', 'version': 1, 'kind': self.KIND, 'dueling': bool(L.net.dueling),
                  'noisy': bool(L.net.noisy), 'random_shift_pad': L.random_shift_pad, 'prioritized': self.PRIORITIZED,
-                 'param_count': L.plan.param_count, 'opt_state_floats': L.plan.opt_state_floats}, directory)
+                 'cql_alpha': L.cql_alpha, 'param_count': L.plan.param_count, 'opt_state_floats': L.plan.opt_state_floats}, directory)
     blobs = {}
     for name in self._CHECKPOINT_BLOBS:
       path = os.path.join(directory, name + '.npy')
@@ -471,10 +473,12 @@ class Dqn(_DeviceAgent):
 
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
                batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
-               target_network_update_period, grad_error_bound, rng_key, use_cuda_graph=True, random_shift_pad=0):
+               target_network_update_period, grad_error_bound, rng_key, use_cuda_graph=True, random_shift_pad=0,
+               cql_alpha=0.0):
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
+                grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad,
+                cql_alpha=cql_alpha)
 
 
 class DoubleQ(Dqn):
@@ -492,10 +496,11 @@ class Munchausen(_DeviceAgent):
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
                batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
                target_network_update_period, grad_error_bound, rng_key, use_cuda_graph=True, munchausen_alpha=0.9,
-               entropy_temperature=0.03, log_policy_clip=-1.0, random_shift_pad=0):
+               entropy_temperature=0.03, log_policy_clip=-1.0, random_shift_pad=0, cql_alpha=0.0):
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
                 grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad,
+                cql_alpha=cql_alpha,
                 munchausen_alpha=munchausen_alpha, entropy_temperature=entropy_temperature, log_policy_clip=log_policy_clip)
 
 
@@ -506,10 +511,12 @@ class PrioritizedDqn(_DeviceAgent):
 
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
                batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
-               target_network_update_period, grad_error_bound, rng_key, use_cuda_graph=True, random_shift_pad=0):
+               target_network_update_period, grad_error_bound, rng_key, use_cuda_graph=True, random_shift_pad=0,
+               cql_alpha=0.0):
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
+                grad_error_bound=grad_error_bound, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad,
+                cql_alpha=cql_alpha)
 
 
 class C51(_DeviceAgent):
@@ -518,11 +525,11 @@ class C51(_DeviceAgent):
 
   def __init__(self, preprocessor, sample_network_input, network, support, optimizer, transition_accumulator,
                replay, batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
-               target_network_update_period, rng_key, use_cuda_graph=True, random_shift_pad=0):
+               target_network_update_period, rng_key, use_cuda_graph=True, random_shift_pad=0, cql_alpha=0.0):
     _check_support(support, network)
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
+                use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad, cql_alpha=cql_alpha)
 
 
 class QrDqn(_DeviceAgent):
@@ -531,14 +538,16 @@ class QrDqn(_DeviceAgent):
 
   def __init__(self, preprocessor, sample_network_input, network, quantiles, optimizer, transition_accumulator,
                replay, batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
-               target_network_update_period, huber_param, rng_key, use_cuda_graph=True, random_shift_pad=0):
+               target_network_update_period, huber_param, rng_key, use_cuda_graph=True, random_shift_pad=0,
+               cql_alpha=0.0):
     q = np.asarray(quantiles, dtype=np.float64)
     n = network.num_quantiles
     if len(q) != n or not np.allclose(q, (np.arange(n) + 0.5) / n, rtol=0, atol=1e-6):
       raise ValueError('quantiles must be the %d midpoints (i + 0.5) / n' % n)
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                huber_param=huber_param, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
+                huber_param=huber_param, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad,
+                cql_alpha=cql_alpha)
 
 
 class Rainbow(_DeviceAgent):
@@ -549,11 +558,11 @@ class Rainbow(_DeviceAgent):
 
   def __init__(self, preprocessor, sample_network_input, network, support, optimizer, transition_accumulator,
                replay, batch_size, min_replay_capacity_fraction, learn_period, target_network_update_period,
-               rng_key, use_cuda_graph=True, random_shift_pad=0):
+               rng_key, use_cuda_graph=True, random_shift_pad=0, cql_alpha=0.0):
     _check_support(support, network)
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 None, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
+                use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad, cql_alpha=cql_alpha)
 
 
 class Iqn(_DeviceAgent):
@@ -563,7 +572,7 @@ class Iqn(_DeviceAgent):
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
                batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
                target_network_update_period, huber_param, tau_samples_policy, tau_samples_s_tm1, tau_samples_s_t,
-               rng_key, use_cuda_graph=True, jax_prng_taus=False, random_shift_pad=0):
+               rng_key, use_cuda_graph=True, jax_prng_taus=False, random_shift_pad=0, cql_alpha=0.0):
     """`jax_prng_taus=True`: `rng_key` is treated as a jax PRNG key (`jax.random.PRNGKey(seed)` = [0, seed]) and the tau
     samples of every update and every action selection follow the reference's key chain bit for bit
     (iqn/agent.py:182-190, 207, 220-222; threefry2x32 + jax.random.split/uniform, csrc/dz_jaxprng.cu).  The default keeps
@@ -573,7 +582,8 @@ class Iqn(_DeviceAgent):
       raise ValueError('tau sample counts must match the NetworkSpec')
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
-                huber_param=huber_param, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad)
+                huber_param=huber_param, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad,
+                cql_alpha=cql_alpha)
     if jax_prng_taus:
       key = np.asarray(rng_key, dtype=np.uint32).reshape(-1)
       if key.size != 2:
@@ -598,13 +608,14 @@ class MunchausenIqn(_DeviceAgent):
                batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
                target_network_update_period, huber_param, tau_samples_policy, tau_samples_s_tm1, tau_samples_s_t,
                rng_key, use_cuda_graph=True, munchausen_alpha=0.9, entropy_temperature=0.03, log_policy_clip=-1.0,
-               random_shift_pad=0):
+               random_shift_pad=0, cql_alpha=0.0):
     if (network.tau_samples_policy, network.tau_samples_s_tm1, network.tau_samples_s_t) != (
         tau_samples_policy, tau_samples_s_tm1, tau_samples_s_t):
       raise ValueError('tau sample counts must match the NetworkSpec')
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
                 huber_param=huber_param, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad,
+                cql_alpha=cql_alpha,
                 munchausen_alpha=munchausen_alpha, entropy_temperature=entropy_temperature, log_policy_clip=log_policy_clip)
 
 
@@ -620,12 +631,14 @@ class Fqf(_DeviceAgent):
   def __init__(self, preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay,
                batch_size, exploration_epsilon, min_replay_capacity_fraction, learn_period,
                target_network_update_period, huber_param, rng_key, use_cuda_graph=True, num_fractions=32,
-               fraction_learning_rate=2.5e-9, fraction_opt_eps=1e-5, fraction_rms_decay=0.95, random_shift_pad=0):
+               fraction_learning_rate=2.5e-9, fraction_opt_eps=1e-5, fraction_rms_decay=0.95, random_shift_pad=0,
+               cql_alpha=0.0):
     if network.num_fractions != num_fractions:
       raise ValueError('num_fractions must match the NetworkSpec')
     self._setup(preprocessor, sample_network_input, network, optimizer, transition_accumulator, replay, batch_size,
                 exploration_epsilon, min_replay_capacity_fraction, learn_period, target_network_update_period, rng_key,
                 huber_param=huber_param, use_cuda_graph=use_cuda_graph, random_shift_pad=random_shift_pad,
+                cql_alpha=cql_alpha,
                 fraction_learning_rate=fraction_learning_rate, fraction_opt_eps=fraction_opt_eps,
                 fraction_rms_decay=fraction_rms_decay)
 
@@ -1083,6 +1096,93 @@ class VectorTrainer:
     ret, length, count = state['episodes']
     self._episode_return, self._episode_length, self._num_episodes = (np.array(ret), np.array(length),
                                                                       np.array(count))
+
+
+class OfflineTrainer:
+  """Trains an agent offline from the fixed replay it holds (DESIGN.md §20): learner steps only, no acting and no
+  inserts, as in offline RL on a recorded dataset (Agarwal, Schuurmans & Norouzi, ICML 2020).  Combine it with the
+  agent's `cql_alpha` for conservative Q-learning (Kumar et al., NeurIPS 2020).
+
+  It uses `train_agent`'s learner, replay and CUDA graph in place: `step(n)` runs n of the agent's own learner steps
+  (`_learn()`, host draws in the reference's order; a prioritized replay keeps writing priorities back).  After update
+  u (counted from 1 across calls) with u % target_update_period == 0 it syncs the target network and reads the
+  device's error flags, as `step` does on the agent's target-update cadence.  The default period is the agent's own
+  cadence counted in updates, max(1, target_network_update_period // learn_period).  Nothing else of the agent moves:
+  not `frame_t`, the exploration schedule, the acting RandomState or the replay's contents, and no
+  `min_replay_capacity` gate applies.  A dataset is a replay filled by any other means, e.g. by a `VectorTrainer`
+  whose agent never reaches its learning gate, saved with `replay.save_checkpoint` and restored with
+  `load_checkpoint`."""
+
+  def __init__(self, train_agent: _DeviceAgent, target_update_period: Optional[int] = None):
+    if not isinstance(train_agent, _DeviceAgent):
+      raise TypeError('OfflineTrainer needs one of the device agents, got %s' % type(train_agent).__name__)
+    if target_update_period is None:
+      target_update_period = max(1, train_agent._target_network_update_period // train_agent._learn_period)
+    if int(target_update_period) != target_update_period or target_update_period < 1:
+      raise ValueError('target_update_period must be an integer >= 1, got %r' % (target_update_period,))
+    self._agent = train_agent
+    self._period = int(target_update_period)
+    self._updates = 0
+
+  @property
+  def agent(self) -> _DeviceAgent:
+    return self._agent
+
+  @property
+  def target_update_period(self) -> int:
+    return self._period
+
+  @property
+  def updates(self) -> int:
+    """Learner steps taken so far (restored by `set_state` / `load_checkpoint`)."""
+    return self._updates
+
+  def step(self, num_updates: int = 1) -> None:
+    """`num_updates` learner steps on the replay; ValueError on an empty replay."""
+    if self._agent._replay.size == 0:
+      raise ValueError('offline training needs a non-empty replay')
+    for _ in range(int(num_updates)):
+      self._agent._learn()
+      self._updates += 1
+      if self._updates % self._period == 0:
+        self._agent.learner.sync_target()
+        self._agent.check_device_flags()
+
+  def get_state(self) -> Mapping[str, Any]:
+    """The agent's state plus `updates` and the replay's RandomState, which the agent's state leaves to the run."""
+    return dict(self._own_state(), agent=self._agent.get_state())
+
+  def set_state(self, state: Mapping[str, Any]) -> None:
+    self._agent.set_state(state['agent'])
+    self._set_own_state(state)
+
+  def save_checkpoint(self, directory: str) -> None:
+    """The agent's checkpoint directory (`_DeviceAgent.save_checkpoint`, its replay included) in `agent/`, plus
+    `updates`, the period and the replay's RandomState pickled in `offline.pkl`."""
+    from dqn_zoo_b200 import checkpoint as ck
+    os.makedirs(directory, exist_ok=True)
+    self._agent.save_checkpoint(os.path.join(directory, 'agent'))
+    ck.write_bytes(os.path.join(directory, 'offline.pkl'), pickle.dumps(self._own_state(), protocol=pickle.HIGHEST_PROTOCOL))
+
+  def load_checkpoint(self, directory: str) -> None:
+    """Restores `save_checkpoint` of a trainer with the same target-update period over the same kind of agent."""
+    try:
+      with open(os.path.join(directory, 'offline.pkl'), 'rb') as f:
+        state = pickle.load(f)
+    except (OSError, pickle.UnpicklingError, EOFError) as e:
+      raise ValueError('%s is not a readable offline trainer checkpoint: %s' % (directory, e)) from e
+    if state.get('target_update_period') != self._period:
+      raise ValueError('checkpoint target_update_period %r != %d' % (state.get('target_update_period'), self._period))
+    self._agent.load_checkpoint(os.path.join(directory, 'agent'))
+    self._set_own_state(state)
+
+  def _own_state(self) -> Mapping[str, Any]:
+    return {'format': 'dqn_zoo_b200.offline', 'version': 1, 'updates': self._updates,
+            'target_update_period': self._period, 'replay_rng': self._agent._replay._rng_state()}
+
+  def _set_own_state(self, state: Mapping[str, Any]) -> None:
+    self._updates = int(state['updates'])
+    self._agent._replay._set_rng_state(state['replay_rng'])
 
 
 class VectorEvaluator:

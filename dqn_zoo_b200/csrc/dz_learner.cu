@@ -331,6 +331,26 @@ __host__ __device__ inline float dueling_transpose(const float* dq, int A, float
   return s;
 }
 
+// ---- CQL(H) per-example arithmetic (DESIGN.md §20), shared by every loss kernel's cql variant and its host twin
+// dz_test_cql_example.  From the online network's expected values q [A] on s_tm1: R = logsumexp_a q_a - q_{a_tm1} with
+// the max subtracted, evaluated as (m - q_{a_tm1}) + log S, two non-negative terms, so R >= 0 holds in fp32 too; and
+// g_a = cot (softmax(q)_a - [a = a_tm1]), the gradient of cot R wrt q_a (cot = alpha w_b / B).  Every sum runs serially
+// in action order, so example b's bits do not depend on B.  q and g may live in global or shared memory; g may not
+// alias q.  Returns R.
+struct CqlArgs {
+  float alpha;          // > 0 in the cql variant of each loss kernel (the off variant reads nothing here)
+  float* regularizer;   // [B] R_b, or NULL
+};
+
+__host__ __device__ inline float cql_example(const float* q, int A, int at, float cot, float* g) {
+  float m = q[0];
+  for (int a = 1; a < A; ++a) m = fmaxf(m, q[a]);
+  float s = 0.f;
+  for (int a = 0; a < A; ++a) s += expf(q[a] - m);
+  for (int a = 0; a < A; ++a) g[a] = cot * (expf(q[a] - m) / s - (a == at ? 1.0f : 0.0f));
+  return (m - q[at]) + logf(s);
+}
+
 // ---- random-shift augmentation (DESIGN.md §18): the largest pad, and the shared-memory stage of random_shift_kernel,
 // which holds the source rows of one band of output rows (84x84x4 and 84x92x4 observations: one band)
 constexpr int kShiftMaxPad = 16;
@@ -343,6 +363,7 @@ static int validate(const dz_learner_config& c) {
     return fail(DZ_EINVAL, "dueling: only dqn, double_q, prioritized and munchausen take the dueling network");
   if (c.noisy != 0 && c.noisy != 1) return fail(DZ_EINVAL, "noisy must be 0 or 1");
   if (c.prioritized != 0 && c.prioritized != 1) return fail(DZ_EINVAL, "prioritized must be 0 or 1");
+  if (!std::isfinite(c.cql_alpha) || c.cql_alpha < 0.f) return fail(DZ_EINVAL, "cql_alpha must be finite and >= 0");
   if (c.noisy && c.kind == DZ_RAINBOW) return fail(DZ_EINVAL, "noisy: rainbow's network is noisy already");
   if (c.noisy && !dueling_allowed(c.kind))
     return fail(DZ_EINVAL, "noisy: only dqn, double_q, prioritized and munchausen take noisy layers");
@@ -877,8 +898,10 @@ __device__ __forceinline__ float block_max(float v, float* smem) {
   return t;
 }
 
-// dqn / double_q / prioritized: rlax.q_learning / double_q_learning, clip_gradient, l2_loss.
-__global__ void __launch_bounds__(64) loss_q_kernel(LossArgs L) {
+// dqn / double_q / prioritized: rlax.q_learning / double_q_learning, clip_gradient, l2_loss.  kCql (DESIGN.md §20): the
+// CQL term on the online head's q-values, its gradient added to dout unclipped.
+template <bool kCql>
+__global__ void __launch_bounds__(64) loss_q_kernel(LossArgs L, CqlArgs cq) {
   dz::pdl_enter();
   int b = blockIdx.x;
   if (threadIdx.x != 0) return;
@@ -893,16 +916,28 @@ __global__ void __launch_bounds__(64) loss_q_kernel(LossArgs L) {
   float td = target - q_tm1[at];
   float w = L.w ? L.w[b] : 1.0f;
   float g = fminf(fmaxf(w * td / (float)L.B, -L.bound), L.bound);  // cotangent reaching clip_gradient
-  for (int a = 0; a < L.A; ++a) L.dout[(long long)b * L.A + a] = (a == at) ? -g : 0.f;
-  L.per_example[b] = td;
-  if (L.priorities) L.priorities[b] = fabsf(td);                   // prioritized/agent.py:201
-  L.loss_terms[b] = w * 0.5f * td * td;
+  if constexpr (kCql) {
+    float* d = L.dout + (long long)b * L.A;
+    const float R = cql_example(q_tm1, L.A, at, cq.alpha * w / (float)L.B, d);
+    d[at] -= g;
+    L.per_example[b] = td;
+    if (L.priorities) L.priorities[b] = fabsf(td);
+    if (cq.regularizer) cq.regularizer[b] = R;
+    L.loss_terms[b] = w * fmaf(cq.alpha, R, 0.5f * td * td);
+  } else {
+    for (int a = 0; a < L.A; ++a) L.dout[(long long)b * L.A + a] = (a == at) ? -g : 0.f;
+    L.per_example[b] = td;
+    if (L.priorities) L.priorities[b] = fabsf(td);                   // prioritized/agent.py:201
+    L.loss_terms[b] = w * 0.5f * td * td;
+  }
 }
 
 // munchausen: one warp per example, lane a holding action a of the target network's passes on s_tm1 (out1) and s_t
 // (out2); the target of DESIGN.md §13, then dqn's clip_gradient + l2_loss on td = target - q(s_tm1, a_tm1).  The
-// per-example value is the loss 0.5 td^2; the priority is |td|, the dqn family's rule on the soft target.
-__global__ void __launch_bounds__(128) loss_munchausen_kernel(LossArgs L, float alpha, float tau, float l0) {
+// per-example value is the loss 0.5 td^2; the priority is |td|, the dqn family's rule on the soft target.  kCql
+// (DESIGN.md §20): lane 0 adds the CQL term on the online head's q-values (out0), its gradient unclipped.
+template <bool kCql>
+__global__ void __launch_bounds__(128) loss_munchausen_kernel(LossArgs L, float alpha, float tau, float l0, CqlArgs cq) {
   dz::pdl_enter();
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -921,20 +956,36 @@ __global__ void __launch_bounds__(128) loss_munchausen_kernel(LossArgs L, float 
   const float td = m.target - L.out0[row + at];
   const float w = L.w ? L.w[b] : 1.0f;
   const float g = fminf(fmaxf(w * td / (float)L.B, -L.bound), L.bound);   // cotangent reaching clip_gradient
-  if (act) L.dout[row + lane] = lane == at ? -g : 0.f;
-  if (lane == 0) {
-    const float loss = 0.5f * td * td;
-    L.per_example[b] = loss;
-    if (L.priorities) L.priorities[b] = fabsf(td);
-    L.loss_terms[b] = w * loss;
+  if constexpr (kCql) {
+    if (lane == 0) {
+      const float R = cql_example(L.out0 + row, A, at, cq.alpha * w / (float)L.B, L.dout + row);
+      L.dout[row + at] -= g;
+      const float loss = 0.5f * td * td;
+      L.per_example[b] = loss;
+      if (L.priorities) L.priorities[b] = fabsf(td);
+      if (cq.regularizer) cq.regularizer[b] = R;
+      L.loss_terms[b] = w * fmaf(cq.alpha, R, loss);
+    }
+  } else {
+    if (act) L.dout[row + lane] = lane == at ? -g : 0.f;
+    if (lane == 0) {
+      const float loss = 0.5f * td * td;
+      L.per_example[b] = loss;
+      if (L.priorities) L.priorities[b] = fabsf(td);
+      L.loss_terms[b] = w * loss;
+    }
   }
 }
 
 // c51 / rainbow: categorical_[double_]q_learning with categorical_l2_project + cross entropy.
 // One CTA (4 warps) per example.  Everything the example's loss reads from the three head passes is first staged in
 // shared memory; softmaxes then run one warp per (pass, action) with shuffle reductions, so the whole kernel has six
-// block barriers.  Dynamic shared memory: categorical_loss_smem().
-__global__ void __launch_bounds__(128) loss_categorical_staged_kernel(LossArgs L) {
+// block barriers.  Dynamic shared memory: categorical_loss_smem().  kCql (DESIGN.md §20): step 1 also takes every
+// action's expected value Q_a under the online(s_tm1) pass, step 2 the CQL coefficients of those Q_a, and step 5 chains
+// them through dQ_a / dlogit_{a,k} = p_{a,k} (z_k - Q_a) into every action's logits (rainbow: through the aggregation's
+// transpose into dadv and dval).
+template <bool kCql>
+__global__ void __launch_bounds__(128) loss_categorical_staged_kernel(LossArgs L, CqlArgs cq) {
   dz::pdl_enter();
   extern __shared__ float sm[];
   const int b = blockIdx.x, K = L.atoms, A = L.A, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -949,6 +1000,8 @@ __global__ void __launch_bounds__(128) loss_categorical_staged_kernel(LossArgs L
   float* zs = scal + 4;          // [K] support atoms
   float* st_adv = zs + K;        // [3][A*K] head outputs of this example for pass 0 / 1 / 2
   float* st_val = st_adv + 3 * A * K;   // [3][K] value-stream outputs (rainbow)
+  // kCql, after st_val: [A] Q_a of online(s_tm1), [A] max and [A] denominator of each action's softmax of that pass,
+  // [A] the CQL gradient wrt Q_a, [1] R (indexed from st_val + 3K inside the kCql blocks)
   const bool rb = L.kind == DZ_RAINBOW;
   // Everything this example's loss reads from the three head passes goes to shared memory in ONE round of coalesced,
   // independent loads; the phases below are then shared-memory arithmetic instead of ~10 dependent global round trips.
@@ -1015,6 +1068,14 @@ __global__ void __launch_bounds__(128) loss_categorical_staged_kernel(LossArgs L
     for (int k = lane; k < K; k += 32) s += (expf(logit_of(rb ? 1 : 2, a, k) - mx) / den) * support(k);
     s = warp_sum(s);
     if (lane == 0) qsel[a] = s;
+    if constexpr (kCql) {
+      warp_softmax(0, a, nullptr, mx, den);
+      float s0 = 0.f;
+      for (int k = lane; k < K; k += 32) s0 += (expf(logit_of(0, a, k) - mx) / den) * support(k);
+      s0 = warp_sum(s0);
+      float* cq = st_val + 3 * K;
+      if (lane == 0) { cq[a] = s0; cq[A + a] = mx; cq[2 * A + a] = den; }
+    }
   }
   __syncthreads();
   int best = 0;
@@ -1027,6 +1088,10 @@ __global__ void __launch_bounds__(128) loss_categorical_staged_kernel(LossArgs L
   if (warp == 1) {
     warp_softmax(0, at, p_tm1, mx_tm1, den_tm1);
     if (lane == 0) { scal[2] = mx_tm1; scal[3] = den_tm1; }
+  }
+  if constexpr (kCql) {
+    float* q0 = st_val + 3 * K;
+    if (tid == 64) q0[4 * A] = cql_example(q0, A, at, cq.alpha * (L.w ? L.w[b] : 1.0f) / (float)L.B, q0 + 3 * A);
   }
   __syncthreads();
   // 3. rlax.categorical_l2_project(r + discount*z, p, z)
@@ -1064,6 +1129,36 @@ __global__ void __launch_bounds__(128) loss_categorical_staged_kernel(LossArgs L
   const float w = L.w ? L.w[b] : 1.0f;
   const float cot = w / (float)L.B;
   // 5. gradient wrt the pass-0 head outputs
+  if constexpr (kCql) {
+    const float* q0 = st_val + 3 * K;
+    // the CQL gradient wrt logit k of action a (pass 0)
+    auto cql_dlogit = [&](int a, int k) {
+      const float p0 = expf(logit_of(0, a, k) - q0[A + a]) / q0[2 * A + a];
+      return q0[3 * A + a] * (p0 * (support(k) - q0[a]));
+    };
+    if (rb) {
+      for (int k = tid; k < K; k += blockDim.x) {
+        const float dl = cot * (p_tm1[k] * psum - proj[k]);
+        float s = 0.f;
+        for (int a = 0; a < A; ++a) s += (a == at ? dl : 0.f) + cql_dlogit(a, k);
+        L.dval[(long long)b * K + k] = s;
+        const float m = s / (float)A;
+        for (int a = 0; a < A; ++a) L.dadv[((long long)b * A + a) * K + k] = ((a == at ? dl : 0.f) + cql_dlogit(a, k)) - m;
+      }
+    } else {
+      for (int i = tid; i < A * K; i += blockDim.x) {
+        int a = i / K, k = i - a * K;
+        L.dout[(long long)b * A * K + i] = ((a == at) ? cot * (p_tm1[k] * psum - proj[k]) : 0.f) + cql_dlogit(a, k);
+      }
+    }
+    if (tid == 0) {
+      L.per_example[b] = loss;
+      if (L.priorities) L.priorities[b] = fminf(fmaxf(fabsf(loss), 0.f), 100.f);
+      if (cq.regularizer) cq.regularizer[b] = q0[4 * A];
+      L.loss_terms[b] = w * fmaf(cq.alpha, q0[4 * A], loss);
+    }
+    return;
+  }
   if (rb) {
     for (int k = tid; k < K; k += blockDim.x) {
       float dl = cot * (p_tm1[k] * psum - proj[k]);
@@ -1086,16 +1181,22 @@ __global__ void __launch_bounds__(128) loss_categorical_staged_kernel(LossArgs L
 
 // 6K + A + 4 floats of working arrays, K support atoms, and the staged [3][A*K] head outputs and [3][K] value outputs.
 // The largest configuration validate() accepts (A = 64, K = 128) needs 103,696 bytes, more than the default 48 KB.
+// cql_alpha > 0 adds 4A + 1 floats (kCql's Q_a, softmax maxima and denominators, coefficients and R).
 size_t categorical_loss_smem(const dz_learner_config& c) {
   const size_t A = c.num_actions, K = c.num_atoms;
-  return (6 * K + A + 4 + K + 3 * A * K + 3 * K) * sizeof(float);
+  return (6 * K + A + 4 + K + 3 * A * K + 3 * K + (c.cql_alpha > 0.f ? 4 * A + 1 : 0)) * sizeof(float);
 }
 
 // rlax.quantile_regression_loss of example b's N source quantiles src (at taus tau) against its Nt targets tgt, all in
 // shared memory, and the gradient wrt the pass-0 head outputs in IQN's layout (nonzero at a_tm1 only): the tail of
-// loss_quantile_kernel, which keeps its own inline copy so that its code generation stays as it was.
+// loss_quantile_kernel, which keeps its own inline copy so that its code generation stays as it was.  kCql (DESIGN.md
+// §20): dout also takes the CQL gradient coef[a] * dQ_a / dZ_{i,a}, with the row weight roww[i] (fqf) or 1/N (the mean),
+// and the loss term alpha r[0]; cql_quantile_head prepares coef and r.
+template <bool kCql = false>
 __device__ __forceinline__ void quantile_huber_tail(const LossArgs& L, int b, int at, int N, int Nt, const float* tgt,
-                                                    const float* src, const float* tau, float* red) {
+                                                    const float* src, const float* tau, float* red,
+                                                    const CqlArgs* cq = nullptr, const float* coef = nullptr,
+                                                    const float* roww = nullptr, const float* r = nullptr) {
   const int A = L.A, tid = threadIdx.x;
   const float kappa = L.kappa;
   const float w = L.w ? L.w[b] : 1.0f;
@@ -1121,19 +1222,43 @@ __device__ __forceinline__ void quantile_huber_tail(const LossArgs& L, int b, in
     }
     total += acc / (float)Nt;
     float g = -cot * gacc / (float)Nt;  // d loss / d src_i  (delta = target - src)
-    for (int a = 0; a < A; ++a) L.dout[((long long)b * N + i) * A + a] = (a == at) ? g : 0.f;
+    if constexpr (kCql) {
+      const float rw = roww ? roww[i] : 1.0f / (float)N;
+      for (int a = 0; a < A; ++a) L.dout[((long long)b * N + i) * A + a] = ((a == at) ? g : 0.f) + coef[a] * rw;
+    } else {
+      for (int a = 0; a < A; ++a) L.dout[((long long)b * N + i) * A + a] = (a == at) ? g : 0.f;
+    }
   }
   total = block_sum(total, red);
   if (tid == 0) {
     L.per_example[b] = total;
     if (L.priorities) L.priorities[b] = fminf(fmaxf(fabsf(total), 0.f), 100.f);   // rainbow's rule, DESIGN.md §19
-    L.loss_terms[b] = w * total;
+    if constexpr (kCql) {
+      if (cq->regularizer) cq->regularizer[b] = r[0];
+      L.loss_terms[b] = w * fmaf(cq->alpha, r[0], total);
+    } else {
+      L.loss_terms[b] = w * total;
+    }
   }
 }
 
+// kCql's head of the quantile kernels (DESIGN.md §20): Q_a of online(s_tm1)'s N rows z0 [N][A], their mean or, with
+// roww, sum_i roww[i] z0[i][a] (fqf), one thread per action in row order; then R to r[0] and the coefficients coef [A]
+// (cql_example).  q, coef and r are shared memory; every thread of the CTA calls it.
+__device__ __forceinline__ void cql_quantile_head(const float* z0, int N, int A, const float* roww, int at, float cot,
+                                                  float* q, float* coef, float* r) {
+  const int tid = threadIdx.x;
+  if (tid < A) q[tid] = roww ? fqf_weighted_q(z0, roww, N, A, tid) : miqn_mean(z0, N, A, tid);
+  __syncthreads();
+  if (tid == 0) r[0] = cql_example(q, A, at, cot, coef);
+  __syncthreads();
+}
+
 // qrdqn / iqn: rlax.quantile_q_learning with quantile_regression_loss (Huber kappa).
-// Layouts: qrdqn out[b, q*A + a] (networks.py:308), iqn out[(b*N + n)*A + a] (networks.py:286-287).
-__global__ void __launch_bounds__(256) loss_quantile_kernel(LossArgs L) {
+// Layouts: qrdqn out[b, q*A + a] (networks.py:308), iqn out[(b*N + n)*A + a] (networks.py:286-287).  kCql (DESIGN.md
+// §20): Q_a is the mean of the pass-0 quantiles, and the tail is quantile_huber_tail's cql variant.
+template <bool kCql>
+__global__ void __launch_bounds__(256) loss_quantile_kernel(LossArgs L, CqlArgs cq) {
   dz::pdl_enter();
   extern __shared__ float sm[];
   const int b = blockIdx.x, A = L.A, tid = threadIdx.x;
@@ -1167,6 +1292,14 @@ __global__ void __launch_bounds__(256) loss_quantile_kernel(LossArgs L) {
     tau[i] = iqn ? L.taus0[(long long)b * N + i] : ((float)i + 0.5f) / (float)N;  // qrdqn/run_atari.py:137
   }
   __syncthreads();
+  if constexpr (kCql) {
+    float* cq_q = tau + N;        // [A]
+    float* cq_coef = cq_q + A;    // [A]
+    float* cq_r = cq_coef + A;    // [1]
+    cql_quantile_head(dist_s, N, A, nullptr, at, cq.alpha * (L.w ? L.w[b] : 1.0f) / (float)L.B, cq_q, cq_coef, cq_r);
+    quantile_huber_tail<true>(L, b, at, N, Nt, tgt, src, tau, red, &cq, cq_coef, nullptr, cq_r);
+    return;
+  }
   const float kappa = L.kappa;
   const float w = L.w ? L.w[b] : 1.0f;
   const float cot = w / (float)L.B;
@@ -1206,7 +1339,9 @@ __global__ void __launch_bounds__(256) loss_quantile_kernel(LossArgs L) {
 // action a: both softmaxes, the log-policy bonus and the entropy term E = sum_a pi(a|s_t) h(a); (3) the N' targets
 // y_j = r + bonus + disc (sum_a pi(a|s_t) zbar_j(s_t, a) + E); (4) IQN's quantile-Huber term of online(s_tm1)'s N
 // samples at a_tm1 against them and (5) dout in IQN's layout (quantile_huber_tail).  The per-example value is the loss.
-__global__ void __launch_bounds__(256) loss_munchausen_iqn_kernel(LossArgs L, float alpha, float tau_e, float l0) {
+// kCql (DESIGN.md §20): Q_a is the mean of online(s_tm1)'s N samples, and the tail is quantile_huber_tail's cql variant.
+template <bool kCql>
+__global__ void __launch_bounds__(256) loss_munchausen_iqn_kernel(LossArgs L, float alpha, float tau_e, float l0, CqlArgs cq) {
   dz::pdl_enter();
   extern __shared__ float sm[];
   const int b = blockIdx.x, A = L.A, tid = threadIdx.x;
@@ -1247,11 +1382,21 @@ __global__ void __launch_bounds__(256) loss_munchausen_iqn_kernel(LossArgs L, fl
     tau[i] = L.taus0[(long long)b * N + i];
   }
   __syncthreads();
-  quantile_huber_tail(L, b, at, N, Nt, tgt, src, tau, red);
+  if constexpr (kCql) {
+    float* cq_q = tau + N;        // [A]
+    float* cq_coef = cq_q + A;    // [A]
+    float* cq_r = cq_coef + A;    // [1]
+    cql_quantile_head(dist_s, N, A, nullptr, at, cq.alpha * (L.w ? L.w[b] : 1.0f) / (float)L.B, cq_q, cq_coef, cq_r);
+    quantile_huber_tail<true>(L, b, at, N, Nt, tgt, src, tau, red, &cq, cq_coef, nullptr, cq_r);
+  } else {
+    quantile_huber_tail(L, b, at, N, Nt, tgt, src, tau, red);
+  }
 }
 
+// cql_alpha > 0 adds 2A + 1 floats (the cql variant's Q_a, coefficients and R).
 size_t munchausen_iqn_loss_smem(const dz_learner_config& c) {
-  return (32 + 3 * (size_t)c.num_actions + 2 + c.tau_samples_s_t + 2 * (size_t)c.tau_samples_s_tm1) * sizeof(float);
+  return (32 + 3 * (size_t)c.num_actions + 2 + c.tau_samples_s_t + 2 * (size_t)c.tau_samples_s_tm1 +
+          (c.cql_alpha > 0.f ? 2 * (size_t)c.num_actions + 1 : 0)) * sizeof(float);
 }
 
 // ---- fqf (DESIGN.md §15) ------------------------------------------------------------------------
@@ -1323,8 +1468,12 @@ struct FqfLossArgs {
 // sum_i w'_i Zbar(s_t, a, tau_hat'_i), one thread per action, first maximum; (2) the targets y_j = r + discount
 // Zbar(s_t, a*, tau_hat_j); (3) the fraction gradient at a_tm1 chained to dlogits (fqf_dlogits, thread 0); (4) IQN's
 // quantile-Huber term of online(s_tm1)'s N samples at a_tm1 against the targets and dout in IQN's layout
-// (quantile_huber_tail).  The per-example value, and the priority's source, is the quantile loss.
-__global__ void __launch_bounds__(256) loss_fqf_kernel(LossArgs L, FqfLossArgs f) {
+// (quantile_huber_tail).  The per-example value, and the priority's source, is the quantile loss.  kCql (DESIGN.md §20):
+// Q_a = sum_i w_i Z(s_tm1, tau_hat_i, a) with the interval weights w_i of s_tm1's proposal, formed from q_tm1 by
+// fqf_fractions' recurrence (the bits fraction_forward_kernel wrote) and held constant, and the tail is
+// quantile_huber_tail's cql variant.
+template <bool kCql>
+__global__ void __launch_bounds__(256) loss_fqf_kernel(LossArgs L, FqfLossArgs f, CqlArgs cq) {
   dz::pdl_enter();
   extern __shared__ float sm[];
   const int b = blockIdx.x, A = L.A, N = L.N, tid = threadIdx.x;
@@ -1357,11 +1506,31 @@ __global__ void __launch_bounds__(256) loss_fqf_kernel(LossArgs L, FqfLossArgs f
   if (tid == 0) fqf_dlogits(ftau, src, q, N, (L.w ? L.w[b] : 1.0f) / (float)L.B, dl);
   __syncthreads();
   for (int k = tid; k < N; k += blockDim.x) f.dlogits[(long long)b * N + k] = dl[k];
-  quantile_huber_tail(L, b, at, N, N, tgt, src, tau, red);
+  if constexpr (kCql) {
+    float* cw = dl + N;           // [N] interval weights of s_tm1's proposal
+    float* cq_q = cw + N;         // [A]
+    float* cq_coef = cq_q + A;    // [A]
+    float* cq_r = cq_coef + A;    // [1]
+    if (tid == 0) {
+      float t = 0.f;              // tau_i; tau_N = 1
+      for (int i = 0; i < N; ++i) {
+        const float next = i + 1 < N ? fminf(t + q[i], 1.f) : 1.f;
+        cw[i] = next - t;
+        t = next;
+      }
+    }
+    __syncthreads();
+    cql_quantile_head(z0, N, A, cw, at, cq.alpha * (L.w ? L.w[b] : 1.0f) / (float)L.B, cq_q, cq_coef, cq_r);
+    quantile_huber_tail<true>(L, b, at, N, N, tgt, src, tau, red, &cq, cq_coef, cw, cq_r);
+  } else {
+    quantile_huber_tail(L, b, at, N, N, tgt, src, tau, red);
+  }
 }
 
+// cql_alpha > 0 adds N + 2A + 1 floats (the cql variant's interval weights, Q_a, coefficients and R).
 size_t fqf_loss_smem(const dz_learner_config& c) {
-  return (32 + (size_t)c.num_actions + 6 * (size_t)c.num_fractions) * sizeof(float);
+  return (32 + (size_t)c.num_actions + 6 * (size_t)c.num_fractions +
+          (c.cql_alpha > 0.f ? (size_t)c.num_fractions + 2 * (size_t)c.num_actions + 1 : 0)) * sizeof(float);
 }
 
 __global__ void loss_mean_kernel(const float* __restrict__ terms, int B, float* loss, float* max_seen, const float* priorities) {
@@ -3497,37 +3666,48 @@ int run_optimizer(dz_learner* l, float* user_norm, bool apply, void* stream) {
 // whether priorities are written: writes_priorities) is set here.  With `side`, loss_mean_kernel runs on the side stream forked after the loss kernel and
 // *mean_stream receives it; without, everything runs on `stream`.  dz_test_loss and dz_test_loss_fqf run this same
 // function.
+// cql_alpha > 0 (DESIGN.md §20) selects each kernel's cql variant, which writes R_b to `regularizer` when it is given;
+// the launch count is the same at every alpha.
 int launch_loss(const dz_learner_config& c, LossArgs& L, int B, void* stream, SideStream* side, float* d_loss, float* max_seen,
-                void** mean_stream, const FqfLossArgs* fqf = nullptr) {
+                void** mean_stream, const FqfLossArgs* fqf = nullptr, float* regularizer = nullptr) {
   L.kind = c.kind; L.B = B; L.A = c.num_actions; L.atoms = c.num_atoms;
   L.vmax = c.vmax; L.bound = c.grad_error_bound; L.kappa = c.huber_param;
   if (!writes_priorities(c)) L.priorities = nullptr;
+  const bool cql = c.cql_alpha > 0.f;
+  const CqlArgs cq{c.cql_alpha, regularizer};
+#define DZ_LAUNCH_LOSS(name, kernel, grid, block, smem, ...)                                   \
+  do {                                                                                         \
+    if (cql) DZ_LAUNCH_NAMED(name, kernel<true>, grid, block, smem, stream, __VA_ARGS__, cq);  \
+    else DZ_LAUNCH_NAMED(name, kernel<false>, grid, block, smem, stream, __VA_ARGS__, cq);     \
+  } while (0)
   if (c.kind == DZ_DQN || c.kind == DZ_DOUBLE_Q || c.kind == DZ_PRIORITIZED) {
-    DZ_LAUNCH(loss_q_kernel, B, 64, 0, stream, L);
+    DZ_LAUNCH_LOSS("loss_q_kernel", loss_q_kernel, B, 64, 0, L);
   } else if (c.kind == DZ_MUNCHAUSEN) {
-    DZ_LAUNCH(loss_munchausen_kernel, (B + 3) / 4, 128, 0, stream, L, c.munchausen_alpha, c.entropy_temperature,
-              c.log_policy_clip);
+    DZ_LAUNCH_LOSS("loss_munchausen_kernel", loss_munchausen_kernel, (B + 3) / 4, 128, 0, L, c.munchausen_alpha,
+                   c.entropy_temperature, c.log_policy_clip);
   } else if (c.kind == DZ_C51 || c.kind == DZ_RAINBOW) {
     // More than the default 48 KB of dynamic shared memory at large num_actions x num_atoms; the attribute is per
     // device, so it is set for the current one.
     const size_t smem = categorical_loss_smem(c);
     if (smem > 48 * 1024)
-      DZ_CUDA_OK(cudaFuncSetAttribute(loss_categorical_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    DZ_LAUNCH_NAMED("loss_categorical_kernel", loss_categorical_staged_kernel, B, 128, smem, stream, L);
+      DZ_CUDA_OK(cudaFuncSetAttribute(cql ? loss_categorical_staged_kernel<true> : loss_categorical_staged_kernel<false>,
+                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    DZ_LAUNCH_LOSS("loss_categorical_kernel", loss_categorical_staged_kernel, B, 128, smem, L);
   } else if (proposes_fractions(c.kind)) {
     if (!fqf) return fail(DZ_EINVAL, "fqf's loss needs the fraction buffers of a learner step");
     L.N = c.num_fractions; L.Ksel = c.num_fractions; L.Nt = c.num_fractions;
-    DZ_LAUNCH(loss_fqf_kernel, B, 256, fqf_loss_smem(c), stream, L, *fqf);
+    DZ_LAUNCH_LOSS("loss_fqf_kernel", loss_fqf_kernel, B, 256, fqf_loss_smem(c), L, *fqf);
   } else if (c.kind == DZ_MUNCHAUSEN_IQN) {
     L.N = c.tau_samples_s_tm1; L.Ksel = c.tau_samples_policy; L.Nt = c.tau_samples_s_t;
-    DZ_LAUNCH(loss_munchausen_iqn_kernel, B, 256, munchausen_iqn_loss_smem(c), stream, L, c.munchausen_alpha,
-              c.entropy_temperature, c.log_policy_clip);
+    DZ_LAUNCH_LOSS("loss_munchausen_iqn_kernel", loss_munchausen_iqn_kernel, B, 256, munchausen_iqn_loss_smem(c), L,
+                   c.munchausen_alpha, c.entropy_temperature, c.log_policy_clip);
   } else {
     if (c.kind == DZ_QRDQN) { L.N = c.num_quantiles; L.Ksel = c.num_quantiles; L.Nt = c.num_quantiles; }
     else { L.N = c.tau_samples_s_tm1; L.Ksel = c.tau_samples_policy; L.Nt = c.tau_samples_s_t; }
-    size_t smem = (32 + c.num_actions + L.Nt + 2 * L.N) * sizeof(float);
-    DZ_LAUNCH(loss_quantile_kernel, B, 256, smem, stream, L);
+    size_t smem = (32 + c.num_actions + L.Nt + 2 * L.N + (cql ? 2 * c.num_actions + 1 : 0)) * sizeof(float);
+    DZ_LAUNCH_LOSS("loss_quantile_kernel", loss_quantile_kernel, B, 256, smem, L);
   }
+#undef DZ_LAUNCH_LOSS
   void* ms = side ? side->fork(stream, stream) : stream;
   DZ_LAUNCH(loss_mean_kernel, 1, 32, 0, ms, L.loss_terms, B, d_loss, max_seen, L.priorities);
   if (mean_stream) *mean_stream = ms;
@@ -3731,7 +3911,7 @@ int update_impl(dz_learner* l, const dz_batch* batch, const dz_update_outputs* o
   {   // the scalar loss / running max priority and replay.update_priorities(ids, priorities) (rainbow/agent.py:198) are
       // independent of the backward pass: both leave the critical path for the side stream
     void* ls = stream;
-    DZ_TRY(launch_loss(c, L, B, stream, &l->side, out->d_loss, max_seen, &ls, fqf ? &fl : nullptr));
+    DZ_TRY(launch_loss(c, L, B, stream, &l->side, out->d_loss, max_seen, &ls, fqf ? &fl : nullptr, out->d_regularizer));
     if (wb) DZ_TRY(launch_update_priorities(wb->view, wb->indices, wb->priorities, B, wb->alpha, wb->view->capacity, ls));
   }
 
@@ -4362,6 +4542,15 @@ int dz_test_dueling_example(const float* adv, float v, const float* dq, int32_t 
   if (A < 1 || A > kDuelingMaxActions) return fail(DZ_EINVAL, "dueling example: A must be in [1,64]");
   dueling_aggregate(adv, v, A, out);
   out[2 * A] = dueling_transpose(dq, A, out + A);
+  return DZ_OK;
+}
+
+// Host twin of every loss kernel's CQL arithmetic: cql_example, the function their cql variants run (tests only).
+int dz_test_cql_example(const float* q, int32_t A, int32_t a_tm1, float cot, float* out) {
+  if (!q || !out) return fail(DZ_EINVAL, "cql example: NULL buffer");
+  if (A < 1 || A > 64) return fail(DZ_EINVAL, "cql example: A must be in [1,64]");
+  if (a_tm1 < 0 || a_tm1 >= A) return fail(DZ_EINVAL, "cql example: a_tm1 out of range");
+  out[A] = cql_example(q, A, a_tm1, cot, out);
   return DZ_OK;
 }
 

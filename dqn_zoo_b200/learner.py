@@ -136,6 +136,16 @@ def check_network(net: NetworkSpec) -> None:
 MAX_RANDOM_SHIFT_PAD = 16
 
 
+def check_cql_alpha(alpha) -> float:
+  """The CQL weight (DESIGN.md §20) as a float; ValueError unless it is a finite real number >= 0."""
+  if isinstance(alpha, (bool, np.bool_)) or not isinstance(alpha, (int, float, np.integer, np.floating)):
+    raise ValueError('cql_alpha must be a real number, got %r' % (alpha,))
+  alpha = float(alpha)
+  if not math.isfinite(alpha) or alpha < 0.0:
+    raise ValueError('cql_alpha must be finite and >= 0, got %r' % (alpha,))
+  return alpha
+
+
 def check_random_shift_pad(pad, obs_shape) -> int:
   """The random-shift pad (DESIGN.md §18) as an int; ValueError unless it is an integer in [0, 16] and less than
   min(H, W)."""
@@ -218,7 +228,7 @@ class Learner:
                grad_error_bound: float = 1.0 / 32, huber_param: float = 1.0, munchausen_alpha: float = 0.9,
                entropy_temperature: float = 0.03, log_policy_clip: float = -1.0, fraction_learning_rate: float = 2.5e-9,
                fraction_opt_eps: float = 1e-5, fraction_rms_decay: float = 0.95, device=None, random_shift_pad: int = 0,
-               prioritized: bool = False):
+               prioritized: bool = False, cql_alpha: float = 0.0):
     """`munchausen_alpha`, `entropy_temperature` (tau) and `log_policy_clip` (l0) are Munchausen DQN's and
     Munchausen-IQN's (DESIGN.md §13, §14, defaults the paper's Atari values); the library rejects tau <= 0, alpha < 0,
     l0 > 0 and non-finite values for those kinds, and the other kinds ignore them.  `fraction_learning_rate`,
@@ -228,9 +238,12 @@ class Learner:
     the [B, 4] int32 `shifts`, which `generate_randomness` draws; acting never sees a shift.  ValueError unless p is an
     integer in [0, 16] and less than min(H, W).  `prioritized=True` makes every update fill `.priorities` by the kind's
     rule and lets `learn` sample by priority and write them back (DESIGN.md §19); prioritized and rainbow do so
-    whatever it says."""
+    whatever it says.  `cql_alpha` > 0 adds conservative Q-learning's alpha (logsumexp_a Q(s_tm1, a) - Q(s_tm1, a_tm1))
+    to each example's loss (CQL(H), DESIGN.md §20) and fills `.regularizer` [B] with that difference; 0 is off.
+    ValueError unless it is finite and >= 0."""
     check_network(net)
     random_shift_pad = check_random_shift_pad(random_shift_pad, net.obs_shape)
+    cql_alpha = check_cql_alpha(cql_alpha)
     if not torch.cuda.is_available():
       raise RuntimeError('dqn_zoo_b200.learner needs a CUDA device (there is no CPU fallback)')
     self.net = net
@@ -256,7 +269,9 @@ class Learner:
     cfg.noisy = 1 if net.noisy else 0
     cfg.random_shift_pad = random_shift_pad
     cfg.prioritized = 1 if prioritized else 0
+    cfg.cql_alpha = cql_alpha
     self.random_shift_pad = random_shift_pad
+    self.cql_alpha = cql_alpha
     self.cfg = cfg
     plan = _lib.LearnerPlan()
     _lib.call('dz_learner_plan_query', C.byref(cfg), C.byref(plan))
@@ -283,6 +298,7 @@ class Learner:
     self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
     self.per_example = torch.zeros(batch_size, dtype=torch.float32, device=dev)
     self.priorities = torch.zeros(batch_size, dtype=torch.float32, device=dev)
+    self.regularizer = torch.zeros(batch_size, dtype=torch.float32, device=dev)   # cql_alpha > 0: R_b of the last update
     self.grad_norm = torch.zeros(1, dtype=torch.float32, device=dev)
     self.max_seen_priority = torch.ones(1, dtype=torch.float32, device=dev)   # rainbow/agent.py:79
     self.q_out = torch.zeros(64, dtype=torch.float32, device=dev)
@@ -409,7 +425,7 @@ class Learner:
                        self.taus.data_ptr() if draws_taus(self.kind) else 0,
                        self.noise.data_ptr() if noisy_layers(self.net) else 0, self._shifts_ptr())
     out = _lib.UpdateOutputs(self.loss.data_ptr(), self.per_example.data_ptr(), self.priorities.data_ptr(),
-                             self.grad_norm.data_ptr())
+                             self.grad_norm.data_ptr(), self.regularizer.data_ptr())
     _lib.call('dz_learner_update', self._h, C.byref(batch), C.byref(out), 1 if apply_update else 0, _cstream())
     self._keep = (keep, w)
 
@@ -484,7 +500,7 @@ class Learner:
     io.d_taus = self.taus.data_ptr() if draws_taus(self.kind) else 0
     io.d_noise = self.noise.data_ptr() if noisy_layers(self.net) else 0
     io.update_out = _lib.UpdateOutputs(self.loss.data_ptr(), self.per_example.data_ptr(), self.priorities.data_ptr(),
-                                       self.grad_norm.data_ptr())
+                                       self.grad_norm.data_ptr(), self.regularizer.data_ptr())
     io.d_max_seen_priority = self.max_seen_priority.data_ptr()
     io.priority_exponent = float(priority_exponent)
     io.d_shifts = self._shifts_ptr()

@@ -386,6 +386,17 @@ typedef struct dz_learner_config {
    * The importance weights d_weights scale each example's loss term and its gradient (fqf: the fraction loss's too)
    * whatever the field says. */
   int32_t prioritized;
+  /* Conservative Q-learning, CQL(H) (Kumar, Zhou, Tucker & Levine, NeurIPS 2020; DESIGN.md §20), for every kind and
+   * network option: alpha finite and >= 0 (DZ_EINVAL otherwise); 0, as a zero-filled tail leaves it: off, and the step
+   * is what it is without the field.  alpha > 0 adds alpha R_b to each example's loss before its importance weight,
+   * R_b = logsumexp_a Q_a(s_tm1) - Q_{a_tm1}(s_tm1) >= 0, with Q_a the online network's expected value on s_tm1:
+   *   dqn, double_q, prioritized, munchausen   the head output q_a (after the dueling aggregation)
+   *   c51, rainbow                             sum_k softmax(logits_a)_k z_k (rainbow: the dueling-aggregated logits)
+   *   qrdqn, iqn, munchausen_iqn               the mean of the pass-0 quantiles (iqn: over the N s_tm1 tau samples)
+   *   fqf                                      sum_i w_i Z(s_tm1, tau_hat_i, a), the proposal's w_i held constant
+   * The gradient of the added term is not clipped by grad_error_bound.  The per-example values, the priorities and
+   * fqf's fraction loss are the kind's own, unchanged. */
+  float cql_alpha;
 } dz_learner_config;
 
 typedef struct dz_learner_plan {
@@ -445,6 +456,8 @@ typedef struct dz_update_outputs {
                                 dz_learner_config.prioritized = 1 by the rule table there; else untouched;
                                 may be NULL */
   float* d_grad_norm;    /* [1] global gradient norm before clipping; may be NULL */
+  float* d_regularizer;  /* [B] the CQL regulariser R_b (dz_learner_config.cql_alpha), unweighted and without alpha:
+                                written when cql_alpha > 0, else untouched; may be NULL */
 } dz_update_outputs;
 
 /* jit(update): forward passes, loss, backward, clip, optimizer, parameter update.
@@ -703,6 +716,11 @@ int dz_test_fqf_example(const float* logits, const float* F_tau, const float* F_
  * q_a = v + (adv_a - m) with m = (sum_a adv_a) / A to out[0, A), dadv_a = dq_a - (sum_a dq_a) / A to out[A, 2A) and
  * dval = sum_a dq_a to out[2A].  Sums run in action order.  DZ_EINVAL for A outside [1, 64] or a NULL buffer; tests only. */
 int dz_test_dueling_example(const float* adv, float v, const float* dq, int32_t A, float* out);
+/* Host twin of the CQL(H) arithmetic of every loss kernel (DESIGN.md §20), the function their cql variants run: from
+ * the expected values q [A] of one example on s_tm1 it writes g_a = cot (softmax(q)_a - [a = a_tm1]) to out[0, A) and
+ * R = logsumexp_a q_a - q_{a_tm1} (max-subtracted) to out[A].  Sums run in action order.  DZ_EINVAL for A outside
+ * [1, 64], a_tm1 outside [0, A) or a NULL buffer; tests only. */
+int dz_test_cql_example(const float* q, int32_t A, int32_t a_tm1, float cot, float* out);
 /* The loss section of a learner step (the agent kind's loss kernel, then the scalar loss and the running max priority)
  * on caller-owned device buffers, all enqueued on `stream`; tests only.  cfg is validated as
  * dz_learner_create does, with batch = B and its observation fields replaced by a legal geometry.  d_out[p]: the head
