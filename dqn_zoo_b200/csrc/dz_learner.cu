@@ -4779,6 +4779,19 @@ int dz_test_learner_buffer(dz_learner* l, const char* name, float** d_ptr, int64
     *d_ptr = l->out[p]; *count = (int64_t)l->B * l->n_head[p] * l->d.out;
   }
   else if (n == "dh1") { *d_ptr = l->dh1[0]; *count = rows0 * 512; }
+  else if (n == "dh1_val") { *d_ptr = l->dh1[1]; *count = l->dh1[1] ? rows0 * 512 : 0; }
+  else if (n == "dact1" || n == "dact2" || n == "dact3" || n == "dact1_hi" || n == "dact2_hi" || n == "dact3_hi" ||
+           n == "dact1_lo" || n == "dact2_lo" || n == "dact3_lo" || n == "act1_lo" || n == "act2_lo") {
+    const bool act = n[1] == 'c';   // "act1_lo", "act2_lo"
+    const int layer = n[act ? 3 : 4] - '0';
+    const int64_t per[3] = {(int64_t)l->B * l->d.h1 * l->d.w1 * 32, (int64_t)l->B * l->d.h2 * l->d.w2 * 64,
+                            (int64_t)l->B * l->d.feat};
+    float* f32[3] = {l->dact1, l->dact2, l->dact3};
+    if (n.size() == (act ? 4u : 5u)) *d_ptr = f32[layer - 1];
+    else if (!l->um) return fail(DZ_EINVAL, "%s is not materialised on the fp32-FMA torso", name);
+    else *d_ptr = act ? um_act_lo(l->um, layer) : n.back() == 'i' ? um_dact_hi(l->um, layer) : um_dact_lo(l->um, layer);
+    *count = per[layer - 1];
+  }
   else if (n == "iqn_hi") {
     if (l->pk_on) return fail(DZ_EINVAL, "iqn_hi is not materialised on the packed tensor-core path");
     *d_ptr = l->hi[0]; *count = l->hi[0] ? rows0 * l->d.feat : 0;

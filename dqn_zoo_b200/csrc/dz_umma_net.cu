@@ -1457,6 +1457,9 @@ float* um_act_f32(UmNet* n, int layer, int pass) {
   return (layer < 3 ? n->act_hi[layer - 1] : n->act_f32[layer - 1]) + per[layer - 1] * pass;
 }
 float* um_dact_f32(UmNet* n, int layer) { return n->dact_f32[layer - 1]; }
+float* um_act_lo(UmNet* n, int layer) { return layer < 3 ? n->act_lo[layer - 1] : nullptr; }
+float* um_dact_hi(UmNet* n, int layer) { return n->dact_hi[layer - 1]; }
+float* um_dact_lo(UmNet* n, int layer) { return n->dact_lo[layer - 1]; }
 float* um_h1_f32(UmNet* n, int pass, int stream) { return n->h1_buf + ((int64_t)pass * n->d.nstream + stream) * n->d.B * 512; }
 float* um_dh1_f32(UmNet* n, int stream) { return n->dh1_f32 + (int64_t)stream * n->d.B * 512; }
 float* um_dh1_hi(UmNet* n, int stream) { return n->dh1_hi + (int64_t)stream * n->d.B * 512; }

@@ -41,6 +41,9 @@ int um_net_mma_path(UmNet* n, const char* tag);   // UM_PATH_MMA_SYNC / UM_PATH_
 // Buffers the rest of the learner reads / writes (fp32 views of the activations and gradients).
 float* um_act_f32(UmNet* n, int layer, int pass);      // layer 1..3 -> [B][h][w][C] (layers 1, 2: the tf32 hi image)
 float* um_dact_f32(UmNet* n, int layer);               // layer 1..3: d loss / d (pre-ReLU masked) activation of pass 0
+float* um_act_lo(UmNet* n, int layer);                 // layer 1, 2: tf32 lo image of pass 0's activation (hi: um_act_f32)
+float* um_dact_hi(UmNet* n, int layer);                // layer 1..3: tf32 hi / lo of um_dact_f32, the operands of the next GEMM
+float* um_dact_lo(UmNet* n, int layer);
 float* um_h1_f32(UmNet* n, int pass, int stream);      // [B][512] (post-ReLU)
 float* um_dh1_f32(UmNet* n, int stream);               // [B][512] gradient wrt h1 (already masked), INPUT of um_backward_fc
 float* um_dh1_hi(UmNet* n, int stream);               // tf32 hi / lo of dh1 (written by the producer or by um_split_dh1)

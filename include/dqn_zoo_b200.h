@@ -687,9 +687,12 @@ int dz_test_pong_step(const dz_pong_config* cfg, int32_t* state, int32_t action,
                       int32_t* record);
 
 /* Device pointer + element count of an internal learner buffer of the last update (pass 0: "act1", "act2", "act3",
- * "h1", "h1_val", "dh1", "iqn_e0", "iqn_hi", "iqn_dhi"; fqf's proposals: "fqf_tau" [2][B][N+1] and "fqf_tau_hat"
- * [2][B][N], application 0 from online(s_tm1)'s features and 1 from target(s_t)'s, and "fqf_dlogits" [B][N]);
- * tests/tools only. */
+ * "h1", "h1_val", "dh1", "dh1_val", "iqn_e0", "iqn_hi", "iqn_dhi"; the fp32 input gradients of the conv layers' masked
+ * outputs "dact1", "dact2", "dact3"; on the tensor-core torso only, where "act1" and "act2" are the tf32 hi images,
+ * their lo images "act1_lo", "act2_lo" and the tf32 hi / lo split of each input gradient that the next GEMM reads,
+ * "dact1_hi" .. "dact3_hi" and "dact1_lo" .. "dact3_lo" (DZ_EINVAL on the fp32-FMA torso); fqf's proposals: "fqf_tau"
+ * [2][B][N+1] and "fqf_tau_hat" [2][B][N], application 0 from online(s_tm1)'s features and 1 from target(s_t)'s, and
+ * "fqf_dlogits" [B][N]); tests/tools only. */
 int dz_test_learner_buffer(dz_learner* l, const char* name, float** d_ptr, int64_t* count);
 /* The per-example arithmetic of the munchausen loss kernel evaluated on the HOST by the same source (fp32, expf / logf):
  * q_tm1 = online(s_tm1), qbar_tm1 = target(s_tm1), qbar_t = target(s_t), each [A] (1 <= A <= 18).  Writes the target
